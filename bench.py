@@ -6,14 +6,18 @@ T_text=150) synthetic text, exactly 800 decoder frames per row (gate_threshold =
 gate never fires, max_decoder_steps = 800; SURVEY.md section 8(d)) -> encoder, 800-step persistent
 decoder, postnet.  51,200 mel frames per GPU per step.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
   value : frames/s with the text ids already resident in HBM (device tensors through the nn.Module API)
   e2e   : frames/s through the C-ABI t2_infer_host with HOST buffers (pinned text in, mel_postnet out)
   roofline     : the persistent decoder kernel, algorithmic FLOPs (38,350,592 per frame) / CUDA-event time
   cpu_baseline : the oracle port (oracle/tacotron2_oracle.py, torch CPU, all host threads) on a bounded sample
-  --impl reference : the same metric from the CPU oracle port alone (the reference is pure Python and
-                     /root/reference does not exist on the GPU box; DESIGN.md "reference arm")
+  --impl reference : the same metric from the CPU oracle port alone (the reference is pure Python;
+                     DESIGN.md "reference arm")
+  --dump-outputs DIR : after the timed steps, what Tacotron2.inference returned in the last timed step (rank 0) as
+                       DIR/<name>.npy -- mel_outputs, mel_outputs_postnet, gate_outputs, alignments (float32) and
+                       mel_lengths (float64), 63.7 MB in all; the inputs are the same on every run with the same
+                       arguments, so two builds can be compared output for output
 """
 import argparse
 import json
@@ -44,7 +48,7 @@ def load_max_mhz():
     try:
         return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["sm_max_mhz"])
     except Exception:
-        return 1965.0
+        return 1980.0                      # H100 SXM maximum SM clock
 
 
 def load_peaks():
@@ -52,11 +56,11 @@ def load_peaks():
     if os.path.isfile(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense FP16 989 TFLOP/s, HBM3 3.35 TB/s at 700 W), not measured"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -178,8 +182,8 @@ class CpuPort:
 
 
 def run_reference(args, rank):
-    """--impl reference: the reference's algorithm on the host cores (the oracle port: the reference is pure Python and
-    /root/reference does not exist on the GPU box), same metric / config as the GPU arm.  The first warm-up pass runs the
+    """--impl reference: the reference's algorithm on the host cores (the oracle port: the reference is pure Python),
+    same metric / config as the GPU arm.  The first warm-up pass runs the
     complete workload; if K such passes would not fit ~4 minutes the timed passes measure a bounded number of decoder steps
     and extrapolate (stated in config.workload)."""
     if rank != 0:
@@ -385,6 +389,15 @@ def eager_gpu_context():
         return {"unavailable": str(e)[:120]}
 
 
+def dump_outputs(d, outputs, lengths):
+    """What a caller of the timed path receives: Tacotron2.inference's four outputs (float32) and mel_lengths (float64)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in zip(("mel_outputs", "mel_outputs_postnet", "gate_outputs", "alignments"), outputs):
+        np.save(os.path.join(d, name + ".npy"), t.detach().float().cpu().numpy())
+    np.save(os.path.join(d, "mel_lengths.npy"), lengths.detach().cpu().numpy().astype(np.float64))
+
+
 def _launch_counter():
     from tacotron2_b200 import _capi
     return _capi.lib().t2_kernel_launch_count
@@ -399,6 +412,8 @@ def main():
     ap.add_argument("--decoder-impl", default="auto", choices=["auto", "stepwise", "persistent"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the train / config5 / eager_gpu blocks (A/B runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path returned in its last step as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -407,6 +422,7 @@ def main():
         run_reference(args, rank)
         return
     args.warmup = max(args.warmup, 3)
+    torch.manual_seed(1234 + rank)       # the engine's dropout seeds derive from torch's seed: same inputs on every run
 
     import torch.distributed as dist
     import tacotron2_b200 as t2
@@ -429,7 +445,7 @@ def main():
     text = rand_text(B_PER_GPU, T_TEXT, 100 + rank)
     text_dev = text.cuda()
     text_host = text.clone().pin_memory()
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")    # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")    # > 50 MB L2 of an H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -453,11 +469,14 @@ def main():
 
     import contextlib
 
+    last_out = []
+
     def step_device():
         # the reference prints "Warning! Reached max decoder steps" to stdout (model.py:446); this
         # workload reaches the cap by construction, keep stdout for the single JSON line
         with torch.no_grad(), contextlib.redirect_stdout(sys.stderr):
             out = model.inference(text_dev)
+        last_out[:] = [out]
         return out
 
     out_host = None
@@ -480,6 +499,8 @@ def main():
     launches0 = L.t2_kernel_launch_count()
     ms_dev = timed(step_device, args.steps)
     launches = L.t2_kernel_launch_count() - launches0
+    if args.dump_outputs and rank == 0:           # before any other call can reuse the engine's buffers
+        dump_outputs(args.dump_outputs, last_out[0], model.mel_lengths)
     barrier()
     ms_e2e = timed(step_host, args.steps)
     barrier()

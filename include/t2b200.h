@@ -1,5 +1,5 @@
 /*
- * t2b200.h -- C ABI of libt2b200.so, the B200 (sm_100a) Tacotron 2 mel-spectrogram engine.
+ * t2b200.h -- C ABI of libt2b200.so, the H100 (sm_90a) Tacotron 2 mel-spectrogram engine.
  *
  * The reference (NVIDIA/tacotron2) has no FFI / plugin layer: its hot path is ordinary Python
  * methods on nn.Modules (SURVEY.md section 8(b)).  This header is therefore the boundary a
@@ -77,7 +77,7 @@ typedef struct T2Config {
 /* Decoder implementations selectable at run time (both are CUDA; there is no CPU path). */
 #define T2_IMPL_AUTO        0   /* persistent kernel when the shape allows, else STEPWISE */
 #define T2_IMPL_STEPWISE    1   /* one fp32 kernel sequence per step (bring-up / cross-check) */
-#define T2_IMPL_PERSISTENT  2   /* one persistent cooperative tcgen05 kernel for the whole loop */
+#define T2_IMPL_PERSISTENT  2   /* one persistent cooperative wgmma kernel for the whole loop */
 
 #define T2_MODE_INFER    0      /* Decoder.inference: free running, prenet on the fed-back frame */
 #define T2_MODE_TEACHER  1      /* Decoder.forward : teacher forced, exactly n_steps_cap steps  */
@@ -340,15 +340,15 @@ int    t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_
 
 /* ---- self tests (libt2b200_selftest.so only: the same sources built with -DT2_SELFTEST; not part of the product
  * library) -------------------------------------------------------------------------------------------------
- * t2_selftest_umma: runs the tcgen05 split-fp16 GEMM engine used by the persistent decoder on a
+ * t2_selftest_umma: runs the wgmma split-fp16 GEMM engine used by the persistent decoder on a
  * (64 x K) x (N x K)^T problem and writes C (64 x N) fp32. */
 #ifdef T2_SELFTEST
 int t2_selftest_umma(const float* A, const float* W, int32_t N, int32_t K, int32_t passes,
                      float* C, void* stream);
-/* Micro-benchmark: SM cycles for `reps` back-to-back tcgen05.mma (M x N x 16, fp16, operands resident in
- * shared memory) -> out_host[0] = issue cycles, out_host[1] = issue + completion cycles. */
+/* Micro-benchmark: SM cycles for `reps` back-to-back wgmma of one warpgroup (M = 64, N in {32, 64, 128}, K = 16, fp16,
+ * operands resident in shared memory) -> out_host[0] = issue cycles, out_host[1] = issue + completion cycles. */
 int t2_selftest_mma_rate(int32_t M, int32_t N, int32_t reps, int32_t alternate_d, int64_t* out_host);
-/* `reps` groups of `group` back-to-back MMAs, each group followed by tcgen05.commit + a wait for it (one K chunk of a
+/* `reps` groups of `group` back-to-back MMAs, each group followed by a commit + a wait for it (one K chunk of a
  * streaming event): out_host[0] = total SM cycles. */
 int t2_selftest_mma_group(int32_t M, int32_t N, int32_t group, int32_t reps, int64_t* out_host);
 /* The training path's general tensor-core GEMM (gemm_tc.cu): row-major C = op(A) . op(B) + beta C, strided batch. */

@@ -7,10 +7,9 @@ from the reference's *behaviour*: no ``nn.Module`` is used, every function takes
 ("port") leg of ``bench.py``; the product package ``tacotron2_b200`` never imports it.
 
 Parity pinning: the reference ships no tests / golden vectors (SURVEY.md section 4), so this
-oracle is pinned by executing the unmodified reference ``model.py`` in the build container
-(``oracle/ref_import.py``) -- see ``tests/test_oracle_vs_reference.py`` (runs where
-``/root/reference`` exists) and the committed fixtures under ``tests/golden`` generated by
-``tools/make_golden.py`` from the reference itself.
+oracle is pinned by executing the unmodified reference ``model.py`` (``oracle/ref_import.py``):
+``tools/make_golden.py`` stores what the reference computed under ``tests/golden``, and
+``tests/test_oracle_vs_reference.py`` / ``tests/test_oracle_golden.py`` compare the oracle with it.
 
 All arithmetic is done by torch CPU fp32 tensor ops (matmul / conv1d); an optional
 ``mm`` hook lets precision studies swap the matmul (tools/precision_study.py).

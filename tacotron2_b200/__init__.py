@@ -1,4 +1,4 @@
-"""tacotron2_b200 -- a B200-native (sm_100a) Tacotron 2 mel-spectrogram engine behind the
+"""tacotron2_b200 -- an H100-native (sm_90a) Tacotron 2 mel-spectrogram engine behind the
 NVIDIA/tacotron2 nn.Module API.  See DESIGN.md / INTEGRATION.md."""
 from ._engine import dropout_masks, invalidate_weights  # noqa: F401
 from .hparams import create_hparams  # noqa: F401

@@ -134,7 +134,7 @@ class Engine:
                 dev = t.device
                 break
         if dev is None:
-            raise RuntimeError("tacotron2_b200: the model must live on a CUDA device (B200); there is no "
+            raise RuntimeError("tacotron2_b200: the model must live on a CUDA device (H100); there is no "
                                "CPU path -- call .cuda() first")
         key = (_weights_generation[0],) + tuple(
             (named[n].data_ptr(), named[n]._version, named[n].dtype) if n in named else None for n, _ in self.spec)

@@ -191,7 +191,7 @@ static int check_cfg(const T2Config* c) {
                   c->attention_location_n_filters == kLocF && c->attention_location_kernel_size == kLocK &&
                   c->postnet_embedding_dim == kPost && c->postnet_kernel_size == kConvK && c->postnet_n_convolutions == 5 &&
                   c->n_symbols > 0;
-  if (!ok) return fail(T2_ERR_UNSUPPORTED, "hyper-parameters differ from the reference defaults the sm_100a kernels are built for");
+  if (!ok) return fail(T2_ERR_UNSUPPORTED, "hyper-parameters differ from the reference defaults the sm_90a kernels are built for");
   return T2_OK;
 }
 
@@ -213,7 +213,7 @@ int t2_model_create(T2Model** out, const T2Config* cfg, const void* const* weigh
   T2_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp p;
   T2_CUDA(cudaGetDeviceProperties(&p, dev));
-  if (p.major != 10) return fail(T2_ERR_UNSUPPORTED, "libt2b200 is built for sm_100a only (device is sm_%d%d)", p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) return fail(T2_ERR_UNSUPPORTED, "libt2b200 is built for sm_90a only (device is sm_%d%d)", p.major, p.minor);
   T2Model* m = new T2Model();
   m->cfg = *cfg; m->device = dev; m->sm_count = p.multiProcessorCount;
   int r = set_weights(m, weights, n_weights);

@@ -1,5 +1,5 @@
 // Tensor-core conv1d / GEMM for the Encoder (model.py:157-167, 174-175), the BiLSTM input projection
-// (model.py:169-171) and the Postnet (model.py:112-146): split-fp16 implicit GEMM on tcgen05.
+// (model.py:169-171) and the Postnet (model.py:112-146): split-fp16 implicit GEMM on wgmma.
 //
 //   out[(b,t), n] = epilogue( sum_{tap, ci} W[n][tap][ci] * x[(b, t + tap - pad), ci] )
 //
@@ -11,7 +11,7 @@
 //   (K-major no-swizzle canonical layout with LBO = 2112 between k8 groups, SBO = 128 between 8-row groups.)
 // * Weights are packed per (n-tile, 64-channel chunk, tap) as [hi | lo] SWIZZLE_128B planes and streamed
 //   through a ring; within a cluster the weight stage is fetched once and TMA-multicast.
-// * fp32-grade: hi*hi + lo*hi + hi*lo, 3 MMAs (M=128, N=n_tile, K=16) per 16 channels, fp32 in TMEM.
+// * fp32-grade: hi*hi + lo*hi + hi*lo, 3 MMAs (M=64 per warpgroup, N=n_tile, K=16) per 16 channels, fp32 in registers.
 // * Epilogue: folded BatchNorm scale/shift (+bias), ReLU / tanh, and either the next layer's planes,
 //   fp32 rows (LSTM gate pre-activations) or the final (B, 80, T) tensor with the residual (model.py:511/524).
 #include <stdlib.h>
@@ -27,7 +27,7 @@ constexpr int kTile = 128;                 // output rows per CTA
 constexpr int kHalo = 4;                   // input rows = kTile + 4
 constexpr int kSeg = (kTile + kHalo) * 16; // bytes of one k8 plane segment of a tile = 2112
 constexpr int kAStage = 16 * kSeg;         // 8 k8 groups x (hi, lo) = 33792 bytes per 64-channel chunk
-constexpr int kThreadsC = 192;             // warp 0 producer, warp 1 MMA issuer, warps 2-5 epilogue
+constexpr int kThreadsC = 384;             // warp 0 producer; warpgroups 1 / 2: MMA + epilogue
 constexpr unsigned long long kWd = 1ull << 32;
 
 __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) {
@@ -55,28 +55,23 @@ template <int NT, int NH, int WS>   // NT = weight rows per stage (MMA N), NH = 
 __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr int kWStage = NT * 64 * 2 * 2;   // hi + lo planes of NT rows x 64 k
-  constexpr int kTmem = NT * NH <= 128 ? 128 : 256;
+  constexpr int kOutPitch = NT * NH + 4;     // fp32 output tile [128][kOutPitch] (reuses the operand stages)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mt = blockIdx.x, nt = blockIdx.y;
   uint8_t* s_w = smem;                                   // WS x kWStage (1024-aligned: SWIZZLE_128B)
   uint8_t* s_a = smem + WS * kWStage;                    // 2 x kAStage
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + 2 * kAStage);
   uint64_t* a_full = bars; uint64_t* a_empty = bars + 2;
-  uint64_t* w_full = bars + 4; uint64_t* w_empty = bars + 4 + WS; uint64_t* acc = bars + 4 + 2 * WS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5 + 2 * WS);
+  uint64_t* w_full = bars + 4; uint64_t* w_empty = bars + 4 + WS;
   const uint32_t cs = p.cluster, rank = cs > 1 ? ptx::cluster_ctarank() : 0;
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < WS; ++i) { ptx::mbar_init(&w_full[i], 1); ptx::mbar_init(&w_empty[i], cs); }
-    ptx::mbar_init(acc, 1);
+    // a stage is released by the 2 MMA warpgroups (a weight stage: of every CTA of the cluster)
+    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
+    for (int i = 0; i < WS; ++i) { ptx::mbar_init(&w_full[i], 1); ptx::mbar_init(&w_empty[i], 2 * cs); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<kTmem>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
   if (cs > 1) ptx::cluster_sync_all();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const bool tile_live = mt < p.n_tiles_m;     // grid.x is rounded up to the cluster size
 
   if (warp == 0) {
@@ -110,21 +105,28 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = ptx::make_idesc_f16(128, NT);
-      uint32_t wst = 0, wph = 0;
-      const int tap0 = p.taps == 1 ? 2 : 0;   // a GEMM (taps == 1) reads the centre rows of the halo tile
-      for (int c = 0; c < p.nchunks; ++c) {
-        const int sa = c & 1;
-        wait_bar(&a_full[sa], (c >> 1) & 1);
-        const uint32_t ab = ptx::smem_u32(s_a + sa * kAStage);
-        for (int th = 0; th < p.taps * NH; ++th) {
-          const int tap = th / NH, h = th - tap * NH;
+  } else if (tid >= 128) {
+    // ---- MMA warpgroups 1 / 2: output rows [64 wg, 64 wg + 64) of the tile, all NT * NH columns in registers ----
+    const int wg = (tid >> 7) - 1, wt = tid & 127;
+    float d[NH][NT / 2];
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) d[h][i] = 0.f;
+      ptx::wg_fence_regs<NT / 2>(d[h]);
+    }
+    uint32_t wst = 0, wph = 0;
+    const int tap0 = p.taps == 1 ? 2 : 0;   // a GEMM (taps == 1) reads the centre rows of the halo tile
+    for (int c = 0; c < p.nchunks; ++c) {
+      const int sa = c & 1;
+      wait_bar(&a_full[sa], (c >> 1) & 1);
+      const uint32_t ab = ptx::smem_u32(s_a + sa * kAStage) + (uint32_t)wg * (64 * 16);
+      for (int tap = 0; tap < p.taps; ++tap) {
+#pragma unroll
+        for (int h = 0; h < NH; ++h) {
           wait_bar(&w_full[wst], wph);
-          ptx::tc_fence_after();
           const uint32_t wb = ptx::smem_u32(s_w + wst * kWStage);
-          const uint32_t dcol = tmem + h * NT;
+          ptx::wg_fence();
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk) {
             const uint32_t aoff = (2 * kk) * kSeg + (tap + tap0) * 16;
@@ -132,35 +134,46 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
             const uint64_t a_lo = ptx::make_smem_desc(ab + 8 * kSeg + aoff, kSeg, 128);
             const uint64_t b_hi = ptx::make_sw128_desc(wb + kk * 32);
             const uint64_t b_lo = ptx::make_sw128_desc(wb + NT * 128 + kk * 32);
-            ptx::umma_f16(dcol, a_hi, b_hi, idesc, (c | tap | kk) != 0 ? 1u : 0u);
-            ptx::umma_f16(dcol, a_lo, b_hi, idesc, 1u);
-            ptx::umma_f16(dcol, a_hi, b_lo, idesc, 1u);
+            ptx::wgmma_f16<NT>(d[h], a_hi, b_hi);
+            ptx::wgmma_f16<NT>(d[h], a_lo, b_hi);
+            ptx::wgmma_f16<NT>(d[h], a_hi, b_lo);
           }
-          if (cs == 1) ptx::umma_commit(&w_empty[wst]);
-          else ptx::umma_commit_mc(&w_empty[wst], (uint16_t)((1u << cs) - 1u));
+          ptx::wg_commit();
+          ptx::wg_wait<0>();
+          ptx::wg_fence_regs<NT / 2>(d[h]);
+          if (wt == 0) {                     // this warpgroup is done with the weight stage in every CTA of the cluster
+            if (cs == 1) ptx::mbar_arrive(&w_empty[wst]);
+            else for (uint32_t r = 0; r < cs; ++r) ptx::mbar_arrive_cluster(&w_empty[wst], r);
+          }
           if (++wst == WS) { wst = 0; wph ^= 1; }
         }
-        ptx::umma_commit(&a_empty[sa]);
       }
-      ptx::umma_commit(acc);
+      if (wt == 0) ptx::mbar_arrive(&a_empty[sa]);
     }
-    __syncwarp();
-  } else {
-    // ---- epilogue: 4 warps, TMEM lane quadrant = warp % 4, lane = output row of the tile ----
-    wait_bar(acc, 0);
-    ptx::tc_fence_after();
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
+    // every stage this CTA receives has been consumed: the operand stages become the fp32 output tile
+    ptx::named_bar_sync(1, 256);
+    float* s_out = reinterpret_cast<float*>(smem);
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int i = 0; i < NT / 2; i += 2) {
+        const int r = wg * 64 + ptx::wg_frag_row(i, wt), col = h * NT + ptx::wg_frag_col(i, wt);
+        *reinterpret_cast<float2*>(s_out + r * kOutPitch + col) = make_float2(d[h][i], d[h][i + 1]);
+      }
+    ptx::named_bar_sync(1, 256);
+    // ---- epilogue: thread = (output row r of the tile, half of the 8-column groups) ----
+    const int ct = tid - 128, r = ct & 127, chalf = ct >> 7;
     const long prow = (long)mt * kTile + r;          // padded row index p
     const int span = p.T + p.seq_pad;
     const int b = (int)(prow / span), pt = (int)(prow - (long)b * span) - p.seq_pad / 2;
     const bool valid = tile_live && b < p.B && pt >= 0 && pt < p.T;
-    const uint32_t tl = tmem + ((uint32_t)(quad * 32) << 16);
     const int n0 = nt * NT * NH;
     if (tile_live) {
-      for (int c0 = 0; c0 < NT * NH; c0 += 8) {
+      for (int c0 = chalf * 8; c0 < NT * NH; c0 += 16) {
         float v[8];
-        ptx::tmem_ld8(tl + c0, v);
+        const float4 v0 = *reinterpret_cast<const float4*>(s_out + r * kOutPitch + c0);
+        const float4 v1 = *reinterpret_cast<const float4*>(s_out + r * kOutPitch + c0 + 4);
+        v[0] = v0.x; v[1] = v0.y; v[2] = v0.z; v[3] = v0.w; v[4] = v1.x; v[5] = v1.y; v[6] = v1.z; v[7] = v1.w;
         if (n0 + c0 >= p.cout) continue;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -206,10 +219,9 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
       }
     }
   }
-  ptx::tc_fence_before();
   __syncthreads();
   if (cs > 1) {
-    // peers' multicast commits target our w_empty barriers: drain before leaving (producer thread state is
+    // peers' consumers arrive on our w_empty barriers: drain before leaving (producer thread state is
     // gone here, so wait on the parity each barrier reaches after its last use)
     if (tid == 0) {
       const int total = p.nchunks * p.taps * NH;
@@ -221,7 +233,6 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
     __syncthreads();
     ptx::cluster_sync_all();
   }
-  if (warp == 2) ptx::tmem_dealloc<kTmem>(tmem);
 }
 
 // ---- layout conversion kernels ---------------------------------------------------------------------
@@ -308,7 +319,7 @@ __global__ void fold_bn_bias_kernel(const float* cbias, const float* g, const fl
 template <int NT, int NH, int WS>
 int launch_conv(const ConvParams& p, int n_tiles_n, cudaStream_t s) {
   constexpr int kWStage = NT * 64 * 2 * 2;
-  const size_t smem = (size_t)WS * kWStage + 2 * kAStage + (5 + 2 * WS) * 8 + 64;
+  const size_t smem = (size_t)WS * kWStage + 2 * kAStage + (4 + 2 * WS) * 8 + 64;
   T2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, NH, WS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));

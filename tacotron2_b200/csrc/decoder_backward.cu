@@ -35,7 +35,7 @@ int blas_handle(T2Model* m, cudaStream_t s, cublasHandle_t* out) {
   if (cublasSetStream(*out, s) != CUBLAS_STATUS_SUCCESS) return fail(T2_ERR_CUDA, "cublasSetStream failed");
   return T2_OK;
 }
-// Every dense product of the training path goes through gemm_rm(): our tcgen05 split-fp16 GEMM (gemm_tc.cu) by default;
+// Every dense product of the training path goes through gemm_rm(): our wgmma split-fp16 GEMM (gemm_tc.cu) by default;
 // T2_GEMM=cublas selects plain cuBLAS fp32 sgemm, kept only as the independent cross-check of tests/test_gpu_backward.py.
 bool use_cublas_gemm() {
   static int v = -1;
@@ -679,7 +679,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   do {                                                                \
     if (prof && T - 1 - t < kProfSteps) cudaEventRecord(pev[T - 1 - t][i], s); \
   } while (0)
-  // skinny GEMMs: tcgen05 split-fp16 engine (default) or the fp32 SIMT kernel (T2_BWD_GEMM=simt, cross-check)
+  // skinny GEMMs: wgmma split-fp16 engine (default) or the fp32 SIMT kernel (T2_BWD_GEMM=simt, cross-check)
   bool tc_gemm = true;
   {
     const char* e = getenv("T2_BWD_GEMM");
@@ -776,7 +776,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   float* const* G = a->grads;
   const float* x2 = a->teacher_prenet;
   const int TBi = (int)TB;
-  // LSTM weight / bias gradients: our tcgen05 split-fp16 engine (default) or plain cuBLAS fp32 GEMMs (T2_WGRAD=cublas)
+  // LSTM weight / bias gradients: our wgmma split-fp16 engine (default) or plain cuBLAS fp32 GEMMs (T2_WGRAD=cublas)
   bool tc_wgrad = true;
   {
     const char* e = getenv("T2_WGRAD");

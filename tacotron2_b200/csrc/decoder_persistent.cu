@@ -1,13 +1,13 @@
 // T2_IMPL_PERSISTENT: the whole autoregressive decoder loop (model.py:381-454) as ONE persistent
-// cooperative sm_100a kernel.
+// cooperative sm_90a kernel.
 //
 //   * 128 CTAs (one per SM) in clusters, 512 threads each.  CTA c owns hidden units [8c, 8c+8) of BOTH
 //     LSTM cells (attention_rnn, decoder_rnn): their cell state lives in registers for the whole loop,
-//     their gate pre-activations accumulate in tensor memory (TMEM) across events.
+//     their gate pre-activations accumulate in a shared-memory fp32 tile across events.
 //   * "activation driven" schedule: whenever a new activation block (x2, ah, ctx, dh, x1) is complete,
 //     every CTA streams it ONCE through a shared-memory ring (bulk async copies on the TMA engine; the
 //     activation chunk is multicast to the CTAs of a cluster) together with the slices of every weight
-//     matrix that consumes it, and ONE elected thread issues tcgen05.mma:
+//     matrix that consumes it, and three warpgroups issue wgmma (one consumer slice each):
 //        x2_t  -> att gates += W_ih^a[:, :256] x2                          -> ah_t, ac_t
 //        ah_t  -> dec gates += W_ih^d[:, :1024] ah ; att gates(t+1) += W_hh^a ah ; q = W_q ah
 //        ctx_t -> dec gates += W_ih^d[:, 1024:] ctx ; att gates(t+1) += W_ih^a[:, 256:] ctx ;
@@ -17,13 +17,13 @@
 //     W_P stacks linear_projection, gate_layer and (W_1 . W_proj), so the first prenet layer of the
 //     NEXT step is computed from [dh; ctx] directly (model.py:97-100, 373-378, 449).
 //   * fp32-grade arithmetic on fp16 tensor cores: every operand is split x = hi + lo (two fp16).  The
-//     activation chunk image [hi rows 0-63 | lo rows 64-127] is ONE M=128 A operand; the weight rows of
-//     all consumers of an event are concatenated along N as [W_hi ; W_lo] per consumer, so ONE MMA per
-//     16-wide K step gives all four partial products (hi.hi, lo.hi, hi.lo, lo.lo) in fp32 (the SS-mode
-//     MMA is bound by its 128-row A read, not by N: measured ~125 cycles for any N <= 160):
-//        D[128 x 2N] += [X_hi; X_lo] . [W_hi; W_lo]^T
-//     gates[r] = D[r][hi] + D[r][lo] + D[64+r][hi] + D[64+r][lo]  (summed in the epilogue).
-//     Accumulators are always accumulated into and zeroed by the epilogue that consumed them.
+//     activation chunk image is [X_hi rows 0-63 | X_lo rows 64-127]; the weight rows of all consumers of
+//     an event are concatenated as [W_hi ; W_lo] per consumer.  A warpgroup owns a slice of <= 32 weight
+//     rows of one consumer and accumulates all four partial products (hi.hi, lo.hi, hi.lo, lo.lo) of the
+//     whole event in one 64 x n fp32 register accumulator (4 wgmma m64nNk16 per 16-wide K step):
+//        D[64 x n] += X_hi . W_hi^T + X_lo . W_hi^T + X_hi . W_lo^T + X_lo . W_lo^T
+//     and adds it to the shared-memory accumulator tile once the event's last chunk is in.  Accumulators
+//     are always accumulated into and zeroed by the epilogue that consumed them.
 //   * location-sensitive attention (model.py:43-86): location conv + dense are fused into one 62-tap
 //     filter bank evaluated as a tensor-core GEMM over an im2col image of the previous / cumulative
 //     weights (kept in shared memory across steps); energies, softmax and context per batch row on a
@@ -44,24 +44,26 @@ namespace {
 
 constexpr int kG = 128;               // CTAs
 constexpr int kThreads = 512;
-constexpr int kWarps = kThreads / 32;
 constexpr int kStages = 4;             // ring stages of the helper kernels (self test, backward GEMMs)
-constexpr int kMaxStages = 5;          // the decoder kernel takes 5 when shared memory allows (T_enc <~ 330), else 4
+constexpr int kMaxStages = 5;          // ring stages of the decoder kernel: 4 by default (T2_STAGES: 3-5 where shared memory allows)
 constexpr int kRows = 64;             // batch rows per launch (zero padded)
 constexpr int kXChunkBytes = 2 * kRows * kChunkK * 2;    // [hi 64 rows | lo 64 rows] x 64 k fp16 = 16 KiB
-// accumulator columns: each consumer owns [hi-part n | lo-part n]: att 0-63, dec 64-127, shared slot 128-159
-constexpr int kColA = 0, kColD = 64, kColS = 128;
-constexpr int kNA = 32, kND = 32, kNS = 16;               // weight rows (hi) per consumer
-constexpr int kHiCols = 80;                               // max weight rows of one event (hi) -> MMA N <= 160
-constexpr int kColAtt = 160;                              // attention pa accumulators: 2 tiles x 128 columns
-constexpr int kTmemCols = 512;
+// accumulator columns (shared memory, fp32 [64 batch rows][kAccPitch]): att 0-31, dec 32-63, shared slot 64-79
+constexpr int kColA = 0, kColD = 32, kColS = 64;
+constexpr int kHiCols = 80;                               // max weight rows of one event (hi)
+constexpr int kAccPitch = 84;                             // floats per accumulator row (80 + 4: fewer bank conflicts)
+constexpr int kAccBytes = kRows * kAccPitch * 4;
+constexpr int kMmaWgs = 3;                                // warpgroups 1-3 issue the MMAs of an event (one piece each)
+constexpr int kAttRound = 64;                             // encoder positions per attention pa GEMM
+constexpr int kAttPlane = kAttRound * 128;                // one fp16 plane of the im2col image (64 positions x 64 taps)
+constexpr int kPaPitch = kAttRound + 4;                   // floats per attention dim of the pa tile
+constexpr int kPaBytes = kAtt * kPaPitch * 4;
 constexpr int kWStageMax = 2 * kHiCols * kChunkK * 2;    // hi + lo planes of up to 80 weight rows = 20 KiB
 constexpr int kStageBytes = kXChunkBytes + kWStageMax;   // 36 KiB
 constexpr int kNumEvents = 5;         // x2, ah, ctx, dh, x1
 constexpr int kPCols = 344;           // 80 mel + 1 gate + 256 x1 + 7 pad
 constexpr int kQCta0 = 0, kQCtas = 16, kX2Cta0 = 16, kX2Ctas = 32, kPCta0 = 48, kPCtas = 43;
 constexpr int kWeffBytes = kAtt * kChunkK * 2 * 2;        // fused location filter image (hi+lo) = 32 KiB
-constexpr int kXchStride = 33;
 constexpr unsigned long long kWatchdogCycles = 1ull << 32;   // ~2 s
 
 struct EventPlan {
@@ -88,7 +90,7 @@ struct PersistentPack {
   CtaPlan* plans = nullptr;           // device, kG entries
   float* wp_all = nullptr;            // (344, 1536) fp32: proj | gate | W1.Wproj | zero pad
   float* bias_p = nullptr;            // (344): proj bias | gate bias | W1.b_proj | 0
-  float* bias_a = nullptr;            // (kG, 32) att LSTM bias in TMEM column order
+  float* bias_a = nullptr;            // (kG, 32) att LSTM bias in accumulator column order
   float* bias_d = nullptr;            // (kG, 32)
   int32_t* rows = nullptr;            // row tables for packing
   float* weff = nullptr;              // (128, 64) fp32 fused location filter W_ld . W_loc (62 taps + 2 zero)
@@ -332,11 +334,9 @@ struct Ring {
   uint8_t* stage0;    // kStages buffers of kStageBytes each
   __device__ __forceinline__ uint8_t* stage(uint32_t s) const { return stage0 + s * kStageBytes; }
   uint64_t* full;     // [kStages]
-  uint64_t* empty;    // [kStages]
-  uint64_t* acc;      // accumulator-ready barrier
+  uint64_t* empty;    // [kStages], released once by each MMA warpgroup of every CTA of the cluster
   uint32_t p_stage, p_phase;   // producer cursor (thread 0 of warp 0)
-  uint32_t c_stage, c_phase;   // consumer cursor (thread 0 of warp 1)
-  uint32_t acc_phase;          // all threads
+  uint32_t c_stage, c_phase;   // consumer cursor (threads of the MMA warpgroups 1-3)
   uint64_t pol_x, pol_w;       // L2 eviction policies of the activation / weight streams
   uint32_t cs, rank;           // cluster size (1 = no multicast) and this CTA's rank in it
   uint32_t pre;                // stages whose weight chunk was already issued for the upcoming event
@@ -360,11 +360,30 @@ __device__ __forceinline__ void prefetch_weights(Ring& rg, const EventPlan& nx, 
   rg.pre = n;
 }
 
-// Streams `chunks` K-chunks of the activation image x_img plus this CTA's weight rows through the ring
-// and issues the MMAs (1 per 16-wide K step).  Called by all threads; returns after the accumulators are
-// complete.  Every MMA accumulates (the epilogues zero what they consume).
+// One warpgroup's slice of an event: `m` (<= 32) weight rows starting at hi-plane row `wrow` of a consumer with
+// `n` hi rows (its lo rows start n rows later), accumulated over every K chunk of the event.
+template <int M>
+__device__ __forceinline__ void event_mma(float* d, uint32_t xs, uint32_t w_hi, uint32_t w_lo) {
+  ptx::wg_fence();
+#pragma unroll
+  for (int kk = 0; kk < kChunkK / 16; ++kk) {
+    const uint64_t a_hi = ptx::make_sw128_desc(xs + kk * 32), a_lo = ptx::make_sw128_desc(xs + kRows * 128 + kk * 32);
+    const uint64_t b_hi = ptx::make_sw128_desc(w_hi + kk * 32), b_lo = ptx::make_sw128_desc(w_lo + kk * 32);
+    ptx::wgmma_f16<M>(d, a_hi, b_hi);
+    ptx::wgmma_f16<M>(d, a_lo, b_hi);
+    ptx::wgmma_f16<M>(d, a_hi, b_lo);
+    ptx::wgmma_f16<M>(d, a_lo, b_lo);
+  }
+  ptx::wg_commit();
+  ptx::wg_wait<0>();
+  ptx::wg_fence_regs<M / 2>(d);
+}
+
+// Streams `chunks` K-chunks of the activation image x_img plus this CTA's weight rows through the ring;
+// warpgroups 1-3 issue the MMAs and add their slices to the accumulator tile s_acc.  Called by all threads;
+// returns after the accumulators are complete.  Every MMA accumulates (the epilogues zero what they consume).
 __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const uint8_t* x_img,
-                                          const uint8_t* w_img, int chunks, uint32_t tmem_base,
+                                          const uint8_t* w_img, int chunks, float* s_acc,
                                           DecoderCtrl* ctrl, const EventPlan* next,
                                           const unsigned int* ready = nullptr, unsigned int ready_target = 0) {
   // ready (16 counters, one per K chunk of the activation; null = the caller synchronised already): chunk i of x_img is
@@ -419,32 +438,38 @@ __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const u
       if (next != nullptr && next->nrows != 0) prefetch_weights(rg, *next, w_img, ctrl);
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = ptx::make_idesc_f16(128, 2u * (uint32_t)ep.nrows);
-      const uint32_t d = tmem_base + (uint32_t)ep.col0;
-      for (int i = 0; i < chunks; ++i) {
-        mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
-        ptx::tc_fence_after();
-        const uint32_t xs = ptx::smem_u32(rg.stage(rg.c_stage));
-        const uint32_t ws = xs + kXChunkBytes;
+  } else if (warp >= 4) {
+    // this warpgroup's slice: consumers are cut into slices of <= 32 weight rows, slice i goes to warpgroup 1 + i
+    const int wt = threadIdx.x & 127;
+    int left = (warp >> 2) - 1, wrow = 0, n = 0, m = 0, acol = 0;
+    for (int c = 0, roff = 0, col = ep.col0; c < ep.ncons; roff += 2 * ep.n[c], col += ep.n[c], ++c)
+      for (int j0 = 0; j0 < ep.n[c]; j0 += 32)
+        if (left-- == 0) { wrow = roff + j0; n = ep.n[c]; m = min(32, ep.n[c] - j0); acol = col + j0; }
+    float d[16];
 #pragma unroll
-        for (int kk = 0; kk < kChunkK / 16; ++kk) {
-          const uint64_t a = ptx::make_sw128_desc(xs + kk * 32);                          // [X_hi ; X_lo], M = 128
-          const uint64_t b = ptx::make_sw128_desc(ws + kk * 32);                          // [W_hi ; W_lo] per consumer
-          ptx::umma_f16(d, a, b, idesc, 1u);
-        }
-        if (rg.cs == 1) ptx::umma_commit(&rg.empty[rg.c_stage]);   // frees the stage once these MMAs have read it
-        else ptx::umma_commit_mc(&rg.empty[rg.c_stage], (uint16_t)((1u << rg.cs) - 1u));
-        if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
+    for (int i = 0; i < 16; ++i) d[i] = 0.f;
+    ptx::wg_fence_regs<16>(d);
+    for (int i = 0; i < chunks; ++i) {
+      mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
+      const uint32_t xs = ptx::smem_u32(rg.stage(rg.c_stage));
+      const uint32_t w_hi = xs + kXChunkBytes + (uint32_t)wrow * 128, w_lo = w_hi + (uint32_t)n * 128;
+      if (m == 32) event_mma<32>(d, xs, w_hi, w_lo);
+      else if (m == 24) event_mma<24>(d, xs, w_hi, w_lo);
+      else if (m == 16) event_mma<16>(d, xs, w_hi, w_lo);
+      else if (m == 8) event_mma<8>(d, xs, w_hi, w_lo);
+      if (wt == 0) {                     // this warpgroup is done with the stage (in every CTA of the cluster)
+        if (rg.cs == 1) ptx::mbar_arrive(&rg.empty[rg.c_stage]);
+        else for (uint32_t r = 0; r < rg.cs; ++r) ptx::mbar_arrive_cluster(&rg.empty[rg.c_stage], r);
       }
-      ptx::umma_commit(rg.acc);
+      if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
     }
-    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int col = ptx::wg_frag_col(i, wt);
+      if (col < m) s_acc[ptx::wg_frag_row(i, wt) * kAccPitch + acol + col] += d[i];
+    }
   }
-  mbar_wait(rg.acc, rg.acc_phase, ctrl, 202);
-  rg.acc_phase ^= 1;
-  ptx::tc_fence_after();
+  __syncthreads();
 }
 
 // keep bits (bit i = element idx0+i is kept) of 8 consecutive dropout elements, Philox4x32-10 one block per 4
@@ -465,17 +490,11 @@ __device__ __forceinline__ uint32_t philox_keep8(uint64_t seed, uint32_t site, u
   return bits;
 }
 
-// this lane's 8 accumulator columns of a consumer with n hi-columns at `base`: hi-part + lo-part, then
-// zero both (they are consumed)
-__device__ __forceinline__ void acc_take8(uint32_t t_lane, int base, int n, int col, float* s) {
-  float a[8], b[8];
-  ptx::tmem_ld8(t_lane + base + col, a);
-  ptx::tmem_ld8(t_lane + base + n + col, b);
+// accumulator columns [base + col, base + col + 8) of batch row `row`, then zero them (they are consumed)
+__device__ __forceinline__ void acc_take8(float* s_acc, int row, int base, int col, float* s) {
+  float* a = s_acc + row * kAccPitch + base + col;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) s[i] = a[i] + b[i];
-  ptx::tmem_zero8(t_lane + base + col);
-  ptx::tmem_zero8(t_lane + base + n + col);
-  ptx::tmem_wait_st();
+  for (int i = 0; i < 8; ++i) { s[i] = a[i]; a[i] = 0.f; }
 }
 
 // training stash (decoder.h DecoderStash): gate activations, cell state and (post-dropout) hidden state of
@@ -543,9 +562,9 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   rg.ns = (uint32_t)p.nstages;
   rg.stage0 = sp; sp += p.nstages * kStageBytes;
   uint8_t* s_weff = sp; sp += kWeffBytes;                                     // fused location filter image
+  float* s_acc = reinterpret_cast<float*>(sp); sp += kAccBytes;                // event accumulators
   uint64_t* bars = reinterpret_cast<uint64_t*>(sp); sp += 16 * sizeof(uint64_t);
-  rg.full = bars; rg.empty = bars + kMaxStages; rg.acc = bars + 2 * kMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sp); sp += 16;
+  rg.full = bars; rg.empty = bars + kMaxStages;
   int* s_live = reinterpret_cast<int*>(sp); sp += 16;
   int* s_flag = s_live + 1;                                                    // stop flag broadcast of wait_counter
   float* s_bias_a = reinterpret_cast<float*>(sp); sp += 32 * 4;
@@ -558,25 +577,21 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   long long* s_prof = reinterpret_cast<long long*>(sp); sp += 24 * 8;         // phase profile, accumulated on chip
   float* s_pad0 = reinterpret_cast<float*>(sp); sp += ((TP + 3) & ~3) * 4;   // previous weights (padded)
   float* s_pad1 = reinterpret_cast<float*>(sp); sp += ((TP + 3) & ~3) * 4;   // cumulative weights (padded)
-  // one region, two tenants that are never live together: the hi/lo accumulator exchange of the event epilogues
-  // (s_xch) and the attention's weights / energy partial sums (s_e, s_ep)
-  float* s_xch = reinterpret_cast<float*>(sp);                                // [64][33] lo-row halves of the accumulators
   float* s_e = reinterpret_cast<float*>(sp);                                  // [ntiles * 128] attention weights
   float* s_ep = s_e + ntiles * 128;                                           // [4][ntiles * 128] energy partial sums: one writer
                                                                               // per (group, position), summed in a fixed
                                                                               // order -> bit-reproducible (no shared-memory atomics)
   (void)s_red;
 
-  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = rg.acc_phase = 0;
+  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.cs = p.cluster; rg.rank = p.cluster > 1 ? ptx::cluster_ctarank() : 0;
   rg.pre = 0;
 
   if (tid == 0) {
-    for (int s = 0; s < p.nstages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], rg.cs); }
-    ptx::mbar_init(rg.acc, 1);
+    for (int s = 0; s < p.nstages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs * rg.cs); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<kTmemCols>(tmem_slot);
+  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;   // every MMA accumulates
   for (int i = tid; i < 32; i += kThreads) { s_bias_a[i] = p.bias_a[cta * 32 + i]; s_bias_d[i] = p.bias_d[cta * 32 + i]; }
   for (int i = tid; i < kWeffBytes / 16; i += kThreads)
     reinterpret_cast<uint4*>(s_weff)[i] = reinterpret_cast<const uint4*>(p.weff_img)[i];
@@ -589,35 +604,25 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   for (int i = tid; i < kAtt; i += kThreads) s_v[i] = p.w_v[i];
   if (tid < 8) s_bias_p[tid] = (cta >= kPCta0 && cta < kPCta0 + kPCtas) ? p.bias_p[(cta - kPCta0) * 8 + tid] : 0.f;
   for (int i = tid; i < TP; i += kThreads) { s_pad0[i] = 0.f; s_pad1[i] = 0.f; }   // model.py:274-277
-  ptx::fence_proxy_async();       // s_weff is read by tcgen05.mma (async proxy)
-  ptx::tc_fence_before();
+  ptx::fence_proxy_async();       // s_weff is read by wgmma (async proxy)
   __syncthreads();
   if (p.cluster > 1) ptx::cluster_sync_all();   // peers' mbarriers are initialised before anyone multicasts
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const CtaPlan& plan = p.plans[cta];
   DecoderCtrl* ctrl = p.ctrl;
   unsigned int bar_target = 0;
   const uint32_t bar_cs = p.hier_barrier ? rg.cs : 1;
-  // epilogue role of this thread: TMEM lane quadrant quad = warp % 4 (hardware rule), column group
-  // cg = warp / 4.  Accumulator lane = MMA row: lanes 0-63 are the X_hi rows (batch rows), lanes 64-127
-  // the X_lo rows of the same batch rows; quadrants 2/3 hand their partial sums to quadrants 0/1.
+  // epilogue role of this thread: quad = warp % 4, column group cg = warp / 4.  Quadrants 0/1 own batch rows
+  // 0-63 (row = accumulator row); the threads of quadrants 2/3 (is_lo) take side jobs (dropout bits).
   const int quad = warp & 3, cg = warp >> 2;
   const int row = (quad & 1) * 32 + lane;               // batch row of this lane
   const bool is_lo = quad >= 2;
   const bool erow = !is_lo && row < p.B;
-  const uint32_t t_lane = tmem_base + ((uint32_t)(quad * 32) << 16);
   float c_att[2] = {0.f, 0.f}, c_dec[2] = {0.f, 0.f};  // cell states of units 8*cta + 2*cg + {0,1}
   const bool has_q = cta >= kQCta0 && cta < kQCta0 + kQCtas;
   const bool has_x2 = cta >= kX2Cta0 && cta < kX2Cta0 + kX2Ctas;
   const bool has_p = cta >= kPCta0 && cta < kPCta0 + kPCtas;
   const int halfk = (kLocK - 1) / 2;
-  // zero the LSTM / shared-slot accumulators once (every MMA accumulates)
-  for (int c = cg * 40; c < cg * 40 + 40; c += 8) ptx::tmem_zero8(t_lane + c);
-  ptx::tmem_wait_st();
-  ptx::tc_fence_before();
-  __syncthreads();
   // phase profile (cycles, accumulated over steps) on three sample CTAs; see t2_decoder_profile()
   const int prof_slot = cta == 0 ? 0 : (cta == 60 ? 1 : (cta == 100 ? 2 : -1));
   long long prof_last = clock64();
@@ -630,38 +635,23 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       prof_last = now_;                                                    \
     }                                                                      \
   } while (0)
-  // LSTM epilogue shared by both cells: take the 8 gate columns (2 units x i,f,g,o) of this lane,
-  // combine hi-row and lo-row partial sums through shared memory, return them in g[] for batch rows
-#define T2_TAKE_GATES(colbase, n_, g)                                                        \
-  do {                                                                                   \
-    acc_take8(t_lane, (colbase), (n_), cg * 8, g);                                       \
-    if (is_lo) {                                                                         \
-      _Pragma("unroll") for (int i_ = 0; i_ < 8; ++i_) s_xch[row * kXchStride + cg * 8 + i_] = g[i_]; \
-    }                                                                                    \
-    ptx::tc_fence_before();                                                              \
-    __syncthreads();                                                                     \
-    if (!is_lo) {                                                                        \
-      _Pragma("unroll") for (int i_ = 0; i_ < 8; ++i_) g[i_] += s_xch[row * kXchStride + cg * 8 + i_]; \
-    }                                                                                    \
+  // LSTM epilogue shared by both cells: take the 8 gate columns (2 units x i,f,g,o) of this lane's batch row
+#define T2_TAKE_GATES(colbase, g)                          \
+  do {                                                     \
+    if (!is_lo) acc_take8(s_acc, row, (colbase), cg * 8, g); \
   } while (0)
 
   // epilogue of E4 on the prenet-2 CTAs: x2 = relu(W_2 x1) * mask * 2 -> x2 image            model.py:97-100
   auto x2_epilogue = [&]() {
     float g[8];
-    if (cg == 0) acc_take8(t_lane, kColS, kNS, 0, g);
-    if (cg == 0 && is_lo) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) s_xch[row * kXchStride + i] = g[i];
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
+    if (cg == 0 && !is_lo) acc_take8(s_acc, row, kColS, 0, g);
     if (cg == 0 && erow) {
       const int col0 = (cta - kX2Cta0) * 8;
       float r[8];
       const uint32_t bits = s_mask[row];
 #pragma unroll
       for (int j = 0; j < 8; ++j)
-        r[j] = ((bits >> j) & 1u) ? fmaxf(g[j] + s_xch[row * kXchStride + j], 0.f) * 2.f : 0.f;
+        r[j] = ((bits >> j) & 1u) ? fmaxf(g[j], 0.f) * 2.f : 0.f;
 #pragma unroll
       for (int j = 0; j < 8; j += 2) store_split2(p.x2_img, row, col0 + j, r[j], r[j + 1]);
     }
@@ -672,10 +662,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     // ======== E0: x2_t -> attention LSTM gates, epilogue -> ah_t ==================== model.py:352-356
     {
       const uint8_t* x2 = p.infer ? p.x2_img : p.teacher_x2_img + (size_t)t * 4 * kXChunkBytes;
-      run_event(rg, plan.ev[0], x2, p.wimg, 4, tmem_base, ctrl, &plan.ev[1]);
+      run_event(rg, plan.ev[0], x2, p.wimg, 4, s_acc, ctrl, &plan.ev[1]);
       T2_PROF(0);
       float g[8];
-      T2_TAKE_GATES(kColA, kNA, g);
+      T2_TAKE_GATES(kColA, g);
       if (erow) {
         float hv[2], sg[4][2];
 #pragma unroll
@@ -732,20 +722,14 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         }
         s_mask[row] = bits;
       }
-      run_event(rg, plan.ev[1], p.ah_img, p.wimg, 16, tmem_base, ctrl, nullptr,    // the attention phase reuses the ring as scratch
+      run_event(rg, plan.ev[1], p.ah_img, p.wimg, 16, s_acc, ctrl, nullptr,    // the attention phase reuses the ring as scratch
                 p.chunk_ready ? ctrl->ah_count : nullptr, 8u * (unsigned int)(t + 1));
-      if (has_q) {
+      if (has_q && cg == 0 && !is_lo) {
         float g[8];
-        if (cg == 0) acc_take8(t_lane, kColS, kNS, 0, g);
-        if (cg == 0 && is_lo) {
+        acc_take8(s_acc, row, kColS, 0, g);
+        if (erow) {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) s_xch[row * kXchStride + i] = g[i];
-        }
-        ptx::tc_fence_before();
-        __syncthreads();
-        if (cg == 0 && erow) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) p.q[row * kAtt + (cta - kQCta0) * 8 + j] = g[j] + s_xch[row * kXchStride + j];
+          for (int j = 0; j < 8; ++j) p.q[row * kAtt + (cta - kQCta0) * 8 + j] = g[j];
         }
       }
       T2_PROF(3);
@@ -758,20 +742,20 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     const bool att_cta = (cta & 63) < p.B;
     const int att_b = cta & 63, ahalf = cta >> 6;
     uint8_t* aimg = rg.stage0;
-    // the idle operand ring during the attention phase: [im2col image: hi plane | lo plane][encoder-memory rows of this CTA]
-    const int att_rounds = (T + 255) >> 8;
-    const int img_plane = att_rounds > 1 ? 32768 : max(4096, ((T + 15) & ~15) * 128);
-    const int img_bytes = 2 * img_plane;
-    const int smem_rows = min(T, (p.nstages * kStageBytes - img_bytes) / (kEnc / 2 * 4));   // memory rows staged in the ring
-    // pa^T = Weff . A^T on the tensor cores (fused model.py:23-25), i.e. the fused filter bank is the M = 128 operand (TMEM lane =
-    // attention dim d) and the positions are the N dimension (accumulator column = position, N = T_enc rounded up
-    // to 16, <= 256 per round).  Every warp then owns a slice of POSITIONS of all 128 dims, so the 19,200 tanh of a
-    // row spread evenly over the four SM sub-partitions for any T_enc (position-major tiles put the partial last
-    // tile on one sub-partition: 64 vs 32 tanh per thread at T_enc = 150), the processed-memory reads are
-    // coalesced (lanes = consecutive dims) and can be issued before the q barrier.
+    // the idle operand ring during the attention phase: [im2col image: hi plane | lo plane][pa tile][encoder-memory rows
+    // of this CTA]
+    const int att_rounds = (T + kAttRound - 1) / kAttRound;
+    const int img_bytes = 2 * kAttPlane;
+    float* s_pa = reinterpret_cast<float*>(aimg + img_bytes);                       // [128 dims][kPaPitch] fp32
+    const int smem_rows = min(T, (p.nstages * kStageBytes - img_bytes - kPaBytes) / (kEnc / 2 * 4));   // memory rows staged in the ring
+    // pa^T = Weff . A^T on the tensor cores (fused model.py:23-25), i.e. the fused filter bank is the M = 128 operand
+    // (attention dim d; warpgroups 0 / 1 take dims 0-63 / 64-127) and kAttRound positions are the N dimension.  The
+    // tile goes to shared memory, where every warp then owns a slice of POSITIONS of all 128 dims, so the tanh of a
+    // row spread evenly over the four SM sub-partitions for any T_enc, the processed-memory reads are coalesced
+    // (lanes = consecutive dims) and can be issued before the q barrier.
     auto att_im2col_mma_tr = [&](int r0) {
-      const int jbase = r0 * 256, cnt = min(T - jbase, 256), npad = (cnt + 15) & ~15;
-      for (int item = tid; item < npad * 8; item += kThreads) {
+      const int jbase = r0 * kAttRound, cnt = min(T - jbase, kAttRound);
+      for (int item = tid; item < kAttRound * 8; item += kThreads) {
         const int jj = item >> 3, g8 = item & 7, j = jbase + jj;
         __align__(16) __half hh[8];
         __align__(16) __half ll[8];
@@ -784,33 +768,40 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         }
         uint8_t* dst = aimg + (jj >> 3) * 1024 + (jj & 7) * 128 + ((g8 ^ (jj & 7)) * 16);
         *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(hh);
-        *reinterpret_cast<uint4*>(dst + img_plane) = *reinterpret_cast<const uint4*>(ll);
+        *reinterpret_cast<uint4*>(dst + kAttPlane) = *reinterpret_cast<const uint4*>(ll);
       }
       ptx::fence_proxy_async();
       __syncthreads();
-      if (warp == 1) {
-        if (lane == 0) {
-          ptx::tc_fence_after();
-          const uint32_t ws = ptx::smem_u32(s_weff), ps = ptx::smem_u32(aimg);
-          const uint32_t idesc = ptx::make_idesc_f16(128, (uint32_t)npad);
-          const uint32_t d = tmem_base + kColAtt;
+      if (warp < 8) {
+        const int wg = warp >> 2, wt = tid & 127;
+        const uint32_t ws = ptx::smem_u32(s_weff) + (uint32_t)wg * (64 * 128), ps = ptx::smem_u32(aimg);
+        float d[kAttRound / 2];
 #pragma unroll
-          for (int kk = 0; kk < kChunkK / 16; ++kk) {
-            const uint64_t w_hi = ptx::make_sw128_desc(ws + kk * 32);
-            const uint64_t w_lo = ptx::make_sw128_desc(ws + 16384 + kk * 32);
-            const uint64_t p_hi = ptx::make_sw128_desc(ps + kk * 32);
-            const uint64_t p_lo = ptx::make_sw128_desc(ps + (uint32_t)img_plane + kk * 32);
-            ptx::umma_f16(d, w_hi, p_hi, idesc, kk > 0 ? 1u : 0u);
-            ptx::umma_f16(d, w_lo, p_hi, idesc, 1u);
-            ptx::umma_f16(d, w_hi, p_lo, idesc, 1u);
-          }
-          ptx::umma_commit(rg.acc);
+        for (int i = 0; i < kAttRound / 2; ++i) d[i] = 0.f;
+        ptx::wg_fence_regs<kAttRound / 2>(d);
+        ptx::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < kChunkK / 16; ++kk) {
+          const uint64_t w_hi = ptx::make_sw128_desc(ws + kk * 32);
+          const uint64_t w_lo = ptx::make_sw128_desc(ws + kAtt * 128 + kk * 32);
+          const uint64_t p_hi = ptx::make_sw128_desc(ps + kk * 32);
+          const uint64_t p_lo = ptx::make_sw128_desc(ps + kAttPlane + kk * 32);
+          ptx::wgmma_f16<kAttRound>(d, w_hi, p_hi);
+          ptx::wgmma_f16<kAttRound>(d, w_lo, p_hi);
+          ptx::wgmma_f16<kAttRound>(d, w_hi, p_lo);
         }
-        __syncwarp();
+        ptx::wg_commit();
+        ptx::wg_wait<0>();
+        ptx::wg_fence_regs<kAttRound / 2>(d);
+#pragma unroll
+        for (int i = 0; i < kAttRound / 2; i += 2)
+          *reinterpret_cast<float2*>(s_pa + (wg * 64 + ptx::wg_frag_row(i, wt)) * kPaPitch + ptx::wg_frag_col(i, wt)) =
+              make_float2(d[i], d[i + 1]);
       }
+      __syncthreads();
     };
     auto stage_memory_rows = [&](int j0, int j1) {     // cp.async this CTA's half of memory rows [j0, j1) into the ring
-      const uint32_t sbase = ptx::smem_u32(rg.stage0) + (uint32_t)img_bytes;
+      const uint32_t sbase = ptx::smem_u32(rg.stage0) + (uint32_t)(img_bytes + kPaBytes);
       const float* msrc = p.memory + (long)att_b * T * kEnc + ahalf * (kEnc / 2);
       for (int i = j0 * 64 + tid; i < j1 * 64; i += kThreads) {
         const int j = i >> 6, c4 = i & 63;
@@ -821,7 +812,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       asm volatile("cp.async.commit_group;" ::: "memory");
     };
     grid_arrive(ctrl, bar_target);                                             // B2 (arrive): q written
-    const int adim = quad * 32 + lane;     // this thread's attention dim = its TMEM lane
+    const int adim = quad * 32 + lane;     // this thread's attention dim
     float pm_next[8];                      // processed-memory values of the thread's next chunk of 8 positions (software pipeline)
     auto load_pm = [&](const float* pmr, int j0, int cnt) {
 #pragma unroll
@@ -830,7 +821,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     if (att_cta) {
       att_im2col_mma_tr(0);
       stage_memory_rows(0, smem_rows);     // everything the context needs is in flight before the q barrier
-      load_pm(p.pm + (long)att_b * T * kAtt + adim, cg * 8, min(T, 256));
+      load_pm(p.pm + (long)att_b * T * kAtt + adim, cg * 8, min(T, kAttRound));
     }
     T2_PROF(15);
     grid_wait(ctrl, bar_target);                                               // B2 (wait): q complete
@@ -844,11 +835,8 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         const float qd = s_q[adim], vd = s_v[adim];
         const int nrounds = att_rounds;
         for (int r0 = 0; r0 < nrounds; ++r0) {
-          const int jbase = r0 * 256, cnt = min(T - jbase, 256), nch = (((cnt + 15) & ~15) >> 3);
+          const int jbase = r0 * kAttRound, cnt = min(T - jbase, kAttRound), nch = (cnt + 7) >> 3;
           if (r0 > 0) att_im2col_mma_tr(r0);
-          mbar_wait(rg.acc, rg.acc_phase, ctrl, 203);
-          rg.acc_phase ^= 1;
-          ptx::tc_fence_after();
           T2_PROF(16);
           // energies e_j = sum_d v_d tanh(q_d + pa_dj + pm_jd): this thread adds dim d = adim for the 8 positions of
           // each of its chunks, then the 32 dims of the warp are summed with a transpose-reduce (9 shuffles per 8
@@ -863,7 +851,11 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
             for (int e = 0; e < 8; ++e) pm8[e] = pm_next[e];
             if (c + 4 < nch) load_pm(pmr, j0 + 32, cnt);           // next chunk's loads fly during this chunk's tanh
             float g[8], sv[8];
-            ptx::tmem_ld8(t_lane + kColAtt + j0, g);
+            {
+              const float4 g0 = *reinterpret_cast<const float4*>(s_pa + adim * kPaPitch + j0);
+              const float4 g1 = *reinterpret_cast<const float4*>(s_pa + adim * kPaPitch + j0 + 4);
+              g[0] = g0.x; g[1] = g0.y; g[2] = g0.z; g[3] = g0.w; g[4] = g1.x; g[5] = g1.y; g[6] = g1.z; g[7] = g1.w;
+            }
 #pragma unroll
             for (int e = 0; e < 8; ++e) sv[e] = vd * tanh_fast(qd + g[e] + pm8[e]);
             float r4[4], r2[2], r1;
@@ -893,7 +885,6 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
             const int jj = j0 + ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
             if ((lane & 3) == 0 && jj < cnt) s_ep[quad * eN + jbase + jj] = r1;
           }
-          ptx::tc_fence_before();
           __syncthreads();
           T2_PROF(17);
         }
@@ -925,7 +916,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       T2_PROF(18);
       {                                                           // context = aw . memory  model.py:83-84
         const int c4 = tid & 63, jg = tid >> 6;                   // 64 float4 = this CTA's 256 columns; 8 j-groups
-        const float4* ms = reinterpret_cast<const float4*>(rg.stage0 + img_bytes);
+        const float4* ms = reinterpret_cast<const float4*>(rg.stage0 + img_bytes + kPaBytes);
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 4
         for (int j = jg; j < smem_rows; j += 8) {
@@ -961,10 +952,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     T2_PROF(6);
     // ======== E2: ctx_t -> dec gates (rest), next att gates, projection (part); epilogue -> dh_t
     {
-      run_event(rg, plan.ev[2], p.ctx_img, p.wimg, 8, tmem_base, ctrl, &plan.ev[3]);
+      run_event(rg, plan.ev[2], p.ctx_img, p.wimg, 8, s_acc, ctrl, &plan.ev[3]);
       T2_PROF(7);
       float g[8];
-      T2_TAKE_GATES(kColD, kND, g);
+      T2_TAKE_GATES(kColD, g);
       if (erow) {
         float hv[2], sg[4][2];
 #pragma unroll
@@ -996,25 +987,20 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     }
     // ======== E3: dh_t -> projection (rest), next dec gates (part); epilogue -> mel, gate, x1
     {
-      run_event(rg, plan.ev[3], p.dh_img, p.wimg, 16, tmem_base, ctrl,
+      run_event(rg, plan.ev[3], p.dh_img, p.wimg, 16, s_acc, ctrl,
                 (!p.infer && t + 1 < p.cap) ? &plan.ev[0] : nullptr,    // INFER: the loop may end after this step
                 p.chunk_ready ? ctrl->dh_count : nullptr, 8u * (unsigned int)(t + 1));
       T2_PROF(10);
       if (tid == 0) *s_live = 0;
       float g[8];
-      if (has_p && cg == 0) acc_take8(t_lane, kColS, kNS, 0, g);
-      if (has_p && cg == 0 && is_lo) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s_xch[row * kXchStride + i] = g[i];
-      }
-      ptx::tc_fence_before();
-      __syncthreads();
+      if (has_p && cg == 0 && !is_lo) acc_take8(s_acc, row, kColS, 0, g);
+      __syncthreads();                                                         // s_live is reset before anyone counts
       if (has_p && cg == 0 && erow) {
         const int pc0 = (cta - kPCta0) * 8;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int pc = pc0 + j;
-          const float v = g[j] + s_xch[row * kXchStride + j] + s_bias_p[j];
+          const float v = g[j] + s_bias_p[j];
           if (pc < kMel) {
             p.mel[((long)row * p.cap + t) * kMel + pc] = v;                    // model.py:375-376
           } else if (pc == kMel) {
@@ -1055,7 +1041,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       if (has_x2) {
         stop |= wait_counter(&ctrl->x1_count, (unsigned int)(kPCtas * (t + 1)), s_flag, ctrl, 102);
         if (!stop) {
-          run_event(rg, plan.ev[4], p.x1_img, p.wimg, 4, tmem_base, ctrl, nullptr);    // E4: x1 -> x2_(t+1)  model.py:97-100
+          run_event(rg, plan.ev[4], p.x1_img, p.wimg, 4, s_acc, ctrl, nullptr);    // E4: x1 -> x2_(t+1)  model.py:97-100
           x2_epilogue();
         }
         signal_counter(&ctrl->x2_count, 1u + (stop ? kStopFlag : 0u));
@@ -1087,9 +1073,6 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     __syncthreads();
     ptx::cluster_sync_all();
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) ptx::tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 }  // namespace
@@ -1100,17 +1083,17 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
 static size_t persistent_smem_bytes(int T, int nstages) {
   const int TP = T + kLocK - 1;
   const int ntiles = (T + 127) / 128;
-  const size_t xch = (size_t)kRows * kXchStride * 4, att = (size_t)5 * ntiles * 128 * 4;   // one shared region
-  return (size_t)nstages * kStageBytes + kWeffBytes + 16 * 8 + 16 + 16 + 2 * 32 * 4 + kAtt * 4 + kAtt * 4 + 32 * 4 +
-         kRows * 4 + 32 + 24 * 8 + 2 * (size_t)((TP + 3) & ~3) * 4 + (xch > att ? xch : att) + 1024;
+  const size_t att = (size_t)5 * ntiles * 128 * 4;      // attention weights + energy partial sums
+  return (size_t)nstages * kStageBytes + kWeffBytes + kAccBytes + 16 * 8 + 16 + 2 * 32 * 4 + kAtt * 4 + kAtt * 4 + 32 * 4 +
+         kRows * 4 + 32 + 24 * 8 + 2 * (size_t)((TP + 3) & ~3) * 4 + att + 1024;
 }
 constexpr size_t kSmemLimit = 227 * 1024;
-// 5 ring stages when they fit beside the T_enc-dependent attention state (T_enc <~ 330), else 4
+// 4 ring stages when they fit beside the T_enc-dependent attention state (T_enc <~ 680 on sm_90's 227 KiB), else 3
 static int persistent_stages(int T) {
-  int want = 4;                 // 5 stages measured no faster than 4 on B200 (profiles/r02_decoder_ab.md): default 4
+  int want = 4;
   const char* e = getenv("T2_STAGES");
   if (e && atoi(e) >= 3 && atoi(e) <= kMaxStages) want = atoi(e);
-  while (want > 4 && persistent_smem_bytes(T, want) > kSmemLimit) --want;
+  while (want > 3 && persistent_smem_bytes(T, want) > kSmemLimit) --want;
   return want;
 }
 
@@ -1125,7 +1108,7 @@ size_t persistent_ws_bytes(int B, int T, int cap) {
 bool persistent_supported(const T2Model* m, const T2DecoderArgs* a) {
   if (!m->pk) return false;
   if (m->sm_count < kG) return false;
-  if (persistent_smem_bytes(a->T_enc, 4) > kSmemLimit) return false;
+  if (persistent_smem_bytes(a->T_enc, 3) > kSmemLimit) return false;
   return true;
 }
 
@@ -1307,10 +1290,8 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
   const size_t smem = persistent_smem_bytes(T, p.nstages);
   T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-  // TMA multicast of the activation chunks over clusters (T2_CLUSTER = 2 / 4 / 8) is implemented and
-  // validated, but measured slower than independent fetches on B200 (53.8 vs 55.1 / 56.0 us per step for
-  // cluster 1 / 2 / 4, same box): the stream is latency bound, not L2-bandwidth bound, and the multicast
-  // couples the 4 rings of a cluster in lock step.  Default: no cluster.
+  // TMA multicast of the activation chunks over clusters (T2_CLUSTER = 2 / 4 / 8): the stream is latency bound,
+  // not L2-bandwidth bound, and the multicast couples the rings of a cluster in lock step.  Default: no cluster.
   int want = 1;
   {
     const char* e = getenv("T2_CLUSTER");
@@ -1318,9 +1299,8 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
     if (want != 1 && want != 2 && want != 4 && want != 8) want = 1;
   }
   {
-    // the hierarchical (cluster barrier + 1 poller per cluster) variant measured slower than the flat
-    // 128-way barrier on B200 (profiles/r01_decoder_v10_ncu_summary.md) and is not combined with the
-    // split-phase B2 barrier: kept in the source for reference, always off
+    // the hierarchical (cluster barrier + 1 poller per cluster) variant is not combined with the split-phase B2
+    // barrier: kept in the source for reference, always off
     p.hier_barrier = 0;
   }
   cudaLaunchConfig_t cfg;
@@ -1361,60 +1341,33 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
 
 #ifdef T2_SELFTEST
 // ---------------------------------------------------------------------------------------------
-// self test of the tcgen05 engine: C (64 x N) = 2 * A (64 x K) . W (N x K)^T with the same run_event()
-// (two accumulating passes over the ring) and the same hi/lo accumulator read-out as the decoder.
+// self test of the wgmma event engine: C (64 x N) = 2 * A (64 x K) . W (N x K)^T with the same run_event()
+// (two accumulating passes over the ring) and the same accumulator tile as the decoder.
 // ---------------------------------------------------------------------------------------------
 namespace {
 __global__ void __launch_bounds__(kThreads, 1)
 selftest_kernel(const uint8_t* x_img, const uint8_t* w_img, EventPlan ep, int chunks, float* C, int N,
                 DecoderCtrl* ctrl) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   uint8_t* sp = smem_raw;
   Ring rg;
   rg.stage0 = sp; sp += kStages * kStageBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sp); sp += 16 * sizeof(uint64_t);
-  rg.full = bars; rg.empty = bars + kStages; rg.acc = bars + 2 * kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sp); sp += 16;
-  float* s_xch = reinterpret_cast<float*>(sp);                 // [64][80]
-  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = rg.acc_phase = 0;
+  rg.full = bars; rg.empty = bars + kStages;
+  float* s_acc = reinterpret_cast<float*>(sp);                 // [64][kAccPitch]
+  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pol_x = rg.pol_w = ptx::policy_evict_last();
   rg.cs = 1; rg.rank = 0; rg.pre = 0; rg.ns = kStages;
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], 1); }
-    ptx::mbar_init(rg.acc, 1);
+    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<kTmemCols>(tmem_slot);
-  ptx::tc_fence_before();
+  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int quad = warp & 3, cg = warp >> 2;
-  const uint32_t t_lane = tmem_base + ((uint32_t)(quad * 32) << 16);
-  for (int c = cg * 40; c < cg * 40 + 40; c += 8) ptx::tmem_zero8(t_lane + c);
-  ptx::tmem_wait_st();
-  ptx::tc_fence_before();
-  __syncthreads();
-  run_event(rg, ep, x_img, w_img, chunks, tmem_base, ctrl, &ep);      // second pass uses the prefetched weights
-  ptx::tc_fence_before();
-  __syncthreads();
-  run_event(rg, ep, x_img, w_img, chunks, tmem_base, ctrl, nullptr);
-  const int row = (quad & 1) * 32 + lane;
-  float g[kHiCols / 8][8];
-  for (int c0 = cg * 8; c0 < N; c0 += 8 * (kWarps / 4)) {
-    acc_take8(t_lane, 0, N, c0, g[c0 / 32]);
-    if (quad >= 2)
-      for (int j = 0; j < 8; ++j) s_xch[row * kHiCols + c0 + j] = g[c0 / 32][j];
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (quad < 2)
-    for (int c0 = cg * 8; c0 < N; c0 += 8 * (kWarps / 4))
-      for (int j = 0; j < 8; ++j) C[row * N + c0 + j] = g[c0 / 32][j] + s_xch[row * kHiCols + c0 + j];
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) ptx::tmem_dealloc<kTmemCols>(tmem_base);
+  run_event(rg, ep, x_img, w_img, chunks, s_acc, ctrl, &ep);      // second pass uses the prefetched weights
+  run_event(rg, ep, x_img, w_img, chunks, s_acc, ctrl, nullptr);
+  for (int i = tid; i < kRows * N; i += kThreads) C[i] = s_acc[(i / N) * kAccPitch + i % N];
 }
 }  // namespace
 
@@ -1434,7 +1387,7 @@ int selftest_umma(const float* A, const float* W, int N, int K, int passes, floa
   T2_LAUNCH_CHECK();
   pack_rows_image_kernel<<<chunks, 256, 0, s>>>(W, N, K, wimg);
   T2_LAUNCH_CHECK();
-  const size_t smem = (size_t)kStages * kStageBytes + 16 * 8 + 16 + (size_t)kRows * kHiCols * 4 + 64;
+  const size_t smem = (size_t)kStages * kStageBytes + 16 * 8 + kAccBytes;
   T2_CUDA(cudaFuncSetAttribute(selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   selftest_kernel<<<1, kThreads, smem, s>>>(ximg, wimg, ep, chunks, C, N, ctrl);
   T2_LAUNCH_CHECK();
@@ -1451,8 +1404,8 @@ int selftest_umma(const float* A, const float* W, int N, int K, int passes, floa
 //   P[split][b][col] = inv_scale[b] * sum_{n in the split's chunks} dG_scaled[b][n] * Wcat[n][col]
 // dG (64 x 4096) arrives as a split-fp16 activation image whose rows were scaled by a power of two
 // (row maximum in [0.5, 1): gradients span many orders of magnitude, fp16 does not); Wcat = [W_ih | W_hh]
-// is streamed as W^T images (rows = output columns, K = gate rows).  Same ring / MMA / accumulator read-out
-// as the forward events (run_event): M = 128 stacked [X_hi ; X_lo], one MMA per 16-wide K step.
+// is streamed as W^T images (rows = output columns, K = gate rows).  Same ring / MMA / accumulator tile
+// as the forward events (run_event): the output columns are cut into <= 32-column slices, one per MMA warpgroup.
 // ---------------------------------------------------------------------------------------------
 namespace {
 constexpr int kBwdTileB = 80, kBwdTileE = 64;       // output columns per CTA: 2560 = 32 x 80, 1792 = 28 x 64
@@ -1482,64 +1435,32 @@ __global__ void __launch_bounds__(kThreads, 1)
 bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w_img, const BwdCta* __restrict__ plans,
                 const float* __restrict__ inv_scale, float* __restrict__ P, int ldp, DecoderCtrl* ctrl) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   const BwdCta pc = plans[blockIdx.x];
   uint8_t* sp = smem_raw;
   Ring rg;
   rg.stage0 = sp; sp += kStages * kStageBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sp); sp += 16 * sizeof(uint64_t);
-  rg.full = bars; rg.empty = bars + kStages; rg.acc = bars + 2 * kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sp); sp += 16;
-  float* s_xch = reinterpret_cast<float*>(sp);                 // [64][80]
-  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = rg.acc_phase = 0;
+  rg.full = bars; rg.empty = bars + kStages;
+  float* s_acc = reinterpret_cast<float*>(sp);                 // [64][kAccPitch]
+  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pol_x = ptx::policy_evict_last(); rg.pol_w = ptx::policy_evict_first();
   rg.cs = 1; rg.rank = 0; rg.pre = 0; rg.ns = kStages;
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], 1); }
-    ptx::mbar_init(rg.acc, 1);
+    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<kTmemCols>(tmem_slot);
-  ptx::tc_fence_before();
+  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int quad = warp & 3, cg = warp >> 2;
-  const uint32_t t_lane = tmem_base + ((uint32_t)(quad * 32) << 16);
-  for (int c = cg * 40; c < cg * 40 + 40; c += 8) ptx::tmem_zero8(t_lane + c);
-  ptx::tmem_wait_st();
-  ptx::tc_fence_before();
-  __syncthreads();
-  run_event(rg, pc.ep, x_img + (size_t)pc.chunk0 * kXChunkBytes, w_img, pc.nchunks, tmem_base, ctrl, nullptr);
+  run_event(rg, pc.ep, x_img + (size_t)pc.chunk0 * kXChunkBytes, w_img, pc.nchunks, s_acc, ctrl, nullptr);
   const int N = pc.ep.nrows;
-  const int row = (quad & 1) * 32 + lane;
-  float g[kHiCols / 32 + 1][8];
-  for (int c0 = cg * 8; c0 < N; c0 += 8 * (kWarps / 4)) {
-    acc_take8(t_lane, 0, N, c0, g[c0 / 32]);
-    if (quad >= 2)
-      for (int j = 0; j < 8; ++j) s_xch[row * kHiCols + c0 + j] = g[c0 / 32][j];
+  for (int i = tid; i < kRows * N; i += kThreads) {
+    const int row = i / N, c = i - row * N;
+    P[((size_t)pc.split * kRows + row) * ldp + pc.col0 + c] = s_acc[row * kAccPitch + c] * inv_scale[row];
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (quad < 2) {
-    const float sc = inv_scale[row];
-    float* out = P + ((size_t)pc.split * kRows + row) * ldp + pc.col0;
-    for (int c0 = cg * 8; c0 < N; c0 += 8 * (kWarps / 4)) {
-      float4 v0, v1;
-      v0.x = (g[c0 / 32][0] + s_xch[row * kHiCols + c0 + 0]) * sc; v0.y = (g[c0 / 32][1] + s_xch[row * kHiCols + c0 + 1]) * sc;
-      v0.z = (g[c0 / 32][2] + s_xch[row * kHiCols + c0 + 2]) * sc; v0.w = (g[c0 / 32][3] + s_xch[row * kHiCols + c0 + 3]) * sc;
-      v1.x = (g[c0 / 32][4] + s_xch[row * kHiCols + c0 + 4]) * sc; v1.y = (g[c0 / 32][5] + s_xch[row * kHiCols + c0 + 5]) * sc;
-      v1.z = (g[c0 / 32][6] + s_xch[row * kHiCols + c0 + 6]) * sc; v1.w = (g[c0 / 32][7] + s_xch[row * kHiCols + c0 + 7]) * sc;
-      *reinterpret_cast<float4*>(out + c0) = v0;
-      *reinterpret_cast<float4*>(out + c0 + 4) = v1;
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) ptx::tmem_dealloc<kTmemCols>(tmem_base);
 }
 
-size_t bwd_gemm_smem() { return (size_t)kStages * kStageBytes + 16 * 8 + 16 + (size_t)kRows * kHiCols * 4 + 64; }
+size_t bwd_gemm_smem() { return (size_t)kStages * kStageBytes + 16 * 8 + kAccBytes; }
 }  // namespace
 
 int bwd_gemm_ctas(int which) { return which == 0 ? (2560 / kBwdTileB) * kBwdGemmSplit : (1792 / kBwdTileE) * kBwdGemmSplit; }

@@ -1,4 +1,4 @@
-// General fp32-grade GEMM of the training path on the tensor cores (tcgen05, split fp16), replacing every plain
+// General fp32-grade GEMM of the training path on the tensor cores (wgmma, split fp16), replacing every plain
 // library GEMM (cuBLAS sgemm) the backward pass used in round 1:
 //
 //     C (M x N, row-major, ldc) = op(A) . op(B) + beta * C        ta: A is stored (K x M), tb: B is stored (N x K)
@@ -7,10 +7,10 @@
 // op(B)^T from global memory (coalesced along whichever dimension is contiguous), multiplies every row of op(A) / column
 // of op(B) by a power of two derived from its largest magnitude over K (a pre-pass; gradients span many orders of
 // magnitude, fp16 does not), splits x = hi + lo into two fp16 planes and writes them as K-major SWIZZLE_128B operand
-// images into shared memory (double buffered).  One thread issues hi.hi + lo.hi + hi.lo per 16-wide K step into a
-// 128 x 128 fp32 accumulator in tensor memory.  Long accumulation chains in TMEM lose accuracy (DESIGN.md section 4), so
-// every K chunk is its own chain (hi.hi and the cross terms in separate accumulators), drained into fp32 registers
-// (64 per thread) while the tensor pipe works on the next chunk.  Small-tile /
+// images into shared memory (double buffered).  Two warpgroups issue hi.hi + lo.hi + hi.lo per 16-wide K step, each into
+// 64 x 128 fp32 register accumulators.  Long accumulation chains on the tensor cores lose accuracy (DESIGN.md section 4),
+// so every K chunk is its own chain (hi.hi and the cross terms in separate accumulators), added to fp32 running sums
+// (64 per thread) once the chunk's MMAs completed.  Small-tile /
 // large-K shapes (the time-batched weight gradients: K = T x B = 51,200) are split along K over CTAs; the partial tiles
 // are added in a fixed order by a reduce kernel (bit-reproducible).
 #include <stdlib.h>
@@ -164,20 +164,19 @@ __device__ __forceinline__ void tile_store(const float (&v)[4][8], bool kc, int 
   }
 }
 
-// Shared memory: [2 operand buffers x 64 KiB][transposing stage 33 KiB][mbarriers, TMEM slot]; the epilogue's output tile
-// reuses the operand buffers.  TMEM: 4 accumulators of 128 columns, [chunk parity][hi.hi | cross terms]: one accumulation
-// chain = ONE K chunk (4 hi.hi MMAs in one accumulator, 8 cross-term MMAs in the other), drained into fp32 registers two
-// chunks later while the tensor pipe works on the other parity -- the tensor core's accumulator update truncates, so the
-// error grows with the chain length: 4 / 8 accumulations per chain keep the result at fp32 sgemm quality (~1e-7).
-constexpr int kTmemColsG = 512;
-constexpr int kSmemG = 2 * kBufBytes + kStageBytesG + 256;
+// Shared memory: [2 operand buffers x 64 KiB][transposing stage 33 KiB]; the epilogue's output tile reuses the operand
+// buffers.  Warpgroup w (threads 128 w ..) owns rows [64 w, 64 w + 64) of the tile: per K chunk it issues hi.hi into one
+// register accumulator and the cross terms (lo.hi, hi.lo) into another (4 / 8 wgmma of 64 x 128 x 16), waits for them
+// and adds both to its fp32 running sums -- one accumulation chain = ONE K chunk: the tensor core's accumulator update
+// truncates, so the error grows with the chain length; 4 / 8 accumulations per chain keep the result at fp32 sgemm
+// quality (~1e-7).  The operand buffers are double buffered, so one CTA-wide barrier per chunk orders the next chunk's
+// stores after the MMAs that read the same buffer two chunks earlier.
+constexpr int kSmemG = 2 * kBufBytes + kStageBytesG;
 
 __global__ void __launch_bounds__(kThreadsG, 1) gemm_tc_kernel(const GemmP p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   float* stage = reinterpret_cast<float*>(smem_raw + 2 * kBufBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + 2 * kBufBytes + kStageBytesG);
-  uint32_t& tmem_slot = *reinterpret_cast<uint32_t*>(smem_raw + 2 * kBufBytes + kStageBytesG + 64);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
   const int bz = blockIdx.z, batch = bz / p.splits, split = bz - batch * p.splits;
   const int m0 = blockIdx.y * kBM, n0 = blockIdx.x * kBN;
   const float* A = p.A + (long)batch * p.sA;
@@ -185,83 +184,55 @@ __global__ void __launch_bounds__(kThreadsG, 1) gemm_tc_kernel(const GemmP p) {
   const int nchunks = (p.K + kBK - 1) / kBK;
   const int c0 = split * p.chunks_per_split, c1 = min(nchunks, c0 + p.chunks_per_split);
   const bool a_kc = !p.ta, b_kc = p.tb != 0;
-
-  if (tid == 0) { ptx::mbar_init(&bars[0], 1); ptx::mbar_init(&bars[1], 1); ptx::fence_barrier_init(); }
-  if (warp == 0) ptx::tmem_alloc<kTmemColsG>(&tmem_slot);
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const int quad = warp & 3, chalf = warp >> 2;                    // TMEM lane quadrant (hardware: warp % 4), column half
-  const uint32_t t_lane = tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(chalf * 64);
   float acc[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
-  // adds the two accumulators of chain `it` (chunk parity it & 1) to the registers, after its MMAs completed
-  auto drain = [&](int it) {
-    const int par = it & 1;
-    while (!ptx::mbar_try_wait(&bars[par], (uint32_t)((it >> 1) & 1))) {}
-    ptx::tc_fence_after();
-#pragma unroll
-    for (int c = 0; c < 64; c += 8) {
-      float g[8], h[8];
-      ptx::tmem_ld8(t_lane + (uint32_t)(par * 256) + c, g);
-      ptx::tmem_ld8(t_lane + (uint32_t)(par * 256 + 128) + c, h);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) acc[c + i] += g[i] + h[i];
-    }
-    ptx::tc_fence_before();
-  };
-
   int it = 0;
   for (int c = c0; c < c1; ++c, ++it) {
-    const int buf = it & 1;
-    uint8_t* sb = smem_raw + buf * kBufBytes;
-    float va[4][8], vb[4][8];
-    tile_fetch(A, p.lda, a_kc, m0, c * kBK, p.M, p.K, va);         // both operands' loads in flight during the drain below
-    tile_fetch(B, p.ldb, b_kc, n0, c * kBK, p.N, p.K, vb);
-    if (it >= 2) drain(it - 2);             // chain it-2 read this operand buffer and wrote this accumulator parity
-    tile_store(va, a_kc, m0, p.M, p.amax, stage, reinterpret_cast<__half*>(sb), reinterpret_cast<__half*>(sb + kPlane));
-    tile_store(vb, b_kc, n0, p.N, p.bmax, stage, reinterpret_cast<__half*>(sb + 2 * kPlane), reinterpret_cast<__half*>(sb + 3 * kPlane));
+    uint8_t* sb = smem_raw + (it & 1) * kBufBytes;
+    {
+      float va[4][8], vb[4][8];
+      tile_fetch(A, p.lda, a_kc, m0, c * kBK, p.M, p.K, va);       // both operands' loads in flight together
+      tile_fetch(B, p.ldb, b_kc, n0, c * kBK, p.N, p.K, vb);
+      tile_store(va, a_kc, m0, p.M, p.amax, stage, reinterpret_cast<__half*>(sb), reinterpret_cast<__half*>(sb + kPlane));
+      tile_store(vb, b_kc, n0, p.N, p.bmax, stage, reinterpret_cast<__half*>(sb + 2 * kPlane), reinterpret_cast<__half*>(sb + 3 * kPlane));
+    }
     ptx::fence_proxy_async();
     __syncthreads();
-    if (tid == 0) {
-      ptx::tc_fence_after();
-      const uint32_t a_hi = ptx::smem_u32(sb), a_lo = a_hi + kPlane, b_hi = a_hi + 2 * kPlane, b_lo = a_hi + 3 * kPlane;
-      const uint32_t idesc = ptx::make_idesc_f16(kBM, kBN);
-      const uint32_t d_hh = tmem + (uint32_t)(buf * 256), d_x = d_hh + 128;
+    const uint32_t a_hi = ptx::smem_u32(sb) + (uint32_t)wg * (64 * 128), a_lo = a_hi + kPlane;
+    const uint32_t b_hi = ptx::smem_u32(sb) + 2 * kPlane, b_lo = b_hi + kPlane;
+    float dh[64], dx[64];
 #pragma unroll
-      for (int kk = 0; kk < kBK / 16; ++kk) {
-        const uint64_t dah = ptx::make_sw128_desc(a_hi + kk * 32), dal = ptx::make_sw128_desc(a_lo + kk * 32);
-        const uint64_t dbh = ptx::make_sw128_desc(b_hi + kk * 32), dbl = ptx::make_sw128_desc(b_lo + kk * 32);
-        ptx::umma_f16(d_hh, dah, dbh, idesc, kk > 0 ? 1u : 0u);
-        ptx::umma_f16(d_x, dal, dbh, idesc, kk > 0 ? 1u : 0u);
-        ptx::umma_f16(d_x, dah, dbl, idesc, 1u);
-      }
-      ptx::umma_commit(&bars[buf]);
+    for (int i = 0; i < 64; ++i) { dh[i] = 0.f; dx[i] = 0.f; }
+    ptx::wg_fence_regs<64>(dh);
+    ptx::wg_fence_regs<64>(dx);
+    ptx::wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < kBK / 16; ++kk) {
+      const uint64_t dah = ptx::make_sw128_desc(a_hi + kk * 32), dal = ptx::make_sw128_desc(a_lo + kk * 32);
+      const uint64_t dbh = ptx::make_sw128_desc(b_hi + kk * 32), dbl = ptx::make_sw128_desc(b_lo + kk * 32);
+      ptx::wgmma_f16<kBN>(dh, dah, dbh);
+      ptx::wgmma_f16<kBN>(dx, dal, dbh);
+      ptx::wgmma_f16<kBN>(dx, dah, dbl);
     }
+    ptx::wg_commit();
+    ptx::wg_wait<0>();
+    ptx::wg_fence_regs<64>(dh);
+    ptx::wg_fence_regs<64>(dx);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] += dh[i] + dx[i];
   }
-  if (it >= 2) drain(it - 2);
-  if (it >= 1) drain(it - 1);
   __syncthreads();                          // every MMA is complete: the operand buffers become the output tile
 
   // ---- epilogue: undo the scales, transpose through shared memory, coalesced stores -----------------------------------
   float* tile = reinterpret_cast<float*>(smem_raw);                 // [128][kStagePitch]
-  {
-    const int r = quad * 32 + lane, m = m0 + r;
-    const float ia = (m < p.M) ? 1.f / scale_of(p.amax[m]) : 0.f;
-    float* trow = tile + r * kStagePitch + chalf * 64;
 #pragma unroll
-    for (int j = 0; j < 64; j += 4) {
-      const int n = n0 + chalf * 64 + j;
-      float4 v;
-      v.x = acc[j + 0] * (ia / scale_of(n + 0 < p.N ? p.bmax[n + 0] : 0u));
-      v.y = acc[j + 1] * (ia / scale_of(n + 1 < p.N ? p.bmax[n + 1] : 0u));
-      v.z = acc[j + 2] * (ia / scale_of(n + 2 < p.N ? p.bmax[n + 2] : 0u));
-      v.w = acc[j + 3] * (ia / scale_of(n + 3 < p.N ? p.bmax[n + 3] : 0u));
-      *reinterpret_cast<float4*>(trow + j) = v;
-    }
+  for (int i = 0; i < 64; ++i) {
+    const int r = wg * 64 + ptx::wg_frag_row(i, wt), col = ptx::wg_frag_col(i, wt);
+    const int m = m0 + r, n = n0 + col;
+    const float ia = (m < p.M) ? 1.f / scale_of(p.amax[m]) : 0.f;
+    tile[r * kStagePitch + col] = acc[i] * (ia / scale_of(n < p.N ? p.bmax[n] : 0u));
   }
   __syncthreads();
   if (p.part) {                             // partial tile of this K split: contiguous 128 x 128
@@ -296,9 +267,6 @@ __global__ void __launch_bounds__(kThreadsG, 1) gemm_tc_kernel(const GemmP p) {
       }
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc<kTmemColsG>(tmem);
 }
 
 // C = beta C + sum over the K splits of the partial tiles, fixed order
@@ -373,8 +341,9 @@ int gemm_tc(T2Model* m, cudaStream_t s, const GemmTc& g) {
   const int ntm = (g.M + kBM - 1) / kBM, ntn = (g.N + kBN - 1) / kBN, nchunks = (g.K + kBK - 1) / kBK;
   const long tiles = (long)ntm * ntn * batch;
   int splits = 1;
-  if (tiles < 120 && nchunks >= 8) {         // fill one wave of CTAs (1 CTA / SM: 161 KiB of shared memory)
-    splits = tiles <= 74 ? (int)(148 / tiles) : 2;
+  const int sms = m->sm_count > 0 ? m->sm_count : 132;
+  if (tiles * 5 < sms * 4 && nchunks >= 8) {   // fill one wave of CTAs (1 CTA / SM: 161 KiB of shared memory)
+    splits = tiles <= sms / 2 ? (int)(sms / tiles) : 2;
     if (splits > nchunks / 4) splits = nchunks / 4;
     if (splits < 1) splits = 1;
   }

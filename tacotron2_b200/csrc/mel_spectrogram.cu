@@ -9,7 +9,7 @@
 //                        -> mel_basis (n_mel, cutoff) x magnitudes: second GEMM                     (layers.py:78)
 //                        -> log(clamp(., clip_val)), written as (B, n_mel, n_frames)                (layers.py:79, audio_processing.py:78-84)
 //
-// Both products run on gemm_tc.cu (split-fp16 tcgen05, fp32-grade).
+// Both products run on gemm_tc.cu (split-fp16 wgmma, fp32-grade).
 #include "gemm_tc.h"
 
 namespace t2 {

@@ -1,114 +1,120 @@
-// Micro-benchmark of tcgen05.mma issue / execution cost on shared-memory-resident operands (no streaming):
-// cycles for R back-to-back MMAs (kind::f16, fp32 accumulate), measured by the issuing thread from the
-// first issue to the completion of the final tcgen05.commit.  Drives the design notes in DESIGN.md.
+// Micro-benchmark of wgmma issue / execution cost on shared-memory-resident operands (no streaming):
+// cycles for R back-to-back MMAs (m64nNk16, fp16 operands, fp32 accumulate) issued by one warpgroup, measured
+// by its first thread from the first issue to the completion of the final commit group.  Drives the design notes
+// in DESIGN.md.
 #include "common.cuh"
 #include "umma.cuh"
 
 namespace t2 {
 namespace {
 
-__global__ void __launch_bounds__(128, 1)
-mma_rate_kernel(int M, int N, int reps, int alternate_d, int a_in_tmem, long long* out) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  // operands: A 128 rows x 64 k, B 256 rows x 64 k (SWIZZLE_128B images), contents irrelevant (finite)
-  for (int i = tid; i < (128 + 256) * 64; i += 128) reinterpret_cast<__half*>(smem)[i] = __float2half(0.001f * (i & 63));
-  if (tid == 0) { ptx::mbar_init(&bar, 1); ptx::fence_barrier_init(); }
-  if (warp == 0) ptx::tmem_alloc<512>(&tmem_slot);
+// operands: A 128 rows x 64 k, B 256 rows x 64 k (SWIZZLE_128B images), contents irrelevant (finite)
+__device__ __forceinline__ void fill_operands(uint8_t* smem) {
+  for (int i = threadIdx.x; i < (128 + 256) * 64; i += 128) reinterpret_cast<__half*>(smem)[i] = __float2half(0.001f * (i & 63));
   ptx::fence_proxy_async();
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  if (tid == 0) {
-    const uint32_t as = ptx::smem_u32(smem), bs = as + 128 * 128;
-    const uint32_t idesc = ptx::make_idesc_f16(M, N);
-    long long t0 = clock64();
-    for (int r = 0; r < reps; ++r) {
-      const int kk = r & 3;
-      const uint64_t a = ptx::make_sw128_desc(as + kk * 32);
-      const uint64_t b = ptx::make_sw128_desc(bs + kk * 32);
-      const uint32_t d = tmem + ((alternate_d && (r & 1)) ? 256 : 0);
-      ptx::umma_f16(d, a, b, idesc, r > 1 ? 1u : 0u);
-    }
-    long long t1 = clock64();
-    ptx::umma_commit(&bar);
-    while (!ptx::mbar_try_wait(&bar, 0)) {}
-    long long t2 = clock64();
+}
+
+template <int N>
+__device__ __forceinline__ void keep_alive(const float* d, long long* out) {
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) s += d[i];
+  if (s == 1234.5f) out[1] = -1;     // never true for these operands; keeps the MMAs from being optimised away
+}
+
+template <int N>
+__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int reps, int alternate_d, long long* out) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  fill_operands(smem);
+  const uint32_t as = ptx::smem_u32(smem), bs = as + 128 * 128;
+  float d0[N / 2], d1[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+  ptx::wg_fence_regs<N / 2>(d0);
+  ptx::wg_fence_regs<N / 2>(d1);
+  ptx::wg_fence();
+  const long long t0 = clock64();
+  for (int r = 0; r < reps; ++r) {
+    const int kk = r & 3;
+    const uint64_t a = ptx::make_sw128_desc(as + kk * 32), b = ptx::make_sw128_desc(bs + kk * 32);
+    if (alternate_d && (r & 1)) ptx::wgmma_f16<N>(d1, a, b);
+    else ptx::wgmma_f16<N>(d0, a, b);
+  }
+  const long long t1 = clock64();
+  ptx::wg_commit();
+  ptx::wg_wait<0>();
+  ptx::wg_fence_regs<N / 2>(d0);
+  ptx::wg_fence_regs<N / 2>(d1);
+  const long long t2 = clock64();
+  if (threadIdx.x == 0) {
     out[0] = t1 - t0;   // issue time
     out[1] = t2 - t0;   // issue + drain
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc<512>(tmem);
+  keep_alive<N>(d0, out);
+  keep_alive<N>(d1, out);
 }
 
-// groups of `group` MMAs, each group followed by tcgen05.commit + a wait for its completion (what one K chunk of a
-// streaming event does): out[0] = cycles for `reps` groups, i.e. the cost of a COLD group incl. the commit round trip
-__global__ void __launch_bounds__(128, 1)
-mma_group_kernel(int M, int N, int group, int reps, long long* out) {
+// groups of `group` MMAs, each group followed by a commit + a wait for its completion (what one K chunk of a
+// streaming event does): out[0] = cycles for `reps` groups, i.e. the cost of a COLD group incl. the wait round trip
+template <int N>
+__global__ void __launch_bounds__(128, 1) mma_group_kernel(int group, int reps, long long* out) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  for (int i = tid; i < (128 + 256) * 64; i += 128) reinterpret_cast<__half*>(smem)[i] = __float2half(0.001f * (i & 63));
-  if (tid == 0) { ptx::mbar_init(&bar, 1); ptx::fence_barrier_init(); }
-  if (warp == 0) ptx::tmem_alloc<512>(&tmem_slot);
-  ptx::fence_proxy_async();
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  if (tid == 0) {
-    const uint32_t as = ptx::smem_u32(smem), bs = as + 128 * 128;
-    const uint32_t idesc = ptx::make_idesc_f16(M, N);
-    uint32_t phase = 0;
-    long long t0 = clock64();
-    for (int r = 0; r < reps; ++r) {
-      for (int g = 0; g < group; ++g) {
-        const int kk = g & 3;
-        ptx::umma_f16(tmem, ptx::make_sw128_desc(as + kk * 32), ptx::make_sw128_desc(bs + kk * 32), idesc, (r | g) ? 1u : 0u);
-      }
-      ptx::umma_commit(&bar);
-      while (!ptx::mbar_try_wait(&bar, phase)) {}
-      phase ^= 1;
+  fill_operands(smem);
+  const uint32_t as = ptx::smem_u32(smem), bs = as + 128 * 128;
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  ptx::wg_fence_regs<N / 2>(d);
+  const long long t0 = clock64();
+  for (int r = 0; r < reps; ++r) {
+    ptx::wg_fence();
+    for (int g = 0; g < group; ++g) {
+      const int kk = g & 3;
+      ptx::wgmma_f16<N>(d, ptx::make_sw128_desc(as + kk * 32), ptx::make_sw128_desc(bs + kk * 32));
     }
+    ptx::wg_commit();
+    ptx::wg_wait<0>();
+    ptx::wg_fence_regs<N / 2>(d);
+  }
+  if (threadIdx.x == 0) {
     out[0] = clock64() - t0;
     out[1] = 0;
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc<512>(tmem);
+  keep_alive<N>(d, out);
+}
+
+constexpr size_t kBenchSmem = (128 + 256) * 128 + 1024;
+
+int run_bench(void (*k)(int, int, long long*), int a0, int a1, long long* out_host, cudaStream_t s) {
+  long long* d = nullptr;
+  T2_CUDA(cudaMalloc((void**)&d, 16));
+  T2_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBenchSmem));
+  k<<<1, 128, kBenchSmem, s>>>(a0, a1, d);
+  T2_LAUNCH_CHECK();
+  T2_CUDA(cudaStreamSynchronize(s));
+  T2_CUDA(cudaMemcpy(out_host, d, 16, cudaMemcpyDeviceToHost));
+  cudaFree(d);
+  return T2_OK;
 }
 
 }  // namespace
 
+// M is the warpgroup's 64 rows; N in {32, 64, 128}
 int mma_group(int M, int N, int group, int reps, long long* out_host, cudaStream_t s) {
-  long long* d = nullptr;
-  T2_CUDA(cudaMalloc((void**)&d, 16));
-  const size_t smem = (128 + 256) * 128 + 1024;
-  T2_CUDA(cudaFuncSetAttribute(mma_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  mma_group_kernel<<<1, 128, smem, s>>>(M, N, group, reps, d);
-  T2_LAUNCH_CHECK();
-  T2_CUDA(cudaStreamSynchronize(s));
-  T2_CUDA(cudaMemcpy(out_host, d, 16, cudaMemcpyDeviceToHost));
-  cudaFree(d);
-  return T2_OK;
+  if (M != 64) return fail(T2_ERR_INVALID, "mma_group: M must be 64 (one warpgroup)");
+  if (N == 32) return run_bench(mma_group_kernel<32>, group, reps, out_host, s);
+  if (N == 64) return run_bench(mma_group_kernel<64>, group, reps, out_host, s);
+  if (N == 128) return run_bench(mma_group_kernel<128>, group, reps, out_host, s);
+  return fail(T2_ERR_INVALID, "mma_group: N in {32, 64, 128}");
 }
 
 int mma_rate(int M, int N, int reps, int alternate_d, long long* out_host, cudaStream_t s) {
-  long long* d = nullptr;
-  T2_CUDA(cudaMalloc((void**)&d, 16));
-  const size_t smem = (128 + 256) * 128 + 1024;
-  T2_CUDA(cudaFuncSetAttribute(mma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  mma_rate_kernel<<<1, 128, smem, s>>>(M, N, reps, alternate_d, 0, d);
-  T2_LAUNCH_CHECK();
-  T2_CUDA(cudaStreamSynchronize(s));
-  T2_CUDA(cudaMemcpy(out_host, d, 16, cudaMemcpyDeviceToHost));
-  cudaFree(d);
-  return T2_OK;
+  if (M != 64) return fail(T2_ERR_INVALID, "mma_rate: M must be 64 (one warpgroup)");
+  if (N == 32) return run_bench(mma_rate_kernel<32>, reps, alternate_d, out_host, s);
+  if (N == 64) return run_bench(mma_rate_kernel<64>, reps, alternate_d, out_host, s);
+  if (N == 128) return run_bench(mma_rate_kernel<128>, reps, alternate_d, out_host, s);
+  return fail(T2_ERR_INVALID, "mma_rate: N in {32, 64, 128}");
 }
 
 }  // namespace t2

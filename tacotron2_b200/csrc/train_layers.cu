@@ -332,7 +332,7 @@ int tc_train_conv(T2Model* m, const float* xp, int cin, const uint8_t* wimg, int
   return tc_conv(c, s);
 }
 
-// ---- conv weight gradient on the tcgen05 engine (wgrad_tc.cu) ---------------------------------------------------------
+// ---- conv weight gradient on the wgmma engine (wgrad_tc.cu) ---------------------------------------------------------
 // dW_k[co][ci] = sum_r G_z[r][co] X[r + k - 2][ci]: K = padded rows in chunks of 64, A = G_z^T images (per-channel power-of-two
 // scale), B = X^T images, one set per tap (source rows shifted by k - 2), 128 x 256 tiles, K splits reduced in a fixed order.
 struct WgConvWs { uint8_t* img_a; uint8_t* img_b; float* part; float* stat; float* scale; float* inv; float* colsum; WgJob* jobs; };
@@ -455,7 +455,7 @@ int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
   T2_LAUNCH_CHECK();
   if (G[L.wbase + 3]) T2_CUDA(cudaMemcpyAsync(G[L.wbase + 3], sums, (size_t)L.cout * 4, cudaMemcpyDeviceToDevice, s));           // d beta
   if (G[L.wbase + 2]) T2_CUDA(cudaMemcpyAsync(G[L.wbase + 2], sums + L.cout, (size_t)L.cout * 4, cudaMemcpyDeviceToDevice, s));  // d gamma
-  if (wg) {   // weight + bias gradient on our tcgen05 engine
+  if (wg) {   // weight + bias gradient on our wgmma engine
     T2_TRY(conv_wgrad_tc(L, B, T, gz_p, xp, G[L.wbase], G[L.wbase + 1], *wg, s));
   } else {
     if (G[L.wbase + 1]) T2_TRY(colsum_rm(m, s, gz_p, L.cout, Mp, L.cout, G[L.wbase + 1]));      // d conv bias

@@ -1,5 +1,5 @@
-// sm_100a primitives used by the persistent decoder: mbarrier, bulk async copy (TMA engine,
-// SASS UBLKCP), tcgen05 (TMEM alloc / mma / commit / ld), descriptors.  Inline PTX only.
+// sm_90a primitives of the tensor-core kernels: mbarrier, bulk async copy (TMA engine, multicast over
+// clusters), wgmma (warpgroup MMA on shared-memory descriptors), descriptors.  Inline PTX only.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -38,10 +38,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ---- proxies / fences ---------------------------------------------------------------------------
-// generic-proxy writes (st.global / st.shared) -> async-proxy reads (bulk copies, tcgen05.mma)
+// generic-proxy writes (st.global / st.shared) -> async-proxy reads (bulk copies, wgmma)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---- bulk async copy global -> shared (1-D, contiguous; completion on an mbarrier) ----------------
 __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
@@ -98,112 +96,122 @@ __device__ __forceinline__ float4 ldg_f4_hint(const float* p, uint64_t policy) {
   return v;
 }
 
-// ---- tensor memory ------------------------------------------------------------------------------
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {   // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {     // the same warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, fp16 operands, fp32 accumulate; single thread issues
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// ---- cluster-scope mbarrier arrive (releases a stage that peers filled by multicast) --------------
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta_rank) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+      "r"(cta_rank)
       : "memory");
 }
-// all previously issued tcgen05.mma of this thread complete -> one arrive on the mbarrier
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// named barrier of `count` threads (whole warps), id 1..15 (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// the same, arriving on the mbarrier at this offset in every CTA of cta_mask (frees multicast-fed stages)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// TMEM -> registers: thread i of the warp reads lane (base_lane + i), 8 / 16 consecutive columns
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---- wgmma (warpgroup MMA, sm_90a) --------------------------------------------------------------
+// D (64 x N, fp32, registers of the 128 threads of a warpgroup) += A (64 x 16, smem desc) . B (N x 16, smem desc)^T,
+// fp16 operands, both K-major.  Accumulator fragment: thread t (warp w = t / 32 of the warpgroup, lane l) holds
+// d[i] = D[row][col] with row = 16 w + l / 4 + 8 ((i / 2) % 2), col = 8 (i / 4) + 2 (l % 4) + i % 2.
+// Callers zero the accumulators themselves (every MMA accumulates).
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across wgmma issue and wait
+template <int kRegs>
+__device__ __forceinline__ void wg_fence_regs(float* d) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < kRegs; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+__device__ __forceinline__ int wg_frag_row(int i, int lane_in_wg) { return ((lane_in_wg >> 5) << 4) + ((lane_in_wg & 31) >> 2) + (((i >> 1) & 1) << 3); }
+__device__ __forceinline__ int wg_frag_col(int i, int lane_in_wg) { return ((i >> 2) << 3) + ((lane_in_wg & 3) << 1) + (i & 1); }
 
-// split form: issue the load, do other work, then wait (the wait names the registers so no use is scheduled before it)
-__device__ __forceinline__ void tmem_ld8_issue(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t a_desc, uint64_t b_desc);
+template <>
+__device__ __forceinline__ void wgmma_f16<8>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0,%1,%2,%3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "l"(a_desc), "l"(b_desc));
 }
-__device__ __forceinline__ void tmem_ld8_wait(uint32_t (&r)[8]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7])::"memory");
+template <>
+__device__ __forceinline__ void wgmma_f16<16>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "l"(a_desc), "l"(b_desc));
 }
-
-// registers -> TMEM: zero 8 consecutive columns of this thread's lane
-__device__ __forceinline__ void tmem_zero8(uint32_t taddr) {
-  const uint32_t z = 0u;
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1};" ::"r"(taddr), "r"(z) : "memory");
+template <>
+__device__ __forceinline__ void wgmma_f16<24>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n24k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+               : "l"(a_desc), "l"(b_desc));
 }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+template <>
+__device__ __forceinline__ void wgmma_f16<32>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(a_desc), "l"(b_desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16<64>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(a_desc), "l"(b_desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16<80>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+               : "l"(a_desc), "l"(b_desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+               : "l"(a_desc), "l"(b_desc));
+}
 
 // ---- descriptors --------------------------------------------------------------------------------
 // shared-memory matrix descriptor, K-major, no swizzle ("interleaved" canonical layout):
 // core matrix = 8 rows x 16 bytes stored as 128 contiguous bytes; lbo = byte distance between core
-// matrices adjacent in K, sbo = byte distance between 8-row groups.  (cute::UMMA::SmemDescriptor)
+// matrices adjacent in K, sbo = byte distance between 8-row groups.  (cute GMMA K-major INTERLEAVE)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;   // descriptor version (Blackwell)
-  return d;                 // base_offset 0, lbo_mode 0, layout_type 0 = SWIZZLE_NONE
+  return d;                 // base_offset 0, layout_type 0 = no swizzle
 }
 // K-major SWIZZLE_128B descriptor: rows are 128 contiguous bytes (64 fp16 = one K chunk), 8-row atoms of
 // 1024 bytes, 16-byte units XOR-swizzled by the row index inside the atom; the atom base must be
-// 1024-byte aligned.  A 16-wide K step advances the start address by 32 bytes.  (cute::UMMA K-major B128)
+// 1024-byte aligned.  A 16-wide K step advances the start address by 32 bytes.  (cute GMMA K-major SW128)
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;                       // leading byte offset: unused for swizzled K-major (1)
   d |= (uint64_t)(1024u >> 4) << 32;            // stride byte offset between 8-row atoms
-  d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                       // layout type SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                       // layout type SWIZZLE_128B
   return d;
 }
-// instruction descriptor kind::f16: D fp32, A/B fp16, both K-major
-__device__ __forceinline__ uint32_t make_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-__device__ __forceinline__ uint32_t make_idesc_f16_m64(uint32_t N) { return make_idesc_f16(64, N); }
 
 }  // namespace ptx
 
 // ---- operand images ---------------------------------------------------------------------------------
 // A K-chunk (64 columns) of an operand with R rows is stored as two planes [hi][lo] of fp16, each in
-// the tcgen05 K-major SWIZZLE_128B layout: row r is 128 contiguous bytes, rows are grouped in 8-row
+// the wgmma K-major SWIZZLE_128B layout: row r is 128 contiguous bytes, rows are grouped in 8-row
 // atoms of 1024 bytes, and the 16-byte unit (k/8) of row r sits at unit position (k/8) ^ (r%8):
 //     byte(r, k) = (r/8)*1024 + (r%8)*128 + (((k/8) ^ (r%8)) * 16) + (k%8)*2
 // so one plane is R*128 bytes and one contiguous bulk copy brings the whole chunk into shared memory
-// ready for tcgen05.mma (atoms 1024-byte aligned in shared memory).
+// ready for wgmma (atoms 1024-byte aligned in shared memory).
 constexpr int kChunkK = 64;
 __host__ __device__ inline uint32_t img_elem_offset(int r, int k) {   // in fp16 elements within a plane
   return (uint32_t)((r >> 3) * 512 + (r & 7) * 64 + ((((k >> 3) ^ (r & 7)) & 7) * 8) + (k & 7));

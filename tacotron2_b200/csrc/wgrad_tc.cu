@@ -1,10 +1,11 @@
-// Time-batched weight gradients of the two decoder LSTMs on the tensor cores (tcgen05, split fp16):
+// Time-batched weight gradients of the two decoder LSTMs on the tensor cores (wgmma, split fp16):
 //     dW[g][k] = sum over all (t, b) of dG[t, b, g] * X[t, b, k]            (4096 x 1792 and 4096 x 2560, K = T x B)
 // One decoder step = one K chunk of 64 batch rows.  Both operands are turned into K-major SWIZZLE_128B operand
 // images once (rows = gates / input features, K = batch row of one step): dG^T scaled per gate row by a power of two
 // (max over all steps in [0.5, 1): gradients span many orders of magnitude, fp16 does not), X^T as is.  A CTA owns a
 // 128 (gates) x 256 (features) tile of one K split (kWgSeg steps), streams [A hi|lo 32 KB][B hi|lo 64 KB] stages and
-// issues hi.hi + hi.lo + lo.hi per 16-wide K step into a 128 x 256 fp32 TMEM accumulator; the K splits are added by a
+// issues hi.hi + hi.lo + lo.hi per 16-wide K step into 128 x 256 fp32 register accumulators (two warpgroups of 64 gate
+// rows each); the K splits are added by a
 // reduce kernel in a fixed order (bit-reproducible, and the accumulation chains stay short).
 // The column statistics pass also yields the bias gradients (column sums of dG).
 #include <stdlib.h>
@@ -25,7 +26,7 @@ constexpr int kABytes = 2 * kTM * 128;               // [hi | lo] planes of 128 
 constexpr int kBBytes = 2 * kTN * 128;               // 64 KB
 constexpr int kStageB = kABytes + kBBytes;           // 96 KB
 constexpr int kWgStages = 2;
-constexpr int kWgThreads = 192;                      // warp 0: producer, warp 1: MMA issuer, warps 2-5: epilogue
+constexpr int kWgThreads = 384;                      // warp 0: producer; warpgroups 1 / 2: MMA + epilogue
 constexpr int kStatSplit = 64;
 
 // ---- column statistics of dG (rows x 4096): max |.| and sum per column ---------------------------------
@@ -110,18 +111,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const WgJob* __
   const WgJob job = jobs[blockIdx.x];
   uint8_t* stage0 = smem_raw;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + kWgStages * kStageB);
-  uint64_t* full = bars; uint64_t* empty = bars + kWgStages; uint64_t* accb = bars + 2 * kWgStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* full = bars; uint64_t* empty = bars + kWgStages;
   if (tid == 0) {
-    for (int s = 0; s < kWgStages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 1); }
-    ptx::mbar_init(accb, 1);
+    for (int s = 0; s < kWgStages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 2); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<256>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   if (warp == 0) {
     if (lane == 0) {
       const uint64_t pol = ptx::policy_evict_last();     // tiles are shared by the concurrently resident CTAs (job order)
@@ -136,47 +131,48 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const WgJob* __
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = ptx::make_idesc_f16(kTM, kTN);
-      uint32_t s = 0, ph = 0;
-      for (int i = 0; i < job.nchunks; ++i) {
-        wg_wait(&full[s], ph);
-        ptx::tc_fence_after();
-        const uint32_t a_hi = ptx::smem_u32(stage0 + (size_t)s * kStageB), a_lo = a_hi + kTM * 128;
-        const uint32_t b_hi = a_hi + kABytes, b_lo = b_hi + kTN * 128;
+  } else if (tid >= 128) {
+    // warpgroup 1 / 2: gate rows [64 wg, 64 wg + 64) x all 256 feature columns (two 64 x 128 accumulators)
+    const int wg = (tid >> 7) - 1, wt = tid & 127;
+    float d0[64], d1[64];
 #pragma unroll
-        for (int kk = 0; kk < kChunkK / 16; ++kk) {
-          const uint64_t dah = ptx::make_sw128_desc(a_hi + kk * 32), dal = ptx::make_sw128_desc(a_lo + kk * 32);
-          const uint64_t dbh = ptx::make_sw128_desc(b_hi + kk * 32), dbl = ptx::make_sw128_desc(b_lo + kk * 32);
-          ptx::umma_f16(tmem, dah, dbh, idesc, (i > 0 || kk > 0) ? 1u : 0u);
-          ptx::umma_f16(tmem, dah, dbl, idesc, 1u);
-          ptx::umma_f16(tmem, dal, dbh, idesc, 1u);
-        }
-        ptx::umma_commit(&empty[s]);
-        if (++s == kWgStages) { s = 0; ph ^= 1; }
+    for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+    ptx::wg_fence_regs<64>(d0);
+    ptx::wg_fence_regs<64>(d1);
+    uint32_t s = 0, ph = 0;
+    for (int i = 0; i < job.nchunks; ++i) {
+      wg_wait(&full[s], ph);
+      const uint32_t a_hi = ptx::smem_u32(stage0 + (size_t)s * kStageB) + (uint32_t)wg * (64 * 128), a_lo = a_hi + kTM * 128;
+      const uint32_t b_hi = ptx::smem_u32(stage0 + (size_t)s * kStageB) + kABytes, b_lo = b_hi + kTN * 128;
+      ptx::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < kChunkK / 16; ++kk) {
+        const uint64_t dah = ptx::make_sw128_desc(a_hi + kk * 32), dal = ptx::make_sw128_desc(a_lo + kk * 32);
+        const uint64_t dbh0 = ptx::make_sw128_desc(b_hi + kk * 32), dbh1 = ptx::make_sw128_desc(b_hi + 128 * 128 + kk * 32);
+        const uint64_t dbl0 = ptx::make_sw128_desc(b_lo + kk * 32), dbl1 = ptx::make_sw128_desc(b_lo + 128 * 128 + kk * 32);
+        ptx::wgmma_f16<128>(d0, dah, dbh0);
+        ptx::wgmma_f16<128>(d1, dah, dbh1);
+        ptx::wgmma_f16<128>(d0, dah, dbl0);
+        ptx::wgmma_f16<128>(d1, dah, dbl1);
+        ptx::wgmma_f16<128>(d0, dal, dbh0);
+        ptx::wgmma_f16<128>(d1, dal, dbh1);
       }
-      ptx::umma_commit(accb);
+      ptx::wg_commit();
+      ptx::wg_wait<0>();
+      ptx::wg_fence_regs<64>(d0);
+      ptx::wg_fence_regs<64>(d1);
+      if (wt == 0) ptx::mbar_arrive(&empty[s]);          // this warpgroup's MMAs have read the stage
+      if (++s == kWgStages) { s = 0; ph ^= 1; }
     }
-    __syncwarp();
-  } else {
-    // epilogue: warp w reads TMEM lane quadrant w % 4 (rows quad*32 + lane), all 256 columns
-    wg_wait(accb, 0);
-    ptx::tc_fence_after();
-    const int quad = warp & 3, row = quad * 32 + lane;
-    const uint32_t t_lane = tmem + ((uint32_t)(quad * 32) << 16);
-    const float sc = job.inv_scale[row];
-    float* out = job.out + (size_t)row * job.ldo;
-    for (int c0 = 0; c0 < kTN; c0 += 8) {
-      float v[8];
-      ptx::tmem_ld8(t_lane + c0, v);
-      *reinterpret_cast<float4*>(out + c0) = make_float4(v[0] * sc, v[1] * sc, v[2] * sc, v[3] * sc);
-      *reinterpret_cast<float4*>(out + c0 + 4) = make_float4(v[4] * sc, v[5] * sc, v[6] * sc, v[7] * sc);
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int row = wg * 64 + ptx::wg_frag_row(i, wt), col = ptx::wg_frag_col(i, wt);
+      const float sc = job.inv_scale[row];
+      float* out = job.out + (size_t)row * job.ldo + col;
+      *reinterpret_cast<float2*>(out) = make_float2(d0[i] * sc, d0[i + 1] * sc);
+      *reinterpret_cast<float2*>(out + 128) = make_float2(d1[i] * sc, d1[i + 1] * sc);
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) ptx::tmem_dealloc<256>(tmem);
 }
 
 // partial sums (nsplit, 4096, ldc) -> the parameter gradients: columns [0, c_ih) -> W_ih (4096 x c_ih), the rest -> W_hh (4096 x 1024)

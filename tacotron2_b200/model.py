@@ -1,9 +1,9 @@
-"""The reference's nn.Module surface (model.py) over the B200 engine.
+"""The reference's nn.Module surface (model.py) over the H100 engine.
 
 Same class names, constructor signatures, attribute names, parameter registration order (hence the
 same ``state_dict`` keys AND the same random initialisation under a given torch seed) as
 NVIDIA/tacotron2 ``model.py`` -- so ``train.py`` / ``inference.ipynb`` / published checkpoints work
-unchanged -- but ``forward`` / ``inference`` run hand-written sm_100a kernels through libt2b200.so:
+unchanged -- but ``forward`` / ``inference`` run hand-written sm_90a kernels through libt2b200.so:
 
     Tacotron2.inference  (model.py:517-529)  -> encoder kernels -> persistent decoder kernel -> postnet
     Tacotron2.forward    (model.py:499-515)  -> encoder -> teacher-forced decoder -> postnet -> parse_output

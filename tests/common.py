@@ -116,3 +116,23 @@ def rel_err(a, b):
     a = a.detach().double().cpu(); b = b.detach().double().cpu()
     den = float(b.abs().max())
     return float((a - b).abs().max()) / (den if den > 0 else 1.0)
+
+
+def stft_inputs(seed=0, n=6000):
+    """A seeded 2-row test signal in [-1, 1]: two tones plus noise, and clipped noise."""
+    g = torch.Generator().manual_seed(seed)
+    t = torch.arange(n) / 22050.0
+    return torch.stack([0.3 * torch.sin(2 * math.pi * 220 * t) + 0.2 * torch.sin(2 * math.pi * 1870 * t) + 0.05 * torch.randn(n, generator=g),
+                        (0.5 * torch.randn(n, generator=g)).clamp(-1, 1)])
+
+
+def tensor_digest(t):
+    """dtype, shape and SHA-256 of the bytes of a CPU tensor: equal digests <=> bit-identical tensors."""
+    import hashlib
+    t = t.detach().contiguous().cpu()
+    return "%s %s %s" % (t.dtype, tuple(t.shape), hashlib.sha256(t.numpy().tobytes()).hexdigest())
+
+
+def sample_index(numel, n, seed):
+    """Seeded flat indices at which a large fixture tensor is stored (with its full-tensor statistics)."""
+    return torch.randint(0, numel, (min(n, numel),), generator=torch.Generator().manual_seed(seed))

@@ -36,16 +36,17 @@ def test_state_dict_layout_matches_reference_table():
 
 
 def test_same_seed_same_init_as_reference():
-    from oracle.ref_import import default_hparams, import_reference_model, reference_available
-    if not reference_available():
-        pytest.skip("reference tree not present")
-    ref = import_reference_model()
-    torch.manual_seed(1234)
-    a = ref.Tacotron2(default_hparams()).state_dict()
+    """Under torch.manual_seed(1234) every tensor of the state_dict is bit-identical to the reference's (dtype, shape and
+    SHA-256 of the bytes the reference produced, tests/golden/reference_live.npz, tools/make_golden.py live)."""
+    import numpy as np
+    from tests.common import GOLDEN_DIR, tensor_digest
+    gold = np.load(os.path.join(GOLDEN_DIR, "reference_live.npz"))
+    keys, digests = [str(k) for k in gold["sd/keys"]], [str(d) for d in gold["init1234/digest"]]
     torch.manual_seed(1234)
     b = t2.Tacotron2(t2.create_hparams()).state_dict()
-    for k in a:
-        assert torch.equal(a[k], b[k]), k
+    assert list(b.keys()) == keys
+    for k, d in zip(keys, digests):
+        assert tensor_digest(b[k]) == d, k
 
 
 def test_load_state_dict_roundtrip_and_attributes():
@@ -147,49 +148,36 @@ def test_ctypes_structs_match_c_layout(tmp_path):
 
 
 def test_text_mel_collate_matches_reference_semantics():
-    """tacotron2_b200.data_utils.TextMelCollate vs the reference's collate function (data_utils.py:67-111): executed live
-    when /root/reference is present, otherwise checked against its documented properties."""
-    import importlib.util
-    import types
+    """tacotron2_b200.data_utils.TextMelCollate vs the reference's collate function (data_utils.py:67-111): its documented
+    properties, and bit-equality (dtype, shape, SHA-256 of the bytes) with what the reference's TextMelCollate returned for
+    the same batches (tests/golden/reference_live.npz, tools/make_golden.py live; 20 random ragged batches per
+    n_frames_per_step with ties in the text lengths)."""
+    import numpy as np
     from tacotron2_b200.data_utils import TextMelCollate
+    from tests.common import GOLDEN_DIR, tensor_digest
+    gold = np.load(os.path.join(GOLDEN_DIR, "reference_live.npz"))["collate/digest"]
     g = torch.Generator().manual_seed(0)
-    batch = []
-    for n_text, n_mel in [(7, 13), (12, 5), (3, 21), (12, 9), (1, 1)]:
-        batch.append((torch.randint(1, 148, (n_text,), generator=g), torch.randn(80, n_mel, generator=g)))
+    fixed = [(torch.randint(1, 148, (n_text,), generator=g), torch.randn(80, n_mel, generator=g))
+             for n_text, n_mel in [(7, 13), (12, 5), (3, 21), (12, 9), (1, 1)]]
+    case = 0
     for nfs in (1, 2):
-        out = TextMelCollate(nfs)(batch)
-        text, tl, mel, gate, ol = out
-        assert tl.tolist() == sorted(tl.tolist(), reverse=True) and mel.shape[2] % nfs == 0 and mel.shape[2] >= int(ol.max())
-        for i in range(len(batch)):
-            assert int((text[i] != 0).sum()) == int(tl[i]) and bool((mel[i, :, int(ol[i]):] == 0).all())
-            assert gate[i].tolist() == [0.0] * (int(ol[i]) - 1) + [1.0] * (mel.shape[2] - int(ol[i]) + 1)
-        ref_path = "/root/reference/data_utils.py"
-        if not os.path.isfile(ref_path):
-            continue
-        saved = {k: sys.modules.get(k) for k in ("layers", "utils", "text", "librosa", "librosa.filters", "librosa.util",
-                                                 "stft", "audio_processing")}
-        try:
-            for k in ("layers", "utils", "text"):
-                sys.modules[k] = types.ModuleType(k)
-            sys.modules["utils"].load_wav_to_torch = sys.modules["utils"].load_filepaths_and_text = None
-            sys.modules["text"].text_to_sequence = None
-            spec = importlib.util.spec_from_file_location("t2_reference_data_utils", ref_path)
-            mod = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(mod)
-        finally:
-            for k, v in saved.items():
-                sys.modules.pop(k, None)
-                if v is not None:
-                    sys.modules[k] = v
-        ref = mod.TextMelCollate(nfs)(batch)
-        for a, b in zip(out, ref):
-            assert a.dtype == b.dtype and torch.equal(a, b)
-        for trial in range(20):                      # random ragged batches (ties in the text lengths included)
+        batches = [fixed]
+        for trial in range(20):
             n = int(torch.randint(1, 9, (1,), generator=g))
-            rb = [(torch.randint(1, 148, (int(torch.randint(1, 12, (1,), generator=g)),), generator=g),
-                   torch.randn(80, int(torch.randint(1, 30, (1,), generator=g)), generator=g)) for _ in range(n)]
-            for a, b in zip(TextMelCollate(nfs)(rb), mod.TextMelCollate(nfs)(rb)):
-                assert a.dtype == b.dtype and torch.equal(a, b)
+            batches.append([(torch.randint(1, 148, (int(torch.randint(1, 12, (1,), generator=g)),), generator=g),
+                             torch.randn(80, int(torch.randint(1, 30, (1,), generator=g)), generator=g)) for _ in range(n)])
+        for bi, batch in enumerate(batches):
+            out = TextMelCollate(nfs)(batch)
+            if bi == 0:
+                text, tl, mel, gate, ol = out
+                assert tl.tolist() == sorted(tl.tolist(), reverse=True) and mel.shape[2] % nfs == 0 and mel.shape[2] >= int(ol.max())
+                for i in range(len(batch)):
+                    assert int((text[i] != 0).sum()) == int(tl[i]) and bool((mel[i, :, int(ol[i]):] == 0).all())
+                    assert gate[i].tolist() == [0.0] * (int(ol[i]) - 1) + [1.0] * (mel.shape[2] - int(ol[i]) + 1)
+            assert len(out) == gold.shape[1]
+            for j, a in enumerate(out):
+                assert tensor_digest(a) == str(gold[case, j]), (nfs, bi, j)
+            case += 1
 
 
 def test_parse_batch_returns_the_reference_structure():
@@ -261,23 +249,23 @@ def test_engine_cache_key_and_invalidation():
 
 def test_bench_roofline_traffic_is_keyed_to_the_kernel_source(tmp_path, monkeypatch):
     """bench.py takes roofline.traffic from profiles/decoder_traffic.json only while decoder_persistent.cu still hashes to the
-    captured source; anything else gives None (never a stale literal)."""
+    captured source; anything else (a modified source, no capture at all) gives None (never a stale literal)."""
     import hashlib
     import json
     import bench
     src = open(os.path.join(ROOT, "tacotron2_b200", "csrc", "decoder_persistent.cu"), "rb").read()
-    rec = json.load(open(os.path.join(ROOT, "profiles", "decoder_traffic.json")))
-    val, why = bench.decoder_traffic()
-    if rec["source_sha16"] == hashlib.sha256(src).hexdigest()[:16]:
-        assert val == rec["dram_bytes_per_step"] and val > 1e6
-    else:
-        assert val is None and "stale" in why
-    # a modified source invalidates the record
+    rec = {"source_sha16": hashlib.sha256(src).hexdigest()[:16], "dram_bytes_per_step": 2.5e7, "capture": "test record"}
     fake = tmp_path / "repo"
     (fake / "profiles").mkdir(parents=True)
     (fake / "tacotron2_b200" / "csrc").mkdir(parents=True)
-    (fake / "profiles" / "decoder_traffic.json").write_text(json.dumps(rec))
-    (fake / "tacotron2_b200" / "csrc" / "decoder_persistent.cu").write_bytes(src + b"\n// edited\n")
+    (fake / "tacotron2_b200" / "csrc" / "decoder_persistent.cu").write_bytes(src)
     monkeypatch.setattr(bench, "ROOT", str(fake))
+    val, why = bench.decoder_traffic()
+    assert val is None and "unavailable" in why                    # no capture
+    (fake / "profiles" / "decoder_traffic.json").write_text(json.dumps(rec))
+    val, why = bench.decoder_traffic()
+    assert val == rec["dram_bytes_per_step"] and why == "test record"
+    # a modified source invalidates the record
+    (fake / "tacotron2_b200" / "csrc" / "decoder_persistent.cu").write_bytes(src + b"\n// edited\n")
     val, why = bench.decoder_traffic()
     assert val is None and "stale" in why

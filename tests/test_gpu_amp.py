@@ -1,4 +1,4 @@
-"""GPU (B200): the mixed-precision training flow (BASELINE.json configs[2] / [3] say "fp16": the reference trains through
+"""GPU (H100): the mixed-precision training flow (BASELINE.json configs[2] / [3] say "fp16": the reference trains through
 Apex AMP O2, train.py:173-176, 222-236) -- tacotron2_b200.amp + AmpFusedClipAdam (t2_amp_adam_step).
 
 (1) the optimizer step alone against torch: unscale -> clip_grad_norm_ on fp32 master gradients -> torch.optim.Adam ->

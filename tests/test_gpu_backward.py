@@ -1,4 +1,4 @@
-"""GPU (B200): gradients of the CUDA training path vs torch autograd through the CPU oracle (the oracle's
+"""GPU (H100): gradients of the CUDA training path vs torch autograd through the CPU oracle (the oracle's
 autograd is pinned against the reference's own autograd in tests/test_oracle_vs_reference.py and by
 tests/golden/grad_*.npz).  Same weights, inputs and dropout masks on both sides.
 
@@ -51,7 +51,7 @@ def oracle_decoder_grads(sd, memory, mels, lens, pk, ak, dk, d_mel, d_gate, d_al
 @pytest.mark.parametrize("B,Te,T,training,use_align", [(3, 19, 7, True, False), (5, 40, 12, True, True),
                                                        (4, 150, 9, False, False), (64, 33, 5, True, False)])
 def test_decoder_backward_vs_oracle_autograd(B, Te, T, training, use_align, gemm, monkeypatch):
-    """gemm = tc: the reverse recurrence's skinny GEMMs and the time-batched LSTM weight gradients on the tcgen05
+    """gemm = tc: the reverse recurrence's skinny GEMMs and the time-batched LSTM weight gradients on the wgmma
     split-fp16 engines (default); simt: fp32 SIMT kernels / plain cuBLAS fp32 GEMMs (cross-check)."""
     monkeypatch.setenv("T2_BWD_GEMM", gemm)
     monkeypatch.setenv("T2_WGRAD", "tc" if gemm == "tc" else "cublas")
@@ -199,7 +199,7 @@ def test_postnet_and_encoder_modules_backward_vs_oracle(B, T):
 
 def test_full_size_backward_tensor_core_vs_simt_gemms_and_determinism(monkeypatch):
     """B=64, T_enc=150 (the benchmark shape), 24 teacher-forced steps, Philox dropout: the gradients with the reverse
-    recurrence's GEMMs on the tcgen05 engine agree with the fp32 SIMT kernels, and two runs are bit-identical."""
+    recurrence's GEMMs on the wgmma engine agree with the fp32 SIMT kernels, and two runs are bit-identical."""
     torch.manual_seed(7)
     model = t2.Tacotron2(t2.create_hparams()).cuda().train()
     dec = model.decoder
@@ -231,7 +231,7 @@ def test_full_size_backward_tensor_core_vs_simt_gemms_and_determinism(monkeypatc
     diff = {n: rel_err(x, y) for n, x, y in zip(names, a, b) if not torch.equal(x, y)}
     assert not diff, "backward is not bit-reproducible: %s" % diff
     worst = max(rel_err(x, y) for x, y in zip(a, c))
-    print("full-size backward: tcgen05 vs SIMT GEMMs worst rel diff %.2e" % worst)
+    print("full-size backward: wgmma vs SIMT GEMMs worst rel diff %.2e" % worst)
     assert worst < 1e-4
 
 

@@ -1,4 +1,4 @@
-"""GPU (B200): the CUDA path through the public nn.Module API / C-ABI vs (a) the golden vectors
+"""GPU (H100): the CUDA path through the public nn.Module API / C-ABI vs (a) the golden vectors
 produced by the reference model.py and (b) the CPU oracle on fresh seeded inputs.
 
 Tolerance (north_star): mel frames within 1e-3 relative fp32 -- measured as max|a-b| / max|b| --
@@ -34,13 +34,13 @@ def test_native_library_is_loaded():
     L = _capi.lib()
     info = (C.c_int32 * 5)()
     _capi.check(L.t2_device_info(info))
-    assert info[1] == 10, "sm_100 device expected, got sm_%d%d" % (info[1], info[2])
+    assert (info[1], info[2]) == (9, 0), "sm_90 device expected, got sm_%d%d" % (info[1], info[2])
 
 
 @pytest.mark.parametrize("passes,tol", [(3, 2e-5), (1, 2e-3)])
 @pytest.mark.parametrize("N,K", [(32, 256), (8, 64), (64, 1024), (80, 192), (48, 1024)])
 def test_umma_split_gemm_selftest(N, K, passes, tol):
-    """tcgen05 engine of the persistent decoder: C = 2 * A (64xK) . W (NxK)^T (two accumulating runs)."""
+    """wgmma engine of the persistent decoder: C = 2 * A (64xK) . W (NxK)^T (two accumulating runs)."""
     g = torch.Generator().manual_seed(N * 1000 + K)
     A = torch.randn(64, K, generator=g).cuda()
     W = (torch.randn(N, K, generator=g) / K ** 0.5).cuda()
@@ -96,7 +96,7 @@ def test_teacher_forced_forward_matches_reference_golden(name, training, impl, i
 @pytest.mark.parametrize("B,T", [(5, 33), (12, 140)])
 def test_encoder_and_postnet_modules_vs_oracle(B, T, conv_impl, monkeypatch):
     """Encoder (conv stack + packed BiLSTM) and Postnet as stand-alone modules; both conv engines
-    (tcgen05 implicit GEMM and the fp32 SIMT path)."""
+    (wgmma implicit GEMM and the fp32 SIMT path)."""
     monkeypatch.setenv("T2_CONV_IMPL", conv_impl)
     sd = synth_state_dict(9, scale=1.5)
     model = make_model(sd)
@@ -248,7 +248,7 @@ GEMM_CASES = [
 
 @pytest.mark.parametrize("case", GEMM_CASES)
 def test_training_path_tensor_core_gemm_vs_fp64(case):
-    """gemm_tc.cu (the tcgen05 split-fp16 GEMM that replaced every cuBLAS sgemm of the training path) against torch fp64:
+    """gemm_tc.cu (the wgmma split-fp16 GEMM that replaced every cuBLAS sgemm of the training path) against torch fp64:
     fp32-grade accuracy (error <= 2e-5 of the result's maximum; cuBLAS fp32 lands at ~1e-6) for gradient-like operands
     many orders of magnitude below 1, rows of wildly different magnitude, unaligned / padded leading dimensions."""
     ta, tb, M, N, K, pa, pb, pc, beta, batch, sa, sb = case

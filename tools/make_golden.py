@@ -1,5 +1,5 @@
-"""Generates tests/golden/*.npz by executing the UNMODIFIED reference model.py (build container
-only -- needs /root/reference).  Run:  python tools/make_golden.py
+"""Generates tests/golden/*.npz by executing the UNMODIFIED reference model.py (needs a checkout of
+NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live]
 
 Every file holds the inputs' seeds, the reference outputs and a checksum of the synthetic weights
 (tests/common.synth_state_dict) so a drift of the generator is detected instead of silently
@@ -14,9 +14,10 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from oracle.ref_import import (MaskInjector, default_hparams, import_reference_model,  # noqa: E402
+from oracle.ref_import import (REFERENCE_DIR, MaskInjector, default_hparams, import_reference_model,  # noqa: E402
                                injected_dropout)
-from tests.common import GOLDEN_DIR, keep_mask, rand_text, synth_state_dict, weights_checksum  # noqa: E402
+from tests.common import (GOLDEN_DIR, keep_mask, rand_text, sample_index, stft_inputs,  # noqa: E402
+                          synth_state_dict, tensor_digest, weights_checksum)
 
 torch.set_num_threads(8)
 ref = import_reference_model()
@@ -258,14 +259,20 @@ def gate_targets(ol, T_mel):
     return gt
 
 
+def import_reference_loss():
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("ref_loss_function", os.path.join(REFERENCE_DIR, "loss_function.py"))
+    lf = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(lf)
+    return lf
+
+
 def grad_case(name, training, B, T_text, T_mel, wseed, seed, wscale=2.0, n_samples=96, keep_outputs=True,
               ref64=False):
     """Full training step of the REFERENCE (forward + Tacotron2Loss + backward, autograd) with injected dropout
     masks; the fixture keeps the loss and, per parameter, sum / abs-sum / max of the gradient plus 96 sampled entries."""
     import importlib.util
-    spec = importlib.util.spec_from_file_location("ref_loss_function", "/root/reference/loss_function.py")
-    lf = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(lf)
+    lf = import_reference_loss()
     sd = synth_state_dict(wseed, scale=wscale)
     g = torch.Generator().manual_seed(seed)
     text = rand_text(B, T_text, seed + 1)
@@ -349,25 +356,18 @@ def import_reference_stft():
     lu.pad_center, lu.tiny, lf.mel = pad_center, (lambda x: np.finfo(np.float32).tiny), None
     lib.util, lib.filters = lu, lf
     sys.modules.update({"librosa": lib, "librosa.util": lu, "librosa.filters": lf})
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, REFERENCE_DIR)
     try:
-        spec = importlib.util.spec_from_file_location("t2_reference_stft", "/root/reference/stft.py")
+        spec = importlib.util.spec_from_file_location("t2_reference_stft", os.path.join(REFERENCE_DIR, "stft.py"))
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
     finally:
-        sys.path.remove("/root/reference")
+        sys.path.remove(REFERENCE_DIR)
         for k, v in saved.items():
             sys.modules.pop(k, None)
             if v is not None:
                 sys.modules[k] = v
     return mod
-
-
-def stft_inputs(seed=0, n=6000):
-    g = torch.Generator().manual_seed(seed)
-    t = torch.arange(n) / 22050.0
-    return torch.stack([0.3 * torch.sin(2 * np.pi * 220 * t) + 0.2 * torch.sin(2 * np.pi * 1870 * t) + 0.05 * torch.randn(n, generator=g),
-                        (0.5 * torch.randn(n, generator=g)).clamp(-1, 1)])
 
 
 def stft_case():
@@ -379,7 +379,121 @@ def stft_case():
     save("stft_mag", y=y, mag=mag, basis_abs_sum=ref_stft.forward_basis.double().abs().sum())
 
 
+def import_reference_data_utils():
+    """The reference's data_utils.py with empty stand-ins for the modules only its dataset class needs."""
+    import importlib.util
+    import types
+    saved = {k: sys.modules.get(k) for k in ("layers", "utils", "text", "librosa", "librosa.filters", "librosa.util",
+                                             "stft", "audio_processing")}
+    try:
+        for k in ("layers", "utils", "text"):
+            sys.modules[k] = types.ModuleType(k)
+        sys.modules["utils"].load_wav_to_torch = sys.modules["utils"].load_filepaths_and_text = None
+        sys.modules["text"].text_to_sequence = None
+        spec = importlib.util.spec_from_file_location("t2_reference_data_utils", os.path.join(REFERENCE_DIR, "data_utils.py"))
+        mod = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(mod)
+    finally:
+        for k, v in saved.items():
+            sys.modules.pop(k, None)
+            if v is not None:
+                sys.modules[k] = v
+    return mod
+
+
+def collate_batches(nfs_list=(1, 2), trials=20):
+    """The text / mel batches of tests/test_boundary_cpu.py::test_text_mel_collate_matches_reference_semantics, in order:
+    per n_frames_per_step the fixed 5-row batch, then `trials` random ragged batches (ties in the text lengths included)."""
+    g = torch.Generator().manual_seed(0)
+    fixed = [(torch.randint(1, 148, (n_text,), generator=g), torch.randn(80, n_mel, generator=g))
+             for n_text, n_mel in [(7, 13), (12, 5), (3, 21), (12, 9), (1, 1)]]
+    out = []
+    for nfs in nfs_list:
+        out.append((nfs, fixed))
+        for _ in range(trials):
+            n = int(torch.randint(1, 9, (1,), generator=g))
+            out.append((nfs, [(torch.randint(1, 148, (int(torch.randint(1, 12, (1,), generator=g)),), generator=g),
+                               torch.randn(80, int(torch.randint(1, 30, (1,), generator=g)), generator=g)) for _ in range(n)]))
+    return out
+
+
+def reference_live_case():
+    """What tests/test_oracle_vs_reference.py and the collate test compare against, computed by the reference itself:
+    batched inference (B=1, 12 steps), the state_dict layout and seeded initialisation, a full training step's loss / gradients (sum, abs-sum, max,
+    sum of squares and 96 sampled entries per parameter), stft.STFT bases (sampled) and magnitudes for three filter / hop
+    settings, and TextMelCollate on the batches of collate_batches()."""
+    arrays = {}
+    # inference, B=1: model.inference with injected prenet masks
+    sd = synth_state_dict(5, gate_bias=-10.0, scale=2.0)
+    model = build(sd)
+    model.decoder.max_decoder_steps = 12
+    text = rand_text(1, 19, 3)
+    keep = keep_mask((12, 2, 1, 256), 0.5, 4)
+    masks = [keep[t, l].bool() for t in range(12) for l in range(2)]
+    with torch.no_grad(), injected_dropout(ref, MaskInjector(masks)):
+        r = model.inference(text)
+    for k, v in zip(("mel", "post", "gate", "align"), r):
+        arrays["infer/" + k] = v
+    # state_dict layout, and the initialisation under torch.manual_seed(1234) as SHA-256 digests of every tensor's bytes
+    torch.manual_seed(1234)
+    sdr = ref.Tacotron2(default_hparams()).state_dict()
+    arrays["init1234/digest"] = np.array([tensor_digest(v) for v in sdr.values()])
+    arrays["sd/keys"] = np.array(list(sdr.keys()))
+    arrays["sd/shapes"] = np.array([list(v.shape) + [0] * (4 - v.dim()) for v in sdr.values()], dtype=np.int64)
+    # training step (tests/test_oracle_vs_reference.py::test_reference_training_step_gradients_live)
+    lf = import_reference_loss()
+    B, T, Tm, seed = 3, 15, 8, 91
+    sd = synth_state_dict(4321, scale=2.0)
+    g = torch.Generator().manual_seed(seed)
+    text = rand_text(B, T, seed + 1)
+    tl = torch.sort(torch.randint(T // 3, T + 1, (B,), generator=g), descending=True)[0]
+    tl[0] = T
+    ol = torch.randint(Tm // 3, Tm + 1, (B,), generator=g)
+    ol[1] = Tm
+    mels = torch.randn(B, 80, Tm, generator=g)
+    gt = torch.zeros(B, Tm)
+    for i, n in enumerate(ol.tolist()):
+        mels[i, :, n:] = 0.0
+        gt[i, n - 1:] = 1.0
+    m = dict(pk=keep_mask((Tm + 1, 2, B, 256), 0.5, seed + 2), ak=keep_mask((Tm, B, 1024), 0.1, seed + 3),
+             dk=keep_mask((Tm, B, 1024), 0.1, seed + 4), ek=keep_mask((3, B, 512, T), 0.5, seed + 5),
+             qk4=keep_mask((4, B, 512, Tm), 0.5, seed + 6), qk1=keep_mask((B, 80, Tm), 0.5, seed + 7))
+    model = build(sd, True)
+    masks = [m["ek"][i].bool() for i in range(3)] + [m["pk"][:, 0].bool(), m["pk"][:, 1].bool()]
+    for t in range(Tm):
+        masks += [m["ak"][t].bool(), m["dk"][t].bool()]
+    masks += [m["qk4"][i].bool() for i in range(4)] + [m["qk1"].bool()]
+    with injected_dropout(ref, MaskInjector(masks)):
+        out = model((text, tl, mels, int(tl.max()), ol))
+    loss = lf.Tacotron2Loss()(out, (mels, gt))
+    loss.backward()
+    arrays["train/loss"] = loss.detach()
+    for k, p_ in model.named_parameters():
+        gr = p_.grad.detach().double().reshape(-1)
+        idx = grad_sample_index(k, gr.numel())
+        arrays["train/g/" + k] = torch.cat((torch.stack((gr.sum(), gr.abs().sum(), gr.abs().max(), (gr * gr).sum())), gr[idx]))
+    # stft.STFT
+    mod = import_reference_stft()
+    for fl, hop, win in ((1024, 256, 1024), (800, 200, 800), (512, 128, 400)):
+        st = mod.STFT(fl, hop, win)
+        y = stft_inputs(seed=fl, n=5000)
+        mag, _ = st.transform(y)
+        for name, v in (("basis", st.forward_basis[:, 0, :]), ("mag", mag)):
+            v = v.detach().double().reshape(-1)
+            arrays["stft/%d/%s_shape" % (fl, name)] = np.array((st.forward_basis[:, 0, :] if name == "basis" else mag).shape)
+            arrays["stft/%d/%s_sample" % (fl, name)] = v[sample_index(v.numel(), 2048, fl)]
+            arrays["stft/%d/%s_stats" % (fl, name)] = torch.stack((v.sum(), v.abs().sum(), (v * v).sum(), v.abs().max()))
+    # TextMelCollate
+    du = import_reference_data_utils()
+    arrays["collate/digest"] = np.array([[tensor_digest(v) for v in du.TextMelCollate(nfs)(batch)]
+                                         for nfs, batch in collate_batches()])
+    save("reference_live", **arrays)
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "live":
+        reference_live_case()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "stft":
         stft_case()
         sys.exit(0)

@@ -45,6 +45,7 @@ def main():
                "dram_bytes_per_launch": dram, "dram_bytes_per_step": dram / steps, "duration": "%s %s" % dur,
                "capture": "ncu --set full --clock-control none, %s (%d decoder steps in the launch); %s" % (os.path.basename(rep), steps, os.path.basename(out_md))}
     if kernel == "decoder_persistent_kernel":
+        os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
         json.dump(traffic, open(os.path.join(ROOT, "profiles", "decoder_traffic.json"), "w"), indent=1)
     with open(out_md, "a") as f:
         f.write("\n".join(lines) + "\n\nDRAM traffic %.3f GB per launch = %.2f MB per decoder step (%d steps).\n" % (dram / 1e9, dram / steps / 1e6, steps))

@@ -1,8 +1,8 @@
 """Precision study (build-container tool, not product): how do reduced-precision GEMM operands
 propagate through the autoregressive decoder recurrence?  Uses the oracle's ``mm`` hook to
 round operands before an fp32-accumulated matmul.  Drives DESIGN.md section "precision"."""
-import sys, torch
-sys.path.insert(0, '/root/repo')
+import os, sys, torch
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import tacotron2_oracle as O
 from oracle.ref_import import default_hparams, import_reference_model
 
