@@ -345,6 +345,11 @@ int    t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_
 #ifdef T2_SELFTEST
 int t2_selftest_umma(const float* A, const float* W, int32_t N, int32_t K, int32_t passes,
                      float* C, void* stream);
+/* t2_selftest_event: the same engine on an event plan given as its consumers' row counts (consumers_host[0..n_consumers),
+ * host memory; 1-3 consumers of 8, 16, 24 or 32 rows): C (64 x N) = 2 A (64 x K) . W (N x K)^T with N the sum of
+ * the rows, W's rows in consumer order, K a multiple of 64 up to 1024. */
+int t2_selftest_event(const float* A, const float* W, const int32_t* consumers_host, int32_t n_consumers, int32_t K,
+                      float* C, void* stream);
 /* Micro-benchmark: SM cycles for `reps` back-to-back wgmma of one warpgroup (M = 64, N in {32, 64, 128}, K = 16, fp16,
  * operands resident in shared memory) -> out_host[0] = issue cycles, out_host[1] = issue + completion cycles. */
 int t2_selftest_mma_rate(int32_t M, int32_t N, int32_t reps, int32_t alternate_d, int64_t* out_host);

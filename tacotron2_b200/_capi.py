@@ -203,7 +203,7 @@ def lib():
 
 
 SELFTEST_LIB_PATH = os.path.join(_HERE, "libt2b200_selftest.so")
-SELFTEST_EXPORTS = ["t2_selftest_umma", "t2_selftest_mma_rate", "t2_selftest_mma_group", "t2_selftest_gemm_tc", "t2_selftest_colsum"]
+SELFTEST_EXPORTS = ["t2_selftest_umma", "t2_selftest_event", "t2_selftest_mma_rate", "t2_selftest_mma_group", "t2_selftest_gemm_tc", "t2_selftest_colsum"]
 _selftest_lib = None
 
 
@@ -216,6 +216,8 @@ def selftest_lib():
         L = C.CDLL(SELFTEST_LIB_PATH)
         L.t2_last_error.restype = C.c_char_p
         L.t2_selftest_umma.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        L.t2_selftest_event.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p,
+                                        C.c_void_p]
         L.t2_selftest_mma_rate.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]
         L.t2_selftest_mma_group.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]
         L.t2_selftest_gemm_tc.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,

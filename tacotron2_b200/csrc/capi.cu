@@ -33,6 +33,7 @@ size_t encoder_ws_bytes(int B, int T);
 int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s);
 size_t postnet_ws_bytes(int B, int T);
 int selftest_umma(const float* A, const float* W, int N, int K, int passes, float* C, cudaStream_t s);
+int selftest_event(const float* A, const float* W, const int* cons, int ncons, int K, float* C, cudaStream_t s);
 int mma_rate(int M, int N, int reps, int alternate_d, long long* out_host, cudaStream_t s);
 int mma_group(int M, int N, int group, int reps, long long* out_host, cudaStream_t s);
 
@@ -402,6 +403,11 @@ int t2_selftest_mma_group(int32_t M, int32_t N, int32_t group, int32_t reps, int
 
 int t2_selftest_umma(const float* A, const float* W, int32_t N, int32_t K, int32_t passes, float* C, void* stream) {
   return selftest_umma(A, W, N, K, passes, C, (cudaStream_t)stream);
+}
+
+int t2_selftest_event(const float* A, const float* W, const int32_t* consumers, int32_t n_consumers, int32_t K, float* C,
+                      void* stream) {
+  return selftest_event(A, W, consumers, n_consumers, K, C, (cudaStream_t)stream);
 }
 
 // C = op(A) . op(B) + beta C through the training path's tensor-core GEMM (gemm_tc.cu); batch > 1: strided batch

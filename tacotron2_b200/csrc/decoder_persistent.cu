@@ -7,7 +7,7 @@
 //   * "activation driven" schedule: whenever a new activation block (x2, ah, ctx, dh, x1) is complete,
 //     every CTA streams it ONCE through a shared-memory ring (bulk async copies on the TMA engine; the
 //     activation chunk is multicast to the CTAs of a cluster) together with the slices of every weight
-//     matrix that consumes it, and three warpgroups issue wgmma (one consumer slice each):
+//     matrix that consumes it, and three warpgroups issue wgmma:
 //        x2_t  -> att gates += W_ih^a[:, :256] x2                          -> ah_t, ac_t
 //        ah_t  -> dec gates += W_ih^d[:, :1024] ah ; att gates(t+1) += W_hh^a ah ; q = W_q ah
 //        ctx_t -> dec gates += W_ih^d[:, 1024:] ctx ; att gates(t+1) += W_ih^a[:, 256:] ctx ;
@@ -18,12 +18,14 @@
 //     NEXT step is computed from [dh; ctx] directly (model.py:97-100, 373-378, 449).
 //   * fp32-grade arithmetic on fp16 tensor cores: every operand is split x = hi + lo (two fp16).  The
 //     activation chunk image is [X_hi rows 0-63 | X_lo rows 64-127]; the weight rows of all consumers of
-//     an event are concatenated as [W_hi ; W_lo] per consumer.  A warpgroup owns a slice of <= 32 weight
-//     rows of one consumer and accumulates all four partial products (hi.hi, lo.hi, hi.lo, lo.lo) of the
-//     whole event in one 64 x n fp32 register accumulator (4 wgmma m64nNk16 per 16-wide K step):
-//        D[64 x n] += X_hi . W_hi^T + X_lo . W_hi^T + X_hi . W_lo^T + X_lo . W_lo^T
-//     and adds it to the shared-memory accumulator tile once the event's last chunk is in.  Accumulators
-//     are always accumulated into and zeroed by the epilogue that consumed them.
+//     an event are concatenated as [W_hi ; W_lo] per consumer.  All four partial products (hi.hi, lo.hi,
+//     hi.lo, lo.lo) are kept.  Warpgroup 1 + c owns consumer c (<= 32 rows) and takes its [W_hi ; W_lo]
+//     rows as ONE wide B operand (N = 2n), so a 16-wide K step is two wgmma m64n(2n)k16 instead of four
+//     m64nnk16, and each X plane is read once per consumer and K step:
+//        D[64 x 2n] += X_hi . [W_hi ; W_lo]^T + X_lo . [W_hi ; W_lo]^T
+//     At the end of the event the warpgroup adds the W_hi and W_lo column halves of D and adds the sum to
+//     the shared-memory accumulator tile.  Accumulators are always accumulated into and zeroed by the
+//     epilogue that consumed them.
 //   * location-sensitive attention (model.py:43-86): location conv + dense are fused into one 62-tap
 //     filter bank evaluated as a tensor-core GEMM over an im2col image of the previous / cumulative
 //     weights (kept in shared memory across steps); energies, softmax and context per batch row on a
@@ -360,28 +362,85 @@ __device__ __forceinline__ void prefetch_weights(Ring& rg, const EventPlan& nx, 
   rg.pre = n;
 }
 
-// One warpgroup's slice of an event: `m` (<= 32) weight rows starting at hi-plane row `wrow` of a consumer with
-// `n` hi rows (its lo rows start n rows later), accumulated over every K chunk of the event.
-template <int M>
-__device__ __forceinline__ void event_mma(float* d, uint32_t xs, uint32_t w_hi, uint32_t w_lo) {
-  ptx::wg_fence();
-#pragma unroll
-  for (int kk = 0; kk < kChunkK / 16; ++kk) {
-    const uint64_t a_hi = ptx::make_sw128_desc(xs + kk * 32), a_lo = ptx::make_sw128_desc(xs + kRows * 128 + kk * 32);
-    const uint64_t b_hi = ptx::make_sw128_desc(w_hi + kk * 32), b_lo = ptx::make_sw128_desc(w_lo + kk * 32);
-    ptx::wgmma_f16<M>(d, a_hi, b_hi);
-    ptx::wgmma_f16<M>(d, a_lo, b_hi);
-    ptx::wgmma_f16<M>(d, a_hi, b_lo);
-    ptx::wgmma_f16<M>(d, a_lo, b_lo);
+// How the three MMA warpgroups split an event.  Each consumer's rows sit in the stage as [n hi rows | n lo rows], so
+// warpgroup 1 + c takes consumer c (n <= 32 rows) as ONE wgmma B operand of N = 2 n rows [W_hi; W_lo] and multiplies it
+// with A = X_hi and A = X_lo: two wgmma per 16-wide K step, each reading its activation plane and the consumer's rows
+// once (instead of four with separate hi / lo B operands, each re-reading an A plane).  N stays <= 64 (32 accumulator
+// registers): the kernel runs at the 128-register limit of 512 threads, and a wider accumulator spills.
+// all_widths = false: the consumer widths run_event<false> (decoder, backward GEMMs) is built for
+inline bool event_plan_fits(const EventPlan& ep, bool all_widths) {
+  if (ep.ncons < 1 || ep.ncons > kMmaWgs) return false;
+  for (int c = 0; c < ep.ncons; ++c)
+    if (ep.n[c] != 16 && ep.n[c] != 32 && !(all_widths && (ep.n[c] == 8 || ep.n[c] == 24))) return false;
+  return true;
+}
+// `rows` output rows of one matrix as consumers that fit the warpgroups: 32, 32, rest (rows <= 80, a multiple of 8)
+inline void plan_one_matrix(EventPlan& ep, int rows) {
+  ep.ncons = 0; ep.nrows = rows;
+  for (int r = rows; r > 0 && ep.ncons < 3; ) {
+    const int n = ep.ncons < 2 && r >= 32 ? 32 : r;
+    ep.n[ep.ncons++] = n; r -= n;
   }
-  ptx::wg_commit();
-  ptx::wg_wait<0>();
-  ptx::wg_fence_regs<M / 2>(d);
+  ep.w_bytes = (uint32_t)rows * 256;
+}
+// image rows of the hi and lo copies of row r (counted over all consumers) of a plan
+__device__ __forceinline__ void plan_image_rows(const EventPlan& ep, int r, int& hi, int& lo) {
+  int roff = 0;
+  for (int c = 0; c < ep.ncons; ++c) {
+    if (r < ep.n[c]) { hi = roff + r; lo = hi + ep.n[c]; return; }
+    r -= ep.n[c]; roff += 2 * ep.n[c];
+  }
+  hi = lo = 0;
+}
+
+__device__ __forceinline__ void release_stage(const Ring& rg, uint32_t s) {
+  // this warpgroup is done with the stage (in every CTA of the cluster: the stage was filled by multicast)
+  if (rg.cs == 1) ptx::mbar_arrive(&rg.empty[s]);
+  else for (uint32_t r = 0; r < rg.cs; ++r) ptx::mbar_arrive_cluster(&rg.empty[s], r);
+}
+
+// One MMA warpgroup's consumer of an event: D (64 x 2n) = X_hi . B^T + X_lo . B^T over all `chunks` stages, where B is
+// the consumer's 2n weight-image rows [W_hi; W_lo] from row w_row0 of each stage; then both column halves of D are
+// added to the accumulator tile from column acol.  Each chunk's stage is released as soon as its MMAs are done: keeping
+// a commit group in flight across chunks would hold every stage one chunk longer, i.e. make the ring one stage shallower
+// for the producer, and the stream waits on L2 latency rather than on the tensor core (measured slower).
+template <int N>
+__device__ __forceinline__ void event_wg(Ring& rg, int chunks, uint32_t w_row0, float* s_acc, int acol, DecoderCtrl* ctrl) {
+  const bool leader = (threadIdx.x & 127) == 0;
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  for (int i = 0; i < chunks; ++i) {
+    mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
+    const uint32_t xs = ptx::smem_u32(rg.stage(rg.c_stage));
+    const uint32_t ws = xs + kXChunkBytes + w_row0 * 128;
+    ptx::wg_fence_regs<N / 2>(d);
+    ptx::wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < kChunkK / 16; ++kk) {
+      const uint64_t b = ptx::make_sw128_desc(ws + kk * 32);
+      ptx::wgmma_f16<N>(d, ptx::make_sw128_desc(xs + kk * 32), b);                  // X_hi
+      ptx::wgmma_f16<N>(d, ptx::make_sw128_desc(xs + kRows * 128 + kk * 32), b);    // X_lo
+    }
+    ptx::wg_commit();
+    ptx::wg_wait<0>();
+    ptx::wg_fence_regs<N / 2>(d);
+    if (leader) release_stage(rg, rg.c_stage);
+    if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
+  }
+  const int wt = threadIdx.x & 127;
+#pragma unroll
+  for (int j = 0; j < N / 4; ++j)      // registers [0, N/4) hold the W_hi columns, [N/4, N/2) the W_lo ones
+    s_acc[ptx::wg_frag_row(j, wt) * kAccPitch + acol + ptx::wg_frag_col(j, wt)] += d[j] + d[N / 4 + j];
 }
 
 // Streams `chunks` K-chunks of the activation image x_img plus this CTA's weight rows through the ring;
-// warpgroups 1-3 issue the MMAs and add their slices to the accumulator tile s_acc.  Called by all threads;
+// warpgroups 1-3 issue the MMAs (one consumer each) and add their products to the accumulator tile s_acc.  Called by all threads;
 // returns after the accumulators are complete.  Every MMA accumulates (the epilogues zero what they consume).
+// The decoder's and the backward GEMMs' consumers have 32 or 16 rows (event_plan_fits(ep, false)); only the self test
+// instantiates the 8- and 24-row consumers (kAllWidths): every width is a copy of the whole chunk loop, and the
+// decoder kernel runs its code once per step, so each copy costs instruction-cache misses.
+template <bool kAllWidths = false>
 __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const uint8_t* x_img,
                                           const uint8_t* w_img, int chunks, float* s_acc,
                                           DecoderCtrl* ctrl, const EventPlan* next,
@@ -439,34 +498,20 @@ __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const u
     }
     __syncwarp();
   } else if (warp >= 4) {
-    // this warpgroup's slice: consumers are cut into slices of <= 32 weight rows, slice i goes to warpgroup 1 + i
-    const int wt = threadIdx.x & 127;
-    int left = (warp >> 2) - 1, wrow = 0, n = 0, m = 0, acol = 0;
-    for (int c = 0, roff = 0, col = ep.col0; c < ep.ncons; roff += 2 * ep.n[c], col += ep.n[c], ++c)
-      for (int j0 = 0; j0 < ep.n[c]; j0 += 32)
-        if (left-- == 0) { wrow = roff + j0; n = ep.n[c]; m = min(32, ep.n[c] - j0); acol = col + j0; }
-    float d[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) d[i] = 0.f;
-    ptx::wg_fence_regs<16>(d);
-    for (int i = 0; i < chunks; ++i) {
-      mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
-      const uint32_t xs = ptx::smem_u32(rg.stage(rg.c_stage));
-      const uint32_t w_hi = xs + kXChunkBytes + (uint32_t)wrow * 128, w_lo = w_hi + (uint32_t)n * 128;
-      if (m == 32) event_mma<32>(d, xs, w_hi, w_lo);
-      else if (m == 24) event_mma<24>(d, xs, w_hi, w_lo);
-      else if (m == 16) event_mma<16>(d, xs, w_hi, w_lo);
-      else if (m == 8) event_mma<8>(d, xs, w_hi, w_lo);
-      if (wt == 0) {                     // this warpgroup is done with the stage (in every CTA of the cluster)
-        if (rg.cs == 1) ptx::mbar_arrive(&rg.empty[rg.c_stage]);
-        else for (uint32_t r = 0; r < rg.cs; ++r) ptx::mbar_arrive_cluster(&rg.empty[rg.c_stage], r);
+    const int c = (warp >> 2) - 1;        // this warpgroup's consumer
+    if (c < ep.ncons) {
+      int w_row0 = 0, acol = ep.col0;
+      for (int i = 0; i < c; ++i) { w_row0 += 2 * ep.n[i]; acol += ep.n[i]; }
+      if (ep.n[c] == 32) event_wg<64>(rg, chunks, w_row0, s_acc, acol, ctrl);
+      else if (!kAllWidths || ep.n[c] == 16) event_wg<32>(rg, chunks, w_row0, s_acc, acol, ctrl);
+      else if (ep.n[c] == 24) event_wg<48>(rg, chunks, w_row0, s_acc, acol, ctrl);
+      else event_wg<16>(rg, chunks, w_row0, s_acc, acol, ctrl);
+    } else {                              // no rows for this warpgroup: it still releases every stage it was counted for
+      for (int i = 0; i < chunks; ++i) {
+        mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
+        if ((threadIdx.x & 127) == 0) release_stage(rg, rg.c_stage);
+        if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
       }
-      if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
-    }
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int col = ptx::wg_frag_col(i, wt);
-      if (col < m) s_acc[ptx::wg_frag_row(i, wt) * kAccPitch + acol + col] += d[i];
     }
   }
   __syncthreads();
@@ -1138,6 +1183,8 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
     if (hp) set(2, 8, kColA, {32, 32, 16}); else set(2, 8, kColA, {32, 32});
     if (hp) set(3, 16, kColD, {32, 16}); else set(3, 16, kColD, {32});
     if (hx) set(4, 4, kColS, {16}); else { pl.ev[4].w_off = (uint32_t)off; }
+    for (int ev = 0; ev < kNumEvents; ++ev)
+      if (pl.ev[ev].nrows != 0 && !event_plan_fits(pl.ev[ev], false)) return fail(T2_ERR_INVALID, "event plan does not fit the MMA warpgroups");
   }
   if (off >= (size_t)4 << 30) return fail(T2_ERR_INVALID, "W image too large");
   if (!pk->wimg) {
@@ -1342,7 +1389,8 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
 #ifdef T2_SELFTEST
 // ---------------------------------------------------------------------------------------------
 // self test of the wgmma event engine: C (64 x N) = 2 * A (64 x K) . W (N x K)^T with the same run_event()
-// (two accumulating passes over the ring) and the same accumulator tile as the decoder.
+// (two accumulating passes over the ring) and the same accumulator tile as the decoder.  The N rows of W are
+// the plan's consumers in order.
 // ---------------------------------------------------------------------------------------------
 namespace {
 __global__ void __launch_bounds__(kThreads, 1)
@@ -1365,27 +1413,36 @@ selftest_kernel(const uint8_t* x_img, const uint8_t* w_img, EventPlan ep, int ch
   }
   for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;
   __syncthreads();
-  run_event(rg, ep, x_img, w_img, chunks, s_acc, ctrl, &ep);      // second pass uses the prefetched weights
-  run_event(rg, ep, x_img, w_img, chunks, s_acc, ctrl, nullptr);
+  run_event<true>(rg, ep, x_img, w_img, chunks, s_acc, ctrl, &ep);      // second pass uses the prefetched weights
+  run_event<true>(rg, ep, x_img, w_img, chunks, s_acc, ctrl, nullptr);
   for (int i = tid; i < kRows * N; i += kThreads) C[i] = s_acc[(i / N) * kAccPitch + i % N];
 }
-}  // namespace
 
-int selftest_umma(const float* A, const float* W, int N, int K, int passes, float* C, cudaStream_t s) {
-  (void)passes;
-  if (N % 8 != 0 || N < 8 || N > kHiCols || K % kChunkK != 0 || K <= 0)
-    return fail(T2_ERR_INVALID, "selftest_umma: N in {8..80 step 8}, K %% 64 == 0");
-  const int chunks = K / kChunkK;
+// (N x K) fp32 row-major -> K/64 chunks of the plan's weight image (every consumer [n hi rows | n lo rows])
+__global__ void pack_plan_image_kernel(const float* __restrict__ W, int K, EventPlan ep, uint8_t* __restrict__ wimg) {
+  const int chunk = blockIdx.x;
+  __half* img = reinterpret_cast<__half*>(wimg + (size_t)chunk * ep.w_bytes);
+  for (int i = threadIdx.x; i < ep.nrows * 64; i += blockDim.x) {
+    const int r = i >> 6, k = i & 63;
+    int hr, lr;
+    plan_image_rows(ep, r, hr, lr);
+    __half h, l;
+    split_fp16(W[(long)r * K + chunk * 64 + k], h, l);
+    img[img_elem_offset(hr, k)] = h;
+    img[img_elem_offset(lr, k)] = l;
+  }
+}
+
+int selftest_plan(const float* A, const float* W, const EventPlan& ep, int K, float* C, cudaStream_t s) {
+  const int chunks = K / kChunkK, N = ep.nrows;
   uint8_t *ximg = nullptr, *wimg = nullptr; DecoderCtrl* ctrl = nullptr;
   T2_CUDA(cudaMalloc((void**)&ximg, (size_t)chunks * kXChunkBytes));
-  T2_CUDA(cudaMalloc((void**)&wimg, (size_t)chunks * N * 256));
+  T2_CUDA(cudaMalloc((void**)&wimg, (size_t)chunks * ep.w_bytes));
   T2_CUDA(cudaMalloc((void**)&ctrl, sizeof(DecoderCtrl)));
   T2_CUDA(cudaMemsetAsync(ctrl, 0, sizeof(DecoderCtrl), s));
-  EventPlan ep; memset(&ep, 0, sizeof(ep));
-  ep.ncons = 1; ep.n[0] = N; ep.nrows = N; ep.col0 = 0; ep.w_bytes = N * 256; ep.w_off = 0; ep.chunks = chunks;
   rows_to_image_kernel<<<dim3(chunks, 1), 256, 0, s>>>(A, K, kRows, K, 0, ximg, 0);
   T2_LAUNCH_CHECK();
-  pack_rows_image_kernel<<<chunks, 256, 0, s>>>(W, N, K, wimg);
+  pack_plan_image_kernel<<<chunks, 256, 0, s>>>(W, K, ep, wimg);
   T2_LAUNCH_CHECK();
   const size_t smem = (size_t)kStages * kStageBytes + 16 * 8 + kAccBytes;
   T2_CUDA(cudaFuncSetAttribute(selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1395,7 +1452,28 @@ int selftest_umma(const float* A, const float* W, int N, int K, int passes, floa
   cudaFree(ximg); cudaFree(wimg); cudaFree(ctrl);
   return T2_OK;
 }
+}  // namespace
 
+int selftest_umma(const float* A, const float* W, int N, int K, int passes, float* C, cudaStream_t s) {
+  (void)passes;
+  if (N % 8 != 0 || N < 8 || N > kHiCols || K % kChunkK != 0 || K <= 0)
+    return fail(T2_ERR_INVALID, "selftest_umma: N in {8..80 step 8}, K %% 64 == 0");
+  EventPlan ep; memset(&ep, 0, sizeof(ep));
+  plan_one_matrix(ep, N);
+  ep.chunks = K / kChunkK;
+  return selftest_plan(A, W, ep, K, C, s);
+}
+
+int selftest_event(const float* A, const float* W, const int* cons, int ncons, int K, float* C, cudaStream_t s) {
+  EventPlan ep; memset(&ep, 0, sizeof(ep));
+  if (ncons < 1 || ncons > 3 || K % kChunkK != 0 || K <= 0 || K > 16 * kChunkK)
+    return fail(T2_ERR_INVALID, "selftest_event: 1-3 consumers, K a multiple of 64 up to 1024");
+  for (int i = 0; i < ncons; ++i) { ep.n[i] = cons[i]; ep.nrows += cons[i]; }
+  ep.ncons = ncons; ep.w_bytes = (uint32_t)ep.nrows * 256; ep.chunks = K / kChunkK;
+  if (!event_plan_fits(ep, true))
+    return fail(T2_ERR_INVALID, "selftest_event: 1-3 consumers of 8, 16, 24 or 32 rows");
+  return selftest_plan(A, W, ep, K, C, s);
+}
 
 #endif  // T2_SELFTEST
 
@@ -1405,7 +1483,7 @@ int selftest_umma(const float* A, const float* W, int N, int K, int passes, floa
 // dG (64 x 4096) arrives as a split-fp16 activation image whose rows were scaled by a power of two
 // (row maximum in [0.5, 1): gradients span many orders of magnitude, fp16 does not); Wcat = [W_ih | W_hh]
 // is streamed as W^T images (rows = output columns, K = gate rows).  Same ring / MMA / accumulator tile
-// as the forward events (run_event): the output columns are cut into <= 32-column slices, one per MMA warpgroup.
+// as the forward events (run_event): a tile of output columns is planned as consumers of 32, 32 and 16 columns.
 // ---------------------------------------------------------------------------------------------
 namespace {
 constexpr int kBwdTileB = 80, kBwdTileE = 64;       // output columns per CTA: 2560 = 32 x 80, 1792 = 28 x 64
@@ -1417,17 +1495,18 @@ __global__ void pack_bwd_wimg_kernel(const float* __restrict__ w0, int cols0, co
   const int j = blockIdx.x;
   if (j >= pc.nchunks) return;
   const int n = pc.ep.nrows;
-  __half* hi = reinterpret_cast<__half*>(wimg + pc.ep.w_off + (size_t)j * pc.ep.w_bytes);
-  __half* lo = hi + n * kChunkK;
+  __half* img = reinterpret_cast<__half*>(wimg + pc.ep.w_off + (size_t)j * pc.ep.w_bytes);
   const int n0 = (pc.chunk0 + j) * kChunkK;
   for (int i = threadIdx.x; i < n * kChunkK; i += blockDim.x) {
     const int k = i / n, r = i - k * n;            // r fastest: coalesced along the weight matrix' columns
     const int col = pc.col0 + r;
     const float v = col < cols0 ? w0[(long)(n0 + k) * cols0 + col] : w1[(long)(n0 + k) * cols1 + (col - cols0)];
+    int hr, lr;
+    plan_image_rows(pc.ep, r, hr, lr);
     __half h, l;
     split_fp16(v, h, l);
-    const uint32_t e = img_elem_offset(r, k);
-    hi[e] = h; lo[e] = l;
+    img[img_elem_offset(hr, k)] = h;
+    img[img_elem_offset(lr, k)] = l;
   }
 }
 
@@ -1483,7 +1562,8 @@ int bwd_gemm_prepare(T2Model* m, cudaStream_t s) {
           memset(&c, 0, sizeof(c));
           c.chunk0 = sp * chunks / kBwdGemmSplit; c.nchunks = (sp + 1) * chunks / kBwdGemmSplit - c.chunk0;
           c.col0 = t * tile; c.split = sp;
-          c.ep.nrows = tile; c.ep.col0 = 0; c.ep.ncons = 1; c.ep.n[0] = tile; c.ep.w_bytes = w_bytes; c.ep.chunks = c.nchunks;
+          plan_one_matrix(c.ep, tile);    // 80 = 32 + 32 + 16, 64 = 32 + 32 columns (event_plan_fits(c.ep, false))
+          c.ep.col0 = 0; c.ep.chunks = c.nchunks;
           c.ep.w_off = (uint32_t)(((size_t)t * chunks + c.chunk0) * w_bytes);
         }
       T2_CUDA(cudaMalloc((void**)&pk->bwd_plans[which], sizeof(BwdCta) * ncta));

@@ -131,13 +131,6 @@ __device__ __forceinline__ int wg_frag_col(int i, int lane_in_wg) { return ((i >
 template <int N>
 __device__ __forceinline__ void wgmma_f16(float* d, uint64_t a_desc, uint64_t b_desc);
 template <>
-__device__ __forceinline__ void wgmma_f16<8>(float* d, uint64_t a_desc, uint64_t b_desc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0,%1,%2,%3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "l"(a_desc), "l"(b_desc));
-}
-template <>
 __device__ __forceinline__ void wgmma_f16<16>(float* d, uint64_t a_desc, uint64_t b_desc) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
                "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
@@ -145,17 +138,17 @@ __device__ __forceinline__ void wgmma_f16<16>(float* d, uint64_t a_desc, uint64_
                : "l"(a_desc), "l"(b_desc));
 }
 template <>
-__device__ __forceinline__ void wgmma_f16<24>(float* d, uint64_t a_desc, uint64_t b_desc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n24k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 0, 0;\n\t}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
-               : "l"(a_desc), "l"(b_desc));
-}
-template <>
 __device__ __forceinline__ void wgmma_f16<32>(float* d, uint64_t a_desc, uint64_t b_desc) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
                "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(a_desc), "l"(b_desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16<48>(float* d, uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
                : "l"(a_desc), "l"(b_desc));
 }
 template <>
