@@ -559,7 +559,6 @@ struct KParams {
   const uint8_t* wimg;
   const float* bias_a; const float* bias_d; const float* bias_p;
   const uint8_t* weff_img; const float* w_v;
-  float l2_pin_frac;
   // tensors
   const float* memory; const float* pm; const int32_t* mem_len;
   const uint8_t* prenet_keep; const uint8_t* att_keep; const uint8_t* dec_keep;
@@ -640,12 +639,11 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   for (int i = tid; i < 32; i += kThreads) { s_bias_a[i] = p.bias_a[cta * 32 + i]; s_bias_d[i] = p.bias_d[cta * 32 + i]; }
   for (int i = tid; i < kWeffBytes / 16; i += kThreads)
     reinterpret_cast<uint4*>(s_weff)[i] = reinterpret_cast<const uint4*>(p.weff_img)[i];
-  {
-    uint64_t pol;
-    asm volatile("createpolicy.fractional.L2::evict_last.L2::evict_first.b64 %0, %1;" : "=l"(pol) : "f"(p.l2_pin_frac));
-    rg.pol_w = pol;
-    rg.pol_x = ptx::policy_evict_last();
-  }
+  // The weight image (73.5 MiB, all of it streamed every step) is larger than the 50 MB L2, so its lines are marked to go
+  // first; the activation chunks that every CTA reads keep evict_last.  Keeping half of the weight lines with evict_last
+  // priority instead made the decoder step ~9 µs slower on H100 (DESIGN §6.1).
+  rg.pol_w = ptx::policy_evict_first();
+  rg.pol_x = ptx::policy_evict_last();
   for (int i = tid; i < kAtt; i += kThreads) s_v[i] = p.w_v[i];
   if (tid < 8) s_bias_p[tid] = (cta >= kPCta0 && cta < kPCta0 + kPCtas) ? p.bias_p[(cta - kPCta0) * 8 + tid] : 0.f;
   for (int i = tid; i < TP; i += kThreads) { s_pad0[i] = 0.f; s_pad1[i] = 0.f; }   // model.py:274-277
@@ -1293,10 +1291,6 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
   p.q = (float*)img;
   p.plans = pk->plans; p.wimg = pk->wimg; p.bias_a = pk->bias_a; p.bias_d = pk->bias_d; p.bias_p = pk->bias_p;
   p.weff_img = pk->weff_img; p.w_v = m->w[W_ATT_V];
-  {
-    const char* e = getenv("T2_L2_PIN_FRAC");   // fraction of weight-image lines kept with evict_last priority
-    p.l2_pin_frac = e ? (float)atof(e) : 0.5f;
-  }
   p.memory = a->memory + (size_t)b0 * T * kEnc; p.pm = w.pm;
   p.mem_len = a->memory_lengths ? a->memory_lengths + b0 : nullptr;
   p.prenet_keep = a->prenet_keep; p.att_keep = a->att_keep; p.dec_keep = a->dec_keep;
