@@ -274,7 +274,9 @@ int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) {
   int impl = a->impl;
   if (impl == T2_IMPL_AUTO) impl = persistent_supported(m, a) ? T2_IMPL_PERSISTENT : T2_IMPL_STEPWISE;
   if (impl == T2_IMPL_PERSISTENT) {
-    if (!persistent_supported(m, a)) return fail(T2_ERR_UNSUPPORTED, "persistent decoder does not support this shape/mode");
+    if (!persistent_supported(m, a))
+      return fail(T2_ERR_UNSUPPORTED, "persistent decoder does not support T_enc=%d on this device (at most 2274, and >= 128 SMs)",
+                  a->T_enc);
     return decoder_run_persistent(m, a, (cudaStream_t)stream);
   }
   // only the persistent kernel writes the training stash: a backward pass over a stash the stepwise path left

@@ -47,7 +47,8 @@ namespace {
 constexpr int kG = 128;               // CTAs
 constexpr int kThreads = 512;
 constexpr int kStages = 4;             // ring stages of the helper kernels (self test, backward GEMMs)
-constexpr int kMaxStages = 5;          // ring stages of the decoder kernel: 4 by default (T2_STAGES: 3-5 where shared memory allows)
+constexpr int kMaxStages = 5;          // ring barriers reserved by the decoder kernel; it runs 4 stages up to T_enc = 896, else 3
+                                       // (5 never fit in 227 KiB; T2_STAGES = 3 forces the 3-stage ring)
 constexpr int kRows = 64;             // batch rows per launch (zero padded)
 constexpr int kXChunkBytes = 2 * kRows * kChunkK * 2;    // [hi 64 rows | lo 64 rows] x 64 k fp16 = 16 KiB
 // accumulator columns (shared memory, fp32 [64 batch rows][kAccPitch]): att 0-31, dec 32-63, shared slot 64-79
@@ -569,7 +570,7 @@ struct KParams {
   float* mel; float* gate; float* align; int32_t* mel_lengths; int32_t* n_steps;
   DecoderCtrl* ctrl;
   int B, T, cap, infer, training, cluster, hier_barrier;
-  int nstages;                      // operand ring stages (4 or 5)
+  int nstages;                      // operand ring stages (4, or 3 when T_enc > 896)
   int chunk_ready;                  // 1: ah / dh hand-over through per-chunk arrival counters instead of barriers B1 / B4
   int b0, Btot;                     // this launch handles batch rows [b0, b0 + B) of Btot (dropout mask / Philox indexing)
   float gate_threshold, score_mask_value, p_att, p_dec;
@@ -1131,7 +1132,9 @@ static size_t persistent_smem_bytes(int T, int nstages) {
          kRows * 4 + 32 + 24 * 8 + 2 * (size_t)((TP + 3) & ~3) * 4 + att + 1024;
 }
 constexpr size_t kSmemLimit = 227 * 1024;
-// 4 ring stages when they fit beside the T_enc-dependent attention state (T_enc <~ 680 on sm_90's 227 KiB), else 3
+// 4 ring stages when they fit beside the T_enc-dependent attention state (T_enc <= 896 on sm_90's 227 KiB), else 3
+// (T_enc <= 2274; longer memories are refused, see persistent_supported).  The idle ring stages encoder-memory rows
+// 0-93 at 4 stages and 0-57 at 3 for the attention context; later rows are read from L2.
 static int persistent_stages(int T) {
   int want = 4;
   const char* e = getenv("T2_STAGES");

@@ -210,6 +210,8 @@ size_t stepwise_attention_smem(int T) {
 int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
   const int B = a->B, T = a->T_enc, cap = a->n_steps_cap;
   const bool infer = a->mode == T2_MODE_INFER;
+  const size_t att_smem = stepwise_attention_smem(T);
+  if (att_smem > 200 * 1024) return fail(T2_ERR_INVALID, "T_enc=%d too long for the stepwise attention kernel (at most 1282)", T);
   DecoderWs w;
   T2_TRY(decoder_ws_carve(a, &w));
   T2_CUDA(cudaMemsetAsync(w.state_begin, 0, w.state_bytes, s));   // model.py:258-284 (zeros)
@@ -222,8 +224,6 @@ int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
     g.M = B * T; g.N = kAtt; g.C = w.pm; g.ldc = kAtt;
     T2_TRY(gemm_f32(g, s));
   }
-  const size_t att_smem = stepwise_attention_smem(T);
-  if (att_smem > 200 * 1024) return fail(T2_ERR_INVALID, "T_enc=%d too long for the stepwise attention kernel", T);
   T2_CUDA(cudaFuncSetAttribute(attention_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)att_smem));
   const int* skip = &w.ctrl->all_done;
