@@ -243,7 +243,6 @@ int t2_model_destroy(T2Model* m) {
   cudaFree(m->tc_enc_wih);
   persistent_pack_destroy(m);
   gemm_tc_destroy(m);
-  blas_destroy(m);
   delete m;
   return T2_OK;
 }

@@ -10,7 +10,7 @@
 //   tile addressed with the descriptor start shifted by tap*16 bytes -- no im2col, 5x reuse from SMEM.
 //   (K-major no-swizzle canonical layout with LBO = 2112 between k8 groups, SBO = 128 between 8-row groups.)
 // * Weights are packed per (n-tile, 64-channel chunk, tap) as [hi | lo] SWIZZLE_128B planes and streamed
-//   through a ring; within a cluster the weight stage is fetched once and TMA-multicast.
+//   through a ring; within a cluster of 2 CTAs the weight stage is fetched once and TMA-multicast.
 // * fp32-grade: hi*hi + lo*hi + hi*lo, 3 MMAs (M=64 per warpgroup, N=n_tile, K=16) per 16 channels, fp32 in registers.
 // * Epilogue: folded BatchNorm scale/shift (+bias), ReLU / tanh, and either the next layer's planes,
 //   fp32 rows (LSTM gate pre-activations) or the final (B, 80, T) tensor with the residual (model.py:511/524).
@@ -28,6 +28,7 @@ constexpr int kHalo = 4;                   // input rows = kTile + 4
 constexpr int kSeg = (kTile + kHalo) * 16; // bytes of one k8 plane segment of a tile = 2112
 constexpr int kAStage = 16 * kSeg;         // 8 k8 groups x (hi, lo) = 33792 bytes per 64-channel chunk
 constexpr int kThreadsC = 384;             // warp 0 producer; warpgroups 1 / 2: MMA + epilogue
+constexpr int kCluster = 2;                // CTAs of a cluster share each weight stage by multicast
 constexpr unsigned long long kWd = 1ull << 32;
 
 __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) {
@@ -48,7 +49,6 @@ struct ConvParams {
   __half* out_planes; long out_plane_rows;
   float* out_f32; long ldo; int out_seq_rows;  // out_mode 1: row of (b, t) = b * out_seq_rows + t
   const float* residual; long res_batch_stride; const int32_t* row_len;
-  int cluster;
 };
 
 template <int NT, int NH, int WS>   // NT = weight rows per stage (MMA N), NH = n-halves per CTA, WS = weight stages
@@ -63,15 +63,15 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + 2 * kAStage);
   uint64_t* a_full = bars; uint64_t* a_empty = bars + 2;
   uint64_t* w_full = bars + 4; uint64_t* w_empty = bars + 4 + WS;
-  const uint32_t cs = p.cluster, rank = cs > 1 ? ptx::cluster_ctarank() : 0;
+  const uint32_t rank = ptx::cluster_ctarank();
   if (tid == 0) {
     // a stage is released by the 2 MMA warpgroups (a weight stage: of every CTA of the cluster)
     for (int i = 0; i < 2; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
-    for (int i = 0; i < WS; ++i) { ptx::mbar_init(&w_full[i], 1); ptx::mbar_init(&w_empty[i], 2 * cs); }
+    for (int i = 0; i < WS; ++i) { ptx::mbar_init(&w_full[i], 1); ptx::mbar_init(&w_empty[i], 2 * kCluster); }
     ptx::fence_barrier_init();
   }
   __syncthreads();
-  if (cs > 1) ptx::cluster_sync_all();
+  ptx::cluster_sync_all();
   const bool tile_live = mt < p.n_tiles_m;     // grid.x is rounded up to the cluster size
 
   if (warp == 0) {
@@ -93,13 +93,9 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
           wait_bar(&w_empty[wst], wph ^ 1);
           ptx::mbar_arrive_expect_tx(&w_full[wst], kWStage);
           const uint8_t* wsrc = p.wimg + (((size_t)(nt * NH + h) * p.nchunks + c) * p.taps + tap) * kWStage;
-          if (cs == 1) {
-            ptx::bulk_g2s_hint(s_w + wst * kWStage, wsrc, kWStage, &w_full[wst], pol_w);
-          } else {
-            const uint32_t slice = kWStage / cs;
-            ptx::bulk_g2s_mc_hint(s_w + wst * kWStage + rank * slice, wsrc + rank * slice, slice, &w_full[wst],
-                                  (uint16_t)((1u << cs) - 1u), pol_w);
-          }
+          const uint32_t slice = kWStage / kCluster;
+          ptx::bulk_g2s_mc_hint(s_w + wst * kWStage + rank * slice, wsrc + rank * slice, slice, &w_full[wst],
+                                (uint16_t)((1u << kCluster) - 1u), pol_w);
           if (++wst == WS) { wst = 0; wph ^= 1; }
         }
       }
@@ -141,10 +137,8 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
           ptx::wg_commit();
           ptx::wg_wait<0>();
           ptx::wg_fence_regs<NT / 2>(d[h]);
-          if (wt == 0) {                     // this warpgroup is done with the weight stage in every CTA of the cluster
-            if (cs == 1) ptx::mbar_arrive(&w_empty[wst]);
-            else for (uint32_t r = 0; r < cs; ++r) ptx::mbar_arrive_cluster(&w_empty[wst], r);
-          }
+          if (wt == 0)                       // this warpgroup is done with the weight stage in every CTA of the cluster
+            for (int r = 0; r < kCluster; ++r) ptx::mbar_arrive_cluster(&w_empty[wst], r);
           if (++wst == WS) { wst = 0; wph ^= 1; }
         }
       }
@@ -220,19 +214,17 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
     }
   }
   __syncthreads();
-  if (cs > 1) {
-    // peers' consumers arrive on our w_empty barriers: drain before leaving (producer thread state is
-    // gone here, so wait on the parity each barrier reaches after its last use)
-    if (tid == 0) {
-      const int total = p.nchunks * p.taps * NH;
-      for (int i = 0; i < WS; ++i) {
-        const int uses = (total - i + WS - 1) / WS;       // number of times stage i was filled
-        if (uses > 0) wait_bar(&w_empty[i], (uses - 1) & 1);
-      }
+  // peers' consumers arrive on our w_empty barriers: drain before leaving (producer thread state is
+  // gone here, so wait on the parity each barrier reaches after its last use)
+  if (tid == 0) {
+    const int total = p.nchunks * p.taps * NH;
+    for (int i = 0; i < WS; ++i) {
+      const int uses = (total - i + WS - 1) / WS;       // number of times stage i was filled
+      if (uses > 0) wait_bar(&w_empty[i], (uses - 1) & 1);
     }
-    __syncthreads();
-    ptx::cluster_sync_all();
   }
+  __syncthreads();
+  ptx::cluster_sync_all();
 }
 
 // ---- layout conversion kernels ---------------------------------------------------------------------
@@ -323,14 +315,12 @@ int launch_conv(const ConvParams& p, int n_tiles_n, cudaStream_t s) {
   T2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, NH, WS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  const int gx = ((p.n_tiles_m + p.cluster - 1) / p.cluster) * p.cluster;
+  const int gx = ((p.n_tiles_m + kCluster - 1) / kCluster) * kCluster;
   cfg.gridDim = dim3(gx, n_tiles_n); cfg.blockDim = dim3(kThreadsC); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  if (p.cluster > 1) {
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = p.cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-  }
+  cudaLaunchAttribute at;
+  at.id = cudaLaunchAttributeClusterDimension;
+  at.val.clusterDim.x = kCluster; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+  cfg.attrs = &at; cfg.numAttrs = 1;
   cudaError_t e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<NT, NH, WS>, p);
   if (e != cudaSuccess) return fail(T2_ERR_CUDA, "conv_tc launch failed: %s", cudaGetErrorString(e));
   g_launch_count++;
@@ -395,9 +385,6 @@ int tc_conv(const TcConvArgs& a, cudaStream_t s) {
   p.out_f32 = a.out_f32; p.ldo = a.ldo; p.out_seq_rows = a.out_seq_rows > 0 ? a.out_seq_rows : a.T;
   p.residual = a.residual; p.row_len = a.row_len;
   p.res_batch_stride = a.res_batch_stride ? a.res_batch_stride : (long)a.T * a.cout;
-  const char* e = getenv("T2_CONV_CLUSTER");
-  p.cluster = e ? atoi(e) : 2;
-  if (p.cluster != 1 && p.cluster != 2 && p.cluster != 4) p.cluster = 2;
   // weights are packed in stages of nt_rows rows; a CTA covers 2 stages' worth of columns when cout allows
   if (a.nt_rows == 128) return launch_conv<128, 2, 4>(p, (a.cout + 255) / 256, s);
   if (a.nt_rows == 80) return launch_conv<80, 1, 4>(p, (a.cout + 79) / 80, s);

@@ -9,9 +9,8 @@
 //                   location layer backward -> carries for aw_{t-1}, awc_{t-1}            (model.py:43-86)
 //   KD lstm_bwd   : g_ah = carry + dG_dec part + g_q W_q -> mask -> LSTMCell backward      -> dG_att[t], g_ac
 //   KE skinny_nn  : [g_x2 | g_ctx' | g_ah'] partials = dG_att[t] . [W_ih^a | W_hh^a]      (model.py:352-354)
-// Phase 2 (time batched, plain library GEMMs through cuBLAS): every weight gradient is dG^T . X over all
+// Phase 2 (time batched, on the tensor-core GEMMs gemm_tc / wgrad_tc): every weight gradient is dG^T . X over all
 // T x B rows; d_memory = d_pm W_m + sum_t aw_t (x) g_ctx_t.
-#include <cublas_v2.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -22,47 +21,6 @@
 #include "wgrad_tc.h"
 
 namespace t2 {
-
-// ---- cuBLAS plumbing (plain time-batched GEMMs) ------------------------------------------------
-int blas_handle(T2Model* m, cudaStream_t s, cublasHandle_t* out) {
-  if (!m->blas) {
-    cublasHandle_t h;
-    if (cublasCreate(&h) != CUBLAS_STATUS_SUCCESS) return fail(T2_ERR_CUDA, "cublasCreate failed");
-    cublasSetMathMode(h, CUBLAS_DEFAULT_MATH);
-    m->blas = h;
-  }
-  *out = (cublasHandle_t)m->blas;
-  if (cublasSetStream(*out, s) != CUBLAS_STATUS_SUCCESS) return fail(T2_ERR_CUDA, "cublasSetStream failed");
-  return T2_OK;
-}
-// Every dense product of the training path goes through gemm_rm(): our wgmma split-fp16 GEMM (gemm_tc.cu) by default;
-// T2_GEMM=cublas selects plain cuBLAS fp32 sgemm, kept only as the independent cross-check of tests/test_gpu_backward.py.
-bool use_cublas_gemm() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("T2_GEMM"); v = (e && !strcmp(e, "cublas")) ? 1 : 0; }
-  return v == 1;
-}
-// row-major C (M x N) = op(A) . op(B) + beta C;  ta: A is stored (K x M);  tb: B is stored (N x K)
-int gemm_rm(T2Model* m, cudaStream_t s, bool ta, bool tb, int M, int N, int K, const float* A, long lda, const float* B, long ldb,
-            float* C, long ldc, float beta) {
-  if (!use_cublas_gemm()) return gemm_tc_rm(m, s, ta, tb, M, N, K, A, lda, B, ldb, C, ldc, beta);
-  cublasHandle_t h;
-  T2_TRY(blas_handle(m, s, &h));
-  const float alpha = 1.f;
-  cublasStatus_t st = cublasSgemm(h, tb ? CUBLAS_OP_T : CUBLAS_OP_N, ta ? CUBLAS_OP_T : CUBLAS_OP_N, N, M, K, &alpha, B,
-                                  (int)ldb, A, (int)lda, &beta, C, (int)ldc);
-  if (st != CUBLAS_STATUS_SUCCESS) return fail(T2_ERR_CUDA, "cublasSgemm failed (%d) M=%d N=%d K=%d", (int)st, M, N, K);
-  g_launch_count++;
-  return T2_OK;
-}
-int gemm_rm_wgrad(T2Model* m, cudaStream_t s, bool ta, bool tb, int M, int N, int K, const float* A, long lda, const float* B,
-                  long ldb, float* C, long ldc, float beta) {
-  return gemm_rm(m, s, ta, tb, M, N, K, A, lda, B, ldb, C, ldc, beta);
-}
-// out[c] = sum over rows of X[r * ld + c] (bias gradients; round 1 multiplied by a vector of ones through cuBLAS)
-int colsum_rm(T2Model* m, cudaStream_t s, const float* X, long ld, long rows, int cols, float* out) {
-  return colsum_f32(m, s, X, ld, rows, cols, out);
-}
 
 namespace {
 
@@ -657,10 +615,10 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     T2_LAUNCH_CHECK();
   }
   // processed_memory (model.py:288) and the processed queries of all steps (model.py:57)
-  T2_TRY(gemm_rm(m, s, false, true, B * Te, kAtt, kEnc, a->memory, kEnc, m->w[W_ATT_MEMORY], kEnc, w.pm, kAtt, 0.f));
-  T2_TRY(gemm_rm(m, s, false, true, (int)TB, kAtt, kARnn, st.ha + (size_t)B * kARnn, kARnn, m->w[W_ATT_QUERY], kARnn, w.q, kAtt, 0.f));
+  T2_TRY(gemm_tc_rm(m, s, false, true, B * Te, kAtt, kEnc, a->memory, kEnc, m->w[W_ATT_MEMORY], kEnc, w.pm, kAtt, 0.f));
+  T2_TRY(gemm_tc_rm(m, s, false, true, (int)TB, kAtt, kARnn, st.ha + (size_t)B * kARnn, kARnn, m->w[W_ATT_QUERY], kARnn, w.q, kAtt, 0.f));
   // projection / gate contribution to g_dh and g_ctx of every step: [d_mel_t ; d_gate_t] . [W_proj ; W_gate]  (model.py:373-378)
-  T2_TRY(gemm_rm(m, s, false, false, (int)TB, kDRnn + kEnc, 81, w.dy, 81, m->projgate_w, kDRnn + kEnc, w.gproj, kDRnn + kEnc, 0.f));
+  T2_TRY(gemm_tc_rm(m, s, false, false, (int)TB, kDRnn + kEnc, 81, w.dy, 81, m->projgate_w, kDRnn + kEnc, w.gproj, kDRnn + kEnc, 0.f));
   T2_CUDA(cudaFuncSetAttribute(att_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 
   // T2_BWD_PROFILE=1: CUDA-event time per kernel class over the first 64 steps (stderr), for tuning
@@ -776,7 +734,8 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   float* const* G = a->grads;
   const float* x2 = a->teacher_prenet;
   const int TBi = (int)TB;
-  // LSTM weight / bias gradients: our wgmma split-fp16 engine (default) or plain cuBLAS fp32 GEMMs (T2_WGRAD=cublas)
+  // LSTM weight / bias gradients: the time-batched wgrad_tc engine (default) or, as a cross-check (T2_WGRAD=cublas),
+  // separate gemm_tc products and column sums
   bool tc_wgrad = true;
   {
     const char* e = getenv("T2_WGRAD");
@@ -786,42 +745,42 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     T2_TRY(wgrad_tc_run(m, B, T, w.dga, w.dgd, x2, st, G, w.wg, w.wg_bytes, s));
   } else {
   if (G[W_ARNN_WIH]) {   // [x2_t | ctx_{t-1}]                                             model.py:352
-      T2_TRY(gemm_rm_wgrad(m, s, true, false, 4096, kPre, TBi, w.dga, 4096, x2, kPre, G[W_ARNN_WIH], kPre + kEnc, 0.f));
-      T2_TRY(gemm_rm_wgrad(m, s, true, false, 4096, kEnc, TBi, w.dga, 4096, st.ctx, kEnc, G[W_ARNN_WIH] + kPre, kPre + kEnc, 0.f));
+      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kPre, TBi, w.dga, 4096, x2, kPre, G[W_ARNN_WIH], kPre + kEnc, 0.f));
+      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kEnc, TBi, w.dga, 4096, st.ctx, kEnc, G[W_ARNN_WIH] + kPre, kPre + kEnc, 0.f));
     }
-    if (G[W_ARNN_WHH]) T2_TRY(gemm_rm_wgrad(m, s, true, false, 4096, kARnn, TBi, w.dga, 4096, st.ha, kARnn, G[W_ARNN_WHH], kARnn, 0.f));
+    if (G[W_ARNN_WHH]) T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kARnn, TBi, w.dga, 4096, st.ha, kARnn, G[W_ARNN_WHH], kARnn, 0.f));
     if (G[W_ARNN_BIH] || G[W_ARNN_BHH]) {
-      T2_TRY(colsum_rm(m, s, w.dga, 4096, TBi, 4096, w.tmp));
+      T2_TRY(colsum_f32(m, s, w.dga, 4096, TBi, 4096, w.tmp));
       if (G[W_ARNN_BIH]) T2_CUDA(cudaMemcpyAsync(G[W_ARNN_BIH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
       if (G[W_ARNN_BHH]) T2_CUDA(cudaMemcpyAsync(G[W_ARNN_BHH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
     }
     if (G[W_DRNN_WIH]) {   // [ah_t | ctx_t]                                                 model.py:366-367
-      T2_TRY(gemm_rm_wgrad(m, s, true, false, 4096, kARnn, TBi, w.dgd, 4096, st.ha + (size_t)B * kARnn, kARnn, G[W_DRNN_WIH], kARnn + kEnc, 0.f));
-      T2_TRY(gemm_rm_wgrad(m, s, true, false, 4096, kEnc, TBi, w.dgd, 4096, st.ctx + (size_t)B * kEnc, kEnc, G[W_DRNN_WIH] + kARnn, kARnn + kEnc, 0.f));
+      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kARnn, TBi, w.dgd, 4096, st.ha + (size_t)B * kARnn, kARnn, G[W_DRNN_WIH], kARnn + kEnc, 0.f));
+      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kEnc, TBi, w.dgd, 4096, st.ctx + (size_t)B * kEnc, kEnc, G[W_DRNN_WIH] + kARnn, kARnn + kEnc, 0.f));
     }
-    if (G[W_DRNN_WHH]) T2_TRY(gemm_rm_wgrad(m, s, true, false, 4096, kDRnn, TBi, w.dgd, 4096, st.hd, kDRnn, G[W_DRNN_WHH], kDRnn, 0.f));
+    if (G[W_DRNN_WHH]) T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kDRnn, TBi, w.dgd, 4096, st.hd, kDRnn, G[W_DRNN_WHH], kDRnn, 0.f));
     if (G[W_DRNN_BIH] || G[W_DRNN_BHH]) {
-      T2_TRY(colsum_rm(m, s, w.dgd, 4096, TBi, 4096, w.tmp));
+      T2_TRY(colsum_f32(m, s, w.dgd, 4096, TBi, 4096, w.tmp));
       if (G[W_DRNN_BIH]) T2_CUDA(cudaMemcpyAsync(G[W_DRNN_BIH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
       if (G[W_DRNN_BHH]) T2_CUDA(cudaMemcpyAsync(G[W_DRNN_BHH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
     }
   }
   // projection + gate on [dh_t | ctx_t]                                                   model.py:373-378
   if (G[W_PROJ_W]) {
-    T2_TRY(gemm_rm(m, s, true, false, kMel, kDRnn, TBi, w.dy, 81, st.hd + (size_t)B * kDRnn, kDRnn, G[W_PROJ_W], kDRnn + kEnc, 0.f));
-    T2_TRY(gemm_rm(m, s, true, false, kMel, kEnc, TBi, w.dy, 81, st.ctx + (size_t)B * kEnc, kEnc, G[W_PROJ_W] + kDRnn, kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(m, s, true, false, kMel, kDRnn, TBi, w.dy, 81, st.hd + (size_t)B * kDRnn, kDRnn, G[W_PROJ_W], kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(m, s, true, false, kMel, kEnc, TBi, w.dy, 81, st.ctx + (size_t)B * kEnc, kEnc, G[W_PROJ_W] + kDRnn, kDRnn + kEnc, 0.f));
   }
   if (G[W_GATE_W]) {
-    T2_TRY(gemm_rm(m, s, true, false, 1, kDRnn, TBi, w.dy + 80, 81, st.hd + (size_t)B * kDRnn, kDRnn, G[W_GATE_W], kDRnn + kEnc, 0.f));
-    T2_TRY(gemm_rm(m, s, true, false, 1, kEnc, TBi, w.dy + 80, 81, st.ctx + (size_t)B * kEnc, kEnc, G[W_GATE_W] + kDRnn, kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(m, s, true, false, 1, kDRnn, TBi, w.dy + 80, 81, st.hd + (size_t)B * kDRnn, kDRnn, G[W_GATE_W], kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(m, s, true, false, 1, kEnc, TBi, w.dy + 80, 81, st.ctx + (size_t)B * kEnc, kEnc, G[W_GATE_W] + kDRnn, kDRnn + kEnc, 0.f));
   }
   if (G[W_PROJ_B] || G[W_GATE_B]) {
-    T2_TRY(colsum_rm(m, s, w.dy, 81, TBi, 81, w.tmp));
+    T2_TRY(colsum_f32(m, s, w.dy, 81, TBi, 81, w.tmp));
     if (G[W_PROJ_B]) T2_CUDA(cudaMemcpyAsync(G[W_PROJ_B], w.tmp, 80 * 4, cudaMemcpyDeviceToDevice, s));
     if (G[W_GATE_B]) T2_CUDA(cudaMemcpyAsync(G[W_GATE_B], w.tmp + 80, 4, cudaMemcpyDeviceToDevice, s));
   }
   if (G[W_ATT_QUERY])
-    T2_TRY(gemm_rm(m, s, true, false, kAtt, kARnn, TBi, w.dq, kAtt, st.ha + (size_t)B * kARnn, kARnn, G[W_ATT_QUERY], kARnn, 0.f));
+    T2_TRY(gemm_tc_rm(m, s, true, false, kAtt, kARnn, TBi, w.dq, kAtt, st.ha + (size_t)B * kARnn, kARnn, G[W_ATT_QUERY], kARnn, 0.f));
   if (G[W_ATT_V]) {
     sum_rows_kernel<<<1, 128, 0, s>>>(w.dv, G[W_ATT_V], B, 128);
     T2_LAUNCH_CHECK();
@@ -830,43 +789,26 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     const long n = (long)TB * Te * kColsLd;
     im2col_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->align, w.awc, w.cols, B, T, Te);
     T2_LAUNCH_CHECK();
-    // K = T*B*Te can exceed what one call accumulates accurately in fp32 order-wise; split per step block
-    const long R = (long)TB * Te;
-    // cuBLAS cross-check: K = T*B*Te in blocks of 2^20 rows (one fp32 accumulation order per block); our GEMM drains its
-    // accumulator every 64 rows and splits K over the SMs, so it takes the whole K in one call
-    const long chunk = use_cublas_gemm() ? (1L << 20) : R;
-    for (long r0 = 0; r0 < R; r0 += chunk) {
-      const int k = (int)(R - r0 < chunk ? R - r0 : chunk);
-      T2_TRY(gemm_rm(m, s, true, false, kAtt, kColsLd, k, w.gs + r0 * kAtt, kAtt, w.cols + r0 * kColsLd, kColsLd, w.dweff, kColsLd,
-                     r0 ? 1.f : 0.f));
-    }
+    // K = T*B*Te rows in one call: the GEMM drains its accumulator every 64 rows and splits K over the SMs
+    const int R = (int)((long)TB * Te);
+    T2_TRY(gemm_tc_rm(m, s, true, false, kAtt, kColsLd, R, w.gs, kAtt, w.cols, kColsLd, w.dweff, kColsLd, 0.f));
     dweff_split_kernel<<<(kAtt * kLocF + 255) / 256, 256, 0, s>>>(w.dweff, m->w[W_ATT_LOC_DENSE], m->w[W_ATT_LOC_CONV],
                                                                   G[W_ATT_LOC_DENSE], G[W_ATT_LOC_CONV]);
     T2_LAUNCH_CHECK();
   }
   // d_pm = sum_t g_s[t]  -> memory_layer gradient and its share of d_memory              model.py:288
-  T2_TRY(colsum_rm(m, s, w.gs, (long)B * Te * kAtt, T, B * Te * kAtt, w.dpm));
+  T2_TRY(colsum_f32(m, s, w.gs, (long)B * Te * kAtt, T, B * Te * kAtt, w.dpm));
   if (G[W_ATT_MEMORY])
-    T2_TRY(gemm_rm(m, s, true, false, kAtt, kEnc, B * Te, w.dpm, kAtt, a->memory, kEnc, G[W_ATT_MEMORY], kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(m, s, true, false, kAtt, kEnc, B * Te, w.dpm, kAtt, a->memory, kEnc, G[W_ATT_MEMORY], kEnc, 0.f));
   if (a->d_memory) {
-    T2_TRY(gemm_rm(m, s, false, false, B * Te, kEnc, kAtt, w.dpm, kAtt, m->w[W_ATT_MEMORY], kEnc, a->d_memory, kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(m, s, false, false, B * Te, kEnc, kAtt, w.dpm, kAtt, m->w[W_ATT_MEMORY], kEnc, a->d_memory, kEnc, 0.f));
     // + sum_t aw_t[b] (x) g_ctx_t[b]: per row b, (Te x T) . (T x 512)                      model.py:83-84
-    if (!use_cublas_gemm()) {
-      GemmTc g;        // d_memory[b] (Te x 512) += align[b]^T (T x Te stored) . dctx[:, b, :] (T x 512, rows B * 512 apart)
-      g.ta = true; g.tb = false; g.M = Te; g.N = kEnc; g.K = T;
-      g.A = a->align; g.lda = Te; g.strideA = (long)T * Te;
-      g.B = w.dctx; g.ldb = (long)B * kEnc; g.strideB = kEnc;
-      g.C = a->d_memory; g.ldc = kEnc; g.strideC = (long)Te * kEnc; g.beta = 1.f; g.batch = B;
-      T2_TRY(gemm_tc(m, s, g));
-    } else {
-      cublasHandle_t bl;
-      T2_TRY(blas_handle(m, s, &bl));
-      const float alpha = 1.f, beta = 1.f;
-      cublasStatus_t stt = cublasSgemmStridedBatched(bl, CUBLAS_OP_N, CUBLAS_OP_T, kEnc, Te, T, &alpha, w.dctx, B * kEnc, (long long)kEnc,
-                                                     a->align, Te, (long long)T * Te, &beta, a->d_memory, kEnc, (long long)Te * kEnc, B);
-      if (stt != CUBLAS_STATUS_SUCCESS) return fail(T2_ERR_CUDA, "cublasSgemmStridedBatched failed (%d)", (int)stt);
-      g_launch_count++;
-    }
+    GemmTc g;        // d_memory[b] (Te x 512) += align[b]^T (T x Te stored) . dctx[:, b, :] (T x 512, rows B * 512 apart)
+    g.ta = true; g.tb = false; g.M = Te; g.N = kEnc; g.K = T;
+    g.A = a->align; g.lda = Te; g.strideA = (long)T * Te;
+    g.B = w.dctx; g.ldb = (long)B * kEnc; g.strideB = kEnc;
+    g.C = a->d_memory; g.ldc = kEnc; g.strideC = (long)Te * kEnc; g.beta = 1.f; g.batch = B;
+    T2_TRY(gemm_tc(m, s, g));
   }
   if (prof) {
     cudaEventRecord(ph[2], s);
@@ -910,18 +852,13 @@ int prenet_backward(T2Model* m, const T2PrenetBwdArgs* a, cudaStream_t s) {
   const long n = (long)M * kPre;
   prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->d_out, x2, dz2, n);
   T2_LAUNCH_CHECK();
-  if (a->grads[W_PRENET1]) T2_TRY(gemm_rm(m, s, true, false, kPre, kPre, M, dz2, kPre, x1, kPre, a->grads[W_PRENET1], kPre, 0.f));
+  if (a->grads[W_PRENET1]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kPre, M, dz2, kPre, x1, kPre, a->grads[W_PRENET1], kPre, 0.f));
   // d_x1 = dz2 . W2  -> through dropout o relu of layer 1
-  T2_TRY(gemm_rm(m, s, false, false, M, kPre, kPre, dz2, kPre, m->w[W_PRENET1], kPre, dz1, kPre, 0.f));
+  T2_TRY(gemm_tc_rm(m, s, false, false, M, kPre, kPre, dz2, kPre, m->w[W_PRENET1], kPre, dz1, kPre, 0.f));
   prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(dz1, x1, dz1, n);
   T2_LAUNCH_CHECK();
-  if (a->grads[W_PRENET0]) T2_TRY(gemm_rm(m, s, true, false, kPre, kMel, M, dz1, kPre, a->frames, kMel, a->grads[W_PRENET0], kMel, 0.f));
+  if (a->grads[W_PRENET0]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kMel, M, dz1, kPre, a->frames, kMel, a->grads[W_PRENET0], kMel, 0.f));
   return T2_OK;
-}
-
-void blas_destroy(T2Model* m) {
-  if (m->blas) cublasDestroy((cublasHandle_t)m->blas);
-  m->blas = nullptr;
 }
 
 }  // namespace t2

@@ -1,13 +1,12 @@
 // T2_IMPL_PERSISTENT: the whole autoregressive decoder loop (model.py:381-454) as ONE persistent
 // cooperative sm_90a kernel.
 //
-//   * 128 CTAs (one per SM) in clusters, 512 threads each.  CTA c owns hidden units [8c, 8c+8) of BOTH
+//   * 128 CTAs (one per SM), 512 threads each.  CTA c owns hidden units [8c, 8c+8) of BOTH
 //     LSTM cells (attention_rnn, decoder_rnn): their cell state lives in registers for the whole loop,
 //     their gate pre-activations accumulate in a shared-memory fp32 tile across events.
 //   * "activation driven" schedule: whenever a new activation block (x2, ah, ctx, dh, x1) is complete,
-//     every CTA streams it ONCE through a shared-memory ring (bulk async copies on the TMA engine; the
-//     activation chunk is multicast to the CTAs of a cluster) together with the slices of every weight
-//     matrix that consumes it, and three warpgroups issue wgmma:
+//     every CTA streams it ONCE through a shared-memory ring (bulk async copies on the TMA engine)
+//     together with the slices of every weight matrix that consumes it, and three warpgroups issue wgmma:
 //        x2_t  -> att gates += W_ih^a[:, :256] x2                          -> ah_t, ac_t
 //        ah_t  -> dec gates += W_ih^d[:, :1024] ah ; att gates(t+1) += W_hh^a ah ; q = W_q ah
 //        ctx_t -> dec gates += W_ih^d[:, 1024:] ctx ; att gates(t+1) += W_ih^a[:, 256:] ctx ;
@@ -30,7 +29,8 @@
 //     filter bank evaluated as a tensor-core GEMM over an im2col image of the previous / cumulative
 //     weights (kept in shared memory across steps); energies, softmax and context per batch row on a
 //     CTA pair with warp-shuffle reductions.
-//   * events are separated by a grid-wide barrier (monotonic global counter, red.release / ld.acquire).
+//   * events are separated by a grid-wide barrier or by producer-scoped counters (monotonic global counters:
+//     fence.acq_rel + relaxed red to arrive, relaxed polls + one fence to wait).
 #include <stdlib.h>
 #include <string.h>
 
@@ -47,8 +47,8 @@ namespace {
 constexpr int kG = 128;               // CTAs
 constexpr int kThreads = 512;
 constexpr int kStages = 4;             // ring stages of the helper kernels (self test, backward GEMMs)
-constexpr int kMaxStages = 5;          // ring barriers reserved by the decoder kernel; it runs 4 stages up to T_enc = 896, else 3
-                                       // (5 never fit in 227 KiB; T2_STAGES = 3 forces the 3-stage ring)
+constexpr int kMaxStages = 4;          // the decoder kernel runs 4 stages up to T_enc = 896, else 3
+                                       // (T2_STAGES = 3 forces the 3-stage ring)
 constexpr int kRows = 64;             // batch rows per launch (zero padded)
 constexpr int kXChunkBytes = 2 * kRows * kChunkK * 2;    // [hi 64 rows | lo 64 rows] x 64 k fp16 = 16 KiB
 // accumulator columns (shared memory, fp32 [64 batch rows][kAccPitch]): att 0-31, dec 32-63, shared slot 64-79
@@ -236,32 +236,11 @@ __device__ __forceinline__ void poll_acquire(unsigned int* cnt, unsigned int tar
   asm volatile("fence.acq_rel.gpu;" ::: "memory");
 }
 
-// grid-wide barrier: one monotonically increasing arrival counter; arrive = red.release, wait = poll with
-// ld.acquire until the counter reaches this barrier's target (no reset / generation hop).  Also orders
-// the generic-proxy stores of the epilogues before the async-proxy (bulk copy) reads of the next event.
-__device__ __forceinline__ void grid_barrier(DecoderCtrl* ctrl, unsigned int& target, uint32_t cs, uint32_t rank) {
+// grid-wide barrier: one monotonically increasing arrival counter; arrive = arrive_release, wait = poll_acquire
+// until the counter reaches this barrier's target (no reset / generation hop).  Also orders the generic-proxy
+// stores of the epilogues before the async-proxy (bulk copy) reads of the next event.
+__device__ __forceinline__ void grid_barrier(DecoderCtrl* ctrl, unsigned int& target) {
   ptx::fence_proxy_async();
-  if (cs > 1) {
-    // hierarchical: hardware cluster barrier, one global arrival + one poller per cluster, cluster barrier
-    // again to release the other ranks (16-32 global participants instead of 128)
-    __threadfence();
-    ptx::cluster_sync_all();
-    target += gridDim.x / cs;
-    if (rank == 0 && threadIdx.x == 0) {
-      asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(&ctrl->bar_count) : "memory");
-      const unsigned long long t0 = clock64();
-      while (true) {
-        unsigned int c;
-        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(c) : "l"(&ctrl->bar_count) : "memory");
-        if ((int)(c - target) >= 0) break;
-        if (clock64() - t0 > kWatchdogCycles) watchdog_trap(ctrl, 100);
-      }
-      __threadfence();
-    }
-    ptx::cluster_sync_all();
-    ptx::fence_proxy_async();
-    return;
-  }
   __syncthreads();
   target += gridDim.x;
   if (threadIdx.x == 0) {
@@ -337,11 +316,10 @@ struct Ring {
   uint8_t* stage0;    // kStages buffers of kStageBytes each
   __device__ __forceinline__ uint8_t* stage(uint32_t s) const { return stage0 + s * kStageBytes; }
   uint64_t* full;     // [kStages]
-  uint64_t* empty;    // [kStages], released once by each MMA warpgroup of every CTA of the cluster
+  uint64_t* empty;    // [kStages], released once by each MMA warpgroup
   uint32_t p_stage, p_phase;   // producer cursor (thread 0 of warp 0)
   uint32_t c_stage, c_phase;   // consumer cursor (threads of the MMA warpgroups 1-3)
   uint64_t pol_x, pol_w;       // L2 eviction policies of the activation / weight streams
-  uint32_t cs, rank;           // cluster size (1 = no multicast) and this CTA's rank in it
   uint32_t pre;                // stages whose weight chunk was already issued for the upcoming event
   uint32_t ns;                 // number of stages
 };
@@ -394,12 +372,6 @@ __device__ __forceinline__ void plan_image_rows(const EventPlan& ep, int r, int&
   hi = lo = 0;
 }
 
-__device__ __forceinline__ void release_stage(const Ring& rg, uint32_t s) {
-  // this warpgroup is done with the stage (in every CTA of the cluster: the stage was filled by multicast)
-  if (rg.cs == 1) ptx::mbar_arrive(&rg.empty[s]);
-  else for (uint32_t r = 0; r < rg.cs; ++r) ptx::mbar_arrive_cluster(&rg.empty[s], r);
-}
-
 // One MMA warpgroup's consumer of an event: D (64 x 2n) = X_hi . B^T + X_lo . B^T over all `chunks` stages, where B is
 // the consumer's 2n weight-image rows [W_hi; W_lo] from row w_row0 of each stage; then both column halves of D are
 // added to the accumulator tile from column acol.  Each chunk's stage is released as soon as its MMAs are done: keeping
@@ -426,7 +398,7 @@ __device__ __forceinline__ void event_wg(Ring& rg, int chunks, uint32_t w_row0, 
     ptx::wg_commit();
     ptx::wg_wait<0>();
     ptx::wg_fence_regs<N / 2>(d);
-    if (leader) release_stage(rg, rg.c_stage);
+    if (leader) ptx::mbar_arrive(&rg.empty[rg.c_stage]);
     if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
   }
   const int wt = threadIdx.x & 127;
@@ -452,7 +424,7 @@ __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const u
   // that streams it, the bulk-copy producer fetches a chunk as soon as ITS 8 producers have arrived, so the stragglers'
   // skew and the arrival latency overlap with the streaming of the chunks that are already there.
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (ep.nrows == 0) {                 // this CTA (and its whole cluster) has no consumer of this activation
+  if (ep.nrows == 0) {                 // this CTA has no consumer of this activation
     if (threadIdx.x == 0 && next != nullptr && next->nrows != 0 && rg.pre == 0) prefetch_weights(rg, *next, w_img, ctrl);
     return;
   }
@@ -485,13 +457,7 @@ __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const u
           asm volatile("fence.acq_rel.gpu;" ::: "memory");
           ptx::fence_proxy_async();
         }
-        if (rg.cs == 1) {
-          ptx::bulk_g2s_hint(st, x_img + (size_t)i * kXChunkBytes, kXChunkBytes, &rg.full[rg.p_stage], rg.pol_x);
-        } else {   // every CTA of the cluster fetches 1/cs of the activation chunk and multicasts it to all
-          const uint32_t slice = kXChunkBytes / rg.cs;
-          ptx::bulk_g2s_mc_hint(st + rg.rank * slice, x_img + (size_t)i * kXChunkBytes + rg.rank * slice, slice,
-                                &rg.full[rg.p_stage], (uint16_t)((1u << rg.cs) - 1u), rg.pol_x);
-        }
+        ptx::bulk_g2s_hint(st, x_img + (size_t)i * kXChunkBytes, kXChunkBytes, &rg.full[rg.p_stage], rg.pol_x);
         if (++rg.p_stage == rg.ns) { rg.p_stage = 0; rg.p_phase ^= 1; }
       }
       rg.pre = 0;
@@ -510,7 +476,7 @@ __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const u
     } else {                              // no rows for this warpgroup: it still releases every stage it was counted for
       for (int i = 0; i < chunks; ++i) {
         mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
-        if ((threadIdx.x & 127) == 0) release_stage(rg, rg.c_stage);
+        if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&rg.empty[rg.c_stage]);
         if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
       }
     }
@@ -569,9 +535,8 @@ struct KParams {
   float* q;                         // (64, 128) fp32
   float* mel; float* gate; float* align; int32_t* mel_lengths; int32_t* n_steps;
   DecoderCtrl* ctrl;
-  int B, T, cap, infer, training, cluster, hier_barrier;
+  int B, T, cap, infer, training;
   int nstages;                      // operand ring stages (4, or 3 when T_enc > 896)
-  int chunk_ready;                  // 1: ah / dh hand-over through per-chunk arrival counters instead of barriers B1 / B4
   int b0, Btot;                     // this launch handles batch rows [b0, b0 + B) of Btot (dropout mask / Philox indexing)
   float gate_threshold, score_mask_value, p_att, p_dec;
   uint64_t seed;
@@ -629,11 +594,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   (void)s_red;
 
   rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
-  rg.cs = p.cluster; rg.rank = p.cluster > 1 ? ptx::cluster_ctarank() : 0;
   rg.pre = 0;
 
   if (tid == 0) {
-    for (int s = 0; s < p.nstages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs * rg.cs); }
+    for (int s = 0; s < p.nstages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
     ptx::fence_barrier_init();
   }
   for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;   // every MMA accumulates
@@ -650,12 +614,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   for (int i = tid; i < TP; i += kThreads) { s_pad0[i] = 0.f; s_pad1[i] = 0.f; }   // model.py:274-277
   ptx::fence_proxy_async();       // s_weff is read by wgmma (async proxy)
   __syncthreads();
-  if (p.cluster > 1) ptx::cluster_sync_all();   // peers' mbarriers are initialised before anyone multicasts
 
   const CtaPlan& plan = p.plans[cta];
   DecoderCtrl* ctrl = p.ctrl;
   unsigned int bar_target = 0;
-  const uint32_t bar_cs = p.hier_barrier ? rg.cs : 1;
   // epilogue role of this thread: quad = warp % 4, column group cg = warp / 4.  Quadrants 0/1 own batch rows
   // 0-63 (row = accumulator row); the threads of quadrants 2/3 (is_lo) take side jobs (dropout bits).
   const int quad = warp & 3, cg = warp >> 2;
@@ -735,8 +697,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         if (p.st.ga) stash_lstm(p.st.ga, p.st.ca, p.st.ha, t, p.Btot, p.b0 + row, cta * 8 + cg * 2, sg, c_att, hv);
       }
       T2_PROF(1);
-      if (p.chunk_ready) signal_counter(&ctrl->ah_count[cta >> 3], 1u);                        // this CTA's 8 columns of ah_t are written
-      else grid_barrier(ctrl, bar_target, bar_cs, rg.rank);                                     // B1: ah_t complete
+      signal_counter(&ctrl->ah_count[cta >> 3], 1u);                        // this CTA's 8 columns of ah_t are written
       T2_PROF(2);
     }
     // ======== E1: ah_t -> dec gates (part), next att gates (part), query ===== model.py:57, 366-369
@@ -767,7 +728,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         s_mask[row] = bits;
       }
       run_event(rg, plan.ev[1], p.ah_img, p.wimg, 16, s_acc, ctrl, nullptr,    // the attention phase reuses the ring as scratch
-                p.chunk_ready ? ctrl->ah_count : nullptr, 8u * (unsigned int)(t + 1));
+                ctrl->ah_count, 8u * (unsigned int)(t + 1));
       if (has_q && cg == 0 && !is_lo) {
         float g[8];
         acc_take8(s_acc, row, kColS, 0, g);
@@ -992,7 +953,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       T2_PROF(19);
     }
     T2_PROF(5);
-    grid_barrier(ctrl, bar_target, bar_cs, rg.rank);                                            // B3: ctx_t complete
+    grid_barrier(ctrl, bar_target);                                                             // B3: ctx_t complete
     T2_PROF(6);
     // ======== E2: ctx_t -> dec gates (rest), next att gates, projection (part); epilogue -> dh_t
     {
@@ -1025,15 +986,14 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         if (p.st.ga) stash_lstm(p.st.gd, p.st.cd, p.st.hd, t, p.Btot, p.b0 + row, cta * 8 + cg * 2, sg, c_dec, hv);
       }
       T2_PROF(8);
-      if (p.chunk_ready) signal_counter(&ctrl->dh_count[cta >> 3], 1u);                        // this CTA's 8 columns of dh_t are written
-      else grid_barrier(ctrl, bar_target, bar_cs, rg.rank);                                     // B4: dh_t complete
+      signal_counter(&ctrl->dh_count[cta >> 3], 1u);                        // this CTA's 8 columns of dh_t are written
       T2_PROF(9);
     }
     // ======== E3: dh_t -> projection (rest), next dec gates (part); epilogue -> mel, gate, x1
     {
       run_event(rg, plan.ev[3], p.dh_img, p.wimg, 16, s_acc, ctrl,
                 (!p.infer && t + 1 < p.cap) ? &plan.ev[0] : nullptr,    // INFER: the loop may end after this step
-                p.chunk_ready ? ctrl->dh_count : nullptr, 8u * (unsigned int)(t + 1));
+                ctrl->dh_count, 8u * (unsigned int)(t + 1));
       T2_PROF(10);
       if (tid == 0) *s_live = 0;
       float g[8];
@@ -1105,17 +1065,6 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     for (int b = tid; b < p.B; b += kThreads)
       if (!p.infer || !__ldcg(&ctrl->done[b])) p.mel_lengths[b] = ns;
     if (tid == 0) atomicMax(p.n_steps, ns);
-  }
-  if (p.cluster > 1) {
-    // every stage this CTA filled has been released by all peers (their commits arrive on OUR
-    // barriers) before anyone leaves, then leave together
-    if (tid == 0)
-      for (int s = 0; s < p.nstages; ++s) {
-        mbar_wait(&rg.empty[rg.p_stage], rg.p_phase ^ 1, ctrl, 204);
-        if (++rg.p_stage == rg.ns) { rg.p_stage = 0; rg.p_phase ^= 1; }
-      }
-    __syncthreads();
-    ptx::cluster_sync_all();
   }
 }
 
@@ -1325,60 +1274,18 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
     p.teacher_x2_img = timg;
   }
   p.nstages = persistent_stages(T);
-  {
-  }
-  {
-    const char* e = getenv("T2_CHUNK_READY");      // "0": full grid barriers B1 / B4 (cross-check / A-B)
-    p.chunk_ready = (e && !strcmp(e, "0")) ? 0 : 1;
-  }
   const size_t smem = persistent_smem_bytes(T, p.nstages);
   T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-  // TMA multicast of the activation chunks over clusters (T2_CLUSTER = 2 / 4 / 8): the stream is latency bound,
-  // not L2-bandwidth bound, and the multicast couples the rings of a cluster in lock step.  Default: no cluster.
-  int want = 1;
-  {
-    const char* e = getenv("T2_CLUSTER");
-    if (e) want = atoi(e);
-    if (want != 1 && want != 2 && want != 4 && want != 8) want = 1;
-  }
-  {
-    // the hierarchical (cluster barrier + 1 poller per cluster) variant is not combined with the split-phase B2
-    // barrier: kept in the source for reference, always off
-    p.hier_barrier = 0;
-  }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(kG); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute attrs[2];
-  // largest cluster size for which all 128 CTAs are co-resident (GPCs of 16-20 SMs: 8 does not always fit)
-  for (p.cluster = want; p.cluster > 1; p.cluster >>= 1) {
-    attrs[0].id = cudaLaunchAttributeClusterDimension;
-    attrs[0].val.clusterDim.x = p.cluster; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-    cfg.attrs = attrs; cfg.numAttrs = 1;
-    int max_clusters = 0;
-    if (cudaOccupancyMaxActiveClusters(&max_clusters, decoder_persistent_kernel, &cfg) == cudaSuccess &&
-        max_clusters * p.cluster >= kG)
-      break;
-    (void)cudaGetLastError();
-  }
-  int na = 0;
-  if (p.cluster > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = p.cluster; attrs[na].val.clusterDim.y = 1; attrs[na].val.clusterDim.z = 1; ++na;
-  }
-  attrs[na].id = cudaLaunchAttributeCooperative; attrs[na].val.cooperative = 1; ++na;   // co-residency of all 128 CTAs
-  cfg.attrs = attrs; cfg.numAttrs = na;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, decoder_persistent_kernel, p);
-  if (le != cudaSuccess && p.cluster > 1) {
-    // cooperative + cluster launch rejected: co-residency was established by the occupancy query above
-    (void)cudaGetLastError();
-    cfg.numAttrs = 1;
-    le = cudaLaunchKernelEx(&cfg, decoder_persistent_kernel, p);
-  }
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeCooperative; attr.val.cooperative = 1;   // co-residency of all 128 CTAs
+  cfg.attrs = &attr; cfg.numAttrs = 1;
+  const cudaError_t le = cudaLaunchKernelEx(&cfg, decoder_persistent_kernel, p);
   if (le != cudaSuccess) return fail(T2_ERR_CUDA, "persistent decoder launch failed: %s", cudaGetErrorString(le));
-  if (getenv("T2_VERBOSE")) fprintf(stderr, "[t2b200] persistent decoder: B=%d T_enc=%d cap=%d cluster=%d stages=%d chunk_ready=%d smem=%zu\n",
-                                    B, T, cap, p.cluster, p.nstages, p.chunk_ready, smem);
+  if (getenv("T2_VERBOSE")) fprintf(stderr, "[t2b200] persistent decoder: B=%d T_enc=%d cap=%d stages=%d smem=%zu\n",
+                                    B, T, cap, p.nstages, smem);
   g_launch_count++;
   return T2_OK;
 }
@@ -1403,7 +1310,7 @@ selftest_kernel(const uint8_t* x_img, const uint8_t* w_img, EventPlan ep, int ch
   float* s_acc = reinterpret_cast<float*>(sp);                 // [64][kAccPitch]
   rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pol_x = rg.pol_w = ptx::policy_evict_last();
-  rg.cs = 1; rg.rank = 0; rg.pre = 0; rg.ns = kStages;
+  rg.pre = 0; rg.ns = kStages;
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
     ptx::fence_barrier_init();
@@ -1521,7 +1428,7 @@ bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w
   float* s_acc = reinterpret_cast<float*>(sp);                 // [64][kAccPitch]
   rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pol_x = ptx::policy_evict_last(); rg.pol_w = ptx::policy_evict_first();
-  rg.cs = 1; rg.rank = 0; rg.pre = 0; rg.ns = kStages;
+  rg.pre = 0; rg.ns = kStages;
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
     ptx::fence_barrier_init();

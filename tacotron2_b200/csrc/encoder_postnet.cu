@@ -341,7 +341,7 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
   if (a->stash) {
     // autograd path: fp32 conv stack with the activations kept for the backward pass (train_layers.cu)
     const float* xl = nullptr;
-    T2_TRY(encoder_convs_train(m, a, s, &xl, &st_gates, &st_c, pl0));
+    T2_TRY(encoder_convs_train(m, a, s, &xl, &st_gates, &st_c));
     GemmArgs g;
     g.seg[0] = {xl, kEnc, m->enc_lstm_wih, kEnc, kEnc};
     g.M = B * T; g.N = 8 * kEncH; g.C = gin; g.ldc = 8 * kEncH; g.bias = m->enc_lstm_b;
@@ -388,7 +388,7 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
   }
   T2_CUDA(cudaMemsetAsync(hbuf0, 0, (size_t)2 * B * kEncH * 4, s));
   T2_CUDA(cudaMemsetAsync(cbuf, 0, (size_t)2 * B * kEncH * 4, s));
-  if (B <= 64 && m->sm_count >= 128 && getenv("T2_ENC_LSTM_STEPWISE") == nullptr) {
+  if (B <= 64 && m->sm_count >= 128) {
     // persistent recurrence: one cooperative launch for all T steps of both directions
     T2_CUDA(cudaMemsetAsync(hbuf1, 0, (size_t)2 * B * kEncH * 4, s));
     T2_CUDA(cudaMemsetAsync(lctrl, 0, 256, s));

@@ -1,5 +1,5 @@
-// General fp32-grade GEMM of the training path on the tensor cores (wgmma, split fp16), replacing every plain
-// library GEMM (cuBLAS sgemm) the backward pass used in round 1:
+// General fp32-grade GEMM of the training path on the tensor cores (wgmma, split fp16); every dense product of the
+// training path that is not a time-batched LSTM weight gradient (wgrad_tc.cu) or a conv input gradient (conv_tc.cu):
 //
 //     C (M x N, row-major, ldc) = op(A) . op(B) + beta * C        ta: A is stored (K x M), tb: B is stored (N x K)
 //

@@ -30,7 +30,6 @@ struct T2Model {
 
   // ---- packed operands of the persistent decoder kernel (owned; see decoder_persistent.cu) ----
   void* pk = nullptr;            // opaque PersistentPack*
-  void* blas = nullptr;          // cublasHandle_t: only for the T2_GEMM=cublas cross-check of the training path, created lazily
   void* gemm_ws = nullptr; size_t gemm_ws_bytes = 0;   // scratch of gemm_tc.cu (operand scales, split-K partial tiles)
 };
 
@@ -38,5 +37,4 @@ namespace t2 {
 int pack_model(T2Model* m, cudaStream_t s);          // (re)builds every packed copy
 int persistent_pack_create(T2Model* m, cudaStream_t s);
 void persistent_pack_destroy(T2Model* m);
-void blas_destroy(T2Model* m);
 }  // namespace t2

@@ -4,8 +4,10 @@
 // Conv stacks: activations live in a "padded rows" layout -- sequence b occupies rows [b (T+4) + 2, b (T+4) + 2 + T)
 // of a (B (T+4), C) channels-last matrix, the 2 rows either side are zero -- so the k=5 convolution is the sum of 5
 // plain GEMMs on row-shifted views of the same buffer (no im2col): forward z = sum_k X[r+k-2] W_k^T, input
-// gradient g_x = sum_k G_z[r+2-k] W_k, weight gradient dW_k = G_z^T X[r+k-2].  These are plain library GEMMs
-// (cuBLAS); BatchNorm statistics / normalisation / activation / dropout and their backward are our kernels.
+// gradient g_x = sum_k G_z[r+2-k] W_k, weight gradient dW_k = G_z^T X[r+k-2].  The forward runs these products on the
+// tensor-core GEMM (gemm_tc.cu), the input gradient on the implicit-GEMM conv engine (conv_tc.cu) and the weight gradient
+// on the wgmma wgrad engine (wgrad_tc.cu); BatchNorm statistics / normalisation / activation / dropout and their backward
+// are our kernels.
 // BiLSTM backward: reverse recurrence with one skinny GEMM + one elementwise kernel per step and direction.
 #include <stdlib.h>
 #include <string.h>
@@ -13,16 +15,11 @@
 #include "conv_tc.h"
 #include "decoder.h"
 #include "gemm_f32.cuh"
+#include "gemm_tc.h"
 #include "train_layers.h"
 #include "wgrad_tc.h"
 
 namespace t2 {
-
-int colsum_rm(T2Model* m, cudaStream_t s, const float* X, long ld, long rows, int cols, float* out);
-int gemm_rm(T2Model* m, cudaStream_t s, bool ta, bool tb, int M, int N, int K, const float* A, long lda, const float* B, long ldb,
-            float* C, long ldc, float beta);
-int gemm_rm_wgrad(T2Model* m, cudaStream_t s, bool ta, bool tb, int M, int N, int K, const float* A, long lda, const float* B, long ldb,
-                  float* C, long ldc, float beta);
 
 namespace {
 
@@ -278,27 +275,12 @@ struct ConvLayer {
   const float* wpk;                  // packed fp32 weights (cout, 5, cin)
   int wbase;                         // index of conv.weight in the state_dict table
   uint32_t site; const uint8_t* keep;
-  const uint8_t* wimg_fwd;           // tensor-core weight image of the forward conv (conv_tc.cu), packed by pack_model
   uint8_t** wimg_dgrad;              // storage of the flipped / transposed image of the input-gradient conv
 };
-// tensor-core conv path of the training forward / input gradient: planes scratch (null = row-shifted GEMMs through gemm_rm)
-struct TcTrain { __half* planes; };
-// T2_CONV_TRAIN: which training-mode convolutions run on the implicit-GEMM conv engine (conv_tc.cu) instead of 5 row-shifted
-// products on the general tensor-core GEMM (gemm_tc.cu through gemm_rm; cuBLAS only with T2_GEMM=cublas).  Default "dgrad": the
-// input gradients only -- the conv engine accumulates ~100-480 MMAs in one TMEM chain (3e-6 ... 1e-5 output error; the
-// accumulator update truncates) and near-constant BatchNorm channels amplify that to a 2e-2 gradient error on one
-// ill-conditioned test shape, so the training FORWARD uses gemm_tc (one chain per 64-wide K chunk, 7e-7);
-// "both" / "fwd" / "cublas" (= "gemm": neither on conv_tc) select the other combinations.
-int tc_train_mode() {
-  const char* e = getenv("T2_CONV_TRAIN");
-  if (!e) return 2;
-  if (e[0] == 'b') return 3;
-  if (e[0] == 'c') return 0;
-  if (e[0] == 'f') return 1;
-  if (e[0] == 'd') return 2;
-  return 3;
-}
-bool use_tc_train() { return tc_train_mode() != 0; }
+// The training FORWARD convs stay on 5 row-shifted gemm_tc products (one accumulation chain per 64-wide K chunk, 7e-7):
+// the conv engine accumulates ~100-480 MMAs in one chain (3e-6 ... 1e-5 output error; the accumulator update truncates)
+// and near-constant BatchNorm channels amplify that to a 2e-2 gradient error on one ill-conditioned test shape.  The
+// input gradients run on the conv engine.
 // Wd[ci][co][k'] = W[co][ci][4 - k']: the input gradient of a k=5 'same' conv is a conv of G_z with this kernel
 __global__ void flip_conv_w_kernel(const float* __restrict__ w, float* __restrict__ wd, int cout, int cin) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -319,15 +301,15 @@ __global__ void global_scale_kernel(const float* __restrict__ scale, int C, floa
 }
 int tc_train_conv(T2Model* m, const float* xp, int cin, const uint8_t* wimg, int cout, int B, int T, float* outp, __half* planes,
                   const float* in_scale, const float* out_scale, cudaStream_t s) {
-  // outp[padded rows][cout] = conv_k5(xp[padded rows][cin]) (no bias), split-fp16 tensor-core engine; the input may be
-  // pre-scaled by the device scalar *in_scale (a power of two) with out_scale[c] = 1 / *in_scale undoing it
+  // outp[padded rows][cout] = conv_k5(xp[padded rows][cin]) (no bias), split-fp16 tensor-core engine; the input is
+  // pre-scaled by the device scalar *in_scale (a power of two) and out_scale[c] = 1 / *in_scale undoes it
   const int c_pad = cin < 128 ? 128 : cin;
   T2_TRY(tc_rows_to_planes_scaled(xp + (long)kPadRows * cin, (long)(T + 2 * kPadRows) * cin, cin, c_pad, nullptr, B, T, planes,
                                   in_scale, s));
   TcConvArgs c;
   memset(&c, 0, sizeof(c));
   c.in = planes; c.cin_pad = c_pad; c.wimg = wimg; c.taps = kConvK; c.B = B; c.T = T; c.cout = cout; c.nt_rows = cout >= 128 ? 128 : 80;
-  c.scale = out_scale ? out_scale : m->ones; c.shift = m->zeros; c.act = 0; c.out_mode = 1;
+  c.scale = out_scale; c.shift = m->zeros; c.act = 0; c.out_mode = 1;
   c.out_f32 = outp + (long)kPadRows * cout; c.ldo = cout; c.out_seq_rows = T + 2 * kPadRows;
   return tc_conv(c, s);
 }
@@ -402,16 +384,12 @@ int conv_wgrad_tc(const ConvLayer& L, int B, int T, const float* gz_p, const flo
 }
 
 int conv_fwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_t seed, const float* xp, float* zp,
-             float* stats, float* yp, float* y_plain, bool update_running, float* partial, const TcTrain* tc, cudaStream_t s) {
+             float* stats, float* yp, float* y_plain, bool update_running, float* partial, cudaStream_t s) {
   const long Mp = (long)B * (T + 2 * kPadRows);
   const int Me = (int)(Mp - 2 * kPadRows);
-  if (tc && (tc_train_mode() & 1)) {
-    T2_TRY(tc_train_conv(m, xp, L.cin, L.wimg_fwd, L.cout, B, T, zp, tc->planes, nullptr, nullptr, s));
-  } else {
-    for (int k = 0; k < kConvK; ++k)
-      T2_TRY(gemm_rm(m, s, false, true, Me, L.cout, L.cin, xp + (long)k * L.cin, L.cin, L.wpk + (long)k * L.cin, (long)kConvK * L.cin,
-                     zp + (long)kPadRows * L.cout, L.cout, k ? 1.f : 0.f));
-  }
+  for (int k = 0; k < kConvK; ++k)
+    T2_TRY(gemm_tc_rm(m, s, false, true, Me, L.cout, L.cin, xp + (long)k * L.cin, L.cin, L.wpk + (long)k * L.cin, (long)kConvK * L.cin,
+                      zp + (long)kPadRows * L.cout, L.cout, k ? 1.f : 0.f));
   {
     float* rm = const_cast<float*>(m->w[L.wbase + 4]); float* rv = const_cast<float*>(m->w[L.wbase + 5]);
     const long M = (long)B * T;
@@ -436,10 +414,11 @@ int conv_fwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
 }
 
 // g: gradient wrt the layer output (padded or plain rows).  Writes gx_p (padded rows, garbage in the pad rows) when
-// non-null, and the gradients of conv.weight / conv.bias / bn.weight / bn.bias.
+// non-null, and the gradients of conv.weight / conv.bias / bn.weight / bn.bias.  planes: scratch of
+// tc_planes_bytes(B, T, 512) for the input-gradient conv.
 int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_t seed, const float* g, int g_padded,
              const float* xp, const float* zp, const float* stats, const float* yp, float* gz_p, float* gx_p, float* sums, float* dwpk,
-             const float* ones, float* const* G, const WgConvWs* wg, const TcTrain* tc, cudaStream_t s) {
+             const float* ones, float* const* G, const WgConvWs* wg, __half* planes, cudaStream_t s) {
   const long Mp = (long)B * (T + 2 * kPadRows);
   const int Me = (int)(Mp - 2 * kPadRows);
   float* partial = sums + 2 * L.cout;      // (kRedSplit, 2, cout) scratch behind the two result rows
@@ -458,17 +437,17 @@ int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
   if (wg) {   // weight + bias gradient on our wgmma engine
     T2_TRY(conv_wgrad_tc(L, B, T, gz_p, xp, G[L.wbase], G[L.wbase + 1], *wg, s));
   } else {
-    if (G[L.wbase + 1]) T2_TRY(colsum_rm(m, s, gz_p, L.cout, Mp, L.cout, G[L.wbase + 1]));      // d conv bias
+    if (G[L.wbase + 1]) T2_TRY(colsum_f32(m, s, gz_p, L.cout, Mp, L.cout, G[L.wbase + 1]));      // d conv bias
     if (G[L.wbase]) {
       for (int k = 0; k < kConvK; ++k)
-        T2_TRY(gemm_rm_wgrad(m, s, true, false, L.cout, L.cin, Me, gz_p + (long)kPadRows * L.cout, L.cout, xp + (long)k * L.cin, L.cin,
-                       dwpk + (long)k * L.cin, (long)kConvK * L.cin, 0.f));
+        T2_TRY(gemm_tc_rm(m, s, true, false, L.cout, L.cin, Me, gz_p + (long)kPadRows * L.cout, L.cout, xp + (long)k * L.cin, L.cin,
+                          dwpk + (long)k * L.cin, (long)kConvK * L.cin, 0.f));
       const long nw = (long)L.cout * L.cin * kConvK;
       unpack_conv_grad_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(dwpk, G[L.wbase], L.cout, L.cin, kConvK);
       T2_LAUNCH_CHECK();
     }
   }
-  if (gx_p && tc && wg && (tc_train_mode() & 2)) {   // input gradient = conv of G_z with the flipped / transposed kernel on the tensor-core engine
+  if (gx_p && wg) {   // input gradient = conv of G_z with the flipped / transposed kernel on the tensor-core engine
     // G_z is pre-scaled by a power of two (from the per-channel statistics of the weight-gradient pass): fp16 range
     global_scale_kernel<<<1, 256, 0, s>>>(wg->scale, L.cout, wg->colsum, wg->stat);      // colsum[0] = s_g, stat[0..512) = 1 / s_g
     T2_LAUNCH_CHECK();
@@ -477,11 +456,11 @@ int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
     flip_conv_w_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(m->w[L.wbase], m->dgrad_tmp, L.cout, L.cin);
     T2_LAUNCH_CHECK();
     T2_TRY(tc_pack_weights(m->dgrad_tmp, L.cin, L.cout, kConvK, L.cin >= 128 ? 128 : 80, L.wimg_dgrad, s));
-    T2_TRY(tc_train_conv(m, gz_p, L.cout, *L.wimg_dgrad, L.cin, B, T, gx_p, tc->planes, wg->colsum, wg->stat, s));
-  } else if (gx_p) {
+    T2_TRY(tc_train_conv(m, gz_p, L.cout, *L.wimg_dgrad, L.cin, B, T, gx_p, planes, wg->colsum, wg->stat, s));
+  } else if (gx_p) {   // without the weight-gradient engine's channel statistics (T2_WGRAD=cublas): row-shifted GEMMs
     for (int k = 0; k < kConvK; ++k)
-      T2_TRY(gemm_rm(m, s, false, false, Me, L.cin, L.cout, gz_p + (long)(2 * kPadRows - k) * L.cout, L.cout, L.wpk + (long)k * L.cin,
-                     (long)kConvK * L.cin, gx_p + (long)kPadRows * L.cin, L.cin, k ? 1.f : 0.f));
+      T2_TRY(gemm_tc_rm(m, s, false, false, Me, L.cin, L.cout, gz_p + (long)(2 * kPadRows - k) * L.cout, L.cout, L.wpk + (long)k * L.cin,
+                        (long)kConvK * L.cin, gx_p + (long)kPadRows * L.cin, L.cin, k ? 1.f : 0.f));
   }
   return T2_OK;
 }
@@ -628,7 +607,7 @@ static void post_layers(T2Model* m, int training, const uint8_t* keep, int B, in
     L[i].cin = kPostCh[i]; L[i].cout = kPostCh[i + 1]; L[i].act = i == 4 ? ACT_NONE : ACT_TANH; L[i].dropout = training;
     L[i].wpk = m->post_conv_w[i]; L[i].wbase = W_POST_CONV0 + 7 * i; L[i].site = 2000 + i;
     L[i].keep = (training && keep) ? keep + (size_t)i * B * kPost * T : nullptr;     // [(B,512,T)] x 4 + (B,80,T)
-    L[i].wimg_fwd = m->tc_post_conv[i]; L[i].wimg_dgrad = &m->tc_dgrad_post[i];
+    L[i].wimg_dgrad = &m->tc_dgrad_post[i];
   }
 }
 
@@ -645,14 +624,9 @@ int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
   T2_LAUNCH_CHECK();
   ConvLayer L[5];
   post_layers(m, a->training, a->keep, B, T, L);
-  TcTrain tcw; const TcTrain* tc = nullptr;
-  if (use_tc_train()) {   // a->ws is at least postnet_ws_bytes(): room for the input planes of one layer
-    if (a->ws_bytes < tc_planes_bytes(B, T, kPost) + 512) return fail(T2_ERR_WORKSPACE, "postnet workspace too small");
-    tcw.planes = (__half*)a256((size_t)a->ws); tc = &tcw;
-  }
   for (int i = 0; i < 5; ++i)
     T2_TRY(conv_fwd(m, L[i], B, T, a->training, a->seed, st.x[i], st.z[i], st.stats[i], st.x[i + 1], nullptr, a->training != 0,
-                    st.stats[i] + 2 * L[i].cout, tc, s));
+                    st.stats[i] + 2 * L[i].cout, s));
   rows_to_bct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.x[5], a->add_residual ? st.x[0] : nullptr, a->mel_post, B, T, kMel);
   T2_LAUNCH_CHECK();
   return T2_OK;
@@ -686,8 +660,7 @@ int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
     if (!(e && e[0] == 'c')) { wgconv_bytes(B, T, &wgws, (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023)); wg = &wgws; }
   }
   p = (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023) + wgconv_bytes(B, T, nullptr, nullptr);
-  TcTrain tcw; const TcTrain* tc = nullptr;
-  if (use_tc_train()) { tcw.planes = (__half*)a256((size_t)p); tc = &tcw; }
+  __half* planes = (__half*)a256((size_t)p);
   fill1_kernel<<<(unsigned)((Mp + 255) / 256), 256, 0, s>>>(ones, 1.f, (long)Mp);
   T2_LAUNCH_CHECK();
   const long n = (long)B * T * kMel;
@@ -703,7 +676,7 @@ int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
       T2_LAUNCH_CHECK();
     }
     T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.x[i], st.z[i], st.stats[i], st.x[i + 1], gz, gx, sums, dwpk,
-                    ones, a->grads, wg, tc, s));
+                    ones, a->grads, wg, planes, s));
     g = gx; g_padded = 1;
     gx = gx == gxa ? gxb : gxa;
   }
@@ -724,12 +697,12 @@ static void enc_layers(T2Model* m, int training, const uint8_t* keep, int B, int
     L[i].cin = kEnc; L[i].cout = kEnc; L[i].act = ACT_RELU; L[i].dropout = training;
     L[i].wpk = m->enc_conv_w[i]; L[i].wbase = W_ENC_CONV0 + 7 * i; L[i].site = 1000 + i;
     L[i].keep = (training && keep) ? keep + (size_t)i * B * kEnc * T : nullptr;
-    L[i].wimg_fwd = m->tc_enc_conv[i]; L[i].wimg_dgrad = &m->tc_dgrad_enc[i];
+    L[i].wimg_dgrad = &m->tc_dgrad_enc[i];
   }
 }
 
 // conv stack of the training forward: fills the stash and returns the LSTM input rows (B*T, 512)
-int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, const float** xl, float** gates, float** cst, void* planes) {
+int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, const float** xl, float** gates, float** cst) {
   const int B = a->B, T = a->T;
   if (a->stash_bytes < encoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder stash too small");
   EncStash st;
@@ -742,11 +715,9 @@ int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, cons
   T2_LAUNCH_CHECK();
   ConvLayer L[3];
   enc_layers(m, a->training, a->keep, B, T, L);
-  TcTrain tcw; const TcTrain* tc = nullptr;
-  if (use_tc_train() && planes) { tcw.planes = (__half*)planes; tc = &tcw; }
   for (int i = 0; i < 3; ++i)
     T2_TRY(conv_fwd(m, L[i], B, T, a->training, a->seed, st.cs.x[i], st.cs.z[i], st.cs.stats[i], st.cs.x[i + 1], i == 2 ? st.xl : nullptr,
-                    a->training != 0, st.cs.stats[i] + 2 * L[i].cout, tc, s));
+                    a->training != 0, st.cs.stats[i] + 2 * L[i].cout, s));
   *xl = st.xl; *gates = st.gates; *cst = st.cst;
   return T2_OK;
 }
@@ -797,8 +768,7 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
     if (!(e && e[0] == 'c')) { wgconv_bytes(B, T, &wgws, (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023)); wg = &wgws; }
   }
   p = (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023) + wgconv_bytes(B, T, nullptr, nullptr);
-  TcTrain tcw; const TcTrain* tc = nullptr;
-  if (use_tc_train()) { tcw.planes = (__half*)a256((size_t)p); tc = &tcw; }
+  __half* planes = (__half*)a256((size_t)p);
   fill1_kernel<<<(unsigned)((n_ones + 255) / 256), 256, 0, s>>>(ones, 1.f, (long)n_ones);
   T2_LAUNCH_CHECK();
   T2_CUDA(cudaMemsetAsync(g_c, 0, (size_t)2 * 64 * kEncH * 4, s));
@@ -819,15 +789,15 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   for (int dir = 0; dir < 2; ++dir) {
     const int wb = W_ENC_LSTM + 4 * dir;
     const float* dGd = dG + (size_t)dir * 4 * kEncH;          // rows (b, t), row stride 2048
-    if (G[wb]) T2_TRY(gemm_rm(m, s, true, false, 4 * kEncH, kEnc, BT, dGd, 8 * kEncH, st.xl, kEnc, G[wb], kEnc, 0.f));
-    if (G[wb + 1]) T2_TRY(gemm_rm(m, s, true, false, 4 * kEncH, kEncH, BT, dGd, 8 * kEncH, hp + (size_t)dir * kEncH, kEnc, G[wb + 1], kEncH, 0.f));
+    if (G[wb]) T2_TRY(gemm_tc_rm(m, s, true, false, 4 * kEncH, kEnc, BT, dGd, 8 * kEncH, st.xl, kEnc, G[wb], kEnc, 0.f));
+    if (G[wb + 1]) T2_TRY(gemm_tc_rm(m, s, true, false, 4 * kEncH, kEncH, BT, dGd, 8 * kEncH, hp + (size_t)dir * kEncH, kEnc, G[wb + 1], kEncH, 0.f));
     if (G[wb + 2] || G[wb + 3]) {
-      T2_TRY(colsum_rm(m, s, dGd, 8 * kEncH, BT, 4 * kEncH, tmp));
+      T2_TRY(colsum_f32(m, s, dGd, 8 * kEncH, BT, 4 * kEncH, tmp));
       if (G[wb + 2]) T2_CUDA(cudaMemcpyAsync(G[wb + 2], tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
       if (G[wb + 3]) T2_CUDA(cudaMemcpyAsync(G[wb + 3], tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
     }
     // gradient wrt the LSTM input: dG_dir (BT x 1024) . W_ih_dir (1024 x 512)
-    T2_TRY(gemm_rm(m, s, false, false, BT, kEnc, 4 * kEncH, dGd, 8 * kEncH, m->w[wb], kEnc, dxl, kEnc, dir ? 1.f : 0.f));
+    T2_TRY(gemm_tc_rm(m, s, false, false, BT, kEnc, 4 * kEncH, dGd, 8 * kEncH, m->w[wb], kEnc, dxl, kEnc, dir ? 1.f : 0.f));
   }
   // ---- conv stack ----
   ConvLayer L[3];
@@ -837,7 +807,7 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   for (int i = 2; i >= 0; --i) {
     const bool need_gx = i > 0 || a->d_embedded || (a->text && G[W_EMB]);
     T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.cs.x[i], st.cs.z[i], st.cs.stats[i], st.cs.x[i + 1], gz,
-                    need_gx ? gx : nullptr, sums, dwpk, ones, G, wg, tc, s));
+                    need_gx ? gx : nullptr, sums, dwpk, ones, G, wg, planes, s));
     g = gx; g_padded = 1;
     gx = gx == gxa ? gxb : gxa;
   }

@@ -10,8 +10,7 @@ size_t postnet_backward_ws_bytes(int B, int T);
 int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s);
 
 size_t encoder_stash_bytes(int B, int T);
-int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, const float** xl, float** gates, float** cst,
-                        void* planes /* scratch of tc_planes_bytes(B, T, 512) for the tensor-core convs, or null */);
+int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, const float** xl, float** gates, float** cst);
 int encoder_stash_output(const T2EncoderArgs* a, cudaStream_t s);
 size_t encoder_backward_ws_bytes(int B, int T);
 int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s);

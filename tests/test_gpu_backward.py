@@ -52,7 +52,7 @@ def oracle_decoder_grads(sd, memory, mels, lens, pk, ak, dk, d_mel, d_gate, d_al
                                                        (4, 150, 9, False, False), (64, 33, 5, True, False)])
 def test_decoder_backward_vs_oracle_autograd(B, Te, T, training, use_align, gemm, monkeypatch):
     """gemm = tc: the reverse recurrence's skinny GEMMs and the time-batched LSTM weight gradients on the wgmma
-    split-fp16 engines (default); simt: fp32 SIMT kernels / plain cuBLAS fp32 GEMMs (cross-check)."""
+    split-fp16 engines (default); simt: fp32 SIMT kernels / separate gemm_tc products and column sums (cross-check)."""
     monkeypatch.setenv("T2_BWD_GEMM", gemm)
     monkeypatch.setenv("T2_WGRAD", "tc" if gemm == "tc" else "cublas")
     sd = synth_state_dict(seed=21, scale=2.0)
