@@ -434,7 +434,8 @@ class Engine:
     def postnet(self, mel_btc, lengths=None, add_residual=True, training=False, keep=None, stash=None, seed=None):
         """mel_btc: (B, T, 80) time-major rows (batch stride may exceed T*80).  Returns (B, 80, T)."""
         L = _capi.lib()
-        assert mel_btc.dtype == torch.float32 and mel_btc.stride(2) == 1 and mel_btc.stride(1) == mel_btc.shape[2]
+        # a single frame (T = 1) may carry any time stride: torch calls such a tensor contiguous and keeps it as it is
+        assert mel_btc.dtype == torch.float32 and mel_btc.stride(2) == 1 and (mel_btc.stride(1) == mel_btc.shape[2] or mel_btc.shape[1] == 1)
         B, T = int(mel_btc.shape[0]), int(mel_btc.shape[1])
         out = torch.empty(B, self.hp.n_mel_channels, T, device=self.device, dtype=torch.float32)
         ws = self._workspace("post", L.t2_postnet_workspace_bytes(self.handle, B, T))

@@ -288,16 +288,26 @@ __global__ void flip_conv_w_kernel(const float* __restrict__ w, float* __restric
   const int k = (int)(i % kConvK); const long r = i / kConvK; const int ci = (int)(r % cin); const int co = (int)(r / cin);
   wd[((long)ci * cout + co) * kConvK + (kConvK - 1 - k)] = w[i];
 }
-// s_g = the smallest per-channel power-of-two scale (= the scale of the largest channel); out_vec[0..512) = 1 / s_g
-__global__ void global_scale_kernel(const float* __restrict__ scale, int C, float* __restrict__ s_g, float* __restrict__ out_vec) {
-  __shared__ float sm;
-  if (threadIdx.x == 0) {
-    float m = scale[0];
-    for (int i = 1; i < C; ++i) m = fminf(m, scale[i]);
-    sm = m; *s_g = m;
-  }
+// s_g = the power-of-two scale of the largest channel of G_z: max |G_z| = f 2^e with f in [0.5, 1) gives s_g = 2^-e, with
+// the clamp of the per-channel scales (wg_colstats_finalize_kernel).  It is read from the column maxima wg_colstats left
+// in its partials, so all-zero channels play no part (their own scale is 1, which would win a minimum over the channel
+// scales whenever max |G_z| < 0.5 and leave tiny gradients unscaled, in the fp16 subnormal range); s_g = 1 when G_z is
+// all zero.  out_vec[0..512) = 1 / s_g.  part and out_vec may alias: every read precedes the first barrier.
+__global__ void __launch_bounds__(256) global_scale_kernel(const float* part, int C, float* __restrict__ s_g, float* out_vec) {
+  __shared__ float red[256];
+  float mx = 0.f;
+  for (int i = threadIdx.x; i < kWgStatSplit * C; i += 256) mx = fmaxf(mx, part[(long)(i / C) * 2 * C + i % C]);
+  red[threadIdx.x] = mx;
   __syncthreads();
-  for (int i = threadIdx.x; i < 512; i += blockDim.x) out_vec[i] = 1.f / sm;
+  for (int h = 128; h > 0; h >>= 1) {
+    if (threadIdx.x < h) red[threadIdx.x] = fmaxf(red[threadIdx.x], red[threadIdx.x + h]);
+    __syncthreads();
+  }
+  int e = 0;
+  if (red[0] > 0.f && red[0] < 3.0e38f) frexpf(red[0], &e);
+  e = e < -100 ? -100 : (e > 100 ? 100 : e);
+  if (threadIdx.x == 0) *s_g = ldexpf(1.f, -e);
+  for (int i = threadIdx.x; i < 512; i += 256) out_vec[i] = ldexpf(1.f, e);
 }
 int tc_train_conv(T2Model* m, const float* xp, int cin, const uint8_t* wimg, int cout, int B, int T, float* outp, __half* planes,
                   const float* in_scale, const float* out_scale, cudaStream_t s) {
@@ -449,7 +459,7 @@ int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
   }
   if (gx_p && wg) {   // input gradient = conv of G_z with the flipped / transposed kernel on the tensor-core engine
     // G_z is pre-scaled by a power of two (from the per-channel statistics of the weight-gradient pass): fp16 range
-    global_scale_kernel<<<1, 256, 0, s>>>(wg->scale, L.cout, wg->colsum, wg->stat);      // colsum[0] = s_g, stat[0..512) = 1 / s_g
+    global_scale_kernel<<<1, 256, 0, s>>>(wg->stat, L.cout, wg->colsum, wg->stat);       // colsum[0] = s_g, stat[0..512) = 1 / s_g
     T2_LAUNCH_CHECK();
     if (!m->dgrad_tmp) T2_CUDA(cudaMalloc((void**)&m->dgrad_tmp, (size_t)kPost * kPost * kConvK * 4));
     const long nw = (long)L.cout * L.cin * kConvK;

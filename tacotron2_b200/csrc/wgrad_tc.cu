@@ -27,7 +27,7 @@ constexpr int kBBytes = 2 * kTN * 128;               // 64 KB
 constexpr int kStageB = kABytes + kBBytes;           // 96 KB
 constexpr int kWgStages = 2;
 constexpr int kWgThreads = 384;                      // warp 0: producer; warpgroups 1 / 2: MMA + epilogue
-constexpr int kStatSplit = 64;
+constexpr int kStatSplit = kWgStatSplit;
 
 // ---- column statistics of dG (rows x 4096): max |.| and sum per column ---------------------------------
 __global__ void __launch_bounds__(256) wg_colstats_kernel(const float* __restrict__ x, long rows, int C, float* __restrict__ part) {

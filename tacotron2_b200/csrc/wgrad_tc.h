@@ -15,6 +15,8 @@ struct WgJob {                          // one CTA: a 128 x 256 output tile of o
 };
 constexpr int kWgTileA = 2 * 128 * 128, kWgTileB = 2 * 256 * 128;   // bytes of one A / B tile of one chunk
 int wg_run_jobs(const std::vector<WgJob>& jobs, WgJob* jobs_dev, cudaStream_t s);
+// wg_colstats leaves its per-split partials in stat_ws: kWgStatSplit x [column max |x| (C) | column sum (C)]
+constexpr int kWgStatSplit = 64;
 size_t wg_colstats_ws_bytes(int C);
 int wg_colstats(const float* x, long rows, int C, float* stat_ws, float* scale, float* inv_scale, float* colsum, cudaStream_t s);
 int wg_transpose_images(const float* src, long ld, long row0, long rows_total, int chunk_rows, int nchunks, int C, int TR,
