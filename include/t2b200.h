@@ -163,6 +163,33 @@ typedef struct T2DecoderArgs {
 size_t t2_decoder_workspace_bytes(const T2Model* m, int32_t B, int32_t T_enc, int32_t n_steps_cap);
 int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);
 
+/* ---- Resumable decoder stream: the INFER loop of t2_decoder_run in chunks of steps -------------
+ * The same persistent kernel stops after a number of steps and resumes exactly where it stopped, so
+ * the steps of all chunks together compute bit for bit what one t2_decoder_run computes (dropout is
+ * keyed by the absolute step).  Everything that lives across a step boundary is kept in the caller's
+ * `state` buffer (t2_decoder_stream_state_bytes), one block per 64-row slice: several streams can be
+ * alive on one model at a time, and t2_decoder_run's workspace is not used.
+ *   dec: as for t2_decoder_run with mode = INFER (memory_lengths, teacher_prenet, att_keep, dec_keep,
+ *        ws and stash are not used).  mel / gate / align are the full n_steps_cap-sized buffers; each
+ *        run writes its steps at their absolute indices.  mel_lengths[b] = -1 while row b is live,
+ *        then its length, as t2_decoder_run.  T2_IMPL_STEPWISE and encoder lengths the persistent
+ *        kernel does not take are refused with T2_ERR_UNSUPPORTED.
+ *   status: device int32 (2 x ceil(B / 64)): [steps run, stopped] per slice, written by every run.
+ * begin zeroes the state, sets mel_lengths to -1 and computes the processed memory; it does not
+ * touch mel / gate / align (zero them first, as for t2_decoder_run).  run advances every slice that
+ * has not stopped by up to n_steps steps (one launch per slice, no host synchronisation);
+ * status_host is the caller's copy of `status` after the previous run (NULL after begin): slices it
+ * marks stopped are not launched again. */
+typedef struct T2DecoderStreamArgs {
+  T2DecoderArgs dec;
+  void* state; size_t state_bytes;
+  int32_t* status;
+} T2DecoderStreamArgs;
+size_t t2_decoder_stream_state_bytes(const T2Model* m, int32_t B, int32_t T_enc);
+int    t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stream);
+int    t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n_steps, const int32_t* status_host,
+                             void* stream);
+
 /* ---- Decoder backward (the autograd graph of Decoder.forward, model.py:381-416) ----------------
  * Reverse-time recurrence over the stash of a TEACHER run with the same memory / teacher_prenet / masks /
  * seed, then the time-batched weight gradients.  B <= 64.

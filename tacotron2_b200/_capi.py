@@ -24,6 +24,7 @@ EXPORTS = [
     "t2_clip_adam_workspace_bytes", "t2_clip_adam_step", "t2_amp_adam_workspace_bytes", "t2_amp_adam_step",
     "t2_loss_workspace_bytes", "t2_tacotron2_loss",
     "t2_mel_spectrogram_frames", "t2_mel_spectrogram_workspace_bytes", "t2_mel_spectrogram", "t2_collate",
+    "t2_decoder_stream_state_bytes", "t2_decoder_stream_begin", "t2_decoder_stream_run",
 ]
 
 
@@ -62,6 +63,10 @@ class T2DecoderArgs(C.Structure):
                 ("mel_lengths", C.c_void_p), ("n_steps", C.c_void_p),
                 ("ws", C.c_void_p), ("ws_bytes", C.c_size_t),
                 ("stash", C.c_void_p), ("stash_bytes", C.c_size_t)]
+
+
+class T2DecoderStreamArgs(C.Structure):
+    _fields_ = [("dec", T2DecoderArgs), ("state", C.c_void_p), ("state_bytes", C.c_size_t), ("status", C.c_void_p)]
 
 
 class T2DecoderBwdArgs(C.Structure):
@@ -169,6 +174,10 @@ def lib():
         getattr(L, n).argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     L.t2_encoder_forward.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_decoder_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderArgs), C.c_void_p]
+    L.t2_decoder_stream_state_bytes.restype = C.c_size_t
+    L.t2_decoder_stream_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    L.t2_decoder_stream_begin.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_void_p]
+    L.t2_decoder_stream_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_int32, C.c_void_p, C.c_void_p]
     L.t2_postnet_forward.argtypes = [C.c_void_p, C.POINTER(T2PostnetArgs), C.c_void_p]
     L.t2_clip_adam_workspace_bytes.restype = C.c_size_t
     L.t2_clip_adam_workspace_bytes.argtypes = [C.c_int64, C.c_int32]

@@ -338,6 +338,12 @@ class Engine:
         self._last_decoder_args = (a, memory, len32, teacher_prenet, pk, ak, dk, ws, mel, gate, align, mel_lengths, n_steps)
         return mel, gate, align, mel_lengths, n_steps
 
+    def decoder_stream(self, memory, n_steps_cap, prenet_keep=None, gate_threshold=0.5, score_mask_value=-float("inf"),
+                       impl=None, seed=None):
+        """Begins a resumable INFER run of the persistent decoder (t2_decoder_stream_begin); see DecoderStream."""
+        return DecoderStream(self, memory, n_steps_cap, prenet_keep, gate_threshold, score_mask_value,
+                             self.impl if impl is None else impl, next_seed() if seed is None else seed)
+
     def decoder_profile(self):
         """Per-phase SM cycles of the last persistent decoder run: dict phase -> [cta0, cta60, cta100]."""
         a = self._last_decoder_args[0]
@@ -474,3 +480,55 @@ class Engine:
                                         next_seed(), self.impl if impl is None else impl, mel.data_ptr(),
                                         lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
         return mel, lens, ns
+
+
+class DecoderStream:
+    """One resumable decoder run: full-size output buffers (mel (B, cap, 80), gate (B, cap), align (B, cap, T_enc),
+    mel_lengths (B,) with -1 for live rows) and the per-stream state buffer that carries everything across a chunk
+    boundary.  ``run(n)`` advances every live 64-row slice by up to n steps and takes the one host sync of the chunk."""
+
+    def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed):
+        L = _capi.lib()
+        dev = eng.device
+        self.eng = eng
+        self.memory = memory.to(device=dev, dtype=torch.float32).contiguous()
+        B, T = int(self.memory.shape[0]), int(self.memory.shape[1])
+        self.B, self.T_enc, self.cap = B, T, int(cap)
+        f32 = dict(device=dev, dtype=torch.float32)
+        self.mel = torch.zeros(B, self.cap, eng.hp.n_mel_channels, **f32)
+        self.gate = torch.zeros(B, self.cap, **f32)
+        self.align = torch.zeros(B, self.cap, T, **f32)
+        self.mel_lengths = torch.empty(B, device=dev, dtype=torch.int32)
+        self.n_steps = torch.zeros(1, device=dev, dtype=torch.int32)
+        self.n_slices = (B + 63) // 64
+        self.status = torch.zeros(2 * self.n_slices, device=dev, dtype=torch.int32)
+        self.status_host = None                      # the caller's copy of `status` after the last run
+        self.state = torch.empty(int(L.t2_decoder_stream_state_bytes(eng.handle, B, T)), dtype=torch.uint8, device=dev)
+        self.keep = _u8(prenet_keep, dev)
+        a = _capi.T2DecoderStreamArgs()
+        d = a.dec
+        d.mode, d.impl, d.training = _capi.MODE_INFER, impl, 0
+        d.memory, d.B, d.T_enc, d.n_steps_cap = self.memory.data_ptr(), B, T, self.cap
+        d.prenet_keep = self.keep.data_ptr() if self.keep is not None else None
+        d.seed = seed
+        d.gate_threshold, d.score_mask_value = float(gate_threshold), float(score_mask_value)
+        d.mel, d.gate, d.align = self.mel.data_ptr(), self.gate.data_ptr(), self.align.data_ptr()
+        d.mel_lengths, d.n_steps = self.mel_lengths.data_ptr(), self.n_steps.data_ptr()
+        a.state, a.state_bytes, a.status = self.state.data_ptr(), self.state.numel(), self.status.data_ptr()
+        self.args = a
+        with torch.cuda.device(dev):
+            _capi.check(L.t2_decoder_stream_begin(eng.handle, C.byref(a), eng._stream()))
+
+    def run(self, n):
+        """Advance by up to n steps.  Returns (live_steps, n_total, finished): the steps run by the slices that are still
+        live (None when none is), the most steps any slice has run, and whether every slice has stopped."""
+        sh = self.status_host
+        with torch.cuda.device(self.eng.device):
+            _capi.check(_capi.lib().t2_decoder_stream_run(self.eng.handle, C.byref(self.args), int(n),
+                                                          C.c_void_p(sh.data_ptr()) if sh is not None else None,
+                                                          self.eng._stream()))
+        self.status_host = self.status.cpu()         # the one host sync of the chunk
+        steps = self.status_host[0::2].tolist()
+        stopped = self.status_host[1::2].tolist()
+        live = [s for s, x in zip(steps, stopped) if not x]
+        return (min(live) if live else None), max(steps), not live

@@ -287,6 +287,41 @@ int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) {
   return decoder_run_stepwise(m, a, (cudaStream_t)stream);
 }
 
+size_t t2_decoder_stream_state_bytes(const T2Model*, int32_t B, int32_t T_enc) {
+  return B > 0 && T_enc > 0 ? persistent_stream_state_bytes(B, T_enc) : 0;
+}
+
+static int check_stream_args(const T2Model* m, const T2DecoderStreamArgs* s) {
+  if (!m || !s) return fail(T2_ERR_INVALID, "decoder stream: null model / args");
+  const T2DecoderArgs* a = &s->dec;
+  if (a->B <= 0 || a->B > kMaxBatch) return fail(T2_ERR_INVALID, "decoder stream: B=%d outside [1, %d]", a->B, kMaxBatch);
+  if (a->T_enc <= 0) return fail(T2_ERR_INVALID, "decoder stream: empty encoder memory (T_enc=%d)", a->T_enc);
+  if (a->n_steps_cap <= 0) return fail(T2_ERR_INVALID, "decoder stream: n_steps_cap=%d", a->n_steps_cap);
+  if (!a->memory || !a->mel || !a->gate || !a->align || !a->mel_lengths || !a->n_steps || !s->state || !s->status)
+    return fail(T2_ERR_INVALID, "decoder stream: null tensor pointer");
+  if (a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "decoder stream: mode must be INFER (got %d)", a->mode);
+  if (a->impl == T2_IMPL_STEPWISE)
+    return fail(T2_ERR_UNSUPPORTED, "decoder stream: needs the persistent decoder, which resumes from saved state "
+                                    "(impl = STEPWISE was requested)");
+  if (a->impl != T2_IMPL_AUTO && a->impl != T2_IMPL_PERSISTENT) return fail(T2_ERR_INVALID, "decoder stream: bad impl %d", a->impl);
+  if (!persistent_supported(m, a))
+    return fail(T2_ERR_UNSUPPORTED, "decoder stream: the persistent decoder does not support T_enc=%d on this device "
+                                    "(at most 2274, and >= 128 SMs)", a->T_enc);
+  if (s->state_bytes < persistent_stream_state_bytes(a->B, a->T_enc)) return fail(T2_ERR_WORKSPACE, "decoder stream state too small");
+  return T2_OK;
+}
+
+int t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stream) {
+  T2_TRY(check_stream_args(m, a));
+  return persistent_stream_begin(m, &a->dec, a->state, a->status, (cudaStream_t)stream);
+}
+
+int t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n_steps, const int32_t* status_host, void* stream) {
+  T2_TRY(check_stream_args(m, a));
+  if (n_steps < 1) return fail(T2_ERR_INVALID, "decoder stream: n_steps=%d (at least 1 step per run)", n_steps);
+  return persistent_stream_run(m, &a->dec, a->state, a->status, n_steps, status_host, (cudaStream_t)stream);
+}
+
 size_t t2_decoder_stash_bytes(const T2Model*, int32_t B, int32_t, int32_t T_mel) { return decoder_stash_bytes(B, T_mel); }
 size_t t2_decoder_backward_workspace_bytes(const T2Model*, int32_t B, int32_t T_enc, int32_t T_mel) {
   return decoder_backward_ws_bytes(B, T_enc, T_mel);

@@ -65,6 +65,11 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s);
 size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel);
 int prenet_backward(T2Model* m, const T2PrenetBwdArgs* a, cudaStream_t s);
 bool persistent_supported(const T2Model* m, const T2DecoderArgs* a);
+// resumable persistent decoder (t2_decoder_stream_*): state = per 64-row slice, status = [steps run, stopped] per slice
+size_t persistent_stream_state_bytes(int B, int T_enc);
+int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, cudaStream_t s);
+int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n,
+                          const int32_t* status_host, cudaStream_t s);
 
 // tensor-core skinny GEMMs of the decoder backward (decoder_persistent.cu): which = 0 decoder LSTM (2560 columns),
 // 1 attention LSTM (1792 columns); K = 4096 gate rows in kBwdGemmSplit partial sums

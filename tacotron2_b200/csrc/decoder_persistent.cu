@@ -541,6 +541,14 @@ struct KParams {
   float gate_threshold, score_mask_value, p_att, p_dec;
   uint64_t seed;
   DecoderStash st;                  // training stash for the backward pass (st.ga == nullptr: none)
+  int t_begin, t_end;               // this launch runs steps [t_begin, t_end); the whole loop: 0, cap
+  // resumable stream (t2_decoder_stream_run; rs_acc == nullptr: none).  The prologue restores and the epilogue saves the
+  // on-chip state that lives past a step boundary; the activation images, q and the processed memory stay in place.
+  float* rs_acc;                    // (kG, kRows x kAccPitch) accumulator tiles: next-step partial products
+  float* rs_cell;                   // (kG, 4 column groups, kRows) float4 {c_att[0], c_att[1], c_dec[0], c_dec[1]}
+  float* rs_att;                    // (kG, 2, padded TP) previous | cumulative attention weights
+  int32_t* rs_done;                 // (kRows) stop latch
+  int32_t* rs_status;               // out: [steps run, stopped]
 };
 
 __device__ __forceinline__ void store_split2(uint8_t* img, int row, int k, float v0, float v1) {
@@ -600,7 +608,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     for (int s = 0; s < p.nstages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
     ptx::fence_barrier_init();
   }
-  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;   // every MMA accumulates
+  const bool resume = p.rs_acc != nullptr;       // a stream's chunk: its state was zeroed by begin or saved by the last chunk
+  const int tpp = (TP + 3) & ~3;
+  for (int i = tid; i < kRows * kAccPitch; i += kThreads)                  // every MMA accumulates
+    s_acc[i] = resume ? p.rs_acc[(size_t)cta * kRows * kAccPitch + i] : 0.f;
   for (int i = tid; i < 32; i += kThreads) { s_bias_a[i] = p.bias_a[cta * 32 + i]; s_bias_d[i] = p.bias_d[cta * 32 + i]; }
   for (int i = tid; i < kWeffBytes / 16; i += kThreads)
     reinterpret_cast<uint4*>(s_weff)[i] = reinterpret_cast<const uint4*>(p.weff_img)[i];
@@ -611,12 +622,18 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   rg.pol_x = ptx::policy_evict_last();
   for (int i = tid; i < kAtt; i += kThreads) s_v[i] = p.w_v[i];
   if (tid < 8) s_bias_p[tid] = (cta >= kPCta0 && cta < kPCta0 + kPCtas) ? p.bias_p[(cta - kPCta0) * 8 + tid] : 0.f;
-  for (int i = tid; i < TP; i += kThreads) { s_pad0[i] = 0.f; s_pad1[i] = 0.f; }   // model.py:274-277
+  for (int i = tid; i < TP; i += kThreads) {                                        // model.py:274-277
+    s_pad0[i] = resume ? p.rs_att[((size_t)cta * 2 + 0) * tpp + i] : 0.f;
+    s_pad1[i] = resume ? p.rs_att[((size_t)cta * 2 + 1) * tpp + i] : 0.f;
+  }
+  const CtaPlan& plan = p.plans[cta];
+  DecoderCtrl* ctrl = p.ctrl;
+  const bool has_p = cta >= kPCta0 && cta < kPCta0 + kPCtas;
+  const bool gate_cta = has_p && (cta - kPCta0) * 8 <= kMel && (cta - kPCta0) * 8 + 8 > kMel;   // owns the gate column
+  if (resume && gate_cta && tid < p.B) ctrl->done[tid] = p.rs_done[tid];
   ptx::fence_proxy_async();       // s_weff is read by wgmma (async proxy)
   __syncthreads();
 
-  const CtaPlan& plan = p.plans[cta];
-  DecoderCtrl* ctrl = p.ctrl;
   unsigned int bar_target = 0;
   // epilogue role of this thread: quad = warp % 4, column group cg = warp / 4.  Quadrants 0/1 own batch rows
   // 0-63 (row = accumulator row); the threads of quadrants 2/3 (is_lo) take side jobs (dropout bits).
@@ -625,9 +642,13 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   const bool is_lo = quad >= 2;
   const bool erow = !is_lo && row < p.B;
   float c_att[2] = {0.f, 0.f}, c_dec[2] = {0.f, 0.f};  // cell states of units 8*cta + 2*cg + {0,1}
+  float4* rs_cell = resume ? reinterpret_cast<float4*>(p.rs_cell) + ((size_t)cta * 4 + cg) * kRows + row : nullptr;
+  if (resume && !is_lo) {
+    const float4 c = *rs_cell;
+    c_att[0] = c.x; c_att[1] = c.y; c_dec[0] = c.z; c_dec[1] = c.w;
+  }
   const bool has_q = cta >= kQCta0 && cta < kQCta0 + kQCtas;
   const bool has_x2 = cta >= kX2Cta0 && cta < kX2Cta0 + kX2Ctas;
-  const bool has_p = cta >= kPCta0 && cta < kPCta0 + kPCtas;
   const int halfk = (kLocK - 1) / 2;
   // phase profile (cycles, accumulated over steps) on three sample CTAs; see t2_decoder_profile()
   const int prof_slot = cta == 0 ? 0 : (cta == 60 ? 1 : (cta == 100 ? 2 : -1));
@@ -663,8 +684,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     }
   };
 
-  int t = 0;
-  for (; t < p.cap; ++t) {
+  // the hand-over counters and the grid barrier count from zero in every launch: their targets are relative to t_begin,
+  // while dropout keys, output indices and the stop test use the absolute step t
+  int t = p.t_begin;
+  for (; t < p.t_end; ++t) {
     // ======== E0: x2_t -> attention LSTM gates, epilogue -> ah_t ==================== model.py:352-356
     {
       const uint8_t* x2 = p.infer ? p.x2_img : p.teacher_x2_img + (size_t)t * 4 * kXChunkBytes;
@@ -728,7 +751,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         s_mask[row] = bits;
       }
       run_event(rg, plan.ev[1], p.ah_img, p.wimg, 16, s_acc, ctrl, nullptr,    // the attention phase reuses the ring as scratch
-                ctrl->ah_count, 8u * (unsigned int)(t + 1));
+                ctrl->ah_count, 8u * (unsigned int)(t + 1 - p.t_begin));
       if (has_q && cg == 0 && !is_lo) {
         float g[8];
         acc_take8(s_acc, row, kColS, 0, g);
@@ -993,7 +1016,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     {
       run_event(rg, plan.ev[3], p.dh_img, p.wimg, 16, s_acc, ctrl,
                 (!p.infer && t + 1 < p.cap) ? &plan.ev[0] : nullptr,    // INFER: the loop may end after this step
-                ctrl->dh_count, 8u * (unsigned int)(t + 1));
+                ctrl->dh_count, 8u * (unsigned int)(t + 1 - p.t_begin));
       T2_PROF(10);
       if (tid == 0) *s_live = 0;
       float g[8];
@@ -1032,7 +1055,6 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         }
       }
       __syncthreads();
-      const bool gate_cta = has_p && (cta - kPCta0) * 8 <= kMel && (cta - kPCta0) * 8 + 8 > kMel;
       if (gate_cta && tid == 0) atomicMax(p.n_steps, t + 1);
       T2_PROF(11);
       if (!p.infer) continue;                                                  // teacher forcing: x2 is precomputed
@@ -1043,7 +1065,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       bool stop = t + 1 == p.cap;
       if (has_p) signal_counter(&ctrl->x1_count, 1u + ((gate_cta && *s_live == 0) ? kStopFlag : 0u));
       if (has_x2) {
-        stop |= wait_counter(&ctrl->x1_count, (unsigned int)(kPCtas * (t + 1)), s_flag, ctrl, 102);
+        stop |= wait_counter(&ctrl->x1_count, (unsigned int)(kPCtas * (t + 1 - p.t_begin)), s_flag, ctrl, 102);
         if (!stop) {
           run_event(rg, plan.ev[4], p.x1_img, p.wimg, 4, s_acc, ctrl, nullptr);    // E4: x1 -> x2_(t+1)  model.py:97-100
           x2_epilogue();
@@ -1051,20 +1073,35 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         signal_counter(&ctrl->x2_count, 1u + (stop ? kStopFlag : 0u));
       }
       T2_PROF(12);
-      stop |= wait_counter(&ctrl->x2_count, (unsigned int)(kX2Ctas * (t + 1)), s_flag, ctrl, 103);
+      stop |= wait_counter(&ctrl->x2_count, (unsigned int)(kX2Ctas * (t + 1 - p.t_begin)), s_flag, ctrl, 103);
       T2_PROF(14);
       if (stop) { ++t; break; }
     }
   }
   if (prof_slot >= 0 && tid == 0)
     for (int i = 0; i < 24; ++i) ctrl->prof[prof_slot][i] = s_prof[i];
+  if (resume) {    // every step ended with a wait that closes with __syncthreads: the shared-memory state is complete
+    for (int i = tid; i < kRows * kAccPitch; i += kThreads) p.rs_acc[(size_t)cta * kRows * kAccPitch + i] = s_acc[i];
+    for (int i = tid; i < TP; i += kThreads) {
+      p.rs_att[((size_t)cta * 2 + 0) * tpp + i] = s_pad0[i];
+      p.rs_att[((size_t)cta * 2 + 1) * tpp + i] = s_pad1[i];
+    }
+    if (!is_lo) *rs_cell = make_float4(c_att[0], c_att[1], c_dec[0], c_dec[1]);
+    if (gate_cta && tid < p.B) p.rs_done[tid] = ctrl->done[tid];
+  }
   // rows that never fired: length = number of steps run (model.py:445-447)
   if (cta == 0) {
     __syncthreads();
     const int ns = p.infer ? t : p.cap;
-    for (int b = tid; b < p.B; b += kThreads)
-      if (!p.infer || !__ldcg(&ctrl->done[b])) p.mel_lengths[b] = ns;
-    if (tid == 0) atomicMax(p.n_steps, ns);
+    // a stream's chunk that reached t_end with rows still live and steps left has not ended the loop
+    bool ended = true;
+    if (resume) ended = t >= p.cap || __syncthreads_count(tid < p.B && !__ldcg(&ctrl->done[tid])) == 0;
+    if (ended) {
+      for (int b = tid; b < p.B; b += kThreads)
+        if (!p.infer || !__ldcg(&ctrl->done[b])) p.mel_lengths[b] = ns;
+      if (tid == 0) atomicMax(p.n_steps, ns);
+    }
+    if (resume && tid == 0) { p.rs_status[0] = t; p.rs_status[1] = ended ? 1 : 0; }
   }
 }
 
@@ -1219,40 +1256,77 @@ int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
   return T2_OK;
 }
 
-static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t s, int b0, int nb) {
+constexpr size_t kImagesBytes = (size_t)(4 + 16 + 8 + 16 + 4) * kXChunkBytes + (size_t)kRows * kAtt * 4;   // + q
+
+// processed_memory = memory_layer(memory) of batch rows [b0, b0 + nb)                    (model.py:288)
+static int processed_memory(T2Model* m, const T2DecoderArgs* a, int b0, int nb, float* pm, cudaStream_t s) {
+  GemmArgs g;
+  g.seg[0] = {a->memory + (size_t)b0 * a->T_enc * kEnc, kEnc, m->w[W_ATT_MEMORY], kEnc, kEnc};
+  g.M = nb * a->T_enc; g.N = kAtt; g.C = pm; g.ldc = kAtt;
+  return gemm_f32(g, s);
+}
+
+// the parameters of one launch over batch rows [b0, b0 + nb) that do not depend on where its state lives
+static void slice_params(T2Model* m, const T2DecoderArgs* a, int b0, int nb, KParams* pp) {
   PersistentPack* pk = (PersistentPack*)m->pk;
-  const int B = nb, T = a->T_enc, cap = a->n_steps_cap;
-  DecoderWs w;
-  T2_TRY(decoder_ws_carve(a, &w));
-  T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
-  T2_CUDA(cudaMemsetAsync(w.persistent, 0, (size_t)(4 + 16 + 8 + 16 + 4) * kXChunkBytes + (size_t)kRows * kAtt * 4, s));  // zero images (model.py:258-284)
-  {  // processed_memory = memory_layer(memory)                                  (model.py:288)
-    GemmArgs g;
-    g.seg[0] = {a->memory + (size_t)b0 * T * kEnc, kEnc, m->w[W_ATT_MEMORY], kEnc, kEnc};
-    g.M = B * T; g.N = kAtt; g.C = w.pm; g.ldc = kAtt;
-    T2_TRY(gemm_f32(g, s));
-  }
-  KParams p;
+  KParams& p = *pp;
+  const int T = a->T_enc, cap = a->n_steps_cap;
   memset(&p, 0, sizeof(p));
-  uint8_t* img = (uint8_t*)w.persistent;
-  p.x2_img = img; img += 4 * kXChunkBytes;
-  p.ah_img = img; img += 16 * kXChunkBytes;
-  p.ctx_img = img; img += 8 * kXChunkBytes;
-  p.dh_img = img; img += 16 * kXChunkBytes;
-  p.x1_img = img; img += 4 * kXChunkBytes;
-  p.q = (float*)img;
   p.plans = pk->plans; p.wimg = pk->wimg; p.bias_a = pk->bias_a; p.bias_d = pk->bias_d; p.bias_p = pk->bias_p;
   p.weff_img = pk->weff_img; p.w_v = m->w[W_ATT_V];
-  p.memory = a->memory + (size_t)b0 * T * kEnc; p.pm = w.pm;
+  p.memory = a->memory + (size_t)b0 * T * kEnc;
   p.mem_len = a->memory_lengths ? a->memory_lengths + b0 : nullptr;
   p.prenet_keep = a->prenet_keep; p.att_keep = a->att_keep; p.dec_keep = a->dec_keep;
   p.mel = a->mel + (size_t)b0 * cap * kMel; p.gate = a->gate + (size_t)b0 * cap; p.align = a->align + (size_t)b0 * cap * T;
   p.mel_lengths = a->mel_lengths + b0; p.n_steps = a->n_steps;
-  p.ctrl = w.ctrl;
   p.b0 = b0; p.Btot = a->B;
-  p.B = B; p.T = T; p.cap = cap; p.infer = a->mode == T2_MODE_INFER; p.training = a->training;
+  p.B = nb; p.T = T; p.cap = cap; p.infer = a->mode == T2_MODE_INFER; p.training = a->training;
   p.gate_threshold = a->gate_threshold; p.score_mask_value = a->score_mask_value;
   p.p_att = m->cfg.p_attention_dropout; p.p_dec = m->cfg.p_decoder_dropout; p.seed = a->seed;
+  p.t_begin = 0; p.t_end = cap;
+}
+
+// x2 | ah | ctx | dh | x1 activation images, then q
+static void carve_images(uint8_t* img, KParams* p) {
+  p->x2_img = img; img += 4 * kXChunkBytes;
+  p->ah_img = img; img += 16 * kXChunkBytes;
+  p->ctx_img = img; img += 8 * kXChunkBytes;
+  p->dh_img = img; img += 16 * kXChunkBytes;
+  p->x1_img = img; img += 4 * kXChunkBytes;
+  p->q = (float*)img;
+}
+
+static int launch_persistent(KParams& p, cudaStream_t s) {
+  p.nstages = persistent_stages(p.T);
+  const size_t smem = persistent_smem_bytes(p.T, p.nstages);
+  T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(kG); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeCooperative; attr.val.cooperative = 1;   // co-residency of all 128 CTAs
+  cfg.attrs = &attr; cfg.numAttrs = 1;
+  const cudaError_t le = cudaLaunchKernelEx(&cfg, decoder_persistent_kernel, p);
+  if (le != cudaSuccess) return fail(T2_ERR_CUDA, "persistent decoder launch failed: %s", cudaGetErrorString(le));
+  if (getenv("T2_VERBOSE")) fprintf(stderr, "[t2b200] persistent decoder: B=%d T_enc=%d cap=%d stages=%d smem=%zu steps=%d-%d\n",
+                                    p.B, p.T, p.cap, p.nstages, smem, p.t_begin, p.t_end);
+  g_launch_count++;
+  return T2_OK;
+}
+
+static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t s, int b0, int nb) {
+  const int T = a->T_enc, cap = a->n_steps_cap;
+  DecoderWs w;
+  T2_TRY(decoder_ws_carve(a, &w));
+  T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
+  T2_CUDA(cudaMemsetAsync(w.persistent, 0, kImagesBytes, s));  // zero images (model.py:258-284)
+  T2_TRY(processed_memory(m, a, b0, nb, w.pm, s));
+  KParams p;
+  slice_params(m, a, b0, nb, &p);
+  carve_images((uint8_t*)w.persistent, &p);
+  p.pm = w.pm;
+  p.ctrl = w.ctrl;
+  const int B = nb;
   if (a->stash) {
     if (p.infer) return fail(T2_ERR_INVALID, "the training stash needs T2_MODE_TEACHER");
     if (a->stash_bytes < decoder_stash_bytes(a->B, cap)) return fail(T2_ERR_WORKSPACE, "decoder stash too small");
@@ -1273,20 +1347,74 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
     T2_LAUNCH_CHECK();
     p.teacher_x2_img = timg;
   }
-  p.nstages = persistent_stages(T);
-  const size_t smem = persistent_smem_bytes(T, p.nstages);
-  T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(kG); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeCooperative; attr.val.cooperative = 1;   // co-residency of all 128 CTAs
-  cfg.attrs = &attr; cfg.numAttrs = 1;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, decoder_persistent_kernel, p);
-  if (le != cudaSuccess) return fail(T2_ERR_CUDA, "persistent decoder launch failed: %s", cudaGetErrorString(le));
-  if (getenv("T2_VERBOSE")) fprintf(stderr, "[t2b200] persistent decoder: B=%d T_enc=%d cap=%d stages=%d smem=%zu\n",
-                                    B, T, cap, p.nstages, smem);
-  g_launch_count++;
+  return launch_persistent(p, s);
+}
+
+// ---------------------------------------------------------------------------------------------
+// resumable stream (t2_decoder_stream_*): every 64-row slice owns a block of the caller's state buffer
+// ---------------------------------------------------------------------------------------------
+struct StreamSlice {
+  DecoderCtrl* ctrl;     // counters zeroed before every launch; the stop latch is carried in `done`
+  uint8_t* images;       // activation images + q (kImagesBytes)
+  float* acc; float* cell; float* att; int32_t* done;
+  float* pm;             // processed memory of the slice's rows (nb, T, 128)
+};
+static size_t align1k(size_t x) { return (x + 1023) & ~(size_t)1023; }
+static size_t stream_slice_bytes(int nb, int T) {
+  const size_t tpp = (size_t)((T + kLocK - 1 + 3) & ~3);
+  return align1k(sizeof(DecoderCtrl)) + align1k(kImagesBytes) + align1k((size_t)kG * kRows * kAccPitch * 4) +
+         align1k((size_t)kG * 4 * kRows * 16) + align1k((size_t)kG * 2 * tpp * 4) + align1k((size_t)kRows * 4) +
+         align1k((size_t)nb * T * kAtt * 4);
+}
+static StreamSlice stream_slice(void* state, int B, int T, int b0) {
+  uint8_t* p = (uint8_t*)(((uintptr_t)state + 1023) & ~(uintptr_t)1023);
+  for (int b = 0; b < b0; b += kRows) p += stream_slice_bytes(B - b < kRows ? B - b : kRows, T);
+  const int nb = B - b0 < kRows ? B - b0 : kRows;
+  const size_t tpp = (size_t)((T + kLocK - 1 + 3) & ~3);
+  StreamSlice sl;
+  sl.ctrl = (DecoderCtrl*)p; p += align1k(sizeof(DecoderCtrl));
+  sl.images = p; p += align1k(kImagesBytes);
+  sl.acc = (float*)p; p += align1k((size_t)kG * kRows * kAccPitch * 4);
+  sl.cell = (float*)p; p += align1k((size_t)kG * 4 * kRows * 16);
+  sl.att = (float*)p; p += align1k((size_t)kG * 2 * tpp * 4);
+  sl.done = (int32_t*)p; p += align1k((size_t)kRows * 4);
+  sl.pm = (float*)p; p += align1k((size_t)nb * T * kAtt * 4);
+  return sl;
+}
+
+size_t persistent_stream_state_bytes(int B, int T) {
+  size_t n = 1024;
+  for (int b0 = 0; b0 < B; b0 += kRows) n += stream_slice_bytes(B - b0 < kRows ? B - b0 : kRows, T);
+  return n;
+}
+
+int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, cudaStream_t s) {
+  T2_CUDA(cudaMemsetAsync(state, 0, persistent_stream_state_bytes(a->B, a->T_enc), s));   // model.py:258-284
+  T2_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * 2 * ((a->B + kRows - 1) / kRows), s));
+  T2_CUDA(cudaMemsetAsync(a->mel_lengths, 0xff, sizeof(int32_t) * a->B, s));                // -1: still live
+  T2_CUDA(cudaMemsetAsync(a->n_steps, 0, sizeof(int32_t), s));
+  for (int b0 = 0; b0 < a->B; b0 += kRows)
+    T2_TRY(processed_memory(m, a, b0, a->B - b0 < kRows ? a->B - b0 : kRows, stream_slice(state, a->B, a->T_enc, b0).pm, s));
+  return T2_OK;
+}
+
+int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n,
+                          const int32_t* status_host, cudaStream_t s) {
+  for (int b0 = 0, si = 0; b0 < a->B; b0 += kRows, ++si) {
+    const int t0 = status_host ? status_host[2 * si] : 0;
+    if ((status_host && status_host[2 * si + 1]) || t0 >= a->n_steps_cap) continue;    // this slice has stopped
+    const StreamSlice sl = stream_slice(state, a->B, a->T_enc, b0);
+    T2_CUDA(cudaMemsetAsync(sl.ctrl, 0, sizeof(DecoderCtrl), s));
+    KParams p;
+    slice_params(m, a, b0, a->B - b0 < kRows ? a->B - b0 : kRows, &p);
+    carve_images(sl.images, &p);
+    p.pm = sl.pm;
+    p.ctrl = sl.ctrl;
+    p.t_begin = t0;
+    p.t_end = n < a->n_steps_cap - t0 ? t0 + n : a->n_steps_cap;
+    p.rs_acc = sl.acc; p.rs_cell = sl.cell; p.rs_att = sl.att; p.rs_done = sl.done; p.rs_status = status + 2 * si;
+    T2_TRY(launch_persistent(p, s));
+  }
   return T2_OK;
 }
 

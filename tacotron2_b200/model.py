@@ -427,6 +427,45 @@ class Decoder(_EngineOwner, nn.Module):
         dt = memory.dtype
         return (mel[:, :n].transpose(1, 2).to(dt), gate[:, :n].unsqueeze(-1).to(dt), align[:, :n].to(dt))
 
+    def _stream_chunks(self, memory, chunk_steps, halo):
+        """The persistent decoder in chunks of chunk_steps steps.  Yields (t0, t1, finished, stream): frames [t0, t1) are
+        the new ones that every row has produced and that no frame within `halo` steps of them can still change, i.e. all
+        frames up to the steps run less `halo` while any row is live, and all of them once every 64-row slice has
+        stopped.  Before the last tuple, self.mel_lengths and the max-steps warning are set as by inference()."""
+        chunk_steps = int(chunk_steps)
+        if chunk_steps < 1:
+            raise ValueError("tacotron2_b200: chunk_steps must be >= 1 (got %d)" % chunk_steps)
+        eng = self._t2_engine()
+        st = eng.decoder_stream(memory, self.max_decoder_steps, prenet_keep=current_masks()["prenet"],
+                                gate_threshold=self.gate_threshold)
+        t0 = 0
+        while True:
+            live_steps, n, finished = st.run(chunk_steps)
+            t1 = n if finished else max(t0, live_steps - halo)
+            if finished:
+                self.mel_lengths = st.mel_lengths
+                if n == self.max_decoder_steps and bool((st.mel_lengths >= n).any()):     # as inference()
+                    fired = torch.sigmoid(st.gate[:, n - 1]) > self.gate_threshold
+                    if not bool(fired.all()):
+                        print("Warning! Reached max decoder steps")                             # model.py:446
+            if t1 > t0 or finished:
+                yield t0, t1, finished, st
+            if finished:
+                return
+            t0 = t1
+
+    def inference_stream(self, memory, chunk_steps=32):
+        """inference() in chunks of ``chunk_steps`` decoder steps, as a generator: one item per chunk that produced
+        frames, a dict with ``frames`` = (t0, t1) (the same for every row), ``mel_outputs`` (B, n_mel, t1-t0),
+        ``gate_outputs`` (B, t1-t0, 1), ``alignments`` (B, t1-t0, T_enc), ``mel_lengths`` (B,) int32 on the device with -1
+        for rows that are still live, and ``finished``.  A decoder frame is handed out as soon as every row has produced
+        it; concatenated along time the items are bit-identical to inference() (same weights, memory, masks / seed)."""
+        dt = memory.dtype
+        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0):
+            yield dict(frames=(t0, t1), mel_outputs=st.mel[:, t0:t1].transpose(1, 2).to(dt),
+                       gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
+                       mel_lengths=st.mel_lengths.clone(), finished=finished)
+
 
 class _DecoderFn(torch.autograd.Function):
     """Decoder.forward (model.py:381-416) as one autograd node: forward = the persistent teacher-forced kernel with
@@ -581,3 +620,50 @@ class Tacotron2(_EngineOwner, nn.Module):
             pad = ~get_mask_from_lengths(lengths.long(), mel_outputs.size(2))
             mel_outputs = mel_outputs.masked_fill(pad.unsqueeze(1), 0.0)
         return self.parse_output([mel_outputs, mel_outputs_postnet, gate_outputs, alignments])
+
+    def inference_stream(self, inputs, chunk_steps=32):
+        """inference() as a generator that hands out frames while the decoder runs (README "streaming inference").
+
+        The encoder runs once; the decoder runs in chunks of ``chunk_steps`` steps.  Each item is a dict describing frames
+        [t0, t1) (``frames``, the same for every row): ``mel_outputs`` and ``mel_outputs_postnet`` (B, n_mel, t1-t0),
+        ``gate_outputs`` (B, t1-t0, 1), ``alignments`` (B, t1-t0, T_enc), ``mel_lengths`` (B,) int32 on the device with -1
+        for rows that are still live, and ``finished``.  The postnet's five k=5 convolutions see +-10 frames, so frame t is
+        handed out once the decoder has run step t+10 or every row has stopped; it is never revised.  Concatenated along
+        time the items are bit-identical to inference() with the same weights, inputs and dropout masks / seed.  After the
+        last item ``self.mel_lengths`` and the max-steps warning are as after inference().  Evaluation mode only: in
+        training mode BatchNorm normalises over the whole sequence, so no frame is final before the last one."""
+        if self.training:
+            raise RuntimeError("tacotron2_b200: inference_stream needs eval mode (training-mode BatchNorm uses the statistics "
+                               "of the whole sequence, so no postnet frame is final before the decoder ends)")
+        eng = self._t2_engine()
+        memory = eng.encoder(text=inputs, lengths=None, training=False, keep=current_masks()["enc"])
+        dt = self._t2_out_dtype()
+        memory = memory.to(dt)
+        multi = inputs.size(0) > 1
+        halo = POSTNET_HALO
+        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo):
+            if finished:
+                self.mel_lengths = st.mel_lengths
+            lengths = st.mel_lengths
+            # postnet over input frames [w0, w1): its zero padding reaches only output frames outside [t0, t1)
+            w0, w1 = max(0, t0 - halo), (t1 if finished else t1 + halo)
+            mel_btc = st.mel[:, w0:w1]
+            if dt != torch.float32:                    # inference() feeds the postnet the model-dtype mel (ipynb:89-90)
+                mel_btc = mel_btc.to(dt)
+            if mel_btc.dtype != torch.float32:
+                mel_btc = mel_btc.float().contiguous()
+            win_len = None
+            if multi:                                  # frames at t >= length count as zero; live rows have none
+                win_len = torch.where(lengths < 0, torch.full_like(lengths, w1 - w0), (lengths - w0).clamp(min=0))
+            post = eng.postnet(mel_btc, win_len, True, False, None)[:, :, t0 - w0:t1 - w0].to(dt)
+            mel_outputs = st.mel[:, t0:t1].transpose(1, 2).to(dt)
+            if multi:
+                t = torch.arange(t0, t1, device=lengths.device)
+                pad = (lengths[:, None] >= 0) & (t[None, :] >= lengths[:, None])
+                mel_outputs = mel_outputs.masked_fill(pad.unsqueeze(1), 0.0)
+            yield dict(frames=(t0, t1), mel_outputs=mel_outputs, mel_outputs_postnet=post,
+                       gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
+                       mel_lengths=lengths.clone(), finished=finished)
+
+
+POSTNET_HALO = 10     # frames each side a postnet output depends on: 5 convolutions with k = 5 (model.py:103-146)
