@@ -357,7 +357,9 @@ int t2_collate(const T2CollateArgs* a, void* stream);
 /* ---- Tacotron2.inference end to end with HOST buffers (model.py:517-529) ----------------------
  * text_host (B, T_text) int64 in (pinned) host memory -> mel_post_host (B, 80, T_cap) fp32,
  * mel_lengths_host (B), n_steps_host (1).  Copies H2D, runs encoder -> decoder -> postnet on
- * `stream`, copies D2H and synchronises the stream.  ws is device memory of
+ * `stream`, copies D2H and synchronises the stream.  The postnet runs over the n_steps decoded
+ * frames, as Tacotron2.inference does (so frames [0, n_steps) equal its mel_outputs_postnet); frames
+ * beyond each row's length are zero.  Seed: the decoder's prenet dropout.  ws is device memory of
  * t2_infer_workspace_bytes(). */
 size_t t2_infer_workspace_bytes(const T2Model* m, int32_t B, int32_t T_text, int32_t max_steps);
 int    t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_text,

@@ -147,7 +147,7 @@ def decode_step(sd, st, memory, x, mask=None, att_keep=None, dec_keep=None,
 
 
 def decoder_inference(sd, memory, prenet_keep, gate_threshold=0.5, max_decoder_steps=1000,
-                      mm=None, return_states=False):
+                      mm=None, return_states=False, att_keep=None, dec_keep=None, training=False):
     """Decoder.inference model.py:418-454, generalised to B>1 with a per-row stop latch
     (SURVEY.md section 8(a) row A9):
 
@@ -158,6 +158,8 @@ def decoder_inference(sd, memory, prenet_keep, gate_threshold=0.5, max_decoder_s
 
     For B == 1 this is exactly the reference loop.  ``prenet_keep``: uint8/bool tensor
     (n_steps_cap, 2, B, prenet_dim) of keep masks (step t consumes [t,0] then [t,1]).
+    att_keep / dec_keep (n_steps_cap, B, 1024): the hidden-state dropout of decode() (model.py:355-356,
+    370-371), applied only when ``training`` (a module in train() mode runs inference with it).
     Returns mel (B, 80, T), gate (B, T, 1), align (B, T, T_enc), mel_lengths (B) int32.
     """
     B = memory.shape[0]
@@ -169,7 +171,9 @@ def decoder_inference(sd, memory, prenet_keep, gate_threshold=0.5, max_decoder_s
     while True:
         t = len(mels)
         px = prenet(sd, x, prenet_keep[t, 0], prenet_keep[t, 1], mm)             # :436
-        mel, gate, aw = decode_step(sd, st, memory, px, None, mm=mm)             # :437
+        ak = att_keep[t] if (training and att_keep is not None) else None
+        dk = dec_keep[t] if (training and dec_keep is not None) else None
+        mel, gate, aw = decode_step(sd, st, memory, px, None, ak, dk, mm=mm)     # :437
         mels.append(mel); gates.append(gate); aligns.append(aw)
         if return_states:
             states.append({k: v.clone() for k, v in st.items() if k != "pm"})
@@ -307,18 +311,22 @@ def postnet(sd, x, training=False, keep=None, wgrad_x0=None):
     return x
 
 
-def tacotron2_inference(sd, text, prenet_keep, gate_threshold=0.5, max_decoder_steps=1000):
+def tacotron2_inference(sd, text, prenet_keep, gate_threshold=0.5, max_decoder_steps=1000,
+                        training=False, enc_keep=None, att_keep=None, dec_keep=None, post_keep=None):
     """Tacotron2.inference model.py:517-529 (+ batched stop latch, see decoder_inference).
     For B > 1 decoder frames at t >= mel_lengths[b] are zeroed BEFORE the postnet (the same
-    convention parse_output uses for training, model.py:487-497); B == 1 is the reference."""
+    convention parse_output uses for training, model.py:487-497); B == 1 is the reference.
+    ``training``: the model is in train() mode -- batch statistics in every BatchNorm and the
+    encoder / decoder / postnet dropout with the given keep masks (post_keep at the decoded length)."""
     emb = sd["embedding.weight"][text].transpose(1, 2)                           # :518
-    memory = encoder(sd, emb, None, False)                                       # :519
+    memory = encoder(sd, emb, None, training, enc_keep)                          # :519
     mel, gate, align, lengths = decoder_inference(sd, memory, prenet_keep, gate_threshold,
-                                                  max_decoder_steps)             # :520-521
+                                                  max_decoder_steps, att_keep=att_keep,
+                                                  dec_keep=dec_keep, training=training)  # :520-521
     if mel.shape[0] > 1:
         pad = ~get_mask_from_lengths(lengths.long(), mel.shape[2])
         mel = mel.masked_fill(pad.unsqueeze(1), 0.0)
-    post = mel + postnet(sd, mel, False)                                         # :523-524
+    post = mel + postnet(sd, mel, training, post_keep)                           # :523-524
     if mel.shape[0] > 1:
         post = post.masked_fill(pad.unsqueeze(1), 0.0)
     return mel, post, gate, align, lengths

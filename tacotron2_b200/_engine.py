@@ -57,7 +57,7 @@ _tls = threading.local()
 @contextlib.contextmanager
 def dropout_masks(prenet=None, att=None, dec=None, enc=None, post=None):
     """uint8 keep masks (1 = keep).  prenet: (steps, 2, B, 256) [Decoder.forward: steps = T_mel+1];
-    att / dec: (T_mel, B, 1024); enc: (3, B, 512, T_text); post: list/tuple of 5 masks in the
+    att / dec: (T_mel, B, 1024) [training-mode inference: (max_decoder_steps, B, 1024)]; enc: (3, B, 512, T_text); post: list/tuple of 5 masks in the
     reference layout [(B,512,T)]*4 + [(B,80,T)] (training only).  None => in-kernel Philox."""
     prev = getattr(_tls, "masks", None)
     _tls.masks = dict(prenet=prenet, att=att, dec=dec, enc=enc, post=post)
@@ -466,8 +466,9 @@ class Engine:
         return out
 
     # -- end to end with host buffers (bench e2e leg) ------------------------------------------------
-    def infer_host(self, text_host, max_steps, gate_threshold=0.5, impl=None, out_host=None):
-        """text_host: pinned int64 (B, T).  Returns (mel_post_host (B,80,max_steps), lengths, n_steps)."""
+    def infer_host(self, text_host, max_steps, gate_threshold=0.5, impl=None, out_host=None, seed=None):
+        """text_host: pinned int64 (B, T).  Returns (mel_post_host (B,80,max_steps), lengths, n_steps).  seed: the
+        Philox seed of the decoder's prenet dropout (default: next_seed())."""
         L = _capi.lib()
         B, T = int(text_host.shape[0]), int(text_host.shape[1])
         ws = self._workspace("e2e", L.t2_infer_workspace_bytes(self.handle, B, T, max_steps))
@@ -477,7 +478,7 @@ class Engine:
         mel, lens, ns = out_host
         with torch.cuda.device(self.device):
             _capi.check(L.t2_infer_host(self.handle, text_host.data_ptr(), B, T, int(max_steps), float(gate_threshold),
-                                        next_seed(), self.impl if impl is None else impl, mel.data_ptr(),
+                                        next_seed() if seed is None else seed, self.impl if impl is None else impl, mel.data_ptr(),
                                         lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
         return mel, lens, ns
 

@@ -408,13 +408,26 @@ int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_tex
   da.seed = seed; da.gate_threshold = gate_threshold; da.score_mask_value = -INFINITY;
   da.mel = mel; da.gate = gate; da.align = align; da.mel_lengths = lens; da.n_steps = nsteps; da.ws = sub; da.ws_bytes = sb;
   T2_TRY(t2_decoder_run(m, &da, s));
-  // the postnet runs over the full cap; frames beyond each row's length are zeroed (lengths mask)
-  T2PostnetArgs pa; memset(&pa, 0, sizeof(pa));
-  pa.mel = mel; pa.lengths = lens; pa.add_residual = 1; pa.B = B; pa.T = max_steps; pa.mel_post = post; pa.ws = sub; pa.ws_bytes = sb;
-  T2_TRY(postnet_forward(m, &pa, s));
-  T2_CUDA(cudaMemcpyAsync(mel_post_host, post, (size_t)B * max_steps * kMel * 4, cudaMemcpyDeviceToHost, s));
-  T2_CUDA(cudaMemcpyAsync(mel_lengths_host, lens, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+  // the postnet runs over the n decoded frames, as Tacotron2.inference does: its convolutions zero-pad every layer at
+  // frame n, and a longer window would feed the last rows' final frames the activations of zero input instead
   T2_CUDA(cudaMemcpyAsync(n_steps_host, nsteps, 4, cudaMemcpyDeviceToHost, s));
+  T2_CUDA(cudaStreamSynchronize(s));
+  const int n = n_steps_host[0];
+  if (n < 1 || n > max_steps) return fail(T2_ERR_CUDA, "infer_host: decoder reported %d steps", n);
+  // frames beyond each row's length are zeroed (lengths mask); (B, 80, n) rows -> host rows of pitch max_steps
+  T2PostnetArgs pa; memset(&pa, 0, sizeof(pa));
+  pa.mel = mel; pa.mel_batch_stride = (long)max_steps * kMel; pa.lengths = lens; pa.add_residual = 1; pa.B = B; pa.T = n;
+  pa.mel_post = post; pa.ws = sub; pa.ws_bytes = sb;
+  T2_TRY(postnet_forward(m, &pa, s));
+  T2_CUDA(cudaMemcpy2DAsync(mel_post_host, (size_t)max_steps * 4, post, (size_t)n * 4, (size_t)n * 4, (size_t)B * kMel,
+                            cudaMemcpyDeviceToHost, s));
+  if (n < max_steps) {   // frames past the last step: zeros
+    float* tail = post + (size_t)B * kMel * n;
+    T2_CUDA(cudaMemsetAsync(tail, 0, (size_t)B * kMel * (max_steps - n) * 4, s));
+    T2_CUDA(cudaMemcpy2DAsync(mel_post_host + n, (size_t)max_steps * 4, tail, (size_t)(max_steps - n) * 4,
+                              (size_t)(max_steps - n) * 4, (size_t)B * kMel, cudaMemcpyDeviceToHost, s));
+  }
+  T2_CUDA(cudaMemcpyAsync(mel_lengths_host, lens, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
   T2_CUDA(cudaStreamSynchronize(s));
   return T2_OK;
 }

@@ -413,11 +413,14 @@ class Decoder(_EngineOwner, nn.Module):
     def inference(self, memory):
         """Free-running pass (model.py:418-454), batched: per-row stop latch, see README "batched
         inference".  Returns mel (B, n_mel, T), gate (B, T, 1), alignments (B, T, T_enc); T = steps
-        until every row has fired (or max_decoder_steps); ``self.mel_lengths`` holds per-row lengths."""
+        until every row has fired (or max_decoder_steps); ``self.mel_lengths`` holds per-row lengths.  In training mode
+        the attention / decoder hidden states take their dropout as in the reference's decode() (model.py:355-356,
+        370-371); injected att / dec masks are (max_decoder_steps, B, 1024)."""
         eng = self._t2_engine()
+        masks = current_masks()
         mel, gate, align, lengths, n_steps = eng.decoder(
-            memory, _capi.MODE_INFER, self.max_decoder_steps, prenet_keep=current_masks()["prenet"],
-            gate_threshold=self.gate_threshold)
+            memory, _capi.MODE_INFER, self.max_decoder_steps, training=self.training, prenet_keep=masks["prenet"],
+            att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold)
         n = int(n_steps.item())                      # the one host sync of the whole loop (model.py:443 syncs every step)
         self.mel_lengths = lengths
         if n == self.max_decoder_steps and bool((lengths >= n).any()):
@@ -459,7 +462,12 @@ class Decoder(_EngineOwner, nn.Module):
         frames, a dict with ``frames`` = (t0, t1) (the same for every row), ``mel_outputs`` (B, n_mel, t1-t0),
         ``gate_outputs`` (B, t1-t0, 1), ``alignments`` (B, t1-t0, T_enc), ``mel_lengths`` (B,) int32 on the device with -1
         for rows that are still live, and ``finished``.  A decoder frame is handed out as soon as every row has produced
-        it; concatenated along time the items are bit-identical to inference() (same weights, memory, masks / seed)."""
+        it; concatenated along time the items are bit-identical to inference() (same weights, memory, masks / seed).
+        Evaluation mode only: the resumable decoder applies no hidden-state dropout, which inference() does in training
+        mode."""
+        if self.training:
+            raise RuntimeError("tacotron2_b200: Decoder.inference_stream needs eval mode (in training mode inference() "
+                               "applies the attention / decoder dropout, which the resumable decoder does not)")
         dt = memory.dtype
         for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0):
             yield dict(frames=(t0, t1), mel_outputs=st.mel[:, t0:t1].transpose(1, 2).to(dt),
