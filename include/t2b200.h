@@ -21,6 +21,10 @@
  *     CUDA device unless its name ends in _host; all float tensors are fp32, contiguous;
  *   - the caller owns every buffer; the library allocates only inside T2Model (packed weights) and
  *     never frees caller memory; scratch comes from the caller-provided workspace (size queries);
+ *   - a workspace, stash or stream state buffer needs no particular alignment: each call aligns its
+ *     base itself, and the byte count its size query returns already includes that reserve, so a
+ *     buffer of exactly that many bytes at any address is enough.  A stash is laid out the same way
+ *     by the forward call that fills it and the backward call that reads it;
  *   - work is enqueued on the given stream (a cudaStream_t passed as void*); no call synchronises
  *     the device unless documented (t2_infer_host does, it returns host data);
  *   - every function returns 0 on success or a negative T2_ERR_* code; t2_last_error() returns a

@@ -37,8 +37,6 @@ int selftest_event(const float* A, const float* W, const int* cons, int ncons, i
 int mma_rate(int M, int N, int reps, int alternate_d, long long* out_host, cudaStream_t s);
 int mma_group(int M, int N, int group, int reps, long long* out_host, cudaStream_t s);
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // ---- weight packing -----------------------------------------------------------------------------
 // conv weight (co, ci, k) -> (co, k, ci) so a conv is a GEMM over K = taps x Cin on channels-last rows
 __global__ void permute_conv_kernel(const float* __restrict__ w, float* __restrict__ out, int co, int ci, int k) {
@@ -116,40 +114,34 @@ int pack_model(T2Model* m, cudaStream_t s) {
 }
 
 // ---- decoder workspace --------------------------------------------------------------------------
+static void decoder_ws_layout(Carve& c, int B, int T, int cap, DecoderWs* w) {
+  w->pm = c.take<float>((size_t)B * T * kAtt);
+  // the zero-initialised states: packed floats, one block that one memset clears
+  w->state_begin = c.take<char>(0);
+  const size_t state0 = c.off;
+  w->ah = c.take<float>((size_t)B * kARnn, alignof(float)); w->ac = c.take<float>((size_t)B * kARnn, alignof(float));
+  w->dh = c.take<float>((size_t)B * kDRnn, alignof(float)); w->dc = c.take<float>((size_t)B * kDRnn, alignof(float));
+  w->ctx = c.take<float>((size_t)B * kEnc, alignof(float));
+  w->aw = c.take<float>((size_t)B * T, alignof(float)); w->awc = c.take<float>((size_t)B * T, alignof(float));
+  w->state_bytes = c.off - state0;
+  w->x1 = c.take<float>((size_t)B * kPre); w->x2 = c.take<float>((size_t)B * kPre);
+  w->gates = c.take<float>((size_t)B * 4 * kARnn);
+  w->proj = c.take<float>((size_t)B * (kMel + 1));
+  w->ctrl = c.take<DecoderCtrl>(1);
+  persistent_ws_layout(c, cap, w);
+}
+
 size_t decoder_ws_bytes(int B, int T, int cap) {
-  size_t n = 0;
-  n += align256((size_t)B * T * kAtt * 4);                                   // pm
-  n += align256(((size_t)B * (2 * kARnn + 2 * kDRnn + kEnc) + 2 * (size_t)B * T) * 4);  // state
-  n += 2 * align256((size_t)B * kPre * 4);                                   // x1 x2
-  n += align256((size_t)B * 4 * kARnn * 4);                                  // gates
-  n += align256((size_t)B * (kMel + 1) * 4);                                 // proj
-  n += align256(sizeof(DecoderCtrl));
-  n += align256(persistent_ws_bytes(B, T, cap));
-  return n + 256;
+  Carve c(nullptr, kDecoderWsAlign);
+  DecoderWs w;
+  decoder_ws_layout(c, B, T, cap, &w);
+  return c.bytes();
 }
 
 int decoder_ws_carve(const T2DecoderArgs* a, DecoderWs* w) {
-  const int B = a->B, T = a->T_enc;
-  if (a->ws_bytes < decoder_ws_bytes(B, T, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
-  char* p = (char*)(((uintptr_t)a->ws + 255) & ~(uintptr_t)255);
-  w->pm = (float*)p; p += align256((size_t)B * T * kAtt * 4);
-  w->state_begin = p;
-  w->state_bytes = ((size_t)B * (2 * kARnn + 2 * kDRnn + kEnc) + 2 * (size_t)B * T) * 4;
-  float* f = (float*)p;
-  w->ah = f; f += (size_t)B * kARnn;
-  w->ac = f; f += (size_t)B * kARnn;
-  w->dh = f; f += (size_t)B * kDRnn;
-  w->dc = f; f += (size_t)B * kDRnn;
-  w->ctx = f; f += (size_t)B * kEnc;
-  w->aw = f; f += (size_t)B * T;
-  w->awc = f; f += (size_t)B * T;
-  p += align256(w->state_bytes);
-  w->x1 = (float*)p; p += align256((size_t)B * kPre * 4);
-  w->x2 = (float*)p; p += align256((size_t)B * kPre * 4);
-  w->gates = (float*)p; p += align256((size_t)B * 4 * kARnn * 4);
-  w->proj = (float*)p; p += align256((size_t)B * (kMel + 1) * 4);
-  w->ctrl = (DecoderCtrl*)p; p += align256(sizeof(DecoderCtrl));
-  w->persistent = p; w->persistent_bytes = persistent_ws_bytes(B, T, a->n_steps_cap);
+  if (a->ws_bytes < decoder_ws_bytes(a->B, a->T_enc, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
+  Carve c(a->ws, kDecoderWsAlign);
+  decoder_ws_layout(c, a->B, a->T_enc, a->n_steps_cap, w);
   return T2_OK;
 }
 
@@ -332,7 +324,7 @@ int t2_decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, void* stream) {
     return fail(T2_ERR_INVALID, "decoder backward: null argument");
   return decoder_backward(m, a, (cudaStream_t)stream);
 }
-size_t t2_prenet_backward_workspace_bytes(const T2Model*, int32_t M) { return (size_t)4 * M * kPre * 4 + 1024; }
+size_t t2_prenet_backward_workspace_bytes(const T2Model*, int32_t M) { return prenet_backward_ws_bytes(M); }
 int t2_prenet_backward(T2Model* m, const T2PrenetBwdArgs* a, void* stream) {
   if (!m || !a || !a->frames || !a->d_out || !a->grads || !a->ws || a->M <= 0) return fail(T2_ERR_INVALID, "prenet backward: bad argument");
   return prenet_backward(m, a, (cudaStream_t)stream);
@@ -363,30 +355,30 @@ int t2_postnet_forward(T2Model* m, const T2PostnetArgs* a, void* stream) {
 }
 
 // ---- end to end with host buffers ------------------------------------------------------------------
-static void infer_carve(int B, int Tt, int S, char* base, int64_t** text, float** memory, float** mel, float** gate,
-                        float** align, float** post, int32_t** lens, int32_t** nsteps, char** sub, size_t* sub_bytes,
-                        size_t* total) {
-  char* p = base;
-  auto take = [&](size_t n) { char* r = p; p += align256(n); return r; };
-  *text = (int64_t*)take((size_t)B * Tt * 8);
-  *memory = (float*)take((size_t)B * Tt * kEnc * 4);
-  *mel = (float*)take((size_t)B * S * kMel * 4);
-  *gate = (float*)take((size_t)B * S * 4);
-  *align = (float*)take((size_t)B * S * Tt * 4);
-  *post = (float*)take((size_t)B * S * kMel * 4);
-  *lens = (int32_t*)take((size_t)B * 4);
-  *nsteps = (int32_t*)take(256);
+struct InferWs {
+  int64_t* text; float *memory, *mel, *gate, *align, *post; int32_t *lens, *nsteps;
+  char* sub; size_t sub_bytes;   // the workspace of the encoder, the decoder and the postnet in turn
+};
+static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w) {
+  w->text = c.take<int64_t>((size_t)B * Tt);
+  w->memory = c.take<float>((size_t)B * Tt * kEnc);
+  w->mel = c.take<float>((size_t)B * S * kMel);
+  w->gate = c.take<float>((size_t)B * S);
+  w->align = c.take<float>((size_t)B * S * Tt);
+  w->post = c.take<float>((size_t)B * S * kMel);
+  w->lens = c.take<int32_t>(B);
+  w->nsteps = c.take<int32_t>(1);
   size_t sb = encoder_ws_bytes(B, Tt);
   if (decoder_ws_bytes(B, Tt, S) > sb) sb = decoder_ws_bytes(B, Tt, S);
   if (postnet_ws_bytes(B, S) > sb) sb = postnet_ws_bytes(B, S);
-  *sub = take(sb); *sub_bytes = sb;
-  *total = (size_t)(p - base) + 256;
+  w->sub = c.take<char>(sb); w->sub_bytes = sb;
 }
 
 size_t t2_infer_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32_t max_steps) {
-  int64_t* a; float *b, *c, *d, *e, *f; int32_t *g, *h; char* s; size_t sb, total;
-  infer_carve(B, T_text, max_steps, nullptr, &a, &b, &c, &d, &e, &f, &g, &h, &s, &sb, &total);
-  return total;
+  Carve c(nullptr);
+  InferWs w;
+  infer_layout(c, B, T_text, max_steps, &w);
+  return c.bytes();
 }
 
 int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_text, int32_t max_steps,
@@ -396,38 +388,38 @@ int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_tex
     return fail(T2_ERR_INVALID, "infer_host: null argument");
   if (ws_bytes < t2_infer_workspace_bytes(m, B, T_text, max_steps)) return fail(T2_ERR_WORKSPACE, "infer workspace too small");
   cudaStream_t s = (cudaStream_t)stream;
-  int64_t* text; float *memory, *mel, *gate, *align, *post; int32_t *lens, *nsteps; char* sub; size_t sb, total;
-  char* base = (char*)(((uintptr_t)ws + 255) & ~(uintptr_t)255);
-  infer_carve(B, T_text, max_steps, base, &text, &memory, &mel, &gate, &align, &post, &lens, &nsteps, &sub, &sb, &total);
-  T2_CUDA(cudaMemcpyAsync(text, text_host, (size_t)B * T_text * 8, cudaMemcpyHostToDevice, s));
+  Carve c(ws);
+  InferWs w;
+  infer_layout(c, B, T_text, max_steps, &w);
+  T2_CUDA(cudaMemcpyAsync(w.text, text_host, (size_t)B * T_text * 8, cudaMemcpyHostToDevice, s));
   T2EncoderArgs ea; memset(&ea, 0, sizeof(ea));
-  ea.text = text; ea.B = B; ea.T = T_text; ea.memory = memory; ea.ws = sub; ea.ws_bytes = sb;
+  ea.text = w.text; ea.B = B; ea.T = T_text; ea.memory = w.memory; ea.ws = w.sub; ea.ws_bytes = w.sub_bytes;
   T2_TRY(encoder_forward(m, &ea, s));
   T2DecoderArgs da; memset(&da, 0, sizeof(da));
-  da.mode = T2_MODE_INFER; da.impl = impl; da.memory = memory; da.B = B; da.T_enc = T_text; da.n_steps_cap = max_steps;
+  da.mode = T2_MODE_INFER; da.impl = impl; da.memory = w.memory; da.B = B; da.T_enc = T_text; da.n_steps_cap = max_steps;
   da.seed = seed; da.gate_threshold = gate_threshold; da.score_mask_value = -INFINITY;
-  da.mel = mel; da.gate = gate; da.align = align; da.mel_lengths = lens; da.n_steps = nsteps; da.ws = sub; da.ws_bytes = sb;
+  da.mel = w.mel; da.gate = w.gate; da.align = w.align; da.mel_lengths = w.lens; da.n_steps = w.nsteps; da.ws = w.sub; da.ws_bytes = w.sub_bytes;
   T2_TRY(t2_decoder_run(m, &da, s));
   // the postnet runs over the n decoded frames, as Tacotron2.inference does: its convolutions zero-pad every layer at
   // frame n, and a longer window would feed the last rows' final frames the activations of zero input instead
-  T2_CUDA(cudaMemcpyAsync(n_steps_host, nsteps, 4, cudaMemcpyDeviceToHost, s));
+  T2_CUDA(cudaMemcpyAsync(n_steps_host, w.nsteps, 4, cudaMemcpyDeviceToHost, s));
   T2_CUDA(cudaStreamSynchronize(s));
   const int n = n_steps_host[0];
   if (n < 1 || n > max_steps) return fail(T2_ERR_CUDA, "infer_host: decoder reported %d steps", n);
   // frames beyond each row's length are zeroed (lengths mask); (B, 80, n) rows -> host rows of pitch max_steps
   T2PostnetArgs pa; memset(&pa, 0, sizeof(pa));
-  pa.mel = mel; pa.mel_batch_stride = (long)max_steps * kMel; pa.lengths = lens; pa.add_residual = 1; pa.B = B; pa.T = n;
-  pa.mel_post = post; pa.ws = sub; pa.ws_bytes = sb;
+  pa.mel = w.mel; pa.mel_batch_stride = (long)max_steps * kMel; pa.lengths = w.lens; pa.add_residual = 1; pa.B = B; pa.T = n;
+  pa.mel_post = w.post; pa.ws = w.sub; pa.ws_bytes = w.sub_bytes;
   T2_TRY(postnet_forward(m, &pa, s));
-  T2_CUDA(cudaMemcpy2DAsync(mel_post_host, (size_t)max_steps * 4, post, (size_t)n * 4, (size_t)n * 4, (size_t)B * kMel,
+  T2_CUDA(cudaMemcpy2DAsync(mel_post_host, (size_t)max_steps * 4, w.post, (size_t)n * 4, (size_t)n * 4, (size_t)B * kMel,
                             cudaMemcpyDeviceToHost, s));
   if (n < max_steps) {   // frames past the last step: zeros
-    float* tail = post + (size_t)B * kMel * n;
+    float* tail = w.post + (size_t)B * kMel * n;
     T2_CUDA(cudaMemsetAsync(tail, 0, (size_t)B * kMel * (max_steps - n) * 4, s));
     T2_CUDA(cudaMemcpy2DAsync(mel_post_host + n, (size_t)max_steps * 4, tail, (size_t)(max_steps - n) * 4,
                               (size_t)(max_steps - n) * 4, (size_t)B * kMel, cudaMemcpyDeviceToHost, s));
   }
-  T2_CUDA(cudaMemcpyAsync(mel_lengths_host, lens, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+  T2_CUDA(cudaMemcpyAsync(mel_lengths_host, w.lens, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
   T2_CUDA(cudaStreamSynchronize(s));
   return T2_OK;
 }

@@ -68,6 +68,27 @@ enum W : int {
 };
 static_assert(W_POST_CONV0 + 5 * 7 == W_COUNT, "state_dict table");
 
+// ---- buffer layouts ------------------------------------------------------------------------------
+// Bump allocator over one buffer.  Each buffer has one layout function that take()s its regions in order; the size
+// query runs it on a null base, where it only measures (take() then returns the region's offset), and the code that
+// uses the buffer runs it on the real base, so the two cannot disagree.  The base is first aligned up to `max_align`, the largest alignment
+// the layout asks for, so both runs produce the same offsets whatever the caller's alignment; bytes() includes that
+// reserve.  Alignments are powers of two.
+struct Carve {
+  char* base;
+  size_t off = 0, max_align;
+  __host__ __device__ __forceinline__ explicit Carve(void* b, size_t max_align = 256)
+      : base((char*)b + (-(uintptr_t)b & (max_align - 1))), max_align(max_align) {}
+  template <typename T>
+  __host__ __device__ __forceinline__ T* take(size_t count, size_t align = 256) {
+    off = (off + align - 1) & ~(align - 1);
+    T* r = reinterpret_cast<T*>(base + off);
+    off += count * sizeof(T);
+    return r;
+  }
+  __host__ __device__ __forceinline__ size_t bytes() const { return off + max_align - 1; }
+};
+
 // ---- Philox4x32-10 (counter based RNG for the production dropout path) -------------------------
 __host__ __device__ inline void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3,
                                               uint32_t k0, uint32_t k1, uint32_t out[4]) {

@@ -31,8 +31,10 @@ struct DecoderWs {
   float* gates;            // (B, 4096)
   float* proj;             // (B, 81)
   DecoderCtrl* ctrl;
-  char* persistent; size_t persistent_bytes;  // extra region used by the persistent kernel
+  uint8_t* images;         // persistent kernel: activation images and q (decoder_persistent.cu)
+  uint8_t* teacher_img;    // persistent kernel, teacher forcing: the x2 images of every step
 };
+constexpr size_t kDecoderWsAlign = 1024;   // largest alignment of a decoder workspace region (teacher_img)
 
 // Training stash written by the persistent kernel in teacher-forced mode and read by the backward pass
 // (decoder_backward.cu).  All fp32, step-major.  h = the hidden state that recurs (after dropout).
@@ -42,27 +44,22 @@ struct DecoderStash {
   float* cd = nullptr; float* hd = nullptr;
   float* ctx = nullptr;                                       // (T + 1, B, 512), slot 0 = zeros
 };
-inline size_t decoder_stash_bytes(int B, int T) {
-  return ((size_t)2 * T * B * 4096 + (size_t)4 * (T + 1) * B * 1024 + (size_t)(T + 1) * B * 512) * sizeof(float);
+inline void decoder_stash_layout(Carve& c, int B, int T, DecoderStash* s) {
+  s->ga = c.take<float>((size_t)T * B * 4096); s->gd = c.take<float>((size_t)T * B * 4096);
+  s->ca = c.take<float>((size_t)(T + 1) * B * 1024); s->ha = c.take<float>((size_t)(T + 1) * B * 1024);
+  s->cd = c.take<float>((size_t)(T + 1) * B * 1024); s->hd = c.take<float>((size_t)(T + 1) * B * 1024);
+  s->ctx = c.take<float>((size_t)(T + 1) * B * 512);
 }
-inline void decoder_stash_carve(void* base, int B, int T, DecoderStash* s) {
-  float* f = (float*)base;
-  s->ga = f; f += (size_t)T * B * 4096;
-  s->gd = f; f += (size_t)T * B * 4096;
-  s->ca = f; f += (size_t)(T + 1) * B * 1024;
-  s->ha = f; f += (size_t)(T + 1) * B * 1024;
-  s->cd = f; f += (size_t)(T + 1) * B * 1024;
-  s->hd = f; f += (size_t)(T + 1) * B * 1024;
-  s->ctx = f;
-}
+inline size_t decoder_stash_bytes(int B, int T) { Carve c(nullptr); DecoderStash s; decoder_stash_layout(c, B, T, &s); return c.bytes(); }
 
 size_t decoder_ws_bytes(int B, int T, int cap);
-size_t persistent_ws_bytes(int B, int T, int cap);
+void persistent_ws_layout(Carve& c, int cap, DecoderWs* w);
 int decoder_ws_carve(const T2DecoderArgs* a, DecoderWs* w);
 int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
 int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
 int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s);
 size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel);
+size_t prenet_backward_ws_bytes(int M);
 int prenet_backward(T2Model* m, const T2PrenetBwdArgs* a, cudaStream_t s);
 bool persistent_supported(const T2Model* m, const T2DecoderArgs* a);
 // resumable persistent decoder (t2_decoder_stream_*): state = per 64-row slice, status = [steps run, stopped] per slice

@@ -542,42 +542,39 @@ struct BwdWs {
   float *dga, *dgd, *q, *dq, *awc, *pm, *dpm, *dctx, *dy, *gs, *cols, *pb, *pe, *gdc, *gac, *cacc, *gcat, *dv, *ones, *weff,
       *dweff, *tmp, *gproj, *weffT, *inv_scale;
   uint8_t *img_d, *img_a; DecoderCtrl* ctrl;
-  void* wg; size_t wg_bytes;
+  WgradWs wg;
 };
-size_t carve(char* base, int B, int Te, int T, BwdWs* w) {
-  uintptr_t p = (uintptr_t)base;
-  auto take = [&](size_t n) { float* r = (float*)p; p += (n * sizeof(float) + 255) & ~(size_t)255; return r; };
+void bwd_ws_layout(Carve& c, int B, int Te, int T, BwdWs* w) {
   const size_t TB = (size_t)T * B;
-  BwdWs d;
-  d.dga = take(TB * 4096); d.dgd = take(TB * 4096);
-  d.q = take(TB * 128); d.dq = take(TB * 128);
-  d.awc = take((size_t)B * T * Te);
-  d.pm = take((size_t)B * Te * 128); d.dpm = take((size_t)B * Te * 128);
-  d.dctx = take(TB * 512); d.dy = take(TB * 81);
-  d.gs = take(TB * Te * 128); d.cols = take(TB * Te * kColsLd);
-  d.pb = take((size_t)kSplitMax * 64 * kPBld); d.pe = take((size_t)kSplitMax * 64 * kPEld);
-  d.gdc = take((size_t)64 * 1024); d.gac = take((size_t)64 * 1024);
-  d.cacc = take((size_t)2 * B * Te); d.gcat = take((size_t)2 * 2 * B * 2 * Te);
-  d.dv = take((size_t)B * 128);
+  w->dga = c.take<float>(TB * 4096); w->dgd = c.take<float>(TB * 4096);
+  w->q = c.take<float>(TB * 128); w->dq = c.take<float>(TB * 128);
+  w->awc = c.take<float>((size_t)B * T * Te);
+  w->pm = c.take<float>((size_t)B * Te * 128); w->dpm = c.take<float>((size_t)B * Te * 128);
+  w->dctx = c.take<float>(TB * 512); w->dy = c.take<float>(TB * 81);
+  w->gs = c.take<float>(TB * Te * 128); w->cols = c.take<float>(TB * Te * kColsLd);
+  w->pb = c.take<float>((size_t)kSplitMax * 64 * kPBld); w->pe = c.take<float>((size_t)kSplitMax * 64 * kPEld);
+  w->gdc = c.take<float>((size_t)64 * 1024); w->gac = c.take<float>((size_t)64 * 1024);
+  w->cacc = c.take<float>((size_t)2 * B * Te); w->gcat = c.take<float>((size_t)2 * 2 * B * 2 * Te);
+  w->dv = c.take<float>((size_t)B * 128);
   const size_t n_ones = TB > (size_t)B * Te ? TB : (size_t)B * Te;
-  d.ones = take(n_ones);
-  d.weff = take((size_t)kAtt * kTaps); d.dweff = take((size_t)kAtt * kColsLd);
-  d.tmp = take(4096);
-  d.gproj = take(TB * 1536); d.weffT = take((size_t)kAtt * kTaps);
-  d.inv_scale = take(128);
-  d.img_d = (uint8_t*)take(kBwdImgBytes / 4 + 256); d.img_a = (uint8_t*)take(kBwdImgBytes / 4 + 256);
-  d.img_d = (uint8_t*)(((uintptr_t)d.img_d + 1023) & ~(uintptr_t)1023);
-  d.img_a = (uint8_t*)(((uintptr_t)d.img_a + 1023) & ~(uintptr_t)1023);
-  d.ctrl = (DecoderCtrl*)take(sizeof(DecoderCtrl) / 4 + 64);
-  d.wg_bytes = wgrad_tc_ws_bytes(B, T);
-  d.wg = take(d.wg_bytes / 4 + 64);
-  if (w) *w = d;
-  return (size_t)(p - (uintptr_t)base);
+  w->ones = c.take<float>(n_ones);
+  w->weff = c.take<float>((size_t)kAtt * kTaps); w->dweff = c.take<float>((size_t)kAtt * kColsLd);
+  w->tmp = c.take<float>(4096);
+  w->gproj = c.take<float>(TB * 1536); w->weffT = c.take<float>((size_t)kAtt * kTaps);
+  w->inv_scale = c.take<float>(128);
+  w->img_d = c.take<uint8_t>(kBwdImgBytes, 1024); w->img_a = c.take<uint8_t>(kBwdImgBytes, 1024);
+  w->ctrl = c.take<DecoderCtrl>(1);
+  wgrad_tc_layout(c, T, &w->wg);
 }
 
 }  // namespace
 
-size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel) { return carve(nullptr, B, T_enc, T_mel, nullptr) + 256; }
+size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel) {
+  Carve c(nullptr, 1024);
+  BwdWs w;
+  bwd_ws_layout(c, B, T_enc, T_mel, &w);
+  return c.bytes();
+}
 
 int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   const int B = a->B, Te = a->T_enc, T = a->T_mel;
@@ -589,9 +586,11 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   if (a->ws_bytes < decoder_backward_ws_bytes(B, Te, T)) return fail(T2_ERR_WORKSPACE, "decoder backward workspace too small");
   if (a->stash_bytes < decoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "decoder stash too small");
   DecoderStash st;
-  decoder_stash_carve(const_cast<void*>(a->stash), B, T, &st);
+  Carve sc(const_cast<void*>(a->stash));
+  decoder_stash_layout(sc, B, T, &st);
   BwdWs w;
-  carve((char*)(((uintptr_t)a->ws + 255) & ~(uintptr_t)255), B, Te, T, &w);
+  Carve wc(a->ws, 1024);
+  bwd_ws_layout(wc, B, Te, T, &w);
   const size_t TB = (size_t)T * B;
   const int training = a->training;
   const float p_att = m->cfg.p_attention_dropout, p_dec = m->cfg.p_decoder_dropout;
@@ -742,7 +741,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     if (e && e[0] == 'c') tc_wgrad = false;
   }
   if (tc_wgrad) {
-    T2_TRY(wgrad_tc_run(m, B, T, w.dga, w.dgd, x2, st, G, w.wg, w.wg_bytes, s));
+    T2_TRY(wgrad_tc_run(m, B, T, w.dga, w.dgd, x2, st, G, w.wg, s));
   } else {
   if (G[W_ARNN_WIH]) {   // [x2_t | ctx_{t-1}]                                             model.py:352
       T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kPre, TBi, w.dga, 4096, x2, kPre, G[W_ARNN_WIH], kPre + kEnc, 0.f));
@@ -831,33 +830,39 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------
 // Prenet backward (model.py:97-100): recompute both layers with the same masks, then two plain GEMMs each.
 // ---------------------------------------------------------------------------------------------
+struct PrenetBwdWs { float *x1, *x2, *dz2, *dz1; };   // (M, 256) each
+static void prenet_backward_ws_layout(Carve& c, int M, PrenetBwdWs* w) {
+  w->x1 = c.take<float>((size_t)M * kPre); w->x2 = c.take<float>((size_t)M * kPre);
+  w->dz2 = c.take<float>((size_t)M * kPre); w->dz1 = c.take<float>((size_t)M * kPre);
+}
+size_t prenet_backward_ws_bytes(int M) { Carve c(nullptr); PrenetBwdWs w; prenet_backward_ws_layout(c, M, &w); return c.bytes(); }
+
 int prenet_backward(T2Model* m, const T2PrenetBwdArgs* a, cudaStream_t s) {
   const int M = a->M;
   if (a->n_grads != W_COUNT) return fail(T2_ERR_INVALID, "prenet backward: expected %d gradient pointers", (int)W_COUNT);
-  if (a->ws_bytes < (size_t)4 * M * kPre * 4 + 1024) return fail(T2_ERR_WORKSPACE, "prenet backward workspace too small");
-  float* x1 = (float*)(((uintptr_t)a->ws + 255) & ~(uintptr_t)255);
-  float* x2 = x1 + (size_t)M * kPre;
-  float* dz2 = x2 + (size_t)M * kPre;
-  float* dz1 = dz2 + (size_t)M * kPre;
+  if (a->ws_bytes < prenet_backward_ws_bytes(M)) return fail(T2_ERR_WORKSPACE, "prenet backward workspace too small");
+  Carve c(a->ws);
+  PrenetBwdWs w;
+  prenet_backward_ws_layout(c, M, &w);
   GemmArgs g;
   g.seg[0] = {a->frames, kMel, m->w[W_PRENET0], kMel, kMel};
-  g.M = M; g.N = kPre; g.C = x1; g.ldc = kPre; g.act = ACT_RELU; g.p_drop = 0.5f;
+  g.M = M; g.N = kPre; g.C = w.x1; g.ldc = kPre; g.act = ACT_RELU; g.p_drop = 0.5f;
   if (a->keep) { g.keep = a->keep; g.ldkeep = kPre; } else { g.philox = 1; g.seed = a->seed; g.site = 0xA0; }
   T2_TRY(gemm_f32(g, s));
   GemmArgs h;
-  h.seg[0] = {x1, kPre, m->w[W_PRENET1], kPre, kPre};
-  h.M = M; h.N = kPre; h.C = x2; h.ldc = kPre; h.act = ACT_RELU; h.p_drop = 0.5f;
+  h.seg[0] = {w.x1, kPre, m->w[W_PRENET1], kPre, kPre};
+  h.M = M; h.N = kPre; h.C = w.x2; h.ldc = kPre; h.act = ACT_RELU; h.p_drop = 0.5f;
   if (a->keep) { h.keep = a->keep + (size_t)M * kPre; h.ldkeep = kPre; } else { h.philox = 1; h.seed = a->seed; h.site = 0xA1; }
   T2_TRY(gemm_f32(h, s));
   const long n = (long)M * kPre;
-  prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->d_out, x2, dz2, n);
+  prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->d_out, w.x2, w.dz2, n);
   T2_LAUNCH_CHECK();
-  if (a->grads[W_PRENET1]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kPre, M, dz2, kPre, x1, kPre, a->grads[W_PRENET1], kPre, 0.f));
-  // d_x1 = dz2 . W2  -> through dropout o relu of layer 1
-  T2_TRY(gemm_tc_rm(m, s, false, false, M, kPre, kPre, dz2, kPre, m->w[W_PRENET1], kPre, dz1, kPre, 0.f));
-  prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(dz1, x1, dz1, n);
+  if (a->grads[W_PRENET1]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kPre, M, w.dz2, kPre, w.x1, kPre, a->grads[W_PRENET1], kPre, 0.f));
+  // d_x1 = w.dz2 . W2  -> through dropout o relu of layer 1
+  T2_TRY(gemm_tc_rm(m, s, false, false, M, kPre, kPre, w.dz2, kPre, m->w[W_PRENET1], kPre, w.dz1, kPre, 0.f));
+  prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.dz1, w.x1, w.dz1, n);
   T2_LAUNCH_CHECK();
-  if (a->grads[W_PRENET0]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kMel, M, dz1, kPre, a->frames, kMel, a->grads[W_PRENET0], kMel, 0.f));
+  if (a->grads[W_PRENET0]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kMel, M, w.dz1, kPre, a->frames, kMel, a->grads[W_PRENET0], kMel, 0.f));
   return T2_OK;
 }
 

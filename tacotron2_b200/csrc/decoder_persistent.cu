@@ -324,6 +324,50 @@ struct Ring {
   uint32_t ns;                 // number of stages
 };
 
+// Dynamic shared memory of the persistent decoder for (T_enc, ring stages): the kernel carves it and the host sizes
+// the launch from it, which decides the ring depth and the longest T_enc.  The regions are packed in this order.
+struct PersistentSmem {
+  uint8_t* stage0;                 // ring stages
+  uint8_t* weff;                   // fused location filter image
+  float* acc;                      // event accumulators
+  uint64_t* bars;                  // 16 slots: full[kMaxStages] | empty[kMaxStages]
+  int* live;                       // [0] live rows, [1] stop flag broadcast of wait_counter
+  float *bias_a, *bias_d, *v, *q;
+  float* red;                      // unused; kept so the regions after it stay where they are
+  uint32_t* mask;                  // prenet keep bits of step t+1 (8 per row)
+  float* bias_p;                   // bias of this CTA's 8 projection columns
+  long long* prof;                 // phase profile, accumulated on chip
+  float *pad0, *pad1;              // previous | cumulative attention weights (padded)
+  float* e;                        // [ntiles * 128] attention weights
+  float* ep;                       // [4][ntiles * 128] energy partial sums
+};
+__host__ __device__ __forceinline__ void persistent_smem_layout(Carve& c, int T, int nstages, PersistentSmem* s) {
+  const int tpp = (T + kLocK - 1 + 3) & ~3, ntiles = (T + 127) >> 7;
+  s->stage0 = c.take<uint8_t>((size_t)nstages * kStageBytes, 1);
+  s->weff = c.take<uint8_t>(kWeffBytes, 1);
+  s->acc = c.take<float>(kAccBytes / 4, 1);
+  s->bars = c.take<uint64_t>(16, 1);
+  s->live = c.take<int>(4, 1);
+  s->bias_a = c.take<float>(32, 1); s->bias_d = c.take<float>(32, 1);
+  s->v = c.take<float>(kAtt, 1); s->q = c.take<float>(kAtt, 1);
+  s->red = c.take<float>(32, 1);
+  s->mask = c.take<uint32_t>(kRows, 1);
+  s->bias_p = c.take<float>(8, 1);
+  s->prof = c.take<long long>(24, 1);
+  s->pad0 = c.take<float>(tpp, 1); s->pad1 = c.take<float>(tpp, 1);
+  s->e = c.take<float>((size_t)ntiles * 128, 1);
+  s->ep = c.take<float>((size_t)4 * ntiles * 128, 1);
+}
+
+// Dynamic shared memory of the self test and the backward GEMMs: ring stages, barriers, then the accumulator tile
+struct GemmSmem { uint8_t* stage0; uint64_t* bars; float* acc; };
+__host__ __device__ __forceinline__ void gemm_smem_layout(Carve& c, GemmSmem* s) {
+  s->stage0 = c.take<uint8_t>((size_t)kStages * kStageBytes, 1);
+  s->bars = c.take<uint64_t>(16, 1);
+  s->acc = c.take<float>(kAccBytes / 4, 1);      // [64][kAccPitch]
+}
+size_t gemm_smem_bytes() { Carve c(nullptr, 1); GemmSmem s; gemm_smem_layout(c, &s); return c.bytes(); }
+
 // Weight chunks do not depend on the grid barrier that separates two events (only the activation does):
 // the producer arms the first kStages stages of the NEXT event and issues their weight copies right after
 // the current event's last chunk, so their L2 / HBM latency overlaps the epilogue and the barrier.
@@ -575,31 +619,24 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   const int ntiles = (T + 127) >> 7;
 
   // ---- shared memory carve-up ----
-  uint8_t* sp = smem_raw;
+  Carve sc(smem_raw, 1);
+  PersistentSmem sm;
+  persistent_smem_layout(sc, T, p.nstages, &sm);
   Ring rg;
   rg.ns = (uint32_t)p.nstages;
-  rg.stage0 = sp; sp += p.nstages * kStageBytes;
-  uint8_t* s_weff = sp; sp += kWeffBytes;                                     // fused location filter image
-  float* s_acc = reinterpret_cast<float*>(sp); sp += kAccBytes;                // event accumulators
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sp); sp += 16 * sizeof(uint64_t);
-  rg.full = bars; rg.empty = bars + kMaxStages;
-  int* s_live = reinterpret_cast<int*>(sp); sp += 16;
-  int* s_flag = s_live + 1;                                                    // stop flag broadcast of wait_counter
-  float* s_bias_a = reinterpret_cast<float*>(sp); sp += 32 * 4;
-  float* s_bias_d = reinterpret_cast<float*>(sp); sp += 32 * 4;
-  float* s_v = reinterpret_cast<float*>(sp); sp += kAtt * 4;
-  float* s_q = reinterpret_cast<float*>(sp); sp += kAtt * 4;
-  float* s_red = reinterpret_cast<float*>(sp); sp += 32 * 4;
-  uint32_t* s_mask = reinterpret_cast<uint32_t*>(sp); sp += kRows * 4;        // prenet keep bits of step t+1 (8 per row)
-  float* s_bias_p = reinterpret_cast<float*>(sp); sp += 8 * 4;                // bias of this CTA's 8 projection columns
-  long long* s_prof = reinterpret_cast<long long*>(sp); sp += 24 * 8;         // phase profile, accumulated on chip
-  float* s_pad0 = reinterpret_cast<float*>(sp); sp += ((TP + 3) & ~3) * 4;   // previous weights (padded)
-  float* s_pad1 = reinterpret_cast<float*>(sp); sp += ((TP + 3) & ~3) * 4;   // cumulative weights (padded)
-  float* s_e = reinterpret_cast<float*>(sp);                                  // [ntiles * 128] attention weights
-  float* s_ep = s_e + ntiles * 128;                                           // [4][ntiles * 128] energy partial sums: one writer
-                                                                              // per (group, position), summed in a fixed
-                                                                              // order -> bit-reproducible (no shared-memory atomics)
-  (void)s_red;
+  rg.stage0 = sm.stage0;
+  uint8_t* s_weff = sm.weff;
+  float* s_acc = sm.acc;
+  rg.full = sm.bars; rg.empty = sm.bars + kMaxStages;
+  int* s_live = sm.live;
+  int* s_flag = s_live + 1;
+  float *s_bias_a = sm.bias_a, *s_bias_d = sm.bias_d, *s_v = sm.v, *s_q = sm.q;
+  uint32_t* s_mask = sm.mask;
+  float* s_bias_p = sm.bias_p;
+  long long* s_prof = sm.prof;
+  float *s_pad0 = sm.pad0, *s_pad1 = sm.pad1;
+  float* s_e = sm.e;
+  float* s_ep = sm.ep;     // one writer per (group, position), summed in a fixed order -> bit-reproducible
 
   rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pre = 0;
@@ -1110,12 +1147,12 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
+constexpr size_t kSmemReserve = 1024;    // headroom past the last region
 static size_t persistent_smem_bytes(int T, int nstages) {
-  const int TP = T + kLocK - 1;
-  const int ntiles = (T + 127) / 128;
-  const size_t att = (size_t)5 * ntiles * 128 * 4;      // attention weights + energy partial sums
-  return (size_t)nstages * kStageBytes + kWeffBytes + kAccBytes + 16 * 8 + 16 + 2 * 32 * 4 + kAtt * 4 + kAtt * 4 + 32 * 4 +
-         kRows * 4 + 32 + 24 * 8 + 2 * (size_t)((TP + 3) & ~3) * 4 + att + 1024;
+  Carve c(nullptr, 1);
+  PersistentSmem s;
+  persistent_smem_layout(c, T, nstages, &s);
+  return c.bytes() + kSmemReserve;
 }
 constexpr size_t kSmemLimit = 227 * 1024;
 // 4 ring stages when they fit beside the T_enc-dependent attention state (T_enc <= 896 on sm_90's 227 KiB), else 3
@@ -1129,12 +1166,13 @@ static int persistent_stages(int T) {
   return want;
 }
 
-size_t persistent_ws_bytes(int B, int T, int cap) {
-  (void)B; (void)T;
-  // activation images: x2 (4 chunks), ah (16), ctx (8), dh (16), x1 (4)  + q (64 x 128 fp32)
-  // + (teacher forcing) the x2 images of every step: cap x 4 chunks
-  return (size_t)(4 + 16 + 8 + 16 + 4) * kXChunkBytes + (size_t)kRows * kAtt * 4 + 1024 +
-         (size_t)cap * 4 * kXChunkBytes;
+constexpr size_t kImagesBytes = (size_t)(4 + 16 + 8 + 16 + 4) * kXChunkBytes + (size_t)kRows * kAtt * 4;   // + q
+
+// the persistent kernel's part of the decoder workspace: activation images x2 (4 chunks), ah (16), ctx (8), dh (16),
+// x1 (4) and q (64 x 128 fp32); for teacher forcing the x2 images of every step (cap x 4 chunks)
+void persistent_ws_layout(Carve& c, int cap, DecoderWs* w) {
+  w->images = c.take<uint8_t>(kImagesBytes);
+  w->teacher_img = c.take<uint8_t>((size_t)cap * 4 * kXChunkBytes, 1024);
 }
 
 bool persistent_supported(const T2Model* m, const T2DecoderArgs* a) {
@@ -1256,8 +1294,6 @@ int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
   return T2_OK;
 }
 
-constexpr size_t kImagesBytes = (size_t)(4 + 16 + 8 + 16 + 4) * kXChunkBytes + (size_t)kRows * kAtt * 4;   // + q
-
 // processed_memory = memory_layer(memory) of batch rows [b0, b0 + nb)                    (model.py:288)
 static int processed_memory(T2Model* m, const T2DecoderArgs* a, int b0, int nb, float* pm, cudaStream_t s) {
   GemmArgs g;
@@ -1319,18 +1355,19 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
   DecoderWs w;
   T2_TRY(decoder_ws_carve(a, &w));
   T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
-  T2_CUDA(cudaMemsetAsync(w.persistent, 0, kImagesBytes, s));  // zero images (model.py:258-284)
+  T2_CUDA(cudaMemsetAsync(w.images, 0, kImagesBytes, s));  // zero images (model.py:258-284)
   T2_TRY(processed_memory(m, a, b0, nb, w.pm, s));
   KParams p;
   slice_params(m, a, b0, nb, &p);
-  carve_images((uint8_t*)w.persistent, &p);
+  carve_images(w.images, &p);
   p.pm = w.pm;
   p.ctrl = w.ctrl;
   const int B = nb;
   if (a->stash) {
     if (p.infer) return fail(T2_ERR_INVALID, "the training stash needs T2_MODE_TEACHER");
     if (a->stash_bytes < decoder_stash_bytes(a->B, cap)) return fail(T2_ERR_WORKSPACE, "decoder stash too small");
-    decoder_stash_carve(a->stash, a->B, cap, &p.st);
+    Carve c(a->stash);
+    decoder_stash_layout(c, a->B, cap, &p.st);
     if (b0 == 0) {   // slot 0 of the recurrent states = the zero initial states (model.py:258-284)
       float* z[5] = {p.st.ca, p.st.ha, p.st.cd, p.st.hd, p.st.ctx};
       for (int i = 0; i < 5; ++i)
@@ -1340,12 +1377,10 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
   if (!p.infer) {
     // teacher forcing (model.py:396-405): the prenet outputs of all steps are known up front -> convert
     // them once into x2 operand images, the kernel then skips the prenet events and their two barriers
-    uint8_t* timg = (uint8_t*)p.q + (size_t)kRows * kAtt * 4;
-    timg = (uint8_t*)(((uintptr_t)timg + 1023) & ~(uintptr_t)1023);
-    rows_to_image_kernel<<<dim3(4, cap), 256, 0, s>>>(a->teacher_prenet + (size_t)b0 * kPre, kPre, B, kPre, (long)a->B * kPre, timg,
-                                                      (long)4 * kXChunkBytes);
+    rows_to_image_kernel<<<dim3(4, cap), 256, 0, s>>>(a->teacher_prenet + (size_t)b0 * kPre, kPre, B, kPre, (long)a->B * kPre,
+                                                      w.teacher_img, (long)4 * kXChunkBytes);
     T2_LAUNCH_CHECK();
-    p.teacher_x2_img = timg;
+    p.teacher_x2_img = w.teacher_img;
   }
   return launch_persistent(p, s);
 }
@@ -1359,34 +1394,27 @@ struct StreamSlice {
   float* acc; float* cell; float* att; int32_t* done;
   float* pm;             // processed memory of the slice's rows (nb, T, 128)
 };
-static size_t align1k(size_t x) { return (x + 1023) & ~(size_t)1023; }
-static size_t stream_slice_bytes(int nb, int T) {
+// the slices one after the other; returns slice `b0 / kRows` (any slice when only measuring)
+static StreamSlice stream_state_layout(Carve& c, int B, int T, int b0) {
   const size_t tpp = (size_t)((T + kLocK - 1 + 3) & ~3);
-  return align1k(sizeof(DecoderCtrl)) + align1k(kImagesBytes) + align1k((size_t)kG * kRows * kAccPitch * 4) +
-         align1k((size_t)kG * 4 * kRows * 16) + align1k((size_t)kG * 2 * tpp * 4) + align1k((size_t)kRows * 4) +
-         align1k((size_t)nb * T * kAtt * 4);
+  StreamSlice want = {};
+  for (int b = 0; b < B; b += kRows) {
+    const int nb = B - b < kRows ? B - b : kRows;
+    StreamSlice sl;
+    sl.ctrl = c.take<DecoderCtrl>(1, 1024);
+    sl.images = c.take<uint8_t>(kImagesBytes, 1024);
+    sl.acc = c.take<float>((size_t)kG * kRows * kAccPitch, 1024);
+    sl.cell = c.take<float>((size_t)kG * 4 * kRows * 4, 1024);
+    sl.att = c.take<float>((size_t)kG * 2 * tpp, 1024);
+    sl.done = c.take<int32_t>(kRows, 1024);
+    sl.pm = c.take<float>((size_t)nb * T * kAtt, 1024);
+    if (b == b0) want = sl;
+  }
+  return want;
 }
-static StreamSlice stream_slice(void* state, int B, int T, int b0) {
-  uint8_t* p = (uint8_t*)(((uintptr_t)state + 1023) & ~(uintptr_t)1023);
-  for (int b = 0; b < b0; b += kRows) p += stream_slice_bytes(B - b < kRows ? B - b : kRows, T);
-  const int nb = B - b0 < kRows ? B - b0 : kRows;
-  const size_t tpp = (size_t)((T + kLocK - 1 + 3) & ~3);
-  StreamSlice sl;
-  sl.ctrl = (DecoderCtrl*)p; p += align1k(sizeof(DecoderCtrl));
-  sl.images = p; p += align1k(kImagesBytes);
-  sl.acc = (float*)p; p += align1k((size_t)kG * kRows * kAccPitch * 4);
-  sl.cell = (float*)p; p += align1k((size_t)kG * 4 * kRows * 16);
-  sl.att = (float*)p; p += align1k((size_t)kG * 2 * tpp * 4);
-  sl.done = (int32_t*)p; p += align1k((size_t)kRows * 4);
-  sl.pm = (float*)p; p += align1k((size_t)nb * T * kAtt * 4);
-  return sl;
-}
+static StreamSlice stream_slice(void* state, int B, int T, int b0) { Carve c(state, 1024); return stream_state_layout(c, B, T, b0); }
 
-size_t persistent_stream_state_bytes(int B, int T) {
-  size_t n = 1024;
-  for (int b0 = 0; b0 < B; b0 += kRows) n += stream_slice_bytes(B - b0 < kRows ? B - b0 : kRows, T);
-  return n;
-}
+size_t persistent_stream_state_bytes(int B, int T) { Carve c(nullptr, 1024); stream_state_layout(c, B, T, 0); return c.bytes(); }
 
 int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, cudaStream_t s) {
   T2_CUDA(cudaMemsetAsync(state, 0, persistent_stream_state_bytes(a->B, a->T_enc), s));   // model.py:258-284
@@ -1430,12 +1458,13 @@ selftest_kernel(const uint8_t* x_img, const uint8_t* w_img, EventPlan ep, int ch
                 DecoderCtrl* ctrl) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int tid = threadIdx.x;
-  uint8_t* sp = smem_raw;
+  Carve sc(smem_raw, 1);
+  GemmSmem sm;
+  gemm_smem_layout(sc, &sm);
   Ring rg;
-  rg.stage0 = sp; sp += kStages * kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sp); sp += 16 * sizeof(uint64_t);
-  rg.full = bars; rg.empty = bars + kStages;
-  float* s_acc = reinterpret_cast<float*>(sp);                 // [64][kAccPitch]
+  rg.stage0 = sm.stage0;
+  rg.full = sm.bars; rg.empty = sm.bars + kStages;
+  float* s_acc = sm.acc;
   rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pol_x = rg.pol_w = ptx::policy_evict_last();
   rg.pre = 0; rg.ns = kStages;
@@ -1476,7 +1505,7 @@ int selftest_plan(const float* A, const float* W, const EventPlan& ep, int K, fl
   T2_LAUNCH_CHECK();
   pack_plan_image_kernel<<<chunks, 256, 0, s>>>(W, K, ep, wimg);
   T2_LAUNCH_CHECK();
-  const size_t smem = (size_t)kStages * kStageBytes + 16 * 8 + kAccBytes;
+  const size_t smem = gemm_smem_bytes();
   T2_CUDA(cudaFuncSetAttribute(selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   selftest_kernel<<<1, kThreads, smem, s>>>(ximg, wimg, ep, chunks, C, N, ctrl);
   T2_LAUNCH_CHECK();
@@ -1548,12 +1577,13 @@ bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int tid = threadIdx.x;
   const BwdCta pc = plans[blockIdx.x];
-  uint8_t* sp = smem_raw;
+  Carve sc(smem_raw, 1);
+  GemmSmem sm;
+  gemm_smem_layout(sc, &sm);
   Ring rg;
-  rg.stage0 = sp; sp += kStages * kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sp); sp += 16 * sizeof(uint64_t);
-  rg.full = bars; rg.empty = bars + kStages;
-  float* s_acc = reinterpret_cast<float*>(sp);                 // [64][kAccPitch]
+  rg.stage0 = sm.stage0;
+  rg.full = sm.bars; rg.empty = sm.bars + kStages;
+  float* s_acc = sm.acc;
   rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pol_x = ptx::policy_evict_last(); rg.pol_w = ptx::policy_evict_first();
   rg.pre = 0; rg.ns = kStages;
@@ -1571,7 +1601,6 @@ bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w
   }
 }
 
-size_t bwd_gemm_smem() { return (size_t)kStages * kStageBytes + 16 * 8 + kAccBytes; }
 }  // namespace
 
 int bwd_gemm_ctas(int which) { return which == 0 ? (2560 / kBwdTileB) * kBwdGemmSplit : (1792 / kBwdTileE) * kBwdGemmSplit; }
@@ -1615,7 +1644,7 @@ int bwd_gemm_prepare(T2Model* m, cudaStream_t s) {
 int bwd_gemm_run(T2Model* m, int which, const uint8_t* x_img, const float* inv_scale, float* P, int ldp, DecoderCtrl* ctrl,
                  cudaStream_t s) {
   PersistentPack* pk = (PersistentPack*)m->pk;
-  const size_t smem = bwd_gemm_smem();
+  const size_t smem = gemm_smem_bytes();
   static bool attr_set = false;
   if (!attr_set) {
     T2_CUDA(cudaFuncSetAttribute(bwd_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -273,15 +273,28 @@ enc_lstm_persistent_kernel(const float* __restrict__ gin, const float* __restric
 }
 
 // ---- host side ----------------------------------------------------------------------------------
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 static bool use_tc() { const char* e = getenv("T2_CONV_IMPL"); return !(e && e[0] == 's'); }   // "simt" selects the fp32 SIMT path
 
-size_t encoder_ws_bytes(int B, int T) {
-  const size_t act = align256((size_t)B * T * kEnc * 4);
-  return 2 * act + align256((size_t)B * T * 8 * kEncH * 4) + 3 * align256((size_t)2 * B * kEncH * 4) +
-         2 * align256(8 * kEncH * 4) + 1024 + 2 * align256(tc_planes_bytes(B, T, kEnc));
+struct EncoderWs {
+  float *x0, *x1;          // (B, T, 512) activations of the fp32 conv path
+  float* gin;              // (B, T, 2048) LSTM input projections, forward | reverse
+  float* h;                // (2, 2, B, 256): two h buffers (read / write) of both directions
+  float* c;                // (2, B, 256)
+  float *scale, *shift;    // (2048) folded BatchNorm / bias
+  EncLstmCtrl* lctrl;
+  __half *pl0, *pl1;       // tensor-core activation planes
+};
+static void encoder_ws_layout(Carve& c, int B, int T, EncoderWs* w) {
+  w->x0 = c.take<float>((size_t)B * T * kEnc); w->x1 = c.take<float>((size_t)B * T * kEnc);
+  w->gin = c.take<float>((size_t)B * T * 8 * kEncH);
+  w->h = c.take<float>((size_t)2 * 2 * B * kEncH);
+  w->c = c.take<float>((size_t)2 * B * kEncH);
+  w->scale = c.take<float>(8 * kEncH); w->shift = c.take<float>(8 * kEncH);
+  w->lctrl = c.take<EncLstmCtrl>(1);
+  w->pl0 = c.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
+  w->pl1 = c.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
 }
+size_t encoder_ws_bytes(int B, int T) { Carve c(nullptr); EncoderWs w; encoder_ws_layout(c, B, T, &w); return c.bytes(); }
 
 static int conv_bn_layer(T2Model* m, const float* x, float* y, int B, int T, int cin, int cout,
                          const float* wpk, int wbase, int act, int training, const uint8_t* keep,
@@ -321,20 +334,9 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
   const int B = a->B, T = a->T;
   if (B <= 0 || T <= 0) return fail(T2_ERR_INVALID, "encoder: empty batch");
   if (a->ws_bytes < encoder_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder workspace too small");
-  char* p = (char*)a->ws;
-  const size_t act = align256((size_t)B * T * kEnc * 4);
-  float* x0 = (float*)p; p += act;
-  float* x1 = (float*)p; p += act;
-  float* gin = (float*)p; p += align256((size_t)B * T * 8 * kEncH * 4);
-  float* hbuf0 = (float*)p; p += align256((size_t)2 * B * kEncH * 4);
-  float* hbuf1 = (float*)p; p += align256((size_t)2 * B * kEncH * 4);
-  float* cbuf = (float*)p; p += align256((size_t)2 * B * kEncH * 4);
-  float* scale = (float*)p; p += align256(8 * kEncH * 4);
-  float* shift = (float*)p; p += align256(8 * kEncH * 4);
-  EncLstmCtrl* lctrl = (EncLstmCtrl*)p; p += 256;
-  p = (char*)align256((size_t)p);
-  __half* pl0 = (__half*)p; p += align256(tc_planes_bytes(B, T, kEnc));
-  __half* pl1 = (__half*)p; p += align256(tc_planes_bytes(B, T, kEnc));
+  Carve cv(a->ws);
+  EncoderWs w;
+  encoder_ws_layout(cv, B, T, &w);
   const bool tc = use_tc() && !a->training && !a->stash;
   float* st_gates = nullptr; float* st_c = nullptr;
 
@@ -344,61 +346,61 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
     T2_TRY(encoder_convs_train(m, a, s, &xl, &st_gates, &st_c));
     GemmArgs g;
     g.seg[0] = {xl, kEnc, m->enc_lstm_wih, kEnc, kEnc};
-    g.M = B * T; g.N = 8 * kEncH; g.C = gin; g.ldc = 8 * kEncH; g.bias = m->enc_lstm_b;
+    g.M = B * T; g.N = 8 * kEncH; g.C = w.gin; g.ldc = 8 * kEncH; g.bias = m->enc_lstm_b;
     T2_TRY(gemm_f32(g, s));
   } else if (tc) {
     // tensor-core path: planes -> 3 x (conv k5 + folded BN + ReLU) -> LSTM input projection (fp32 rows)
-    if (a->embedded) T2_TRY(tc_rows_to_planes(a->embedded, (long)T * kEnc, kEnc, kEnc, nullptr, B, T, pl0, s));
-    else T2_TRY(tc_embed_to_planes(a->text, m->w[W_EMB], m->cfg.n_symbols, B, T, pl0, s));
-    __half* cur = pl0; __half* nxt = pl1;
+    if (a->embedded) T2_TRY(tc_rows_to_planes(a->embedded, (long)T * kEnc, kEnc, kEnc, nullptr, B, T, w.pl0, s));
+    else T2_TRY(tc_embed_to_planes(a->text, m->w[W_EMB], m->cfg.n_symbols, B, T, w.pl0, s));
+    __half* cur = w.pl0; __half* nxt = w.pl1;
     for (int i = 0; i < 3; ++i) {                                                           // model.py:174-175, 194
       const int wb = W_ENC_CONV0 + 7 * i;
-      T2_TRY(tc_fold_bn(m->w[wb + 1], m->w[wb + 2], m->w[wb + 3], m->w[wb + 4], m->w[wb + 5], m->cfg.bn_eps, scale, shift, kEnc, s));
+      T2_TRY(tc_fold_bn(m->w[wb + 1], m->w[wb + 2], m->w[wb + 3], m->w[wb + 4], m->w[wb + 5], m->cfg.bn_eps, w.scale, w.shift, kEnc, s));
       TcConvArgs c; memset(&c, 0, sizeof(c));
       c.in = cur; c.cin_pad = kEnc; c.wimg = m->tc_enc_conv[i]; c.taps = kConvK; c.B = B; c.T = T; c.cout = kEnc; c.nt_rows = 128;
-      c.scale = scale; c.shift = shift; c.act = 1; c.out_mode = 0; c.out_planes = nxt;
+      c.scale = w.scale; c.shift = w.shift; c.act = 1; c.out_mode = 0; c.out_planes = nxt;
       T2_TRY(tc_conv(c, s));
       __half* tmp = cur; cur = nxt; nxt = tmp;
     }
-    T2_TRY(tc_fold_bn(m->enc_lstm_b, nullptr, nullptr, nullptr, nullptr, 0.f, scale, shift, 8 * kEncH, s));
+    T2_TRY(tc_fold_bn(m->enc_lstm_b, nullptr, nullptr, nullptr, nullptr, 0.f, w.scale, w.shift, 8 * kEncH, s));
     TcConvArgs c; memset(&c, 0, sizeof(c));
     c.in = cur; c.cin_pad = kEnc; c.wimg = m->tc_enc_wih; c.taps = 1; c.B = B; c.T = T; c.cout = 8 * kEncH; c.nt_rows = 128;
-    c.scale = scale; c.shift = shift; c.act = 0; c.out_mode = 1; c.out_f32 = gin; c.ldo = 8 * kEncH;
+    c.scale = w.scale; c.shift = w.shift; c.act = 0; c.out_mode = 1; c.out_f32 = w.gin; c.ldo = 8 * kEncH;
     T2_TRY(tc_conv(c, s));
   } else {
     if (a->embedded) {
-      T2_CUDA(cudaMemcpyAsync(x0, a->embedded, (size_t)B * T * kEnc * 4, cudaMemcpyDeviceToDevice, s));
+      T2_CUDA(cudaMemcpyAsync(w.x0, a->embedded, (size_t)B * T * kEnc * 4, cudaMemcpyDeviceToDevice, s));
     } else {
-      embed_kernel<<<B * T, 128, 0, s>>>(a->text, m->w[W_EMB], x0, B * T, m->cfg.n_symbols);   // model.py:503/518
+      embed_kernel<<<B * T, 128, 0, s>>>(a->text, m->w[W_EMB], w.x0, B * T, m->cfg.n_symbols);   // model.py:503/518
       T2_LAUNCH_CHECK();
     }
-    float* cur = x0; float* nxt = x1;
+    float* cur = w.x0; float* nxt = w.x1;
     for (int i = 0; i < 3; ++i) {                                                             // model.py:174-175
       const uint8_t* keep = (a->training && a->keep) ? a->keep + (size_t)i * B * kEnc * T : nullptr;
       T2_TRY(conv_bn_layer(m, cur, nxt, B, T, kEnc, kEnc, m->enc_conv_w[i], W_ENC_CONV0 + 7 * i, ACT_RELU,
-                           a->training, keep, a->seed, 1000 + i, scale, shift, 0, nullptr, nullptr, s));
+                           a->training, keep, a->seed, 1000 + i, w.scale, w.shift, 0, nullptr, nullptr, s));
       float* tmp = cur; cur = nxt; nxt = tmp;
     }
     {  // W_ih x + b_ih + b_hh for every time step and both directions
       GemmArgs g;
       g.seg[0] = {cur, kEnc, m->enc_lstm_wih, kEnc, kEnc};
-      g.M = B * T; g.N = 8 * kEncH; g.C = gin; g.ldc = 8 * kEncH; g.bias = m->enc_lstm_b;
+      g.M = B * T; g.N = 8 * kEncH; g.C = w.gin; g.ldc = 8 * kEncH; g.bias = m->enc_lstm_b;
       T2_TRY(gemm_f32(g, s));
     }
   }
-  T2_CUDA(cudaMemsetAsync(hbuf0, 0, (size_t)2 * B * kEncH * 4, s));
-  T2_CUDA(cudaMemsetAsync(cbuf, 0, (size_t)2 * B * kEncH * 4, s));
+  float* hin = w.h; float* hout = w.h + (size_t)2 * B * kEncH;
+  T2_CUDA(cudaMemsetAsync(hin, 0, (size_t)2 * B * kEncH * 4, s));
+  T2_CUDA(cudaMemsetAsync(w.c, 0, (size_t)2 * B * kEncH * 4, s));
   if (B <= 64 && m->sm_count >= 128) {
     // persistent recurrence: one cooperative launch for all T steps of both directions
-    T2_CUDA(cudaMemsetAsync(hbuf1, 0, (size_t)2 * B * kEncH * 4, s));
-    T2_CUDA(cudaMemsetAsync(lctrl, 0, 256, s));
-    float* hb = hbuf0;   // hbuf0 and hbuf1 are adjacent (2 x (2, B, 256) when align256 adds no padding)
-    if (hbuf1 != hbuf0 + (size_t)2 * B * kEncH) return fail(T2_ERR_INVALID, "encoder: h buffers not adjacent");
+    T2_CUDA(cudaMemsetAsync(hout, 0, (size_t)2 * B * kEncH * 4, s));
+    T2_CUDA(cudaMemsetAsync(w.lctrl, 0, sizeof(EncLstmCtrl), s));
+    float* hb = w.h;
     const size_t psm = (size_t)(kEncH * 16 + kEncH * 64) * sizeof(float);
     T2_CUDA(cudaFuncSetAttribute(enc_lstm_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     const float* whf = m->w[W_ENC_LSTM + 1]; const float* whr = m->w[W_ENC_LSTM + 5];
     const int32_t* lens = a->lengths; float* mem = a->memory; int Bv = B, Tv = T;
-    void* args[] = {(void*)&gin, (void*)&whf, (void*)&whr, (void*)&hb, (void*)&mem, (void*)&lens, (void*)&Bv, (void*)&Tv, (void*)&lctrl,
+    void* args[] = {(void*)&w.gin, (void*)&whf, (void*)&whr, (void*)&hb, (void*)&mem, (void*)&lens, (void*)&Bv, (void*)&Tv, (void*)&w.lctrl,
                     (void*)&st_gates, (void*)&st_c};
     T2_CUDA(cudaLaunchCooperativeKernel((void*)enc_lstm_persistent_kernel, dim3(128), dim3(256), args, psm, s));
     g_launch_count++;
@@ -408,47 +410,49 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
   if (a->stash) return fail(T2_ERR_UNSUPPORTED, "encoder: the training stash needs B <= 64 (persistent BiLSTM kernel)");
   const size_t smem = (64 * kEncH + 64 * (kEncH + 1)) * sizeof(float);
   T2_CUDA(cudaFuncSetAttribute(enc_lstm_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  float* hin = hbuf0; float* hout = hbuf1;
   for (int step = 0; step < T; ++step) {
     enc_lstm_step_kernel<<<dim3(16, 2, (B + 63) / 64), 256, smem, s>>>(
-        gin, m->w[W_ENC_LSTM + 1], m->w[W_ENC_LSTM + 5], hin, hout, cbuf, a->memory, a->lengths, B, T, step);
+        w.gin, m->w[W_ENC_LSTM + 1], m->w[W_ENC_LSTM + 5], hin, hout, w.c, a->memory, a->lengths, B, T, step);
     T2_LAUNCH_CHECK();
     float* tmp = hin; hin = hout; hout = tmp;
   }
   return T2_OK;
 }
 
-size_t postnet_ws_bytes(int B, int T) {
-  return 2 * align256((size_t)B * T * kPost * 4) + align256((size_t)B * T * kMel * 4) + 2 * align256(kPost * 4) + 1024 +
-         2 * align256(tc_planes_bytes(B, T, kPost));
+struct PostnetWs {
+  float *y0, *y1;          // (B, T, 512) activations of the fp32 conv path
+  float* xin;              // (B, T, 80) masked input rows
+  float *scale, *shift;    // (512) folded BatchNorm
+  __half *pl0, *pl1;       // tensor-core activation planes
+};
+static void postnet_ws_layout(Carve& c, int B, int T, PostnetWs* w) {
+  w->y0 = c.take<float>((size_t)B * T * kPost); w->y1 = c.take<float>((size_t)B * T * kPost);
+  w->xin = c.take<float>((size_t)B * T * kMel);
+  w->scale = c.take<float>(kPost); w->shift = c.take<float>(kPost);
+  w->pl0 = c.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
+  w->pl1 = c.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
 }
+size_t postnet_ws_bytes(int B, int T) { Carve c(nullptr); PostnetWs w; postnet_ws_layout(c, B, T, &w); return c.bytes(); }
 
 int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
   const int B = a->B, T = a->T;
   if (B <= 0 || T <= 0) return fail(T2_ERR_INVALID, "postnet: empty batch");
   if (a->ws_bytes < postnet_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet workspace too small");
-  char* p = (char*)a->ws;
-  const size_t act = align256((size_t)B * T * kPost * 4);
-  float* y0 = (float*)p; p += act;
-  float* y1 = (float*)p; p += act;
-  float* xin = (float*)p; p += align256((size_t)B * T * kMel * 4);
-  float* scale = (float*)p; p += align256(kPost * 4);
-  float* shift = (float*)p; p += align256(kPost * 4);
-  p = (char*)align256((size_t)p);
-  __half* pl0 = (__half*)p; p += align256(tc_planes_bytes(B, T, kPost));
-  __half* pl1 = (__half*)p; p += align256(tc_planes_bytes(B, T, kPost));
+  Carve cv(a->ws);
+  PostnetWs w;
+  postnet_ws_layout(cv, B, T, &w);
   if (use_tc() && !a->training) {
     // tensor-core path (model.py:141-146 + residual :511/:524): mel -> planes -> 4 x (conv+BN+tanh) -> conv+BN (+mel)
     const long bs = a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel;
-    T2_TRY(tc_rows_to_planes(a->mel, bs, kMel, 128, a->lengths, B, T, pl0, s));
-    __half* cur = pl0; __half* nxt = pl1;
+    T2_TRY(tc_rows_to_planes(a->mel, bs, kMel, 128, a->lengths, B, T, w.pl0, s));
+    __half* cur = w.pl0; __half* nxt = w.pl1;
     for (int i = 0; i < 5; ++i) {
       const int wb = W_POST_CONV0 + 7 * i;
       const int cout = i == 4 ? kMel : kPost;
-      T2_TRY(tc_fold_bn(m->w[wb + 1], m->w[wb + 2], m->w[wb + 3], m->w[wb + 4], m->w[wb + 5], m->cfg.bn_eps, scale, shift, cout, s));
+      T2_TRY(tc_fold_bn(m->w[wb + 1], m->w[wb + 2], m->w[wb + 3], m->w[wb + 4], m->w[wb + 5], m->cfg.bn_eps, w.scale, w.shift, cout, s));
       TcConvArgs c; memset(&c, 0, sizeof(c));
       c.in = cur; c.cin_pad = i == 0 ? 128 : kPost; c.wimg = m->tc_post_conv[i]; c.taps = kConvK; c.B = B; c.T = T;
-      c.cout = cout; c.nt_rows = i == 4 ? 80 : 128; c.scale = scale; c.shift = shift; c.act = i == 4 ? 0 : 2;
+      c.cout = cout; c.nt_rows = i == 4 ? 80 : 128; c.scale = w.scale; c.shift = w.shift; c.act = i == 4 ? 0 : 2;
       if (i < 4) { c.out_mode = 0; c.out_planes = nxt; }
       else { c.out_mode = 2; c.out_f32 = a->mel_post; c.residual = a->add_residual ? a->mel : nullptr; c.res_batch_stride = bs; c.row_len = a->lengths; }
       T2_TRY(tc_conv(c, s));
@@ -458,9 +462,9 @@ int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
   }
   const long n_in = (long)B * T * kMel;
   mask_rows_kernel<<<(unsigned)((n_in + 255) / 256), 256, 0, s>>>(
-      a->mel, a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel, xin, a->lengths, B, T, kMel);
+      a->mel, a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel, w.xin, a->lengths, B, T, kMel);
   T2_LAUNCH_CHECK();
-  const float* cur = xin; float* nxt = y0;
+  const float* cur = w.xin; float* nxt = w.y0;
   for (int i = 0; i < 5; ++i) {                                      // model.py:141-146
     const int cin = i == 0 ? kMel : kPost, cout = i == 4 ? kMel : kPost;
     const bool last = i == 4;
@@ -468,19 +472,19 @@ int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
     if (a->training && a->keep) keep = a->keep + (i < 4 ? (size_t)i * B * kPost * T : (size_t)4 * B * kPost * T);   // [(B,512,T)]*4 + (B,80,T)
     if (last && !a->training) {
       T2_TRY(conv_bn_layer(m, cur, a->mel_post, B, T, cin, cout, m->post_conv_w[i], W_POST_CONV0 + 7 * i,
-                           ACT_NONE, 0, nullptr, 0, 0, scale, shift, 1, a->add_residual ? xin : nullptr, a->lengths, s));
+                           ACT_NONE, 0, nullptr, 0, 0, w.scale, w.shift, 1, a->add_residual ? w.xin : nullptr, a->lengths, s));
     } else {
       T2_TRY(conv_bn_layer(m, cur, nxt, B, T, cin, cout, m->post_conv_w[i], W_POST_CONV0 + 7 * i,
-                           last ? ACT_NONE : ACT_TANH, a->training, keep, a->seed, 2000 + i, scale, shift, 0,
+                           last ? ACT_NONE : ACT_TANH, a->training, keep, a->seed, 2000 + i, w.scale, w.shift, 0,
                            nullptr, nullptr, s));
       if (last) {   // training-mode last layer: separate transpose + residual
         const long n = (long)B * T * kMel;
         transpose_residual_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(
-            nxt, a->add_residual ? xin : nullptr, a->lengths, a->mel_post, B, T, kMel);
+            nxt, a->add_residual ? w.xin : nullptr, a->lengths, a->mel_post, B, T, kMel);
         T2_LAUNCH_CHECK();
         return T2_OK;
       }
-      cur = nxt; nxt = (nxt == y0) ? y1 : y0;
+      cur = nxt; nxt = (nxt == w.y0) ? w.y1 : w.y0;
     }
   }
   return T2_OK;

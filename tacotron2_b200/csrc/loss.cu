@@ -78,12 +78,14 @@ __global__ void loss_final_kernel(const double* __restrict__ part, int nblk, dou
   out[0] = out[1] + out[2] + out[3];     // summed in fp32 like the reference: (mel + post) + gate
 }
 
+double* loss_ws_layout(Carve& c) { return c.take<double>(3 * kLossSplit); }   // per-block partial sums
+
 }  // namespace
 }  // namespace t2
 
 extern "C" {
 
-size_t t2_loss_workspace_bytes(void) { return (size_t)3 * t2::kLossSplit * sizeof(double) + 256; }
+size_t t2_loss_workspace_bytes(void) { t2::Carve c(nullptr); t2::loss_ws_layout(c); return c.bytes(); }
 
 int t2_tacotron2_loss(const T2LossArgs* a, void* stream) {
   using namespace t2;
@@ -92,7 +94,8 @@ int t2_tacotron2_loss(const T2LossArgs* a, void* stream) {
   if (a->B <= 0 || a->C <= 0 || a->T <= 0) return fail(T2_ERR_INVALID, "loss: empty batch");
   if (a->ws_bytes < t2_loss_workspace_bytes()) return fail(T2_ERR_WORKSPACE, "loss workspace too small");
   cudaStream_t s = (cudaStream_t)stream;
-  double* part = (double*)(((uintptr_t)a->ws + 255) & ~(uintptr_t)255);
+  Carve c(a->ws);
+  double* part = loss_ws_layout(c);
   const long n_mel = (long)a->B * a->C * a->T;
   int nblk = (int)((n_mel + 256 * 8 - 1) / (256 * 8));
   nblk = nblk < 1 ? 1 : (nblk > kLossSplit ? kLossSplit : nblk);

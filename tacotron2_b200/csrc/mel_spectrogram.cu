@@ -50,7 +50,14 @@ __global__ void log_transpose_kernel(const float* __restrict__ mel, int n_frames
   }
 }
 
-inline size_t a256m(size_t x) { return (x + 255) & ~(size_t)255; }
+struct MelSpecWs { float *ypad, *ft, *mag, *mel; };
+void mel_ws_layout(Carve& c, int B, int n, int fl, int hop, int n_mel, MelSpecWs* w) {
+  const long frames = n / hop + 1, cutoff = fl / 2 + 1;
+  w->ypad = c.take<float>((size_t)B * (n + fl));                // reflect-padded signal
+  w->ft = c.take<float>((size_t)B * frames * 2 * cutoff);       // Fourier transform (real | imaginary)
+  w->mag = c.take<float>((size_t)B * frames * cutoff);
+  w->mel = c.take<float>((size_t)B * frames * n_mel);           // (B frames, n_mel) before the log / transpose
+}
 
 }  // namespace
 }  // namespace t2
@@ -61,9 +68,10 @@ int32_t t2_mel_spectrogram_frames(int32_t n_samples, int32_t hop_length) { retur
 
 size_t t2_mel_spectrogram_workspace_bytes(int32_t B, int32_t n_samples, int32_t filter_length, int32_t hop_length, int32_t n_mel) {
   using namespace t2;
-  const long frames = n_samples / hop_length + 1, cutoff = filter_length / 2 + 1;
-  return a256m((size_t)B * (n_samples + filter_length) * 4) + a256m((size_t)B * frames * 2 * cutoff * 4) +
-         a256m((size_t)B * frames * cutoff * 4) + a256m((size_t)B * frames * n_mel * 4) + 1024;
+  Carve c(nullptr);
+  MelSpecWs w;
+  mel_ws_layout(c, B, n_samples, filter_length, hop_length, n_mel, &w);
+  return c.bytes();
 }
 
 int t2_mel_spectrogram(const T2MelSpecArgs* a, void* stream) {
@@ -76,25 +84,23 @@ int t2_mel_spectrogram(const T2MelSpecArgs* a, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   const int frames = n / hop + 1, cutoff = fl / 2 + 1;
   const long padded = (long)n + fl;
-  char* p = (char*)(((uintptr_t)a->ws + 255) & ~(uintptr_t)255);
-  float* ypad = (float*)p; p += a256m((size_t)B * padded * 4);
-  float* ft = (float*)p; p += a256m((size_t)B * frames * 2 * cutoff * 4);
-  float* mag = (float*)p; p += a256m((size_t)B * frames * cutoff * 4);
-  float* mel = (float*)p;
+  Carve c(a->ws);
+  MelSpecWs w;
+  mel_ws_layout(c, B, n, fl, hop, n_mel, &w);
   static T2Model scratch_owner;               // only its GEMM scratch is used (grown on demand, kept for the process)
-  reflect_pad_kernel<<<dim3((unsigned)((padded + 255) / 256 > 1024 ? 1024 : (padded + 255) / 256), B), 256, 0, s>>>(a->y, n, fl / 2, ypad);
+  reflect_pad_kernel<<<dim3((unsigned)((padded + 255) / 256 > 1024 ? 1024 : (padded + 255) / 256), B), 256, 0, s>>>(a->y, n, fl / 2, w.ypad);
   T2_LAUNCH_CHECK();
-  GemmTc g;                                   // ft[b] (frames x 2 cutoff) = frames(b) . forward_basis^T
+  GemmTc g;                                   // w.ft[b] (frames x 2 cutoff) = frames(b) . forward_basis^T
   g.ta = false; g.tb = true; g.M = frames; g.N = 2 * cutoff; g.K = fl;
-  g.A = ypad; g.lda = hop; g.strideA = padded;
+  g.A = w.ypad; g.lda = hop; g.strideA = padded;
   g.B = a->forward_basis; g.ldb = fl; g.strideB = 0;
-  g.C = ft; g.ldc = 2 * cutoff; g.strideC = (long)frames * 2 * cutoff; g.batch = B;
+  g.C = w.ft; g.ldc = 2 * cutoff; g.strideC = (long)frames * 2 * cutoff; g.batch = B;
   T2_TRY(gemm_tc(&scratch_owner, s, g));
   const long rows = (long)B * frames;
-  magnitude_kernel<<<(unsigned)((rows * cutoff + 255) / 256 > 4096 ? 4096 : (rows * cutoff + 255) / 256), 256, 0, s>>>(ft, rows, cutoff, mag);
+  magnitude_kernel<<<(unsigned)((rows * cutoff + 255) / 256 > 4096 ? 4096 : (rows * cutoff + 255) / 256), 256, 0, s>>>(w.ft, rows, cutoff, w.mag);
   T2_LAUNCH_CHECK();
-  T2_TRY(gemm_tc_rm(&scratch_owner, s, false, true, (int)rows, n_mel, cutoff, mag, cutoff, a->mel_basis, cutoff, mel, n_mel, 0.f));
-  log_transpose_kernel<<<dim3((frames + 31) / 32, (n_mel + 31) / 32, B), dim3(32, 8), 0, s>>>(mel, frames, n_mel, a->clip_val, a->mel);
+  T2_TRY(gemm_tc_rm(&scratch_owner, s, false, true, (int)rows, n_mel, cutoff, w.mag, cutoff, a->mel_basis, cutoff, w.mel, n_mel, 0.f));
+  log_transpose_kernel<<<dim3((frames + 31) / 32, (n_mel + 31) / 32, B), dim3(32, 8), 0, s>>>(w.mel, frames, n_mel, a->clip_val, a->mel);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }

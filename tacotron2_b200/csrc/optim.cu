@@ -137,14 +137,29 @@ __global__ void __launch_bounds__(256) amp_adam_kernel(const AmpChunk* __restric
   }
 }
 
+// per-chunk partial sums of squares, the derived scalars (Coef = float coefficient | AmpDerived), the chunk table
+template <typename Coef, typename C>
+void adam_ws_layout(Carve& c, size_t nchunk, double** partial, Coef** coef, C** chunks) {
+  *partial = c.take<double>(nchunk);
+  *coef = c.take<Coef>(1);
+  *chunks = c.take<C>(nchunk);
+}
+// the chunk count is at most this bound, so the layout of the bound covers every call
+inline size_t max_chunks(int64_t total_elements, int32_t n_tensors) {
+  return (size_t)(total_elements / kChunk) + (size_t)n_tensors + 1;
+}
+
 }  // namespace
 }  // namespace t2
 
 extern "C" {
 
 size_t t2_clip_adam_workspace_bytes(int64_t total_elements, int32_t n_tensors) {
-  const size_t chunks = (size_t)(total_elements / t2::kChunk) + (size_t)n_tensors + 1;
-  return chunks * (sizeof(t2::Chunk) + sizeof(double)) + 1024;
+  using namespace t2;
+  Carve c(nullptr);
+  double* partial; float* coef; Chunk* chunks;
+  adam_ws_layout(c, max_chunks(total_elements, n_tensors), &partial, &coef, &chunks);
+  return c.bytes();
 }
 
 int t2_clip_adam_step(const T2AdamArgs* a, void* stream) {
@@ -166,10 +181,9 @@ int t2_clip_adam_step(const T2AdamArgs* a, void* stream) {
   }
   if (a->ws_bytes < t2_clip_adam_workspace_bytes(total, a->n)) return fail(T2_ERR_WORKSPACE, "clip_adam workspace too small");
   const size_t nchunk = chunks.size();
-  char* p = (char*)(((uintptr_t)a->ws + 255) & ~(uintptr_t)255);
-  double* partial = (double*)p; p += ((nchunk * sizeof(double) + 255) & ~(size_t)255);
-  float* coef = (float*)p; p += 256;
-  Chunk* d_chunks = (Chunk*)p;
+  Carve c(a->ws);
+  double* partial; float* coef; Chunk* d_chunks;
+  adam_ws_layout(c, nchunk, &partial, &coef, &d_chunks);
   T2_CUDA(cudaMemcpyAsync(d_chunks, chunks.data(), nchunk * sizeof(Chunk), cudaMemcpyHostToDevice, s));   // pageable: staged before return
   sumsq_kernel<<<(unsigned)nchunk, 256, 0, s>>>(d_chunks, partial);
   T2_LAUNCH_CHECK();
@@ -184,8 +198,11 @@ int t2_clip_adam_step(const T2AdamArgs* a, void* stream) {
 }
 
 size_t t2_amp_adam_workspace_bytes(int64_t total_elements, int32_t n_tensors) {
-  const size_t chunks = (size_t)(total_elements / t2::kChunk) + (size_t)n_tensors + 1;
-  return chunks * (sizeof(t2::AmpChunk) + sizeof(double)) + 2048;
+  using namespace t2;
+  Carve c(nullptr);
+  double* partial; AmpDerived* derived; AmpChunk* chunks;
+  adam_ws_layout(c, max_chunks(total_elements, n_tensors), &partial, &derived, &chunks);
+  return c.bytes();
 }
 
 int t2_amp_adam_step(const T2AmpAdamArgs* a, void* stream) {
@@ -211,10 +228,9 @@ int t2_amp_adam_step(const T2AmpAdamArgs* a, void* stream) {
   }
   if (a->ws_bytes < t2_amp_adam_workspace_bytes(total, a->n)) return fail(T2_ERR_WORKSPACE, "amp_adam workspace too small");
   const size_t nchunk = chunks.size();
-  char* p = (char*)(((uintptr_t)a->ws + 255) & ~(uintptr_t)255);
-  double* partial = (double*)p; p += ((nchunk * sizeof(double) + 255) & ~(size_t)255);
-  AmpDerived* derived = (AmpDerived*)p; p += 256;
-  AmpChunk* d_chunks = (AmpChunk*)p;
+  Carve c(a->ws);
+  double* partial; AmpDerived* derived; AmpChunk* d_chunks;
+  adam_ws_layout(c, nchunk, &partial, &derived, &d_chunks);
   T2_CUDA(cudaMemcpyAsync(d_chunks, chunks.data(), nchunk * sizeof(AmpChunk), cudaMemcpyHostToDevice, s));
   amp_sumsq_kernel<<<(unsigned)nchunk, 256, 0, s>>>(d_chunks, a->state, partial);
   T2_LAUNCH_CHECK();

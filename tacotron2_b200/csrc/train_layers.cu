@@ -26,7 +26,6 @@ namespace {
 constexpr int kPadRows = 2;
 inline long prow(int b, int t, int T) { return (long)b * (T + 2 * kPadRows) + kPadRows + t; }
 __device__ __forceinline__ long d_prow(int b, int t, int T) { return (long)b * (T + 2 * kPadRows) + kPadRows + t; }
-size_t a256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // ---- layout conversion ---------------------------------------------------------------------------
 // rows (B, T, C) with batch stride -> padded rows (valid rows only; the buffer was zeroed)
@@ -328,21 +327,18 @@ int tc_train_conv(T2Model* m, const float* xp, int cin, const uint8_t* wimg, int
 // dW_k[co][ci] = sum_r G_z[r][co] X[r + k - 2][ci]: K = padded rows in chunks of 64, A = G_z^T images (per-channel power-of-two
 // scale), B = X^T images, one set per tap (source rows shifted by k - 2), 128 x 256 tiles, K splits reduced in a fixed order.
 struct WgConvWs { uint8_t* img_a; uint8_t* img_b; float* part; float* stat; float* scale; float* inv; float* colsum; WgJob* jobs; };
-size_t wgconv_bytes(int B, int T, WgConvWs* w, char* base) {
+// T2_WGRAD=cublas: the conv weight gradients through gemm_tc instead (cross-check); the region stays in the layout
+static bool wgrad_cublas() { const char* e = getenv("T2_WGRAD"); return e && e[0] == 'c'; }
+void wgconv_layout(Carve& c, int B, int T, WgConvWs* w) {    // every region 1024-aligned
   const long Mp = (long)B * (T + 2 * kPadRows);
   const long nch = (Mp + 63) / 64;
   const int seg = wgrad_seg((int)nch), nsplit = (int)((nch + seg - 1) / seg);
-  uintptr_t p = (uintptr_t)base;
-  auto take = [&](size_t n) { uintptr_t r = p; p += (n + 1023) & ~(size_t)1023; return r; };
-  WgConvWs d;
-  d.img_a = (uint8_t*)take((size_t)nch * 4 * kWgTileA);                 // cout <= 512: 4 tiles of 128 rows
-  d.img_b = (uint8_t*)take((size_t)kConvK * nch * 2 * kWgTileB);        // cin <= 512: 2 tiles of 256 rows, 5 taps
-  d.part = (float*)take((size_t)nsplit * 512 * (kConvK * 512) * 4);
-  d.stat = (float*)take(wg_colstats_ws_bytes(512));
-  d.scale = (float*)take(512 * 4); d.inv = (float*)take(512 * 4); d.colsum = (float*)take(512 * 4);
-  d.jobs = (WgJob*)take((size_t)2048 * sizeof(WgJob));
-  if (w) *w = d;
-  return (size_t)(p - (uintptr_t)base) + 1024;
+  w->img_a = c.take<uint8_t>((size_t)nch * 4 * kWgTileA, 1024);                 // cout <= 512: 4 tiles of 128 rows
+  w->img_b = c.take<uint8_t>((size_t)kConvK * nch * 2 * kWgTileB, 1024);        // cin <= 512: 2 tiles of 256 rows, 5 taps
+  w->part = c.take<float>((size_t)nsplit * 512 * (kConvK * 512), 1024);
+  w->stat = c.take<float>(wg_colstats_ws_bytes(512) / sizeof(float), 1024);
+  w->scale = c.take<float>(512, 1024); w->inv = c.take<float>(512, 1024); w->colsum = c.take<float>(512, 1024);
+  w->jobs = c.take<WgJob>(2048, 1024);
 }
 __global__ void wgconv_reduce_kernel(const float* __restrict__ part, int nsplit, int coutP, int ldp, int cinP, int cout, int cin,
                                      float* __restrict__ dW) {
@@ -479,16 +475,12 @@ int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
 struct StackStash {        // L conv layers: X_0..X_L (padded), Z_0..Z_{L-1} (padded), stats (2 C each)
   float* x[6]; float* z[5]; float* stats[5];
 };
-size_t stack_carve(char* base, int B, int T, int L, const int* ch, StackStash* st) {
-  uintptr_t p = (uintptr_t)base;
+void stack_layout(Carve& c, int B, int T, int L, const int* ch, StackStash* st) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
-  StackStash d;
-  memset(&d, 0, sizeof(d));
-  for (int l = 0; l <= L; ++l) { d.x[l] = (float*)p; p += a256(Mp * ch[l] * 4); }
-  for (int l = 0; l < L; ++l) { d.z[l] = (float*)p; p += a256(Mp * ch[l + 1] * 4); }
-  for (int l = 0; l < L; ++l) { d.stats[l] = (float*)p; p += a256((size_t)(2 + kRedSplit) * ch[l + 1] * 4); }   // + reduction scratch
-  if (st) *st = d;
-  return (size_t)(p - (uintptr_t)base);
+  memset(st, 0, sizeof(*st));
+  for (int l = 0; l <= L; ++l) st->x[l] = c.take<float>(Mp * ch[l]);
+  for (int l = 0; l < L; ++l) st->z[l] = c.take<float>(Mp * ch[l + 1]);
+  for (int l = 0; l < L; ++l) st->stats[l] = c.take<float>((size_t)(2 + kRedSplit) * ch[l + 1]);   // + reduction scratch
 }
 const int kPostCh[6] = {kMel, kPost, kPost, kPost, kPost, kMel};
 const int kEncCh[4] = {kEnc, kEnc, kEnc, kEnc};
@@ -500,16 +492,18 @@ struct EncStash {
   float* cst;      // (B, T, 512) cell states
   float* mem;      // (B, T, 512) copy of the output (h of every valid step)
 };
-size_t enc_carve(char* base, int B, int T, EncStash* st) {
-  uintptr_t p = (uintptr_t)base;
-  EncStash d;
-  p += stack_carve((char*)p, B, T, 3, kEncCh, &d.cs);
-  d.xl = (float*)p; p += a256((size_t)B * T * kEnc * 4);
-  d.gates = (float*)p; p += a256((size_t)B * T * 8 * kEncH * 4);
-  d.cst = (float*)p; p += a256((size_t)B * T * kEnc * 4);
-  d.mem = (float*)p; p += a256((size_t)B * T * kEnc * 4);
-  if (st) *st = d;
-  return (size_t)(p - (uintptr_t)base);
+void enc_stash_layout(Carve& c, int B, int T, EncStash* st) {
+  stack_layout(c, B, T, 3, kEncCh, &st->cs);
+  st->xl = c.take<float>((size_t)B * T * kEnc);
+  st->gates = c.take<float>((size_t)B * T * 8 * kEncH);
+  st->cst = c.take<float>((size_t)B * T * kEnc); st->mem = c.take<float>((size_t)B * T * kEnc);
+}
+// the stash of a forward call, laid out on the caller's buffer
+EncStash enc_stash(const void* stash, int B, int T) {
+  Carve c(const_cast<void*>(stash));
+  EncStash st;
+  enc_stash_layout(c, B, T, &st);
+  return st;
 }
 
 // ---- encoder LSTM backward ------------------------------------------------------------------------------
@@ -610,7 +604,7 @@ __global__ void enc_hprev_kernel(const float* __restrict__ mem, float* __restric
 // ---------------------------------------------------------------------------------------------------
 // Postnet
 // ---------------------------------------------------------------------------------------------------
-size_t postnet_stash_bytes(int B, int T) { return stack_carve(nullptr, B, T, 5, kPostCh, nullptr) + 256; }
+size_t postnet_stash_bytes(int B, int T) { Carve c(nullptr); StackStash st; stack_layout(c, B, T, 5, kPostCh, &st); return c.bytes(); }
 
 static void post_layers(T2Model* m, int training, const uint8_t* keep, int B, int T, ConvLayer* L) {
   for (int i = 0; i < 5; ++i) {
@@ -626,8 +620,9 @@ int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
   if (a->lengths) return fail(T2_ERR_UNSUPPORTED, "postnet: the training stash path takes no length mask (model.py:510)");
   if (a->stash_bytes < postnet_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet stash too small");
   StackStash st;
-  const size_t used = stack_carve((char*)a256((size_t)a->stash), B, T, 5, kPostCh, &st);
-  T2_CUDA(cudaMemsetAsync(st.x[0], 0, used, s));      // zero pad rows everywhere
+  Carve c(a->stash);
+  stack_layout(c, B, T, 5, kPostCh, &st);
+  T2_CUDA(cudaMemsetAsync(st.x[0], 0, c.off, s));      // zero pad rows everywhere
   const long n = (long)B * T * kMel;
   rows_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->mel, a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel,
                                                                      st.x[0], B, T, kMel);
@@ -642,10 +637,28 @@ int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
   return T2_OK;
 }
 
-size_t postnet_backward_ws_bytes(int B, int T) {
+struct PostBwdWs {
+  float *gz, *gxa, *gxb;   // padded rows (B (T+4), 512)
+  float* grow;             // (B T, 80) output gradient rows
+  float *ones, *dwpk, *sums;
+  WgConvWs wg;
+  __half* planes;
+};
+static void postnet_backward_ws_layout(Carve& c, int B, int T, PostBwdWs* w) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
-  return 3 * a256(Mp * kPost * 4) + a256((size_t)B * T * kMel * 4) + a256(Mp * 4) + a256((size_t)kPost * kPost * kConvK * 4) +
-         a256((size_t)(2 + 2 * kRedSplit) * kPost * 4) + wgconv_bytes(B, T, nullptr, nullptr) + a256(tc_planes_bytes(B, T, kPost)) + 8192;
+  w->gz = c.take<float>(Mp * kPost); w->gxa = c.take<float>(Mp * kPost); w->gxb = c.take<float>(Mp * kPost);
+  w->grow = c.take<float>((size_t)B * T * kMel);
+  w->ones = c.take<float>(Mp);
+  w->dwpk = c.take<float>((size_t)kPost * kPost * kConvK);
+  w->sums = c.take<float>((size_t)(2 + 2 * kRedSplit) * kPost);
+  wgconv_layout(c, B, T, &w->wg);
+  w->planes = c.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
+}
+size_t postnet_backward_ws_bytes(int B, int T) {
+  Carve c(nullptr, 1024);
+  PostBwdWs w;
+  postnet_backward_ws_layout(c, B, T, &w);
+  return c.bytes();
 }
 
 int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
@@ -654,44 +667,34 @@ int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
   if (a->ws_bytes < postnet_backward_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet backward workspace too small");
   if (a->stash_bytes < postnet_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet stash too small");
   StackStash st;
-  stack_carve((char*)a256((size_t)a->stash), B, T, 5, kPostCh, &st);
+  Carve sc(const_cast<void*>(a->stash));
+  stack_layout(sc, B, T, 5, kPostCh, &st);
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
-  char* p = (char*)a256((size_t)a->ws);
-  float* gz = (float*)p; p += a256(Mp * kPost * 4);
-  float* gxa = (float*)p; p += a256(Mp * kPost * 4);
-  float* gxb = (float*)p; p += a256(Mp * kPost * 4);
-  float* grow = (float*)p; p += a256((size_t)B * T * kMel * 4);
-  float* ones = (float*)p; p += a256(Mp * 4);
-  float* dwpk = (float*)p; p += a256((size_t)kPost * kPost * kConvK * 4);
-  float* sums = (float*)p; p += a256((size_t)(2 + 2 * kRedSplit) * kPost * 4);
-  WgConvWs wgws; const WgConvWs* wg = nullptr;
-  {
-    const char* e = getenv("T2_WGRAD");
-    if (!(e && e[0] == 'c')) { wgconv_bytes(B, T, &wgws, (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023)); wg = &wgws; }
-  }
-  p = (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023) + wgconv_bytes(B, T, nullptr, nullptr);
-  __half* planes = (__half*)a256((size_t)p);
-  fill1_kernel<<<(unsigned)((Mp + 255) / 256), 256, 0, s>>>(ones, 1.f, (long)Mp);
+  PostBwdWs w;
+  Carve wc(a->ws, 1024);
+  postnet_backward_ws_layout(wc, B, T, &w);
+  const WgConvWs* wg = wgrad_cublas() ? nullptr : &w.wg;
+  fill1_kernel<<<(unsigned)((Mp + 255) / 256), 256, 0, s>>>(w.ones, 1.f, (long)Mp);
   T2_LAUNCH_CHECK();
   const long n = (long)B * T * kMel;
-  bct_to_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->d_mel_post, grow, B, T, kMel);     // (B,80,T) -> rows
+  bct_to_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->d_mel_post, w.grow, B, T, kMel);     // (B,80,T) -> rows
   T2_LAUNCH_CHECK();
   ConvLayer L[5];
   post_layers(m, a->training, a->keep, B, T, L);
-  const float* g = grow; int g_padded = 0;
-  float* gx = gxa;
+  const float* g = w.grow; int g_padded = 0;
+  float* gx = w.gxa;
   for (int i = 4; i >= 0; --i) {
     if (i == 0 && a->wgrad_lengths) {   // the stash is consumed by this call: mask the stored input in place
       mask_padded_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.x[0], a->wgrad_lengths, B, T, kMel);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.x[i], st.z[i], st.stats[i], st.x[i + 1], gz, gx, sums, dwpk,
-                    ones, a->grads, wg, planes, s));
+    T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.x[i], st.z[i], st.stats[i], st.x[i + 1], w.gz, gx, w.sums, w.dwpk,
+                    w.ones, a->grads, wg, w.planes, s));
     g = gx; g_padded = 1;
-    gx = gx == gxa ? gxb : gxa;
+    gx = gx == w.gxa ? w.gxb : w.gxa;
   }
   if (a->d_mel) {   // gradient wrt the postnet input (B, T, 80) (+ the residual branch, model.py:511)
-    padded_to_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(g, a->add_residual ? grow : nullptr, a->d_mel, B, T, kMel);
+    padded_to_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(g, a->add_residual ? w.grow : nullptr, a->d_mel, B, T, kMel);
     T2_LAUNCH_CHECK();
   }
   return T2_OK;
@@ -700,7 +703,7 @@ int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------------
 // Encoder
 // ---------------------------------------------------------------------------------------------------
-size_t encoder_stash_bytes(int B, int T) { return enc_carve(nullptr, B, T, nullptr) + 256; }
+size_t encoder_stash_bytes(int B, int T) { Carve c(nullptr); EncStash st; enc_stash_layout(c, B, T, &st); return c.bytes(); }
 
 static void enc_layers(T2Model* m, int training, const uint8_t* keep, int B, int T, ConvLayer* L) {
   for (int i = 0; i < 3; ++i) {
@@ -715,10 +718,8 @@ static void enc_layers(T2Model* m, int training, const uint8_t* keep, int B, int
 int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, const float** xl, float** gates, float** cst) {
   const int B = a->B, T = a->T;
   if (a->stash_bytes < encoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder stash too small");
-  EncStash st;
-  enc_carve((char*)a256((size_t)a->stash), B, T, &st);
-  const size_t cs_bytes = stack_carve(nullptr, B, T, 3, kEncCh, nullptr);
-  T2_CUDA(cudaMemsetAsync(st.cs.x[0], 0, cs_bytes, s));
+  const EncStash st = enc_stash(a->stash, B, T);
+  T2_CUDA(cudaMemsetAsync(st.cs.x[0], 0, (char*)st.xl - (char*)st.cs.x[0], s));   // the conv stack, pad rows included
   const long n = (long)B * T * kEnc;
   if (a->embedded) rows_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->embedded, (long)T * kEnc, st.cs.x[0], B, T, kEnc);
   else embed_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->text, m->w[W_EMB], st.cs.x[0], B, T, m->cfg.n_symbols);
@@ -733,93 +734,101 @@ int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, cons
 }
 // after the LSTM ran: keep a copy of the output for the backward pass
 int encoder_stash_output(const T2EncoderArgs* a, cudaStream_t s) {
-  EncStash st;
-  enc_carve((char*)a256((size_t)a->stash), a->B, a->T, &st);
+  const EncStash st = enc_stash(a->stash, a->B, a->T);
   T2_CUDA(cudaMemcpyAsync(st.mem, a->memory, (size_t)a->B * a->T * kEnc * 4, cudaMemcpyDeviceToDevice, s));
   return T2_OK;
 }
 
-size_t encoder_backward_ws_bytes(int B, int T) {
+constexpr int kEncBwdSplit = 8;   // K splits of the W_hh products in the reverse recurrence
+struct EncBwdWs {
+  float* dG;               // (B, T, 2 dirs, 1024)
+  float *hp, *dxl;         // (B T, 512)
+  float* part;             // (2, kEncBwdSplit, 64, 256)
+  float* g_c;              // (2, 64, 256)
+  float *gz, *gxa, *gxb;   // padded rows (B (T+4), 512)
+  float *ones, *dwpk, *sums, *tmp;
+  WgConvWs wg;
+  __half* planes;
+};
+static size_t enc_bwd_n_ones(int B, int T) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
-  constexpr int nsplit = 8;
-  return a256((size_t)B * T * 8 * kEncH * 4) + a256((size_t)B * T * kEnc * 4) * 2 + a256((size_t)2 * nsplit * 64 * kEncH * 4) +
-         a256((size_t)2 * 64 * kEncH * 4) + 3 * a256(Mp * kEnc * 4) + a256((Mp > (size_t)B * T ? Mp : (size_t)B * T) * 4) +
-         a256((size_t)kEnc * kEnc * kConvK * 4) + a256((size_t)(2 + 2 * kRedSplit) * kEnc * 4) + a256(8 * kEncH * 4) +
-         wgconv_bytes(B, T, nullptr, nullptr) + a256(tc_planes_bytes(B, T, kEnc)) + 8192;
+  return Mp > (size_t)B * T ? Mp : (size_t)B * T;
+}
+static void encoder_backward_ws_layout(Carve& c, int B, int T, EncBwdWs* w) {
+  const size_t Mp = (size_t)B * (T + 2 * kPadRows);
+  w->dG = c.take<float>((size_t)B * T * 8 * kEncH);
+  w->hp = c.take<float>((size_t)B * T * kEnc); w->dxl = c.take<float>((size_t)B * T * kEnc);
+  w->part = c.take<float>((size_t)2 * kEncBwdSplit * 64 * kEncH);
+  w->g_c = c.take<float>((size_t)2 * 64 * kEncH);
+  w->gz = c.take<float>(Mp * kEnc); w->gxa = c.take<float>(Mp * kEnc); w->gxb = c.take<float>(Mp * kEnc);
+  w->ones = c.take<float>(enc_bwd_n_ones(B, T));
+  w->dwpk = c.take<float>((size_t)kEnc * kEnc * kConvK);
+  w->sums = c.take<float>((size_t)(2 + 2 * kRedSplit) * kEnc);
+  w->tmp = c.take<float>(8 * kEncH);
+  wgconv_layout(c, B, T, &w->wg);
+  w->planes = c.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
+}
+size_t encoder_backward_ws_bytes(int B, int T) {
+  Carve c(nullptr, 1024);
+  EncBwdWs w;
+  encoder_backward_ws_layout(c, B, T, &w);
+  return c.bytes();
 }
 
 int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   const int B = a->B, T = a->T;
-  constexpr int nsplit = 8;
+  constexpr int nsplit = kEncBwdSplit;
   if (B < 1 || B > 64) return fail(T2_ERR_UNSUPPORTED, "encoder backward: 1 <= B <= 64 (got %d)", B);
   if (a->n_grads != W_COUNT) return fail(T2_ERR_INVALID, "encoder backward: expected %d gradient pointers", (int)W_COUNT);
   if (a->ws_bytes < encoder_backward_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder backward workspace too small");
   if (a->stash_bytes < encoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder stash too small");
-  EncStash st;
-  enc_carve((char*)a256((size_t)a->stash), B, T, &st);
-  const size_t Mp = (size_t)B * (T + 2 * kPadRows);
-  char* p = (char*)a256((size_t)a->ws);
-  float* dG = (float*)p; p += a256((size_t)B * T * 8 * kEncH * 4);       // (B, T, 2 dirs, 1024)
-  float* hp = (float*)p; p += a256((size_t)B * T * kEnc * 4);
-  float* dxl = (float*)p; p += a256((size_t)B * T * kEnc * 4);
-  float* part = (float*)p; p += a256((size_t)2 * nsplit * 64 * kEncH * 4);
-  float* g_c = (float*)p; p += a256((size_t)2 * 64 * kEncH * 4);
-  float* gz = (float*)p; p += a256(Mp * kEnc * 4);
-  float* gxa = (float*)p; p += a256(Mp * kEnc * 4);
-  float* gxb = (float*)p; p += a256(Mp * kEnc * 4);
-  const size_t n_ones = Mp > (size_t)B * T ? Mp : (size_t)B * T;
-  float* ones = (float*)p; p += a256(n_ones * 4);
-  float* dwpk = (float*)p; p += a256((size_t)kEnc * kEnc * kConvK * 4);
-  float* sums = (float*)p; p += a256((size_t)(2 + 2 * kRedSplit) * kEnc * 4);
-  float* tmp = (float*)p; p += a256(8 * kEncH * 4);
-  WgConvWs wgws; const WgConvWs* wg = nullptr;
-  {
-    const char* e = getenv("T2_WGRAD");
-    if (!(e && e[0] == 'c')) { wgconv_bytes(B, T, &wgws, (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023)); wg = &wgws; }
-  }
-  p = (char*)(((uintptr_t)p + 1023) & ~(uintptr_t)1023) + wgconv_bytes(B, T, nullptr, nullptr);
-  __half* planes = (__half*)a256((size_t)p);
-  fill1_kernel<<<(unsigned)((n_ones + 255) / 256), 256, 0, s>>>(ones, 1.f, (long)n_ones);
+  const EncStash st = enc_stash(a->stash, B, T);
+  EncBwdWs w;
+  Carve wc(a->ws, 1024);
+  encoder_backward_ws_layout(wc, B, T, &w);
+  const WgConvWs* wg = wgrad_cublas() ? nullptr : &w.wg;
+  const size_t n_ones = enc_bwd_n_ones(B, T);
+  fill1_kernel<<<(unsigned)((n_ones + 255) / 256), 256, 0, s>>>(w.ones, 1.f, (long)n_ones);
   T2_LAUNCH_CHECK();
-  T2_CUDA(cudaMemsetAsync(g_c, 0, (size_t)2 * 64 * kEncH * 4, s));
+  T2_CUDA(cudaMemsetAsync(w.g_c, 0, (size_t)2 * 64 * kEncH * 4, s));
   // ---- BiLSTM: reverse recurrence of both directions (model.py:169-171, 180-188) ----
   for (int step = 0; step < T; ++step) {
-    enc_lstm_bwd_kernel<<<dim3(2, B), 256, 0, s>>>(a->d_memory, part, step > 0, st.gates, st.cst, a->lengths, g_c, dG, B, T, step, nsplit);
+    enc_lstm_bwd_kernel<<<dim3(2, B), 256, 0, s>>>(a->d_memory, w.part, step > 0, st.gates, st.cst, a->lengths, w.g_c, w.dG, B, T, step, nsplit);
     T2_LAUNCH_CHECK();
     if (step + 1 < T) {
-      enc_whh_bwd_kernel<<<dim3(2, nsplit, 2), 256, 0, s>>>(dG, m->w[W_ENC_LSTM + 1], m->w[W_ENC_LSTM + 5], part, B, T, step, nsplit);
+      enc_whh_bwd_kernel<<<dim3(2, nsplit, 2), 256, 0, s>>>(w.dG, m->w[W_ENC_LSTM + 1], m->w[W_ENC_LSTM + 5], w.part, B, T, step, nsplit);
       T2_LAUNCH_CHECK();
     }
   }
   float* const* G = a->grads;
   const int BT = B * T;
   const long n = (long)BT * kEnc;
-  enc_hprev_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.mem, hp, B, T);
+  enc_hprev_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.mem, w.hp, B, T);
   T2_LAUNCH_CHECK();
   for (int dir = 0; dir < 2; ++dir) {
     const int wb = W_ENC_LSTM + 4 * dir;
-    const float* dGd = dG + (size_t)dir * 4 * kEncH;          // rows (b, t), row stride 2048
+    const float* dGd = w.dG + (size_t)dir * 4 * kEncH;          // rows (b, t), row stride 2048
     if (G[wb]) T2_TRY(gemm_tc_rm(m, s, true, false, 4 * kEncH, kEnc, BT, dGd, 8 * kEncH, st.xl, kEnc, G[wb], kEnc, 0.f));
-    if (G[wb + 1]) T2_TRY(gemm_tc_rm(m, s, true, false, 4 * kEncH, kEncH, BT, dGd, 8 * kEncH, hp + (size_t)dir * kEncH, kEnc, G[wb + 1], kEncH, 0.f));
+    if (G[wb + 1]) T2_TRY(gemm_tc_rm(m, s, true, false, 4 * kEncH, kEncH, BT, dGd, 8 * kEncH, w.hp + (size_t)dir * kEncH, kEnc, G[wb + 1], kEncH, 0.f));
     if (G[wb + 2] || G[wb + 3]) {
-      T2_TRY(colsum_f32(m, s, dGd, 8 * kEncH, BT, 4 * kEncH, tmp));
-      if (G[wb + 2]) T2_CUDA(cudaMemcpyAsync(G[wb + 2], tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
-      if (G[wb + 3]) T2_CUDA(cudaMemcpyAsync(G[wb + 3], tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
+      T2_TRY(colsum_f32(m, s, dGd, 8 * kEncH, BT, 4 * kEncH, w.tmp));
+      if (G[wb + 2]) T2_CUDA(cudaMemcpyAsync(G[wb + 2], w.tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
+      if (G[wb + 3]) T2_CUDA(cudaMemcpyAsync(G[wb + 3], w.tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
     }
     // gradient wrt the LSTM input: dG_dir (BT x 1024) . W_ih_dir (1024 x 512)
-    T2_TRY(gemm_tc_rm(m, s, false, false, BT, kEnc, 4 * kEncH, dGd, 8 * kEncH, m->w[wb], kEnc, dxl, kEnc, dir ? 1.f : 0.f));
+    T2_TRY(gemm_tc_rm(m, s, false, false, BT, kEnc, 4 * kEncH, dGd, 8 * kEncH, m->w[wb], kEnc, w.dxl, kEnc, dir ? 1.f : 0.f));
   }
   // ---- conv stack ----
   ConvLayer L[3];
   enc_layers(m, a->training, a->keep, B, T, L);
-  const float* g = dxl; int g_padded = 0;
-  float* gx = gxa;
+  const float* g = w.dxl; int g_padded = 0;
+  float* gx = w.gxa;
   for (int i = 2; i >= 0; --i) {
     const bool need_gx = i > 0 || a->d_embedded || (a->text && G[W_EMB]);
-    T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.cs.x[i], st.cs.z[i], st.cs.stats[i], st.cs.x[i + 1], gz,
-                    need_gx ? gx : nullptr, sums, dwpk, ones, G, wg, planes, s));
+    T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.cs.x[i], st.cs.z[i], st.cs.stats[i], st.cs.x[i + 1], w.gz,
+                    need_gx ? gx : nullptr, w.sums, w.dwpk, w.ones, G, wg, w.planes, s));
     g = gx; g_padded = 1;
-    gx = gx == gxa ? gxb : gxa;
+    gx = gx == w.gxa ? w.gxb : w.gxa;
   }
   if (a->d_embedded) {
     padded_to_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(g, nullptr, a->d_embedded, B, T, kEnc);

@@ -187,66 +187,57 @@ __global__ void wg_reduce_kernel(const float* __restrict__ part, int nsplit, int
   else if (g_hh) g_hh[r * 1024 + (c - c_ih)] = s;
 }
 
-size_t al(size_t x) { return (x + 1023) & ~(size_t)1023; }
-
 }  // namespace
 
-size_t wgrad_tc_ws_bytes(int B, int T) {
-  (void)B;
+constexpr int kWgMaxJobs = 8192;
+
+void wgrad_tc_layout(Carve& c, int T, WgradWs* w) {
   const int seg = wgrad_seg(T), nsplit = (T + seg - 1) / seg;
-  return 2 * al((size_t)T * 4096 * 128 * 2) +                                   // dG^T images of both LSTMs
-         al((size_t)T * 256 * 256) + 3 * al((size_t)(T + 1) * 1024 * 256) +    // x2, ctx (512), ha, hd images (ctx sized like ha)
-         al((size_t)nsplit * 4096 * (1792 + 2560) * 4) +                        // partial sums
-         al((size_t)kStatSplit * 2 * 4096 * 4) + 4 * al(4096 * 4) + al((size_t)8192 * sizeof(WgJob) + 1024) + 8192;
+  for (int l = 0; l < 2; ++l) w->img_a[l] = c.take<uint8_t>((size_t)T * 4096 * 256, 1024);
+  w->img_x2 = c.take<uint8_t>((size_t)T * 256 * 256, 1024);
+  w->img_ctx = c.take<uint8_t>((size_t)(T + 1) * 1024 * 256, 1024);
+  w->img_ha = c.take<uint8_t>((size_t)(T + 1) * 1024 * 256, 1024);
+  w->img_hd = c.take<uint8_t>((size_t)(T + 1) * 1024 * 256, 1024);
+  w->part = c.take<float>((size_t)nsplit * 4096 * (1792 + 2560), 1024);
+  w->stat = c.take<float>((size_t)kStatSplit * 2 * 4096, 1024);
+  w->scale = c.take<float>(4096, 1024);
+  for (int l = 0; l < 2; ++l) w->inv[l] = c.take<float>(4096, 1024);
+  w->colsum = c.take<float>(4096, 1024);
+  w->jobs = c.take<WgJob>(kWgMaxJobs, 1024);
 }
 
 // dga / dgd: (T, B, 4096) fp32; x2 (T, B, 256); stash slots ctx (T+1, B, 512), ha / hd (T+1, B, 1024).
 int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, const float* x2, const DecoderStash& st,
-                 float* const* G, void* ws, size_t ws_bytes, cudaStream_t s) {
+                 float* const* G, const WgradWs& w, cudaStream_t s) {
   (void)m;
-  if (ws_bytes < wgrad_tc_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "wgrad workspace too small");
   const int seg = wgrad_seg(T), nsplit = (T + seg - 1) / seg;
-  uint8_t* p = (uint8_t*)al((size_t)ws);
-  uint8_t* img_a[2];
-  img_a[0] = p; p += al((size_t)T * 4096 * 256);
-  img_a[1] = p; p += al((size_t)T * 4096 * 256);
-  uint8_t* img_x2 = p; p += al((size_t)T * 256 * 256);
-  uint8_t* img_ctx = p; p += al((size_t)(T + 1) * 1024 * 256);
-  uint8_t* img_ha = p; p += al((size_t)(T + 1) * 1024 * 256);
-  uint8_t* img_hd = p; p += al((size_t)(T + 1) * 1024 * 256);
-  float* part = (float*)p; p += al((size_t)nsplit * 4096 * (1792 + 2560) * 4);
-  float* stat = (float*)p; p += al((size_t)kStatSplit * 2 * 4096 * 4);
-  float* scale = (float*)p; p += al(4096 * 4);
-  float* inv[2]; inv[0] = (float*)p; p += al(4096 * 4); inv[1] = (float*)p; p += al(4096 * 4);
-  float* colsum = (float*)p; p += al(4096 * 4);
-  WgJob* jobs_d = (WgJob*)p;
   const long rows = (long)T * B;
   const float* dG[2] = {dga, dgd};
   const int bias_idx[2][2] = {{W_ARNN_BIH, W_ARNN_BHH}, {W_DRNN_BIH, W_DRNN_BHH}};
   for (int l = 0; l < 2; ++l) {
-    wg_colstats_kernel<<<dim3(4096 / 32, kStatSplit), 256, 0, s>>>(dG[l], rows, 4096, stat);
+    wg_colstats_kernel<<<dim3(4096 / 32, kStatSplit), 256, 0, s>>>(dG[l], rows, 4096, w.stat);
     T2_LAUNCH_CHECK();
-    wg_colstats_finalize_kernel<<<4096 / 128, 128, 0, s>>>(stat, 4096, scale, inv[l], colsum);
+    wg_colstats_finalize_kernel<<<4096 / 128, 128, 0, s>>>(w.stat, 4096, w.scale, w.inv[l], w.colsum);
     T2_LAUNCH_CHECK();
     for (int k = 0; k < 2; ++k)
-      if (G[bias_idx[l][k]]) T2_CUDA(cudaMemcpyAsync(G[bias_idx[l][k]], colsum, 4096 * 4, cudaMemcpyDeviceToDevice, s));
-    wg_transpose_img_kernel<<<dim3(4096 / 64, T), 256, 0, s>>>(dG[l], 4096, 0, rows, B, 4096, kTM, scale, img_a[l]);
+      if (G[bias_idx[l][k]]) T2_CUDA(cudaMemcpyAsync(G[bias_idx[l][k]], w.colsum, 4096 * 4, cudaMemcpyDeviceToDevice, s));
+    wg_transpose_img_kernel<<<dim3(4096 / 64, T), 256, 0, s>>>(dG[l], 4096, 0, rows, B, 4096, kTM, w.scale, w.img_a[l]);
     T2_LAUNCH_CHECK();
   }
-  wg_transpose_img_kernel<<<dim3(256 / 64, T), 256, 0, s>>>(x2, 256, 0, rows, B, 256, kTN, nullptr, img_x2);
+  wg_transpose_img_kernel<<<dim3(256 / 64, T), 256, 0, s>>>(x2, 256, 0, rows, B, 256, kTN, nullptr, w.img_x2);
   T2_LAUNCH_CHECK();
-  wg_transpose_img_kernel<<<dim3(512 / 64, T + 1), 256, 0, s>>>(st.ctx, 512, 0, rows + B, B, 512, kTN, nullptr, img_ctx);
+  wg_transpose_img_kernel<<<dim3(512 / 64, T + 1), 256, 0, s>>>(st.ctx, 512, 0, rows + B, B, 512, kTN, nullptr, w.img_ctx);
   T2_LAUNCH_CHECK();
-  wg_transpose_img_kernel<<<dim3(1024 / 64, T + 1), 256, 0, s>>>(st.ha, 1024, 0, rows + B, B, 1024, kTN, nullptr, img_ha);
+  wg_transpose_img_kernel<<<dim3(1024 / 64, T + 1), 256, 0, s>>>(st.ha, 1024, 0, rows + B, B, 1024, kTN, nullptr, w.img_ha);
   T2_LAUNCH_CHECK();
-  wg_transpose_img_kernel<<<dim3(1024 / 64, T + 1), 256, 0, s>>>(st.hd, 1024, 0, rows + B, B, 1024, kTN, nullptr, img_hd);
+  wg_transpose_img_kernel<<<dim3(1024 / 64, T + 1), 256, 0, s>>>(st.hd, 1024, 0, rows + B, B, 1024, kTN, nullptr, w.img_hd);
   T2_LAUNCH_CHECK();
   // job table: LSTM l, feature tile j (of its concatenated input), gate tile i, K split sp
   struct Grp { const uint8_t* img; int ntile; int t0; };   // feature group: image, 256-row tiles per chunk, first chunk
-  const Grp att[3] = {{img_x2, 1, 0}, {img_ctx, 2, 0}, {img_ha, 4, 0}};      // [x2_t | ctx_(t-1) | ah_(t-1)]   model.py:352
-  const Grp dec[3] = {{img_ha, 4, 1}, {img_ctx, 2, 1}, {img_hd, 4, 0}};      // [ah_t | ctx_t | dh_(t-1)]       model.py:366-367
+  const Grp att[3] = {{w.img_x2, 1, 0}, {w.img_ctx, 2, 0}, {w.img_ha, 4, 0}};      // [x2_t | ctx_(t-1) | ah_(t-1)]   model.py:352
+  const Grp dec[3] = {{w.img_ha, 4, 1}, {w.img_ctx, 2, 1}, {w.img_hd, 4, 0}};      // [ah_t | ctx_t | dh_(t-1)]       model.py:366-367
   const int ldc[2] = {1792, 2560};
-  float* part_l[2] = {part, part + (size_t)nsplit * 4096 * 1792};
+  float* part_l[2] = {w.part, w.part + (size_t)nsplit * 4096 * 1792};
   // CTA order = L2 locality: all tiles of one K split (one 100-step window of the images) run together, gate tile outer,
   // feature tile inner, so concurrently resident CTAs share their A and B tiles (ncu: 25.8 GB of DRAM reads for 2.2 GB of
   // operands in the gate-tile-inner order)
@@ -261,18 +252,18 @@ int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, c
             WgJob j;
             const int c0 = sp * seg, n = (T - c0) < seg ? (T - c0) : seg;
             j.a_stride = (uint32_t)(4096 / kTM) * kABytes; j.b_stride = (uint32_t)gr[g].ntile * kBBytes;
-            j.a = img_a[l] + (size_t)c0 * j.a_stride + (size_t)i * kABytes;
+            j.a = w.img_a[l] + (size_t)c0 * j.a_stride + (size_t)i * kABytes;
             j.b = gr[g].img + (size_t)(c0 + gr[g].t0) * j.b_stride + (size_t)jt * kBBytes;
             j.nchunks = n;
             j.out = part_l[l] + ((size_t)sp * 4096 + (size_t)i * kTM) * ldc[l] + col;
             j.ldo = ldc[l];
-            j.inv_scale = inv[l] + i * kTM;
+            j.inv_scale = w.inv[l] + i * kTM;
             jobs.push_back(j);
           }
       }
   }
-  if (jobs.size() > 8192) return fail(T2_ERR_UNSUPPORTED, "wgrad: too many jobs (T too long)");
-  T2_TRY(wg_run_jobs(jobs, jobs_d, s));
+  if (jobs.size() > kWgMaxJobs) return fail(T2_ERR_UNSUPPORTED, "wgrad: too many jobs (T too long)");
+  T2_TRY(wg_run_jobs(jobs, w.jobs, s));
   {
     const long n = (long)4096 * 1792;
     wg_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(part_l[0], nsplit, 1792, 768, G[W_ARNN_WIH], G[W_ARNN_WHH]);

@@ -24,8 +24,15 @@ int wg_transpose_images(const float* src, long ld, long row0, long rows_total, i
 
 constexpr int kWgSeg = 100;      // decoder steps (K chunks of 64 batch rows) per K split
 inline int wgrad_seg(int T) { int seg = kWgSeg; while ((T + seg - 1) / seg > 15) seg += 50; return seg; }
-size_t wgrad_tc_ws_bytes(int B, int T);
+struct WgradWs {                        // every region 1024-aligned
+  uint8_t* img_a[2];                    // dG^T images of both LSTMs
+  uint8_t *img_x2, *img_ctx, *img_ha, *img_hd;   // operand images (ctx sized like ha)
+  float* part;                          // K-split partial sums of both LSTMs
+  float *stat, *scale, *inv[2], *colsum;
+  WgJob* jobs;
+};
+void wgrad_tc_layout(Carve& c, int T, WgradWs* w);
 int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, const float* x2, const DecoderStash& st,
-                 float* const* G, void* ws, size_t ws_bytes, cudaStream_t s);
+                 float* const* G, const WgradWs& w, cudaStream_t s);
 
 }  // namespace t2
