@@ -371,6 +371,48 @@ int    t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_
                      float* mel_post_host, int32_t* mel_lengths_host, int32_t* n_steps_host,
                      void* ws, size_t ws_bytes, void* stream);
 
+/* ---- WaveGlow vocoder inference (waveglow/glow.py: WaveGlow.infer, glow.py:251-293) ---------------
+ * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  The kernels are built for the
+ * published configuration (waveglow/config.json); t2_waveglow_create returns T2_ERR_UNSUPPORTED for anything else.
+ * Precision tier: fp16 = 0 uses split-fp16 (hi + lo) operands with fp32 accumulation and fp32 state ("fp32 grade");
+ * fp16 = 1 (a module converted with .half()) uses single fp16 operands with fp32 accumulation. */
+typedef struct T2WaveGlow T2WaveGlow;   /* opaque: configuration + packed device-side weights */
+typedef struct T2WaveGlowConfig {
+  int32_t n_mel_channels;              /* 80  */
+  int32_t n_flows;                     /* 12  */
+  int32_t n_group;                     /* 8   */
+  int32_t n_early_every;               /* 4   */
+  int32_t n_early_size;                /* 2   */
+  int32_t wn_n_layers;                 /* 8   */
+  int32_t wn_kernel_size;              /* 3   */
+  int32_t wn_n_channels;               /* 256 */
+  int32_t fp16;                        /* 1: the weight table holds __half tensors (except convinv, always fp32) */
+} T2WaveGlowConfig;
+
+/* Entries of the WaveGlow weight table: the reference state_dict in its own order (686 tensors).  Weight-normed
+ * convolutions contribute (bias, weight_g, weight_v); the library folds g * v / ||v|| when it packs.  After
+ * remove_weightnorm a weight_g entry may be NULL and the weight_v entry is then the plain weight. */
+#define T2_WAVEGLOW_NUM_WEIGHTS 686
+
+int t2_waveglow_create(T2WaveGlow** out, const T2WaveGlowConfig* cfg, const void* const* weights, int32_t n_weights,
+                       void* stream);
+int t2_waveglow_refresh(T2WaveGlow* h, const void* const* weights, int32_t n_weights, void* stream);
+int t2_waveglow_destroy(T2WaveGlow* h);
+
+/* mel (B, 80, T_mel), fp32 or (io_half) __half.  lengths (B) int32 in mel frames or NULL: row b's samples
+ * [0, 256 lengths[b]) equal an infer of that row's first lengths[b] frames alone; later samples are zero.
+ * z (B, 8, 32 T_mel) fp32 or NULL: the standard-normal draws, channels in draw order (the 4 initial ones, then the
+ * early blocks of flow 8 and flow 4); NULL => in-kernel Philox4x32-10 keyed by (seed, row, channel, group column).
+ * audio (B, 256 T_mel) out, in the mel's dtype. */
+typedef struct T2WaveGlowArgs {
+  const void* mel; int32_t B, T_mel; const int32_t* lengths; int32_t io_half;
+  float sigma; const float* z; uint64_t seed;
+  void* audio;
+  void* ws; size_t ws_bytes;
+} T2WaveGlowArgs;
+size_t t2_waveglow_workspace_bytes(const T2WaveGlow* h, int32_t B, int32_t T_mel);
+int    t2_waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, void* stream);
+
 /* ---- self tests (libt2b200_selftest.so only: the same sources built with -DT2_SELFTEST; not part of the product
  * library) -------------------------------------------------------------------------------------------------
  * t2_selftest_umma: runs the wgmma split-fp16 GEMM engine used by the persistent decoder on a

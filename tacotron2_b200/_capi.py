@@ -25,7 +25,10 @@ EXPORTS = [
     "t2_loss_workspace_bytes", "t2_tacotron2_loss",
     "t2_mel_spectrogram_frames", "t2_mel_spectrogram_workspace_bytes", "t2_mel_spectrogram", "t2_collate",
     "t2_decoder_stream_state_bytes", "t2_decoder_stream_begin", "t2_decoder_stream_run",
+    "t2_waveglow_create", "t2_waveglow_refresh", "t2_waveglow_destroy", "t2_waveglow_workspace_bytes",
+    "t2_waveglow_infer",
 ]
+T2_WAVEGLOW_NUM_WEIGHTS = 686
 
 
 class T2Config(C.Structure):
@@ -142,6 +145,18 @@ class T2PostnetBwdArgs(C.Structure):
                 ("grads", C.POINTER(C.c_void_p)), ("n_grads", C.c_int32), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
 
 
+class T2WaveGlowConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in (
+        "n_mel_channels", "n_flows", "n_group", "n_early_every", "n_early_size", "wn_n_layers", "wn_kernel_size",
+        "wn_n_channels", "fp16")]
+
+
+class T2WaveGlowArgs(C.Structure):
+    _fields_ = [("mel", C.c_void_p), ("B", C.c_int32), ("T_mel", C.c_int32), ("lengths", C.c_void_p),
+                ("io_half", C.c_int32), ("sigma", C.c_float), ("z", C.c_void_p), ("seed", C.c_uint64),
+                ("audio", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
 _lib = None
 
 
@@ -205,6 +220,13 @@ def lib():
                                 C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_size_t, C.c_void_p]
     L.t2_decoder_profile.argtypes = [C.POINTER(T2DecoderArgs), C.POINTER(C.c_int64)]
+    L.t2_waveglow_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(T2WaveGlowConfig), C.POINTER(C.c_void_p),
+                                     C.c_int32, C.c_void_p]
+    L.t2_waveglow_refresh.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.c_void_p]
+    L.t2_waveglow_destroy.argtypes = [C.c_void_p]
+    L.t2_waveglow_workspace_bytes.restype = C.c_size_t
+    L.t2_waveglow_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    L.t2_waveglow_infer.argtypes = [C.c_void_p, C.POINTER(T2WaveGlowArgs), C.c_void_p]
     if L.t2_abi_version() != 1:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L

@@ -9,6 +9,7 @@
 #include "gemm_tc.h"
 #include "gemm_f32.cuh"
 #include "train_layers.h"
+#include "waveglow.h"
 
 namespace t2 {
 
@@ -431,6 +432,22 @@ int t2_decoder_profile(const T2DecoderArgs* a, int64_t* out_host) {
   T2_CUDA(cudaDeviceSynchronize());
   T2_CUDA(cudaMemcpy(out_host, w.ctrl->prof, sizeof(long long) * 72, cudaMemcpyDeviceToHost));
   return T2_OK;
+}
+
+// ---- WaveGlow (waveglow.cu) ----
+int t2_waveglow_create(T2WaveGlow** out, const T2WaveGlowConfig* cfg, const void* const* weights, int32_t n_weights,
+                       void* stream) {
+  return waveglow_create(out, cfg, weights, n_weights, (cudaStream_t)stream);
+}
+int t2_waveglow_refresh(T2WaveGlow* h, const void* const* weights, int32_t n_weights, void* stream) {
+  return waveglow_refresh(h, weights, n_weights, (cudaStream_t)stream);
+}
+int t2_waveglow_destroy(T2WaveGlow* h) { return waveglow_destroy(h); }
+size_t t2_waveglow_workspace_bytes(const T2WaveGlow*, int32_t B, int32_t T_mel) {
+  return B > 0 && T_mel > 0 ? waveglow_ws_bytes(B, T_mel) : 0;
+}
+int t2_waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, void* stream) {
+  return waveglow_infer(h, a, (cudaStream_t)stream);
 }
 
 #ifdef T2_SELFTEST   // libt2b200_selftest.so only

@@ -1,0 +1,733 @@
+// WaveGlow inference (waveglow/glow.py:251-293, WaveGlow.infer) on sm_90a.
+//
+// Every dense product is one implicit GEMM on wgmma (wg_gemm_kernel) over "k8 planes" (see conv_tc.cu): for each
+// group of 8 channels a hi and a lo plane of [rows][8] fp16, one row per group column (8 audio samples).  A GEMM's K
+// is a list of segments, each a run of 64-channel chunks of some planes read at a row shift, so the dilated k=3
+// convolution of a WN layer and its conditioning 1x1 convolution are ONE GEMM over
+//     [h(t - d); h(t); h(t + d); spect(t)]      K = 3 * 256 + 640 = 1408, N = 512
+// whose epilogue applies tanh * sigmoid (glow.py:34-40) -- cond_layer(spect) (glow.py:159) is never materialised.
+//
+// Rows: sequence b's group column t is row kGuard + b * span + t, span = 32 T_mel + kGuard; the kGuard = 128 rows
+// after every sequence (and before the first) are zero, which is the zero padding of the largest dilation (128).
+// With lengths, the rows t >= 32 len_b are kept zero as well, so a row sees exactly the padding it has alone.
+//
+//   upsample (glow.py:252-258)   ConvTranspose1d(80, 80, 1024, stride 256) as one GEMM over frames: output column
+//                                n = mel * 256 + phase, K = 4 taps (frames F - j) x 80 mels; the epilogue writes the
+//                                trimmed, unfolded (640, 32 T_mel) conditioning planes directly.
+//   per flow (glow.py:271-290)   start (CUDA cores) -> 8 x [gate GEMM, res/skip GEMM] -> flow tail (CUDA cores, one
+//                                thread per column): end, (a1 - b) / exp(s), the inverse 1x1 conv, the early noise,
+//                                and the next flow's start (or the final (B, 8 L) interleave, glow.py:292).
+//
+// Tiers: fp32-grade = hi*hi + lo*hi + hi*lo (3 MMAs per K step); fp16 = hi*hi only, lo planes neither read nor written.
+#include <math.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "conv_tc.h"
+#include "umma.cuh"
+#include "waveglow.h"
+
+struct T2WaveGlow {
+  int fp16;
+  uint8_t* up_img = nullptr; float* up_bias = nullptr;
+  uint8_t* gate_img[12][8] = {}; float* gate_bias = nullptr;     // (12, 8, 512), packed column order
+  uint8_t* rs_img[12][8] = {};   float* rs_bias = nullptr;       // (12, 8, 512)
+  struct t2_flow_w* flows = nullptr;
+  float* tmp = nullptr;                                         // fp32 staging of the matrices being packed
+};
+
+struct t2_flow_w {                 // per flow, fp32, weight norm folded
+  float end_w[8][256]; float end_b[8];
+  float winv[8][8];
+  float start_w[256][4]; float start_b[256];
+};
+
+namespace t2 {
+namespace {
+
+constexpr int kFlows = 12, kLayers = 8, kC = 256, kCond = 640, kGroup = 8;
+constexpr int kTile = 128;                  // rows (group columns / frames) per CTA
+constexpr int kGuard = 128;                 // zero rows around each sequence in the column domain (max dilation)
+constexpr int kFGuard = 4;                  // frame domain: 4 zero frames after each sequence (3 taps look back)
+constexpr int kSeg = kTile * 16;            // one k8 plane of a tile: 2048 bytes
+constexpr int kAStage = 16 * kSeg;          // 8 k8 groups x (hi, lo) = one 64-channel chunk
+constexpr int kNT = 128, kNH = 2, kWS = 4;  // MMA N per weight stage, stages per CTA column tile, weight ring
+constexpr int kWStage = kNT * 64 * 2 * 2;
+constexpr int kOutPitch = kNT * kNH + 4;
+constexpr int kThreads = 384;               // warp 0 producer; warpgroups 1 / 2: MMA + epilogue
+constexpr int kCluster = 2;                 // the CTAs of a cluster share each weight stage by multicast
+constexpr int kUpK = 4 * 128;               // upsample K: 4 taps x 80 mels padded to 128
+constexpr unsigned long long kWd = 1ull << 32;
+
+__device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) {
+  if (ptx::mbar_try_wait(bar, parity)) return;
+  const unsigned long long t0 = clock64();
+  while (!ptx::mbar_try_wait(bar, parity))
+    if (clock64() - t0 > kWd) __trap();
+}
+
+enum { EPI_UPSAMPLE = 0, EPI_GATE = 1, EPI_RESSKIP = 2 };
+
+struct Seg { const __half* planes; long rows; int shift, nchunks; };
+struct GemmParams {
+  Seg seg[4]; int nseg, nchunks;
+  long row0;                        // plane row of tile row 0 of the A operands
+  const uint8_t* wimg;
+  int n_tiles_m;
+  int B, span, T; const int32_t* len; int len_mul;   // tile row q = b * span + t is data when t < T (and < len_b * len_mul)
+  const float* bias;
+  __half* out; long out_rows, out_row0;              // planes the epilogue writes
+  float* skip; int first, res_tiles;                 // RESSKIP: column tiles < res_tiles are the residual half
+  int col_span;                                      // UPSAMPLE: span of the column domain
+};
+
+template <int PASSES>
+__device__ __forceinline__ void store8(__half* planes, long rows, int grp, long row, const float* v) {
+  __align__(16) __half hh[8];
+  __align__(16) __half ll[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) split_fp16(v[i], hh[i], ll[i]);
+  __half* dst = planes + (((long)grp * 2) * rows + row) * 8;
+  *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(hh);
+  if (PASSES == 3) *reinterpret_cast<uint4*>(dst + rows * 8) = *reinterpret_cast<const uint4*>(ll);
+}
+template <int PASSES>
+__device__ __forceinline__ void load8(const __half* planes, long rows, int grp, long row, float* v) {
+  const __half* src = planes + (((long)grp * 2) * rows + row) * 8;
+  __align__(16) __half hh[8];
+  __align__(16) __half ll[8];
+  *reinterpret_cast<uint4*>(hh) = *reinterpret_cast<const uint4*>(src);
+  if (PASSES == 3) *reinterpret_cast<uint4*>(ll) = *reinterpret_cast<const uint4*>(src + rows * 8);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = __half2float(hh[i]) + (PASSES == 3 ? __half2float(ll[i]) : 0.f);
+}
+
+template <int EPI, int PASSES>
+__global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  constexpr uint32_t kABytes = PASSES == 3 ? kAStage : kAStage / 2;
+  constexpr uint32_t kWBytes = PASSES == 3 ? kWStage : kWStage / 2;   // the hi plane comes first in a stage
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int mt = blockIdx.x, nt = blockIdx.y;
+  uint8_t* s_w = smem;
+  uint8_t* s_a = smem + kWS * kWStage;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + 2 * kAStage);
+  uint64_t* a_full = bars; uint64_t* a_empty = bars + 2;
+  uint64_t* w_full = bars + 4; uint64_t* w_empty = bars + 4 + kWS;
+  const uint32_t rank = ptx::cluster_ctarank();
+  if (tid == 0) {
+    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], 2); }
+    for (int i = 0; i < kWS; ++i) { ptx::mbar_init(&w_full[i], 1); ptx::mbar_init(&w_empty[i], 2 * kCluster); }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+  ptx::cluster_sync_all();
+  const bool tile_live = mt < p.n_tiles_m;     // grid.x is rounded up to the cluster size
+
+  if (warp == 0) {
+    if (lane == 0) {
+      const uint64_t pol_w = ptx::policy_evict_last(), pol_a = ptx::policy_evict_first();
+      uint32_t wst = 0, wph = 0;
+      const int mrow = tile_live ? mt : 0;     // dead tiles (cluster padding) stream tile 0 and discard
+      for (int c = 0; c < p.nchunks; ++c) {
+        const int sa = c & 1;
+        wait_bar(&a_empty[sa], ((c >> 1) & 1) ^ 1);
+        ptx::mbar_arrive_expect_tx(&a_full[sa], kABytes);
+        const __half* base = nullptr; long rows = 0; int shift = 0, cc = 0, rem = c;
+        bool found = false;
+#pragma unroll
+        for (int s = 0; s < 4; ++s)
+          if (!found && s < p.nseg) {
+            if (rem < p.seg[s].nchunks) { base = p.seg[s].planes; rows = p.seg[s].rows; shift = p.seg[s].shift; cc = rem; found = true; }
+            else rem -= p.seg[s].nchunks;
+          }
+        const long r0 = p.row0 + (long)mrow * kTile + shift;
+        for (int g = 0; g < 8; ++g)
+          for (int hl = 0; hl < (PASSES == 3 ? 2 : 1); ++hl) {
+            const __half* src = base + (((long)(cc * 8 + g) * 2 + hl) * rows + r0) * 8;
+            ptx::bulk_g2s_hint(s_a + sa * kAStage + (hl * 8 + g) * kSeg, src, kSeg, &a_full[sa], pol_a);
+          }
+        for (int h = 0; h < kNH; ++h) {
+          wait_bar(&w_empty[wst], wph ^ 1);
+          ptx::mbar_arrive_expect_tx(&w_full[wst], kWBytes);
+          const uint8_t* wsrc = p.wimg + ((size_t)(nt * kNH + h) * p.nchunks + c) * kWStage;
+          const uint32_t slice = kWBytes / kCluster;
+          ptx::bulk_g2s_mc_hint(s_w + wst * kWStage + rank * slice, wsrc + rank * slice, slice, &w_full[wst],
+                                (uint16_t)((1u << kCluster) - 1u), pol_w);
+          if (++wst == kWS) { wst = 0; wph ^= 1; }
+        }
+      }
+    }
+    __syncwarp();
+  } else if (tid >= 128) {
+    const int wg = (tid >> 7) - 1, wt = tid & 127;
+    float d[kNH][kNT / 2];
+#pragma unroll
+    for (int h = 0; h < kNH; ++h) {
+#pragma unroll
+      for (int i = 0; i < kNT / 2; ++i) d[h][i] = 0.f;
+      ptx::wg_fence_regs<kNT / 2>(d[h]);
+    }
+    uint32_t wst = 0, wph = 0;
+    for (int c = 0; c < p.nchunks; ++c) {
+      const int sa = c & 1;
+      wait_bar(&a_full[sa], (c >> 1) & 1);
+      const uint32_t ab = ptx::smem_u32(s_a + sa * kAStage) + (uint32_t)wg * (64 * 16);
+#pragma unroll
+      for (int h = 0; h < kNH; ++h) {
+        wait_bar(&w_full[wst], wph);
+        const uint32_t wb = ptx::smem_u32(s_w + wst * kWStage);
+        ptx::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint32_t aoff = (2 * kk) * kSeg;
+          const uint64_t a_hi = ptx::make_smem_desc(ab + aoff, kSeg, 128);
+          const uint64_t b_hi = ptx::make_sw128_desc(wb + kk * 32);
+          ptx::wgmma_f16<kNT>(d[h], a_hi, b_hi);
+          if (PASSES == 3) {
+            const uint64_t a_lo = ptx::make_smem_desc(ab + 8 * kSeg + aoff, kSeg, 128);
+            const uint64_t b_lo = ptx::make_sw128_desc(wb + kNT * 128 + kk * 32);
+            ptx::wgmma_f16<kNT>(d[h], a_lo, b_hi);
+            ptx::wgmma_f16<kNT>(d[h], a_hi, b_lo);
+          }
+        }
+        ptx::wg_commit();
+        ptx::wg_wait<0>();
+        ptx::wg_fence_regs<kNT / 2>(d[h]);
+        if (wt == 0)
+          for (int r = 0; r < kCluster; ++r) ptx::mbar_arrive_cluster(&w_empty[wst], r);
+        if (++wst == kWS) { wst = 0; wph ^= 1; }
+      }
+      if (wt == 0) ptx::mbar_arrive(&a_empty[sa]);
+    }
+    // every stage this CTA receives has been consumed: the operand stages become the fp32 output tile
+    ptx::named_bar_sync(1, 256);
+    float* s_out = reinterpret_cast<float*>(smem);
+#pragma unroll
+    for (int h = 0; h < kNH; ++h)
+#pragma unroll
+      for (int i = 0; i < kNT / 2; i += 2) {
+        const int r = wg * 64 + ptx::wg_frag_row(i, wt), col = h * kNT + ptx::wg_frag_col(i, wt);
+        *reinterpret_cast<float2*>(s_out + r * kOutPitch + col) = make_float2(d[h][i], d[h][i + 1]);
+      }
+    ptx::named_bar_sync(1, 256);
+    // ---- epilogue: thread = (tile row r, half of the columns) ----
+    const int ct = tid - 128, r = ct & 127, half = ct >> 7;
+    const long q = (long)mt * kTile + r;
+    const int b = (int)(q / p.span), t = (int)(q - (long)b * p.span);
+    const bool data = tile_live && b < p.B && t < p.T;
+    const bool valid = data && (p.len == nullptr || t < p.len[b] * p.len_mul);
+    const float* row = s_out + r * kOutPitch;
+    if (tile_live) {
+      if (EPI == EPI_GATE) {
+        // columns [0, 128) of the tile are the tanh inputs of channels nt*128 + c, [128, 256) their sigmoid inputs
+        const float* bias = p.bias + nt * 256;
+        for (int g = 0; g < 8; ++g) {
+          const int c0 = half * 64 + g * 8;
+          float v[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float xt = row[c0 + i] + bias[c0 + i], xs = row[128 + c0 + i] + bias[128 + c0 + i];
+            v[i] = valid ? tanhf(xt) * (1.f / (1.f + expf(-xs))) : 0.f;
+          }
+          store8<PASSES>(p.out, p.out_rows, nt * 16 + (c0 >> 3), p.out_row0 + q, v);
+        }
+      } else if (EPI == EPI_RESSKIP) {
+        if (nt < p.res_tiles) {            // audio = audio + res_skip_acts[:, :256]  (glow.py:170)
+          for (int g = 0; g < 16; ++g) {
+            const int c0 = half * 128 + g * 8;
+            float v[8];
+            load8<PASSES>(p.out, p.out_rows, c0 >> 3, p.out_row0 + q, v);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = valid ? v[i] + (row[c0 + i] + p.bias[c0 + i]) : 0.f;
+            store8<PASSES>(p.out, p.out_rows, c0 >> 3, p.out_row0 + q, v);
+          }
+        } else {                           // output = output + res_skip_acts[:, 256:]  (glow.py:171, 173)
+          const int n0 = nt * 256 + half * 128;
+          float* sk = p.skip + q * kC + half * 128;
+          for (int c = 0; c < 128; c += 4) {
+            float4 x = make_float4(row[half * 128 + c] + p.bias[n0 + c], row[half * 128 + c + 1] + p.bias[n0 + c + 1],
+                                   row[half * 128 + c + 2] + p.bias[n0 + c + 2], row[half * 128 + c + 3] + p.bias[n0 + c + 3]);
+            if (!p.first) {
+              const float4 o = *reinterpret_cast<const float4*>(sk + c);
+              x.x += o.x; x.y += o.y; x.z += o.z; x.w += o.w;
+            }
+            *reinterpret_cast<float4*>(sk + c) = x;
+          }
+        }
+      } else {                             // EPI_UPSAMPLE: tile column tile nt = mel channel, column = phase
+        if (data) {
+          const float bo = p.bias[nt];
+          const long crow = p.out_row0 + (long)b * p.col_span + 32L * t + half * 16;
+          for (int k = 0; k < 16; ++k) {
+            float v[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = row[half * 128 + k * 8 + i] + bo;
+            store8<PASSES>(p.out, p.out_rows, nt, crow + k, v);
+          }
+        }
+      }
+    }
+  }
+  __syncthreads();
+  // peers' consumers arrive on our w_empty barriers: drain before leaving
+  if (tid == 0) {
+    const int total = p.nchunks * kNH;
+    for (int i = 0; i < kWS; ++i) {
+      const int uses = (total - i + kWS - 1) / kWS;
+      if (uses > 0) wait_bar(&w_empty[i], (uses - 1) & 1);
+    }
+  }
+  __syncthreads();
+  ptx::cluster_sync_all();
+}
+
+template <int EPI, int PASSES>
+int launch_gemm(const GemmParams& p, int n_tiles_n, cudaStream_t s) {
+  const size_t smem = (size_t)kWS * kWStage + 2 * kAStage + (4 + 2 * kWS) * 8 + 64;
+  static_assert(kTile * kOutPitch * 4 <= kWS * kWStage + 2 * kAStage, "output tile reuses the operand stages");
+  T2_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<EPI, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  const int gx = ((p.n_tiles_m + kCluster - 1) / kCluster) * kCluster;
+  cfg.gridDim = dim3(gx, n_tiles_n); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+  cudaLaunchAttribute at;
+  at.id = cudaLaunchAttributeClusterDimension;
+  at.val.clusterDim.x = kCluster; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+  cfg.attrs = &at; cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, wg_gemm_kernel<EPI, PASSES>, p);
+  if (e != cudaSuccess) return fail(T2_ERR_CUDA, "waveglow gemm launch failed: %s", cudaGetErrorString(e));
+  g_launch_count++;
+  return T2_OK;
+}
+
+template <int EPI>
+int gemm(const GemmParams& p, int n_tiles_n, bool fp16, cudaStream_t s) {
+  return fp16 ? launch_gemm<EPI, 1>(p, n_tiles_n, s) : launch_gemm<EPI, 3>(p, n_tiles_n, s);
+}
+
+// ---- Philox normal draws ----------------------------------------------------------------------------
+// z(b, c, t): Philox4x32-10 with counter (t, b, c, kNoiseTag) and key (seed lo, seed hi); Box-Muller on the first
+// two output words: u1 = ((o0 >> 8) + 1) 2^-24 in (0, 1], u2 = (o1 >> 8) 2^-24, z = sqrt(-2 ln u1) cos(2 pi u2).
+constexpr uint32_t kNoiseTag = 0x3c6ef372u;
+__device__ __forceinline__ float philox_normal(uint64_t seed, int b, int c, int t) {
+  uint32_t o[4];
+  philox4x32_10((uint32_t)t, (uint32_t)b, (uint32_t)c, kNoiseTag, (uint32_t)seed, (uint32_t)(seed >> 32), o);
+  const float u1 = (float)((o[0] >> 8) + 1u) * (1.0f / 16777216.0f);
+  const float u2 = (float)(o[1] >> 8) * (1.0f / 16777216.0f);
+  return sqrtf(-2.0f * logf(u1)) * cosf(6.28318530717958647692f * u2);
+}
+
+struct TailParams {
+  const t2_flow_w* fw;
+  int k;                 // flow whose WN just ran (-1: none, draw the initial noise)
+  int next;              // flow whose start runs next, -1: write the audio
+  int B, span, T; const int32_t* len; long n_rows;
+  float sigma; const float* z; uint64_t seed;
+  const float* skip; float* aud;
+  __half* h; long h_rows;
+  void* audio; int io_half;
+};
+
+__device__ __forceinline__ int n_rem_of(int k) { return 8 - 2 * (k / 4); }   // 4 (k >= 8), 6 (k >= 4), 8
+
+template <int PASSES>
+__global__ void __launch_bounds__(128) flow_tail_kernel(const TailParams p) {
+  const long q = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= p.n_rows) return;
+  const int b = (int)(q / p.span), t = (int)(q - (long)b * p.span);
+  const bool data = b < p.B && t < p.T;
+  const bool valid = data && (p.len == nullptr || t < p.len[b] * 32);
+  const int L = p.T;
+  auto noise = [&](int c) -> float {
+    if (!valid) return 0.f;
+    return p.sigma * (p.z ? p.z[((long)b * kGroup + c) * L + t] : philox_normal(p.seed, b, c, t));
+  };
+  float a[8];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) a[c] = 0.f;
+  if (p.k < 0) {                                   // glow.py:260-269
+#pragma unroll
+    for (int c = 0; c < 4; ++c) a[c] = noise(c);
+  } else if (valid) {
+    const t2_flow_w& f = p.fw[p.k];
+    const int nr = n_rem_of(p.k), nh = nr / 2;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) if (c < nr) a[c] = p.aud[q * 8 + c];
+    // end (glow.py:175) over the accumulated skip output
+    float o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] = 0.f;
+    const float* sk = p.skip + q * kC;
+    for (int c = 0; c < kC; c += 4) {
+      const float4 s4 = *reinterpret_cast<const float4*>(sk + c);
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (j < 2 * nh) {
+          const float4 w4 = *reinterpret_cast<const float4*>(&f.end_w[j][c]);
+          o[j] = fmaf(w4.x, s4.x, fmaf(w4.y, s4.y, fmaf(w4.z, s4.z, fmaf(w4.w, s4.w, o[j]))));
+        }
+    }
+    // audio_1 = (audio_1 - b) / exp(s)  (glow.py:278-281)
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (i < nh) a[nh + i] = (a[nh + i] - (o[i] + f.end_b[i])) / expf(o[nh + i] + f.end_b[nh + i]);
+    // inverse 1x1 convolution (glow.py:283, 91-96)
+    float na[8];
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      float acc = 0.f;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) if (r < nr && c < nr) acc = fmaf(f.winv[r][c], a[c], acc);
+      na[r] = acc;
+    }
+    if (p.k % 4 == 0 && p.k > 0) {                 // early output: cat(sigma * z, audio)  (glow.py:285-290)
+      const int zc = p.k == 8 ? 4 : 6;
+#pragma unroll
+      for (int r = 7; r >= 2; --r) a[r] = na[r - 2];
+      a[0] = noise(zc); a[1] = noise(zc + 1);
+    } else {
+#pragma unroll
+      for (int r = 0; r < 8; ++r) a[r] = na[r];
+    }
+  }
+  if (p.next >= 0) {
+#pragma unroll
+    for (int c = 0; c < 8; ++c) p.aud[q * 8 + c] = valid ? a[c] : 0.f;
+    // start of the next flow (glow.py:155): h = W_start a[:n_half] + b
+    const t2_flow_w& f = p.fw[p.next];
+    const int nh = n_rem_of(p.next) / 2;
+    for (int g = 0; g < kC / 8; ++g) {
+      float v[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int c = g * 8 + i;
+        float acc = f.start_b[c];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) if (j < nh) acc = fmaf(f.start_w[c][j], a[j], acc);
+        v[i] = valid ? acc : 0.f;
+      }
+      store8<PASSES>(p.h, p.h_rows, g, kGuard + q, v);
+    }
+  } else if (data) {                               // glow.py:292: audio[b, 8 t + c]
+    const long o0 = (long)b * 8 * L + 8L * t;
+    if (p.io_half) {
+      __half* out = reinterpret_cast<__half*>(p.audio) + o0;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) out[c] = __float2half_rn(valid ? a[c] : 0.f);
+    } else {
+      float* out = reinterpret_cast<float*>(p.audio) + o0;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) out[c] = valid ? a[c] : 0.f;
+    }
+  }
+}
+
+// mel (B, 80, T) -> frame-domain planes (16 groups, channels >= 80 zero); frames >= len zero; every row written
+__global__ void mel_to_planes_kernel(const void* __restrict__ mel, int io_half, int B, int T, const int32_t* __restrict__ len,
+                                     __half* __restrict__ planes, long rows, int passes) {
+  const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int g = blockIdx.y;
+  if (row >= rows) return;
+  const long q = row - kFGuard;
+  const int span = T + kFGuard;
+  int b = -1, f = -1;
+  if (q >= 0) { b = (int)(q / span); f = (int)(q - (long)b * span); }
+  const bool valid = b >= 0 && b < B && f < T && (len == nullptr || f < len[b]);
+  float v[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int c = g * 8 + i;
+    float x = 0.f;
+    if (valid && c < 80) {
+      const long idx = ((long)b * 80 + c) * T + f;
+      x = io_half ? __half2float(reinterpret_cast<const __half*>(mel)[idx]) : reinterpret_cast<const float*>(mel)[idx];
+    }
+    v[i] = x;
+  }
+  if (passes == 3) store8<3>(planes, rows, g, row, v);
+  else store8<1>(planes, rows, g, row, v);
+}
+
+// ---- weight packing ----------------------------------------------------------------------------------
+__device__ __forceinline__ float ldw(const void* p, long i, int half) {
+  return half ? __half2float(reinterpret_cast<const __half*>(p)[i]) : reinterpret_cast<const float*>(p)[i];
+}
+// g / ||v|| of row n of a weight-normed tensor (1 when g is null: the weight is plain); 256 threads
+__device__ float wn_scale(const void* v, const void* g, long n, int per_row, int half) {
+  __shared__ float red[8];
+  __shared__ float res;
+  if (g == nullptr) return 1.f;
+  float ss = 0.f;
+  for (int i = threadIdx.x; i < per_row; i += blockDim.x) { const float x = ldw(v, n * per_row + i, half); ss += x * x; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tot = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+    res = ldw(g, n, half) / sqrtf(tot);
+  }
+  __syncthreads();
+  const float r = res;
+  __syncthreads();
+  return r;
+}
+
+// gate GEMM weight [512][1408]: packed row nn = tile * 256 + h * 128 + r is source row h * 256 + tile * 128 + r
+// (tanh rows, then the matching sigmoid rows); K = [in_layer tap 0 | tap 1 | tap 2 | cond slice]
+__global__ void build_gate_kernel(const void* in_b, const void* in_g, const void* in_v, const void* cond_b,
+                                  const void* cond_g, const void* cond_v, int layer, int half, float* w, float* bias) {
+  const int nn = blockIdx.x;
+  const int n = ((nn >> 7) & 1) * 256 + (nn >> 8) * 128 + (nn & 127);
+  const long nc = (long)layer * 512 + n;
+  const float si = wn_scale(in_v, in_g, n, kC * 3, half);
+  const float sc = wn_scale(cond_v, cond_g, nc, kCond, half);
+  for (int k = threadIdx.x; k < 3 * kC + kCond; k += blockDim.x) {
+    float x;
+    if (k < 3 * kC) { const int tap = k / kC, ci = k % kC; x = ldw(in_v, ((long)n * kC + ci) * 3 + tap, half) * si; }
+    else x = ldw(cond_v, nc * kCond + (k - 3 * kC), half) * sc;
+    w[(long)nn * (3 * kC + kCond) + k] = x;
+  }
+  if (threadIdx.x == 0) bias[nn] = ldw(in_b, n, half) + ldw(cond_b, nc, half);
+}
+
+__global__ void build_rs_kernel(const void* rs_b, const void* rs_g, const void* rs_v, int half, float* w, float* bias) {
+  const int n = blockIdx.x;
+  const float s = wn_scale(rs_v, rs_g, n, kC, half);
+  for (int k = threadIdx.x; k < kC; k += blockDim.x) w[(long)n * kC + k] = ldw(rs_v, (long)n * kC + k, half) * s;
+  if (threadIdx.x == 0) bias[n] = ldw(rs_b, n, half);
+}
+
+// upsample as a GEMM: row n = o * 256 + phase, k = tap * 128 + i:  W[i][o][phase + 256 tap]
+__global__ void build_up_kernel(const void* up_w, const void* up_b, int half, float* w, float* bias) {
+  const int n = blockIdx.x, o = n >> 8, ph = n & 255;
+  for (int k = threadIdx.x; k < kUpK; k += blockDim.x) {
+    const int tap = k >> 7, i = k & 127;
+    w[(long)n * kUpK + k] = i < 80 ? ldw(up_w, ((long)i * 80 + o) * 1024 + ph + 256 * tap, half) : 0.f;
+  }
+  if (threadIdx.x == 0 && ph == 0) bias[o] = ldw(up_b, o, half);
+}
+
+// start / end / inverse W of one flow; W^-1 by Gauss-Jordan with partial pivoting in double (once, at pack time)
+__global__ void build_flow_kernel(const void* st_b, const void* st_g, const void* st_v, const void* end_w, const void* end_b,
+                                  const float* convinv, int nr, int half, t2_flow_w* f) {
+  const int nh = nr / 2;
+  for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) {
+    const int j = i / 256, c = i % 256;
+    f->end_w[j][c] = j < nr ? ldw(end_w, (long)j * kC + c, half) : 0.f;
+  }
+  if (threadIdx.x < 8) f->end_b[threadIdx.x] = threadIdx.x < nr ? ldw(end_b, threadIdx.x, half) : 0.f;
+  for (int c = 0; c < kC; ++c) {
+    const float s = wn_scale(st_v, st_g, c, nh, half);
+    if (threadIdx.x < 4) f->start_w[c][threadIdx.x] = threadIdx.x < nh ? ldw(st_v, (long)c * nh + threadIdx.x, half) * s : 0.f;
+    if (threadIdx.x == 0) f->start_b[c] = ldw(st_b, c, half);
+  }
+  if (threadIdx.x == 0) {
+    double m[8][16];
+    for (int r = 0; r < nr; ++r)
+      for (int c = 0; c < 2 * nr; ++c) m[r][c] = c < nr ? (double)convinv[r * nr + c] : (c - nr == r ? 1.0 : 0.0);
+    for (int c = 0; c < nr; ++c) {
+      int piv = c;
+      for (int r = c + 1; r < nr; ++r) if (fabs(m[r][c]) > fabs(m[piv][c])) piv = r;
+      for (int j = 0; j < 2 * nr; ++j) { const double x = m[c][j]; m[c][j] = m[piv][j]; m[piv][j] = x; }
+      const double d = m[c][c];
+      for (int j = 0; j < 2 * nr; ++j) m[c][j] /= d;
+      for (int r = 0; r < nr; ++r)
+        if (r != c) { const double e = m[r][c]; for (int j = 0; j < 2 * nr; ++j) m[r][j] -= e * m[c][j]; }
+    }
+    for (int r = 0; r < 8; ++r)
+      for (int c = 0; c < 8; ++c) f->winv[r][c] = (r < nr && c < nr) ? (float)m[r][nr + c] : 0.f;
+  }
+}
+
+// weight table indices (state_dict order): upsample (2), WN.k (56 each), convinv.k
+constexpr int kWUpW = 0, kWUpB = 1;
+constexpr int wn_base(int k) { return 2 + 56 * k; }
+constexpr int kWConvinv = 2 + 56 * kFlows;
+static_assert(kWConvinv + kFlows == T2_WAVEGLOW_NUM_WEIGHTS, "waveglow weight table");
+
+int check_weights(const void* const* w, int n) {
+  if (n != T2_WAVEGLOW_NUM_WEIGHTS) return fail(T2_ERR_INVALID, "waveglow: expected %d weight pointers, got %d", T2_WAVEGLOW_NUM_WEIGHTS, n);
+  for (int i = 0; i < n; ++i) {
+    const int o = (i - 2) % 56;            // weight_g entries may be null (plain weights after remove_weightnorm)
+    const bool g_entry = i >= 2 && i < kWConvinv && ((o < 51 && o % 3 == 1) || o == 54);
+    if (w[i] == nullptr && !g_entry) return fail(T2_ERR_INVALID, "waveglow: weight %d is null", i);
+  }
+  return T2_OK;
+}
+
+struct WsLayout {
+  __half* x; long x_rows;
+  __half* spect; __half* h; __half* acts; long rows;
+  float* skip; float* aud;
+};
+struct Dims { int L, span, ntm, spanf, ntf; };
+Dims dims_of(int B, int T) {
+  Dims d;
+  d.L = 32 * T; d.span = d.L + kGuard;
+  d.ntm = (int)(((long)B * d.span + kTile - 1) / kTile);
+  d.spanf = T + kFGuard;
+  d.ntf = (int)(((long)B * d.spanf + kTile - 1) / kTile);
+  return d;
+}
+void ws_layout(Carve& c, int B, int T, WsLayout* o) {
+  const Dims d = dims_of(B, T);
+  o->x_rows = kFGuard + (long)d.ntf * kTile;
+  o->rows = kGuard + (long)d.ntm * kTile + kGuard;
+  o->x = c.take<__half>((size_t)16 * 2 * o->x_rows * 8, 1024);
+  o->spect = c.take<__half>((size_t)80 * 2 * o->rows * 8, 1024);
+  o->h = c.take<__half>((size_t)32 * 2 * o->rows * 8, 1024);
+  o->acts = c.take<__half>((size_t)32 * 2 * o->rows * 8, 1024);
+  o->skip = c.take<float>((size_t)d.ntm * kTile * kC, 1024);
+  o->aud = c.take<float>((size_t)d.ntm * kTile * 8, 1024);
+}
+
+}  // namespace
+
+// ---- host API -----------------------------------------------------------------------------------------
+static int pack(T2WaveGlow* m, const void* const* w, cudaStream_t s) {
+  const int half = m->fp16;
+  build_up_kernel<<<80 * 256, 256, 0, s>>>(w[kWUpW], w[kWUpB], half, m->tmp, m->up_bias);
+  T2_LAUNCH_CHECK();
+  T2_TRY(tc_pack_weights(m->tmp, 80 * 256, kUpK, 1, kNT, &m->up_img, s));
+  for (int k = 0; k < kFlows; ++k) {
+    const int base = wn_base(k);
+    const int nr = k >= 8 ? 4 : (k >= 4 ? 6 : 8);
+    for (int l = 0; l < kLayers; ++l) {
+      const int in = base + 3 * l, rs = base + 24 + 3 * l;
+      float* gb = m->gate_bias + ((size_t)k * kLayers + l) * 512;
+      build_gate_kernel<<<512, 256, 0, s>>>(w[in], w[in + 1], w[in + 2], w[base + 53], w[base + 54], w[base + 55], l, half,
+                                             m->tmp, gb);
+      T2_LAUNCH_CHECK();
+      T2_TRY(tc_pack_weights(m->tmp, 512, 3 * kC + kCond, 1, kNT, &m->gate_img[k][l], s));
+      const int nrs = l < kLayers - 1 ? 512 : 256;
+      float* rb = m->rs_bias + ((size_t)k * kLayers + l) * 512;
+      build_rs_kernel<<<nrs, 256, 0, s>>>(w[rs], w[rs + 1], w[rs + 2], half, m->tmp, rb);
+      T2_LAUNCH_CHECK();
+      T2_TRY(tc_pack_weights(m->tmp, nrs, kC, 1, kNT, &m->rs_img[k][l], s));
+    }
+    build_flow_kernel<<<1, 256, 0, s>>>(w[base + 48], w[base + 49], w[base + 50], w[base + 51], w[base + 52],
+                                        reinterpret_cast<const float*>(w[kWConvinv + k]), nr, half, m->flows + k);
+    T2_LAUNCH_CHECK();
+  }
+  return T2_OK;
+}
+
+int waveglow_create(T2WaveGlow** out, const T2WaveGlowConfig* c, const void* const* w, int n, cudaStream_t s) {
+  if (!out || !c || !w) return fail(T2_ERR_INVALID, "waveglow: null argument");
+  const bool ok = c->n_mel_channels == 80 && c->n_flows == kFlows && c->n_group == kGroup && c->n_early_every == 4 &&
+                  c->n_early_size == 2 && c->wn_n_layers == kLayers && c->wn_kernel_size == 3 && c->wn_n_channels == kC &&
+                  (c->fp16 == 0 || c->fp16 == 1);
+  if (!ok)
+    return fail(T2_ERR_UNSUPPORTED, "waveglow: configuration differs from the published one the sm_90a kernels are built for "
+                                    "(n_mel 80, 12 flows, group 8, early 4 / 2, WN 8 layers x 256 channels, kernel 3)");
+  T2_TRY(check_weights(w, n));
+  int dev = 0;
+  T2_CUDA(cudaGetDevice(&dev));
+  cudaDeviceProp p;
+  T2_CUDA(cudaGetDeviceProperties(&p, dev));
+  if (p.major != 9 || p.minor != 0) return fail(T2_ERR_UNSUPPORTED, "libt2b200 is built for sm_90a only (device is sm_%d%d)", p.major, p.minor);
+  T2WaveGlow* m = new T2WaveGlow();
+  m->fp16 = c->fp16;
+  int r = T2_OK;
+  if (cudaMalloc((void**)&m->up_bias, 80 * sizeof(float)) != cudaSuccess ||
+      cudaMalloc((void**)&m->gate_bias, (size_t)kFlows * kLayers * 512 * sizeof(float)) != cudaSuccess ||
+      cudaMalloc((void**)&m->rs_bias, (size_t)kFlows * kLayers * 512 * sizeof(float)) != cudaSuccess ||
+      cudaMalloc((void**)&m->flows, kFlows * sizeof(t2_flow_w)) != cudaSuccess ||
+      cudaMalloc((void**)&m->tmp, (size_t)80 * 256 * kUpK * sizeof(float)) != cudaSuccess)
+    r = fail(T2_ERR_CUDA, "waveglow: out of device memory for the packed weights");
+  if (r == T2_OK) r = pack(m, w, s);
+  if (r != T2_OK) { waveglow_destroy(m); return r; }
+  *out = m;
+  return T2_OK;
+}
+
+int waveglow_refresh(T2WaveGlow* m, const void* const* w, int n, cudaStream_t s) {
+  if (!m || !w) return fail(T2_ERR_INVALID, "waveglow: null argument");
+  T2_TRY(check_weights(w, n));
+  return pack(m, w, s);
+}
+
+int waveglow_destroy(T2WaveGlow* m) {
+  if (!m) return T2_OK;
+  cudaFree(m->up_img); cudaFree(m->up_bias); cudaFree(m->gate_bias); cudaFree(m->rs_bias); cudaFree(m->flows); cudaFree(m->tmp);
+  for (int k = 0; k < kFlows; ++k)
+    for (int l = 0; l < kLayers; ++l) { cudaFree(m->gate_img[k][l]); cudaFree(m->rs_img[k][l]); }
+  delete m;
+  return T2_OK;
+}
+
+size_t waveglow_ws_bytes(int B, int T) {
+  Carve c(nullptr, 1024);
+  WsLayout o;
+  ws_layout(c, B, T, &o);
+  return c.bytes();
+}
+
+int waveglow_infer(T2WaveGlow* m, const T2WaveGlowArgs* a, cudaStream_t s) {
+  if (!m || !a || !a->mel || !a->audio || !a->ws) return fail(T2_ERR_INVALID, "waveglow: null argument");
+  if (a->B <= 0 || a->T_mel <= 0) return fail(T2_ERR_INVALID, "waveglow: empty input (B=%d, T_mel=%d)", a->B, a->T_mel);
+  if ((long)a->B * (32L * a->T_mel + kGuard) > (1L << 30)) return fail(T2_ERR_INVALID, "waveglow: input too large");
+  if (a->ws_bytes < waveglow_ws_bytes(a->B, a->T_mel)) return fail(T2_ERR_WORKSPACE, "waveglow workspace too small");
+  const int B = a->B, T = a->T_mel, fp16 = m->fp16, passes = fp16 ? 1 : 3;
+  const Dims d = dims_of(B, T);
+  Carve c(a->ws, 1024);
+  WsLayout o;
+  ws_layout(c, B, T, &o);
+  // guard rows must read as zero; every tile row is rewritten by the kernels below
+  T2_CUDA(cudaMemsetAsync(o.spect, 0, (size_t)80 * 2 * o.rows * 16, s));
+  T2_CUDA(cudaMemsetAsync(o.h, 0, (size_t)32 * 2 * o.rows * 16, s));
+  T2_CUDA(cudaMemsetAsync(o.acts, 0, (size_t)32 * 2 * o.rows * 16, s));
+  mel_to_planes_kernel<<<dim3((unsigned)((o.x_rows + 127) / 128), 16), 128, 0, s>>>(a->mel, a->io_half, B, T, a->lengths,
+                                                                                  o.x, o.x_rows, passes);
+  T2_LAUNCH_CHECK();
+  // upsample + trim + unfold (glow.py:252-258)
+  GemmParams u;
+  memset(&u, 0, sizeof(u));
+  for (int j = 0; j < 4; ++j) u.seg[j] = Seg{o.x, o.x_rows, -j, 2};
+  u.nseg = 4; u.nchunks = 8; u.row0 = kFGuard; u.wimg = m->up_img; u.n_tiles_m = d.ntf;
+  u.B = B; u.span = d.spanf; u.T = T; u.bias = m->up_bias;
+  u.out = o.spect; u.out_rows = o.rows; u.out_row0 = kGuard; u.col_span = d.span;
+  T2_TRY(gemm<EPI_UPSAMPLE>(u, 80, fp16, s));
+
+  TailParams tp;
+  memset(&tp, 0, sizeof(tp));
+  tp.fw = m->flows; tp.B = B; tp.span = d.span; tp.T = d.L; tp.len = a->lengths; tp.n_rows = (long)d.ntm * kTile;
+  tp.sigma = a->sigma; tp.z = a->z; tp.seed = a->seed; tp.skip = o.skip; tp.aud = o.aud; tp.h = o.h; tp.h_rows = o.rows;
+  tp.audio = a->audio; tp.io_half = a->io_half;
+  const unsigned tail_blocks = (unsigned)((tp.n_rows + 127) / 128);
+  auto tail = [&](int k, int next) -> int {
+    tp.k = k; tp.next = next;
+    if (fp16) flow_tail_kernel<1><<<tail_blocks, 128, 0, s>>>(tp);
+    else flow_tail_kernel<3><<<tail_blocks, 128, 0, s>>>(tp);
+    T2_LAUNCH_CHECK();
+    return T2_OK;
+  };
+  T2_TRY(tail(-1, kFlows - 1));
+  GemmParams g;
+  memset(&g, 0, sizeof(g));
+  g.row0 = kGuard; g.n_tiles_m = d.ntm; g.B = B; g.span = d.span; g.T = d.L; g.len = a->lengths; g.len_mul = 32;
+  g.out_rows = o.rows; g.out_row0 = kGuard; g.skip = o.skip;
+  for (int k = kFlows - 1; k >= 0; --k) {
+    for (int l = 0; l < kLayers; ++l) {
+      const int dil = 1 << l;
+      // in_layer(audio) + cond_layer(spect)[slice] -> tanh * sigmoid  (glow.py:161-166)
+      g.seg[0] = Seg{o.h, o.rows, -dil, 4}; g.seg[1] = Seg{o.h, o.rows, 0, 4}; g.seg[2] = Seg{o.h, o.rows, dil, 4};
+      g.seg[3] = Seg{o.spect, o.rows, 0, 10};
+      g.nseg = 4; g.nchunks = 22; g.wimg = m->gate_img[k][l]; g.bias = m->gate_bias + ((size_t)k * kLayers + l) * 512;
+      g.out = o.acts;
+      T2_TRY(gemm<EPI_GATE>(g, 2, fp16, s));
+      // res_skip_layers (glow.py:168-173)
+      g.seg[0] = Seg{o.acts, o.rows, 0, 4};
+      g.nseg = 1; g.nchunks = 4; g.wimg = m->rs_img[k][l]; g.bias = m->rs_bias + ((size_t)k * kLayers + l) * 512;
+      g.out = o.h; g.first = l == 0; g.res_tiles = l < kLayers - 1 ? 1 : 0;
+      T2_TRY(gemm<EPI_RESSKIP>(g, l < kLayers - 1 ? 2 : 1, fp16, s));
+    }
+    T2_TRY(tail(k, k > 0 ? k - 1 : -1));
+  }
+  return T2_OK;
+}
+
+}  // namespace t2

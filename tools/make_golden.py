@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz by executing the UNMODIFIED reference model.py (needs a checkout of
-NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live]
+NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live|waveglow]
 
 Every file holds the inputs' seeds, the reference outputs and a checksum of the synthetic weights
 (tests/common.synth_state_dict) so a drift of the generator is detected instead of silently
@@ -490,7 +490,95 @@ def reference_live_case():
     save("reference_live", **arrays)
 
 
+# ---- WaveGlow (waveglow/glow.py, run on the CPU with the noise injected) ----------------------------------------
+def import_reference_glow(z_queue):
+    """The reference's glow.py with one shim: ``torch.cuda.FloatTensor(*size).normal_()`` (glow.py:265, 289) returns
+    the next injected draw from ``z_queue`` instead of touching CUDA."""
+    import importlib.util
+    import types
+    spec = importlib.util.spec_from_file_location("t2_reference_glow", os.path.join(REFERENCE_DIR, "waveglow", "glow.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+
+    class _Draw:
+        def __init__(self, *size):
+            self.size = tuple(size)
+
+        def normal_(self):
+            z = z_queue.pop(0)
+            assert tuple(z.shape) == self.size, (tuple(z.shape), self.size)
+            return z.clone()
+
+    class _TorchProxy(types.ModuleType):
+        def __getattr__(self, name):
+            return getattr(torch, name)
+
+    proxy = _TorchProxy("torch")
+    proxy.cuda = types.SimpleNamespace(FloatTensor=_Draw, HalfTensor=_Draw)
+    mod.torch = proxy
+    return mod
+
+
+def reference_waveglow_infer(sd, mel, sigma, z):
+    """Reference WaveGlow.infer with z (B, 8, L) split into its three draws in draw order."""
+    from tests.waveglow_common import CONFIG
+    queue = [z[:, 0:4].contiguous(), z[:, 4:6].contiguous(), z[:, 6:8].contiguous()]
+    glow = import_reference_glow(queue)
+    model = glow.WaveGlow(**CONFIG)
+    model.load_state_dict(sd)
+    with torch.no_grad():
+        out = model.infer(mel, sigma=sigma)
+    assert not queue
+    return out
+
+
+def waveglow_init_case():
+    from tests.waveglow_common import CONFIG
+    glow = import_reference_glow([])
+    torch.manual_seed(1234)
+    model = glow.WaveGlow(**CONFIG)
+    sd = model.state_dict()
+    keys = list(sd)
+    shapes = [",".join(str(x) for x in sd[k].shape) for k in keys]
+    digests = [tensor_digest(sd[k]) for k in keys]
+    model = glow.WaveGlow.remove_weightnorm(model)
+    sd2 = model.state_dict()
+    save("waveglow_init", keys=np.array(keys), shapes=np.array(shapes), digests=np.array(digests),
+         removed_keys=np.array(list(sd2)), removed_digests=np.array([tensor_digest(sd2[k]) for k in sd2]))
+
+
+def waveglow_infer_case(name, B, T, sigma, wseed, mseed, zseed):
+    from tests.waveglow_common import mel_input, noise, synth_state_dict
+    sd = synth_state_dict(wseed)
+    mel, z = mel_input(B, T, mseed), noise(B, T, zseed)
+    audio = reference_waveglow_infer(sd, mel, sigma, z)
+    save(name, mel=mel, z=z, audio=audio, sigma=sigma, wseed=wseed, checksum=weights_checksum(sd))
+
+
+def waveglow_full_case(name, B, T, sigma, wseed, mseed, zseed, n_samples=4096):
+    """Large fixture: inputs regenerated from their seeds, outputs as seeded sample entries + full-tensor statistics."""
+    from tests.waveglow_common import mel_input, noise, synth_state_dict
+    sd = synth_state_dict(wseed)
+    mel, z = mel_input(B, T, mseed), noise(B, T, zseed)
+    audio = reference_waveglow_infer(sd, mel, sigma, z)
+    idx = sample_index(audio.numel(), n_samples, 5)
+    a = audio.double()
+    save(name, B=B, T=T, sigma=sigma, wseed=wseed, mseed=mseed, zseed=zseed, checksum=weights_checksum(sd),
+         mel_digest=tensor_digest(mel), z_digest=tensor_digest(z), idx=idx, samples=audio.reshape(-1)[idx],
+         stats=np.array([float(a.mean()), float(a.std()), float(a.abs().max()), float(a.abs().mean())]))
+
+
+def waveglow_cases():
+    waveglow_init_case()
+    waveglow_infer_case("waveglow_b1_t50_s0", 1, 50, 0.0, 7, 41, 42)
+    waveglow_infer_case("waveglow_b3_t37_s666", 3, 37, 0.666, 7, 43, 44)
+    waveglow_full_case("waveglow_full_b2_t800", 2, 800, 0.666, 7, 45, 46)
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "waveglow":
+        waveglow_cases()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "live":
         reference_live_case()
         sys.exit(0)
