@@ -413,6 +413,26 @@ typedef struct T2WaveGlowArgs {
 size_t t2_waveglow_workspace_bytes(const T2WaveGlow* h, int32_t B, int32_t T_mel);
 int    t2_waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, void* stream);
 
+/* Windowed inference: the audio of some frames of a longer sequence from a window of its mel, bit-identical to the
+ * same samples of t2_waveglow_infer over the whole sequence.  wg.mel holds frames [frame0, frame0 + T_mel) of the
+ * sequence and wg.lengths are relative to the window (frames >= lengths[b] count as zero).  The audio of the
+ * window-relative frames [out0, out1) is written to wg.audio, (B, 256 (out1 - out0)).  The noise is keyed by the
+ * absolute group column 32 frame0 + t: Philox as above, or an injected wg.z (B, 8, 32 z_frames) read at absolute
+ * columns, z_frames >= frame0 + T_mel.  at_end: the window ends where the sequence ends.
+ * The audio of a frame depends on the 99 frames before it and the 96 after it (t2_waveglow_window_halo: left, right).  The call returns T2_ERR_INVALID, launching nothing, when out0 is closer than the left
+ * halo to a window start that is not the sequence's start (frame0 > 0), or out1 closer than the right halo to a
+ * window end that is not the sequence's end (at_end = 0).  Workspace: t2_waveglow_workspace_bytes(h, B, T_mel).
+ * t2_waveglow_infer is this call with frame0 = 0, [out0, out1) = [0, T_mel), z_frames = T_mel and at_end = 1. */
+typedef struct T2WaveGlowWindowArgs {
+  T2WaveGlowArgs wg;
+  int32_t frame0;
+  int32_t out0, out1;
+  int32_t z_frames;
+  int32_t at_end;
+} T2WaveGlowWindowArgs;
+void   t2_waveglow_window_halo(int32_t* left, int32_t* right);
+int    t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void* stream);
+
 /* ---- self tests (libt2b200_selftest.so only: the same sources built with -DT2_SELFTEST; not part of the product
  * library) -------------------------------------------------------------------------------------------------
  * t2_selftest_umma: runs the wgmma split-fp16 GEMM engine used by the persistent decoder on a

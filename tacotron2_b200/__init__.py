@@ -6,9 +6,9 @@ from .layers import TacotronSTFT  # noqa: F401
 from .loss_function import Tacotron2Loss  # noqa: F401
 from .model import Decoder, Encoder, Postnet, Tacotron2  # noqa: F401
 from . import amp  # noqa: F401
-from .glow import WaveGlow, waveglow_noise  # noqa: F401
+from .glow import WaveGlow, waveglow_noise, window_halo  # noqa: F401
 from .optim import AmpFusedClipAdam, FusedClipAdam  # noqa: F401
 
 __all__ = ["Tacotron2", "Encoder", "Decoder", "Postnet", "Tacotron2Loss", "create_hparams", "dropout_masks",
            "FusedClipAdam", "AmpFusedClipAdam", "amp", "invalidate_weights", "TacotronSTFT",
-           "WaveGlow", "waveglow_noise"]
+           "WaveGlow", "waveglow_noise", "window_halo"]

@@ -26,7 +26,7 @@ EXPORTS = [
     "t2_mel_spectrogram_frames", "t2_mel_spectrogram_workspace_bytes", "t2_mel_spectrogram", "t2_collate",
     "t2_decoder_stream_state_bytes", "t2_decoder_stream_begin", "t2_decoder_stream_run",
     "t2_waveglow_create", "t2_waveglow_refresh", "t2_waveglow_destroy", "t2_waveglow_workspace_bytes",
-    "t2_waveglow_infer",
+    "t2_waveglow_infer", "t2_waveglow_infer_window", "t2_waveglow_window_halo",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686
 
@@ -157,6 +157,11 @@ class T2WaveGlowArgs(C.Structure):
                 ("audio", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
 
 
+class T2WaveGlowWindowArgs(C.Structure):
+    _fields_ = [("wg", T2WaveGlowArgs), ("frame0", C.c_int32), ("out0", C.c_int32), ("out1", C.c_int32),
+                ("z_frames", C.c_int32), ("at_end", C.c_int32)]
+
+
 _lib = None
 
 
@@ -227,6 +232,9 @@ def lib():
     L.t2_waveglow_workspace_bytes.restype = C.c_size_t
     L.t2_waveglow_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.t2_waveglow_infer.argtypes = [C.c_void_p, C.POINTER(T2WaveGlowArgs), C.c_void_p]
+    L.t2_waveglow_infer_window.argtypes = [C.c_void_p, C.POINTER(T2WaveGlowWindowArgs), C.c_void_p]
+    L.t2_waveglow_window_halo.restype = None
+    L.t2_waveglow_window_halo.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     if L.t2_abi_version() != 1:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L

@@ -449,6 +449,10 @@ size_t t2_waveglow_workspace_bytes(const T2WaveGlow*, int32_t B, int32_t T_mel) 
 int t2_waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, void* stream) {
   return waveglow_infer(h, a, (cudaStream_t)stream);
 }
+int t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void* stream) {
+  return waveglow_infer_window(h, a, (cudaStream_t)stream);
+}
+void t2_waveglow_window_halo(int32_t* left, int32_t* right) { waveglow_window_halo(left, right); }
 
 #ifdef T2_SELFTEST   // libt2b200_selftest.so only
 int t2_selftest_mma_rate(int32_t M, int32_t N, int32_t reps, int32_t alternate_d, int64_t* out_host) {

@@ -21,6 +21,7 @@
 // Tiers: fp32-grade = hi*hi + lo*hi + hi*lo (3 MMAs per K step); fp16 = hi*hi only, lo planes neither read nor written.
 #include <math.h>
 #include <stdlib.h>
+#include <algorithm>
 #include <string.h>
 
 #include "conv_tc.h"
@@ -57,6 +58,14 @@ constexpr int kOutPitch = kNT * kNH + 4;
 constexpr int kThreads = 384;               // warp 0 producer; warpgroups 1 / 2: MMA + epilogue
 constexpr int kCluster = 2;                 // the CTAs of a cluster share each weight stage by multicast
 constexpr int kUpK = 4 * 128;               // upsample K: 4 taps x 80 mels padded to 128
+// Receptive field of infer, in group columns (32 per frame).  One flow: the WN's dilated k = 3 layers reach
+// +-(1 + 2 + ... + 128) = +-255 columns; start, end, the coupling, the inverse 1x1 conv and the noise act per column.
+// Twelve flows: +-3060.  The upsample gives a column of frame f the frames f-3 ... f.  So the audio of frames [t0, t1)
+// is fixed by the frames [t0 - 96 - 3, t1 + 96).
+constexpr int kFlowReach = 255;
+constexpr int kUpLook = 3;
+constexpr int kHaloRight = (kFlows * kFlowReach + 31) / 32;   // 96 frames
+constexpr int kHaloLeft = kHaloRight + kUpLook;                // 99 frames
 constexpr unsigned long long kWd = 1ull << 32;
 
 __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) {
@@ -73,8 +82,9 @@ struct GemmParams {
   Seg seg[4]; int nseg, nchunks;
   long row0;                        // plane row of tile row 0 of the A operands
   const uint8_t* wimg;
-  int n_tiles_m;
+  int n_tiles_m, mt0;               // M tiles; the grid starts at tile mt0 (set by launch_gemm)
   int B, span, T; const int32_t* len; int len_mul;   // tile row q = b * span + t is data when t < T (and < len_b * len_mul)
+  int lo, hi;                       // only rows with t in [lo, hi) are needed: a cluster holding none of them exits
   const float* bias;
   __half* out; long out_rows, out_row0;              // planes the epilogue writes
   float* skip; int first, res_tiles;                 // RESSKIP: column tiles < res_tiles are the residual half
@@ -102,13 +112,35 @@ __device__ __forceinline__ void load8(const __half* planes, long rows, int grp, 
   for (int i = 0; i < 8; ++i) v[i] = __half2float(hh[i]) + (PASSES == 3 ? __half2float(ll[i]) : 0.f);
 }
 
+// does M tile mt hold a row q = b * span + t with b < B and t in [lo, hi)?
+// (B * span <= 2^30, so int arithmetic suffices)
+__device__ __forceinline__ bool tile_needed(const GemmParams& p, int mt) {
+  if (mt >= p.n_tiles_m) return false;
+  const int q0 = mt * kTile;
+  for (int b = q0 / p.span; b < p.B && b * p.span < q0 + kTile; ++b) {
+    const int s0 = b * p.span;
+    if (max(q0 - s0, p.lo) < min(q0 + kTile - s0, p.hi)) return true;
+  }
+  return false;
+}
+
 template <int EPI, int PASSES>
 __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr uint32_t kABytes = PASSES == 3 ? kAStage : kAStage / 2;
   constexpr uint32_t kWBytes = PASSES == 3 ? kWStage : kWStage / 2;   // the hi plane comes first in a stage
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int mt = blockIdx.x, nt = blockIdx.y;
+  const int mt = p.mt0 + blockIdx.x, nt = blockIdx.y;
+  if (p.lo > 0 || p.hi < p.T) {
+    // both CTAs of a cluster take the same decision before any barrier: skip when neither tile holds a needed row.
+    // A skipped tile writes nothing; its guard rows keep the zeros they were cleared to.  (With the full range every
+    // launched cluster holds data rows.)
+    const int c0 = p.mt0 + (int)(blockIdx.x & ~(unsigned)(kCluster - 1));
+    bool need = false;
+#pragma unroll
+    for (int i = 0; i < kCluster; ++i) need = need || tile_needed(p, c0 + i);
+    if (!need) return;
+  }
   uint8_t* s_w = smem;
   uint8_t* s_a = smem + kWS * kWStage;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_a + 2 * kAStage);
@@ -283,13 +315,16 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
 }
 
 template <int EPI, int PASSES>
-int launch_gemm(const GemmParams& p, int n_tiles_n, cudaStream_t s) {
+int launch_gemm(GemmParams p, int n_tiles_n, cudaStream_t s) {
   const size_t smem = (size_t)kWS * kWStage + 2 * kAStage + (4 + 2 * kWS) * 8 + 64;
   static_assert(kTile * kOutPitch * 4 <= kWS * kWStage + 2 * kAStage, "output tile reuses the operand stages");
   T2_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<EPI, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  const int gx = ((p.n_tiles_m + kCluster - 1) / kCluster) * kCluster;
+  // the grid spans the tiles from the first needed row (sequence 0, t = lo) to the last (sequence B-1, t = hi-1)
+  p.mt0 = p.lo / kTile;
+  const int last = (int)(((long)(p.B - 1) * p.span + p.hi - 1) / kTile);
+  const int gx = ((last - p.mt0 + 1 + kCluster - 1) / kCluster) * kCluster;
   cfg.gridDim = dim3(gx, n_tiles_n); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
   cudaLaunchAttribute at;
   at.id = cudaLaunchAttributeClusterDimension;
@@ -328,20 +363,27 @@ struct TailParams {
   __half* h; long h_rows;
   void* audio; int io_half;
 };
+// The window's fields are a separate kernel argument: added to TailParams they changed the tail kernel's code (39 -> 32
+// registers, more constant-bank reloads) and made it about 30 % slower on the full sequence.
+struct TailRange {
+  int lo, hi;            // rows with t in [lo, hi) are computed; with next = -1 they are the audio written
+  int col0; long z_stride;   // noise of window column t: absolute column col0 + t; rows of an injected z
+};
 
 __device__ __forceinline__ int n_rem_of(int k) { return 8 - 2 * (k / 4); }   // 4 (k >= 8), 6 (k >= 4), 8
 
 template <int PASSES>
-__global__ void __launch_bounds__(128) flow_tail_kernel(const TailParams p) {
+__global__ void __launch_bounds__(128) flow_tail_kernel(const TailParams p, const TailRange w) {
   const long q = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= p.n_rows) return;
   const int b = (int)(q / p.span), t = (int)(q - (long)b * p.span);
   const bool data = b < p.B && t < p.T;
+  if (data && (t < w.lo || t >= w.hi)) return;     // not needed by what follows
   const bool valid = data && (p.len == nullptr || t < p.len[b] * 32);
-  const int L = p.T;
   auto noise = [&](int c) -> float {
     if (!valid) return 0.f;
-    return p.sigma * (p.z ? p.z[((long)b * kGroup + c) * L + t] : philox_normal(p.seed, b, c, t));
+    const int ta = w.col0 + t;
+    return p.sigma * (p.z ? p.z[((long)b * kGroup + c) * w.z_stride + ta] : philox_normal(p.seed, b, c, ta));
   };
   float a[8];
 #pragma unroll
@@ -409,8 +451,8 @@ __global__ void __launch_bounds__(128) flow_tail_kernel(const TailParams p) {
       }
       store8<PASSES>(p.h, p.h_rows, g, kGuard + q, v);
     }
-  } else if (data) {                               // glow.py:292: audio[b, 8 t + c]
-    const long o0 = (long)b * 8 * L + 8L * t;
+  } else if (data) {                               // glow.py:292: audio[b, 8 (t - lo) + c], rows of 8 (hi - lo)
+    const long o0 = (long)b * 8 * (w.hi - w.lo) + 8L * (t - w.lo);
     if (p.io_half) {
       __half* out = reinterpret_cast<__half*>(p.audio) + o0;
 #pragma unroll
@@ -666,17 +708,48 @@ size_t waveglow_ws_bytes(int B, int T) {
   return c.bytes();
 }
 
+void waveglow_window_halo(int* left, int* right) {
+  if (left) *left = kHaloLeft;
+  if (right) *right = kHaloRight;
+}
+
 int waveglow_infer(T2WaveGlow* m, const T2WaveGlowArgs* a, cudaStream_t s) {
-  if (!m || !a || !a->mel || !a->audio || !a->ws) return fail(T2_ERR_INVALID, "waveglow: null argument");
+  if (!a) return fail(T2_ERR_INVALID, "waveglow: null argument");
+  T2WaveGlowWindowArgs w;
+  memset(&w, 0, sizeof(w));
+  w.wg = *a;
+  w.frame0 = 0; w.out0 = 0; w.out1 = a->T_mel; w.z_frames = a->T_mel; w.at_end = 1;
+  return waveglow_infer_window(m, &w, s);
+}
+
+int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStream_t s) {
+  if (!m || !wa || !wa->wg.mel || !wa->wg.audio || !wa->wg.ws) return fail(T2_ERR_INVALID, "waveglow: null argument");
+  const T2WaveGlowArgs* a = &wa->wg;
   if (a->B <= 0 || a->T_mel <= 0) return fail(T2_ERR_INVALID, "waveglow: empty input (B=%d, T_mel=%d)", a->B, a->T_mel);
-  if ((long)a->B * (32L * a->T_mel + kGuard) > (1L << 30)) return fail(T2_ERR_INVALID, "waveglow: input too large");
+  if ((long)a->B * (32L * a->T_mel + kGuard) > (1L << 30) || 32L * ((long)wa->frame0 + a->T_mel) > (1L << 30))
+    return fail(T2_ERR_INVALID, "waveglow: input too large");
+  const int frame0 = wa->frame0, out0 = wa->out0, out1 = wa->out1;
+  if (frame0 < 0 || out0 < 0 || out1 <= out0 || out1 > a->T_mel)
+    return fail(T2_ERR_INVALID, "waveglow window: output frames [%d, %d) are not a non-empty range of the window's %d "
+                "frames (frame0 %d)", out0, out1, a->T_mel, frame0);
+  if (frame0 > 0 && out0 < kHaloLeft)
+    return fail(T2_ERR_INVALID, "waveglow window: output frames start %d frames after a window start that is not the "
+                "sequence's start; the left halo is %d frames", out0, kHaloLeft);
+  if (!wa->at_end && out1 + kHaloRight > a->T_mel)
+    return fail(T2_ERR_INVALID, "waveglow window: output frames end %d frames before a window end that is not the "
+                "sequence's end; the right halo is %d frames", a->T_mel - out1, kHaloRight);
+  if (a->z && wa->z_frames < frame0 + a->T_mel)
+    return fail(T2_ERR_INVALID, "waveglow window: z holds %d frames, the window ends at frame %d", wa->z_frames,
+                frame0 + a->T_mel);
   if (a->ws_bytes < waveglow_ws_bytes(a->B, a->T_mel)) return fail(T2_ERR_WORKSPACE, "waveglow workspace too small");
   const int B = a->B, T = a->T_mel, fp16 = m->fp16, passes = fp16 ? 1 : 3;
   const Dims d = dims_of(B, T);
   Carve c(a->ws, 1024);
   WsLayout o;
   ws_layout(c, B, T, &o);
-  // guard rows must read as zero; every tile row is rewritten by the kernels below
+  // Guard rows must read as zero: they are cleared here and only ever rewritten with zeros.  With per-flow ranges
+  // (below) the rows a flow does not need are not rewritten and may hold stale values from earlier flows or calls
+  // (skip and aud are not cleared at all); that is safe because no needed row reads an unneeded one.
   T2_CUDA(cudaMemsetAsync(o.spect, 0, (size_t)80 * 2 * o.rows * 16, s));
   T2_CUDA(cudaMemsetAsync(o.h, 0, (size_t)32 * 2 * o.rows * 16, s));
   T2_CUDA(cudaMemsetAsync(o.acts, 0, (size_t)32 * 2 * o.rows * 16, s));
@@ -688,29 +761,41 @@ int waveglow_infer(T2WaveGlow* m, const T2WaveGlowArgs* a, cudaStream_t s) {
   memset(&u, 0, sizeof(u));
   for (int j = 0; j < 4; ++j) u.seg[j] = Seg{o.x, o.x_rows, -j, 2};
   u.nseg = 4; u.nchunks = 8; u.row0 = kFGuard; u.wimg = m->up_img; u.n_tiles_m = d.ntf;
-  u.B = B; u.span = d.spanf; u.T = T; u.bias = m->up_bias;
+  u.B = B; u.span = d.spanf; u.T = T; u.lo = 0; u.hi = T; u.bias = m->up_bias;
   u.out = o.spect; u.out_rows = o.rows; u.out_row0 = kGuard; u.col_span = d.span;
   T2_TRY(gemm<EPI_UPSAMPLE>(u, 80, fp16, s));
 
+  // Per-flow column ranges.  The audio columns [32 out0, 32 out1) need the output of the flow that runs with n flows
+  // still to follow over those columns widened by n * kFlowReach; that flow's WN layers run over one reach more.
+  // Everything is clipped to the window: at a sequence edge the zero padding is the sequence's own.
+  auto widen = [&](int n, int* lo, int* hi) {
+    *lo = (int)std::max(0L, 32L * out0 - (long)kFlowReach * n);
+    *hi = (int)std::min((long)d.L, 32L * out1 + (long)kFlowReach * n);
+  };
   TailParams tp;
   memset(&tp, 0, sizeof(tp));
   tp.fw = m->flows; tp.B = B; tp.span = d.span; tp.T = d.L; tp.len = a->lengths; tp.n_rows = (long)d.ntm * kTile;
-  tp.sigma = a->sigma; tp.z = a->z; tp.seed = a->seed; tp.skip = o.skip; tp.aud = o.aud; tp.h = o.h; tp.h_rows = o.rows;
+  tp.sigma = a->sigma; tp.z = a->z; tp.seed = a->seed;
+  TailRange tr;
+  tr.col0 = 32 * frame0; tr.z_stride = 32L * wa->z_frames;
+  tp.skip = o.skip; tp.aud = o.aud; tp.h = o.h; tp.h_rows = o.rows;
   tp.audio = a->audio; tp.io_half = a->io_half;
   const unsigned tail_blocks = (unsigned)((tp.n_rows + 127) / 128);
-  auto tail = [&](int k, int next) -> int {
-    tp.k = k; tp.next = next;
-    if (fp16) flow_tail_kernel<1><<<tail_blocks, 128, 0, s>>>(tp);
-    else flow_tail_kernel<3><<<tail_blocks, 128, 0, s>>>(tp);
+  auto tail = [&](int k, int next) -> int {   // k flows follow this tail (k = 12: the initial draw)
+    tp.k = k < kFlows ? k : -1; tp.next = next;
+    widen(k, &tr.lo, &tr.hi);
+    if (fp16) flow_tail_kernel<1><<<tail_blocks, 128, 0, s>>>(tp, tr);
+    else flow_tail_kernel<3><<<tail_blocks, 128, 0, s>>>(tp, tr);
     T2_LAUNCH_CHECK();
     return T2_OK;
   };
-  T2_TRY(tail(-1, kFlows - 1));
+  T2_TRY(tail(kFlows, kFlows - 1));
   GemmParams g;
   memset(&g, 0, sizeof(g));
   g.row0 = kGuard; g.n_tiles_m = d.ntm; g.B = B; g.span = d.span; g.T = d.L; g.len = a->lengths; g.len_mul = 32;
   g.out_rows = o.rows; g.out_row0 = kGuard; g.skip = o.skip;
   for (int k = kFlows - 1; k >= 0; --k) {
+    widen(k + 1, &g.lo, &g.hi);
     for (int l = 0; l < kLayers; ++l) {
       const int dil = 1 << l;
       // in_layer(audio) + cond_layer(spect)[slice] -> tanh * sigmoid  (glow.py:161-166)

@@ -11,5 +11,7 @@ int    waveglow_refresh(T2WaveGlow* h, const void* const* weights, int n, cudaSt
 int    waveglow_destroy(T2WaveGlow* h);
 size_t waveglow_ws_bytes(int B, int T_mel);
 int    waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, cudaStream_t s);
+int    waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, cudaStream_t s);
+void   waveglow_window_halo(int* left, int* right);
 
 }  // namespace t2

@@ -176,6 +176,26 @@ class WaveGlow(torch.nn.Module):
         first lengths[b] frames alone; later samples are zero."""
         return self._engine().infer(self, spect, sigma, lengths, getattr(_tls, "z", None))
 
+    def infer_stream(self, items, sigma=1.0):
+        """infer() over the items of ``Tacotron2.inference_stream(...)``, as a generator that hands out audio as soon as
+        no later mel frame can change it.
+
+        Each item is a dict: ``samples`` = (s0, s1), the same for every row; ``audio`` (B, s1 - s0) in the mel's dtype;
+        ``mel_lengths`` and ``finished`` of the mel item it came from.  The audio of frame t depends on the mel frames
+        t - 99 ... t + 96 (``window_halo()``), so while a row is live an item holds the audio of every frame up to the
+        final mel frames less 96, and the last item (``finished``) holds the rest; mel items that make no audio final
+        yield nothing.  Each item runs one windowed inference over the frames its audio depends on.  Concatenated along
+        time the audio is bit-identical to ``infer(mel_outputs_postnet, sigma, lengths=model.mel_lengths)`` after
+        ``model.inference(...)``, with the same weights and inputs and the same injected noise (``waveglow_noise``, read
+        when infer_stream is called) or torch seed: the stream draws its Philox seed from torch's generator once, at its
+        first mel item.  A stopped row's samples past 256 * mel_lengths are zero.
+
+        The stream keeps on the device only the final mel frames later windows can still need (at most the two halos and
+        one item's frames).  Several streams, and infer, can be used on one WaveGlow at a time: each stream has its own
+        frames, noise seed and position, and they share the module's workspace, so all of them must enqueue on the same
+        CUDA stream (torch's current stream), as successive infer calls do."""
+        return self._engine().stream(self, items, sigma, getattr(_tls, "z", None))
+
 
 class _WaveGlowEngine:
     """One T2WaveGlow handle (packed weights on one device) + a cached workspace."""
@@ -239,40 +259,129 @@ class _WaveGlowEngine:
         except Exception:
             pass
 
+    def _spect(self, spect, what):
+        if spect.dim() != 3 or spect.shape[1] != self.cfg[0]:
+            raise ValueError("%s: spect must be (B, %d, T_mel), got %s" % (what, self.cfg[0], tuple(spect.shape)))
+        if spect.dtype not in (torch.float32, torch.float16):
+            raise TypeError("%s: spect must be float32 or float16, got %s" % (what, spect.dtype))
+        return spect.to(self.device).contiguous()
+
+    def _z(self, z, B, T):
+        """Injected noise as fp32 on the device, (B, n_group, 32 T') with T' >= T frames; returns (tensor, T')."""
+        zt = z.to(device=self.device, dtype=torch.float32).contiguous()
+        if zt.dim() != 3 or tuple(zt.shape[:2]) != (B, N_GROUP) or zt.shape[2] % 32 or zt.shape[2] < 32 * T:
+            raise ValueError("waveglow_noise: z must be (%d, %d, 32 T_mel) with T_mel >= %d, got %s" %
+                             (B, N_GROUP, T, tuple(z.shape)))
+        return zt, zt.shape[2] // 32
+
+    def _draw_seed(self):
+        # Philox seed drawn from torch's default generator: reproducible under torch.manual_seed, fresh on every call
+        seed = int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64).item())
+        self.last_seed = seed
+        return seed
+
+    def _args(self, spect, len32, zt, sigma, seed, audio):
+        """T2WaveGlowArgs over spect (B, n_mel, T) on the device, with a workspace of the engine's cache."""
+        B, T = int(spect.shape[0]), int(spect.shape[2])
+        a = _capi.T2WaveGlowArgs()
+        a.mel, a.B, a.T_mel, a.io_half = spect.data_ptr(), B, T, int(spect.dtype == torch.float16)
+        if len32 is not None:
+            a.lengths = len32.data_ptr()
+        if zt is not None:
+            a.z = zt.data_ptr()
+        a.sigma, a.seed = float(sigma), seed
+        nbytes = int(_capi.lib().t2_waveglow_workspace_bytes(self.handle, B, T))
+        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != self.device:
+            self._ws = None
+            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        a.audio, a.ws, a.ws_bytes = audio.data_ptr(), self._ws.data_ptr(), self._ws.numel()
+        return a
+
     def infer(self, module, spect, sigma, lengths, z):
         self.ensure(module)
-        if spect.dim() != 3 or spect.shape[1] != self.cfg[0]:
-            raise ValueError("WaveGlow.infer: spect must be (B, %d, T_mel), got %s" % (self.cfg[0], tuple(spect.shape)))
-        if spect.dtype not in (torch.float32, torch.float16):
-            raise TypeError("WaveGlow.infer: spect must be float32 or float16, got %s" % spect.dtype)
+        spect = self._spect(spect, "WaveGlow.infer")
         dev = self.device
-        spect = spect.to(dev).contiguous()
         B, T = int(spect.shape[0]), int(spect.shape[2])
         L = _capi.lib()
         audio = torch.empty(B, HOP * T, device=dev, dtype=spect.dtype)
-        a = _capi.T2WaveGlowArgs()
-        a.mel, a.B, a.T_mel, a.io_half = spect.data_ptr(), B, T, int(spect.dtype == torch.float16)
         len32 = None
         if lengths is not None:
             len32 = torch.as_tensor(lengths).to(device=dev, dtype=torch.int32).contiguous()
             if tuple(len32.shape) != (B,):
                 raise ValueError("WaveGlow.infer: lengths must have shape (%d,)" % B)
-            a.lengths = len32.data_ptr()
         zt = None
         if z is not None:
             zt = z.to(device=dev, dtype=torch.float32).contiguous()
             if tuple(zt.shape) != (B, N_GROUP, 32 * T):
                 raise ValueError("waveglow_noise: z must be (%d, %d, %d), got %s" % (B, N_GROUP, 32 * T, tuple(z.shape)))
-            a.z = zt.data_ptr()
-        a.sigma = float(sigma)
-        # Philox seed drawn from torch's default generator: reproducible under torch.manual_seed, fresh on every call
-        a.seed = int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64).item())
-        self.last_seed = a.seed
-        nbytes = int(L.t2_waveglow_workspace_bytes(self.handle, B, T))
-        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != dev:
-            self._ws = None
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        a.audio, a.ws, a.ws_bytes = audio.data_ptr(), self._ws.data_ptr(), self._ws.numel()
+        a = self._args(spect, len32, zt, sigma, self._draw_seed(), audio)
         with torch.cuda.device(dev):
             _capi.check(L.t2_waveglow_infer(self.handle, C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
         return audio
+
+    def infer_window(self, spect, len32, zt, z_frames, sigma, seed, frame0, out0, out1, at_end):
+        """Audio (B, 256 (out1 - out0)) of the window-relative frames [out0, out1) of spect, which holds the frames
+        [frame0, frame0 + T) of a sequence (t2_waveglow_infer_window).  Call ensure() first."""
+        B = int(spect.shape[0])
+        audio = torch.empty(B, HOP * (out1 - out0), device=self.device, dtype=spect.dtype)
+        w = _capi.T2WaveGlowWindowArgs()
+        w.wg = self._args(spect, len32, zt, sigma, seed, audio)
+        w.frame0, w.out0, w.out1, w.at_end = frame0, out0, out1, int(at_end)
+        w.z_frames = z_frames if zt is not None else 0
+        with torch.cuda.device(self.device):
+            _capi.check(_capi.lib().t2_waveglow_infer_window(
+                self.handle, C.byref(w), C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)))
+        return audio
+
+    @torch.no_grad()
+    def stream(self, module, items, sigma, z):
+        """The generator behind WaveGlow.infer_stream."""
+        left, right = window_halo()
+        kept = zt = z_frames = seed = None
+        base = held = a0 = 0           # kept: the final mel frames [base, held); audio of frames [0, a0) is handed out
+        for item in items:
+            f0, f1 = item["frames"]
+            post, finished = item["mel_outputs_postnet"], bool(item["finished"])
+            if f0 != held:
+                raise ValueError("WaveGlow.infer_stream: mel items must be consecutive (frames %s after %d)" % ((f0, f1), held))
+            if kept is None:           # the first item: weights, the noise seed (one draw, as infer)
+                self.ensure(module)
+                kept = self._spect(post, "WaveGlow.infer_stream")
+                B = int(kept.shape[0])
+                if z is not None:
+                    zt, z_frames = self._z(z, B, f1)
+                seed = self._draw_seed()
+            else:
+                kept = torch.cat((kept, post.to(kept.dtype)), 2)
+            held = f1
+            # audio of frame t is final once the mel frames up to t + right are (or the mel stream has ended)
+            a1 = held if finished else max(a0, held - right)
+            if a1 == a0 and not finished:
+                continue
+            lengths = item["mel_lengths"]
+            audio = kept.new_empty(B, 0)
+            if a1 > a0:
+                # the window is every kept frame: [max(0, a0 - left), held)
+                w0, w1 = base, held
+                # window-relative lengths on the device: live rows (-1) run past the window, stopped rows end inside it
+                # or after it
+                win_len = torch.where(lengths < 0, torch.full_like(lengths, w1 - w0),
+                                      (lengths - w0).clamp(min=0, max=w1 - w0)).to(torch.int32).contiguous()
+                audio = self.infer_window(kept.contiguous(), win_len, zt, z_frames, sigma, seed, w0, a0 - w0, a1 - w0,
+                                          finished)
+            yield dict(samples=(HOP * a0, HOP * a1), audio=audio, mel_lengths=lengths, finished=finished)
+            a0 = a1
+            if finished:
+                return
+            # later windows start at a0 - left: drop the frames before it, so the stream holds at most the two halos
+            # and one item's frames whatever max_decoder_steps is
+            drop = max(0, a0 - left) - base
+            kept, base = kept[:, :, drop:], base + drop
+
+
+def window_halo():
+    """(left, right): the mel frames before and after a frame that its WaveGlow audio depends on
+    (t2_waveglow_window_halo)."""
+    left, right = C.c_int32(), C.c_int32()
+    _capi.lib().t2_waveglow_window_halo(C.byref(left), C.byref(right))
+    return left.value, right.value
