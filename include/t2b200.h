@@ -433,6 +433,62 @@ typedef struct T2WaveGlowWindowArgs {
 void   t2_waveglow_window_halo(int32_t* left, int32_t* right);
 int    t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void* stream);
 
+/* ---- WaveGlow denoiser (waveglow/denoiser.py: Denoiser, over stft.py:69-136 and audio_processing.py:7-56) -------
+ * A separate handle holding the packed STFT bases.  The kernels are built for the reference default: filter_length
+ * 1024, hop 256, win_length 1024, periodic Hann window; t2_denoiser_create returns T2_ERR_UNSUPPORTED for anything
+ * else.  forward_basis and inverse_basis are the reference's windowed bases, fp32 (1026, 1, 1024) on the device.
+ * Arithmetic: split-fp16 operands with fp32 accumulation (fp32 grade); the reference denoises in fp32. */
+typedef struct T2Denoiser T2Denoiser;   /* opaque: packed device-side bases */
+#define T2_WINDOW_HANN 0
+typedef struct T2DenoiserConfig {
+  int32_t filter_length;               /* 1024 */
+  int32_t hop_length;                  /* 256  */
+  int32_t win_length;                  /* 1024 */
+  int32_t window;                      /* T2_WINDOW_HANN */
+} T2DenoiserConfig;
+int t2_denoiser_create(T2Denoiser** out, const T2DenoiserConfig* cfg, const float* forward_basis,
+                       const float* inverse_basis, void* stream);
+int t2_denoiser_refresh(T2Denoiser* h, const float* forward_basis, const float* inverse_basis, void* stream);
+int t2_denoiser_destroy(T2Denoiser* h);
+/* bias_spec (denoiser.py:36-38): bias_out (513) = the STFT magnitude of frame 0 of audio (n > 512 fp32 samples on the
+ * device, reflect-padded by 512). */
+int t2_denoiser_bias(T2Denoiser* h, const float* audio, int32_t n, float* bias_out, void* stream);
+
+/* Denoiser.forward (denoiser.py:40-45): audio (B, n), fp32 or (io_half) __half -> out (B, 256 floor(n / 256)) fp32:
+ * magnitudes lose strength * bias (513 fp32), clamped at 0, with the phase kept.  lengths (B) int32 in samples or NULL:
+ * row b is denoised as its first lengths[b] samples alone (reflect-padded at its own end), and its output from sample
+ * 256 floor(lengths[b] / 256) on is zero; a row of <= 512 samples cannot be padded and gives zeros.  Without lengths
+ * n must exceed 512.  Amplitude: the GEMM operands are split fp16 values, so every sample must stay below 65504 in
+ * magnitude (int16-scale audio up to 32767 is fine; any fp16 input is) and strength must be >= 0; larger values give
+ * inf or NaN.  out must be 16-byte aligned (T2_ERR_INVALID otherwise).  Workspace: t2_denoiser_workspace_bytes(h, B, n). */
+typedef struct T2DenoiserArgs {
+  const void* audio; int32_t B, n; const int32_t* lengths; int32_t io_half;
+  const float* bias; float strength;
+  float* out;
+  void* ws; size_t ws_bytes;
+} T2DenoiserArgs;
+size_t t2_denoiser_workspace_bytes(const T2Denoiser* h, int32_t B, int32_t n);
+int    t2_denoiser_run(T2Denoiser* h, const T2DenoiserArgs* a, void* stream);
+
+/* Windowed denoising: some output blocks of a longer sequence from a window of its audio, bit-identical to the same
+ * samples of t2_denoiser_run over the whole sequence.  dn.audio holds samples [s0, s0 + n) of the sequence, s0 a
+ * multiple of 256.  The output blocks [out0, out1), relative to the window (block k = samples 256 k ... 256 k + 255),
+ * are written to dn.out, (B, 256 (out1 - out0)).  dn.lengths are relative to the window: lengths[b] in [0, n] ends
+ * row b there; a negative or larger value (or NULL) ends it at the window's end when at_end, else the row goes on past
+ * the window.  An output block depends on the 3 blocks of audio before it and the 3 after it
+ * (t2_denoiser_window_halo: left, right).  The call returns T2_ERR_INVALID, launching nothing, when out0 is closer
+ * than the left halo to a window start that is not the sequence's start (s0 > 0), or out1 closer than the right halo
+ * to a window end that is not the sequence's end (at_end = 0).  Workspace: t2_denoiser_workspace_bytes(h, B, n).
+ * t2_denoiser_run is this call with s0 = 0, [out0, out1) = [0, n / 256) and at_end = 1. */
+typedef struct T2DenoiserWindowArgs {
+  T2DenoiserArgs dn;
+  int32_t s0;
+  int32_t out0, out1;
+  int32_t at_end;
+} T2DenoiserWindowArgs;
+void   t2_denoiser_window_halo(int32_t* left, int32_t* right);
+int    t2_denoiser_run_window(T2Denoiser* h, const T2DenoiserWindowArgs* a, void* stream);
+
 /* ---- self tests (libt2b200_selftest.so only: the same sources built with -DT2_SELFTEST; not part of the product
  * library) -------------------------------------------------------------------------------------------------
  * t2_selftest_umma: runs the wgmma split-fp16 GEMM engine used by the persistent decoder on a

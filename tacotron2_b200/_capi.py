@@ -27,6 +27,8 @@ EXPORTS = [
     "t2_decoder_stream_state_bytes", "t2_decoder_stream_begin", "t2_decoder_stream_run",
     "t2_waveglow_create", "t2_waveglow_refresh", "t2_waveglow_destroy", "t2_waveglow_workspace_bytes",
     "t2_waveglow_infer", "t2_waveglow_infer_window", "t2_waveglow_window_halo",
+    "t2_denoiser_create", "t2_denoiser_refresh", "t2_denoiser_destroy", "t2_denoiser_bias",
+    "t2_denoiser_workspace_bytes", "t2_denoiser_run", "t2_denoiser_run_window", "t2_denoiser_window_halo",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686
 
@@ -162,6 +164,21 @@ class T2WaveGlowWindowArgs(C.Structure):
                 ("z_frames", C.c_int32), ("at_end", C.c_int32)]
 
 
+class T2DenoiserConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("filter_length", "hop_length", "win_length", "window")]
+
+
+class T2DenoiserArgs(C.Structure):
+    _fields_ = [("audio", C.c_void_p), ("B", C.c_int32), ("n", C.c_int32), ("lengths", C.c_void_p),
+                ("io_half", C.c_int32), ("bias", C.c_void_p), ("strength", C.c_float), ("out", C.c_void_p),
+                ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
+class T2DenoiserWindowArgs(C.Structure):
+    _fields_ = [("dn", T2DenoiserArgs), ("s0", C.c_int32), ("out0", C.c_int32), ("out1", C.c_int32),
+                ("at_end", C.c_int32)]
+
+
 _lib = None
 
 
@@ -235,6 +252,17 @@ def lib():
     L.t2_waveglow_infer_window.argtypes = [C.c_void_p, C.POINTER(T2WaveGlowWindowArgs), C.c_void_p]
     L.t2_waveglow_window_halo.restype = None
     L.t2_waveglow_window_halo.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.t2_denoiser_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(T2DenoiserConfig), C.c_void_p, C.c_void_p,
+                                     C.c_void_p]
+    L.t2_denoiser_refresh.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.t2_denoiser_destroy.argtypes = [C.c_void_p]
+    L.t2_denoiser_bias.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    L.t2_denoiser_workspace_bytes.restype = C.c_size_t
+    L.t2_denoiser_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    L.t2_denoiser_run.argtypes = [C.c_void_p, C.POINTER(T2DenoiserArgs), C.c_void_p]
+    L.t2_denoiser_run_window.argtypes = [C.c_void_p, C.POINTER(T2DenoiserWindowArgs), C.c_void_p]
+    L.t2_denoiser_window_halo.restype = None
+    L.t2_denoiser_window_halo.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     if L.t2_abi_version() != 1:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L

@@ -10,6 +10,7 @@
 #include "gemm_f32.cuh"
 #include "train_layers.h"
 #include "waveglow.h"
+#include "denoiser.h"
 
 namespace t2 {
 
@@ -453,6 +454,29 @@ int t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void*
   return waveglow_infer_window(h, a, (cudaStream_t)stream);
 }
 void t2_waveglow_window_halo(int32_t* left, int32_t* right) { waveglow_window_halo(left, right); }
+
+// ---- WaveGlow denoiser (denoiser.cu) ----
+int t2_denoiser_create(T2Denoiser** out, const T2DenoiserConfig* cfg, const float* forward_basis,
+                       const float* inverse_basis, void* stream) {
+  return denoiser_create(out, cfg, forward_basis, inverse_basis, (cudaStream_t)stream);
+}
+int t2_denoiser_refresh(T2Denoiser* h, const float* forward_basis, const float* inverse_basis, void* stream) {
+  return denoiser_refresh(h, forward_basis, inverse_basis, (cudaStream_t)stream);
+}
+int t2_denoiser_destroy(T2Denoiser* h) { return denoiser_destroy(h); }
+int t2_denoiser_bias(T2Denoiser* h, const float* audio, int32_t n, float* bias_out, void* stream) {
+  return denoiser_bias(h, audio, n, bias_out, (cudaStream_t)stream);
+}
+size_t t2_denoiser_workspace_bytes(const T2Denoiser*, int32_t B, int32_t n) {
+  return B > 0 && n > 0 ? denoiser_ws_bytes(B, n) : 0;
+}
+int t2_denoiser_run(T2Denoiser* h, const T2DenoiserArgs* a, void* stream) {
+  return denoiser_run(h, a, (cudaStream_t)stream);
+}
+int t2_denoiser_run_window(T2Denoiser* h, const T2DenoiserWindowArgs* a, void* stream) {
+  return denoiser_run_window(h, a, (cudaStream_t)stream);
+}
+void t2_denoiser_window_halo(int32_t* left, int32_t* right) { denoiser_window_halo(left, right); }
 
 #ifdef T2_SELFTEST   // libt2b200_selftest.so only
 int t2_selftest_mma_rate(int32_t M, int32_t N, int32_t reps, int32_t alternate_d, int64_t* out_host) {

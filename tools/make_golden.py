@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz by executing the UNMODIFIED reference model.py (needs a checkout of
-NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live|waveglow]
+NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live|waveglow|denoiser]
 
 Every file holds the inputs' seeds, the reference outputs and a checksum of the synthetic weights
 (tests/common.synth_state_dict) so a drift of the generator is detected instead of silently
@@ -575,7 +575,75 @@ def waveglow_cases():
     waveglow_full_case("waveglow_full_b2_t800", 2, 800, 0.666, 7, 45, 46)
 
 
+def denoiser_case(seed=3, n=256 * 40 + 100, strengths=(0.01, 0.1, 3.0), n_samples=4096):
+    """The reference's own waveglow/denoiser.py on the CPU: bias_spec of the reference WaveGlow with
+    synth_state_dict(7) (fp32, mode 'zeros'), both bases, and the denoised seeded 2-row signal stft_inputs(seed, n) at
+    three strengths.  Shims: the librosa stand-ins of import_reference_stft plus normalize, the noise shim of
+    import_reference_glow (sigma = 0, so the draws are zeros), and .cuda() as a no-op while the fixture is made."""
+    import importlib.util
+    import types
+    from tests.waveglow_common import CONFIG, synth_state_dict
+
+    def pad_center(data, size, axis=-1, **kw):
+        n_ = data.shape[axis]
+        lpad = int((size - n_) // 2)
+        lengths = [(0, 0)] * data.ndim
+        lengths[axis] = (lpad, int(size - n_ - lpad))
+        return np.pad(data, lengths, mode="constant")
+
+    def normalize(S, norm=np.inf, **kw):       # audio_processing.py:48 calls it with norm=None: no normalisation
+        assert norm is None
+        return S
+    names = ("librosa", "librosa.util", "librosa.filters", "audio_processing", "stft", "layers")
+    saved = {k: sys.modules.get(k) for k in names}
+    lib, lu, lf = types.ModuleType("librosa"), types.ModuleType("librosa.util"), types.ModuleType("librosa.filters")
+    lu.pad_center, lu.tiny, lu.normalize, lf.mel = pad_center, (lambda x: np.finfo(np.float32).tiny), normalize, None
+    lib.util, lib.filters = lu, lf
+    sys.modules.update({"librosa": lib, "librosa.util": lu, "librosa.filters": lf})
+    for k in ("audio_processing", "stft", "layers"):
+        sys.modules.pop(k, None)
+    module_cuda, tensor_cuda = torch.nn.Module.cuda, torch.Tensor.cuda
+    torch.nn.Module.cuda = lambda self, *a, **kw: self
+    torch.Tensor.cuda = lambda self, *a, **kw: self
+    sys.path.insert(0, REFERENCE_DIR)
+    try:
+        spec = importlib.util.spec_from_file_location("t2_reference_denoiser",
+                                                      os.path.join(REFERENCE_DIR, "waveglow", "denoiser.py"))
+        mod = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(mod)
+        L = 88 * 32
+        glow = import_reference_glow([torch.zeros(1, 4, L), torch.zeros(1, 2, L), torch.zeros(1, 2, L)])
+        sd = synth_state_dict(7)
+        model = glow.WaveGlow(**CONFIG)
+        model.load_state_dict(sd)
+        den = mod.Denoiser(model)
+        y = stft_inputs(seed, n)
+        with torch.no_grad():
+            outs = {"out_%g" % s: den(y, strength=s) for s in strengths}
+        sdict = den.state_dict()
+    finally:
+        torch.nn.Module.cuda, torch.Tensor.cuda = module_cuda, tensor_cuda
+        sys.path.remove(REFERENCE_DIR)
+        for k, v in saved.items():
+            sys.modules.pop(k, None)
+            if v is not None:
+                sys.modules[k] = v
+    fb, ib = sdict["stft.forward_basis"], sdict["stft.inverse_basis"]
+    idx = sample_index(fb.numel(), n_samples, 7)
+    stats = lambda t: np.array([float(t.double().sum()), float(t.double().abs().sum()), float(t.double().abs().max())])  # noqa: E731
+    for s in strengths:
+        mag = den.stft.transform(y)[0]
+        print("strength %g: %.1f %% of the bins clamp to 0" % (s, 100.0 * float((mag - den.bias_spec * s <= 0).double().mean())))
+    save("denoiser_b2", seed=seed, n=n, strengths=np.array(strengths), wseed=7, checksum=weights_checksum(sd),
+         keys=np.array(list(sdict)), shapes=np.array([",".join(str(x) for x in sdict[k].shape) for k in sdict]),
+         bias_spec=sdict["bias_spec"], basis_idx=idx, forward_samples=fb.reshape(-1)[idx],
+         inverse_samples=ib.reshape(-1)[idx], forward_stats=stats(fb), inverse_stats=stats(ib), **outs)
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "denoiser":
+        denoiser_case()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "waveglow":
         waveglow_cases()
         sys.exit(0)
