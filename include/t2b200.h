@@ -15,6 +15,7 @@
  *       initialize_decoder_states             model.py:258-289        (inside: processed_memory GEMM)
  *     Postnet.forward (+ residual add)        model.py:141-146, 511, 524  -> t2_postnet_forward
  *     Tacotron2.inference, host buffers       model.py:517-529     -> t2_infer_host
+ *       ... over texts of different lengths                        -> t2_infer_host_lengths
  *
  * Conventions
  *   - plain C types only; every tensor argument is a raw pointer into DEVICE memory of the current
@@ -118,6 +119,12 @@ typedef struct T2EncoderArgs {
 } T2EncoderArgs;
 size_t t2_encoder_workspace_bytes(const T2Model* m, int32_t B, int32_t T);
 int    t2_encoder_forward(T2Model* m, const T2EncoderArgs* a, void* stream);
+/* Encoder.inference over a batch of texts of different lengths: row b is encoded exactly as its first lengths[b]
+ * symbols alone (a B = 1 call with T = lengths[b]), bit for bit.  lengths (B) int32, each in [1, T], in any order (not
+ * checked here: the caller validates them); NULL = every row T long, the same as t2_encoder_forward without lengths.
+ * Symbols at t >= lengths[b] are not read and memory there is zero.  Evaluation only: training must be 0 and stash
+ * NULL (T2_ERR_INVALID otherwise).  Workspace: t2_encoder_workspace_bytes(m, B, T). */
+int    t2_encoder_infer(T2Model* m, const T2EncoderArgs* a, void* stream);
 
 /* Encoder backward (autograd graph of Encoder.forward, model.py:173-190): the stash of a forward call with the same
  * text / embedded, lengths, training, keep and seed; d_memory (B, T, 512) -> gradients of the encoder parameters
@@ -152,6 +159,10 @@ int    t2_encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, void* stream);
  * Outputs (row-major): mel (B, T_cap, 80), gate (B, T_cap), align (B, T_cap, T_enc) where
  * T_cap = n_steps_cap; entries at t >= *n_steps are left untouched.  mel_lengths (B) int32,
  * n_steps (1) int32 on the device. */
+/* In INFER mode every reduction over encoder positions of row b -- the masked softmax, the location filter near the
+ * row's end, the context over staged and L2-resident memory rows -- runs in the order a call with T_enc =
+ * memory_lengths[b] uses, so a row of a ragged batch equals its own B = 1 call on memory[b, :memory_lengths[b]] bit
+ * for bit (persistent implementation; the stepwise one sums positions in a fixed order too). */
 typedef struct T2DecoderArgs {
   int32_t mode, impl, training;
   const float* memory; const int32_t* memory_lengths; int32_t B, T_enc, n_steps_cap;
@@ -173,11 +184,11 @@ int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);
  * keyed by the absolute step).  Everything that lives across a step boundary is kept in the caller's
  * `state` buffer (t2_decoder_stream_state_bytes), one block per 64-row slice: several streams can be
  * alive on one model at a time, and t2_decoder_run's workspace is not used.
- *   dec: as for t2_decoder_run with mode = INFER (memory_lengths, teacher_prenet, att_keep, dec_keep,
- *        ws and stash are not used).  mel / gate / align are the full n_steps_cap-sized buffers; each
- *        run writes its steps at their absolute indices.  mel_lengths[b] = -1 while row b is live,
- *        then its length, as t2_decoder_run.  T2_IMPL_STEPWISE and encoder lengths the persistent
- *        kernel does not take are refused with T2_ERR_UNSUPPORTED.
+ *   dec: as for t2_decoder_run with mode = INFER (teacher_prenet, att_keep, dec_keep, ws and stash are
+ *        not used; memory_lengths is, as by t2_decoder_run).  mel / gate / align are the full
+ *        n_steps_cap-sized buffers; each run writes its steps at their absolute indices.  mel_lengths[b] =
+ *        -1 while row b is live, then its length, as t2_decoder_run.  T2_IMPL_STEPWISE and encoder
+ *        lengths the persistent kernel does not take are refused with T2_ERR_UNSUPPORTED.
  *   status: device int32 (2 x ceil(B / 64)): [steps run, stopped] per slice, written by every run.
  * begin zeroes the state, sets mel_lengths to -1 and computes the processed memory; it does not
  * touch mel / gate / align (zero them first, as for t2_decoder_run).  run advances every slice that
@@ -253,6 +264,11 @@ typedef struct T2PostnetArgs {
 } T2PostnetArgs;
 size_t t2_postnet_workspace_bytes(const T2Model* m, int32_t B, int32_t T);
 int    t2_postnet_forward(T2Model* m, const T2PostnetArgs* a, void* stream);
+/* The postnet of a ragged inference batch: as t2_postnet_forward, but row b is computed exactly as its first lengths[b]
+ * frames alone (a B = 1 call with T = lengths[b]), bit for bit -- every hidden layer is zero at t >= lengths[b] too, the
+ * padding each convolution sees at that length, where t2_postnet_forward runs the hidden layers over the zero frames.
+ * lengths NULL: the same as t2_postnet_forward.  Evaluation only: training must be 0 and stash NULL. */
+int    t2_postnet_infer(T2Model* m, const T2PostnetArgs* a, void* stream);
 
 /* Postnet backward (model.py:141-146 + the residual of :511): d_mel_post (B, 80, T) -> d_mel (B, T, 80) (gradient wrt
  * the input rows, including the residual branch when add_residual) and the postnet parameter gradients. */
@@ -370,6 +386,27 @@ int    t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_
                      int32_t max_steps, float gate_threshold, uint64_t seed, int32_t impl,
                      float* mel_post_host, int32_t* mel_lengths_host, int32_t* n_steps_host,
                      void* ws, size_t ws_bytes, void* stream);
+
+/* t2_infer_host over texts of different lengths: input_lengths_host (B) int64 in (pinned) host memory, each in
+ * [1, T_text], any order.  Row b's outputs equal those of t2_infer_host on text_host[b, :input_lengths_host[b]] alone
+ * (B = 1, same seed and impl) bit for bit, up to that call's n_steps; the ids at t >= input_lengths_host[b] are
+ * ignored.  When every length is T_text the outputs are t2_infer_host's (an equal-length batch keeps its batched
+ * postnet, see t2_postnet_infer).  A length outside [1, T_text] or a NULL input_lengths_host is T2_ERR_INVALID before anything is enqueued.
+ * ws: device memory of t2_infer_lengths_workspace_bytes(). */
+typedef struct T2InferArgs {
+  const int64_t* text_host;            /* (B, T_text) */
+  const int64_t* input_lengths_host;   /* (B) */
+  int32_t B, T_text, max_steps;
+  float gate_threshold;
+  uint64_t seed;
+  int32_t impl;
+  float* mel_post_host;                /* out (B, 80, max_steps) */
+  int32_t* mel_lengths_host;           /* out (B) */
+  int32_t* n_steps_host;               /* out (1) */
+  void* ws; size_t ws_bytes;
+} T2InferArgs;
+size_t t2_infer_lengths_workspace_bytes(const T2Model* m, int32_t B, int32_t T_text, int32_t max_steps);
+int    t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream);
 
 /* ---- WaveGlow vocoder inference (waveglow/glow.py: WaveGlow.infer, glow.py:251-293) ---------------
  * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  The kernels are built for the

@@ -16,6 +16,7 @@ EXPORTS = [
     "t2_model_destroy", "t2_encoder_workspace_bytes", "t2_encoder_forward",
     "t2_decoder_workspace_bytes", "t2_decoder_run", "t2_prenet_forward",
     "t2_postnet_workspace_bytes", "t2_postnet_forward", "t2_infer_workspace_bytes", "t2_infer_host",
+    "t2_encoder_infer", "t2_postnet_infer", "t2_infer_lengths_workspace_bytes", "t2_infer_host_lengths",
     "t2_kernel_launch_count", "t2_decoder_profile",
     "t2_decoder_stash_bytes", "t2_decoder_backward_workspace_bytes", "t2_decoder_backward",
     "t2_prenet_backward_workspace_bytes", "t2_prenet_backward",
@@ -55,6 +56,13 @@ class T2EncoderBwdArgs(C.Structure):
                 ("training", C.c_int32), ("keep", C.c_void_p), ("seed", C.c_uint64),
                 ("stash", C.c_void_p), ("stash_bytes", C.c_size_t), ("d_memory", C.c_void_p), ("d_embedded", C.c_void_p),
                 ("grads", C.POINTER(C.c_void_p)), ("n_grads", C.c_int32), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
+class T2InferArgs(C.Structure):
+    _fields_ = [("text_host", C.c_void_p), ("input_lengths_host", C.c_void_p), ("B", C.c_int32), ("T_text", C.c_int32),
+                ("max_steps", C.c_int32), ("gate_threshold", C.c_float), ("seed", C.c_uint64), ("impl", C.c_int32),
+                ("mel_post_host", C.c_void_p), ("mel_lengths_host", C.c_void_p), ("n_steps_host", C.c_void_p),
+                ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
 
 
 class T2DecoderArgs(C.Structure):
@@ -205,17 +213,19 @@ def lib():
               "t2_encoder_backward_workspace_bytes", "t2_postnet_stash_bytes", "t2_postnet_backward_workspace_bytes"):
         getattr(L, n).restype = C.c_size_t
         getattr(L, n).argtypes = [C.c_void_p, C.c_int32, C.c_int32]
-    for n in ("t2_decoder_workspace_bytes", "t2_infer_workspace_bytes", "t2_decoder_stash_bytes",
-              "t2_decoder_backward_workspace_bytes"):
+    for n in ("t2_decoder_workspace_bytes", "t2_infer_workspace_bytes", "t2_infer_lengths_workspace_bytes",
+              "t2_decoder_stash_bytes", "t2_decoder_backward_workspace_bytes"):
         getattr(L, n).restype = C.c_size_t
         getattr(L, n).argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     L.t2_encoder_forward.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
+    L.t2_encoder_infer.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_decoder_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderArgs), C.c_void_p]
     L.t2_decoder_stream_state_bytes.restype = C.c_size_t
     L.t2_decoder_stream_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.t2_decoder_stream_begin.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_void_p]
     L.t2_decoder_stream_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_int32, C.c_void_p, C.c_void_p]
     L.t2_postnet_forward.argtypes = [C.c_void_p, C.POINTER(T2PostnetArgs), C.c_void_p]
+    L.t2_postnet_infer.argtypes = [C.c_void_p, C.POINTER(T2PostnetArgs), C.c_void_p]
     L.t2_clip_adam_workspace_bytes.restype = C.c_size_t
     L.t2_clip_adam_workspace_bytes.argtypes = [C.c_int64, C.c_int32]
     L.t2_clip_adam_step.argtypes = [C.POINTER(T2AdamArgs), C.c_void_p]
@@ -241,6 +251,7 @@ def lib():
     L.t2_infer_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                 C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_size_t, C.c_void_p]
+    L.t2_infer_host_lengths.argtypes = [C.c_void_p, C.POINTER(T2InferArgs), C.c_void_p]
     L.t2_decoder_profile.argtypes = [C.POINTER(T2DecoderArgs), C.POINTER(C.c_int64)]
     L.t2_waveglow_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(T2WaveGlowConfig), C.POINTER(C.c_void_p),
                                      C.c_int32, C.c_void_p]

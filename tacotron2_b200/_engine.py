@@ -202,7 +202,10 @@ class Engine:
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     # -- encoder ---------------------------------------------------------------------------------
-    def encoder(self, text=None, embedded=None, lengths=None, training=False, keep=None, stash=None, seed=None):
+    def encoder(self, text=None, embedded=None, lengths=None, training=False, keep=None, stash=None, seed=None,
+                per_row=False):
+        """per_row: t2_encoder_infer -- row b is encoded as its first lengths[b] positions alone (lengths in any order);
+        otherwise lengths has Encoder.forward's packed-sequence meaning (t2_encoder_forward)."""
         L = _capi.lib()
         src = text if text is not None else embedded
         B, T = int(src.shape[0]), int(src.shape[1])
@@ -227,7 +230,7 @@ class Engine:
         if stash is not None:
             a.stash, a.stash_bytes = stash.data_ptr(), stash.numel()
         with torch.cuda.device(self.device):
-            _capi.check(L.t2_encoder_forward(self.handle, C.byref(a), self._stream()))
+            _capi.check((L.t2_encoder_infer if per_row else L.t2_encoder_forward)(self.handle, C.byref(a), self._stream()))
         return memory
 
     def stash_buffer(self, kind, *dims):
@@ -339,10 +342,10 @@ class Engine:
         return mel, gate, align, mel_lengths, n_steps
 
     def decoder_stream(self, memory, n_steps_cap, prenet_keep=None, gate_threshold=0.5, score_mask_value=-float("inf"),
-                       impl=None, seed=None):
+                       impl=None, seed=None, memory_lengths=None):
         """Begins a resumable INFER run of the persistent decoder (t2_decoder_stream_begin); see DecoderStream."""
         return DecoderStream(self, memory, n_steps_cap, prenet_keep, gate_threshold, score_mask_value,
-                             self.impl if impl is None else impl, next_seed() if seed is None else seed)
+                             self.impl if impl is None else impl, next_seed() if seed is None else seed, memory_lengths)
 
     def decoder_profile(self):
         """Per-phase SM cycles of the last persistent decoder run: dict phase -> [cta0, cta60, cta100]."""
@@ -437,8 +440,10 @@ class Engine:
         return out
 
     # -- postnet ---------------------------------------------------------------------------------
-    def postnet(self, mel_btc, lengths=None, add_residual=True, training=False, keep=None, stash=None, seed=None):
-        """mel_btc: (B, T, 80) time-major rows (batch stride may exceed T*80).  Returns (B, 80, T)."""
+    def postnet(self, mel_btc, lengths=None, add_residual=True, training=False, keep=None, stash=None, seed=None,
+                per_row=False):
+        """mel_btc: (B, T, 80) time-major rows (batch stride may exceed T*80).  Returns (B, 80, T).  per_row
+        (t2_postnet_infer): row b is computed as its first lengths[b] frames alone."""
         L = _capi.lib()
         # a single frame (T = 1) may carry any time stride: torch calls such a tensor contiguous and keeps it as it is
         assert mel_btc.dtype == torch.float32 and mel_btc.stride(2) == 1 and (mel_btc.stride(1) == mel_btc.shape[2] or mel_btc.shape[1] == 1)
@@ -462,23 +467,36 @@ class Engine:
         if stash is not None:
             a.stash, a.stash_bytes = stash.data_ptr(), stash.numel()
         with torch.cuda.device(self.device):
-            _capi.check(L.t2_postnet_forward(self.handle, C.byref(a), self._stream()))
+            _capi.check((L.t2_postnet_infer if per_row else L.t2_postnet_forward)(self.handle, C.byref(a), self._stream()))
         return out
 
     # -- end to end with host buffers (bench e2e leg) ------------------------------------------------
-    def infer_host(self, text_host, max_steps, gate_threshold=0.5, impl=None, out_host=None, seed=None):
+    def infer_host(self, text_host, max_steps, gate_threshold=0.5, impl=None, out_host=None, seed=None, input_lengths_host=None):
         """text_host: pinned int64 (B, T).  Returns (mel_post_host (B,80,max_steps), lengths, n_steps).  seed: the
-        Philox seed of the decoder's prenet dropout (default: next_seed())."""
+        Philox seed of the decoder's prenet dropout (default: next_seed()).  input_lengths_host: pinned int64 (B) or None;
+        given, t2_infer_host_lengths runs each row as its first input_lengths_host[b] symbols alone."""
         L = _capi.lib()
         B, T = int(text_host.shape[0]), int(text_host.shape[1])
-        ws = self._workspace("e2e", L.t2_infer_workspace_bytes(self.handle, B, T, max_steps))
         if out_host is None:
             out_host = (torch.empty(B, self.hp.n_mel_channels, max_steps, dtype=torch.float32).pin_memory(),
                         torch.empty(B, dtype=torch.int32).pin_memory(), torch.empty(1, dtype=torch.int32).pin_memory())
         mel, lens, ns = out_host
+        seed = next_seed() if seed is None else seed
+        impl = self.impl if impl is None else impl
+        if input_lengths_host is not None:
+            ws = self._workspace("e2e", L.t2_infer_lengths_workspace_bytes(self.handle, B, T, max_steps))
+            a = _capi.T2InferArgs()
+            a.text_host, a.input_lengths_host = text_host.data_ptr(), input_lengths_host.data_ptr()
+            a.B, a.T_text, a.max_steps, a.gate_threshold, a.seed, a.impl = B, T, int(max_steps), float(gate_threshold), seed, impl
+            a.mel_post_host, a.mel_lengths_host, a.n_steps_host = mel.data_ptr(), lens.data_ptr(), ns.data_ptr()
+            a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
+            with torch.cuda.device(self.device):
+                _capi.check(L.t2_infer_host_lengths(self.handle, C.byref(a), self._stream()))
+            return mel, lens, ns
+        ws = self._workspace("e2e", L.t2_infer_workspace_bytes(self.handle, B, T, max_steps))
         with torch.cuda.device(self.device):
             _capi.check(L.t2_infer_host(self.handle, text_host.data_ptr(), B, T, int(max_steps), float(gate_threshold),
-                                        next_seed() if seed is None else seed, self.impl if impl is None else impl, mel.data_ptr(),
+                                        seed, impl, mel.data_ptr(),
                                         lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
         return mel, lens, ns
 
@@ -488,7 +506,7 @@ class DecoderStream:
     mel_lengths (B,) with -1 for live rows) and the per-stream state buffer that carries everything across a chunk
     boundary.  ``run(n)`` advances every live 64-row slice by up to n steps and takes the one host sync of the chunk."""
 
-    def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed):
+    def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed, memory_lengths=None):
         L = _capi.lib()
         dev = eng.device
         self.eng = eng
@@ -506,10 +524,12 @@ class DecoderStream:
         self.status_host = None                      # the caller's copy of `status` after the last run
         self.state = torch.empty(int(L.t2_decoder_stream_state_bytes(eng.handle, B, T)), dtype=torch.uint8, device=dev)
         self.keep = _u8(prenet_keep, dev)
+        self.len32 = None if memory_lengths is None else memory_lengths.to(device=dev, dtype=torch.int32).contiguous()
         a = _capi.T2DecoderStreamArgs()
         d = a.dec
         d.mode, d.impl, d.training = _capi.MODE_INFER, impl, 0
         d.memory, d.B, d.T_enc, d.n_steps_cap = self.memory.data_ptr(), B, T, self.cap
+        d.memory_lengths = self.len32.data_ptr() if self.len32 is not None else None
         d.prenet_keep = self.keep.data_ptr() if self.keep is not None else None
         d.seed = seed
         d.gate_threshold, d.score_mask_value = float(gate_threshold), float(score_mask_value)

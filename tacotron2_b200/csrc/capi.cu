@@ -30,9 +30,9 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
-int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s);
+int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per_row);
 size_t encoder_ws_bytes(int B, int T);
-int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s);
+int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s, bool per_row);
 size_t postnet_ws_bytes(int B, int T);
 int selftest_umma(const float* A, const float* W, int N, int K, int passes, float* C, cudaStream_t s);
 int selftest_event(const float* A, const float* W, const int* cons, int ncons, int K, float* C, cudaStream_t s);
@@ -244,7 +244,13 @@ int t2_model_destroy(T2Model* m) {
 size_t t2_encoder_workspace_bytes(const T2Model*, int32_t B, int32_t T) { return encoder_ws_bytes(B, T); }
 int t2_encoder_forward(T2Model* m, const T2EncoderArgs* a, void* stream) {
   if (!m || !a || (!a->text && !a->embedded) || !a->memory || !a->ws) return fail(T2_ERR_INVALID, "encoder: null argument");
-  return encoder_forward(m, a, (cudaStream_t)stream);
+  return encoder_forward(m, a, (cudaStream_t)stream, false);
+}
+
+int t2_encoder_infer(T2Model* m, const T2EncoderArgs* a, void* stream) {
+  if (!m || !a || (!a->text && !a->embedded) || !a->memory || !a->ws) return fail(T2_ERR_INVALID, "encoder infer: null argument");
+  if (a->training || a->stash) return fail(T2_ERR_INVALID, "encoder infer: evaluation only (training = 0, no stash)");
+  return encoder_forward(m, a, (cudaStream_t)stream, true);
 }
 
 size_t t2_encoder_stash_bytes(const T2Model*, int32_t B, int32_t T) { return encoder_stash_bytes(B, T); }
@@ -353,15 +359,22 @@ size_t t2_postnet_workspace_bytes(const T2Model*, int32_t B, int32_t T) { return
 int t2_postnet_forward(T2Model* m, const T2PostnetArgs* a, void* stream) {
   if (!m || !a || !a->mel || !a->mel_post || !a->ws) return fail(T2_ERR_INVALID, "postnet: null argument");
   if (a->stash) return postnet_forward_train(m, a, (cudaStream_t)stream);
-  return postnet_forward(m, a, (cudaStream_t)stream);
+  return postnet_forward(m, a, (cudaStream_t)stream, false);
+}
+
+int t2_postnet_infer(T2Model* m, const T2PostnetArgs* a, void* stream) {
+  if (!m || !a || !a->mel || !a->mel_post || !a->ws) return fail(T2_ERR_INVALID, "postnet infer: null argument");
+  if (a->training || a->stash) return fail(T2_ERR_INVALID, "postnet infer: evaluation only (training = 0, no stash)");
+  return postnet_forward(m, a, (cudaStream_t)stream, true);
 }
 
 // ---- end to end with host buffers ------------------------------------------------------------------
 struct InferWs {
   int64_t* text; float *memory, *mel, *gate, *align, *post; int32_t *lens, *nsteps;
   char* sub; size_t sub_bytes;   // the workspace of the encoder, the decoder and the postnet in turn
+  int32_t* in_lens;              // t2_infer_host_lengths: the input lengths (B)
 };
-static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w) {
+static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w, bool with_lengths = false) {
   w->text = c.take<int64_t>((size_t)B * Tt);
   w->memory = c.take<float>((size_t)B * Tt * kEnc);
   w->mel = c.take<float>((size_t)B * S * kMel);
@@ -374,6 +387,7 @@ static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w) {
   if (decoder_ws_bytes(B, Tt, S) > sb) sb = decoder_ws_bytes(B, Tt, S);
   if (postnet_ws_bytes(B, S) > sb) sb = postnet_ws_bytes(B, S);
   w->sub = c.take<char>(sb); w->sub_bytes = sb;
+  w->in_lens = with_lengths ? c.take<int32_t>(B) : nullptr;
 }
 
 size_t t2_infer_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32_t max_steps) {
@@ -383,22 +397,46 @@ size_t t2_infer_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32
   return c.bytes();
 }
 
-int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_text, int32_t max_steps,
-                  float gate_threshold, uint64_t seed, int32_t impl, float* mel_post_host,
-                  int32_t* mel_lengths_host, int32_t* n_steps_host, void* ws, size_t ws_bytes, void* stream) {
+size_t t2_infer_lengths_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32_t max_steps) {
+  Carve c(nullptr);
+  InferWs w;
+  infer_layout(c, B, T_text, max_steps, &w, true);
+  return c.bytes();
+}
+
+// Tacotron2.inference end to end; in_lens_host (B) or null: each row b is its first in_lens_host[b] symbols alone
+static int infer_host(T2Model* m, const int64_t* text_host, const int64_t* in_lens_host, int32_t B, int32_t T_text,
+                      int32_t max_steps, float gate_threshold, uint64_t seed, int32_t impl, float* mel_post_host,
+                      int32_t* mel_lengths_host, int32_t* n_steps_host, void* ws, size_t ws_bytes, cudaStream_t s) {
   if (!m || !text_host || !mel_post_host || !mel_lengths_host || !n_steps_host || !ws)
     return fail(T2_ERR_INVALID, "infer_host: null argument");
-  if (ws_bytes < t2_infer_workspace_bytes(m, B, T_text, max_steps)) return fail(T2_ERR_WORKSPACE, "infer workspace too small");
-  cudaStream_t s = (cudaStream_t)stream;
+  const bool with_lengths = in_lens_host != nullptr;
+  const size_t need = with_lengths ? t2_infer_lengths_workspace_bytes(m, B, T_text, max_steps)
+                                   : t2_infer_workspace_bytes(m, B, T_text, max_steps);
+  if (ws_bytes < need) return fail(T2_ERR_WORKSPACE, "infer workspace too small");
+  std::vector<int32_t> lens32;
+  bool ragged = false;             // some text shorter than T_text: each row's postnet is its own B = 1 postnet
+  if (with_lengths) {              // checked here, before anything is enqueued
+    lens32.resize(B > 0 ? B : 0);
+    for (int b = 0; b < B; ++b) {
+      if (in_lens_host[b] < 1 || in_lens_host[b] > T_text)
+        return fail(T2_ERR_INVALID, "infer_host: input_lengths[%d] = %lld outside [1, %d]", b, (long long)in_lens_host[b], T_text);
+      lens32[b] = (int32_t)in_lens_host[b];
+      ragged |= lens32[b] < T_text;
+    }
+  }
   Carve c(ws);
   InferWs w;
-  infer_layout(c, B, T_text, max_steps, &w);
+  infer_layout(c, B, T_text, max_steps, &w, with_lengths);
   T2_CUDA(cudaMemcpyAsync(w.text, text_host, (size_t)B * T_text * 8, cudaMemcpyHostToDevice, s));
+  // pageable source: the call returns once lens32 has been staged, so the vector may go out of scope
+  if (with_lengths) T2_CUDA(cudaMemcpyAsync(w.in_lens, lens32.data(), (size_t)B * 4, cudaMemcpyHostToDevice, s));
   T2EncoderArgs ea; memset(&ea, 0, sizeof(ea));
-  ea.text = w.text; ea.B = B; ea.T = T_text; ea.memory = w.memory; ea.ws = w.sub; ea.ws_bytes = w.sub_bytes;
-  T2_TRY(encoder_forward(m, &ea, s));
+  ea.text = w.text; ea.lengths = w.in_lens; ea.B = B; ea.T = T_text; ea.memory = w.memory; ea.ws = w.sub; ea.ws_bytes = w.sub_bytes;
+  T2_TRY(encoder_forward(m, &ea, s, true));
   T2DecoderArgs da; memset(&da, 0, sizeof(da));
-  da.mode = T2_MODE_INFER; da.impl = impl; da.memory = w.memory; da.B = B; da.T_enc = T_text; da.n_steps_cap = max_steps;
+  da.mode = T2_MODE_INFER; da.impl = impl; da.memory = w.memory; da.memory_lengths = w.in_lens;
+  da.B = B; da.T_enc = T_text; da.n_steps_cap = max_steps;
   da.seed = seed; da.gate_threshold = gate_threshold; da.score_mask_value = -INFINITY;
   da.mel = w.mel; da.gate = w.gate; da.align = w.align; da.mel_lengths = w.lens; da.n_steps = w.nsteps; da.ws = w.sub; da.ws_bytes = w.sub_bytes;
   T2_TRY(t2_decoder_run(m, &da, s));
@@ -412,7 +450,7 @@ int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_tex
   T2PostnetArgs pa; memset(&pa, 0, sizeof(pa));
   pa.mel = w.mel; pa.mel_batch_stride = (long)max_steps * kMel; pa.lengths = w.lens; pa.add_residual = 1; pa.B = B; pa.T = n;
   pa.mel_post = w.post; pa.ws = w.sub; pa.ws_bytes = w.sub_bytes;
-  T2_TRY(postnet_forward(m, &pa, s));
+  T2_TRY(postnet_forward(m, &pa, s, ragged));
   T2_CUDA(cudaMemcpy2DAsync(mel_post_host, (size_t)max_steps * 4, w.post, (size_t)n * 4, (size_t)n * 4, (size_t)B * kMel,
                             cudaMemcpyDeviceToHost, s));
   if (n < max_steps) {   // frames past the last step: zeros
@@ -424,6 +462,20 @@ int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_tex
   T2_CUDA(cudaMemcpyAsync(mel_lengths_host, w.lens, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
   T2_CUDA(cudaStreamSynchronize(s));
   return T2_OK;
+}
+
+int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_text, int32_t max_steps,
+                  float gate_threshold, uint64_t seed, int32_t impl, float* mel_post_host,
+                  int32_t* mel_lengths_host, int32_t* n_steps_host, void* ws, size_t ws_bytes, void* stream) {
+  return infer_host(m, text_host, nullptr, B, T_text, max_steps, gate_threshold, seed, impl, mel_post_host, mel_lengths_host,
+                    n_steps_host, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+int t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream) {
+  if (!a) return fail(T2_ERR_INVALID, "infer_host_lengths: null args");
+  if (!a->input_lengths_host) return fail(T2_ERR_INVALID, "infer_host_lengths: null input_lengths_host (use t2_infer_host)");
+  return infer_host(m, a->text_host, a->input_lengths_host, a->B, a->T_text, a->max_steps, a->gate_threshold, a->seed, a->impl,
+                    a->mel_post_host, a->mel_lengths_host, a->n_steps_host, a->ws, a->ws_bytes, (cudaStream_t)stream);
 }
 
 int t2_decoder_profile(const T2DecoderArgs* a, int64_t* out_host) {

@@ -161,6 +161,8 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
     const int span = p.T + p.seq_pad;
     const int b = (int)(prow / span), pt = (int)(prow - (long)b * span) - p.seq_pad / 2;
     const bool valid = tile_live && b < p.B && pt >= 0 && pt < p.T;
+    // planes output: frames t >= row_len[b] are written as zeros, the padding a sequence of that length has alone
+    const bool in_len = valid && (p.out_mode != 0 || p.row_len == nullptr || pt < p.row_len[b]);
     const int n0 = nt * NT * NH;
     if (tile_live) {
       for (int c0 = chalf * 8; c0 < NT * NH; c0 += 16) {
@@ -175,7 +177,7 @@ __global__ void __launch_bounds__(kThreadsC, 1) conv_tc_kernel(const ConvParams 
           float x = v[i] * p.scale[n] + p.shift[n];
           if (p.act == 1) x = fmaxf(x, 0.f);
           else if (p.act == 2) x = tanhf(x);
-          v[i] = valid ? x : 0.f;
+          v[i] = in_len ? x : 0.f;
         }
         if (p.out_mode == 0) {          // next layer's planes (zeros in the padding rows)
           __align__(16) __half hh[8];
@@ -255,9 +257,10 @@ __global__ void rows_to_planes_kernel(const float* __restrict__ x, long batch_st
   *reinterpret_cast<uint4*>(dst + plane_rows * 8) = *reinterpret_cast<const uint4*>(ll);
 }
 
-// embedding gather straight into planes (model.py:503 / 518)
+// embedding gather straight into planes (model.py:503 / 518); symbols at t >= len[b] are not read, their rows are zero
 __global__ void embed_to_planes_kernel(const int64_t* __restrict__ text, const float* __restrict__ emb, int n_symbols,
-                                       int B, int T, __half* __restrict__ planes, long plane_rows) {
+                                       const int32_t* __restrict__ len, int B, int T, __half* __restrict__ planes,
+                                       long plane_rows) {
   const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int g = blockIdx.y;
   if (row >= plane_rows) return;
@@ -265,7 +268,7 @@ __global__ void embed_to_planes_kernel(const int64_t* __restrict__ text, const f
   const int span = T + 4;
   int b = -1, t = -1;
   if (prow >= 0) { b = (int)(prow / span); t = (int)(prow - (long)b * span) - 2; }
-  const bool valid = b >= 0 && b < B && t >= 0 && t < T;
+  const bool valid = b >= 0 && b < B && t >= 0 && t < T && (len == nullptr || t < len[b]);
   __align__(16) __half hh[8];
   __align__(16) __half ll[8];
   long id = 0;
@@ -358,10 +361,11 @@ int tc_rows_to_planes(const float* x, long batch_stride, int C, int c_pad, const
   return tc_rows_to_planes_scaled(x, batch_stride, C, c_pad, len, B, T, planes, nullptr, s);
 }
 
-int tc_embed_to_planes(const int64_t* text, const float* emb, int n_symbols, int B, int T, __half* planes,
-                       cudaStream_t s) {
+int tc_embed_to_planes(const int64_t* text, const float* emb, int n_symbols, const int32_t* len, int B, int T,
+                       __half* planes, cudaStream_t s) {
   const long rows = tc_plane_rows(B, T);
-  embed_to_planes_kernel<<<dim3((unsigned)((rows + 127) / 128), kEnc / 8), 128, 0, s>>>(text, emb, n_symbols, B, T, planes, rows);
+  embed_to_planes_kernel<<<dim3((unsigned)((rows + 127) / 128), kEnc / 8), 128, 0, s>>>(text, emb, n_symbols, len, B, T,
+                                                                                       planes, rows);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }

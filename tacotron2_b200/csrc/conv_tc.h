@@ -17,7 +17,8 @@ struct TcConvArgs {
   __half* out_planes;
   float* out_f32; long ldo;
   int out_seq_rows;                       // out_mode 1: output row of (b, t) = b * out_seq_rows + t (0 = T)
-  const float* residual; long res_batch_stride; const int32_t* row_len;
+  const float* residual; long res_batch_stride;
+  const int32_t* row_len;                 // (B) or null: out_mode 0 writes zero rows and out_mode 2 zeros at t >= row_len[b]
 };
 
 long tc_plane_rows(int B, int T);
@@ -27,8 +28,8 @@ int tc_rows_to_planes(const float* x, long batch_stride, int C, int c_pad, const
                       __half* planes, cudaStream_t s);
 int tc_rows_to_planes_scaled(const float* x, long batch_stride, int C, int c_pad, const int32_t* len, int B, int T,
                              __half* planes, const float* in_scale /* device scalar or null */, cudaStream_t s);
-int tc_embed_to_planes(const int64_t* text, const float* emb, int n_symbols, int B, int T, __half* planes,
-                       cudaStream_t s);
+int tc_embed_to_planes(const int64_t* text, const float* emb, int n_symbols, const int32_t* len /* or null */, int B,
+                       int T, __half* planes, cudaStream_t s);
 int tc_fold_bn(const float* cbias, const float* g, const float* b, const float* mean, const float* var, float eps,
                float* scale, float* shift, int C, cudaStream_t s);
 int tc_conv(const TcConvArgs& a, cudaStream_t s);

@@ -581,6 +581,7 @@ struct KParams {
   DecoderCtrl* ctrl;
   int B, T, cap, infer, training;
   int nstages;                      // operand ring stages (4, or 3 when T_enc > 896)
+  int t4max;                        // longest T_enc that runs with 4 stages (0: every T_enc runs with 3)
   int b0, Btot;                     // this launch handles batch rows [b0, b0 + B) of Btot (dropout mask / Philox indexing)
   float gate_threshold, score_mask_value, p_att, p_dec;
   uint64_t seed;
@@ -594,6 +595,14 @@ struct KParams {
   int32_t* rs_done;                 // (kRows) stop latch
   int32_t* rs_status;               // out: [steps run, stopped]
 };
+
+// encoder-memory rows of a T_enc-long row that the attention phase stages in an idle ring of `nstages` stages; the rest
+// is read from L2.  The same on the host and the device: the context of a row sums its positions in the grouping a
+// launch sized for that row's own length stages (see the context below).
+__host__ __device__ constexpr int staged_rows(int T, int nstages) {
+  return T < (nstages * kStageBytes - 2 * kAttPlane - kPaBytes) / (kEnc / 2 * 4)
+             ? T : (nstages * kStageBytes - 2 * kAttPlane - kPaBytes) / (kEnc / 2 * 4);
+}
 
 __device__ __forceinline__ void store_split2(uint8_t* img, int row, int k, float v0, float v1) {
   // two adjacent K elements (k even) of an activation image: 4-byte stores into the hi and lo planes
@@ -812,7 +821,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     const int att_rounds = (T + kAttRound - 1) / kAttRound;
     const int img_bytes = 2 * kAttPlane;
     float* s_pa = reinterpret_cast<float*>(aimg + img_bytes);                       // [128 dims][kPaPitch] fp32
-    const int smem_rows = min(T, (p.nstages * kStageBytes - img_bytes - kPaBytes) / (kEnc / 2 * 4));   // memory rows staged in the ring
+    const int smem_rows = staged_rows(T, p.nstages);                        // memory rows staged in the ring
     // pa^T = Weff . A^T on the tensor cores (fused model.py:23-25), i.e. the fused filter bank is the M = 128 operand
     // (attention dim d; warpgroups 0 / 1 take dims 0-63 / 64-127) and kAttRound positions are the N dimension.  The
     // tile goes to shared memory, where every warp then owns a slice of POSITIONS of all 128 dims, so the tanh of a
@@ -956,7 +965,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       }
       // mask + softmax (model.py:79-82): every warp reduces all T energies itself (shuffles only, no
       // cross-warp exchange), then the threads split the normalised write-out
-      const int len = p.mem_len ? p.mem_len[b] : T;
+      const int len = p.mem_len ? min(p.mem_len[b], T) : T;
       const int eN = ntiles * 128;
       // masked energies once (the four 32-dim partial sums added in a fixed order), in place in the first partial-sum plane
       for (int j = tid; j < T; j += kThreads)
@@ -980,17 +989,30 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       __syncthreads();
       T2_PROF(18);
       {                                                           // context = aw . memory  model.py:83-84
+        // j-group jg sums positions jg, jg + 8, ... below `split`, then split + jg, split + jg + 8, ... below `clen`.
+        // INFER: clen = len and split = the rows a launch sized for T_enc = len stages, so the grouping is a function of
+        // the row's own length, not of the launch's T_enc, and a row of a ragged batch gets the bits it gets alone
+        // (positions >= len have weight 0 and are skipped).  Without lengths, len = T_enc and split = smem_rows.
+        // TEACHER keeps the launch's grouping over all T_enc positions.
         const int c4 = tid & 63, jg = tid >> 6;                   // 64 float4 = this CTA's 256 columns; 8 j-groups
         const float4* ms = reinterpret_cast<const float4*>(rg.stage0 + img_bytes + kPaBytes);
+        const float* mp = p.memory + (long)b * T * kEnc + ahalf * (kEnc / 2) + c4 * 4;
+        const int clen = p.infer ? len : T;
+        const int split = p.infer ? staged_rows(len, len <= p.t4max ? 4 : 3) : smem_rows;   // >= smem_rows if clen > smem_rows
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        int j = jg;
 #pragma unroll 4
-        for (int j = jg; j < smem_rows; j += 8) {
+        for (; j < min(split, smem_rows); j += 8) {
           const float4 m = ms[j * 64 + c4];
           const float a = s_e[j];
           acc.x = fmaf(a, m.x, acc.x); acc.y = fmaf(a, m.y, acc.y); acc.z = fmaf(a, m.z, acc.z); acc.w = fmaf(a, m.w, acc.w);
         }
-        const float* mp = p.memory + (long)b * T * kEnc + ahalf * (kEnc / 2) + c4 * 4;
-        for (int j = smem_rows + jg; j < T; j += 8) {             // rows that did not fit in the ring
+        for (; j < split; j += 8) {                               // staged for a launch of this length, not for this one
+          const float4 m = __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc));
+          const float a = s_e[j];
+          acc.x = fmaf(a, m.x, acc.x); acc.y = fmaf(a, m.y, acc.y); acc.z = fmaf(a, m.z, acc.z); acc.w = fmaf(a, m.w, acc.w);
+        }
+        for (j = split + jg; j < clen; j += 8) {                  // rows that did not fit in the ring
           const float4 m = __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc));
           const float a = s_e[j];
           acc.x = fmaf(a, m.x, acc.x); acc.y = fmaf(a, m.y, acc.y); acc.z = fmaf(a, m.z, acc.z); acc.w = fmaf(a, m.w, acc.w);
@@ -1332,8 +1354,20 @@ static void carve_images(uint8_t* img, KParams* p) {
   p->q = (float*)img;
 }
 
+// the longest T_enc that persistent_stages() runs with 4 stages (0 when none does); stages fall as T_enc grows
+static int persistent_t4max() {
+  if (persistent_stages(1) < 4) return 0;
+  int lo = 1, hi = 1 << 16;                 // persistent_stages(lo) == 4, persistent_stages(hi) == 3
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) / 2;
+    if (persistent_stages(mid) == 4) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 static int launch_persistent(KParams& p, cudaStream_t s) {
   p.nstages = persistent_stages(p.T);
+  p.t4max = persistent_t4max();
   const size_t smem = persistent_smem_bytes(p.T, p.nstages);
   T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchConfig_t cfg;

@@ -94,6 +94,15 @@ __global__ void mask_rows_kernel(const float* __restrict__ in, long in_batch_str
   out[i] = (len == nullptr || t < len[b]) ? in[(long)b * in_batch_stride + (long)t * C + c] : 0.f;
 }
 
+// frames t >= len[b] of channels-last rows (B, T, C) set to zero, in place
+__global__ void zero_past_len_kernel(float* x, const int32_t* __restrict__ len, int B, int T, int C) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)B * T * C) return;
+  const long row = i / C;
+  const int b = (int)(row / T), t = (int)(row % T);
+  if (t >= len[b]) x[i] = 0.f;
+}
+
 // (B*T, C) channels-last -> (B, C, T) with optional residual and length mask (training-mode tail of
 // the postnet; the eval path fuses this into the last conv's epilogue)
 __global__ void transpose_residual_kernel(const float* __restrict__ y, const float* __restrict__ R,
@@ -330,7 +339,11 @@ static int conv_bn_layer(T2Model* m, const float* x, float* y, int B, int T, int
   return T2_OK;
 }
 
-int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
+// per_row (t2_encoder_infer): each row b is encoded as its first lengths[b] symbols alone -- the inputs at t >= lengths[b]
+// and every conv layer's outputs there are zero, the padding the row has at T = lengths[b].  Otherwise lengths only
+// masks the BiLSTM (pack_padded_sequence, model.py:180-188) and the convolutions see the padded inputs as the
+// reference's do.
+int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per_row) {
   const int B = a->B, T = a->T;
   if (B <= 0 || T <= 0) return fail(T2_ERR_INVALID, "encoder: empty batch");
   if (a->ws_bytes < encoder_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder workspace too small");
@@ -339,6 +352,7 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
   encoder_ws_layout(cv, B, T, &w);
   const bool tc = use_tc() && !a->training && !a->stash;
   float* st_gates = nullptr; float* st_c = nullptr;
+  const int32_t* conv_len = per_row ? a->lengths : nullptr;
 
   if (a->stash) {
     // autograd path: fp32 conv stack with the activations kept for the backward pass (train_layers.cu)
@@ -350,15 +364,15 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
     T2_TRY(gemm_f32(g, s));
   } else if (tc) {
     // tensor-core path: planes -> 3 x (conv k5 + folded BN + ReLU) -> LSTM input projection (fp32 rows)
-    if (a->embedded) T2_TRY(tc_rows_to_planes(a->embedded, (long)T * kEnc, kEnc, kEnc, nullptr, B, T, w.pl0, s));
-    else T2_TRY(tc_embed_to_planes(a->text, m->w[W_EMB], m->cfg.n_symbols, B, T, w.pl0, s));
+    if (a->embedded) T2_TRY(tc_rows_to_planes(a->embedded, (long)T * kEnc, kEnc, kEnc, conv_len, B, T, w.pl0, s));
+    else T2_TRY(tc_embed_to_planes(a->text, m->w[W_EMB], m->cfg.n_symbols, conv_len, B, T, w.pl0, s));
     __half* cur = w.pl0; __half* nxt = w.pl1;
     for (int i = 0; i < 3; ++i) {                                                           // model.py:174-175, 194
       const int wb = W_ENC_CONV0 + 7 * i;
       T2_TRY(tc_fold_bn(m->w[wb + 1], m->w[wb + 2], m->w[wb + 3], m->w[wb + 4], m->w[wb + 5], m->cfg.bn_eps, w.scale, w.shift, kEnc, s));
       TcConvArgs c; memset(&c, 0, sizeof(c));
       c.in = cur; c.cin_pad = kEnc; c.wimg = m->tc_enc_conv[i]; c.taps = kConvK; c.B = B; c.T = T; c.cout = kEnc; c.nt_rows = 128;
-      c.scale = w.scale; c.shift = w.shift; c.act = 1; c.out_mode = 0; c.out_planes = nxt;
+      c.scale = w.scale; c.shift = w.shift; c.act = 1; c.out_mode = 0; c.out_planes = nxt; c.row_len = conv_len;
       T2_TRY(tc_conv(c, s));
       __half* tmp = cur; cur = nxt; nxt = tmp;
     }
@@ -374,11 +388,20 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s) {
       embed_kernel<<<B * T, 128, 0, s>>>(a->text, m->w[W_EMB], w.x0, B * T, m->cfg.n_symbols);   // model.py:503/518
       T2_LAUNCH_CHECK();
     }
+    const long n_rows = (long)B * T * kEnc;
+    auto zero_padding = [&](float* x) -> int {      // per_row: frames t >= lengths[b] of x become zero (in place)
+      if (!conv_len) return T2_OK;
+      zero_past_len_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, s>>>(x, conv_len, B, T, kEnc);
+      T2_LAUNCH_CHECK();
+      return T2_OK;
+    };
+    T2_TRY(zero_padding(w.x0));
     float* cur = w.x0; float* nxt = w.x1;
     for (int i = 0; i < 3; ++i) {                                                             // model.py:174-175
       const uint8_t* keep = (a->training && a->keep) ? a->keep + (size_t)i * B * kEnc * T : nullptr;
       T2_TRY(conv_bn_layer(m, cur, nxt, B, T, kEnc, kEnc, m->enc_conv_w[i], W_ENC_CONV0 + 7 * i, ACT_RELU,
                            a->training, keep, a->seed, 1000 + i, w.scale, w.shift, 0, nullptr, nullptr, s));
+      T2_TRY(zero_padding(nxt));
       float* tmp = cur; cur = nxt; nxt = tmp;
     }
     {  // W_ih x + b_ih + b_hh for every time step and both directions
@@ -434,8 +457,12 @@ static void postnet_ws_layout(Carve& c, int B, int T, PostnetWs* w) {
 }
 size_t postnet_ws_bytes(int B, int T) { Carve c(nullptr); PostnetWs w; postnet_ws_layout(c, B, T, &w); return c.bytes(); }
 
-int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
+// per_row (t2_postnet_infer): every layer's output at t >= lengths[b] is zero too, so row b gets the zero padding each
+// convolution sees when the row is its first lengths[b] frames alone.  Otherwise only the input and the output are
+// masked and the hidden layers run over the zero frames.
+int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s, bool per_row) {
   const int B = a->B, T = a->T;
+  const int32_t* layer_len = per_row ? a->lengths : nullptr;
   if (B <= 0 || T <= 0) return fail(T2_ERR_INVALID, "postnet: empty batch");
   if (a->ws_bytes < postnet_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet workspace too small");
   Carve cv(a->ws);
@@ -453,7 +480,7 @@ int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
       TcConvArgs c; memset(&c, 0, sizeof(c));
       c.in = cur; c.cin_pad = i == 0 ? 128 : kPost; c.wimg = m->tc_post_conv[i]; c.taps = kConvK; c.B = B; c.T = T;
       c.cout = cout; c.nt_rows = i == 4 ? 80 : 128; c.scale = w.scale; c.shift = w.shift; c.act = i == 4 ? 0 : 2;
-      if (i < 4) { c.out_mode = 0; c.out_planes = nxt; }
+      if (i < 4) { c.out_mode = 0; c.out_planes = nxt; c.row_len = layer_len; }
       else { c.out_mode = 2; c.out_f32 = a->mel_post; c.residual = a->add_residual ? a->mel : nullptr; c.res_batch_stride = bs; c.row_len = a->lengths; }
       T2_TRY(tc_conv(c, s));
       __half* tmp = cur; cur = nxt; nxt = tmp;
@@ -477,6 +504,11 @@ int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
       T2_TRY(conv_bn_layer(m, cur, nxt, B, T, cin, cout, m->post_conv_w[i], W_POST_CONV0 + 7 * i,
                            last ? ACT_NONE : ACT_TANH, a->training, keep, a->seed, 2000 + i, w.scale, w.shift, 0,
                            nullptr, nullptr, s));
+      if (layer_len && !last) {
+        const long n = (long)B * T * cout;
+        zero_past_len_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(nxt, layer_len, B, T, cout);
+        T2_LAUNCH_CHECK();
+      }
       if (last) {   // training-mode last layer: separate transpose + residual
         const long n = (long)B * T * kMel;
         transpose_residual_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(

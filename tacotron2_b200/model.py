@@ -139,6 +139,37 @@ def _wants_grad(module, *tensors):
                                         any(p_.requires_grad for p_ in module.parameters()))
 
 
+def _check_lengths(lengths, B, T, name):
+    """Per-row lengths of a ragged inference batch: (B,) integers, each in 1..T, on the host or the device.  Raises before
+    anything is launched; returns them as a tensor (None stays None)."""
+    if lengths is None:
+        return None
+    if not torch.is_tensor(lengths):
+        lengths = torch.as_tensor(lengths)
+    if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+        raise TypeError("tacotron2_b200: %s must hold integers (got %s)" % (name, lengths.dtype))
+    if tuple(lengths.shape) != (B,):
+        raise ValueError("tacotron2_b200: %s must have shape (%d,) (got %s)" % (name, B, tuple(lengths.shape)))
+    host = lengths.cpu()
+    lo, hi = int(host.min()), int(host.max())
+    if lo < 1 or hi > T:
+        raise ValueError("tacotron2_b200: %s must lie in 1..%d (got %d..%d)" % (name, T, lo, hi))
+    return lengths
+
+
+def _ragged(lengths, T):
+    """Whether some text of the batch is shorter than T_text.  Then each row's postnet is its own B=1 postnet: every layer
+    is zero past the row's frame count.  An equal-length batch (no lengths, or all of them T_text) keeps the batched
+    postnet, whose hidden layers run over the zero frames past an early-stopping row's end (README "batched inference")."""
+    return lengths is not None and int(lengths.min()) < T
+
+
+def _require_no_grad_with_lengths(module, what):
+    if torch.is_grad_enabled() and any(p_.requires_grad for p_ in module.parameters()):
+        raise NotImplementedError("tacotron2_b200: %s with per-row lengths has no autograd node; call it under "
+                                  "torch.no_grad()" % what)
+
+
 MAX_TRAIN_ROWS = 64   # rows per GPU of one autograd call: the backward kernels and the training stash are sized for one
                       # 64-row launch (BASELINE.json configs[2] / [3] are B=64 per GPU); larger batches: split and accumulate
 
@@ -320,8 +351,17 @@ class Encoder(_EngineOwner, nn.Module):
         semantics, model.py:180-188) -> (B, T, 512)."""
         return self._run(x, input_lengths)
 
-    def inference(self, x):
-        return self._run(x, None)
+    def inference(self, x, input_lengths=None):
+        """x (B, 512, T) embedded text -> (B, T, 512).  input_lengths (B,) integers in 1..T, any order: row b is encoded
+        as x[b:b+1, :, :input_lengths[b]] alone, bit for bit (the columns past it are ignored), and its memory past
+        input_lengths[b] is zero, as pad_packed_sequence leaves it."""
+        if input_lengths is None:
+            return self._run(x, None)
+        lengths = _check_lengths(input_lengths, x.size(0), x.size(2), "input_lengths")
+        _require_no_grad_with_lengths(self, "Encoder.inference")
+        eng = self._t2_engine()
+        out = eng.encoder(embedded=x.transpose(1, 2).detach(), lengths=lengths, training=False, per_row=True)
+        return out.to(x.dtype)
 
 
 class Decoder(_EngineOwner, nn.Module):
@@ -410,16 +450,20 @@ class Decoder(_EngineOwner, nn.Module):
             mel, gate, align, _ = self._teacher_forward(memory, decoder_inputs, memory_lengths, False)
         return mel.transpose(1, 2).to(dt), gate.to(dt), align.to(dt)
 
-    def inference(self, memory):
+    def inference(self, memory, memory_lengths=None):
         """Free-running pass (model.py:418-454), batched: per-row stop latch, see README "batched
         inference".  Returns mel (B, n_mel, T), gate (B, T, 1), alignments (B, T, T_enc); T = steps
         until every row has fired (or max_decoder_steps); ``self.mel_lengths`` holds per-row lengths.  In training mode
         the attention / decoder hidden states take their dropout as in the reference's decode() (model.py:355-356,
-        370-371); injected att / dec masks are (max_decoder_steps, B, 1024)."""
+        370-371); injected att / dec masks are (max_decoder_steps, B, 1024).  memory_lengths (B,) integers in 1..T_enc,
+        any order: row b attends to memory[b, :memory_lengths[b]] only and its outputs equal those of a call on that
+        slice alone, bit for bit; its alignments past memory_lengths[b] are zero."""
+        memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
         eng = self._t2_engine()
         masks = current_masks()
         mel, gate, align, lengths, n_steps = eng.decoder(
-            memory, _capi.MODE_INFER, self.max_decoder_steps, training=self.training, prenet_keep=masks["prenet"],
+            memory, _capi.MODE_INFER, self.max_decoder_steps, memory_lengths=memory_lengths, training=self.training,
+            prenet_keep=masks["prenet"],
             att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold)
         n = int(n_steps.item())                      # the one host sync of the whole loop (model.py:443 syncs every step)
         self.mel_lengths = lengths
@@ -430,7 +474,7 @@ class Decoder(_EngineOwner, nn.Module):
         dt = memory.dtype
         return (mel[:, :n].transpose(1, 2).to(dt), gate[:, :n].unsqueeze(-1).to(dt), align[:, :n].to(dt))
 
-    def _stream_chunks(self, memory, chunk_steps, halo):
+    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None):
         """The persistent decoder in chunks of chunk_steps steps.  Yields (t0, t1, finished, stream): frames [t0, t1) are
         the new ones that every row has produced and that no frame within `halo` steps of them can still change, i.e. all
         frames up to the steps run less `halo` while any row is live, and all of them once every 64-row slice has
@@ -440,7 +484,7 @@ class Decoder(_EngineOwner, nn.Module):
             raise ValueError("tacotron2_b200: chunk_steps must be >= 1 (got %d)" % chunk_steps)
         eng = self._t2_engine()
         st = eng.decoder_stream(memory, self.max_decoder_steps, prenet_keep=current_masks()["prenet"],
-                                gate_threshold=self.gate_threshold)
+                                gate_threshold=self.gate_threshold, memory_lengths=memory_lengths)
         t0 = 0
         while True:
             live_steps, n, finished = st.run(chunk_steps)
@@ -457,19 +501,20 @@ class Decoder(_EngineOwner, nn.Module):
                 return
             t0 = t1
 
-    def inference_stream(self, memory, chunk_steps=32):
+    def inference_stream(self, memory, chunk_steps=32, memory_lengths=None):
         """inference() in chunks of ``chunk_steps`` decoder steps, as a generator: one item per chunk that produced
         frames, a dict with ``frames`` = (t0, t1) (the same for every row), ``mel_outputs`` (B, n_mel, t1-t0),
         ``gate_outputs`` (B, t1-t0, 1), ``alignments`` (B, t1-t0, T_enc), ``mel_lengths`` (B,) int32 on the device with -1
         for rows that are still live, and ``finished``.  A decoder frame is handed out as soon as every row has produced
-        it; concatenated along time the items are bit-identical to inference() (same weights, memory, masks / seed).
-        Evaluation mode only: the resumable decoder applies no hidden-state dropout, which inference() does in training
-        mode."""
+        it; concatenated along time the items are bit-identical to inference() (same weights, memory, memory_lengths,
+        masks / seed).  Evaluation mode only: the resumable decoder applies no hidden-state dropout, which inference()
+        does in training mode."""
         if self.training:
             raise RuntimeError("tacotron2_b200: Decoder.inference_stream needs eval mode (in training mode inference() "
                                "applies the attention / decoder dropout, which the resumable decoder does not)")
+        memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
         dt = memory.dtype
-        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0):
+        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths):
             yield dict(frames=(t0, t1), mel_outputs=st.mel[:, t0:t1].transpose(1, 2).to(dt),
                        gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
                        mel_lengths=st.mel_lengths.clone(), finished=finished)
@@ -608,14 +653,21 @@ class Tacotron2(_EngineOwner, nn.Module):
             outputs = [o.to(cast) for o in outputs]
         return self.parse_output(outputs, output_lengths)
 
-    def inference(self, inputs):
+    def inference(self, inputs, input_lengths=None):
         """model.py:517-529, batched.  For B > 1 frames at t >= mel_lengths[b] of mel_outputs and
         mel_outputs_postnet are zero (same convention as parse_output); ``self.mel_lengths`` holds
-        the per-row lengths.  B == 1 is exactly the reference."""
+        the per-row lengths.  B == 1 is exactly the reference.
+
+        input_lengths (B,) integers in 1..T_text, on the host or the device, in any order: texts of different lengths in
+        one batch.  Row b then computes what ``inference(inputs[b:b+1, :input_lengths[b]])`` computes, bit for bit (its
+        frames up to the batch's step count, alignments[b, :, :input_lengths[b]], mel_lengths[b]); the ids past its length
+        are ignored and alignments[b, :, input_lengths[b]:] is zero.  None: every row is T_text long."""
+        lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
         eng = self._t2_engine()
-        memory = eng.encoder(text=inputs, lengths=None, training=self.training, keep=current_masks()["enc"])
+        memory = eng.encoder(text=inputs, lengths=lengths_in, training=self.training, keep=current_masks()["enc"],
+                             per_row=lengths_in is not None)
         memory = memory.to(self._t2_out_dtype())     # a .half() model hands half tensors between its modules (ipynb:89-90)
-        mel_outputs, gate_outputs, alignments = self.decoder.inference(memory)
+        mel_outputs, gate_outputs, alignments = self.decoder.inference(memory, memory_lengths=lengths_in)
         lengths = self.decoder.mel_lengths
         self.mel_lengths = lengths
         mel_btc = mel_outputs.transpose(1, 2)
@@ -623,13 +675,14 @@ class Tacotron2(_EngineOwner, nn.Module):
             mel_btc = mel_btc.float().contiguous()
         multi = inputs.size(0) > 1
         mel_outputs_postnet = eng.postnet(mel_btc, lengths if multi else None, True, self.training,
-                                          current_masks()["post"]).to(mel_outputs.dtype)
+                                          current_masks()["post"], per_row=_ragged(lengths_in, inputs.size(1))
+                                          ).to(mel_outputs.dtype)
         if multi:
             pad = ~get_mask_from_lengths(lengths.long(), mel_outputs.size(2))
             mel_outputs = mel_outputs.masked_fill(pad.unsqueeze(1), 0.0)
         return self.parse_output([mel_outputs, mel_outputs_postnet, gate_outputs, alignments])
 
-    def inference_stream(self, inputs, chunk_steps=32):
+    def inference_stream(self, inputs, chunk_steps=32, input_lengths=None):
         """inference() as a generator that hands out frames while the decoder runs (README "streaming inference").
 
         The encoder runs once; the decoder runs in chunks of ``chunk_steps`` steps.  Each item is a dict describing frames
@@ -638,18 +691,22 @@ class Tacotron2(_EngineOwner, nn.Module):
         for rows that are still live, and ``finished``.  The postnet's five k=5 convolutions see +-10 frames, so frame t is
         handed out once the decoder has run step t+10 or every row has stopped; it is never revised.  Concatenated along
         time the items are bit-identical to inference() with the same weights, inputs and dropout masks / seed.  After the
-        last item ``self.mel_lengths`` and the max-steps warning are as after inference().  Evaluation mode only: in
-        training mode BatchNorm normalises over the whole sequence, so no frame is final before the last one."""
+        last item ``self.mel_lengths`` and the max-steps warning are as after inference().  input_lengths: as for
+        inference(), whose output the items then concatenate to.  Evaluation mode only: in training mode BatchNorm
+        normalises over the whole sequence, so no frame is final before the last one."""
         if self.training:
             raise RuntimeError("tacotron2_b200: inference_stream needs eval mode (training-mode BatchNorm uses the statistics "
                                "of the whole sequence, so no postnet frame is final before the decoder ends)")
+        lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
         eng = self._t2_engine()
-        memory = eng.encoder(text=inputs, lengths=None, training=False, keep=current_masks()["enc"])
+        memory = eng.encoder(text=inputs, lengths=lengths_in, training=False, keep=current_masks()["enc"],
+                             per_row=lengths_in is not None)
         dt = self._t2_out_dtype()
         memory = memory.to(dt)
         multi = inputs.size(0) > 1
+        ragged = _ragged(lengths_in, inputs.size(1))
         halo = POSTNET_HALO
-        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo):
+        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in):
             if finished:
                 self.mel_lengths = st.mel_lengths
             lengths = st.mel_lengths
@@ -663,7 +720,7 @@ class Tacotron2(_EngineOwner, nn.Module):
             win_len = None
             if multi:                                  # frames at t >= length count as zero; live rows have none
                 win_len = torch.where(lengths < 0, torch.full_like(lengths, w1 - w0), (lengths - w0).clamp(min=0))
-            post = eng.postnet(mel_btc, win_len, True, False, None)[:, :, t0 - w0:t1 - w0].to(dt)
+            post = eng.postnet(mel_btc, win_len, True, False, None, per_row=ragged)[:, :, t0 - w0:t1 - w0].to(dt)
             mel_outputs = st.mel[:, t0:t1].transpose(1, 2).to(dt)
             if multi:
                 t = torch.arange(t0, t1, device=lengths.device)

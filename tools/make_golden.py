@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz by executing the UNMODIFIED reference model.py (needs a checkout of
-NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live|waveglow|denoiser]
+NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live|waveglow|denoiser|ragged]
 
 Every file holds the inputs' seeds, the reference outputs and a checksum of the synthetic weights
 (tests/common.synth_state_dict) so a drift of the generator is detected instead of silently
@@ -115,6 +115,49 @@ def infer_case(name, B, T_text, max_steps, quantile, wseed, tseed, mseed, wscale
     save(name, B=B, T_text=T_text, max_steps=max_steps, wseed=wseed, wscale=wscale, tseed=tseed, mseed=mseed,
          gate_bias=bias, gate_sign=sign, wsum=weights_checksum(sd), memory=memory, mel=mel, mel_masked=mel_masked,
          mel_post=post, gate=gate, align=align, mel_lengths=lengths, gate_margin=margin)
+
+
+def ragged_case(name="infer_ragged_b4_t40", lengths=(23, 40, 7, 31), max_steps=40, quantiles=(0.97, 0.95, 0.93, 0.9),
+                wseed=1234, tseed=81, mseed=82, wscale=2.0):
+    """Texts of different lengths, each run ALONE through the reference's own Tacotron2.inference (B = 1 on
+    text[b, :lengths[b]] with the prenet masks keep[:, :, b]).  The engine runs them as one ragged batch
+    (input_lengths); the ids past each row's length in `text` are padding it must ignore.  Outputs are stored
+    zero-padded to the longest run: mel / mel_post (B, 80, S), gate (B, S, 1), align (B, S, T_text)."""
+    B, T_text = len(lengths), max(lengths)
+    text = rand_text(B, T_text, tseed)
+    keep = keep_mask((max_steps, 2, B, 256), 0.5, mseed)
+    bl = int(np.argmax(lengths))
+
+    def run(sd):
+        model = build(sd)
+        model.decoder.max_decoder_steps = max_steps
+        rows = []
+        for b, L in enumerate(lengths):
+            masks = [keep[t, l, b:b + 1].bool() for t in range(max_steps) for l in range(2)]
+            with torch.no_grad(), injected_dropout(ref, MaskInjector(masks)):
+                rows.append(model.inference(text[b:b + 1, :L]))
+        n = [int(r[0].shape[2]) for r in rows]
+        margin = min(float((torch.sigmoid(r[2][0, :, 0]) - 0.5).abs().min()) for r in rows)
+        return rows, n, margin
+
+    best = None
+    for q in quantiles:
+        sign, bias = calibrate_gate(synth_state_dict(wseed, scale=wscale), text[bl:bl + 1, :lengths[bl]],
+                                    keep[:, :, bl:bl + 1], max_steps, q)
+        sd = synth_state_dict(wseed, gate_bias=bias, scale=wscale, gate_sign=sign)
+        rows, n, margin = run(sd)
+        score = margin if (len(set(n)) > 2 and min(n) > 2) else margin * 1e-3
+        if best is None or score > best[0]:
+            best = (score, sign, bias, sd, rows, n, margin)
+    _, sign, bias, sd, rows, n, margin = best
+    S = max(n)
+    mel = torch.zeros(B, 80, S); post = torch.zeros(B, 80, S); gate = torch.zeros(B, S, 1); align = torch.zeros(B, S, T_text)
+    for b, (r, nb) in enumerate(zip(rows, n)):
+        mel[b, :, :nb] = r[0][0]; post[b, :, :nb] = r[1][0]; gate[b, :nb] = r[2][0]; align[b, :nb, :lengths[b]] = r[3][0]
+    print(name, "input lengths", list(lengths), "mel lengths", n, "gate margin", margin)
+    save(name, B=B, T_text=T_text, max_steps=max_steps, wseed=wseed, wscale=wscale, tseed=tseed, mseed=mseed,
+         gate_bias=bias, gate_sign=sign, wsum=weights_checksum(sd), input_lengths=np.array(lengths), mel=mel,
+         mel_post=post, gate=gate, align=align, mel_lengths=np.array(n, dtype=np.int32), gate_margin=margin)
 
 
 def ref_free_running(model, text, keep, steps):
@@ -641,6 +684,9 @@ def denoiser_case(seed=3, n=256 * 40 + 100, strengths=(0.01, 0.1, 3.0), n_sample
 
 
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "ragged":
+        ragged_case()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "denoiser":
         denoiser_case()
         sys.exit(0)
