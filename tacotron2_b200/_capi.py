@@ -1,8 +1,11 @@
 """ctypes binding of libt2b200.so (include/t2b200.h).  Importing this module never touches CUDA;
 ``lib()`` loads the shared library and raises loudly when it is missing -- there is NO CPU or
-PyTorch fallback for the hot path."""
+PyTorch fallback for the hot path.  ``call`` runs a library entry point on torch's current stream, and ``Workspace``
+caches the device buffers the entry points take."""
 import ctypes as C
 import os
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("T2B200_LIB") or os.path.join(_HERE, "libt2b200.so")   # T2B200_LIB: A/B test builds
@@ -318,3 +321,32 @@ class T2Error(RuntimeError):
 def check(rc):
     if rc != 0:
         raise T2Error("libt2b200 error %d: %s" % (rc, lib().t2_last_error().decode()))
+
+
+def call(fn, device, *args):
+    """fn(*args, stream) on `device`, where stream is torch's current CUDA stream there; raises T2Error on failure."""
+    with torch.cuda.device(device):
+        check(fn(*args, C.c_void_p(torch.cuda.current_stream(device).cuda_stream)))
+
+
+def byte_buffer(nbytes, device):
+    """An uninitialised device buffer of nbytes bytes (workspaces, stashes, stream state)."""
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+
+
+class Workspace:
+    """Device workspaces by tag, reused while large enough.  A larger request or another device frees the old buffer
+    before it allocates the new one, so the two never coexist."""
+
+    def __init__(self):
+        self._bufs = {}
+
+    def get(self, tag, nbytes, device):
+        t = self._bufs.get(tag)
+        if t is None or t.numel() < nbytes or t.device != device:
+            t = self._bufs[tag] = None
+            t = self._bufs[tag] = byte_buffer(nbytes, device)
+        return t
+
+    def __getitem__(self, tag):
+        return self._bufs[tag]

@@ -95,57 +95,109 @@ def next_seed():
     return (torch.initial_seed() * 1000003 + _seed_counter[0]) & 0xFFFFFFFFFFFFFFFF
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
+def _i32(x, device):
+    """Per-row lengths as contiguous int32 on the device (None stays None)."""
+    return None if x is None else x.to(device=device, dtype=torch.int32).contiguous()
 
 
 def _u8(mask, device):
+    """A keep mask as contiguous uint8 on the device; a list / tuple of masks is concatenated flat, in order."""
     if mask is None:
         return None
+    if isinstance(mask, (list, tuple)):
+        mask = torch.cat([k.to(torch.uint8).reshape(-1) for k in mask])
     return mask.to(device=device, dtype=torch.uint8).contiguous()
 
 
-class Engine:
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _source(text, embedded, device):
+    """The encoder's input on the device: (text int64, None) or (None, embedded fp32)."""
+    if text is not None:
+        return text.to(device=device, dtype=torch.int64).contiguous(), None
+    return None, embedded.to(device=device, dtype=torch.float32).contiguous()
+
+
+class _Handle:
+    """One library object (t2_<kind>_create / _refresh / _destroy) holding packed copies of a module's tensors on one
+    device, and its cached workspaces.  The copies are keyed on the global weights generation and each tensor's pointer,
+    torch version counter and dtype: the first call creates the object, a call with another key refreshes it, and one on
+    another device, or with other `extra` key parts, replaces it.  Subclasses supply ``_pack`` and ``_config``."""
+
+    kind = what = None      # the library object; the module named in the error for a module that is not on a GPU
+
+    def __init__(self):
+        self.handle = self.key = self.held = self.device = self.extra = None
+        self._ws = _capi.Workspace()
+
+    def invalidate(self):
+        """Forget the cache key: the next call re-packs every device-side copy from the live tensors."""
+        self.key = None
+
+    def _ensure(self, dev, tensors, extra=(), force=False):
+        """tensors: the module's tensors in table order (None: absent); extra: key parts the object is created with."""
+        if dev is None or dev.type != "cuda":
+            raise RuntimeError("%s must live on a CUDA device (H100); there is no CPU path -- call .cuda() first" % self.what)
+        key = (_weights_generation[0],) + tuple(extra) + tuple(
+            None if t is None else (t.data_ptr(), t._version, t.dtype) for t in tensors)
+        if self.handle is not None and key == self.key and dev == self.device and not force:
+            return
+        held, args = self._pack(tensors, dev, *extra)
+        L = _capi.lib()
+        if self.handle is None or (dev, extra) != (self.device, self.extra):
+            self.close()
+            cfg, h = self._config(*extra), C.c_void_p()
+            _capi.call(getattr(L, "t2_%s_create" % self.kind), dev, C.byref(h), C.byref(cfg), *args)
+            self.handle = h
+        else:
+            _capi.call(getattr(L, "t2_%s_refresh" % self.kind), dev, self.handle, *args)
+        self.key, self.held, self.device, self.extra = key, held, dev, extra
+
+    def close(self):
+        if self.handle is not None:
+            getattr(_capi.lib(), "t2_%s_destroy" % self.kind)(self.handle)
+            self.handle = self.key = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _call(self, fn, *args):
+        """A library entry point on this object (the handle goes first, the stream last)."""
+        _capi.call(fn, self.device, self.handle, *args)
+
+
+class Engine(_Handle):
     """One T2Model handle (packed weights on one device) + cached workspaces."""
 
+    kind, what = "model", "tacotron2_b200: the model"
+
     def __init__(self, hp):
+        super().__init__()
         self.hp = hp
         self.spec = weight_table_spec(hp)
-        self.handle = None
-        self.key = None
-        self.held = None
-        self.device = None
-        self._ws = {}
         self.impl = _capi.IMPL_AUTO
 
     # -- weights ---------------------------------------------------------------------------------
-    def invalidate(self):
-        """Forget the cache key: the next call re-packs every device-side copy from the live parameters."""
-        self.key = None
-
     def ensure(self, named, force=False):
         """named: dict full-name -> tensor (missing entries are replaced by zeros).  The packed copies are rebuilt when the
         key (global generation, per-tensor pointer / torch version counter / dtype) changed or when `force` is set.
         Writes through ``.data`` do not move torch's version counter: callers doing that use
         ``model.invalidate_weights()`` / ``tacotron2_b200.invalidate_weights()``."""
-        dev = None
-        for t in named.values():
-            if t.is_cuda:
-                dev = t.device
-                break
-        if dev is None:
-            raise RuntimeError("tacotron2_b200: the model must live on a CUDA device (H100); there is no "
-                               "CPU path -- call .cuda() first")
-        key = (_weights_generation[0],) + tuple(
-            (named[n].data_ptr(), named[n]._version, named[n].dtype) if n in named else None for n, _ in self.spec)
-        if self.handle is not None and key == self.key and dev == self.device and not force:
-            return
-        L = _capi.lib()
+        dev = next((t.device for t in named.values() if t.is_cuda), None)
+        self._ensure(dev, [named.get(n) for n, _ in self.spec], force=force)
+
+    def _pack(self, tensors, dev):
         held, ptrs = [], (C.c_void_p * _capi.T2_NUM_WEIGHTS)()
-        for i, (n, shape) in enumerate(self.spec):
-            t = named.get(n)
+        for i, ((n, shape), t) in enumerate(zip(self.spec, tensors)):
             if n.endswith("num_batches_tracked"):
-                ptrs[i] = None
                 continue
             if t is None:
                 t = torch.zeros(shape, device=dev, dtype=torch.float32)
@@ -159,47 +211,21 @@ class Engine:
                     t = t.float().contiguous()
             held.append(t)
             ptrs[i] = t.data_ptr()
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        with torch.cuda.device(dev):
-            if self.handle is None or dev != self.device:
-                self.close()
-                hp = self.hp
-                cfg = _capi.T2Config(
-                    hp.n_mel_channels, hp.n_symbols, hp.symbols_embedding_dim, hp.encoder_kernel_size,
-                    hp.encoder_n_convolutions, hp.encoder_embedding_dim, hp.attention_rnn_dim,
-                    hp.decoder_rnn_dim, hp.prenet_dim, hp.attention_dim, hp.attention_location_n_filters,
-                    hp.attention_location_kernel_size, hp.postnet_embedding_dim, hp.postnet_kernel_size,
-                    hp.postnet_n_convolutions, hp.p_attention_dropout, hp.p_decoder_dropout, 1e-5)
-                if hp.n_frames_per_step != 1:
-                    raise RuntimeError("n_frames_per_step != 1 is not supported (hparams.py:56)")
-                h = C.c_void_p()
-                _capi.check(L.t2_model_create(C.byref(h), C.byref(cfg), ptrs, _capi.T2_NUM_WEIGHTS, stream))
-                self.handle = h
-            else:
-                _capi.check(L.t2_model_refresh(self.handle, ptrs, _capi.T2_NUM_WEIGHTS, stream))
-        self.key, self.held, self.device = key, held, dev
+        return held, (ptrs, _capi.T2_NUM_WEIGHTS)
 
-    def close(self):
-        if self.handle is not None:
-            _capi.lib().t2_model_destroy(self.handle)
-            self.handle = None
-            self.key = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _config(self):
+        hp = self.hp
+        if hp.n_frames_per_step != 1:
+            raise RuntimeError("n_frames_per_step != 1 is not supported (hparams.py:56)")
+        return _capi.T2Config(
+            hp.n_mel_channels, hp.n_symbols, hp.symbols_embedding_dim, hp.encoder_kernel_size,
+            hp.encoder_n_convolutions, hp.encoder_embedding_dim, hp.attention_rnn_dim,
+            hp.decoder_rnn_dim, hp.prenet_dim, hp.attention_dim, hp.attention_location_n_filters,
+            hp.attention_location_kernel_size, hp.postnet_embedding_dim, hp.postnet_kernel_size,
+            hp.postnet_n_convolutions, hp.p_attention_dropout, hp.p_decoder_dropout, 1e-5)
 
     def _workspace(self, tag, nbytes):
-        t = self._ws.get(tag)
-        if t is None or t.numel() < nbytes or t.device != self.device:
-            t = torch.empty(int(nbytes), dtype=torch.uint8, device=self.device)
-            self._ws[tag] = t
-        return t
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return self._ws.get(tag, nbytes, self.device)
 
     # -- encoder ---------------------------------------------------------------------------------
     def encoder(self, text=None, embedded=None, lengths=None, training=False, keep=None, stash=None, seed=None,
@@ -207,94 +233,48 @@ class Engine:
         """per_row: t2_encoder_infer -- row b is encoded as its first lengths[b] positions alone (lengths in any order);
         otherwise lengths has Encoder.forward's packed-sequence meaning (t2_encoder_forward)."""
         L = _capi.lib()
+        text, embedded = _source(text, embedded, self.device)
         src = text if text is not None else embedded
         B, T = int(src.shape[0]), int(src.shape[1])
         memory = torch.empty(B, T, self.hp.encoder_embedding_dim, device=self.device, dtype=torch.float32)
         ws = self._workspace("enc", L.t2_encoder_workspace_bytes(self.handle, B, T))
-        a = _capi.T2EncoderArgs()
-        if text is not None:
-            text = text.to(device=self.device, dtype=torch.int64).contiguous()
-            a.text = text.data_ptr()
-        else:
-            embedded = embedded.to(device=self.device, dtype=torch.float32).contiguous()
-            a.embedded = embedded.data_ptr()
-        len32 = None
-        if lengths is not None:
-            len32 = lengths.to(device=self.device, dtype=torch.int32).contiguous()
-            a.lengths = len32.data_ptr()
-        keep = _u8(keep, self.device)
-        a.B, a.T, a.training = B, T, int(bool(training))
-        a.keep = keep.data_ptr() if keep is not None else None
-        a.seed = next_seed() if seed is None else seed
-        a.memory, a.ws, a.ws_bytes = memory.data_ptr(), ws.data_ptr(), ws.numel()
-        if stash is not None:
-            a.stash, a.stash_bytes = stash.data_ptr(), stash.numel()
-        with torch.cuda.device(self.device):
-            _capi.check((L.t2_encoder_infer if per_row else L.t2_encoder_forward)(self.handle, C.byref(a), self._stream()))
+        len32, keep = _i32(lengths, self.device), _u8(keep, self.device)
+        a = _capi.T2EncoderArgs(_ptr(text), _ptr(embedded), _ptr(len32), B, T, int(bool(training)), _ptr(keep),
+                                next_seed() if seed is None else seed, memory.data_ptr(), ws.data_ptr(), ws.numel(),
+                                _ptr(stash), 0 if stash is None else stash.numel())
+        self._call(L.t2_encoder_infer if per_row else L.t2_encoder_forward, C.byref(a))
         return memory
 
     def stash_buffer(self, kind, *dims):
-        n = getattr(_capi.lib(), "t2_%s_stash_bytes" % kind)(self.handle, *dims)
-        return torch.empty(int(n), dtype=torch.uint8, device=self.device)
+        return _capi.byte_buffer(getattr(_capi.lib(), "t2_%s_stash_bytes" % kind)(self.handle, *dims), self.device)
 
     def encoder_backward(self, text, embedded, lengths, training, keep, seed, stash, d_memory, want_d_embedded, named_grads):
         L = _capi.lib()
         B, T = int(d_memory.shape[0]), int(d_memory.shape[1])
         f32 = dict(device=self.device, dtype=torch.float32)
-        a = _capi.T2EncoderBwdArgs()
-        if text is not None:
-            text = text.to(device=self.device, dtype=torch.int64).contiguous()
-            a.text = text.data_ptr()
-        else:
-            embedded = embedded.to(**f32).contiguous()
-            a.embedded = embedded.data_ptr()
-        len32 = None
-        if lengths is not None:
-            len32 = lengths.to(device=self.device, dtype=torch.int32).contiguous()
-            a.lengths = len32.data_ptr()
-        keep = _u8(keep, self.device)
-        a.B, a.T, a.training = B, T, int(bool(training))
-        a.keep = keep.data_ptr() if keep is not None else None
-        a.seed = seed
-        a.stash, a.stash_bytes = stash.data_ptr(), stash.numel()
+        text, embedded = _source(text, embedded, self.device)
+        len32, keep = _i32(lengths, self.device), _u8(keep, self.device)
         d_memory = d_memory.to(**f32).contiguous()
-        a.d_memory = d_memory.data_ptr()
         d_emb = torch.empty(B, T, self.hp.encoder_embedding_dim, **f32) if want_d_embedded else None
-        a.d_embedded = d_emb.data_ptr() if d_emb is not None else None
-        ptrs = self.grad_table(named_grads)
-        a.grads, a.n_grads = ptrs, _capi.T2_NUM_WEIGHTS
         ws = self._workspace("enc_bwd", L.t2_encoder_backward_workspace_bytes(self.handle, B, T))
-        a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
-        with torch.cuda.device(self.device):
-            _capi.check(L.t2_encoder_backward(self.handle, C.byref(a), self._stream()))
+        a = _capi.T2EncoderBwdArgs(_ptr(text), _ptr(embedded), _ptr(len32), B, T, int(bool(training)), _ptr(keep), seed,
+                                   stash.data_ptr(), stash.numel(), d_memory.data_ptr(), _ptr(d_emb),
+                                   self.grad_table(named_grads), _capi.T2_NUM_WEIGHTS, ws.data_ptr(), ws.numel())
+        self._call(L.t2_encoder_backward, C.byref(a))
         return d_emb
 
     def postnet_backward(self, B, T, training, add_residual, keep, seed, stash, d_mel_post, named_grads, wgrad_lengths=None):
         """d_mel_post (B, 80, T) -> d_mel (B, T, 80)."""
         L = _capi.lib()
         f32 = dict(device=self.device, dtype=torch.float32)
-        a = _capi.T2PostnetBwdArgs()
-        a.B, a.T, a.training, a.add_residual = B, T, int(bool(training)), int(bool(add_residual))
-        if keep is not None and isinstance(keep, (list, tuple)):
-            keep = torch.cat([k.to(torch.uint8).reshape(-1) for k in keep])
-        keep = _u8(keep, self.device)
-        a.keep = keep.data_ptr() if keep is not None else None
-        a.seed = seed
-        wl32 = None
-        if wgrad_lengths is not None:
-            wl32 = wgrad_lengths.to(device=self.device, dtype=torch.int32).contiguous()
-            a.wgrad_lengths = wl32.data_ptr()
-        a.stash, a.stash_bytes = stash.data_ptr(), stash.numel()
+        keep, wl32 = _u8(keep, self.device), _i32(wgrad_lengths, self.device)
         d_mel_post = d_mel_post.to(**f32).contiguous()
-        a.d_mel_post = d_mel_post.data_ptr()
         d_mel = torch.empty(B, T, self.hp.n_mel_channels, **f32)
-        a.d_mel = d_mel.data_ptr()
-        ptrs = self.grad_table(named_grads)
-        a.grads, a.n_grads = ptrs, _capi.T2_NUM_WEIGHTS
         ws = self._workspace("post_bwd", L.t2_postnet_backward_workspace_bytes(self.handle, B, T))
-        a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
-        with torch.cuda.device(self.device):
-            _capi.check(L.t2_postnet_backward(self.handle, C.byref(a), self._stream()))
+        a = _capi.T2PostnetBwdArgs(B, T, int(bool(training)), int(bool(add_residual)), _ptr(keep), seed, _ptr(wl32),
+                                   stash.data_ptr(), stash.numel(), d_mel_post.data_ptr(), d_mel.data_ptr(),
+                                   self.grad_table(named_grads), _capi.T2_NUM_WEIGHTS, ws.data_ptr(), ws.numel())
+        self._call(L.t2_postnet_backward, C.byref(a))
         return d_mel
 
     # -- decoder ---------------------------------------------------------------------------------
@@ -313,31 +293,17 @@ class Engine:
         mel_lengths = torch.zeros(B, device=self.device, dtype=torch.int32)
         n_steps = torch.zeros(1, device=self.device, dtype=torch.int32)
         ws = self._workspace("dec", L.t2_decoder_workspace_bytes(self.handle, B, T, cap))
-        a = _capi.T2DecoderArgs()
-        a.mode, a.impl, a.training = mode, self.impl if impl is None else impl, int(bool(training))
-        a.memory = memory.data_ptr()
-        len32 = None
-        if memory_lengths is not None:
-            len32 = memory_lengths.to(device=self.device, dtype=torch.int32).contiguous()
-            a.memory_lengths = len32.data_ptr()
-        a.B, a.T_enc, a.n_steps_cap = B, T, cap
+        len32 = _i32(memory_lengths, self.device)
         if teacher_prenet is not None:
             teacher_prenet = teacher_prenet.contiguous()
-            a.teacher_prenet = teacher_prenet.data_ptr()
         pk, ak, dk = _u8(prenet_keep, self.device), _u8(att_keep, self.device), _u8(dec_keep, self.device)
-        a.prenet_keep = pk.data_ptr() if pk is not None else None
-        a.att_keep = ak.data_ptr() if ak is not None else None
-        a.dec_keep = dk.data_ptr() if dk is not None else None
-        a.seed = next_seed() if seed is None else seed
-        if stash is not None:
-            a.stash, a.stash_bytes = stash.data_ptr(), stash.numel()
-        a.gate_threshold = float(gate_threshold)
-        a.score_mask_value = float(score_mask_value)
-        a.mel, a.gate, a.align = mel.data_ptr(), gate.data_ptr(), align.data_ptr()
-        a.mel_lengths, a.n_steps = mel_lengths.data_ptr(), n_steps.data_ptr()
-        a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
-        with torch.cuda.device(self.device):
-            _capi.check(L.t2_decoder_run(self.handle, C.byref(a), self._stream()))
+        a = _capi.T2DecoderArgs(mode, self.impl if impl is None else impl, int(bool(training)), memory.data_ptr(),
+                                _ptr(len32), B, T, cap, _ptr(teacher_prenet), _ptr(pk), _ptr(ak), _ptr(dk),
+                                next_seed() if seed is None else seed, float(gate_threshold), float(score_mask_value),
+                                mel.data_ptr(), gate.data_ptr(), align.data_ptr(), mel_lengths.data_ptr(),
+                                n_steps.data_ptr(), ws.data_ptr(), ws.numel(),
+                                _ptr(stash), 0 if stash is None else stash.numel())
+        self._call(L.t2_decoder_run, C.byref(a))
         self._last_decoder_args = (a, memory, len32, teacher_prenet, pk, ak, dk, ws, mel, gate, align, mel_lengths, n_steps)
         return mel, gate, align, mel_lengths, n_steps
 
@@ -358,13 +324,9 @@ class Engine:
         return {names[i]: [int(out[s * 24 + i]) for s in range(3)] for i in range(len(names))}
 
     def grad_table(self, named_grads):
-        """(ctypes pointer array of T2_NUM_WEIGHTS entries, held tensors): named_grads maps full state_dict names to
-        the contiguous fp32 tensors the library overwrites with that parameter's gradient."""
-        ptrs = (C.c_void_p * _capi.T2_NUM_WEIGHTS)()
-        for i, (n, _) in enumerate(self.spec):
-            t = named_grads.get(n)
-            ptrs[i] = t.data_ptr() if t is not None else None
-        return ptrs
+        """ctypes pointer array of T2_NUM_WEIGHTS entries: named_grads maps full state_dict names to the contiguous fp32
+        tensors the library overwrites with that parameter's gradient."""
+        return (C.c_void_p * _capi.T2_NUM_WEIGHTS)(*[_ptr(named_grads.get(n)) for n, _ in self.spec])
 
     def decoder_stash(self, B, T_enc, T_mel):
         return self.stash_buffer("decoder", B, T_enc, T_mel)
@@ -380,63 +342,38 @@ class Engine:
         d_memory = torch.empty(B, Te, self.hp.encoder_embedding_dim, **f32)
         d_prenet = torch.empty(T, B, self.hp.prenet_dim, **f32)
         ws = self._workspace("dec_bwd", L.t2_decoder_backward_workspace_bytes(self.handle, B, Te, T))
-        a = _capi.T2DecoderBwdArgs()
-        memory = memory.contiguous()
-        a.memory = memory.data_ptr()
-        len32 = None
-        if memory_lengths is not None:
-            len32 = memory_lengths.to(device=self.device, dtype=torch.int32).contiguous()
-            a.memory_lengths = len32.data_ptr()
-        a.B, a.T_enc, a.T_mel, a.training = B, Te, T, int(bool(training))
-        a.teacher_prenet = teacher_prenet.data_ptr()
+        memory, len32 = memory.contiguous(), _i32(memory_lengths, self.device)
         ak, dk = _u8(att_keep, self.device), _u8(dec_keep, self.device)
-        a.att_keep = ak.data_ptr() if ak is not None else None
-        a.dec_keep = dk.data_ptr() if dk is not None else None
-        a.seed, a.score_mask_value = seed, float(score_mask_value)
-        a.align, a.stash, a.stash_bytes = align.data_ptr(), stash.data_ptr(), stash.numel()
         d_mel, d_gate = d_mel.to(**f32).contiguous(), d_gate.to(**f32).contiguous()
-        a.d_mel, a.d_gate = d_mel.data_ptr(), d_gate.data_ptr()
         if d_align is not None:
             d_align = d_align.to(**f32).contiguous()
-            a.d_align = d_align.data_ptr()
-        a.d_memory, a.d_prenet = d_memory.data_ptr(), d_prenet.data_ptr()
-        ptrs = self.grad_table(named_grads)
-        a.grads, a.n_grads = ptrs, _capi.T2_NUM_WEIGHTS
-        a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
-        with torch.cuda.device(self.device):
-            _capi.check(L.t2_decoder_backward(self.handle, C.byref(a), self._stream()))
+        a = _capi.T2DecoderBwdArgs(memory.data_ptr(), _ptr(len32), B, Te, T, int(bool(training)), teacher_prenet.data_ptr(),
+                                   _ptr(ak), _ptr(dk), seed, float(score_mask_value), align.data_ptr(),
+                                   stash.data_ptr(), stash.numel(), d_mel.data_ptr(), d_gate.data_ptr(), _ptr(d_align),
+                                   d_memory.data_ptr(), d_prenet.data_ptr(), self.grad_table(named_grads),
+                                   _capi.T2_NUM_WEIGHTS, ws.data_ptr(), ws.numel())
+        self._call(L.t2_decoder_backward, C.byref(a))
         return d_memory, d_prenet
 
     def prenet_backward(self, frames, keep, seed, d_out, named_grads):
         L = _capi.lib()
         frames = frames.to(device=self.device, dtype=torch.float32).contiguous()
         M = int(frames.shape[0])
-        d_out = d_out.contiguous()
+        d_out, keep = d_out.contiguous(), _u8(keep, self.device)
         ws = self._workspace("pre_bwd", L.t2_prenet_backward_workspace_bytes(self.handle, M))
-        keep = _u8(keep, self.device)
-        a = _capi.T2PrenetBwdArgs()
-        a.frames, a.M = frames.data_ptr(), M
-        a.keep = keep.data_ptr() if keep is not None else None
-        a.seed, a.d_out = seed, d_out.data_ptr()
-        ptrs = self.grad_table(named_grads)
-        a.grads, a.n_grads = ptrs, _capi.T2_NUM_WEIGHTS
-        a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
-        with torch.cuda.device(self.device):
-            _capi.check(L.t2_prenet_backward(self.handle, C.byref(a), self._stream()))
+        a = _capi.T2PrenetBwdArgs(frames.data_ptr(), M, _ptr(keep), seed, d_out.data_ptr(), self.grad_table(named_grads),
+                                  _capi.T2_NUM_WEIGHTS, ws.data_ptr(), ws.numel())
+        self._call(L.t2_prenet_backward, C.byref(a))
 
     def prenet(self, frames, keep=None, seed=None):
         """frames (M, 80) -> (M, 256); keep (2, M, 256) uint8 or None."""
-        L = _capi.lib()
         frames = frames.to(device=self.device, dtype=torch.float32).contiguous()
         M = int(frames.shape[0])
         out = torch.empty(M, self.hp.prenet_dim, device=self.device, dtype=torch.float32)
         ws = self._workspace("pre", M * self.hp.prenet_dim * 4)
         keep = _u8(keep, self.device)
-        with torch.cuda.device(self.device):
-            _capi.check(L.t2_prenet_forward(self.handle, frames.data_ptr(), M,
-                                            keep.data_ptr() if keep is not None else None,
-                                            next_seed() if seed is None else seed,
-                                            out.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
+        self._call(_capi.lib().t2_prenet_forward, frames.data_ptr(), M, _ptr(keep), next_seed() if seed is None else seed,
+                   out.data_ptr(), ws.data_ptr(), ws.numel())
         return out
 
     # -- postnet ---------------------------------------------------------------------------------
@@ -450,24 +387,11 @@ class Engine:
         B, T = int(mel_btc.shape[0]), int(mel_btc.shape[1])
         out = torch.empty(B, self.hp.n_mel_channels, T, device=self.device, dtype=torch.float32)
         ws = self._workspace("post", L.t2_postnet_workspace_bytes(self.handle, B, T))
-        a = _capi.T2PostnetArgs()
-        a.mel, a.mel_batch_stride = mel_btc.data_ptr(), int(mel_btc.stride(0))
-        len32 = None
-        if lengths is not None:
-            len32 = lengths.to(device=self.device, dtype=torch.int32).contiguous()
-            a.lengths = len32.data_ptr()
-        a.B, a.T, a.training = B, T, int(bool(training))
-        if keep is not None and isinstance(keep, (list, tuple)):
-            keep = torch.cat([k.to(torch.uint8).reshape(-1) for k in keep])
-        keep = _u8(keep, self.device)
-        a.keep = keep.data_ptr() if keep is not None else None
-        a.seed = next_seed() if seed is None else seed
-        a.add_residual = int(bool(add_residual))
-        a.mel_post, a.ws, a.ws_bytes = out.data_ptr(), ws.data_ptr(), ws.numel()
-        if stash is not None:
-            a.stash, a.stash_bytes = stash.data_ptr(), stash.numel()
-        with torch.cuda.device(self.device):
-            _capi.check((L.t2_postnet_infer if per_row else L.t2_postnet_forward)(self.handle, C.byref(a), self._stream()))
+        len32, keep = _i32(lengths, self.device), _u8(keep, self.device)
+        a = _capi.T2PostnetArgs(mel_btc.data_ptr(), int(mel_btc.stride(0)), _ptr(len32), B, T, int(bool(training)),
+                                _ptr(keep), next_seed() if seed is None else seed, int(bool(add_residual)),
+                                out.data_ptr(), ws.data_ptr(), ws.numel(), _ptr(stash), 0 if stash is None else stash.numel())
+        self._call(L.t2_postnet_infer if per_row else L.t2_postnet_forward, C.byref(a))
         return out
 
     # -- end to end with host buffers (bench e2e leg) ------------------------------------------------
@@ -485,19 +409,14 @@ class Engine:
         impl = self.impl if impl is None else impl
         if input_lengths_host is not None:
             ws = self._workspace("e2e", L.t2_infer_lengths_workspace_bytes(self.handle, B, T, max_steps))
-            a = _capi.T2InferArgs()
-            a.text_host, a.input_lengths_host = text_host.data_ptr(), input_lengths_host.data_ptr()
-            a.B, a.T_text, a.max_steps, a.gate_threshold, a.seed, a.impl = B, T, int(max_steps), float(gate_threshold), seed, impl
-            a.mel_post_host, a.mel_lengths_host, a.n_steps_host = mel.data_ptr(), lens.data_ptr(), ns.data_ptr()
-            a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
-            with torch.cuda.device(self.device):
-                _capi.check(L.t2_infer_host_lengths(self.handle, C.byref(a), self._stream()))
+            a = _capi.T2InferArgs(text_host.data_ptr(), input_lengths_host.data_ptr(), B, T, int(max_steps),
+                                  float(gate_threshold), seed, impl, mel.data_ptr(), lens.data_ptr(), ns.data_ptr(),
+                                  ws.data_ptr(), ws.numel())
+            self._call(L.t2_infer_host_lengths, C.byref(a))
             return mel, lens, ns
         ws = self._workspace("e2e", L.t2_infer_workspace_bytes(self.handle, B, T, max_steps))
-        with torch.cuda.device(self.device):
-            _capi.check(L.t2_infer_host(self.handle, text_host.data_ptr(), B, T, int(max_steps), float(gate_threshold),
-                                        seed, impl, mel.data_ptr(),
-                                        lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()))
+        self._call(L.t2_infer_host, text_host.data_ptr(), B, T, int(max_steps), float(gate_threshold), seed, impl,
+                   mel.data_ptr(), lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel())
         return mel, lens, ns
 
 
@@ -522,32 +441,19 @@ class DecoderStream:
         self.n_slices = (B + 63) // 64
         self.status = torch.zeros(2 * self.n_slices, device=dev, dtype=torch.int32)
         self.status_host = None                      # the caller's copy of `status` after the last run
-        self.state = torch.empty(int(L.t2_decoder_stream_state_bytes(eng.handle, B, T)), dtype=torch.uint8, device=dev)
-        self.keep = _u8(prenet_keep, dev)
-        self.len32 = None if memory_lengths is None else memory_lengths.to(device=dev, dtype=torch.int32).contiguous()
-        a = _capi.T2DecoderStreamArgs()
-        d = a.dec
-        d.mode, d.impl, d.training = _capi.MODE_INFER, impl, 0
-        d.memory, d.B, d.T_enc, d.n_steps_cap = self.memory.data_ptr(), B, T, self.cap
-        d.memory_lengths = self.len32.data_ptr() if self.len32 is not None else None
-        d.prenet_keep = self.keep.data_ptr() if self.keep is not None else None
-        d.seed = seed
-        d.gate_threshold, d.score_mask_value = float(gate_threshold), float(score_mask_value)
-        d.mel, d.gate, d.align = self.mel.data_ptr(), self.gate.data_ptr(), self.align.data_ptr()
-        d.mel_lengths, d.n_steps = self.mel_lengths.data_ptr(), self.n_steps.data_ptr()
-        a.state, a.state_bytes, a.status = self.state.data_ptr(), self.state.numel(), self.status.data_ptr()
-        self.args = a
-        with torch.cuda.device(dev):
-            _capi.check(L.t2_decoder_stream_begin(eng.handle, C.byref(a), eng._stream()))
+        self.state = _capi.byte_buffer(L.t2_decoder_stream_state_bytes(eng.handle, B, T), dev)
+        self.keep, self.len32 = _u8(prenet_keep, dev), _i32(memory_lengths, dev)
+        d = _capi.T2DecoderArgs(_capi.MODE_INFER, impl, 0, self.memory.data_ptr(), _ptr(self.len32), B, T, self.cap,
+                                None, _ptr(self.keep), None, None, seed, float(gate_threshold), float(score_mask_value),
+                                self.mel.data_ptr(), self.gate.data_ptr(), self.align.data_ptr(),
+                                self.mel_lengths.data_ptr(), self.n_steps.data_ptr())
+        self.args = _capi.T2DecoderStreamArgs(d, self.state.data_ptr(), self.state.numel(), self.status.data_ptr())
+        eng._call(L.t2_decoder_stream_begin, C.byref(self.args))
 
     def run(self, n):
         """Advance by up to n steps.  Returns (live_steps, n_total, finished): the steps run by the slices that are still
         live (None when none is), the most steps any slice has run, and whether every slice has stopped."""
-        sh = self.status_host
-        with torch.cuda.device(self.eng.device):
-            _capi.check(_capi.lib().t2_decoder_stream_run(self.eng.handle, C.byref(self.args), int(n),
-                                                          C.c_void_p(sh.data_ptr()) if sh is not None else None,
-                                                          self.eng._stream()))
+        self.eng._call(_capi.lib().t2_decoder_stream_run, C.byref(self.args), int(n), _ptr(self.status_host))
         self.status_host = self.status.cpu()         # the one host sync of the chunk
         steps = self.status_host[0::2].tolist()
         stopped = self.status_host[1::2].tolist()

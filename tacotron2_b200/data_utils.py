@@ -74,7 +74,6 @@ class DeviceTextMelCollate:
         a.text_flat, a.text_offsets, a.mel_flat, a.mel_offsets = (t.data_ptr() for t in (text_flat, text_off, mel_flat, mel_off))
         a.B, a.n_mel, a.T_max, a.L_pad, a.order = B, n_mel, T_max, L_pad, order.data_ptr()
         a.text_padded, a.input_lengths, a.mel_padded, a.gate_padded, a.output_lengths = (t.data_ptr() for t in out)
-        with torch.cuda.device(dev):
-            _capi.check(L.t2_collate(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        _capi.call(L.t2_collate, dev, C.byref(a))
         self.order = order
         return out

@@ -12,6 +12,8 @@ import numpy as np
 import torch
 
 from . import _capi
+from . import _engine
+from ._stream import FinalWindow
 from .layers import _windowed_fourier_basis
 
 HOP = 256
@@ -79,7 +81,7 @@ class Denoiser(torch.nn.Module):
 
     def _engine(self):
         if self._t2 is None:
-            self._t2 = _DenoiserEngine()
+            self._t2 = _DenoiserEngine(self.stft)
         return self._t2
 
     @torch.no_grad()
@@ -99,15 +101,13 @@ class Denoiser(torch.nn.Module):
             raise ValueError("Denoiser.forward: %d samples cannot be reflect-padded by 512 (the reference needs n > 512)" % n)
         len32 = None
         if lengths is not None:
-            len32 = torch.as_tensor(lengths).to(device=eng.device, dtype=torch.int32).contiguous()
+            len32 = _engine._i32(torch.as_tensor(lengths), eng.device)
             if tuple(len32.shape) != (B,):
                 raise ValueError("Denoiser.forward: lengths must have shape (%d,), got %s" % (B, tuple(len32.shape)))
         out = torch.empty(B, 1, HOP * (n // HOP), device=eng.device, dtype=torch.float32)
         if n // HOP == 0:
             return out
-        a = eng.args(self, audio, len32, strength, out)
-        with torch.cuda.device(eng.device):
-            _capi.check(_capi.lib().t2_denoiser_run(eng.handle, C.byref(a), eng.stream()))
+        eng._call(_capi.lib().t2_denoiser_run, C.byref(eng.args(self, audio, len32, strength, out)))
         return out
 
     @torch.no_grad()
@@ -124,97 +124,48 @@ class Denoiser(torch.nn.Module):
         lengths=256 * model.mel_lengths)[:, 0]``.  The stream keeps only the audio later windows can still need: the
         two halos plus one item.  It shares the module's workspace with forward, so both enqueue on the same CUDA
         stream (torch's current stream)."""
-        left, right = denoiser_halo()
         eng = self._engine()
-        kept = None
-        base = held = d0 = 0           # kept: the audio [base, held) in samples; blocks [0, d0) are handed out
+        win = FinalWindow("Denoiser.stream: audio items", "samples", 1, *denoiser_halo(), unit=HOP)
         for item in items:
-            s0, s1 = item["samples"]
-            finished = bool(item["finished"])
-            if s0 != held:
-                raise ValueError("Denoiser.stream: audio items must be consecutive (samples %s after %d)" % ((s0, s1), held))
-            if kept is None:
+            win.check(item)
+            x = item["audio"]
+            if win.kept is None:
                 eng.ensure(self)
-                kept = eng.audio(item["audio"], "Denoiser.stream")
-            else:
-                kept = torch.cat((kept, item["audio"].to(device=kept.device, dtype=kept.dtype)), 1)
-            held = s1
-            # block k is final once the audio up to block k + right is (or the audio has ended)
-            d1 = held // HOP if finished else max(d0, held // HOP - right)
-            if d1 == d0 and not finished:
+                x = eng.audio(x, "Denoiser.stream")
+            span = win.add(item, x)
+            if span is None:
                 continue
-            lengths = item["mel_lengths"]
-            B = int(kept.shape[0])
-            out = torch.empty(B, HOP * (d1 - d0), device=eng.device, dtype=torch.float32)
-            if d1 > d0:
-                # window-relative row ends on the device: live rows (-1) go on past the window; stopped rows end at
-                # 256 * mel_lengths, inside the window or after it
-                lengths = lengths.to(eng.device)
-                win_len = torch.where(lengths < 0, torch.full_like(lengths, -1),
-                                      (HOP * lengths - base).clamp(min=0)).to(torch.int32).contiguous()
-                a = eng.args(self, kept.contiguous(), win_len, strength, out)
-                w = _capi.T2DenoiserWindowArgs()
-                w.dn, w.s0, w.out0, w.out1, w.at_end = a, base, d0 - base // HOP, d1 - base // HOP, int(finished)
-                with torch.cuda.device(eng.device):
-                    _capi.check(_capi.lib().t2_denoiser_run_window(eng.handle, C.byref(w), eng.stream()))
+            (d0, d1), finished, kept = span, bool(item["finished"]), win.kept
+            out = torch.empty(int(kept.shape[0]), HOP * (d1 - d0), device=eng.device, dtype=torch.float32)
+            if d1 > d0:                # the window is every kept sample; -1: a row that does not end in it goes on
+                a = eng.args(self, kept.contiguous(), win.lengths(item["mel_lengths"], -1), strength, out)
+                w = _capi.T2DenoiserWindowArgs(a, win.base, d0 - win.base // HOP, d1 - win.base // HOP, int(finished))
+                eng._call(_capi.lib().t2_denoiser_run_window, C.byref(w))
             yield dict(samples=(HOP * d0, HOP * d1), audio=out, mel_lengths=item["mel_lengths"], finished=finished)
-            d0 = d1
             if finished:
                 return
-            # later windows start at block d0 - left: drop the audio before it
-            drop = HOP * max(0, d0 - left) - base
-            kept, base = kept[:, drop:], base + drop
 
 
-class _DenoiserEngine:
+class _DenoiserEngine(_engine._Handle):
     """One T2Denoiser handle (packed bases on one device) + a cached workspace."""
 
-    def __init__(self):
-        self.handle = None
-        self.key = None
-        self.held = None
-        self.device = None
-        self._ws = None
+    kind, what = "denoiser", "tacotron2_b200.Denoiser"
+    stream = _engine._Handle._stream      # the name callers of the window entry points use
+
+    def __init__(self, stft):
+        super().__init__()
+        self.cfg = (int(stft.filter_length), int(stft.hop_length), int(stft.win_length))
 
     def ensure(self, module):
         st = module.stft
-        fb, ib = st.forward_basis, st.inverse_basis
-        dev = fb.device
-        if dev.type != "cuda":
-            raise RuntimeError("tacotron2_b200.Denoiser must live on a CUDA device (H100); there is no CPU path -- "
-                               "call .cuda() first")
-        key = (fb.data_ptr(), fb._version, ib.data_ptr(), ib._version, dev)
-        if self.handle is not None and key == self.key:
-            return
-        f = fb.detach().to(torch.float32).contiguous()
-        i = ib.detach().to(device=dev, dtype=torch.float32).contiguous()
-        L = _capi.lib()
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        with torch.cuda.device(dev):
-            if self.handle is None or dev != self.device:
-                self.close()
-                cfg = _capi.T2DenoiserConfig(int(st.filter_length), int(st.hop_length), int(st.win_length), 0)
-                h = C.c_void_p()
-                _capi.check(L.t2_denoiser_create(C.byref(h), C.byref(cfg), f.data_ptr(), i.data_ptr(), stream))
-                self.handle = h
-            else:
-                _capi.check(L.t2_denoiser_refresh(self.handle, f.data_ptr(), i.data_ptr(), stream))
-        self.key, self.held, self.device = key, (f, i), dev
+        self._ensure(st.forward_basis.device, (st.forward_basis, st.inverse_basis))
 
-    def close(self):
-        if self.handle is not None:
-            _capi.lib().t2_denoiser_destroy(self.handle)
-            self.handle = None
-            self.key = None
+    def _pack(self, bases, dev):
+        f, i = (b.detach().to(device=dev, dtype=torch.float32).contiguous() for b in bases)
+        return (f, i), (f.data_ptr(), i.data_ptr())
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+    def _config(self):
+        return _capi.T2DenoiserConfig(*self.cfg, 0)
 
     def audio(self, audio, what):
         """audio (B, n) on the device: fp16 stays fp16 (converted as it is packed), any other real dtype becomes fp32."""
@@ -232,9 +183,7 @@ class _DenoiserEngine:
         self.ensure(module)
         x = bias_audio.to(device=self.device, dtype=torch.float32).contiguous()
         out = torch.empty(module.stft.filter_length // 2 + 1, device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            _capi.check(_capi.lib().t2_denoiser_bias(self.handle, x.data_ptr(), int(x.shape[-1]), out.data_ptr(),
-                                                     self.stream()))
+        self._call(_capi.lib().t2_denoiser_bias, x.data_ptr(), int(x.shape[-1]), out.data_ptr())
         return out
 
     def args(self, module, audio, len32, strength, out):
@@ -244,18 +193,10 @@ class _DenoiserEngine:
         if bias.numel() != module.stft.filter_length // 2 + 1 or bias.device != self.device:
             raise ValueError("Denoiser: bias_spec must hold %d values on %s" % (module.stft.filter_length // 2 + 1,
                                                                                self.device))
-        a = _capi.T2DenoiserArgs()
-        a.audio, a.B, a.n, a.io_half = audio.data_ptr(), B, n, int(audio.dtype == torch.float16)
-        if len32 is not None:
-            a.lengths = len32.data_ptr()
         self._bias = bias.detach().to(torch.float32).contiguous()
-        a.bias, a.strength, a.out = self._bias.data_ptr(), float(strength), out.data_ptr()
-        nbytes = int(_capi.lib().t2_denoiser_workspace_bytes(self.handle, B, n))
-        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != self.device:
-            self._ws = None
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        a.ws, a.ws_bytes = self._ws.data_ptr(), self._ws.numel()
-        return a
+        ws = self._ws.get("run", _capi.lib().t2_denoiser_workspace_bytes(self.handle, B, n), self.device)
+        return _capi.T2DenoiserArgs(audio.data_ptr(), B, n, _engine._ptr(len32), int(audio.dtype == torch.float16),
+                                    self._bias.data_ptr(), float(strength), out.data_ptr(), ws.data_ptr(), ws.numel())
 
 
 def denoiser_halo():

@@ -13,6 +13,7 @@ import torch
 
 from . import _capi
 from . import _engine
+from ._stream import FinalWindow
 
 N_MEL, N_FLOWS, N_GROUP, N_EARLY_EVERY, N_EARLY_SIZE = 80, 12, 8, 4, 2
 WN_CONFIG = dict(n_layers=8, n_channels=256, kernel_size=3)
@@ -145,7 +146,7 @@ class WaveGlow(torch.nn.Module):
     def invalidate_weights(self):
         """Re-pack the engine's weights on the next call (after writes through ``.data`` that torch does not count)."""
         if self._t2 is not None:
-            self._t2.key = None
+            self._t2.invalidate()
 
     def _weight_table(self):
         """(tensor or None) x 686 in the engine's table order: the reference state_dict order with weight-normed
@@ -197,67 +198,36 @@ class WaveGlow(torch.nn.Module):
         return self._engine().stream(self, items, sigma, getattr(_tls, "z", None))
 
 
-class _WaveGlowEngine:
+class _WaveGlowEngine(_engine._Handle):
     """One T2WaveGlow handle (packed weights on one device) + a cached workspace."""
 
+    kind, what = "waveglow", "tacotron2_b200.WaveGlow"
+
     def __init__(self, cfg):
+        super().__init__()
         self.cfg = cfg
-        self.handle = None
-        self.key = None
-        self.held = None
-        self.device = None
-        self.fp16 = None
-        self._ws = None
         self.last_seed = None
 
     def ensure(self, module):
-        table = module._weight_table()
-        dev = module.upsample.weight.device
-        if dev.type != "cuda":
-            raise RuntimeError("tacotron2_b200.WaveGlow must live on a CUDA device (H100); there is no CPU path -- "
-                               "call .cuda() first")
-        fp16 = module.upsample.weight.dtype == torch.float16
-        key = (_engine._weights_generation[0], fp16) + tuple(
-            None if t is None else (t.data_ptr(), t._version, t.dtype) for t in table)
-        if self.handle is not None and key == self.key and dev == self.device:
-            return
-        n_conv = _capi.T2_WAVEGLOW_NUM_WEIGHTS - len(module.convinv)
-        want = torch.float16 if fp16 else torch.float32
+        w = module.upsample.weight
+        self._ensure(w.device, module._weight_table(), (w.dtype == torch.float16,))
+
+    def _pack(self, table, dev, fp16):
+        n_conv = _capi.T2_WAVEGLOW_NUM_WEIGHTS - self.cfg[1]      # the table ends with one convinv weight per flow
         held, ptrs = [], (C.c_void_p * _capi.T2_WAVEGLOW_NUM_WEIGHTS)()
         for i, t in enumerate(table[:_capi.T2_WAVEGLOW_NUM_WEIGHTS]):
             if t is None:
-                ptrs[i] = None
                 continue
             t = t.detach()
-            dt = torch.float32 if i >= n_conv else want     # convinv: always fp32 (the notebook keeps it so)
+            dt = torch.float32 if i >= n_conv or not fp16 else torch.float16    # convinv: always fp32 (as the notebook)
             if t.dtype != dt or not t.is_contiguous():
                 t = t.to(dt).contiguous()
             held.append(t)
             ptrs[i] = t.data_ptr()
-        L = _capi.lib()
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        with torch.cuda.device(dev):
-            if self.handle is None or dev != self.device or fp16 != self.fp16:
-                self.close()
-                cfg = _capi.T2WaveGlowConfig(*[int(x) if x is not None else -1 for x in self.cfg], int(fp16))
-                h = C.c_void_p()
-                _capi.check(L.t2_waveglow_create(C.byref(h), C.byref(cfg), ptrs, _capi.T2_WAVEGLOW_NUM_WEIGHTS, stream))
-                self.handle = h
-            else:
-                _capi.check(L.t2_waveglow_refresh(self.handle, ptrs, _capi.T2_WAVEGLOW_NUM_WEIGHTS, stream))
-        self.key, self.held, self.device, self.fp16 = key, held, dev, fp16
+        return held, (ptrs, _capi.T2_WAVEGLOW_NUM_WEIGHTS)
 
-    def close(self):
-        if self.handle is not None:
-            _capi.lib().t2_waveglow_destroy(self.handle)
-            self.handle = None
-            self.key = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _config(self, fp16):
+        return _capi.T2WaveGlowConfig(*[int(x) if x is not None else -1 for x in self.cfg], int(fp16))
 
     def _spect(self, spect, what):
         if spect.dim() != 3 or spect.shape[1] != self.cfg[0]:
@@ -283,30 +253,19 @@ class _WaveGlowEngine:
     def _args(self, spect, len32, zt, sigma, seed, audio):
         """T2WaveGlowArgs over spect (B, n_mel, T) on the device, with a workspace of the engine's cache."""
         B, T = int(spect.shape[0]), int(spect.shape[2])
-        a = _capi.T2WaveGlowArgs()
-        a.mel, a.B, a.T_mel, a.io_half = spect.data_ptr(), B, T, int(spect.dtype == torch.float16)
-        if len32 is not None:
-            a.lengths = len32.data_ptr()
-        if zt is not None:
-            a.z = zt.data_ptr()
-        a.sigma, a.seed = float(sigma), seed
-        nbytes = int(_capi.lib().t2_waveglow_workspace_bytes(self.handle, B, T))
-        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != self.device:
-            self._ws = None
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        a.audio, a.ws, a.ws_bytes = audio.data_ptr(), self._ws.data_ptr(), self._ws.numel()
-        return a
+        ws = self._ws.get("infer", _capi.lib().t2_waveglow_workspace_bytes(self.handle, B, T), self.device)
+        return _capi.T2WaveGlowArgs(spect.data_ptr(), B, T, _engine._ptr(len32), int(spect.dtype == torch.float16),
+                                    float(sigma), _engine._ptr(zt), seed, audio.data_ptr(), ws.data_ptr(), ws.numel())
 
     def infer(self, module, spect, sigma, lengths, z):
         self.ensure(module)
         spect = self._spect(spect, "WaveGlow.infer")
         dev = self.device
         B, T = int(spect.shape[0]), int(spect.shape[2])
-        L = _capi.lib()
         audio = torch.empty(B, HOP * T, device=dev, dtype=spect.dtype)
         len32 = None
         if lengths is not None:
-            len32 = torch.as_tensor(lengths).to(device=dev, dtype=torch.int32).contiguous()
+            len32 = _engine._i32(torch.as_tensor(lengths), dev)
             if tuple(len32.shape) != (B,):
                 raise ValueError("WaveGlow.infer: lengths must have shape (%d,)" % B)
         zt = None
@@ -315,68 +274,43 @@ class _WaveGlowEngine:
             if tuple(zt.shape) != (B, N_GROUP, 32 * T):
                 raise ValueError("waveglow_noise: z must be (%d, %d, %d), got %s" % (B, N_GROUP, 32 * T, tuple(z.shape)))
         a = self._args(spect, len32, zt, sigma, self._draw_seed(), audio)
-        with torch.cuda.device(dev):
-            _capi.check(L.t2_waveglow_infer(self.handle, C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        self._call(_capi.lib().t2_waveglow_infer, C.byref(a))
         return audio
 
     def infer_window(self, spect, len32, zt, z_frames, sigma, seed, frame0, out0, out1, at_end):
         """Audio (B, 256 (out1 - out0)) of the window-relative frames [out0, out1) of spect, which holds the frames
         [frame0, frame0 + T) of a sequence (t2_waveglow_infer_window).  Call ensure() first."""
-        B = int(spect.shape[0])
-        audio = torch.empty(B, HOP * (out1 - out0), device=self.device, dtype=spect.dtype)
-        w = _capi.T2WaveGlowWindowArgs()
-        w.wg = self._args(spect, len32, zt, sigma, seed, audio)
-        w.frame0, w.out0, w.out1, w.at_end = frame0, out0, out1, int(at_end)
-        w.z_frames = z_frames if zt is not None else 0
-        with torch.cuda.device(self.device):
-            _capi.check(_capi.lib().t2_waveglow_infer_window(
-                self.handle, C.byref(w), C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)))
+        audio = torch.empty(int(spect.shape[0]), HOP * (out1 - out0), device=self.device, dtype=spect.dtype)
+        w = _capi.T2WaveGlowWindowArgs(self._args(spect, len32, zt, sigma, seed, audio), frame0, out0, out1,
+                                       z_frames if zt is not None else 0, int(at_end))
+        self._call(_capi.lib().t2_waveglow_infer_window, C.byref(w))
         return audio
 
     @torch.no_grad()
     def stream(self, module, items, sigma, z):
         """The generator behind WaveGlow.infer_stream."""
-        left, right = window_halo()
-        kept = zt = z_frames = seed = None
-        base = held = a0 = 0           # kept: the final mel frames [base, held); audio of frames [0, a0) is handed out
+        win = FinalWindow("WaveGlow.infer_stream: mel items", "frames", 2, *window_halo())
+        zt = z_frames = seed = None
         for item in items:
-            f0, f1 = item["frames"]
-            post, finished = item["mel_outputs_postnet"], bool(item["finished"])
-            if f0 != held:
-                raise ValueError("WaveGlow.infer_stream: mel items must be consecutive (frames %s after %d)" % ((f0, f1), held))
-            if kept is None:           # the first item: weights, the noise seed (one draw, as infer)
+            win.check(item)
+            post = item["mel_outputs_postnet"]
+            if win.kept is None:       # the first item: weights, the noise seed (one draw, as infer)
                 self.ensure(module)
-                kept = self._spect(post, "WaveGlow.infer_stream")
-                B = int(kept.shape[0])
+                post = self._spect(post, "WaveGlow.infer_stream")
                 if z is not None:
-                    zt, z_frames = self._z(z, B, f1)
+                    zt, z_frames = self._z(z, int(post.shape[0]), item["frames"][1])
                 seed = self._draw_seed()
-            else:
-                kept = torch.cat((kept, post.to(kept.dtype)), 2)
-            held = f1
-            # audio of frame t is final once the mel frames up to t + right are (or the mel stream has ended)
-            a1 = held if finished else max(a0, held - right)
-            if a1 == a0 and not finished:
+            span = win.add(item, post)
+            if span is None:
                 continue
-            lengths = item["mel_lengths"]
-            audio = kept.new_empty(B, 0)
-            if a1 > a0:
-                # the window is every kept frame: [max(0, a0 - left), held)
-                w0, w1 = base, held
-                # window-relative lengths on the device: live rows (-1) run past the window, stopped rows end inside it
-                # or after it
-                win_len = torch.where(lengths < 0, torch.full_like(lengths, w1 - w0),
-                                      (lengths - w0).clamp(min=0, max=w1 - w0)).to(torch.int32).contiguous()
-                audio = self.infer_window(kept.contiguous(), win_len, zt, z_frames, sigma, seed, w0, a0 - w0, a1 - w0,
-                                          finished)
-            yield dict(samples=(HOP * a0, HOP * a1), audio=audio, mel_lengths=lengths, finished=finished)
-            a0 = a1
+            (a0, a1), finished, kept = span, bool(item["finished"]), win.kept
+            audio = kept.new_empty(kept.shape[0], 0)
+            if a1 > a0:                # the window is every kept frame; a row that does not end in it ends at its end
+                audio = self.infer_window(kept.contiguous(), win.lengths(item["mel_lengths"], win.held - win.base), zt,
+                                          z_frames, sigma, seed, win.base, a0 - win.base, a1 - win.base, finished)
+            yield dict(samples=(HOP * a0, HOP * a1), audio=audio, mel_lengths=item["mel_lengths"], finished=finished)
             if finished:
                 return
-            # later windows start at a0 - left: drop the frames before it, so the stream holds at most the two halos
-            # and one item's frames whatever max_decoder_steps is
-            drop = max(0, a0 - left) - base
-            kept, base = kept[:, :, drop:], base + drop
 
 
 def window_halo():

@@ -2,7 +2,11 @@
 They only *hold* parameters (``linear_layer.weight``, ``conv.weight`` ... are the state_dict keys the
 published checkpoints use); the arithmetic of the hot path is done by libt2b200.so.
 TacotronSTFT (layers.py:42-80): the log-mel extraction of the data path, on the GPU through ``t2_mel_spectrogram``."""
+import ctypes as C
+
 import torch
+
+from . import _capi
 
 
 class LinearNorm(torch.nn.Module):
@@ -85,7 +89,7 @@ class TacotronSTFT(torch.nn.Module):
         self.filter_length, self.hop_length, self.win_length = filter_length, hop_length, win_length
         self.register_buffer("mel_basis", _slaney_mel_filterbank(sampling_rate, filter_length, n_mel_channels, mel_fmin, mel_fmax))
         self.register_buffer("forward_basis", _windowed_fourier_basis(filter_length, win_length))
-        self._ws = None
+        self._ws = _capi.Workspace()
 
     def spectral_normalize(self, magnitudes):
         return torch.log(torch.clamp(magnitudes, min=1e-5))             # audio_processing.py:78-84, C = 1
@@ -95,8 +99,6 @@ class TacotronSTFT(torch.nn.Module):
 
     def mel_spectrogram(self, y):
         """y (B, T) in [-1, 1] -> (B, n_mel_channels, T // hop_length + 1)."""
-        import ctypes as C
-        from . import _capi
         if not y.is_cuda or not self.mel_basis.is_cuda:
             raise RuntimeError("tacotron2_b200.TacotronSTFT: CUDA tensors only (move the module and the audio to the GPU)")
         assert torch.min(y.data) >= -1                                  # layers.py:74-75
@@ -106,15 +108,10 @@ class TacotronSTFT(torch.nn.Module):
         B, n = int(y32.shape[0]), int(y32.shape[1])
         frames = int(L.t2_mel_spectrogram_frames(n, self.hop_length))
         out = torch.empty(B, self.n_mel_channels, frames, device=y.device, dtype=torch.float32)
-        nbytes = int(L.t2_mel_spectrogram_workspace_bytes(B, n, self.filter_length, self.hop_length, self.n_mel_channels))
-        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != y.device:
-            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
-        a = _capi.T2MelSpecArgs()
-        a.y, a.B, a.n_samples = y32.data_ptr(), B, n
-        a.filter_length, a.hop_length, a.n_mel = self.filter_length, self.hop_length, self.n_mel_channels
-        a.forward_basis, a.mel_basis = self.forward_basis.data_ptr(), self.mel_basis.data_ptr()
-        a.clip_val, a.mel = 1e-5, out.data_ptr()
-        a.ws, a.ws_bytes = self._ws.data_ptr(), self._ws.numel()
-        with torch.cuda.device(y.device):
-            _capi.check(L.t2_mel_spectrogram(C.byref(a), C.c_void_p(torch.cuda.current_stream(y.device).cuda_stream)))
+        ws = self._ws.get("mel", L.t2_mel_spectrogram_workspace_bytes(B, n, self.filter_length, self.hop_length,
+                                                                       self.n_mel_channels), y.device)
+        a = _capi.T2MelSpecArgs(y32.data_ptr(), B, n, self.filter_length, self.hop_length, self.n_mel_channels,
+                                self.forward_basis.data_ptr(), self.mel_basis.data_ptr(), 1e-5, out.data_ptr(),
+                                ws.data_ptr(), ws.numel())
+        _capi.call(L.t2_mel_spectrogram, y.device, C.byref(a))
         return out

@@ -24,16 +24,11 @@ class _FusedLossFn(torch.autograd.Function):
         need = [ctx.needs_input_grad[i] for i in range(3)]
         d = [torch.empty_like(x) if n else None for x, n in zip((mel_c, post_c, gate_c), need)]
         out = torch.empty(4, **f32)
-        ws = torch.empty(int(L.t2_loss_workspace_bytes()), dtype=torch.uint8, device=mel.device)
-        a = _capi.T2LossArgs()
-        a.mel, a.mel_post, a.gate = mel_c.data_ptr(), post_c.data_ptr(), gate_c.data_ptr()
-        a.mel_target, a.gate_target, a.output_lengths = tgt.data_ptr(), gt.data_ptr(), None
-        a.B, a.C, a.T = int(B), int(Cm), int(T)
-        a.loss = out.data_ptr()
-        a.d_mel, a.d_mel_post, a.d_gate = (x.data_ptr() if x is not None else None for x in d)
-        a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
-        with torch.cuda.device(mel.device):
-            _capi.check(L.t2_tacotron2_loss(C.byref(a), C.c_void_p(torch.cuda.current_stream(mel.device).cuda_stream)))
+        ws = _capi.byte_buffer(L.t2_loss_workspace_bytes(), mel.device)
+        a = _capi.T2LossArgs(mel_c.data_ptr(), post_c.data_ptr(), gate_c.data_ptr(), tgt.data_ptr(), gt.data_ptr(), None,
+                             int(B), int(Cm), int(T), out.data_ptr(), *(x.data_ptr() if x is not None else None for x in d),
+                             ws.data_ptr(), ws.numel())
+        _capi.call(L.t2_tacotron2_loss, mel.device, C.byref(a))
         ctx.seeds = d
         ctx.dtypes = (mel.dtype, post.dtype, gate.dtype)
         ctx.gate_shape = gate.shape

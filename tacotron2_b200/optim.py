@@ -18,7 +18,7 @@ from ._engine import bump_weights_generation
 class FusedClipAdam(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
-        self._ws = None
+        self._ws = _capi.Workspace()
 
     @torch.no_grad()
     def step(self, closure=None, max_norm=None):
@@ -45,45 +45,41 @@ class FusedClipAdam(torch.optim.Optimizer):
                 st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                 st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
         norm = torch.zeros((), device=dev, dtype=torch.float32)
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
         total = sum(p.numel() for p in all_p)
-        nbytes = L.t2_clip_adam_workspace_bytes(total, len(all_p))
-        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != dev:
-            self._ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+        ws = self._ws.get("adam", L.t2_clip_adam_workspace_bytes(total, len(all_p)), dev)
         first = True
-        with torch.cuda.device(dev):
-            for g, ps in groups:
-                if not ps:
-                    continue
-                # one group = one launch set; the clip coefficient is computed over ALL parameters (first launch set);
-                # further groups get max_norm = 0 after their gradients were pre-scaled -> keep it simple: single group
-                if not first:
-                    raise RuntimeError("FusedClipAdam: one param group only (train.py uses one)")
-                first = False
-                n = len(ps)
-                arr = lambda ts: (C.c_void_p * n)(*[t.data_ptr() for t in ts])
-                # "step" is a CPU scalar tensor here; checkpoints written by older torch.optim.Adam hold a Python int
-                steps = {int(float(self.state[p]["step"])) for p in ps}
-                if len(steps) != 1:
-                    raise RuntimeError("FusedClipAdam: parameters with different step counts %s (a parameter skipped "
-                                       "updates because its .grad was None); one bias correction per launch" % sorted(steps))
-                step = steps.pop() + 1
-                a = _capi.T2AdamArgs()
-                a.n = n
-                pa, ga = arr(ps), arr([p.grad for p in ps])
-                ma, va = arr([self.state[p]["exp_avg"] for p in ps]), arr([self.state[p]["exp_avg_sq"] for p in ps])
-                ne = (C.c_int64 * n)(*[p.numel() for p in ps])
-                a.params, a.grads, a.exp_avg, a.exp_avg_sq, a.numel = pa, ga, ma, va, ne
-                a.lr, (a.beta1, a.beta2) = float(g["lr"]), [float(b) for b in g["betas"]]
-                a.eps, a.weight_decay = float(g["eps"]), float(g["weight_decay"])
-                a.max_norm = float(max_norm) if max_norm else 0.0
-                a.step = step
-                a.grad_norm = norm.data_ptr()
-                a.ws, a.ws_bytes = self._ws.data_ptr(), self._ws.numel()
-                _capi.check(L.t2_clip_adam_step(C.byref(a), stream))
-                for p in ps:
-                    st = self.state[p]
-                    st["step"] = st["step"] + 1 if torch.is_tensor(st["step"]) else torch.tensor(float(st["step"]) + 1.0)
+        for g, ps in groups:
+            if not ps:
+                continue
+            # one group = one launch set; the clip coefficient is computed over ALL parameters (first launch set);
+            # further groups get max_norm = 0 after their gradients were pre-scaled -> keep it simple: single group
+            if not first:
+                raise RuntimeError("FusedClipAdam: one param group only (train.py uses one)")
+            first = False
+            n = len(ps)
+            arr = lambda ts: (C.c_void_p * n)(*[t.data_ptr() for t in ts])
+            # "step" is a CPU scalar tensor here; checkpoints written by older torch.optim.Adam hold a Python int
+            steps = {int(float(self.state[p]["step"])) for p in ps}
+            if len(steps) != 1:
+                raise RuntimeError("FusedClipAdam: parameters with different step counts %s (a parameter skipped "
+                                   "updates because its .grad was None); one bias correction per launch" % sorted(steps))
+            step = steps.pop() + 1
+            a = _capi.T2AdamArgs()
+            a.n = n
+            pa, ga = arr(ps), arr([p.grad for p in ps])
+            ma, va = arr([self.state[p]["exp_avg"] for p in ps]), arr([self.state[p]["exp_avg_sq"] for p in ps])
+            ne = (C.c_int64 * n)(*[p.numel() for p in ps])
+            a.params, a.grads, a.exp_avg, a.exp_avg_sq, a.numel = pa, ga, ma, va, ne
+            a.lr, (a.beta1, a.beta2) = float(g["lr"]), [float(b) for b in g["betas"]]
+            a.eps, a.weight_decay = float(g["eps"]), float(g["weight_decay"])
+            a.max_norm = float(max_norm) if max_norm else 0.0
+            a.step = step
+            a.grad_norm = norm.data_ptr()
+            a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
+            _capi.call(L.t2_clip_adam_step, dev, C.byref(a))
+            for p in ps:
+                st = self.state[p]
+                st["step"] = st["step"] + 1 if torch.is_tensor(st["step"]) else torch.tensor(float(st["step"]) + 1.0)
         bump_weights_generation()       # parameters changed underneath torch's version counters
         return norm
 
@@ -113,7 +109,7 @@ class AmpFusedClipAdam(torch.optim.Optimizer):
         self._init_scale = float(init_scale)
         self._dev_state = None          # device floats: [loss scale, good steps, optimizer steps taken, last step skipped]
         self._skipped = None
-        self._ws = None
+        self._ws = _capi.Workspace()
 
     def _state_tensor(self, dev):
         if self._dev_state is None or self._dev_state.device != dev:
@@ -186,13 +182,9 @@ class AmpFusedClipAdam(torch.optim.Optimizer):
         a.growth_interval, a.growth_factor, a.backoff_factor = self.growth_interval, self.growth_factor, self.backoff_factor
         norm = torch.zeros((), device=dev, dtype=torch.float32)
         a.state, a.grad_norm, a.skipped = state.data_ptr(), norm.data_ptr(), self._skipped.data_ptr()
-        total = sum(p.numel() for p in ps)
-        nbytes = L.t2_amp_adam_workspace_bytes(total, n)
-        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != dev:
-            self._ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
-        a.ws, a.ws_bytes = self._ws.data_ptr(), self._ws.numel()
-        with torch.cuda.device(dev):
-            _capi.check(L.t2_amp_adam_step(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        ws = self._ws.get("adam", L.t2_amp_adam_workspace_bytes(sum(p.numel() for p in ps), n), dev)
+        a.ws, a.ws_bytes = ws.data_ptr(), ws.numel()
+        _capi.call(L.t2_amp_adam_step, dev, C.byref(a))
         bump_weights_generation()
         return norm
 

@@ -278,6 +278,27 @@ def test_stays_inside_exact_size_buffers(windowed):
     assert torch.equal(o.view(torch.float32).view(B, -1), ref)
 
 
+def test_invalidate_weights_refreshes_the_denoiser(monkeypatch):
+    """tacotron2_b200.invalidate_weights() makes the Denoiser re-pack its bases on its next call, as it does every other
+    engine; the output keeps its bits."""
+    den = t2.Denoiser(vocoder())
+    y = stft_inputs(22, 256 * 16 + 30).cuda()
+    before = den(y, strength=0.1)
+    L, refreshed = _capi.lib(), []
+    real = L.t2_denoiser_refresh
+
+    def refresh(*args):
+        refreshed.append(args[0])
+        return real(*args)
+    monkeypatch.setattr(L, "t2_denoiser_refresh", refresh)
+    again = den(y, strength=0.1)
+    assert refreshed == []                       # same bases, same key: nothing to re-pack
+    t2.invalidate_weights()
+    after = den(y, strength=0.1)
+    assert len(refreshed) == 1
+    assert torch.equal(again, before) and torch.equal(after, before)
+
+
 def test_mode_normal_builds_and_denoises():
     torch.manual_seed(18)
     den = t2.Denoiser(vocoder(), mode='normal')
