@@ -358,7 +358,6 @@ int t2_prenet_forward(T2Model* m, const float* frames, int32_t M, const uint8_t*
 size_t t2_postnet_workspace_bytes(const T2Model*, int32_t B, int32_t T) { return postnet_ws_bytes(B, T); }
 int t2_postnet_forward(T2Model* m, const T2PostnetArgs* a, void* stream) {
   if (!m || !a || !a->mel || !a->mel_post || !a->ws) return fail(T2_ERR_INVALID, "postnet: null argument");
-  if (a->stash) return postnet_forward_train(m, a, (cudaStream_t)stream);
   return postnet_forward(m, a, (cudaStream_t)stream, false);
 }
 

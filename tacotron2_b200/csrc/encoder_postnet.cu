@@ -1,122 +1,11 @@
-// Encoder (model.py:149-201) and Postnet (model.py:103-146): v0 implementation on the fp32 SIMT
-// GEMM engine with channels-last activations (conv1d == GEMM over K = taps x Cin).
-#include <stdlib.h>
-
+// Encoder (model.py:149-201) and Postnet (model.py:103-146) forwards: the evaluation-mode conv stacks on the tensor-core
+// conv engine, the training-mode ones handed to train_layers.cu, and the encoder BiLSTM.
 #include "conv_tc.h"
 #include "gemm_f32.cuh"
 #include "train_layers.h"
 #include "model.h"
 
 namespace t2 {
-
-// ---- small kernels ----------------------------------------------------------------------------
-__global__ void embed_kernel(const int64_t* __restrict__ text, const float* __restrict__ emb,
-                             float* __restrict__ out, int rows, int n_symbols) {
-  const int r = blockIdx.x;
-  if (r >= rows) return;
-  long id = text[r];
-  if (id < 0) id = 0;
-  if (id >= n_symbols) id = n_symbols - 1;
-  const float4* src = reinterpret_cast<const float4*>(emb + id * kEnc);
-  float4* dst = reinterpret_cast<float4*>(out + (long)r * kEnc);
-  for (int i = threadIdx.x; i < kEnc / 4; i += blockDim.x) dst[i] = src[i];
-}
-
-// eval-mode BatchNorm folded to y = x*scale + shift                    (model.py:118, 165)
-__global__ void bn_fold_kernel(const float* g, const float* b, const float* mean, const float* var,
-                               float eps, float* scale, float* shift, int C) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const float s = g[c] / sqrtf(var[c] + eps);
-  scale[c] = s;
-  shift[c] = b[c] - mean[c] * s;
-}
-
-// training-mode BatchNorm statistics over M rows (biased variance, padded positions included,
-// as the reference does) + running-stat update with momentum 0.1 (unbiased variance).
-__global__ void __launch_bounds__(256)
-bn_batch_stats_kernel(const float* __restrict__ x, int M, int C, const float* g, const float* b,
-                      float eps, float* scale, float* shift, float* run_mean, float* run_var) {
-  __shared__ float red[8][33];
-  const int cl = threadIdx.x & 31, rg = threadIdx.x >> 5;
-  const int c = blockIdx.x * 32 + cl;
-  float s = 0.f;
-  if (c < C) for (int r = rg; r < M; r += 8) s += x[(long)r * C + c];
-  red[rg][cl] = s;
-  __syncthreads();
-  float mean = 0.f;
-  for (int i = 0; i < 8; ++i) mean += red[i][cl];
-  mean /= (float)M;
-  __syncthreads();
-  float q = 0.f;
-  if (c < C) for (int r = rg; r < M; r += 8) { const float d = x[(long)r * C + c] - mean; q = fmaf(d, d, q); }
-  red[rg][cl] = q;
-  __syncthreads();
-  if (rg == 0 && c < C) {
-    float var = 0.f;
-    for (int i = 0; i < 8; ++i) var += red[i][cl];
-    var /= (float)M;
-    const float sc = g[c] / sqrtf(var + eps);
-    scale[c] = sc;
-    shift[c] = b[c] - mean * sc;
-    if (run_mean) {
-      run_mean[c] = 0.9f * run_mean[c] + 0.1f * mean;
-      run_var[c] = 0.9f * run_var[c] + 0.1f * var * ((float)M / (float)(M > 1 ? M - 1 : 1));
-    }
-  }
-}
-
-// y = act(x*scale + shift) with optional dropout; in place on (M, C)
-__global__ void bn_apply_kernel(float* x, long n, int C, const float* scale, const float* shift,
-                                int act, const uint8_t* keep, long keep_ld_t, int T, int philox,
-                                uint64_t seed, uint32_t site, float p_drop) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int c = (int)(i % C);
-  float v = x[i] * scale[c] + shift[c];
-  if (act == ACT_RELU) v = fmaxf(v, 0.f);
-  else if (act == ACT_TANH) v = tanhf(v);
-  if (keep) {   // reference-layout mask (B, C, T): row m = b*T + t
-    const long mrow = i / C; const long b = mrow / T, t = mrow % T;
-    v = keep[(b * C + c) * (long)T + t] ? v * (1.f / (1.f - p_drop)) : 0.f;
-  } else if (philox) {
-    v = philox_keep(seed, site, (uint64_t)i, p_drop) ? v * (1.f / (1.f - p_drop)) : 0.f;
-  }
-  x[i] = v;
-}
-
-__global__ void mask_rows_kernel(const float* __restrict__ in, long in_batch_stride, float* __restrict__ out,
-                                 const int32_t* __restrict__ len, int B, int T, int C) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long)B * T * C) return;
-  const long row = i / C; const int b = (int)(row / T), t = (int)(row % T);
-  const int c = (int)(i - row * C);
-  out[i] = (len == nullptr || t < len[b]) ? in[(long)b * in_batch_stride + (long)t * C + c] : 0.f;
-}
-
-// frames t >= len[b] of channels-last rows (B, T, C) set to zero, in place
-__global__ void zero_past_len_kernel(float* x, const int32_t* __restrict__ len, int B, int T, int C) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long)B * T * C) return;
-  const long row = i / C;
-  const int b = (int)(row / T), t = (int)(row % T);
-  if (t >= len[b]) x[i] = 0.f;
-}
-
-// (B*T, C) channels-last -> (B, C, T) with optional residual and length mask (training-mode tail of
-// the postnet; the eval path fuses this into the last conv's epilogue)
-__global__ void transpose_residual_kernel(const float* __restrict__ y, const float* __restrict__ R,
-                                          const int32_t* __restrict__ len, float* __restrict__ out,
-                                          int B, int T, int C) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long)B * T * C) return;
-  const int t = (int)(i % T); const long r = i / T; const int c = (int)(r % C); const int b = (int)(r / C);
-  const long m = (long)b * T + t;
-  float v = y[m * C + c];
-  if (R) v += R[m * C + c];
-  if (len && t >= len[b]) v = 0.f;
-  out[i] = v;
-}
 
 // One time step of both directions of the encoder BiLSTM (model.py:169-171, 180-188).
 // grid (16 unit blocks, 2 directions, batch chunks of 64); 256 threads = 64 rows x 4 unit groups.
@@ -282,62 +171,31 @@ enc_lstm_persistent_kernel(const float* __restrict__ gin, const float* __restric
 }
 
 // ---- host side ----------------------------------------------------------------------------------
-static bool use_tc() { const char* e = getenv("T2_CONV_IMPL"); return !(e && e[0] == 's'); }   // "simt" selects the fp32 SIMT path
-
+// Two conv paths: evaluation-mode forwards without a stash run on the tensor-core inference convs (conv_tc.cu); every
+// training-mode forward and every forward under autograd (a stash) runs on the training conv stack (train_layers.cu).
+// A call runs one of them, so the inference planes and the training stack share their bytes of the workspace.
 struct EncoderWs {
-  float *x0, *x1;          // (B, T, 512) activations of the fp32 conv path
   float* gin;              // (B, T, 2048) LSTM input projections, forward | reverse
   float* h;                // (2, 2, B, 256): two h buffers (read / write) of both directions
   float* c;                // (2, B, 256)
   float *scale, *shift;    // (2048) folded BatchNorm / bias
   EncLstmCtrl* lctrl;
   __half *pl0, *pl1;       // tensor-core activation planes
+  void* train;             // the training conv stack without a stash (on the planes' bytes)
 };
 static void encoder_ws_layout(Carve& c, int B, int T, EncoderWs* w) {
-  w->x0 = c.take<float>((size_t)B * T * kEnc); w->x1 = c.take<float>((size_t)B * T * kEnc);
   w->gin = c.take<float>((size_t)B * T * 8 * kEncH);
   w->h = c.take<float>((size_t)2 * 2 * B * kEncH);
   w->c = c.take<float>((size_t)2 * B * kEncH);
   w->scale = c.take<float>(8 * kEncH); w->shift = c.take<float>(8 * kEncH);
   w->lctrl = c.take<EncLstmCtrl>(1);
-  w->pl0 = c.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
-  w->pl1 = c.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
+  Carve planes = c;
+  w->pl0 = planes.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
+  w->pl1 = planes.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
+  w->train = c.take<char>(encoder_convs_train_ws_bytes(B, T));
+  if (planes.off > c.off) c.off = planes.off;
 }
 size_t encoder_ws_bytes(int B, int T) { Carve c(nullptr); EncoderWs w; encoder_ws_layout(c, B, T, &w); return c.bytes(); }
-
-static int conv_bn_layer(T2Model* m, const float* x, float* y, int B, int T, int cin, int cout,
-                         const float* wpk, int wbase, int act, int training, const uint8_t* keep,
-                         uint64_t seed, uint32_t site, float* scale, float* shift,
-                         int out_transposed, const float* R, const int32_t* row_len,
-                         cudaStream_t s) {
-  // wbase: index of conv.weight in the state_dict table (conv.bias, bn.weight, bn.bias,
-  // running_mean, running_var follow)
-  const float* cbias = m->w[wbase + 1];
-  GemmArgs g;
-  g.seg[0] = {x, cin, wpk, (long)kConvK * cin, kConvK * cin};
-  g.M = B * T; g.N = cout; g.C = y; g.ldc = cout; g.bias = cbias;
-  g.conv_T = T; g.conv_cin = cin; g.conv_pad = (kConvK - 1) / 2;
-  if (!training) {
-    bn_fold_kernel<<<(cout + 127) / 128, 128, 0, s>>>(m->w[wbase + 2], m->w[wbase + 3], m->w[wbase + 4],
-                                                      m->w[wbase + 5], m->cfg.bn_eps, scale, shift, cout);
-    T2_LAUNCH_CHECK();
-    g.scale = scale; g.shift = shift; g.act = act;
-    g.out_transposed = out_transposed; g.R = R; g.ldr = cout; g.row_len = row_len;
-    return gemm_f32(g, s);
-  }
-  // training: raw conv -> batch statistics -> normalise + activation + dropout
-  if (out_transposed) return fail(T2_ERR_UNSUPPORTED, "training-mode final postnet layer uses the generic path");
-  T2_TRY(gemm_f32(g, s));
-  bn_batch_stats_kernel<<<(cout + 31) / 32, 256, 0, s>>>(
-      y, B * T, cout, m->w[wbase + 2], m->w[wbase + 3], m->cfg.bn_eps, scale, shift,
-      const_cast<float*>(m->w[wbase + 4]), const_cast<float*>(m->w[wbase + 5]));
-  T2_LAUNCH_CHECK();
-  const long n = (long)B * T * cout;
-  bn_apply_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(y, n, cout, scale, shift, act, keep, T, T,
-                                                              keep ? 0 : 1, seed, site, 0.5f);
-  T2_LAUNCH_CHECK();
-  return T2_OK;
-}
 
 // per_row (t2_encoder_infer): each row b is encoded as its first lengths[b] symbols alone -- the inputs at t >= lengths[b]
 // and every conv layer's outputs there are zero, the padding the row has at T = lengths[b].  Otherwise lengths only
@@ -347,22 +205,24 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per
   const int B = a->B, T = a->T;
   if (B <= 0 || T <= 0) return fail(T2_ERR_INVALID, "encoder: empty batch");
   if (a->ws_bytes < encoder_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder workspace too small");
+  const bool persistent = B <= 64 && m->sm_count >= 128;      // the BiLSTM as one cooperative launch
+  if (a->stash && !persistent)
+    return fail(T2_ERR_UNSUPPORTED, "encoder: the training stash needs B <= 64 and >= 128 SMs (persistent BiLSTM kernel)");
   Carve cv(a->ws);
   EncoderWs w;
   encoder_ws_layout(cv, B, T, &w);
-  const bool tc = use_tc() && !a->training && !a->stash;
   float* st_gates = nullptr; float* st_c = nullptr;
   const int32_t* conv_len = per_row ? a->lengths : nullptr;
 
-  if (a->stash) {
-    // autograd path: fp32 conv stack with the activations kept for the backward pass (train_layers.cu)
+  if (a->training || a->stash) {
+    // training conv stack (fp32), then W_ih x + b_ih + b_hh for every time step and both directions
     const float* xl = nullptr;
-    T2_TRY(encoder_convs_train(m, a, s, &xl, &st_gates, &st_c));
+    T2_TRY(encoder_convs_train(m, a, w.train, s, &xl, &st_gates, &st_c));
     GemmArgs g;
     g.seg[0] = {xl, kEnc, m->enc_lstm_wih, kEnc, kEnc};
     g.M = B * T; g.N = 8 * kEncH; g.C = w.gin; g.ldc = 8 * kEncH; g.bias = m->enc_lstm_b;
     T2_TRY(gemm_f32(g, s));
-  } else if (tc) {
+  } else {
     // tensor-core path: planes -> 3 x (conv k5 + folded BN + ReLU) -> LSTM input projection (fp32 rows)
     if (a->embedded) T2_TRY(tc_rows_to_planes(a->embedded, (long)T * kEnc, kEnc, kEnc, conv_len, B, T, w.pl0, s));
     else T2_TRY(tc_embed_to_planes(a->text, m->w[W_EMB], m->cfg.n_symbols, conv_len, B, T, w.pl0, s));
@@ -381,40 +241,11 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per
     c.in = cur; c.cin_pad = kEnc; c.wimg = m->tc_enc_wih; c.taps = 1; c.B = B; c.T = T; c.cout = 8 * kEncH; c.nt_rows = 128;
     c.scale = w.scale; c.shift = w.shift; c.act = 0; c.out_mode = 1; c.out_f32 = w.gin; c.ldo = 8 * kEncH;
     T2_TRY(tc_conv(c, s));
-  } else {
-    if (a->embedded) {
-      T2_CUDA(cudaMemcpyAsync(w.x0, a->embedded, (size_t)B * T * kEnc * 4, cudaMemcpyDeviceToDevice, s));
-    } else {
-      embed_kernel<<<B * T, 128, 0, s>>>(a->text, m->w[W_EMB], w.x0, B * T, m->cfg.n_symbols);   // model.py:503/518
-      T2_LAUNCH_CHECK();
-    }
-    const long n_rows = (long)B * T * kEnc;
-    auto zero_padding = [&](float* x) -> int {      // per_row: frames t >= lengths[b] of x become zero (in place)
-      if (!conv_len) return T2_OK;
-      zero_past_len_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, s>>>(x, conv_len, B, T, kEnc);
-      T2_LAUNCH_CHECK();
-      return T2_OK;
-    };
-    T2_TRY(zero_padding(w.x0));
-    float* cur = w.x0; float* nxt = w.x1;
-    for (int i = 0; i < 3; ++i) {                                                             // model.py:174-175
-      const uint8_t* keep = (a->training && a->keep) ? a->keep + (size_t)i * B * kEnc * T : nullptr;
-      T2_TRY(conv_bn_layer(m, cur, nxt, B, T, kEnc, kEnc, m->enc_conv_w[i], W_ENC_CONV0 + 7 * i, ACT_RELU,
-                           a->training, keep, a->seed, 1000 + i, w.scale, w.shift, 0, nullptr, nullptr, s));
-      T2_TRY(zero_padding(nxt));
-      float* tmp = cur; cur = nxt; nxt = tmp;
-    }
-    {  // W_ih x + b_ih + b_hh for every time step and both directions
-      GemmArgs g;
-      g.seg[0] = {cur, kEnc, m->enc_lstm_wih, kEnc, kEnc};
-      g.M = B * T; g.N = 8 * kEncH; g.C = w.gin; g.ldc = 8 * kEncH; g.bias = m->enc_lstm_b;
-      T2_TRY(gemm_f32(g, s));
-    }
   }
   float* hin = w.h; float* hout = w.h + (size_t)2 * B * kEncH;
   T2_CUDA(cudaMemsetAsync(hin, 0, (size_t)2 * B * kEncH * 4, s));
   T2_CUDA(cudaMemsetAsync(w.c, 0, (size_t)2 * B * kEncH * 4, s));
-  if (B <= 64 && m->sm_count >= 128) {
+  if (persistent) {
     // persistent recurrence: one cooperative launch for all T steps of both directions
     T2_CUDA(cudaMemsetAsync(hout, 0, (size_t)2 * B * kEncH * 4, s));
     T2_CUDA(cudaMemsetAsync(w.lctrl, 0, sizeof(EncLstmCtrl), s));
@@ -430,7 +261,6 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per
     if (a->stash) T2_TRY(encoder_stash_output(a, s));
     return T2_OK;
   }
-  if (a->stash) return fail(T2_ERR_UNSUPPORTED, "encoder: the training stash needs B <= 64 (persistent BiLSTM kernel)");
   const size_t smem = (64 * kEncH + 64 * (kEncH + 1)) * sizeof(float);
   T2_CUDA(cudaFuncSetAttribute(enc_lstm_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   for (int step = 0; step < T; ++step) {
@@ -443,17 +273,17 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per
 }
 
 struct PostnetWs {
-  float *y0, *y1;          // (B, T, 512) activations of the fp32 conv path
-  float* xin;              // (B, T, 80) masked input rows
   float *scale, *shift;    // (512) folded BatchNorm
   __half *pl0, *pl1;       // tensor-core activation planes
+  void* train;             // the training conv stack without a stash (on the planes' bytes)
 };
 static void postnet_ws_layout(Carve& c, int B, int T, PostnetWs* w) {
-  w->y0 = c.take<float>((size_t)B * T * kPost); w->y1 = c.take<float>((size_t)B * T * kPost);
-  w->xin = c.take<float>((size_t)B * T * kMel);
   w->scale = c.take<float>(kPost); w->shift = c.take<float>(kPost);
-  w->pl0 = c.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
-  w->pl1 = c.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
+  Carve planes = c;
+  w->pl0 = planes.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
+  w->pl1 = planes.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
+  w->train = c.take<char>(postnet_forward_train_ws_bytes(B, T));
+  if (planes.off > c.off) c.off = planes.off;
 }
 size_t postnet_ws_bytes(int B, int T) { Carve c(nullptr); PostnetWs w; postnet_ws_layout(c, B, T, &w); return c.bytes(); }
 
@@ -468,56 +298,22 @@ int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s, bool per
   Carve cv(a->ws);
   PostnetWs w;
   postnet_ws_layout(cv, B, T, &w);
-  if (use_tc() && !a->training) {
-    // tensor-core path (model.py:141-146 + residual :511/:524): mel -> planes -> 4 x (conv+BN+tanh) -> conv+BN (+mel)
-    const long bs = a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel;
-    T2_TRY(tc_rows_to_planes(a->mel, bs, kMel, 128, a->lengths, B, T, w.pl0, s));
-    __half* cur = w.pl0; __half* nxt = w.pl1;
-    for (int i = 0; i < 5; ++i) {
-      const int wb = W_POST_CONV0 + 7 * i;
-      const int cout = i == 4 ? kMel : kPost;
-      T2_TRY(tc_fold_bn(m->w[wb + 1], m->w[wb + 2], m->w[wb + 3], m->w[wb + 4], m->w[wb + 5], m->cfg.bn_eps, w.scale, w.shift, cout, s));
-      TcConvArgs c; memset(&c, 0, sizeof(c));
-      c.in = cur; c.cin_pad = i == 0 ? 128 : kPost; c.wimg = m->tc_post_conv[i]; c.taps = kConvK; c.B = B; c.T = T;
-      c.cout = cout; c.nt_rows = i == 4 ? 80 : 128; c.scale = w.scale; c.shift = w.shift; c.act = i == 4 ? 0 : 2;
-      if (i < 4) { c.out_mode = 0; c.out_planes = nxt; c.row_len = layer_len; }
-      else { c.out_mode = 2; c.out_f32 = a->mel_post; c.residual = a->add_residual ? a->mel : nullptr; c.res_batch_stride = bs; c.row_len = a->lengths; }
-      T2_TRY(tc_conv(c, s));
-      __half* tmp = cur; cur = nxt; nxt = tmp;
-    }
-    return T2_OK;
-  }
-  const long n_in = (long)B * T * kMel;
-  mask_rows_kernel<<<(unsigned)((n_in + 255) / 256), 256, 0, s>>>(
-      a->mel, a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel, w.xin, a->lengths, B, T, kMel);
-  T2_LAUNCH_CHECK();
-  const float* cur = w.xin; float* nxt = w.y0;
-  for (int i = 0; i < 5; ++i) {                                      // model.py:141-146
-    const int cin = i == 0 ? kMel : kPost, cout = i == 4 ? kMel : kPost;
-    const bool last = i == 4;
-    const uint8_t* keep = nullptr;
-    if (a->training && a->keep) keep = a->keep + (i < 4 ? (size_t)i * B * kPost * T : (size_t)4 * B * kPost * T);   // [(B,512,T)]*4 + (B,80,T)
-    if (last && !a->training) {
-      T2_TRY(conv_bn_layer(m, cur, a->mel_post, B, T, cin, cout, m->post_conv_w[i], W_POST_CONV0 + 7 * i,
-                           ACT_NONE, 0, nullptr, 0, 0, w.scale, w.shift, 1, a->add_residual ? w.xin : nullptr, a->lengths, s));
-    } else {
-      T2_TRY(conv_bn_layer(m, cur, nxt, B, T, cin, cout, m->post_conv_w[i], W_POST_CONV0 + 7 * i,
-                           last ? ACT_NONE : ACT_TANH, a->training, keep, a->seed, 2000 + i, w.scale, w.shift, 0,
-                           nullptr, nullptr, s));
-      if (layer_len && !last) {
-        const long n = (long)B * T * cout;
-        zero_past_len_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(nxt, layer_len, B, T, cout);
-        T2_LAUNCH_CHECK();
-      }
-      if (last) {   // training-mode last layer: separate transpose + residual
-        const long n = (long)B * T * kMel;
-        transpose_residual_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(
-            nxt, a->add_residual ? w.xin : nullptr, a->lengths, a->mel_post, B, T, kMel);
-        T2_LAUNCH_CHECK();
-        return T2_OK;
-      }
-      cur = nxt; nxt = (nxt == w.y0) ? w.y1 : w.y0;
-    }
+  if (a->training || a->stash) return postnet_forward_train(m, a, w.train, s);
+  // tensor-core path (model.py:141-146 + residual :511/:524): mel -> planes -> 4 x (conv+BN+tanh) -> conv+BN (+mel)
+  const long bs = a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel;
+  T2_TRY(tc_rows_to_planes(a->mel, bs, kMel, 128, a->lengths, B, T, w.pl0, s));
+  __half* cur = w.pl0; __half* nxt = w.pl1;
+  for (int i = 0; i < 5; ++i) {
+    const int wb = W_POST_CONV0 + 7 * i;
+    const int cout = i == 4 ? kMel : kPost;
+    T2_TRY(tc_fold_bn(m->w[wb + 1], m->w[wb + 2], m->w[wb + 3], m->w[wb + 4], m->w[wb + 5], m->cfg.bn_eps, w.scale, w.shift, cout, s));
+    TcConvArgs c; memset(&c, 0, sizeof(c));
+    c.in = cur; c.cin_pad = i == 0 ? 128 : kPost; c.wimg = m->tc_post_conv[i]; c.taps = kConvK; c.B = B; c.T = T;
+    c.cout = cout; c.nt_rows = i == 4 ? 80 : 128; c.scale = w.scale; c.shift = w.shift; c.act = i == 4 ? 0 : 2;
+    if (i < 4) { c.out_mode = 0; c.out_planes = nxt; c.row_len = layer_len; }
+    else { c.out_mode = 2; c.out_f32 = a->mel_post; c.residual = a->add_residual ? a->mel : nullptr; c.res_batch_stride = bs; c.row_len = a->lengths; }
+    T2_TRY(tc_conv(c, s));
+    __half* tmp = cur; cur = nxt; nxt = tmp;
   }
   return T2_OK;
 }

@@ -3,7 +3,6 @@
 
 namespace t2 {
 
-template <bool CONV>
 __global__ void __launch_bounds__(256) gemm_f32_kernel(const GemmArgs a) {
   if (a.skip_flag != nullptr && *a.skip_flag != 0) return;
   __shared__ __align__(16) float As[16][64 + 4];
@@ -20,24 +19,12 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(const GemmArgs a) {
 
   const int am = m0 + lrow;
   const int wn = n0 + lrow;
-  int conv_t = 0;
-  if (CONV) conv_t = am % a.conv_T;
 
   for (int s = 0; s < a.nseg; ++s) {
     const GemmSeg sg = a.seg[s];
     for (int k0 = 0; k0 < sg.K; k0 += 16) {
       float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (am < a.M) {
-        if (CONV) {
-          const int tap = k0 / a.conv_cin;
-          const int ci = k0 - tap * a.conv_cin + lk;
-          const int ts = conv_t + tap - a.conv_pad;
-          if (ts >= 0 && ts < a.conv_T)
-            av = *reinterpret_cast<const float4*>(sg.A + (long)(am + tap - a.conv_pad) * sg.lda + ci);
-        } else {
-          av = *reinterpret_cast<const float4*>(sg.A + (long)am * sg.lda + k0 + lk);
-        }
-      }
+      if (am < a.M) av = *reinterpret_cast<const float4*>(sg.A + (long)am * sg.lda + k0 + lk);
       float4 wv = make_float4(0.f, 0.f, 0.f, 0.f);
       if (wn < a.N) wv = *reinterpret_cast<const float4*>(sg.W + (long)wn * sg.ldw + k0 + lk);
       As[lk + 0][lrow] = av.x; As[lk + 1][lrow] = av.y; As[lk + 2][lrow] = av.z; As[lk + 3][lrow] = av.w;
@@ -69,19 +56,11 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(const GemmArgs a) {
       if (n >= a.N) continue;
       float v = acc[i][j];
       if (a.bias) v += a.bias[n];
-      if (a.scale) v = v * a.scale[n] + a.shift[n];
       if (a.act == ACT_RELU) v = fmaxf(v, 0.f);
       else if (a.act == ACT_TANH) v = tanhf(v);
       if (a.keep) v = a.keep[(long)m * a.ldkeep + n] ? v * inv_keep : 0.f;
       else if (a.philox) v = philox_keep(a.seed, a.site, (uint64_t)m * a.N + n, a.p_drop) ? v * inv_keep : 0.f;
-      if (a.out_transposed) {
-        const int b = m / a.conv_T, t = m - b * a.conv_T;
-        if (a.R) v += a.R[(long)m * a.ldr + n];
-        if (a.row_len && t >= a.row_len[b]) v = 0.f;
-        a.C[((long)b * a.N + n) * a.conv_T + t] = v;
-      } else {
-        a.C[(long)m * a.ldc + n] = v;
-      }
+      a.C[(long)m * a.ldc + n] = v;
     }
   }
 }
@@ -92,10 +71,7 @@ int gemm_f32(const GemmArgs& a, cudaStream_t s) {
     if (a.seg[i].K % 16 != 0 || (a.seg[i].lda & 3) || (a.seg[i].ldw & 3))
       return fail(T2_ERR_INVALID, "gemm_f32: K %% 16 / ld %% 4 violated (seg %d: K=%d)", i, a.seg[i].K);
   dim3 grid((a.N + 63) / 64, (a.M + 63) / 64);
-  if (a.conv_T > 0 && a.conv_cin > 0)
-    gemm_f32_kernel<true><<<grid, 256, 0, s>>>(a);
-  else
-    gemm_f32_kernel<false><<<grid, 256, 0, s>>>(a);
+  gemm_f32_kernel<<<grid, 256, 0, s>>>(a);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }

@@ -1,13 +1,13 @@
-// fp32 SIMT GEMM  C = epilogue( sum_s A_s (M x K_s) * W_s (N x K_s)^T )  -- the bring-up /
-// cross-check engine (T2_IMPL_STEPWISE, encoder/postnet v0).  Up to 3 K-segments avoid
-// materialising torch.cat() of the reference (model.py:352, 366-367, 373-374).
+// fp32 SIMT GEMM  C = epilogue( sum_s A_s (M x K_s) * W_s (N x K_s)^T )  -- the stepwise decoder (T2_IMPL_STEPWISE), the
+// decoders' processed memory, the prenet forward / backward and the encoder's LSTM input projection behind the training
+// conv stack.  Up to 3 K-segments avoid materialising torch.cat() of the reference (model.py:352, 366-367, 373-374).
 #pragma once
 #include "common.cuh"
 
 namespace t2 {
 
 struct GemmSeg {
-  const float* A; long lda;   // (M, K) row-major (conv mode: (B*T, Cin) channels-last)
+  const float* A; long lda;   // (M, K) row-major
   const float* W; long ldw;   // (N, K) row-major
   int K;                      // multiple of 16
 };
@@ -20,18 +20,10 @@ struct GemmArgs {
   int M = 0, N = 0;
   float* C = nullptr; long ldc = 0;
   const float* bias = nullptr;    // (N) added to the accumulator
-  const float* scale = nullptr;   // (N) y = (acc + bias) * scale + shift   (folded BatchNorm)
-  const float* shift = nullptr;   // (N)
   int act = ACT_NONE;
   // dropout on the output: explicit keep mask (M, N) uint8 or Philox(seed, site); p = drop prob
   const uint8_t* keep = nullptr; long ldkeep = 0;
   int philox = 0; uint64_t seed = 0; uint32_t site = 0; float p_drop = 0.f;
-  // conv1d mode (seg[0] only): rows are (b, t), T rows per sequence, K = taps * Cin and
-  // W is [N][tap][Cin]; the A row of tap j is row (t + j - pad) of the same sequence or zeros.
-  int conv_T = 0, conv_cin = 0, conv_pad = 0;
-  // output mode 1: C is (B, N, T) (transposed per sequence) and R (M, ldr) is added (residual)
-  int out_transposed = 0; const float* R = nullptr; long ldr = 0;
-  const int32_t* row_len = nullptr;  // out mode 1: zero the output where t >= row_len[b]
   const int* skip_flag = nullptr;    // device flag: when *skip_flag != 0 the kernel is a no-op
 };
 

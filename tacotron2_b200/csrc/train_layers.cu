@@ -1,5 +1,6 @@
-// Training path of the Encoder (model.py:173-190) and the Postnet (model.py:141-146): forward with a stash and
-// the hand-derived backward.  fp32.
+// Training path of the Encoder (model.py:173-190) and the Postnet (model.py:141-146): the conv stacks of every
+// training-mode forward and every forward under autograd (with a stash for the backward pass or without one), and the
+// hand-derived backward.  fp32.
 //
 // Conv stacks: activations live in a "padded rows" layout -- sequence b occupies rows [b (T+4) + 2, b (T+4) + 2 + T)
 // of a (B (T+4), C) channels-last matrix, the 2 rows either side are zero -- so the k=5 convolution is the sum of 5
@@ -28,12 +29,14 @@ inline long prow(int b, int t, int T) { return (long)b * (T + 2 * kPadRows) + kP
 __device__ __forceinline__ long d_prow(int b, int t, int T) { return (long)b * (T + 2 * kPadRows) + kPadRows + t; }
 
 // ---- layout conversion ---------------------------------------------------------------------------
-// rows (B, T, C) with batch stride -> padded rows (valid rows only; the buffer was zeroed)
-__global__ void rows_to_padded_kernel(const float* __restrict__ x, long batch_stride, float* __restrict__ xp, int B, int T, int C) {
+// rows (B, T, C) with batch stride -> padded rows (valid rows only; the buffer was zeroed).  len (B) or null: frames
+// t >= len[b] count as zero
+__global__ void rows_to_padded_kernel(const float* __restrict__ x, long batch_stride, const int32_t* __restrict__ len,
+                                      float* __restrict__ xp, int B, int T, int C) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long)B * T * C) return;
   const int c = (int)(i % C); const long r = i / C; const int t = (int)(r % T); const int b = (int)(r / T);
-  xp[d_prow(b, t, T) * C + c] = x[(long)b * batch_stride + (long)t * C + c];
+  xp[d_prow(b, t, T) * C + c] = (len == nullptr || t < len[b]) ? x[(long)b * batch_stride + (long)t * C + c] : 0.f;
 }
 __global__ void embed_to_padded_kernel(const int64_t* __restrict__ text, const float* __restrict__ emb, float* __restrict__ xp,
                                        int B, int T, int n_symbols) {
@@ -202,14 +205,16 @@ __global__ void fill1_kernel(float* p, float v, long n) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
 }
-// (B*T, C) plain or padded rows (valid) -> (B, C, T) with optional residual
-__global__ void rows_to_bct_kernel(const float* __restrict__ yp, const float* __restrict__ res_p, float* __restrict__ out, int B, int T, int C) {
+// padded rows (valid) -> (B, C, T) with optional residual; len (B) or null: zero at t >= len[b]
+__global__ void rows_to_bct_kernel(const float* __restrict__ yp, const float* __restrict__ res_p, const int32_t* __restrict__ len,
+                                   float* __restrict__ out, int B, int T, int C) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long)B * T * C) return;
   const int t = (int)(i % T); const long r = i / T; const int c = (int)(r % C); const int b = (int)(r / C);
   const long pr = d_prow(b, t, T);
   float v = yp[pr * C + c];
   if (res_p) v += res_p[pr * C + c];
+  if (len && t >= len[b]) v = 0.f;
   out[i] = v;
 }
 // gradient (B, C, T) -> plain rows (B*T, C)
@@ -482,6 +487,22 @@ void stack_layout(Carve& c, int B, int T, int L, const int* ch, StackStash* st) 
   for (int l = 0; l < L; ++l) st->z[l] = c.take<float>(Mp * ch[l + 1]);
   for (int l = 0; l < L; ++l) st->stats[l] = c.take<float>((size_t)(2 + kRedSplit) * ch[l + 1]);   // + reduction scratch
 }
+// The same stack without a stash (a training-mode forward outside autograd), laid out on the caller's workspace.  Nothing
+// is kept for a backward pass: two padded buffers take turns as the layers' inputs and outputs, and one z / statistics
+// region serves every layer.  keep_input: the input gets a buffer of its own (the postnet adds it back as the residual).
+// The activation buffers come first, z and the statistics last.
+void stack_ws_layout(Carve& c, int B, int T, int L, const int* ch, bool keep_input, StackStash* st) {
+  const size_t Mp = (size_t)B * (T + 2 * kPadRows);
+  int cmax = 0;
+  for (int l = 0; l <= L; ++l) cmax = ch[l] > cmax ? ch[l] : cmax;
+  memset(st, 0, sizeof(*st));
+  float* in = keep_input ? c.take<float>(Mp * ch[0]) : nullptr;
+  float* buf[2] = {c.take<float>(Mp * cmax), c.take<float>(Mp * cmax)};
+  for (int l = 0; l <= L; ++l) st->x[l] = (l == 0 && in) ? in : buf[l & 1];
+  float* z = c.take<float>(Mp * cmax);
+  float* stats = c.take<float>((size_t)(2 + kRedSplit) * cmax);
+  for (int l = 0; l < L; ++l) { st->z[l] = z; st->stats[l] = stats; }
+}
 const int kPostCh[6] = {kMel, kPost, kPost, kPost, kPost, kMel};
 const int kEncCh[4] = {kEnc, kEnc, kEnc, kEnc};
 
@@ -605,6 +626,12 @@ __global__ void enc_hprev_kernel(const float* __restrict__ mem, float* __restric
 // Postnet
 // ---------------------------------------------------------------------------------------------------
 size_t postnet_stash_bytes(int B, int T) { Carve c(nullptr); StackStash st; stack_layout(c, B, T, 5, kPostCh, &st); return c.bytes(); }
+size_t postnet_forward_train_ws_bytes(int B, int T) {
+  Carve c(nullptr);
+  StackStash st;
+  stack_ws_layout(c, B, T, 5, kPostCh, true, &st);
+  return c.bytes();
+}
 
 static void post_layers(T2Model* m, int training, const uint8_t* keep, int B, int T, ConvLayer* L) {
   for (int i = 0; i < 5; ++i) {
@@ -615,24 +642,31 @@ static void post_layers(T2Model* m, int training, const uint8_t* keep, int B, in
   }
 }
 
-int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, cudaStream_t s) {
+int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, void* ws, cudaStream_t s) {
   const int B = a->B, T = a->T;
-  if (a->lengths) return fail(T2_ERR_UNSUPPORTED, "postnet: the training stash path takes no length mask (model.py:510)");
-  if (a->stash_bytes < postnet_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet stash too small");
+  if (a->stash && a->lengths) return fail(T2_ERR_UNSUPPORTED, "postnet: the training stash path takes no length mask (model.py:510)");
+  if (a->stash && a->stash_bytes < postnet_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet stash too small");
   StackStash st;
-  Carve c(a->stash);
-  stack_layout(c, B, T, 5, kPostCh, &st);
-  T2_CUDA(cudaMemsetAsync(st.x[0], 0, c.off, s));      // zero pad rows everywhere
+  if (a->stash) {
+    Carve c(a->stash);
+    stack_layout(c, B, T, 5, kPostCh, &st);
+    T2_CUDA(cudaMemsetAsync(st.x[0], 0, c.off, s));      // zero pad rows everywhere
+  } else {
+    Carve c(ws);
+    stack_ws_layout(c, B, T, 5, kPostCh, true, &st);
+    T2_CUDA(cudaMemsetAsync(st.x[0], 0, (char*)st.z[0] - (char*)st.x[0], s));   // the activations, pad rows included
+  }
   const long n = (long)B * T * kMel;
   rows_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->mel, a->mel_batch_stride ? a->mel_batch_stride : (long)T * kMel,
-                                                                     st.x[0], B, T, kMel);
+                                                                     a->lengths, st.x[0], B, T, kMel);
   T2_LAUNCH_CHECK();
   ConvLayer L[5];
   post_layers(m, a->training, a->keep, B, T, L);
   for (int i = 0; i < 5; ++i)
     T2_TRY(conv_fwd(m, L[i], B, T, a->training, a->seed, st.x[i], st.z[i], st.stats[i], st.x[i + 1], nullptr, a->training != 0,
                     st.stats[i] + 2 * L[i].cout, s));
-  rows_to_bct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.x[5], a->add_residual ? st.x[0] : nullptr, a->mel_post, B, T, kMel);
+  rows_to_bct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.x[5], a->add_residual ? st.x[0] : nullptr, a->lengths, a->mel_post,
+                                                                  B, T, kMel);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }
@@ -714,22 +748,44 @@ static void enc_layers(T2Model* m, int training, const uint8_t* keep, int B, int
   }
 }
 
-// conv stack of the training forward: fills the stash and returns the LSTM input rows (B*T, 512)
-int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, const float** xl, float** gates, float** cst) {
+size_t encoder_convs_train_ws_bytes(int B, int T) {
+  Carve c(nullptr);
+  StackStash st;
+  stack_ws_layout(c, B, T, 3, kEncCh, false, &st);
+  return c.bytes();
+}
+
+// conv stack of the training forward: returns the LSTM input rows (B*T, 512).  With a stash it fills the stash and
+// returns where the BiLSTM keeps its gates / cell states; without one it runs on ws and *gates = *cst = null.
+int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, void* ws, cudaStream_t s, const float** xl, float** gates, float** cst) {
   const int B = a->B, T = a->T;
-  if (a->stash_bytes < encoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder stash too small");
-  const EncStash st = enc_stash(a->stash, B, T);
-  T2_CUDA(cudaMemsetAsync(st.cs.x[0], 0, (char*)st.xl - (char*)st.cs.x[0], s));   // the conv stack, pad rows included
+  if (a->stash && a->stash_bytes < encoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder stash too small");
+  StackStash cs;
+  float* rows;     // the last layer's output as plain rows
+  if (a->stash) {
+    const EncStash st = enc_stash(a->stash, B, T);
+    cs = st.cs;
+    T2_CUDA(cudaMemsetAsync(cs.x[0], 0, (char*)st.xl - (char*)cs.x[0], s));   // the conv stack, pad rows included
+    rows = st.xl; *gates = st.gates; *cst = st.cst;
+  } else {
+    Carve c(ws);
+    stack_ws_layout(c, B, T, 3, kEncCh, false, &cs);
+    T2_CUDA(cudaMemsetAsync(cs.x[0], 0, (char*)cs.z[0] - (char*)cs.x[0], s));   // the activations, pad rows included
+    rows = cs.x[3]; *gates = nullptr; *cst = nullptr;   // nothing reads x[3] as padded rows: it holds the plain ones
+  }
   const long n = (long)B * T * kEnc;
-  if (a->embedded) rows_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->embedded, (long)T * kEnc, st.cs.x[0], B, T, kEnc);
-  else embed_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->text, m->w[W_EMB], st.cs.x[0], B, T, m->cfg.n_symbols);
+  if (a->embedded)
+    rows_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->embedded, (long)T * kEnc, nullptr, cs.x[0], B, T, kEnc);
+  else embed_to_padded_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->text, m->w[W_EMB], cs.x[0], B, T, m->cfg.n_symbols);
   T2_LAUNCH_CHECK();
   ConvLayer L[3];
   enc_layers(m, a->training, a->keep, B, T, L);
-  for (int i = 0; i < 3; ++i)
-    T2_TRY(conv_fwd(m, L[i], B, T, a->training, a->seed, st.cs.x[i], st.cs.z[i], st.cs.stats[i], st.cs.x[i + 1], i == 2 ? st.xl : nullptr,
-                    a->training != 0, st.cs.stats[i] + 2 * L[i].cout, s));
-  *xl = st.xl; *gates = st.gates; *cst = st.cst;
+  for (int i = 0; i < 3; ++i) {
+    float* yp = (i == 2 && !a->stash) ? nullptr : cs.x[i + 1];
+    T2_TRY(conv_fwd(m, L[i], B, T, a->training, a->seed, cs.x[i], cs.z[i], cs.stats[i], yp, i == 2 ? rows : nullptr,
+                    a->training != 0, cs.stats[i] + 2 * L[i].cout, s));
+  }
+  *xl = rows;
   return T2_OK;
 }
 // after the LSTM ran: keep a copy of the output for the backward pass

@@ -348,8 +348,9 @@ def _train_step(sd, text, tl, ol, mels, gt, masks=None):
 @gpu
 @pytest.mark.parametrize("training", [False, True])
 def test_teacher_forced_forward_without_grad_philox_equals_rebuilt_masks(training, seed_log):
-    """Under no_grad the encoder and postnet take the no-stash path (bn_apply_kernel) rather than the autograd stash path;
-    in eval mode only the prenet dropout is active."""
+    """In training mode under no_grad the encoder and postnet run the training conv stack without a stash (its
+    bn_act_kernel draws the dropout masks) rather than with the autograd stash; in eval mode only the prenet dropout is
+    active."""
     sd, text, tl, ol, mels, gt = _ragged_case(8, 30, 20, seed=9)
     outs = []
     for masks in (None, "rebuilt"):

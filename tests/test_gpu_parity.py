@@ -92,28 +92,37 @@ def test_teacher_forced_forward_matches_reference_golden(name, training, impl, i
         assert rel_err(sd_after["encoder.convolutions.0.1.running_var"], torch.from_numpy(g["bn0_running_var"])) < 1e-4
 
 
-@pytest.mark.parametrize("conv_impl", ["tc", "simt"])
+@pytest.mark.parametrize("conv_path", ["tc", "train"])
 @pytest.mark.parametrize("B,T", [(5, 33), (12, 140)])
-def test_encoder_and_postnet_modules_vs_oracle(B, T, conv_impl, monkeypatch):
-    """Encoder (conv stack + packed BiLSTM) and Postnet as stand-alone modules; both conv engines
-    (wgmma implicit GEMM and the fp32 SIMT path)."""
-    monkeypatch.setenv("T2_CONV_IMPL", conv_impl)
+def test_encoder_and_postnet_modules_vs_oracle(B, T, conv_path):
+    """Encoder (conv stack + packed BiLSTM) and Postnet as stand-alone modules on both conv paths: tc = evaluation mode
+    (wgmma implicit-GEMM convs); train = training mode without autograd (the training conv stack: batch statistics and
+    injected dropout masks)."""
+    training = conv_path == "train"
     sd = synth_state_dict(9, scale=1.5)
-    model = make_model(sd)
+    model = make_model(sd, training=training)
     g = torch.Generator().manual_seed(0)
     text = rand_text(B, T, 2)
     lengths = torch.sort(torch.randint(1, T + 1, (B,), generator=g), descending=True)[0]
     lengths[0] = T; lengths[-1] = 1
     emb = sd["embedding.weight"][text].transpose(1, 2)
+    x = torch.randn(max(B // 2, 1), 80, T + 8, generator=g)
+    enc_keep = post_keep = None
+    if training:
+        enc_keep = keep_mask((3, B, 512, T), 0.5, 10)
+        post_keep = [keep_mask((x.shape[0], 512, x.shape[2]), 0.5, 11 + i) for i in range(4)] + \
+                    [keep_mask((x.shape[0], 80, x.shape[2]), 0.5, 15)]
     with torch.no_grad():
-        ref_inf = O.encoder(sd, emb, None)
-        ref_fwd = O.encoder(sd, emb, lengths)
-        got_inf = model.encoder.inference(emb.cuda())
-        got_fwd = model.encoder(emb.cuda(), lengths.cuda())
+        ref_inf = O.encoder(sd, emb, None, training, enc_keep)
+        ref_fwd = O.encoder(sd, emb, lengths, training, enc_keep)
+        with t2.dropout_masks(enc=enc_keep):
+            got_inf = model.encoder.inference(emb.cuda())
+            got_fwd = model.encoder(emb.cuda(), lengths.cuda())
         assert rel_err(got_inf, ref_inf) < 1e-4 and rel_err(got_fwd, ref_fwd) < 1e-4
         assert float(got_fwd[-1, 1:].abs().max()) == 0.0                       # zeros at padded positions
-        x = torch.randn(max(B // 2, 1), 80, T + 8, generator=g)
-        assert rel_err(model.postnet(x.cuda()), O.postnet(sd, x)) < 1e-4
+        with t2.dropout_masks(post=post_keep):
+            got_post = model.postnet(x.cuda())
+        assert rel_err(got_post, O.postnet(sd, x, training, post_keep)) < 1e-4
 
 
 @pytest.mark.parametrize("impl,impl_name", IMPLS)

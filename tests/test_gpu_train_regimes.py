@@ -1,5 +1,5 @@
 """The training backward across gradient scales, zero-gradient channels, its K-split regimes and the inference conv tiles,
-against the oracle in float64.
+against the oracle in float64; the training-mode conv stack forward without autograd.
 
 Every gradient comes from three split-fp16 engines: gemm_tc (the LSTM products and the forward convs), wgrad_tc (the decoder
 LSTM and the conv weight gradients) and conv_tc (the conv input gradients).  Each scales its fp32 operands by powers of two
@@ -14,8 +14,8 @@ before splitting them into fp16 hi / lo halves, so:
   single-chunk last segments and on both sides of the switch.
 * conv_tc runs 128-row tiles of the padded rows, in clusters of 2 (an odd tile count adds a padding tile).
 
-Bars: 1e-3 relative (max |a - b| / max |b|) on gradients, as tests/test_gpu_backward.py; 1e-4 on the inference Encoder and
-Postnet outputs, as tests/test_gpu_parity.py.  Every case prints its worst error."""
+Bars: 1e-3 relative (max |a - b| / max |b|) on gradients, as tests/test_gpu_backward.py; 1e-4 on Encoder and Postnet
+outputs, as tests/test_gpu_parity.py.  Every case prints its worst error."""
 import contextlib
 import math
 
@@ -320,8 +320,7 @@ def test_conv_weight_gradient_k_splits_vs_fp64(module, B, T):
 # B (T + 4) padded rows in 128-row tiles, clusters of 2: (1, 124) one tile, (1, 125) one row past it, (2, 60) one tile,
 # (3, 81) and (64, 2) odd tile counts (+ the cluster's padding tile), (1, 1) a single frame
 @pytest.mark.parametrize("B,T", [(1, 1), (1, 124), (1, 125), (2, 60), (3, 81), (64, 2)])
-def test_inference_conv_tiles_vs_fp64(B, T, monkeypatch):
-    monkeypatch.setenv("T2_CONV_IMPL", "tc")
+def test_inference_conv_tiles_vs_fp64(B, T):
     sd = synth_state_dict(9, scale=1.5)         # the weights and embedded-text inputs of test_gpu_parity's module test
     model = engine_model(sd, False)
     emb = sd["embedding.weight"][rand_text(B, T, B * 1000 + T)].transpose(1, 2).contiguous()
@@ -336,6 +335,52 @@ def test_inference_conv_tiles_vs_fp64(B, T, monkeypatch):
     e_mem, e_post = rel_err(mem, ref_mem), rel_err(post, ref_post)
     print("inference convs B=%d T=%d: encoder %.2e, postnet %.2e" % (B, T, e_mem, e_post))
     assert e_mem < INFER_TOL and e_post < INFER_TOL
+
+
+# ---- training-mode forwards outside autograd ------------------------------------------------------------------------
+def training_forward(sd, module, x, lens, keep, grad):
+    """A training-mode <module>.forward on a fresh model, with or without autograd: its output and the BatchNorm running
+    statistics it left."""
+    mod = getattr(engine_model(sd, True), module)
+    masks = dict(enc=keep) if module == "encoder" else dict(post=keep)
+    with torch.set_grad_enabled(grad), t2.dropout_masks(**masks):
+        out = mod(x.cuda(), lens.cuda()) if module == "encoder" else mod(x.cuda())
+    torch.cuda.synchronize()
+    return out.detach(), {k: v.clone() for k, v in mod.state_dict().items() if "running" in k}
+
+
+@pytest.mark.parametrize("module,B,T", [("encoder", 5, 33), ("encoder", 64, 40), ("postnet", 3, 41), ("postnet", 2, 1)])
+def test_training_forward_without_autograd_equals_autograd_forward(module, B, T):
+    """Both run the training conv stack (under autograd with a stash for the backward pass), so the output and the updated
+    BatchNorm running statistics are the same bits.  Fresh models from one state dict, the same injected dropout masks."""
+    sd = weights()
+    x, lens, keep, _ = module_case(module, B, T, seed=B * 1000 + T)
+    out_ng, run_ng = training_forward(sd, module, x, lens, keep, False)
+    out_ag, run_ag = training_forward(sd, module, x, lens, keep, True)
+    assert torch.equal(out_ng, out_ag)
+    bad = [k for k in run_ng if not torch.equal(run_ng[k], run_ag[k])]
+    assert not bad, bad
+
+
+def test_training_postnet_with_lengths_vs_fp64():
+    """The training-mode postnet with per-row lengths, as Tacotron2.inference on a training-mode model runs it for B > 1:
+    input frames at t >= lengths[b] hold real values but count as zero, and the output there is zero.  The rows sit in a
+    wider buffer (batch stride > T * 80), like the decoder's output."""
+    B, T = 4, 37
+    sd = weights()
+    g = torch.Generator().manual_seed(5)
+    rows = torch.randn(B, T + 6, 80, generator=g).cuda()[:, :T]
+    lens = torch.tensor([T, 20, 1, 9], dtype=torch.int32)
+    keep = [keep_mask((B, 512, T), 0.5, 60 + i) for i in range(4)] + [keep_mask((B, 80, T), 0.5, 64)]
+    with torch.no_grad():
+        got = engine_model(sd, True)._t2_engine().postnet(rows, lens.cuda(), True, True, keep).cpu()
+    past = torch.arange(T)[None, :] >= lens[:, None].long()                    # (B, T)
+    x = rows.cpu().double().transpose(1, 2).masked_fill(past[:, None, :], 0.0)
+    ref = (O.postnet(to64(sd, "cpu"), x, True, keep) + x).masked_fill(past[:, None, :], 0.0)
+    err = rel_err(got, ref)
+    print("training postnet with lengths %s: %.2e" % (lens.tolist(), err))
+    assert err < INFER_TOL
+    assert not bool(got.masked_select(past[:, None, :]).any())
 
 
 # ---- C: shape changes on one model ----------------------------------------------------------------------------------
