@@ -95,11 +95,6 @@ int pack_model(T2Model* m, cudaStream_t s) {
   T2_CUDA(cudaMemcpyAsync(m->projgate_w + (size_t)kMel * kdc, m->w[W_GATE_W], (size_t)kdc * 4, cudaMemcpyDeviceToDevice, s));
   T2_CUDA(cudaMemcpyAsync(m->projgate_b, m->w[W_PROJ_B], kMel * 4, cudaMemcpyDeviceToDevice, s));
   T2_CUDA(cudaMemcpyAsync(m->projgate_b + kMel, m->w[W_GATE_B], 4, cudaMemcpyDeviceToDevice, s));
-  if (!m->ones) {
-    T2_TRY(dmalloc(&m->ones, (size_t)8192));
-    std::vector<float> h(8192, 1.f);
-    T2_CUDA(cudaMemcpy(m->ones, h.data(), 8192 * 4, cudaMemcpyHostToDevice));
-  }
   if (!m->zeros) {
     T2_TRY(dmalloc(&m->zeros, (size_t)8192));
     T2_CUDA(cudaMemsetAsync(m->zeros, 0, 8192 * 4, s));
@@ -229,7 +224,7 @@ int t2_model_destroy(T2Model* m) {
   for (int i = 0; i < 3; ++i) cudaFree(m->enc_conv_w[i]);
   for (int i = 0; i < 5; ++i) cudaFree(m->post_conv_w[i]);
   cudaFree(m->enc_lstm_wih); cudaFree(m->enc_lstm_b); cudaFree(m->arnn_b); cudaFree(m->drnn_b);
-  cudaFree(m->projgate_w); cudaFree(m->projgate_b); cudaFree(m->zeros); cudaFree(m->ones); cudaFree(m->dgrad_tmp);
+  cudaFree(m->projgate_w); cudaFree(m->projgate_b); cudaFree(m->zeros); cudaFree(m->dgrad_tmp);
   for (int i = 0; i < 3; ++i) cudaFree(m->tc_dgrad_enc[i]);
   for (int i = 0; i < 5; ++i) cudaFree(m->tc_dgrad_post[i]);
   for (int i = 0; i < 3; ++i) cudaFree(m->tc_enc_conv[i]);

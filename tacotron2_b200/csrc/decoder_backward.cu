@@ -3,15 +3,15 @@
 // checked against torch autograd through the oracle).
 //
 // Phase 1 (reverse time, 5 kernels per step; carries = gradients wrt the step-t states coming from t+1):
-//   KA lstm_bwd   : g_dh = carry + W_P^T [d_mel_t ; d_gate_t]  -> dropout mask -> LSTMCell backward  -> dG_dec[t], g_dc
-//   KB skinny_nn  : [g_ah | g_ctx | g_dh'] partials = dG_dec[t] . [W_ih^d | W_hh^d]        (model.py:366-369)
-//   KC attention  : g_ctx total -> g_aw -> softmax backward -> g_s = g_e v (1 - tanh^2) -> g_q, g_pm (stashed),
-//                   location layer backward -> carries for aw_{t-1}, awc_{t-1}            (model.py:43-86)
-//   KD lstm_bwd   : g_ah = carry + dG_dec part + g_q W_q -> mask -> LSTMCell backward      -> dG_att[t], g_ac
-//   KE skinny_nn  : [g_x2 | g_ctx' | g_ah'] partials = dG_att[t] . [W_ih^a | W_hh^a]      (model.py:352-354)
-// Phase 2 (time batched, on the tensor-core GEMMs gemm_tc / wgrad_tc): every weight gradient is dG^T . X over all
+//   KA lstm_bwd_row : g_dh = carry + W_P^T [d_mel_t ; d_gate_t]  -> dropout mask -> LSTMCell backward -> dG_dec[t], g_dc
+//   KB bwd_gemm_run : [g_ah | g_ctx | g_dh'] partials = dG_dec[t] . [W_ih^d | W_hh^d]      (model.py:366-369)
+//   KC attention    : g_ctx total -> g_aw -> softmax backward -> g_s = g_e v (1 - tanh^2) -> g_q, g_pm (stashed),
+//                     location layer backward -> carries for aw_{t-1}, awc_{t-1}          (model.py:43-86)
+//   KD lstm_bwd_row : g_ah = carry + dG_dec part + g_q W_q -> mask -> LSTMCell backward    -> dG_att[t], g_ac
+//   KE bwd_gemm_run : [g_x2 | g_ctx' | g_ah'] partials = dG_att[t] . [W_ih^a | W_hh^a]    (model.py:352-354)
+// KB / KE are the wgmma split-fp16 skinny GEMM: kBwdGemmSplit partial sums over the reduction, summed by the consumer.
+// Phase 2 (time batched, on the tensor-core GEMMs wgrad_tc / gemm_tc): every weight gradient is dG^T . X over all
 // T x B rows; d_memory = d_pm W_m + sum_t aw_t (x) g_ctx_t.
-#include <stdlib.h>
 #include <string.h>
 
 #include "decoder.h"
@@ -24,9 +24,6 @@ namespace t2 {
 
 namespace {
 
-constexpr int kSplitB = 7;       // reduction splits of the skinny GEMMs (partials summed by the consumer):
-constexpr int kSplitE = 10;      // 20 x 7 = 14 x 10 = 140 CTAs = one wave of one CTA per SM
-constexpr int kSplitMax = 10;
 constexpr int kPBld = 1536 + 1024;   // [g_ah (1024) | g_ctx (512) | g_dh' (1024)]
 constexpr int kPEld = 768 + 1024;    // [g_x2 (256) | g_ctx' (512) | g_ah' (1024)]
 constexpr int kTaps = 2 * kLocK;     // 62 taps of the fused location filter
@@ -39,7 +36,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// LSTMCell backward for one step (KA / KD).  grid (1024 / 256, B), block 256: thread = one hidden unit.
+// LSTMCell backward for one step (KA / KD).  grid B, block 1024: block = one batch row, thread = one hidden unit.
 // ---------------------------------------------------------------------------------------------
 struct LstmBwdArgs {
   // g_h = sum over sources of sum_s src[(s * 64 + b) * ld + off + unit]  +  sum_o vec[b][o] * Wv[o][unit]
@@ -54,54 +51,12 @@ struct LstmBwdArgs {
   const float* c; const float* c_prev;     // (B, 1024)
   float* g_c;                              // (B, 1024) carry, in/out
   float* dG;                               // (B, 4096) out
-  uint8_t* img; float* inv_scale;          // tensor-core path: scaled split-fp16 operand image of dG + 1/scale per row
+  uint8_t* img; float* inv_scale;          // scaled split-fp16 operand image of dG + 1/scale per row
 };
 
-__global__ void __launch_bounds__(256) lstm_bwd_kernel(const LstmBwdArgs a) {
-  __shared__ float s_vec[128];
-  const int b = blockIdx.y, unit = blockIdx.x * 256 + threadIdx.x;
-  for (int i = threadIdx.x; i < a.nvec; i += 256) s_vec[i] = a.vec[(long)b * a.ldvec + i];
-  __syncthreads();
-  float g_h = a.add ? a.add[(long)b * a.ldadd + unit] : 0.f;
-  if (a.src0) {
-#pragma unroll 5
-    for (int s = 0; s < a.ns0; ++s) g_h += a.src0[((long)s * 64 + b) * a.ld0 + a.off0 + unit];
-  }
-  if (a.src1) {
-#pragma unroll 5
-    for (int s = 0; s < a.ns1; ++s) g_h += a.src1[((long)s * 64 + b) * a.ld1 + a.off1 + unit];
-  }
-  {
-    float p4[4] = {0.f, 0.f, 0.f, 0.f};     // nvec is a multiple of 4 (0 or 128)
-#pragma unroll 4
-    for (int o = 0; o < a.nvec; o += 4) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) p4[i] = fmaf(s_vec[o + i], __ldg(a.Wv + (long)(o + i) * a.ldwv + unit), p4[i]);
-    }
-    g_h += (p4[0] + p4[1]) + (p4[2] + p4[3]);
-  }
-  if (a.dropout) {
-    const long idx = (long)b * 1024 + unit;
-    const bool keep = a.keep ? a.keep[idx] != 0 : philox_keep(a.seed, a.site, (uint64_t)idx, a.p);
-    g_h = keep ? g_h * (1.f / (1.f - a.p)) : 0.f;
-  }
-  const float* gp = a.gates + (long)b * 4096 + unit;
-  const float gi = gp[0], gf = gp[1024], gg = gp[2048], go = gp[3072];
-  const float c = a.c[(long)b * 1024 + unit], cp = a.c_prev[(long)b * 1024 + unit];
-  const float tc = tanhf(c);
-  const float d_o = g_h * tc;
-  const float d_c = a.g_c[(long)b * 1024 + unit] + g_h * go * (1.f - tc * tc);
-  float* dg = a.dG + (long)b * 4096 + unit;
-  dg[0] = d_c * gg * gi * (1.f - gi);
-  dg[1024] = d_c * cp * gf * (1.f - gf);
-  dg[2048] = d_c * gi * (1.f - gg * gg);
-  dg[3072] = d_o * go * (1.f - go);
-  a.g_c[(long)b * 1024 + unit] = d_c * gf;
-}
-
-// Same computation with one block per batch row (1024 threads = hidden units): the block knows the row maximum of
-// dG, scales the row by a power of two into [0.5, 1) and writes it as the split-fp16 operand image of the
-// tensor-core GEMM (gradients span many orders of magnitude; fp16 does not) next to the fp32 copy.
+// The block knows the row maximum of dG, scales the row by a power of two into [0.5, 1) and writes it as the
+// split-fp16 operand image of the tensor-core GEMM (gradients span many orders of magnitude; fp16 does not) next to
+// the fp32 copy.
 __global__ void __launch_bounds__(1024) lstm_bwd_row_kernel(const LstmBwdArgs a) {
   __shared__ float s_vec[128];
   __shared__ float s_max[32];
@@ -170,84 +125,6 @@ __global__ void __launch_bounds__(1024) lstm_bwd_row_kernel(const LstmBwdArgs a)
     const uint32_t eo = img_elem_offset(b, k & 63);
     hi[eo] = h; lo[eo] = l;
   }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Skinny "NN" GEMM (KB / KE): P[s][m][col] = sum_{n in split s} A[m][n] * W[n][col], m < 64.
-// The output columns are the concatenation of up to two weight matrices (row-major, N x ncols each).
-// grid (total_cols / 128, kSplit), block 256, tile 64 x 128, 8 x 4 outputs per thread.
-// ---------------------------------------------------------------------------------------------
-struct SkinnyArgs {
-  const float* A; int lda; int rows; int nred;
-  const float* W0; int ldw0; int cols0;
-  const float* W1; int ldw1; int cols1;
-  float* P; int ldp;
-  int nsplit;                               // gridDim.y; the nred / 32 chunks are divided as evenly as possible
-};
-
-__global__ void __launch_bounds__(256) skinny_nn_kernel(const SkinnyArgs a) {
-  constexpr int BK = 32;
-  __shared__ __align__(16) float As[BK][64 + 4];
-  __shared__ __align__(16) float Bs[BK][128];
-  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
-  const int tiles0 = a.cols0 >> 7;
-  const int ct = blockIdx.x;
-  const float* W; int ldw; int col_out;
-  if (ct < tiles0) { W = a.W0 + ct * 128; ldw = a.ldw0; col_out = ct * 128; }
-  else { W = a.W1 + (ct - tiles0) * 128; ldw = a.ldw1; col_out = ct * 128; }
-  const int nchunks = a.nred / BK;
-  const int n_begin = (int)((long)blockIdx.y * nchunks / a.nsplit) * BK;
-  const int n_end = (int)((long)(blockIdx.y + 1) * nchunks / a.nsplit) * BK;
-  float acc[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  float4 ra[2], rb[4];
-  auto load = [&](int n0) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int idx = tid * 2 + i, r = idx >> 3, q = idx & 7;
-      ra[i] = r < a.rows ? *reinterpret_cast<const float4*>(a.A + (long)r * a.lda + n0 + q * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int idx = tid + i * 256, kk = idx >> 5, c4 = idx & 31;
-      rb[i] = __ldg(reinterpret_cast<const float4*>(W + (long)(n0 + kk) * ldw + c4 * 4));
-    }
-  };
-  load(n_begin);
-  for (int n0 = n_begin; n0 < n_end; n0 += BK) {
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int idx = tid * 2 + i, r = idx >> 3, q = idx & 7;
-      As[q * 4 + 0][r] = ra[i].x; As[q * 4 + 1][r] = ra[i].y; As[q * 4 + 2][r] = ra[i].z; As[q * 4 + 3][r] = ra[i].w;
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int idx = tid + i * 256, kk = idx >> 5, c4 = idx & 31;
-      *reinterpret_cast<float4*>(&Bs[kk][c4 * 4]) = rb[i];
-    }
-    __syncthreads();
-    if (n0 + BK < n_end) load(n0 + BK);
-#pragma unroll
-    for (int kk = 0; kk < BK; ++kk) {
-      const float4 a0 = *reinterpret_cast<const float4*>(&As[kk][ty * 8]);
-      const float4 a1 = *reinterpret_cast<const float4*>(&As[kk][ty * 8 + 4]);
-      const float4 b = *reinterpret_cast<const float4*>(&Bs[kk][tx * 4]);
-      const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-      const float bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-    }
-  }
-  float* out = a.P + ((long)blockIdx.y * 64 + ty * 8) * a.ldp + col_out + tx * 4;
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-    *reinterpret_cast<float4*>(out + (long)i * a.ldp) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -539,8 +416,8 @@ __global__ void prenet_dz_kernel(const float* g, const float* __restrict__ act, 
 }
 
 struct BwdWs {
-  float *dga, *dgd, *q, *dq, *awc, *pm, *dpm, *dctx, *dy, *gs, *cols, *pb, *pe, *gdc, *gac, *cacc, *gcat, *dv, *ones, *weff,
-      *dweff, *tmp, *gproj, *weffT, *inv_scale;
+  float *dga, *dgd, *q, *dq, *awc, *pm, *dpm, *dctx, *dy, *gs, *cols, *pb, *pe, *gdc, *gac, *cacc, *gcat, *dv, *weff, *dweff,
+      *tmp, *gproj, *weffT, *inv_scale;
   uint8_t *img_d, *img_a; DecoderCtrl* ctrl;
   WgradWs wg;
 };
@@ -552,12 +429,10 @@ void bwd_ws_layout(Carve& c, int B, int Te, int T, BwdWs* w) {
   w->pm = c.take<float>((size_t)B * Te * 128); w->dpm = c.take<float>((size_t)B * Te * 128);
   w->dctx = c.take<float>(TB * 512); w->dy = c.take<float>(TB * 81);
   w->gs = c.take<float>(TB * Te * 128); w->cols = c.take<float>(TB * Te * kColsLd);
-  w->pb = c.take<float>((size_t)kSplitMax * 64 * kPBld); w->pe = c.take<float>((size_t)kSplitMax * 64 * kPEld);
+  w->pb = c.take<float>((size_t)kBwdGemmSplit * 64 * kPBld); w->pe = c.take<float>((size_t)kBwdGemmSplit * 64 * kPEld);
   w->gdc = c.take<float>((size_t)64 * 1024); w->gac = c.take<float>((size_t)64 * 1024);
   w->cacc = c.take<float>((size_t)2 * B * Te); w->gcat = c.take<float>((size_t)2 * 2 * B * 2 * Te);
   w->dv = c.take<float>((size_t)B * 128);
-  const size_t n_ones = TB > (size_t)B * Te ? TB : (size_t)B * Te;
-  w->ones = c.take<float>(n_ones);
   w->weff = c.take<float>((size_t)kAtt * kTaps); w->dweff = c.take<float>((size_t)kAtt * kColsLd);
   w->tmp = c.take<float>(4096);
   w->gproj = c.take<float>(TB * 1536); w->weffT = c.take<float>((size_t)kAtt * kTaps);
@@ -609,9 +484,6 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     T2_LAUNCH_CHECK();
     weff_kernel<<<(kAtt * kTaps + 255) / 256, 256, 0, s>>>(m->w[W_ATT_LOC_DENSE], m->w[W_ATT_LOC_CONV], w.weff, w.weffT);
     T2_LAUNCH_CHECK();
-    const size_t n_ones = TB > (size_t)B * Te ? TB : (size_t)B * Te;
-    fill_kernel<<<(unsigned)((n_ones + 255) / 256), 256, 0, s>>>(w.ones, 1.f, (long)n_ones);
-    T2_LAUNCH_CHECK();
   }
   // processed_memory (model.py:288) and the processed queries of all steps (model.py:57)
   T2_TRY(gemm_tc_rm(m, s, false, true, B * Te, kAtt, kEnc, a->memory, kEnc, m->w[W_ATT_MEMORY], kEnc, w.pm, kAtt, 0.f));
@@ -619,151 +491,65 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   // projection / gate contribution to g_dh and g_ctx of every step: [d_mel_t ; d_gate_t] . [W_proj ; W_gate]  (model.py:373-378)
   T2_TRY(gemm_tc_rm(m, s, false, false, (int)TB, kDRnn + kEnc, 81, w.dy, 81, m->projgate_w, kDRnn + kEnc, w.gproj, kDRnn + kEnc, 0.f));
   T2_CUDA(cudaFuncSetAttribute(att_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-
-  // T2_BWD_PROFILE=1: CUDA-event time per kernel class over the first 64 steps (stderr), for tuning
-  const bool prof = getenv("T2_BWD_PROFILE") != nullptr;
-  constexpr int kProfSteps = 64;
-  static cudaEvent_t pev[kProfSteps][6];
-  static bool pev_init = false;
-  if (prof && !pev_init) {
-    for (int i = 0; i < kProfSteps; ++i)
-      for (int j = 0; j < 6; ++j) cudaEventCreate(&pev[i][j]);
-    pev_init = true;
-  }
-  cudaEvent_t ph[4];
-  if (prof) { for (int i = 0; i < 4; ++i) cudaEventCreate(&ph[i]); cudaEventRecord(ph[0], s); }
-#define T2_TICK(i)                                                    \
-  do {                                                                \
-    if (prof && T - 1 - t < kProfSteps) cudaEventRecord(pev[T - 1 - t][i], s); \
-  } while (0)
-  // skinny GEMMs: wgmma split-fp16 engine (default) or the fp32 SIMT kernel (T2_BWD_GEMM=simt, cross-check)
-  bool tc_gemm = true;
-  {
-    const char* e = getenv("T2_BWD_GEMM");
-    if (e && e[0] == 's') tc_gemm = false;
-  }
-  const int nsB = tc_gemm ? kBwdGemmSplit : kSplitB, nsE = tc_gemm ? kBwdGemmSplit : kSplitE;
-  if (tc_gemm) {
-    T2_TRY(bwd_gemm_prepare(m, s));
-    T2_CUDA(cudaMemsetAsync(w.img_d, 0, kBwdImgBytes, s));      // rows >= B stay zero
-    T2_CUDA(cudaMemsetAsync(w.img_a, 0, kBwdImgBytes, s));
-    T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
-    fill_kernel<<<1, 128, 0, s>>>(w.inv_scale, 1.f, 128);
-    T2_LAUNCH_CHECK();
-  }
+  // skinny GEMMs (KB / KE): weight images, zeroed operand images, control block and unit scales
+  T2_TRY(bwd_gemm_prepare(m, s));
+  T2_CUDA(cudaMemsetAsync(w.img_d, 0, kBwdImgBytes, s));      // rows >= B stay zero
+  T2_CUDA(cudaMemsetAsync(w.img_a, 0, kBwdImgBytes, s));
+  T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
+  fill_kernel<<<1, 128, 0, s>>>(w.inv_scale, 1.f, 128);
+  T2_LAUNCH_CHECK();
   // ---- phase 1: reverse-time recurrence ---------------------------------------------------------------
   for (int t = T - 1; t >= 0; --t) {
-    T2_TICK(0);
     const int carry = t < T - 1;
     {  // KA
       LstmBwdArgs k;
       memset(&k, 0, sizeof(k));
-      k.src0 = carry ? w.pb : nullptr; k.ld0 = kPBld; k.off0 = 1536; k.ns0 = nsB;
+      k.src0 = carry ? w.pb : nullptr; k.ld0 = kPBld; k.off0 = 1536; k.ns0 = kBwdGemmSplit;
       k.add = w.gproj + (size_t)t * B * 1536; k.ldadd = 1536;
       k.img = w.img_d; k.inv_scale = w.inv_scale;
       k.keep = a->dec_keep ? a->dec_keep + (size_t)t * B * kDRnn : nullptr;
       k.dropout = training; k.seed = a->seed; k.site = (uint32_t)(t * 4 + 3); k.p = p_dec;
       k.gates = st.gd + (size_t)t * B * 4096; k.c = st.cd + (size_t)(t + 1) * B * kDRnn; k.c_prev = st.cd + (size_t)t * B * kDRnn;
       k.g_c = w.gdc; k.dG = w.dgd + (size_t)t * B * 4096;
-      if (tc_gemm) lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
-      else lstm_bwd_kernel<<<dim3(4, B), 256, 0, s>>>(k);
+      lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TICK(1);
-    if (tc_gemm) {
-      T2_TRY(bwd_gemm_run(m, 0, w.img_d, w.inv_scale, w.pb, kPBld, w.ctrl, s));
-    } else
-    {  // KB
-      SkinnyArgs k;
-      k.A = w.dgd + (size_t)t * B * 4096; k.lda = 4096; k.rows = B; k.nred = 4096;
-      k.W0 = m->w[W_DRNN_WIH]; k.ldw0 = kARnn + kEnc; k.cols0 = kARnn + kEnc;
-      k.W1 = m->w[W_DRNN_WHH]; k.ldw1 = kDRnn; k.cols1 = kDRnn;
-      k.P = w.pb; k.ldp = kPBld; k.nsplit = kSplitB;
-      skinny_nn_kernel<<<dim3(kPBld / 128, kSplitB), 256, 0, s>>>(k);
-      T2_LAUNCH_CHECK();
-    }
-    T2_TICK(2);
+    T2_TRY(bwd_gemm_run(m, 0, w.img_d, w.inv_scale, w.pb, kPBld, w.ctrl, s));   // KB
     {  // KC
       AttBwdArgs k;
       memset(&k, 0, sizeof(k));
       k.t = t; k.T = T; k.B = B; k.Te = Te; k.carry = carry; k.len = a->memory_lengths;
       k.memory = a->memory; k.pm = w.pm; k.q = w.q; k.v = m->w[W_ATT_V]; k.weff = w.weff;
       k.align = a->align; k.awc = w.awc; k.d_align = a->d_align;
-      k.PE = w.pe; k.PB = w.pb; k.nsE = nsE; k.nsB = nsB; k.gproj = w.gproj; k.weffT = w.weffT;
+      k.PE = w.pe; k.PB = w.pb; k.nsE = kBwdGemmSplit; k.nsB = kBwdGemmSplit; k.gproj = w.gproj; k.weffT = w.weffT;
       k.dctx = w.dctx; k.dx2 = a->d_prenet; k.dq = w.dq; k.gs = w.gs; k.gcat = w.gcat; k.cacc = w.cacc; k.dv = w.dv;
       att_bwd_kernel<<<dim3(2, B), kAttT, smem, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TICK(3);
     {  // KD
       LstmBwdArgs k;
       memset(&k, 0, sizeof(k));
-      k.src0 = carry ? w.pe : nullptr; k.ld0 = kPEld; k.off0 = 768; k.ns0 = nsE;
-      k.src1 = w.pb; k.ld1 = kPBld; k.off1 = 0; k.ns1 = nsB;
+      k.src0 = carry ? w.pe : nullptr; k.ld0 = kPEld; k.off0 = 768; k.ns0 = kBwdGemmSplit;
+      k.src1 = w.pb; k.ld1 = kPBld; k.off1 = 0; k.ns1 = kBwdGemmSplit;
       k.img = w.img_a; k.inv_scale = w.inv_scale + 64;
       k.vec = w.dq + (size_t)t * B * 128; k.nvec = 128; k.ldvec = 128; k.Wv = m->w[W_ATT_QUERY]; k.ldwv = kARnn;
       k.keep = a->att_keep ? a->att_keep + (size_t)t * B * kARnn : nullptr;
       k.dropout = training; k.seed = a->seed; k.site = (uint32_t)(t * 4 + 2); k.p = p_att;
       k.gates = st.ga + (size_t)t * B * 4096; k.c = st.ca + (size_t)(t + 1) * B * kARnn; k.c_prev = st.ca + (size_t)t * B * kARnn;
       k.g_c = w.gac; k.dG = w.dga + (size_t)t * B * 4096;
-      if (tc_gemm) lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
-      else lstm_bwd_kernel<<<dim3(4, B), 256, 0, s>>>(k);
+      lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TICK(4);
-    if (tc_gemm) {
-      T2_TRY(bwd_gemm_run(m, 1, w.img_a, w.inv_scale + 64, w.pe, kPEld, w.ctrl, s));
-    } else
-    {  // KE
-      SkinnyArgs k;
-      k.A = w.dga + (size_t)t * B * 4096; k.lda = 4096; k.rows = B; k.nred = 4096;
-      k.W0 = m->w[W_ARNN_WIH]; k.ldw0 = kPre + kEnc; k.cols0 = kPre + kEnc;
-      k.W1 = m->w[W_ARNN_WHH]; k.ldw1 = kARnn; k.cols1 = kARnn;
-      k.P = w.pe; k.ldp = kPEld; k.nsplit = kSplitE;
-      skinny_nn_kernel<<<dim3(kPEld / 128, kSplitE), 256, 0, s>>>(k);
-      T2_LAUNCH_CHECK();
-    }
-    T2_TICK(5);
+    T2_TRY(bwd_gemm_run(m, 1, w.img_a, w.inv_scale + 64, w.pe, kPEld, w.ctrl, s));   // KE
   }
-  if (prof) cudaEventRecord(ph[1], s);
-  reduce_pe_x2_kernel<<<B, 256, 0, s>>>(w.pe, a->d_prenet, B, nsE);
+  reduce_pe_x2_kernel<<<B, 256, 0, s>>>(w.pe, a->d_prenet, B, kBwdGemmSplit);
   T2_LAUNCH_CHECK();
 
   // ---- phase 2: time-batched gradients --------------------------------------------------------------------
   float* const* G = a->grads;
-  const float* x2 = a->teacher_prenet;
   const int TBi = (int)TB;
-  // LSTM weight / bias gradients: the time-batched wgrad_tc engine (default) or, as a cross-check (T2_WGRAD=cublas),
-  // separate gemm_tc products and column sums
-  bool tc_wgrad = true;
-  {
-    const char* e = getenv("T2_WGRAD");
-    if (e && e[0] == 'c') tc_wgrad = false;
-  }
-  if (tc_wgrad) {
-    T2_TRY(wgrad_tc_run(m, B, T, w.dga, w.dgd, x2, st, G, w.wg, s));
-  } else {
-  if (G[W_ARNN_WIH]) {   // [x2_t | ctx_{t-1}]                                             model.py:352
-      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kPre, TBi, w.dga, 4096, x2, kPre, G[W_ARNN_WIH], kPre + kEnc, 0.f));
-      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kEnc, TBi, w.dga, 4096, st.ctx, kEnc, G[W_ARNN_WIH] + kPre, kPre + kEnc, 0.f));
-    }
-    if (G[W_ARNN_WHH]) T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kARnn, TBi, w.dga, 4096, st.ha, kARnn, G[W_ARNN_WHH], kARnn, 0.f));
-    if (G[W_ARNN_BIH] || G[W_ARNN_BHH]) {
-      T2_TRY(colsum_f32(m, s, w.dga, 4096, TBi, 4096, w.tmp));
-      if (G[W_ARNN_BIH]) T2_CUDA(cudaMemcpyAsync(G[W_ARNN_BIH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
-      if (G[W_ARNN_BHH]) T2_CUDA(cudaMemcpyAsync(G[W_ARNN_BHH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
-    }
-    if (G[W_DRNN_WIH]) {   // [ah_t | ctx_t]                                                 model.py:366-367
-      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kARnn, TBi, w.dgd, 4096, st.ha + (size_t)B * kARnn, kARnn, G[W_DRNN_WIH], kARnn + kEnc, 0.f));
-      T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kEnc, TBi, w.dgd, 4096, st.ctx + (size_t)B * kEnc, kEnc, G[W_DRNN_WIH] + kARnn, kARnn + kEnc, 0.f));
-    }
-    if (G[W_DRNN_WHH]) T2_TRY(gemm_tc_rm(m, s, true, false, 4096, kDRnn, TBi, w.dgd, 4096, st.hd, kDRnn, G[W_DRNN_WHH], kDRnn, 0.f));
-    if (G[W_DRNN_BIH] || G[W_DRNN_BHH]) {
-      T2_TRY(colsum_f32(m, s, w.dgd, 4096, TBi, 4096, w.tmp));
-      if (G[W_DRNN_BIH]) T2_CUDA(cudaMemcpyAsync(G[W_DRNN_BIH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
-      if (G[W_DRNN_BHH]) T2_CUDA(cudaMemcpyAsync(G[W_DRNN_BHH], w.tmp, 4096 * 4, cudaMemcpyDeviceToDevice, s));
-    }
-  }
+  // LSTM weight / bias gradients on the time-batched wgrad_tc engine
+  T2_TRY(wgrad_tc_run(m, B, T, w.dga, w.dgd, a->teacher_prenet, st, G, w.wg, s));
   // projection + gate on [dh_t | ctx_t]                                                   model.py:373-378
   if (G[W_PROJ_W]) {
     T2_TRY(gemm_tc_rm(m, s, true, false, kMel, kDRnn, TBi, w.dy, 81, st.hd + (size_t)B * kDRnn, kDRnn, G[W_PROJ_W], kDRnn + kEnc, 0.f));
@@ -808,21 +594,6 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     g.B = w.dctx; g.ldb = (long)B * kEnc; g.strideB = kEnc;
     g.C = a->d_memory; g.ldc = kEnc; g.strideC = (long)Te * kEnc; g.beta = 1.f; g.batch = B;
     T2_TRY(gemm_tc(m, s, g));
-  }
-  if (prof) {
-    cudaEventRecord(ph[2], s);
-    cudaStreamSynchronize(s);
-    float acc[5] = {0, 0, 0, 0, 0};
-    const int n = T < kProfSteps ? T : kProfSteps;
-    for (int i = 0; i < n; ++i)
-      for (int j = 0; j < 5; ++j) { float ms = 0; cudaEventElapsedTime(&ms, pev[i][j], pev[i][j + 1]); acc[j] += ms; }
-    float m01 = 0, m12 = 0;
-    cudaEventElapsedTime(&m01, ph[0], ph[1]);
-    cudaEventElapsedTime(&m12, ph[1], ph[2]);
-    fprintf(stderr, "[t2b200] decoder backward: loop %.2f ms (%d steps), batched gradients %.2f ms; per step us: lstm_dec %.1f "
-            "gemm_dec %.1f attention %.1f lstm_att %.1f gemm_att %.1f\n", m01, T, m12, acc[0] / n * 1e3f, acc[1] / n * 1e3f,
-            acc[2] / n * 1e3f, acc[3] / n * 1e3f, acc[4] / n * 1e3f);
-    for (int i = 0; i < 4; ++i) cudaEventDestroy(ph[i]);
   }
   return T2_OK;
 }

@@ -26,7 +26,6 @@ struct T2Model {
   // training: input-gradient convolutions = the same engine with flipped / transposed weights (re-packed per backward)
   uint8_t* tc_dgrad_enc[3] = {}; uint8_t* tc_dgrad_post[5] = {};
   float* dgrad_tmp = nullptr;    // (512, 512, 5) fp32 scratch for the flipped weights
-  float* ones = nullptr;         // 8192 ones
 
   // ---- packed operands of the persistent decoder kernel (owned; see decoder_persistent.cu) ----
   void* pk = nullptr;            // opaque PersistentPack*

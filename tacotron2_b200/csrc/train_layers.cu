@@ -10,7 +10,6 @@
 // on the wgmma wgrad engine (wgrad_tc.cu); BatchNorm statistics / normalisation / activation / dropout and their backward
 // are our kernels.
 // BiLSTM backward: reverse recurrence with one skinny GEMM + one elementwise kernel per step and direction.
-#include <stdlib.h>
 #include <string.h>
 
 #include "conv_tc.h"
@@ -187,13 +186,6 @@ __global__ void bn_bwd_apply_kernel(const float* __restrict__ g, int g_padded, c
   }
   gz[pr * C + c] = v * gamma[c] * rstd;
 }
-// packed (co, k, ci) weight gradient -> state_dict layout (co, ci, k)
-__global__ void unpack_conv_grad_kernel(const float* __restrict__ gp, float* __restrict__ g, int co, int ci, int k) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long)co * ci * k) return;
-  const int kk = (int)(i % k); const long r = i / k; const int c = (int)(r % ci); const int o = (int)(r / ci);
-  g[i] = gp[((long)o * k + kk) * ci + c];
-}
 // zero the rows t >= len[b] of a padded-rows buffer
 __global__ void mask_padded_rows_kernel(float* __restrict__ xp, const int32_t* __restrict__ len, int B, int T, int C) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -332,8 +324,6 @@ int tc_train_conv(T2Model* m, const float* xp, int cin, const uint8_t* wimg, int
 // dW_k[co][ci] = sum_r G_z[r][co] X[r + k - 2][ci]: K = padded rows in chunks of 64, A = G_z^T images (per-channel power-of-two
 // scale), B = X^T images, one set per tap (source rows shifted by k - 2), 128 x 256 tiles, K splits reduced in a fixed order.
 struct WgConvWs { uint8_t* img_a; uint8_t* img_b; float* part; float* stat; float* scale; float* inv; float* colsum; WgJob* jobs; };
-// T2_WGRAD=cublas: the conv weight gradients through gemm_tc instead (cross-check); the region stays in the layout
-static bool wgrad_cublas() { const char* e = getenv("T2_WGRAD"); return e && e[0] == 'c'; }
 void wgconv_layout(Carve& c, int B, int T, WgConvWs* w) {    // every region 1024-aligned
   const long Mp = (long)B * (T + 2 * kPadRows);
   const long nch = (Mp + 63) / 64;
@@ -428,10 +418,9 @@ int conv_fwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
 // non-null, and the gradients of conv.weight / conv.bias / bn.weight / bn.bias.  planes: scratch of
 // tc_planes_bytes(B, T, 512) for the input-gradient conv.
 int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_t seed, const float* g, int g_padded,
-             const float* xp, const float* zp, const float* stats, const float* yp, float* gz_p, float* gx_p, float* sums, float* dwpk,
-             const float* ones, float* const* G, const WgConvWs* wg, __half* planes, cudaStream_t s) {
+             const float* xp, const float* zp, const float* stats, const float* yp, float* gz_p, float* gx_p, float* sums,
+             float* const* G, const WgConvWs& wg, __half* planes, cudaStream_t s) {
   const long Mp = (long)B * (T + 2 * kPadRows);
-  const int Me = (int)(Mp - 2 * kPadRows);
   float* partial = sums + 2 * L.cout;      // (kRedSplit, 2, cout) scratch behind the two result rows
   bn_bwd_reduce_kernel<<<dim3((L.cout + 31) / 32, kRedSplit), 256, 0, s>>>(g, g_padded, yp, zp, stats, B, T, L.cout, L.act, L.dropout,
                                                                             L.keep, seed, L.site, partial);
@@ -445,33 +434,18 @@ int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
   T2_LAUNCH_CHECK();
   if (G[L.wbase + 3]) T2_CUDA(cudaMemcpyAsync(G[L.wbase + 3], sums, (size_t)L.cout * 4, cudaMemcpyDeviceToDevice, s));           // d beta
   if (G[L.wbase + 2]) T2_CUDA(cudaMemcpyAsync(G[L.wbase + 2], sums + L.cout, (size_t)L.cout * 4, cudaMemcpyDeviceToDevice, s));  // d gamma
-  if (wg) {   // weight + bias gradient on our wgmma engine
-    T2_TRY(conv_wgrad_tc(L, B, T, gz_p, xp, G[L.wbase], G[L.wbase + 1], *wg, s));
-  } else {
-    if (G[L.wbase + 1]) T2_TRY(colsum_f32(m, s, gz_p, L.cout, Mp, L.cout, G[L.wbase + 1]));      // d conv bias
-    if (G[L.wbase]) {
-      for (int k = 0; k < kConvK; ++k)
-        T2_TRY(gemm_tc_rm(m, s, true, false, L.cout, L.cin, Me, gz_p + (long)kPadRows * L.cout, L.cout, xp + (long)k * L.cin, L.cin,
-                          dwpk + (long)k * L.cin, (long)kConvK * L.cin, 0.f));
-      const long nw = (long)L.cout * L.cin * kConvK;
-      unpack_conv_grad_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(dwpk, G[L.wbase], L.cout, L.cin, kConvK);
-      T2_LAUNCH_CHECK();
-    }
-  }
-  if (gx_p && wg) {   // input gradient = conv of G_z with the flipped / transposed kernel on the tensor-core engine
+  // weight + bias gradient on our wgmma engine
+  T2_TRY(conv_wgrad_tc(L, B, T, gz_p, xp, G[L.wbase], G[L.wbase + 1], wg, s));
+  if (gx_p) {   // input gradient = conv of G_z with the flipped / transposed kernel on the tensor-core engine
     // G_z is pre-scaled by a power of two (from the per-channel statistics of the weight-gradient pass): fp16 range
-    global_scale_kernel<<<1, 256, 0, s>>>(wg->stat, L.cout, wg->colsum, wg->stat);       // colsum[0] = s_g, stat[0..512) = 1 / s_g
+    global_scale_kernel<<<1, 256, 0, s>>>(wg.stat, L.cout, wg.colsum, wg.stat);       // colsum[0] = s_g, stat[0..512) = 1 / s_g
     T2_LAUNCH_CHECK();
     if (!m->dgrad_tmp) T2_CUDA(cudaMalloc((void**)&m->dgrad_tmp, (size_t)kPost * kPost * kConvK * 4));
     const long nw = (long)L.cout * L.cin * kConvK;
     flip_conv_w_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(m->w[L.wbase], m->dgrad_tmp, L.cout, L.cin);
     T2_LAUNCH_CHECK();
     T2_TRY(tc_pack_weights(m->dgrad_tmp, L.cin, L.cout, kConvK, L.cin >= 128 ? 128 : 80, L.wimg_dgrad, s));
-    T2_TRY(tc_train_conv(m, gz_p, L.cout, *L.wimg_dgrad, L.cin, B, T, gx_p, planes, wg->colsum, wg->stat, s));
-  } else if (gx_p) {   // without the weight-gradient engine's channel statistics (T2_WGRAD=cublas): row-shifted GEMMs
-    for (int k = 0; k < kConvK; ++k)
-      T2_TRY(gemm_tc_rm(m, s, false, false, Me, L.cin, L.cout, gz_p + (long)(2 * kPadRows - k) * L.cout, L.cout, L.wpk + (long)k * L.cin,
-                        (long)kConvK * L.cin, gx_p + (long)kPadRows * L.cin, L.cin, k ? 1.f : 0.f));
+    T2_TRY(tc_train_conv(m, gz_p, L.cout, *L.wimg_dgrad, L.cin, B, T, gx_p, planes, wg.colsum, wg.stat, s));
   }
   return T2_OK;
 }
@@ -674,7 +648,7 @@ int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, void* ws, cudaStre
 struct PostBwdWs {
   float *gz, *gxa, *gxb;   // padded rows (B (T+4), 512)
   float* grow;             // (B T, 80) output gradient rows
-  float *ones, *dwpk, *sums;
+  float* sums;
   WgConvWs wg;
   __half* planes;
 };
@@ -682,8 +656,6 @@ static void postnet_backward_ws_layout(Carve& c, int B, int T, PostBwdWs* w) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
   w->gz = c.take<float>(Mp * kPost); w->gxa = c.take<float>(Mp * kPost); w->gxb = c.take<float>(Mp * kPost);
   w->grow = c.take<float>((size_t)B * T * kMel);
-  w->ones = c.take<float>(Mp);
-  w->dwpk = c.take<float>((size_t)kPost * kPost * kConvK);
   w->sums = c.take<float>((size_t)(2 + 2 * kRedSplit) * kPost);
   wgconv_layout(c, B, T, &w->wg);
   w->planes = c.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
@@ -703,13 +675,9 @@ int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
   StackStash st;
   Carve sc(const_cast<void*>(a->stash));
   stack_layout(sc, B, T, 5, kPostCh, &st);
-  const size_t Mp = (size_t)B * (T + 2 * kPadRows);
   PostBwdWs w;
   Carve wc(a->ws, 1024);
   postnet_backward_ws_layout(wc, B, T, &w);
-  const WgConvWs* wg = wgrad_cublas() ? nullptr : &w.wg;
-  fill1_kernel<<<(unsigned)((Mp + 255) / 256), 256, 0, s>>>(w.ones, 1.f, (long)Mp);
-  T2_LAUNCH_CHECK();
   const long n = (long)B * T * kMel;
   bct_to_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->d_mel_post, w.grow, B, T, kMel);     // (B,80,T) -> rows
   T2_LAUNCH_CHECK();
@@ -722,8 +690,8 @@ int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
       mask_padded_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.x[0], a->wgrad_lengths, B, T, kMel);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.x[i], st.z[i], st.stats[i], st.x[i + 1], w.gz, gx, w.sums, w.dwpk,
-                    w.ones, a->grads, wg, w.planes, s));
+    T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.x[i], st.z[i], st.stats[i], st.x[i + 1], w.gz, gx, w.sums,
+                    a->grads, w.wg, w.planes, s));
     g = gx; g_padded = 1;
     gx = gx == w.gxa ? w.gxb : w.gxa;
   }
@@ -802,14 +770,10 @@ struct EncBwdWs {
   float* part;             // (2, kEncBwdSplit, 64, 256)
   float* g_c;              // (2, 64, 256)
   float *gz, *gxa, *gxb;   // padded rows (B (T+4), 512)
-  float *ones, *dwpk, *sums, *tmp;
+  float *sums, *tmp;
   WgConvWs wg;
   __half* planes;
 };
-static size_t enc_bwd_n_ones(int B, int T) {
-  const size_t Mp = (size_t)B * (T + 2 * kPadRows);
-  return Mp > (size_t)B * T ? Mp : (size_t)B * T;
-}
 static void encoder_backward_ws_layout(Carve& c, int B, int T, EncBwdWs* w) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
   w->dG = c.take<float>((size_t)B * T * 8 * kEncH);
@@ -817,8 +781,6 @@ static void encoder_backward_ws_layout(Carve& c, int B, int T, EncBwdWs* w) {
   w->part = c.take<float>((size_t)2 * kEncBwdSplit * 64 * kEncH);
   w->g_c = c.take<float>((size_t)2 * 64 * kEncH);
   w->gz = c.take<float>(Mp * kEnc); w->gxa = c.take<float>(Mp * kEnc); w->gxb = c.take<float>(Mp * kEnc);
-  w->ones = c.take<float>(enc_bwd_n_ones(B, T));
-  w->dwpk = c.take<float>((size_t)kEnc * kEnc * kConvK);
   w->sums = c.take<float>((size_t)(2 + 2 * kRedSplit) * kEnc);
   w->tmp = c.take<float>(8 * kEncH);
   wgconv_layout(c, B, T, &w->wg);
@@ -842,10 +804,6 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   EncBwdWs w;
   Carve wc(a->ws, 1024);
   encoder_backward_ws_layout(wc, B, T, &w);
-  const WgConvWs* wg = wgrad_cublas() ? nullptr : &w.wg;
-  const size_t n_ones = enc_bwd_n_ones(B, T);
-  fill1_kernel<<<(unsigned)((n_ones + 255) / 256), 256, 0, s>>>(w.ones, 1.f, (long)n_ones);
-  T2_LAUNCH_CHECK();
   T2_CUDA(cudaMemsetAsync(w.g_c, 0, (size_t)2 * 64 * kEncH * 4, s));
   // ---- BiLSTM: reverse recurrence of both directions (model.py:169-171, 180-188) ----
   for (int step = 0; step < T; ++step) {
@@ -882,7 +840,7 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   for (int i = 2; i >= 0; --i) {
     const bool need_gx = i > 0 || a->d_embedded || (a->text && G[W_EMB]);
     T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.cs.x[i], st.cs.z[i], st.cs.stats[i], st.cs.x[i + 1], w.gz,
-                    need_gx ? gx : nullptr, w.sums, w.dwpk, w.ones, G, wg, w.planes, s));
+                    need_gx ? gx : nullptr, w.sums, G, w.wg, w.planes, s));
     g = gx; g_padded = 1;
     gx = gx == w.gxa ? w.gxb : w.gxa;
   }

@@ -11,6 +11,7 @@ from oracle import tacotron2_oracle as O
 from tests.common import keep_mask, rel_err, synth_state_dict
 from tests.test_oracle_golden import (GRADS, check_grads_vs_fixture, check_grads_vs_fp64_fixture, full_grad_inputs,
                                       grad_inputs, load, oracle_train_step)
+from tests.test_gpu_train_regimes import to64
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -47,14 +48,10 @@ def oracle_decoder_grads(sd, memory, mels, lens, pk, ak, dk, d_mel, d_gate, d_al
     return (mel.detach(), gate.detach(), align.detach()), {k: sdg[k].grad for k in names}, mem.grad
 
 
-@pytest.mark.parametrize("gemm", ["tc", "simt"])
 @pytest.mark.parametrize("B,Te,T,training,use_align", [(3, 19, 7, True, False), (5, 40, 12, True, True),
                                                        (4, 150, 9, False, False), (64, 33, 5, True, False)])
-def test_decoder_backward_vs_oracle_autograd(B, Te, T, training, use_align, gemm, monkeypatch):
-    """gemm = tc: the reverse recurrence's skinny GEMMs and the time-batched LSTM weight gradients on the wgmma
-    split-fp16 engines (default); simt: fp32 SIMT kernels / separate gemm_tc products and column sums (cross-check)."""
-    monkeypatch.setenv("T2_BWD_GEMM", gemm)
-    monkeypatch.setenv("T2_WGRAD", "tc" if gemm == "tc" else "cublas")
+def test_decoder_backward_vs_oracle_autograd(B, Te, T, training, use_align):
+    """The reverse recurrence's skinny GEMMs and the time-batched LSTM weight gradients on the wgmma split-fp16 engines."""
     sd = synth_state_dict(seed=21, scale=2.0)
     memory, mels, lens, pk, ak, dk, d_mel, d_gate, d_align = decoder_case(B, Te, T, seed=100 + B)
     if not use_align:
@@ -79,7 +76,7 @@ def test_decoder_backward_vs_oracle_autograd(B, Te, T, training, use_align, gemm
         assert p.grad is not None, k
         errs[k] = rel_err(p.grad, ref_g["decoder." + k])
     bad = {k: v for k, v in errs.items() if not v < TOL}
-    print("decoder backward [%s] B=%d Te=%d T=%d: worst %.2e" % (gemm, B, Te, T, max(errs.values())))
+    print("decoder backward B=%d Te=%d T=%d: worst %.2e" % (B, Te, T, max(errs.values())))
     assert not bad, bad
 
 
@@ -197,42 +194,53 @@ def test_postnet_and_encoder_modules_backward_vs_oracle(B, T):
     assert not bad, bad
 
 
-def test_full_size_backward_tensor_core_vs_simt_gemms_and_determinism(monkeypatch):
-    """B=64, T_enc=150 (the benchmark shape), 24 teacher-forced steps, Philox dropout: the gradients with the reverse
-    recurrence's GEMMs on the wgmma engine agree with the fp32 SIMT kernels, and two runs are bit-identical."""
+def test_full_size_backward_vs_fp64_and_determinism():
+    """B=64, T_enc=150 (the benchmark shape), 24 teacher-forced steps, injected dropout masks: two runs are bit-identical,
+    and d_memory and every decoder parameter gradient are within 1e-4 of the oracle's autograd in float64 (or 4 x the fp32
+    oracle's own deviation from float64 where that exceeds 2.5e-5, the yardstick of DESIGN section 2)."""
     torch.manual_seed(7)
     model = t2.Tacotron2(t2.create_hparams()).cuda().train()
     dec = model.decoder
     B, Te, T = 64, 150, 24
     g = torch.Generator().manual_seed(3)
-    memory = torch.randn(B, Te, 512, generator=g).cuda()
-    mels = torch.randn(B, 80, T, generator=g).cuda()
+    memory = torch.randn(B, Te, 512, generator=g)
+    mels = torch.randn(B, 80, T, generator=g)
     lens = torch.sort(torch.randint(75, Te + 1, (B,), generator=g), descending=True)[0]
     lens[0] = Te
-    d_mel = torch.randn(B, 80, T, generator=g).cuda()
-    d_gate = torch.randn(B, T, generator=g).cuda()
+    d_mel = torch.randn(B, 80, T, generator=g)
+    d_gate = torch.randn(B, T, generator=g)
     pk = keep_mask((T + 1, 2, B, 256), 0.5, 1)
     ak, dk = keep_mask((T, B, 1024), 0.1, 2), keep_mask((T, B, 1024), 0.1, 3)
 
-    def run(mode):
-        monkeypatch.setenv("T2_BWD_GEMM", mode)
-        monkeypatch.setenv("T2_WGRAD", "tc" if mode == "tc" else "cublas")
+    def run():
         for p in dec.parameters():
             p.grad = None
-        mem = memory.clone().requires_grad_(True)
+        mem = memory.cuda().requires_grad_(True)
         with t2.dropout_masks(prenet=pk, att=ak, dec=dk):
-            mel, gate, _ = dec(mem, mels, lens.cuda())
-            ((mel * d_mel).sum() + (gate * d_gate).sum()).backward()
+            mel, gate, _ = dec(mem, mels.cuda(), lens.cuda())
+            ((mel * d_mel.cuda()).sum() + (gate * d_gate.cuda()).sum()).backward()
         torch.cuda.synchronize()
         return [mem.grad.clone()] + [p.grad.clone() for p in dec.parameters()]
 
-    a, b, c = run("tc"), run("tc"), run("simt")
+    a, b = run(), run()
     names = ["d_memory"] + [k for k, _ in dec.named_parameters()]
     diff = {n: rel_err(x, y) for n, x, y in zip(names, a, b) if not torch.equal(x, y)}
     assert not diff, "backward is not bit-reproducible: %s" % diff
-    worst = max(rel_err(x, y) for x, y in zip(a, c))
-    print("full-size backward: wgmma vs SIMT GEMMs worst rel diff %.2e" % worst)
-    assert worst < 1e-4
+
+    sd = {k: v.cpu() for k, v in model.state_dict().items()}
+    _, ref32, ref32_dmem = oracle_decoder_grads(sd, memory, mels, lens, pk, ak, dk, d_mel, d_gate, None, True)
+    _, ref64, ref64_dmem = oracle_decoder_grads(to64(sd, "cpu"), memory.double(), mels.double(), lens, pk, ak, dk, d_mel.double(),
+                                                d_gate.double(), None, True)
+    ref32["d_memory"], ref64["d_memory"] = ref32_dmem, ref64_dmem
+    errs, bars = {}, {}
+    for n, x in zip(names, a):
+        k = n if n == "d_memory" else "decoder." + n
+        errs[n] = rel_err(x, ref64[k])
+        bars[n] = max(1e-4, 4.0 * rel_err(ref32[k], ref64[k]))
+    worst = max(errs, key=errs.get)
+    print("full-size backward vs fp64: worst %.2e (%s, bar %.2e)" % (errs[worst], worst, bars[worst]))
+    bad = {n: (e, bars[n]) for n, e in errs.items() if not e < bars[n]}
+    assert not bad, bad
 
 
 def test_fused_clip_adam_matches_torch():

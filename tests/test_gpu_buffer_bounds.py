@@ -6,7 +6,7 @@ sized exactly as its query reports and placed 256 bytes past a 512-byte boundary
 byte pattern (the buffer itself starts out filled with the pattern too).  The canaries must be intact afterwards and the
 outputs bit-identical to the first run.  The cases sit on the layout edges: one row / one frame, more than 64 rows, the
 decoder's shared-memory regimes (T_enc 94 / 95, 896 / 897, 2274), the stepwise decoder's longest memory, the backward
-passes with the tensor-core and the SIMT / gemm_tc weight-gradient paths."""
+passes."""
 import contextlib
 from unittest import mock
 
@@ -156,14 +156,8 @@ def test_infer_host():
 
 # ---- backward passes --------------------------------------------------------------------------------------------------
 
-BWD_PATHS = [{}, {"T2_BWD_GEMM": "simt", "T2_WGRAD": "cublas"}]
-
-
-@pytest.mark.parametrize("env", BWD_PATHS, ids=["tc", "simt"])
 @pytest.mark.parametrize("Te", [95, 408])
-def test_decoder_teacher_stash_and_backward(Te, env, monkeypatch):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_decoder_teacher_stash_and_backward(Te):
     B, T = 64, 5
     memory = randn(B, Te, 512, seed=Te, scale=0.5)
     prenet = torch.relu(randn((T + 1) * B, 256, seed=Te + 1))
@@ -180,10 +174,7 @@ def test_decoder_teacher_stash_and_backward(Te, env, monkeypatch):
     same_both_ways(run)
 
 
-@pytest.mark.parametrize("env", BWD_PATHS, ids=["tc", "simt"])
-def test_encoder_backward(env, monkeypatch):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_encoder_backward():
     B, T = 64, 37
     text = rand_text(B, T, seed=11).cuda()
     d_memory = randn(B, T, 512, seed=12)
@@ -199,10 +190,7 @@ def test_encoder_backward(env, monkeypatch):
     same_both_ways(run)
 
 
-@pytest.mark.parametrize("env", BWD_PATHS, ids=["tc", "simt"])
-def test_postnet_backward(env, monkeypatch):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_postnet_backward():
     B, T = 64, 37
     mel = randn(B, T, 80, seed=13)
     d_out = randn(B, 80, T, seed=14)
@@ -216,10 +204,7 @@ def test_postnet_backward(env, monkeypatch):
     same_both_ways(run)
 
 
-@pytest.mark.parametrize("env", BWD_PATHS, ids=["tc", "simt"])
-def test_prenet_backward(env, monkeypatch):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_prenet_backward():
     M = 64 * 6
     frames, d_out = randn(M, 80, seed=15), randn(M, 256, seed=16)
 
