@@ -205,6 +205,34 @@ int    t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* s
 int    t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n_steps, const int32_t* status_host,
                              void* stream);
 
+/* ---- Continuous batching on a decoder stream: its rows as slots ---------------------------------
+ * A row's bits depend neither on its neighbours nor on T_enc, and between two runs all of its state is
+ * in `state`, so a row can be handed another text there.  Such a session runs every chunk as local
+ * steps [0, n): t2_decoder_stream_run with status_host = NULL (every slice starts at step 0; a
+ * status_host of [0, 1] pairs skips slices) on a stream whose n_steps_cap is n + 1 -- the kernel keeps
+ * no step counter in `state`, and a step reads the keep mask of the step after it.  mel / gate / align
+ * are chunk buffers (B, n + 1, .), prenet_keep (n + 1, 2, B, 256) holds at [i, :, b] the mask of row b's
+ * own step (steps it has run before the chunk) + i, and dec.seed is the chunk's Philox seed; the caller
+ * rewrites them (and memory / memory_lengths rows) between runs.  mel_lengths[b] becomes the local step
+ * + 1 at which row b fired in the chunk; a slice ends a chunk early once all its rows have fired.
+ *   admit:   rows (host, n_rows ascending row indices): each listed row goes back to the state begin
+ *            gives it -- its accumulator rows, LSTM cells, previous / cumulative attention weights,
+ *            rows of the activation images and of the query, stop latch, mel_lengths[row] = -1 -- and
+ *            its processed memory is recomputed from memory[row] (one reset launch whatever n_rows is,
+ *            and one GEMM per run of consecutive rows).  No other row's state is written.
+ *   collect: rows (host): the first n_frames frames of chunk row `row` -- mel, gate and
+ *            align[:, :T_text] -- are copied to mel (n_frames, 80), gate (n_frames), align (n_frames,
+ *            T_text) of the entry: the request's own buffers at its own step offset.  One launch per
+ *            64-row slice with entries.
+ * Both refuse rows outside [0, B), counts outside the chunk buffers and null pointers before any launch. */
+typedef struct T2CollectRow {
+  int32_t row, n_frames, T_text, reserved;
+  float* mel; float* gate; float* align;
+} T2CollectRow;
+int    t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int32_t* rows, int32_t n_rows, void* stream);
+int    t2_decoder_stream_collect(T2Model* m, const T2DecoderStreamArgs* a, const T2CollectRow* rows, int32_t n_rows,
+                                 void* stream);
+
 /* ---- Decoder backward (the autograd graph of Decoder.forward, model.py:381-416) ----------------
  * Reverse-time recurrence over the stash of a TEACHER run with the same memory / teacher_prenet / masks /
  * seed, then the time-batched weight gradients.  B <= 64.

@@ -9,7 +9,8 @@ from . import amp  # noqa: F401
 from .glow import WaveGlow, waveglow_noise, window_halo  # noqa: F401
 from .denoiser import Denoiser, denoiser_halo  # noqa: F401
 from .optim import AmpFusedClipAdam, FusedClipAdam  # noqa: F401
+from .serving import InferenceServer  # noqa: F401
 
 __all__ = ["Tacotron2", "Encoder", "Decoder", "Postnet", "Tacotron2Loss", "create_hparams", "dropout_masks",
            "FusedClipAdam", "AmpFusedClipAdam", "amp", "invalidate_weights", "TacotronSTFT",
-           "WaveGlow", "waveglow_noise", "window_halo", "Denoiser", "denoiser_halo"]
+           "WaveGlow", "waveglow_noise", "window_halo", "Denoiser", "denoiser_halo", "InferenceServer"]

@@ -29,6 +29,7 @@ EXPORTS = [
     "t2_loss_workspace_bytes", "t2_tacotron2_loss",
     "t2_mel_spectrogram_frames", "t2_mel_spectrogram_workspace_bytes", "t2_mel_spectrogram", "t2_collate",
     "t2_decoder_stream_state_bytes", "t2_decoder_stream_begin", "t2_decoder_stream_run",
+    "t2_decoder_stream_admit", "t2_decoder_stream_collect",
     "t2_waveglow_create", "t2_waveglow_refresh", "t2_waveglow_destroy", "t2_waveglow_workspace_bytes",
     "t2_waveglow_infer", "t2_waveglow_infer_window", "t2_waveglow_window_halo",
     "t2_denoiser_create", "t2_denoiser_refresh", "t2_denoiser_destroy", "t2_denoiser_bias",
@@ -83,6 +84,11 @@ class T2DecoderArgs(C.Structure):
 
 class T2DecoderStreamArgs(C.Structure):
     _fields_ = [("dec", T2DecoderArgs), ("state", C.c_void_p), ("state_bytes", C.c_size_t), ("status", C.c_void_p)]
+
+
+class T2CollectRow(C.Structure):
+    _fields_ = [("row", C.c_int32), ("n_frames", C.c_int32), ("T_text", C.c_int32), ("reserved", C.c_int32),
+                ("mel", C.c_void_p), ("gate", C.c_void_p), ("align", C.c_void_p)]
 
 
 class T2DecoderBwdArgs(C.Structure):
@@ -227,6 +233,10 @@ def lib():
     L.t2_decoder_stream_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.t2_decoder_stream_begin.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_void_p]
     L.t2_decoder_stream_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_int32, C.c_void_p, C.c_void_p]
+    L.t2_decoder_stream_admit.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.POINTER(C.c_int32), C.c_int32,
+                                          C.c_void_p]
+    L.t2_decoder_stream_collect.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.POINTER(T2CollectRow), C.c_int32,
+                                            C.c_void_p]
     L.t2_postnet_forward.argtypes = [C.c_void_p, C.POINTER(T2PostnetArgs), C.c_void_p]
     L.t2_postnet_infer.argtypes = [C.c_void_p, C.POINTER(T2PostnetArgs), C.c_void_p]
     L.t2_clip_adam_workspace_bytes.restype = C.c_size_t

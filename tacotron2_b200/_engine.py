@@ -420,10 +420,23 @@ class Engine(_Handle):
         return mel, lens, ns
 
 
+def f32_buffer(device, *shape):
+    """A zeroed fp32 tensor over a byte buffer of exactly its size (the allocation the buffer-bounds tests place)."""
+    n = 1
+    for d in shape:
+        n *= int(d)
+    return _capi.byte_buffer(4 * n, device).view(torch.float32).zero_().view(*shape)
+
+
 class DecoderStream:
     """One resumable decoder run: full-size output buffers (mel (B, cap, 80), gate (B, cap), align (B, cap, T_enc),
     mel_lengths (B,) with -1 for live rows) and the per-stream state buffer that carries everything across a chunk
-    boundary.  ``run(n)`` advances every live 64-row slice by up to n steps and takes the one host sync of the chunk."""
+    boundary.  ``run(n)`` advances every live 64-row slice by up to n steps and takes the one host sync of the chunk.
+
+    Continuous batching (serving.py) uses the rows as slots: ``cap`` is the chunk length + 1, the buffers hold one chunk,
+    ``chunk`` runs local steps [0, n), ``admit`` resets rows for new texts and ``collect`` hands a chunk's frames to the
+    requests' own buffers.  ``memory``, ``len32`` and ``keep`` are the tensors the kernel reads: such a session rewrites
+    their rows in place between chunks."""
 
     def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed, memory_lengths=None):
         L = _capi.lib()
@@ -433,13 +446,14 @@ class DecoderStream:
         B, T = int(self.memory.shape[0]), int(self.memory.shape[1])
         self.B, self.T_enc, self.cap = B, T, int(cap)
         f32 = dict(device=dev, dtype=torch.float32)
-        self.mel = torch.zeros(B, self.cap, eng.hp.n_mel_channels, **f32)
-        self.gate = torch.zeros(B, self.cap, **f32)
-        self.align = torch.zeros(B, self.cap, T, **f32)
-        self.mel_lengths = torch.empty(B, device=dev, dtype=torch.int32)
+        self.mel = f32_buffer(dev, B, self.cap, eng.hp.n_mel_channels)
+        self.gate = f32_buffer(dev, B, self.cap)
+        self.align = f32_buffer(dev, B, self.cap, T)
         self.n_steps = torch.zeros(1, device=dev, dtype=torch.int32)
         self.n_slices = (B + 63) // 64
-        self.status = torch.zeros(2 * self.n_slices, device=dev, dtype=torch.int32)
+        # mel_lengths | status in one tensor: what the host reads back after a chunk is one copy
+        self.readback = torch.zeros(B + 2 * self.n_slices, device=dev, dtype=torch.int32)
+        self.mel_lengths, self.status = self.readback[:B], self.readback[B:]
         self.status_host = None                      # the caller's copy of `status` after the last run
         self.state = _capi.byte_buffer(L.t2_decoder_stream_state_bytes(eng.handle, B, T), dev)
         self.keep, self.len32 = _u8(prenet_keep, dev), _i32(memory_lengths, dev)
@@ -459,3 +473,29 @@ class DecoderStream:
         stopped = self.status_host[1::2].tolist()
         live = [s for s, x in zip(steps, stopped) if not x]
         return (min(live) if live else None), max(steps), not live
+
+    # -- continuous batching ------------------------------------------------------------------------
+    def admit(self, rows):
+        """rows (ascending ints): back to the state begin gives them, processed memory from memory[row] / len32[row]."""
+        arr = (C.c_int32 * len(rows))(*rows)
+        self.eng._call(_capi.lib().t2_decoder_stream_admit, C.byref(self.args), arr, len(rows))
+
+    def launch_chunk(self, n, seed, skip_slices=()):
+        """Enqueue local steps [0, n) of every 64-row slice not in skip_slices (n < cap) under the Philox seed `seed`."""
+        assert 1 <= n < self.cap
+        self.args.dec.seed = seed
+        host = torch.tensor([[0, int(i in skip_slices)] for i in range(self.n_slices)], dtype=torch.int32)
+        self.eng._call(_capi.lib().t2_decoder_stream_run, C.byref(self.args), int(n), host.data_ptr())
+
+    def collect(self, entries):
+        """entries: (row, n_frames, T_text, mel, gate, align) -- the chunk's first n_frames frames of `row` go to the fp32
+        tensors mel (n_frames, 80), gate (n_frames,), align (n_frames, T_text) (views at the request's own step offset)."""
+        arr = (_capi.T2CollectRow * len(entries))(*[
+            _capi.T2CollectRow(r, n, T, 0, mel.data_ptr(), gate.data_ptr(), align.data_ptr())
+            for r, n, T, mel, gate, align in entries])
+        self.eng._call(_capi.lib().t2_decoder_stream_collect, C.byref(self.args), arr, len(entries))
+
+    def read_chunk(self):
+        """The one host sync of a chunk: (mel_lengths per row: local firing step + 1 or -1, steps run per slice)."""
+        host = self.readback.cpu().tolist()
+        return host[:self.B], host[self.B::2]

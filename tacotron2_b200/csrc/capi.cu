@@ -317,6 +317,29 @@ int t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n_st
   return persistent_stream_run(m, &a->dec, a->state, a->status, n_steps, status_host, (cudaStream_t)stream);
 }
 
+int t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int32_t* rows, int32_t n_rows, void* stream) {
+  T2_TRY(check_stream_args(m, a));
+  if (n_rows < 1 || n_rows > a->dec.B || !rows) return fail(T2_ERR_INVALID, "decoder stream admit: n_rows=%d outside [1, B=%d]", n_rows, a->dec.B);
+  if (!a->dec.memory_lengths) return fail(T2_ERR_INVALID, "decoder stream admit: the stream has no memory_lengths");
+  for (int i = 0; i < n_rows; ++i)
+    if (rows[i] < 0 || rows[i] >= a->dec.B || (i > 0 && rows[i] <= rows[i - 1]))
+      return fail(T2_ERR_INVALID, "decoder stream admit: rows must be ascending and inside [0, B=%d) (rows[%d]=%d)", a->dec.B, i, rows[i]);
+  return persistent_stream_admit(m, &a->dec, a->state, rows, n_rows, (cudaStream_t)stream);
+}
+
+int t2_decoder_stream_collect(T2Model* m, const T2DecoderStreamArgs* a, const T2CollectRow* rows, int32_t n_rows, void* stream) {
+  T2_TRY(check_stream_args(m, a));
+  if (n_rows < 1 || n_rows > a->dec.B || !rows) return fail(T2_ERR_INVALID, "decoder stream collect: n_rows=%d outside [1, B=%d]", n_rows, a->dec.B);
+  for (int i = 0; i < n_rows; ++i) {
+    const T2CollectRow& r = rows[i];
+    if (r.row < 0 || r.row >= a->dec.B || r.n_frames < 0 || r.n_frames > a->dec.n_steps_cap || r.T_text < 1 || r.T_text > a->dec.T_enc)
+      return fail(T2_ERR_INVALID, "decoder stream collect: entry %d (row %d, %d frames, T_text %d) outside B=%d, n_steps_cap=%d, T_enc=%d",
+                  i, r.row, r.n_frames, r.T_text, a->dec.B, a->dec.n_steps_cap, a->dec.T_enc);
+    if (!r.mel || !r.gate || !r.align) return fail(T2_ERR_INVALID, "decoder stream collect: entry %d has a null destination", i);
+  }
+  return persistent_stream_collect(&a->dec, rows, n_rows, (cudaStream_t)stream);
+}
+
 size_t t2_decoder_stash_bytes(const T2Model*, int32_t B, int32_t, int32_t T_mel) { return decoder_stash_bytes(B, T_mel); }
 size_t t2_decoder_backward_workspace_bytes(const T2Model*, int32_t B, int32_t T_enc, int32_t T_mel) {
   return decoder_backward_ws_bytes(B, T_enc, T_mel);

@@ -67,6 +67,10 @@ size_t persistent_stream_state_bytes(int B, int T_enc);
 int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, cudaStream_t s);
 int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n,
                           const int32_t* status_host, cudaStream_t s);
+// continuous batching: rows (ascending) back to the state begin gives them + their processed memory; a chunk's frames of
+// the listed rows to the requests' own buffers
+int persistent_stream_admit(T2Model* m, const T2DecoderArgs* a, void* state, const int32_t* rows, int n_rows, cudaStream_t s);
+int persistent_stream_collect(const T2DecoderArgs* a, const T2CollectRow* rows, int n_rows, cudaStream_t s);
 
 // tensor-core skinny GEMMs of the decoder backward (decoder_persistent.cu): which = 0 decoder LSTM (2560 columns),
 // 1 attention LSTM (1792 columns); K = 4096 gate rows in kBwdGemmSplit partial sums

@@ -1188,7 +1188,8 @@ static int persistent_stages(int T) {
   return want;
 }
 
-constexpr size_t kImagesBytes = (size_t)(4 + 16 + 8 + 16 + 4) * kXChunkBytes + (size_t)kRows * kAtt * 4;   // + q
+constexpr int kImageChunks = 4 + 16 + 8 + 16 + 4;          // K chunks of the x2, ah, ctx, dh and x1 images
+constexpr size_t kImagesBytes = (size_t)kImageChunks * kXChunkBytes + (size_t)kRows * kAtt * 4;   // + q
 
 // the persistent kernel's part of the decoder workspace: activation images x2 (4 chunks), ah (16), ctx (8), dh (16),
 // x1 (4) and q (64 x 128 fp32); for teacher forcing the x2 images of every step (cap x 4 chunks)
@@ -1429,7 +1430,7 @@ struct StreamSlice {
   float* pm;             // processed memory of the slice's rows (nb, T, 128)
 };
 // the slices one after the other; returns slice `b0 / kRows` (any slice when only measuring)
-static StreamSlice stream_state_layout(Carve& c, int B, int T, int b0) {
+__host__ __device__ static StreamSlice stream_state_layout(Carve& c, int B, int T, int b0) {
   const size_t tpp = (size_t)((T + kLocK - 1 + 3) & ~3);
   StreamSlice want = {};
   for (int b = 0; b < B; b += kRows) {
@@ -1476,6 +1477,90 @@ int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32
     p.t_end = n < a->n_steps_cap - t0 ? t0 + n : a->n_steps_cap;
     p.rs_acc = sl.acc; p.rs_cell = sl.cell; p.rs_att = sl.att; p.rs_done = sl.done; p.rs_status = status + 2 * si;
     T2_TRY(launch_persistent(p, s));
+  }
+  return T2_OK;
+}
+
+
+// ---------------------------------------------------------------------------------------------
+// continuous batching (t2_decoder_stream_admit / _collect): a stream whose rows are slots.  Between two chunks a row is
+// put back to the state begin gives it and handed another text; after a chunk the frames of every occupied row go to
+// the buffers of the request that holds it.
+// ---------------------------------------------------------------------------------------------
+namespace {
+struct RowMask { uint64_t w[kMaxBatch / 64]; };      // bit b: row b is listed
+
+// Block (r, slice) puts row r of its slice back to the state persistent_stream_begin leaves: zero is the initial value
+// of every piece (model.py:258-284 starts both LSTMs, the attention weights and the context at zero, and an accumulator
+// tile holds the partial products of zero activations).  It writes the row's own entries only.
+__global__ void __launch_bounds__(256) stream_admit_kernel(void* state, int B, int T, RowMask mask, int32_t* mel_lengths) {
+  const int lr = blockIdx.x, b0 = blockIdx.y * kRows, row = b0 + lr, tid = threadIdx.x;
+  if (row >= B || !((mask.w[row >> 6] >> (row & 63)) & 1ull)) return;
+  Carve c(state, 1024);
+  const StreamSlice sl = stream_state_layout(c, B, T, b0);
+  const int tpp = (T + kLocK - 1 + 3) & ~3;
+  for (int i = tid; i < kG * kAccPitch; i += 256)                  // its accumulator row in every CTA's tile
+    sl.acc[((size_t)(i / kAccPitch) * kRows + lr) * kAccPitch + i % kAccPitch] = 0.f;
+  for (int i = tid; i < kG * 4; i += 256)                          // its cell states: (CTA, column group)
+    reinterpret_cast<float4*>(sl.cell)[(size_t)i * kRows + lr] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = tid; i < 4 * tpp; i += 256)                         // previous | cumulative weights of CTAs lr and lr + 64
+    sl.att[(size_t)(lr + 64 * (i / (2 * tpp))) * 2 * tpp + i % (2 * tpp)] = 0.f;
+  for (int i = tid; i < kImageChunks * 2 * (kChunkK / 2); i += 256) {   // its row in both planes of every image chunk
+    const int chunk = i / kChunkK, plane = (i / (kChunkK / 2)) & 1, k = (i % (kChunkK / 2)) * 2;
+    __half* pl = reinterpret_cast<__half*>(sl.images + (size_t)chunk * kXChunkBytes) + plane * kRows * kChunkK;
+    *reinterpret_cast<uint32_t*>(pl + img_elem_offset(lr, k)) = 0u;
+  }
+  float* q = reinterpret_cast<float*>(sl.images + (size_t)kImageChunks * kXChunkBytes);
+  for (int i = tid; i < kAtt; i += 256) q[lr * kAtt + i] = 0.f;
+  if (tid == 0) { sl.done[lr] = 0; mel_lengths[row] = -1; }
+}
+
+struct CollectBatch { T2CollectRow r[kRows]; int n; };   // the listed rows of one 64-row slice, by value
+
+// block (t, i): frame t of the chunk buffers of row r[i].row -> frame t of that request's own buffers
+__global__ void __launch_bounds__(128) stream_collect_kernel(const CollectBatch cb, const float* __restrict__ mel,
+                                                             const float* __restrict__ gate, const float* __restrict__ align,
+                                                             int cap, int T) {
+  const T2CollectRow r = cb.r[blockIdx.y];
+  const int t = blockIdx.x, tid = threadIdx.x;
+  if (t >= r.n_frames) return;
+  const size_t src = (size_t)r.row * cap + t;
+  for (int i = tid; i < kMel; i += 128) r.mel[(size_t)t * kMel + i] = mel[src * kMel + i];
+  if (tid == 0) r.gate[t] = gate[src];
+  for (int i = tid; i < r.T_text; i += 128) r.align[(size_t)t * r.T_text + i] = align[src * T + i];
+}
+}  // namespace
+
+int persistent_stream_admit(T2Model* m, const T2DecoderArgs* a, void* state, const int32_t* rows, int n_rows, cudaStream_t s) {
+  RowMask mask;
+  memset(&mask, 0, sizeof(mask));
+  for (int i = 0; i < n_rows; ++i) mask.w[rows[i] >> 6] |= 1ull << (rows[i] & 63);
+  stream_admit_kernel<<<dim3(kRows, (a->B + kRows - 1) / kRows), 256, 0, s>>>(state, a->B, a->T_enc, mask, a->mel_lengths);
+  T2_LAUNCH_CHECK();
+  // processed memory of the listed rows: one GEMM per run of consecutive rows of a slice (rows are ascending)
+  for (int i = 0; i < n_rows;) {
+    int j = i + 1;
+    while (j < n_rows && rows[j] == rows[j - 1] + 1 && rows[j] / kRows == rows[i] / kRows) ++j;
+    const int b0 = rows[i] / kRows * kRows;
+    T2_TRY(processed_memory(m, a, rows[i], j - i, stream_slice(state, a->B, a->T_enc, b0).pm + (size_t)(rows[i] - b0) * a->T_enc * kAtt, s));
+    i = j;
+  }
+  return T2_OK;
+}
+
+int persistent_stream_collect(const T2DecoderArgs* a, const T2CollectRow* rows, int n_rows, cudaStream_t s) {
+  for (int b0 = 0; b0 < a->B; b0 += kRows) {
+    CollectBatch cb;
+    cb.n = 0;
+    int frames = 0;
+    for (int i = 0; i < n_rows; ++i)
+      if (rows[i].row >= b0 && rows[i].row < b0 + kRows && rows[i].n_frames > 0) {
+        cb.r[cb.n++] = rows[i];
+        frames = rows[i].n_frames > frames ? rows[i].n_frames : frames;
+      }
+    if (cb.n == 0) continue;
+    stream_collect_kernel<<<dim3(frames, cb.n), 128, 0, s>>>(cb, a->mel, a->gate, a->align, a->n_steps_cap, a->T_enc);
+    T2_LAUNCH_CHECK();
   }
   return T2_OK;
 }

@@ -730,5 +730,40 @@ class Tacotron2(_EngineOwner, nn.Module):
                        gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
                        mel_lengths=lengths.clone(), finished=finished)
 
+    def inference_server(self, slots=64, max_text_len=200, chunk_steps=32, seed=None):
+        """Continuous batching (README "serving a queue"): an ``InferenceServer`` that keeps ``slots`` decoder rows in
+        flight and refills a row with the next queued text as soon as its request has stopped.
+
+            server = model.inference_server(slots=64, max_text_len=200, chunk_steps=32)
+            rid = server.submit(text_ids, max_decoder_steps=None)      # 1-D integer tensor of 1..max_text_len ids
+            for result in server.run(): ...                            # or server.step(), one chunk at a time
+
+        A result is a dict: ``id``, ``mel_outputs`` / ``mel_outputs_postnet`` (1, n_mel, L), ``gate_outputs`` (1, L, 1),
+        ``alignments`` (1, L, T_text), ``mel_length`` and ``hit_max_steps`` -- the names and shapes inference() returns for
+        that text alone.  With injected prenet masks it equals that call bit for bit (serving.py).  Evaluation mode and the
+        persistent decoder only, as inference_stream.  The server owns its decoder state: several servers, streams and
+        inference() calls can be alive on one model.  seed: the session's Philox seed (default: the next engine seed)."""
+        from .serving import EngineBackend, InferenceServer
+        if self.training:
+            raise RuntimeError("tacotron2_b200: inference_server needs eval mode (training-mode BatchNorm uses the statistics "
+                               "of the whole sequence, so no postnet frame is final before the decoder ends)")
+        server = InferenceServer(None, slots, max_text_len, chunk_steps, self.decoder.max_decoder_steps)
+        server.backend = EngineBackend(self, server.slots, server.max_text_len, server.chunk_steps, seed)
+        return server
+
+    def inference_many(self, texts, slots=64, max_text_len=None, chunk_steps=32, max_decoder_steps=None):
+        """Every text of ``texts`` (1-D integer tensors) through an inference_server; returns the results in input order.
+        max_text_len: default the longest text; max_decoder_steps: one limit for all, or one per text."""
+        texts = list(texts)
+        if not texts:
+            return []
+        if max_text_len is None:
+            max_text_len = max(int(torch.as_tensor(t).numel()) for t in texts)
+        limits = max_decoder_steps if isinstance(max_decoder_steps, (list, tuple)) else [max_decoder_steps] * len(texts)
+        server = self.inference_server(min(int(slots), len(texts)), max(1, max_text_len), chunk_steps)
+        ids = [server.submit(t, limit) for t, limit in zip(texts, limits)]
+        results = {r["id"]: r for r in server.run()}
+        return [results[i] for i in ids]
+
 
 POSTNET_HALO = 10     # frames each side a postnet output depends on: 5 convolutions with k = 5 (model.py:103-146)
