@@ -1,10 +1,14 @@
-// The implicit GEMM on wgmma shared by WaveGlow (waveglow.cu) and the denoiser (denoiser.cu).
+// The implicit GEMM on wgmma shared by the Tacotron2 convolutions (conv_tc.cu), WaveGlow (waveglow.cu) and the denoiser
+// (denoiser.cu).
 //
 // A and the output are "k8 planes" (see conv_tc.cu): for each group of 8 channels a hi and a lo plane of [rows][8]
 // fp16.  The GEMM's K is a list of segments, each a run of 64-channel chunks of some planes read at a row shift, so a
 // strided or dilated convolution is one GEMM over shifted views of the same planes.  Every output row is computed
 // from its own A rows in a fixed order, so a row gets the same bits wherever it sits in a tile.  The epilogue is
 // chosen at compile time (EPI_*).
+//
+// The Tacotron2 convs (EPI_CONV) load one A tile of 132 rows per chunk instead: a k5 conv's 5 taps are that same tile
+// addressed with the descriptor start shifted by tap * 16 bytes, so the tile crosses shared memory once per chunk.
 //
 // Tiers: fp32-grade = hi*hi + lo*hi + hi*lo (3 MMAs per K step); fp16 = hi*hi only, lo planes neither read nor written.
 #pragma once
@@ -17,12 +21,8 @@
 namespace t2 {
 namespace {
 
-constexpr int kTile = 128;                  // rows (group columns / frames) per CTA
-constexpr int kSeg = kTile * 16;            // one k8 plane of a tile: 2048 bytes
-constexpr int kAStage = 16 * kSeg;          // 8 k8 groups x (hi, lo) = one 64-channel chunk
-constexpr int kNT = 128, kNH = 2, kWS = 4;  // MMA N per weight stage, stages per CTA column tile, weight ring
-constexpr int kWStage = kNT * 64 * 2 * 2;
-constexpr int kOutPitch = kNT * kNH + 4;
+constexpr int kTile = 128;                  // output rows (group columns / frames / padded rows) per CTA
+constexpr int kNT = 128, kWS = 4;           // MMA N per weight stage unless a caller picks another; weight ring stages
 constexpr int kThreads = 384;               // warp 0 producer; warpgroups 1 / 2: MMA + epilogue
 constexpr int kCluster = 2;                 // the CTAs of a cluster share each weight stage by multicast
 constexpr int kC = 256;                     // WaveGlow: WN channels (the skip rows of EPI_RESSKIP)
@@ -44,7 +44,13 @@ __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) {
     if (clock64() - t0 > kWd) __trap();
 }
 
-enum { EPI_UPSAMPLE = 0, EPI_GATE = 1, EPI_RESSKIP = 2, EPI_SPECTRAL = 3, EPI_OVERLAP = 4 };
+enum { EPI_UPSAMPLE = 0, EPI_GATE = 1, EPI_RESSKIP = 2, EPI_SPECTRAL = 3, EPI_OVERLAP = 4, EPI_CONV = 5 };
+
+// A tile rows beyond the output tile: EPI_CONV's tile m0 reads padded rows [m0 - 2, m0 + 130), every other epilogue
+// 128 rows per segment.
+constexpr int a_halo(int epi) { return epi == EPI_CONV ? 4 : 0; }
+constexpr int a_stage_bytes(int epi) { return 16 * (kTile + a_halo(epi)) * 16; }   // 8 k8 groups x (hi, lo) of a chunk
+constexpr int w_stage_bytes(int nt) { return nt * 64 * 2 * 2; }                    // hi + lo planes of nt rows x 64 k
 
 struct Seg { const __half* planes; long rows; int shift, nchunks; };
 struct GemmParams {
@@ -61,6 +67,13 @@ struct GemmParams {
   float strength;                                    // SPECTRAL: the magnitude loses bias * strength
   float* audio; long audio_pitch;                    // OVERLAP: fp32 rows (B, audio_pitch); row t writes block t - lo
   const double* wsq;                                 // OVERLAP: the squared window (1024)
+  // CONV: tile row q is padded row b * span + 2 + t (span = T + 4); y = act(acc * scale + bias), act 0 none, 1 relu,
+  // 2 tanh; out_mode 0 writes the planes `out`, 1 fp32 rows (row of (b, t) = b * out_seq_rows + t, pitch ldo),
+  // 2 fp32 (B, cout, T) plus the residual (B, T, cout); len: frames t >= len[b] are zeros in modes 0 and 2.
+  int taps;                                          // CONV: 5 (conv k5) or 1 (a GEMM on the centre rows)
+  const float* scale; int act, out_mode, cout;
+  float* out_f32; long ldo; int out_seq_rows;
+  const float* residual; long res_batch_stride;
 };
 
 template <int PASSES>
@@ -96,14 +109,20 @@ __device__ __forceinline__ bool tile_needed(const GemmParams& p, int mt) {
   return false;
 }
 
-template <int EPI, int PASSES>
+// NT = MMA N per weight stage, NH = weight stages (N halves) per CTA column tile
+template <int EPI, int PASSES, int NT = kNT, int NH = 2>
 __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
+  constexpr int kHalo = a_halo(EPI), kSeg = (kTile + kHalo) * 16, kAStage = a_stage_bytes(EPI);
+  constexpr int kWStage = w_stage_bytes(NT), kOutPitch = NT * NH + 4;
   constexpr uint32_t kABytes = PASSES == 3 ? kAStage : kAStage / 2;
   constexpr uint32_t kWBytes = PASSES == 3 ? kWStage : kWStage / 2;   // the hi plane comes first in a stage
+  // tap k reads the A tile from row tap0 + k; a single tap reads the centre rows of a halo tile
+  const int taps = EPI == EPI_CONV ? p.taps : 1, tap0 = taps == 1 ? kHalo / 2 : 0;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mt = p.mt0 + blockIdx.x, nt = blockIdx.y;
-  if (p.lo > 0 || p.hi < p.T) {
+  // EPI_CONV computes every tile: its planes epilogue is what writes the zero padding rows the next layer reads
+  if (EPI != EPI_CONV && (p.lo > 0 || p.hi < p.T)) {
     // both CTAs of a cluster take the same decision before any barrier: skip when neither tile holds a needed row.
     // A skipped tile writes nothing; its guard rows keep the zeros they were cleared to.  (With the full range every
     // launched cluster holds data rows.)
@@ -151,10 +170,11 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
             const __half* src = base + (((long)(cc * 8 + g) * 2 + hl) * rows + r0) * 8;
             ptx::bulk_g2s_hint(s_a + sa * kAStage + (hl * 8 + g) * kSeg, src, kSeg, &a_full[sa], pol_a);
           }
-        for (int h = 0; h < kNH; ++h) {
+        for (int th = 0; th < taps * NH; ++th) {
+          const int tap = th / NH, h = th - tap * NH;
           wait_bar(&w_empty[wst], wph ^ 1);
           ptx::mbar_arrive_expect_tx(&w_full[wst], kWBytes);
-          const uint8_t* wsrc = p.wimg + ((size_t)(nt * kNH + h) * p.nchunks + c) * kWStage;
+          const uint8_t* wsrc = p.wimg + (((size_t)(nt * NH + h) * p.nchunks + c) * taps + tap) * kWStage;
           const uint32_t slice = kWBytes / kCluster;
           ptx::bulk_g2s_mc_hint(s_w + wst * kWStage + rank * slice, wsrc + rank * slice, slice, &w_full[wst],
                                 (uint16_t)((1u << kCluster) - 1u), pol_w);
@@ -165,42 +185,44 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
     __syncwarp();
   } else if (tid >= 128) {
     const int wg = (tid >> 7) - 1, wt = tid & 127;
-    float d[kNH][kNT / 2];
+    float d[NH][NT / 2];
 #pragma unroll
-    for (int h = 0; h < kNH; ++h) {
+    for (int h = 0; h < NH; ++h) {
 #pragma unroll
-      for (int i = 0; i < kNT / 2; ++i) d[h][i] = 0.f;
-      ptx::wg_fence_regs<kNT / 2>(d[h]);
+      for (int i = 0; i < NT / 2; ++i) d[h][i] = 0.f;
+      ptx::wg_fence_regs<NT / 2>(d[h]);
     }
     uint32_t wst = 0, wph = 0;
     for (int c = 0; c < p.nchunks; ++c) {
       const int sa = c & 1;
       wait_bar(&a_full[sa], (c >> 1) & 1);
       const uint32_t ab = ptx::smem_u32(s_a + sa * kAStage) + (uint32_t)wg * (64 * 16);
+      for (int tap = 0; tap < taps; ++tap) {
 #pragma unroll
-      for (int h = 0; h < kNH; ++h) {
-        wait_bar(&w_full[wst], wph);
-        const uint32_t wb = ptx::smem_u32(s_w + wst * kWStage);
-        ptx::wg_fence();
+        for (int h = 0; h < NH; ++h) {
+          wait_bar(&w_full[wst], wph);
+          const uint32_t wb = ptx::smem_u32(s_w + wst * kWStage);
+          ptx::wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint32_t aoff = (2 * kk) * kSeg;
-          const uint64_t a_hi = ptx::make_smem_desc(ab + aoff, kSeg, 128);
-          const uint64_t b_hi = ptx::make_sw128_desc(wb + kk * 32);
-          ptx::wgmma_f16<kNT>(d[h], a_hi, b_hi);
-          if (PASSES == 3) {
-            const uint64_t a_lo = ptx::make_smem_desc(ab + 8 * kSeg + aoff, kSeg, 128);
-            const uint64_t b_lo = ptx::make_sw128_desc(wb + kNT * 128 + kk * 32);
-            ptx::wgmma_f16<kNT>(d[h], a_lo, b_hi);
-            ptx::wgmma_f16<kNT>(d[h], a_hi, b_lo);
+          for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t aoff = (2 * kk) * kSeg + (tap + tap0) * 16;
+            const uint64_t a_hi = ptx::make_smem_desc(ab + aoff, kSeg, 128);
+            const uint64_t b_hi = ptx::make_sw128_desc(wb + kk * 32);
+            ptx::wgmma_f16<NT>(d[h], a_hi, b_hi);
+            if (PASSES == 3) {
+              const uint64_t a_lo = ptx::make_smem_desc(ab + 8 * kSeg + aoff, kSeg, 128);
+              const uint64_t b_lo = ptx::make_sw128_desc(wb + NT * 128 + kk * 32);
+              ptx::wgmma_f16<NT>(d[h], a_lo, b_hi);
+              ptx::wgmma_f16<NT>(d[h], a_hi, b_lo);
+            }
           }
+          ptx::wg_commit();
+          ptx::wg_wait<0>();
+          ptx::wg_fence_regs<NT / 2>(d[h]);
+          if (wt == 0)                       // this warpgroup is done with the weight stage in every CTA of the cluster
+            for (int r = 0; r < kCluster; ++r) ptx::mbar_arrive_cluster(&w_empty[wst], r);
+          if (++wst == kWS) { wst = 0; wph ^= 1; }
         }
-        ptx::wg_commit();
-        ptx::wg_wait<0>();
-        ptx::wg_fence_regs<kNT / 2>(d[h]);
-        if (wt == 0)
-          for (int r = 0; r < kCluster; ++r) ptx::mbar_arrive_cluster(&w_empty[wst], r);
-        if (++wst == kWS) { wst = 0; wph ^= 1; }
       }
       if (wt == 0) ptx::mbar_arrive(&a_empty[sa]);
     }
@@ -208,10 +230,10 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
     ptx::named_bar_sync(1, 256);
     float* s_out = reinterpret_cast<float*>(smem);
 #pragma unroll
-    for (int h = 0; h < kNH; ++h)
+    for (int h = 0; h < NH; ++h)
 #pragma unroll
-      for (int i = 0; i < kNT / 2; i += 2) {
-        const int r = wg * 64 + ptx::wg_frag_row(i, wt), col = h * kNT + ptx::wg_frag_col(i, wt);
+      for (int i = 0; i < NT / 2; i += 2) {
+        const int r = wg * 64 + ptx::wg_frag_row(i, wt), col = h * NT + ptx::wg_frag_col(i, wt);
         *reinterpret_cast<float2*>(s_out + r * kOutPitch + col) = make_float2(d[h][i], d[h][i + 1]);
       }
     ptx::named_bar_sync(1, 256);
@@ -317,13 +339,59 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
             *reinterpret_cast<float4*>(dst + c) = make_float4(v[0], v[1], v[2], v[3]);
           }
         }
+      } else if (EPI == EPI_CONV) {
+        // thread = (tile row r, every other group of 8 columns); frame pt of sequence b is tile row q
+        const int pt = t - 2;
+        const bool in_seq = b < p.B && pt >= 0 && pt < p.T;
+        // planes output: frames t >= len[b] are written as zeros, the padding a sequence of that length has alone
+        const bool in_len = in_seq && (p.out_mode != 0 || p.len == nullptr || pt < p.len[b]);
+        const int n0 = nt * NT * NH;
+        for (int c0 = half * 8; c0 < NT * NH; c0 += 16) {
+          float v[8];
+          const float4 v0 = *reinterpret_cast<const float4*>(row + c0);
+          const float4 v1 = *reinterpret_cast<const float4*>(row + c0 + 4);
+          v[0] = v0.x; v[1] = v0.y; v[2] = v0.z; v[3] = v0.w; v[4] = v1.x; v[5] = v1.y; v[6] = v1.z; v[7] = v1.w;
+          if (n0 + c0 >= p.cout) continue;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int n = n0 + c0 + i;
+            float x = v[i] * p.scale[n] + p.bias[n];
+            if (p.act == 1) x = fmaxf(x, 0.f);
+            else if (p.act == 2) x = tanhf(x);
+            v[i] = in_len ? x : 0.f;
+          }
+          if (p.out_mode == 0) {          // next layer's planes (zeros in the padding rows); plane row = q + 2
+            const int g = (n0 + c0) >> 3;
+            store8<3>(p.out, p.out_rows, g, q + 2, v);
+            // the 2 guard rows at both ends of the plane stay zero
+            if (q == 0 || q == (long)p.n_tiles_m * kTile - 1) {
+              const float z[8] = {};
+              const long gr = q == 0 ? 0 : q + 3;
+              for (int k = 0; k < 2; ++k) store8<3>(p.out, p.out_rows, g, gr + k, z);
+            }
+          } else if (in_seq && p.out_mode == 1) {   // fp32 rows (b * out_seq_rows + t, ldo)
+            float* o = p.out_f32 + ((long)b * p.out_seq_rows + pt) * p.ldo + n0 + c0;
+            *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
+            *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
+          } else if (in_seq && p.out_mode == 2) {   // (B, cout, T) + residual (B, T, cout), masked beyond len
+            const bool keep = p.len == nullptr || pt < p.len[b];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int n = n0 + c0 + i;
+              float x = v[i];
+              if (p.residual) x += p.residual[(long)b * p.res_batch_stride + (long)pt * p.cout + n];
+              p.out_f32[((long)b * p.cout + n) * p.T + pt] = keep ? x : 0.f;
+            }
+          }
+        }
       }
     }
   }
   __syncthreads();
-  // peers' consumers arrive on our w_empty barriers: drain before leaving
+  // peers' consumers arrive on our w_empty barriers: drain before leaving (producer thread state is gone here, so wait
+  // on the parity each barrier reaches after its last use)
   if (tid == 0) {
-    const int total = p.nchunks * kNH;
+    const int total = p.nchunks * taps * NH;
     for (int i = 0; i < kWS; ++i) {
       const int uses = (total - i + kWS - 1) / kWS;
       if (uses > 0) wait_bar(&w_empty[i], (uses - 1) & 1);
@@ -333,11 +401,12 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
   ptx::cluster_sync_all();
 }
 
-template <int EPI, int PASSES>
+template <int EPI, int PASSES, int NT = kNT, int NH = 2>
 int launch_gemm(GemmParams p, int n_tiles_n, cudaStream_t s) {
-  const size_t smem = (size_t)kWS * kWStage + 2 * kAStage + (4 + 2 * kWS) * 8 + 64;
-  static_assert(kTile * kOutPitch * 4 <= kWS * kWStage + 2 * kAStage, "output tile reuses the operand stages");
-  T2_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<EPI, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  constexpr int kOperands = kWS * w_stage_bytes(NT) + 2 * a_stage_bytes(EPI);
+  static_assert(kTile * (NT * NH + 4) * 4 <= kOperands, "output tile reuses the operand stages");
+  const size_t smem = (size_t)kOperands + (4 + 2 * kWS) * 8 + 64;
+  T2_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<EPI, PASSES, NT, NH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   // the grid spans the tiles from the first needed row (sequence 0, t = lo) to the last (sequence B-1, t = hi-1)
@@ -349,7 +418,7 @@ int launch_gemm(GemmParams p, int n_tiles_n, cudaStream_t s) {
   at.id = cudaLaunchAttributeClusterDimension;
   at.val.clusterDim.x = kCluster; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
   cfg.attrs = &at; cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, wg_gemm_kernel<EPI, PASSES>, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, wg_gemm_kernel<EPI, PASSES, NT, NH>, p);
   if (e != cudaSuccess) return fail(T2_ERR_CUDA, "wgmma gemm launch failed: %s", cudaGetErrorString(e));
   g_launch_count++;
   return T2_OK;

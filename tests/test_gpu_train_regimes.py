@@ -2,8 +2,8 @@
 against the oracle in float64; the training-mode conv stack forward without autograd.
 
 Every gradient comes from three split-fp16 engines: gemm_tc (the LSTM products and the forward convs), wgrad_tc (the decoder
-LSTM and the conv weight gradients) and conv_tc (the conv input gradients).  Each scales its fp32 operands by powers of two
-before splitting them into fp16 hi / lo halves, so:
+LSTM and the conv weight gradients) and wg_gemm with its conv epilogue (the conv input gradients, through conv_tc).  Each
+scales its fp32 operands by powers of two before splitting them into fp16 hi / lo halves, so:
 
 * A backward is linear in its upstream gradient and every scale is a power of two: multiplying the seeds by 2^k must
   multiply every gradient by exactly 2^k (bit for bit), at any magnitude and with channels whose gradient is all zero (a
@@ -12,7 +12,7 @@ before splitting them into fp16 hi / lo halves, so:
 * wgrad_tc splits its K dimension (decoder steps, or 64-row chunks of the conv's padded rows) into segments of
   wgrad_seg(n) = 100 chunks, 150 once there would be more than 15 segments; the cases below land on full, partial and
   single-chunk last segments and on both sides of the switch.
-* conv_tc runs 128-row tiles of the padded rows, in clusters of 2 (an odd tile count adds a padding tile).
+* wg_gemm runs a conv on 128-row tiles of the padded rows, in clusters of 2 (an odd tile count adds a padding tile).
 
 Bars: 1e-3 relative (max |a - b| / max |b|) on gradients, as tests/test_gpu_backward.py; 1e-4 on Encoder and Postnet
 outputs, as tests/test_gpu_parity.py.  Every case prints its worst error."""
