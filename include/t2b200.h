@@ -577,6 +577,15 @@ int t2_selftest_gemm_tc(int32_t ta, int32_t tb, int32_t M, int32_t N, int32_t K,
                         const float* B, int64_t ldb, float* C, int64_t ldc, float beta, int32_t batch,
                         int64_t strideA, int64_t strideB, int64_t strideC, void* stream);
 int t2_selftest_colsum(const float* X, int64_t ld, int64_t rows, int32_t cols, float* out, void* stream);
+/* t2_waveglow_infer_window's own launch sequence for `a`, left after its first n_launches launches (0 ... 207: mel to
+ * planes, the upsample GEMM, the initial tail, then per flow 11 ... 0 eight (gate GEMM, res/skip GEMM) pairs and a
+ * tail), and the workspace as it then stands unpacked into fp32 device buffers; a NULL buffer is skipped.  Row
+ * q = b * span + t, span = 32 T_mel + 128, rows = 128 ceil(B span / 128); channel c of the planes (spect, h, acts) is
+ * hi + lo in the fp32-grade tier and hi in the fp16 tier.  skip and aud are not cleared between calls: rows no launch
+ * has written yet hold what an earlier call left. */
+int t2_selftest_waveglow_state(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, int32_t n_launches, float* spect /* (rows, 640) */,
+                               float* hbuf /* (rows, 256) */, float* acts /* (rows, 256) */, float* skip /* (rows, 256) */,
+                               float* aud /* (rows, 8) */, void* stream);
 #endif
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* After a T2_IMPL_PERSISTENT run with the same args / workspace: SM cycles spent per phase of the

@@ -294,7 +294,8 @@ def lib():
 
 
 SELFTEST_LIB_PATH = os.path.join(_HERE, "libt2b200_selftest.so")
-SELFTEST_EXPORTS = ["t2_selftest_umma", "t2_selftest_event", "t2_selftest_mma_rate", "t2_selftest_mma_group", "t2_selftest_gemm_tc", "t2_selftest_colsum"]
+SELFTEST_EXPORTS = ["t2_selftest_umma", "t2_selftest_event", "t2_selftest_mma_rate", "t2_selftest_mma_group", "t2_selftest_gemm_tc", "t2_selftest_colsum",
+                    "t2_selftest_waveglow_state"]
 _selftest_lib = None
 
 
@@ -315,6 +316,12 @@ def selftest_lib():
                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_float, C.c_int32, C.c_int64,
                                           C.c_int64, C.c_int64, C.c_void_p]
         L.t2_selftest_colsum.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]
+        L.t2_selftest_waveglow_state.argtypes = [C.c_void_p, C.POINTER(T2WaveGlowWindowArgs), C.c_int32] + [C.c_void_p] * 6
+        L.t2_waveglow_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(T2WaveGlowConfig), C.POINTER(C.c_void_p),
+                                         C.c_int32, C.c_void_p]
+        L.t2_waveglow_destroy.argtypes = [C.c_void_p]
+        L.t2_waveglow_workspace_bytes.restype = C.c_size_t
+        L.t2_waveglow_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         _selftest_lib = L
     return _selftest_lib
 

@@ -579,6 +579,10 @@ int t2_selftest_colsum(const float* X, int64_t ld, int64_t rows, int32_t cols, f
   static T2Model scratch_owner;
   return colsum_f32(&scratch_owner, (cudaStream_t)stream, X, ld, rows, cols, out);
 }
+int t2_selftest_waveglow_state(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, int32_t n_launches, float* spect, float* hbuf,
+                               float* acts, float* skip, float* aud, void* stream) {
+  return waveglow_state(h, a, n_launches, spect, hbuf, acts, skip, aud, (cudaStream_t)stream);
+}
 #endif
 
 }  // extern "C"

@@ -47,6 +47,17 @@ namespace t2 {
 namespace {
 
 constexpr int kFlows = 12, kLayers = 8, kCond = 640, kGroup = 8;
+#ifdef T2_SELFTEST
+// waveglow_infer_window enqueues mel_to_planes, the upsample GEMM, the initial tail, then per flow 8 x (gate GEMM,
+// res/skip GEMM) and a tail.
+constexpr int kLaunches = 3 + kFlows * (2 * kLayers + 1);
+// waveglow_state reads the workspace between two launches: waveglow_infer_window returns before launch g_stop_before
+// (counted from 0; -1: never).  The product build has no stop points.
+int g_stop_before = -1, g_launched = 0;
+#define WG_STOP_POINT() do { if (g_launched++ == g_stop_before) return T2_OK; } while (0)
+#else
+#define WG_STOP_POINT() do {} while (0)
+#endif
 constexpr int kGuard = 128;                 // zero rows around each sequence in the column domain (max dilation)
 constexpr int kFGuard = 4;                  // frame domain: 4 zero frames after each sequence (3 taps look back)
 constexpr int kUpK = 4 * 128;               // upsample K: 4 taps x 80 mels padded to 128
@@ -344,6 +355,21 @@ void ws_layout(Carve& c, int B, int T, WsLayout* o) {
   o->aud = c.take<float>((size_t)d.ntm * kTile * 8, 1024);
 }
 
+#ifdef T2_SELFTEST
+// planes -> fp32 rows (n_rows, 8 groups): tile row q is plane row kGuard + q; hi + lo in the fp32 tier, hi in the fp16 tier
+__global__ void unpack_planes_kernel(const __half* __restrict__ planes, long rows, int passes, long n_rows,
+                                     float* __restrict__ out) {
+  const long q = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int g = blockIdx.y, groups = gridDim.y;
+  if (q >= n_rows) return;
+  float v[8];
+  if (passes == 3) load8<3>(planes, rows, g, kGuard + q, v);
+  else load8<1>(planes, rows, g, kGuard + q, v);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) out[(q * groups + g) * 8 + i] = v[i];
+}
+#endif
+
 }  // namespace
 
 // ---- host API -----------------------------------------------------------------------------------------
@@ -471,6 +497,7 @@ int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStr
   T2_CUDA(cudaMemsetAsync(o.spect, 0, (size_t)80 * 2 * o.rows * 16, s));
   T2_CUDA(cudaMemsetAsync(o.h, 0, (size_t)32 * 2 * o.rows * 16, s));
   T2_CUDA(cudaMemsetAsync(o.acts, 0, (size_t)32 * 2 * o.rows * 16, s));
+  WG_STOP_POINT();
   mel_to_planes_kernel<<<dim3((unsigned)((o.x_rows + 127) / 128), 16), 128, 0, s>>>(a->mel, a->io_half, B, T, a->lengths,
                                                                                   o.x, o.x_rows, passes);
   T2_LAUNCH_CHECK();
@@ -481,6 +508,7 @@ int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStr
   u.nseg = 4; u.nchunks = 8; u.row0 = kFGuard; u.wimg = m->up_img; u.n_tiles_m = d.ntf;
   u.B = B; u.span = d.spanf; u.T = T; u.lo = 0; u.hi = T; u.bias = m->up_bias;
   u.out = o.spect; u.out_rows = o.rows; u.out_row0 = kGuard; u.col_span = d.span;
+  WG_STOP_POINT();
   T2_TRY(gemm<EPI_UPSAMPLE>(u, 80, fp16, s));
 
   // Per-flow column ranges.  The audio columns [32 out0, 32 out1) need the output of the flow that runs with n flows
@@ -507,6 +535,7 @@ int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStr
     T2_LAUNCH_CHECK();
     return T2_OK;
   };
+  WG_STOP_POINT();
   T2_TRY(tail(kFlows, kFlows - 1));
   GemmParams g;
   memset(&g, 0, sizeof(g));
@@ -521,16 +550,44 @@ int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStr
       g.seg[3] = Seg{o.spect, o.rows, 0, 10};
       g.nseg = 4; g.nchunks = 22; g.wimg = m->gate_img[k][l]; g.bias = m->gate_bias + ((size_t)k * kLayers + l) * 512;
       g.out = o.acts;
+      WG_STOP_POINT();
       T2_TRY(gemm<EPI_GATE>(g, 2, fp16, s));
       // res_skip_layers (glow.py:168-173)
       g.seg[0] = Seg{o.acts, o.rows, 0, 4};
       g.nseg = 1; g.nchunks = 4; g.wimg = m->rs_img[k][l]; g.bias = m->rs_bias + ((size_t)k * kLayers + l) * 512;
       g.out = o.h; g.first = l == 0; g.res_tiles = l < kLayers - 1 ? 1 : 0;
+      WG_STOP_POINT();
       T2_TRY(gemm<EPI_RESSKIP>(g, l < kLayers - 1 ? 2 : 1, fp16, s));
     }
+    WG_STOP_POINT();
     T2_TRY(tail(k, k > 0 ? k - 1 : -1));
   }
   return T2_OK;
 }
+
+#ifdef T2_SELFTEST
+int waveglow_state(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, int n_launches, float* spect, float* hbuf, float* acts,
+                   float* skip, float* aud, cudaStream_t s) {
+  if (n_launches < 0 || n_launches > kLaunches)
+    return fail(T2_ERR_INVALID, "waveglow state: n_launches %d is not in [0, %d]", n_launches, kLaunches);
+  g_launched = 0; g_stop_before = n_launches;
+  const int r = waveglow_infer_window(m, wa, s);
+  g_stop_before = -1;
+  T2_TRY(r);
+  const int B = wa->wg.B, T = wa->wg.T_mel, passes = m->fp16 ? 1 : 3;
+  Carve c(wa->wg.ws, 1024);
+  WsLayout o;
+  ws_layout(c, B, T, &o);
+  const long n = (long)dims_of(B, T).ntm * kTile;
+  const unsigned blocks = (unsigned)((n + 127) / 128);
+  if (spect) unpack_planes_kernel<<<dim3(blocks, kCond / 8), 128, 0, s>>>(o.spect, o.rows, passes, n, spect);
+  if (hbuf) unpack_planes_kernel<<<dim3(blocks, kC / 8), 128, 0, s>>>(o.h, o.rows, passes, n, hbuf);
+  if (acts) unpack_planes_kernel<<<dim3(blocks, kC / 8), 128, 0, s>>>(o.acts, o.rows, passes, n, acts);
+  T2_CUDA(cudaGetLastError());
+  if (skip) T2_CUDA(cudaMemcpyAsync(skip, o.skip, (size_t)n * kC * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if (aud) T2_CUDA(cudaMemcpyAsync(aud, o.aud, (size_t)n * 8 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return T2_OK;
+}
+#endif
 
 }  // namespace t2

@@ -13,5 +13,9 @@ size_t waveglow_ws_bytes(int B, int T_mel);
 int    waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, cudaStream_t s);
 int    waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, cudaStream_t s);
 void   waveglow_window_halo(int* left, int* right);
+#ifdef T2_SELFTEST
+int    waveglow_state(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, int n_launches, float* spect, float* hbuf, float* acts,
+                      float* skip, float* aud, cudaStream_t s);
+#endif
 
 }  // namespace t2

@@ -1,4 +1,7 @@
-"""WaveGlow.infer on the H100 against the reference's fixtures and the fp64 oracle (bar: 1e-3 relative)."""
+"""WaveGlow.infer on the H100 against the reference's fixtures (bar: 1e-3 relative) and the fp64 oracle.
+
+E64_BAR: the fp32-grade tier's audio against the fp64 oracle measures 0.9e-5 ... 1.3e-5 on an H100 over these cases;
+the bar is about 4 x that.  (tests/test_gpu_waveglow_stages.py holds each of the 207 launches to its own bar.)"""
 import os
 
 import numpy as np
@@ -13,6 +16,8 @@ import tacotron2_b200 as t2
 from tacotron2_b200 import _capi
 
 pytestmark = pytest.mark.gpu
+
+E64_BAR = 5e-5
 
 _SD = {}
 
@@ -54,7 +59,7 @@ def test_fp32_tier_matches_reference_and_fp64_oracle(name):
     truth = WO.infer(sd7(), mel.cuda().double(), sigma, z.cuda().double())
     e_ref, e64 = rel_err(out, torch.from_numpy(g["audio"])), rel_err(out, truth)
     print("%s: engine vs reference %.2e, vs fp64 oracle %.2e" % (name, e_ref, e64))
-    assert e_ref <= 1e-3 and e64 <= 1e-3
+    assert e_ref <= 1e-3 and e64 <= E64_BAR
 
 
 def test_ragged_rows_are_bit_identical_to_their_own_runs():
@@ -70,7 +75,7 @@ def test_ragged_rows_are_bit_identical_to_their_own_runs():
     truth = WO.infer(sd7(), mel[:1].cuda().double(), 0.666, z[:1].cuda().double())
     e = rel_err(out[0], truth[0])
     print("ragged: full-length row vs fp64 oracle %.2e" % e)
-    assert e <= 1e-3
+    assert e <= E64_BAR
 
 
 def test_philox_noise_matches_host_rebuild_and_is_reproducible():
@@ -86,7 +91,7 @@ def test_philox_noise_matches_host_rebuild_and_is_reproducible():
     truth = WO.infer(sd7(), mel.cuda().double(), 0.666, philox_noise(seed, B, T).cuda().double())
     e = rel_err(a, truth)
     print("philox: engine vs fp64 oracle on the host-rebuilt noise %.2e" % e)
-    assert e <= 1e-3
+    assert e <= E64_BAR
     c = run(m, mel, 0.666)                     # the next call draws fresh noise
     assert not torch.equal(a, c)
 

@@ -98,6 +98,42 @@ def test_oracle_fp64_is_consistent_across_rows():
     assert rel_err(both[1:], one) < 1e-12
 
 
+def test_oracle_steps_compose_to_infer_bit_for_bit():
+    """infer is the composition of the oracle's named steps.  Its fp64 and fp16-emulating outputs on a seeded case are
+    the bits recorded before infer was split into steps (tests/golden/waveglow_oracle_b2_t3.npz, one CPU thread), and the
+    steps called one by one -- as the per-launch GPU tests call them, each gate computing its own slice of the
+    conditioning -- give the same audio."""
+    g = load("waveglow_oracle_b2_t3")
+    sd = synth_state_dict(7)
+    sd16 = {k: (v.half() if not k.startswith("convinv") else v) for k, v in sd.items()}
+    mel, z, sigma = mel_input(2, 3, 101), noise(2, 3, 102), 0.666
+
+    def by_steps(sd, mel, z):
+        spect = WO.upsample_unfold(sd, mel)
+        aud = sigma * z[:, :WO.n_remaining(11)]
+        for k in reversed(range(12)):
+            h = WO.start(sd, k, aud)
+            skip = torch.zeros_like(h)
+            for l in range(8):
+                acts = WO.gate(sd, k, l, h, spect)
+                h, skip = WO.res_skip(sd, k, l, acts, h, skip)
+            aud = WO.flow_tail(sd, k, aud, skip, z, sigma)
+        return aud.permute(0, 2, 1).contiguous().view(mel.shape[0], -1)
+
+    threads = torch.get_num_threads()
+    torch.set_num_threads(1)
+    try:
+        a64 = WO.infer(sd, mel, sigma, z)
+        a16 = WO.infer(sd16, mel.half(), sigma, z.half(), torch.float16)
+        s64, s16 = by_steps(sd, mel.double(), z.double()), by_steps(sd16, mel.half(), z.half())
+    finally:
+        torch.set_num_threads(threads)
+    assert a64.dtype == torch.float64 and a16.dtype == torch.float16
+    assert np.array_equal(a64.numpy(), g["a64"]) and np.array_equal(a16.numpy(), g["a16"])
+    assert torch.equal(s64, a64) and torch.equal(s16, a16)
+    assert [WO.n_remaining(k) for k in (11, 8, 7, 4, 3, 0)] == [4, 4, 6, 6, 8, 8]
+
+
 def test_waveglow_ctypes_structs_match_c_layout(tmp_path):
     src = tmp_path / "layout.c"
     fields = {
