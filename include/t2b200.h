@@ -554,6 +554,51 @@ typedef struct T2DenoiserWindowArgs {
 void   t2_denoiser_window_halo(int32_t* left, int32_t* right);
 int    t2_denoiser_run_window(T2Denoiser* h, const T2DenoiserWindowArgs* a, void* stream);
 
+/* ---- STFT transform / inverse and Griffin-Lim (stft.py:69-141, audio_processing.py:59-75) -------------------------
+ * They run on the T2Denoiser handle: it holds the packed STFT bases, so the same configuration rules apply (filter_length
+ * 1024, hop 256, win_length 1024, periodic Hann; other configurations are refused by t2_denoiser_create with
+ * T2_ERR_UNSUPPORTED) and the same arithmetic (split-fp16 operands, fp32 accumulation).  Each row's operands are scaled
+ * by a power of two taken on the device from its largest magnitude (or sample) and the fp32 outputs undo it exactly:
+ * inputs of any scale are supported away from fp32 overflow and underflow, and a power-of-two scale of a row's input
+ * scales its output bit for bit.  Every row's output depends only on that row.  Invalid arguments return
+ * T2_ERR_INVALID (too small a workspace T2_ERR_WORKSPACE) before anything is launched. */
+
+/* transform (stft.py:69-94): audio (B, n) fp32 -> magnitude and phase (atan2), each (B, 513, n / 256 + 1) fp32.
+ * lengths (B) int32 in samples or NULL: row b is transformed as its first lengths[b] samples alone (a value outside
+ * [0, n] counts as n) and its frames from lengths[b] / 256 + 1 on are zero; a row of <= 512 samples cannot be
+ * reflect-padded and gives zeros.  Without lengths n must exceed 512.
+ * Workspace: t2_stft_transform_workspace_bytes(h, B, n). */
+typedef struct T2StftTransformArgs {
+  const float* audio; int32_t B, n; const int32_t* lengths;
+  float* magnitude; float* phase;
+  void* ws; size_t ws_bytes;
+} T2StftTransformArgs;
+size_t t2_stft_transform_workspace_bytes(const T2Denoiser* h, int32_t B, int32_t n);
+int    t2_stft_transform(T2Denoiser* h, const T2StftTransformArgs* a, void* stream);
+
+/* inverse (stft.py:96-136): magnitude and phase (B, 513, F) fp32, F >= 4 -> out (B, 256 (F - 1)) fp32, 16-byte
+ * aligned.  lengths (B) int32 in frames or NULL: row b is the inverse of its first lengths[b] frames alone (a value
+ * outside [0, F] counts as F), and its output from sample 256 (lengths[b] - 1) on is zero; a row of fewer than 4 frames
+ * gives zeros.  Workspace: t2_stft_inverse_workspace_bytes(h, B, F). */
+typedef struct T2StftInverseArgs {
+  const float* magnitude; const float* phase; int32_t B, F; const int32_t* lengths;
+  float* out;
+  void* ws; size_t ws_bytes;
+} T2StftInverseArgs;
+size_t t2_stft_inverse_workspace_bytes(const T2Denoiser* h, int32_t B, int32_t F);
+int    t2_stft_inverse(T2Denoiser* h, const T2StftInverseArgs* a, void* stream);
+
+/* Griffin-Lim (audio_processing.py:59-75): signal = inverse(magnitude, inv.phase), then n_iters >= 0 times signal =
+ * inverse(magnitude, phase of transform(signal)); out = the final signal.  inv.phase holds the initial angles; shapes
+ * and lengths as t2_stft_inverse.  3 n_iters + 2 kernel launches, no host synchronisation.
+ * Workspace: t2_griffin_lim_workspace_bytes(h, B, F). */
+typedef struct T2GriffinLimArgs {
+  T2StftInverseArgs inv;
+  int32_t n_iters;
+} T2GriffinLimArgs;
+size_t t2_griffin_lim_workspace_bytes(const T2Denoiser* h, int32_t B, int32_t F);
+int    t2_griffin_lim(T2Denoiser* h, const T2GriffinLimArgs* a, void* stream);
+
 /* ---- self tests (libt2b200_selftest.so only: the same sources built with -DT2_SELFTEST; not part of the product
  * library) -------------------------------------------------------------------------------------------------
  * t2_selftest_umma: runs the wgmma split-fp16 GEMM engine used by the persistent decoder on a

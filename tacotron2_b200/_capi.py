@@ -34,6 +34,8 @@ EXPORTS = [
     "t2_waveglow_infer", "t2_waveglow_infer_window", "t2_waveglow_window_halo",
     "t2_denoiser_create", "t2_denoiser_refresh", "t2_denoiser_destroy", "t2_denoiser_bias",
     "t2_denoiser_workspace_bytes", "t2_denoiser_run", "t2_denoiser_run_window", "t2_denoiser_window_halo",
+    "t2_stft_transform_workspace_bytes", "t2_stft_transform", "t2_stft_inverse_workspace_bytes", "t2_stft_inverse",
+    "t2_griffin_lim_workspace_bytes", "t2_griffin_lim",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686
 
@@ -196,6 +198,20 @@ class T2DenoiserWindowArgs(C.Structure):
                 ("at_end", C.c_int32)]
 
 
+class T2StftTransformArgs(C.Structure):
+    _fields_ = [("audio", C.c_void_p), ("B", C.c_int32), ("n", C.c_int32), ("lengths", C.c_void_p),
+                ("magnitude", C.c_void_p), ("phase", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
+class T2StftInverseArgs(C.Structure):
+    _fields_ = [("magnitude", C.c_void_p), ("phase", C.c_void_p), ("B", C.c_int32), ("F", C.c_int32),
+                ("lengths", C.c_void_p), ("out", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
+class T2GriffinLimArgs(C.Structure):
+    _fields_ = [("inv", T2StftInverseArgs), ("n_iters", C.c_int32)]
+
+
 _lib = None
 
 
@@ -287,6 +303,11 @@ def lib():
     L.t2_denoiser_run_window.argtypes = [C.c_void_p, C.POINTER(T2DenoiserWindowArgs), C.c_void_p]
     L.t2_denoiser_window_halo.restype = None
     L.t2_denoiser_window_halo.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    for n, args in (("t2_stft_transform", T2StftTransformArgs), ("t2_stft_inverse", T2StftInverseArgs),
+                    ("t2_griffin_lim", T2GriffinLimArgs)):
+        getattr(L, n + "_workspace_bytes").restype = C.c_size_t
+        getattr(L, n + "_workspace_bytes").argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+        getattr(L, n).argtypes = [C.c_void_p, C.POINTER(args), C.c_void_p]
     if L.t2_abi_version() != 1:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L

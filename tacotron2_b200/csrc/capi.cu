@@ -524,7 +524,7 @@ int t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void*
 }
 void t2_waveglow_window_halo(int32_t* left, int32_t* right) { waveglow_window_halo(left, right); }
 
-// ---- WaveGlow denoiser (denoiser.cu) ----
+// ---- WaveGlow denoiser, STFT and Griffin-Lim (denoiser.cu) ----
 int t2_denoiser_create(T2Denoiser** out, const T2DenoiserConfig* cfg, const float* forward_basis,
                        const float* inverse_basis, void* stream) {
   return denoiser_create(out, cfg, forward_basis, inverse_basis, (cudaStream_t)stream);
@@ -546,6 +546,24 @@ int t2_denoiser_run_window(T2Denoiser* h, const T2DenoiserWindowArgs* a, void* s
   return denoiser_run_window(h, a, (cudaStream_t)stream);
 }
 void t2_denoiser_window_halo(int32_t* left, int32_t* right) { denoiser_window_halo(left, right); }
+size_t t2_stft_transform_workspace_bytes(const T2Denoiser*, int32_t B, int32_t n) {
+  return B > 0 && n > 0 ? stft_ws_bytes(B, n, false) : 0;
+}
+int t2_stft_transform(T2Denoiser* h, const T2StftTransformArgs* a, void* stream) {
+  return stft_transform(h, a, (cudaStream_t)stream);
+}
+size_t t2_stft_inverse_workspace_bytes(const T2Denoiser*, int32_t B, int32_t F) {
+  return B > 0 && F >= 4 ? stft_ws_bytes(B, 256 * (F - 1), false) : 0;
+}
+int t2_stft_inverse(T2Denoiser* h, const T2StftInverseArgs* a, void* stream) {
+  return stft_inverse(h, a, (cudaStream_t)stream);
+}
+size_t t2_griffin_lim_workspace_bytes(const T2Denoiser*, int32_t B, int32_t F) {
+  return B > 0 && F >= 4 ? stft_ws_bytes(B, 256 * (F - 1), true) : 0;
+}
+int t2_griffin_lim(T2Denoiser* h, const T2GriffinLimArgs* a, void* stream) {
+  return griffin_lim(h, a, (cudaStream_t)stream);
+}
 
 #ifdef T2_SELFTEST   // libt2b200_selftest.so only
 int t2_selftest_mma_rate(int32_t M, int32_t N, int32_t reps, int32_t alternate_d, int64_t* out_host) {

@@ -17,6 +17,16 @@
 // Rows of one sequence b: q = b * span + t, span = F + 4 for F = n / 256 + 1 frames.  The padded block i sits at plane
 // row 1 + b * span + i; spectrum row t holds frame t - 1 (t = 0 and t > F are zero frames); output row t is block t.
 // Only the fp32-grade tier (split fp16, 3 MMAs) exists: the reference denoises in fp32.
+//
+// The public STFT (stft.py:69-141) and Griffin-Lim (audio_processing.py:59-75) run on the same two GEMMs and planes:
+//   transform     row scale, pack, forward with EPI_MAGPHASE (fp32 magnitude and atan2 phase)
+//   inverse       spec_pack_kernel ((magnitude, phase) -> spectrum planes), inverse
+//   Griffin-Lim   spec_pack_kernel, inverse, then per iteration: pack (of the previous signal), forward with
+//                 EPI_PROJECT (the target magnitude on the current phase), inverse: 3 n_iters + 2 launches.
+// Their operands are scaled per row by a power of two taken on the device from the row's largest target magnitude (or
+// sample): the stored spectrum then peaks in [1, 2) and audio in [0.5, 1), the ranges in which the denoiser runs
+// unit-scale audio, whatever the caller's scale.  The fp32 outputs undo it exactly.
+#include <cooperative_groups.h>
 #include <math.h>
 #include <string.h>
 #include <algorithm>
@@ -99,9 +109,10 @@ __device__ __forceinline__ int frame_end(RowEnd r, int s0, int F) {
 // audio (B, n) -> padded block planes: plane row 1 + b * span + i holds the padded samples 256 i ... 256 i + 255, i.e.
 // the window samples u = 256 i + c - 512, reflected at the sequence's start (s0 = 0) and at a closed row's end.
 // Samples no output needs (outside the window, or of a row too short to pad) are zero.  Every plane row is written.
+// scale (or NULL): the samples of row b are packed times scale[b].
 __global__ void pack_kernel(const void* __restrict__ audio, int io_half, int B, int n, const int32_t* __restrict__ len,
                             int at_end, int s0, int F, int span, __half* __restrict__ planes, long rows,
-                            int32_t* __restrict__ fend) {
+                            int32_t* __restrict__ fend, const float* __restrict__ scale) {
   const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int g = blockIdx.y;
   if (blockIdx.x == 0 && g == 0)
@@ -116,6 +127,7 @@ __global__ void pack_kernel(const void* __restrict__ audio, int io_half, int B, 
   if (b >= 0 && b < B && i < F + 3) {
     const RowEnd r = row_end(len, b, n, at_end);
     const int lim = r.closed ? r.e : n;
+    const float sc = scale ? scale[b] : 1.f;
     if (!(r.closed && s0 + r.e <= kFilter / 2)) {
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
@@ -124,7 +136,7 @@ __global__ void pack_kernel(const void* __restrict__ audio, int io_half, int B, 
         else if (u >= lim) u = r.closed ? 2 * r.e - 2 - u : -1;
         if (u >= 0 && u < lim) {
           const long idx = (long)b * n + u;
-          v[k] = io_half ? __half2float(reinterpret_cast<const __half*>(audio)[idx]) : reinterpret_cast<const float*>(audio)[idx];
+          v[k] = (io_half ? __half2float(reinterpret_cast<const __half*>(audio)[idx]) : reinterpret_cast<const float*>(audio)[idx]) * sc;
         }
       }
     }
@@ -173,6 +185,138 @@ void dn_layout(Carve& c, int B, int n, DnLayout* o) {
   o->blk = c.take<__half>((size_t)kBlkGroups * 2 * o->rows * 8, 1024);
   o->spec = c.take<__half>((size_t)kSpecGroups * 2 * o->rows * 8, 1024);
   o->fend = c.take<int32_t>((size_t)B, 256);
+}
+
+// The STFT entry points' workspace: the denoiser's, the per-row scales, each row's length in samples (Griffin-Lim's
+// packs read it) and, for Griffin-Lim, the fp32 signal (B, n) between iterations.
+struct StLayout { DnLayout dn; float* scale; float* unscale; int32_t* len; float* sig; };
+void st_layout(Carve& c, int B, int n, bool signal, StLayout* o) {
+  dn_layout(c, B, n, &o->dn);
+  o->scale = c.take<float>((size_t)B, 256);
+  o->unscale = c.take<float>((size_t)B, 256);
+  o->len = c.take<int32_t>((size_t)B, 256);
+  o->sig = signal ? c.take<float>((size_t)B * n, 256) : nullptr;
+}
+
+// forward transform over the spectrum rows [lo, hi) of the layout (rows = frames; see the file comment)
+GemmParams forward_params(const T2Denoiser* m, const DnDims& d, const DnLayout& o, int B, int lo, int hi) {
+  GemmParams f;
+  memset(&f, 0, sizeof(f));
+  for (int j = 0; j < 4; ++j) f.seg[j] = Seg{o.blk, o.rows, j - 1, kHop / 64};
+  f.nseg = 4; f.nchunks = 4 * (kHop / 64); f.row0 = 1; f.wimg = m->fwd_img; f.n_tiles_m = d.ntm;
+  f.B = B; f.span = d.span; f.T = d.F + 1; f.len = o.fend; f.len_mul = 1;
+  f.lo = lo; f.hi = hi;
+  f.out = o.spec; f.out_rows = o.rows; f.out_row0 = 0;
+  return f;
+}
+
+// inverse transform + overlap-add + envelope over the output blocks [lo, hi), written to audio (B, 256 (hi - lo))
+GemmParams inverse_params(const T2Denoiser* m, const DnDims& d, const DnLayout& o, int B, int lo, int hi, float* audio) {
+  GemmParams v;
+  memset(&v, 0, sizeof(v));
+  for (int sh = 0; sh < 4; ++sh) v.seg[sh] = Seg{o.spec, o.rows, sh, kSpecCh / 64};
+  v.nseg = 4; v.nchunks = 4 * (kSpecCh / 64); v.row0 = 0; v.wimg = m->inv_img; v.n_tiles_m = d.ntm;
+  v.B = B; v.span = d.span; v.T = d.F - 1; v.len = o.fend; v.len_mul = 1;
+  v.lo = lo; v.hi = hi;
+  v.audio = audio; v.audio_pitch = (long)kHop * (hi - lo); v.wsq = m->wsq;
+  return v;
+}
+
+// ---- per-row scales: the largest |value| of a row, over the CTAs of a cluster, to a power of two -----------------
+constexpr int kRowCluster = 8, kRowThreads = 512;
+
+// max |x[r * ld + c]| over r < R, c < lim: the CTAs of the cluster take every kRowCluster-th element; every thread of
+// the cluster gets the result.  Rows of the cluster's blocks are independent of every other cluster's.
+__device__ float cluster_row_max(const float* __restrict__ x, int R, long ld, int lim) {
+  namespace cg = cooperative_groups;
+  __shared__ float red[kRowThreads / 32 + 1];
+  cg::cluster_group cl = cg::this_cluster();
+  const long total = (long)R * lim, stride = (long)kRowCluster * blockDim.x;
+  float mx = 0.f;
+  for (long i = (long)cl.block_rank() * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const long r = i / lim;
+    mx = fmaxf(mx, fabsf(x[r * ld + (i - r * lim)]));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float v = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v = fmaxf(v, red[w]);
+    red[kRowThreads / 32] = v;
+  }
+  cl.sync();
+  float v = 0.f;
+  for (int r = 0; r < kRowCluster; ++r) v = fmaxf(v, *cl.map_shared_rank(&red[kRowThreads / 32], r));
+  cl.sync();                                  // no CTA leaves while a peer may still read its shared memory
+  return v;
+}
+
+// 2^k with mx 2^k in [2^(top - 1), 2^top); 1 for a row of zeros (or inf / NaN)
+__device__ __forceinline__ float pow2_scale(float mx, int top) {
+  if (!(mx > 0.f) || isinf(mx)) return 1.f;
+  int e;
+  frexpf(mx, &e);
+  return ldexpf(1.f, min(max(top - e, -126), 127));
+}
+
+// transform: scale[b] brings row b's largest |sample| (of its first lengths[b] samples) into [0.5, 1)
+__global__ void __cluster_dims__(kRowCluster, 1, 1) __launch_bounds__(kRowThreads)
+audio_scale_kernel(const float* __restrict__ audio, int n, const int32_t* __restrict__ len, float* __restrict__ scale,
+                   float* __restrict__ unscale) {
+  const int b = blockIdx.y;
+  const float mx = cluster_row_max(audio + (long)b * n, 1, n, row_end(len, b, n, 1).e);
+  if (cooperative_groups::this_cluster().block_rank() == 0 && threadIdx.x == 0) {
+    const float s = pow2_scale(mx, 0);
+    scale[b] = s;
+    unscale[b] = 1.f / s;
+  }
+}
+
+// inverse / Griffin-Lim input: (magnitude, phase) (B, 513, F) fp32 -> the spectrum planes the inverse GEMM reads,
+// (m cos phase, m sin phase) scale[b] / 512 at plane row b * span + 1 + f, zeros in the other rows of the sequence.
+// Row b has Fb = frames[b] frames (F for NULL or a value outside [0, F]); a row of fewer than 4 frames (at most 512
+// samples) cannot be reflect-padded by its transforms and gives zeros.  scale[b] brings the row's largest magnitude to
+// [512, 1024), the range of the spectrum of unit-scale audio.  Also writes unscale = 1 / scale, the row's length in
+// samples, 256 (Fb - 1), and fend as pack_kernel computes it from that length.  One cluster per row.
+__global__ void __cluster_dims__(kRowCluster, 1, 1) __launch_bounds__(kRowThreads)
+spec_pack_kernel(const float* __restrict__ mag, const float* __restrict__ phase, const int32_t* __restrict__ frames,
+                 int F, int span, __half* __restrict__ planes, long rows, float* __restrict__ scale,
+                 float* __restrict__ unscale, int32_t* __restrict__ len, int32_t* __restrict__ fend) {
+  const int b = blockIdx.y, rank = (int)cooperative_groups::this_cluster().block_rank();
+  const int l = frames ? frames[b] : -1;
+  const int Fb = l >= 0 && l <= F ? l : F;
+  const int fe = Fb >= 4 ? Fb + 1 : 0;
+  const float* mb = mag + (long)b * kBins * F;
+  const float* pb = phase + (long)b * kBins * F;
+  const float s = pow2_scale(cluster_row_max(mb, kBins, F, fe ? Fb : 0), 10), sc = s * kSpecScale;
+  if (rank == 0 && threadIdx.x == 0) {
+    scale[b] = s;
+    unscale[b] = 1.f / s;
+    len[b] = fe ? kHop * (Fb - 1) : 0;
+    fend[b] = fe;
+  }
+  // item (j, t): j < 65 is bins 8 j ... 8 j + 7 of row t (real parts to group j, imaginary to group 65 + j); j in
+  // [65, 71) zeroes group 65 + j, the padding groups 130 ... 135
+  const int items = (kSpecGroups - kImGroup0) * span;
+  for (int it = rank * blockDim.x + threadIdx.x; it < items; it += kRowCluster * blockDim.x) {
+    const int j = it / span, t = it - j * span;
+    const long q = (long)b * span + t;
+    float re[8], im[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int bin = 8 * j + i;
+      re[i] = im[i] = 0.f;
+      if (j < kImGroup0 && bin < kBins && t >= 1 && t < fe) {
+        const float m = mb[(long)bin * F + t - 1], ph = pb[(long)bin * F + t - 1];
+        re[i] = __fmul_rn(m, cosf(ph)) * sc;
+        im[i] = __fmul_rn(m, sinf(ph)) * sc;
+      }
+    }
+    if (j < kImGroup0) store8<kPassesFp32>(planes, rows, j, q, re);
+    store8<kPassesFp32>(planes, rows, kImGroup0 + j, q, im);
+  }
 }
 
 }  // namespace
@@ -285,27 +429,114 @@ int denoiser_run_window(T2Denoiser* m, const T2DenoiserWindowArgs* wa, cudaStrea
   DnLayout o;
   dn_layout(c, B, n, &o);
   pack_kernel<<<dim3((unsigned)((o.rows + 127) / 128), kBlkGroups), 128, 0, s>>>(
-      a->audio, a->io_half, B, n, a->lengths, wa->at_end, s0, d.F, d.span, o.blk, o.rows, o.fend);
+      a->audio, a->io_half, B, n, a->lengths, wa->at_end, s0, d.F, d.span, o.blk, o.rows, o.fend, nullptr);
   T2_LAUNCH_CHECK();
   // forward transform + spectral gate over the spectrum rows the output blocks read: [out0, out1 + 3)
-  GemmParams f;
-  memset(&f, 0, sizeof(f));
-  for (int j = 0; j < 4; ++j) f.seg[j] = Seg{o.blk, o.rows, j - 1, kHop / 64};
-  f.nseg = 4; f.nchunks = 4 * (kHop / 64); f.row0 = 1; f.wimg = m->fwd_img; f.n_tiles_m = d.ntm;
-  f.B = B; f.span = d.span; f.T = d.F + 1; f.len = o.fend; f.len_mul = 1;
-  f.lo = out0; f.hi = std::min(d.span, out1 + kHalo);
+  GemmParams f = forward_params(m, d, o, B, out0, std::min(d.span, out1 + kHalo));
   f.bias = a->bias; f.strength = a->strength;
-  f.out = o.spec; f.out_rows = o.rows; f.out_row0 = 0;
   T2_TRY((launch_gemm<EPI_SPECTRAL, kPassesFp32>(f, kFwdTiles, s)));
   // inverse transform + overlap-add + envelope over the output blocks [out0, out1)
-  GemmParams v;
-  memset(&v, 0, sizeof(v));
-  for (int sh = 0; sh < 4; ++sh) v.seg[sh] = Seg{o.spec, o.rows, sh, kSpecCh / 64};
-  v.nseg = 4; v.nchunks = 4 * (kSpecCh / 64); v.row0 = 0; v.wimg = m->inv_img; v.n_tiles_m = d.ntm;
-  v.B = B; v.span = d.span; v.T = d.F - 1; v.len = o.fend; v.len_mul = 1;
-  v.lo = out0; v.hi = out1;
-  v.audio = a->out; v.audio_pitch = (long)kHop * (out1 - out0); v.wsq = m->wsq;
-  T2_TRY((launch_gemm<EPI_OVERLAP, kPassesFp32>(v, 1, s)));
+  T2_TRY((launch_gemm<EPI_OVERLAP, kPassesFp32>(inverse_params(m, d, o, B, out0, out1, a->out), 1, s)));
+  return T2_OK;
+}
+
+// ---- public STFT transform / inverse and Griffin-Lim ----------------------------------------------------------------
+// Checks shared by the entry points that take a (B, 513, F) spectrum; F >= 4 frames make 256 (F - 1) > 512 samples,
+// which the reference's reflect padding needs.
+static int check_spectrum(const char* what, T2Denoiser* m, const T2StftInverseArgs* a, bool signal) {
+  if (!m || !a || !a->magnitude || !a->phase || !a->out || !a->ws) return fail(T2_ERR_INVALID, "%s: null argument", what);
+  if (a->B <= 0) return fail(T2_ERR_INVALID, "%s: empty batch (B=%d)", what, a->B);
+  if (a->F < 4)
+    return fail(T2_ERR_INVALID, "%s: %d frames give %d samples, which cannot be reflect-padded by 512 (at least 4 "
+                "frames are needed)", what, a->F, kHop * (a->F - 1));
+  if ((long)a->B * (a->F + 4) > (1L << 30) || (long)kHop * (a->F - 1) > (1L << 31) - 1)
+    return fail(T2_ERR_INVALID, "%s: input too large", what);
+  if (reinterpret_cast<uintptr_t>(a->out) % 16)
+    return fail(T2_ERR_INVALID, "%s: out must be 16-byte aligned (the epilogue writes it with 16-byte stores)", what);
+  if (a->ws_bytes < stft_ws_bytes(a->B, kHop * (a->F - 1), signal)) return fail(T2_ERR_WORKSPACE, "%s workspace too small", what);
+  return T2_OK;
+}
+
+size_t stft_ws_bytes(int B, int n, bool signal) {
+  Carve c(nullptr, 1024);
+  StLayout o;
+  st_layout(c, B, n, signal, &o);
+  return c.bytes();
+}
+
+int stft_transform(T2Denoiser* m, const T2StftTransformArgs* a, cudaStream_t s) {
+  if (!m || !a || !a->audio || !a->magnitude || !a->phase || !a->ws) return fail(T2_ERR_INVALID, "stft transform: null argument");
+  const int B = a->B, n = a->n;
+  if (B <= 0 || n <= 0) return fail(T2_ERR_INVALID, "stft transform: empty input (B=%d, n=%d)", B, n);
+  if ((long)B * (n / kHop + 5) > (1L << 30)) return fail(T2_ERR_INVALID, "stft transform: input too large");
+  if (!a->lengths && n <= kFilter / 2)
+    return fail(T2_ERR_INVALID, "stft transform: %d samples cannot be reflect-padded by 512", n);
+  if (a->ws_bytes < stft_ws_bytes(B, n, false)) return fail(T2_ERR_WORKSPACE, "stft transform workspace too small");
+  const DnDims d = dn_dims(B, n);
+  Carve c(a->ws, 1024);
+  StLayout o;
+  st_layout(c, B, n, false, &o);
+  audio_scale_kernel<<<dim3(kRowCluster, B), kRowThreads, 0, s>>>(a->audio, n, a->lengths, o.scale, o.unscale);
+  T2_LAUNCH_CHECK();
+  pack_kernel<<<dim3((unsigned)((o.dn.rows + 127) / 128), kBlkGroups), 128, 0, s>>>(
+      a->audio, 0, B, n, a->lengths, 1, 0, d.F, d.span, o.dn.blk, o.dn.rows, o.dn.fend, o.scale);
+  T2_LAUNCH_CHECK();
+  GemmParams f = forward_params(m, d, o.dn, B, 0, d.F + 1);
+  f.row_scale = o.unscale; f.mag_out = a->magnitude; f.phase_out = a->phase;
+  T2_TRY((launch_gemm<EPI_MAGPHASE, kPassesFp32>(f, kFwdTiles, s)));
+  return T2_OK;
+}
+
+// spectrum planes from (magnitude, phase), then the inverse into out (times unscale: the caller's units) or, with
+// unscale NULL, into the scaled signal Griffin-Lim iterates on
+static int spec_pack(const T2StftInverseArgs* a, const DnDims& d, const StLayout& o, cudaStream_t s) {
+  spec_pack_kernel<<<dim3(kRowCluster, a->B), kRowThreads, 0, s>>>(a->magnitude, a->phase, a->lengths, d.F, d.span,
+                                                                  o.dn.spec, o.dn.rows, o.scale, o.unscale, o.len,
+                                                                  o.dn.fend);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
+}
+static int inverse_to(T2Denoiser* m, int B, const DnDims& d, const StLayout& o, float* out, const float* unscale,
+                      cudaStream_t s) {
+  GemmParams v = inverse_params(m, d, o.dn, B, 0, d.F - 1, out);
+  v.row_scale = unscale;
+  return launch_gemm<EPI_OVERLAP, kPassesFp32>(v, 1, s);
+}
+
+int stft_inverse(T2Denoiser* m, const T2StftInverseArgs* a, cudaStream_t s) {
+  T2_TRY(check_spectrum("stft inverse", m, a, false));
+  const int B = a->B, n = kHop * (a->F - 1);
+  const DnDims d = dn_dims(B, n);
+  Carve c(a->ws, 1024);
+  StLayout o;
+  st_layout(c, B, n, false, &o);
+  T2_TRY(spec_pack(a, d, o, s));
+  return inverse_to(m, B, d, o, a->out, o.unscale, s);
+}
+
+int griffin_lim(T2Denoiser* m, const T2GriffinLimArgs* g, cudaStream_t s) {
+  if (!g) return fail(T2_ERR_INVALID, "griffin_lim: null argument");
+  const T2StftInverseArgs* a = &g->inv;
+  T2_TRY(check_spectrum("griffin_lim", m, a, true));
+  if (g->n_iters < 0) return fail(T2_ERR_INVALID, "griffin_lim: n_iters = %d is negative", g->n_iters);
+  const int B = a->B, n = kHop * (a->F - 1);
+  const DnDims d = dn_dims(B, n);
+  Carve c(a->ws, 1024);
+  StLayout o;
+  st_layout(c, B, n, true, &o);
+  // signal = inverse(S, angles); then n_iters times: signal = inverse(S, phase of transform(signal))
+  T2_TRY(spec_pack(a, d, o, s));
+  T2_TRY(inverse_to(m, B, d, o, g->n_iters == 0 ? a->out : o.sig, g->n_iters == 0 ? o.unscale : nullptr, s));
+  for (int i = 1; i <= g->n_iters; ++i) {
+    pack_kernel<<<dim3((unsigned)((o.dn.rows + 127) / 128), kBlkGroups), 128, 0, s>>>(
+        o.sig, 0, B, n, o.len, 1, 0, d.F, d.span, o.dn.blk, o.dn.rows, o.dn.fend, nullptr);
+    T2_LAUNCH_CHECK();
+    GemmParams f = forward_params(m, d, o.dn, B, 0, std::min(d.span, d.F - 1 + kHalo));
+    f.target = a->magnitude; f.row_scale = o.scale;
+    T2_TRY((launch_gemm<EPI_PROJECT, kPassesFp32>(f, kFwdTiles, s)));
+    const bool last = i == g->n_iters;
+    T2_TRY(inverse_to(m, B, d, o, last ? a->out : o.sig, last ? o.unscale : nullptr, s));
+  }
   return T2_OK;
 }
 

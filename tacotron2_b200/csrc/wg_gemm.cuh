@@ -27,7 +27,7 @@ constexpr int kThreads = 384;               // warp 0 producer; warpgroups 1 / 2
 constexpr int kCluster = 2;                 // the CTAs of a cluster share each weight stage by multicast
 constexpr int kC = 256;                     // WaveGlow: WN channels (the skip rows of EPI_RESSKIP)
 constexpr unsigned long long kWd = 1ull << 32;
-// Denoiser spectrum planes (EPI_SPECTRAL writes them, EPI_OVERLAP's GEMM reads them): the real parts of the 513 bins
+// Denoiser spectrum planes (EPI_SPECTRAL / EPI_PROJECT write them, EPI_OVERLAP's GEMM reads them): the real parts of the 513 bins
 // in groups 0 ... 64, the imaginary parts in groups 65 ... 129, zero up to 136 groups = 17 whole 64-channel chunks.
 constexpr int kBins = 513, kImGroup0 = 65, kSpecGroups = 136;
 // Operand ranges (a split fp16 value overflows at 65504).  The audio is packed as it is, so its samples must stay below
@@ -44,7 +44,8 @@ __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) {
     if (clock64() - t0 > kWd) __trap();
 }
 
-enum { EPI_UPSAMPLE = 0, EPI_GATE = 1, EPI_RESSKIP = 2, EPI_SPECTRAL = 3, EPI_OVERLAP = 4, EPI_CONV = 5 };
+enum { EPI_UPSAMPLE = 0, EPI_GATE = 1, EPI_RESSKIP = 2, EPI_SPECTRAL = 3, EPI_OVERLAP = 4, EPI_CONV = 5, EPI_PROJECT = 6,
+       EPI_MAGPHASE = 7 };
 
 // A tile rows beyond the output tile: EPI_CONV's tile m0 reads padded rows [m0 - 2, m0 + 130), every other epilogue
 // 128 rows per segment.
@@ -67,6 +68,10 @@ struct GemmParams {
   float strength;                                    // SPECTRAL: the magnitude loses bias * strength
   float* audio; long audio_pitch;                    // OVERLAP: fp32 rows (B, audio_pitch); row t writes block t - lo
   const double* wsq;                                 // OVERLAP: the squared window (1024)
+  const float* row_scale;                            // PROJECT: the target times row_scale[b]; MAGPHASE and (when set)
+                                                     // OVERLAP: the output times row_scale[b].  Powers of two.
+  const float* target;                               // PROJECT: magnitudes (B, 513, T - 1) fp32
+  float* mag_out; float* phase_out;                  // MAGPHASE: (B, 513, T - 1) fp32
   // CONV: tile row q is padded row b * span + 2 + t (span = T + 4); y = act(acc * scale + bias), act 0 none, 1 relu,
   // 2 tanh; out_mode 0 writes the planes `out`, 1 fp32 rows (row of (b, t) = b * out_seq_rows + t, pitch ldo),
   // 2 fp32 (B, cout, T) plus the residual (B, T, cout); len: frames t >= len[b] are zeros in modes 0 and 2.
@@ -292,11 +297,14 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
             store8<PASSES>(p.out, p.out_rows, nt, crow + k, v);
           }
         }
-      } else if (EPI == EPI_SPECTRAL) {
-        // Denoiser forward transform.  Columns [0, 128) of the tile are the real parts of the bins nt * 128 + c,
-        // [128, 256) their imaginary parts.  Row t is frame t - 1 (t = 0: the zero frame before the sequence).
-        // mag' = max(|X| - strength * bias, 0); X' = X mag' / |X|, and (mag', 0) where |X| = 0 (atan2(0, 0) = 0).
+      } else if (EPI == EPI_SPECTRAL || EPI == EPI_PROJECT) {
+        // Denoiser forward transform, and Griffin-Lim's projection.  Columns [0, 128) of the tile are the real parts of
+        // the bins nt * 128 + c, [128, 256) their imaginary parts.  Row t is frame t - 1 (t = 0: the zero frame before
+        // the sequence).  SPECTRAL: mag' = max(|X| - strength * bias, 0); PROJECT: mag' = target[b, bin, t - 1] *
+        // row_scale[b].  X' = X mag' / |X|, and (mag', 0) where |X| = 0 (atan2(0, 0) = 0).
         const bool live = valid && t >= 1;
+        const float* tgt = EPI == EPI_PROJECT && live ? p.target + (long)b * kBins * (p.T - 1) + (t - 1) : nullptr;
+        const float rs = EPI == EPI_PROJECT && live ? p.row_scale[b] : 0.f;
         for (int g = 0; g < 8; ++g) {
           const int j = nt * 16 + half * 8 + g;        // bins 8 j ... 8 j + 7
           float re[8], im[8];
@@ -304,9 +312,14 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
           for (int i = 0; i < 8; ++i) {
             const float x = row[half * 64 + g * 8 + i], y = row[128 + half * 64 + g * 8 + i];
             const int bin = 8 * j + i;
-            const float bias = bin < kBins ? p.bias[bin] : 0.f;
             const float mag = sqrtf(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
-            const float m = fmaxf(__fsub_rn(mag, __fmul_rn(bias, p.strength)), 0.f);
+            float m;
+            if (EPI == EPI_PROJECT) {
+              m = live && bin < kBins ? tgt[(long)bin * (p.T - 1)] * rs : 0.f;
+            } else {
+              const float bias = bin < kBins ? p.bias[bin] : 0.f;
+              m = fmaxf(__fsub_rn(mag, __fmul_rn(bias, p.strength)), 0.f);
+            }
             const float s = mag > 0.f ? m / mag : 0.f;
             re[i] = live ? (mag > 0.f ? x * s : m) * kSpecScale : 0.f;
             im[i] = live ? y * s * kSpecScale : 0.f;
@@ -314,8 +327,24 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
           if (j < kImGroup0) store8<PASSES>(p.out, p.out_rows, j, p.out_row0 + q, re);
           if (kImGroup0 + j < kSpecGroups) store8<PASSES>(p.out, p.out_rows, kImGroup0 + j, p.out_row0 + q, im);
         }
+      } else if (EPI == EPI_MAGPHASE) {
+        // Public STFT transform: columns as above; row t in [1, T) is frame t - 1 of the (B, 513, T - 1) outputs.  The
+        // magnitude leaves the packing scale (row_scale[b] undoes it exactly); the phase does not depend on it.
+        if (data && t >= 1) {
+          const long F = p.T - 1;
+          const float us = valid ? p.row_scale[b] : 0.f;
+          float* mo = p.mag_out + (long)b * kBins * F + (t - 1);
+          float* po = p.phase_out + (long)b * kBins * F + (t - 1);
+          for (int c = 0; c < 64; ++c) {
+            const int bin = nt * 128 + half * 64 + c;
+            if (bin >= kBins) break;
+            const float x = row[half * 64 + c], y = row[128 + half * 64 + c];
+            mo[(long)bin * F] = valid ? sqrtf(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))) * us : 0.f;
+            po[(long)bin * F] = valid ? atan2f(y, x) : 0.f;
+          }
+        }
       } else if (EPI == EPI_OVERLAP) {
-        // Denoiser inverse transform.  Row t is block t of the trimmed output: the MMA has already added the four
+        // Denoiser / STFT inverse transform.  Row t is block t of the trimmed output: the MMA has already added the four
         // frames t - 1 ... t + 2 that overlap it.  p.len[b] = 1 + the number of frames of row b (frame f exists when
         // f >= 0 and f + 1 < len); its output ends at block len - 2.
         if (b < p.B && t >= p.lo && t < p.hi) {
@@ -333,6 +362,7 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
               for (int f = t - 1; f <= t + 2; ++f)
                 if (f >= 0 && f + 1 < fend) env = (float)((double)env + p.wsq[256 * (t + 2 - f) + col]);
               float y = row[col] * (1.f / (kSpecScale * kInvBasisScale));
+              if (p.row_scale) y *= p.row_scale[b];
               if (env > FLT_MIN) y = y / env;
               v[i] = in_row ? y * 4.f : 0.f;
             }

@@ -1,12 +1,14 @@
 """LinearNorm / ConvNorm with the reference's parameter names and initialisation (layers.py:8-39).
 They only *hold* parameters (``linear_layer.weight``, ``conv.weight`` ... are the state_dict keys the
 published checkpoints use); the arithmetic of the hot path is done by libt2b200.so.
-TacotronSTFT (layers.py:42-80): the log-mel extraction of the data path, on the GPU through ``t2_mel_spectrogram``."""
+TacotronSTFT (layers.py:42-80): the log-mel extraction of the data path, on the GPU through ``t2_mel_spectrogram``, and
+its ``stft_fn``, the STFT that ``audio_processing.griffin_lim`` takes."""
 import ctypes as C
 
 import torch
 
 from . import _capi
+from .stft import STFT, _windowed_fourier_basis  # noqa: F401  (layers.py re-exports STFT, as the reference's does)
 
 
 class LinearNorm(torch.nn.Module):
@@ -38,21 +40,6 @@ class ConvNorm(torch.nn.Module):
 
 
 # ---- TacotronSTFT: log-mel extraction on the GPU (layers.py:42-80, stft.py:44-94) -----------------------------------
-def _windowed_fourier_basis(filter_length, win_length):
-    """Rows 0 .. n/2 = real part, rows n/2+1 .. n+1 = imaginary part of the first n/2 + 1 DFT bins (exp(-2 pi i k t / n)),
-    each multiplied by the periodic hann window zero-padded symmetrically to filter_length (stft.py:44-63)."""
-    import numpy as np
-    n, cutoff = int(filter_length), int(filter_length) // 2 + 1
-    if win_length > n:
-        raise ValueError("win_length must not exceed filter_length (stft.py:56)")
-    phase = (2.0 * np.pi / n) * np.outer(np.arange(cutoff), np.arange(n))
-    window = np.zeros(n)
-    left = (n - win_length) // 2
-    window[left:left + win_length] = 0.5 - 0.5 * np.cos(2.0 * np.pi * np.arange(win_length) / win_length)
-    basis = np.vstack((np.cos(phase), -np.sin(phase))).astype(np.float32)
-    return torch.from_numpy(basis * window.astype(np.float32))
-
-
 def _slaney_mel_filterbank(sampling_rate, n_fft, n_mels, fmin, fmax):
     """The filterbank the reference takes from librosa 0.6.0 (``librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax)``,
     layers.py:50-51; librosa is a dependency outside the reference tree): triangular filters on the Slaney mel scale
@@ -80,13 +67,15 @@ def _slaney_mel_filterbank(sampling_rate, n_fft, n_mels, fmin, fmax):
 class TacotronSTFT(torch.nn.Module):
     """layers.py:42-80 with the same constructor, the ``mel_basis`` buffer and ``mel_spectrogram(y)``; the transform
     itself (reflect padding, windowed DFT as a tensor-core GEMM over overlapping frames, magnitude, mel projection, log
-    compression) is ``t2_mel_spectrogram`` of libt2b200.  CUDA tensors only."""
+    compression) is ``t2_mel_spectrogram`` of libt2b200.  ``stft_fn`` is the reference's STFT submodule (its
+    ``transform`` / ``inverse`` and Griffin-Lim run on the denoiser's GEMMs).  CUDA tensors only."""
 
     def __init__(self, filter_length=1024, hop_length=256, win_length=1024, n_mel_channels=80, sampling_rate=22050,
                  mel_fmin=0.0, mel_fmax=8000.0):
         super(TacotronSTFT, self).__init__()
         self.n_mel_channels, self.sampling_rate = n_mel_channels, sampling_rate
         self.filter_length, self.hop_length, self.win_length = filter_length, hop_length, win_length
+        self.stft_fn = STFT(filter_length, hop_length, win_length)
         self.register_buffer("mel_basis", _slaney_mel_filterbank(sampling_rate, filter_length, n_mel_channels, mel_fmin, mel_fmax))
         self.register_buffer("forward_basis", _windowed_fourier_basis(filter_length, win_length))
         self._ws = _capi.Workspace()

@@ -683,12 +683,66 @@ def denoiser_case(seed=3, n=256 * 40 + 100, strengths=(0.01, 0.1, 3.0), n_sample
          inverse_samples=ib.reshape(-1)[idx], forward_stats=stats(fb), inverse_stats=stats(ib), **outs)
 
 
+def griffin_lim_case(seed=5, n=256 * 24 + 100, np_seed=1234, iters=(0, 1, 30)):
+    """The reference's own audio_processing.griffin_lim over its stft.STFT(1024, 256, 1024) on the CPU: the target is
+    the magnitude of the seeded 2-row signal stft_inputs(seed, n); before each call np.random.seed(np_seed), so every
+    run starts from the same angles.  Shims: the librosa stand-ins of denoiser_case."""
+    import importlib.util
+    import types
+
+    def pad_center(data, size, axis=-1, **kw):
+        n_ = data.shape[axis]
+        lpad = int((size - n_) // 2)
+        lengths = [(0, 0)] * data.ndim
+        lengths[axis] = (lpad, int(size - n_ - lpad))
+        return np.pad(data, lengths, mode="constant")
+
+    def normalize(S, norm=np.inf, **kw):       # audio_processing.py:48 calls it with norm=None: no normalisation
+        assert norm is None
+        return S
+    names = ("librosa", "librosa.util", "librosa.filters", "audio_processing", "stft")
+    saved = {k: sys.modules.get(k) for k in names}
+    lib, lu, lf = types.ModuleType("librosa"), types.ModuleType("librosa.util"), types.ModuleType("librosa.filters")
+    lu.pad_center, lu.tiny, lu.normalize, lf.mel = pad_center, (lambda x: np.finfo(np.float32).tiny), normalize, None
+    lib.util, lib.filters = lu, lf
+    sys.modules.update({"librosa": lib, "librosa.util": lu, "librosa.filters": lf})
+    for k in ("audio_processing", "stft"):
+        sys.modules.pop(k, None)
+    sys.path.insert(0, REFERENCE_DIR)
+    try:
+        spec = importlib.util.spec_from_file_location("audio_processing", os.path.join(REFERENCE_DIR, "audio_processing.py"))
+        ap = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(ap)
+        sys.modules["audio_processing"] = ap
+        spec = importlib.util.spec_from_file_location("t2_reference_stft", os.path.join(REFERENCE_DIR, "stft.py"))
+        st = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(st)
+        stft_fn = st.STFT(1024, 256, 1024)
+        y = stft_inputs(seed, n)
+        with torch.no_grad():
+            mag, _ = stft_fn.transform(y)
+            outs = {}
+            for k in iters:
+                np.random.seed(np_seed)
+                outs["out_%d" % k] = ap.griffin_lim(mag, stft_fn, n_iters=k)
+    finally:
+        sys.path.remove(REFERENCE_DIR)
+        for k, v in saved.items():
+            sys.modules.pop(k, None)
+            if v is not None:
+                sys.modules[k] = v
+    save("griffin_lim_b2", seed=seed, n=n, np_seed=np_seed, iters=np.array(iters), mag=mag, **outs)
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "ragged":
         ragged_case()
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "denoiser":
         denoiser_case()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "griffin_lim":
+        griffin_lim_case()
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "waveglow":
         waveglow_cases()
