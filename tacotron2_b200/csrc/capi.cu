@@ -100,11 +100,16 @@ int pack_model(T2Model* m, cudaStream_t s) {
     T2_CUDA(cudaMemsetAsync(m->zeros, 0, 8192 * 4, s));
   }
   // tensor-core conv / GEMM weight images
-  for (int i = 0; i < 3; ++i) T2_TRY(tc_pack_weights(m->w[W_ENC_CONV0 + 7 * i], kEnc, kEnc, kConvK, 128, &m->tc_enc_conv[i], s));
-  T2_TRY(tc_pack_weights(m->enc_lstm_wih, 8 * kEncH, kEnc, 1, 128, &m->tc_enc_wih, s));
+  for (int i = 0; i < 3; ++i) {
+    T2_TRY(dmalloc(&m->tc_enc_conv[i], tc_weights_bytes(kEnc, kEnc, kConvK, 128)));
+    T2_TRY(tc_pack_weights(m->w[W_ENC_CONV0 + 7 * i], kEnc, kEnc, kConvK, 128, m->tc_enc_conv[i], s));
+  }
+  T2_TRY(dmalloc(&m->tc_enc_wih, tc_weights_bytes(8 * kEncH, kEnc, 1, 128)));
+  T2_TRY(tc_pack_weights(m->enc_lstm_wih, 8 * kEncH, kEnc, 1, 128, m->tc_enc_wih, s));
   for (int i = 0; i < 5; ++i) {
-    const int ci = i == 0 ? kMel : kPost, co = i == 4 ? kMel : kPost;
-    T2_TRY(tc_pack_weights(m->w[W_POST_CONV0 + 7 * i], co, ci, kConvK, i == 4 ? 80 : 128, &m->tc_post_conv[i], s));
+    const int ci = i == 0 ? kMel : kPost, co = i == 4 ? kMel : kPost, nt = i == 4 ? 80 : 128;
+    T2_TRY(dmalloc(&m->tc_post_conv[i], tc_weights_bytes(co, ci, kConvK, nt)));
+    T2_TRY(tc_pack_weights(m->w[W_POST_CONV0 + 7 * i], co, ci, kConvK, nt, m->tc_post_conv[i], s));
   }
   T2_TRY(persistent_pack_create(m, s));
   return T2_OK;
@@ -224,14 +229,11 @@ int t2_model_destroy(T2Model* m) {
   for (int i = 0; i < 3; ++i) cudaFree(m->enc_conv_w[i]);
   for (int i = 0; i < 5; ++i) cudaFree(m->post_conv_w[i]);
   cudaFree(m->enc_lstm_wih); cudaFree(m->enc_lstm_b); cudaFree(m->arnn_b); cudaFree(m->drnn_b);
-  cudaFree(m->projgate_w); cudaFree(m->projgate_b); cudaFree(m->zeros); cudaFree(m->dgrad_tmp);
-  for (int i = 0; i < 3; ++i) cudaFree(m->tc_dgrad_enc[i]);
-  for (int i = 0; i < 5; ++i) cudaFree(m->tc_dgrad_post[i]);
+  cudaFree(m->projgate_w); cudaFree(m->projgate_b); cudaFree(m->zeros);
   for (int i = 0; i < 3; ++i) cudaFree(m->tc_enc_conv[i]);
   for (int i = 0; i < 5; ++i) cudaFree(m->tc_post_conv[i]);
   cudaFree(m->tc_enc_wih);
   persistent_pack_destroy(m);
-  gemm_tc_destroy(m);
   delete m;
   return T2_OK;
 }
@@ -583,19 +585,31 @@ int t2_selftest_event(const float* A, const float* W, const int32_t* consumers, 
   return selftest_event(A, W, consumers, n_consumers, K, C, (cudaStream_t)stream);
 }
 
-// C = op(A) . op(B) + beta C through the training path's tensor-core GEMM (gemm_tc.cu); batch > 1: strided batch
+// C = op(A) . op(B) + beta C through the training path's tensor-core GEMM (gemm_tc.cu); batch > 1: strided batch.
+// The scratch is allocated and freed in stream order around the call.
 int t2_selftest_gemm_tc(int32_t ta, int32_t tb, int32_t M, int32_t N, int32_t K, const float* A, int64_t lda, const float* B,
                         int64_t ldb, float* C, int64_t ldc, float beta, int32_t batch, int64_t strideA, int64_t strideB,
                         int64_t strideC, void* stream) {
-  static T2Model scratch_owner;            // only its GEMM scratch is used
+  cudaStream_t s = (cudaStream_t)stream;
   GemmTc g;
   g.ta = ta != 0; g.tb = tb != 0; g.M = M; g.N = N; g.K = K; g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc;
   g.beta = beta; g.batch = batch; g.strideA = strideA; g.strideB = strideB; g.strideC = strideC;
-  return gemm_tc(&scratch_owner, (cudaStream_t)stream, g);
+  if (M <= 0 || N <= 0 || K <= 0) return gemm_tc(kGemmTcSms, s, g);      // refused before it needs scratch
+  g.ws_bytes = gemm_tc_ws_bytes(M, N, K, batch);
+  T2_CUDA(cudaMallocAsync(&g.ws, g.ws_bytes, s));
+  const int r = gemm_tc(kGemmTcSms, s, g);
+  T2_CUDA(cudaFreeAsync(g.ws, s));
+  return r;
 }
 int t2_selftest_colsum(const float* X, int64_t ld, int64_t rows, int32_t cols, float* out, void* stream) {
-  static T2Model scratch_owner;
-  return colsum_f32(&scratch_owner, (cudaStream_t)stream, X, ld, rows, cols, out);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (rows <= 0 || cols <= 0) return colsum_f32(s, nullptr, 0, X, ld, rows, cols, out);
+  const size_t bytes = colsum_ws_bytes(rows, cols);
+  void* ws = nullptr;
+  T2_CUDA(cudaMallocAsync(&ws, bytes, s));
+  const int r = colsum_f32(s, ws, bytes, X, ld, rows, cols, out);
+  T2_CUDA(cudaFreeAsync(ws, s));
+  return r;
 }
 int t2_selftest_waveglow_state(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, int32_t n_launches, float* spect, float* hbuf,
                                float* acts, float* skip, float* aud, void* stream) {

@@ -105,11 +105,13 @@ long tc_plane_rows(int B, int T) {
 }
 size_t tc_planes_bytes(int B, int T, int c_pad) { return (size_t)(c_pad / 8) * 2 * tc_plane_rows(B, T) * 16; }
 
-int tc_pack_weights(const float* w, int cout, int cin, int taps, int nt_rows, uint8_t** img, cudaStream_t s) {
+size_t tc_weights_bytes(int cout, int cin, int taps, int nt_rows) {
+  return (size_t)((cout + nt_rows - 1) / nt_rows) * ((cin + 63) / 64) * taps * nt_rows * 256;
+}
+
+int tc_pack_weights(const float* w, int cout, int cin, int taps, int nt_rows, uint8_t* img, cudaStream_t s) {
   const int nchunks = (cin + 63) / 64, n_tiles_n = (cout + nt_rows - 1) / nt_rows;
-  const size_t bytes = (size_t)n_tiles_n * nchunks * taps * nt_rows * 256;
-  if (!*img) T2_CUDA(cudaMalloc((void**)img, bytes));
-  pack_conv_w_kernel<<<n_tiles_n * nchunks * taps, 256, 0, s>>>(w, cout, cin, taps, nt_rows, nchunks, *img);
+  pack_conv_w_kernel<<<n_tiles_n * nchunks * taps, 256, 0, s>>>(w, cout, cin, taps, nt_rows, nchunks, img);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }

@@ -23,7 +23,9 @@ struct TcConvArgs {
 
 long tc_plane_rows(int B, int T);
 size_t tc_planes_bytes(int B, int T, int c_pad);
-int tc_pack_weights(const float* w, int cout, int cin, int taps, int nt_rows, uint8_t** img, cudaStream_t s);
+// W (cout, cin, taps) -> img, a buffer of tc_weights_bytes(cout, cin, taps, nt_rows)
+size_t tc_weights_bytes(int cout, int cin, int taps, int nt_rows);
+int tc_pack_weights(const float* w, int cout, int cin, int taps, int nt_rows, uint8_t* img, cudaStream_t s);
 int tc_rows_to_planes(const float* x, long batch_stride, int C, int c_pad, const int32_t* len, int B, int T,
                       __half* planes, cudaStream_t s);
 int tc_rows_to_planes_scaled(const float* x, long batch_stride, int C, int c_pad, const int32_t* len, int B, int T,

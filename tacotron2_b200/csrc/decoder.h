@@ -76,8 +76,9 @@ int persistent_stream_collect(const T2DecoderArgs* a, const T2CollectRow* rows, 
 // 1 attention LSTM (1792 columns); K = 4096 gate rows in kBwdGemmSplit partial sums
 constexpr int kBwdGemmSplit = 4;
 constexpr int kBwdImgBytes = 64 * 16384;     // activation image of one (64 x 4096) operand
-int bwd_gemm_prepare(T2Model* m, cudaStream_t s);
-int bwd_gemm_run(T2Model* m, int which, const uint8_t* x_img, const float* inv_scale, float* P, int ldp, DecoderCtrl* ctrl,
-                 cudaStream_t s);
+size_t bwd_wimg_bytes(int which);     // the W^T image of [W_ih | W_hh] of one LSTM
+int bwd_gemm_prepare(T2Model* m, uint8_t* const* wimg, cudaStream_t s);
+int bwd_gemm_run(T2Model* m, int which, const uint8_t* w_img, const uint8_t* x_img, const float* inv_scale, float* P, int ldp,
+                 DecoderCtrl* ctrl, cudaStream_t s);
 
 }  // namespace t2

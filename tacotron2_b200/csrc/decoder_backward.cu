@@ -14,6 +14,8 @@
 // T x B rows; d_memory = d_pm W_m + sum_t aw_t (x) g_ctx_t.
 #include <string.h>
 
+#include <algorithm>
+
 #include "decoder.h"
 #include "gemm_f32.cuh"
 #include "umma.cuh"
@@ -419,6 +421,8 @@ struct BwdWs {
   float *dga, *dgd, *q, *dq, *awc, *pm, *dpm, *dctx, *dy, *gs, *cols, *pb, *pe, *gdc, *gac, *cacc, *gcat, *dv, *weff, *dweff,
       *tmp, *gproj, *weffT, *inv_scale;
   uint8_t *img_d, *img_a; DecoderCtrl* ctrl;
+  uint8_t* bwd_wimg[2];                // W^T images of the skinny GEMMs (bwd_gemm_prepare)
+  void* gemm; size_t gemm_bytes;       // scratch of the gemm_tc products and column sums, shared in stream order
   WgradWs wg;
 };
 void bwd_ws_layout(Carve& c, int B, int Te, int T, BwdWs* w) {
@@ -439,6 +443,15 @@ void bwd_ws_layout(Carve& c, int B, int Te, int T, BwdWs* w) {
   w->inv_scale = c.take<float>(128);
   w->img_d = c.take<uint8_t>(kBwdImgBytes, 1024); w->img_a = c.take<uint8_t>(kBwdImgBytes, 1024);
   w->ctrl = c.take<DecoderCtrl>(1);
+  for (int i = 0; i < 2; ++i) w->bwd_wimg[i] = c.take<uint8_t>(bwd_wimg_bytes(i), 1024);
+  const int BTe = B * Te, TBi = (int)TB;
+  w->gemm_bytes = std::max({gemm_tc_ws_bytes(BTe, kAtt, kEnc), gemm_tc_ws_bytes(TBi, kAtt, kARnn),
+                            gemm_tc_ws_bytes(TBi, kDRnn + kEnc, 81), gemm_tc_ws_bytes(kMel, kDRnn, TBi),
+                            gemm_tc_ws_bytes(kMel, kEnc, TBi), gemm_tc_ws_bytes(1, kDRnn, TBi), gemm_tc_ws_bytes(1, kEnc, TBi),
+                            colsum_ws_bytes(TBi, 81), gemm_tc_ws_bytes(kAtt, kARnn, TBi),
+                            gemm_tc_ws_bytes(kAtt, kColsLd, (int)(TB * Te)), colsum_ws_bytes(T, BTe * kAtt),
+                            gemm_tc_ws_bytes(kAtt, kEnc, BTe), gemm_tc_ws_bytes(BTe, kEnc, kAtt), gemm_tc_ws_bytes(Te, kEnc, T, B)});
+  w->gemm = c.take<char>(w->gemm_bytes);
   wgrad_tc_layout(c, T, &w->wg);
 }
 
@@ -486,13 +499,17 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     T2_LAUNCH_CHECK();
   }
   // processed_memory (model.py:288) and the processed queries of all steps (model.py:57)
-  T2_TRY(gemm_tc_rm(m, s, false, true, B * Te, kAtt, kEnc, a->memory, kEnc, m->w[W_ATT_MEMORY], kEnc, w.pm, kAtt, 0.f));
-  T2_TRY(gemm_tc_rm(m, s, false, true, (int)TB, kAtt, kARnn, st.ha + (size_t)B * kARnn, kARnn, m->w[W_ATT_QUERY], kARnn, w.q, kAtt, 0.f));
+  const int sms = m->sm_count;
+  T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, false, true, B * Te, kAtt, kEnc, a->memory, kEnc, m->w[W_ATT_MEMORY], kEnc, w.pm,
+                    kAtt, 0.f));
+  T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, false, true, (int)TB, kAtt, kARnn, st.ha + (size_t)B * kARnn, kARnn,
+                    m->w[W_ATT_QUERY], kARnn, w.q, kAtt, 0.f));
   // projection / gate contribution to g_dh and g_ctx of every step: [d_mel_t ; d_gate_t] . [W_proj ; W_gate]  (model.py:373-378)
-  T2_TRY(gemm_tc_rm(m, s, false, false, (int)TB, kDRnn + kEnc, 81, w.dy, 81, m->projgate_w, kDRnn + kEnc, w.gproj, kDRnn + kEnc, 0.f));
+  T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, false, false, (int)TB, kDRnn + kEnc, 81, w.dy, 81, m->projgate_w, kDRnn + kEnc,
+                    w.gproj, kDRnn + kEnc, 0.f));
   T2_CUDA(cudaFuncSetAttribute(att_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // skinny GEMMs (KB / KE): weight images, zeroed operand images, control block and unit scales
-  T2_TRY(bwd_gemm_prepare(m, s));
+  T2_TRY(bwd_gemm_prepare(m, w.bwd_wimg, s));
   T2_CUDA(cudaMemsetAsync(w.img_d, 0, kBwdImgBytes, s));      // rows >= B stay zero
   T2_CUDA(cudaMemsetAsync(w.img_a, 0, kBwdImgBytes, s));
   T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
@@ -514,7 +531,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
       lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(bwd_gemm_run(m, 0, w.img_d, w.inv_scale, w.pb, kPBld, w.ctrl, s));   // KB
+    T2_TRY(bwd_gemm_run(m, 0, w.bwd_wimg[0], w.img_d, w.inv_scale, w.pb, kPBld, w.ctrl, s));   // KB
     {  // KC
       AttBwdArgs k;
       memset(&k, 0, sizeof(k));
@@ -540,7 +557,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
       lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(bwd_gemm_run(m, 1, w.img_a, w.inv_scale + 64, w.pe, kPEld, w.ctrl, s));   // KE
+    T2_TRY(bwd_gemm_run(m, 1, w.bwd_wimg[1], w.img_a, w.inv_scale + 64, w.pe, kPEld, w.ctrl, s));   // KE
   }
   reduce_pe_x2_kernel<<<B, 256, 0, s>>>(w.pe, a->d_prenet, B, kBwdGemmSplit);
   T2_LAUNCH_CHECK();
@@ -552,20 +569,25 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   T2_TRY(wgrad_tc_run(m, B, T, w.dga, w.dgd, a->teacher_prenet, st, G, w.wg, s));
   // projection + gate on [dh_t | ctx_t]                                                   model.py:373-378
   if (G[W_PROJ_W]) {
-    T2_TRY(gemm_tc_rm(m, s, true, false, kMel, kDRnn, TBi, w.dy, 81, st.hd + (size_t)B * kDRnn, kDRnn, G[W_PROJ_W], kDRnn + kEnc, 0.f));
-    T2_TRY(gemm_tc_rm(m, s, true, false, kMel, kEnc, TBi, w.dy, 81, st.ctx + (size_t)B * kEnc, kEnc, G[W_PROJ_W] + kDRnn, kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, true, false, kMel, kDRnn, TBi, w.dy, 81, st.hd + (size_t)B * kDRnn, kDRnn,
+                      G[W_PROJ_W], kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, true, false, kMel, kEnc, TBi, w.dy, 81, st.ctx + (size_t)B * kEnc, kEnc,
+                      G[W_PROJ_W] + kDRnn, kDRnn + kEnc, 0.f));
   }
   if (G[W_GATE_W]) {
-    T2_TRY(gemm_tc_rm(m, s, true, false, 1, kDRnn, TBi, w.dy + 80, 81, st.hd + (size_t)B * kDRnn, kDRnn, G[W_GATE_W], kDRnn + kEnc, 0.f));
-    T2_TRY(gemm_tc_rm(m, s, true, false, 1, kEnc, TBi, w.dy + 80, 81, st.ctx + (size_t)B * kEnc, kEnc, G[W_GATE_W] + kDRnn, kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, true, false, 1, kDRnn, TBi, w.dy + 80, 81, st.hd + (size_t)B * kDRnn, kDRnn,
+                      G[W_GATE_W], kDRnn + kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, true, false, 1, kEnc, TBi, w.dy + 80, 81, st.ctx + (size_t)B * kEnc, kEnc,
+                      G[W_GATE_W] + kDRnn, kDRnn + kEnc, 0.f));
   }
   if (G[W_PROJ_B] || G[W_GATE_B]) {
-    T2_TRY(colsum_f32(m, s, w.dy, 81, TBi, 81, w.tmp));
+    T2_TRY(colsum_f32(s, w.gemm, w.gemm_bytes, w.dy, 81, TBi, 81, w.tmp));
     if (G[W_PROJ_B]) T2_CUDA(cudaMemcpyAsync(G[W_PROJ_B], w.tmp, 80 * 4, cudaMemcpyDeviceToDevice, s));
     if (G[W_GATE_B]) T2_CUDA(cudaMemcpyAsync(G[W_GATE_B], w.tmp + 80, 4, cudaMemcpyDeviceToDevice, s));
   }
   if (G[W_ATT_QUERY])
-    T2_TRY(gemm_tc_rm(m, s, true, false, kAtt, kARnn, TBi, w.dq, kAtt, st.ha + (size_t)B * kARnn, kARnn, G[W_ATT_QUERY], kARnn, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, true, false, kAtt, kARnn, TBi, w.dq, kAtt, st.ha + (size_t)B * kARnn, kARnn,
+                      G[W_ATT_QUERY], kARnn, 0.f));
   if (G[W_ATT_V]) {
     sum_rows_kernel<<<1, 128, 0, s>>>(w.dv, G[W_ATT_V], B, 128);
     T2_LAUNCH_CHECK();
@@ -576,24 +598,27 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     T2_LAUNCH_CHECK();
     // K = T*B*Te rows in one call: the GEMM drains its accumulator every 64 rows and splits K over the SMs
     const int R = (int)((long)TB * Te);
-    T2_TRY(gemm_tc_rm(m, s, true, false, kAtt, kColsLd, R, w.gs, kAtt, w.cols, kColsLd, w.dweff, kColsLd, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, true, false, kAtt, kColsLd, R, w.gs, kAtt, w.cols, kColsLd, w.dweff, kColsLd, 0.f));
     dweff_split_kernel<<<(kAtt * kLocF + 255) / 256, 256, 0, s>>>(w.dweff, m->w[W_ATT_LOC_DENSE], m->w[W_ATT_LOC_CONV],
                                                                   G[W_ATT_LOC_DENSE], G[W_ATT_LOC_CONV]);
     T2_LAUNCH_CHECK();
   }
   // d_pm = sum_t g_s[t]  -> memory_layer gradient and its share of d_memory              model.py:288
-  T2_TRY(colsum_f32(m, s, w.gs, (long)B * Te * kAtt, T, B * Te * kAtt, w.dpm));
+  T2_TRY(colsum_f32(s, w.gemm, w.gemm_bytes, w.gs, (long)B * Te * kAtt, T, B * Te * kAtt, w.dpm));
   if (G[W_ATT_MEMORY])
-    T2_TRY(gemm_tc_rm(m, s, true, false, kAtt, kEnc, B * Te, w.dpm, kAtt, a->memory, kEnc, G[W_ATT_MEMORY], kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, true, false, kAtt, kEnc, B * Te, w.dpm, kAtt, a->memory, kEnc, G[W_ATT_MEMORY],
+                      kEnc, 0.f));
   if (a->d_memory) {
-    T2_TRY(gemm_tc_rm(m, s, false, false, B * Te, kEnc, kAtt, w.dpm, kAtt, m->w[W_ATT_MEMORY], kEnc, a->d_memory, kEnc, 0.f));
+    T2_TRY(gemm_tc_rm(sms, s, w.gemm, w.gemm_bytes, false, false, B * Te, kEnc, kAtt, w.dpm, kAtt, m->w[W_ATT_MEMORY], kEnc,
+                      a->d_memory, kEnc, 0.f));
     // + sum_t aw_t[b] (x) g_ctx_t[b]: per row b, (Te x T) . (T x 512)                      model.py:83-84
     GemmTc g;        // d_memory[b] (Te x 512) += align[b]^T (T x Te stored) . dctx[:, b, :] (T x 512, rows B * 512 apart)
     g.ta = true; g.tb = false; g.M = Te; g.N = kEnc; g.K = T;
     g.A = a->align; g.lda = Te; g.strideA = (long)T * Te;
     g.B = w.dctx; g.ldb = (long)B * kEnc; g.strideB = kEnc;
     g.C = a->d_memory; g.ldc = kEnc; g.strideC = (long)Te * kEnc; g.beta = 1.f; g.batch = B;
-    T2_TRY(gemm_tc(m, s, g));
+    g.ws = w.gemm; g.ws_bytes = w.gemm_bytes;
+    T2_TRY(gemm_tc(sms, s, g));
   }
   return T2_OK;
 }
@@ -601,10 +626,15 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------
 // Prenet backward (model.py:97-100): recompute both layers with the same masks, then two plain GEMMs each.
 // ---------------------------------------------------------------------------------------------
-struct PrenetBwdWs { float *x1, *x2, *dz2, *dz1; };   // (M, 256) each
+struct PrenetBwdWs {
+  float *x1, *x2, *dz2, *dz1;       // (M, 256) each
+  void* gemm; size_t gemm_bytes;    // scratch of the three products
+};
 static void prenet_backward_ws_layout(Carve& c, int M, PrenetBwdWs* w) {
   w->x1 = c.take<float>((size_t)M * kPre); w->x2 = c.take<float>((size_t)M * kPre);
   w->dz2 = c.take<float>((size_t)M * kPre); w->dz1 = c.take<float>((size_t)M * kPre);
+  w->gemm_bytes = std::max({gemm_tc_ws_bytes(kPre, kPre, M), gemm_tc_ws_bytes(M, kPre, kPre), gemm_tc_ws_bytes(kPre, kMel, M)});
+  w->gemm = c.take<char>(w->gemm_bytes);
 }
 size_t prenet_backward_ws_bytes(int M) { Carve c(nullptr); PrenetBwdWs w; prenet_backward_ws_layout(c, M, &w); return c.bytes(); }
 
@@ -628,12 +658,17 @@ int prenet_backward(T2Model* m, const T2PrenetBwdArgs* a, cudaStream_t s) {
   const long n = (long)M * kPre;
   prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a->d_out, w.x2, w.dz2, n);
   T2_LAUNCH_CHECK();
-  if (a->grads[W_PRENET1]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kPre, M, w.dz2, kPre, w.x1, kPre, a->grads[W_PRENET1], kPre, 0.f));
+  if (a->grads[W_PRENET1])
+    T2_TRY(gemm_tc_rm(m->sm_count, s, w.gemm, w.gemm_bytes, true, false, kPre, kPre, M, w.dz2, kPre, w.x1, kPre, a->grads[W_PRENET1],
+                      kPre, 0.f));
   // d_x1 = w.dz2 . W2  -> through dropout o relu of layer 1
-  T2_TRY(gemm_tc_rm(m, s, false, false, M, kPre, kPre, w.dz2, kPre, m->w[W_PRENET1], kPre, w.dz1, kPre, 0.f));
+  T2_TRY(gemm_tc_rm(m->sm_count, s, w.gemm, w.gemm_bytes, false, false, M, kPre, kPre, w.dz2, kPre, m->w[W_PRENET1], kPre, w.dz1,
+                    kPre, 0.f));
   prenet_dz_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.dz1, w.x1, w.dz1, n);
   T2_LAUNCH_CHECK();
-  if (a->grads[W_PRENET0]) T2_TRY(gemm_tc_rm(m, s, true, false, kPre, kMel, M, w.dz1, kPre, a->frames, kMel, a->grads[W_PRENET0], kMel, 0.f));
+  if (a->grads[W_PRENET0])
+    T2_TRY(gemm_tc_rm(m->sm_count, s, w.gemm, w.gemm_bytes, true, false, kPre, kMel, M, w.dz1, kPre, a->frames, kMel,
+                      a->grads[W_PRENET0], kMel, 0.f));
   return T2_OK;
 }
 

@@ -98,10 +98,11 @@ struct PersistentPack {
   int32_t* rows = nullptr;            // row tables for packing
   float* weff = nullptr;              // (128, 64) fp32 fused location filter W_ld . W_loc (62 taps + 2 zero)
   uint8_t* weff_img = nullptr;        // its split-fp16 operand image (32 KiB)
-  // backward skinny GEMMs (training): W^T images of [W_ih | W_hh] of the decoder (0) and attention (1) LSTM
-  uint8_t* bwd_wimg[2] = {nullptr, nullptr};
-  struct BwdCta* bwd_plans[2] = {nullptr, nullptr};
+  // backward skinny GEMMs (training): CTA plans of the decoder (0) and attention (1) LSTM (their weight images are packed
+  // into the backward workspace by every call)
+  BwdCta* bwd_plans[2] = {nullptr, nullptr};
 };
+std::vector<BwdCta> bwd_gemm_plans(int which);   // the CTA plans of a backward skinny GEMM
 
 // ---------------------------------------------------------------------------------------------
 // packing kernels (model create time)
@@ -1235,6 +1236,7 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
       if (pl.ev[ev].nrows != 0 && !event_plan_fits(pl.ev[ev], false)) return fail(T2_ERR_INVALID, "event plan does not fit the MMA warpgroups");
   }
   if (off >= (size_t)4 << 30) return fail(T2_ERR_INVALID, "W image too large");
+  const std::vector<BwdCta> bwd_plans[2] = {bwd_gemm_plans(0), bwd_gemm_plans(1)};
   if (!pk->wimg) {
     pk->wimg_bytes = off + 1024;
     T2_CUDA(cudaMalloc((void**)&pk->wimg, pk->wimg_bytes));
@@ -1246,13 +1248,17 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
     T2_CUDA(cudaMalloc((void**)&pk->rows, (size_t)4 * kG * 32 * 4));
     T2_CUDA(cudaMalloc((void**)&pk->weff, (size_t)kAtt * kChunkK * 4));
     T2_CUDA(cudaMalloc((void**)&pk->weff_img, (size_t)kWeffBytes));
+    for (int which = 0; which < 2; ++which) T2_CUDA(cudaMalloc((void**)&pk->bwd_plans[which], sizeof(BwdCta) * bwd_plans[which].size()));
   }
   fuse_location_kernel<<<kAtt, kChunkK, 0, s>>>(m->w[W_ATT_LOC_DENSE], m->w[W_ATT_LOC_CONV], pk->weff);
   T2_LAUNCH_CHECK();
   pack_rows_image_kernel<<<1, 256, 0, s>>>(pk->weff, kAtt, kChunkK, pk->weff_img);
   T2_LAUNCH_CHECK();
   T2_CUDA(cudaMemcpyAsync(pk->plans, plans.data(), sizeof(CtaPlan) * kG, cudaMemcpyHostToDevice, s));
-  T2_CUDA(cudaStreamSynchronize(s));   // `plans` is a host temporary
+  for (int which = 0; which < 2; ++which)
+    T2_CUDA(cudaMemcpyAsync(pk->bwd_plans[which], bwd_plans[which].data(), sizeof(BwdCta) * bwd_plans[which].size(),
+                            cudaMemcpyHostToDevice, s));
+  T2_CUDA(cudaStreamSynchronize(s));   // `plans` and `bwd_plans` are host temporaries
   // ---- W_P = [proj (80) ; gate (1) ; W1.Wproj (256) ; 0 (7)] and its bias ----
   T2_CUDA(cudaMemsetAsync(pk->wp_all, 0, (size_t)kPCols * kdc * 4, s));
   T2_CUDA(cudaMemsetAsync(pk->bias_p, 0, (size_t)kPCols * 4, s));
@@ -1300,7 +1306,7 @@ void persistent_pack_destroy(T2Model* m) {
   if (!pk) return;
   cudaFree(pk->wimg); cudaFree(pk->plans); cudaFree(pk->wp_all); cudaFree(pk->bias_p);
   cudaFree(pk->bias_a); cudaFree(pk->bias_d); cudaFree(pk->rows); cudaFree(pk->weff); cudaFree(pk->weff_img);
-  for (int i = 0; i < 2; ++i) { cudaFree(pk->bwd_wimg[i]); cudaFree(pk->bwd_plans[i]); }
+  for (int i = 0; i < 2; ++i) cudaFree(pk->bwd_plans[i]);
   delete pk;
   m->pk = nullptr;
 }
@@ -1724,52 +1730,52 @@ bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w
 
 int bwd_gemm_ctas(int which) { return which == 0 ? (2560 / kBwdTileB) * kBwdGemmSplit : (1792 / kBwdTileE) * kBwdGemmSplit; }
 
-// (re)builds the W^T images of both LSTMs from the caller's current fp32 weights (once per backward call)
-int bwd_gemm_prepare(T2Model* m, cudaStream_t s) {
+namespace {
+constexpr int kBwdChunks = 4 * kARnn / kChunkK;                   // 64 K chunks
+int bwd_tile(int which) { return which == 0 ? kBwdTileB : kBwdTileE; }
+uint32_t bwd_w_bytes(int which) { return (uint32_t)(2 * bwd_tile(which) * kChunkK * 2); }
+
+std::vector<BwdCta> bwd_gemm_plans(int which) {
+  const int tile = bwd_tile(which), ntile = (which == 0 ? 2560 : 1792) / tile;
+  const uint32_t w_bytes = bwd_w_bytes(which);
+  std::vector<BwdCta> plans(ntile * kBwdGemmSplit);
+  for (int t = 0; t < ntile; ++t)
+    for (int sp = 0; sp < kBwdGemmSplit; ++sp) {
+      BwdCta& c = plans[t * kBwdGemmSplit + sp];
+      memset(&c, 0, sizeof(c));
+      c.chunk0 = sp * kBwdChunks / kBwdGemmSplit; c.nchunks = (sp + 1) * kBwdChunks / kBwdGemmSplit - c.chunk0;
+      c.col0 = t * tile; c.split = sp;
+      plan_one_matrix(c.ep, tile);    // 80 = 32 + 32 + 16, 64 = 32 + 32 columns (event_plan_fits(c.ep, false))
+      c.ep.col0 = 0; c.ep.chunks = c.nchunks;
+      c.ep.w_off = (uint32_t)(((size_t)t * kBwdChunks + c.chunk0) * w_bytes);
+    }
+  return plans;
+}
+}  // namespace
+
+size_t bwd_wimg_bytes(int which) { return (size_t)((which == 0 ? 2560 : 1792) / bwd_tile(which)) * kBwdChunks * bwd_w_bytes(which); }
+
+// packs the W^T images of both LSTMs from the caller's current fp32 weights into wimg[0 / 1] (bwd_wimg_bytes)
+int bwd_gemm_prepare(T2Model* m, uint8_t* const* wimg, cudaStream_t s) {
   PersistentPack* pk = (PersistentPack*)m->pk;
   if (!pk) return fail(T2_ERR_INVALID, "backward GEMM: model has no persistent pack");
   for (int which = 0; which < 2; ++which) {
-    const int tile = which == 0 ? kBwdTileB : kBwdTileE;
-    const int cols = which == 0 ? 2560 : 1792;
-    const int ntile = cols / tile, ncta = ntile * kBwdGemmSplit;
-    const int chunks = 4 * kARnn / kChunkK;                    // 64 K chunks
-    const uint32_t w_bytes = (uint32_t)(2 * tile * kChunkK * 2);
-    if (!pk->bwd_plans[which]) {
-      std::vector<BwdCta> plans(ncta);
-      for (int t = 0; t < ntile; ++t)
-        for (int sp = 0; sp < kBwdGemmSplit; ++sp) {
-          BwdCta& c = plans[t * kBwdGemmSplit + sp];
-          memset(&c, 0, sizeof(c));
-          c.chunk0 = sp * chunks / kBwdGemmSplit; c.nchunks = (sp + 1) * chunks / kBwdGemmSplit - c.chunk0;
-          c.col0 = t * tile; c.split = sp;
-          plan_one_matrix(c.ep, tile);    // 80 = 32 + 32 + 16, 64 = 32 + 32 columns (event_plan_fits(c.ep, false))
-          c.ep.col0 = 0; c.ep.chunks = c.nchunks;
-          c.ep.w_off = (uint32_t)(((size_t)t * chunks + c.chunk0) * w_bytes);
-        }
-      T2_CUDA(cudaMalloc((void**)&pk->bwd_plans[which], sizeof(BwdCta) * ncta));
-      T2_CUDA(cudaMemcpyAsync(pk->bwd_plans[which], plans.data(), sizeof(BwdCta) * ncta, cudaMemcpyHostToDevice, s));
-      T2_CUDA(cudaStreamSynchronize(s));
-      T2_CUDA(cudaMalloc((void**)&pk->bwd_wimg[which], (size_t)ntile * chunks * w_bytes));
-    }
     const float* w0 = m->w[which == 0 ? W_DRNN_WIH : W_ARNN_WIH];
     const float* w1 = m->w[which == 0 ? W_DRNN_WHH : W_ARNN_WHH];
     const int cols0 = which == 0 ? kARnn + kEnc : kPre + kEnc;
-    pack_bwd_wimg_kernel<<<dim3(chunks / kBwdGemmSplit, ncta), 256, 0, s>>>(w0, cols0, w1, kARnn, pk->bwd_plans[which], pk->bwd_wimg[which]);
+    pack_bwd_wimg_kernel<<<dim3(kBwdChunks / kBwdGemmSplit, bwd_gemm_ctas(which)), 256, 0, s>>>(w0, cols0, w1, kARnn,
+                                                                                             pk->bwd_plans[which], wimg[which]);
     T2_LAUNCH_CHECK();
   }
   return T2_OK;
 }
 
-int bwd_gemm_run(T2Model* m, int which, const uint8_t* x_img, const float* inv_scale, float* P, int ldp, DecoderCtrl* ctrl,
-                 cudaStream_t s) {
+int bwd_gemm_run(T2Model* m, int which, const uint8_t* w_img, const uint8_t* x_img, const float* inv_scale, float* P, int ldp,
+                 DecoderCtrl* ctrl, cudaStream_t s) {
   PersistentPack* pk = (PersistentPack*)m->pk;
   const size_t smem = gemm_smem_bytes();
-  static bool attr_set = false;
-  if (!attr_set) {
-    T2_CUDA(cudaFuncSetAttribute(bwd_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
-  bwd_gemm_kernel<<<bwd_gemm_ctas(which), kThreads, smem, s>>>(x_img, pk->bwd_wimg[which], pk->bwd_plans[which], inv_scale, P, ldp, ctrl);
+  T2_CUDA(cudaFuncSetAttribute(bwd_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  bwd_gemm_kernel<<<bwd_gemm_ctas(which), kThreads, smem, s>>>(x_img, w_img, pk->bwd_plans[which], inv_scale, P, ldp, ctrl);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }

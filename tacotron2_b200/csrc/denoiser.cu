@@ -325,10 +325,10 @@ static int pack(T2Denoiser* m, const float* fwd, const float* inv, cudaStream_t 
   T2_CUDA(cudaMemcpyAsync(m->fwd, fwd, (size_t)kBasisRows * kFilter * sizeof(float), cudaMemcpyDeviceToDevice, s));
   build_fwd_kernel<<<kFwdN, 256, 0, s>>>(fwd, m->tmp);
   T2_LAUNCH_CHECK();
-  T2_TRY(tc_pack_weights(m->tmp, kFwdN, kFilter, 1, kNT, &m->fwd_img, s));
+  T2_TRY(tc_pack_weights(m->tmp, kFwdN, kFilter, 1, kNT, m->fwd_img, s));
   build_inv_kernel<<<kHop, 256, 0, s>>>(inv, m->tmp);
   T2_LAUNCH_CHECK();
-  T2_TRY(tc_pack_weights(m->tmp, kHop, kInvK, 1, kNT, &m->inv_img, s));
+  T2_TRY(tc_pack_weights(m->tmp, kHop, kInvK, 1, kNT, m->inv_img, s));
   return T2_OK;
 }
 
@@ -347,7 +347,9 @@ int denoiser_create(T2Denoiser** out, const T2DenoiserConfig* c, const float* fw
   int r = T2_OK;
   if (cudaMalloc((void**)&m->fwd, (size_t)kBasisRows * kFilter * sizeof(float)) != cudaSuccess ||
       cudaMalloc((void**)&m->wsq, kFilter * sizeof(double)) != cudaSuccess ||
-      cudaMalloc((void**)&m->tmp, (size_t)std::max(kFwdN * kFilter, kHop * kInvK) * sizeof(float)) != cudaSuccess)
+      cudaMalloc((void**)&m->tmp, (size_t)std::max(kFwdN * kFilter, kHop * kInvK) * sizeof(float)) != cudaSuccess ||
+      cudaMalloc((void**)&m->fwd_img, tc_weights_bytes(kFwdN, kFilter, 1, kNT)) != cudaSuccess ||
+      cudaMalloc((void**)&m->inv_img, tc_weights_bytes(kHop, kInvK, 1, kNT)) != cudaSuccess)
     r = fail(T2_ERR_CUDA, "denoiser: out of device memory for the packed bases");
   if (r == T2_OK) {
     build_wsq_kernel<<<kFilter / 256, 256, 0, s>>>(m->wsq);

@@ -318,43 +318,40 @@ __global__ void colsum_final_kernel(const float* __restrict__ part, int nsplit, 
 
 }  // namespace
 
-static int gemm_scratch(T2Model* m, size_t bytes, char** out) {
-  if (m->gemm_ws_bytes < bytes) {
-    if (m->gemm_ws) T2_CUDA(cudaFree(m->gemm_ws));
-    m->gemm_ws = nullptr; m->gemm_ws_bytes = 0;
-    const size_t want = bytes + (bytes >> 2) + (1 << 20);
-    T2_CUDA(cudaMalloc(&m->gemm_ws, want));
-    m->gemm_ws_bytes = want;
-  }
-  *out = (char*)m->gemm_ws;
-  return T2_OK;
-}
-
-void gemm_tc_destroy(T2Model* m) {
-  if (m->gemm_ws) cudaFree(m->gemm_ws);
-  m->gemm_ws = nullptr; m->gemm_ws_bytes = 0;
-}
-
-int gemm_tc(T2Model* m, cudaStream_t s, const GemmTc& g) {
-  if (g.M <= 0 || g.N <= 0 || g.K <= 0) return fail(T2_ERR_INVALID, "gemm_tc: empty problem %d x %d x %d", g.M, g.N, g.K);
-  const int batch = g.batch > 0 ? g.batch : 1;
-  const int ntm = (g.M + kBM - 1) / kBM, ntn = (g.N + kBN - 1) / kBN, nchunks = (g.K + kBK - 1) / kBK;
-  const long tiles = (long)ntm * ntn * batch;
+// The split rule: small-tile / large-K problems are split along K so that they fill one wave of CTAs (1 CTA / SM:
+// 161 KiB of shared memory).  Scratch: [amax (M)][bmax (N)][partial tiles of the K splits].
+struct Plan { int ntm, ntn, splits, cps; long tiles; size_t off_part, bytes; };
+static Plan plan(int M, int N, int K, int batch, int sms) {
+  Plan p;
+  p.ntm = (M + kBM - 1) / kBM; p.ntn = (N + kBN - 1) / kBN;
+  const int nchunks = (K + kBK - 1) / kBK;
+  p.tiles = (long)p.ntm * p.ntn * batch;
   int splits = 1;
-  const int sms = m->sm_count > 0 ? m->sm_count : 132;
-  if (tiles * 5 < sms * 4 && nchunks >= 8) {   // fill one wave of CTAs (1 CTA / SM: 161 KiB of shared memory)
-    splits = tiles <= sms / 2 ? (int)(sms / tiles) : 2;
+  if (p.tiles * 5 < sms * 4 && nchunks >= 8) {
+    splits = p.tiles <= sms / 2 ? (int)(sms / p.tiles) : 2;
     if (splits > nchunks / 4) splits = nchunks / 4;
     if (splits < 1) splits = 1;
   }
-  const int cps = (nchunks + splits - 1) / splits;
-  splits = (nchunks + cps - 1) / cps;
-  // scratch: [amax (batch x M)][bmax (batch x N)][partials]
+  p.cps = (nchunks + splits - 1) / splits;
+  p.splits = (nchunks + p.cps - 1) / p.cps;
+  p.off_part = (((size_t)M + N) * 4 + 255) & ~(size_t)255;
+  p.bytes = p.off_part + (p.splits > 1 ? (size_t)p.tiles * p.splits * kBM * kBN * 4 : 0);
+  return p;
+}
+
+// The split count never falls as the SM count grows, so the plan for a full GH100 (144 SMs) bounds every sm_90a device.
+size_t gemm_tc_ws_bytes(int M, int N, int K, int batch) {
+  return M > 0 && N > 0 && K > 0 ? plan(M, N, K, batch > 0 ? batch : 1, 144).bytes : 0;
+}
+
+int gemm_tc(int sm_count, cudaStream_t s, const GemmTc& g) {
+  if (g.M <= 0 || g.N <= 0 || g.K <= 0) return fail(T2_ERR_INVALID, "gemm_tc: empty problem %d x %d x %d", g.M, g.N, g.K);
+  const int batch = g.batch > 0 ? g.batch : 1;
+  const Plan pl = plan(g.M, g.N, g.K, batch, sm_count);
+  const int ntm = pl.ntm, ntn = pl.ntn, splits = pl.splits, cps = pl.cps;
+  if (g.ws_bytes < pl.bytes) return fail(T2_ERR_WORKSPACE, "gemm_tc: scratch of %zu bytes, %zu needed", g.ws_bytes, pl.bytes);
   const size_t n_a = (size_t)g.M, n_b = (size_t)g.N;
-  const size_t off_part = ((n_a + n_b) * 4 + 255) & ~(size_t)255;
-  const size_t part_bytes = splits > 1 ? (size_t)tiles * splits * kBM * kBN * 4 : 0;
-  char* ws = nullptr;
-  T2_TRY(gemm_scratch(m, off_part + part_bytes, &ws));
+  char* ws = (char*)g.ws;
   unsigned int* amax = (unsigned int*)ws;
   unsigned int* bmax = amax + n_a;
   // one scale per row of op(A) / column of op(B), shared by the batch entries (maximum over the batch)
@@ -374,17 +371,13 @@ int gemm_tc(T2Model* m, cudaStream_t s, const GemmTc& g) {
   }
   GemmP p;
   memset(&p, 0, sizeof(p));
-  p.A = g.A; p.B = g.B; p.C = g.C; p.part = splits > 1 ? (float*)(ws + off_part) : nullptr;
+  p.A = g.A; p.B = g.B; p.C = g.C; p.part = splits > 1 ? (float*)(ws + pl.off_part) : nullptr;
   p.amax = amax; p.bmax = bmax;
   p.lda = g.lda; p.ldb = g.ldb; p.ldc = g.ldc; p.sA = g.strideA; p.sB = g.strideB; p.sC = g.strideC;
   p.M = g.M; p.N = g.N; p.K = g.K; p.ta = g.ta ? 1 : 0; p.tb = g.tb ? 1 : 0; p.splits = splits; p.chunks_per_split = cps;
   p.batch = batch; p.beta = g.beta;
-  static bool attr_set = false;
   const size_t smem = (size_t)kSmemG;
-  if (!attr_set) {
-    T2_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  T2_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   gemm_tc_kernel<<<dim3(ntn, ntm, batch * splits), kThreadsG, smem, s>>>(p);
   T2_LAUNCH_CHECK();
   if (splits > 1) {
@@ -396,21 +389,24 @@ int gemm_tc(T2Model* m, cudaStream_t s, const GemmTc& g) {
   return T2_OK;
 }
 
-int gemm_tc_rm(T2Model* m, cudaStream_t s, bool ta, bool tb, int M, int N, int K, const float* A, long lda, const float* B,
-               long ldb, float* C, long ldc, float beta) {
+int gemm_tc_rm(int sm_count, cudaStream_t s, void* ws, size_t ws_bytes, bool ta, bool tb, int M, int N, int K, const float* A,
+               long lda, const float* B, long ldb, float* C, long ldc, float beta) {
   GemmTc g;
   g.ta = ta; g.tb = tb; g.M = M; g.N = N; g.K = K; g.A = A; g.lda = lda; g.B = B; g.ldb = ldb; g.C = C; g.ldc = ldc; g.beta = beta;
-  return gemm_tc(m, s, g);
+  g.ws = ws; g.ws_bytes = ws_bytes;
+  return gemm_tc(sm_count, s, g);
 }
 
-int colsum_f32(T2Model* m, cudaStream_t s, const float* X, long ld, long rows, int cols, float* out) {
+static int colsum_splits(long rows) {
+  const long nsplit = rows / 64;
+  return nsplit < 1 ? 1 : (nsplit > kColSplit ? kColSplit : (int)nsplit);
+}
+size_t colsum_ws_bytes(long rows, int cols) { return (size_t)colsum_splits(rows) * cols * 4; }
+
+int colsum_f32(cudaStream_t s, void* ws, size_t ws_bytes, const float* X, long ld, long rows, int cols, float* out) {
   if (rows <= 0 || cols <= 0) return fail(T2_ERR_INVALID, "colsum: empty input");
-  char* ws = nullptr;
-  // the partial sums live behind the GEMM scratch header so a colsum never clobbers a GEMM in flight on the same stream
-  // (stream order) -- both use the scratch only inside their own launches
-  int nsplit = (int)(rows / 64);
-  nsplit = nsplit < 1 ? 1 : (nsplit > kColSplit ? kColSplit : nsplit);
-  T2_TRY(gemm_scratch(m, (size_t)nsplit * cols * 4, &ws));
+  const int nsplit = colsum_splits(rows);
+  if (ws_bytes < colsum_ws_bytes(rows, cols)) return fail(T2_ERR_WORKSPACE, "colsum: scratch too small");
   colsum_part_kernel<<<dim3((cols + 31) / 32, nsplit), 256, 0, s>>>(X, ld, rows, cols, (float*)ws);
   T2_LAUNCH_CHECK();
   colsum_final_kernel<<<(cols + 255) / 256, 256, 0, s>>>((const float*)ws, nsplit, cols, out);

@@ -10,6 +10,8 @@
 //                        -> log(clamp(., clip_val)), written as (B, n_mel, n_frames)                (layers.py:79, audio_processing.py:78-84)
 //
 // Both products run on gemm_tc.cu (split-fp16 wgmma, fp32-grade).
+#include <algorithm>
+
 #include "gemm_tc.h"
 
 namespace t2 {
@@ -50,13 +52,16 @@ __global__ void log_transpose_kernel(const float* __restrict__ mel, int n_frames
   }
 }
 
-struct MelSpecWs { float *ypad, *ft, *mag, *mel; };
+struct MelSpecWs { float *ypad, *ft, *mag, *mel; void* gemm; size_t gemm_bytes; };
 void mel_ws_layout(Carve& c, int B, int n, int fl, int hop, int n_mel, MelSpecWs* w) {
   const long frames = n / hop + 1, cutoff = fl / 2 + 1;
   w->ypad = c.take<float>((size_t)B * (n + fl));                // reflect-padded signal
   w->ft = c.take<float>((size_t)B * frames * 2 * cutoff);       // Fourier transform (real | imaginary)
   w->mag = c.take<float>((size_t)B * frames * cutoff);
   w->mel = c.take<float>((size_t)B * frames * n_mel);           // (B frames, n_mel) before the log / transpose
+  w->gemm_bytes = std::max(gemm_tc_ws_bytes((int)frames, (int)(2 * cutoff), fl, B),
+                           gemm_tc_ws_bytes((int)(B * frames), n_mel, (int)cutoff));
+  w->gemm = c.take<char>(w->gemm_bytes);                        // scratch of both products
 }
 
 }  // namespace
@@ -87,7 +92,6 @@ int t2_mel_spectrogram(const T2MelSpecArgs* a, void* stream) {
   Carve c(a->ws);
   MelSpecWs w;
   mel_ws_layout(c, B, n, fl, hop, n_mel, &w);
-  static T2Model scratch_owner;               // only its GEMM scratch is used (grown on demand, kept for the process)
   reflect_pad_kernel<<<dim3((unsigned)((padded + 255) / 256 > 1024 ? 1024 : (padded + 255) / 256), B), 256, 0, s>>>(a->y, n, fl / 2, w.ypad);
   T2_LAUNCH_CHECK();
   GemmTc g;                                   // w.ft[b] (frames x 2 cutoff) = frames(b) . forward_basis^T
@@ -95,11 +99,13 @@ int t2_mel_spectrogram(const T2MelSpecArgs* a, void* stream) {
   g.A = w.ypad; g.lda = hop; g.strideA = padded;
   g.B = a->forward_basis; g.ldb = fl; g.strideB = 0;
   g.C = w.ft; g.ldc = 2 * cutoff; g.strideC = (long)frames * 2 * cutoff; g.batch = B;
-  T2_TRY(gemm_tc(&scratch_owner, s, g));
+  g.ws = w.gemm; g.ws_bytes = w.gemm_bytes;
+  T2_TRY(gemm_tc(kGemmTcSms, s, g));
   const long rows = (long)B * frames;
   magnitude_kernel<<<(unsigned)((rows * cutoff + 255) / 256 > 4096 ? 4096 : (rows * cutoff + 255) / 256), 256, 0, s>>>(w.ft, rows, cutoff, w.mag);
   T2_LAUNCH_CHECK();
-  T2_TRY(gemm_tc_rm(&scratch_owner, s, false, true, (int)rows, n_mel, cutoff, w.mag, cutoff, a->mel_basis, cutoff, w.mel, n_mel, 0.f));
+  T2_TRY(gemm_tc_rm(kGemmTcSms, s, w.gemm, w.gemm_bytes, false, true, (int)rows, n_mel, cutoff, w.mag, cutoff, a->mel_basis, cutoff,
+                    w.mel, n_mel, 0.f));
   log_transpose_kernel<<<dim3((frames + 31) / 32, (n_mel + 31) / 32, B), dim3(32, 8), 0, s>>>(w.mel, frames, n_mel, a->clip_val, a->mel);
   T2_LAUNCH_CHECK();
   return T2_OK;

@@ -23,13 +23,9 @@ struct T2Model {
   uint8_t* tc_enc_conv[3] = {};  // (512, 512, 5)  n-tile 256
   uint8_t* tc_enc_wih = nullptr; // (2048, 512)    n-tile 256, taps = 1
   uint8_t* tc_post_conv[5] = {}; // n-tile 256 (layers 0-3), 80 (layer 4)
-  // training: input-gradient convolutions = the same engine with flipped / transposed weights (re-packed per backward)
-  uint8_t* tc_dgrad_enc[3] = {}; uint8_t* tc_dgrad_post[5] = {};
-  float* dgrad_tmp = nullptr;    // (512, 512, 5) fp32 scratch for the flipped weights
 
   // ---- packed operands of the persistent decoder kernel (owned; see decoder_persistent.cu) ----
   void* pk = nullptr;            // opaque PersistentPack*
-  void* gemm_ws = nullptr; size_t gemm_ws_bytes = 0;   // scratch of gemm_tc.cu (operand scales, split-K partial tiles)
 };
 
 namespace t2 {

@@ -12,6 +12,8 @@
 // BiLSTM backward: reverse recurrence with one skinny GEMM + one elementwise kernel per step and direction.
 #include <string.h>
 
+#include <algorithm>
+
 #include "conv_tc.h"
 #include "decoder.h"
 #include "gemm_f32.cuh"
@@ -26,6 +28,8 @@ namespace {
 constexpr int kPadRows = 2;
 inline long prow(int b, int t, int T) { return (long)b * (T + 2 * kPadRows) + kPadRows + t; }
 __device__ __forceinline__ long d_prow(int b, int t, int T) { return (long)b * (T + 2 * kPadRows) + kPadRows + t; }
+// M of the forward conv GEMMs: the padded rows from the first valid row to the last
+inline int conv_fwd_rows(int B, int T) { return B * (T + 2 * kPadRows) - 2 * kPadRows; }
 
 // ---- layout conversion ---------------------------------------------------------------------------
 // rows (B, T, C) with batch stride -> padded rows (valid rows only; the buffer was zeroed).  len (B) or null: frames
@@ -271,7 +275,6 @@ struct ConvLayer {
   const float* wpk;                  // packed fp32 weights (cout, 5, cin)
   int wbase;                         // index of conv.weight in the state_dict table
   uint32_t site; const uint8_t* keep;
-  uint8_t** wimg_dgrad;              // storage of the flipped / transposed image of the input-gradient conv
 };
 // The training FORWARD convs stay on 5 row-shifted gemm_tc products (one accumulation chain per 64-wide K chunk, 7e-7):
 // the conv engine accumulates ~100-480 MMAs in one chain (3e-6 ... 1e-5 output error; the accumulator update truncates)
@@ -323,7 +326,7 @@ int tc_train_conv(T2Model* m, const float* xp, int cin, const uint8_t* wimg, int
 // ---- conv weight gradient on the wgmma engine (wgrad_tc.cu) ---------------------------------------------------------
 // dW_k[co][ci] = sum_r G_z[r][co] X[r + k - 2][ci]: K = padded rows in chunks of 64, A = G_z^T images (per-channel power-of-two
 // scale), B = X^T images, one set per tap (source rows shifted by k - 2), 128 x 256 tiles, K splits reduced in a fixed order.
-struct WgConvWs { uint8_t* img_a; uint8_t* img_b; float* part; float* stat; float* scale; float* inv; float* colsum; WgJob* jobs; };
+struct WgConvWs { uint8_t* img_a; uint8_t* img_b; float* part; float* stat; float* scale; float* inv; float* colsum; };
 void wgconv_layout(Carve& c, int B, int T, WgConvWs* w) {    // every region 1024-aligned
   const long Mp = (long)B * (T + 2 * kPadRows);
   const long nch = (Mp + 63) / 64;
@@ -333,7 +336,6 @@ void wgconv_layout(Carve& c, int B, int T, WgConvWs* w) {    // every region 102
   w->part = c.take<float>((size_t)nsplit * 512 * (kConvK * 512), 1024);
   w->stat = c.take<float>(wg_colstats_ws_bytes(512) / sizeof(float), 1024);
   w->scale = c.take<float>(512, 1024); w->inv = c.take<float>(512, 1024); w->colsum = c.take<float>(512, 1024);
-  w->jobs = c.take<WgJob>(2048, 1024);
 }
 __global__ void wgconv_reduce_kernel(const float* __restrict__ part, int nsplit, int coutP, int ldp, int cinP, int cout, int cin,
                                      float* __restrict__ dW) {
@@ -360,37 +362,22 @@ int conv_wgrad_tc(const ConvLayer& L, int B, int T, const float* gz_p, const flo
   const size_t b_img = (size_t)nch * ntB * kWgTileB;
   for (int k = 0; k < kConvK; ++k)
     T2_TRY(wg_transpose_images(xp, L.cin, k - kPadRows, Mp, 64, nch, L.cin, 256, nullptr, w.img_b + (size_t)k * b_img, s));
-  std::vector<WgJob> jobs;
-  for (int k = 0; k < kConvK; ++k)
-    for (int ia = 0; ia < ntA; ++ia)
-      for (int jb = 0; jb < ntB; ++jb)
-        for (int sp = 0; sp < nsplit; ++sp) {
-          WgJob j;
-          const int c0 = sp * seg, n = (nch - c0) < seg ? (nch - c0) : seg;
-          j.a_stride = (uint32_t)ntA * kWgTileA; j.b_stride = (uint32_t)ntB * kWgTileB;
-          j.a = w.img_a + (size_t)c0 * j.a_stride + (size_t)ia * kWgTileA;
-          j.b = w.img_b + (size_t)k * b_img + (size_t)c0 * j.b_stride + (size_t)jb * kWgTileB;
-          j.nchunks = n;
-          j.out = w.part + ((size_t)sp * coutP + (size_t)ia * 128) * ldp + (size_t)k * cinP + (size_t)jb * 256;
-          j.ldo = ldp;
-          j.inv_scale = w.inv + ia * 128;
-          jobs.push_back(j);
-        }
-  if (jobs.size() > 2048) return fail(T2_ERR_UNSUPPORTED, "conv wgrad: too many jobs");
-  T2_TRY(wg_run_jobs(jobs, w.jobs, s));
+  const WgConvJobs jobs = {w.img_a, w.img_b, b_img, w.part, w.inv, nch, seg, nsplit, ntA, ntB, coutP, cinP, ldp};
+  T2_TRY(wg_run_jobs(jobs, s));
   const long n = (long)L.cout * L.cin * kConvK;
   wgconv_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.part, nsplit, coutP, ldp, cinP, L.cout, L.cin, dW);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }
 
+// gemm / gemm_bytes: the scratch of the forward GEMMs (stack_ws_layout)
 int conv_fwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_t seed, const float* xp, float* zp,
-             float* stats, float* yp, float* y_plain, bool update_running, float* partial, cudaStream_t s) {
-  const long Mp = (long)B * (T + 2 * kPadRows);
-  const int Me = (int)(Mp - 2 * kPadRows);
+             float* stats, float* yp, float* y_plain, bool update_running, float* partial, void* gemm, size_t gemm_bytes,
+             cudaStream_t s) {
+  const int Me = conv_fwd_rows(B, T);
   for (int k = 0; k < kConvK; ++k)
-    T2_TRY(gemm_tc_rm(m, s, false, true, Me, L.cout, L.cin, xp + (long)k * L.cin, L.cin, L.wpk + (long)k * L.cin, (long)kConvK * L.cin,
-                      zp + (long)kPadRows * L.cout, L.cout, k ? 1.f : 0.f));
+    T2_TRY(gemm_tc_rm(m->sm_count, s, gemm, gemm_bytes, false, true, Me, L.cout, L.cin, xp + (long)k * L.cin, L.cin,
+                      L.wpk + (long)k * L.cin, (long)kConvK * L.cin, zp + (long)kPadRows * L.cout, L.cout, k ? 1.f : 0.f));
   {
     float* rm = const_cast<float*>(m->w[L.wbase + 4]); float* rv = const_cast<float*>(m->w[L.wbase + 5]);
     const long M = (long)B * T;
@@ -414,12 +401,27 @@ int conv_fwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
   return T2_OK;
 }
 
+// The scratch of conv_bwd, shared by the layers of a stack in stream order.  Every layer of either stack has at most 512
+// input and 512 output channels.
+struct ConvBwdWs {
+  WgConvWs wg;
+  __half* planes;          // input planes of the input-gradient conv
+  float* wflip;            // (512, 512, 5) the flipped / transposed weights of the input-gradient conv
+  uint8_t* wimg;           // their packed image
+};
+void conv_bwd_layout(Carve& c, int B, int T, ConvBwdWs* w) {
+  wgconv_layout(c, B, T, &w->wg);
+  w->planes = c.take<__half>(tc_planes_bytes(B, T, 512) / sizeof(__half));
+  w->wflip = c.take<float>((size_t)512 * 512 * kConvK);
+  w->wimg = c.take<uint8_t>(tc_weights_bytes(512, 512, kConvK, 128), 1024);
+}
+
 // g: gradient wrt the layer output (padded or plain rows).  Writes gx_p (padded rows, garbage in the pad rows) when
-// non-null, and the gradients of conv.weight / conv.bias / bn.weight / bn.bias.  planes: scratch of
-// tc_planes_bytes(B, T, 512) for the input-gradient conv.
+// non-null, and the gradients of conv.weight / conv.bias / bn.weight / bn.bias.
 int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_t seed, const float* g, int g_padded,
              const float* xp, const float* zp, const float* stats, const float* yp, float* gz_p, float* gx_p, float* sums,
-             float* const* G, const WgConvWs& wg, __half* planes, cudaStream_t s) {
+             float* const* G, const ConvBwdWs& cw, cudaStream_t s) {
+  const WgConvWs& wg = cw.wg;
   const long Mp = (long)B * (T + 2 * kPadRows);
   float* partial = sums + 2 * L.cout;      // (kRedSplit, 2, cout) scratch behind the two result rows
   bn_bwd_reduce_kernel<<<dim3((L.cout + 31) / 32, kRedSplit), 256, 0, s>>>(g, g_padded, yp, zp, stats, B, T, L.cout, L.act, L.dropout,
@@ -440,12 +442,11 @@ int conv_bwd(T2Model* m, const ConvLayer& L, int B, int T, int training, uint64_
     // G_z is pre-scaled by a power of two (from the per-channel statistics of the weight-gradient pass): fp16 range
     global_scale_kernel<<<1, 256, 0, s>>>(wg.stat, L.cout, wg.colsum, wg.stat);       // colsum[0] = s_g, stat[0..512) = 1 / s_g
     T2_LAUNCH_CHECK();
-    if (!m->dgrad_tmp) T2_CUDA(cudaMalloc((void**)&m->dgrad_tmp, (size_t)kPost * kPost * kConvK * 4));
     const long nw = (long)L.cout * L.cin * kConvK;
-    flip_conv_w_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(m->w[L.wbase], m->dgrad_tmp, L.cout, L.cin);
+    flip_conv_w_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(m->w[L.wbase], cw.wflip, L.cout, L.cin);
     T2_LAUNCH_CHECK();
-    T2_TRY(tc_pack_weights(m->dgrad_tmp, L.cin, L.cout, kConvK, L.cin >= 128 ? 128 : 80, L.wimg_dgrad, s));
-    T2_TRY(tc_train_conv(m, gz_p, L.cout, *L.wimg_dgrad, L.cin, B, T, gx_p, planes, wg.colsum, wg.stat, s));
+    T2_TRY(tc_pack_weights(cw.wflip, L.cin, L.cout, kConvK, L.cin >= 128 ? 128 : 80, cw.wimg, s));
+    T2_TRY(tc_train_conv(m, gz_p, L.cout, cw.wimg, L.cin, B, T, gx_p, cw.planes, wg.colsum, wg.stat, s));
   }
   return T2_OK;
 }
@@ -464,11 +465,15 @@ void stack_layout(Carve& c, int B, int T, int L, const int* ch, StackStash* st) 
 // The same stack without a stash (a training-mode forward outside autograd), laid out on the caller's workspace.  Nothing
 // is kept for a backward pass: two padded buffers take turns as the layers' inputs and outputs, and one z / statistics
 // region serves every layer.  keep_input: the input gets a buffer of its own (the postnet adds it back as the residual).
-// The activation buffers come first, z and the statistics last.
-void stack_ws_layout(Carve& c, int B, int T, int L, const int* ch, bool keep_input, StackStash* st) {
+// The activation buffers come first, then z and the statistics, and last the scratch of the forward GEMMs, which a
+// forward with a stash uses too.
+void stack_ws_layout(Carve& c, int B, int T, int L, const int* ch, bool keep_input, StackStash* st, void** gemm,
+                     size_t* gemm_bytes) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
   int cmax = 0;
+  *gemm_bytes = 0;
   for (int l = 0; l <= L; ++l) cmax = ch[l] > cmax ? ch[l] : cmax;
+  for (int l = 0; l < L; ++l) *gemm_bytes = std::max(*gemm_bytes, gemm_tc_ws_bytes(conv_fwd_rows(B, T), ch[l + 1], ch[l]));
   memset(st, 0, sizeof(*st));
   float* in = keep_input ? c.take<float>(Mp * ch[0]) : nullptr;
   float* buf[2] = {c.take<float>(Mp * cmax), c.take<float>(Mp * cmax)};
@@ -476,6 +481,7 @@ void stack_ws_layout(Carve& c, int B, int T, int L, const int* ch, bool keep_inp
   float* z = c.take<float>(Mp * cmax);
   float* stats = c.take<float>((size_t)(2 + kRedSplit) * cmax);
   for (int l = 0; l < L; ++l) { st->z[l] = z; st->stats[l] = stats; }
+  *gemm = c.take<char>(*gemm_bytes);
 }
 const int kPostCh[6] = {kMel, kPost, kPost, kPost, kPost, kMel};
 const int kEncCh[4] = {kEnc, kEnc, kEnc, kEnc};
@@ -603,7 +609,8 @@ size_t postnet_stash_bytes(int B, int T) { Carve c(nullptr); StackStash st; stac
 size_t postnet_forward_train_ws_bytes(int B, int T) {
   Carve c(nullptr);
   StackStash st;
-  stack_ws_layout(c, B, T, 5, kPostCh, true, &st);
+  void* gemm; size_t gemm_bytes;
+  stack_ws_layout(c, B, T, 5, kPostCh, true, &st, &gemm, &gemm_bytes);
   return c.bytes();
 }
 
@@ -612,7 +619,6 @@ static void post_layers(T2Model* m, int training, const uint8_t* keep, int B, in
     L[i].cin = kPostCh[i]; L[i].cout = kPostCh[i + 1]; L[i].act = i == 4 ? ACT_NONE : ACT_TANH; L[i].dropout = training;
     L[i].wpk = m->post_conv_w[i]; L[i].wbase = W_POST_CONV0 + 7 * i; L[i].site = 2000 + i;
     L[i].keep = (training && keep) ? keep + (size_t)i * B * kPost * T : nullptr;     // [(B,512,T)] x 4 + (B,80,T)
-    L[i].wimg_dgrad = &m->tc_dgrad_post[i];
   }
 }
 
@@ -621,13 +627,14 @@ int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, void* ws, cudaStre
   if (a->stash && a->lengths) return fail(T2_ERR_UNSUPPORTED, "postnet: the training stash path takes no length mask (model.py:510)");
   if (a->stash && a->stash_bytes < postnet_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "postnet stash too small");
   StackStash st;
+  void* gemm; size_t gemm_bytes;
+  Carve wc(ws);
+  stack_ws_layout(wc, B, T, 5, kPostCh, true, &st, &gemm, &gemm_bytes);
   if (a->stash) {
     Carve c(a->stash);
     stack_layout(c, B, T, 5, kPostCh, &st);
     T2_CUDA(cudaMemsetAsync(st.x[0], 0, c.off, s));      // zero pad rows everywhere
   } else {
-    Carve c(ws);
-    stack_ws_layout(c, B, T, 5, kPostCh, true, &st);
     T2_CUDA(cudaMemsetAsync(st.x[0], 0, (char*)st.z[0] - (char*)st.x[0], s));   // the activations, pad rows included
   }
   const long n = (long)B * T * kMel;
@@ -638,7 +645,7 @@ int postnet_forward_train(T2Model* m, const T2PostnetArgs* a, void* ws, cudaStre
   post_layers(m, a->training, a->keep, B, T, L);
   for (int i = 0; i < 5; ++i)
     T2_TRY(conv_fwd(m, L[i], B, T, a->training, a->seed, st.x[i], st.z[i], st.stats[i], st.x[i + 1], nullptr, a->training != 0,
-                    st.stats[i] + 2 * L[i].cout, s));
+                    st.stats[i] + 2 * L[i].cout, gemm, gemm_bytes, s));
   rows_to_bct_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st.x[5], a->add_residual ? st.x[0] : nullptr, a->lengths, a->mel_post,
                                                                   B, T, kMel);
   T2_LAUNCH_CHECK();
@@ -649,16 +656,14 @@ struct PostBwdWs {
   float *gz, *gxa, *gxb;   // padded rows (B (T+4), 512)
   float* grow;             // (B T, 80) output gradient rows
   float* sums;
-  WgConvWs wg;
-  __half* planes;
+  ConvBwdWs cw;
 };
 static void postnet_backward_ws_layout(Carve& c, int B, int T, PostBwdWs* w) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
   w->gz = c.take<float>(Mp * kPost); w->gxa = c.take<float>(Mp * kPost); w->gxb = c.take<float>(Mp * kPost);
   w->grow = c.take<float>((size_t)B * T * kMel);
   w->sums = c.take<float>((size_t)(2 + 2 * kRedSplit) * kPost);
-  wgconv_layout(c, B, T, &w->wg);
-  w->planes = c.take<__half>(tc_planes_bytes(B, T, kPost) / sizeof(__half));
+  conv_bwd_layout(c, B, T, &w->cw);
 }
 size_t postnet_backward_ws_bytes(int B, int T) {
   Carve c(nullptr, 1024);
@@ -691,7 +696,7 @@ int postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, cudaStream_t s) {
       T2_LAUNCH_CHECK();
     }
     T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.x[i], st.z[i], st.stats[i], st.x[i + 1], w.gz, gx, w.sums,
-                    a->grads, w.wg, w.planes, s));
+                    a->grads, w.cw, s));
     g = gx; g_padded = 1;
     gx = gx == w.gxa ? w.gxb : w.gxa;
   }
@@ -712,23 +717,27 @@ static void enc_layers(T2Model* m, int training, const uint8_t* keep, int B, int
     L[i].cin = kEnc; L[i].cout = kEnc; L[i].act = ACT_RELU; L[i].dropout = training;
     L[i].wpk = m->enc_conv_w[i]; L[i].wbase = W_ENC_CONV0 + 7 * i; L[i].site = 1000 + i;
     L[i].keep = (training && keep) ? keep + (size_t)i * B * kEnc * T : nullptr;
-    L[i].wimg_dgrad = &m->tc_dgrad_enc[i];
   }
 }
 
 size_t encoder_convs_train_ws_bytes(int B, int T) {
   Carve c(nullptr);
   StackStash st;
-  stack_ws_layout(c, B, T, 3, kEncCh, false, &st);
+  void* gemm; size_t gemm_bytes;
+  stack_ws_layout(c, B, T, 3, kEncCh, false, &st, &gemm, &gemm_bytes);
   return c.bytes();
 }
 
 // conv stack of the training forward: returns the LSTM input rows (B*T, 512).  With a stash it fills the stash and
-// returns where the BiLSTM keeps its gates / cell states; without one it runs on ws and *gates = *cst = null.
+// returns where the BiLSTM keeps its gates / cell states; without one it runs on ws and *gates = *cst = null.  Either way
+// the GEMMs take their scratch from ws.
 int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, void* ws, cudaStream_t s, const float** xl, float** gates, float** cst) {
   const int B = a->B, T = a->T;
   if (a->stash && a->stash_bytes < encoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder stash too small");
   StackStash cs;
+  void* gemm; size_t gemm_bytes;
+  Carve wc(ws);
+  stack_ws_layout(wc, B, T, 3, kEncCh, false, &cs, &gemm, &gemm_bytes);
   float* rows;     // the last layer's output as plain rows
   if (a->stash) {
     const EncStash st = enc_stash(a->stash, B, T);
@@ -736,8 +745,6 @@ int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, void* ws, cudaStream
     T2_CUDA(cudaMemsetAsync(cs.x[0], 0, (char*)st.xl - (char*)cs.x[0], s));   // the conv stack, pad rows included
     rows = st.xl; *gates = st.gates; *cst = st.cst;
   } else {
-    Carve c(ws);
-    stack_ws_layout(c, B, T, 3, kEncCh, false, &cs);
     T2_CUDA(cudaMemsetAsync(cs.x[0], 0, (char*)cs.z[0] - (char*)cs.x[0], s));   // the activations, pad rows included
     rows = cs.x[3]; *gates = nullptr; *cst = nullptr;   // nothing reads x[3] as padded rows: it holds the plain ones
   }
@@ -751,7 +758,7 @@ int encoder_convs_train(T2Model* m, const T2EncoderArgs* a, void* ws, cudaStream
   for (int i = 0; i < 3; ++i) {
     float* yp = (i == 2 && !a->stash) ? nullptr : cs.x[i + 1];
     T2_TRY(conv_fwd(m, L[i], B, T, a->training, a->seed, cs.x[i], cs.z[i], cs.stats[i], yp, i == 2 ? rows : nullptr,
-                    a->training != 0, cs.stats[i] + 2 * L[i].cout, s));
+                    a->training != 0, cs.stats[i] + 2 * L[i].cout, gemm, gemm_bytes, s));
   }
   *xl = rows;
   return T2_OK;
@@ -771,8 +778,8 @@ struct EncBwdWs {
   float* g_c;              // (2, 64, 256)
   float *gz, *gxa, *gxb;   // padded rows (B (T+4), 512)
   float *sums, *tmp;
-  WgConvWs wg;
-  __half* planes;
+  void* gemm; size_t gemm_bytes;   // scratch of the BiLSTM's weight / input gradient GEMMs and bias column sums
+  ConvBwdWs cw;
 };
 static void encoder_backward_ws_layout(Carve& c, int B, int T, EncBwdWs* w) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
@@ -783,8 +790,11 @@ static void encoder_backward_ws_layout(Carve& c, int B, int T, EncBwdWs* w) {
   w->gz = c.take<float>(Mp * kEnc); w->gxa = c.take<float>(Mp * kEnc); w->gxb = c.take<float>(Mp * kEnc);
   w->sums = c.take<float>((size_t)(2 + 2 * kRedSplit) * kEnc);
   w->tmp = c.take<float>(8 * kEncH);
-  wgconv_layout(c, B, T, &w->wg);
-  w->planes = c.take<__half>(tc_planes_bytes(B, T, kEnc) / sizeof(__half));
+  const int BT = B * T;
+  w->gemm_bytes = std::max({gemm_tc_ws_bytes(4 * kEncH, kEnc, BT), gemm_tc_ws_bytes(4 * kEncH, kEncH, BT),
+                            gemm_tc_ws_bytes(BT, kEnc, 4 * kEncH), colsum_ws_bytes(BT, 4 * kEncH)});
+  w->gemm = c.take<char>(w->gemm_bytes);
+  conv_bwd_layout(c, B, T, &w->cw);
 }
 size_t encoder_backward_ws_bytes(int B, int T) {
   Carve c(nullptr, 1024);
@@ -822,15 +832,20 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   for (int dir = 0; dir < 2; ++dir) {
     const int wb = W_ENC_LSTM + 4 * dir;
     const float* dGd = w.dG + (size_t)dir * 4 * kEncH;          // rows (b, t), row stride 2048
-    if (G[wb]) T2_TRY(gemm_tc_rm(m, s, true, false, 4 * kEncH, kEnc, BT, dGd, 8 * kEncH, st.xl, kEnc, G[wb], kEnc, 0.f));
-    if (G[wb + 1]) T2_TRY(gemm_tc_rm(m, s, true, false, 4 * kEncH, kEncH, BT, dGd, 8 * kEncH, w.hp + (size_t)dir * kEncH, kEnc, G[wb + 1], kEncH, 0.f));
+    if (G[wb])
+      T2_TRY(gemm_tc_rm(m->sm_count, s, w.gemm, w.gemm_bytes, true, false, 4 * kEncH, kEnc, BT, dGd, 8 * kEncH, st.xl, kEnc, G[wb],
+                        kEnc, 0.f));
+    if (G[wb + 1])
+      T2_TRY(gemm_tc_rm(m->sm_count, s, w.gemm, w.gemm_bytes, true, false, 4 * kEncH, kEncH, BT, dGd, 8 * kEncH,
+                        w.hp + (size_t)dir * kEncH, kEnc, G[wb + 1], kEncH, 0.f));
     if (G[wb + 2] || G[wb + 3]) {
-      T2_TRY(colsum_f32(m, s, dGd, 8 * kEncH, BT, 4 * kEncH, w.tmp));
+      T2_TRY(colsum_f32(s, w.gemm, w.gemm_bytes, dGd, 8 * kEncH, BT, 4 * kEncH, w.tmp));
       if (G[wb + 2]) T2_CUDA(cudaMemcpyAsync(G[wb + 2], w.tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
       if (G[wb + 3]) T2_CUDA(cudaMemcpyAsync(G[wb + 3], w.tmp, 4 * kEncH * 4, cudaMemcpyDeviceToDevice, s));
     }
     // gradient wrt the LSTM input: dG_dir (BT x 1024) . W_ih_dir (1024 x 512)
-    T2_TRY(gemm_tc_rm(m, s, false, false, BT, kEnc, 4 * kEncH, dGd, 8 * kEncH, m->w[wb], kEnc, w.dxl, kEnc, dir ? 1.f : 0.f));
+    T2_TRY(gemm_tc_rm(m->sm_count, s, w.gemm, w.gemm_bytes, false, false, BT, kEnc, 4 * kEncH, dGd, 8 * kEncH, m->w[wb], kEnc, w.dxl,
+                      kEnc, dir ? 1.f : 0.f));
   }
   // ---- conv stack ----
   ConvLayer L[3];
@@ -840,7 +855,7 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   for (int i = 2; i >= 0; --i) {
     const bool need_gx = i > 0 || a->d_embedded || (a->text && G[W_EMB]);
     T2_TRY(conv_bwd(m, L[i], B, T, a->training, a->seed, g, g_padded, st.cs.x[i], st.cs.z[i], st.cs.stats[i], st.cs.x[i + 1], w.gz,
-                    need_gx ? gx : nullptr, w.sums, G, w.wg, w.planes, s));
+                    need_gx ? gx : nullptr, w.sums, G, w.cw, s));
     g = gx; g_padded = 1;
     gx = gx == w.gxa ? w.gxb : w.gxa;
   }

@@ -377,7 +377,7 @@ static int pack(T2WaveGlow* m, const void* const* w, cudaStream_t s) {
   const int half = m->fp16;
   build_up_kernel<<<80 * 256, 256, 0, s>>>(w[kWUpW], w[kWUpB], half, m->tmp, m->up_bias);
   T2_LAUNCH_CHECK();
-  T2_TRY(tc_pack_weights(m->tmp, 80 * 256, kUpK, 1, kNT, &m->up_img, s));
+  T2_TRY(tc_pack_weights(m->tmp, 80 * 256, kUpK, 1, kNT, m->up_img, s));
   for (int k = 0; k < kFlows; ++k) {
     const int base = wn_base(k);
     const int nr = k >= 8 ? 4 : (k >= 4 ? 6 : 8);
@@ -387,12 +387,12 @@ static int pack(T2WaveGlow* m, const void* const* w, cudaStream_t s) {
       build_gate_kernel<<<512, 256, 0, s>>>(w[in], w[in + 1], w[in + 2], w[base + 53], w[base + 54], w[base + 55], l, half,
                                              m->tmp, gb);
       T2_LAUNCH_CHECK();
-      T2_TRY(tc_pack_weights(m->tmp, 512, 3 * kC + kCond, 1, kNT, &m->gate_img[k][l], s));
+      T2_TRY(tc_pack_weights(m->tmp, 512, 3 * kC + kCond, 1, kNT, m->gate_img[k][l], s));
       const int nrs = l < kLayers - 1 ? 512 : 256;
       float* rb = m->rs_bias + ((size_t)k * kLayers + l) * 512;
       build_rs_kernel<<<nrs, 256, 0, s>>>(w[rs], w[rs + 1], w[rs + 2], half, m->tmp, rb);
       T2_LAUNCH_CHECK();
-      T2_TRY(tc_pack_weights(m->tmp, nrs, kC, 1, kNT, &m->rs_img[k][l], s));
+      T2_TRY(tc_pack_weights(m->tmp, nrs, kC, 1, kNT, m->rs_img[k][l], s));
     }
     build_flow_kernel<<<1, 256, 0, s>>>(w[base + 48], w[base + 49], w[base + 50], w[base + 51], w[base + 52],
                                         reinterpret_cast<const float*>(w[kWConvinv + k]), nr, half, m->flows + k);
@@ -422,8 +422,14 @@ int waveglow_create(T2WaveGlow** out, const T2WaveGlowConfig* c, const void* con
       cudaMalloc((void**)&m->gate_bias, (size_t)kFlows * kLayers * 512 * sizeof(float)) != cudaSuccess ||
       cudaMalloc((void**)&m->rs_bias, (size_t)kFlows * kLayers * 512 * sizeof(float)) != cudaSuccess ||
       cudaMalloc((void**)&m->flows, kFlows * sizeof(t2_flow_w)) != cudaSuccess ||
-      cudaMalloc((void**)&m->tmp, (size_t)80 * 256 * kUpK * sizeof(float)) != cudaSuccess)
+      cudaMalloc((void**)&m->tmp, (size_t)80 * 256 * kUpK * sizeof(float)) != cudaSuccess ||
+      cudaMalloc((void**)&m->up_img, tc_weights_bytes(80 * 256, kUpK, 1, kNT)) != cudaSuccess)
     r = fail(T2_ERR_CUDA, "waveglow: out of device memory for the packed weights");
+  for (int k = 0; k < kFlows; ++k)
+    for (int l = 0; l < kLayers && r == T2_OK; ++l)
+      if (cudaMalloc((void**)&m->gate_img[k][l], tc_weights_bytes(512, 3 * kC + kCond, 1, kNT)) != cudaSuccess ||
+          cudaMalloc((void**)&m->rs_img[k][l], tc_weights_bytes(l < kLayers - 1 ? 512 : 256, kC, 1, kNT)) != cudaSuccess)
+        r = fail(T2_ERR_CUDA, "waveglow: out of device memory for the packed weights");
   if (r == T2_OK) r = pack(m, w, s);
   if (r != T2_OK) { waveglow_destroy(m); return r; }
   *out = m;

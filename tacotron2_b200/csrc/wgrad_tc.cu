@@ -11,8 +11,6 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <vector>
-
 #include "decoder.h"
 #include "umma.cuh"
 #include "wgrad_tc.h"
@@ -105,10 +103,12 @@ __device__ __forceinline__ void wg_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const WgJob* __restrict__ jobs) {
+// Jobs: the CTA table as a function of blockIdx.x (WgDecJobs, WgConvJobs)
+template <class Jobs>
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const Jobs jobs) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const WgJob job = jobs[blockIdx.x];
+  const WgJob job = jobs((int)blockIdx.x);
   uint8_t* stage0 = smem_raw;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + kWgStages * kStageB);
   uint64_t* full = bars; uint64_t* empty = bars + kWgStages;
@@ -187,9 +187,52 @@ __global__ void wg_reduce_kernel(const float* __restrict__ part, int nsplit, int
   else if (g_hh) g_hh[r * 1024 + (c - c_ih)] = s;
 }
 
-}  // namespace
+template <class Jobs>
+int wg_launch(const Jobs& jobs, int n, cudaStream_t s) {
+  const size_t smem = (size_t)kWgStages * kStageB + 256;
+  T2_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<Jobs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  wgrad_tc_kernel<Jobs><<<n, kWgThreads, smem, s>>>(jobs);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
+}
 
-constexpr int kWgMaxJobs = 8192;
+// The CTAs of the decoder LSTM weight gradients, in launch order: LSTM l, K split sp, gate tile i, feature tile (of the
+// LSTM's concatenated input, group by group).  This order is L2 locality: all tiles of one K split (one 100-step window
+// of the images) run together, gate tile outer, feature tile inner, so concurrently resident CTAs share their A and B
+// tiles (ncu: 25.8 GB of DRAM reads for 2.2 GB of operands in the gate-tile-inner order).
+struct WgDecJobs {
+  struct Grp { const uint8_t* img; int ntile; int t0; };   // feature group: image, 256-row tiles per chunk, first chunk
+  Grp grp[2][3];
+  const uint8_t* img_a[2];
+  float* part[2];
+  const float* inv[2];
+  int T, seg, nsplit;
+  __device__ WgJob operator()(int idx) const {
+    const int n0 = nsplit * (4096 / kTM) * (1792 / kTN);      // CTAs of the attention LSTM
+    const int l = idx >= n0 ? 1 : 0;
+    if (l) idx -= n0;
+    const int ldc = l ? 2560 : 1792, ntf = ldc / kTN;
+    int jt = idx % ntf;
+    const int col = jt * kTN;
+    idx /= ntf;
+    const int i = idx % (4096 / kTM), sp = idx / (4096 / kTM);
+    int g = 0;
+    while (jt >= grp[l][g].ntile) jt -= grp[l][g++].ntile;
+    const Grp gr = grp[l][g];
+    const int c0 = sp * seg;
+    WgJob j;
+    j.a_stride = (uint32_t)(4096 / kTM) * kABytes; j.b_stride = (uint32_t)gr.ntile * kBBytes;
+    j.a = img_a[l] + (size_t)c0 * j.a_stride + (size_t)i * kABytes;
+    j.b = gr.img + (size_t)(c0 + gr.t0) * j.b_stride + (size_t)jt * kBBytes;
+    j.nchunks = min(T - c0, seg);
+    j.out = part[l] + ((size_t)sp * 4096 + (size_t)i * kTM) * ldc + col;
+    j.ldo = ldc;
+    j.inv_scale = inv[l] + i * kTM;
+    return j;
+  }
+};
+
+}  // namespace
 
 void wgrad_tc_layout(Carve& c, int T, WgradWs* w) {
   const int seg = wgrad_seg(T), nsplit = (T + seg - 1) / seg;
@@ -203,7 +246,6 @@ void wgrad_tc_layout(Carve& c, int T, WgradWs* w) {
   w->scale = c.take<float>(4096, 1024);
   for (int l = 0; l < 2; ++l) w->inv[l] = c.take<float>(4096, 1024);
   w->colsum = c.take<float>(4096, 1024);
-  w->jobs = c.take<WgJob>(kWgMaxJobs, 1024);
 }
 
 // dga / dgd: (T, B, 4096) fp32; x2 (T, B, 256); stash slots ctx (T+1, B, 512), ha / hd (T+1, B, 1024).
@@ -232,38 +274,13 @@ int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, c
   T2_LAUNCH_CHECK();
   wg_transpose_img_kernel<<<dim3(1024 / 64, T + 1), 256, 0, s>>>(st.hd, 1024, 0, rows + B, B, 1024, kTN, nullptr, w.img_hd);
   T2_LAUNCH_CHECK();
-  // job table: LSTM l, feature tile j (of its concatenated input), gate tile i, K split sp
-  struct Grp { const uint8_t* img; int ntile; int t0; };   // feature group: image, 256-row tiles per chunk, first chunk
-  const Grp att[3] = {{w.img_x2, 1, 0}, {w.img_ctx, 2, 0}, {w.img_ha, 4, 0}};      // [x2_t | ctx_(t-1) | ah_(t-1)]   model.py:352
-  const Grp dec[3] = {{w.img_ha, 4, 1}, {w.img_ctx, 2, 1}, {w.img_hd, 4, 0}};      // [ah_t | ctx_t | dh_(t-1)]       model.py:366-367
-  const int ldc[2] = {1792, 2560};
+  WgDecJobs jobs;
+  jobs.grp[0][0] = {w.img_x2, 1, 0}; jobs.grp[0][1] = {w.img_ctx, 2, 0}; jobs.grp[0][2] = {w.img_ha, 4, 0};   // [x2_t | ctx_(t-1) | ah_(t-1)]   model.py:352
+  jobs.grp[1][0] = {w.img_ha, 4, 1}; jobs.grp[1][1] = {w.img_ctx, 2, 1}; jobs.grp[1][2] = {w.img_hd, 4, 0};   // [ah_t | ctx_t | dh_(t-1)]       model.py:366-367
   float* part_l[2] = {w.part, w.part + (size_t)nsplit * 4096 * 1792};
-  // CTA order = L2 locality: all tiles of one K split (one 100-step window of the images) run together, gate tile outer,
-  // feature tile inner, so concurrently resident CTAs share their A and B tiles (ncu: 25.8 GB of DRAM reads for 2.2 GB of
-  // operands in the gate-tile-inner order)
-  std::vector<WgJob> jobs;
-  for (int l = 0; l < 2; ++l) {
-    const Grp* gr = l == 0 ? att : dec;
-    for (int sp = 0; sp < nsplit; ++sp)
-      for (int i = 0; i < 4096 / kTM; ++i) {
-        int col = 0;
-        for (int g = 0; g < 3; ++g)
-          for (int jt = 0; jt < gr[g].ntile; ++jt, col += kTN) {
-            WgJob j;
-            const int c0 = sp * seg, n = (T - c0) < seg ? (T - c0) : seg;
-            j.a_stride = (uint32_t)(4096 / kTM) * kABytes; j.b_stride = (uint32_t)gr[g].ntile * kBBytes;
-            j.a = w.img_a[l] + (size_t)c0 * j.a_stride + (size_t)i * kABytes;
-            j.b = gr[g].img + (size_t)(c0 + gr[g].t0) * j.b_stride + (size_t)jt * kBBytes;
-            j.nchunks = n;
-            j.out = part_l[l] + ((size_t)sp * 4096 + (size_t)i * kTM) * ldc[l] + col;
-            j.ldo = ldc[l];
-            j.inv_scale = w.inv[l] + i * kTM;
-            jobs.push_back(j);
-          }
-      }
-  }
-  if (jobs.size() > kWgMaxJobs) return fail(T2_ERR_UNSUPPORTED, "wgrad: too many jobs (T too long)");
-  T2_TRY(wg_run_jobs(jobs, w.jobs, s));
+  for (int l = 0; l < 2; ++l) { jobs.img_a[l] = w.img_a[l]; jobs.part[l] = part_l[l]; jobs.inv[l] = w.inv[l]; }
+  jobs.T = T; jobs.seg = seg; jobs.nsplit = nsplit;
+  T2_TRY(wg_launch(jobs, nsplit * (4096 / kTM) * ((1792 + 2560) / kTN), s));
   {
     const long n = (long)4096 * 1792;
     wg_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(part_l[0], nsplit, 1792, 768, G[W_ARNN_WIH], G[W_ARNN_WHH]);
@@ -279,20 +296,7 @@ int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, c
 
 
 // ---- generic entry points (also used by the conv-stack weight gradients in train_layers.cu) ------------------------
-int wg_run_jobs(const std::vector<WgJob>& jobs, WgJob* jobs_dev, cudaStream_t s) {
-  if (jobs.empty()) return T2_OK;
-  T2_CUDA(cudaMemcpyAsync(jobs_dev, jobs.data(), jobs.size() * sizeof(WgJob), cudaMemcpyHostToDevice, s));
-  T2_CUDA(cudaStreamSynchronize(s));            // the host vector must outlive the copy
-  const size_t smem = (size_t)kWgStages * kStageB + 256;
-  static bool attr = false;
-  if (!attr) {
-    T2_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = true;
-  }
-  wgrad_tc_kernel<<<(unsigned)jobs.size(), kWgThreads, smem, s>>>(jobs_dev);
-  T2_LAUNCH_CHECK();
-  return T2_OK;
-}
+int wg_run_jobs(const WgConvJobs& jobs, cudaStream_t s) { return wg_launch(jobs, jobs.count(), s); }
 size_t wg_colstats_ws_bytes(int C) { return (size_t)kStatSplit * 2 * C * sizeof(float); }
 int wg_colstats(const float* x, long rows, int C, float* stat_ws, float* scale, float* inv_scale, float* colsum, cudaStream_t s) {
   wg_colstats_kernel<<<dim3((C + 31) / 32, kStatSplit), 256, 0, s>>>(x, rows, C, stat_ws);
