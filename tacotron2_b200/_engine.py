@@ -320,7 +320,8 @@ class Engine(_Handle):
         _capi.check(_capi.lib().t2_decoder_profile(C.byref(a), out))
         names = ["E0 x2->att gemm", "E0 epilogue(ah)", "B1", "E1 ah->dec/att/q gemm", "B2", "attention", "B3",
                  "E2 ctx gemm", "E2 epilogue(dh)", "B4", "E3 dh gemm", "E3 epilogue(mel/x1)", "B5", "E4 x1 gemm+epi", "B6",
-                 "att:im2col", "att:mma", "att:energies", "att:softmax", "att:context"]
+                 "att:before B2 (pa copy or round 0)", "att:pa rounds 1+ or tile wait", "att:energies", "att:softmax",
+                 "att:context", "att:next step's pa (in B6)"]
         return {names[i]: [int(out[s * 24 + i]) for s in range(3)] for i in range(len(names))}
 
     def grad_table(self, named_grads):

@@ -130,7 +130,7 @@ static void decoder_ws_layout(Carve& c, int B, int T, int cap, DecoderWs* w) {
   w->gates = c.take<float>((size_t)B * 4 * kARnn);
   w->proj = c.take<float>((size_t)B * (kMel + 1));
   w->ctrl = c.take<DecoderCtrl>(1);
-  persistent_ws_layout(c, cap, w);
+  persistent_ws_layout(c, T, cap, w);
 }
 
 size_t decoder_ws_bytes(int B, int T, int cap) {

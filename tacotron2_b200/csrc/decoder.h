@@ -33,6 +33,7 @@ struct DecoderWs {
   DecoderCtrl* ctrl;
   uint8_t* images;         // persistent kernel: activation images and q (decoder_persistent.cu)
   uint8_t* teacher_img;    // persistent kernel, teacher forcing: the x2 images of every step
+  float* pa;               // persistent kernel, inference: the location term of the next step (decoder_persistent.cu)
 };
 constexpr size_t kDecoderWsAlign = 1024;   // largest alignment of a decoder workspace region (teacher_img)
 
@@ -53,7 +54,7 @@ inline void decoder_stash_layout(Carve& c, int B, int T, DecoderStash* s) {
 inline size_t decoder_stash_bytes(int B, int T) { Carve c(nullptr); DecoderStash s; decoder_stash_layout(c, B, T, &s); return c.bytes(); }
 
 size_t decoder_ws_bytes(int B, int T, int cap);
-void persistent_ws_layout(Carve& c, int cap, DecoderWs* w);
+void persistent_ws_layout(Carve& c, int T, int cap, DecoderWs* w);
 int decoder_ws_carve(const T2DecoderArgs* a, DecoderWs* w);
 int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
 int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);

@@ -331,7 +331,7 @@ struct PersistentSmem {
   uint8_t* stage0;                 // ring stages
   uint8_t* weff;                   // fused location filter image
   float* acc;                      // event accumulators
-  uint64_t* bars;                  // 16 slots: full[kMaxStages] | empty[kMaxStages]
+  uint64_t* bars;                  // 16 slots: full[kMaxStages] | empty[kMaxStages] | pa tile
   int* live;                       // [0] live rows, [1] stop flag broadcast of wait_counter
   float *bias_a, *bias_d, *v, *q;
   float* red;                      // unused; kept so the regions after it stay where they are
@@ -578,6 +578,8 @@ struct KParams {
   uint8_t* x2_img; uint8_t* ah_img; uint8_t* ctx_img; uint8_t* dh_img; uint8_t* x1_img;
   const uint8_t* teacher_x2_img;   // (cap, 4 chunks) or null
   float* q;                         // (64, 128) fp32
+  float* pa;                        // (64, 128, pa_pitch(T)) fp32 location term of the next step; null: computed in the
+                                    // attention phase (TEACHER, or a tile that does not fit the ring)
   float* mel; float* gate; float* align; int32_t* mel_lengths; int32_t* n_steps;
   DecoderCtrl* ctrl;
   int B, T, cap, infer, training;
@@ -597,13 +599,25 @@ struct KParams {
   int32_t* rs_status;               // out: [steps run, stopped]
 };
 
-// encoder-memory rows of a T_enc-long row that the attention phase stages in an idle ring of `nstages` stages; the rest
-// is read from L2.  The same on the host and the device: the context of a row sums its positions in the grouping a
-// launch sized for that row's own length stages (see the context below).
+// encoder-memory rows of a T_enc-long row that the attention phase stages in an idle ring of `nstages` stages beside the
+// im2col image and one round's pa tile; the rest is read from L2.  The same on the host and the device: the context of a
+// row sums its positions in the grouping a launch sized for that row's own length stages (see the context below), also
+// where the ring holds a whole precomputed pa tile instead and fewer rows are physically staged.
 __host__ __device__ constexpr int staged_rows(int T, int nstages) {
   return T < (nstages * kStageBytes - 2 * kAttPlane - kPaBytes) / (kEnc / 2 * 4)
              ? T : (nstages * kStageBytes - 2 * kAttPlane - kPaBytes) / (kEnc / 2 * 4);
 }
+
+// INFER precomputes the location term pa of step t+1 during the x2 wait of step t (see the kernel) into a global buffer of
+// one fp32 tile [128 dims][pa_pitch(T)] per batch row.  The pitch covers the energies' last chunk of 8 positions, and it is
+// an odd number of 16-byte units (whole units for the bulk copy; odd so that the float4 reads of 8 consecutive dims at one
+// position hit distinct banks).
+__host__ __device__ constexpr int pa_pitch(int T) { return ((T + 7) & ~7) + 4; }
+__host__ __device__ constexpr int pa_tile_bytes(int T) { return kAtt * pa_pitch(T) * 4; }
+// The whole tile is copied into the idle ring before the q barrier, so it must fit there: T_enc <= 280 at 4 stages (<= 208
+// with 3 stages forced; the 3-stage layout otherwise only runs T_enc > 896).  Longer memories compute pa after the q
+// barrier round by round, as TEACHER does.
+__host__ __device__ constexpr bool pa_tile_fits(int T, int nstages) { return pa_tile_bytes(T) <= nstages * kStageBytes; }
 
 __device__ __forceinline__ void store_split2(uint8_t* img, int row, int k, float v0, float v1) {
   // two adjacent K elements (k even) of an activation image: 4-byte stores into the hi and lo planes
@@ -651,8 +665,11 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
   rg.pre = 0;
 
+  uint64_t* bar_pa = sm.bars + 2 * kMaxStages;   // bulk copy of this step's pa tile
+  uint32_t pa_phase = 0;
   if (tid == 0) {
     for (int s = 0; s < p.nstages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
+    ptx::mbar_init(bar_pa, 1);
     ptx::fence_barrier_init();
   }
   const bool resume = p.rs_acc != nullptr;       // a stream's chunk: its state was zeroed by begin or saved by the last chunk
@@ -812,23 +829,34 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     // ======== attention for batch row (cta mod 64) ============================ model.py:43-86, 358-365
     // CTAs b and b+64 both evaluate row b's energies / softmax (no exchange needed, bit-identical); each
     // produces one half of the context columns, the first writes the alignment row.  Everything that only
-    // needs THIS CTA's state (im2col of its attention weights, the pa GEMM, staging encoder memory rows)
-    // runs between the arrival at barrier B2 and the wait for it.
+    // needs THIS CTA's state (the pa tile, staging encoder memory rows) runs between the arrival at barrier B2 and the
+    // wait for it.
+    // The location term pa of step t depends only on the attention weights of step t-1.  With p.pa (INFER, tile fits the
+    // ring) CTA b+64 computes it for row b during the x2 wait of step t-1, when its ring is idle, and both CTAs of the pair
+    // bulk-copy the whole tile before B2; after B2 the energies are one pass over all positions.  Otherwise (TEACHER: no
+    // x2 wait, the ring holds the prefetched E0 weights; or a T_enc whose tile does not fit) pa is computed here, 64
+    // positions per round, round 0 before the B2 wait.
     const bool att_cta = (cta & 63) < p.B;
     const int att_b = cta & 63, ahalf = cta >> 6;
+    const bool pa_pre = p.pa != nullptr;
+    const int pa_p = pa_pitch(T);
+    float* pa_row = pa_pre ? p.pa + (size_t)att_b * kAtt * pa_p : nullptr;
     uint8_t* aimg = rg.stage0;
-    // the idle operand ring during the attention phase: [im2col image: hi plane | lo plane][pa tile][encoder-memory rows
-    // of this CTA]
+    // the idle operand ring during the attention phase: [im2col image: hi plane | lo plane][pa tile of one round]
+    // [encoder-memory rows of this CTA], or with p.pa [pa tile of all positions][encoder-memory rows of this CTA]
     const int att_rounds = (T + kAttRound - 1) / kAttRound;
     const int img_bytes = 2 * kAttPlane;
     float* s_pa = reinterpret_cast<float*>(aimg + img_bytes);                       // [128 dims][kPaPitch] fp32
-    const int smem_rows = staged_rows(T, p.nstages);                        // memory rows staged in the ring
+    const int mem_off = pa_pre ? pa_tile_bytes(T) : img_bytes + kPaBytes;         // ring bytes before the memory rows
+    const int smem_rows = pa_pre ? min(T, (p.nstages * kStageBytes - mem_off) / (kEnc / 2 * 4))
+                                 : staged_rows(T, p.nstages);                       // memory rows staged in the ring
     // pa^T = Weff . A^T on the tensor cores (fused model.py:23-25), i.e. the fused filter bank is the M = 128 operand
     // (attention dim d; warpgroups 0 / 1 take dims 0-63 / 64-127) and kAttRound positions are the N dimension.  The
-    // tile goes to shared memory, where every warp then owns a slice of POSITIONS of all 128 dims, so the tanh of a
-    // row spread evenly over the four SM sub-partitions for any T_enc, the processed-memory reads are coalesced
-    // (lanes = consecutive dims) and can be issued before the q barrier.
-    auto att_im2col_mma_tr = [&](int r0) {
+    // tile of round r0 goes to dst[dim * pitch + position - 64 r0] (positions below `bound`): in shared memory every warp
+    // then owns a slice of POSITIONS of all 128 dims, so the tanh of a row spread evenly over the four SM sub-partitions
+    // for any T_enc, the processed-memory reads are coalesced (lanes = consecutive dims) and can be issued before the q
+    // barrier.
+    auto att_pa_round = [&](int r0, float* dst, int pitch, int bound) {
       const int jbase = r0 * kAttRound, cnt = min(T - jbase, kAttRound);
       for (int item = tid; item < kAttRound * 8; item += kThreads) {
         const int jj = item >> 3, g8 = item & 7, j = jbase + jj;
@@ -869,14 +897,17 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         ptx::wg_wait<0>();
         ptx::wg_fence_regs<kAttRound / 2>(d);
 #pragma unroll
-        for (int i = 0; i < kAttRound / 2; i += 2)
-          *reinterpret_cast<float2*>(s_pa + (wg * 64 + ptx::wg_frag_row(i, wt)) * kPaPitch + ptx::wg_frag_col(i, wt)) =
-              make_float2(d[i], d[i + 1]);
+        for (int i = 0; i < kAttRound / 2; i += 2) {
+          const int col = ptx::wg_frag_col(i, wt);
+          float* o = dst + (wg * 64 + ptx::wg_frag_row(i, wt)) * pitch + col;
+          if (col + 1 < bound) *reinterpret_cast<float2*>(o) = make_float2(d[i], d[i + 1]);
+          else if (col < bound) *o = d[i];
+        }
       }
       __syncthreads();
     };
     auto stage_memory_rows = [&](int j0, int j1) {     // cp.async this CTA's half of memory rows [j0, j1) into the ring
-      const uint32_t sbase = ptx::smem_u32(rg.stage0) + (uint32_t)(img_bytes + kPaBytes);
+      const uint32_t sbase = ptx::smem_u32(rg.stage0) + (uint32_t)mem_off;
       const float* msrc = p.memory + (long)att_b * T * kEnc + ahalf * (kEnc / 2);
       for (int i = j0 * 64 + tid; i < j1 * 64; i += kThreads) {
         const int j = i >> 6, c4 = i & 63;
@@ -894,7 +925,17 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       for (int e = 0; e < 8; ++e) pm_next[e] = (j0 + e < cnt) ? __ldg(pmr + (long)(j0 + e) * kAtt) : 0.f;
     };
     if (att_cta) {
-      att_im2col_mma_tr(0);
+      if (pa_pre) {
+        // CTA b+64 wrote this tile before it signalled its ah columns of this step, or in the launch of the previous
+        // chunk, or the buffer was zeroed before step 0 (the attention weights start at zero, so pa is +0.0); thread 0
+        // acquired every ah counter in E1.
+        if (tid == 0) {
+          ptx::mbar_arrive_expect_tx(bar_pa, (uint32_t)pa_tile_bytes(T));
+          ptx::bulk_g2s_hint(rg.stage0, pa_row, (uint32_t)pa_tile_bytes(T), bar_pa, rg.pol_w);
+        }
+      } else {
+        att_pa_round(0, s_pa, kPaPitch, kAttRound);
+      }
       stage_memory_rows(0, smem_rows);     // everything the context needs is in flight before the q barrier
       load_pm(p.pm + (long)att_b * T * kAtt + adim, cg * 8, min(T, kAttRound));
     }
@@ -908,10 +949,15 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       {
         const int eN = ntiles * 128;
         const float qd = s_q[adim], vd = s_v[adim];
-        const int nrounds = att_rounds;
+        // with the copied tile: one pass over all T positions; else one round of 64 positions per pa GEMM.  Chunks of 8
+        // positions start at multiples of 8 either way, so every energy is the same sum in the same order.
+        const int nrounds = pa_pre ? 1 : att_rounds, rlen = pa_pre ? T : kAttRound;
+        const float* s_tile = pa_pre ? reinterpret_cast<const float*>(rg.stage0) : s_pa;
+        const int tpitch = pa_pre ? pa_p : kPaPitch;
+        if (pa_pre) { mbar_wait(bar_pa, pa_phase, ctrl, 207); pa_phase ^= 1; }
         for (int r0 = 0; r0 < nrounds; ++r0) {
-          const int jbase = r0 * kAttRound, cnt = min(T - jbase, kAttRound), nch = (cnt + 7) >> 3;
-          if (r0 > 0) att_im2col_mma_tr(r0);
+          const int jbase = r0 * kAttRound, cnt = min(T - jbase, rlen), nch = (cnt + 7) >> 3;
+          if (r0 > 0) att_pa_round(r0, s_pa, kPaPitch, kAttRound);
           T2_PROF(16);
           // energies e_j = sum_d v_d tanh(q_d + pa_dj + pm_jd): this thread adds dim d = adim for the 8 positions of
           // each of its chunks, then the 32 dims of the warp are summed with a transpose-reduce (9 shuffles per 8
@@ -927,8 +973,8 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
             if (c + 4 < nch) load_pm(pmr, j0 + 32, cnt);           // next chunk's loads fly during this chunk's tanh
             float g[8], sv[8];
             {
-              const float4 g0 = *reinterpret_cast<const float4*>(s_pa + adim * kPaPitch + j0);
-              const float4 g1 = *reinterpret_cast<const float4*>(s_pa + adim * kPaPitch + j0 + 4);
+              const float4 g0 = *reinterpret_cast<const float4*>(s_tile + adim * tpitch + j0);
+              const float4 g1 = *reinterpret_cast<const float4*>(s_tile + adim * tpitch + j0 + 4);
               g[0] = g0.x; g[1] = g0.y; g[2] = g0.z; g[3] = g0.w; g[4] = g1.x; g[5] = g1.y; g[6] = g1.z; g[7] = g1.w;
             }
 #pragma unroll
@@ -993,10 +1039,11 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         // j-group jg sums positions jg, jg + 8, ... below `split`, then split + jg, split + jg + 8, ... below `clen`.
         // INFER: clen = len and split = the rows a launch sized for T_enc = len stages, so the grouping is a function of
         // the row's own length, not of the launch's T_enc, and a row of a ragged batch gets the bits it gets alone
-        // (positions >= len have weight 0 and are skipped).  Without lengths, len = T_enc and split = smem_rows.
-        // TEACHER keeps the launch's grouping over all T_enc positions.
+        // (positions >= len have weight 0 and are skipped).  Without lengths, len = T_enc and split = staged_rows(T_enc).
+        // TEACHER keeps the launch's grouping over all T_enc positions.  The grouping does not depend on where a row
+        // lives: rows [smem_rows, split) are read from L2 (the precomputed pa tile leaves fewer rows of the ring).
         const int c4 = tid & 63, jg = tid >> 6;                   // 64 float4 = this CTA's 256 columns; 8 j-groups
-        const float4* ms = reinterpret_cast<const float4*>(rg.stage0 + img_bytes + kPaBytes);
+        const float4* ms = reinterpret_cast<const float4*>(rg.stage0 + mem_off);
         const float* mp = p.memory + (long)b * T * kEnc + ahalf * (kEnc / 2) + c4 * 4;
         const int clen = p.infer ? len : T;
         const int split = p.infer ? staged_rows(len, len <= p.t4max ? 4 : 3) : smem_rows;   // >= smem_rows if clen > smem_rows
@@ -1133,6 +1180,14 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         signal_counter(&ctrl->x2_count, 1u + (stop ? kStopFlag : 0u));
       }
       T2_PROF(12);
+      // The upper CTA of an attention pair is idle until x2 arrives and its ring is empty (E3 armed no next event): it
+      // computes the location term of step t+1 from this step's attention weights, every round, into row b's block of
+      // p.pa.  A resumed chunk reads it from there.  Its ah signal of step t+1 orders these stores before both CTAs of the
+      // pair copy the tile.
+      if (pa_pre && ahalf == 1 && att_cta && t + 1 < p.cap)
+        for (int r0 = 0; r0 < att_rounds; ++r0)
+          att_pa_round(r0, pa_row + r0 * kAttRound, pa_p, min(T - r0 * kAttRound, kAttRound));
+      T2_PROF(20);
       stop |= wait_counter(&ctrl->x2_count, (unsigned int)(kX2Ctas * (t + 1 - p.t_begin)), s_flag, ctrl, 103);
       T2_PROF(14);
       if (stop) { ++t; break; }
@@ -1180,7 +1235,8 @@ static size_t persistent_smem_bytes(int T, int nstages) {
 constexpr size_t kSmemLimit = 227 * 1024;
 // 4 ring stages when they fit beside the T_enc-dependent attention state (T_enc <= 896 on sm_90's 227 KiB), else 3
 // (T_enc <= 2274; longer memories are refused, see persistent_supported).  The idle ring stages encoder-memory rows
-// 0-93 at 4 stages and 0-57 at 3 for the attention context; later rows are read from L2.
+// 0-93 at 4 stages and 0-57 at 3 for the attention context (fewer beside a precomputed pa tile); later rows are read
+// from L2.
 static int persistent_stages(int T) {
   int want = 4;
   const char* e = getenv("T2_STAGES");
@@ -1192,11 +1248,17 @@ static int persistent_stages(int T) {
 constexpr int kImageChunks = 4 + 16 + 8 + 16 + 4;          // K chunks of the x2, ah, ctx, dh and x1 images
 constexpr size_t kImagesBytes = (size_t)kImageChunks * kXChunkBytes + (size_t)kRows * kAtt * 4;   // + q
 
+// the next step's location term of 64 rows (KParams::pa); none where no ring depth holds its tile
+__host__ __device__ static size_t pa_buffer_floats(int T) { return pa_tile_fits(T, kMaxStages) ? (size_t)kRows * pa_tile_bytes(T) / 4 : 0; }
+// whether a launch computes pa during the x2 wait (INFER, and the tile fits the ring it runs with)
+static bool pa_precomputed(int T, bool infer) { return infer && pa_tile_fits(T, persistent_stages(T)); }
+
 // the persistent kernel's part of the decoder workspace: activation images x2 (4 chunks), ah (16), ctx (8), dh (16),
-// x1 (4) and q (64 x 128 fp32); for teacher forcing the x2 images of every step (cap x 4 chunks)
-void persistent_ws_layout(Carve& c, int cap, DecoderWs* w) {
+// x1 (4) and q (64 x 128 fp32); for teacher forcing the x2 images of every step (cap x 4 chunks); the pa buffer
+void persistent_ws_layout(Carve& c, int T, int cap, DecoderWs* w) {
   w->images = c.take<uint8_t>(kImagesBytes);
   w->teacher_img = c.take<uint8_t>((size_t)cap * 4 * kXChunkBytes, 1024);
+  w->pa = c.take<float>(pa_buffer_floats(T), 16);
 }
 
 bool persistent_supported(const T2Model* m, const T2DecoderArgs* a) {
@@ -1401,6 +1463,10 @@ static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t
   KParams p;
   slice_params(m, a, b0, nb, &p);
   carve_images(w.images, &p);
+  if (pa_precomputed(T, p.infer)) {      // zero attention weights -> pa of step 0 is +0.0
+    T2_CUDA(cudaMemsetAsync(w.pa, 0, pa_buffer_floats(T) * 4, s));
+    p.pa = w.pa;
+  }
   p.pm = w.pm;
   p.ctrl = w.ctrl;
   const int B = nb;
@@ -1434,6 +1500,7 @@ struct StreamSlice {
   uint8_t* images;       // activation images + q (kImagesBytes)
   float* acc; float* cell; float* att; int32_t* done;
   float* pm;             // processed memory of the slice's rows (nb, T, 128)
+  float* pa;             // location term of the next step (KParams::pa)
 };
 // the slices one after the other; returns slice `b0 / kRows` (any slice when only measuring)
 __host__ __device__ static StreamSlice stream_state_layout(Carve& c, int B, int T, int b0) {
@@ -1449,6 +1516,7 @@ __host__ __device__ static StreamSlice stream_state_layout(Carve& c, int B, int 
     sl.att = c.take<float>((size_t)kG * 2 * tpp, 1024);
     sl.done = c.take<int32_t>(kRows, 1024);
     sl.pm = c.take<float>((size_t)nb * T * kAtt, 1024);
+    sl.pa = c.take<float>(pa_buffer_floats(T), 1024);
     if (b == b0) want = sl;
   }
   return want;
@@ -1482,6 +1550,7 @@ int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32
     p.t_begin = t0;
     p.t_end = n < a->n_steps_cap - t0 ? t0 + n : a->n_steps_cap;
     p.rs_acc = sl.acc; p.rs_cell = sl.cell; p.rs_att = sl.att; p.rs_done = sl.done; p.rs_status = status + 2 * si;
+    if (pa_precomputed(a->T_enc, p.infer)) p.pa = sl.pa;      // zeroed by begin, left by the previous chunk
     T2_TRY(launch_persistent(p, s));
   }
   return T2_OK;
@@ -1518,6 +1587,8 @@ __global__ void __launch_bounds__(256) stream_admit_kernel(void* state, int B, i
   }
   float* q = reinterpret_cast<float*>(sl.images + (size_t)kImageChunks * kXChunkBytes);
   for (int i = tid; i < kAtt; i += 256) q[lr * kAtt + i] = 0.f;
+  const size_t pa_row = pa_buffer_floats(T) / kRows;                // its pa tile (zero weights -> zero location term)
+  for (size_t i = tid; i < pa_row; i += 256) sl.pa[lr * pa_row + i] = 0.f;
   if (tid == 0) { sl.done[lr] = 0; mel_lengths[row] = -1; }
 }
 
