@@ -601,14 +601,11 @@ int    t2_griffin_lim(T2Denoiser* h, const T2GriffinLimArgs* a, void* stream);
 
 /* ---- self tests (libt2b200_selftest.so only: the same sources built with -DT2_SELFTEST; not part of the product
  * library) -------------------------------------------------------------------------------------------------
- * t2_selftest_umma: runs the wgmma split-fp16 GEMM engine used by the persistent decoder on a
- * (64 x K) x (N x K)^T problem and writes C (64 x N) fp32. */
+ * t2_selftest_event: the wgmma split-fp16 event engine of the persistent decoder and the decoder backward, on an event
+ * plan given as its consumers' row counts (consumers_host[0..n_consumers), host memory; 1-3 consumers of 16 or 32 rows),
+ * run by the backward's skinny GEMM kernel: C (64 x N) = A (64 x K) . W (N x K)^T fp32 with N the sum of the rows, W's
+ * rows in consumer order, K a multiple of 64 up to 1024. */
 #ifdef T2_SELFTEST
-int t2_selftest_umma(const float* A, const float* W, int32_t N, int32_t K, int32_t passes,
-                     float* C, void* stream);
-/* t2_selftest_event: the same engine on an event plan given as its consumers' row counts (consumers_host[0..n_consumers),
- * host memory; 1-3 consumers of 8, 16, 24 or 32 rows): C (64 x N) = 2 A (64 x K) . W (N x K)^T with N the sum of
- * the rows, W's rows in consumer order, K a multiple of 64 up to 1024. */
 int t2_selftest_event(const float* A, const float* W, const int32_t* consumers_host, int32_t n_consumers, int32_t K,
                       float* C, void* stream);
 /* Micro-benchmark: SM cycles for `reps` back-to-back wgmma of one warpgroup (M = 64, N in {32, 64, 128}, K = 16, fp16,

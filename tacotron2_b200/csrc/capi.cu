@@ -34,7 +34,6 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per
 size_t encoder_ws_bytes(int B, int T);
 int postnet_forward(T2Model* m, const T2PostnetArgs* a, cudaStream_t s, bool per_row);
 size_t postnet_ws_bytes(int B, int T);
-int selftest_umma(const float* A, const float* W, int N, int K, int passes, float* C, cudaStream_t s);
 int selftest_event(const float* A, const float* W, const int* cons, int ncons, int K, float* C, cudaStream_t s);
 int mma_rate(int M, int N, int reps, int alternate_d, long long* out_host, cudaStream_t s);
 int mma_group(int M, int N, int group, int reps, long long* out_host, cudaStream_t s);
@@ -112,6 +111,7 @@ int pack_model(T2Model* m, cudaStream_t s) {
     T2_TRY(tc_pack_weights(m->w[W_POST_CONV0 + 7 * i], co, ci, kConvK, nt, m->tc_post_conv[i], s));
   }
   T2_TRY(persistent_pack_create(m, s));
+  T2_TRY(backward_plans_create(m, s));
   return T2_OK;
 }
 
@@ -234,6 +234,7 @@ int t2_model_destroy(T2Model* m) {
   for (int i = 0; i < 5; ++i) cudaFree(m->tc_post_conv[i]);
   cudaFree(m->tc_enc_wih);
   persistent_pack_destroy(m);
+  backward_plans_destroy(m);
   delete m;
   return T2_OK;
 }
@@ -574,10 +575,6 @@ int t2_selftest_mma_rate(int32_t M, int32_t N, int32_t reps, int32_t alternate_d
 
 int t2_selftest_mma_group(int32_t M, int32_t N, int32_t group, int32_t reps, int64_t* out_host) {
   return mma_group(M, N, group, reps, (long long*)out_host, 0);
-}
-
-int t2_selftest_umma(const float* A, const float* W, int32_t N, int32_t K, int32_t passes, float* C, void* stream) {
-  return selftest_umma(A, W, N, K, passes, C, (cudaStream_t)stream);
 }
 
 int t2_selftest_event(const float* A, const float* W, const int32_t* consumers, int32_t n_consumers, int32_t K, float* C,

@@ -72,14 +72,9 @@ int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32
 // the listed rows to the requests' own buffers
 int persistent_stream_admit(T2Model* m, const T2DecoderArgs* a, void* state, const int32_t* rows, int n_rows, cudaStream_t s);
 int persistent_stream_collect(const T2DecoderArgs* a, const T2CollectRow* rows, int n_rows, cudaStream_t s);
-
-// tensor-core skinny GEMMs of the decoder backward (decoder_persistent.cu): which = 0 decoder LSTM (2560 columns),
-// 1 attention LSTM (1792 columns); K = 4096 gate rows in kBwdGemmSplit partial sums
-constexpr int kBwdGemmSplit = 4;
-constexpr int kBwdImgBytes = 64 * 16384;     // activation image of one (64 x 4096) operand
-size_t bwd_wimg_bytes(int which);     // the W^T image of [W_ih | W_hh] of one LSTM
-int bwd_gemm_prepare(T2Model* m, uint8_t* const* wimg, cudaStream_t s);
-int bwd_gemm_run(T2Model* m, int which, const uint8_t* w_img, const uint8_t* x_img, const float* inv_scale, float* P, int ldp,
-                 DecoderCtrl* ctrl, cudaStream_t s);
+// fp32 rows (n_rows x K, ld) -> split-fp16 activation images of the event engine (event_engine.cuh), one per blockIdx.y;
+// grid (K / 64, images) (decoder_persistent.cu)
+__global__ void rows_to_image_kernel(const float* __restrict__ src, long ld, int n_rows, int K,
+                                     long src_block_stride, uint8_t* __restrict__ dst, long dst_block_stride);
 
 }  // namespace t2

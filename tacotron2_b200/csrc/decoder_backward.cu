@@ -15,10 +15,11 @@
 #include <string.h>
 
 #include <algorithm>
+#include <vector>
 
 #include "decoder.h"
+#include "event_engine.cuh"
 #include "gemm_f32.cuh"
-#include "umma.cuh"
 #include "gemm_tc.h"
 #include "wgrad_tc.h"
 
@@ -127,6 +128,127 @@ __global__ void __launch_bounds__(1024) lstm_bwd_row_kernel(const LstmBwdArgs a)
     const uint32_t eo = img_elem_offset(b, k & 63);
     hi[eo] = h; lo[eo] = l;
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Skinny GEMMs (KB / KE) on the tensor cores:
+//   P[split][b][col] = inv_scale[b] * sum_{n in the split's chunks} dG_scaled[b][n] * Wcat[n][col]
+// dG (64 x 4096) arrives as a split-fp16 activation image whose rows were scaled by a power of two
+// (row maximum in [0.5, 1): gradients span many orders of magnitude, fp16 does not); Wcat = [W_ih | W_hh]
+// is streamed as W^T images (rows = output columns, K = gate rows).  Same ring / MMA / accumulator tile
+// as the decoder's events (event_engine.cuh): a tile of output columns is planned as consumers of 32, 32 and 16 columns.
+// which = 0: decoder LSTM (2560 columns), 1: attention LSTM (1792 columns); K = 4096 gate rows in kBwdGemmSplit partial sums.
+// ---------------------------------------------------------------------------------------------
+constexpr int kBwdGemmSplit = 4;
+constexpr int kBwdImgBytes = 64 * 16384;            // activation image of one (64 x 4096) operand
+constexpr int kBwdTileB = 80, kBwdTileE = 64;       // output columns per CTA: 2560 = 32 x 80, 1792 = 28 x 64
+constexpr int kBwdChunks = 4 * kARnn / kChunkK;     // 64 K chunks
+
+struct BwdCta {          // one CTA of a backward skinny GEMM: a tile of output columns x a range of K chunks
+  EventPlan ep;
+  int32_t chunk0, nchunks;   // K chunks (64 gate rows each) of this CTA
+  int32_t col0, split;       // first output column, index of the K split (partials)
+};
+
+// Wcat = [W0 | W1]: element (n, col) is w0[n * ld0 + col * cs0] for col < cols0, else w1[n * cols1 + col - cols0]
+__global__ void pack_bwd_wimg_kernel(const float* __restrict__ w0, long ld0, long cs0, int cols0, const float* __restrict__ w1,
+                                     int cols1, const BwdCta* __restrict__ plans, uint8_t* __restrict__ wimg) {
+  // grid (max chunks per CTA, n_cta): image block of chunk j of CTA c: rows = its output columns, k = 64 gate rows
+  const BwdCta& pc = plans[blockIdx.y];
+  const int j = blockIdx.x;
+  if (j >= pc.nchunks) return;
+  const int n = pc.ep.nrows;
+  __half* img = reinterpret_cast<__half*>(wimg + pc.ep.w_off + (size_t)j * pc.ep.w_bytes);
+  const int n0 = (pc.chunk0 + j) * kChunkK;
+  for (int i = threadIdx.x; i < n * kChunkK; i += blockDim.x) {
+    const int k = i / n, r = i - k * n;            // r fastest: coalesced along the weight matrix' columns
+    const int col = pc.col0 + r;
+    const float v = col < cols0 ? w0[(n0 + k) * ld0 + col * cs0] : w1[(long)(n0 + k) * cols1 + (col - cols0)];
+    int hr, lr;
+    plan_image_rows(pc.ep, r, hr, lr);
+    __half h, l;
+    split_fp16(v, h, l);
+    img[img_elem_offset(hr, k)] = h;
+    img[img_elem_offset(lr, k)] = l;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w_img, const BwdCta* __restrict__ plans,
+                const float* __restrict__ inv_scale, float* __restrict__ P, int ldp, DecoderCtrl* ctrl) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const int tid = threadIdx.x;
+  const BwdCta pc = plans[blockIdx.x];
+  Carve sc(smem_raw, 1);
+  GemmSmem sm;
+  gemm_smem_layout(sc, &sm);
+  Ring rg;
+  rg.stage0 = sm.stage0;
+  rg.full = sm.bars; rg.empty = sm.bars + kStages;
+  float* s_acc = sm.acc;
+  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
+  rg.pol_x = ptx::policy_evict_last(); rg.pol_w = ptx::policy_evict_first();
+  rg.pre = 0; rg.ns = kStages;
+  if (tid == 0) {
+    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
+    ptx::fence_barrier_init();
+  }
+  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;
+  __syncthreads();
+  run_event(rg, pc.ep, x_img + (size_t)pc.chunk0 * kXChunkBytes, w_img, pc.nchunks, s_acc, ctrl, nullptr);
+  const int N = pc.ep.nrows;
+  for (int i = tid; i < kRows * N; i += kThreads) {
+    const int row = i / N, c = i - row * N;
+    P[((size_t)pc.split * kRows + row) * ldp + pc.col0 + c] = s_acc[row * kAccPitch + c] * inv_scale[row];
+  }
+}
+
+int bwd_gemm_ctas(int which) { return which == 0 ? (2560 / kBwdTileB) * kBwdGemmSplit : (1792 / kBwdTileE) * kBwdGemmSplit; }
+int bwd_tile(int which) { return which == 0 ? kBwdTileB : kBwdTileE; }
+uint32_t bwd_w_bytes(int which) { return (uint32_t)(2 * bwd_tile(which) * kChunkK * 2); }
+size_t bwd_wimg_bytes(int which) { return (size_t)((which == 0 ? 2560 : 1792) / bwd_tile(which)) * kBwdChunks * bwd_w_bytes(which); }
+// the device CTA plans of one skinny GEMM: T2Model::bwd_plans holds those of which = 0, then those of which = 1
+const BwdCta* bwd_plans(const T2Model* m, int which) { return (const BwdCta*)m->bwd_plans + (which == 0 ? 0 : bwd_gemm_ctas(0)); }
+
+std::vector<BwdCta> bwd_gemm_plans(int which) {
+  const int tile = bwd_tile(which), ntile = (which == 0 ? 2560 : 1792) / tile;
+  const uint32_t w_bytes = bwd_w_bytes(which);
+  std::vector<BwdCta> plans(ntile * kBwdGemmSplit);
+  for (int t = 0; t < ntile; ++t)
+    for (int sp = 0; sp < kBwdGemmSplit; ++sp) {
+      BwdCta& c = plans[t * kBwdGemmSplit + sp];
+      memset(&c, 0, sizeof(c));
+      c.chunk0 = sp * kBwdChunks / kBwdGemmSplit; c.nchunks = (sp + 1) * kBwdChunks / kBwdGemmSplit - c.chunk0;
+      c.col0 = t * tile; c.split = sp;
+      plan_one_matrix(c.ep, tile);    // 80 = 32 + 32 + 16, 64 = 32 + 32 columns (event_plan_fits)
+      c.ep.col0 = 0; c.ep.chunks = c.nchunks;
+      c.ep.w_off = (uint32_t)(((size_t)t * kBwdChunks + c.chunk0) * w_bytes);
+    }
+  return plans;
+}
+
+// packs the W^T images of both LSTMs from the caller's current fp32 weights into wimg[0 / 1] (bwd_wimg_bytes)
+int bwd_gemm_prepare(T2Model* m, uint8_t* const* wimg, cudaStream_t s) {
+  if (!m->bwd_plans) return fail(T2_ERR_INVALID, "backward GEMM: model has no CTA plans");
+  for (int which = 0; which < 2; ++which) {
+    const float* w0 = m->w[which == 0 ? W_DRNN_WIH : W_ARNN_WIH];
+    const float* w1 = m->w[which == 0 ? W_DRNN_WHH : W_ARNN_WHH];
+    const int cols0 = which == 0 ? kARnn + kEnc : kPre + kEnc;
+    pack_bwd_wimg_kernel<<<dim3(kBwdChunks / kBwdGemmSplit, bwd_gemm_ctas(which)), 256, 0, s>>>(w0, cols0, 1, cols0, w1, kARnn,
+                                                                                             bwd_plans(m, which), wimg[which]);
+    T2_LAUNCH_CHECK();
+  }
+  return T2_OK;
+}
+
+// one launch of the n_cta CTAs of `plans` (device)
+int bwd_gemm_run(const BwdCta* plans, int n_cta, const uint8_t* w_img, const uint8_t* x_img, const float* inv_scale, float* P,
+                 int ldp, DecoderCtrl* ctrl, cudaStream_t s) {
+  const size_t smem = gemm_smem_bytes();
+  T2_CUDA(cudaFuncSetAttribute(bwd_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  bwd_gemm_kernel<<<n_cta, kThreads, smem, s>>>(x_img, w_img, plans, inv_scale, P, ldp, ctrl);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -457,6 +579,23 @@ void bwd_ws_layout(Carve& c, int B, int Te, int T, BwdWs* w) {
 
 }  // namespace
 
+// The skinny GEMMs' CTA plans depend on the shapes only: built once with the model, so a backward call copies nothing
+int backward_plans_create(T2Model* m, cudaStream_t s) {
+  if (m->bwd_plans) return T2_OK;
+  std::vector<BwdCta> plans = bwd_gemm_plans(0);
+  const std::vector<BwdCta> att = bwd_gemm_plans(1);
+  plans.insert(plans.end(), att.begin(), att.end());
+  T2_CUDA(cudaMalloc(&m->bwd_plans, sizeof(BwdCta) * plans.size()));
+  T2_CUDA(cudaMemcpyAsync(m->bwd_plans, plans.data(), sizeof(BwdCta) * plans.size(), cudaMemcpyHostToDevice, s));
+  T2_CUDA(cudaStreamSynchronize(s));   // `plans` is a host temporary
+  return T2_OK;
+}
+
+void backward_plans_destroy(T2Model* m) {
+  cudaFree(m->bwd_plans);
+  m->bwd_plans = nullptr;
+}
+
 size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel) {
   Carve c(nullptr, 1024);
   BwdWs w;
@@ -531,7 +670,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
       lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(bwd_gemm_run(m, 0, w.bwd_wimg[0], w.img_d, w.inv_scale, w.pb, kPBld, w.ctrl, s));   // KB
+    T2_TRY(bwd_gemm_run(bwd_plans(m, 0), bwd_gemm_ctas(0), w.bwd_wimg[0], w.img_d, w.inv_scale, w.pb, kPBld, w.ctrl, s));   // KB
     {  // KC
       AttBwdArgs k;
       memset(&k, 0, sizeof(k));
@@ -557,7 +696,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
       lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(bwd_gemm_run(m, 1, w.bwd_wimg[1], w.img_a, w.inv_scale + 64, w.pe, kPEld, w.ctrl, s));   // KE
+    T2_TRY(bwd_gemm_run(bwd_plans(m, 1), bwd_gemm_ctas(1), w.bwd_wimg[1], w.img_a, w.inv_scale + 64, w.pe, kPEld, w.ctrl, s));   // KE
   }
   reduce_pe_x2_kernel<<<B, 256, 0, s>>>(w.pe, a->d_prenet, B, kBwdGemmSplit);
   T2_LAUNCH_CHECK();
@@ -671,5 +810,45 @@ int prenet_backward(T2Model* m, const T2PrenetBwdArgs* a, cudaStream_t s) {
                       a->grads[W_PRENET0], kMel, 0.f));
   return T2_OK;
 }
+
+#ifdef T2_SELFTEST
+// ---------------------------------------------------------------------------------------------
+// self test of the event engine: C (64 x N) = A (64 x K) . W (N x K)^T for the plan whose consumers have cons[0..ncons)
+// rows, on the skinny GEMM kernel with one CTA and unit row scales.  The N rows of W are the plan's consumers in order.
+// ---------------------------------------------------------------------------------------------
+int selftest_event(const float* A, const float* W, const int* cons, int ncons, int K, float* C, cudaStream_t s) {
+  if (ncons < 1 || ncons > 3 || K % kChunkK != 0 || K <= 0 || K > 16 * kChunkK)
+    return fail(T2_ERR_INVALID, "selftest_event: 1-3 consumers, K a multiple of 64 up to 1024");
+  BwdCta pc;
+  memset(&pc, 0, sizeof(pc));
+  for (int i = 0; i < ncons; ++i) { pc.ep.n[i] = cons[i]; pc.ep.nrows += cons[i]; }
+  pc.ep.ncons = ncons; pc.ep.w_bytes = (uint32_t)pc.ep.nrows * 256; pc.ep.chunks = pc.nchunks = K / kChunkK;
+  if (!event_plan_fits(pc.ep)) return fail(T2_ERR_INVALID, "selftest_event: 1-3 consumers of 16 or 32 rows");
+  const int chunks = pc.nchunks, N = pc.ep.nrows;
+  uint8_t *ximg, *wimg; BwdCta* plan; float* ones; DecoderCtrl* ctrl;
+  auto layout = [&](Carve& c) {
+    ximg = c.take<uint8_t>((size_t)chunks * kXChunkBytes); wimg = c.take<uint8_t>((size_t)chunks * pc.ep.w_bytes);
+    plan = c.take<BwdCta>(1); ones = c.take<float>(kRows); ctrl = c.take<DecoderCtrl>(1);
+  };
+  Carve size(nullptr);
+  layout(size);
+  void* buf = nullptr;
+  T2_CUDA(cudaMalloc(&buf, size.bytes()));
+  Carve c(buf);
+  layout(c);
+  T2_CUDA(cudaMemcpyAsync(plan, &pc, sizeof(pc), cudaMemcpyHostToDevice, s));
+  T2_CUDA(cudaMemsetAsync(ctrl, 0, sizeof(DecoderCtrl), s));
+  fill_kernel<<<1, kRows, 0, s>>>(ones, 1.f, kRows);
+  T2_LAUNCH_CHECK();
+  rows_to_image_kernel<<<dim3(chunks, 1), 256, 0, s>>>(A, K, kRows, K, 0, ximg, 0);
+  T2_LAUNCH_CHECK();
+  pack_bwd_wimg_kernel<<<dim3(chunks, 1), 256, 0, s>>>(W, 1, K, N, nullptr, 0, plan, wimg);     // Wcat = W^T
+  T2_LAUNCH_CHECK();
+  T2_TRY(bwd_gemm_run(plan, 1, wimg, ximg, ones, C, N, ctrl, s));
+  T2_CUDA(cudaStreamSynchronize(s));
+  cudaFree(buf);
+  return T2_OK;
+}
+#endif  // T2_SELFTEST
 
 }  // namespace t2

@@ -37,55 +37,29 @@
 #include <vector>
 
 #include "decoder.h"
+#include "event_engine.cuh"
 #include "gemm_f32.cuh"
-#include "umma.cuh"
 
 namespace t2 {
 
 namespace {
 
 constexpr int kG = 128;               // CTAs
-constexpr int kThreads = 512;
-constexpr int kStages = 4;             // ring stages of the helper kernels (self test, backward GEMMs)
 constexpr int kMaxStages = 4;          // the decoder kernel runs 4 stages up to T_enc = 896, else 3
                                        // (T2_STAGES = 3 forces the 3-stage ring)
-constexpr int kRows = 64;             // batch rows per launch (zero padded)
-constexpr int kXChunkBytes = 2 * kRows * kChunkK * 2;    // [hi 64 rows | lo 64 rows] x 64 k fp16 = 16 KiB
 // accumulator columns (shared memory, fp32 [64 batch rows][kAccPitch]): att 0-31, dec 32-63, shared slot 64-79
 constexpr int kColA = 0, kColD = 32, kColS = 64;
-constexpr int kHiCols = 80;                               // max weight rows of one event (hi)
-constexpr int kAccPitch = 84;                             // floats per accumulator row (80 + 4: fewer bank conflicts)
-constexpr int kAccBytes = kRows * kAccPitch * 4;
-constexpr int kMmaWgs = 3;                                // warpgroups 1-3 issue the MMAs of an event (one piece each)
 constexpr int kAttRound = 64;                             // encoder positions per attention pa GEMM
 constexpr int kAttPlane = kAttRound * 128;                // one fp16 plane of the im2col image (64 positions x 64 taps)
 constexpr int kPaPitch = kAttRound + 4;                   // floats per attention dim of the pa tile
 constexpr int kPaBytes = kAtt * kPaPitch * 4;
-constexpr int kWStageMax = 2 * kHiCols * kChunkK * 2;    // hi + lo planes of up to 80 weight rows = 20 KiB
-constexpr int kStageBytes = kXChunkBytes + kWStageMax;   // 36 KiB
 constexpr int kNumEvents = 5;         // x2, ah, ctx, dh, x1
 constexpr int kPCols = 344;           // 80 mel + 1 gate + 256 x1 + 7 pad
 constexpr int kQCta0 = 0, kQCtas = 16, kX2Cta0 = 16, kX2Ctas = 32, kPCta0 = 48, kPCtas = 43;
 constexpr int kWeffBytes = kAtt * kChunkK * 2 * 2;        // fused location filter image (hi+lo) = 32 KiB
-constexpr unsigned long long kWatchdogCycles = 1ull << 32;   // ~2 s
 
-struct EventPlan {
-  uint32_t w_off;       // byte offset of this CTA's first chunk in the W image buffer
-  uint32_t w_bytes;     // W bytes per chunk = 2 x nrows x 128
-  int32_t nrows;        // hi weight rows of all consumers (MMA N = 2 x nrows); 0 = this CTA skips the event
-  int32_t col0;         // accumulator column of the first consumer
-  int32_t ncons;
-  int32_t n[3];         // rows per consumer (packing only)
-  int32_t chunks;       // K chunks of this event (bounds the weight prefetch)
-};
 struct CtaPlan {
   EventPlan ev[kNumEvents];
-};
-
-struct BwdCta {          // one CTA of a backward skinny GEMM: a tile of output columns x a range of K chunks
-  EventPlan ep;
-  int32_t chunk0, nchunks;   // K chunks (64 gate rows each) of this CTA
-  int32_t col0, split;       // first output column, index of the K split (partials)
 };
 
 struct PersistentPack {
@@ -98,11 +72,7 @@ struct PersistentPack {
   int32_t* rows = nullptr;            // row tables for packing
   float* weff = nullptr;              // (128, 64) fp32 fused location filter W_ld . W_loc (62 taps + 2 zero)
   uint8_t* weff_img = nullptr;        // its split-fp16 operand image (32 KiB)
-  // backward skinny GEMMs (training): CTA plans of the decoder (0) and attention (1) LSTM (their weight images are packed
-  // into the backward workspace by every call)
-  BwdCta* bwd_plans[2] = {nullptr, nullptr};
 };
-std::vector<BwdCta> bwd_gemm_plans(int which);   // the CTA plans of a backward skinny GEMM
 
 // ---------------------------------------------------------------------------------------------
 // packing kernels (model create time)
@@ -182,6 +152,8 @@ __global__ void pack_lstm_bias_kernel(const float* __restrict__ b_sum, float* __
   out[i] = b_sum[g * 1024 + cta * 8 + ul];
 }
 
+}  // namespace
+
 // fp32 rows (n_rows x K, ld) -> activation images: chunks x [hi rows 0-63 | lo rows 64-127] x 64 k
 __global__ void rows_to_image_kernel(const float* __restrict__ src, long ld, int n_rows, int K,
                                      long src_block_stride, uint8_t* __restrict__ dst, long dst_block_stride) {
@@ -201,23 +173,11 @@ __global__ void rows_to_image_kernel(const float* __restrict__ src, long ld, int
   }
 }
 
+namespace {
+
 // ---------------------------------------------------------------------------------------------
 // device helpers
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void watchdog_trap(DecoderCtrl* ctrl, int code) {
-  if (ctrl) ctrl->error = code;
-  __threadfence_system();
-  __trap();
-}
-
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, DecoderCtrl* ctrl, int code) {
-  if (ptx::mbar_try_wait(bar, parity)) return;
-  const unsigned long long t0 = clock64();
-  while (!ptx::mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > kWatchdogCycles) watchdog_trap(ctrl, code);
-  }
-}
-
 // One thread of a CTA publishes the CTA's stores (ordered before it by __syncthreads) and bumps a counter: a single
 // gpu-scope fence followed by a relaxed reduction (fence + relaxed atomic = release; __threadfence() followed by
 // red.release paid for two fences).  The waiting side polls with relaxed loads and fences once after the value
@@ -313,18 +273,6 @@ __device__ __forceinline__ float warp_max_f(float v) {
   return v;
 }
 
-struct Ring {
-  uint8_t* stage0;    // kStages buffers of kStageBytes each
-  __device__ __forceinline__ uint8_t* stage(uint32_t s) const { return stage0 + s * kStageBytes; }
-  uint64_t* full;     // [kStages]
-  uint64_t* empty;    // [kStages], released once by each MMA warpgroup
-  uint32_t p_stage, p_phase;   // producer cursor (thread 0 of warp 0)
-  uint32_t c_stage, c_phase;   // consumer cursor (threads of the MMA warpgroups 1-3)
-  uint64_t pol_x, pol_w;       // L2 eviction policies of the activation / weight streams
-  uint32_t pre;                // stages whose weight chunk was already issued for the upcoming event
-  uint32_t ns;                 // number of stages
-};
-
 // Dynamic shared memory of the persistent decoder for (T_enc, ring stages): the kernel carves it and the host sizes
 // the launch from it, which decides the ring depth and the longest T_enc.  The regions are packed in this order.
 struct PersistentSmem {
@@ -358,175 +306,6 @@ __host__ __device__ __forceinline__ void persistent_smem_layout(Carve& c, int T,
   s->pad0 = c.take<float>(tpp, 1); s->pad1 = c.take<float>(tpp, 1);
   s->e = c.take<float>((size_t)ntiles * 128, 1);
   s->ep = c.take<float>((size_t)4 * ntiles * 128, 1);
-}
-
-// Dynamic shared memory of the self test and the backward GEMMs: ring stages, barriers, then the accumulator tile
-struct GemmSmem { uint8_t* stage0; uint64_t* bars; float* acc; };
-__host__ __device__ __forceinline__ void gemm_smem_layout(Carve& c, GemmSmem* s) {
-  s->stage0 = c.take<uint8_t>((size_t)kStages * kStageBytes, 1);
-  s->bars = c.take<uint64_t>(16, 1);
-  s->acc = c.take<float>(kAccBytes / 4, 1);      // [64][kAccPitch]
-}
-size_t gemm_smem_bytes() { Carve c(nullptr, 1); GemmSmem s; gemm_smem_layout(c, &s); return c.bytes(); }
-
-// Weight chunks do not depend on the grid barrier that separates two events (only the activation does):
-// the producer arms the first kStages stages of the NEXT event and issues their weight copies right after
-// the current event's last chunk, so their L2 / HBM latency overlaps the epilogue and the barrier.
-__device__ __forceinline__ void prefetch_weights(Ring& rg, const EventPlan& nx, const uint8_t* w_img,
-                                                 DecoderCtrl* ctrl) {
-  uint32_t s = rg.p_stage, ph = rg.p_phase;
-  const uint32_t n = min(rg.ns, (uint32_t)nx.chunks);
-  for (uint32_t i = 0; i < n; ++i) {
-    mbar_wait(&rg.empty[s], ph ^ 1, ctrl, 205);
-    ptx::mbar_arrive_expect_tx(&rg.full[s], kXChunkBytes + nx.w_bytes);
-    ptx::bulk_g2s_hint(rg.stage(s) + kXChunkBytes, w_img + nx.w_off + (size_t)i * nx.w_bytes, nx.w_bytes,
-                       &rg.full[s], rg.pol_w);
-    if (++s == rg.ns) { s = 0; ph ^= 1; }
-  }
-  rg.pre = n;
-}
-
-// How the three MMA warpgroups split an event.  Each consumer's rows sit in the stage as [n hi rows | n lo rows], so
-// warpgroup 1 + c takes consumer c (n <= 32 rows) as ONE wgmma B operand of N = 2 n rows [W_hi; W_lo] and multiplies it
-// with A = X_hi and A = X_lo: two wgmma per 16-wide K step, each reading its activation plane and the consumer's rows
-// once (instead of four with separate hi / lo B operands, each re-reading an A plane).  N stays <= 64 (32 accumulator
-// registers): the kernel runs at the 128-register limit of 512 threads, and a wider accumulator spills.
-// all_widths = false: the consumer widths run_event<false> (decoder, backward GEMMs) is built for
-inline bool event_plan_fits(const EventPlan& ep, bool all_widths) {
-  if (ep.ncons < 1 || ep.ncons > kMmaWgs) return false;
-  for (int c = 0; c < ep.ncons; ++c)
-    if (ep.n[c] != 16 && ep.n[c] != 32 && !(all_widths && (ep.n[c] == 8 || ep.n[c] == 24))) return false;
-  return true;
-}
-// `rows` output rows of one matrix as consumers that fit the warpgroups: 32, 32, rest (rows <= 80, a multiple of 8)
-inline void plan_one_matrix(EventPlan& ep, int rows) {
-  ep.ncons = 0; ep.nrows = rows;
-  for (int r = rows; r > 0 && ep.ncons < 3; ) {
-    const int n = ep.ncons < 2 && r >= 32 ? 32 : r;
-    ep.n[ep.ncons++] = n; r -= n;
-  }
-  ep.w_bytes = (uint32_t)rows * 256;
-}
-// image rows of the hi and lo copies of row r (counted over all consumers) of a plan
-__device__ __forceinline__ void plan_image_rows(const EventPlan& ep, int r, int& hi, int& lo) {
-  int roff = 0;
-  for (int c = 0; c < ep.ncons; ++c) {
-    if (r < ep.n[c]) { hi = roff + r; lo = hi + ep.n[c]; return; }
-    r -= ep.n[c]; roff += 2 * ep.n[c];
-  }
-  hi = lo = 0;
-}
-
-// One MMA warpgroup's consumer of an event: D (64 x 2n) = X_hi . B^T + X_lo . B^T over all `chunks` stages, where B is
-// the consumer's 2n weight-image rows [W_hi; W_lo] from row w_row0 of each stage; then both column halves of D are
-// added to the accumulator tile from column acol.  Each chunk's stage is released as soon as its MMAs are done: keeping
-// a commit group in flight across chunks would hold every stage one chunk longer, i.e. make the ring one stage shallower
-// for the producer, and the stream waits on L2 latency rather than on the tensor core (measured slower).
-template <int N>
-__device__ __forceinline__ void event_wg(Ring& rg, int chunks, uint32_t w_row0, float* s_acc, int acol, DecoderCtrl* ctrl) {
-  const bool leader = (threadIdx.x & 127) == 0;
-  float d[N / 2];
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
-  for (int i = 0; i < chunks; ++i) {
-    mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
-    const uint32_t xs = ptx::smem_u32(rg.stage(rg.c_stage));
-    const uint32_t ws = xs + kXChunkBytes + w_row0 * 128;
-    ptx::wg_fence_regs<N / 2>(d);
-    ptx::wg_fence();
-#pragma unroll
-    for (int kk = 0; kk < kChunkK / 16; ++kk) {
-      const uint64_t b = ptx::make_sw128_desc(ws + kk * 32);
-      ptx::wgmma_f16<N>(d, ptx::make_sw128_desc(xs + kk * 32), b);                  // X_hi
-      ptx::wgmma_f16<N>(d, ptx::make_sw128_desc(xs + kRows * 128 + kk * 32), b);    // X_lo
-    }
-    ptx::wg_commit();
-    ptx::wg_wait<0>();
-    ptx::wg_fence_regs<N / 2>(d);
-    if (leader) ptx::mbar_arrive(&rg.empty[rg.c_stage]);
-    if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
-  }
-  const int wt = threadIdx.x & 127;
-#pragma unroll
-  for (int j = 0; j < N / 4; ++j)      // registers [0, N/4) hold the W_hi columns, [N/4, N/2) the W_lo ones
-    s_acc[ptx::wg_frag_row(j, wt) * kAccPitch + acol + ptx::wg_frag_col(j, wt)] += d[j] + d[N / 4 + j];
-}
-
-// Streams `chunks` K-chunks of the activation image x_img plus this CTA's weight rows through the ring;
-// warpgroups 1-3 issue the MMAs (one consumer each) and add their products to the accumulator tile s_acc.  Called by all threads;
-// returns after the accumulators are complete.  Every MMA accumulates (the epilogues zero what they consume).
-// The decoder's and the backward GEMMs' consumers have 32 or 16 rows (event_plan_fits(ep, false)); only the self test
-// instantiates the 8- and 24-row consumers (kAllWidths): every width is a copy of the whole chunk loop, and the
-// decoder kernel runs its code once per step, so each copy costs instruction-cache misses.
-template <bool kAllWidths = false>
-__device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const uint8_t* x_img,
-                                          const uint8_t* w_img, int chunks, float* s_acc,
-                                          DecoderCtrl* ctrl, const EventPlan* next,
-                                          const unsigned int* ready = nullptr, unsigned int ready_target = 0) {
-  // ready (16 counters, one per K chunk of the activation; null = the caller synchronised already): chunk i of x_img is
-  // complete once ready[i] >= ready_target.  The activation blocks ah / dh are written in 8-column slices by 128 CTAs, i.e.
-  // a 64-column chunk has 8 producers: instead of a 128-way barrier between the epilogue that writes a block and the event
-  // that streams it, the bulk-copy producer fetches a chunk as soon as ITS 8 producers have arrived, so the stragglers'
-  // skew and the arrival latency overlap with the streaming of the chunks that are already there.
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (ep.nrows == 0) {                 // this CTA has no consumer of this activation
-    if (threadIdx.x == 0 && next != nullptr && next->nrows != 0 && rg.pre == 0) prefetch_weights(rg, *next, w_img, ctrl);
-    return;
-  }
-  if (warp == 0) {
-    if (lane == 0) {
-      int nready = ready ? 0 : chunks;     // chunks [0, nready) are known to be complete
-      for (int i = 0; i < chunks; ++i) {
-        uint8_t* st = rg.stage(rg.p_stage);
-        if ((uint32_t)i >= rg.pre) {     // not armed / issued ahead of time
-          mbar_wait(&rg.empty[rg.p_stage], rg.p_phase ^ 1, ctrl, 200);
-          ptx::mbar_arrive_expect_tx(&rg.full[rg.p_stage], kXChunkBytes + ep.w_bytes);
-          ptx::bulk_g2s_hint(st + kXChunkBytes, w_img + ep.w_off + (size_t)i * ep.w_bytes, ep.w_bytes,
-                             &rg.full[rg.p_stage], rg.pol_w);
-        }
-        if (i >= nready) {               // all 16 counters in one round trip; take the leading run of complete chunks
-          const unsigned long long t0 = clock64();
-          while (true) {
-            uint32_t c[16];
-#pragma unroll
-            for (int j = 0; j < 16; j += 4)
-              asm volatile("ld.relaxed.gpu.global.v4.u32 {%0,%1,%2,%3}, [%4];"
-                           : "=r"(c[j]), "=r"(c[j + 1]), "=r"(c[j + 2]), "=r"(c[j + 3]) : "l"(ready + j) : "memory");
-            uint32_t mask = 0;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) mask |= ((int)(c[j] - ready_target) >= 0 ? 1u : 0u) << j;
-            const int run = __ffs((int)~(mask >> i)) - 1;          // complete chunks starting at i
-            if (run > 0) { nready = min(chunks, i + run); break; }
-            if (clock64() - t0 > kWatchdogCycles) watchdog_trap(ctrl, 206);
-          }
-          asm volatile("fence.acq_rel.gpu;" ::: "memory");
-          ptx::fence_proxy_async();
-        }
-        ptx::bulk_g2s_hint(st, x_img + (size_t)i * kXChunkBytes, kXChunkBytes, &rg.full[rg.p_stage], rg.pol_x);
-        if (++rg.p_stage == rg.ns) { rg.p_stage = 0; rg.p_phase ^= 1; }
-      }
-      rg.pre = 0;
-      if (next != nullptr && next->nrows != 0) prefetch_weights(rg, *next, w_img, ctrl);
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int c = (warp >> 2) - 1;        // this warpgroup's consumer
-    if (c < ep.ncons) {
-      int w_row0 = 0, acol = ep.col0;
-      for (int i = 0; i < c; ++i) { w_row0 += 2 * ep.n[i]; acol += ep.n[i]; }
-      if (ep.n[c] == 32) event_wg<64>(rg, chunks, w_row0, s_acc, acol, ctrl);
-      else if (!kAllWidths || ep.n[c] == 16) event_wg<32>(rg, chunks, w_row0, s_acc, acol, ctrl);
-      else if (ep.n[c] == 24) event_wg<48>(rg, chunks, w_row0, s_acc, acol, ctrl);
-      else event_wg<16>(rg, chunks, w_row0, s_acc, acol, ctrl);
-    } else {                              // no rows for this warpgroup: it still releases every stage it was counted for
-      for (int i = 0; i < chunks; ++i) {
-        mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
-        if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&rg.empty[rg.c_stage]);
-        if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
-      }
-    }
-  }
-  __syncthreads();
 }
 
 // keep bits (bit i = element idx0+i is kept) of 8 consecutive dropout elements, Philox4x32-10 one block per 4
@@ -1295,10 +1074,9 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
     if (hp) set(3, 16, kColD, {32, 16}); else set(3, 16, kColD, {32});
     if (hx) set(4, 4, kColS, {16}); else { pl.ev[4].w_off = (uint32_t)off; }
     for (int ev = 0; ev < kNumEvents; ++ev)
-      if (pl.ev[ev].nrows != 0 && !event_plan_fits(pl.ev[ev], false)) return fail(T2_ERR_INVALID, "event plan does not fit the MMA warpgroups");
+      if (pl.ev[ev].nrows != 0 && !event_plan_fits(pl.ev[ev])) return fail(T2_ERR_INVALID, "event plan does not fit the MMA warpgroups");
   }
   if (off >= (size_t)4 << 30) return fail(T2_ERR_INVALID, "W image too large");
-  const std::vector<BwdCta> bwd_plans[2] = {bwd_gemm_plans(0), bwd_gemm_plans(1)};
   if (!pk->wimg) {
     pk->wimg_bytes = off + 1024;
     T2_CUDA(cudaMalloc((void**)&pk->wimg, pk->wimg_bytes));
@@ -1310,17 +1088,13 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
     T2_CUDA(cudaMalloc((void**)&pk->rows, (size_t)4 * kG * 32 * 4));
     T2_CUDA(cudaMalloc((void**)&pk->weff, (size_t)kAtt * kChunkK * 4));
     T2_CUDA(cudaMalloc((void**)&pk->weff_img, (size_t)kWeffBytes));
-    for (int which = 0; which < 2; ++which) T2_CUDA(cudaMalloc((void**)&pk->bwd_plans[which], sizeof(BwdCta) * bwd_plans[which].size()));
   }
   fuse_location_kernel<<<kAtt, kChunkK, 0, s>>>(m->w[W_ATT_LOC_DENSE], m->w[W_ATT_LOC_CONV], pk->weff);
   T2_LAUNCH_CHECK();
   pack_rows_image_kernel<<<1, 256, 0, s>>>(pk->weff, kAtt, kChunkK, pk->weff_img);
   T2_LAUNCH_CHECK();
   T2_CUDA(cudaMemcpyAsync(pk->plans, plans.data(), sizeof(CtaPlan) * kG, cudaMemcpyHostToDevice, s));
-  for (int which = 0; which < 2; ++which)
-    T2_CUDA(cudaMemcpyAsync(pk->bwd_plans[which], bwd_plans[which].data(), sizeof(BwdCta) * bwd_plans[which].size(),
-                            cudaMemcpyHostToDevice, s));
-  T2_CUDA(cudaStreamSynchronize(s));   // `plans` and `bwd_plans` are host temporaries
+  T2_CUDA(cudaStreamSynchronize(s));   // `plans` is a host temporary
   // ---- W_P = [proj (80) ; gate (1) ; W1.Wproj (256) ; 0 (7)] and its bias ----
   T2_CUDA(cudaMemsetAsync(pk->wp_all, 0, (size_t)kPCols * kdc * 4, s));
   T2_CUDA(cudaMemsetAsync(pk->bias_p, 0, (size_t)kPCols * 4, s));
@@ -1368,7 +1142,6 @@ void persistent_pack_destroy(T2Model* m) {
   if (!pk) return;
   cudaFree(pk->wimg); cudaFree(pk->plans); cudaFree(pk->wp_all); cudaFree(pk->bias_p);
   cudaFree(pk->bias_a); cudaFree(pk->bias_d); cudaFree(pk->rows); cudaFree(pk->weff); cudaFree(pk->weff_img);
-  for (int i = 0; i < 2; ++i) cudaFree(pk->bwd_plans[i]);
   delete pk;
   m->pk = nullptr;
 }
@@ -1639,215 +1412,6 @@ int persistent_stream_collect(const T2DecoderArgs* a, const T2CollectRow* rows, 
     stream_collect_kernel<<<dim3(frames, cb.n), 128, 0, s>>>(cb, a->mel, a->gate, a->align, a->n_steps_cap, a->T_enc);
     T2_LAUNCH_CHECK();
   }
-  return T2_OK;
-}
-
-#ifdef T2_SELFTEST
-// ---------------------------------------------------------------------------------------------
-// self test of the wgmma event engine: C (64 x N) = 2 * A (64 x K) . W (N x K)^T with the same run_event()
-// (two accumulating passes over the ring) and the same accumulator tile as the decoder.  The N rows of W are
-// the plan's consumers in order.
-// ---------------------------------------------------------------------------------------------
-namespace {
-__global__ void __launch_bounds__(kThreads, 1)
-selftest_kernel(const uint8_t* x_img, const uint8_t* w_img, EventPlan ep, int chunks, float* C, int N,
-                DecoderCtrl* ctrl) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const int tid = threadIdx.x;
-  Carve sc(smem_raw, 1);
-  GemmSmem sm;
-  gemm_smem_layout(sc, &sm);
-  Ring rg;
-  rg.stage0 = sm.stage0;
-  rg.full = sm.bars; rg.empty = sm.bars + kStages;
-  float* s_acc = sm.acc;
-  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
-  rg.pol_x = rg.pol_w = ptx::policy_evict_last();
-  rg.pre = 0; rg.ns = kStages;
-  if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
-    ptx::fence_barrier_init();
-  }
-  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;
-  __syncthreads();
-  run_event<true>(rg, ep, x_img, w_img, chunks, s_acc, ctrl, &ep);      // second pass uses the prefetched weights
-  run_event<true>(rg, ep, x_img, w_img, chunks, s_acc, ctrl, nullptr);
-  for (int i = tid; i < kRows * N; i += kThreads) C[i] = s_acc[(i / N) * kAccPitch + i % N];
-}
-
-// (N x K) fp32 row-major -> K/64 chunks of the plan's weight image (every consumer [n hi rows | n lo rows])
-__global__ void pack_plan_image_kernel(const float* __restrict__ W, int K, EventPlan ep, uint8_t* __restrict__ wimg) {
-  const int chunk = blockIdx.x;
-  __half* img = reinterpret_cast<__half*>(wimg + (size_t)chunk * ep.w_bytes);
-  for (int i = threadIdx.x; i < ep.nrows * 64; i += blockDim.x) {
-    const int r = i >> 6, k = i & 63;
-    int hr, lr;
-    plan_image_rows(ep, r, hr, lr);
-    __half h, l;
-    split_fp16(W[(long)r * K + chunk * 64 + k], h, l);
-    img[img_elem_offset(hr, k)] = h;
-    img[img_elem_offset(lr, k)] = l;
-  }
-}
-
-int selftest_plan(const float* A, const float* W, const EventPlan& ep, int K, float* C, cudaStream_t s) {
-  const int chunks = K / kChunkK, N = ep.nrows;
-  uint8_t *ximg = nullptr, *wimg = nullptr; DecoderCtrl* ctrl = nullptr;
-  T2_CUDA(cudaMalloc((void**)&ximg, (size_t)chunks * kXChunkBytes));
-  T2_CUDA(cudaMalloc((void**)&wimg, (size_t)chunks * ep.w_bytes));
-  T2_CUDA(cudaMalloc((void**)&ctrl, sizeof(DecoderCtrl)));
-  T2_CUDA(cudaMemsetAsync(ctrl, 0, sizeof(DecoderCtrl), s));
-  rows_to_image_kernel<<<dim3(chunks, 1), 256, 0, s>>>(A, K, kRows, K, 0, ximg, 0);
-  T2_LAUNCH_CHECK();
-  pack_plan_image_kernel<<<chunks, 256, 0, s>>>(W, K, ep, wimg);
-  T2_LAUNCH_CHECK();
-  const size_t smem = gemm_smem_bytes();
-  T2_CUDA(cudaFuncSetAttribute(selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  selftest_kernel<<<1, kThreads, smem, s>>>(ximg, wimg, ep, chunks, C, N, ctrl);
-  T2_LAUNCH_CHECK();
-  T2_CUDA(cudaStreamSynchronize(s));
-  cudaFree(ximg); cudaFree(wimg); cudaFree(ctrl);
-  return T2_OK;
-}
-}  // namespace
-
-int selftest_umma(const float* A, const float* W, int N, int K, int passes, float* C, cudaStream_t s) {
-  (void)passes;
-  if (N % 8 != 0 || N < 8 || N > kHiCols || K % kChunkK != 0 || K <= 0)
-    return fail(T2_ERR_INVALID, "selftest_umma: N in {8..80 step 8}, K %% 64 == 0");
-  EventPlan ep; memset(&ep, 0, sizeof(ep));
-  plan_one_matrix(ep, N);
-  ep.chunks = K / kChunkK;
-  return selftest_plan(A, W, ep, K, C, s);
-}
-
-int selftest_event(const float* A, const float* W, const int* cons, int ncons, int K, float* C, cudaStream_t s) {
-  EventPlan ep; memset(&ep, 0, sizeof(ep));
-  if (ncons < 1 || ncons > 3 || K % kChunkK != 0 || K <= 0 || K > 16 * kChunkK)
-    return fail(T2_ERR_INVALID, "selftest_event: 1-3 consumers, K a multiple of 64 up to 1024");
-  for (int i = 0; i < ncons; ++i) { ep.n[i] = cons[i]; ep.nrows += cons[i]; }
-  ep.ncons = ncons; ep.w_bytes = (uint32_t)ep.nrows * 256; ep.chunks = K / kChunkK;
-  if (!event_plan_fits(ep, true))
-    return fail(T2_ERR_INVALID, "selftest_event: 1-3 consumers of 8, 16, 24 or 32 rows");
-  return selftest_plan(A, W, ep, K, C, s);
-}
-
-#endif  // T2_SELFTEST
-
-// ---------------------------------------------------------------------------------------------
-// Backward skinny GEMMs of the training path on the tensor cores (decoder_backward.cu, KB / KE):
-//   P[split][b][col] = inv_scale[b] * sum_{n in the split's chunks} dG_scaled[b][n] * Wcat[n][col]
-// dG (64 x 4096) arrives as a split-fp16 activation image whose rows were scaled by a power of two
-// (row maximum in [0.5, 1): gradients span many orders of magnitude, fp16 does not); Wcat = [W_ih | W_hh]
-// is streamed as W^T images (rows = output columns, K = gate rows).  Same ring / MMA / accumulator tile
-// as the forward events (run_event): a tile of output columns is planned as consumers of 32, 32 and 16 columns.
-// ---------------------------------------------------------------------------------------------
-namespace {
-constexpr int kBwdTileB = 80, kBwdTileE = 64;       // output columns per CTA: 2560 = 32 x 80, 1792 = 28 x 64
-
-__global__ void pack_bwd_wimg_kernel(const float* __restrict__ w0, int cols0, const float* __restrict__ w1, int cols1,
-                                     const BwdCta* __restrict__ plans, uint8_t* __restrict__ wimg) {
-  // grid (max chunks per CTA, n_cta): image block of chunk j of CTA c: rows = its output columns, k = 64 gate rows
-  const BwdCta& pc = plans[blockIdx.y];
-  const int j = blockIdx.x;
-  if (j >= pc.nchunks) return;
-  const int n = pc.ep.nrows;
-  __half* img = reinterpret_cast<__half*>(wimg + pc.ep.w_off + (size_t)j * pc.ep.w_bytes);
-  const int n0 = (pc.chunk0 + j) * kChunkK;
-  for (int i = threadIdx.x; i < n * kChunkK; i += blockDim.x) {
-    const int k = i / n, r = i - k * n;            // r fastest: coalesced along the weight matrix' columns
-    const int col = pc.col0 + r;
-    const float v = col < cols0 ? w0[(long)(n0 + k) * cols0 + col] : w1[(long)(n0 + k) * cols1 + (col - cols0)];
-    int hr, lr;
-    plan_image_rows(pc.ep, r, hr, lr);
-    __half h, l;
-    split_fp16(v, h, l);
-    img[img_elem_offset(hr, k)] = h;
-    img[img_elem_offset(lr, k)] = l;
-  }
-}
-
-__global__ void __launch_bounds__(kThreads, 1)
-bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w_img, const BwdCta* __restrict__ plans,
-                const float* __restrict__ inv_scale, float* __restrict__ P, int ldp, DecoderCtrl* ctrl) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const int tid = threadIdx.x;
-  const BwdCta pc = plans[blockIdx.x];
-  Carve sc(smem_raw, 1);
-  GemmSmem sm;
-  gemm_smem_layout(sc, &sm);
-  Ring rg;
-  rg.stage0 = sm.stage0;
-  rg.full = sm.bars; rg.empty = sm.bars + kStages;
-  float* s_acc = sm.acc;
-  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
-  rg.pol_x = ptx::policy_evict_last(); rg.pol_w = ptx::policy_evict_first();
-  rg.pre = 0; rg.ns = kStages;
-  if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
-    ptx::fence_barrier_init();
-  }
-  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;
-  __syncthreads();
-  run_event(rg, pc.ep, x_img + (size_t)pc.chunk0 * kXChunkBytes, w_img, pc.nchunks, s_acc, ctrl, nullptr);
-  const int N = pc.ep.nrows;
-  for (int i = tid; i < kRows * N; i += kThreads) {
-    const int row = i / N, c = i - row * N;
-    P[((size_t)pc.split * kRows + row) * ldp + pc.col0 + c] = s_acc[row * kAccPitch + c] * inv_scale[row];
-  }
-}
-
-}  // namespace
-
-int bwd_gemm_ctas(int which) { return which == 0 ? (2560 / kBwdTileB) * kBwdGemmSplit : (1792 / kBwdTileE) * kBwdGemmSplit; }
-
-namespace {
-constexpr int kBwdChunks = 4 * kARnn / kChunkK;                   // 64 K chunks
-int bwd_tile(int which) { return which == 0 ? kBwdTileB : kBwdTileE; }
-uint32_t bwd_w_bytes(int which) { return (uint32_t)(2 * bwd_tile(which) * kChunkK * 2); }
-
-std::vector<BwdCta> bwd_gemm_plans(int which) {
-  const int tile = bwd_tile(which), ntile = (which == 0 ? 2560 : 1792) / tile;
-  const uint32_t w_bytes = bwd_w_bytes(which);
-  std::vector<BwdCta> plans(ntile * kBwdGemmSplit);
-  for (int t = 0; t < ntile; ++t)
-    for (int sp = 0; sp < kBwdGemmSplit; ++sp) {
-      BwdCta& c = plans[t * kBwdGemmSplit + sp];
-      memset(&c, 0, sizeof(c));
-      c.chunk0 = sp * kBwdChunks / kBwdGemmSplit; c.nchunks = (sp + 1) * kBwdChunks / kBwdGemmSplit - c.chunk0;
-      c.col0 = t * tile; c.split = sp;
-      plan_one_matrix(c.ep, tile);    // 80 = 32 + 32 + 16, 64 = 32 + 32 columns (event_plan_fits(c.ep, false))
-      c.ep.col0 = 0; c.ep.chunks = c.nchunks;
-      c.ep.w_off = (uint32_t)(((size_t)t * kBwdChunks + c.chunk0) * w_bytes);
-    }
-  return plans;
-}
-}  // namespace
-
-size_t bwd_wimg_bytes(int which) { return (size_t)((which == 0 ? 2560 : 1792) / bwd_tile(which)) * kBwdChunks * bwd_w_bytes(which); }
-
-// packs the W^T images of both LSTMs from the caller's current fp32 weights into wimg[0 / 1] (bwd_wimg_bytes)
-int bwd_gemm_prepare(T2Model* m, uint8_t* const* wimg, cudaStream_t s) {
-  PersistentPack* pk = (PersistentPack*)m->pk;
-  if (!pk) return fail(T2_ERR_INVALID, "backward GEMM: model has no persistent pack");
-  for (int which = 0; which < 2; ++which) {
-    const float* w0 = m->w[which == 0 ? W_DRNN_WIH : W_ARNN_WIH];
-    const float* w1 = m->w[which == 0 ? W_DRNN_WHH : W_ARNN_WHH];
-    const int cols0 = which == 0 ? kARnn + kEnc : kPre + kEnc;
-    pack_bwd_wimg_kernel<<<dim3(kBwdChunks / kBwdGemmSplit, bwd_gemm_ctas(which)), 256, 0, s>>>(w0, cols0, w1, kARnn,
-                                                                                             pk->bwd_plans[which], wimg[which]);
-    T2_LAUNCH_CHECK();
-  }
-  return T2_OK;
-}
-
-int bwd_gemm_run(T2Model* m, int which, const uint8_t* w_img, const uint8_t* x_img, const float* inv_scale, float* P, int ldp,
-                 DecoderCtrl* ctrl, cudaStream_t s) {
-  PersistentPack* pk = (PersistentPack*)m->pk;
-  const size_t smem = gemm_smem_bytes();
-  T2_CUDA(cudaFuncSetAttribute(bwd_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  bwd_gemm_kernel<<<bwd_gemm_ctas(which), kThreads, smem, s>>>(x_img, w_img, pk->bwd_plans[which], inv_scale, P, ldp, ctrl);
-  T2_LAUNCH_CHECK();
   return T2_OK;
 }
 

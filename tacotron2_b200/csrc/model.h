@@ -26,10 +26,14 @@ struct T2Model {
 
   // ---- packed operands of the persistent decoder kernel (owned; see decoder_persistent.cu) ----
   void* pk = nullptr;            // opaque PersistentPack*
+  // ---- CTA plans of the decoder backward's skinny GEMMs (owned, device; see decoder_backward.cu) ----
+  void* bwd_plans = nullptr;     // opaque BwdCta[]
 };
 
 namespace t2 {
 int pack_model(T2Model* m, cudaStream_t s);          // (re)builds every packed copy
 int persistent_pack_create(T2Model* m, cudaStream_t s);
 void persistent_pack_destroy(T2Model* m);
+int backward_plans_create(T2Model* m, cudaStream_t s);
+void backward_plans_destroy(T2Model* m);
 }  // namespace t2

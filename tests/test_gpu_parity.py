@@ -37,21 +37,6 @@ def test_native_library_is_loaded():
     assert (info[1], info[2]) == (9, 0), "sm_90 device expected, got sm_%d%d" % (info[1], info[2])
 
 
-@pytest.mark.parametrize("passes,tol", [(3, 2e-5), (1, 2e-3)])
-@pytest.mark.parametrize("N,K", [(32, 256), (8, 64), (64, 1024), (80, 192), (48, 1024)])
-def test_umma_split_gemm_selftest(N, K, passes, tol):
-    """wgmma engine of the persistent decoder: C = 2 * A (64xK) . W (NxK)^T (two accumulating runs)."""
-    g = torch.Generator().manual_seed(N * 1000 + K)
-    A = torch.randn(64, K, generator=g).cuda()
-    W = (torch.randn(N, K, generator=g) / K ** 0.5).cuda()
-    Cd = torch.full((64, N), float("nan"), device="cuda")
-    _capi.check_selftest(_capi.selftest_lib().t2_selftest_umma(A.data_ptr(), W.data_ptr(), N, K, passes, Cd.data_ptr(),
-                                             C.c_void_p(torch.cuda.current_stream().cuda_stream)))
-    torch.cuda.synchronize()
-    ref = 2.0 * (A.double() @ W.double().t())
-    assert rel_err(Cd, ref) < tol
-
-
 @pytest.mark.parametrize("impl,impl_name", IMPLS)
 @pytest.mark.parametrize("name", INFER)
 def test_inference_matches_reference_golden(name, impl, impl_name):
