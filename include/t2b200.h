@@ -115,7 +115,8 @@ typedef struct T2EncoderArgs {
   int32_t training; const uint8_t* keep; uint64_t seed;
   float* memory;                       /* out (B, T, 512) */
   void* ws; size_t ws_bytes;
-  void* stash; size_t stash_bytes;     /* optional: activations kept for t2_encoder_backward (B <= 64) */
+  void* stash; size_t stash_bytes;     /* optional: activations kept for t2_encoder_backward (any B; needs
+                                          >= 128 SMs: the BiLSTM runs persistent, once per 64-row slice) */
 } T2EncoderArgs;
 size_t t2_encoder_workspace_bytes(const T2Model* m, int32_t B, int32_t T);
 int    t2_encoder_forward(T2Model* m, const T2EncoderArgs* a, void* stream);
@@ -129,7 +130,9 @@ int    t2_encoder_infer(T2Model* m, const T2EncoderArgs* a, void* stream);
 /* Encoder backward (autograd graph of Encoder.forward, model.py:173-190): the stash of a forward call with the same
  * text / embedded, lengths, training, keep and seed; d_memory (B, T, 512) -> gradients of the encoder parameters
  * (grads[] entries that are non-NULL are overwritten; with `text` also embedding.weight) and, if non-NULL,
- * d_embedded (B, T, 512). */
+ * d_embedded (B, T, 512).  Any B: the BiLSTM's reverse recurrence runs per 64-row slice, the conv stack's backward
+ * (BatchNorm over the whole batch) and the embedding gradient once.  The embedding gradient keeps the B x T symbol
+ * ids in shared memory: B * T <= 51,200 (e.g. B = 128 at T = 400), else T2_ERR_UNSUPPORTED. */
 typedef struct T2EncoderBwdArgs {
   const int64_t* text; const float* embedded; const int32_t* lengths; int32_t B, T;
   int32_t training; const uint8_t* keep; uint64_t seed;
@@ -235,7 +238,8 @@ int    t2_decoder_stream_collect(T2Model* m, const T2DecoderStreamArgs* a, const
 
 /* ---- Decoder backward (the autograd graph of Decoder.forward, model.py:381-416) ----------------
  * Reverse-time recurrence over the stash of a TEACHER run with the same memory / teacher_prenet / masks /
- * seed, then the time-batched weight gradients.  B <= 64.
+ * seed, then the time-batched weight gradients.  Any B >= 1: the recurrence runs its 64-row slices side by side
+ * (a row's phase-1 results do not depend on its slice), the weight gradients take all T_mel x B rows at once.
  *   d_mel (B, T_mel, 80), d_gate (B, T_mel): gradients wrt the mel / gate outputs (same layout as the
  *   outputs); d_align (B, T_mel, T_enc) or NULL.
  *   d_memory (B, T_enc, 512) and d_prenet (T_mel, B, 256) (gradient wrt teacher_prenet) are written.
@@ -601,9 +605,10 @@ int    t2_griffin_lim(T2Denoiser* h, const T2GriffinLimArgs* a, void* stream);
 
 /* ---- self tests (libt2b200_selftest.so only: the same sources built with -DT2_SELFTEST; not part of the product
  * library) -------------------------------------------------------------------------------------------------
- * t2_selftest_event: the wgmma split-fp16 event engine of the persistent decoder and the decoder backward, on an event
- * plan given as its consumers' row counts (consumers_host[0..n_consumers), host memory; 1-3 consumers of 16 or 32 rows),
- * run by the backward's skinny GEMM kernel: C (64 x N) = A (64 x K) . W (N x K)^T fp32 with N the sum of the rows, W's
+ * t2_selftest_event: the wgmma split-fp16 event engine's consumer plans and MMA chunk loop (event_mma, shared by the
+ * persistent decoder's events and the decoder backward), on an event plan given as its consumers' row counts
+ * (consumers_host[0..n_consumers), host memory; 1-3 consumers of 16 or 32 rows), run by the backward's skinny GEMM
+ * kernel with one 64-row slice: C (64 x N) = A (64 x K) . W (N x K)^T fp32 with N the sum of the rows, W's
  * rows in consumer order, K a multiple of 64 up to 1024. */
 #ifdef T2_SELFTEST
 int t2_selftest_event(const float* A, const float* W, const int32_t* consumers_host, int32_t n_consumers, int32_t K,

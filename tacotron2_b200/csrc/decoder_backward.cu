@@ -31,6 +31,7 @@ constexpr int kPBld = 1536 + 1024;   // [g_ah (1024) | g_ctx (512) | g_dh' (1024
 constexpr int kPEld = 768 + 1024;    // [g_x2 (256) | g_ctx' (512) | g_ah' (1024)]
 constexpr int kTaps = 2 * kLocK;     // 62 taps of the fused location filter
 constexpr int kColsLd = 64;
+constexpr int kBwdImgBytes = 64 * 16384;     // activation image of one 64-row slice of a (B x 4096) operand
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -42,9 +43,10 @@ __device__ __forceinline__ float warp_sum(float v) {
 // LSTMCell backward for one step (KA / KD).  grid B, block 1024: block = one batch row, thread = one hidden unit.
 // ---------------------------------------------------------------------------------------------
 struct LstmBwdArgs {
-  // g_h = sum over sources of sum_s src[(s * 64 + b) * ld + off + unit]  +  sum_o vec[b][o] * Wv[o][unit]
+  // g_h = sum over sources of sum_s src[(s * rows + b) * ld + off + unit]  +  sum_o vec[b][o] * Wv[o][unit]
   const float* src0; int ld0, off0, ns0;
   const float* src1; int ld1, off1, ns1;
+  int rows;                                // rows of one partial sum in src0 / src1 (64 per slice)
   const float* add; int ldadd;             // (B, >= 1024) direct term or null
   const float* vec; int nvec, ldvec;       // (B, nvec) rows, row stride ldvec
   const float* Wv; int ldwv;               // (nvec, >= 1024)
@@ -54,7 +56,7 @@ struct LstmBwdArgs {
   const float* c; const float* c_prev;     // (B, 1024)
   float* g_c;                              // (B, 1024) carry, in/out
   float* dG;                               // (B, 4096) out
-  uint8_t* img; float* inv_scale;          // scaled split-fp16 operand image of dG + 1/scale per row
+  uint8_t* img; float* inv_scale;          // scaled split-fp16 operand images of dG (one per 64 rows) + 1/scale per row
 };
 
 // The block knows the row maximum of dG, scales the row by a power of two into [0.5, 1) and writes it as the
@@ -69,11 +71,11 @@ __global__ void __launch_bounds__(1024) lstm_bwd_row_kernel(const LstmBwdArgs a)
   float g_h = a.add ? a.add[(long)b * a.ldadd + unit] : 0.f;
   if (a.src0) {
 #pragma unroll 4
-    for (int s = 0; s < a.ns0; ++s) g_h += a.src0[((long)s * 64 + b) * a.ld0 + a.off0 + unit];
+    for (int s = 0; s < a.ns0; ++s) g_h += a.src0[((long)s * a.rows + b) * a.ld0 + a.off0 + unit];
   }
   if (a.src1) {
 #pragma unroll 4
-    for (int s = 0; s < a.ns1; ++s) g_h += a.src1[((long)s * 64 + b) * a.ld1 + a.off1 + unit];
+    for (int s = 0; s < a.ns1; ++s) g_h += a.src1[((long)s * a.rows + b) * a.ld1 + a.off1 + unit];
   }
   {
     float p4[4] = {0.f, 0.f, 0.f, 0.f};
@@ -123,9 +125,9 @@ __global__ void __launch_bounds__(1024) lstm_bwd_row_kernel(const LstmBwdArgs a)
     const int k = g * 1024 + unit;
     __half h, l;
     split_fp16(d[g] * sc, h, l);
-    __half* hi = reinterpret_cast<__half*>(a.img + (size_t)(k >> 6) * 16384);
+    __half* hi = reinterpret_cast<__half*>(a.img + (size_t)(b >> 6) * kBwdImgBytes + (size_t)(k >> 6) * 16384);
     __half* lo = hi + 64 * kChunkK;
-    const uint32_t eo = img_elem_offset(b, k & 63);
+    const uint32_t eo = img_elem_offset(b & 63, k & 63);
     hi[eo] = h; lo[eo] = l;
   }
 }
@@ -133,14 +135,19 @@ __global__ void __launch_bounds__(1024) lstm_bwd_row_kernel(const LstmBwdArgs a)
 // ---------------------------------------------------------------------------------------------
 // Skinny GEMMs (KB / KE) on the tensor cores:
 //   P[split][b][col] = inv_scale[b] * sum_{n in the split's chunks} dG_scaled[b][n] * Wcat[n][col]
-// dG (64 x 4096) arrives as a split-fp16 activation image whose rows were scaled by a power of two
-// (row maximum in [0.5, 1): gradients span many orders of magnitude, fp16 does not); Wcat = [W_ih | W_hh]
-// is streamed as W^T images (rows = output columns, K = gate rows).  Same ring / MMA / accumulator tile
-// as the decoder's events (event_engine.cuh): a tile of output columns is planned as consumers of 32, 32 and 16 columns.
+// dG (B x 4096) arrives as S = ceil(B / 64) split-fp16 activation images of 64 rows each, whose rows were scaled by a
+// power of two (row maximum in [0.5, 1): gradients span many orders of magnitude, fp16 does not); Wcat = [W_ih | W_hh]
+// is streamed as W^T images (rows = output columns, K = gate rows).  Same stage format and MMA consumers as the
+// decoder's events (event_engine.cuh): a tile of output columns is planned as consumers of 32, 32 and 16 columns.
+// A stage holds one weight chunk and the matching K chunk of up to kBwdSlices activation images; every consumer
+// multiplies the weight chunk with all of them before the stage is released, so a step's weights cross L2 -> shared
+// memory once per kBwdSlices slices.  Each slice has its own accumulators and sees the MMAs in the order of a one-slice
+// launch: a row's partial sums do not depend on which slice it sits in.
 // which = 0: decoder LSTM (2560 columns), 1: attention LSTM (1792 columns); K = 4096 gate rows in kBwdGemmSplit partial sums.
 // ---------------------------------------------------------------------------------------------
 constexpr int kBwdGemmSplit = 4;
-constexpr int kBwdImgBytes = 64 * 16384;            // activation image of one (64 x 4096) operand
+constexpr int kBwdSlices = 2;                       // 64-row slices per CTA: 2 x 32 accumulator registers per consumer
+constexpr int kBwdStageBytes = kBwdSlices * kXChunkBytes + kWStageMax;   // [X slice 0 | X slice 1 | W] = 52 KiB
 constexpr int kBwdTileB = 80, kBwdTileE = 64;       // output columns per CTA: 2560 = 32 x 80, 1792 = 28 x 64
 constexpr int kBwdChunks = 4 * kARnn / kChunkK;     // 64 K chunks
 
@@ -173,33 +180,96 @@ __global__ void pack_bwd_wimg_kernel(const float* __restrict__ w0, long ld0, lon
   }
 }
 
+struct BwdSmem { uint8_t* stage0; uint64_t* bars; };   // kStages stages of kBwdStageBytes, then full / empty barriers
+__host__ __device__ __forceinline__ void bwd_smem_layout(Carve& c, BwdSmem* s) {
+  s->stage0 = c.take<uint8_t>((size_t)kStages * kBwdStageBytes, 1);
+  s->bars = c.take<uint64_t>(2 * kStages, 8);
+}
+size_t bwd_smem_bytes() { Carve c(nullptr, 1); BwdSmem s; bwd_smem_layout(c, &s); return c.bytes(); }
+
+// One MMA warpgroup's consumer: the engine's chunk loop (event_mma) over the NSL slices of each stage; then P row
+// (slice0 + s) * 64 + r = (both column halves of D_s) * inv_scale of that row.
+template <int N, int NSL>
+__device__ __forceinline__ void bwd_consumer(uint8_t* stage0, uint64_t* full, uint64_t* empty, int chunks,
+                                             uint32_t w_row0, DecoderCtrl* ctrl, float* P, int ldp, int col, int rows0,
+                                             const float* inv_scale) {
+  float d[NSL][N / 2];
+#pragma unroll
+  for (int s = 0; s < NSL; ++s)
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[s][i] = 0.f;
+  uint32_t st = 0, ph = 0;
+  event_mma<N, NSL>(stage0, kBwdStageBytes, kBwdSlices * kXChunkBytes, kStages, full, empty, st, ph, chunks, w_row0, ctrl, d);
+  const int wt = threadIdx.x & 127;
+#pragma unroll
+  for (int s = 0; s < NSL; ++s) {
+#pragma unroll
+    for (int j = 0; j < N / 4; ++j) {   // registers [0, N/4) hold the W_hi columns, [N/4, N/2) the W_lo ones
+      const int row = rows0 + s * kRows + ptx::wg_frag_row(j, wt);
+      float v = 0.f;                    // the accumulator tile of the one-slice engine starts at zero
+      v += d[s][j] + d[s][N / 4 + j];
+      P[(size_t)row * ldp + col + ptx::wg_frag_col(j, wt)] = v * inv_scale[row];
+    }
+  }
+}
+
+// grid (CTA plans, slice groups of kBwdSlices); x_img / inv_scale / P rows: nslices images of 64 rows, P = (split, 64 x
+// nslices rows, ldp)
 __global__ void __launch_bounds__(kThreads, 1)
-bwd_gemm_kernel(const uint8_t* __restrict__ x_img, const uint8_t* __restrict__ w_img, const BwdCta* __restrict__ plans,
+bwd_gemm_kernel(const uint8_t* __restrict__ x_img, int nslices, const uint8_t* __restrict__ w_img, const BwdCta* __restrict__ plans,
                 const float* __restrict__ inv_scale, float* __restrict__ P, int ldp, DecoderCtrl* ctrl) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const int tid = threadIdx.x;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const BwdCta pc = plans[blockIdx.x];
+  const int slice0 = blockIdx.y * kBwdSlices, nsl = min(kBwdSlices, nslices - slice0);
   Carve sc(smem_raw, 1);
-  GemmSmem sm;
-  gemm_smem_layout(sc, &sm);
-  Ring rg;
-  rg.stage0 = sm.stage0;
-  rg.full = sm.bars; rg.empty = sm.bars + kStages;
-  float* s_acc = sm.acc;
-  rg.p_stage = rg.p_phase = rg.c_stage = rg.c_phase = 0;
-  rg.pol_x = ptx::policy_evict_last(); rg.pol_w = ptx::policy_evict_first();
-  rg.pre = 0; rg.ns = kStages;
+  BwdSmem sm;
+  bwd_smem_layout(sc, &sm);
+  uint64_t* full = sm.bars;
+  uint64_t* empty = sm.bars + kStages;
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&rg.full[s], 1); ptx::mbar_init(&rg.empty[s], kMmaWgs); }
+    for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], kMmaWgs); }
     ptx::fence_barrier_init();
   }
-  for (int i = tid; i < kRows * kAccPitch; i += kThreads) s_acc[i] = 0.f;
   __syncthreads();
-  run_event(rg, pc.ep, x_img + (size_t)pc.chunk0 * kXChunkBytes, w_img, pc.nchunks, s_acc, ctrl, nullptr);
-  const int N = pc.ep.nrows;
-  for (int i = tid; i < kRows * N; i += kThreads) {
-    const int row = i / N, c = i - row * N;
-    P[((size_t)pc.split * kRows + row) * ldp + pc.col0 + c] = s_acc[row * kAccPitch + c] * inv_scale[row];
+  const EventPlan& ep = pc.ep;
+  if (warp == 0) {
+    if (tid == 0) {
+      const uint64_t pol_x = ptx::policy_evict_last(), pol_w = ptx::policy_evict_first();
+      uint32_t st = 0, ph = 0;
+      for (int i = 0; i < pc.nchunks; ++i) {
+        uint8_t* stage = sm.stage0 + (size_t)st * kBwdStageBytes;
+        mbar_wait(&empty[st], ph ^ 1, ctrl, 200);
+        ptx::mbar_arrive_expect_tx(&full[st], nsl * kXChunkBytes + ep.w_bytes);
+        ptx::bulk_g2s_hint(stage + kBwdSlices * kXChunkBytes, w_img + ep.w_off + (size_t)i * ep.w_bytes, ep.w_bytes, &full[st], pol_w);
+        for (int s = 0; s < nsl; ++s)
+          ptx::bulk_g2s_hint(stage + s * kXChunkBytes, x_img + (size_t)(slice0 + s) * kBwdImgBytes + (size_t)(pc.chunk0 + i) * kXChunkBytes,
+                             kXChunkBytes, &full[st], pol_x);
+        if (++st == kStages) { st = 0; ph ^= 1; }
+      }
+    }
+  } else if (warp >= 4) {
+    const int c = (warp >> 2) - 1;        // this warpgroup's consumer
+    if (c < ep.ncons) {
+      int w_row0 = 0, col = pc.col0;
+      for (int i = 0; i < c; ++i) { w_row0 += 2 * ep.n[i]; col += ep.n[i]; }
+      float* Ps = P + (size_t)pc.split * nslices * kRows * ldp;
+      const int r0 = slice0 * kRows;    // one copy per consumer width and slice count: no branch between the MMAs
+      if (ep.n[c] == 32) {
+        if (nsl == 2) bwd_consumer<64, 2>(sm.stage0, full, empty, pc.nchunks, w_row0, ctrl, Ps, ldp, col, r0, inv_scale);
+        else bwd_consumer<64, 1>(sm.stage0, full, empty, pc.nchunks, w_row0, ctrl, Ps, ldp, col, r0, inv_scale);
+      } else {
+        if (nsl == 2) bwd_consumer<32, 2>(sm.stage0, full, empty, pc.nchunks, w_row0, ctrl, Ps, ldp, col, r0, inv_scale);
+        else bwd_consumer<32, 1>(sm.stage0, full, empty, pc.nchunks, w_row0, ctrl, Ps, ldp, col, r0, inv_scale);
+      }
+    } else {                              // no rows for this warpgroup: it still releases every stage it was counted for
+      uint32_t st = 0, ph = 0;
+      for (int i = 0; i < pc.nchunks; ++i) {
+        mbar_wait(&full[st], ph, ctrl, 201);
+        if ((tid & 127) == 0) ptx::mbar_arrive(&empty[st]);
+        if (++st == kStages) { st = 0; ph ^= 1; }
+      }
+    }
   }
 }
 
@@ -241,12 +311,13 @@ int bwd_gemm_prepare(T2Model* m, uint8_t* const* wimg, cudaStream_t s) {
   return T2_OK;
 }
 
-// one launch of the n_cta CTAs of `plans` (device)
-int bwd_gemm_run(const BwdCta* plans, int n_cta, const uint8_t* w_img, const uint8_t* x_img, const float* inv_scale, float* P,
-                 int ldp, DecoderCtrl* ctrl, cudaStream_t s) {
-  const size_t smem = gemm_smem_bytes();
+// one launch of the n_cta CTAs of `plans` (device) over the nslices 64-row images of x_img
+int bwd_gemm_run(const BwdCta* plans, int n_cta, const uint8_t* w_img, const uint8_t* x_img, int nslices, const float* inv_scale,
+                 float* P, int ldp, DecoderCtrl* ctrl, cudaStream_t s) {
+  const size_t smem = bwd_smem_bytes();
   T2_CUDA(cudaFuncSetAttribute(bwd_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  bwd_gemm_kernel<<<n_cta, kThreads, smem, s>>>(x_img, w_img, plans, inv_scale, P, ldp, ctrl);
+  bwd_gemm_kernel<<<dim3(n_cta, (nslices + kBwdSlices - 1) / kBwdSlices), kThreads, smem, s>>>(x_img, nslices, w_img, plans, inv_scale,
+                                                                                              P, ldp, ctrl);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }
@@ -263,6 +334,7 @@ struct AttBwdArgs {
   const float* d_align;                   // (B,T,Te) or null
   const float* PE; const float* PB;       // partials of step t+1 (KE) and of this step (KB)
   int nsE, nsB;                           // number of partial sums in PE / PB
+  int rows;                               // rows of one partial sum (64 per slice)
   const float* gproj;                     // (T,B,1536) = [d_mel_t ; d_gate_t] . W_PG, all steps (time batched)
   const float* weffT;                     // (62, 128) transposed fused location filter
   float* dctx; float* dx2; float* dq;     // (T,B,512), (T,B,256), (T,B,128)
@@ -318,17 +390,17 @@ __global__ void __launch_bounds__(kAttT) att_bwd_kernel(const AttBwdArgs a) {
     float g = a.gproj[((long)t * B + b) * 1536 + 1024 + c];
     if (a.carry) {
 #pragma unroll 5
-      for (int s = 0; s < a.nsE; ++s) g += a.PE[((long)s * 64 + b) * kPEld + 256 + c];
+      for (int s = 0; s < a.nsE; ++s) g += a.PE[((long)s * a.rows + b) * kPEld + 256 + c];
     }
 #pragma unroll 4
-    for (int s = 0; s < a.nsB; ++s) g += a.PB[((long)s * 64 + b) * kPBld + 1024 + c];
+    for (int s = 0; s < a.nsB; ++s) g += a.PB[((long)s * a.rows + b) * kPBld + 1024 + c];
     s_ctx[c] = g;
     if (h == 0) a.dctx[((long)t * B + b) * 512 + c] = g;
   }
   if (h == 0 && a.carry && tid < 256) {   // gradient wrt the prenet output of step t+1 (first 256 columns of KE's result)
     float g = 0.f;
 #pragma unroll 5
-    for (int s = 0; s < a.nsE; ++s) g += a.PE[((long)s * 64 + b) * kPEld + tid];
+    for (int s = 0; s < a.nsE; ++s) g += a.PE[((long)s * a.rows + b) * kPEld + tid];
     a.dx2[((long)(t + 1) * B + b) * 256 + tid] = g;
   }
   __syncthreads();
@@ -515,11 +587,11 @@ __global__ void im2col_kernel(const float* __restrict__ align, const float* __re
   }
   cols[i] = v;
 }
-__global__ void reduce_pe_x2_kernel(const float* __restrict__ PE, float* __restrict__ dx2, int B, int nsE) {
+__global__ void reduce_pe_x2_kernel(const float* __restrict__ PE, float* __restrict__ dx2, int B, int nsE, int rows) {
   const int b = blockIdx.x, c = threadIdx.x;   // step 0: g_x2 = sum of the partials
   if (b >= B) return;
   float g = 0.f;
-  for (int s = 0; s < nsE; ++s) g += PE[((long)s * 64 + b) * kPEld + c];
+  for (int s = 0; s < nsE; ++s) g += PE[((long)s * rows + b) * kPEld + c];
   dx2[(long)b * 256 + c] = g;
 }
 __global__ void fill_kernel(float* p, float v, long n) {
@@ -547,23 +619,26 @@ struct BwdWs {
   void* gemm; size_t gemm_bytes;       // scratch of the gemm_tc products and column sums, shared in stream order
   WgradWs wg;
 };
+// 64-row slices of the reverse recurrence; per-row buffers of phase 1 hold all of their rows
+int bwd_slices(int B) { return (B + kRows - 1) / kRows; }
 void bwd_ws_layout(Carve& c, int B, int Te, int T, BwdWs* w) {
   const size_t TB = (size_t)T * B;
+  const int S = bwd_slices(B), R = S * kRows;
   w->dga = c.take<float>(TB * 4096); w->dgd = c.take<float>(TB * 4096);
   w->q = c.take<float>(TB * 128); w->dq = c.take<float>(TB * 128);
   w->awc = c.take<float>((size_t)B * T * Te);
   w->pm = c.take<float>((size_t)B * Te * 128); w->dpm = c.take<float>((size_t)B * Te * 128);
   w->dctx = c.take<float>(TB * 512); w->dy = c.take<float>(TB * 81);
   w->gs = c.take<float>(TB * Te * 128); w->cols = c.take<float>(TB * Te * kColsLd);
-  w->pb = c.take<float>((size_t)kBwdGemmSplit * 64 * kPBld); w->pe = c.take<float>((size_t)kBwdGemmSplit * 64 * kPEld);
-  w->gdc = c.take<float>((size_t)64 * 1024); w->gac = c.take<float>((size_t)64 * 1024);
+  w->pb = c.take<float>((size_t)kBwdGemmSplit * R * kPBld); w->pe = c.take<float>((size_t)kBwdGemmSplit * R * kPEld);
+  w->gdc = c.take<float>((size_t)R * 1024); w->gac = c.take<float>((size_t)R * 1024);
   w->cacc = c.take<float>((size_t)2 * B * Te); w->gcat = c.take<float>((size_t)2 * 2 * B * 2 * Te);
   w->dv = c.take<float>((size_t)B * 128);
   w->weff = c.take<float>((size_t)kAtt * kTaps); w->dweff = c.take<float>((size_t)kAtt * kColsLd);
   w->tmp = c.take<float>(4096);
   w->gproj = c.take<float>(TB * 1536); w->weffT = c.take<float>((size_t)kAtt * kTaps);
-  w->inv_scale = c.take<float>(128);
-  w->img_d = c.take<uint8_t>(kBwdImgBytes, 1024); w->img_a = c.take<uint8_t>(kBwdImgBytes, 1024);
+  w->inv_scale = c.take<float>((size_t)2 * R);     // rows of the dG_dec images, then those of the dG_att images
+  w->img_d = c.take<uint8_t>((size_t)S * kBwdImgBytes, 1024); w->img_a = c.take<uint8_t>((size_t)S * kBwdImgBytes, 1024);
   w->ctrl = c.take<DecoderCtrl>(1);
   for (int i = 0; i < 2; ++i) w->bwd_wimg[i] = c.take<uint8_t>(bwd_wimg_bytes(i), 1024);
   const int BTe = B * Te, TBi = (int)TB;
@@ -574,7 +649,7 @@ void bwd_ws_layout(Carve& c, int B, int Te, int T, BwdWs* w) {
                             gemm_tc_ws_bytes(kAtt, kColsLd, (int)(TB * Te)), colsum_ws_bytes(T, BTe * kAtt),
                             gemm_tc_ws_bytes(kAtt, kEnc, BTe), gemm_tc_ws_bytes(BTe, kEnc, kAtt), gemm_tc_ws_bytes(Te, kEnc, T, B)});
   w->gemm = c.take<char>(w->gemm_bytes);
-  wgrad_tc_layout(c, T, &w->wg);
+  wgrad_tc_layout(c, B, T, &w->wg);
 }
 
 }  // namespace
@@ -605,8 +680,7 @@ size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel) {
 
 int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   const int B = a->B, Te = a->T_enc, T = a->T_mel;
-  if (B < 1 || B > 64) return fail(T2_ERR_UNSUPPORTED, "decoder backward: 1 <= B <= 64 (got %d)", B);
-  if (Te < 1 || T < 1) return fail(T2_ERR_INVALID, "decoder backward: bad sizes");
+  if (B < 1 || Te < 1 || T < 1) return fail(T2_ERR_INVALID, "decoder backward: bad sizes");
   const size_t smem = att_bwd_smem(Te);
   if (smem > 220 * 1024) return fail(T2_ERR_UNSUPPORTED, "decoder backward: T_enc = %d too long for the attention kernel", Te);
   if (a->n_grads != W_COUNT) return fail(T2_ERR_INVALID, "decoder backward: expected %d gradient pointers", (int)W_COUNT);
@@ -619,12 +693,13 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   Carve wc(a->ws, 1024);
   bwd_ws_layout(wc, B, Te, T, &w);
   const size_t TB = (size_t)T * B;
+  const int S = bwd_slices(B), R = S * kRows;
   const int training = a->training;
   const float p_att = m->cfg.p_attention_dropout, p_dec = m->cfg.p_decoder_dropout;
 
   // ---- set-up -------------------------------------------------------------------------------------
-  T2_CUDA(cudaMemsetAsync(w.gdc, 0, (size_t)64 * 1024 * 4, s));
-  T2_CUDA(cudaMemsetAsync(w.gac, 0, (size_t)64 * 1024 * 4, s));
+  T2_CUDA(cudaMemsetAsync(w.gdc, 0, (size_t)R * 1024 * 4, s));
+  T2_CUDA(cudaMemsetAsync(w.gac, 0, (size_t)R * 1024 * 4, s));
   T2_CUDA(cudaMemsetAsync(w.dv, 0, (size_t)B * 128 * 4, s));
   T2_CUDA(cudaMemsetAsync(w.cacc, 0, (size_t)2 * B * Te * 4, s));
   T2_CUDA(cudaMemsetAsync(w.gcat, 0, (size_t)8 * B * Te * 4, s));
@@ -649,10 +724,10 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
   T2_CUDA(cudaFuncSetAttribute(att_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // skinny GEMMs (KB / KE): weight images, zeroed operand images, control block and unit scales
   T2_TRY(bwd_gemm_prepare(m, w.bwd_wimg, s));
-  T2_CUDA(cudaMemsetAsync(w.img_d, 0, kBwdImgBytes, s));      // rows >= B stay zero
-  T2_CUDA(cudaMemsetAsync(w.img_a, 0, kBwdImgBytes, s));
+  T2_CUDA(cudaMemsetAsync(w.img_d, 0, (size_t)S * kBwdImgBytes, s));      // rows >= B stay zero
+  T2_CUDA(cudaMemsetAsync(w.img_a, 0, (size_t)S * kBwdImgBytes, s));
   T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
-  fill_kernel<<<1, 128, 0, s>>>(w.inv_scale, 1.f, 128);
+  fill_kernel<<<(2 * R + 127) / 128, 128, 0, s>>>(w.inv_scale, 1.f, 2 * R);
   T2_LAUNCH_CHECK();
   // ---- phase 1: reverse-time recurrence ---------------------------------------------------------------
   for (int t = T - 1; t >= 0; --t) {
@@ -660,7 +735,7 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
     {  // KA
       LstmBwdArgs k;
       memset(&k, 0, sizeof(k));
-      k.src0 = carry ? w.pb : nullptr; k.ld0 = kPBld; k.off0 = 1536; k.ns0 = kBwdGemmSplit;
+      k.src0 = carry ? w.pb : nullptr; k.ld0 = kPBld; k.off0 = 1536; k.ns0 = kBwdGemmSplit; k.rows = R;
       k.add = w.gproj + (size_t)t * B * 1536; k.ldadd = 1536;
       k.img = w.img_d; k.inv_scale = w.inv_scale;
       k.keep = a->dec_keep ? a->dec_keep + (size_t)t * B * kDRnn : nullptr;
@@ -670,14 +745,14 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
       lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(bwd_gemm_run(bwd_plans(m, 0), bwd_gemm_ctas(0), w.bwd_wimg[0], w.img_d, w.inv_scale, w.pb, kPBld, w.ctrl, s));   // KB
+    T2_TRY(bwd_gemm_run(bwd_plans(m, 0), bwd_gemm_ctas(0), w.bwd_wimg[0], w.img_d, S, w.inv_scale, w.pb, kPBld, w.ctrl, s));   // KB
     {  // KC
       AttBwdArgs k;
       memset(&k, 0, sizeof(k));
       k.t = t; k.T = T; k.B = B; k.Te = Te; k.carry = carry; k.len = a->memory_lengths;
       k.memory = a->memory; k.pm = w.pm; k.q = w.q; k.v = m->w[W_ATT_V]; k.weff = w.weff;
       k.align = a->align; k.awc = w.awc; k.d_align = a->d_align;
-      k.PE = w.pe; k.PB = w.pb; k.nsE = kBwdGemmSplit; k.nsB = kBwdGemmSplit; k.gproj = w.gproj; k.weffT = w.weffT;
+      k.PE = w.pe; k.PB = w.pb; k.nsE = kBwdGemmSplit; k.nsB = kBwdGemmSplit; k.rows = R; k.gproj = w.gproj; k.weffT = w.weffT;
       k.dctx = w.dctx; k.dx2 = a->d_prenet; k.dq = w.dq; k.gs = w.gs; k.gcat = w.gcat; k.cacc = w.cacc; k.dv = w.dv;
       att_bwd_kernel<<<dim3(2, B), kAttT, smem, s>>>(k);
       T2_LAUNCH_CHECK();
@@ -686,8 +761,8 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
       LstmBwdArgs k;
       memset(&k, 0, sizeof(k));
       k.src0 = carry ? w.pe : nullptr; k.ld0 = kPEld; k.off0 = 768; k.ns0 = kBwdGemmSplit;
-      k.src1 = w.pb; k.ld1 = kPBld; k.off1 = 0; k.ns1 = kBwdGemmSplit;
-      k.img = w.img_a; k.inv_scale = w.inv_scale + 64;
+      k.src1 = w.pb; k.ld1 = kPBld; k.off1 = 0; k.ns1 = kBwdGemmSplit; k.rows = R;
+      k.img = w.img_a; k.inv_scale = w.inv_scale + R;
       k.vec = w.dq + (size_t)t * B * 128; k.nvec = 128; k.ldvec = 128; k.Wv = m->w[W_ATT_QUERY]; k.ldwv = kARnn;
       k.keep = a->att_keep ? a->att_keep + (size_t)t * B * kARnn : nullptr;
       k.dropout = training; k.seed = a->seed; k.site = (uint32_t)(t * 4 + 2); k.p = p_att;
@@ -696,9 +771,9 @@ int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s) {
       lstm_bwd_row_kernel<<<B, 1024, 0, s>>>(k);
       T2_LAUNCH_CHECK();
     }
-    T2_TRY(bwd_gemm_run(bwd_plans(m, 1), bwd_gemm_ctas(1), w.bwd_wimg[1], w.img_a, w.inv_scale + 64, w.pe, kPEld, w.ctrl, s));   // KE
+    T2_TRY(bwd_gemm_run(bwd_plans(m, 1), bwd_gemm_ctas(1), w.bwd_wimg[1], w.img_a, S, w.inv_scale + R, w.pe, kPEld, w.ctrl, s));   // KE
   }
-  reduce_pe_x2_kernel<<<B, 256, 0, s>>>(w.pe, a->d_prenet, B, kBwdGemmSplit);
+  reduce_pe_x2_kernel<<<B, 256, 0, s>>>(w.pe, a->d_prenet, B, kBwdGemmSplit, R);
   T2_LAUNCH_CHECK();
 
   // ---- phase 2: time-batched gradients --------------------------------------------------------------------
@@ -844,7 +919,7 @@ int selftest_event(const float* A, const float* W, const int* cons, int ncons, i
   T2_LAUNCH_CHECK();
   pack_bwd_wimg_kernel<<<dim3(chunks, 1), 256, 0, s>>>(W, 1, K, N, nullptr, 0, plan, wimg);     // Wcat = W^T
   T2_LAUNCH_CHECK();
-  T2_TRY(bwd_gemm_run(plan, 1, wimg, ximg, ones, C, N, ctrl, s));
+  T2_TRY(bwd_gemm_run(plan, 1, wimg, ximg, 1, ones, C, N, ctrl, s));
   T2_CUDA(cudaStreamSynchronize(s));
   cudaFree(buf);
   return T2_OK;

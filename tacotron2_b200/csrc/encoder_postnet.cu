@@ -205,9 +205,11 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per
   const int B = a->B, T = a->T;
   if (B <= 0 || T <= 0) return fail(T2_ERR_INVALID, "encoder: empty batch");
   if (a->ws_bytes < encoder_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder workspace too small");
-  const bool persistent = B <= 64 && m->sm_count >= 128;      // the BiLSTM as one cooperative launch
+  // the BiLSTM as one cooperative launch per 64-row slice (pack_padded_sequence runs each row on its own, so slicing the
+  // recurrence is exact); only the training stash takes it above 64 rows
+  const bool persistent = (B <= 64 || a->stash) && m->sm_count >= 128;
   if (a->stash && !persistent)
-    return fail(T2_ERR_UNSUPPORTED, "encoder: the training stash needs B <= 64 and >= 128 SMs (persistent BiLSTM kernel)");
+    return fail(T2_ERR_UNSUPPORTED, "encoder: the training stash needs >= 128 SMs (persistent BiLSTM kernel)");
   Carve cv(a->ws);
   EncoderWs w;
   encoder_ws_layout(cv, B, T, &w);
@@ -246,18 +248,27 @@ int encoder_forward(T2Model* m, const T2EncoderArgs* a, cudaStream_t s, bool per
   T2_CUDA(cudaMemsetAsync(hin, 0, (size_t)2 * B * kEncH * 4, s));
   T2_CUDA(cudaMemsetAsync(w.c, 0, (size_t)2 * B * kEncH * 4, s));
   if (persistent) {
-    // persistent recurrence: one cooperative launch for all T steps of both directions
-    T2_CUDA(cudaMemsetAsync(hout, 0, (size_t)2 * B * kEncH * 4, s));
-    T2_CUDA(cudaMemsetAsync(w.lctrl, 0, sizeof(EncLstmCtrl), s));
-    float* hb = w.h;
+    // persistent recurrence: one cooperative launch for all T steps of both directions of a slice's rows
     const size_t psm = (size_t)(kEncH * 16 + kEncH * 64) * sizeof(float);
     T2_CUDA(cudaFuncSetAttribute(enc_lstm_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     const float* whf = m->w[W_ENC_LSTM + 1]; const float* whr = m->w[W_ENC_LSTM + 5];
-    const int32_t* lens = a->lengths; float* mem = a->memory; int Bv = B, Tv = T;
-    void* args[] = {(void*)&w.gin, (void*)&whf, (void*)&whr, (void*)&hb, (void*)&mem, (void*)&lens, (void*)&Bv, (void*)&Tv, (void*)&w.lctrl,
-                    (void*)&st_gates, (void*)&st_c};
-    T2_CUDA(cudaLaunchCooperativeKernel((void*)enc_lstm_persistent_kernel, dim3(128), dim3(256), args, psm, s));
-    g_launch_count++;
+    float* hb = w.h;
+    int Tv = T;
+    for (int b0 = 0; b0 < B; b0 += 64) {
+      int Bv = B - b0 < 64 ? B - b0 : 64;
+      if (b0 > 0) T2_CUDA(cudaMemsetAsync(hin, 0, (size_t)2 * Bv * kEncH * 4, s));
+      T2_CUDA(cudaMemsetAsync(w.h + (size_t)2 * Bv * kEncH, 0, (size_t)2 * Bv * kEncH * 4, s));   // (2 buffers, 2 dirs, Bv, 256)
+      T2_CUDA(cudaMemsetAsync(w.lctrl, 0, sizeof(EncLstmCtrl), s));
+      const float* gin = w.gin + (size_t)b0 * T * 8 * kEncH;
+      float* mem = a->memory + (size_t)b0 * T * kEnc;
+      const int32_t* lens = a->lengths ? a->lengths + b0 : nullptr;
+      float* sg = st_gates ? st_gates + (size_t)b0 * T * 8 * kEncH : nullptr;
+      float* sc = st_c ? st_c + (size_t)b0 * T * kEnc : nullptr;
+      void* args[] = {(void*)&gin, (void*)&whf, (void*)&whr, (void*)&hb, (void*)&mem, (void*)&lens, (void*)&Bv, (void*)&Tv,
+                      (void*)&w.lctrl, (void*)&sg, (void*)&sc};
+      T2_CUDA(cudaLaunchCooperativeKernel((void*)enc_lstm_persistent_kernel, dim3(128), dim3(256), args, psm, s));
+      g_launch_count++;
+    }
     if (a->stash) T2_TRY(encoder_stash_output(a, s));
     return T2_OK;
   }

@@ -1,5 +1,6 @@
-// The streaming "event" engine of the persistent decoder (decoder_persistent.cu) and the training backward's skinny GEMMs
-// (decoder_backward.cu): a CTA of 512 threads streams K chunks of a split-fp16 activation image [X_hi | X_lo] together
+// The streaming "event" engine of the persistent decoder (decoder_persistent.cu), whose consumer plans, operand images
+// and stage format the training backward's skinny GEMMs (decoder_backward.cu) share; those run their own ring, whose
+// stages carry the activation chunks of two 64-row slices.  A CTA of 512 threads streams K chunks of a split-fp16 activation image [X_hi | X_lo] together
 // with its weight rows through a shared-memory ring (bulk async copies issued by thread 0), and MMA warpgroups 1-3 each
 // multiply one consumer's [W_hi; W_lo] rows with both activation planes and add the product to an fp32 accumulator tile
 // in shared memory.
@@ -57,15 +58,6 @@ struct Ring {
   uint32_t ns;                 // number of stages
 };
 
-// Dynamic shared memory of the backward GEMMs: ring stages, barriers, then the accumulator tile
-struct GemmSmem { uint8_t* stage0; uint64_t* bars; float* acc; };
-__host__ __device__ __forceinline__ void gemm_smem_layout(Carve& c, GemmSmem* s) {
-  s->stage0 = c.take<uint8_t>((size_t)kStages * kStageBytes, 1);
-  s->bars = c.take<uint64_t>(16, 1);
-  s->acc = c.take<float>(kAccBytes / 4, 1);      // [64][kAccPitch]
-}
-inline size_t gemm_smem_bytes() { Carve c(nullptr, 1); GemmSmem s; gemm_smem_layout(c, &s); return c.bytes(); }
-
 // Weight chunks do not depend on the grid barrier that separates two events (only the activation does):
 // the producer arms the first kStages stages of the NEXT event and issues their weight copies right after
 // the current event's last chunk, so their L2 / HBM latency overlaps the epilogue and the barrier.
@@ -115,39 +107,56 @@ __device__ __forceinline__ void plan_image_rows(const EventPlan& ep, int r, int&
   hi = lo = 0;
 }
 
-// One MMA warpgroup's consumer of an event: D (64 x 2n) = X_hi . B^T + X_lo . B^T over all `chunks` stages, where B is
-// the consumer's 2n weight-image rows [W_hi; W_lo] from row w_row0 of each stage; then both column halves of D are
-// added to the accumulator tile from column acol.  Each chunk's stage is released as soon as its MMAs are done: keeping
-// a commit group in flight across chunks would hold every stage one chunk longer, i.e. make the ring one stage shallower
-// for the producer, and the stream waits on L2 latency rather than on the tensor core (measured slower).
-template <int N>
-__device__ __forceinline__ void event_wg(Ring& rg, int chunks, uint32_t w_row0, float* s_acc, int acol, DecoderCtrl* ctrl) {
+// The chunk loop of one MMA warpgroup's consumer, shared by the decoder's events (NSL = 1) and the training backward's
+// skinny GEMMs (NSL = 1 or 2 activation slices per stage): for each of `chunks` stages, D_s (64 x 2n) += X_s,hi . B^T +
+// X_s,lo . B^T for every slice s, where X_s is the activation chunk at stage offset s x kXChunkBytes and B is the consumer's
+// 2n weight-image rows [W_hi; W_lo] from row w_row0 of the weights at stage offset w_base.  Every slice sees its MMAs in
+// the order of a one-slice event.  Each chunk's stage is released as soon as its MMAs are done: keeping a commit group in
+// flight across chunks would hold every stage one chunk longer, i.e. make the ring one stage shallower for the producer,
+// and the stream waits on L2 latency rather than on the tensor core (measured slower).
+template <int N, int NSL>
+__device__ __forceinline__ void event_mma(uint8_t* stage0, uint32_t stage_bytes, uint32_t w_base, uint32_t ns, uint64_t* full,
+                                          uint64_t* empty, uint32_t& c_stage, uint32_t& c_phase, int chunks, uint32_t w_row0,
+                                          DecoderCtrl* ctrl, float (&d)[NSL][N / 2]) {
   const bool leader = (threadIdx.x & 127) == 0;
-  float d[N / 2];
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
   for (int i = 0; i < chunks; ++i) {
-    mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
-    const uint32_t xs = ptx::smem_u32(rg.stage(rg.c_stage));
-    const uint32_t ws = xs + kXChunkBytes + w_row0 * 128;
-    ptx::wg_fence_regs<N / 2>(d);
+    mbar_wait(&full[c_stage], c_phase, ctrl, 201);
+    const uint32_t xs = ptx::smem_u32(stage0 + c_stage * stage_bytes);
+    const uint32_t ws = xs + w_base + w_row0 * 128;
+#pragma unroll
+    for (int s = 0; s < NSL; ++s) ptx::wg_fence_regs<N / 2>(d[s]);
     ptx::wg_fence();
 #pragma unroll
     for (int kk = 0; kk < kChunkK / 16; ++kk) {
       const uint64_t b = ptx::make_sw128_desc(ws + kk * 32);
-      ptx::wgmma_f16<N>(d, ptx::make_sw128_desc(xs + kk * 32), b);                  // X_hi
-      ptx::wgmma_f16<N>(d, ptx::make_sw128_desc(xs + kRows * 128 + kk * 32), b);    // X_lo
+#pragma unroll
+      for (int s = 0; s < NSL; ++s) {
+        const uint32_t x = xs + s * kXChunkBytes;
+        ptx::wgmma_f16<N>(d[s], ptx::make_sw128_desc(x + kk * 32), b);                  // X_hi
+        ptx::wgmma_f16<N>(d[s], ptx::make_sw128_desc(x + kRows * 128 + kk * 32), b);    // X_lo
+      }
     }
     ptx::wg_commit();
     ptx::wg_wait<0>();
-    ptx::wg_fence_regs<N / 2>(d);
-    if (leader) ptx::mbar_arrive(&rg.empty[rg.c_stage]);
-    if (++rg.c_stage == rg.ns) { rg.c_stage = 0; rg.c_phase ^= 1; }
+#pragma unroll
+    for (int s = 0; s < NSL; ++s) ptx::wg_fence_regs<N / 2>(d[s]);
+    if (leader) ptx::mbar_arrive(&empty[c_stage]);
+    if (++c_stage == ns) { c_stage = 0; c_phase ^= 1; }
   }
+}
+
+// One MMA warpgroup's consumer of an event: D (64 x 2n) = X_hi . B^T + X_lo . B^T over all `chunks` stages of the ring
+// (event_mma); then both column halves of D are added to the accumulator tile from column acol.
+template <int N>
+__device__ __forceinline__ void event_wg(Ring& rg, int chunks, uint32_t w_row0, float* s_acc, int acol, DecoderCtrl* ctrl) {
+  float d[1][N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[0][i] = 0.f;
+  event_mma<N, 1>(rg.stage0, kStageBytes, kXChunkBytes, rg.ns, rg.full, rg.empty, rg.c_stage, rg.c_phase, chunks, w_row0, ctrl, d);
   const int wt = threadIdx.x & 127;
 #pragma unroll
   for (int j = 0; j < N / 4; ++j)      // registers [0, N/4) hold the W_hi columns, [N/4, N/2) the W_lo ones
-    s_acc[ptx::wg_frag_row(j, wt) * kAccPitch + acol + ptx::wg_frag_col(j, wt)] += d[j] + d[N / 4 + j];
+    s_acc[ptx::wg_frag_row(j, wt) * kAccPitch + acol + ptx::wg_frag_col(j, wt)] += d[0][j] + d[0][N / 4 + j];
 }
 
 // Streams `chunks` K-chunks of the activation image x_img plus this CTA's weight rows through the ring;

@@ -508,11 +508,12 @@ EncStash enc_stash(const void* stash, int B, int T) {
 }
 
 // ---- encoder LSTM backward ------------------------------------------------------------------------------
-// elementwise part of one reverse step of both directions.  grid (2, B), block 256 = hidden units.
+// elementwise part of one reverse step of both directions.  grid (2, B), block 256 = hidden units.  part: (2, nsplit, R, 256)
+// with R = 64 per 64-row slice
 __global__ void __launch_bounds__(256) enc_lstm_bwd_kernel(const float* __restrict__ d_mem, const float* __restrict__ part, int has_part,
                                                            const float* __restrict__ gates, const float* __restrict__ cst,
                                                            const int32_t* __restrict__ lengths, float* __restrict__ g_c,
-                                                           float* __restrict__ dG, int B, int T, int step, int nsplit) {
+                                                           float* __restrict__ dG, int B, int T, int step, int nsplit, int R) {
   const int dir = blockIdx.x, b = blockIdx.y, u = threadIdx.x;
   const int t = dir == 0 ? T - 1 - step : step;          // backward order of each direction
   const bool valid = lengths == nullptr || t < lengths[b];
@@ -525,7 +526,7 @@ __global__ void __launch_bounds__(256) enc_lstm_bwd_kernel(const float* __restri
   }
   float g_h = d_mem[((long)b * T + t) * kEnc + dir * kEncH + u];
   if (has_part)
-    for (int s = 0; s < nsplit; ++s) g_h += part[(((long)dir * nsplit + s) * 64 + b) * kEncH + u];
+    for (int s = 0; s < nsplit; ++s) g_h += part[(((long)dir * nsplit + s) * R + b) * kEncH + u];
   const float* gp = gates + ((long)b * T + t) * (8 * kEncH) + dir * 4 * kEncH + u;
   const float gi = gp[0], gf = gp[kEncH], gg = gp[2 * kEncH], go = gp[3 * kEncH];
   const int tp = dir == 0 ? t - 1 : t + 1;               // previous step of the forward recurrence
@@ -540,14 +541,16 @@ __global__ void __launch_bounds__(256) enc_lstm_bwd_kernel(const float* __restri
   dg[3 * kEncH] = d_o * go * (1.f - go);
   g_c[ci] = d_c * gf;
 }
-// g_h' partials = dG_t (B x 1024) . W_hh (1024 x 256) per direction.  grid (2 column tiles, nsplit, 2 dirs), 64 x 128 tiles
+// g_h' partials = dG_t (B x 1024) . W_hh (1024 x 256) per direction.  grid (2 column tiles, nsplit, 2 dirs x 64-row slices),
+// 64 x 128 tiles; part (2, nsplit, R = 64 x slices, 256)
 __global__ void __launch_bounds__(256) enc_whh_bwd_kernel(const float* __restrict__ dG, const float* __restrict__ whh_f,
                                                           const float* __restrict__ whh_r, float* __restrict__ part, int B, int T,
                                                           int step, int nsplit) {
   constexpr int BK = 32;
   __shared__ __align__(16) float As[BK][64 + 4];
   __shared__ __align__(16) float Bs[BK][128];
-  const int dir = blockIdx.z, tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
+  const int dir = blockIdx.z & 1, b0 = (blockIdx.z >> 1) * 64, R = (gridDim.z >> 1) * 64;
+  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
   const int t = dir == 0 ? T - 1 - step : step;
   const float* W = (dir == 0 ? whh_f : whh_r) + blockIdx.x * 128;
   const int per = 4 * kEncH / nsplit;
@@ -563,7 +566,7 @@ __global__ void __launch_bounds__(256) enc_whh_bwd_kernel(const float* __restric
     for (int i = 0; i < 2; ++i) {
       const int idx = tid * 2 + i, r = idx >> 3, q = idx & 7;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (r < B) v = *reinterpret_cast<const float4*>(dG + (((long)r * T + t) * 2 + dir) * (4 * kEncH) + n0 + q * 4);
+      if (b0 + r < B) v = *reinterpret_cast<const float4*>(dG + (((long)(b0 + r) * T + t) * 2 + dir) * (4 * kEncH) + n0 + q * 4);
       As[q * 4 + 0][r] = v.x; As[q * 4 + 1][r] = v.y; As[q * 4 + 2][r] = v.z; As[q * 4 + 3][r] = v.w;
     }
 #pragma unroll
@@ -585,7 +588,7 @@ __global__ void __launch_bounds__(256) enc_whh_bwd_kernel(const float* __restric
         for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
     }
   }
-  float* out = part + (((long)dir * nsplit + blockIdx.y) * 64 + ty * 8) * kEncH + blockIdx.x * 128 + tx * 4;
+  float* out = part + (((long)dir * nsplit + blockIdx.y) * R + b0 + ty * 8) * kEncH + blockIdx.x * 128 + tx * 4;
 #pragma unroll
   for (int i = 0; i < 8; ++i)
     *reinterpret_cast<float4*>(out + (long)i * kEncH) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
@@ -774,19 +777,21 @@ constexpr int kEncBwdSplit = 8;   // K splits of the W_hh products in the revers
 struct EncBwdWs {
   float* dG;               // (B, T, 2 dirs, 1024)
   float *hp, *dxl;         // (B T, 512)
-  float* part;             // (2, kEncBwdSplit, 64, 256)
-  float* g_c;              // (2, 64, 256)
+  float* part;             // (2, kEncBwdSplit, R, 256), R = 64 per 64-row slice
+  float* g_c;              // (2, R, 256)
   float *gz, *gxa, *gxb;   // padded rows (B (T+4), 512)
   float *sums, *tmp;
   void* gemm; size_t gemm_bytes;   // scratch of the BiLSTM's weight / input gradient GEMMs and bias column sums
   ConvBwdWs cw;
 };
+static int enc_bwd_rows(int B) { return (B + 63) / 64 * 64; }
 static void encoder_backward_ws_layout(Carve& c, int B, int T, EncBwdWs* w) {
   const size_t Mp = (size_t)B * (T + 2 * kPadRows);
+  const int R = enc_bwd_rows(B);
   w->dG = c.take<float>((size_t)B * T * 8 * kEncH);
   w->hp = c.take<float>((size_t)B * T * kEnc); w->dxl = c.take<float>((size_t)B * T * kEnc);
-  w->part = c.take<float>((size_t)2 * kEncBwdSplit * 64 * kEncH);
-  w->g_c = c.take<float>((size_t)2 * 64 * kEncH);
+  w->part = c.take<float>((size_t)2 * kEncBwdSplit * R * kEncH);
+  w->g_c = c.take<float>((size_t)2 * R * kEncH);
   w->gz = c.take<float>(Mp * kEnc); w->gxa = c.take<float>(Mp * kEnc); w->gxb = c.take<float>(Mp * kEnc);
   w->sums = c.take<float>((size_t)(2 + 2 * kRedSplit) * kEnc);
   w->tmp = c.take<float>(8 * kEncH);
@@ -806,7 +811,8 @@ size_t encoder_backward_ws_bytes(int B, int T) {
 int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   const int B = a->B, T = a->T;
   constexpr int nsplit = kEncBwdSplit;
-  if (B < 1 || B > 64) return fail(T2_ERR_UNSUPPORTED, "encoder backward: 1 <= B <= 64 (got %d)", B);
+  if (B < 1 || T < 1) return fail(T2_ERR_INVALID, "encoder backward: bad sizes");
+  const int R = enc_bwd_rows(B);
   if (a->n_grads != W_COUNT) return fail(T2_ERR_INVALID, "encoder backward: expected %d gradient pointers", (int)W_COUNT);
   if (a->ws_bytes < encoder_backward_ws_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder backward workspace too small");
   if (a->stash_bytes < encoder_stash_bytes(B, T)) return fail(T2_ERR_WORKSPACE, "encoder stash too small");
@@ -814,13 +820,15 @@ int encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, cudaStream_t s) {
   EncBwdWs w;
   Carve wc(a->ws, 1024);
   encoder_backward_ws_layout(wc, B, T, &w);
-  T2_CUDA(cudaMemsetAsync(w.g_c, 0, (size_t)2 * 64 * kEncH * 4, s));
-  // ---- BiLSTM: reverse recurrence of both directions (model.py:169-171, 180-188) ----
+  T2_CUDA(cudaMemsetAsync(w.g_c, 0, (size_t)2 * R * kEncH * 4, s));
+  // ---- BiLSTM: reverse recurrence of both directions (model.py:169-171, 180-188); the W_hh products run per 64-row slice ----
   for (int step = 0; step < T; ++step) {
-    enc_lstm_bwd_kernel<<<dim3(2, B), 256, 0, s>>>(a->d_memory, w.part, step > 0, st.gates, st.cst, a->lengths, w.g_c, w.dG, B, T, step, nsplit);
+    enc_lstm_bwd_kernel<<<dim3(2, B), 256, 0, s>>>(a->d_memory, w.part, step > 0, st.gates, st.cst, a->lengths, w.g_c, w.dG, B, T, step,
+                                                   nsplit, R);
     T2_LAUNCH_CHECK();
     if (step + 1 < T) {
-      enc_whh_bwd_kernel<<<dim3(2, nsplit, 2), 256, 0, s>>>(w.dG, m->w[W_ENC_LSTM + 1], m->w[W_ENC_LSTM + 5], w.part, B, T, step, nsplit);
+      enc_whh_bwd_kernel<<<dim3(2, nsplit, 2 * (R / 64)), 256, 0, s>>>(w.dG, m->w[W_ENC_LSTM + 1], m->w[W_ENC_LSTM + 5], w.part, B, T,
+                                                                        step, nsplit);
       T2_LAUNCH_CHECK();
     }
   }

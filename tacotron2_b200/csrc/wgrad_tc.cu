@@ -66,16 +66,18 @@ __global__ void wg_colstats_finalize_kernel(const float* __restrict__ part, int 
 // ---- fp32 rows (chunk t = rows [t*B, t*B + B)) x C columns  ->  transposed operand images -----------------------
 // image of chunk t: C / TR tiles, each [hi plane TR x 128 B | lo plane], element (row = c % TR, k = b) = src[t*B+b][c] * scale[c]
 __global__ void __launch_bounds__(256) wg_transpose_img_kernel(const float* __restrict__ src, long ld, long row0, long rows_total,
-                                                               int chunk_rows, int C, int TR, const float* __restrict__ scale,
+                                                               int chunk_rows, int slices, int C, int TR, const float* __restrict__ scale,
                                                                uint8_t* __restrict__ img) {
-  // chunk t = source rows [row0 + t * chunk_rows, + chunk_rows) (chunk_rows <= 64; the remaining k and rows outside
-  // [0, rows_total) are zero); columns >= C of the last tile are zero rows
+  // group g = source rows [row0 + g * chunk_rows, + chunk_rows) as `slices` chunks of 64 rows: chunk t = slice t % slices
+  // of group t / slices (chunk_rows <= 64 * slices; the remaining k and rows outside [0, rows_total) are zero); columns
+  // >= C of the last tile are zero rows
   __shared__ float tile[64][65];
   const int c0 = blockIdx.x * 64, t = blockIdx.y, tid = threadIdx.x;
+  const int g = t / slices, b0 = (t - g * slices) * 64;
   for (int i = tid; i < 64 * 64; i += 256) {
     const int b = i >> 6, cc = i & 63;
-    const long r = row0 + (long)t * chunk_rows + b;
-    tile[b][cc] = (b < chunk_rows && r >= 0 && r < rows_total && c0 + cc < C) ? src[r * ld + c0 + cc] : 0.f;
+    const long r = row0 + (long)g * chunk_rows + b0 + b;
+    tile[b][cc] = (b0 + b < chunk_rows && r >= 0 && r < rows_total && c0 + cc < C) ? src[r * ld + c0 + cc] : 0.f;
   }
   __syncthreads();
   const int ntile = (C + TR - 1) / TR;
@@ -206,7 +208,7 @@ struct WgDecJobs {
   const uint8_t* img_a[2];
   float* part[2];
   const float* inv[2];
-  int T, seg, nsplit;
+  int T, seg, nsplit;      // T: K chunks (decoder steps x 64-row chunks per step)
   __device__ WgJob operator()(int idx) const {
     const int n0 = nsplit * (4096 / kTM) * (1792 / kTN);      // CTAs of the attention LSTM
     const int l = idx >= n0 ? 1 : 0;
@@ -234,13 +236,17 @@ struct WgDecJobs {
 
 }  // namespace
 
-void wgrad_tc_layout(Carve& c, int T, WgradWs* w) {
-  const int seg = wgrad_seg(T), nsplit = (T + seg - 1) / seg;
-  for (int l = 0; l < 2; ++l) w->img_a[l] = c.take<uint8_t>((size_t)T * 4096 * 256, 1024);
-  w->img_x2 = c.take<uint8_t>((size_t)T * 256 * 256, 1024);
-  w->img_ctx = c.take<uint8_t>((size_t)(T + 1) * 1024 * 256, 1024);
-  w->img_ha = c.take<uint8_t>((size_t)(T + 1) * 1024 * 256, 1024);
-  w->img_hd = c.take<uint8_t>((size_t)(T + 1) * 1024 * 256, 1024);
+// K chunks of 64 rows per decoder step: the B rows of a step as ceil(B / 64) zero-padded chunks
+static int wgrad_step_chunks(int B) { return (B + 63) / 64; }
+
+void wgrad_tc_layout(Carve& c, int B, int T, WgradWs* w) {
+  const int S = wgrad_step_chunks(B), nch = T * S;
+  const int seg = wgrad_seg(nch), nsplit = (nch + seg - 1) / seg;
+  for (int l = 0; l < 2; ++l) w->img_a[l] = c.take<uint8_t>((size_t)nch * 4096 * 256, 1024);
+  w->img_x2 = c.take<uint8_t>((size_t)nch * 256 * 256, 1024);
+  w->img_ctx = c.take<uint8_t>((size_t)(T + 1) * S * 1024 * 256, 1024);
+  w->img_ha = c.take<uint8_t>((size_t)(T + 1) * S * 1024 * 256, 1024);
+  w->img_hd = c.take<uint8_t>((size_t)(T + 1) * S * 1024 * 256, 1024);
   w->part = c.take<float>((size_t)nsplit * 4096 * (1792 + 2560), 1024);
   w->stat = c.take<float>((size_t)kStatSplit * 2 * 4096, 1024);
   w->scale = c.take<float>(4096, 1024);
@@ -252,7 +258,8 @@ void wgrad_tc_layout(Carve& c, int T, WgradWs* w) {
 int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, const float* x2, const DecoderStash& st,
                  float* const* G, const WgradWs& w, cudaStream_t s) {
   (void)m;
-  const int seg = wgrad_seg(T), nsplit = (T + seg - 1) / seg;
+  const int S = wgrad_step_chunks(B), nch = T * S;
+  const int seg = wgrad_seg(nch), nsplit = (nch + seg - 1) / seg;
   const long rows = (long)T * B;
   const float* dG[2] = {dga, dgd};
   const int bias_idx[2][2] = {{W_ARNN_BIH, W_ARNN_BHH}, {W_DRNN_BIH, W_DRNN_BHH}};
@@ -263,23 +270,23 @@ int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, c
     T2_LAUNCH_CHECK();
     for (int k = 0; k < 2; ++k)
       if (G[bias_idx[l][k]]) T2_CUDA(cudaMemcpyAsync(G[bias_idx[l][k]], w.colsum, 4096 * 4, cudaMemcpyDeviceToDevice, s));
-    wg_transpose_img_kernel<<<dim3(4096 / 64, T), 256, 0, s>>>(dG[l], 4096, 0, rows, B, 4096, kTM, w.scale, w.img_a[l]);
+    wg_transpose_img_kernel<<<dim3(4096 / 64, nch), 256, 0, s>>>(dG[l], 4096, 0, rows, B, S, 4096, kTM, w.scale, w.img_a[l]);
     T2_LAUNCH_CHECK();
   }
-  wg_transpose_img_kernel<<<dim3(256 / 64, T), 256, 0, s>>>(x2, 256, 0, rows, B, 256, kTN, nullptr, w.img_x2);
+  wg_transpose_img_kernel<<<dim3(256 / 64, nch), 256, 0, s>>>(x2, 256, 0, rows, B, S, 256, kTN, nullptr, w.img_x2);
   T2_LAUNCH_CHECK();
-  wg_transpose_img_kernel<<<dim3(512 / 64, T + 1), 256, 0, s>>>(st.ctx, 512, 0, rows + B, B, 512, kTN, nullptr, w.img_ctx);
+  wg_transpose_img_kernel<<<dim3(512 / 64, (T + 1) * S), 256, 0, s>>>(st.ctx, 512, 0, rows + B, B, S, 512, kTN, nullptr, w.img_ctx);
   T2_LAUNCH_CHECK();
-  wg_transpose_img_kernel<<<dim3(1024 / 64, T + 1), 256, 0, s>>>(st.ha, 1024, 0, rows + B, B, 1024, kTN, nullptr, w.img_ha);
+  wg_transpose_img_kernel<<<dim3(1024 / 64, (T + 1) * S), 256, 0, s>>>(st.ha, 1024, 0, rows + B, B, S, 1024, kTN, nullptr, w.img_ha);
   T2_LAUNCH_CHECK();
-  wg_transpose_img_kernel<<<dim3(1024 / 64, T + 1), 256, 0, s>>>(st.hd, 1024, 0, rows + B, B, 1024, kTN, nullptr, w.img_hd);
+  wg_transpose_img_kernel<<<dim3(1024 / 64, (T + 1) * S), 256, 0, s>>>(st.hd, 1024, 0, rows + B, B, S, 1024, kTN, nullptr, w.img_hd);
   T2_LAUNCH_CHECK();
   WgDecJobs jobs;
   jobs.grp[0][0] = {w.img_x2, 1, 0}; jobs.grp[0][1] = {w.img_ctx, 2, 0}; jobs.grp[0][2] = {w.img_ha, 4, 0};   // [x2_t | ctx_(t-1) | ah_(t-1)]   model.py:352
-  jobs.grp[1][0] = {w.img_ha, 4, 1}; jobs.grp[1][1] = {w.img_ctx, 2, 1}; jobs.grp[1][2] = {w.img_hd, 4, 0};   // [ah_t | ctx_t | dh_(t-1)]       model.py:366-367
+  jobs.grp[1][0] = {w.img_ha, 4, S}; jobs.grp[1][1] = {w.img_ctx, 2, S}; jobs.grp[1][2] = {w.img_hd, 4, 0};   // [ah_t | ctx_t | dh_(t-1)]       model.py:366-367
   float* part_l[2] = {w.part, w.part + (size_t)nsplit * 4096 * 1792};
   for (int l = 0; l < 2; ++l) { jobs.img_a[l] = w.img_a[l]; jobs.part[l] = part_l[l]; jobs.inv[l] = w.inv[l]; }
-  jobs.T = T; jobs.seg = seg; jobs.nsplit = nsplit;
+  jobs.T = nch; jobs.seg = seg; jobs.nsplit = nsplit;
   T2_TRY(wg_launch(jobs, nsplit * (4096 / kTM) * ((1792 + 2560) / kTN), s));
   {
     const long n = (long)4096 * 1792;
@@ -308,7 +315,7 @@ int wg_colstats(const float* x, long rows, int C, float* stat_ws, float* scale, 
 int wg_transpose_images(const float* src, long ld, long row0, long rows_total, int chunk_rows, int nchunks, int C, int TR,
                         const float* scale, uint8_t* img, cudaStream_t s) {
   const int ntile = (C + TR - 1) / TR;
-  wg_transpose_img_kernel<<<dim3(ntile * TR / 64, nchunks), 256, 0, s>>>(src, ld, row0, rows_total, chunk_rows, C, TR, scale, img);
+  wg_transpose_img_kernel<<<dim3(ntile * TR / 64, nchunks), 256, 0, s>>>(src, ld, row0, rows_total, chunk_rows, 1, C, TR, scale, img);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }

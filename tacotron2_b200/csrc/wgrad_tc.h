@@ -44,15 +44,16 @@ int wg_colstats(const float* x, long rows, int C, float* stat_ws, float* scale, 
 int wg_transpose_images(const float* src, long ld, long row0, long rows_total, int chunk_rows, int nchunks, int C, int TR,
                         const float* scale, uint8_t* img, cudaStream_t s);
 
-constexpr int kWgSeg = 100;      // decoder steps (K chunks of 64 batch rows) per K split
-inline int wgrad_seg(int T) { int seg = kWgSeg; while ((T + seg - 1) / seg > 15) seg += 50; return seg; }
+// K chunks of 64 batch rows per K split; a decoder step is ceil(B / 64) chunks, so `n` = T x ceil(B / 64)
+constexpr int kWgSeg = 100;
+inline int wgrad_seg(int n) { int seg = kWgSeg; while ((n + seg - 1) / seg > 15) seg += 50; return seg; }
 struct WgradWs {                        // every region 1024-aligned
   uint8_t* img_a[2];                    // dG^T images of both LSTMs
   uint8_t *img_x2, *img_ctx, *img_ha, *img_hd;   // operand images (ctx sized like ha)
   float* part;                          // K-split partial sums of both LSTMs
   float *stat, *scale, *inv[2], *colsum;
 };
-void wgrad_tc_layout(Carve& c, int T, WgradWs* w);
+void wgrad_tc_layout(Carve& c, int B, int T, WgradWs* w);
 int wgrad_tc_run(T2Model* m, int B, int T, const float* dga, const float* dgd, const float* x2, const DecoderStash& st,
                  float* const* G, const WgradWs& w, cudaStream_t s);
 

@@ -170,17 +170,6 @@ def _require_no_grad_with_lengths(module, what):
                                   "torch.no_grad()" % what)
 
 
-MAX_TRAIN_ROWS = 64   # rows per GPU of one autograd call: the backward kernels and the training stash are sized for one
-                      # 64-row launch (BASELINE.json configs[2] / [3] are B=64 per GPU); larger batches: split and accumulate
-
-
-def _check_train_rows(B, what):
-    if B > MAX_TRAIN_ROWS:
-        raise RuntimeError("tacotron2_b200: %s under autograd supports at most %d rows per call (got %d): run the batch as "
-                           "%d-row slices and let the gradients accumulate, or wrap inference-only calls in torch.no_grad()"
-                           % (what, MAX_TRAIN_ROWS, B, MAX_TRAIN_ROWS))
-
-
 class _EncoderFn(torch.autograd.Function):
     """Encoder.forward (model.py:173-190) [+ the embedding lookup of model.py:503 when `text` is given] as one autograd
     node: forward = fp32 conv stack + persistent BiLSTM with a stash, backward = t2_encoder_backward."""
@@ -338,7 +327,6 @@ class Encoder(_EngineOwner, nn.Module):
     def _run(self, x, lengths):
         emb = x.transpose(1, 2)                      # (B, T, 512) -- contiguous when x came from the embedding
         if _wants_grad(self, x):
-            _check_train_rows(x.size(0), "Encoder.forward")
             named = [("encoder." + k, p_) for k, p_ in self.named_parameters()]
             return _EncoderFn.apply(self, [n for n, _ in named], None, emb, lengths, self.training,
                                     *[p_ for _, p_ in named]).to(x.dtype)
@@ -444,7 +432,6 @@ class Decoder(_EngineOwner, nn.Module):
         dt = memory.dtype
         params = [p_ for p_ in self.parameters()]
         if torch.is_grad_enabled() and (memory.requires_grad or any(p_.requires_grad for p_ in params)):
-            _check_train_rows(memory.size(0), "Decoder.forward")
             mel, gate, align = _DecoderFn.apply(self, memory, decoder_inputs, memory_lengths, *params)
         else:
             mel, gate, align, _ = self._teacher_forward(memory, decoder_inputs, memory_lengths, False)
@@ -618,8 +605,6 @@ class Tacotron2(_EngineOwner, nn.Module):
     def _forward_packed(self, eng, text_inputs, text_lengths, mels, output_lengths):
         masks = current_masks()
         grad = _wants_grad(self)
-        if grad:
-            _check_train_rows(text_inputs.size(0), "Tacotron2.forward")
         if grad:   # embedding lookup + encoder as one node (the embedding gradient comes out of t2_encoder_backward)
             named = [("embedding.weight", self.embedding.weight)] + [("encoder." + k, p_) for k, p_ in self.encoder.named_parameters()]
             memory = _EncoderFn.apply(self, [n for n, _ in named], text_inputs, None, text_lengths, self.training,
