@@ -166,6 +166,11 @@ int    t2_encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, void* stream);
  * row's end, the context over staged and L2-resident memory rows -- runs in the order a call with T_enc =
  * memory_lengths[b] uses, so a row of a ragged batch equals its own B = 1 call on memory[b, :memory_lengths[b]] bit
  * for bit (persistent implementation; the stepwise one sums positions in a fixed order too). */
+/* Per-row seeds (row_seeds != NULL; INFER, training = 0, prenet_keep NULL -- T2_ERR_INVALID otherwise): row b draws
+ * the prenet keep bit of its step s, layer k, column j as Philox keyed by (row_seeds[b], site 4 s + k, element j), which
+ * is what a B = 1 call with seed = row_seeds[b] draws.  Row b's outputs then equal that call's bit for bit, whatever
+ * its batch, its 64-row slice, the stream chunking or the serving slot.  NULL: one key for the call, element
+ * b * 256 + j. */
 typedef struct T2DecoderArgs {
   int32_t mode, impl, training;
   const float* memory; const int32_t* memory_lengths; int32_t B, T_enc, n_steps_cap;
@@ -177,6 +182,7 @@ typedef struct T2DecoderArgs {
   void* ws; size_t ws_bytes;
   void* stash; size_t stash_bytes;     /* TEACHER only, optional: activations kept for t2_decoder_backward
                                           (t2_decoder_stash_bytes(); opaque to the caller) */
+  const uint64_t* row_seeds;           /* (B) or NULL: per-row Philox keys of the prenet dropout (see below) */
 } T2DecoderArgs;
 size_t t2_decoder_workspace_bytes(const T2Model* m, int32_t B, int32_t T_enc, int32_t n_steps_cap);
 int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);
@@ -202,6 +208,8 @@ typedef struct T2DecoderStreamArgs {
   T2DecoderArgs dec;
   void* state; size_t state_bytes;
   int32_t* status;
+  const int32_t* row_step0;            /* (B) device or NULL: with dec.row_seeds, row b's step (the one its prenet keys
+                                          use) at local step i of a run is row_step0[b] + i instead of the absolute step */
 } T2DecoderStreamArgs;
 size_t t2_decoder_stream_state_bytes(const T2Model* m, int32_t B, int32_t T_enc);
 int    t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stream);
@@ -216,7 +224,8 @@ int    t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n
  * no step counter in `state`, and a step reads the keep mask of the step after it.  mel / gate / align
  * are chunk buffers (B, n + 1, .), prenet_keep (n + 1, 2, B, 256) holds at [i, :, b] the mask of row b's
  * own step (steps it has run before the chunk) + i, and dec.seed is the chunk's Philox seed; the caller
- * rewrites them (and memory / memory_lengths rows) between runs.  mel_lengths[b] becomes the local step
+ * rewrites them (and memory / memory_lengths rows) between runs.  Seeded instead (dec.row_seeds, prenet_keep NULL):
+ * row_step0[b] holds the steps row b's request has run before the chunk, and each request draws its own B = 1 stream.  mel_lengths[b] becomes the local step
  * + 1 at which row b fired in the chunk; a slice ends a chunk early once all its rows have fired.
  *   admit:   rows (host, n_rows ascending row indices): each listed row goes back to the state begin
  *            gives it -- its accumulator rows, LSTM cells, previous / cumulative attention weights,
@@ -436,6 +445,8 @@ typedef struct T2InferArgs {
   int32_t* mel_lengths_host;           /* out (B) */
   int32_t* n_steps_host;               /* out (1) */
   void* ws; size_t ws_bytes;
+  const uint64_t* row_seeds_host;      /* (B) host or NULL: the decoder's row_seeds (row b then equals its B = 1 call
+                                          with seed = row_seeds_host[b]); `seed` is not used when given */
 } T2InferArgs;
 size_t t2_infer_lengths_workspace_bytes(const T2Model* m, int32_t B, int32_t T_text, int32_t max_steps);
 int    t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream);
@@ -472,12 +483,15 @@ int t2_waveglow_destroy(T2WaveGlow* h);
  * [0, 256 lengths[b]) equal an infer of that row's first lengths[b] frames alone; later samples are zero.
  * z (B, 8, 32 T_mel) fp32 or NULL: the standard-normal draws, channels in draw order (the 4 initial ones, then the
  * early blocks of flow 8 and flow 4); NULL => in-kernel Philox4x32-10 keyed by (seed, row, channel, group column).
+ * row_seeds (B) device or NULL: row b's noise is keyed by (row_seeds[b], row 0, channel, group column) instead, the
+ * draws of a B = 1 call with seed = row_seeds[b]; with z given it is T2_ERR_INVALID.
  * audio (B, 256 T_mel) out, in the mel's dtype. */
 typedef struct T2WaveGlowArgs {
   const void* mel; int32_t B, T_mel; const int32_t* lengths; int32_t io_half;
   float sigma; const float* z; uint64_t seed;
   void* audio;
   void* ws; size_t ws_bytes;
+  const uint64_t* row_seeds;
 } T2WaveGlowArgs;
 size_t t2_waveglow_workspace_bytes(const T2WaveGlow* h, int32_t B, int32_t T_mel);
 int    t2_waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, void* stream);

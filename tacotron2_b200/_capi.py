@@ -68,7 +68,7 @@ class T2InferArgs(C.Structure):
     _fields_ = [("text_host", C.c_void_p), ("input_lengths_host", C.c_void_p), ("B", C.c_int32), ("T_text", C.c_int32),
                 ("max_steps", C.c_int32), ("gate_threshold", C.c_float), ("seed", C.c_uint64), ("impl", C.c_int32),
                 ("mel_post_host", C.c_void_p), ("mel_lengths_host", C.c_void_p), ("n_steps_host", C.c_void_p),
-                ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+                ("ws", C.c_void_p), ("ws_bytes", C.c_size_t), ("row_seeds_host", C.c_void_p)]
 
 
 class T2DecoderArgs(C.Structure):
@@ -81,11 +81,12 @@ class T2DecoderArgs(C.Structure):
                 ("mel", C.c_void_p), ("gate", C.c_void_p), ("align", C.c_void_p),
                 ("mel_lengths", C.c_void_p), ("n_steps", C.c_void_p),
                 ("ws", C.c_void_p), ("ws_bytes", C.c_size_t),
-                ("stash", C.c_void_p), ("stash_bytes", C.c_size_t)]
+                ("stash", C.c_void_p), ("stash_bytes", C.c_size_t), ("row_seeds", C.c_void_p)]
 
 
 class T2DecoderStreamArgs(C.Structure):
-    _fields_ = [("dec", T2DecoderArgs), ("state", C.c_void_p), ("state_bytes", C.c_size_t), ("status", C.c_void_p)]
+    _fields_ = [("dec", T2DecoderArgs), ("state", C.c_void_p), ("state_bytes", C.c_size_t), ("status", C.c_void_p),
+                ("row_step0", C.c_void_p)]
 
 
 class T2CollectRow(C.Structure):
@@ -175,7 +176,7 @@ class T2WaveGlowConfig(C.Structure):
 class T2WaveGlowArgs(C.Structure):
     _fields_ = [("mel", C.c_void_p), ("B", C.c_int32), ("T_mel", C.c_int32), ("lengths", C.c_void_p),
                 ("io_half", C.c_int32), ("sigma", C.c_float), ("z", C.c_void_p), ("seed", C.c_uint64),
-                ("audio", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+                ("audio", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t), ("row_seeds", C.c_void_p)]
 
 
 class T2WaveGlowWindowArgs(C.Structure):

@@ -2,6 +2,7 @@
 workspaces, dropout-mask injection.  All arithmetic happens in the shared library."""
 import contextlib
 import ctypes as C
+import numbers
 import threading
 
 import torch
@@ -93,6 +94,40 @@ def next_seed():
     """Philox seed for one engine call: torch's global seed + a call counter."""
     _seed_counter[0] += 1
     return (torch.initial_seed() * 1000003 + _seed_counter[0]) & 0xFFFFFFFFFFFFFFFF
+
+
+def row_seeds(seeds, B, device, what):
+    """Per-utterance seeds as B 64-bit Philox keys, an int64 tensor on `device` holding each key's bit pattern (None
+    stays None).  seeds: B integers in [0, 2**64), as a list, a host tensor or a device tensor; int64 / uint64 values are
+    taken as their 64-bit pattern, narrower integer dtypes must be >= 0.  Raises TypeError / ValueError before anything
+    runs."""
+    if seeds is None:
+        return None
+    if torch.is_tensor(seeds):
+        t = seeds
+        if t.dtype == torch.bool or t.dtype.is_floating_point or t.dtype.is_complex:
+            raise TypeError("%s: seeds must hold integers (got %s)" % (what, t.dtype))
+        if t.dim() != 1 or t.shape[0] != B:
+            raise ValueError("%s: seeds must have shape (%d,) (got %s)" % (what, B, tuple(t.shape)))
+        if t.dtype == torch.uint64:
+            t = t.contiguous().view(torch.int64)
+        elif t.dtype != torch.int64:
+            if t.dtype.is_signed and bool((t < 0).any()):
+                raise ValueError("%s: seeds must lie in [0, 2**64)" % what)
+            t = t.to(torch.int64)
+        return t.to(device=device).contiguous()
+    vals = list(seeds)
+    if len(vals) != B:
+        raise ValueError("%s: seeds must hold %d values (got %d)" % (what, B, len(vals)))
+    bits = []
+    for v in vals:
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+            raise TypeError("%s: seeds must be integers (got %r)" % (what, v))
+        v = int(v)
+        if not 0 <= v < 1 << 64:
+            raise ValueError("%s: seed %d is outside [0, 2**64)" % (what, v))
+        bits.append(v - (1 << 64) if v >= 1 << 63 else v)
+    return torch.tensor(bits, dtype=torch.int64).to(device)
 
 
 def _i32(x, device):
@@ -280,7 +315,8 @@ class Engine(_Handle):
     # -- decoder ---------------------------------------------------------------------------------
     def decoder(self, memory, mode, n_steps_cap, memory_lengths=None, teacher_prenet=None, training=False,
                 prenet_keep=None, att_keep=None, dec_keep=None, gate_threshold=0.5,
-                score_mask_value=-float("inf"), impl=None, stash=None, seed=None):
+                score_mask_value=-float("inf"), impl=None, stash=None, seed=None, row_seeds=None):
+        """row_seeds: None or (B,) int64 on the device (see row_seeds()): per-row prenet keys."""
         L = _capi.lib()
         memory = memory.to(device=self.device, dtype=torch.float32).contiguous()
         B, T = int(memory.shape[0]), int(memory.shape[1])
@@ -302,16 +338,18 @@ class Engine(_Handle):
                                 next_seed() if seed is None else seed, float(gate_threshold), float(score_mask_value),
                                 mel.data_ptr(), gate.data_ptr(), align.data_ptr(), mel_lengths.data_ptr(),
                                 n_steps.data_ptr(), ws.data_ptr(), ws.numel(),
-                                _ptr(stash), 0 if stash is None else stash.numel())
+                                _ptr(stash), 0 if stash is None else stash.numel(), _ptr(row_seeds))
         self._call(L.t2_decoder_run, C.byref(a))
-        self._last_decoder_args = (a, memory, len32, teacher_prenet, pk, ak, dk, ws, mel, gate, align, mel_lengths, n_steps)
+        self._last_decoder_args = (a, memory, len32, teacher_prenet, pk, ak, dk, ws, mel, gate, align, mel_lengths, n_steps,
+                                   row_seeds)
         return mel, gate, align, mel_lengths, n_steps
 
     def decoder_stream(self, memory, n_steps_cap, prenet_keep=None, gate_threshold=0.5, score_mask_value=-float("inf"),
-                       impl=None, seed=None, memory_lengths=None):
+                       impl=None, seed=None, memory_lengths=None, row_seeds=None):
         """Begins a resumable INFER run of the persistent decoder (t2_decoder_stream_begin); see DecoderStream."""
         return DecoderStream(self, memory, n_steps_cap, prenet_keep, gate_threshold, score_mask_value,
-                             self.impl if impl is None else impl, next_seed() if seed is None else seed, memory_lengths)
+                             self.impl if impl is None else impl, next_seed() if seed is None else seed, memory_lengths,
+                             row_seeds)
 
     def decoder_profile(self):
         """Per-phase SM cycles of the last persistent decoder run: dict phase -> [cta0, cta60, cta100]."""
@@ -396,10 +434,12 @@ class Engine(_Handle):
         return out
 
     # -- end to end with host buffers (bench e2e leg) ------------------------------------------------
-    def infer_host(self, text_host, max_steps, gate_threshold=0.5, impl=None, out_host=None, seed=None, input_lengths_host=None):
+    def infer_host(self, text_host, max_steps, gate_threshold=0.5, impl=None, out_host=None, seed=None, input_lengths_host=None,
+                   row_seeds_host=None):
         """text_host: pinned int64 (B, T).  Returns (mel_post_host (B,80,max_steps), lengths, n_steps).  seed: the
         Philox seed of the decoder's prenet dropout (default: next_seed()).  input_lengths_host: pinned int64 (B) or None;
-        given, t2_infer_host_lengths runs each row as its first input_lengths_host[b] symbols alone."""
+        given, t2_infer_host_lengths runs each row as its first input_lengths_host[b] symbols alone.  row_seeds_host: int64
+        (B) host tensor of per-row seeds (needs input_lengths_host): row b then equals its B = 1 call with that seed."""
         L = _capi.lib()
         B, T = int(text_host.shape[0]), int(text_host.shape[1])
         if out_host is None:
@@ -412,9 +452,11 @@ class Engine(_Handle):
             ws = self._workspace("e2e", L.t2_infer_lengths_workspace_bytes(self.handle, B, T, max_steps))
             a = _capi.T2InferArgs(text_host.data_ptr(), input_lengths_host.data_ptr(), B, T, int(max_steps),
                                   float(gate_threshold), seed, impl, mel.data_ptr(), lens.data_ptr(), ns.data_ptr(),
-                                  ws.data_ptr(), ws.numel())
+                                  ws.data_ptr(), ws.numel(), _ptr(row_seeds_host))
             self._call(L.t2_infer_host_lengths, C.byref(a))
             return mel, lens, ns
+        if row_seeds_host is not None:
+            raise ValueError("tacotron2_b200: row_seeds_host needs input_lengths_host (t2_infer_host_lengths)")
         ws = self._workspace("e2e", L.t2_infer_workspace_bytes(self.handle, B, T, max_steps))
         self._call(L.t2_infer_host, text_host.data_ptr(), B, T, int(max_steps), float(gate_threshold), seed, impl,
                    mel.data_ptr(), lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel())
@@ -439,7 +481,8 @@ class DecoderStream:
     requests' own buffers.  ``memory``, ``len32`` and ``keep`` are the tensors the kernel reads: such a session rewrites
     their rows in place between chunks."""
 
-    def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed, memory_lengths=None):
+    def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed, memory_lengths=None,
+                 row_seeds=None):
         L = _capi.lib()
         dev = eng.device
         self.eng = eng
@@ -458,10 +501,11 @@ class DecoderStream:
         self.status_host = None                      # the caller's copy of `status` after the last run
         self.state = _capi.byte_buffer(L.t2_decoder_stream_state_bytes(eng.handle, B, T), dev)
         self.keep, self.len32 = _u8(prenet_keep, dev), _i32(memory_lengths, dev)
+        self.row_seeds = row_seeds      # (B,) int64 bit patterns on the device or None; a session may rewrite them
         d = _capi.T2DecoderArgs(_capi.MODE_INFER, impl, 0, self.memory.data_ptr(), _ptr(self.len32), B, T, self.cap,
                                 None, _ptr(self.keep), None, None, seed, float(gate_threshold), float(score_mask_value),
                                 self.mel.data_ptr(), self.gate.data_ptr(), self.align.data_ptr(),
-                                self.mel_lengths.data_ptr(), self.n_steps.data_ptr())
+                                self.mel_lengths.data_ptr(), self.n_steps.data_ptr(), row_seeds=_ptr(row_seeds))
         self.args = _capi.T2DecoderStreamArgs(d, self.state.data_ptr(), self.state.numel(), self.status.data_ptr())
         eng._call(L.t2_decoder_stream_begin, C.byref(self.args))
 
@@ -481,10 +525,12 @@ class DecoderStream:
         arr = (C.c_int32 * len(rows))(*rows)
         self.eng._call(_capi.lib().t2_decoder_stream_admit, C.byref(self.args), arr, len(rows))
 
-    def launch_chunk(self, n, seed, skip_slices=()):
-        """Enqueue local steps [0, n) of every 64-row slice not in skip_slices (n < cap) under the Philox seed `seed`."""
+    def launch_chunk(self, n, seed, skip_slices=(), row_step0=None):
+        """Enqueue local steps [0, n) of every 64-row slice not in skip_slices (n < cap) under the Philox seed `seed`.
+        row_step0: with row seeds, (B,) int32 on the device -- the steps each row's request ran before this chunk."""
         assert 1 <= n < self.cap
         self.args.dec.seed = seed
+        self.args.row_step0 = _ptr(row_step0)
         host = torch.tensor([[0, int(i in skip_slices)] for i in range(self.n_slices)], dtype=torch.int32)
         self.eng._call(_capi.lib().t2_decoder_stream_run, C.byref(self.args), int(n), host.data_ptr())
 

@@ -147,6 +147,17 @@ int decoder_ws_carve(const T2DecoderArgs* a, DecoderWs* w) {
   return T2_OK;
 }
 
+// per-row prenet keys: evaluation-mode INFER only (the hidden-state dropout of training mode is keyed by the call), and
+// never together with injected masks
+static int check_row_seeds(const T2DecoderArgs* a, const char* what) {
+  if (!a->row_seeds) return T2_OK;
+  if (a->mode != T2_MODE_INFER || a->training)
+    return fail(T2_ERR_INVALID, "%s: row_seeds need mode INFER with training = 0 (mode %d, training %d)", what, a->mode,
+                a->training);
+  if (a->prenet_keep) return fail(T2_ERR_INVALID, "%s: row_seeds and prenet_keep exclude each other", what);
+  return T2_OK;
+}
+
 static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a) {
   if (!m || !a) return fail(T2_ERR_INVALID, "null model / args");
   if (a->B <= 0 || a->B > kMaxBatch) return fail(T2_ERR_INVALID, "decoder: B=%d outside [1, %d]", a->B, kMaxBatch);
@@ -156,7 +167,7 @@ static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a) {
     return fail(T2_ERR_INVALID, "decoder: null tensor pointer");
   if (a->mode == T2_MODE_TEACHER && !a->teacher_prenet) return fail(T2_ERR_INVALID, "decoder: teacher mode needs teacher_prenet");
   if (a->mode != T2_MODE_TEACHER && a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "decoder: bad mode %d", a->mode);
-  return T2_OK;
+  return check_row_seeds(a, "decoder");
 }
 
 }  // namespace t2
@@ -306,7 +317,8 @@ static int check_stream_args(const T2Model* m, const T2DecoderStreamArgs* s) {
     return fail(T2_ERR_UNSUPPORTED, "decoder stream: the persistent decoder does not support T_enc=%d on this device "
                                     "(at most 2274, and >= 128 SMs)", a->T_enc);
   if (s->state_bytes < persistent_stream_state_bytes(a->B, a->T_enc)) return fail(T2_ERR_WORKSPACE, "decoder stream state too small");
-  return T2_OK;
+  if (s->row_step0 && !a->row_seeds) return fail(T2_ERR_INVALID, "decoder stream: row_step0 needs dec.row_seeds");
+  return check_row_seeds(a, "decoder stream");
 }
 
 int t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stream) {
@@ -317,7 +329,7 @@ int t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stre
 int t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n_steps, const int32_t* status_host, void* stream) {
   T2_TRY(check_stream_args(m, a));
   if (n_steps < 1) return fail(T2_ERR_INVALID, "decoder stream: n_steps=%d (at least 1 step per run)", n_steps);
-  return persistent_stream_run(m, &a->dec, a->state, a->status, n_steps, status_host, (cudaStream_t)stream);
+  return persistent_stream_run(m, &a->dec, a->state, a->status, n_steps, status_host, a->row_step0, (cudaStream_t)stream);
 }
 
 int t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int32_t* rows, int32_t n_rows, void* stream) {
@@ -393,6 +405,7 @@ struct InferWs {
   int64_t* text; float *memory, *mel, *gate, *align, *post; int32_t *lens, *nsteps;
   char* sub; size_t sub_bytes;   // the workspace of the encoder, the decoder and the postnet in turn
   int32_t* in_lens;              // t2_infer_host_lengths: the input lengths (B)
+  uint64_t* row_seeds;           // t2_infer_host_lengths: the per-row prenet keys (B)
 };
 static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w, bool with_lengths = false) {
   w->text = c.take<int64_t>((size_t)B * Tt);
@@ -408,6 +421,7 @@ static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w, bool with_l
   if (postnet_ws_bytes(B, S) > sb) sb = postnet_ws_bytes(B, S);
   w->sub = c.take<char>(sb); w->sub_bytes = sb;
   w->in_lens = with_lengths ? c.take<int32_t>(B) : nullptr;
+  w->row_seeds = with_lengths ? c.take<uint64_t>(B) : nullptr;
 }
 
 size_t t2_infer_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32_t max_steps) {
@@ -427,7 +441,8 @@ size_t t2_infer_lengths_workspace_bytes(const T2Model*, int32_t B, int32_t T_tex
 // Tacotron2.inference end to end; in_lens_host (B) or null: each row b is its first in_lens_host[b] symbols alone
 static int infer_host(T2Model* m, const int64_t* text_host, const int64_t* in_lens_host, int32_t B, int32_t T_text,
                       int32_t max_steps, float gate_threshold, uint64_t seed, int32_t impl, float* mel_post_host,
-                      int32_t* mel_lengths_host, int32_t* n_steps_host, void* ws, size_t ws_bytes, cudaStream_t s) {
+                      int32_t* mel_lengths_host, int32_t* n_steps_host, void* ws, size_t ws_bytes, cudaStream_t s,
+                      const uint64_t* row_seeds_host = nullptr) {
   if (!m || !text_host || !mel_post_host || !mel_lengths_host || !n_steps_host || !ws)
     return fail(T2_ERR_INVALID, "infer_host: null argument");
   const bool with_lengths = in_lens_host != nullptr;
@@ -451,6 +466,7 @@ static int infer_host(T2Model* m, const int64_t* text_host, const int64_t* in_le
   T2_CUDA(cudaMemcpyAsync(w.text, text_host, (size_t)B * T_text * 8, cudaMemcpyHostToDevice, s));
   // pageable source: the call returns once lens32 has been staged, so the vector may go out of scope
   if (with_lengths) T2_CUDA(cudaMemcpyAsync(w.in_lens, lens32.data(), (size_t)B * 4, cudaMemcpyHostToDevice, s));
+  if (row_seeds_host) T2_CUDA(cudaMemcpyAsync(w.row_seeds, row_seeds_host, (size_t)B * 8, cudaMemcpyHostToDevice, s));
   T2EncoderArgs ea; memset(&ea, 0, sizeof(ea));
   ea.text = w.text; ea.lengths = w.in_lens; ea.B = B; ea.T = T_text; ea.memory = w.memory; ea.ws = w.sub; ea.ws_bytes = w.sub_bytes;
   T2_TRY(encoder_forward(m, &ea, s, true));
@@ -458,6 +474,7 @@ static int infer_host(T2Model* m, const int64_t* text_host, const int64_t* in_le
   da.mode = T2_MODE_INFER; da.impl = impl; da.memory = w.memory; da.memory_lengths = w.in_lens;
   da.B = B; da.T_enc = T_text; da.n_steps_cap = max_steps;
   da.seed = seed; da.gate_threshold = gate_threshold; da.score_mask_value = -INFINITY;
+  da.row_seeds = row_seeds_host ? w.row_seeds : nullptr;
   da.mel = w.mel; da.gate = w.gate; da.align = w.align; da.mel_lengths = w.lens; da.n_steps = w.nsteps; da.ws = w.sub; da.ws_bytes = w.sub_bytes;
   T2_TRY(t2_decoder_run(m, &da, s));
   // the postnet runs over the n decoded frames, as Tacotron2.inference does: its convolutions zero-pad every layer at
@@ -495,7 +512,8 @@ int t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream) {
   if (!a) return fail(T2_ERR_INVALID, "infer_host_lengths: null args");
   if (!a->input_lengths_host) return fail(T2_ERR_INVALID, "infer_host_lengths: null input_lengths_host (use t2_infer_host)");
   return infer_host(m, a->text_host, a->input_lengths_host, a->B, a->T_text, a->max_steps, a->gate_threshold, a->seed, a->impl,
-                    a->mel_post_host, a->mel_lengths_host, a->n_steps_host, a->ws, a->ws_bytes, (cudaStream_t)stream);
+                    a->mel_post_host, a->mel_lengths_host, a->n_steps_host, a->ws, a->ws_bytes, (cudaStream_t)stream,
+                    a->row_seeds_host);
 }
 
 int t2_decoder_profile(const T2DecoderArgs* a, int64_t* out_host) {

@@ -67,7 +67,7 @@ bool persistent_supported(const T2Model* m, const T2DecoderArgs* a);
 size_t persistent_stream_state_bytes(int B, int T_enc);
 int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, cudaStream_t s);
 int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n,
-                          const int32_t* status_host, cudaStream_t s);
+                          const int32_t* status_host, const int32_t* row_step0, cudaStream_t s);
 // continuous batching: rows (ascending) back to the state begin gives them + their processed memory; a chunk's frames of
 // the listed rows to the requests' own buffers
 int persistent_stream_admit(T2Model* m, const T2DecoderArgs* a, void* state, const int32_t* rows, int n_rows, cudaStream_t s);

@@ -367,6 +367,10 @@ struct KParams {
   int b0, Btot;                     // this launch handles batch rows [b0, b0 + B) of Btot (dropout mask / Philox indexing)
   float gate_threshold, score_mask_value, p_att, p_dec;
   uint64_t seed;
+  // per-row prenet keys (INFER; row_seeds == nullptr: p.seed and element (b0 + row) * 256 + column): row r draws with
+  // key row_seeds[b0 + r], element = column, at its own step row_step0[b0 + r] + t (row_step0 == nullptr: t).  Read from
+  // global memory at the draw: a table in shared memory would cost the 3-stage layout its longest T_enc.
+  const uint64_t* row_seeds; const int32_t* row_step0;
   DecoderStash st;                  // training stash for the backward pass (st.ga == nullptr: none)
   int t_begin, t_end;               // this launch runs steps [t_begin, t_end); the whole loop: 0, cap
   // resumable stream (t2_decoder_stream_run; rs_acc == nullptr: none).  The prologue restores and the epilogue saves the
@@ -572,13 +576,21 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       // (warps 2, 3) draw the prenet dropout bits this CTA needs at the END of this step (x1 columns on the projection CTAs, x2 columns on the prenet-2 CTAs)
       if (p.infer && is_lo && cg == 0 && row < p.B && t + 1 < p.cap && (has_p || has_x2)) {
         uint32_t bits = 0;
+        // Philox key, step and the row's first element: one stream per call (b0 + row) * 256 + column, or per row
+        uint64_t seed = p.seed, e0 = (uint64_t)(p.b0 + row) * kPre;
+        uint32_t step = t + 1;
+        if (p.row_seeds) {
+          seed = p.row_seeds[p.b0 + row];
+          e0 = 0;
+          if (p.row_step0) step += p.row_step0[p.b0 + row];
+        }
         if (has_x2) {
           const int col0 = (cta - kX2Cta0) * 8;
           if (p.prenet_keep) {
             const uint8_t* kp = p.prenet_keep + ((long)(t + 1) * 2 + 1) * p.Btot * kPre + (long)(p.b0 + row) * kPre + col0;
             for (int j = 0; j < 8; ++j) bits |= (kp[j] != 0 ? 1u : 0u) << j;
           } else {
-            bits = philox_keep8(p.seed, (t + 1) * 4 + 1, (uint64_t)(p.b0 + row) * kPre + col0, 0.5f);
+            bits = philox_keep8(seed, step * 4 + 1, e0 + col0, 0.5f);
           }
         } else {
           const int pc0 = (cta - kPCta0) * 8;
@@ -587,7 +599,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
             if (col < 0 || col >= kPre) continue;
             const long idx = (long)(p.b0 + row) * kPre + col;
             const bool keep = p.prenet_keep ? p.prenet_keep[((long)(t + 1) * 2 + 0) * p.Btot * kPre + idx] != 0
-                                            : philox_keep(p.seed, (t + 1) * 4 + 0, idx, 0.5f);
+                                            : philox_keep(seed, step * 4 + 0, e0 + col, 0.5f);
             bits |= (keep ? 1u : 0u) << j;
           }
         }
@@ -1183,6 +1195,7 @@ static void slice_params(T2Model* m, const T2DecoderArgs* a, int b0, int nb, KPa
   p.B = nb; p.T = T; p.cap = cap; p.infer = a->mode == T2_MODE_INFER; p.training = a->training;
   p.gate_threshold = a->gate_threshold; p.score_mask_value = a->score_mask_value;
   p.p_att = m->cfg.p_attention_dropout; p.p_dec = m->cfg.p_decoder_dropout; p.seed = a->seed;
+  p.row_seeds = a->row_seeds;
   p.t_begin = 0; p.t_end = cap;
 }
 
@@ -1309,7 +1322,7 @@ int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int
 }
 
 int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n,
-                          const int32_t* status_host, cudaStream_t s) {
+                          const int32_t* status_host, const int32_t* row_step0, cudaStream_t s) {
   for (int b0 = 0, si = 0; b0 < a->B; b0 += kRows, ++si) {
     const int t0 = status_host ? status_host[2 * si] : 0;
     if ((status_host && status_host[2 * si + 1]) || t0 >= a->n_steps_cap) continue;    // this slice has stopped
@@ -1323,6 +1336,7 @@ int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32
     p.t_begin = t0;
     p.t_end = n < a->n_steps_cap - t0 ? t0 + n : a->n_steps_cap;
     p.rs_acc = sl.acc; p.rs_cell = sl.cell; p.rs_att = sl.att; p.rs_done = sl.done; p.rs_status = status + 2 * si;
+    p.row_step0 = row_step0;
     if (pa_precomputed(a->T_enc, p.infer)) p.pa = sl.pa;      // zeroed by begin, left by the previous chunk
     T2_TRY(launch_persistent(p, s));
   }

@@ -239,14 +239,14 @@ int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
       g.seg[0] = {prev, (t == 0) ? 0L : (long)cap * kMel, m->w[W_PRENET0], kMel, kMel};
       g.M = B; g.N = kPre; g.C = w.x1; g.ldc = kPre; g.act = ACT_RELU; g.p_drop = 0.5f;
       if (a->prenet_keep) { g.keep = a->prenet_keep + ((long)t * 2 + 0) * B * kPre; g.ldkeep = kPre; }
-      else { g.philox = 1; g.seed = a->seed; g.site = t * 4 + 0; }
+      else { g.philox = 1; g.seed = a->seed; g.site = t * 4 + 0; g.row_seeds = a->row_seeds; }
       g.skip_flag = skip;
       T2_TRY(gemm_f32(g, s));
       GemmArgs h;
       h.seg[0] = {w.x1, kPre, m->w[W_PRENET1], kPre, kPre};
       h.M = B; h.N = kPre; h.C = w.x2; h.ldc = kPre; h.act = ACT_RELU; h.p_drop = 0.5f;
       if (a->prenet_keep) { h.keep = a->prenet_keep + ((long)t * 2 + 1) * B * kPre; h.ldkeep = kPre; }
-      else { h.philox = 1; h.seed = a->seed; h.site = t * 4 + 1; }
+      else { h.philox = 1; h.seed = a->seed; h.site = t * 4 + 1; h.row_seeds = a->row_seeds; }
       h.skip_flag = skip;
       T2_TRY(gemm_f32(h, s));
       x2 = w.x2;

@@ -59,7 +59,11 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(const GemmArgs a) {
       if (a.act == ACT_RELU) v = fmaxf(v, 0.f);
       else if (a.act == ACT_TANH) v = tanhf(v);
       if (a.keep) v = a.keep[(long)m * a.ldkeep + n] ? v * inv_keep : 0.f;
-      else if (a.philox) v = philox_keep(a.seed, a.site, (uint64_t)m * a.N + n, a.p_drop) ? v * inv_keep : 0.f;
+      else if (a.philox) {
+        const bool keep = a.row_seeds ? philox_keep(a.row_seeds[m], a.site, (uint64_t)n, a.p_drop)
+                                      : philox_keep(a.seed, a.site, (uint64_t)m * a.N + n, a.p_drop);
+        v = keep ? v * inv_keep : 0.f;
+      }
       a.C[(long)m * a.ldc + n] = v;
     }
   }

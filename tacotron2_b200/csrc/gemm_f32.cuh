@@ -24,6 +24,7 @@ struct GemmArgs {
   // dropout on the output: explicit keep mask (M, N) uint8 or Philox(seed, site); p = drop prob
   const uint8_t* keep = nullptr; long ldkeep = 0;
   int philox = 0; uint64_t seed = 0; uint32_t site = 0; float p_drop = 0.f;
+  const uint64_t* row_seeds = nullptr;   // (M) or null: Philox(row_seeds[m], site), element n instead of seed, m * N + n
   const int* skip_flag = nullptr;    // device flag: when *skip_flag != 0 the kernel is a no-op
 };
 

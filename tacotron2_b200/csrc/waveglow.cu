@@ -101,17 +101,22 @@ struct TailRange {
 
 __device__ __forceinline__ int n_rem_of(int k) { return 8 - 2 * (k / 4); }   // 4 (k >= 8), 6 (k >= 4), 8
 
-template <int PASSES>
-__global__ void __launch_bounds__(128) flow_tail_kernel(const TailParams p, const TailRange w) {
+// SEEDED: row b draws its noise as a B = 1 call with seed row_seeds[b] does -- key row_seeds[b], row index 0.  A
+// template parameter, so that the unseeded instantiation compiles to the code it had before row_seeds existed.
+template <int PASSES, bool SEEDED>
+__global__ void __launch_bounds__(128) flow_tail_kernel(const TailParams p, const TailRange w,
+                                                        const uint64_t* __restrict__ row_seeds) {
   const long q = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= p.n_rows) return;
   const int b = (int)(q / p.span), t = (int)(q - (long)b * p.span);
   const bool data = b < p.B && t < p.T;
   if (data && (t < w.lo || t >= w.hi)) return;     // not needed by what follows
   const bool valid = data && (p.len == nullptr || t < p.len[b] * 32);
+  const uint64_t seed = SEEDED && valid ? row_seeds[b] : p.seed;
   auto noise = [&](int c) -> float {
     if (!valid) return 0.f;
     const int ta = w.col0 + t;
+    if (SEEDED) return p.sigma * philox_normal(seed, 0, c, ta);
     return p.sigma * (p.z ? p.z[((long)b * kGroup + c) * w.z_stride + ta] : philox_normal(p.seed, b, c, ta));
   };
   float a[8];
@@ -488,6 +493,7 @@ int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStr
   if (!wa->at_end && out1 + kHaloRight > a->T_mel)
     return fail(T2_ERR_INVALID, "waveglow window: output frames end %d frames before a window end that is not the "
                 "sequence's end; the right halo is %d frames", a->T_mel - out1, kHaloRight);
+  if (a->z && a->row_seeds) return fail(T2_ERR_INVALID, "waveglow: row_seeds and an injected z exclude each other");
   if (a->z && wa->z_frames < frame0 + a->T_mel)
     return fail(T2_ERR_INVALID, "waveglow window: z holds %d frames, the window ends at frame %d", wa->z_frames,
                 frame0 + a->T_mel);
@@ -536,8 +542,14 @@ int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStr
   auto tail = [&](int k, int next) -> int {   // k flows follow this tail (k = 12: the initial draw)
     tp.k = k < kFlows ? k : -1; tp.next = next;
     widen(k, &tr.lo, &tr.hi);
-    if (fp16) flow_tail_kernel<1><<<tail_blocks, 128, 0, s>>>(tp, tr);
-    else flow_tail_kernel<3><<<tail_blocks, 128, 0, s>>>(tp, tr);
+    const uint64_t* rs = a->row_seeds;
+    if (fp16) {
+      if (rs) flow_tail_kernel<1, true><<<tail_blocks, 128, 0, s>>>(tp, tr, rs);
+      else flow_tail_kernel<1, false><<<tail_blocks, 128, 0, s>>>(tp, tr, nullptr);
+    } else {
+      if (rs) flow_tail_kernel<3, true><<<tail_blocks, 128, 0, s>>>(tp, tr, rs);
+      else flow_tail_kernel<3, false><<<tail_blocks, 128, 0, s>>>(tp, tr, nullptr);
+    }
     T2_LAUNCH_CHECK();
     return T2_OK;
   };

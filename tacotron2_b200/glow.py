@@ -171,13 +171,18 @@ class WaveGlow(torch.nn.Module):
         return self._t2
 
     @torch.no_grad()
-    def infer(self, spect, sigma=1.0, lengths=None):
+    def infer(self, spect, sigma=1.0, lengths=None, seeds=None):
         """mel spectrogram (B, n_mel, T_mel) -> audio (B, 256 T_mel) in the spectrogram's dtype (glow.py:251-293).
         lengths (B) in mel frames, optional: row b's samples [0, 256 lengths[b]) are what infer gives for that row's
-        first lengths[b] frames alone; later samples are zero."""
-        return self._engine().infer(self, spect, sigma, lengths, getattr(_tls, "z", None))
+        first lengths[b] frames alone; later samples are zero.
 
-    def infer_stream(self, items, sigma=1.0):
+        seeds: one noise seed per row, B integers in [0, 2**64) as a list, a host tensor or a device tensor (int64 values
+        are taken as their 64-bit pattern).  Row b then draws the noise of ``infer(spect[b:b+1], sigma, seeds=[seeds[b]])``
+        and equals that call bit for bit in any batch; a B = 1 call with seeds=[s] is the unseeded call whose drawn seed
+        was s.  Not together with ``waveglow_noise``.  None: one seed per call from torch's generator, as before."""
+        return self._engine().infer(self, spect, sigma, lengths, getattr(_tls, "z", None), seeds)
+
+    def infer_stream(self, items, sigma=1.0, seeds=None):
         """infer() over the items of ``Tacotron2.inference_stream(...)``, as a generator that hands out audio as soon as
         no later mel frame can change it.
 
@@ -194,8 +199,9 @@ class WaveGlow(torch.nn.Module):
         The stream keeps on the device only the final mel frames later windows can still need (at most the two halos and
         one item's frames).  Several streams, and infer, can be used on one WaveGlow at a time: each stream has its own
         frames, noise seed and position, and they share the module's workspace, so all of them must enqueue on the same
-        CUDA stream (torch's current stream), as successive infer calls do."""
-        return self._engine().stream(self, items, sigma, getattr(_tls, "z", None))
+        CUDA stream (torch's current stream), as successive infer calls do.  seeds: as for infer(); the stream then
+        equals ``infer(..., seeds=seeds)``."""
+        return self._engine().stream(self, items, sigma, getattr(_tls, "z", None), seeds)
 
 
 class _WaveGlowEngine(_engine._Handle):
@@ -250,18 +256,28 @@ class _WaveGlowEngine(_engine._Handle):
         self.last_seed = seed
         return seed
 
-    def _args(self, spect, len32, zt, sigma, seed, audio):
+    def _args(self, spect, len32, zt, sigma, seed, audio, row_seeds=None):
         """T2WaveGlowArgs over spect (B, n_mel, T) on the device, with a workspace of the engine's cache."""
         B, T = int(spect.shape[0]), int(spect.shape[2])
         ws = self._ws.get("infer", _capi.lib().t2_waveglow_workspace_bytes(self.handle, B, T), self.device)
         return _capi.T2WaveGlowArgs(spect.data_ptr(), B, T, _engine._ptr(len32), int(spect.dtype == torch.float16),
-                                    float(sigma), _engine._ptr(zt), seed, audio.data_ptr(), ws.data_ptr(), ws.numel())
+                                    float(sigma), _engine._ptr(zt), seed, audio.data_ptr(), ws.data_ptr(), ws.numel(),
+                                    _engine._ptr(row_seeds))
 
-    def infer(self, module, spect, sigma, lengths, z):
+    def _row_seeds(self, seeds, z, B, what):
+        """seeds as (B,) int64 bit patterns on the device, or None; refused together with injected noise."""
+        if seeds is None:
+            return None
+        if z is not None:
+            raise ValueError("%s: seeds and waveglow_noise exclude each other" % what)
+        return _engine.row_seeds(seeds, B, self.device, what)
+
+    def infer(self, module, spect, sigma, lengths, z, seeds=None):
         self.ensure(module)
         spect = self._spect(spect, "WaveGlow.infer")
         dev = self.device
         B, T = int(spect.shape[0]), int(spect.shape[2])
+        row_seeds = self._row_seeds(seeds, z, B, "WaveGlow.infer")
         audio = torch.empty(B, HOP * T, device=dev, dtype=spect.dtype)
         len32 = None
         if lengths is not None:
@@ -273,24 +289,25 @@ class _WaveGlowEngine(_engine._Handle):
             zt = z.to(device=dev, dtype=torch.float32).contiguous()
             if tuple(zt.shape) != (B, N_GROUP, 32 * T):
                 raise ValueError("waveglow_noise: z must be (%d, %d, %d), got %s" % (B, N_GROUP, 32 * T, tuple(z.shape)))
-        a = self._args(spect, len32, zt, sigma, self._draw_seed(), audio)
+        # a seeded call draws nothing from torch's generator
+        a = self._args(spect, len32, zt, sigma, 0 if row_seeds is not None else self._draw_seed(), audio, row_seeds)
         self._call(_capi.lib().t2_waveglow_infer, C.byref(a))
         return audio
 
-    def infer_window(self, spect, len32, zt, z_frames, sigma, seed, frame0, out0, out1, at_end):
+    def infer_window(self, spect, len32, zt, z_frames, sigma, seed, frame0, out0, out1, at_end, row_seeds=None):
         """Audio (B, 256 (out1 - out0)) of the window-relative frames [out0, out1) of spect, which holds the frames
         [frame0, frame0 + T) of a sequence (t2_waveglow_infer_window).  Call ensure() first."""
         audio = torch.empty(int(spect.shape[0]), HOP * (out1 - out0), device=self.device, dtype=spect.dtype)
-        w = _capi.T2WaveGlowWindowArgs(self._args(spect, len32, zt, sigma, seed, audio), frame0, out0, out1,
+        w = _capi.T2WaveGlowWindowArgs(self._args(spect, len32, zt, sigma, seed, audio, row_seeds), frame0, out0, out1,
                                        z_frames if zt is not None else 0, int(at_end))
         self._call(_capi.lib().t2_waveglow_infer_window, C.byref(w))
         return audio
 
     @torch.no_grad()
-    def stream(self, module, items, sigma, z):
+    def stream(self, module, items, sigma, z, seeds=None):
         """The generator behind WaveGlow.infer_stream."""
         win = FinalWindow("WaveGlow.infer_stream: mel items", "frames", 2, *window_halo())
-        zt = z_frames = seed = None
+        zt = z_frames = seed = row_seeds = None
         for item in items:
             win.check(item)
             post = item["mel_outputs_postnet"]
@@ -299,7 +316,8 @@ class _WaveGlowEngine(_engine._Handle):
                 post = self._spect(post, "WaveGlow.infer_stream")
                 if z is not None:
                     zt, z_frames = self._z(z, int(post.shape[0]), item["frames"][1])
-                seed = self._draw_seed()
+                row_seeds = self._row_seeds(seeds, z, int(post.shape[0]), "WaveGlow.infer_stream")
+                seed = 0 if row_seeds is not None else self._draw_seed()
             span = win.add(item, post)
             if span is None:
                 continue
@@ -307,7 +325,8 @@ class _WaveGlowEngine(_engine._Handle):
             audio = kept.new_empty(kept.shape[0], 0)
             if a1 > a0:                # the window is every kept frame; a row that does not end in it ends at its end
                 audio = self.infer_window(kept.contiguous(), win.lengths(item["mel_lengths"], win.held - win.base), zt,
-                                          z_frames, sigma, seed, win.base, a0 - win.base, a1 - win.base, finished)
+                                          z_frames, sigma, seed, win.base, a0 - win.base, a1 - win.base, finished,
+                                          row_seeds)
             yield dict(samples=(HOP * a0, HOP * a1), audio=audio, mel_lengths=item["mel_lengths"], finished=finished)
             if finished:
                 return

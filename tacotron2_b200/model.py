@@ -20,6 +20,7 @@ import torch
 from torch import nn
 
 from . import _capi
+from . import _engine as _engine_mod
 from ._engine import Engine, current_masks, next_seed
 from .layers import ConvNorm, LinearNorm
 from .utils import get_mask_from_lengths, to_gpu
@@ -437,21 +438,35 @@ class Decoder(_EngineOwner, nn.Module):
             mel, gate, align, _ = self._teacher_forward(memory, decoder_inputs, memory_lengths, False)
         return mel.transpose(1, 2).to(dt), gate.to(dt), align.to(dt)
 
-    def inference(self, memory, memory_lengths=None):
+    def _row_seeds(self, seeds, B, device, what):
+        """seeds (see inference) as the engine's per-row keys, or None; refused with masks and in training mode."""
+        if seeds is None:
+            return None
+        if self.training:
+            raise ValueError("tacotron2_b200: %s: seeds need eval mode (training-mode BatchNorm mixes the rows and the "
+                             "hidden-state dropout is not keyed per row)" % what)
+        if current_masks()["prenet"] is not None:
+            raise ValueError("tacotron2_b200: %s: seeds and injected prenet masks exclude each other" % what)
+        return _engine_mod.row_seeds(seeds, B, device, "tacotron2_b200: " + what)
+
+    def inference(self, memory, memory_lengths=None, seeds=None):
         """Free-running pass (model.py:418-454), batched: per-row stop latch, see README "batched
         inference".  Returns mel (B, n_mel, T), gate (B, T, 1), alignments (B, T, T_enc); T = steps
         until every row has fired (or max_decoder_steps); ``self.mel_lengths`` holds per-row lengths.  In training mode
         the attention / decoder hidden states take their dropout as in the reference's decode() (model.py:355-356,
         370-371); injected att / dec masks are (max_decoder_steps, B, 1024).  memory_lengths (B,) integers in 1..T_enc,
         any order: row b attends to memory[b, :memory_lengths[b]] only and its outputs equal those of a call on that
-        slice alone, bit for bit; its alignments past memory_lengths[b] are zero."""
+        slice alone, bit for bit; its alignments past memory_lengths[b] are zero.  seeds: B integers in [0, 2**64) (list,
+        host or device tensor), eval mode only: row b draws the prenet dropout of a B = 1 call seeded seeds[b], so its
+        outputs equal that call's bit for bit in any batch."""
         memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
         eng = self._t2_engine()
+        row_seeds = self._row_seeds(seeds, memory.size(0), eng.device, "Decoder.inference")
         masks = current_masks()
         mel, gate, align, lengths, n_steps = eng.decoder(
             memory, _capi.MODE_INFER, self.max_decoder_steps, memory_lengths=memory_lengths, training=self.training,
             prenet_keep=masks["prenet"],
-            att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold)
+            att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold, row_seeds=row_seeds)
         n = int(n_steps.item())                      # the one host sync of the whole loop (model.py:443 syncs every step)
         self.mel_lengths = lengths
         if n == self.max_decoder_steps and bool((lengths >= n).any()):
@@ -461,7 +476,7 @@ class Decoder(_EngineOwner, nn.Module):
         dt = memory.dtype
         return (mel[:, :n].transpose(1, 2).to(dt), gate[:, :n].unsqueeze(-1).to(dt), align[:, :n].to(dt))
 
-    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None):
+    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None, row_seeds=None):
         """The persistent decoder in chunks of chunk_steps steps.  Yields (t0, t1, finished, stream): frames [t0, t1) are
         the new ones that every row has produced and that no frame within `halo` steps of them can still change, i.e. all
         frames up to the steps run less `halo` while any row is live, and all of them once every 64-row slice has
@@ -471,7 +486,7 @@ class Decoder(_EngineOwner, nn.Module):
             raise ValueError("tacotron2_b200: chunk_steps must be >= 1 (got %d)" % chunk_steps)
         eng = self._t2_engine()
         st = eng.decoder_stream(memory, self.max_decoder_steps, prenet_keep=current_masks()["prenet"],
-                                gate_threshold=self.gate_threshold, memory_lengths=memory_lengths)
+                                gate_threshold=self.gate_threshold, memory_lengths=memory_lengths, row_seeds=row_seeds)
         t0 = 0
         while True:
             live_steps, n, finished = st.run(chunk_steps)
@@ -488,20 +503,21 @@ class Decoder(_EngineOwner, nn.Module):
                 return
             t0 = t1
 
-    def inference_stream(self, memory, chunk_steps=32, memory_lengths=None):
+    def inference_stream(self, memory, chunk_steps=32, memory_lengths=None, seeds=None):
         """inference() in chunks of ``chunk_steps`` decoder steps, as a generator: one item per chunk that produced
         frames, a dict with ``frames`` = (t0, t1) (the same for every row), ``mel_outputs`` (B, n_mel, t1-t0),
         ``gate_outputs`` (B, t1-t0, 1), ``alignments`` (B, t1-t0, T_enc), ``mel_lengths`` (B,) int32 on the device with -1
         for rows that are still live, and ``finished``.  A decoder frame is handed out as soon as every row has produced
         it; concatenated along time the items are bit-identical to inference() (same weights, memory, memory_lengths,
-        masks / seed).  Evaluation mode only: the resumable decoder applies no hidden-state dropout, which inference()
-        does in training mode."""
+        masks / seed / seeds).  Evaluation mode only: the resumable decoder applies no hidden-state dropout, which
+        inference() does in training mode."""
         if self.training:
             raise RuntimeError("tacotron2_b200: Decoder.inference_stream needs eval mode (in training mode inference() "
                                "applies the attention / decoder dropout, which the resumable decoder does not)")
         memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
+        row_seeds = self._row_seeds(seeds, memory.size(0), self._t2_engine().device, "Decoder.inference_stream")
         dt = memory.dtype
-        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths):
+        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths, row_seeds):
             yield dict(frames=(t0, t1), mel_outputs=st.mel[:, t0:t1].transpose(1, 2).to(dt),
                        gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
                        mel_lengths=st.mel_lengths.clone(), finished=finished)
@@ -638,7 +654,7 @@ class Tacotron2(_EngineOwner, nn.Module):
             outputs = [o.to(cast) for o in outputs]
         return self.parse_output(outputs, output_lengths)
 
-    def inference(self, inputs, input_lengths=None):
+    def inference(self, inputs, input_lengths=None, seeds=None):
         """model.py:517-529, batched.  For B > 1 frames at t >= mel_lengths[b] of mel_outputs and
         mel_outputs_postnet are zero (same convention as parse_output); ``self.mel_lengths`` holds
         the per-row lengths.  B == 1 is exactly the reference.
@@ -646,13 +662,20 @@ class Tacotron2(_EngineOwner, nn.Module):
         input_lengths (B,) integers in 1..T_text, on the host or the device, in any order: texts of different lengths in
         one batch.  Row b then computes what ``inference(inputs[b:b+1, :input_lengths[b]])`` computes, bit for bit (its
         frames up to the batch's step count, alignments[b, :, :input_lengths[b]], mel_lengths[b]); the ids past its length
-        are ignored and alignments[b, :, input_lengths[b]:] is zero.  None: every row is T_text long."""
+        are ignored and alignments[b, :, input_lengths[b]:] is zero.  None: every row is T_text long.
+
+        seeds: one seed per utterance, B integers in [0, 2**64) as a list, a host tensor or a device tensor (int64 values
+        are taken as their 64-bit pattern); eval mode only, not together with injected prenet masks.  Row b then draws the
+        prenet dropout that ``inference(inputs[b:b+1, :input_lengths[b]], seeds=[seeds[b]])`` draws, so it reproduces that
+        call bit for bit in any batch, slice, stream or server slot.  A B = 1 call with seeds=[s] is the unseeded call
+        whose engine seed was s.  None: one seed per call (the next engine seed), as before."""
         lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
         eng = self._t2_engine()
+        row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference")
         memory = eng.encoder(text=inputs, lengths=lengths_in, training=self.training, keep=current_masks()["enc"],
                              per_row=lengths_in is not None)
         memory = memory.to(self._t2_out_dtype())     # a .half() model hands half tensors between its modules (ipynb:89-90)
-        mel_outputs, gate_outputs, alignments = self.decoder.inference(memory, memory_lengths=lengths_in)
+        mel_outputs, gate_outputs, alignments = self.decoder.inference(memory, memory_lengths=lengths_in, seeds=row_seeds)
         lengths = self.decoder.mel_lengths
         self.mel_lengths = lengths
         mel_btc = mel_outputs.transpose(1, 2)
@@ -667,7 +690,7 @@ class Tacotron2(_EngineOwner, nn.Module):
             mel_outputs = mel_outputs.masked_fill(pad.unsqueeze(1), 0.0)
         return self.parse_output([mel_outputs, mel_outputs_postnet, gate_outputs, alignments])
 
-    def inference_stream(self, inputs, chunk_steps=32, input_lengths=None):
+    def inference_stream(self, inputs, chunk_steps=32, input_lengths=None, seeds=None):
         """inference() as a generator that hands out frames while the decoder runs (README "streaming inference").
 
         The encoder runs once; the decoder runs in chunks of ``chunk_steps`` steps.  Each item is a dict describing frames
@@ -677,13 +700,14 @@ class Tacotron2(_EngineOwner, nn.Module):
         handed out once the decoder has run step t+10 or every row has stopped; it is never revised.  Concatenated along
         time the items are bit-identical to inference() with the same weights, inputs and dropout masks / seed.  After the
         last item ``self.mel_lengths`` and the max-steps warning are as after inference().  input_lengths: as for
-        inference(), whose output the items then concatenate to.  Evaluation mode only: in training mode BatchNorm
-        normalises over the whole sequence, so no frame is final before the last one."""
+        inference(), whose output the items then concatenate to.  seeds: as for inference().  Evaluation mode only: in
+        training mode BatchNorm normalises over the whole sequence, so no frame is final before the last one."""
         if self.training:
             raise RuntimeError("tacotron2_b200: inference_stream needs eval mode (training-mode BatchNorm uses the statistics "
                                "of the whole sequence, so no postnet frame is final before the decoder ends)")
         lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
         eng = self._t2_engine()
+        row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference_stream")
         memory = eng.encoder(text=inputs, lengths=lengths_in, training=False, keep=current_masks()["enc"],
                              per_row=lengths_in is not None)
         dt = self._t2_out_dtype()
@@ -691,7 +715,7 @@ class Tacotron2(_EngineOwner, nn.Module):
         multi = inputs.size(0) > 1
         ragged = _ragged(lengths_in, inputs.size(1))
         halo = POSTNET_HALO
-        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in):
+        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in, row_seeds):
             if finished:
                 self.mel_lengths = st.mel_lengths
             lengths = st.mel_lengths
@@ -736,17 +760,22 @@ class Tacotron2(_EngineOwner, nn.Module):
         server.backend = EngineBackend(self, server.slots, server.max_text_len, server.chunk_steps, seed)
         return server
 
-    def inference_many(self, texts, slots=64, max_text_len=None, chunk_steps=32, max_decoder_steps=None):
+    def inference_many(self, texts, slots=64, max_text_len=None, chunk_steps=32, max_decoder_steps=None, seeds=None):
         """Every text of ``texts`` (1-D integer tensors) through an inference_server; returns the results in input order.
-        max_text_len: default the longest text; max_decoder_steps: one limit for all, or one per text."""
+        max_text_len: default the longest text; max_decoder_steps: one limit for all, or one per text.  seeds: one per text
+        (as for inference()); result i then equals ``inference(texts[i][None], seeds=[seeds[i]])`` bit for bit."""
         texts = list(texts)
         if not texts:
             return []
         if max_text_len is None:
             max_text_len = max(int(torch.as_tensor(t).numel()) for t in texts)
         limits = max_decoder_steps if isinstance(max_decoder_steps, (list, tuple)) else [max_decoder_steps] * len(texts)
+        per_text = [None] * len(texts)
+        if seeds is not None:       # checked before anything runs; the server takes each as a Python int
+            bits = _engine_mod.row_seeds(seeds, len(texts), torch.device("cpu"), "tacotron2_b200: inference_many")
+            per_text = [int(v) & 0xFFFFFFFFFFFFFFFF for v in bits.tolist()]
         server = self.inference_server(min(int(slots), len(texts)), max(1, max_text_len), chunk_steps)
-        ids = [server.submit(t, limit) for t, limit in zip(texts, limits)]
+        ids = [server.submit(t, limit, seed=sd) for t, limit, sd in zip(texts, limits, per_text)]
         results = {r["id"]: r for r in server.run()}
         return [results[i] for i in ids]
 

@@ -7,8 +7,13 @@ that drives the engine is ``EngineBackend`` (``Tacotron2.inference_server`` buil
 
 Step numbering: every chunk runs as local steps [0, n) of the resumable decoder into chunk-sized buffers.  The decoder
 kernel keeps no step counter in its saved state, so a slot's position in its own request is known to the scheduler alone:
-request r that has run s steps has, in the next chunk, its step s + i at local step i."""
+request r that has run s steps has, in the next chunk, its step s + i at local step i.
+
+Seeded requests (``submit(..., seed=s)``) draw the prenet dropout of ``inference(text[None], seeds=[s])``: each chunk
+hands the kernel every slot's seed and its request's step count s, and the slot's local step i draws its request's step
+s + i under that seed."""
 import collections
+import numbers
 
 import torch
 
@@ -18,8 +23,8 @@ WARNING = "Warning! Reached max decoder steps"      # the line Decoder.inference
 class Request:
     """One queued or running utterance."""
 
-    def __init__(self, rid, text, limit, keep):
-        self.id, self.text, self.limit, self.keep = rid, text, limit, keep
+    def __init__(self, rid, text, limit, keep, seed=None):
+        self.id, self.text, self.limit, self.keep, self.seed = rid, text, limit, keep, seed
         self.steps = 0            # decoder steps of this request that earlier chunks ran
         self.slot = None
         self.out = None           # the backend's output buffers of this request
@@ -54,18 +59,22 @@ class InferenceServer:
         self.queue = collections.deque()
         self.table = [None] * slots          # slot -> Request
         self.injected = None                 # whether this session's requests carry prenet masks (fixed by the first)
+        self.seeded = None                   # whether they carry seeds (fixed by the first)
         self.chunks = 0                      # chunks launched
         self.row_steps = 0                   # slots x decoder steps launched, over 64-row slices that ran
         self._next_id = 0
 
     # -- queue --------------------------------------------------------------------------------------
-    def submit(self, text_ids, max_decoder_steps=None, prenet_keep=None):
+    def submit(self, text_ids, max_decoder_steps=None, prenet_keep=None, seed=None):
         """Queues one text: a 1-D integer tensor of 1..max_text_len symbol ids.  max_decoder_steps: this request's own
         limit (default: the model's).  Returns the request id.  Everything is checked here, before anything runs.
 
+        seed: an integer in [0, 2**64).  The request then equals ``inference(text_ids[None], seeds=[seed])`` under its own
+        limit, bit for bit, whatever slot, chunk or neighbours it gets, and its result carries ``seed``.
+
         prenet_keep is the test hook, the counterpart of ``dropout_masks(prenet=...)``: this request's (steps, 2, 256)
         uint8 keep mask with steps >= its limit; row t is the mask of its own step t.  A session takes masks for all of
-        its requests or for none."""
+        its requests or for none, and likewise seeds."""
         if not torch.is_tensor(text_ids):
             text_ids = torch.as_tensor(text_ids)
         if text_ids.dtype.is_floating_point or text_ids.dtype.is_complex or text_ids.dtype == torch.bool:
@@ -86,13 +95,30 @@ class InferenceServer:
                 raise ValueError("tacotron2_b200: prenet_keep must have shape (steps >= %d, 2, 256) (got %s)"
                                  % (limit, tuple(prenet_keep.shape)))
             prenet_keep = prenet_keep.to(device="cpu", dtype=torch.uint8).contiguous()
+        if seed is not None:
+            if torch.is_tensor(seed):
+                if seed.numel() != 1 or seed.dtype == torch.bool or seed.dtype.is_floating_point or seed.dtype.is_complex:
+                    raise TypeError("tacotron2_b200: seed must be one integer (got a %s tensor of shape %s)"
+                                    % (seed.dtype, tuple(seed.shape)))
+                seed = int(seed.item()) & 0xFFFFFFFFFFFFFFFF if seed.dtype == torch.int64 else int(seed.item())
+            if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
+                raise TypeError("tacotron2_b200: seed must be an integer (got %r)" % (seed,))
+            seed = int(seed)
+            if not 0 <= seed < 1 << 64:
+                raise ValueError("tacotron2_b200: seed %d is outside [0, 2**64)" % seed)
+            if prenet_keep is not None:
+                raise ValueError("tacotron2_b200: seed and prenet_keep exclude each other")
+        if self.seeded is None:
+            self.seeded = seed is not None
+        elif self.seeded != (seed is not None):
+            raise ValueError("tacotron2_b200: a server takes a seed for every request or for none")
         if self.injected is None:
             self.injected = prenet_keep is not None
         elif self.injected != (prenet_keep is not None):
             raise ValueError("tacotron2_b200: a server takes prenet_keep for every request or for none")
         rid = self._next_id
         self._next_id += 1
-        self.queue.append(Request(rid, text_ids.detach().to(device="cpu", dtype=torch.int64), limit, prenet_keep))
+        self.queue.append(Request(rid, text_ids.detach().to(device="cpu", dtype=torch.int64), limit, prenet_keep, seed))
         return rid
 
     def idle(self):
@@ -126,7 +152,13 @@ class InferenceServer:
             return []
         n = self.chunk_steps
         keep = self.chunk_mask(occupied) if self.injected else None
-        self.backend.launch(n, self.chunks, keep, [slot for slot, _ in occupied])
+        if self.seeded:     # every slot's request seed and the steps it ran before this chunk (idle slots: 0, 0)
+            seeds, step0 = [0] * self.slots, [0] * self.slots
+            for slot, r in occupied:
+                seeds[slot], step0[slot] = r.seed, r.steps
+            self.backend.launch(n, self.chunks, keep, [slot for slot, _ in occupied], row_seeds=(seeds, step0))
+        else:
+            self.backend.launch(n, self.chunks, keep, [slot for slot, _ in occupied])
         self.chunks += 1
         # before the host knows where a row fired: all the frames the chunk can hold of the request; what lies past
         # its length is cut when the result is made
@@ -177,6 +209,9 @@ class EngineBackend:
         self.stream = eng.decoder_stream(memory, chunk_steps + 1, prenet_keep=keep,
                                          gate_threshold=model.decoder.gate_threshold, memory_lengths=lengths)
         self.keep_ptr = self.stream.args.dec.prenet_keep
+        # a seeded session's per-slot seeds (64-bit patterns) and request step counts, rewritten before every chunk
+        self.row_seeds = torch.zeros(slots, device=dev, dtype=torch.int64)
+        self.row_step0 = torch.zeros(slots, device=dev, dtype=torch.int32)
 
     def admit(self, pairs):
         """pairs: (slot, request), slots ascending.  The new texts run through the encoder as one ragged batch; their
@@ -202,13 +237,22 @@ class EngineBackend:
             r.out = (f32_buffer(dev, r.limit, self.n_mel), f32_buffer(dev, r.limit), f32_buffer(dev, r.limit, lens[i]))
         st.admit([slot for slot, _ in pairs])
 
-    def launch(self, n, chunk_index, keep, slots):
+    def launch(self, n, chunk_index, keep, slots, row_seeds=None):
+        """row_seeds: None or (seeds, step0), one entry per slot (see the module docstring)."""
         st = self.stream
         if keep is not None:
             st.keep.copy_(keep)
         st.args.dec.prenet_keep = self.keep_ptr if keep is not None else None
+        step0 = None
+        if row_seeds is not None:
+            seeds, steps = row_seeds
+            self.row_seeds.copy_(torch.tensor([v - (1 << 64) if v >= 1 << 63 else v for v in seeds], dtype=torch.int64))
+            self.row_step0.copy_(torch.tensor(steps, dtype=torch.int32))
+            step0 = self.row_step0
+        st.args.dec.row_seeds = self.row_seeds.data_ptr() if row_seeds is not None else None
         live = {slot // 64 for slot in slots}
-        st.launch_chunk(n, chunk_seed(self.seed, chunk_index), [i for i in range(st.n_slices) if i not in live])
+        st.launch_chunk(n, chunk_seed(self.seed, chunk_index), [i for i in range(st.n_slices) if i not in live],
+                        row_step0=step0)
 
     def collect(self, entries):
         """entries: (slot, request, its steps before the chunk, frames to take)."""
@@ -237,5 +281,7 @@ class EngineBackend:
                                 mel_outputs_postnet=post[i:i + 1, :, :L].to(dt),
                                 gate_outputs=gate[:L].view(1, L, 1).to(dt), alignments=align[:L].unsqueeze(0).to(dt),
                                 mel_length=L, hit_max_steps=r.hit_max_steps))
+            if r.seed is not None:
+                results[-1]["seed"] = r.seed
             r.out = None
         return results
