@@ -115,36 +115,10 @@ int pack_model(T2Model* m, cudaStream_t s) {
   return T2_OK;
 }
 
-// ---- decoder workspace --------------------------------------------------------------------------
-static void decoder_ws_layout(Carve& c, int B, int T, int cap, DecoderWs* w) {
-  w->pm = c.take<float>((size_t)B * T * kAtt);
-  // the zero-initialised states: packed floats, one block that one memset clears
-  w->state_begin = c.take<char>(0);
-  const size_t state0 = c.off;
-  w->ah = c.take<float>((size_t)B * kARnn, alignof(float)); w->ac = c.take<float>((size_t)B * kARnn, alignof(float));
-  w->dh = c.take<float>((size_t)B * kDRnn, alignof(float)); w->dc = c.take<float>((size_t)B * kDRnn, alignof(float));
-  w->ctx = c.take<float>((size_t)B * kEnc, alignof(float));
-  w->aw = c.take<float>((size_t)B * T, alignof(float)); w->awc = c.take<float>((size_t)B * T, alignof(float));
-  w->state_bytes = c.off - state0;
-  w->x1 = c.take<float>((size_t)B * kPre); w->x2 = c.take<float>((size_t)B * kPre);
-  w->gates = c.take<float>((size_t)B * 4 * kARnn);
-  w->proj = c.take<float>((size_t)B * (kMel + 1));
-  w->ctrl = c.take<DecoderCtrl>(1);
-  persistent_ws_layout(c, T, cap, w);
-}
-
-size_t decoder_ws_bytes(int B, int T, int cap) {
-  Carve c(nullptr, kDecoderWsAlign);
-  DecoderWs w;
-  decoder_ws_layout(c, B, T, cap, &w);
-  return c.bytes();
-}
-
-int decoder_ws_carve(const T2DecoderArgs* a, DecoderWs* w) {
-  if (a->ws_bytes < decoder_ws_bytes(a->B, a->T_enc, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
-  Carve c(a->ws, kDecoderWsAlign);
-  decoder_ws_layout(c, a->B, a->T_enc, a->n_steps_cap, w);
-  return T2_OK;
+// ---- decoder workspace: the implementation is chosen per call (T2_IMPL_AUTO), so it fits either layout ----------------
+static size_t decoder_ws_bytes(int B, int T, int cap) {
+  const size_t sw = stepwise_ws_bytes(B, T), pe = persistent_ws_bytes(B, T, cap);
+  return sw > pe ? sw : pe;
 }
 
 // per-row prenet keys: evaluation-mode INFER only (the hidden-state dropout of training mode is keyed by the call), and
@@ -167,6 +141,7 @@ static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a) {
     return fail(T2_ERR_INVALID, "decoder: null tensor pointer");
   if (a->mode == T2_MODE_TEACHER && !a->teacher_prenet) return fail(T2_ERR_INVALID, "decoder: teacher mode needs teacher_prenet");
   if (a->mode != T2_MODE_TEACHER && a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "decoder: bad mode %d", a->mode);
+  if (a->ws_bytes < decoder_ws_bytes(a->B, a->T_enc, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
   return check_row_seeds(a, "decoder");
 }
 
@@ -518,10 +493,9 @@ int t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream) {
 
 int t2_decoder_profile(const T2DecoderArgs* a, int64_t* out_host) {
   if (!a || !out_host) return fail(T2_ERR_INVALID, "decoder_profile: null argument");
-  DecoderWs w;
-  T2_TRY(decoder_ws_carve(a, &w));
+  if (a->ws_bytes < decoder_ws_bytes(a->B, a->T_enc, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
   T2_CUDA(cudaDeviceSynchronize());
-  T2_CUDA(cudaMemcpy(out_host, w.ctrl->prof, sizeof(long long) * 72, cudaMemcpyDeviceToHost));
+  T2_CUDA(cudaMemcpy(out_host, persistent_ws_ctrl(a)->prof, sizeof(long long) * 72, cudaMemcpyDeviceToHost));
   return T2_OK;
 }
 

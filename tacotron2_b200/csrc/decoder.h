@@ -1,4 +1,5 @@
-// Decoder workspace layout shared by the stepwise and the persistent implementation.
+// Decoder: the control block and the training stash, and the entry points of the stepwise (decoder_stepwise.cu), the
+// persistent (decoder_persistent.cu) and the backward (decoder_backward.cu) implementation.
 #pragma once
 #include "model.h"
 
@@ -21,21 +22,7 @@ struct DecoderCtrl {
   unsigned int dh_count[16]; int pad6_[16];   // the same for dh
 };
 
-struct DecoderWs {
-  float* pm;               // processed_memory (B, T, 128)          model.py:288
-  char* state_begin; size_t state_bytes;   // zero-initialised block (model.py:258-284):
-  float *ah, *ac, *dh, *dc;                // (B, 1024) each
-  float* ctx;              // (B, 512)
-  float *aw, *awc;         // (B, T)
-  float *x1, *x2;          // prenet activations (B, 256)
-  float* gates;            // (B, 4096)
-  float* proj;             // (B, 81)
-  DecoderCtrl* ctrl;
-  uint8_t* images;         // persistent kernel: activation images and q (decoder_persistent.cu)
-  uint8_t* teacher_img;    // persistent kernel, teacher forcing: the x2 images of every step
-  float* pa;               // persistent kernel, inference: the location term of the next step (decoder_persistent.cu)
-};
-constexpr size_t kDecoderWsAlign = 1024;   // largest alignment of a decoder workspace region (teacher_img)
+constexpr size_t kDecoderWsAlign = 1024;   // base alignment of a decoder workspace (the persistent slice block)
 
 // Training stash written by the persistent kernel in teacher-forced mode and read by the backward pass
 // (decoder_backward.cu).  All fp32, step-major.  h = the hidden state that recurs (after dropout).
@@ -53,9 +40,10 @@ inline void decoder_stash_layout(Carve& c, int B, int T, DecoderStash* s) {
 }
 inline size_t decoder_stash_bytes(int B, int T) { Carve c(nullptr); DecoderStash s; decoder_stash_layout(c, B, T, &s); return c.bytes(); }
 
-size_t decoder_ws_bytes(int B, int T, int cap);
-void persistent_ws_layout(Carve& c, int T, int cap, DecoderWs* w);
-int decoder_ws_carve(const T2DecoderArgs* a, DecoderWs* w);
+// t2_decoder_workspace_bytes is the larger of the two implementations' layouts
+size_t stepwise_ws_bytes(int B, int T);
+size_t persistent_ws_bytes(int B, int T, int cap);
+DecoderCtrl* persistent_ws_ctrl(const T2DecoderArgs* a);   // the control block (and phase profile) of a persistent run
 int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
 int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
 int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s);

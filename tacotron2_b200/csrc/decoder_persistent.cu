@@ -273,6 +273,9 @@ __device__ __forceinline__ float warp_max_f(float v) {
   return v;
 }
 
+// floats of a padded attention-weight row: T_enc + the location conv's kLocK - 1 zero taps, rounded up to whole float4
+__host__ __device__ constexpr int att_pad_len(int T) { return (T + kLocK - 1 + 3) & ~3; }
+
 // Dynamic shared memory of the persistent decoder for (T_enc, ring stages): the kernel carves it and the host sizes
 // the launch from it, which decides the ring depth and the longest T_enc.  The regions are packed in this order.
 struct PersistentSmem {
@@ -291,7 +294,7 @@ struct PersistentSmem {
   float* ep;                       // [4][ntiles * 128] energy partial sums
 };
 __host__ __device__ __forceinline__ void persistent_smem_layout(Carve& c, int T, int nstages, PersistentSmem* s) {
-  const int tpp = (T + kLocK - 1 + 3) & ~3, ntiles = (T + 127) >> 7;
+  const int tpp = att_pad_len(T), ntiles = (T + 127) >> 7;
   s->stage0 = c.take<uint8_t>((size_t)nstages * kStageBytes, 1);
   s->weff = c.take<uint8_t>(kWeffBytes, 1);
   s->acc = c.take<float>(kAccBytes / 4, 1);
@@ -353,7 +356,7 @@ struct KParams {
   // tensors
   const float* memory; const float* pm; const int32_t* mem_len;
   const uint8_t* prenet_keep; const uint8_t* att_keep; const uint8_t* dec_keep;
-  // activation images (workspace)
+  // activation images, q and pa: the launch's slice block (SliceState, host side); pm: rows b0.. of the buffer's (B, T, 128)
   uint8_t* x2_img; uint8_t* ah_img; uint8_t* ctx_img; uint8_t* dh_img; uint8_t* x1_img;
   const uint8_t* teacher_x2_img;   // (cap, 4 chunks) or null
   float* q;                         // (64, 128) fp32
@@ -374,7 +377,8 @@ struct KParams {
   DecoderStash st;                  // training stash for the backward pass (st.ga == nullptr: none)
   int t_begin, t_end;               // this launch runs steps [t_begin, t_end); the whole loop: 0, cap
   // resumable stream (t2_decoder_stream_run; rs_acc == nullptr: none).  The prologue restores and the epilogue saves the
-  // on-chip state that lives past a step boundary; the activation images, q and the processed memory stay in place.
+  // on-chip state that lives past a step boundary, in the saved part of the slice block; the activation images, q, pa and
+  // the processed memory stay in place.
   float* rs_acc;                    // (kG, kRows x kAccPitch) accumulator tiles: next-step partial products
   float* rs_cell;                   // (kG, 4 column groups, kRows) float4 {c_att[0], c_att[1], c_dec[0], c_dec[1]}
   float* rs_att;                    // (kG, 2, padded TP) previous | cumulative attention weights
@@ -456,7 +460,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     ptx::fence_barrier_init();
   }
   const bool resume = p.rs_acc != nullptr;       // a stream's chunk: its state was zeroed by begin or saved by the last chunk
-  const int tpp = (TP + 3) & ~3;
+  const int tpp = att_pad_len(T);
   for (int i = tid; i < kRows * kAccPitch; i += kThreads)                  // every MMA accumulates
     s_acc[i] = resume ? p.rs_acc[(size_t)cta * kRows * kAccPitch + i] : 0.f;
   for (int i = tid; i < 32; i += kThreads) { s_bias_a[i] = p.bias_a[cta * 32 + i]; s_bias_d[i] = p.bias_d[cta * 32 + i]; }
@@ -1036,20 +1040,81 @@ static int persistent_stages(int T) {
   return want;
 }
 
-constexpr int kImageChunks = 4 + 16 + 8 + 16 + 4;          // K chunks of the x2, ah, ctx, dh and x1 images
-constexpr size_t kImagesBytes = (size_t)kImageChunks * kXChunkBytes + (size_t)kRows * kAtt * 4;   // + q
-
 // the next step's location term of 64 rows (KParams::pa); none where no ring depth holds its tile
 __host__ __device__ static size_t pa_buffer_floats(int T) { return pa_tile_fits(T, kMaxStages) ? (size_t)kRows * pa_tile_bytes(T) / 4 : 0; }
 // whether a launch computes pa during the x2 wait (INFER, and the tile fits the ring it runs with)
 static bool pa_precomputed(int T, bool infer) { return infer && pa_tile_fits(T, persistent_stages(T)); }
 
-// the persistent kernel's part of the decoder workspace: activation images x2 (4 chunks), ah (16), ctx (8), dh (16),
-// x1 (4) and q (64 x 128 fp32); for teacher forcing the x2 images of every step (cap x 4 chunks); the pa buffer
-void persistent_ws_layout(Carve& c, int T, int cap, DecoderWs* w) {
-  w->images = c.take<uint8_t>(kImagesBytes);
-  w->teacher_img = c.take<uint8_t>((size_t)cap * 4 * kXChunkBytes, 1024);
-  w->pa = c.take<float>(pa_buffer_floats(T), 16);
+// ---------------------------------------------------------------------------------------------
+// device state of the 64-row slices.  A slice buffer is the processed memory of all B rows (B, T_enc, 128), indexed by
+// absolute row, then n_blocks slice blocks of one size: block i sits at blocks + i * stride.  t2_decoder_run has one block,
+// which its consecutive 64-row launches reuse; a stream has one per slice, and those blocks also carry the state a launch
+// saves at its end and restores at its start.
+// ---------------------------------------------------------------------------------------------
+constexpr size_t kSliceAlign = 1024;   // every region of a block, and the stride
+struct SliceState {
+  // every launch; a whole run zeroes the regions before pa with one memset
+  DecoderCtrl* ctrl;                   // counters zeroed before every launch; a stream's stop latch is carried in `done`
+  uint8_t *x2, *ah, *ctx, *dh, *x1;    // activation images of 4, 16, 8, 16 and 4 K chunks
+  float* q;                            // (64, 128)
+  float* pa;                           // location term of the next step (KParams::pa), pa_buffer_floats(T)
+  // saved on-chip state (KParams::rs_*; streams only)
+  float* acc; float* cell; float* att; int32_t* done;
+};
+__host__ __device__ static void slice_block_layout(Carve& c, int T, bool saved, SliceState* s) {
+  s->ctrl = c.take<DecoderCtrl>(1, kSliceAlign);
+  s->x2 = c.take<uint8_t>(4 * kXChunkBytes, kSliceAlign);
+  s->ah = c.take<uint8_t>(16 * kXChunkBytes, kSliceAlign);
+  s->ctx = c.take<uint8_t>(8 * kXChunkBytes, kSliceAlign);
+  s->dh = c.take<uint8_t>(16 * kXChunkBytes, kSliceAlign);
+  s->x1 = c.take<uint8_t>(4 * kXChunkBytes, kSliceAlign);
+  s->q = c.take<float>((size_t)kRows * kAtt, kSliceAlign);
+  s->pa = c.take<float>(pa_buffer_floats(T), kSliceAlign);
+  s->acc = saved ? c.take<float>((size_t)kG * kRows * kAccPitch, kSliceAlign) : nullptr;
+  s->cell = saved ? c.take<float>((size_t)kG * 4 * kRows * 4, kSliceAlign) : nullptr;
+  s->att = saved ? c.take<float>((size_t)kG * 2 * att_pad_len(T), kSliceAlign) : nullptr;
+  s->done = saved ? c.take<int32_t>(kRows, kSliceAlign) : nullptr;
+}
+
+struct SliceBuffer {
+  float* pm;                           // processed memory (B, T, 128)
+  uint8_t* blocks; size_t stride;
+  int T; bool saved;
+  __host__ __device__ SliceState block(int i) const {
+    Carve c(blocks + i * stride, 1);
+    SliceState s;
+    slice_block_layout(c, T, saved, &s);
+    return s;
+  }
+};
+__host__ __device__ static SliceBuffer slice_buffer_layout(Carve& c, int B, int T, int n_blocks, bool saved) {
+  SliceBuffer b;
+  b.T = T; b.saved = saved;
+  b.pm = c.take<float>((size_t)B * T * kAtt, kSliceAlign);
+  Carve one(nullptr, 1);
+  SliceState s;
+  slice_block_layout(one, T, saved, &s);
+  b.stride = (one.off + kSliceAlign - 1) & ~(kSliceAlign - 1);
+  b.blocks = c.take<uint8_t>((n_blocks - 1) * b.stride + one.off, kSliceAlign);
+  return b;
+}
+
+// the persistent decoder's workspace: one slice block, then the teacher-forcing x2 images of every step (cap x 4 chunks)
+static SliceBuffer persistent_ws_layout(Carve& c, int B, int T, int cap, uint8_t** teacher_img) {
+  const SliceBuffer b = slice_buffer_layout(c, B, T, 1, false);
+  *teacher_img = c.take<uint8_t>((size_t)cap * 4 * kXChunkBytes, kSliceAlign);
+  return b;
+}
+size_t persistent_ws_bytes(int B, int T, int cap) {
+  Carve c(nullptr, kDecoderWsAlign);
+  uint8_t* teacher_img;
+  persistent_ws_layout(c, B, T, cap, &teacher_img);
+  return c.bytes();
+}
+DecoderCtrl* persistent_ws_ctrl(const T2DecoderArgs* a) {
+  Carve c(a->ws, kDecoderWsAlign);
+  uint8_t* teacher_img;
+  return persistent_ws_layout(c, a->B, a->T_enc, a->n_steps_cap, &teacher_img).block(0).ctrl;
 }
 
 bool persistent_supported(const T2Model* m, const T2DecoderArgs* a) {
@@ -1158,55 +1223,38 @@ void persistent_pack_destroy(T2Model* m) {
   m->pk = nullptr;
 }
 
-static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t s, int b0, int nb);
-
-int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
-  // batch rows are independent: more than 64 rows run as consecutive launches of <= 64 rows
-  T2_CUDA(cudaMemsetAsync(a->n_steps, 0, sizeof(int32_t), s));
-  for (int b0 = 0; b0 < a->B; b0 += kRows) {
-    const int nb = a->B - b0 < kRows ? a->B - b0 : kRows;
-    T2_TRY(run_persistent_slice(m, a, s, b0, nb));
-  }
-  return T2_OK;
-}
-
-// processed_memory = memory_layer(memory) of batch rows [b0, b0 + nb)                    (model.py:288)
+// processed_memory = memory_layer(memory) of batch rows [b0, b0 + nb) into their rows of pm (B, T, 128)  (model.py:288)
 static int processed_memory(T2Model* m, const T2DecoderArgs* a, int b0, int nb, float* pm, cudaStream_t s) {
   GemmArgs g;
   g.seg[0] = {a->memory + (size_t)b0 * a->T_enc * kEnc, kEnc, m->w[W_ATT_MEMORY], kEnc, kEnc};
-  g.M = nb * a->T_enc; g.N = kAtt; g.C = pm; g.ldc = kAtt;
+  g.M = nb * a->T_enc; g.N = kAtt; g.C = pm + (size_t)b0 * a->T_enc * kAtt; g.ldc = kAtt;
   return gemm_f32(g, s);
 }
 
-// the parameters of one launch over batch rows [b0, b0 + nb) that do not depend on where its state lives
-static void slice_params(T2Model* m, const T2DecoderArgs* a, int b0, int nb, KParams* pp) {
+// the parameters of the launch over batch rows [b0, b0 + 64) (or to B) whose state is block `blk` of `buf`: the whole loop
+// [0, cap), no resume state
+static void slice_params(T2Model* m, const T2DecoderArgs* a, const SliceBuffer& buf, const SliceState& blk, int b0, KParams* pp) {
   PersistentPack* pk = (PersistentPack*)m->pk;
   KParams& p = *pp;
   const int T = a->T_enc, cap = a->n_steps_cap;
   memset(&p, 0, sizeof(p));
   p.plans = pk->plans; p.wimg = pk->wimg; p.bias_a = pk->bias_a; p.bias_d = pk->bias_d; p.bias_p = pk->bias_p;
   p.weff_img = pk->weff_img; p.w_v = m->w[W_ATT_V];
-  p.memory = a->memory + (size_t)b0 * T * kEnc;
+  p.memory = a->memory + (size_t)b0 * T * kEnc; p.pm = buf.pm + (size_t)b0 * T * kAtt;
   p.mem_len = a->memory_lengths ? a->memory_lengths + b0 : nullptr;
   p.prenet_keep = a->prenet_keep; p.att_keep = a->att_keep; p.dec_keep = a->dec_keep;
+  p.x2_img = blk.x2; p.ah_img = blk.ah; p.ctx_img = blk.ctx; p.dh_img = blk.dh; p.x1_img = blk.x1; p.q = blk.q;
   p.mel = a->mel + (size_t)b0 * cap * kMel; p.gate = a->gate + (size_t)b0 * cap; p.align = a->align + (size_t)b0 * cap * T;
   p.mel_lengths = a->mel_lengths + b0; p.n_steps = a->n_steps;
+  p.ctrl = blk.ctrl;
   p.b0 = b0; p.Btot = a->B;
-  p.B = nb; p.T = T; p.cap = cap; p.infer = a->mode == T2_MODE_INFER; p.training = a->training;
+  p.B = a->B - b0 < kRows ? a->B - b0 : kRows; p.T = T; p.cap = cap; p.infer = a->mode == T2_MODE_INFER;
+  p.training = a->training;
+  p.pa = pa_precomputed(T, p.infer) ? blk.pa : nullptr;
   p.gate_threshold = a->gate_threshold; p.score_mask_value = a->score_mask_value;
   p.p_att = m->cfg.p_attention_dropout; p.p_dec = m->cfg.p_decoder_dropout; p.seed = a->seed;
   p.row_seeds = a->row_seeds;
   p.t_begin = 0; p.t_end = cap;
-}
-
-// x2 | ah | ctx | dh | x1 activation images, then q
-static void carve_images(uint8_t* img, KParams* p) {
-  p->x2_img = img; img += 4 * kXChunkBytes;
-  p->ah_img = img; img += 16 * kXChunkBytes;
-  p->ctx_img = img; img += 8 * kXChunkBytes;
-  p->dh_img = img; img += 16 * kXChunkBytes;
-  p->x1_img = img; img += 4 * kXChunkBytes;
-  p->q = (float*)img;
 }
 
 // the longest T_enc that persistent_stages() runs with 4 stages (0 when none does); stages fall as T_enc grows
@@ -1239,110 +1287,83 @@ static int launch_persistent(KParams& p, cudaStream_t s) {
   return T2_OK;
 }
 
-static int run_persistent_slice(T2Model* m, const T2DecoderArgs* a, cudaStream_t s, int b0, int nb) {
-  const int T = a->T_enc, cap = a->n_steps_cap;
-  DecoderWs w;
-  T2_TRY(decoder_ws_carve(a, &w));
-  T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
-  T2_CUDA(cudaMemsetAsync(w.images, 0, kImagesBytes, s));  // zero images (model.py:258-284)
-  T2_TRY(processed_memory(m, a, b0, nb, w.pm, s));
-  KParams p;
-  slice_params(m, a, b0, nb, &p);
-  carve_images(w.images, &p);
-  if (pa_precomputed(T, p.infer)) {      // zero attention weights -> pa of step 0 is +0.0
-    T2_CUDA(cudaMemsetAsync(w.pa, 0, pa_buffer_floats(T) * 4, s));
-    p.pa = w.pa;
-  }
-  p.pm = w.pm;
-  p.ctrl = w.ctrl;
-  const int B = nb;
+int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
+  const int cap = a->n_steps_cap;
+  const bool infer = a->mode == T2_MODE_INFER;
+  DecoderStash st;
   if (a->stash) {
-    if (p.infer) return fail(T2_ERR_INVALID, "the training stash needs T2_MODE_TEACHER");
+    if (infer) return fail(T2_ERR_INVALID, "the training stash needs T2_MODE_TEACHER");
     if (a->stash_bytes < decoder_stash_bytes(a->B, cap)) return fail(T2_ERR_WORKSPACE, "decoder stash too small");
     Carve c(a->stash);
-    decoder_stash_layout(c, a->B, cap, &p.st);
-    if (b0 == 0) {   // slot 0 of the recurrent states = the zero initial states (model.py:258-284)
-      float* z[5] = {p.st.ca, p.st.ha, p.st.cd, p.st.hd, p.st.ctx};
-      for (int i = 0; i < 5; ++i)
-        T2_CUDA(cudaMemsetAsync(z[i], 0, (size_t)a->B * (i < 4 ? kARnn : kEnc) * sizeof(float), s));
+    decoder_stash_layout(c, a->B, cap, &st);
+    float* z[5] = {st.ca, st.ha, st.cd, st.hd, st.ctx};   // slot 0 of the recurrent states = the zero initial states
+    for (int i = 0; i < 5; ++i)                          // (model.py:258-284)
+      T2_CUDA(cudaMemsetAsync(z[i], 0, (size_t)a->B * (i < 4 ? kARnn : kEnc) * sizeof(float), s));
+  }
+  Carve c(a->ws, kDecoderWsAlign);
+  uint8_t* teacher_img;
+  const SliceBuffer buf = persistent_ws_layout(c, a->B, a->T_enc, cap, &teacher_img);
+  const SliceState blk = buf.block(0);
+  T2_CUDA(cudaMemsetAsync(a->n_steps, 0, sizeof(int32_t), s));
+  T2_TRY(processed_memory(m, a, 0, a->B, buf.pm, s));
+  // batch rows are independent: more than 64 rows run as consecutive launches of <= 64 rows on the one block
+  for (int b0 = 0; b0 < a->B; b0 += kRows) {
+    KParams p;
+    slice_params(m, a, buf, blk, b0, &p);
+    // counters, zero images and q (model.py:258-284): the block's regions before pa
+    T2_CUDA(cudaMemsetAsync(blk.ctrl, 0, (uint8_t*)blk.pa - (uint8_t*)blk.ctrl, s));
+    if (p.pa) T2_CUDA(cudaMemsetAsync(p.pa, 0, pa_buffer_floats(a->T_enc) * 4, s));   // zero attention weights -> pa = +0.0
+    p.st = st;
+    if (!infer) {
+      // teacher forcing (model.py:396-405): the prenet outputs of all steps are known up front -> convert
+      // them once into x2 operand images, the kernel then skips the prenet events and their two barriers
+      rows_to_image_kernel<<<dim3(4, cap), 256, 0, s>>>(a->teacher_prenet + (size_t)b0 * kPre, kPre, p.B, kPre,
+                                                        (long)a->B * kPre, teacher_img, (long)4 * kXChunkBytes);
+      T2_LAUNCH_CHECK();
+      p.teacher_x2_img = teacher_img;
     }
+    T2_TRY(launch_persistent(p, s));
   }
-  if (!p.infer) {
-    // teacher forcing (model.py:396-405): the prenet outputs of all steps are known up front -> convert
-    // them once into x2 operand images, the kernel then skips the prenet events and their two barriers
-    rows_to_image_kernel<<<dim3(4, cap), 256, 0, s>>>(a->teacher_prenet + (size_t)b0 * kPre, kPre, B, kPre, (long)a->B * kPre,
-                                                      w.teacher_img, (long)4 * kXChunkBytes);
-    T2_LAUNCH_CHECK();
-    p.teacher_x2_img = w.teacher_img;
-  }
-  return launch_persistent(p, s);
+  return T2_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
-// resumable stream (t2_decoder_stream_*): every 64-row slice owns a block of the caller's state buffer
+// resumable stream (t2_decoder_stream_*): the caller's state buffer is a slice buffer with one block per 64-row slice,
+// saved state included
 // ---------------------------------------------------------------------------------------------
-struct StreamSlice {
-  DecoderCtrl* ctrl;     // counters zeroed before every launch; the stop latch is carried in `done`
-  uint8_t* images;       // activation images + q (kImagesBytes)
-  float* acc; float* cell; float* att; int32_t* done;
-  float* pm;             // processed memory of the slice's rows (nb, T, 128)
-  float* pa;             // location term of the next step (KParams::pa)
-};
-// the slices one after the other; returns slice `b0 / kRows` (any slice when only measuring)
-__host__ __device__ static StreamSlice stream_state_layout(Carve& c, int B, int T, int b0) {
-  const size_t tpp = (size_t)((T + kLocK - 1 + 3) & ~3);
-  StreamSlice want = {};
-  for (int b = 0; b < B; b += kRows) {
-    const int nb = B - b < kRows ? B - b : kRows;
-    StreamSlice sl;
-    sl.ctrl = c.take<DecoderCtrl>(1, 1024);
-    sl.images = c.take<uint8_t>(kImagesBytes, 1024);
-    sl.acc = c.take<float>((size_t)kG * kRows * kAccPitch, 1024);
-    sl.cell = c.take<float>((size_t)kG * 4 * kRows * 4, 1024);
-    sl.att = c.take<float>((size_t)kG * 2 * tpp, 1024);
-    sl.done = c.take<int32_t>(kRows, 1024);
-    sl.pm = c.take<float>((size_t)nb * T * kAtt, 1024);
-    sl.pa = c.take<float>(pa_buffer_floats(T), 1024);
-    if (b == b0) want = sl;
-  }
-  return want;
+__host__ __device__ static SliceBuffer stream_state_layout(Carve& c, int B, int T) {
+  return slice_buffer_layout(c, B, T, (B + kRows - 1) / kRows, true);
 }
-static StreamSlice stream_slice(void* state, int B, int T, int b0) { Carve c(state, 1024); return stream_state_layout(c, B, T, b0); }
+static SliceBuffer stream_state(void* state, int B, int T) { Carve c(state, kSliceAlign); return stream_state_layout(c, B, T); }
 
-size_t persistent_stream_state_bytes(int B, int T) { Carve c(nullptr, 1024); stream_state_layout(c, B, T, 0); return c.bytes(); }
+size_t persistent_stream_state_bytes(int B, int T) { Carve c(nullptr, kSliceAlign); stream_state_layout(c, B, T); return c.bytes(); }
 
 int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, cudaStream_t s) {
   T2_CUDA(cudaMemsetAsync(state, 0, persistent_stream_state_bytes(a->B, a->T_enc), s));   // model.py:258-284
   T2_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * 2 * ((a->B + kRows - 1) / kRows), s));
   T2_CUDA(cudaMemsetAsync(a->mel_lengths, 0xff, sizeof(int32_t) * a->B, s));                // -1: still live
   T2_CUDA(cudaMemsetAsync(a->n_steps, 0, sizeof(int32_t), s));
-  for (int b0 = 0; b0 < a->B; b0 += kRows)
-    T2_TRY(processed_memory(m, a, b0, a->B - b0 < kRows ? a->B - b0 : kRows, stream_slice(state, a->B, a->T_enc, b0).pm, s));
-  return T2_OK;
+  return processed_memory(m, a, 0, a->B, stream_state(state, a->B, a->T_enc).pm, s);
 }
 
 int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n,
                           const int32_t* status_host, const int32_t* row_step0, cudaStream_t s) {
+  const SliceBuffer buf = stream_state(state, a->B, a->T_enc);
   for (int b0 = 0, si = 0; b0 < a->B; b0 += kRows, ++si) {
     const int t0 = status_host ? status_host[2 * si] : 0;
     if ((status_host && status_host[2 * si + 1]) || t0 >= a->n_steps_cap) continue;    // this slice has stopped
-    const StreamSlice sl = stream_slice(state, a->B, a->T_enc, b0);
-    T2_CUDA(cudaMemsetAsync(sl.ctrl, 0, sizeof(DecoderCtrl), s));
+    const SliceState blk = buf.block(si);
+    T2_CUDA(cudaMemsetAsync(blk.ctrl, 0, sizeof(DecoderCtrl), s));   // everything else is zeroed by begin / admit
     KParams p;
-    slice_params(m, a, b0, a->B - b0 < kRows ? a->B - b0 : kRows, &p);
-    carve_images(sl.images, &p);
-    p.pm = sl.pm;
-    p.ctrl = sl.ctrl;
+    slice_params(m, a, buf, blk, b0, &p);                            // pa: left by the previous chunk
     p.t_begin = t0;
     p.t_end = n < a->n_steps_cap - t0 ? t0 + n : a->n_steps_cap;
-    p.rs_acc = sl.acc; p.rs_cell = sl.cell; p.rs_att = sl.att; p.rs_done = sl.done; p.rs_status = status + 2 * si;
+    p.rs_acc = blk.acc; p.rs_cell = blk.cell; p.rs_att = blk.att; p.rs_done = blk.done; p.rs_status = status + 2 * si;
     p.row_step0 = row_step0;
-    if (pa_precomputed(a->T_enc, p.infer)) p.pa = sl.pa;      // zeroed by begin, left by the previous chunk
     T2_TRY(launch_persistent(p, s));
   }
   return T2_OK;
 }
-
 
 // ---------------------------------------------------------------------------------------------
 // continuous batching (t2_decoder_stream_admit / _collect): a stream whose rows are slots.  Between two chunks a row is
@@ -1356,24 +1377,25 @@ struct RowMask { uint64_t w[kMaxBatch / 64]; };      // bit b: row b is listed
 // of every piece (model.py:258-284 starts both LSTMs, the attention weights and the context at zero, and an accumulator
 // tile holds the partial products of zero activations).  It writes the row's own entries only.
 __global__ void __launch_bounds__(256) stream_admit_kernel(void* state, int B, int T, RowMask mask, int32_t* mel_lengths) {
-  const int lr = blockIdx.x, b0 = blockIdx.y * kRows, row = b0 + lr, tid = threadIdx.x;
+  const int lr = blockIdx.x, row = blockIdx.y * kRows + lr, tid = threadIdx.x;
   if (row >= B || !((mask.w[row >> 6] >> (row & 63)) & 1ull)) return;
-  Carve c(state, 1024);
-  const StreamSlice sl = stream_state_layout(c, B, T, b0);
-  const int tpp = (T + kLocK - 1 + 3) & ~3;
+  Carve c(state, kSliceAlign);
+  const SliceState sl = stream_state_layout(c, B, T).block(blockIdx.y);
+  const int tpp = att_pad_len(T);
   for (int i = tid; i < kG * kAccPitch; i += 256)                  // its accumulator row in every CTA's tile
     sl.acc[((size_t)(i / kAccPitch) * kRows + lr) * kAccPitch + i % kAccPitch] = 0.f;
   for (int i = tid; i < kG * 4; i += 256)                          // its cell states: (CTA, column group)
     reinterpret_cast<float4*>(sl.cell)[(size_t)i * kRows + lr] = make_float4(0.f, 0.f, 0.f, 0.f);
   for (int i = tid; i < 4 * tpp; i += 256)                         // previous | cumulative weights of CTAs lr and lr + 64
     sl.att[(size_t)(lr + 64 * (i / (2 * tpp))) * 2 * tpp + i % (2 * tpp)] = 0.f;
-  for (int i = tid; i < kImageChunks * 2 * (kChunkK / 2); i += 256) {   // its row in both planes of every image chunk
-    const int chunk = i / kChunkK, plane = (i / (kChunkK / 2)) & 1, k = (i % (kChunkK / 2)) * 2;
-    __half* pl = reinterpret_cast<__half*>(sl.images + (size_t)chunk * kXChunkBytes) + plane * kRows * kChunkK;
-    *reinterpret_cast<uint32_t*>(pl + img_elem_offset(lr, k)) = 0u;
-  }
-  float* q = reinterpret_cast<float*>(sl.images + (size_t)kImageChunks * kXChunkBytes);
-  for (int i = tid; i < kAtt; i += 256) q[lr * kAtt + i] = 0.f;
+  const struct { uint8_t* img; int chunks; } imgs[5] = {{sl.x2, 4}, {sl.ah, 16}, {sl.ctx, 8}, {sl.dh, 16}, {sl.x1, 4}};
+  for (const auto& im : imgs)
+    for (int i = tid; i < im.chunks * 2 * (kChunkK / 2); i += 256) {   // its row in both planes of every chunk of an image
+      const int chunk = i / kChunkK, plane = (i / (kChunkK / 2)) & 1, k = (i % (kChunkK / 2)) * 2;
+      __half* pl = reinterpret_cast<__half*>(im.img + (size_t)chunk * kXChunkBytes) + plane * kRows * kChunkK;
+      *reinterpret_cast<uint32_t*>(pl + img_elem_offset(lr, k)) = 0u;
+    }
+  for (int i = tid; i < kAtt; i += 256) sl.q[lr * kAtt + i] = 0.f;
   const size_t pa_row = pa_buffer_floats(T) / kRows;                // its pa tile (zero weights -> zero location term)
   for (size_t i = tid; i < pa_row; i += 256) sl.pa[lr * pa_row + i] = 0.f;
   if (tid == 0) { sl.done[lr] = 0; mel_lengths[row] = -1; }
@@ -1401,12 +1423,12 @@ int persistent_stream_admit(T2Model* m, const T2DecoderArgs* a, void* state, con
   for (int i = 0; i < n_rows; ++i) mask.w[rows[i] >> 6] |= 1ull << (rows[i] & 63);
   stream_admit_kernel<<<dim3(kRows, (a->B + kRows - 1) / kRows), 256, 0, s>>>(state, a->B, a->T_enc, mask, a->mel_lengths);
   T2_LAUNCH_CHECK();
-  // processed memory of the listed rows: one GEMM per run of consecutive rows of a slice (rows are ascending)
+  // processed memory of the listed rows: one GEMM per run of consecutive rows (rows are ascending)
+  float* pm = stream_state(state, a->B, a->T_enc).pm;
   for (int i = 0; i < n_rows;) {
     int j = i + 1;
-    while (j < n_rows && rows[j] == rows[j - 1] + 1 && rows[j] / kRows == rows[i] / kRows) ++j;
-    const int b0 = rows[i] / kRows * kRows;
-    T2_TRY(processed_memory(m, a, rows[i], j - i, stream_slice(state, a->B, a->T_enc, b0).pm + (size_t)(rows[i] - b0) * a->T_enc * kAtt, s));
+    while (j < n_rows && rows[j] == rows[j - 1] + 1) ++j;
+    T2_TRY(processed_memory(m, a, rows[i], j - i, pm, s));
     i = j;
   }
   return T2_OK;

@@ -204,6 +204,40 @@ size_t stepwise_attention_smem(int T) {
                           kLocF * T + T + 32);
 }
 
+// workspace of the stepwise decoder
+struct StepwiseWs {
+  float* pm;               // processed_memory (B, T, 128)          model.py:288
+  char* state_begin; size_t state_bytes;   // zero-initialised block (model.py:258-284):
+  float *ah, *ac, *dh, *dc;                // (B, 1024) each
+  float* ctx;              // (B, 512)
+  float *aw, *awc;         // (B, T)
+  float *x1, *x2;          // prenet activations (B, 256)
+  float* gates;            // (B, 4096)
+  float* proj;             // (B, 81)
+  DecoderCtrl* ctrl;
+};
+static void stepwise_ws_layout(Carve& c, int B, int T, StepwiseWs* w) {
+  w->pm = c.take<float>((size_t)B * T * kAtt);
+  // the zero-initialised states: packed floats, one block that one memset clears
+  w->state_begin = c.take<char>(0);
+  const size_t state0 = c.off;
+  w->ah = c.take<float>((size_t)B * kARnn, alignof(float)); w->ac = c.take<float>((size_t)B * kARnn, alignof(float));
+  w->dh = c.take<float>((size_t)B * kDRnn, alignof(float)); w->dc = c.take<float>((size_t)B * kDRnn, alignof(float));
+  w->ctx = c.take<float>((size_t)B * kEnc, alignof(float));
+  w->aw = c.take<float>((size_t)B * T, alignof(float)); w->awc = c.take<float>((size_t)B * T, alignof(float));
+  w->state_bytes = c.off - state0;
+  w->x1 = c.take<float>((size_t)B * kPre); w->x2 = c.take<float>((size_t)B * kPre);
+  w->gates = c.take<float>((size_t)B * 4 * kARnn);
+  w->proj = c.take<float>((size_t)B * (kMel + 1));
+  w->ctrl = c.take<DecoderCtrl>(1);
+}
+size_t stepwise_ws_bytes(int B, int T) {
+  Carve c(nullptr, kDecoderWsAlign);
+  StepwiseWs w;
+  stepwise_ws_layout(c, B, T, &w);
+  return c.bytes();
+}
+
 // ---------------------------------------------------------------------------------------------
 // host orchestration
 // ---------------------------------------------------------------------------------------------
@@ -212,8 +246,9 @@ int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
   const bool infer = a->mode == T2_MODE_INFER;
   const size_t att_smem = stepwise_attention_smem(T);
   if (att_smem > 200 * 1024) return fail(T2_ERR_INVALID, "T_enc=%d too long for the stepwise attention kernel (at most 1282)", T);
-  DecoderWs w;
-  T2_TRY(decoder_ws_carve(a, &w));
+  Carve c(a->ws, kDecoderWsAlign);
+  StepwiseWs w;
+  stepwise_ws_layout(c, B, T, &w);
   T2_CUDA(cudaMemsetAsync(w.state_begin, 0, w.state_bytes, s));   // model.py:258-284 (zeros)
   T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
 

@@ -15,7 +15,7 @@ import torch
 
 import tacotron2_b200 as t2
 from tacotron2_b200 import _capi
-from tacotron2_b200._engine import Engine
+from tacotron2_b200._engine import Engine, f32_buffer
 from tests.common import rand_text, synth_state_dict
 
 pytestmark = pytest.mark.gpu
@@ -143,6 +143,28 @@ def test_decoder_stream():
         for n in (3, 2, 4):
             s.run(n)
         return [s.mel, s.gate, s.align, s.mel_lengths, s.n_steps, s.status]
+    same_both_ways(run)
+
+
+def test_decoder_stream_admit_and_collect():
+    """Continuous batching on 65 rows: after a chunk, rows of both 64-row slices take new texts (admit resets each row in
+    its own slice's block and writes its processed memory), the next chunk runs, and its frames go to the rows' own
+    buffers."""
+    B, Te, n = 65, 95, 4
+    memory = randn(B, Te, 512, seed=21, scale=0.5)
+    lengths = torch.tensor([Te - b % 9 for b in range(B)], dtype=torch.int32)
+    rows = [0, 63, 64]
+    fresh = randn(len(rows), Te, 512, seed=22, scale=0.5)
+
+    def run(eng):
+        s = eng.decoder_stream(memory.clone(), n + 1, impl=_capi.IMPL_PERSISTENT, seed=SEED, memory_lengths=lengths)
+        s.launch_chunk(n, SEED)
+        s.memory[rows] = fresh
+        s.admit(rows)
+        s.launch_chunk(n, SEED + 1)
+        outs = [(f32_buffer("cuda", n, 80), f32_buffer("cuda", n), f32_buffer("cuda", n, int(lengths[r]))) for r in rows]
+        s.collect([(r, n, int(lengths[r]), *o) for r, o in zip(rows, outs)])
+        return [s.mel, s.gate, s.align, s.readback] + [t for o in outs for t in o]
     same_both_ways(run)
 
 
