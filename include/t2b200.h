@@ -387,7 +387,13 @@ int    t2_tacotron2_loss(const T2LossArgs* a, void* stream);
  * y (B, n_samples) fp32 in [-1, 1] (not checked here; the Python mirror asserts it like the reference does).
  * forward_basis (2 * (filter_length / 2 + 1), filter_length): the windowed Fourier basis of stft.py:44-63;
  * mel_basis (n_mel, filter_length / 2 + 1).  mel out: (B, n_mel, n_frames) = log(max(mel_basis . |STFT|, clip_val)),
- * n_frames = n_samples / hop_length + 1 (reflect padding by filter_length / 2 on both sides). */
+ * n_frames = n_samples / hop_length + 1 (reflect padding by filter_length / 2 on both sides).
+ * lengths (device, B int32 sample counts, or NULL): row b is computed as y[b, :lengths[b]] alone -- bit for bit the B = 1
+ * call on those samples -- and its frames from lengths[b] / hop_length + 1 on are zero; samples at or past lengths[b] are
+ * never read.  Each length must lie in [filter_length / 2 + 1, n_samples]: the values live on the device, so the call
+ * cannot refuse them without waiting for the GPU; the device clamps them into that range (the Python mirror refuses
+ * them).  The workspace is t2_mel_spectrogram_workspace_bytes_lengths(B, n_samples, ...).  NULL: the whole batch shares
+ * each frame's operand scale and its GEMM split plan, as before lengths existed. */
 typedef struct T2MelSpecArgs {
   const float* y; int32_t B, n_samples;
   int32_t filter_length, hop_length, n_mel;
@@ -395,9 +401,12 @@ typedef struct T2MelSpecArgs {
   float clip_val;
   float* mel;
   void* ws; size_t ws_bytes;
+  const int32_t* lengths;
 } T2MelSpecArgs;
 int32_t t2_mel_spectrogram_frames(int32_t n_samples, int32_t hop_length);
 size_t  t2_mel_spectrogram_workspace_bytes(int32_t B, int32_t n_samples, int32_t filter_length, int32_t hop_length, int32_t n_mel);
+size_t  t2_mel_spectrogram_workspace_bytes_lengths(int32_t B, int32_t n_max, int32_t filter_length, int32_t hop_length,
+                                                   int32_t n_mel);
 int     t2_mel_spectrogram(const T2MelSpecArgs* a, void* stream);
 
 /* ---- TextMelCollate on the device (data_utils.py:73-111): ragged batch in HBM -> the padded, length-sorted 5-tuple ------------

@@ -28,6 +28,7 @@ EXPORTS = [
     "t2_clip_adam_workspace_bytes", "t2_clip_adam_step", "t2_amp_adam_workspace_bytes", "t2_amp_adam_step",
     "t2_loss_workspace_bytes", "t2_tacotron2_loss",
     "t2_mel_spectrogram_frames", "t2_mel_spectrogram_workspace_bytes", "t2_mel_spectrogram", "t2_collate",
+    "t2_mel_spectrogram_workspace_bytes_lengths",
     "t2_decoder_stream_state_bytes", "t2_decoder_stream_begin", "t2_decoder_stream_run",
     "t2_decoder_stream_admit", "t2_decoder_stream_collect",
     "t2_waveglow_create", "t2_waveglow_refresh", "t2_waveglow_destroy", "t2_waveglow_workspace_bytes",
@@ -142,7 +143,8 @@ class T2LossArgs(C.Structure):
 class T2MelSpecArgs(C.Structure):
     _fields_ = [("y", C.c_void_p), ("B", C.c_int32), ("n_samples", C.c_int32), ("filter_length", C.c_int32),
                 ("hop_length", C.c_int32), ("n_mel", C.c_int32), ("forward_basis", C.c_void_p), ("mel_basis", C.c_void_p),
-                ("clip_val", C.c_float), ("mel", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+                ("clip_val", C.c_float), ("mel", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t),
+                ("lengths", C.c_void_p)]
 
 
 class T2CollateArgs(C.Structure):
@@ -268,6 +270,8 @@ def lib():
     L.t2_mel_spectrogram_frames.argtypes = [C.c_int32, C.c_int32]
     L.t2_mel_spectrogram_workspace_bytes.restype = C.c_size_t
     L.t2_mel_spectrogram_workspace_bytes.argtypes = [C.c_int32] * 5
+    L.t2_mel_spectrogram_workspace_bytes_lengths.restype = C.c_size_t
+    L.t2_mel_spectrogram_workspace_bytes_lengths.argtypes = [C.c_int32] * 5
     L.t2_mel_spectrogram.argtypes = [C.POINTER(T2MelSpecArgs), C.c_void_p]
     L.t2_collate.argtypes = [C.POINTER(T2CollateArgs), C.c_void_p]
     L.t2_encoder_backward.argtypes = [C.c_void_p, C.POINTER(T2EncoderBwdArgs), C.c_void_p]

@@ -30,15 +30,17 @@ constexpr int kBufBytes = 4 * kPlane;             // [A hi | A lo | B hi | B lo]
 constexpr int kTargetExp = 13;                    // scaled row / column maximum in [2^13, 2^14)
 
 // ---- pre-pass: largest magnitude of every row of op(A) / column of op(B) over K (as raw float bits, atomicMax) ------
-// inner (K) contiguous: one warp per outer index
+// inner (K) contiguous: one warp per outer index.  blockIdx.z: batch entry at element stride s_batch, with its own
+// n_outer maxima in out; outer_of (device, per entry, or nullptr): the entry's outer indices past it are not read.
 __global__ void absmax_inner_contig_kernel(const float* __restrict__ X, long s_outer, int n_outer, int n_inner,
-                                           unsigned int* __restrict__ out) {
+                                           unsigned int* __restrict__ out, long s_batch, const int* __restrict__ outer_of) {
   const int o = blockIdx.x * blockDim.y + threadIdx.y;
-  if (o >= n_outer) return;
+  if (o >= (outer_of ? min(n_outer, outer_of[blockIdx.z]) : n_outer)) return;
   const long per = (n_inner + gridDim.y - 1) / gridDim.y;
   const long i0 = blockIdx.y * per, i1 = i0 + per < n_inner ? i0 + per : n_inner;
   float mx = 0.f;
-  const float* r = X + (long)o * s_outer;
+  const float* r = X + blockIdx.z * s_batch + (long)o * s_outer;
+  out += (long)blockIdx.z * n_outer;
   for (long i = i0 + threadIdx.x; i < i1; i += 32) mx = fmaxf(mx, fabsf(r[i]));
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, d));
@@ -77,7 +79,30 @@ struct GemmP {
   long lda, ldb, ldc, sA, sB, sC;                              // leading dimensions, batch strides (elements)
   int M, N, K, ta, tb, splits, chunks_per_split, batch;
   float beta;
+  const int* entry_rows; int sms;                              // ragged entries (GemmTc::entry_rows), planned for sms
 };
+
+// The split rule: small-tile / large-K problems are split along K so that they fill one wave of CTAs (1 CTA / SM:
+// 161 KiB of shared memory).  Scratch: [amax (M)][bmax (N)][partial tiles of the K splits].  The ragged kernel evaluates
+// it on the device for each entry's own row count.
+struct Plan { int ntm, ntn, splits, cps; long tiles; size_t off_part, bytes; };
+__host__ __device__ Plan plan(int M, int N, int K, int batch, int sms) {
+  Plan p;
+  p.ntm = (M + kBM - 1) / kBM; p.ntn = (N + kBN - 1) / kBN;
+  const int nchunks = (K + kBK - 1) / kBK;
+  p.tiles = (long)p.ntm * p.ntn * batch;
+  int splits = 1;
+  if (p.tiles * 5 < sms * 4 && nchunks >= 8) {
+    splits = p.tiles <= sms / 2 ? (int)(sms / p.tiles) : 2;
+    if (splits > nchunks / 4) splits = nchunks / 4;
+    if (splits < 1) splits = 1;
+  }
+  p.cps = (nchunks + splits - 1) / splits;
+  p.splits = (nchunks + p.cps - 1) / p.cps;
+  p.off_part = (((size_t)M + N) * 4 + 255) & ~(size_t)255;
+  p.bytes = p.off_part + (p.splits > 1 ? (size_t)p.tiles * p.splits * kBM * kBN * 4 : 0);
+  return p;
+}
 
 // ---- operand tiles: global fp32 -> registers -> (transposing stage) -> split-fp16 SWIZZLE_128B planes -----------------
 // Every thread owns 4 groups of 8 consecutive elements of the 128 x 64 tile.  `kc`: the K dimension is contiguous in
@@ -173,29 +198,64 @@ __device__ __forceinline__ void tile_store(const float (&v)[4][8], bool kc, int 
 // stores after the MMAs that read the same buffer two chunks earlier.
 constexpr int kSmemG = 2 * kBufBytes + kStageBytesG;
 
+// Ragged entries: add split sp's partial tile, scaled back exactly as the epilogue does, to the entry's C, and restart
+// the accumulators.  As splitk_reduce_kernel, a split plan sums from +0 in split order and an unsplit one stores the
+// tile as it is.  Each thread reads back only what it wrote itself.
+__device__ __forceinline__ void ragged_fold(const GemmP& p, float (&acc)[64], int batch, int M, int m0, int n0,
+                                            const unsigned int* __restrict__ amax, int splits, int sp) {
+  const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127;
+  float* Cb = p.C + (long)batch * p.sC;
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int m = m0 + wg * 64 + ptx::wg_frag_row(i, wt), n = n0 + ptx::wg_frag_col(i, wt);
+    if (m < M && n < p.N) {
+      const float ia = 1.f / scale_of(amax[m]);
+      const float v = __fmul_rn(acc[i], ia / scale_of(p.bmax[n]));
+      float* dst = Cb + (long)m * p.ldc + n;
+      *dst = splits == 1 ? v : __fadd_rn(sp == 0 ? 0.f : *dst, v);
+    }
+    acc[i] = 0.f;
+  }
+}
+
+// kRagged (GemmTc::entry_rows): one CTA per (entry, tile) runs the entry's K splits one after the other and adds each
+// split's scaled partial tile to C in the order splitk_reduce_kernel adds them, so every entry gets the bits of its own
+// batch = 1 call.
+template <bool kRagged>
 __global__ void __launch_bounds__(kThreadsG, 1) gemm_tc_kernel(const GemmP p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   float* stage = reinterpret_cast<float*>(smem_raw + 2 * kBufBytes);
   const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
-  const int bz = blockIdx.z, batch = bz / p.splits, split = bz - batch * p.splits;
+  const int bz = blockIdx.z, batch = kRagged ? bz : bz / p.splits, split = kRagged ? 0 : bz - batch * p.splits;
   const int m0 = blockIdx.y * kBM, n0 = blockIdx.x * kBN;
   const float* A = p.A + (long)batch * p.sA;
   const float* B = p.B + (long)batch * p.sB;
   const int nchunks = (p.K + kBK - 1) / kBK;
-  const int c0 = split * p.chunks_per_split, c1 = min(nchunks, c0 + p.chunks_per_split);
+  int M = p.M, cps = p.chunks_per_split, splits = 1;
+  const unsigned int* amax = p.amax;
+  if constexpr (kRagged) {
+    M = min(p.M, p.entry_rows[batch]);
+    if (m0 >= M) return;                    // the whole CTA: past the entry's rows
+    const Plan pl = plan(M, p.N, p.K, 1, p.sms);
+    cps = pl.cps; splits = pl.splits;
+    amax += (long)batch * p.M;
+  }
+  const int c0 = split * cps, c1 = kRagged ? nchunks : min(nchunks, c0 + cps);
   const bool a_kc = !p.ta, b_kc = p.tb != 0;
   float acc[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-
   int it = 0;
   for (int c = c0; c < c1; ++c, ++it) {
+    if constexpr (kRagged) {
+      if (c > 0 && c % cps == 0) ragged_fold(p, acc, batch, M, m0, n0, amax, splits, c / cps - 1);
+    }
     uint8_t* sb = smem_raw + (it & 1) * kBufBytes;
     {
       float va[4][8], vb[4][8];
-      tile_fetch(A, p.lda, a_kc, m0, c * kBK, p.M, p.K, va);       // both operands' loads in flight together
+      tile_fetch(A, p.lda, a_kc, m0, c * kBK, M, p.K, va);         // both operands' loads in flight together
       tile_fetch(B, p.ldb, b_kc, n0, c * kBK, p.N, p.K, vb);
-      tile_store(va, a_kc, m0, p.M, p.amax, stage, reinterpret_cast<__half*>(sb), reinterpret_cast<__half*>(sb + kPlane));
+      tile_store(va, a_kc, m0, M, amax, stage, reinterpret_cast<__half*>(sb), reinterpret_cast<__half*>(sb + kPlane));
       tile_store(vb, b_kc, n0, p.N, p.bmax, stage, reinterpret_cast<__half*>(sb + 2 * kPlane), reinterpret_cast<__half*>(sb + 3 * kPlane));
     }
     ptx::fence_proxy_async();
@@ -222,6 +282,10 @@ __global__ void __launch_bounds__(kThreadsG, 1) gemm_tc_kernel(const GemmP p) {
     ptx::wg_fence_regs<64>(dx);
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] += dh[i] + dx[i];
+  }
+  if constexpr (kRagged) {
+    ragged_fold(p, acc, batch, M, m0, n0, amax, splits, splits - 1);
+    return;
   }
   __syncthreads();                          // every MMA is complete: the operand buffers become the output tile
 
@@ -318,35 +382,65 @@ __global__ void colsum_final_kernel(const float* __restrict__ part, int nsplit, 
 
 }  // namespace
 
-// The split rule: small-tile / large-K problems are split along K so that they fill one wave of CTAs (1 CTA / SM:
-// 161 KiB of shared memory).  Scratch: [amax (M)][bmax (N)][partial tiles of the K splits].
-struct Plan { int ntm, ntn, splits, cps; long tiles; size_t off_part, bytes; };
-static Plan plan(int M, int N, int K, int batch, int sms) {
-  Plan p;
-  p.ntm = (M + kBM - 1) / kBM; p.ntn = (N + kBN - 1) / kBN;
-  const int nchunks = (K + kBK - 1) / kBK;
-  p.tiles = (long)p.ntm * p.ntn * batch;
-  int splits = 1;
-  if (p.tiles * 5 < sms * 4 && nchunks >= 8) {
-    splits = p.tiles <= sms / 2 ? (int)(sms / p.tiles) : 2;
-    if (splits > nchunks / 4) splits = nchunks / 4;
-    if (splits < 1) splits = 1;
-  }
-  p.cps = (nchunks + splits - 1) / splits;
-  p.splits = (nchunks + p.cps - 1) / p.cps;
-  p.off_part = (((size_t)M + N) * 4 + 255) & ~(size_t)255;
-  p.bytes = p.off_part + (p.splits > 1 ? (size_t)p.tiles * p.splits * kBM * kBN * 4 : 0);
-  return p;
-}
-
 // The split count never falls as the SM count grows, so the plan for a full GH100 (144 SMs) bounds every sm_90a device.
 size_t gemm_tc_ws_bytes(int M, int N, int K, int batch) {
   return M > 0 && N > 0 && K > 0 ? plan(M, N, K, batch > 0 ? batch : 1, 144).bytes : 0;
+}
+// ragged entries: [amax (batch x M)][bmax (N)], no partial tiles
+size_t gemm_tc_ragged_ws_bytes(int M, int N, int batch) {
+  return M > 0 && N > 0 ? (((size_t)(batch > 0 ? batch : 1) * M + N) * 4 + 255) & ~(size_t)255 : 0;
+}
+
+// K splits of the maximum search: enough blocks to saturate HBM on the long-K operands (K up to 7.7 M rows)
+static int absmax_k_splits(int K) {
+  int ysp = K >= 4096 ? 32 : (K >= 512 ? 4 : 1);
+  if (K >= (1 << 16)) { ysp = K >> 9; if (ysp > 1024) ysp = 1024; }
+  return ysp;
+}
+static int launch_bmax(cudaStream_t s, const GemmTc& g, const float* B, int ysp, unsigned int* bmax) {
+  if (g.tb) absmax_inner_contig_kernel<<<dim3((g.N + 7) / 8, ysp), dim3(32, 8), 0, s>>>(B, g.ldb, g.N, g.K, bmax, 0, nullptr);
+  else absmax_outer_contig_kernel<<<dim3((g.N + 31) / 32, ysp), dim3(32, 8), 0, s>>>(B, g.ldb, g.N, g.K, bmax);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
+}
+
+static GemmP gemm_params(const GemmTc& g, int batch, unsigned int* amax, unsigned int* bmax) {
+  GemmP p;
+  memset(&p, 0, sizeof(p));
+  p.A = g.A; p.B = g.B; p.C = g.C; p.amax = amax; p.bmax = bmax;
+  p.lda = g.lda; p.ldb = g.ldb; p.ldc = g.ldc; p.sA = g.strideA; p.sB = g.strideB; p.sC = g.strideC;
+  p.M = g.M; p.N = g.N; p.K = g.K; p.ta = g.ta ? 1 : 0; p.tb = g.tb ? 1 : 0; p.batch = batch; p.beta = g.beta;
+  return p;
+}
+
+// Ragged entries (GemmTc::entry_rows): one pre-pass launch for the row maxima of every entry, one for the shared op(B),
+// one GEMM launch whose CTAs past an entry's rows exit at once.
+static int gemm_tc_ragged(int sm_count, cudaStream_t s, const GemmTc& g, int batch) {
+  if (g.ta || g.strideB != 0 || g.beta != 0.f)
+    return fail(T2_ERR_INVALID, "gemm_tc: ragged entries need a K-contiguous op(A), one op(B) and beta = 0");
+  const size_t need = gemm_tc_ragged_ws_bytes(g.M, g.N, batch);
+  if (g.ws_bytes < need) return fail(T2_ERR_WORKSPACE, "gemm_tc: scratch of %zu bytes, %zu needed", g.ws_bytes, need);
+  unsigned int* amax = (unsigned int*)g.ws;
+  unsigned int* bmax = amax + (size_t)batch * g.M;
+  T2_CUDA(cudaMemsetAsync(g.ws, 0, ((size_t)batch * g.M + g.N) * 4, s));
+  const int ysp = absmax_k_splits(g.K);
+  absmax_inner_contig_kernel<<<dim3((g.M + 7) / 8, ysp, batch), dim3(32, 8), 0, s>>>(g.A, g.lda, g.M, g.K, amax, g.strideA,
+                                                                                    g.entry_rows);
+  T2_LAUNCH_CHECK();
+  T2_TRY(launch_bmax(s, g, g.B, ysp, bmax));
+  GemmP p = gemm_params(g, batch, amax, bmax);
+  p.entry_rows = g.entry_rows; p.sms = sm_count;
+  const Plan pl = plan(g.M, g.N, g.K, 1, sm_count);
+  T2_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemG));
+  gemm_tc_kernel<true><<<dim3(pl.ntn, pl.ntm, batch), kThreadsG, kSmemG, s>>>(p);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
 }
 
 int gemm_tc(int sm_count, cudaStream_t s, const GemmTc& g) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return fail(T2_ERR_INVALID, "gemm_tc: empty problem %d x %d x %d", g.M, g.N, g.K);
   const int batch = g.batch > 0 ? g.batch : 1;
+  if (g.entry_rows) return gemm_tc_ragged(sm_count, s, g, batch);
   const Plan pl = plan(g.M, g.N, g.K, batch, sm_count);
   const int ntm = pl.ntm, ntn = pl.ntn, splits = pl.splits, cps = pl.cps;
   if (g.ws_bytes < pl.bytes) return fail(T2_ERR_WORKSPACE, "gemm_tc: scratch of %zu bytes, %zu needed", g.ws_bytes, pl.bytes);
@@ -359,26 +453,18 @@ int gemm_tc(int sm_count, cudaStream_t s, const GemmTc& g) {
   for (int b = 0; b < batch; ++b) {
     const float* A = g.A + (long)b * g.strideA;
     const float* B = g.B + (long)b * g.strideB;
-    // K splits of the maximum search: enough blocks to saturate HBM on the long-K operands (K up to 7.7 M rows)
-    int ysp = g.K >= 4096 ? 32 : (g.K >= 512 ? 4 : 1);
-    if (g.K >= (1 << 16)) { ysp = g.K >> 9; if (ysp > 1024) ysp = 1024; }
-    if (!g.ta) absmax_inner_contig_kernel<<<dim3((g.M + 7) / 8, ysp), dim3(32, 8), 0, s>>>(A, g.lda, g.M, g.K, amax);
+    const int ysp = absmax_k_splits(g.K);
+    if (!g.ta) absmax_inner_contig_kernel<<<dim3((g.M + 7) / 8, ysp), dim3(32, 8), 0, s>>>(A, g.lda, g.M, g.K, amax, 0, nullptr);
     else absmax_outer_contig_kernel<<<dim3((g.M + 31) / 32, ysp), dim3(32, 8), 0, s>>>(A, g.lda, g.M, g.K, amax);
     T2_LAUNCH_CHECK();
-    if (g.tb) absmax_inner_contig_kernel<<<dim3((g.N + 7) / 8, ysp), dim3(32, 8), 0, s>>>(B, g.ldb, g.N, g.K, bmax);
-    else absmax_outer_contig_kernel<<<dim3((g.N + 31) / 32, ysp), dim3(32, 8), 0, s>>>(B, g.ldb, g.N, g.K, bmax);
-    T2_LAUNCH_CHECK();
+    T2_TRY(launch_bmax(s, g, B, ysp, bmax));
   }
-  GemmP p;
-  memset(&p, 0, sizeof(p));
-  p.A = g.A; p.B = g.B; p.C = g.C; p.part = splits > 1 ? (float*)(ws + pl.off_part) : nullptr;
-  p.amax = amax; p.bmax = bmax;
-  p.lda = g.lda; p.ldb = g.ldb; p.ldc = g.ldc; p.sA = g.strideA; p.sB = g.strideB; p.sC = g.strideC;
-  p.M = g.M; p.N = g.N; p.K = g.K; p.ta = g.ta ? 1 : 0; p.tb = g.tb ? 1 : 0; p.splits = splits; p.chunks_per_split = cps;
-  p.batch = batch; p.beta = g.beta;
+  GemmP p = gemm_params(g, batch, amax, bmax);
+  p.part = splits > 1 ? (float*)(ws + pl.off_part) : nullptr;
+  p.splits = splits; p.chunks_per_split = cps;
   const size_t smem = (size_t)kSmemG;
-  T2_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  gemm_tc_kernel<<<dim3(ntn, ntm, batch * splits), kThreadsG, smem, s>>>(p);
+  T2_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  gemm_tc_kernel<false><<<dim3(ntn, ntm, batch * splits), kThreadsG, smem, s>>>(p);
   T2_LAUNCH_CHECK();
   if (splits > 1) {
     const long total = (long)g.M * g.N * batch;

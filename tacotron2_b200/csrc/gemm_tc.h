@@ -8,6 +8,11 @@ namespace t2 {
 // batch > 1: independent problems at element strides strideA / strideB / strideC (one set of operand scales).
 // ws: the caller's scratch (operand scales, split-K partial tiles) of at least gemm_tc_ws_bytes(M, N, K, batch) bytes,
 // 256-byte aligned; calls on one stream may share it.
+// entry_rows (device, batch entries; the ragged log-mel path): entry b is computed exactly as the batch = 1 call over its
+// first entry_rows[b] rows of op(A) (at most M): its own row scales, the K-split plan of gemm_tc(entry_rows[b], N, K,
+// batch = 1) with its partial tiles added in the same order (inside the CTA, no partial buffer), and rows from
+// entry_rows[b] on of C left unwritten.  Needs a K-contiguous op(A) (!ta), one op(B) for every entry (strideB = 0) and
+// beta = 0; scratch: gemm_tc_ragged_ws_bytes(M, N, batch).
 struct GemmTc {
   bool ta = false, tb = false;
   int M = 0, N = 0, K = 0;
@@ -17,10 +22,12 @@ struct GemmTc {
   float beta = 0.f;
   int batch = 1; long strideA = 0, strideB = 0, strideC = 0;
   void* ws = nullptr; size_t ws_bytes = 0;
+  const int* entry_rows = nullptr;
 };
 // sm_count plans the K splits; calls without a model (mel_spectrogram, the self-tests) plan for kGemmTcSms
 constexpr int kGemmTcSms = 132;
 size_t gemm_tc_ws_bytes(int M, int N, int K, int batch = 1);
+size_t gemm_tc_ragged_ws_bytes(int M, int N, int batch);
 int gemm_tc(int sm_count, cudaStream_t s, const GemmTc& g);
 int gemm_tc_rm(int sm_count, cudaStream_t s, void* ws, size_t ws_bytes, bool ta, bool tb, int M, int N, int K, const float* A,
                long lda, const float* B, long ldb, float* C, long ldc, float beta);

@@ -45,14 +45,33 @@ class DeviceTextMelCollate:
     """``TextMelCollate`` for samples that already live on the GPU (e.g. mels straight out of ``TacotronSTFT.mel_spectrogram``):
     one concatenation + ``t2_collate`` (rank by text length, pad, gate targets) instead of per-row host loops and five H2D
     copies.  Same 5-tuple as the reference's collate function (data_utils.py:73-111), on the device, no host synchronisation:
-    the lengths come from the tensor shapes.  Rows with equal text length keep their input order."""
+    the lengths come from the tensor shapes.  Rows with equal text length keep their input order.
 
-    def __init__(self, n_frames_per_step):
+    With ``stft`` (a ``TacotronSTFT`` on the GPU) the samples are ``(text_ids, audio)`` pairs, audio 1-D in [-1, 1] on the
+    device (the reference's ``TextMelLoader.get_mel`` with ``load_mel_from_disk=False``): the clips are zero-padded into
+    one batch and turned into mels by one ragged ``stft.mel_spectrogram(audio, lengths)`` call, each clip's mel bit for bit
+    its own B = 1 call, before the collation.  The range check of that call waits for the GPU once."""
+
+    def __init__(self, n_frames_per_step, stft=None):
         self.n_frames_per_step = n_frames_per_step
+        self.stft = stft
+
+    def _mels(self, batch):
+        """(text, audio) pairs -> (text, mel) pairs, every mel a (n_mel, n_i // hop + 1) view of one ragged call."""
+        audio = [x[1] for x in batch]
+        if any(a.dim() != 1 for a in audio):
+            raise ValueError("DeviceTextMelCollate: with an stft the samples must be (text, 1-D audio) pairs")
+        n = [int(a.numel()) for a in audio]
+        y = pad_sequence([a.to(torch.float32) for a in audio], batch_first=True)
+        mel = self.stft.mel_spectrogram(y, n)
+        hop = self.stft.hop_length
+        return [(x[0], mel[b, :, :n[b] // hop + 1]) for b, x in enumerate(batch)]
 
     def __call__(self, batch):
         import ctypes as C
         from . import _capi
+        if self.stft is not None:
+            batch = self._mels(batch)
         L = _capi.lib()
         dev = batch[0][1].device
         if dev.type != "cuda":

@@ -8,7 +8,7 @@ import ctypes as C
 import torch
 
 from . import _capi
-from .stft import STFT, _windowed_fourier_basis  # noqa: F401  (layers.py re-exports STFT, as the reference's does)
+from .stft import STFT, _lengths, _windowed_fourier_basis  # noqa: F401  (layers.py re-exports STFT, as the reference's does)
 
 
 class LinearNorm(torch.nn.Module):
@@ -86,21 +86,54 @@ class TacotronSTFT(torch.nn.Module):
     def spectral_de_normalize(self, magnitudes):
         return torch.exp(magnitudes)                                    # audio_processing.py:87-93
 
-    def mel_spectrogram(self, y):
-        """y (B, T) in [-1, 1] -> (B, n_mel_channels, T // hop_length + 1)."""
+    def mel_spectrogram(self, y, lengths=None):
+        """y (B, T) in [-1, 1] -> (B, n_mel_channels, T // hop_length + 1).
+
+        lengths (B) in samples, optional (a list, a host or a device integer tensor): row b is the log-mel of
+        ``y[b, :lengths[b]]`` alone, bit for bit the B = 1 call on those samples, with its frames from
+        lengths[b] // hop_length + 1 on zero; the samples past a row's length are never read and the range check covers
+        each row's own samples only.  Each length must lie in [filter_length // 2 + 1, T].  Without lengths, the rows
+        of a batch share each frame's operand scale (see DESIGN section 6.9), so a row can differ in its last bits from
+        its own B = 1 call."""
         if not y.is_cuda or not self.mel_basis.is_cuda:
             raise RuntimeError("tacotron2_b200.TacotronSTFT: CUDA tensors only (move the module and the audio to the GPU)")
-        assert torch.min(y.data) >= -1                                  # layers.py:74-75
-        assert torch.max(y.data) <= 1
+        if lengths is None:
+            assert torch.min(y.data) >= -1                              # layers.py:74-75
+            assert torch.max(y.data) <= 1
+        else:
+            if y.dim() != 2:
+                raise ValueError("TacotronSTFT.mel_spectrogram: y must be (B, T) with lengths, got %s" % (tuple(y.shape),))
+            host = _sample_lengths(lengths, int(y.shape[0]), int(y.shape[1]), self.filter_length)
+            len32 = torch.tensor(host, dtype=torch.int32).to(y.device, non_blocking=True)
+            own = torch.where(torch.arange(y.shape[1], device=y.device)[None, :] < len32[:, None], y.data, 0)
+            assert torch.min(own) >= -1                                 # layers.py:74-75, each row's own samples
+            assert torch.max(own) <= 1
         L = _capi.lib()
         y32 = y.detach().to(torch.float32).contiguous()
         B, n = int(y32.shape[0]), int(y32.shape[1])
         frames = int(L.t2_mel_spectrogram_frames(n, self.hop_length))
         out = torch.empty(B, self.n_mel_channels, frames, device=y.device, dtype=torch.float32)
-        ws = self._ws.get("mel", L.t2_mel_spectrogram_workspace_bytes(B, n, self.filter_length, self.hop_length,
-                                                                       self.n_mel_channels), y.device)
+        query = L.t2_mel_spectrogram_workspace_bytes if lengths is None else L.t2_mel_spectrogram_workspace_bytes_lengths
+        ws = self._ws.get("mel", query(B, n, self.filter_length, self.hop_length, self.n_mel_channels), y.device)
         a = _capi.T2MelSpecArgs(y32.data_ptr(), B, n, self.filter_length, self.hop_length, self.n_mel_channels,
                                 self.forward_basis.data_ptr(), self.mel_basis.data_ptr(), 1e-5, out.data_ptr(),
-                                ws.data_ptr(), ws.numel())
+                                ws.data_ptr(), ws.numel(), None if lengths is None else len32.data_ptr())
         _capi.call(L.t2_mel_spectrogram, y.device, C.byref(a))
         return out
+
+
+def _sample_lengths(lengths, B, n, filter_length):
+    """Per-row sample counts as a host list of ints: B integers in [filter_length // 2 + 1, n] (what reflect padding by
+    filter_length // 2 needs), from a list or a host / device integer tensor.  Raises TypeError / ValueError."""
+    what = "TacotronSTFT.mel_spectrogram"
+    _lengths(lengths, B, None, what)
+    t = torch.as_tensor(lengths)
+    if t.dtype == torch.bool or t.dtype.is_floating_point or t.dtype.is_complex:
+        raise TypeError("%s: lengths must hold integers (got %s)" % (what, t.dtype))
+    lo = filter_length // 2 + 1
+    vals = [int(v) for v in t.tolist()]
+    for b, v in enumerate(vals):
+        if not lo <= v <= n:
+            raise ValueError("%s: length %d of row %d lies outside [%d, %d] (reflect padding by %d needs more than %d "
+                             "samples, and a row holds at most the %d columns of y)" % (what, v, b, lo, n, lo - 1, lo - 1, n))
+    return vals
