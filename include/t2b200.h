@@ -171,6 +171,19 @@ int    t2_encoder_backward(T2Model* m, const T2EncoderBwdArgs* a, void* stream);
  * is what a B = 1 call with seed = row_seeds[b] draws.  Row b's outputs then equal that call's bit for bit, whatever
  * its batch, its 64-row slice, the stream chunking or the serving slot.  NULL: one key for the call, element
  * b * 256 + j. */
+/* Forced alignment (forced_align and forced_lengths both set; INFER, training = 0, persistent implementation): the
+ * attention weights are given instead of computed, as in Mellotron's inference_noattention.  forced_align
+ * (B, n_steps_cap, T_enc) fp32 and forced_lengths (B) int32 are on the device.  Row b runs forced_lengths[b] steps (the
+ * call clamps each into [1, n_steps_cap] and never reads outside the map); at step t < forced_lengths[b] its context is
+ * sum_j forced_align[b, t, j] * memory[b, j] over j < memory_lengths[b] -- the weights are used as given, not normalised
+ * or checked -- and every other step of the row (its 64-row slice is still running) uses zero weights.  align holds
+ * the weights used: the given ones below memory_lengths[b], zero beyond.  The gate is computed and written but stops
+ * nothing, and gate_threshold plays no part: mel_lengths[b] = forced_lengths[b], and the loop ends when every row has
+ * run its steps.  The prenet, both LSTMs, the projection and the dropout keys are those of the free run, so feeding a
+ * free run's own align and mel_lengths back reproduces its mel and gate bit for bit.  Both NULL: today's behaviour.
+ * T2_ERR_INVALID: only one of the two set, mode TEACHER, or training = 1; T2_ERR_UNSUPPORTED: the stepwise
+ * implementation (requested, or chosen by AUTO for a T_enc the persistent kernel does not take).  The resumable
+ * stream indexes the map by absolute step; continuous batching (admit / collect) and t2_infer_host take no map. */
 typedef struct T2DecoderArgs {
   int32_t mode, impl, training;
   const float* memory; const int32_t* memory_lengths; int32_t B, T_enc, n_steps_cap;
@@ -183,6 +196,8 @@ typedef struct T2DecoderArgs {
   void* stash; size_t stash_bytes;     /* TEACHER only, optional: activations kept for t2_decoder_backward
                                           (t2_decoder_stash_bytes(); opaque to the caller) */
   const uint64_t* row_seeds;           /* (B) or NULL: per-row Philox keys of the prenet dropout (see below) */
+  const float* forced_align;           /* (B, n_steps_cap, T_enc) or NULL: given attention weights (see above) */
+  const int32_t* forced_lengths;       /* (B) or NULL: steps of each row of a forced run */
 } T2DecoderArgs;
 size_t t2_decoder_workspace_bytes(const T2Model* m, int32_t B, int32_t T_enc, int32_t n_steps_cap);
 int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);

@@ -82,7 +82,8 @@ class T2DecoderArgs(C.Structure):
                 ("mel", C.c_void_p), ("gate", C.c_void_p), ("align", C.c_void_p),
                 ("mel_lengths", C.c_void_p), ("n_steps", C.c_void_p),
                 ("ws", C.c_void_p), ("ws_bytes", C.c_size_t),
-                ("stash", C.c_void_p), ("stash_bytes", C.c_size_t), ("row_seeds", C.c_void_p)]
+                ("stash", C.c_void_p), ("stash_bytes", C.c_size_t), ("row_seeds", C.c_void_p),
+                ("forced_align", C.c_void_p), ("forced_lengths", C.c_void_p)]
 
 
 class T2DecoderStreamArgs(C.Structure):

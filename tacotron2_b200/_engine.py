@@ -130,6 +130,72 @@ def row_seeds(seeds, B, device, what):
     return torch.tensor(bits, dtype=torch.int64).to(device)
 
 
+def forced_alignment(alignments, alignment_lengths, B, T_text, device, training, what):
+    """Given attention weights for a forced run as the engine takes them: (map (B, T_map, T_text) fp32 contiguous,
+    lengths (B,) int32), both on `device`; (None, None) without a map.  alignments: a float tensor (B, T_map, T_text) on
+    `device`; alignment_lengths: None (T_map for every row) or B integers in 1..T_map as a list, a host or a device
+    tensor.  Raises TypeError / ValueError naming the argument before anything runs."""
+    if alignments is None:
+        if alignment_lengths is not None:
+            raise ValueError("%s: alignment_lengths needs alignments" % what)
+        return None, None
+    if training:
+        raise ValueError("%s: alignments need eval mode (a forced run is an inference; training-mode inference applies "
+                         "the hidden-state dropout, which a forced run does not take)" % what)
+    if not torch.is_tensor(alignments):
+        raise TypeError("%s: alignments must be a tensor (got %s)" % (what, type(alignments).__name__))
+    if not alignments.dtype.is_floating_point:
+        raise TypeError("%s: alignments must be a float tensor (got %s)" % (what, alignments.dtype))
+    if alignments.dim() != 3 or alignments.shape[0] != B or alignments.shape[1] < 1 or alignments.shape[2] != T_text:
+        raise ValueError("%s: alignments must have shape (%d, T_map >= 1, %d) (got %s)" % (what, B, T_text,
+                                                                                          tuple(alignments.shape)))
+    if alignments.device != torch.device(device):
+        raise ValueError("%s: alignments must be on the model's device %s (got %s)" % (what, device, alignments.device))
+    T_map = int(alignments.shape[1])
+    if alignment_lengths is None:
+        lengths = torch.full((B,), T_map, dtype=torch.int32, device=device)
+    else:
+        lengths = alignment_lengths if torch.is_tensor(alignment_lengths) else torch.as_tensor(alignment_lengths)
+        if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+            raise TypeError("%s: alignment_lengths must hold integers (got %s)" % (what, lengths.dtype))
+        if tuple(lengths.shape) != (B,):
+            raise ValueError("%s: alignment_lengths must have shape (%d,) (got %s)" % (what, B, tuple(lengths.shape)))
+        host = lengths.cpu()
+        lo, hi = int(host.min()), int(host.max())
+        if lo < 1 or hi > T_map:
+            raise ValueError("%s: alignment_lengths must lie in 1..%d (got %d..%d)" % (what, T_map, lo, hi))
+        lengths = lengths.to(device=device, dtype=torch.int32).contiguous()
+    return alignments.to(dtype=torch.float32).contiguous(), lengths
+
+
+def alignments_from_durations(durations):
+    """Durations (B, T_text) of non-negative integer frame counts -> (alignments, alignment_lengths) for a forced
+    ``Tacotron2.inference``: a one-hot map (B, T_map, T_text) fp32 in which symbol j of row b is attended for
+    durations[b, j] consecutive steps, and the steps of each row, durations.sum(1) (int64), both on durations' device;
+    T_map is the longest row.  Rows whose counts sum to 0 are refused."""
+    d = durations if torch.is_tensor(durations) else torch.as_tensor(durations)
+    if d.dtype.is_floating_point or d.dtype.is_complex or d.dtype == torch.bool:
+        raise TypeError("tacotron2_b200: durations must hold integers (got %s)" % d.dtype)
+    if d.dim() != 2 or d.shape[1] < 1:
+        raise ValueError("tacotron2_b200: durations must have shape (B, T_text) (got %s)" % (tuple(d.shape),))
+    d = d.long()
+    if bool((d < 0).any()):
+        raise ValueError("tacotron2_b200: durations must be >= 0")
+    lengths = d.sum(1)
+    empty = (lengths == 0).nonzero().flatten().tolist()
+    if empty:
+        raise ValueError("tacotron2_b200: durations of rows %s sum to 0 frames" % empty)
+    B, T = d.shape
+    total = int(lengths.sum())
+    dev = d.device
+    sym = torch.repeat_interleave(torch.arange(T, device=dev).repeat(B), d.reshape(-1))            # symbol of each step
+    row = torch.repeat_interleave(torch.arange(B, device=dev), lengths)
+    step = torch.arange(total, device=dev) - torch.repeat_interleave(lengths.cumsum(0) - lengths, lengths)
+    out = torch.zeros(B, int(lengths.max()), T, dtype=torch.float32, device=dev)
+    out[row, step, sym] = 1.0
+    return out, lengths
+
+
 def _i32(x, device):
     """Per-row lengths as contiguous int32 on the device (None stays None)."""
     return None if x is None else x.to(device=device, dtype=torch.int32).contiguous()
@@ -315,8 +381,11 @@ class Engine(_Handle):
     # -- decoder ---------------------------------------------------------------------------------
     def decoder(self, memory, mode, n_steps_cap, memory_lengths=None, teacher_prenet=None, training=False,
                 prenet_keep=None, att_keep=None, dec_keep=None, gate_threshold=0.5,
-                score_mask_value=-float("inf"), impl=None, stash=None, seed=None, row_seeds=None):
-        """row_seeds: None or (B,) int64 on the device (see row_seeds()): per-row prenet keys."""
+                score_mask_value=-float("inf"), impl=None, stash=None, seed=None, row_seeds=None, forced_align=None,
+                forced_lengths=None):
+        """row_seeds: None or (B,) int64 on the device (see row_seeds()): per-row prenet keys.  forced_align /
+        forced_lengths: None, or the given attention weights (B, n_steps_cap, T_enc) fp32 and each row's step count (B,)
+        int32, both contiguous on the device (see forced_alignment())."""
         L = _capi.lib()
         memory = memory.to(device=self.device, dtype=torch.float32).contiguous()
         B, T = int(memory.shape[0]), int(memory.shape[1])
@@ -338,18 +407,19 @@ class Engine(_Handle):
                                 next_seed() if seed is None else seed, float(gate_threshold), float(score_mask_value),
                                 mel.data_ptr(), gate.data_ptr(), align.data_ptr(), mel_lengths.data_ptr(),
                                 n_steps.data_ptr(), ws.data_ptr(), ws.numel(),
-                                _ptr(stash), 0 if stash is None else stash.numel(), _ptr(row_seeds))
+                                _ptr(stash), 0 if stash is None else stash.numel(), _ptr(row_seeds),
+                                _ptr(forced_align), _ptr(forced_lengths))
         self._call(L.t2_decoder_run, C.byref(a))
         self._last_decoder_args = (a, memory, len32, teacher_prenet, pk, ak, dk, ws, mel, gate, align, mel_lengths, n_steps,
-                                   row_seeds)
+                                   row_seeds, forced_align, forced_lengths)
         return mel, gate, align, mel_lengths, n_steps
 
     def decoder_stream(self, memory, n_steps_cap, prenet_keep=None, gate_threshold=0.5, score_mask_value=-float("inf"),
-                       impl=None, seed=None, memory_lengths=None, row_seeds=None):
+                       impl=None, seed=None, memory_lengths=None, row_seeds=None, forced_align=None, forced_lengths=None):
         """Begins a resumable INFER run of the persistent decoder (t2_decoder_stream_begin); see DecoderStream."""
         return DecoderStream(self, memory, n_steps_cap, prenet_keep, gate_threshold, score_mask_value,
                              self.impl if impl is None else impl, next_seed() if seed is None else seed, memory_lengths,
-                             row_seeds)
+                             row_seeds, forced_align, forced_lengths)
 
     def decoder_profile(self):
         """Per-phase SM cycles of the last persistent decoder run: dict phase -> [cta0, cta60, cta100]."""
@@ -482,7 +552,7 @@ class DecoderStream:
     their rows in place between chunks."""
 
     def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed, memory_lengths=None,
-                 row_seeds=None):
+                 row_seeds=None, forced_align=None, forced_lengths=None):
         L = _capi.lib()
         dev = eng.device
         self.eng = eng
@@ -502,10 +572,12 @@ class DecoderStream:
         self.state = _capi.byte_buffer(L.t2_decoder_stream_state_bytes(eng.handle, B, T), dev)
         self.keep, self.len32 = _u8(prenet_keep, dev), _i32(memory_lengths, dev)
         self.row_seeds = row_seeds      # (B,) int64 bit patterns on the device or None; a session may rewrite them
+        self.forced = (forced_align, forced_lengths)     # the kernel reads them in every chunk
         d = _capi.T2DecoderArgs(_capi.MODE_INFER, impl, 0, self.memory.data_ptr(), _ptr(self.len32), B, T, self.cap,
                                 None, _ptr(self.keep), None, None, seed, float(gate_threshold), float(score_mask_value),
                                 self.mel.data_ptr(), self.gate.data_ptr(), self.align.data_ptr(),
-                                self.mel_lengths.data_ptr(), self.n_steps.data_ptr(), row_seeds=_ptr(row_seeds))
+                                self.mel_lengths.data_ptr(), self.n_steps.data_ptr(), row_seeds=_ptr(row_seeds),
+                                forced_align=_ptr(forced_align), forced_lengths=_ptr(forced_lengths))
         self.args = _capi.T2DecoderStreamArgs(d, self.state.data_ptr(), self.state.numel(), self.status.data_ptr())
         eng._call(L.t2_decoder_stream_begin, C.byref(self.args))
 

@@ -132,6 +132,17 @@ static int check_row_seeds(const T2DecoderArgs* a, const char* what) {
   return T2_OK;
 }
 
+// given attention weights: both pointers or neither, evaluation-mode INFER only
+static int check_forced(const T2DecoderArgs* a, const char* what) {
+  if (!a->forced_align != !a->forced_lengths)
+    return fail(T2_ERR_INVALID, "%s: forced_align and forced_lengths go together (got only %s)", what,
+                a->forced_align ? "forced_align" : "forced_lengths");
+  if (a->forced_align && (a->mode != T2_MODE_INFER || a->training))
+    return fail(T2_ERR_INVALID, "%s: a forced alignment needs mode INFER with training = 0 (mode %d, training %d)", what,
+                a->mode, a->training);
+  return T2_OK;
+}
+
 static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a) {
   if (!m || !a) return fail(T2_ERR_INVALID, "null model / args");
   if (a->B <= 0 || a->B > kMaxBatch) return fail(T2_ERR_INVALID, "decoder: B=%d outside [1, %d]", a->B, kMaxBatch);
@@ -142,6 +153,7 @@ static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a) {
   if (a->mode == T2_MODE_TEACHER && !a->teacher_prenet) return fail(T2_ERR_INVALID, "decoder: teacher mode needs teacher_prenet");
   if (a->mode != T2_MODE_TEACHER && a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "decoder: bad mode %d", a->mode);
   if (a->ws_bytes < decoder_ws_bytes(a->B, a->T_enc, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
+  T2_TRY(check_forced(a, "decoder"));
   return check_row_seeds(a, "decoder");
 }
 
@@ -262,6 +274,10 @@ int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) {
                   a->T_enc);
     return decoder_run_persistent(m, a, (cudaStream_t)stream);
   }
+  if (a->forced_align)
+    return fail(T2_ERR_UNSUPPORTED, "decoder: a forced alignment needs the persistent implementation (%s)",
+                a->impl == T2_IMPL_STEPWISE ? "impl = STEPWISE was requested"
+                                            : "this shape / device does not fit it: T_enc too large for shared memory or < 128 SMs");
   // only the persistent kernel writes the training stash: a backward pass over a stash the stepwise path left
   // untouched would silently produce garbage gradients
   if (a->stash)
@@ -293,6 +309,7 @@ static int check_stream_args(const T2Model* m, const T2DecoderStreamArgs* s) {
                                     "(at most 2274, and >= 128 SMs)", a->T_enc);
   if (s->state_bytes < persistent_stream_state_bytes(a->B, a->T_enc)) return fail(T2_ERR_WORKSPACE, "decoder stream state too small");
   if (s->row_step0 && !a->row_seeds) return fail(T2_ERR_INVALID, "decoder stream: row_step0 needs dec.row_seeds");
+  T2_TRY(check_forced(a, "decoder stream"));
   return check_row_seeds(a, "decoder stream");
 }
 
@@ -311,6 +328,7 @@ int t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int3
   T2_TRY(check_stream_args(m, a));
   if (n_rows < 1 || n_rows > a->dec.B || !rows) return fail(T2_ERR_INVALID, "decoder stream admit: n_rows=%d outside [1, B=%d]", n_rows, a->dec.B);
   if (!a->dec.memory_lengths) return fail(T2_ERR_INVALID, "decoder stream admit: the stream has no memory_lengths");
+  if (a->dec.forced_align) return fail(T2_ERR_INVALID, "decoder stream admit: continuous batching takes no forced alignment");
   for (int i = 0; i < n_rows; ++i)
     if (rows[i] < 0 || rows[i] >= a->dec.B || (i > 0 && rows[i] <= rows[i - 1]))
       return fail(T2_ERR_INVALID, "decoder stream admit: rows must be ascending and inside [0, B=%d) (rows[%d]=%d)", a->dec.B, i, rows[i]);

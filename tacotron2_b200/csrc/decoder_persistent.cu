@@ -384,6 +384,9 @@ struct KParams {
   float* rs_att;                    // (kG, 2, padded TP) previous | cumulative attention weights
   int32_t* rs_done;                 // (kRows) stop latch
   int32_t* rs_status;               // out: [steps run, stopped]
+  // forced alignment (INFER, the kForced instantiation): rows b0.. of the given attention weights (Btot, cap, T) and
+  // their step counts (Btot), clamped into [1, cap] where they are read
+  const float* forced_align; const int32_t* forced_lengths;
 };
 
 // encoder-memory rows of a T_enc-long row that the attention phase stages in an idle ring of `nstages` stages beside the
@@ -422,6 +425,10 @@ __device__ __forceinline__ void store_split2(uint8_t* img, int row, int k, float
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
+// kForced (INFER with p.forced_align): the attention weights of step t are row t of the given map instead of the softmax
+// of the energies, and row b stops after forced_lengths[b] steps instead of on its gate.  The location term, the energies
+// and the softmax are skipped; the events, barriers and the context routine are those of the free run.
+template <bool kForced>
 __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const KParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -633,7 +640,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     // positions per round, round 0 before the B2 wait.
     const bool att_cta = (cta & 63) < p.B;
     const int att_b = cta & 63, ahalf = cta >> 6;
-    const bool pa_pre = p.pa != nullptr;
+    const bool pa_pre = !kForced && p.pa != nullptr;
     const int pa_p = pa_pitch(T);
     float* pa_row = pa_pre ? p.pa + (size_t)att_b * kAtt * pa_p : nullptr;
     uint8_t* aimg = rg.stage0;
@@ -719,7 +726,19 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
 #pragma unroll
       for (int e = 0; e < 8; ++e) pm_next[e] = (j0 + e < cnt) ? __ldg(pmr + (long)(j0 + e) * kAtt) : 0.f;
     };
-    if (att_cta) {
+    if (att_cta && kForced) {
+      // the weights of step t do not depend on q: row t of the row's map (zero past its text length, and all zero once
+      // the row has run its steps, without reading the map) goes to s_e and the alignment output before the q barrier
+      const int len = p.mem_len ? min(p.mem_len[att_b], T) : T;
+      const int flen = min(max(p.forced_lengths[att_b], 1), p.cap);
+      const float* fa = p.forced_align + ((long)att_b * p.cap + t) * T;
+      for (int j = tid; j < T; j += kThreads) {
+        const float a = (t < flen && j < len) ? __ldg(fa + j) : 0.f;
+        s_e[j] = a;
+        if (ahalf == 0) p.align[((long)att_b * p.cap + t) * T + j] = a;
+      }
+      stage_memory_rows(0, smem_rows);
+    } else if (att_cta) {
       if (pa_pre) {
         // CTA b+64 wrote this tile before it signalled its ah columns of this step, or in the launch of the previous
         // chunk, or the buffer was zeroed before step 0 (the attention weights start at zero, so pa is +0.0); thread 0
@@ -739,93 +758,97 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     T2_PROF(4);
     if (att_cta) {
       const int b = att_b;
-      for (int i = tid; i < kAtt; i += kThreads) s_q[i] = __ldcg(&p.q[b * kAtt + i]);
-      __syncthreads();
-      {
-        const int eN = ntiles * 128;
-        const float qd = s_q[adim], vd = s_v[adim];
-        // with the copied tile: one pass over all T positions; else one round of 64 positions per pa GEMM.  Chunks of 8
-        // positions start at multiples of 8 either way, so every energy is the same sum in the same order.
-        const int nrounds = pa_pre ? 1 : att_rounds, rlen = pa_pre ? T : kAttRound;
-        const float* s_tile = pa_pre ? reinterpret_cast<const float*>(rg.stage0) : s_pa;
-        const int tpitch = pa_pre ? pa_p : kPaPitch;
-        if (pa_pre) { mbar_wait(bar_pa, pa_phase, ctrl, 207); pa_phase ^= 1; }
-        for (int r0 = 0; r0 < nrounds; ++r0) {
-          const int jbase = r0 * kAttRound, cnt = min(T - jbase, rlen), nch = (cnt + 7) >> 3;
-          if (r0 > 0) att_pa_round(r0, s_pa, kPaPitch, kAttRound);
-          T2_PROF(16);
-          // energies e_j = sum_d v_d tanh(q_d + pa_dj + pm_jd): this thread adds dim d = adim for the 8 positions of
-          // each of its chunks, then the 32 dims of the warp are summed with a transpose-reduce (9 shuffles per 8
-          // positions, fixed order); the four 32-dim groups of a position are added in a fixed order at the softmax
-          const float* pmr = p.pm + ((long)b * T + jbase) * kAtt + adim;
-          if (r0 > 0) load_pm(pmr, cg * 8, cnt);
-#pragma unroll 1
-          for (int c = cg; c < nch; c += 4) {
-            const int j0 = c * 8;
-            float pm8[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) pm8[e] = pm_next[e];
-            if (c + 4 < nch) load_pm(pmr, j0 + 32, cnt);           // next chunk's loads fly during this chunk's tanh
-            float g[8], sv[8];
-            {
-              const float4 g0 = *reinterpret_cast<const float4*>(s_tile + adim * tpitch + j0);
-              const float4 g1 = *reinterpret_cast<const float4*>(s_tile + adim * tpitch + j0 + 4);
-              g[0] = g0.x; g[1] = g0.y; g[2] = g0.z; g[3] = g0.w; g[4] = g1.x; g[5] = g1.y; g[6] = g1.z; g[7] = g1.w;
-            }
-#pragma unroll
-            for (int e = 0; e < 8; ++e) sv[e] = vd * tanh_fast(qd + g[e] + pm8[e]);
-            float r4[4], r2[2], r1;
-            {
-              const bool up = (lane & 16) != 0;
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float send = up ? sv[e] : sv[e + 4], keep = up ? sv[e + 4] : sv[e];
-                r4[e] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+      if constexpr (!kForced) {             // the query, the location term and the energies
+        for (int i = tid; i < kAtt; i += kThreads) s_q[i] = __ldcg(&p.q[b * kAtt + i]);
+        __syncthreads();
+        {
+          const int eN = ntiles * 128;
+          const float qd = s_q[adim], vd = s_v[adim];
+          // with the copied tile: one pass over all T positions; else one round of 64 positions per pa GEMM.  Chunks of 8
+          // positions start at multiples of 8 either way, so every energy is the same sum in the same order.
+          const int nrounds = pa_pre ? 1 : att_rounds, rlen = pa_pre ? T : kAttRound;
+          const float* s_tile = pa_pre ? reinterpret_cast<const float*>(rg.stage0) : s_pa;
+          const int tpitch = pa_pre ? pa_p : kPaPitch;
+          if (pa_pre) { mbar_wait(bar_pa, pa_phase, ctrl, 207); pa_phase ^= 1; }
+          for (int r0 = 0; r0 < nrounds; ++r0) {
+            const int jbase = r0 * kAttRound, cnt = min(T - jbase, rlen), nch = (cnt + 7) >> 3;
+            if (r0 > 0) att_pa_round(r0, s_pa, kPaPitch, kAttRound);
+            T2_PROF(16);
+            // energies e_j = sum_d v_d tanh(q_d + pa_dj + pm_jd): this thread adds dim d = adim for the 8 positions of
+            // each of its chunks, then the 32 dims of the warp are summed with a transpose-reduce (9 shuffles per 8
+            // positions, fixed order); the four 32-dim groups of a position are added in a fixed order at the softmax
+            const float* pmr = p.pm + ((long)b * T + jbase) * kAtt + adim;
+            if (r0 > 0) load_pm(pmr, cg * 8, cnt);
+  #pragma unroll 1
+            for (int c = cg; c < nch; c += 4) {
+              const int j0 = c * 8;
+              float pm8[8];
+  #pragma unroll
+              for (int e = 0; e < 8; ++e) pm8[e] = pm_next[e];
+              if (c + 4 < nch) load_pm(pmr, j0 + 32, cnt);           // next chunk's loads fly during this chunk's tanh
+              float g[8], sv[8];
+              {
+                const float4 g0 = *reinterpret_cast<const float4*>(s_tile + adim * tpitch + j0);
+                const float4 g1 = *reinterpret_cast<const float4*>(s_tile + adim * tpitch + j0 + 4);
+                g[0] = g0.x; g[1] = g0.y; g[2] = g0.z; g[3] = g0.w; g[4] = g1.x; g[5] = g1.y; g[6] = g1.z; g[7] = g1.w;
               }
-            }
-            {
-              const bool up = (lane & 8) != 0;
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const float send = up ? r4[e] : r4[e + 2], keep = up ? r4[e + 2] : r4[e];
-                r2[e] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+  #pragma unroll
+              for (int e = 0; e < 8; ++e) sv[e] = vd * tanh_fast(qd + g[e] + pm8[e]);
+              float r4[4], r2[2], r1;
+              {
+                const bool up = (lane & 16) != 0;
+  #pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const float send = up ? sv[e] : sv[e + 4], keep = up ? sv[e + 4] : sv[e];
+                  r4[e] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+                }
               }
+              {
+                const bool up = (lane & 8) != 0;
+  #pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float send = up ? r4[e] : r4[e + 2], keep = up ? r4[e + 2] : r4[e];
+                  r2[e] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+                }
+              }
+              {
+                const bool up = (lane & 4) != 0;
+                const float send = up ? r2[0] : r2[1], keep = up ? r2[1] : r2[0];
+                r1 = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+              }
+              r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
+              r1 += __shfl_xor_sync(0xffffffffu, r1, 1);
+              const int jj = j0 + ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
+              if ((lane & 3) == 0 && jj < cnt) s_ep[quad * eN + jbase + jj] = r1;
             }
-            {
-              const bool up = (lane & 4) != 0;
-              const float send = up ? r2[0] : r2[1], keep = up ? r2[1] : r2[0];
-              r1 = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-            }
-            r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
-            r1 += __shfl_xor_sync(0xffffffffu, r1, 1);
-            const int jj = j0 + ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-            if ((lane & 3) == 0 && jj < cnt) s_ep[quad * eN + jbase + jj] = r1;
+            __syncthreads();
+            T2_PROF(17);
           }
-          __syncthreads();
-          T2_PROF(17);
         }
       }
       // mask + softmax (model.py:79-82): every warp reduces all T energies itself (shuffles only, no
       // cross-warp exchange), then the threads split the normalised write-out
       const int len = p.mem_len ? min(p.mem_len[b], T) : T;
-      const int eN = ntiles * 128;
-      // masked energies once (the four 32-dim partial sums added in a fixed order), in place in the first partial-sum plane
-      for (int j = tid; j < T; j += kThreads)
-        s_ep[j] = (j < len) ? (s_ep[j] + s_ep[eN + j]) + (s_ep[2 * eN + j] + s_ep[3 * eN + j]) : p.score_mask_value;
-      __syncthreads();
-      float mx = -INFINITY;
-      for (int j = lane; j < T; j += 32) mx = fmaxf(mx, s_ep[j]);
-      mx = warp_max_f(mx);
-      float sum = 0.f;
-      for (int j = lane; j < T; j += 32) sum += expf(s_ep[j] - mx);
-      sum = warp_sum_f(sum);
-      const float inv = 1.f / sum;
-      for (int j = tid; j < T; j += kThreads) {
-        const float a = expf(s_ep[j] - mx) * inv;
-        s_e[j] = a;
-        s_pad0[halfk + j] = a;                                                // becomes "previous"
-        s_pad1[halfk + j] += a;                                               // model.py:365
-        if (ahalf == 0) p.align[((long)b * p.cap + t) * T + j] = a;
+      if constexpr (!kForced) {             // the softmax and the previous / cumulative weights
+        const int eN = ntiles * 128;
+        // masked energies once (the four 32-dim partial sums added in a fixed order), in place in the first partial-sum plane
+        for (int j = tid; j < T; j += kThreads)
+          s_ep[j] = (j < len) ? (s_ep[j] + s_ep[eN + j]) + (s_ep[2 * eN + j] + s_ep[3 * eN + j]) : p.score_mask_value;
+        __syncthreads();
+        float mx = -INFINITY;
+        for (int j = lane; j < T; j += 32) mx = fmaxf(mx, s_ep[j]);
+        mx = warp_max_f(mx);
+        float sum = 0.f;
+        for (int j = lane; j < T; j += 32) sum += expf(s_ep[j] - mx);
+        sum = warp_sum_f(sum);
+        const float inv = 1.f / sum;
+        for (int j = tid; j < T; j += kThreads) {
+          const float a = expf(s_ep[j] - mx) * inv;
+          s_e[j] = a;
+          s_pad0[halfk + j] = a;                                                // becomes "previous"
+          s_pad1[halfk + j] += a;                                               // model.py:365
+          if (ahalf == 0) p.align[((long)b * p.cap + t) * T + j] = a;
+        }
       }
       asm volatile("cp.async.wait_group 0;" ::: "memory");
       __syncthreads();
@@ -936,7 +959,9 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
             p.gate[(long)row * p.cap + t] = v;                                 // model.py:378
             if (p.infer) {
               int done = ctrl->done[row];
-              if (!done && sigmoid_exact(v) > p.gate_threshold) {             // model.py:443
+              // model.py:443; forced: the row's step count decides, its gate plays no part
+              if (!done && (kForced ? t + 1 == min(max(p.forced_lengths[row], 1), p.cap)
+                                    : sigmoid_exact(v) > p.gate_threshold)) {
                 done = 1; ctrl->done[row] = 1; p.mel_lengths[row] = t + 1;
               }
               if (!done) atomicAdd(s_live, 1);
@@ -979,7 +1004,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       // computes the location term of step t+1 from this step's attention weights, every round, into row b's block of
       // p.pa.  A resumed chunk reads it from there.  Its ah signal of step t+1 orders these stores before both CTAs of the
       // pair copy the tile.
-      if (pa_pre && ahalf == 1 && att_cta && t + 1 < p.cap)
+      if (!kForced && pa_pre && ahalf == 1 && att_cta && t + 1 < p.cap)
         for (int r0 = 0; r0 < att_rounds; ++r0)
           att_pa_round(r0, pa_row + r0 * kAttRound, pa_p, min(T - r0 * kAttRound, kAttRound));
       T2_PROF(20);
@@ -1255,6 +1280,10 @@ static void slice_params(T2Model* m, const T2DecoderArgs* a, const SliceBuffer& 
   p.p_att = m->cfg.p_attention_dropout; p.p_dec = m->cfg.p_decoder_dropout; p.seed = a->seed;
   p.row_seeds = a->row_seeds;
   p.t_begin = 0; p.t_end = cap;
+  if (a->forced_align) {              // no location term: the forced kernel neither computes nor reads pa
+    p.forced_align = a->forced_align + (size_t)b0 * cap * T; p.forced_lengths = a->forced_lengths + b0;
+    p.pa = nullptr;
+  }
 }
 
 // the longest T_enc that persistent_stages() runs with 4 stages (0 when none does); stages fall as T_enc grows
@@ -1272,14 +1301,15 @@ static int launch_persistent(KParams& p, cudaStream_t s) {
   p.nstages = persistent_stages(p.T);
   p.t4max = persistent_t4max();
   const size_t smem = persistent_smem_bytes(p.T, p.nstages);
-  T2_CUDA(cudaFuncSetAttribute(decoder_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  void (*kernel)(KParams) = p.forced_align ? decoder_persistent_kernel<true> : decoder_persistent_kernel<false>;
+  T2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(kG); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
   cudaLaunchAttribute attr;
   attr.id = cudaLaunchAttributeCooperative; attr.val.cooperative = 1;   // co-residency of all 128 CTAs
   cfg.attrs = &attr; cfg.numAttrs = 1;
-  const cudaError_t le = cudaLaunchKernelEx(&cfg, decoder_persistent_kernel, p);
+  const cudaError_t le = cudaLaunchKernelEx(&cfg, kernel, p);
   if (le != cudaSuccess) return fail(T2_ERR_CUDA, "persistent decoder launch failed: %s", cudaGetErrorString(le));
   if (getenv("T2_VERBOSE")) fprintf(stderr, "[t2b200] persistent decoder: B=%d T_enc=%d cap=%d stages=%d smem=%zu steps=%d-%d\n",
                                     p.B, p.T, p.cap, p.nstages, smem, p.t_begin, p.t_end);

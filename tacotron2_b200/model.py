@@ -449,7 +449,12 @@ class Decoder(_EngineOwner, nn.Module):
             raise ValueError("tacotron2_b200: %s: seeds and injected prenet masks exclude each other" % what)
         return _engine_mod.row_seeds(seeds, B, device, "tacotron2_b200: " + what)
 
-    def inference(self, memory, memory_lengths=None, seeds=None):
+    def _forced(self, alignments, alignment_lengths, memory, device, what):
+        """alignments / alignment_lengths (see inference) as the engine's (map, lengths), or (None, None)."""
+        return _engine_mod.forced_alignment(alignments, alignment_lengths, memory.size(0), memory.size(1), device,
+                                            self.training, "tacotron2_b200: " + what)
+
+    def inference(self, memory, memory_lengths=None, seeds=None, alignments=None, alignment_lengths=None):
         """Free-running pass (model.py:418-454), batched: per-row stop latch, see README "batched
         inference".  Returns mel (B, n_mel, T), gate (B, T, 1), alignments (B, T, T_enc); T = steps
         until every row has fired (or max_decoder_steps); ``self.mel_lengths`` holds per-row lengths.  In training mode
@@ -458,42 +463,55 @@ class Decoder(_EngineOwner, nn.Module):
         any order: row b attends to memory[b, :memory_lengths[b]] only and its outputs equal those of a call on that
         slice alone, bit for bit; its alignments past memory_lengths[b] are zero.  seeds: B integers in [0, 2**64) (list,
         host or device tensor), eval mode only: row b draws the prenet dropout of a B = 1 call seeded seeds[b], so its
-        outputs equal that call's bit for bit in any batch."""
+        outputs equal that call's bit for bit in any batch.
+
+        alignments (B, T_map, T_enc), any float dtype (read as fp32), on the model's device, eval mode only: a forced run
+        (Mellotron's inference_noattention).  Row b runs alignment_lengths[b] steps (B integers in 1..T_map; default
+        T_map) and at step t takes the context sum_j alignments[b, t, j] memory[b, j] over j < memory_lengths[b], with
+        the weights as given; its gate is computed but stops nothing, and max_decoder_steps plays no part.  The returned
+        alignments are the weights used (zero past memory_lengths[b] and past the row's steps); injected prenet masks
+        are (T_map, 2, B, 256).  Row b equals its own B = 1 forced call bit for bit, and a seeded free run fed its own
+        alignments and mel_lengths comes out again bit for bit."""
         memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
         eng = self._t2_engine()
         row_seeds = self._row_seeds(seeds, memory.size(0), eng.device, "Decoder.inference")
+        fa, fl = self._forced(alignments, alignment_lengths, memory, eng.device, "Decoder.inference")
         masks = current_masks()
         mel, gate, align, lengths, n_steps = eng.decoder(
-            memory, _capi.MODE_INFER, self.max_decoder_steps, memory_lengths=memory_lengths, training=self.training,
-            prenet_keep=masks["prenet"],
-            att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold, row_seeds=row_seeds)
+            memory, _capi.MODE_INFER, self.max_decoder_steps if fa is None else fa.size(1), memory_lengths=memory_lengths,
+            training=self.training, prenet_keep=masks["prenet"],
+            att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold, row_seeds=row_seeds,
+            forced_align=fa, forced_lengths=fl)
         n = int(n_steps.item())                      # the one host sync of the whole loop (model.py:443 syncs every step)
         self.mel_lengths = lengths
-        if n == self.max_decoder_steps and bool((lengths >= n).any()):
+        if fa is None and n == self.max_decoder_steps and bool((lengths >= n).any()):
             fired = torch.sigmoid(gate[:, n - 1]) > self.gate_threshold
             if not bool(fired.all()):
                 print("Warning! Reached max decoder steps")                                         # model.py:446
         dt = memory.dtype
         return (mel[:, :n].transpose(1, 2).to(dt), gate[:, :n].unsqueeze(-1).to(dt), align[:, :n].to(dt))
 
-    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None, row_seeds=None):
+    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None, row_seeds=None, forced=(None, None)):
         """The persistent decoder in chunks of chunk_steps steps.  Yields (t0, t1, finished, stream): frames [t0, t1) are
         the new ones that every row has produced and that no frame within `halo` steps of them can still change, i.e. all
         frames up to the steps run less `halo` while any row is live, and all of them once every 64-row slice has
-        stopped.  Before the last tuple, self.mel_lengths and the max-steps warning are set as by inference()."""
+        stopped.  Before the last tuple, self.mel_lengths and the max-steps warning are set as by inference().  forced:
+        the engine's (map, lengths) of a forced run, whose map decides the steps."""
         chunk_steps = int(chunk_steps)
         if chunk_steps < 1:
             raise ValueError("tacotron2_b200: chunk_steps must be >= 1 (got %d)" % chunk_steps)
         eng = self._t2_engine()
-        st = eng.decoder_stream(memory, self.max_decoder_steps, prenet_keep=current_masks()["prenet"],
-                                gate_threshold=self.gate_threshold, memory_lengths=memory_lengths, row_seeds=row_seeds)
+        fa, fl = forced
+        st = eng.decoder_stream(memory, self.max_decoder_steps if fa is None else fa.size(1),
+                                prenet_keep=current_masks()["prenet"], gate_threshold=self.gate_threshold,
+                                memory_lengths=memory_lengths, row_seeds=row_seeds, forced_align=fa, forced_lengths=fl)
         t0 = 0
         while True:
             live_steps, n, finished = st.run(chunk_steps)
             t1 = n if finished else max(t0, live_steps - halo)
             if finished:
                 self.mel_lengths = st.mel_lengths
-                if n == self.max_decoder_steps and bool((st.mel_lengths >= n).any()):     # as inference()
+                if fa is None and n == self.max_decoder_steps and bool((st.mel_lengths >= n).any()):   # as inference()
                     fired = torch.sigmoid(st.gate[:, n - 1]) > self.gate_threshold
                     if not bool(fired.all()):
                         print("Warning! Reached max decoder steps")                             # model.py:446
@@ -503,21 +521,23 @@ class Decoder(_EngineOwner, nn.Module):
                 return
             t0 = t1
 
-    def inference_stream(self, memory, chunk_steps=32, memory_lengths=None, seeds=None):
+    def inference_stream(self, memory, chunk_steps=32, memory_lengths=None, seeds=None, alignments=None,
+                         alignment_lengths=None):
         """inference() in chunks of ``chunk_steps`` decoder steps, as a generator: one item per chunk that produced
         frames, a dict with ``frames`` = (t0, t1) (the same for every row), ``mel_outputs`` (B, n_mel, t1-t0),
         ``gate_outputs`` (B, t1-t0, 1), ``alignments`` (B, t1-t0, T_enc), ``mel_lengths`` (B,) int32 on the device with -1
         for rows that are still live, and ``finished``.  A decoder frame is handed out as soon as every row has produced
         it; concatenated along time the items are bit-identical to inference() (same weights, memory, memory_lengths,
-        masks / seed / seeds).  Evaluation mode only: the resumable decoder applies no hidden-state dropout, which
-        inference() does in training mode."""
+        masks / seed / seeds / alignments).  Evaluation mode only: the resumable decoder applies no hidden-state dropout,
+        which inference() does in training mode."""
         if self.training:
             raise RuntimeError("tacotron2_b200: Decoder.inference_stream needs eval mode (in training mode inference() "
                                "applies the attention / decoder dropout, which the resumable decoder does not)")
         memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
         row_seeds = self._row_seeds(seeds, memory.size(0), self._t2_engine().device, "Decoder.inference_stream")
+        forced = self._forced(alignments, alignment_lengths, memory, self._t2_engine().device, "Decoder.inference_stream")
         dt = memory.dtype
-        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths, row_seeds):
+        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths, row_seeds, forced):
             yield dict(frames=(t0, t1), mel_outputs=st.mel[:, t0:t1].transpose(1, 2).to(dt),
                        gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
                        mel_lengths=st.mel_lengths.clone(), finished=finished)
@@ -654,7 +674,7 @@ class Tacotron2(_EngineOwner, nn.Module):
             outputs = [o.to(cast) for o in outputs]
         return self.parse_output(outputs, output_lengths)
 
-    def inference(self, inputs, input_lengths=None, seeds=None):
+    def inference(self, inputs, input_lengths=None, seeds=None, alignments=None, alignment_lengths=None):
         """model.py:517-529, batched.  For B > 1 frames at t >= mel_lengths[b] of mel_outputs and
         mel_outputs_postnet are zero (same convention as parse_output); ``self.mel_lengths`` holds
         the per-row lengths.  B == 1 is exactly the reference.
@@ -668,29 +688,41 @@ class Tacotron2(_EngineOwner, nn.Module):
         are taken as their 64-bit pattern); eval mode only, not together with injected prenet masks.  Row b then draws the
         prenet dropout that ``inference(inputs[b:b+1, :input_lengths[b]], seeds=[seeds[b]])`` draws, so it reproduces that
         call bit for bit in any batch, slice, stream or server slot.  A B = 1 call with seeds=[s] is the unseeded call
-        whose engine seed was s.  None: one seed per call (the next engine seed), as before."""
+        whose engine seed was s.  None: one seed per call (the next engine seed), as before.
+
+        alignments (B, T_map, T_text), alignment_lengths (B,): a forced run with the given attention weights, eval mode
+        only (README "timing control"; Decoder.inference has the contract).  Row b runs alignment_lengths[b] steps
+        (default T_map), mel_lengths = alignment_lengths, and every row's postnet is its own B = 1 postnet, so row b
+        equals ``inference(inputs[b:b+1, :L_b], alignments=alignments[b:b+1, :alignment_lengths[b], :L_b])`` bit for bit
+        (L_b = input_lengths[b]).  ``alignments_from_durations`` turns per-symbol frame counts into such a map."""
         lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
         eng = self._t2_engine()
         row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference")
+        fa, fl = _engine_mod.forced_alignment(alignments, alignment_lengths, inputs.size(0), inputs.size(1), eng.device,
+                                              self.training, "tacotron2_b200: Tacotron2.inference")
         memory = eng.encoder(text=inputs, lengths=lengths_in, training=self.training, keep=current_masks()["enc"],
                              per_row=lengths_in is not None)
         memory = memory.to(self._t2_out_dtype())     # a .half() model hands half tensors between its modules (ipynb:89-90)
-        mel_outputs, gate_outputs, alignments = self.decoder.inference(memory, memory_lengths=lengths_in, seeds=row_seeds)
+        mel_outputs, gate_outputs, alignments = self.decoder.inference(memory, memory_lengths=lengths_in, seeds=row_seeds,
+                                                                       alignments=fa, alignment_lengths=fl)
         lengths = self.decoder.mel_lengths
         self.mel_lengths = lengths
         mel_btc = mel_outputs.transpose(1, 2)
         if mel_btc.dtype != torch.float32:
             mel_btc = mel_btc.float().contiguous()
         multi = inputs.size(0) > 1
+        # a forced run knows its lengths before it runs: every row's postnet is its own, as for a ragged batch
         mel_outputs_postnet = eng.postnet(mel_btc, lengths if multi else None, True, self.training,
-                                          current_masks()["post"], per_row=_ragged(lengths_in, inputs.size(1))
+                                          current_masks()["post"],
+                                          per_row=_ragged(lengths_in, inputs.size(1)) or (fa is not None and multi)
                                           ).to(mel_outputs.dtype)
         if multi:
             pad = ~get_mask_from_lengths(lengths.long(), mel_outputs.size(2))
             mel_outputs = mel_outputs.masked_fill(pad.unsqueeze(1), 0.0)
         return self.parse_output([mel_outputs, mel_outputs_postnet, gate_outputs, alignments])
 
-    def inference_stream(self, inputs, chunk_steps=32, input_lengths=None, seeds=None):
+    def inference_stream(self, inputs, chunk_steps=32, input_lengths=None, seeds=None, alignments=None,
+                         alignment_lengths=None):
         """inference() as a generator that hands out frames while the decoder runs (README "streaming inference").
 
         The encoder runs once; the decoder runs in chunks of ``chunk_steps`` steps.  Each item is a dict describing frames
@@ -700,7 +732,8 @@ class Tacotron2(_EngineOwner, nn.Module):
         handed out once the decoder has run step t+10 or every row has stopped; it is never revised.  Concatenated along
         time the items are bit-identical to inference() with the same weights, inputs and dropout masks / seed.  After the
         last item ``self.mel_lengths`` and the max-steps warning are as after inference().  input_lengths: as for
-        inference(), whose output the items then concatenate to.  seeds: as for inference().  Evaluation mode only: in
+        inference(), whose output the items then concatenate to.  seeds, alignments, alignment_lengths: as for
+        inference().  Evaluation mode only: in
         training mode BatchNorm normalises over the whole sequence, so no frame is final before the last one."""
         if self.training:
             raise RuntimeError("tacotron2_b200: inference_stream needs eval mode (training-mode BatchNorm uses the statistics "
@@ -708,14 +741,16 @@ class Tacotron2(_EngineOwner, nn.Module):
         lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
         eng = self._t2_engine()
         row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference_stream")
+        forced = _engine_mod.forced_alignment(alignments, alignment_lengths, inputs.size(0), inputs.size(1), eng.device,
+                                              False, "tacotron2_b200: Tacotron2.inference_stream")
         memory = eng.encoder(text=inputs, lengths=lengths_in, training=False, keep=current_masks()["enc"],
                              per_row=lengths_in is not None)
         dt = self._t2_out_dtype()
         memory = memory.to(dt)
         multi = inputs.size(0) > 1
-        ragged = _ragged(lengths_in, inputs.size(1))
+        ragged = _ragged(lengths_in, inputs.size(1)) or (forced[0] is not None and multi)     # as inference()
         halo = POSTNET_HALO
-        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in, row_seeds):
+        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in, row_seeds, forced):
             if finished:
                 self.mel_lengths = st.mel_lengths
             lengths = st.mel_lengths
