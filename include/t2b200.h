@@ -201,6 +201,29 @@ typedef struct T2DecoderArgs {
 } T2DecoderArgs;
 size_t t2_decoder_workspace_bytes(const T2Model* m, int32_t B, int32_t T_enc, int32_t n_steps_cap);
 int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);
+/* Limits (INFER, persistent implementation): guards for free runs whose attention may jump, repeat or never reach the
+ * end of the text.
+ *   window_back, window_front: an attention window (ESPnet's use_att_constraint with backward / forward window).  Let
+ *     p_t(b) be the smallest j < memory_lengths[b] that maximises row b's weights of step t - 1 (0 at step 0, and at the
+ *     first step of a row put back by admit, whose weights are all zero).  At step t the energies of row b at
+ *     j < p_t - window_back and at j >= p_t + window_front get score_mask_value before the softmax, on top of the length
+ *     mask, so the weights outside [p_t - window_back, p_t + window_front) come out 0.  Everything else -- the location
+ *     term (from these weights), the context, both LSTMs, the gate and the dropout keys -- is the free run's.  p_t comes
+ *     from the previous weights, which a stream already saves, so streams and continuous batching need no extra state.
+ *     window_front = 0 (with window_back = 0): no window.  A window with both sides >= memory_lengths[b] masks nothing
+ *     and gives the unwindowed bits.
+ *   max_steps: (B) int32 on the device, or NULL: row b also stops after max_steps[b] steps (clamped into
+ *     [1, n_steps_cap] where read) if its gate has not fired before; mel_lengths[b] is then max_steps[b].  The loop ends
+ *     when every row has stopped, so n_steps_cap = the largest limit wastes no steps on rows that reached theirs.
+ * Row b then equals bit for bit its own B = 1 call with n_steps_cap = max_steps[b] and the same window.
+ * t2_decoder_run_limited with limits = NULL is t2_decoder_run.  T2_ERR_INVALID: limits with forced_align, mode TEACHER,
+ * a negative window side, or window_back != 0 without a window; T2_ERR_UNSUPPORTED: the stepwise implementation
+ * (requested, or chosen by AUTO for a T_enc the persistent kernel does not take).  t2_infer_host takes no limits. */
+typedef struct T2DecoderLimits {
+  int32_t window_back, window_front;
+  const int32_t* max_steps;
+} T2DecoderLimits;
+int    t2_decoder_run_limited(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* limits, void* stream);
 
 /* ---- Resumable decoder stream: the INFER loop of t2_decoder_run in chunks of steps -------------
  * The same persistent kernel stops after a number of steps and resumes exactly where it stopped, so
@@ -225,6 +248,9 @@ typedef struct T2DecoderStreamArgs {
   int32_t* status;
   const int32_t* row_step0;            /* (B) device or NULL: with dec.row_seeds, row b's step (the one its prenet keys
                                           use) at local step i of a run is row_step0[b] + i instead of the absolute step */
+  const T2DecoderLimits* limits;       /* NULL or the limits of t2_decoder_run_limited, read by begin, run and admit: the
+                                          window applies to every chunk; max_steps count absolute steps, so admit
+                                          refuses limits that carry them (T2_ERR_INVALID) */
 } T2DecoderStreamArgs;
 size_t t2_decoder_stream_state_bytes(const T2Model* m, int32_t B, int32_t T_enc);
 int    t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stream);
@@ -675,7 +701,8 @@ int t2_selftest_waveglow_state(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, int
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* After a T2_IMPL_PERSISTENT run with the same args / workspace: SM cycles spent per phase of the
  * persistent kernel, summed over steps, on three sample CTAs (out_host[3][24]; phase list in
- * decoder_persistent.cu).  Synchronises the device. */
+ * decoder_persistent.cu); all zero after a t2_decoder_run_limited run, whose kernel keeps no profile.
+ * Synchronises the device. */
 int t2_decoder_profile(const T2DecoderArgs* a, int64_t* out_host);
 /* number of kernels this library has launched since load (for bench.py's gpu_launches) */
 int64_t t2_kernel_launch_count(void);

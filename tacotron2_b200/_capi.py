@@ -17,7 +17,7 @@ MODE_INFER, MODE_TEACHER = 0, 1
 EXPORTS = [
     "t2_abi_version", "t2_last_error", "t2_device_info", "t2_model_create", "t2_model_refresh",
     "t2_model_destroy", "t2_encoder_workspace_bytes", "t2_encoder_forward",
-    "t2_decoder_workspace_bytes", "t2_decoder_run", "t2_prenet_forward",
+    "t2_decoder_workspace_bytes", "t2_decoder_run", "t2_decoder_run_limited", "t2_prenet_forward",
     "t2_postnet_workspace_bytes", "t2_postnet_forward", "t2_infer_workspace_bytes", "t2_infer_host",
     "t2_encoder_infer", "t2_postnet_infer", "t2_infer_lengths_workspace_bytes", "t2_infer_host_lengths",
     "t2_kernel_launch_count", "t2_decoder_profile",
@@ -86,9 +86,13 @@ class T2DecoderArgs(C.Structure):
                 ("forced_align", C.c_void_p), ("forced_lengths", C.c_void_p)]
 
 
+class T2DecoderLimits(C.Structure):
+    _fields_ = [("window_back", C.c_int32), ("window_front", C.c_int32), ("max_steps", C.c_void_p)]
+
+
 class T2DecoderStreamArgs(C.Structure):
     _fields_ = [("dec", T2DecoderArgs), ("state", C.c_void_p), ("state_bytes", C.c_size_t), ("status", C.c_void_p),
-                ("row_step0", C.c_void_p)]
+                ("row_step0", C.c_void_p), ("limits", C.POINTER(T2DecoderLimits))]
 
 
 class T2CollectRow(C.Structure):
@@ -249,6 +253,7 @@ def lib():
     L.t2_encoder_forward.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_encoder_infer.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_decoder_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderArgs), C.c_void_p]
+    L.t2_decoder_run_limited.argtypes = [C.c_void_p, C.POINTER(T2DecoderArgs), C.POINTER(T2DecoderLimits), C.c_void_p]
     L.t2_decoder_stream_state_bytes.restype = C.c_size_t
     L.t2_decoder_stream_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.t2_decoder_stream_begin.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_void_p]

@@ -168,6 +168,55 @@ def forced_alignment(alignments, alignment_lengths, B, T_text, device, training,
     return alignments.to(dtype=torch.float32).contiguous(), lengths
 
 
+def _integral(v):
+    return isinstance(v, numbers.Integral) and not isinstance(v, bool)
+
+
+def decoder_limits(attention_window, max_decoder_steps, B, device, forced, what):
+    """The limits of a free run as the engine takes them: (window, caps, longest) -- window None or (back, front) ints,
+    caps None or (B,) int32 contiguous on `device`, longest None or max(caps) (the run's n_steps_cap).
+    attention_window: None or two integers (back >= 0, front >= 1); max_decoder_steps: None, one integer or B integers
+    >= 1 (a list, a host or a device tensor).  forced: a forced alignment is given, which takes neither.  Raises
+    TypeError / ValueError naming the argument before anything runs."""
+    if forced and attention_window is not None:
+        raise ValueError("%s: attention_window and alignments exclude each other (a forced run computes no energies)" % what)
+    if forced and max_decoder_steps is not None:
+        raise ValueError("%s: max_decoder_steps and alignments exclude each other (the map decides the steps)" % what)
+    window = None
+    if attention_window is not None:
+        w = attention_window.tolist() if torch.is_tensor(attention_window) else attention_window
+        if not isinstance(w, (tuple, list)) or len(w) != 2 or not all(_integral(v) for v in w):
+            raise TypeError("%s: attention_window must be two integers (back, front) (got %r)" % (what, attention_window))
+        back, front = int(w[0]), int(w[1])
+        if back < 0 or front < 1:
+            raise ValueError("%s: attention_window needs back >= 0 and front >= 1 (got (%d, %d))" % (what, back, front))
+        window = (min(back, 2 ** 31 - 1), min(front, 2 ** 31 - 1))
+    if max_decoder_steps is None:
+        return window, None, None
+    if _integral(max_decoder_steps):
+        host = torch.full((B,), int(max_decoder_steps), dtype=torch.int64)
+    else:
+        caps = max_decoder_steps if torch.is_tensor(max_decoder_steps) else torch.as_tensor(max_decoder_steps)
+        if caps.dtype.is_floating_point or caps.dtype.is_complex or caps.dtype == torch.bool:
+            raise TypeError("%s: max_decoder_steps must hold integers (got %s)" % (what, caps.dtype))
+        if tuple(caps.shape) != (B,):
+            raise ValueError("%s: max_decoder_steps must be one integer or have shape (%d,) (got %s)"
+                             % (what, B, tuple(caps.shape)))
+        host = caps.cpu().to(torch.int64)
+    lo, hi = int(host.min()), int(host.max())
+    if lo < 1 or hi > 2 ** 31 - 1:
+        raise ValueError("%s: max_decoder_steps must lie in 1..2**31-1 (got %d..%d)" % (what, lo, hi))
+    return window, host.to(device=device, dtype=torch.int32).contiguous(), hi
+
+
+def limits_struct(window, caps):
+    """T2DecoderLimits of (window, caps) as decoder_limits() returns them; None when both are None."""
+    if window is None and caps is None:
+        return None
+    back, front = window if window is not None else (0, 0)
+    return _capi.T2DecoderLimits(back, front, _ptr(caps))
+
+
 def alignments_from_durations(durations):
     """Durations (B, T_text) of non-negative integer frame counts -> (alignments, alignment_lengths) for a forced
     ``Tacotron2.inference``: a one-hot map (B, T_map, T_text) fp32 in which symbol j of row b is attended for
@@ -382,10 +431,12 @@ class Engine(_Handle):
     def decoder(self, memory, mode, n_steps_cap, memory_lengths=None, teacher_prenet=None, training=False,
                 prenet_keep=None, att_keep=None, dec_keep=None, gate_threshold=0.5,
                 score_mask_value=-float("inf"), impl=None, stash=None, seed=None, row_seeds=None, forced_align=None,
-                forced_lengths=None):
+                forced_lengths=None, window=None, max_steps=None):
         """row_seeds: None or (B,) int64 on the device (see row_seeds()): per-row prenet keys.  forced_align /
         forced_lengths: None, or the given attention weights (B, n_steps_cap, T_enc) fp32 and each row's step count (B,)
-        int32, both contiguous on the device (see forced_alignment())."""
+        int32, both contiguous on the device (see forced_alignment()).  window / max_steps: None, or the attention window
+        (back, front) and each row's step limit (B,) int32 on the device (see decoder_limits()); either one runs
+        t2_decoder_run_limited."""
         L = _capi.lib()
         memory = memory.to(device=self.device, dtype=torch.float32).contiguous()
         B, T = int(memory.shape[0]), int(memory.shape[1])
@@ -409,17 +460,22 @@ class Engine(_Handle):
                                 n_steps.data_ptr(), ws.data_ptr(), ws.numel(),
                                 _ptr(stash), 0 if stash is None else stash.numel(), _ptr(row_seeds),
                                 _ptr(forced_align), _ptr(forced_lengths))
-        self._call(L.t2_decoder_run, C.byref(a))
+        lim = limits_struct(window, max_steps)
+        if lim is None:
+            self._call(L.t2_decoder_run, C.byref(a))
+        else:
+            self._call(L.t2_decoder_run_limited, C.byref(a), C.byref(lim))
         self._last_decoder_args = (a, memory, len32, teacher_prenet, pk, ak, dk, ws, mel, gate, align, mel_lengths, n_steps,
-                                   row_seeds, forced_align, forced_lengths)
+                                   row_seeds, forced_align, forced_lengths, max_steps)
         return mel, gate, align, mel_lengths, n_steps
 
     def decoder_stream(self, memory, n_steps_cap, prenet_keep=None, gate_threshold=0.5, score_mask_value=-float("inf"),
-                       impl=None, seed=None, memory_lengths=None, row_seeds=None, forced_align=None, forced_lengths=None):
+                       impl=None, seed=None, memory_lengths=None, row_seeds=None, forced_align=None, forced_lengths=None,
+                       window=None, max_steps=None):
         """Begins a resumable INFER run of the persistent decoder (t2_decoder_stream_begin); see DecoderStream."""
         return DecoderStream(self, memory, n_steps_cap, prenet_keep, gate_threshold, score_mask_value,
                              self.impl if impl is None else impl, next_seed() if seed is None else seed, memory_lengths,
-                             row_seeds, forced_align, forced_lengths)
+                             row_seeds, forced_align, forced_lengths, window, max_steps)
 
     def decoder_profile(self):
         """Per-phase SM cycles of the last persistent decoder run: dict phase -> [cta0, cta60, cta100]."""
@@ -552,7 +608,7 @@ class DecoderStream:
     their rows in place between chunks."""
 
     def __init__(self, eng, memory, cap, prenet_keep, gate_threshold, score_mask_value, impl, seed, memory_lengths=None,
-                 row_seeds=None, forced_align=None, forced_lengths=None):
+                 row_seeds=None, forced_align=None, forced_lengths=None, window=None, max_steps=None):
         L = _capi.lib()
         dev = eng.device
         self.eng = eng
@@ -578,7 +634,10 @@ class DecoderStream:
                                 self.mel.data_ptr(), self.gate.data_ptr(), self.align.data_ptr(),
                                 self.mel_lengths.data_ptr(), self.n_steps.data_ptr(), row_seeds=_ptr(row_seeds),
                                 forced_align=_ptr(forced_align), forced_lengths=_ptr(forced_lengths))
+        self.limits = (limits_struct(window, max_steps), max_steps)      # every call reads them
         self.args = _capi.T2DecoderStreamArgs(d, self.state.data_ptr(), self.state.numel(), self.status.data_ptr())
+        if self.limits[0] is not None:
+            self.args.limits = C.pointer(self.limits[0])
         eng._call(L.t2_decoder_stream_begin, C.byref(self.args))
 
     def run(self, n):

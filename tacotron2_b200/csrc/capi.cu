@@ -143,6 +143,18 @@ static int check_forced(const T2DecoderArgs* a, const char* what) {
   return T2_OK;
 }
 
+// limits: evaluation- or training-mode INFER without a forced alignment, and a window of non-negative sides
+static int check_limits(const T2DecoderArgs* a, const T2DecoderLimits* lim, const char* what) {
+  if (!lim) return T2_OK;
+  if (a->forced_align) return fail(T2_ERR_INVALID, "%s: limits and forced_align exclude each other (the map decides the steps)", what);
+  if (a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "%s: limits need mode INFER (got %d)", what, a->mode);
+  if (lim->window_back < 0 || lim->window_front < 0)
+    return fail(T2_ERR_INVALID, "%s: attention window (%d, %d) has a negative side", what, lim->window_back, lim->window_front);
+  if (lim->window_front == 0 && lim->window_back != 0)
+    return fail(T2_ERR_INVALID, "%s: window_back = %d without a window (window_front = 0)", what, lim->window_back);
+  return T2_OK;
+}
+
 static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a) {
   if (!m || !a) return fail(T2_ERR_INVALID, "null model / args");
   if (a->B <= 0 || a->B > kMaxBatch) return fail(T2_ERR_INVALID, "decoder: B=%d outside [1, %d]", a->B, kMaxBatch);
@@ -264,18 +276,20 @@ int t2_postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, void* stream) {
 }
 
 size_t t2_decoder_workspace_bytes(const T2Model*, int32_t B, int32_t T_enc, int32_t cap) { return decoder_ws_bytes(B, T_enc, cap); }
-int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) {
+static int decoder_run(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, void* stream) {
   T2_TRY(check_decoder_args(m, a));
+  T2_TRY(check_limits(a, lim, "decoder"));
   int impl = a->impl;
   if (impl == T2_IMPL_AUTO) impl = persistent_supported(m, a) ? T2_IMPL_PERSISTENT : T2_IMPL_STEPWISE;
   if (impl == T2_IMPL_PERSISTENT) {
     if (!persistent_supported(m, a))
       return fail(T2_ERR_UNSUPPORTED, "persistent decoder does not support T_enc=%d on this device (at most 2274, and >= 128 SMs)",
                   a->T_enc);
-    return decoder_run_persistent(m, a, (cudaStream_t)stream);
+    return decoder_run_persistent(m, a, lim, (cudaStream_t)stream);
   }
-  if (a->forced_align)
-    return fail(T2_ERR_UNSUPPORTED, "decoder: a forced alignment needs the persistent implementation (%s)",
+  if (a->forced_align || lim)
+    return fail(T2_ERR_UNSUPPORTED, "decoder: %s needs the persistent implementation (%s)",
+                a->forced_align ? "a forced alignment" : "limits",
                 a->impl == T2_IMPL_STEPWISE ? "impl = STEPWISE was requested"
                                             : "this shape / device does not fit it: T_enc too large for shared memory or < 128 SMs");
   // only the persistent kernel writes the training stash: a backward pass over a stash the stepwise path left
@@ -285,6 +299,10 @@ int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) {
                 a->impl == T2_IMPL_STEPWISE ? "impl = STEPWISE was requested"
                                             : "this shape / device does not fit it: T_enc too large for shared memory or < 128 SMs");
   return decoder_run_stepwise(m, a, (cudaStream_t)stream);
+}
+int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) { return decoder_run(m, a, nullptr, stream); }
+int t2_decoder_run_limited(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* limits, void* stream) {
+  return decoder_run(m, a, limits, stream);
 }
 
 size_t t2_decoder_stream_state_bytes(const T2Model*, int32_t B, int32_t T_enc) {
@@ -310,6 +328,7 @@ static int check_stream_args(const T2Model* m, const T2DecoderStreamArgs* s) {
   if (s->state_bytes < persistent_stream_state_bytes(a->B, a->T_enc)) return fail(T2_ERR_WORKSPACE, "decoder stream state too small");
   if (s->row_step0 && !a->row_seeds) return fail(T2_ERR_INVALID, "decoder stream: row_step0 needs dec.row_seeds");
   T2_TRY(check_forced(a, "decoder stream"));
+  T2_TRY(check_limits(a, s->limits, "decoder stream"));
   return check_row_seeds(a, "decoder stream");
 }
 
@@ -321,7 +340,8 @@ int t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stre
 int t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n_steps, const int32_t* status_host, void* stream) {
   T2_TRY(check_stream_args(m, a));
   if (n_steps < 1) return fail(T2_ERR_INVALID, "decoder stream: n_steps=%d (at least 1 step per run)", n_steps);
-  return persistent_stream_run(m, &a->dec, a->state, a->status, n_steps, status_host, a->row_step0, (cudaStream_t)stream);
+  return persistent_stream_run(m, &a->dec, a->limits, a->state, a->status, n_steps, status_host, a->row_step0,
+                               (cudaStream_t)stream);
 }
 
 int t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int32_t* rows, int32_t n_rows, void* stream) {
@@ -329,6 +349,9 @@ int t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int3
   if (n_rows < 1 || n_rows > a->dec.B || !rows) return fail(T2_ERR_INVALID, "decoder stream admit: n_rows=%d outside [1, B=%d]", n_rows, a->dec.B);
   if (!a->dec.memory_lengths) return fail(T2_ERR_INVALID, "decoder stream admit: the stream has no memory_lengths");
   if (a->dec.forced_align) return fail(T2_ERR_INVALID, "decoder stream admit: continuous batching takes no forced alignment");
+  if (a->limits && a->limits->max_steps)
+    return fail(T2_ERR_INVALID, "decoder stream admit: limits.max_steps count the stream's absolute steps, which an admitted "
+                                "row does not share (continuous batching limits each request itself)");
   for (int i = 0; i < n_rows; ++i)
     if (rows[i] < 0 || rows[i] >= a->dec.B || (i > 0 && rows[i] <= rows[i - 1]))
       return fail(T2_ERR_INVALID, "decoder stream admit: rows must be ascending and inside [0, B=%d) (rows[%d]=%d)", a->dec.B, i, rows[i]);

@@ -387,6 +387,10 @@ struct KParams {
   // forced alignment (INFER, the kForced instantiation): rows b0.. of the given attention weights (Btot, cap, T) and
   // their step counts (Btot), clamped into [1, cap] where they are read
   const float* forced_align; const int32_t* forced_lengths;
+  // limits (INFER, the kLimited instantiation; win_front == 0: the other two): at step t row r attends only to
+  // [p - win_back, p + win_front), p = the first argmax of its previous weights below its length, and with max_steps
+  // (rows b0.. of (Btot), clamped into [1, cap] where they are read) it stops after max_steps[r] steps at the latest
+  int win_back, win_front; const int32_t* max_steps;
 };
 
 // encoder-memory rows of a T_enc-long row that the attention phase stages in an idle ring of `nstages` stages beside the
@@ -425,11 +429,15 @@ __device__ __forceinline__ void store_split2(uint8_t* img, int row, int k, float
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
-// kForced (INFER with p.forced_align): the attention weights of step t are row t of the given map instead of the softmax
-// of the energies, and row b stops after forced_lengths[b] steps instead of on its gate.  The location term, the energies
-// and the softmax are skipped; the events, barriers and the context routine are those of the free run.
-template <bool kForced>
+// kModeForced (INFER with p.forced_align): the attention weights of step t are row t of the given map instead of the
+// softmax of the energies, and row b stops after forced_lengths[b] steps instead of on its gate.  The location term, the
+// energies and the softmax are skipped; the events, barriers and the context routine are those of the free run.
+// kModeLimited (INFER with limits): the free run, with the energies outside the row's attention window masked before the
+// softmax and a stop latch that also fires at the row's own step limit.  Everything else is the free run's.
+enum : int { kModeFree = 0, kModeForced = 1, kModeLimited = 2 };
+template <int kMode>
 __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const KParams p) {
+  constexpr bool kForced = kMode == kModeForced, kLimited = kMode == kModeLimited;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x;
@@ -508,8 +516,9 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   const bool has_q = cta >= kQCta0 && cta < kQCta0 + kQCtas;
   const bool has_x2 = cta >= kX2Cta0 && cta < kX2Cta0 + kX2Ctas;
   const int halfk = (kLocK - 1) / 2;
-  // phase profile (cycles, accumulated over steps) on three sample CTAs; see t2_decoder_profile()
-  const int prof_slot = cta == 0 ? 0 : (cta == 60 ? 1 : (cta == 100 ? 2 : -1));
+  // phase profile (cycles, accumulated over steps) on three sample CTAs; see t2_decoder_profile().  The limited
+  // instantiation keeps none: its clock registers would push the window's argmax over 128 registers into spills.
+  const int prof_slot = kLimited ? -1 : cta == 0 ? 0 : (cta == 60 ? 1 : (cta == 100 ? 2 : -1));
   long long prof_last = clock64();
   if (tid < 24) s_prof[tid] = 0;
 #define T2_PROF(ph)                                                        \
@@ -831,9 +840,27 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       const int len = p.mem_len ? min(p.mem_len[b], T) : T;
       if constexpr (!kForced) {             // the softmax and the previous / cumulative weights
         const int eN = ntiles * 128;
+        // the attention window [wlo, whi) of this step: p_t is the first position of the largest previous weight below
+        // len (0 while they are all zero).  Every warp reduces it itself from the previous weights, which both CTAs of the
+        // pair hold identically and which the write-out below overwrites only after the barrier that follows the mask.
+        // The weights are >= +0.0 (softmax outputs, or the zeros of begin / admit), so their bit patterns order as their
+        // values: one integer max reduction, then one min reduction over the first position of each lane that holds it.
+        int wlo = 0, whi = len;
+        if constexpr (kLimited) {
+          unsigned bv = 0u;
+          for (int j = lane; j < len; j += 32) bv = max(bv, __float_as_uint(s_pad0[halfk + j]));
+          bv = __reduce_max_sync(0xffffffffu, bv);
+          unsigned bj = (unsigned)len;
+          for (int j = lane; j < len; j += 32)
+            if (__float_as_uint(s_pad0[halfk + j]) == bv) { bj = (unsigned)j; break; }
+          const int pt = (int)__reduce_min_sync(0xffffffffu, bj);
+          wlo = pt - p.win_back;
+          whi = min(len, pt + p.win_front);
+        }
         // masked energies once (the four 32-dim partial sums added in a fixed order), in place in the first partial-sum plane
         for (int j = tid; j < T; j += kThreads)
-          s_ep[j] = (j < len) ? (s_ep[j] + s_ep[eN + j]) + (s_ep[2 * eN + j] + s_ep[3 * eN + j]) : p.score_mask_value;
+          s_ep[j] = (kLimited ? (j >= wlo && j < whi) : j < len)
+                        ? (s_ep[j] + s_ep[eN + j]) + (s_ep[2 * eN + j] + s_ep[3 * eN + j]) : p.score_mask_value;
         __syncthreads();
         float mx = -INFINITY;
         for (int j = lane; j < T; j += 32) mx = fmaxf(mx, s_ep[j]);
@@ -959,9 +986,11 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
             p.gate[(long)row * p.cap + t] = v;                                 // model.py:378
             if (p.infer) {
               int done = ctrl->done[row];
-              // model.py:443; forced: the row's step count decides, its gate plays no part
+              // model.py:443; forced: the row's step count decides, its gate plays no part; limited: its gate or its own
+              // step limit, whichever comes first
               if (!done && (kForced ? t + 1 == min(max(p.forced_lengths[row], 1), p.cap)
-                                    : sigmoid_exact(v) > p.gate_threshold)) {
+                                    : (sigmoid_exact(v) > p.gate_threshold ||
+                                       (kLimited && p.max_steps && t + 1 == min(max(p.max_steps[row], 1), p.cap))))) {
                 done = 1; ctrl->done[row] = 1; p.mel_lengths[row] = t + 1;
               }
               if (!done) atomicAdd(s_live, 1);
@@ -1257,8 +1286,9 @@ static int processed_memory(T2Model* m, const T2DecoderArgs* a, int b0, int nb, 
 }
 
 // the parameters of the launch over batch rows [b0, b0 + 64) (or to B) whose state is block `blk` of `buf`: the whole loop
-// [0, cap), no resume state
-static void slice_params(T2Model* m, const T2DecoderArgs* a, const SliceBuffer& buf, const SliceState& blk, int b0, KParams* pp) {
+// [0, cap), no resume state; lim: the caller's limits or null
+static void slice_params(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, const SliceBuffer& buf,
+                         const SliceState& blk, int b0, KParams* pp) {
   PersistentPack* pk = (PersistentPack*)m->pk;
   KParams& p = *pp;
   const int T = a->T_enc, cap = a->n_steps_cap;
@@ -1284,6 +1314,13 @@ static void slice_params(T2Model* m, const T2DecoderArgs* a, const SliceBuffer& 
     p.forced_align = a->forced_align + (size_t)b0 * cap * T; p.forced_lengths = a->forced_lengths + b0;
     p.pa = nullptr;
   }
+  if (lim) {
+    // a window wider than T_enc on either side masks nothing, so no window (window_front == 0) and overly wide ones run
+    // as (T_enc, T_enc); this also keeps p + win_front inside int
+    p.win_back = lim->window_front == 0 || lim->window_back > T ? T : lim->window_back;
+    p.win_front = lim->window_front == 0 || lim->window_front > T ? T : lim->window_front;
+    p.max_steps = lim->max_steps ? lim->max_steps + b0 : nullptr;
+  }
 }
 
 // the longest T_enc that persistent_stages() runs with 4 stages (0 when none does); stages fall as T_enc grows
@@ -1301,7 +1338,9 @@ static int launch_persistent(KParams& p, cudaStream_t s) {
   p.nstages = persistent_stages(p.T);
   p.t4max = persistent_t4max();
   const size_t smem = persistent_smem_bytes(p.T, p.nstages);
-  void (*kernel)(KParams) = p.forced_align ? decoder_persistent_kernel<true> : decoder_persistent_kernel<false>;
+  void (*kernel)(KParams) = p.forced_align      ? decoder_persistent_kernel<kModeForced>
+                            : p.win_front > 0 ? decoder_persistent_kernel<kModeLimited>
+                                              : decoder_persistent_kernel<kModeFree>;
   T2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -1317,7 +1356,7 @@ static int launch_persistent(KParams& p, cudaStream_t s) {
   return T2_OK;
 }
 
-int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
+int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, cudaStream_t s) {
   const int cap = a->n_steps_cap;
   const bool infer = a->mode == T2_MODE_INFER;
   DecoderStash st;
@@ -1339,7 +1378,7 @@ int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
   // batch rows are independent: more than 64 rows run as consecutive launches of <= 64 rows on the one block
   for (int b0 = 0; b0 < a->B; b0 += kRows) {
     KParams p;
-    slice_params(m, a, buf, blk, b0, &p);
+    slice_params(m, a, lim, buf, blk, b0, &p);
     // counters, zero images and q (model.py:258-284): the block's regions before pa
     T2_CUDA(cudaMemsetAsync(blk.ctrl, 0, (uint8_t*)blk.pa - (uint8_t*)blk.ctrl, s));
     if (p.pa) T2_CUDA(cudaMemsetAsync(p.pa, 0, pa_buffer_floats(a->T_enc) * 4, s));   // zero attention weights -> pa = +0.0
@@ -1376,8 +1415,8 @@ int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int
   return processed_memory(m, a, 0, a->B, stream_state(state, a->B, a->T_enc).pm, s);
 }
 
-int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n,
-                          const int32_t* status_host, const int32_t* row_step0, cudaStream_t s) {
+int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, void* state, int32_t* status,
+                          int n, const int32_t* status_host, const int32_t* row_step0, cudaStream_t s) {
   const SliceBuffer buf = stream_state(state, a->B, a->T_enc);
   for (int b0 = 0, si = 0; b0 < a->B; b0 += kRows, ++si) {
     const int t0 = status_host ? status_host[2 * si] : 0;
@@ -1385,7 +1424,7 @@ int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32
     const SliceState blk = buf.block(si);
     T2_CUDA(cudaMemsetAsync(blk.ctrl, 0, sizeof(DecoderCtrl), s));   // everything else is zeroed by begin / admit
     KParams p;
-    slice_params(m, a, buf, blk, b0, &p);                            // pa: left by the previous chunk
+    slice_params(m, a, lim, buf, blk, b0, &p);                       // pa: left by the previous chunk
     p.t_begin = t0;
     p.t_end = n < a->n_steps_cap - t0 ? t0 + n : a->n_steps_cap;
     p.rs_acc = blk.acc; p.rs_cell = blk.cell; p.rs_att = blk.att; p.rs_done = blk.done; p.rs_status = status + 2 * si;

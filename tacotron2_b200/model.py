@@ -454,7 +454,28 @@ class Decoder(_EngineOwner, nn.Module):
         return _engine_mod.forced_alignment(alignments, alignment_lengths, memory.size(0), memory.size(1), device,
                                             self.training, "tacotron2_b200: " + what)
 
-    def inference(self, memory, memory_lengths=None, seeds=None, alignments=None, alignment_lengths=None):
+    def _limits(self, attention_window, max_decoder_steps, memory, device, forced, what):
+        """attention_window / max_decoder_steps (see inference) as the engine's (window, caps, longest)."""
+        return _engine_mod.decoder_limits(attention_window, max_decoder_steps, memory.size(0), device, forced,
+                                          "tacotron2_b200: " + what)
+
+    def _warn_max_steps(self, lengths, gate, n, caps):
+        """model.py:445-447 after a free run of n steps: the warning, once, if a row stopped at its step limit without its
+        gate firing at that step.  Without caps the limit is max_decoder_steps (the reference's B = 1 rule over the whole
+        batch); with caps (B,) it is each row's own, so row b warns as its own B = 1 call would."""
+        if caps is None:
+            if n != self.max_decoder_steps or not bool((lengths >= n).any()):
+                return
+            fired = torch.sigmoid(gate[:, n - 1]) > self.gate_threshold
+            if not bool(fired.all()):
+                print("Warning! Reached max decoder steps")                                         # model.py:446
+            return
+        fired = torch.sigmoid(gate.gather(1, caps.long()[:, None] - 1)[:, 0]) > self.gate_threshold
+        if bool(((lengths == caps) & ~fired).any()):
+            print("Warning! Reached max decoder steps")                                             # model.py:446
+
+    def inference(self, memory, memory_lengths=None, seeds=None, alignments=None, alignment_lengths=None,
+                  attention_window=None, max_decoder_steps=None):
         """Free-running pass (model.py:418-454), batched: per-row stop latch, see README "batched
         inference".  Returns mel (B, n_mel, T), gate (B, T, 1), alignments (B, T, T_enc); T = steps
         until every row has fired (or max_decoder_steps); ``self.mel_lengths`` holds per-row lengths.  In training mode
@@ -471,50 +492,61 @@ class Decoder(_EngineOwner, nn.Module):
         the weights as given; its gate is computed but stops nothing, and max_decoder_steps plays no part.  The returned
         alignments are the weights used (zero past memory_lengths[b] and past the row's steps); injected prenet masks
         are (T_map, 2, B, 256).  Row b equals its own B = 1 forced call bit for bit, and a seeded free run fed its own
-        alignments and mel_lengths comes out again bit for bit."""
+        alignments and mel_lengths comes out again bit for bit.
+
+        attention_window (back, front), integers with back >= 0 and front >= 1 (README "robust synthesis"; also in
+        training mode): at step t row b may only attend to [p - back, p + front) within its length, p being the first
+        position of its largest attention weight of step t - 1 (0 at step 0); the energies outside get score_mask_value
+        before the softmax, so those weights are exactly 0.  Everything else is the free run's.  max_decoder_steps: one
+        integer or B integers >= 1 (list, host or device tensor): row b stops at its first gate firing or after
+        max_decoder_steps[b] steps, whichever comes first, and the run ends when every row has stopped (injected masks are
+        (max of them, 2, B, 256)); None: self.max_decoder_steps for every row.  Row b equals bit for bit its own B = 1
+        call with self.max_decoder_steps = max_decoder_steps[b] and the same window.  Neither goes with alignments."""
         memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
         eng = self._t2_engine()
         row_seeds = self._row_seeds(seeds, memory.size(0), eng.device, "Decoder.inference")
         fa, fl = self._forced(alignments, alignment_lengths, memory, eng.device, "Decoder.inference")
+        window, caps, longest = self._limits(attention_window, max_decoder_steps, memory, eng.device, fa is not None,
+                                             "Decoder.inference")
         masks = current_masks()
         mel, gate, align, lengths, n_steps = eng.decoder(
-            memory, _capi.MODE_INFER, self.max_decoder_steps if fa is None else fa.size(1), memory_lengths=memory_lengths,
-            training=self.training, prenet_keep=masks["prenet"],
+            memory, _capi.MODE_INFER, fa.size(1) if fa is not None else (longest or self.max_decoder_steps),
+            memory_lengths=memory_lengths, training=self.training, prenet_keep=masks["prenet"],
             att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold, row_seeds=row_seeds,
-            forced_align=fa, forced_lengths=fl)
+            forced_align=fa, forced_lengths=fl, window=window, max_steps=caps)
         n = int(n_steps.item())                      # the one host sync of the whole loop (model.py:443 syncs every step)
         self.mel_lengths = lengths
-        if fa is None and n == self.max_decoder_steps and bool((lengths >= n).any()):
-            fired = torch.sigmoid(gate[:, n - 1]) > self.gate_threshold
-            if not bool(fired.all()):
-                print("Warning! Reached max decoder steps")                                         # model.py:446
+        if fa is None:
+            self._warn_max_steps(lengths, gate, n, caps)
         dt = memory.dtype
         return (mel[:, :n].transpose(1, 2).to(dt), gate[:, :n].unsqueeze(-1).to(dt), align[:, :n].to(dt))
 
-    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None, row_seeds=None, forced=(None, None)):
+    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None, row_seeds=None, forced=(None, None),
+                       limits=(None, None, None)):
         """The persistent decoder in chunks of chunk_steps steps.  Yields (t0, t1, finished, stream): frames [t0, t1) are
         the new ones that every row has produced and that no frame within `halo` steps of them can still change, i.e. all
         frames up to the steps run less `halo` while any row is live, and all of them once every 64-row slice has
         stopped.  Before the last tuple, self.mel_lengths and the max-steps warning are set as by inference().  forced:
-        the engine's (map, lengths) of a forced run, whose map decides the steps."""
+        the engine's (map, lengths) of a forced run, whose map decides the steps; limits: the engine's (window, caps,
+        longest) of a limited one."""
         chunk_steps = int(chunk_steps)
         if chunk_steps < 1:
             raise ValueError("tacotron2_b200: chunk_steps must be >= 1 (got %d)" % chunk_steps)
         eng = self._t2_engine()
         fa, fl = forced
-        st = eng.decoder_stream(memory, self.max_decoder_steps if fa is None else fa.size(1),
+        window, caps, longest = limits
+        st = eng.decoder_stream(memory, fa.size(1) if fa is not None else (longest or self.max_decoder_steps),
                                 prenet_keep=current_masks()["prenet"], gate_threshold=self.gate_threshold,
-                                memory_lengths=memory_lengths, row_seeds=row_seeds, forced_align=fa, forced_lengths=fl)
+                                memory_lengths=memory_lengths, row_seeds=row_seeds, forced_align=fa, forced_lengths=fl,
+                                window=window, max_steps=caps)
         t0 = 0
         while True:
             live_steps, n, finished = st.run(chunk_steps)
             t1 = n if finished else max(t0, live_steps - halo)
             if finished:
                 self.mel_lengths = st.mel_lengths
-                if fa is None and n == self.max_decoder_steps and bool((st.mel_lengths >= n).any()):   # as inference()
-                    fired = torch.sigmoid(st.gate[:, n - 1]) > self.gate_threshold
-                    if not bool(fired.all()):
-                        print("Warning! Reached max decoder steps")                             # model.py:446
+                if fa is None:                                                                  # as inference()
+                    self._warn_max_steps(st.mel_lengths, st.gate, n, caps)
             if t1 > t0 or finished:
                 yield t0, t1, finished, st
             if finished:
@@ -522,13 +554,13 @@ class Decoder(_EngineOwner, nn.Module):
             t0 = t1
 
     def inference_stream(self, memory, chunk_steps=32, memory_lengths=None, seeds=None, alignments=None,
-                         alignment_lengths=None):
+                         alignment_lengths=None, attention_window=None, max_decoder_steps=None):
         """inference() in chunks of ``chunk_steps`` decoder steps, as a generator: one item per chunk that produced
         frames, a dict with ``frames`` = (t0, t1) (the same for every row), ``mel_outputs`` (B, n_mel, t1-t0),
         ``gate_outputs`` (B, t1-t0, 1), ``alignments`` (B, t1-t0, T_enc), ``mel_lengths`` (B,) int32 on the device with -1
         for rows that are still live, and ``finished``.  A decoder frame is handed out as soon as every row has produced
         it; concatenated along time the items are bit-identical to inference() (same weights, memory, memory_lengths,
-        masks / seed / seeds / alignments).  Evaluation mode only: the resumable decoder applies no hidden-state dropout,
+        masks / seed / seeds / alignments / attention_window / max_decoder_steps).  Evaluation mode only: the resumable decoder applies no hidden-state dropout,
         which inference() does in training mode."""
         if self.training:
             raise RuntimeError("tacotron2_b200: Decoder.inference_stream needs eval mode (in training mode inference() "
@@ -536,8 +568,11 @@ class Decoder(_EngineOwner, nn.Module):
         memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
         row_seeds = self._row_seeds(seeds, memory.size(0), self._t2_engine().device, "Decoder.inference_stream")
         forced = self._forced(alignments, alignment_lengths, memory, self._t2_engine().device, "Decoder.inference_stream")
+        limits = self._limits(attention_window, max_decoder_steps, memory, self._t2_engine().device, forced[0] is not None,
+                              "Decoder.inference_stream")
         dt = memory.dtype
-        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths, row_seeds, forced):
+        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths, row_seeds, forced,
+                                                        limits):
             yield dict(frames=(t0, t1), mel_outputs=st.mel[:, t0:t1].transpose(1, 2).to(dt),
                        gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
                        mel_lengths=st.mel_lengths.clone(), finished=finished)
@@ -674,7 +709,8 @@ class Tacotron2(_EngineOwner, nn.Module):
             outputs = [o.to(cast) for o in outputs]
         return self.parse_output(outputs, output_lengths)
 
-    def inference(self, inputs, input_lengths=None, seeds=None, alignments=None, alignment_lengths=None):
+    def inference(self, inputs, input_lengths=None, seeds=None, alignments=None, alignment_lengths=None,
+                  attention_window=None, max_decoder_steps=None):
         """model.py:517-529, batched.  For B > 1 frames at t >= mel_lengths[b] of mel_outputs and
         mel_outputs_postnet are zero (same convention as parse_output); ``self.mel_lengths`` holds
         the per-row lengths.  B == 1 is exactly the reference.
@@ -694,17 +730,25 @@ class Tacotron2(_EngineOwner, nn.Module):
         only (README "timing control"; Decoder.inference has the contract).  Row b runs alignment_lengths[b] steps
         (default T_map), mel_lengths = alignment_lengths, and every row's postnet is its own B = 1 postnet, so row b
         equals ``inference(inputs[b:b+1, :L_b], alignments=alignments[b:b+1, :alignment_lengths[b], :L_b])`` bit for bit
-        (L_b = input_lengths[b]).  ``alignments_from_durations`` turns per-symbol frame counts into such a map."""
+        (L_b = input_lengths[b]).  ``alignments_from_durations`` turns per-symbol frame counts into such a map.
+
+        attention_window (back, front) and max_decoder_steps (one integer or B): guards for free runs on long or
+        out-of-domain text (README "robust synthesis"; Decoder.inference has the contract).  Row b then equals
+        ``inference(inputs[b:b+1, :L_b], attention_window=w)`` with ``decoder.max_decoder_steps = max_decoder_steps[b]``
+        bit for bit.  Neither goes with alignments."""
         lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
         eng = self._t2_engine()
         row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference")
         fa, fl = _engine_mod.forced_alignment(alignments, alignment_lengths, inputs.size(0), inputs.size(1), eng.device,
                                               self.training, "tacotron2_b200: Tacotron2.inference")
+        window, caps, _ = _engine_mod.decoder_limits(attention_window, max_decoder_steps, inputs.size(0), eng.device,
+                                                     fa is not None, "tacotron2_b200: Tacotron2.inference")
         memory = eng.encoder(text=inputs, lengths=lengths_in, training=self.training, keep=current_masks()["enc"],
                              per_row=lengths_in is not None)
         memory = memory.to(self._t2_out_dtype())     # a .half() model hands half tensors between its modules (ipynb:89-90)
         mel_outputs, gate_outputs, alignments = self.decoder.inference(memory, memory_lengths=lengths_in, seeds=row_seeds,
-                                                                       alignments=fa, alignment_lengths=fl)
+                                                                       alignments=fa, alignment_lengths=fl,
+                                                                       attention_window=window, max_decoder_steps=caps)
         lengths = self.decoder.mel_lengths
         self.mel_lengths = lengths
         mel_btc = mel_outputs.transpose(1, 2)
@@ -722,7 +766,7 @@ class Tacotron2(_EngineOwner, nn.Module):
         return self.parse_output([mel_outputs, mel_outputs_postnet, gate_outputs, alignments])
 
     def inference_stream(self, inputs, chunk_steps=32, input_lengths=None, seeds=None, alignments=None,
-                         alignment_lengths=None):
+                         alignment_lengths=None, attention_window=None, max_decoder_steps=None):
         """inference() as a generator that hands out frames while the decoder runs (README "streaming inference").
 
         The encoder runs once; the decoder runs in chunks of ``chunk_steps`` steps.  Each item is a dict describing frames
@@ -732,8 +776,8 @@ class Tacotron2(_EngineOwner, nn.Module):
         handed out once the decoder has run step t+10 or every row has stopped; it is never revised.  Concatenated along
         time the items are bit-identical to inference() with the same weights, inputs and dropout masks / seed.  After the
         last item ``self.mel_lengths`` and the max-steps warning are as after inference().  input_lengths: as for
-        inference(), whose output the items then concatenate to.  seeds, alignments, alignment_lengths: as for
-        inference().  Evaluation mode only: in
+        inference(), whose output the items then concatenate to.  seeds, alignments, alignment_lengths,
+        attention_window, max_decoder_steps: as for inference().  Evaluation mode only: in
         training mode BatchNorm normalises over the whole sequence, so no frame is final before the last one."""
         if self.training:
             raise RuntimeError("tacotron2_b200: inference_stream needs eval mode (training-mode BatchNorm uses the statistics "
@@ -743,6 +787,8 @@ class Tacotron2(_EngineOwner, nn.Module):
         row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference_stream")
         forced = _engine_mod.forced_alignment(alignments, alignment_lengths, inputs.size(0), inputs.size(1), eng.device,
                                               False, "tacotron2_b200: Tacotron2.inference_stream")
+        limits = _engine_mod.decoder_limits(attention_window, max_decoder_steps, inputs.size(0), eng.device,
+                                            forced[0] is not None, "tacotron2_b200: Tacotron2.inference_stream")
         memory = eng.encoder(text=inputs, lengths=lengths_in, training=False, keep=current_masks()["enc"],
                              per_row=lengths_in is not None)
         dt = self._t2_out_dtype()
@@ -750,7 +796,8 @@ class Tacotron2(_EngineOwner, nn.Module):
         multi = inputs.size(0) > 1
         ragged = _ragged(lengths_in, inputs.size(1)) or (forced[0] is not None and multi)     # as inference()
         halo = POSTNET_HALO
-        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in, row_seeds, forced):
+        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in, row_seeds, forced,
+                                                                limits):
             if finished:
                 self.mel_lengths = st.mel_lengths
             lengths = st.mel_lengths
@@ -774,7 +821,7 @@ class Tacotron2(_EngineOwner, nn.Module):
                        gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
                        mel_lengths=lengths.clone(), finished=finished)
 
-    def inference_server(self, slots=64, max_text_len=200, chunk_steps=32, seed=None):
+    def inference_server(self, slots=64, max_text_len=200, chunk_steps=32, seed=None, attention_window=None):
         """Continuous batching (README "serving a queue"): an ``InferenceServer`` that keeps ``slots`` decoder rows in
         flight and refills a row with the next queued text as soon as its request has stopped.
 
@@ -786,19 +833,27 @@ class Tacotron2(_EngineOwner, nn.Module):
         ``alignments`` (1, L, T_text), ``mel_length`` and ``hit_max_steps`` -- the names and shapes inference() returns for
         that text alone.  With injected prenet masks it equals that call bit for bit (serving.py).  Evaluation mode and the
         persistent decoder only, as inference_stream.  The server owns its decoder state: several servers, streams and
-        inference() calls can be alive on one model.  seed: the session's Philox seed (default: the next engine seed)."""
+        inference() calls can be alive on one model.  seed: the session's Philox seed (default: the next engine seed).
+        attention_window: (back, front) for every request of the server, as for inference(); a result then equals
+        ``inference(text[None], attention_window=attention_window)`` under its own limit."""
         from .serving import EngineBackend, InferenceServer
         if self.training:
             raise RuntimeError("tacotron2_b200: inference_server needs eval mode (training-mode BatchNorm uses the statistics "
                                "of the whole sequence, so no postnet frame is final before the decoder ends)")
+        window = _engine_mod.decoder_limits(attention_window, None, 1, torch.device("cpu"), False,
+                                            "tacotron2_b200: inference_server")[0]
         server = InferenceServer(None, slots, max_text_len, chunk_steps, self.decoder.max_decoder_steps)
-        server.backend = EngineBackend(self, server.slots, server.max_text_len, server.chunk_steps, seed)
+        server.backend = EngineBackend(self, server.slots, server.max_text_len, server.chunk_steps, seed, window)
         return server
 
-    def inference_many(self, texts, slots=64, max_text_len=None, chunk_steps=32, max_decoder_steps=None, seeds=None):
+    def inference_many(self, texts, slots=64, max_text_len=None, chunk_steps=32, max_decoder_steps=None, seeds=None,
+                       attention_window=None):
         """Every text of ``texts`` (1-D integer tensors) through an inference_server; returns the results in input order.
         max_text_len: default the longest text; max_decoder_steps: one limit for all, or one per text.  seeds: one per text
-        (as for inference()); result i then equals ``inference(texts[i][None], seeds=[seeds[i]])`` bit for bit."""
+        (as for inference()); result i then equals ``inference(texts[i][None], seeds=[seeds[i]])`` bit for bit.
+        attention_window: one window for every text (see inference_server)."""
+        window = _engine_mod.decoder_limits(attention_window, None, 1, torch.device("cpu"), False,
+                                            "tacotron2_b200: inference_many")[0]
         texts = list(texts)
         if not texts:
             return []
@@ -809,7 +864,8 @@ class Tacotron2(_EngineOwner, nn.Module):
         if seeds is not None:       # checked before anything runs; the server takes each as a Python int
             bits = _engine_mod.row_seeds(seeds, len(texts), torch.device("cpu"), "tacotron2_b200: inference_many")
             per_text = [int(v) & 0xFFFFFFFFFFFFFFFF for v in bits.tolist()]
-        server = self.inference_server(min(int(slots), len(texts)), max(1, max_text_len), chunk_steps)
+        server = self.inference_server(min(int(slots), len(texts)), max(1, max_text_len), chunk_steps,
+                                       attention_window=window)
         ids = [server.submit(t, limit, seed=sd) for t, limit, sd in zip(texts, limits, per_text)]
         results = {r["id"]: r for r in server.run()}
         return [results[i] for i in ids]

@@ -195,7 +195,9 @@ class EngineBackend:
     """The device side of an InferenceServer on one Tacotron2 (eval mode): the slots' encoder memory, one DecoderStream
     whose rows are the slots, each request's own output buffers, and the postnet of finished requests."""
 
-    def __init__(self, model, slots, max_text_len, chunk_steps, seed=None):
+    def __init__(self, model, slots, max_text_len, chunk_steps, seed=None, window=None):
+        """window: None or the (back, front) attention window of every request; it needs no state of its own, since the
+        kernel finds each slot's window from the attention weights that admit zeroes and the stream saves."""
         from ._engine import next_seed
         self.model = model
         eng = self.eng = model._t2_engine()
@@ -207,7 +209,7 @@ class EngineBackend:
         lengths = torch.ones(slots, device=dev, dtype=torch.int32)       # an idle slot attends to one zero position
         keep = torch.ones(chunk_steps + 1, 2, slots, 256, device=dev, dtype=torch.uint8)
         self.stream = eng.decoder_stream(memory, chunk_steps + 1, prenet_keep=keep,
-                                         gate_threshold=model.decoder.gate_threshold, memory_lengths=lengths)
+                                         gate_threshold=model.decoder.gate_threshold, memory_lengths=lengths, window=window)
         self.keep_ptr = self.stream.args.dec.prenet_keep
         # a seeded session's per-slot seeds (64-bit patterns) and request step counts, rewritten before every chunk
         self.row_seeds = torch.zeros(slots, device=dev, dtype=torch.int64)
