@@ -485,7 +485,7 @@ class Engine(_Handle):
         names = ["E0 x2->att gemm", "E0 epilogue(ah)", "B1", "E1 ah->dec/att/q gemm", "B2", "attention", "B3",
                  "E2 ctx gemm", "E2 epilogue(dh)", "B4", "E3 dh gemm", "E3 epilogue(mel/x1)", "B5", "E4 x1 gemm+epi", "B6",
                  "att:before B2 (pa copy or round 0)", "att:pa rounds 1+ or tile wait", "att:energies", "att:softmax",
-                 "att:context", "att:next step's pa (in B6)"]
+                 "att:context", "att:next step's pa (in B6)", "Ed deferred ah->att' gemm (lower CTAs)"]
         return {names[i]: [int(out[s * 24 + i]) for s in range(3)] for i in range(len(names))}
 
     def grad_table(self, named_grads):

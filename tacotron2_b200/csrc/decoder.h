@@ -20,6 +20,7 @@ struct DecoderCtrl {
   unsigned int x2_count; int pad4_[31];    // arrivals of the prenet-2 CTAs: x2 of step t + 1 written
   unsigned int ah_count[16]; int pad5_[16];   // per 64-column chunk of ah: arrivals of its 8 producer CTAs (8 per step)
   unsigned int dh_count[16]; int pad6_[16];   // the same for dh
+  unsigned int q_count; int pad7_[31];     // arrivals of the query CTAs: q of step t written
 };
 
 constexpr size_t kDecoderWsAlign = 1024;   // base alignment of a decoder workspace (the persistent slice block)

@@ -8,7 +8,9 @@
 //     every CTA streams it ONCE through a shared-memory ring (bulk async copies on the TMA engine)
 //     together with the slices of every weight matrix that consumes it, and three warpgroups issue wgmma:
 //        x2_t  -> att gates += W_ih^a[:, :256] x2                          -> ah_t, ac_t
-//        ah_t  -> dec gates += W_ih^d[:, :1024] ah ; att gates(t+1) += W_hh^a ah ; q = W_q ah
+//        ah_t  -> dec gates += W_ih^d[:, :1024] ah ; q = W_q ah
+//        ah_t  -> att gates(t+1) += W_hh^a ah   (Ed: CTA c < 64 streams it for itself and for CTA c + 64 during the
+//                                                attention, which CTA c + 64 runs)
 //        ctx_t -> dec gates += W_ih^d[:, 1024:] ctx ; att gates(t+1) += W_ih^a[:, 256:] ctx ;
 //                 proj += W_P[:, 1024:] ctx                                 -> dh_t, dc_t
 //        dh_t  -> proj += W_P[:, :1024] dh ; dec gates(t+1) += W_hh^d dh   -> mel_t, gate_t, x1
@@ -27,8 +29,8 @@
 //     epilogue that consumed them.
 //   * location-sensitive attention (model.py:43-86): location conv + dense are fused into one 62-tap
 //     filter bank evaluated as a tensor-core GEMM over an im2col image of the previous / cumulative
-//     weights (kept in shared memory across steps); energies, softmax and context per batch row on a
-//     CTA pair with warp-shuffle reductions.
+//     weights (kept in shared memory across steps); energies, softmax and context of batch row b on CTA b + 64
+//     with warp-shuffle reductions.
 //   * events are separated by a grid-wide barrier or by producer-scoped counters (monotonic global counters:
 //     fence.acq_rel + relaxed red to arrive, relaxed polls + one fence to wait).
 #include <stdlib.h>
@@ -53,9 +55,15 @@ constexpr int kAttRound = 64;                             // encoder positions p
 constexpr int kAttPlane = kAttRound * 128;                // one fp16 plane of the im2col image (64 positions x 64 taps)
 constexpr int kPaPitch = kAttRound + 4;                   // floats per attention dim of the pa tile
 constexpr int kPaBytes = kAtt * kPaPitch * 4;
-constexpr int kNumEvents = 5;         // x2, ah, ctx, dh, x1
+constexpr int kNumEvents = 6;         // x2, ah, ctx, dh, x1, deferred ah (Ed)
+constexpr int kEd = 5;
 constexpr int kPCols = 344;           // 80 mel + 1 gate + 256 x1 + 7 pad
 constexpr int kQCta0 = 0, kQCtas = 16, kX2Cta0 = 16, kX2Ctas = 32, kPCta0 = 48, kPCtas = 43;
+constexpr int kAttCta0 = 64;          // CTA kAttCta0 + b runs the attention of batch row b
+// Ed waits for the query counter (true) or starts right after E1, with its first weight chunks prefetched by E1 (false):
+// the query CTAs stream E1 without the deferred stream's HBM traffic, or Ed gets the longer window.  Both ran the decoder
+// step in 65.4-66.0 µs on an H100 at 700 W (DESIGN §6.1).
+constexpr bool kEdAfterQ = true;
 constexpr int kWeffBytes = kAtt * kChunkK * 2 * 2;        // fused location filter image (hi+lo) = 32 KiB
 
 struct CtaPlan {
@@ -121,13 +129,15 @@ __global__ void pack_rows_image_kernel(const float* __restrict__ W, int N, int K
   }
 }
 
-// one consumer of one event: for CTA blockIdx.y, chunk blockIdx.x: rows rows_tab[cta*32 + i] (-1 = zero
-// row) x 64 columns starting at kcol0 + chunk*64 go to rows [roff, roff+n) of the chunk's hi and lo planes
+// consumer cons + blockIdx.z of one event: for CTA blockIdx.y, chunk blockIdx.x: rows rows_tab[z*tab_stride + cta*32 + i]
+// (-1 = zero row) x 64 columns starting at kcol0 + chunk*64 go to rows [roff, roff+n) of the chunk's hi and lo planes
 // (each plane holds the rows of ALL consumers of the event, concatenated).
 __global__ void pack_consumer_kernel(const float* __restrict__ src, int ld, int kcol0,
-                                     const int32_t* __restrict__ rows_tab, const CtaPlan* __restrict__ plans,
+                                     const int32_t* __restrict__ rows_tab, int tab_stride, const CtaPlan* __restrict__ plans,
                                      int ev, int cons, uint8_t* __restrict__ wimg) {
   const int cta = blockIdx.y, chunk = blockIdx.x;
+  cons += blockIdx.z;
+  rows_tab += blockIdx.z * tab_stride;
   const EventPlan& ep = plans[cta].ev[ev];
   if (cons >= ep.ncons) return;
   const int n = ep.n[cons];
@@ -207,24 +217,6 @@ __device__ __forceinline__ void grid_barrier(DecoderCtrl* ctrl, unsigned int& ta
   if (threadIdx.x == 0) {
     arrive_release(&ctrl->bar_count);
     poll_acquire(&ctrl->bar_count, target, ctrl, 100);
-  }
-  __syncthreads();
-  ptx::fence_proxy_async();
-}
-
-// split-phase form of the flat barrier: arrive as soon as this CTA's contribution is written, do work that
-// does not depend on the other CTAs, then wait
-__device__ __forceinline__ void grid_arrive(DecoderCtrl* ctrl, unsigned int& target) {
-  ptx::fence_proxy_async();
-  __syncthreads();
-  target += gridDim.x;
-  if (threadIdx.x == 0) {
-    arrive_release(&ctrl->bar_count);
-  }
-}
-__device__ __forceinline__ void grid_wait(DecoderCtrl* ctrl, unsigned int target) {
-  if (threadIdx.x == 0) {
-    poll_acquire(&ctrl->bar_count, target, ctrl, 101);
   }
   __syncthreads();
   ptx::fence_proxy_async();
@@ -360,6 +352,7 @@ struct KParams {
   uint8_t* x2_img; uint8_t* ah_img; uint8_t* ctx_img; uint8_t* dh_img; uint8_t* x1_img;
   const uint8_t* teacher_x2_img;   // (cap, 4 chunks) or null
   float* q;                         // (64, 128) fp32
+  float* part;                      // (64 lower CTAs, 64, 32) fp32: W_hh^a . ah_t of CTA c + 64's units, from CTA c's Ed
   float* pa;                        // (64, 128, pa_pitch(T)) fp32 location term of the next step; null: computed in the
                                     // attention phase (TEACHER, or a tile that does not fit the ring)
   float* mel; float* gate; float* align; int32_t* mel_lengths; int32_t* n_steps;
@@ -381,7 +374,7 @@ struct KParams {
   // the processed memory stay in place.
   float* rs_acc;                    // (kG, kRows x kAccPitch) accumulator tiles: next-step partial products
   float* rs_cell;                   // (kG, 4 column groups, kRows) float4 {c_att[0], c_att[1], c_dec[0], c_dec[1]}
-  float* rs_att;                    // (kG, 2, padded TP) previous | cumulative attention weights
+  float* rs_att;                    // (64 attention CTAs, 2, padded TP) previous | cumulative attention weights
   int32_t* rs_done;                 // (kRows) stop latch
   int32_t* rs_status;               // out: [steps run, stopped]
   // forced alignment (INFER, the kForced instantiation): rows b0.. of the given attention weights (Btot, cap, T) and
@@ -393,10 +386,10 @@ struct KParams {
   int win_back, win_front; const int32_t* max_steps;
 };
 
-// encoder-memory rows of a T_enc-long row that the attention phase stages in an idle ring of `nstages` stages beside the
-// im2col image and one round's pa tile; the rest is read from L2.  The same on the host and the device: the context of a
-// row sums its positions in the grouping a launch sized for that row's own length stages (see the context below), also
-// where the ring holds a whole precomputed pa tile instead and fewer rows are physically staged.
+// The context's grouping of a T_enc-long row: the half rows (256 columns) of encoder memory that an idle ring of `nstages`
+// stages holds beside the im2col image and one round's pa tile.  The context of a row sums its positions split there, in
+// the grouping a launch sized for that row's own length uses (see the context below), wherever its rows actually live:
+// the attention CTA stages fewer whole rows and reads the rest from L2.
 __host__ __device__ constexpr int staged_rows(int T, int nstages) {
   return T < (nstages * kStageBytes - 2 * kAttPlane - kPaBytes) / (kEnc / 2 * 4)
              ? T : (nstages * kStageBytes - 2 * kAttPlane - kPaBytes) / (kEnc / 2 * 4);
@@ -488,9 +481,11 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   rg.pol_x = ptx::policy_evict_last();
   for (int i = tid; i < kAtt; i += kThreads) s_v[i] = p.w_v[i];
   if (tid < 8) s_bias_p[tid] = (cta >= kPCta0 && cta < kPCta0 + kPCtas) ? p.bias_p[(cta - kPCta0) * 8 + tid] : 0.f;
-  for (int i = tid; i < TP; i += kThreads) {                                        // model.py:274-277
-    s_pad0[i] = resume ? p.rs_att[((size_t)cta * 2 + 0) * tpp + i] : 0.f;
-    s_pad1[i] = resume ? p.rs_att[((size_t)cta * 2 + 1) * tpp + i] : 0.f;
+  // the previous / cumulative attention weights live on the attention CTAs kAttCta0.. (model.py:274-277)
+  const bool upper = cta >= kAttCta0;
+  for (int i = tid; i < TP; i += kThreads) {
+    s_pad0[i] = resume && upper ? p.rs_att[((size_t)(cta - kAttCta0) * 2 + 0) * tpp + i] : 0.f;
+    s_pad1[i] = resume && upper ? p.rs_att[((size_t)(cta - kAttCta0) * 2 + 1) * tpp + i] : 0.f;
   }
   const CtaPlan& plan = p.plans[cta];
   DecoderCtrl* ctrl = p.ctrl;
@@ -508,9 +503,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   const bool is_lo = quad >= 2;
   const bool erow = !is_lo && row < p.B;
   float c_att[2] = {0.f, 0.f}, c_dec[2] = {0.f, 0.f};  // cell states of units 8*cta + 2*cg + {0,1}
-  float4* rs_cell = resume ? reinterpret_cast<float4*>(p.rs_cell) + ((size_t)cta * 4 + cg) * kRows + row : nullptr;
+  // this thread's saved cell states (resume); recomputed where it is used, so that no pointer stays live across the loop
+  auto rs_cell = [&]() { return reinterpret_cast<float4*>(p.rs_cell) + ((size_t)cta * 4 + cg) * kRows + row; };
   if (resume && !is_lo) {
-    const float4 c = *rs_cell;
+    const float4 c = *rs_cell();
     c_att[0] = c.x; c_att[1] = c.y; c_dec[0] = c.z; c_dec[1] = c.w;
   }
   const bool has_q = cta >= kQCta0 && cta < kQCta0 + kQCtas;
@@ -625,42 +621,57 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         }
         s_mask[row] = bits;
       }
-      run_event(rg, plan.ev[1], p.ah_img, p.wimg, 16, s_acc, ctrl, nullptr,    // the attention phase reuses the ring as scratch
+      // the attention phase reuses the ring of an upper CTA as scratch; a lower one goes on with Ed
+      run_event(rg, plan.ev[1], p.ah_img, p.wimg, 16, s_acc, ctrl, upper || kEdAfterQ ? nullptr : &plan.ev[kEd],
                 ctrl->ah_count, 8u * (unsigned int)(t + 1 - p.t_begin));
-      if (has_q && cg == 0 && !is_lo) {
-        float g[8];
-        acc_take8(s_acc, row, kColS, 0, g);
-        if (erow) {
+      if (has_q) {
+        if (cg == 0 && !is_lo) {
+          float g[8];
+          acc_take8(s_acc, row, kColS, 0, g);
+          if (erow) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) p.q[row * kAtt + (cta - kQCta0) * 8 + j] = g[j];
+            for (int j = 0; j < 8; ++j) p.q[row * kAtt + (cta - kQCta0) * 8 + j] = g[j];
+          }
         }
+        signal_counter(&ctrl->q_count, 1u);                                  // B2: this CTA's 8 columns of q are written
       }
       T2_PROF(3);
     }
-    // ======== attention for batch row (cta mod 64) ============================ model.py:43-86, 358-365
-    // CTAs b and b+64 both evaluate row b's energies / softmax (no exchange needed, bit-identical); each
-    // produces one half of the context columns, the first writes the alignment row.  Everything that only
-    // needs THIS CTA's state (the pa tile, staging encoder memory rows) runs between the arrival at barrier B2 and the
-    // wait for it.
+    // ======== Ed: ah_t -> att gates(t+1) += W_hh^a ah of this CTA's units and of its partner's (CTA + 64) ========
+    // The lower CTAs stream it while the upper ones run the attention; E1 acquired every ah chunk.  The partner's sums go
+    // to p.part and are added to its tile after B3, ahead of E2, as the first term of those columns (they are zero before
+    // it), so the addition order is the one of a single event.  Every lower CTA runs it: its units exist at any B.
+    if (!upper) {
+      if (kEdAfterQ) {
+        wait_counter(&ctrl->q_count, (unsigned int)(kQCtas * (t + 1 - p.t_begin)), s_flag, ctrl, 105);
+        T2_PROF(4);
+      }
+      run_event(rg, plan.ev[kEd], p.ah_img, p.wimg, 16, s_acc, ctrl, &plan.ev[2], nullptr, 0,
+                p.part + (size_t)cta * kRows * 32);
+      T2_PROF(21);
+    }
+    // ======== attention for batch row b = cta - kAttCta0 ======================= model.py:43-86, 358-365
+    // CTA b+64 evaluates row b's energies, softmax, alignment row and all 512 context columns; CTA b keeps its ring for
+    // the deferred event Ed below.  Everything that only needs THIS CTA's state (the pa tile, staging encoder memory
+    // rows) runs between the arrival at barrier B2 and the wait for it.
     // The location term pa of step t depends only on the attention weights of step t-1.  With p.pa (INFER, tile fits the
-    // ring) CTA b+64 computes it for row b during the x2 wait of step t-1, when its ring is idle, and both CTAs of the pair
-    // bulk-copy the whole tile before B2; after B2 the energies are one pass over all positions.  Otherwise (TEACHER: no
-    // x2 wait, the ring holds the prefetched E0 weights; or a T_enc whose tile does not fit) pa is computed here, 64
-    // positions per round, round 0 before the B2 wait.
-    const bool att_cta = (cta & 63) < p.B;
-    const int att_b = cta & 63, ahalf = cta >> 6;
+    // ring) the attention CTA computes it during the x2 wait of step t-1, when its ring is idle, and bulk-copies the whole
+    // tile before B2; after B2 the energies are one pass over all positions.  Otherwise (TEACHER: no x2 wait, the ring
+    // holds the prefetched E0 weights; or a T_enc whose tile does not fit) pa is computed here, 64 positions per round,
+    // round 0 before the B2 wait.
+    const bool att_cta = upper && cta - kAttCta0 < p.B;
+    const int att_b = cta & 63;
     const bool pa_pre = !kForced && p.pa != nullptr;
     const int pa_p = pa_pitch(T);
     float* pa_row = pa_pre ? p.pa + (size_t)att_b * kAtt * pa_p : nullptr;
     uint8_t* aimg = rg.stage0;
     // the idle operand ring during the attention phase: [im2col image: hi plane | lo plane][pa tile of one round]
-    // [encoder-memory rows of this CTA], or with p.pa [pa tile of all positions][encoder-memory rows of this CTA]
+    // [encoder-memory rows], or with p.pa [pa tile of all positions][encoder-memory rows]
     const int att_rounds = (T + kAttRound - 1) / kAttRound;
     const int img_bytes = 2 * kAttPlane;
     float* s_pa = reinterpret_cast<float*>(aimg + img_bytes);                       // [128 dims][kPaPitch] fp32
     const int mem_off = pa_pre ? pa_tile_bytes(T) : img_bytes + kPaBytes;         // ring bytes before the memory rows
-    const int smem_rows = pa_pre ? min(T, (p.nstages * kStageBytes - mem_off) / (kEnc / 2 * 4))
-                                 : staged_rows(T, p.nstages);                       // memory rows staged in the ring
+    const int smem_rows = min(T, (p.nstages * kStageBytes - mem_off) / (kEnc * 4));   // memory rows staged in the ring
     // pa^T = Weff . A^T on the tensor cores (fused model.py:23-25), i.e. the fused filter bank is the M = 128 operand
     // (attention dim d; warpgroups 0 / 1 take dims 0-63 / 64-127) and kAttRound positions are the N dimension.  The
     // tile of round r0 goes to dst[dim * pitch + position - 64 r0] (positions below `bound`): in shared memory every warp
@@ -717,18 +728,17 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       }
       __syncthreads();
     };
-    auto stage_memory_rows = [&](int j0, int j1) {     // cp.async this CTA's half of memory rows [j0, j1) into the ring
+    auto stage_memory_rows = [&](int j0, int j1) {     // cp.async memory rows [j0, j1) into the ring
       const uint32_t sbase = ptx::smem_u32(rg.stage0) + (uint32_t)mem_off;
-      const float* msrc = p.memory + (long)att_b * T * kEnc + ahalf * (kEnc / 2);
-      for (int i = j0 * 64 + tid; i < j1 * 64; i += kThreads) {
-        const int j = i >> 6, c4 = i & 63;
+      const float* msrc = p.memory + (long)att_b * T * kEnc;
+      for (int i = j0 * (kEnc / 4) + tid; i < j1 * (kEnc / 4); i += kThreads) {
+        const int j = i >> 7, c4 = i & 127;
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sbase + (uint32_t)i * 16u),
                      "l"(msrc + (long)j * kEnc + c4 * 4)
                      : "memory");
       }
       asm volatile("cp.async.commit_group;" ::: "memory");
     };
-    grid_arrive(ctrl, bar_target);                                             // B2 (arrive): q written
     const int adim = quad * 32 + lane;     // this thread's attention dim
     float pm_next[8];                      // processed-memory values of the thread's next chunk of 8 positions (software pipeline)
     auto load_pm = [&](const float* pmr, int j0, int cnt) {
@@ -744,14 +754,14 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       for (int j = tid; j < T; j += kThreads) {
         const float a = (t < flen && j < len) ? __ldg(fa + j) : 0.f;
         s_e[j] = a;
-        if (ahalf == 0) p.align[((long)att_b * p.cap + t) * T + j] = a;
+        p.align[((long)att_b * p.cap + t) * T + j] = a;
       }
       stage_memory_rows(0, smem_rows);
     } else if (att_cta) {
       if (pa_pre) {
-        // CTA b+64 wrote this tile before it signalled its ah columns of this step, or in the launch of the previous
-        // chunk, or the buffer was zeroed before step 0 (the attention weights start at zero, so pa is +0.0); thread 0
-        // acquired every ah counter in E1.
+        // this CTA wrote the tile before it signalled its ah columns of this step (which fences it for the async
+        // proxy), or in the launch of the previous chunk, or the buffer was zeroed before step 0 (the attention weights
+        // start at zero, so pa is +0.0)
         if (tid == 0) {
           ptx::mbar_arrive_expect_tx(bar_pa, (uint32_t)pa_tile_bytes(T));
           ptx::bulk_g2s_hint(rg.stage0, pa_row, (uint32_t)pa_tile_bytes(T), bar_pa, rg.pol_w);
@@ -763,7 +773,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       load_pm(p.pm + (long)att_b * T * kAtt + adim, cg * 8, min(T, kAttRound));
     }
     T2_PROF(15);
-    grid_wait(ctrl, bar_target);                                               // B2 (wait): q complete
+    if (att_cta) wait_counter(&ctrl->q_count, (unsigned int)(kQCtas * (t + 1 - p.t_begin)), s_flag, ctrl, 104);   // B2
     T2_PROF(4);
     if (att_cta) {
       const int b = att_b;
@@ -841,8 +851,8 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
       if constexpr (!kForced) {             // the softmax and the previous / cumulative weights
         const int eN = ntiles * 128;
         // the attention window [wlo, whi) of this step: p_t is the first position of the largest previous weight below
-        // len (0 while they are all zero).  Every warp reduces it itself from the previous weights, which both CTAs of the
-        // pair hold identically and which the write-out below overwrites only after the barrier that follows the mask.
+        // len (0 while they are all zero).  Every warp reduces it itself from the previous weights, which the write-out
+        // below overwrites only after the barrier that follows the mask.
         // The weights are >= +0.0 (softmax outputs, or the zeros of begin / admit), so their bit patterns order as their
         // values: one integer max reduction, then one min reduction over the first position of each lane that holds it.
         int wlo = 0, whi = len;
@@ -874,7 +884,7 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
           s_e[j] = a;
           s_pad0[halfk + j] = a;                                                // becomes "previous"
           s_pad1[halfk + j] += a;                                               // model.py:365
-          if (ahalf == 0) p.align[((long)b * p.cap + t) * T + j] = a;
+          p.align[((long)b * p.cap + t) * T + j] = a;
         }
       }
       asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -885,44 +895,48 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         // INFER: clen = len and split = the rows a launch sized for T_enc = len stages, so the grouping is a function of
         // the row's own length, not of the launch's T_enc, and a row of a ragged batch gets the bits it gets alone
         // (positions >= len have weight 0 and are skipped).  Without lengths, len = T_enc and split = staged_rows(T_enc).
-        // TEACHER keeps the launch's grouping over all T_enc positions.  The grouping does not depend on where a row
-        // lives: rows [smem_rows, split) are read from L2 (the precomputed pa tile leaves fewer rows of the ring).
-        const int c4 = tid & 63, jg = tid >> 6;                   // 64 float4 = this CTA's 256 columns; 8 j-groups
+        // TEACHER keeps the launch's grouping over all T_enc positions.  `split` counts half rows of 256 columns, as the
+        // ring of a CTA pair that split the columns staged them, so the grouping is not where a row lives: the ring holds
+        // fewer of the whole 512-column rows, and rows [smem_rows, split) are read from L2.
+        const int c4 = tid & 63, jg = tid >> 6;                   // float4 c4 of both column halves; 8 j-groups
         const float4* ms = reinterpret_cast<const float4*>(rg.stage0 + mem_off);
-        const float* mp = p.memory + (long)b * T * kEnc + ahalf * (kEnc / 2) + c4 * 4;
+        const float* mp = p.memory + (long)b * T * kEnc + c4 * 4;
         const int clen = p.infer ? len : T;
-        const int split = p.infer ? staged_rows(len, len <= p.t4max ? 4 : 3) : smem_rows;   // >= smem_rows if clen > smem_rows
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int split = p.infer ? staged_rows(len, len <= p.t4max ? 4 : 3) : staged_rows(T, p.nstages);
+        float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0;     // columns 4 c4 + [0, 4) and 256 + 4 c4 + [0, 4)
+        auto fma4 = [](float4& acc, float a, const float4 m) {
+          acc.x = fmaf(a, m.x, acc.x); acc.y = fmaf(a, m.y, acc.y); acc.z = fmaf(a, m.z, acc.z); acc.w = fmaf(a, m.w, acc.w);
+        };
         int j = jg;
-#pragma unroll 4
+#pragma unroll 2
         for (; j < min(split, smem_rows); j += 8) {
-          const float4 m = ms[j * 64 + c4];
           const float a = s_e[j];
-          acc.x = fmaf(a, m.x, acc.x); acc.y = fmaf(a, m.y, acc.y); acc.z = fmaf(a, m.z, acc.z); acc.w = fmaf(a, m.w, acc.w);
+          fma4(acc0, a, ms[j * (kEnc / 4) + c4]);
+          fma4(acc1, a, ms[j * (kEnc / 4) + kEnc / 8 + c4]);
         }
-        for (; j < split; j += 8) {                               // staged for a launch of this length, not for this one
-          const float4 m = __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc));
+        for (; j < split; j += 8) {                               // not staged
           const float a = s_e[j];
-          acc.x = fmaf(a, m.x, acc.x); acc.y = fmaf(a, m.y, acc.y); acc.z = fmaf(a, m.z, acc.z); acc.w = fmaf(a, m.w, acc.w);
+          fma4(acc0, a, __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc)));
+          fma4(acc1, a, __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc + kEnc / 2)));
         }
-        for (j = split + jg; j < clen; j += 8) {                  // rows that did not fit in the ring
-          const float4 m = __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc));
+        for (j = split + jg; j < clen; j += 8) {
           const float a = s_e[j];
-          acc.x = fmaf(a, m.x, acc.x); acc.y = fmaf(a, m.y, acc.y); acc.z = fmaf(a, m.z, acc.z); acc.w = fmaf(a, m.w, acc.w);
+          fma4(acc0, a, __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc)));
+          fma4(acc1, a, __ldg(reinterpret_cast<const float4*>(mp + (long)j * kEnc + kEnc / 2)));
         }
         __syncthreads();                                          // everyone is done reading the staged rows
-        float* scr = reinterpret_cast<float*>(rg.stage0);         // [8][256] partial sums
-        *reinterpret_cast<float4*>(scr + jg * (kEnc / 2) + c4 * 4) = acc;
+        float* scr = reinterpret_cast<float*>(rg.stage0);         // [8][512] partial sums
+        *reinterpret_cast<float4*>(scr + jg * kEnc + c4 * 4) = acc0;
+        *reinterpret_cast<float4*>(scr + jg * kEnc + kEnc / 2 + c4 * 4) = acc1;
         __syncthreads();
-        if (tid < kEnc / 4) {
+        if (tid < kEnc / 2) {
           const int col = tid * 2;
           float v0 = 0.f, v1 = 0.f;
 #pragma unroll
-          for (int g = 0; g < 8; ++g) { v0 += scr[g * (kEnc / 2) + col]; v1 += scr[g * (kEnc / 2) + col + 1]; }
-          store_split2(p.ctx_img, b, ahalf * (kEnc / 2) + col, v0, v1);
+          for (int g = 0; g < 8; ++g) { v0 += scr[g * kEnc + col]; v1 += scr[g * kEnc + col + 1]; }
+          store_split2(p.ctx_img, b, col, v0, v1);
           if (p.st.ga)
-            *reinterpret_cast<float2*>(p.st.ctx + ((long)(t + 1) * p.Btot + p.b0 + b) * kEnc + ahalf * (kEnc / 2) + col) =
-                make_float2(v0, v1);
+            *reinterpret_cast<float2*>(p.st.ctx + ((long)(t + 1) * p.Btot + p.b0 + b) * kEnc + col) = make_float2(v0, v1);
         }
       }
       T2_PROF(19);
@@ -932,6 +946,14 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
     T2_PROF(6);
     // ======== E2: ctx_t -> dec gates (rest), next att gates, projection (part); epilogue -> dh_t
     {
+      // an upper CTA adds its partner's Ed sums (B3 ordered their stores) to its attention gate columns, while the
+      // producer warp already issues E2's copies; warpgroup 1 adds E2's sums to those columns after this named barrier
+      if (upper && warp > 0) {
+        const float* part = p.part + (size_t)(cta - kAttCta0) * kRows * 32;
+        for (int i = tid - 32; i < kRows * 32; i += kThreads - 32)
+          s_acc[(i >> 5) * kAccPitch + kColA + (i & 31)] += __ldcg(part + i);
+        asm volatile("bar.sync 1, %0;" ::"r"(kThreads - 32) : "memory");
+      }
       run_event(rg, plan.ev[2], p.ctx_img, p.wimg, 8, s_acc, ctrl, &plan.ev[3]);
       T2_PROF(7);
       float g[8];
@@ -1029,11 +1051,10 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
         signal_counter(&ctrl->x2_count, 1u + (stop ? kStopFlag : 0u));
       }
       T2_PROF(12);
-      // The upper CTA of an attention pair is idle until x2 arrives and its ring is empty (E3 armed no next event): it
-      // computes the location term of step t+1 from this step's attention weights, every round, into row b's block of
-      // p.pa.  A resumed chunk reads it from there.  Its ah signal of step t+1 orders these stores before both CTAs of the
-      // pair copy the tile.
-      if (!kForced && pa_pre && ahalf == 1 && att_cta && t + 1 < p.cap)
+      // The attention CTA is idle until x2 arrives and its ring is empty (E3 armed no next event): it computes the
+      // location term of step t+1 from this step's attention weights, every round, into row b's block of p.pa.  A resumed
+      // chunk reads it from there.  Its ah signal of step t+1 orders these stores before it copies the tile.
+      if (!kForced && pa_pre && att_cta && t + 1 < p.cap)
         for (int r0 = 0; r0 < att_rounds; ++r0)
           att_pa_round(r0, pa_row + r0 * kAttRound, pa_p, min(T - r0 * kAttRound, kAttRound));
       T2_PROF(20);
@@ -1047,10 +1068,12 @@ __global__ void __launch_bounds__(kThreads, 1) decoder_persistent_kernel(const K
   if (resume) {    // every step ended with a wait that closes with __syncthreads: the shared-memory state is complete
     for (int i = tid; i < kRows * kAccPitch; i += kThreads) p.rs_acc[(size_t)cta * kRows * kAccPitch + i] = s_acc[i];
     for (int i = tid; i < TP; i += kThreads) {
-      p.rs_att[((size_t)cta * 2 + 0) * tpp + i] = s_pad0[i];
-      p.rs_att[((size_t)cta * 2 + 1) * tpp + i] = s_pad1[i];
+      if (upper) {
+        p.rs_att[((size_t)(cta - kAttCta0) * 2 + 0) * tpp + i] = s_pad0[i];
+        p.rs_att[((size_t)(cta - kAttCta0) * 2 + 1) * tpp + i] = s_pad1[i];
+      }
     }
-    if (!is_lo) *rs_cell = make_float4(c_att[0], c_att[1], c_dec[0], c_dec[1]);
+    if (!is_lo) *rs_cell() = make_float4(c_att[0], c_att[1], c_dec[0], c_dec[1]);
     if (gate_cta && tid < p.B) p.rs_done[tid] = ctrl->done[tid];
   }
   // rows that never fired: length = number of steps run (model.py:445-447)
@@ -1112,6 +1135,7 @@ struct SliceState {
   uint8_t *x2, *ah, *ctx, *dh, *x1;    // activation images of 4, 16, 8, 16 and 4 K chunks
   float* q;                            // (64, 128)
   float* pa;                           // location term of the next step (KParams::pa), pa_buffer_floats(T)
+  float* part;                         // KParams::part
   // saved on-chip state (KParams::rs_*; streams only)
   float* acc; float* cell; float* att; int32_t* done;
 };
@@ -1124,9 +1148,10 @@ __host__ __device__ static void slice_block_layout(Carve& c, int T, bool saved, 
   s->x1 = c.take<uint8_t>(4 * kXChunkBytes, kSliceAlign);
   s->q = c.take<float>((size_t)kRows * kAtt, kSliceAlign);
   s->pa = c.take<float>(pa_buffer_floats(T), kSliceAlign);
+  s->part = c.take<float>((size_t)kAttCta0 * kRows * 32, kSliceAlign);   // KParams::part, written and read within a step
   s->acc = saved ? c.take<float>((size_t)kG * kRows * kAccPitch, kSliceAlign) : nullptr;
   s->cell = saved ? c.take<float>((size_t)kG * 4 * kRows * 4, kSliceAlign) : nullptr;
-  s->att = saved ? c.take<float>((size_t)kG * 2 * att_pad_len(T), kSliceAlign) : nullptr;
+  s->att = saved ? c.take<float>((size_t)(kG - kAttCta0) * 2 * att_pad_len(T), kSliceAlign) : nullptr;
   s->done = saved ? c.take<int32_t>(kRows, kSliceAlign) : nullptr;
 }
 
@@ -1182,7 +1207,9 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
   PersistentPack* pk = (PersistentPack*)m->pk;
   if (!pk) { pk = new PersistentPack(); m->pk = pk; }
   const int kdc = kDRnn + kEnc;
-  // ---- per-CTA plans (host).  Consumers of an event are a contiguous run of [A | D | S] ----
+  // ---- per-CTA plans (host).  Consumers of an event are a contiguous run of [A | D | S].  E1 streams W_ih^d (D) on every
+  // CTA and W_q (S) on the query CTAs; W_hh^a (A) of CTAs c and c + 64 is Ed of CTA c < 64 (its second consumer: the
+  // partner's rows, stored to KParams::part) ----
   std::vector<CtaPlan> plans(kG);
   size_t off = 0;
   for (int c = 0; c < kG; ++c) {
@@ -1200,10 +1227,11 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
       off += (size_t)chunks * e.w_bytes;
     };
     set(0, 4, kColA, {32});
-    if (hq) set(1, 16, kColA, {32, 32, 16}); else set(1, 16, kColA, {32, 32});
+    if (hq) set(1, 16, kColD, {32, 16}); else set(1, 16, kColD, {32});
     if (hp) set(2, 8, kColA, {32, 32, 16}); else set(2, 8, kColA, {32, 32});
     if (hp) set(3, 16, kColD, {32, 16}); else set(3, 16, kColD, {32});
     if (hx) set(4, 4, kColS, {16}); else { pl.ev[4].w_off = (uint32_t)off; }
+    if (c < kAttCta0) set(kEd, 16, kColA, {32, 32}); else { pl.ev[kEd].w_off = (uint32_t)off; }
     for (int ev = 0; ev < kNumEvents; ++ev)
       if (pl.ev[ev].nrows != 0 && !event_plan_fits(pl.ev[ev])) return fail(T2_ERR_INVALID, "event plan does not fit the MMA warpgroups");
   }
@@ -1216,7 +1244,7 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
     T2_CUDA(cudaMalloc((void**)&pk->bias_p, (size_t)kPCols * 4));
     T2_CUDA(cudaMalloc((void**)&pk->bias_a, (size_t)kG * 32 * 4));
     T2_CUDA(cudaMalloc((void**)&pk->bias_d, (size_t)kG * 32 * 4));
-    T2_CUDA(cudaMalloc((void**)&pk->rows, (size_t)4 * kG * 32 * 4));
+    T2_CUDA(cudaMalloc((void**)&pk->rows, (size_t)5 * kG * 32 * 4));
     T2_CUDA(cudaMalloc((void**)&pk->weff, (size_t)kAtt * kChunkK * 4));
     T2_CUDA(cudaMalloc((void**)&pk->weff_img, (size_t)kWeffBytes));
   }
@@ -1238,10 +1266,13 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
   T2_LAUNCH_CHECK();
   pack_lstm_bias_kernel<<<(kG * 32 + 255) / 256, 256, 0, s>>>(m->drnn_b, pk->bias_d);
   T2_LAUNCH_CHECK();
-  // ---- row tables: [0] LSTM gate rows, [1] q rows, [2] P rows, [3] x2 rows (S consumers: 8 real + 8 zero) ----
-  std::vector<int32_t> rows((size_t)4 * kG * 32, -1);
+  // ---- row tables: [0] LSTM gate rows, [1] q rows, [2] P rows, [3] x2 rows (S consumers: 8 real + 8 zero), [4] LSTM
+  // gate rows of the partner CTA c + 64 (c < 64) ----
+  std::vector<int32_t> rows((size_t)5 * kG * 32, -1);
   for (int c = 0; c < kG; ++c) {
     for (int col = 0; col < 32; ++col) rows[(0 * kG + c) * 32 + col] = (col & 3) * 1024 + c * 8 + (col >> 2);
+    if (c < kAttCta0)
+      for (int col = 0; col < 32; ++col) rows[(4 * kG + c) * 32 + col] = (col & 3) * 1024 + (c + kAttCta0) * 8 + (col >> 2);
     if (c >= kQCta0 && c < kQCta0 + kQCtas) for (int j = 0; j < 8; ++j) rows[(1 * kG + c) * 32 + j] = (c - kQCta0) * 8 + j;
     if (c >= kPCta0 && c < kPCta0 + kPCtas) for (int j = 0; j < 8; ++j) rows[(2 * kG + c) * 32 + j] = (c - kPCta0) * 8 + j;
     if (c >= kX2Cta0 && c < kX2Cta0 + kX2Ctas) for (int j = 0; j < 8; ++j) rows[(3 * kG + c) * 32 + j] = (c - kX2Cta0) * 8 + j;
@@ -1250,15 +1281,19 @@ int persistent_pack_create(T2Model* m, cudaStream_t s) {
   T2_CUDA(cudaStreamSynchronize(s));
   const int32_t* r_lstm = pk->rows; const int32_t* r_q = pk->rows + kG * 32;
   const int32_t* r_p = pk->rows + 2 * kG * 32; const int32_t* r_x2 = pk->rows + 3 * kG * 32;
-  auto pack = [&](const float* src, int ld, int kcol0, int chunks, const int32_t* rt, int ev, int cons) -> int {
-    pack_consumer_kernel<<<dim3(chunks, kG), 256, 0, s>>>(src, ld, kcol0, rt, pk->plans, ev, cons, pk->wimg);
+  const int32_t* r_partner = pk->rows + 4 * kG * 32;
+  // consumers [cons, cons + ncons) of one matrix, consumer cons + z with row table rt + z * tab_stride
+  auto pack = [&](const float* src, int ld, int kcol0, int chunks, const int32_t* rt, int ev, int cons, int ncons = 1,
+                  int tab_stride = 0) -> int {
+    pack_consumer_kernel<<<dim3(chunks, kG, ncons), 256, 0, s>>>(src, ld, kcol0, rt, tab_stride, pk->plans, ev, cons, pk->wimg);
     T2_LAUNCH_CHECK();
     return T2_OK;
   };
   T2_TRY(pack(m->w[W_ARNN_WIH], kPre + kEnc, 0, 4, r_lstm, 0, 0));            // E0: att <- x2
-  T2_TRY(pack(m->w[W_ARNN_WHH], kARnn, 0, 16, r_lstm, 1, 0));                 // E1: att' <- ah
-  T2_TRY(pack(m->w[W_DRNN_WIH], kdc, 0, 16, r_lstm, 1, 1));                   //     dec <- ah
-  T2_TRY(pack(m->w[W_ATT_QUERY], kARnn, 0, 16, r_q, 1, 2));                   //     q <- ah
+  T2_TRY(pack(m->w[W_DRNN_WIH], kdc, 0, 16, r_lstm, 1, 0));                   // E1: dec <- ah
+  T2_TRY(pack(m->w[W_ATT_QUERY], kARnn, 0, 16, r_q, 1, 1));                   //     q <- ah
+  T2_TRY(pack(m->w[W_ARNN_WHH], kARnn, 0, 16, r_lstm, kEd, 0, 2,             // Ed: att' <- ah, partner's att' <- ah
+              (int)(r_partner - r_lstm)));
   T2_TRY(pack(m->w[W_ARNN_WIH], kPre + kEnc, kPre, 8, r_lstm, 2, 0));         // E2: att' <- ctx
   T2_TRY(pack(m->w[W_DRNN_WIH], kdc, kARnn, 8, r_lstm, 2, 1));                //     dec <- ctx
   T2_TRY(pack(pk->wp_all, kdc, kDRnn, 8, r_p, 2, 2));                         //     P <- ctx
@@ -1299,6 +1334,7 @@ static void slice_params(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimi
   p.mem_len = a->memory_lengths ? a->memory_lengths + b0 : nullptr;
   p.prenet_keep = a->prenet_keep; p.att_keep = a->att_keep; p.dec_keep = a->dec_keep;
   p.x2_img = blk.x2; p.ah_img = blk.ah; p.ctx_img = blk.ctx; p.dh_img = blk.dh; p.x1_img = blk.x1; p.q = blk.q;
+  p.part = blk.part;
   p.mel = a->mel + (size_t)b0 * cap * kMel; p.gate = a->gate + (size_t)b0 * cap; p.align = a->align + (size_t)b0 * cap * T;
   p.mel_lengths = a->mel_lengths + b0; p.n_steps = a->n_steps;
   p.ctrl = blk.ctrl;
@@ -1455,8 +1491,8 @@ __global__ void __launch_bounds__(256) stream_admit_kernel(void* state, int B, i
     sl.acc[((size_t)(i / kAccPitch) * kRows + lr) * kAccPitch + i % kAccPitch] = 0.f;
   for (int i = tid; i < kG * 4; i += 256)                          // its cell states: (CTA, column group)
     reinterpret_cast<float4*>(sl.cell)[(size_t)i * kRows + lr] = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int i = tid; i < 4 * tpp; i += 256)                         // previous | cumulative weights of CTAs lr and lr + 64
-    sl.att[(size_t)(lr + 64 * (i / (2 * tpp))) * 2 * tpp + i % (2 * tpp)] = 0.f;
+  for (int i = tid; i < 2 * tpp; i += 256)                         // previous | cumulative weights of its attention CTA
+    sl.att[(size_t)lr * 2 * tpp + i] = 0.f;
   const struct { uint8_t* img; int chunks; } imgs[5] = {{sl.x2, 4}, {sl.ah, 16}, {sl.ctx, 8}, {sl.dh, 16}, {sl.x1, 4}};
   for (const auto& im : imgs)
     for (int i = tid; i < im.chunks * 2 * (kChunkK / 2); i += 256) {   // its row in both planes of every chunk of an image

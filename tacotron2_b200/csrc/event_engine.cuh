@@ -146,27 +146,34 @@ __device__ __forceinline__ void event_mma(uint8_t* stage0, uint32_t stage_bytes,
 }
 
 // One MMA warpgroup's consumer of an event: D (64 x 2n) = X_hi . B^T + X_lo . B^T over all `chunks` stages of the ring
-// (event_mma); then both column halves of D are added to the accumulator tile from column acol.
+// (event_mma); then the sum of both column halves of D is added to the accumulator tile from column acol, or, with out,
+// stored to out (64 x n fp32, row-major) for another CTA to add to its tile.
 template <int N>
-__device__ __forceinline__ void event_wg(Ring& rg, int chunks, uint32_t w_row0, float* s_acc, int acol, DecoderCtrl* ctrl) {
+__device__ __forceinline__ void event_wg(Ring& rg, int chunks, uint32_t w_row0, float* s_acc, int acol, DecoderCtrl* ctrl,
+                                         float* out) {
   float d[1][N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) d[0][i] = 0.f;
   event_mma<N, 1>(rg.stage0, kStageBytes, kXChunkBytes, rg.ns, rg.full, rg.empty, rg.c_stage, rg.c_phase, chunks, w_row0, ctrl, d);
   const int wt = threadIdx.x & 127;
 #pragma unroll
-  for (int j = 0; j < N / 4; ++j)      // registers [0, N/4) hold the W_hi columns, [N/4, N/2) the W_lo ones
-    s_acc[ptx::wg_frag_row(j, wt) * kAccPitch + acol + ptx::wg_frag_col(j, wt)] += d[0][j] + d[0][N / 4 + j];
+  for (int j = 0; j < N / 4; ++j) {    // registers [0, N/4) hold the W_hi columns, [N/4, N/2) the W_lo ones
+    const float v = d[0][j] + d[0][N / 4 + j];
+    if (out) out[ptx::wg_frag_row(j, wt) * (N / 2) + ptx::wg_frag_col(j, wt)] = v;
+    else s_acc[ptx::wg_frag_row(j, wt) * kAccPitch + acol + ptx::wg_frag_col(j, wt)] += v;
+  }
 }
 
 // Streams `chunks` K-chunks of the activation image x_img plus this CTA's weight rows through the ring;
 // warpgroups 1-3 issue the MMAs (one consumer each) and add their products to the accumulator tile s_acc.  Called by all threads;
 // returns after the accumulators are complete.  Every MMA accumulates (the epilogues zero what they consume).
-// The plan's consumers have 32 or 16 rows (event_plan_fits).
+// The plan's consumers have 32 or 16 rows (event_plan_fits).  out_last (or null): the last consumer's sums go there
+// (event_wg) instead of into s_acc.
 __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const uint8_t* x_img,
                                           const uint8_t* w_img, int chunks, float* s_acc,
                                           DecoderCtrl* ctrl, const EventPlan* next,
-                                          const unsigned int* ready = nullptr, unsigned int ready_target = 0) {
+                                          const unsigned int* ready = nullptr, unsigned int ready_target = 0,
+                                          float* out_last = nullptr) {
   // ready (16 counters, one per K chunk of the activation; null = the caller synchronised already): chunk i of x_img is
   // complete once ready[i] >= ready_target.  The activation blocks ah / dh are written in 8-column slices by 128 CTAs, i.e.
   // a 64-column chunk has 8 producers: instead of a 128-way barrier between the epilogue that writes a block and the event
@@ -218,8 +225,9 @@ __device__ __forceinline__ void run_event(Ring& rg, const EventPlan& ep, const u
     if (c < ep.ncons) {
       int w_row0 = 0, acol = ep.col0;
       for (int i = 0; i < c; ++i) { w_row0 += 2 * ep.n[i]; acol += ep.n[i]; }
-      if (ep.n[c] == 32) event_wg<64>(rg, chunks, w_row0, s_acc, acol, ctrl);
-      else event_wg<32>(rg, chunks, w_row0, s_acc, acol, ctrl);
+      float* out = c == ep.ncons - 1 ? out_last : nullptr;
+      if (ep.n[c] == 32) event_wg<64>(rg, chunks, w_row0, s_acc, acol, ctrl, out);
+      else event_wg<32>(rg, chunks, w_row0, s_acc, acol, ctrl, out);
     } else {                              // no rows for this warpgroup: it still releases every stage it was counted for
       for (int i = 0; i < chunks; ++i) {
         mbar_wait(&rg.full[rg.c_stage], rg.c_phase, ctrl, 201);
