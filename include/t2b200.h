@@ -502,8 +502,11 @@ size_t t2_infer_lengths_workspace_bytes(const T2Model* m, int32_t B, int32_t T_t
 int    t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream);
 
 /* ---- WaveGlow vocoder inference (waveglow/glow.py: WaveGlow.infer, glow.py:251-293) ---------------
- * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  The kernels are built for the
- * published configuration (waveglow/config.json); t2_waveglow_create returns T2_ERR_UNSUPPORTED for anything else.
+ * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  Supported configurations (the published
+ * one, waveglow/config.json, is the comment beside each field): n_mel_channels 80, n_group 8, wn_kernel_size 3,
+ * wn_n_channels 128, 256, 384 or 512, wn_n_layers 1 ... 10, n_flows 1 ... 16, n_early_every >= 1 and n_early_size even,
+ * leaving the last flow at least 2 channels.  t2_waveglow_create returns T2_ERR_UNSUPPORTED for anything else, before
+ * any launch.
  * Precision tier: fp16 = 0 uses split-fp16 (hi + lo) operands with fp32 accumulation and fp32 state ("fp32 grade");
  * fp16 = 1 (a module converted with .half()) uses single fp16 operands with fp32 accumulation. */
 typedef struct T2WaveGlow T2WaveGlow;   /* opaque: configuration + packed device-side weights */
@@ -519,10 +522,13 @@ typedef struct T2WaveGlowConfig {
   int32_t fp16;                        /* 1: the weight table holds __half tensors (except convinv, always fp32) */
 } T2WaveGlowConfig;
 
-/* Entries of the WaveGlow weight table: the reference state_dict in its own order (686 tensors).  Weight-normed
- * convolutions contribute (bias, weight_g, weight_v); the library folds g * v / ||v|| when it packs.  After
- * remove_weightnorm a weight_g entry may be NULL and the weight_v entry is then the plain weight. */
+/* Entries of the WaveGlow weight table: the reference state_dict in its own order.  Weight-normed convolutions
+ * contribute (bias, weight_g, weight_v); the library folds g * v / ||v|| when it packs.  After remove_weightnorm a
+ * weight_g entry may be NULL and the weight_v entry is then the plain weight.  T2_WAVEGLOW_NUM_WEIGHTS is the published
+ * configuration's count; t2_waveglow_num_weights gives any supported configuration's, 2 + n_flows (6 wn_n_layers + 9),
+ * and 0 for a NULL or unsupported one. */
 #define T2_WAVEGLOW_NUM_WEIGHTS 686
+int32_t t2_waveglow_num_weights(const T2WaveGlowConfig* cfg);
 
 int t2_waveglow_create(T2WaveGlow** out, const T2WaveGlowConfig* cfg, const void* const* weights, int32_t n_weights,
                        void* stream);
@@ -531,8 +537,8 @@ int t2_waveglow_destroy(T2WaveGlow* h);
 
 /* mel (B, 80, T_mel), fp32 or (io_half) __half.  lengths (B) int32 in mel frames or NULL: row b's samples
  * [0, 256 lengths[b]) equal an infer of that row's first lengths[b] frames alone; later samples are zero.
- * z (B, 8, 32 T_mel) fp32 or NULL: the standard-normal draws, channels in draw order (the 4 initial ones, then the
- * early blocks of flow 8 and flow 4); NULL => in-kernel Philox4x32-10 keyed by (seed, row, channel, group column).
+ * z (B, 8, 32 T_mel) fp32 or NULL: the standard-normal draws, channels in draw order (the last flow's channels, then
+ * the early blocks from the last early flow down; published: 4, then flows 8 and 4); NULL => in-kernel Philox4x32-10 keyed by (seed, row, channel, group column).
  * row_seeds (B) device or NULL: row b's noise is keyed by (row_seeds[b], row 0, channel, group column) instead, the
  * draws of a B = 1 call with seed = row_seeds[b]; with z given it is T2_ERR_INVALID.
  * audio (B, 256 T_mel) out, in the mel's dtype. */
@@ -552,7 +558,9 @@ int    t2_waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, void* stream);
  * window-relative frames [out0, out1) is written to wg.audio, (B, 256 (out1 - out0)).  The noise is keyed by the
  * absolute group column 32 frame0 + t: Philox as above, or an injected wg.z (B, 8, 32 z_frames) read at absolute
  * columns, z_frames >= frame0 + T_mel.  at_end: the window ends where the sequence ends.
- * The audio of a frame depends on the 99 frames before it and the 96 after it (t2_waveglow_window_halo: left, right).  The call returns T2_ERR_INVALID, launching nothing, when out0 is closer than the left
+ * The audio of a frame depends on the halo_left frames before it and the halo_right after it: halo_right = ceil(n_flows
+ * (2^wn_n_layers - 1) / 32), halo_left = halo_right + 3 (t2_waveglow_window_halo_config; 99 and 96 for the published
+ * configuration, which t2_waveglow_window_halo returns).  The call returns T2_ERR_INVALID, launching nothing, when out0 is closer than the left
  * halo to a window start that is not the sequence's start (frame0 > 0), or out1 closer than the right halo to a
  * window end that is not the sequence's end (at_end = 0).  Workspace: t2_waveglow_workspace_bytes(h, B, T_mel).
  * t2_waveglow_infer is this call with frame0 = 0, [out0, out1) = [0, T_mel), z_frames = T_mel and at_end = 1. */
@@ -564,6 +572,8 @@ typedef struct T2WaveGlowWindowArgs {
   int32_t at_end;
 } T2WaveGlowWindowArgs;
 void   t2_waveglow_window_halo(int32_t* left, int32_t* right);
+/* The halos of the configuration `cfg` (fp16 is not read); T2_ERR_UNSUPPORTED, writing nothing, for an unsupported one. */
+int    t2_waveglow_window_halo_config(const T2WaveGlowConfig* cfg, int32_t* left, int32_t* right);
 int    t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void* stream);
 
 /* ---- WaveGlow denoiser (waveglow/denoiser.py: Denoiser, over stft.py:69-136 and audio_processing.py:7-56) -------

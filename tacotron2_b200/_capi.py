@@ -32,13 +32,14 @@ EXPORTS = [
     "t2_decoder_stream_state_bytes", "t2_decoder_stream_begin", "t2_decoder_stream_run",
     "t2_decoder_stream_admit", "t2_decoder_stream_collect",
     "t2_waveglow_create", "t2_waveglow_refresh", "t2_waveglow_destroy", "t2_waveglow_workspace_bytes",
-    "t2_waveglow_infer", "t2_waveglow_infer_window", "t2_waveglow_window_halo",
+    "t2_waveglow_infer", "t2_waveglow_infer_window", "t2_waveglow_window_halo", "t2_waveglow_window_halo_config",
+    "t2_waveglow_num_weights",
     "t2_denoiser_create", "t2_denoiser_refresh", "t2_denoiser_destroy", "t2_denoiser_bias",
     "t2_denoiser_workspace_bytes", "t2_denoiser_run", "t2_denoiser_run_window", "t2_denoiser_window_halo",
     "t2_stft_transform_workspace_bytes", "t2_stft_transform", "t2_stft_inverse_workspace_bytes", "t2_stft_inverse",
     "t2_griffin_lim_workspace_bytes", "t2_griffin_lim",
 ]
-T2_WAVEGLOW_NUM_WEIGHTS = 686
+T2_WAVEGLOW_NUM_WEIGHTS = 686       # the published configuration's; t2_waveglow_num_weights gives any other's
 
 
 class T2Config(C.Structure):
@@ -303,6 +304,10 @@ def lib():
     L.t2_waveglow_infer_window.argtypes = [C.c_void_p, C.POINTER(T2WaveGlowWindowArgs), C.c_void_p]
     L.t2_waveglow_window_halo.restype = None
     L.t2_waveglow_window_halo.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.t2_waveglow_window_halo_config.argtypes = [C.POINTER(T2WaveGlowConfig), C.POINTER(C.c_int32),
+                                                 C.POINTER(C.c_int32)]
+    L.t2_waveglow_num_weights.restype = C.c_int32
+    L.t2_waveglow_num_weights.argtypes = [C.POINTER(T2WaveGlowConfig)]
     L.t2_denoiser_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(T2DenoiserConfig), C.c_void_p, C.c_void_p,
                                      C.c_void_p]
     L.t2_denoiser_refresh.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -549,8 +549,8 @@ int t2_waveglow_refresh(T2WaveGlow* h, const void* const* weights, int32_t n_wei
   return waveglow_refresh(h, weights, n_weights, (cudaStream_t)stream);
 }
 int t2_waveglow_destroy(T2WaveGlow* h) { return waveglow_destroy(h); }
-size_t t2_waveglow_workspace_bytes(const T2WaveGlow*, int32_t B, int32_t T_mel) {
-  return B > 0 && T_mel > 0 ? waveglow_ws_bytes(B, T_mel) : 0;
+size_t t2_waveglow_workspace_bytes(const T2WaveGlow* h, int32_t B, int32_t T_mel) {
+  return B > 0 && T_mel > 0 ? waveglow_ws_bytes(h, B, T_mel) : 0;
 }
 int t2_waveglow_infer(T2WaveGlow* h, const T2WaveGlowArgs* a, void* stream) {
   return waveglow_infer(h, a, (cudaStream_t)stream);
@@ -559,6 +559,10 @@ int t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void*
   return waveglow_infer_window(h, a, (cudaStream_t)stream);
 }
 void t2_waveglow_window_halo(int32_t* left, int32_t* right) { waveglow_window_halo(left, right); }
+int t2_waveglow_window_halo_config(const T2WaveGlowConfig* cfg, int32_t* left, int32_t* right) {
+  return waveglow_window_halo_config(cfg, left, right);
+}
+int32_t t2_waveglow_num_weights(const T2WaveGlowConfig* cfg) { return waveglow_num_weights(cfg); }
 
 // ---- WaveGlow denoiser, STFT and Griffin-Lim (denoiser.cu) ----
 int t2_denoiser_create(T2Denoiser** out, const T2DenoiserConfig* cfg, const float* forward_basis,

@@ -25,7 +25,6 @@ constexpr int kTile = 128;                  // output rows (group columns / fram
 constexpr int kNT = 128, kWS = 4;           // MMA N per weight stage unless a caller picks another; weight ring stages
 constexpr int kThreads = 384;               // warp 0 producer; warpgroups 1 / 2: MMA + epilogue
 constexpr int kCluster = 2;                 // the CTAs of a cluster share each weight stage by multicast
-constexpr int kC = 256;                     // WaveGlow: WN channels (the skip rows of EPI_RESSKIP)
 constexpr unsigned long long kWd = 1ull << 32;
 // Denoiser spectrum planes (EPI_SPECTRAL / EPI_PROJECT write them, EPI_OVERLAP's GEMM reads them): the real parts of the 513 bins
 // in groups 0 ... 64, the imaginary parts in groups 65 ... 129, zero up to 136 groups = 17 whole 64-channel chunks.
@@ -63,7 +62,7 @@ struct GemmParams {
   int lo, hi;                       // only rows with t in [lo, hi) are needed: a cluster holding none of them exits
   const float* bias;
   __half* out; long out_rows, out_row0;              // planes the epilogue writes
-  float* skip; int first, res_tiles;                 // RESSKIP: column tiles < res_tiles are the residual half
+  float* skip; int first, res_cols;                  // RESSKIP: output columns < res_cols are the residual half
   int col_span;                                      // UPSAMPLE: span of the column domain
   float strength;                                    // SPECTRAL: the magnitude loses bias * strength
   float* audio; long audio_pitch;                    // OVERLAP: fp32 rows (B, audio_pitch); row t writes block t - lo
@@ -79,6 +78,7 @@ struct GemmParams {
   const float* scale; int act, out_mode, cout;
   float* out_f32; long ldo; int out_seq_rows;
   const float* residual; long res_batch_stride;
+  int skip_cols;                                     // RESSKIP: skip columns (the WN width); later columns are padding
 };
 
 template <int PASSES>
@@ -264,18 +264,19 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
           store8<PASSES>(p.out, p.out_rows, nt * 16 + (c0 >> 3), p.out_row0 + q, v);
         }
       } else if (EPI == EPI_RESSKIP) {
-        if (nt < p.res_tiles) {            // audio = audio + res_skip_acts[:, :256]  (glow.py:170)
+        // each thread's 128 columns lie wholly in the residual half or the skip half (the WN width is a multiple of 128)
+        const int n0 = nt * 256 + half * 128;
+        if (n0 < p.res_cols) {             // audio = audio + res_skip_acts[:, :C]  (glow.py:170)
           for (int g = 0; g < 16; ++g) {
-            const int c0 = half * 128 + g * 8;
+            const int c0 = n0 + g * 8;
             float v[8];
             load8<PASSES>(p.out, p.out_rows, c0 >> 3, p.out_row0 + q, v);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = valid ? v[i] + (row[c0 + i] + p.bias[c0 + i]) : 0.f;
+            for (int i = 0; i < 8; ++i) v[i] = valid ? v[i] + (row[c0 - nt * 256 + i] + p.bias[c0 + i]) : 0.f;
             store8<PASSES>(p.out, p.out_rows, c0 >> 3, p.out_row0 + q, v);
           }
-        } else {                           // output = output + res_skip_acts[:, 256:]  (glow.py:171, 173)
-          const int n0 = nt * 256 + half * 128;
-          float* sk = p.skip + q * kC + half * 128;
+        } else if (n0 - p.res_cols < p.skip_cols) {   // output = output + res_skip_acts[:, C:]  (glow.py:171, 173)
+          float* sk = p.skip + q * p.skip_cols + (n0 - p.res_cols);
           for (int c = 0; c < 128; c += 4) {
             float4 x = make_float4(row[half * 128 + c] + p.bias[n0 + c], row[half * 128 + c + 1] + p.bias[n0 + c + 1],
                                    row[half * 128 + c + 2] + p.bias[n0 + c + 2], row[half * 128 + c + 3] + p.bias[n0 + c + 3]);

@@ -81,7 +81,8 @@ _tls = threading.local()
 @contextlib.contextmanager
 def waveglow_noise(z):
     """Standard-normal draws for the next ``WaveGlow.infer`` calls: (B, n_group, 32 T_mel), channels in draw order
-    (the n_remaining_channels initial ones, then the early blocks of flow 8 and flow 4).  None => in-kernel Philox."""
+    (``noise_channel_order``: the n_remaining_channels initial ones, then each early block from the last early flow
+    down; published: 4, then flows 8 and 4).  None => in-kernel Philox."""
     prev = getattr(_tls, "z", None)
     _tls.z = z
     try:
@@ -148,9 +149,15 @@ class WaveGlow(torch.nn.Module):
         if self._t2 is not None:
             self._t2.invalidate()
 
+    def window_halo(self):
+        """(left, right): the mel frames before and after a frame that this model's audio depends on
+        (t2_waveglow_window_halo_config); (99, 96) for the published configuration."""
+        return config_halo(self._cfg)
+
     def _weight_table(self):
-        """(tensor or None) x 686 in the engine's table order: the reference state_dict order with weight-normed
-        convolutions as (bias, weight_g, weight_v); plain weights (after remove_weightnorm) go in the weight_v slot."""
+        """(tensor or None) x t2_waveglow_num_weights in the engine's table order: the reference state_dict order with
+        weight-normed convolutions as (bias, weight_g, weight_v); plain weights (after remove_weightnorm) go in the
+        weight_v slot."""
         def conv(m):
             if hasattr(m, "weight_v"):
                 return [m.bias, m.weight_g, m.weight_v]
@@ -190,7 +197,8 @@ class WaveGlow(torch.nn.Module):
         ``mel_lengths`` and ``finished`` of the mel item it came from.  The audio of frame t depends on the mel frames
         t - 99 ... t + 96 (``window_halo()``), so while a row is live an item holds the audio of every frame up to the
         final mel frames less 96, and the last item (``finished``) holds the rest; mel items that make no audio final
-        yield nothing.  Each item runs one windowed inference over the frames its audio depends on.  Concatenated along
+        yield nothing.  (99 and 96 are the published configuration's halos; another configuration's are
+        ``self.window_halo()``.)  Each item runs one windowed inference over the frames its audio depends on.  Concatenated along
         time the audio is bit-identical to ``infer(mel_outputs_postnet, sigma, lengths=model.mel_lengths)`` after
         ``model.inference(...)``, with the same weights and inputs and the same injected noise (``waveglow_noise``, read
         when infer_stream is called) or torch seed: the stream draws its Philox seed from torch's generator once, at its
@@ -219,9 +227,10 @@ class _WaveGlowEngine(_engine._Handle):
         self._ensure(w.device, module._weight_table(), (w.dtype == torch.float16,))
 
     def _pack(self, table, dev, fp16):
-        n_conv = _capi.T2_WAVEGLOW_NUM_WEIGHTS - self.cfg[1]      # the table ends with one convinv weight per flow
-        held, ptrs = [], (C.c_void_p * _capi.T2_WAVEGLOW_NUM_WEIGHTS)()
-        for i, t in enumerate(table[:_capi.T2_WAVEGLOW_NUM_WEIGHTS]):
+        n = num_weights(self.cfg) or len(table)    # an unsupported configuration: t2_waveglow_create refuses it
+        n_conv = n - self.cfg[1]                   # the table ends with one convinv weight per flow
+        held, ptrs = [], (C.c_void_p * n)()
+        for i, t in enumerate(table[:n]):
             if t is None:
                 continue
             t = t.detach()
@@ -230,10 +239,10 @@ class _WaveGlowEngine(_engine._Handle):
                 t = t.to(dt).contiguous()
             held.append(t)
             ptrs[i] = t.data_ptr()
-        return held, (ptrs, _capi.T2_WAVEGLOW_NUM_WEIGHTS)
+        return held, (ptrs, n)
 
     def _config(self, fp16):
-        return _capi.T2WaveGlowConfig(*[int(x) if x is not None else -1 for x in self.cfg], int(fp16))
+        return _config_struct(self.cfg, fp16)
 
     def _spect(self, spect, what):
         if spect.dim() != 3 or spect.shape[1] != self.cfg[0]:
@@ -306,7 +315,7 @@ class _WaveGlowEngine(_engine._Handle):
     @torch.no_grad()
     def stream(self, module, items, sigma, z, seeds=None):
         """The generator behind WaveGlow.infer_stream."""
-        win = FinalWindow("WaveGlow.infer_stream: mel items", "frames", 2, *window_halo())
+        win = FinalWindow("WaveGlow.infer_stream: mel items", "frames", 2, *config_halo(self.cfg))
         zt = z_frames = seed = row_seeds = None
         for item in items:
             win.check(item)
@@ -333,8 +342,24 @@ class _WaveGlowEngine(_engine._Handle):
 
 
 def window_halo():
-    """(left, right): the mel frames before and after a frame that its WaveGlow audio depends on
-    (t2_waveglow_window_halo)."""
+    """(left, right): the mel frames before and after a frame that the published WaveGlow's audio depends on
+    (t2_waveglow_window_halo); ``WaveGlow.window_halo()`` gives a model's own."""
     left, right = C.c_int32(), C.c_int32()
     _capi.lib().t2_waveglow_window_halo(C.byref(left), C.byref(right))
+    return left.value, right.value
+
+
+def _config_struct(cfg, fp16=0):
+    return _capi.T2WaveGlowConfig(*[int(x) if x is not None else -1 for x in cfg], int(fp16))
+
+
+def num_weights(cfg):
+    """Length of the engine's weight table for the configuration tuple ``cfg`` (WaveGlow._cfg); 0 if unsupported."""
+    return int(_capi.lib().t2_waveglow_num_weights(C.byref(_config_struct(cfg))))
+
+
+def config_halo(cfg):
+    """(left, right) halos of the configuration tuple ``cfg`` (t2_waveglow_window_halo_config)."""
+    left, right = C.c_int32(), C.c_int32()
+    _capi.check(_capi.lib().t2_waveglow_window_halo_config(C.byref(_config_struct(cfg)), C.byref(left), C.byref(right)))
     return left.value, right.value

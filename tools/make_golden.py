@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz by executing the UNMODIFIED reference model.py (needs a checkout of
-NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live|waveglow|denoiser|ragged]
+NVIDIA/tacotron2).  Run:  T2_REFERENCE_DIR=<reference checkout> python tools/make_golden.py [stft|full|grads|live|waveglow|waveglow_configs|denoiser|ragged]
 
 Every file holds the inputs' seeds, the reference outputs and a checksum of the synthetic weights
 (tests/common.synth_state_dict) so a drift of the generator is detected instead of silently
@@ -611,6 +611,32 @@ def waveglow_full_case(name, B, T, sigma, wseed, mseed, zseed, n_samples=4096):
          stats=np.array([float(a.mean()), float(a.std()), float(a.abs().max()), float(a.abs().mean())]))
 
 
+def waveglow_configs_case():
+    """The reference's WaveGlow.infer for the configurations of tests/waveglow_configs.FIXTURE_CASES, one npz: per case
+    ``<name>/mel``, ``/z`` (draw order), ``/audio``, ``/sigma``, ``/wseed`` and ``/checksum``."""
+    from tacotron2_b200.glow import noise_channel_order
+    from tests.waveglow_configs import FIXTURE_CASES, fixture_inputs, name_of, state_dict_for
+    arrays = {}
+    for cfg, B, T, sigma, wseed, mseed, zseed in FIXTURE_CASES:
+        sd = state_dict_for(cfg, wseed)
+        mel, z = fixture_inputs(B, T, mseed, zseed)
+        queue, c0 = [], 0
+        for _, n in noise_channel_order(cfg["n_flows"], cfg["n_group"], cfg["n_early_every"], cfg["n_early_size"]):
+            queue.append(z[:, c0:c0 + n].contiguous())
+            c0 += n
+        glow = import_reference_glow(queue)
+        model = glow.WaveGlow(**cfg)
+        model.load_state_dict(sd)
+        with torch.no_grad():
+            audio = model.infer(mel, sigma=sigma)
+        assert not queue
+        name = name_of(cfg)
+        print(name, tuple(audio.shape), float(audio.abs().max()))
+        arrays.update({name + "/mel": mel, name + "/z": z, name + "/audio": audio, name + "/sigma": sigma,
+                       name + "/wseed": wseed, name + "/checksum": weights_checksum(sd)})
+    save("waveglow_configs", **arrays)
+
+
 def waveglow_cases():
     waveglow_init_case()
     waveglow_infer_case("waveglow_b1_t50_s0", 1, 50, 0.0, 7, 41, 42)
@@ -746,6 +772,9 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "waveglow":
         waveglow_cases()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "waveglow_configs":
+        waveglow_configs_case()
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "live":
         reference_live_case()

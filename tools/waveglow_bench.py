@@ -1,6 +1,9 @@
 """WaveGlow.infer throughput / latency on the GPU, with the eager oracle (cuDNN) on the same card as context.
 
-    python tools/waveglow_bench.py [--reps 5] [--warmup 2] [--out results/waveglow_bench.json]
+    python tools/waveglow_bench.py [--reps 5] [--warmup 2] [--channels 256 --layers 8 --flows 12] [--no-oracle]
+                                   [--out results/waveglow_bench.json]
+The default shape is the published model's; --channels / --layers / --flows pick another WN width, depth and flow count
+(early outputs every 4 flows, 2 channels), with seeded weights.
 
 Times with CUDA events after warm-up, median over repeats.  Achieved TFLOP/s uses the algorithmic count computed from
 the shapes (flops_per_sample), against the H100 SXM data-sheet dense FP16 peak (989 TFLOP/s); the card name and power
@@ -17,7 +20,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import tacotron2_b200 as t2  # noqa: E402
-from oracle import waveglow_oracle as WO  # noqa: E402
+from tests import waveglow_config_oracle as WO  # noqa: E402
 from tests.waveglow_common import CONFIG, mel_input, noise, synth_state_dict  # noqa: E402
 
 PEAK_FP16 = 989e12
@@ -61,12 +64,22 @@ def main():
     ap.add_argument("--B", type=int, default=64)
     ap.add_argument("--T", type=int, default=800)
     ap.add_argument("--oracle-fp32-rows", type=int, default=8)
+    ap.add_argument("--channels", type=int, default=CONFIG["WN_config"]["n_channels"])
+    ap.add_argument("--layers", type=int, default=CONFIG["WN_config"]["n_layers"])
+    ap.add_argument("--flows", type=int, default=CONFIG["n_flows"])
+    ap.add_argument("--no-oracle", action="store_true", help="time the engine only")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "waveglow_bench needs a GPU"
-    fpsamp = flops_per_sample()
-    sd = synth_state_dict(7)
-    res = {"card": card(), "flops_per_sample": fpsamp, "B": a.B, "T_mel": a.T}
+    cfg = dict(CONFIG, n_flows=a.flows, WN_config=dict(n_layers=a.layers, n_channels=a.channels, kernel_size=3))
+    fpsamp = flops_per_sample(n_ch=a.channels, n_layers=a.layers, n_flows=a.flows)
+    if cfg == CONFIG:
+        sd = synth_state_dict(7)
+    else:
+        from tests.waveglow_configs import state_dict_for
+        sd = state_dict_for(cfg, 7)
+    res = {"card": card(), "config": dict(channels=a.channels, layers=a.layers, flows=a.flows), "flops_per_sample": fpsamp,
+           "B": a.B, "T_mel": a.T}
     print("card:", res["card"], " algorithmic MFLOP per sample: %.2f" % (fpsamp / 1e6))
 
     def record(name, ms, B, T):
@@ -78,7 +91,7 @@ def main():
               (name, B, T, ms, r["samples_per_s"], r["tflops"], 100 * r["share_of_fp16_peak"]))
 
     for half in (True, False):
-        m = t2.WaveGlow(**CONFIG)
+        m = t2.WaveGlow(**cfg)
         m.load_state_dict(sd)
         m = m.cuda()
         if half:
@@ -94,6 +107,12 @@ def main():
         del m
         torch.cuda.empty_cache()
 
+    if a.no_oracle:
+        if a.out:
+            os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
+            with open(a.out, "w") as f:
+                json.dump(res, f, indent=1)
+        return
     # eager oracle (cuDNN): fp16 at the full batch, fp32 with TF32 off on a slice of it
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
