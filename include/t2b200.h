@@ -15,7 +15,6 @@
  *       initialize_decoder_states             model.py:258-289        (inside: processed_memory GEMM)
  *     Postnet.forward (+ residual add)        model.py:141-146, 511, 524  -> t2_postnet_forward
  *     Tacotron2.inference, host buffers       model.py:517-529     -> t2_infer_host
- *       ... over texts of different lengths                        -> t2_infer_host_lengths
  *
  * Conventions
  *   - plain C types only; every tensor argument is a raw pointer into DEVICE memory of the current
@@ -41,7 +40,7 @@
 extern "C" {
 #endif
 
-#define T2_ABI_VERSION 1
+#define T2_ABI_VERSION 2
 
 #define T2_OK               0
 #define T2_ERR_INVALID     -1   /* bad argument / unsupported shape                     */
@@ -198,11 +197,13 @@ typedef struct T2DecoderArgs {
   const uint64_t* row_seeds;           /* (B) or NULL: per-row Philox keys of the prenet dropout (see below) */
   const float* forced_align;           /* (B, n_steps_cap, T_enc) or NULL: given attention weights (see above) */
   const int32_t* forced_lengths;       /* (B) or NULL: steps of each row of a forced run */
+  int32_t window_back, window_front;   /* 0, 0: no attention window (see below) */
+  const int32_t* max_steps;            /* (B) or NULL: each row's step limit (see below) */
 } T2DecoderArgs;
 size_t t2_decoder_workspace_bytes(const T2Model* m, int32_t B, int32_t T_enc, int32_t n_steps_cap);
 int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);
 /* Limits (INFER, persistent implementation): guards for free runs whose attention may jump, repeat or never reach the
- * end of the text.
+ * end of the text.  They are set when window_front != 0, window_back != 0 or max_steps != NULL; a zeroed struct sets none.
  *   window_back, window_front: an attention window (ESPnet's use_att_constraint with backward / forward window).  Let
  *     p_t(b) be the smallest j < memory_lengths[b] that maximises row b's weights of step t - 1 (0 at step 0, and at the
  *     first step of a row put back by admit, whose weights are all zero).  At step t the energies of row b at
@@ -216,14 +217,9 @@ int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);
  *     [1, n_steps_cap] where read) if its gate has not fired before; mel_lengths[b] is then max_steps[b].  The loop ends
  *     when every row has stopped, so n_steps_cap = the largest limit wastes no steps on rows that reached theirs.
  * Row b then equals bit for bit its own B = 1 call with n_steps_cap = max_steps[b] and the same window.
- * t2_decoder_run_limited with limits = NULL is t2_decoder_run.  T2_ERR_INVALID: limits with forced_align, mode TEACHER,
- * a negative window side, or window_back != 0 without a window; T2_ERR_UNSUPPORTED: the stepwise implementation
- * (requested, or chosen by AUTO for a T_enc the persistent kernel does not take).  t2_infer_host takes no limits. */
-typedef struct T2DecoderLimits {
-  int32_t window_back, window_front;
-  const int32_t* max_steps;
-} T2DecoderLimits;
-int    t2_decoder_run_limited(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* limits, void* stream);
+ * T2_ERR_INVALID: limits with forced_align, mode TEACHER, a negative window side, or window_back != 0 without a window;
+ * T2_ERR_UNSUPPORTED: the stepwise implementation (requested, or chosen by AUTO for a T_enc the persistent kernel does
+ * not take).  t2_infer_host takes no limits. */
 
 /* ---- Resumable decoder stream: the INFER loop of t2_decoder_run in chunks of steps -------------
  * The same persistent kernel stops after a number of steps and resumes exactly where it stopped, so
@@ -232,7 +228,8 @@ int    t2_decoder_run_limited(T2Model* m, const T2DecoderArgs* a, const T2Decode
  * `state` buffer (t2_decoder_stream_state_bytes), one block per 64-row slice: several streams can be
  * alive on one model at a time, and t2_decoder_run's workspace is not used.
  *   dec: as for t2_decoder_run with mode = INFER (teacher_prenet, att_keep, dec_keep, ws and stash are
- *        not used; memory_lengths is, as by t2_decoder_run).  mel / gate / align are the full
+ *        not used; memory_lengths is, as by t2_decoder_run).  The limits apply to every chunk; dec.max_steps count
+ *        absolute steps, so admit refuses a stream that carries them (T2_ERR_INVALID).  mel / gate / align are the full
  *        n_steps_cap-sized buffers; each run writes its steps at their absolute indices.  mel_lengths[b] =
  *        -1 while row b is live, then its length, as t2_decoder_run.  T2_IMPL_STEPWISE and encoder
  *        lengths the persistent kernel does not take are refused with T2_ERR_UNSUPPORTED.
@@ -248,9 +245,6 @@ typedef struct T2DecoderStreamArgs {
   int32_t* status;
   const int32_t* row_step0;            /* (B) device or NULL: with dec.row_seeds, row b's step (the one its prenet keys
                                           use) at local step i of a run is row_step0[b] + i instead of the absolute step */
-  const T2DecoderLimits* limits;       /* NULL or the limits of t2_decoder_run_limited, read by begin, run and admit: the
-                                          window applies to every chunk; max_steps count absolute steps, so admit
-                                          refuses limits that carry them (T2_ERR_INVALID) */
 } T2DecoderStreamArgs;
 size_t t2_decoder_stream_state_bytes(const T2Model* m, int32_t B, int32_t T_enc);
 int    t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stream);
@@ -466,27 +460,21 @@ typedef struct T2CollateArgs {
 int t2_collate(const T2CollateArgs* a, void* stream);
 
 /* ---- Tacotron2.inference end to end with HOST buffers (model.py:517-529) ----------------------
- * text_host (B, T_text) int64 in (pinned) host memory -> mel_post_host (B, 80, T_cap) fp32,
+ * text_host (B, T_text) int64 in (pinned) host memory -> mel_post_host (B, 80, max_steps) fp32,
  * mel_lengths_host (B), n_steps_host (1).  Copies H2D, runs encoder -> decoder -> postnet on
  * `stream`, copies D2H and synchronises the stream.  The postnet runs over the n_steps decoded
  * frames, as Tacotron2.inference does (so frames [0, n_steps) equal its mel_outputs_postnet); frames
  * beyond each row's length are zero.  Seed: the decoder's prenet dropout.  ws is device memory of
- * t2_infer_workspace_bytes(). */
-size_t t2_infer_workspace_bytes(const T2Model* m, int32_t B, int32_t T_text, int32_t max_steps);
-int    t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_text,
-                     int32_t max_steps, float gate_threshold, uint64_t seed, int32_t impl,
-                     float* mel_post_host, int32_t* mel_lengths_host, int32_t* n_steps_host,
-                     void* ws, size_t ws_bytes, void* stream);
-
-/* t2_infer_host over texts of different lengths: input_lengths_host (B) int64 in (pinned) host memory, each in
- * [1, T_text], any order.  Row b's outputs equal those of t2_infer_host on text_host[b, :input_lengths_host[b]] alone
- * (B = 1, same seed and impl) bit for bit, up to that call's n_steps; the ids at t >= input_lengths_host[b] are
- * ignored.  When every length is T_text the outputs are t2_infer_host's (an equal-length batch keeps its batched
- * postnet, see t2_postnet_infer).  A length outside [1, T_text] or a NULL input_lengths_host is T2_ERR_INVALID before anything is enqueued.
- * ws: device memory of t2_infer_lengths_workspace_bytes(). */
+ * t2_infer_workspace_bytes().
+ * Texts of different lengths: input_lengths_host (B) int64 in (pinned) host memory, each in [1, T_text], any order, or
+ * NULL (every row T_text long).  Row b's outputs then equal those of a call on text_host[b, :input_lengths_host[b]]
+ * alone (B = 1, same seed and impl) bit for bit, up to that call's n_steps; the ids at t >= input_lengths_host[b] are
+ * ignored.  When every length is T_text the outputs are those of input_lengths_host = NULL (an equal-length batch keeps
+ * its batched postnet, see t2_postnet_infer).  A length outside [1, T_text] is T2_ERR_INVALID before anything is
+ * enqueued.  row_seeds_host needs input_lengths_host (T2_ERR_INVALID otherwise). */
 typedef struct T2InferArgs {
   const int64_t* text_host;            /* (B, T_text) */
-  const int64_t* input_lengths_host;   /* (B) */
+  const int64_t* input_lengths_host;   /* (B) or NULL */
   int32_t B, T_text, max_steps;
   float gate_threshold;
   uint64_t seed;
@@ -498,8 +486,8 @@ typedef struct T2InferArgs {
   const uint64_t* row_seeds_host;      /* (B) host or NULL: the decoder's row_seeds (row b then equals its B = 1 call
                                           with seed = row_seeds_host[b]); `seed` is not used when given */
 } T2InferArgs;
-size_t t2_infer_lengths_workspace_bytes(const T2Model* m, int32_t B, int32_t T_text, int32_t max_steps);
-int    t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream);
+size_t t2_infer_workspace_bytes(const T2Model* m, int32_t B, int32_t T_text, int32_t max_steps);
+int    t2_infer_host(T2Model* m, const T2InferArgs* a, void* stream);
 
 /* ---- WaveGlow vocoder inference (waveglow/glow.py: WaveGlow.infer, glow.py:251-293) ---------------
  * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  Supported configurations (the published
@@ -711,7 +699,7 @@ int t2_selftest_waveglow_state(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, int
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* After a T2_IMPL_PERSISTENT run with the same args / workspace: SM cycles spent per phase of the
  * persistent kernel, summed over steps, on three sample CTAs (out_host[3][24]; phase list in
- * decoder_persistent.cu); all zero after a t2_decoder_run_limited run, whose kernel keeps no profile.
+ * decoder_persistent.cu); all zero after a run with limits, whose kernel keeps no profile.
  * Synchronises the device. */
 int t2_decoder_profile(const T2DecoderArgs* a, int64_t* out_host);
 /* number of kernels this library has launched since load (for bench.py's gpu_launches) */

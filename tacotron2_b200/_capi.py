@@ -17,9 +17,9 @@ MODE_INFER, MODE_TEACHER = 0, 1
 EXPORTS = [
     "t2_abi_version", "t2_last_error", "t2_device_info", "t2_model_create", "t2_model_refresh",
     "t2_model_destroy", "t2_encoder_workspace_bytes", "t2_encoder_forward",
-    "t2_decoder_workspace_bytes", "t2_decoder_run", "t2_decoder_run_limited", "t2_prenet_forward",
+    "t2_decoder_workspace_bytes", "t2_decoder_run", "t2_prenet_forward",
     "t2_postnet_workspace_bytes", "t2_postnet_forward", "t2_infer_workspace_bytes", "t2_infer_host",
-    "t2_encoder_infer", "t2_postnet_infer", "t2_infer_lengths_workspace_bytes", "t2_infer_host_lengths",
+    "t2_encoder_infer", "t2_postnet_infer",
     "t2_kernel_launch_count", "t2_decoder_profile",
     "t2_decoder_stash_bytes", "t2_decoder_backward_workspace_bytes", "t2_decoder_backward",
     "t2_prenet_backward_workspace_bytes", "t2_prenet_backward",
@@ -84,16 +84,13 @@ class T2DecoderArgs(C.Structure):
                 ("mel_lengths", C.c_void_p), ("n_steps", C.c_void_p),
                 ("ws", C.c_void_p), ("ws_bytes", C.c_size_t),
                 ("stash", C.c_void_p), ("stash_bytes", C.c_size_t), ("row_seeds", C.c_void_p),
-                ("forced_align", C.c_void_p), ("forced_lengths", C.c_void_p)]
-
-
-class T2DecoderLimits(C.Structure):
-    _fields_ = [("window_back", C.c_int32), ("window_front", C.c_int32), ("max_steps", C.c_void_p)]
+                ("forced_align", C.c_void_p), ("forced_lengths", C.c_void_p),
+                ("window_back", C.c_int32), ("window_front", C.c_int32), ("max_steps", C.c_void_p)]
 
 
 class T2DecoderStreamArgs(C.Structure):
     _fields_ = [("dec", T2DecoderArgs), ("state", C.c_void_p), ("state_bytes", C.c_size_t), ("status", C.c_void_p),
-                ("row_step0", C.c_void_p), ("limits", C.POINTER(T2DecoderLimits))]
+                ("row_step0", C.c_void_p)]
 
 
 class T2CollectRow(C.Structure):
@@ -247,14 +244,13 @@ def lib():
               "t2_encoder_backward_workspace_bytes", "t2_postnet_stash_bytes", "t2_postnet_backward_workspace_bytes"):
         getattr(L, n).restype = C.c_size_t
         getattr(L, n).argtypes = [C.c_void_p, C.c_int32, C.c_int32]
-    for n in ("t2_decoder_workspace_bytes", "t2_infer_workspace_bytes", "t2_infer_lengths_workspace_bytes",
-              "t2_decoder_stash_bytes", "t2_decoder_backward_workspace_bytes"):
+    for n in ("t2_decoder_workspace_bytes", "t2_infer_workspace_bytes", "t2_decoder_stash_bytes",
+              "t2_decoder_backward_workspace_bytes"):
         getattr(L, n).restype = C.c_size_t
         getattr(L, n).argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     L.t2_encoder_forward.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_encoder_infer.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_decoder_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderArgs), C.c_void_p]
-    L.t2_decoder_run_limited.argtypes = [C.c_void_p, C.POINTER(T2DecoderArgs), C.POINTER(T2DecoderLimits), C.c_void_p]
     L.t2_decoder_stream_state_bytes.restype = C.c_size_t
     L.t2_decoder_stream_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.t2_decoder_stream_begin.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_void_p]
@@ -289,10 +285,7 @@ def lib():
     L.t2_prenet_backward_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
     L.t2_prenet_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64,
                                     C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    L.t2_infer_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
-                                C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                C.c_void_p, C.c_size_t, C.c_void_p]
-    L.t2_infer_host_lengths.argtypes = [C.c_void_p, C.POINTER(T2InferArgs), C.c_void_p]
+    L.t2_infer_host.argtypes = [C.c_void_p, C.POINTER(T2InferArgs), C.c_void_p]
     L.t2_decoder_profile.argtypes = [C.POINTER(T2DecoderArgs), C.POINTER(C.c_int64)]
     L.t2_waveglow_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(T2WaveGlowConfig), C.POINTER(C.c_void_p),
                                      C.c_int32, C.c_void_p]
@@ -324,7 +317,7 @@ def lib():
         getattr(L, n + "_workspace_bytes").restype = C.c_size_t
         getattr(L, n + "_workspace_bytes").argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         getattr(L, n).argtypes = [C.c_void_p, C.POINTER(args), C.c_void_p]
-    if L.t2_abi_version() != 1:
+    if L.t2_abi_version() != 2:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L
     return L

@@ -96,6 +96,14 @@ def next_seed():
     return (torch.initial_seed() * 1000003 + _seed_counter[0]) & 0xFFFFFFFFFFFFFFFF
 
 
+def seed_pattern(v, what):
+    """One seed, an integer in [0, 2**64), as its 64-bit pattern in int64 range; raises ValueError outside."""
+    v = int(v)
+    if not 0 <= v < 1 << 64:
+        raise ValueError("%s: seed %d is outside [0, 2**64)" % (what, v))
+    return v - (1 << 64) if v >= 1 << 63 else v
+
+
 def row_seeds(seeds, B, device, what):
     """Per-utterance seeds as B 64-bit Philox keys, an int64 tensor on `device` holding each key's bit pattern (None
     stays None).  seeds: B integers in [0, 2**64), as a list, a host tensor or a device tensor; int64 / uint64 values are
@@ -119,22 +127,39 @@ def row_seeds(seeds, B, device, what):
     vals = list(seeds)
     if len(vals) != B:
         raise ValueError("%s: seeds must hold %d values (got %d)" % (what, B, len(vals)))
-    bits = []
     for v in vals:
         if isinstance(v, bool) or not isinstance(v, numbers.Integral):
             raise TypeError("%s: seeds must be integers (got %r)" % (what, v))
-        v = int(v)
-        if not 0 <= v < 1 << 64:
-            raise ValueError("%s: seed %d is outside [0, 2**64)" % (what, v))
-        bits.append(v - (1 << 64) if v >= 1 << 63 else v)
-    return torch.tensor(bits, dtype=torch.int64).to(device)
+    return torch.tensor([seed_pattern(v, what) for v in vals], dtype=torch.int64).to(device)
+
+
+def _integer_tensor(x, name, what):
+    """x (a tensor, or anything torch.as_tensor takes) as a tensor of integers; TypeError otherwise."""
+    t = x if torch.is_tensor(x) else torch.as_tensor(x)
+    if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+        raise TypeError("%s: %s must hold integers (got %s)" % (what, name, t.dtype))
+    return t
+
+
+def row_lengths(lengths, B, T, name, device):
+    """Per-row lengths of a ragged inference batch: (B,) integers, each in 1..T, as a list, a host or a device tensor.
+    Returns (lengths as int32 on `device`, whether some row is shorter than T), reading a device tensor back once;
+    (None, False) for None.  Raises TypeError / ValueError before anything is launched."""
+    if lengths is None:
+        return None, False
+    t = _integer_tensor(lengths, name, "tacotron2_b200")
+    if tuple(t.shape) != (B,):
+        raise ValueError("tacotron2_b200: %s must have shape (%d,) (got %s)" % (name, B, tuple(t.shape)))
+    host = t.cpu()
+    lo, hi = int(host.min()), int(host.max())
+    if lo < 1 or hi > T:
+        raise ValueError("tacotron2_b200: %s must lie in 1..%d (got %d..%d)" % (name, T, lo, hi))
+    return t.to(device=device, dtype=torch.int32).contiguous(), lo < T
 
 
 def forced_alignment(alignments, alignment_lengths, B, T_text, device, training, what):
-    """Given attention weights for a forced run as the engine takes them: (map (B, T_map, T_text) fp32 contiguous,
-    lengths (B,) int32), both on `device`; (None, None) without a map.  alignments: a float tensor (B, T_map, T_text) on
-    `device`; alignment_lengths: None (T_map for every row) or B integers in 1..T_map as a list, a host or a device
-    tensor.  Raises TypeError / ValueError naming the argument before anything runs."""
+    """The forced-alignment part of inference_options: given attention weights as the engine takes them, (map (B, T_map,
+    T_text) fp32 contiguous, lengths (B,) int32), both on `device`; (None, None) without a map."""
     if alignments is None:
         if alignment_lengths is not None:
             raise ValueError("%s: alignment_lengths needs alignments" % what)
@@ -155,9 +180,7 @@ def forced_alignment(alignments, alignment_lengths, B, T_text, device, training,
     if alignment_lengths is None:
         lengths = torch.full((B,), T_map, dtype=torch.int32, device=device)
     else:
-        lengths = alignment_lengths if torch.is_tensor(alignment_lengths) else torch.as_tensor(alignment_lengths)
-        if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
-            raise TypeError("%s: alignment_lengths must hold integers (got %s)" % (what, lengths.dtype))
+        lengths = _integer_tensor(alignment_lengths, "alignment_lengths", what)
         if tuple(lengths.shape) != (B,):
             raise ValueError("%s: alignment_lengths must have shape (%d,) (got %s)" % (what, B, tuple(lengths.shape)))
         host = lengths.cpu()
@@ -172,12 +195,9 @@ def _integral(v):
     return isinstance(v, numbers.Integral) and not isinstance(v, bool)
 
 
-def decoder_limits(attention_window, max_decoder_steps, B, device, forced, what):
+def _limits(attention_window, max_decoder_steps, B, device, forced, what):
     """The limits of a free run as the engine takes them: (window, caps, longest) -- window None or (back, front) ints,
-    caps None or (B,) int32 contiguous on `device`, longest None or max(caps) (the run's n_steps_cap).
-    attention_window: None or two integers (back >= 0, front >= 1); max_decoder_steps: None, one integer or B integers
-    >= 1 (a list, a host or a device tensor).  forced: a forced alignment is given, which takes neither.  Raises
-    TypeError / ValueError naming the argument before anything runs."""
+    caps None or (B,) int32 contiguous on `device`, longest None or max(caps) (see inference_options)."""
     if forced and attention_window is not None:
         raise ValueError("%s: attention_window and alignments exclude each other (a forced run computes no energies)" % what)
     if forced and max_decoder_steps is not None:
@@ -194,11 +214,9 @@ def decoder_limits(attention_window, max_decoder_steps, B, device, forced, what)
     if max_decoder_steps is None:
         return window, None, None
     if _integral(max_decoder_steps):
-        host = torch.full((B,), int(max_decoder_steps), dtype=torch.int64)
+        caps = host = torch.full((B,), int(max_decoder_steps), dtype=torch.int64)
     else:
-        caps = max_decoder_steps if torch.is_tensor(max_decoder_steps) else torch.as_tensor(max_decoder_steps)
-        if caps.dtype.is_floating_point or caps.dtype.is_complex or caps.dtype == torch.bool:
-            raise TypeError("%s: max_decoder_steps must hold integers (got %s)" % (what, caps.dtype))
+        caps = _integer_tensor(max_decoder_steps, "max_decoder_steps", what)
         if tuple(caps.shape) != (B,):
             raise ValueError("%s: max_decoder_steps must be one integer or have shape (%d,) (got %s)"
                              % (what, B, tuple(caps.shape)))
@@ -206,15 +224,53 @@ def decoder_limits(attention_window, max_decoder_steps, B, device, forced, what)
     lo, hi = int(host.min()), int(host.max())
     if lo < 1 or hi > 2 ** 31 - 1:
         raise ValueError("%s: max_decoder_steps must lie in 1..2**31-1 (got %d..%d)" % (what, lo, hi))
-    return window, host.to(device=device, dtype=torch.int32).contiguous(), hi
+    return window, caps.to(device=device, dtype=torch.int32).contiguous(), hi
 
 
-def limits_struct(window, caps):
-    """T2DecoderLimits of (window, caps) as decoder_limits() returns them; None when both are None."""
-    if window is None and caps is None:
-        return None
-    back, front = window if window is not None else (0, 0)
-    return _capi.T2DecoderLimits(back, front, _ptr(caps))
+class InferenceOptions:
+    """The per-row options of one inference call in the engine's form (inference_options()).
+
+    lengths: (B,) int32 on the device or None; ragged: some row is shorter than T_enc; row_seeds: (B,) int64 key
+    patterns on the device or None; forced_align / forced_lengths: a forced run's map (B, T_map, T_enc) fp32 and steps
+    (B,) int32, or None; window: (back, front) or None; max_steps: (B,) int32 step limits or None; cap: the run's
+    n_steps_cap when the options fix it (T_map, or the largest limit), else None."""
+
+    def __init__(self, lengths, ragged, row_seeds, forced, limits):
+        self.lengths, self.ragged, self.row_seeds = lengths, ragged, row_seeds
+        self.forced_align, self.forced_lengths = forced
+        self.window, self.max_steps, longest = limits
+        self.cap = self.forced_align.size(1) if self.forced_align is not None else longest
+
+    def decoder_kwargs(self):
+        """The keyword arguments of Engine.decoder / Engine.decoder_stream these options set."""
+        return dict(memory_lengths=self.lengths, row_seeds=self.row_seeds, forced_align=self.forced_align,
+                    forced_lengths=self.forced_lengths, window=self.window, max_steps=self.max_steps)
+
+
+def inference_options(what, B, T_enc, device, training=False, prenet_masks=False, lengths=None,
+                      lengths_name="memory_lengths", seeds=None, alignments=None, alignment_lengths=None,
+                      attention_window=None, max_decoder_steps=None):
+    """The user-facing options of one inference call (``what``, e.g. "Tacotron2.inference") checked once and turned into
+    the engine's form, an InferenceOptions.  Each device tensor among them is read back to the host at most once.
+
+    lengths (named ``lengths_name``): None or B integers in 1..T_enc (see row_lengths).  seeds: None or B integers in
+    [0, 2**64) (see row_seeds); they need eval mode (training False) and no injected prenet masks (prenet_masks False).
+    alignments: None or a float tensor (B, T_map, T_enc) on `device`, eval mode only; alignment_lengths: None (T_map for
+    every row) or B integers in 1..T_map.  attention_window: None or two integers (back >= 0, front >= 1);
+    max_decoder_steps: None, one integer or B integers >= 1; neither goes with alignments.  Raises TypeError /
+    ValueError naming the argument before anything runs."""
+    lengths, ragged = row_lengths(lengths, B, T_enc, lengths_name, device)
+    what = "tacotron2_b200: " + what
+    if seeds is not None:
+        if training:
+            raise ValueError("%s: seeds need eval mode (training-mode BatchNorm mixes the rows and the hidden-state dropout "
+                             "is not keyed per row)" % what)
+        if prenet_masks:
+            raise ValueError("%s: seeds and injected prenet masks exclude each other" % what)
+    keys = row_seeds(seeds, B, device, what)
+    forced = forced_alignment(alignments, alignment_lengths, B, T_enc, device, training, what)
+    limits = _limits(attention_window, max_decoder_steps, B, device, forced[0] is not None, what)
+    return InferenceOptions(lengths, ragged, keys, forced, limits)
 
 
 def alignments_from_durations(durations):
@@ -434,9 +490,8 @@ class Engine(_Handle):
                 forced_lengths=None, window=None, max_steps=None):
         """row_seeds: None or (B,) int64 on the device (see row_seeds()): per-row prenet keys.  forced_align /
         forced_lengths: None, or the given attention weights (B, n_steps_cap, T_enc) fp32 and each row's step count (B,)
-        int32, both contiguous on the device (see forced_alignment()).  window / max_steps: None, or the attention window
-        (back, front) and each row's step limit (B,) int32 on the device (see decoder_limits()); either one runs
-        t2_decoder_run_limited."""
+        int32, both contiguous on the device.  window / max_steps: None, or the attention window (back, front) and each
+        row's step limit (B,) int32 on the device (see InferenceOptions)."""
         L = _capi.lib()
         memory = memory.to(device=self.device, dtype=torch.float32).contiguous()
         B, T = int(memory.shape[0]), int(memory.shape[1])
@@ -453,18 +508,14 @@ class Engine(_Handle):
         if teacher_prenet is not None:
             teacher_prenet = teacher_prenet.contiguous()
         pk, ak, dk = _u8(prenet_keep, self.device), _u8(att_keep, self.device), _u8(dec_keep, self.device)
-        a = _capi.T2DecoderArgs(mode, self.impl if impl is None else impl, int(bool(training)), memory.data_ptr(),
-                                _ptr(len32), B, T, cap, _ptr(teacher_prenet), _ptr(pk), _ptr(ak), _ptr(dk),
-                                next_seed() if seed is None else seed, float(gate_threshold), float(score_mask_value),
-                                mel.data_ptr(), gate.data_ptr(), align.data_ptr(), mel_lengths.data_ptr(),
-                                n_steps.data_ptr(), ws.data_ptr(), ws.numel(),
-                                _ptr(stash), 0 if stash is None else stash.numel(), _ptr(row_seeds),
-                                _ptr(forced_align), _ptr(forced_lengths))
-        lim = limits_struct(window, max_steps)
-        if lim is None:
-            self._call(L.t2_decoder_run, C.byref(a))
-        else:
-            self._call(L.t2_decoder_run_limited, C.byref(a), C.byref(lim))
+        a = decoder_args(mode=mode, impl=self.impl if impl is None else impl, training=int(bool(training)), memory=memory,
+                         memory_lengths=len32, B=B, T_enc=T, n_steps_cap=cap, teacher_prenet=teacher_prenet,
+                         prenet_keep=pk, att_keep=ak, dec_keep=dk, seed=next_seed() if seed is None else seed,
+                         gate_threshold=float(gate_threshold), score_mask_value=float(score_mask_value), mel=mel,
+                         gate=gate, align=align, mel_lengths=mel_lengths, n_steps=n_steps, ws=ws, ws_bytes=ws.numel(),
+                         stash=stash, stash_bytes=0 if stash is None else stash.numel(), row_seeds=row_seeds,
+                         forced_align=forced_align, forced_lengths=forced_lengths, window=window, max_steps=max_steps)
+        self._call(L.t2_decoder_run, C.byref(a))
         self._last_decoder_args = (a, memory, len32, teacher_prenet, pk, ak, dk, ws, mel, gate, align, mel_lengths, n_steps,
                                    row_seeds, forced_align, forced_lengths, max_steps)
         return mel, gate, align, mel_lengths, n_steps
@@ -564,29 +615,31 @@ class Engine(_Handle):
                    row_seeds_host=None):
         """text_host: pinned int64 (B, T).  Returns (mel_post_host (B,80,max_steps), lengths, n_steps).  seed: the
         Philox seed of the decoder's prenet dropout (default: next_seed()).  input_lengths_host: pinned int64 (B) or None;
-        given, t2_infer_host_lengths runs each row as its first input_lengths_host[b] symbols alone.  row_seeds_host: int64
-        (B) host tensor of per-row seeds (needs input_lengths_host): row b then equals its B = 1 call with that seed."""
+        given, each row runs as its first input_lengths_host[b] symbols alone.  row_seeds_host: int64 (B) host tensor of
+        per-row seeds (needs input_lengths_host): row b then equals its B = 1 call with that seed."""
         L = _capi.lib()
         B, T = int(text_host.shape[0]), int(text_host.shape[1])
         if out_host is None:
             out_host = (torch.empty(B, self.hp.n_mel_channels, max_steps, dtype=torch.float32).pin_memory(),
                         torch.empty(B, dtype=torch.int32).pin_memory(), torch.empty(1, dtype=torch.int32).pin_memory())
         mel, lens, ns = out_host
-        seed = next_seed() if seed is None else seed
-        impl = self.impl if impl is None else impl
-        if input_lengths_host is not None:
-            ws = self._workspace("e2e", L.t2_infer_lengths_workspace_bytes(self.handle, B, T, max_steps))
-            a = _capi.T2InferArgs(text_host.data_ptr(), input_lengths_host.data_ptr(), B, T, int(max_steps),
-                                  float(gate_threshold), seed, impl, mel.data_ptr(), lens.data_ptr(), ns.data_ptr(),
-                                  ws.data_ptr(), ws.numel(), _ptr(row_seeds_host))
-            self._call(L.t2_infer_host_lengths, C.byref(a))
-            return mel, lens, ns
-        if row_seeds_host is not None:
-            raise ValueError("tacotron2_b200: row_seeds_host needs input_lengths_host (t2_infer_host_lengths)")
         ws = self._workspace("e2e", L.t2_infer_workspace_bytes(self.handle, B, T, max_steps))
-        self._call(L.t2_infer_host, text_host.data_ptr(), B, T, int(max_steps), float(gate_threshold), seed, impl,
-                   mel.data_ptr(), lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel())
+        a = _capi.T2InferArgs(text_host.data_ptr(), _ptr(input_lengths_host), B, T, int(max_steps), float(gate_threshold),
+                              next_seed() if seed is None else seed, self.impl if impl is None else impl, mel.data_ptr(),
+                              lens.data_ptr(), ns.data_ptr(), ws.data_ptr(), ws.numel(), _ptr(row_seeds_host))
+        self._call(L.t2_infer_host, C.byref(a))
         return mel, lens, ns
+
+
+def decoder_args(window=None, **fields):
+    """A T2DecoderArgs from its fields by name: tensors by their data pointer, None as NULL, fields not given zero.
+    window: None (no window) or (back, front)."""
+    a = _capi.T2DecoderArgs()
+    if window is not None:
+        a.window_back, a.window_front = window
+    for name, v in fields.items():
+        setattr(a, name, v.data_ptr() if torch.is_tensor(v) else v)
+    return a
 
 
 def f32_buffer(device, *shape):
@@ -628,16 +681,13 @@ class DecoderStream:
         self.state = _capi.byte_buffer(L.t2_decoder_stream_state_bytes(eng.handle, B, T), dev)
         self.keep, self.len32 = _u8(prenet_keep, dev), _i32(memory_lengths, dev)
         self.row_seeds = row_seeds      # (B,) int64 bit patterns on the device or None; a session may rewrite them
-        self.forced = (forced_align, forced_lengths)     # the kernel reads them in every chunk
-        d = _capi.T2DecoderArgs(_capi.MODE_INFER, impl, 0, self.memory.data_ptr(), _ptr(self.len32), B, T, self.cap,
-                                None, _ptr(self.keep), None, None, seed, float(gate_threshold), float(score_mask_value),
-                                self.mel.data_ptr(), self.gate.data_ptr(), self.align.data_ptr(),
-                                self.mel_lengths.data_ptr(), self.n_steps.data_ptr(), row_seeds=_ptr(row_seeds),
-                                forced_align=_ptr(forced_align), forced_lengths=_ptr(forced_lengths))
-        self.limits = (limits_struct(window, max_steps), max_steps)      # every call reads them
+        self.held = (forced_align, forced_lengths, max_steps)     # the kernel reads them in every chunk
+        d = decoder_args(mode=_capi.MODE_INFER, impl=impl, memory=self.memory, memory_lengths=self.len32, B=B, T_enc=T,
+                         n_steps_cap=self.cap, prenet_keep=self.keep, seed=seed, gate_threshold=float(gate_threshold),
+                         score_mask_value=float(score_mask_value), mel=self.mel, gate=self.gate, align=self.align,
+                         mel_lengths=self.mel_lengths, n_steps=self.n_steps, row_seeds=row_seeds,
+                         forced_align=forced_align, forced_lengths=forced_lengths, window=window, max_steps=max_steps)
         self.args = _capi.T2DecoderStreamArgs(d, self.state.data_ptr(), self.state.numel(), self.status.data_ptr())
-        if self.limits[0] is not None:
-            self.args.limits = C.pointer(self.limits[0])
         eng._call(L.t2_decoder_stream_begin, C.byref(self.args))
 
     def run(self, n):

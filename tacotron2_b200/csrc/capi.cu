@@ -121,52 +121,36 @@ static size_t decoder_ws_bytes(int B, int T, int cap) {
   return sw > pe ? sw : pe;
 }
 
-// per-row prenet keys: evaluation-mode INFER only (the hidden-state dropout of training mode is keyed by the call), and
-// never together with injected masks
-static int check_row_seeds(const T2DecoderArgs* a, const char* what) {
-  if (!a->row_seeds) return T2_OK;
-  if (a->mode != T2_MODE_INFER || a->training)
-    return fail(T2_ERR_INVALID, "%s: row_seeds need mode INFER with training = 0 (mode %d, training %d)", what, a->mode,
-                a->training);
-  if (a->prenet_keep) return fail(T2_ERR_INVALID, "%s: row_seeds and prenet_keep exclude each other", what);
-  return T2_OK;
-}
-
-// given attention weights: both pointers or neither, evaluation-mode INFER only
-static int check_forced(const T2DecoderArgs* a, const char* what) {
+// the checks t2_decoder_run and the decoder stream share: shape, output pointers, and the per-row options -- per-row
+// prenet keys (evaluation-mode INFER, never with injected masks), a forced alignment (both pointers or neither,
+// evaluation-mode INFER) and limits (INFER without a forced alignment, a window of non-negative sides)
+static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a, const char* what) {
+  if (!m || !a) return fail(T2_ERR_INVALID, "%s: null model / args", what);
+  if (a->B <= 0 || a->B > kMaxBatch) return fail(T2_ERR_INVALID, "%s: B=%d outside [1, %d]", what, a->B, kMaxBatch);
+  if (a->T_enc <= 0) return fail(T2_ERR_INVALID, "%s: empty encoder memory (T_enc=%d)", what, a->T_enc);
+  if (a->n_steps_cap <= 0) return fail(T2_ERR_INVALID, "%s: n_steps_cap=%d", what, a->n_steps_cap);
+  if (!a->memory || !a->mel || !a->gate || !a->align || !a->mel_lengths || !a->n_steps)
+    return fail(T2_ERR_INVALID, "%s: null tensor pointer", what);
   if (!a->forced_align != !a->forced_lengths)
     return fail(T2_ERR_INVALID, "%s: forced_align and forced_lengths go together (got only %s)", what,
                 a->forced_align ? "forced_align" : "forced_lengths");
   if (a->forced_align && (a->mode != T2_MODE_INFER || a->training))
     return fail(T2_ERR_INVALID, "%s: a forced alignment needs mode INFER with training = 0 (mode %d, training %d)", what,
                 a->mode, a->training);
+  if (decoder_has_limits(a)) {
+    if (a->forced_align) return fail(T2_ERR_INVALID, "%s: limits and forced_align exclude each other (the map decides the steps)", what);
+    if (a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "%s: limits need mode INFER (got %d)", what, a->mode);
+    if (a->window_back < 0 || a->window_front < 0)
+      return fail(T2_ERR_INVALID, "%s: attention window (%d, %d) has a negative side", what, a->window_back, a->window_front);
+    if (a->window_front == 0 && a->window_back != 0)
+      return fail(T2_ERR_INVALID, "%s: window_back = %d without a window (window_front = 0)", what, a->window_back);
+  }
+  if (!a->row_seeds) return T2_OK;
+  if (a->mode != T2_MODE_INFER || a->training)
+    return fail(T2_ERR_INVALID, "%s: row_seeds need mode INFER with training = 0 (mode %d, training %d)", what, a->mode,
+                a->training);
+  if (a->prenet_keep) return fail(T2_ERR_INVALID, "%s: row_seeds and prenet_keep exclude each other", what);
   return T2_OK;
-}
-
-// limits: evaluation- or training-mode INFER without a forced alignment, and a window of non-negative sides
-static int check_limits(const T2DecoderArgs* a, const T2DecoderLimits* lim, const char* what) {
-  if (!lim) return T2_OK;
-  if (a->forced_align) return fail(T2_ERR_INVALID, "%s: limits and forced_align exclude each other (the map decides the steps)", what);
-  if (a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "%s: limits need mode INFER (got %d)", what, a->mode);
-  if (lim->window_back < 0 || lim->window_front < 0)
-    return fail(T2_ERR_INVALID, "%s: attention window (%d, %d) has a negative side", what, lim->window_back, lim->window_front);
-  if (lim->window_front == 0 && lim->window_back != 0)
-    return fail(T2_ERR_INVALID, "%s: window_back = %d without a window (window_front = 0)", what, lim->window_back);
-  return T2_OK;
-}
-
-static int check_decoder_args(const T2Model* m, const T2DecoderArgs* a) {
-  if (!m || !a) return fail(T2_ERR_INVALID, "null model / args");
-  if (a->B <= 0 || a->B > kMaxBatch) return fail(T2_ERR_INVALID, "decoder: B=%d outside [1, %d]", a->B, kMaxBatch);
-  if (a->T_enc <= 0) return fail(T2_ERR_INVALID, "decoder: empty encoder memory (T_enc=%d)", a->T_enc);
-  if (a->n_steps_cap <= 0) return fail(T2_ERR_INVALID, "decoder: n_steps_cap=%d", a->n_steps_cap);
-  if (!a->memory || !a->mel || !a->gate || !a->align || !a->mel_lengths || !a->n_steps || !a->ws)
-    return fail(T2_ERR_INVALID, "decoder: null tensor pointer");
-  if (a->mode == T2_MODE_TEACHER && !a->teacher_prenet) return fail(T2_ERR_INVALID, "decoder: teacher mode needs teacher_prenet");
-  if (a->mode != T2_MODE_TEACHER && a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "decoder: bad mode %d", a->mode);
-  if (a->ws_bytes < decoder_ws_bytes(a->B, a->T_enc, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
-  T2_TRY(check_forced(a, "decoder"));
-  return check_row_seeds(a, "decoder");
 }
 
 }  // namespace t2
@@ -276,18 +260,21 @@ int t2_postnet_backward(T2Model* m, const T2PostnetBwdArgs* a, void* stream) {
 }
 
 size_t t2_decoder_workspace_bytes(const T2Model*, int32_t B, int32_t T_enc, int32_t cap) { return decoder_ws_bytes(B, T_enc, cap); }
-static int decoder_run(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, void* stream) {
-  T2_TRY(check_decoder_args(m, a));
-  T2_TRY(check_limits(a, lim, "decoder"));
+int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) {
+  T2_TRY(check_decoder_args(m, a, "decoder"));
+  if (!a->ws) return fail(T2_ERR_INVALID, "decoder: null tensor pointer");
+  if (a->mode == T2_MODE_TEACHER && !a->teacher_prenet) return fail(T2_ERR_INVALID, "decoder: teacher mode needs teacher_prenet");
+  if (a->mode != T2_MODE_TEACHER && a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "decoder: bad mode %d", a->mode);
+  if (a->ws_bytes < decoder_ws_bytes(a->B, a->T_enc, a->n_steps_cap)) return fail(T2_ERR_WORKSPACE, "decoder workspace too small");
   int impl = a->impl;
   if (impl == T2_IMPL_AUTO) impl = persistent_supported(m, a) ? T2_IMPL_PERSISTENT : T2_IMPL_STEPWISE;
   if (impl == T2_IMPL_PERSISTENT) {
     if (!persistent_supported(m, a))
       return fail(T2_ERR_UNSUPPORTED, "persistent decoder does not support T_enc=%d on this device (at most 2274, and >= 128 SMs)",
                   a->T_enc);
-    return decoder_run_persistent(m, a, lim, (cudaStream_t)stream);
+    return decoder_run_persistent(m, a, (cudaStream_t)stream);
   }
-  if (a->forced_align || lim)
+  if (a->forced_align || decoder_has_limits(a))
     return fail(T2_ERR_UNSUPPORTED, "decoder: %s needs the persistent implementation (%s)",
                 a->forced_align ? "a forced alignment" : "limits",
                 a->impl == T2_IMPL_STEPWISE ? "impl = STEPWISE was requested"
@@ -300,23 +287,16 @@ static int decoder_run(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits
                                             : "this shape / device does not fit it: T_enc too large for shared memory or < 128 SMs");
   return decoder_run_stepwise(m, a, (cudaStream_t)stream);
 }
-int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) { return decoder_run(m, a, nullptr, stream); }
-int t2_decoder_run_limited(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* limits, void* stream) {
-  return decoder_run(m, a, limits, stream);
-}
 
 size_t t2_decoder_stream_state_bytes(const T2Model*, int32_t B, int32_t T_enc) {
   return B > 0 && T_enc > 0 ? persistent_stream_state_bytes(B, T_enc) : 0;
 }
 
 static int check_stream_args(const T2Model* m, const T2DecoderStreamArgs* s) {
-  if (!m || !s) return fail(T2_ERR_INVALID, "decoder stream: null model / args");
+  if (!s) return fail(T2_ERR_INVALID, "decoder stream: null model / args");
   const T2DecoderArgs* a = &s->dec;
-  if (a->B <= 0 || a->B > kMaxBatch) return fail(T2_ERR_INVALID, "decoder stream: B=%d outside [1, %d]", a->B, kMaxBatch);
-  if (a->T_enc <= 0) return fail(T2_ERR_INVALID, "decoder stream: empty encoder memory (T_enc=%d)", a->T_enc);
-  if (a->n_steps_cap <= 0) return fail(T2_ERR_INVALID, "decoder stream: n_steps_cap=%d", a->n_steps_cap);
-  if (!a->memory || !a->mel || !a->gate || !a->align || !a->mel_lengths || !a->n_steps || !s->state || !s->status)
-    return fail(T2_ERR_INVALID, "decoder stream: null tensor pointer");
+  T2_TRY(check_decoder_args(m, a, "decoder stream"));
+  if (!s->state || !s->status) return fail(T2_ERR_INVALID, "decoder stream: null tensor pointer");
   if (a->mode != T2_MODE_INFER) return fail(T2_ERR_INVALID, "decoder stream: mode must be INFER (got %d)", a->mode);
   if (a->impl == T2_IMPL_STEPWISE)
     return fail(T2_ERR_UNSUPPORTED, "decoder stream: needs the persistent decoder, which resumes from saved state "
@@ -327,9 +307,7 @@ static int check_stream_args(const T2Model* m, const T2DecoderStreamArgs* s) {
                                     "(at most 2274, and >= 128 SMs)", a->T_enc);
   if (s->state_bytes < persistent_stream_state_bytes(a->B, a->T_enc)) return fail(T2_ERR_WORKSPACE, "decoder stream state too small");
   if (s->row_step0 && !a->row_seeds) return fail(T2_ERR_INVALID, "decoder stream: row_step0 needs dec.row_seeds");
-  T2_TRY(check_forced(a, "decoder stream"));
-  T2_TRY(check_limits(a, s->limits, "decoder stream"));
-  return check_row_seeds(a, "decoder stream");
+  return T2_OK;
 }
 
 int t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stream) {
@@ -340,8 +318,7 @@ int t2_decoder_stream_begin(T2Model* m, const T2DecoderStreamArgs* a, void* stre
 int t2_decoder_stream_run(T2Model* m, const T2DecoderStreamArgs* a, int32_t n_steps, const int32_t* status_host, void* stream) {
   T2_TRY(check_stream_args(m, a));
   if (n_steps < 1) return fail(T2_ERR_INVALID, "decoder stream: n_steps=%d (at least 1 step per run)", n_steps);
-  return persistent_stream_run(m, &a->dec, a->limits, a->state, a->status, n_steps, status_host, a->row_step0,
-                               (cudaStream_t)stream);
+  return persistent_stream_run(m, &a->dec, a->state, a->status, n_steps, status_host, a->row_step0, (cudaStream_t)stream);
 }
 
 int t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int32_t* rows, int32_t n_rows, void* stream) {
@@ -349,7 +326,7 @@ int t2_decoder_stream_admit(T2Model* m, const T2DecoderStreamArgs* a, const int3
   if (n_rows < 1 || n_rows > a->dec.B || !rows) return fail(T2_ERR_INVALID, "decoder stream admit: n_rows=%d outside [1, B=%d]", n_rows, a->dec.B);
   if (!a->dec.memory_lengths) return fail(T2_ERR_INVALID, "decoder stream admit: the stream has no memory_lengths");
   if (a->dec.forced_align) return fail(T2_ERR_INVALID, "decoder stream admit: continuous batching takes no forced alignment");
-  if (a->limits && a->limits->max_steps)
+  if (a->dec.max_steps)
     return fail(T2_ERR_INVALID, "decoder stream admit: limits.max_steps count the stream's absolute steps, which an admitted "
                                 "row does not share (continuous batching limits each request itself)");
   for (int i = 0; i < n_rows; ++i)
@@ -420,10 +397,10 @@ int t2_postnet_infer(T2Model* m, const T2PostnetArgs* a, void* stream) {
 struct InferWs {
   int64_t* text; float *memory, *mel, *gate, *align, *post; int32_t *lens, *nsteps;
   char* sub; size_t sub_bytes;   // the workspace of the encoder, the decoder and the postnet in turn
-  int32_t* in_lens;              // t2_infer_host_lengths: the input lengths (B)
-  uint64_t* row_seeds;           // t2_infer_host_lengths: the per-row prenet keys (B)
+  int32_t* in_lens;              // the input lengths (B), when given
+  uint64_t* row_seeds;           // the per-row prenet keys (B), when given
 };
-static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w, bool with_lengths = false) {
+static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w) {
   w->text = c.take<int64_t>((size_t)B * Tt);
   w->memory = c.take<float>((size_t)B * Tt * kEnc);
   w->mel = c.take<float>((size_t)B * S * kMel);
@@ -436,8 +413,8 @@ static void infer_layout(Carve& c, int B, int Tt, int S, InferWs* w, bool with_l
   if (decoder_ws_bytes(B, Tt, S) > sb) sb = decoder_ws_bytes(B, Tt, S);
   if (postnet_ws_bytes(B, S) > sb) sb = postnet_ws_bytes(B, S);
   w->sub = c.take<char>(sb); w->sub_bytes = sb;
-  w->in_lens = with_lengths ? c.take<int32_t>(B) : nullptr;
-  w->row_seeds = with_lengths ? c.take<uint64_t>(B) : nullptr;
+  w->in_lens = c.take<int32_t>(B);
+  w->row_seeds = c.take<uint64_t>(B);
 }
 
 size_t t2_infer_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32_t max_steps) {
@@ -447,27 +424,18 @@ size_t t2_infer_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32
   return c.bytes();
 }
 
-size_t t2_infer_lengths_workspace_bytes(const T2Model*, int32_t B, int32_t T_text, int32_t max_steps) {
-  Carve c(nullptr);
-  InferWs w;
-  infer_layout(c, B, T_text, max_steps, &w, true);
-  return c.bytes();
-}
-
-// Tacotron2.inference end to end; in_lens_host (B) or null: each row b is its first in_lens_host[b] symbols alone
-static int infer_host(T2Model* m, const int64_t* text_host, const int64_t* in_lens_host, int32_t B, int32_t T_text,
-                      int32_t max_steps, float gate_threshold, uint64_t seed, int32_t impl, float* mel_post_host,
-                      int32_t* mel_lengths_host, int32_t* n_steps_host, void* ws, size_t ws_bytes, cudaStream_t s,
-                      const uint64_t* row_seeds_host = nullptr) {
-  if (!m || !text_host || !mel_post_host || !mel_lengths_host || !n_steps_host || !ws)
+// Tacotron2.inference end to end; a->input_lengths_host (B) or null: each row b is its first input_lengths_host[b] symbols alone
+int t2_infer_host(T2Model* m, const T2InferArgs* a, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!m || !a || !a->text_host || !a->mel_post_host || !a->mel_lengths_host || !a->n_steps_host || !a->ws)
     return fail(T2_ERR_INVALID, "infer_host: null argument");
-  const bool with_lengths = in_lens_host != nullptr;
-  const size_t need = with_lengths ? t2_infer_lengths_workspace_bytes(m, B, T_text, max_steps)
-                                   : t2_infer_workspace_bytes(m, B, T_text, max_steps);
-  if (ws_bytes < need) return fail(T2_ERR_WORKSPACE, "infer workspace too small");
+  const int B = a->B, T_text = a->T_text, max_steps = a->max_steps;
+  const int64_t* in_lens_host = a->input_lengths_host;
+  if (a->row_seeds_host && !in_lens_host) return fail(T2_ERR_INVALID, "infer_host: row_seeds_host needs input_lengths_host");
+  if (a->ws_bytes < t2_infer_workspace_bytes(m, B, T_text, max_steps)) return fail(T2_ERR_WORKSPACE, "infer workspace too small");
   std::vector<int32_t> lens32;
   bool ragged = false;             // some text shorter than T_text: each row's postnet is its own B = 1 postnet
-  if (with_lengths) {              // checked here, before anything is enqueued
+  if (in_lens_host) {              // checked here, before anything is enqueued
     lens32.resize(B > 0 ? B : 0);
     for (int b = 0; b < B; ++b) {
       if (in_lens_host[b] < 1 || in_lens_host[b] > T_text)
@@ -476,34 +444,36 @@ static int infer_host(T2Model* m, const int64_t* text_host, const int64_t* in_le
       ragged |= lens32[b] < T_text;
     }
   }
-  Carve c(ws);
+  Carve c(a->ws);
   InferWs w;
-  infer_layout(c, B, T_text, max_steps, &w, with_lengths);
-  T2_CUDA(cudaMemcpyAsync(w.text, text_host, (size_t)B * T_text * 8, cudaMemcpyHostToDevice, s));
+  infer_layout(c, B, T_text, max_steps, &w);
+  T2_CUDA(cudaMemcpyAsync(w.text, a->text_host, (size_t)B * T_text * 8, cudaMemcpyHostToDevice, s));
   // pageable source: the call returns once lens32 has been staged, so the vector may go out of scope
-  if (with_lengths) T2_CUDA(cudaMemcpyAsync(w.in_lens, lens32.data(), (size_t)B * 4, cudaMemcpyHostToDevice, s));
-  if (row_seeds_host) T2_CUDA(cudaMemcpyAsync(w.row_seeds, row_seeds_host, (size_t)B * 8, cudaMemcpyHostToDevice, s));
+  if (in_lens_host) T2_CUDA(cudaMemcpyAsync(w.in_lens, lens32.data(), (size_t)B * 4, cudaMemcpyHostToDevice, s));
+  if (a->row_seeds_host) T2_CUDA(cudaMemcpyAsync(w.row_seeds, a->row_seeds_host, (size_t)B * 8, cudaMemcpyHostToDevice, s));
   T2EncoderArgs ea; memset(&ea, 0, sizeof(ea));
-  ea.text = w.text; ea.lengths = w.in_lens; ea.B = B; ea.T = T_text; ea.memory = w.memory; ea.ws = w.sub; ea.ws_bytes = w.sub_bytes;
+  ea.text = w.text; ea.lengths = in_lens_host ? w.in_lens : nullptr; ea.B = B; ea.T = T_text; ea.memory = w.memory;
+  ea.ws = w.sub; ea.ws_bytes = w.sub_bytes;
   T2_TRY(encoder_forward(m, &ea, s, true));
   T2DecoderArgs da; memset(&da, 0, sizeof(da));
-  da.mode = T2_MODE_INFER; da.impl = impl; da.memory = w.memory; da.memory_lengths = w.in_lens;
+  da.mode = T2_MODE_INFER; da.impl = a->impl; da.memory = w.memory; da.memory_lengths = ea.lengths;
   da.B = B; da.T_enc = T_text; da.n_steps_cap = max_steps;
-  da.seed = seed; da.gate_threshold = gate_threshold; da.score_mask_value = -INFINITY;
-  da.row_seeds = row_seeds_host ? w.row_seeds : nullptr;
+  da.seed = a->seed; da.gate_threshold = a->gate_threshold; da.score_mask_value = -INFINITY;
+  da.row_seeds = a->row_seeds_host ? w.row_seeds : nullptr;
   da.mel = w.mel; da.gate = w.gate; da.align = w.align; da.mel_lengths = w.lens; da.n_steps = w.nsteps; da.ws = w.sub; da.ws_bytes = w.sub_bytes;
   T2_TRY(t2_decoder_run(m, &da, s));
   // the postnet runs over the n decoded frames, as Tacotron2.inference does: its convolutions zero-pad every layer at
   // frame n, and a longer window would feed the last rows' final frames the activations of zero input instead
-  T2_CUDA(cudaMemcpyAsync(n_steps_host, w.nsteps, 4, cudaMemcpyDeviceToHost, s));
+  T2_CUDA(cudaMemcpyAsync(a->n_steps_host, w.nsteps, 4, cudaMemcpyDeviceToHost, s));
   T2_CUDA(cudaStreamSynchronize(s));
-  const int n = n_steps_host[0];
+  const int n = a->n_steps_host[0];
   if (n < 1 || n > max_steps) return fail(T2_ERR_CUDA, "infer_host: decoder reported %d steps", n);
   // frames beyond each row's length are zeroed (lengths mask); (B, 80, n) rows -> host rows of pitch max_steps
   T2PostnetArgs pa; memset(&pa, 0, sizeof(pa));
   pa.mel = w.mel; pa.mel_batch_stride = (long)max_steps * kMel; pa.lengths = w.lens; pa.add_residual = 1; pa.B = B; pa.T = n;
   pa.mel_post = w.post; pa.ws = w.sub; pa.ws_bytes = w.sub_bytes;
   T2_TRY(postnet_forward(m, &pa, s, ragged));
+  float* mel_post_host = a->mel_post_host;
   T2_CUDA(cudaMemcpy2DAsync(mel_post_host, (size_t)max_steps * 4, w.post, (size_t)n * 4, (size_t)n * 4, (size_t)B * kMel,
                             cudaMemcpyDeviceToHost, s));
   if (n < max_steps) {   // frames past the last step: zeros
@@ -512,24 +482,9 @@ static int infer_host(T2Model* m, const int64_t* text_host, const int64_t* in_le
     T2_CUDA(cudaMemcpy2DAsync(mel_post_host + n, (size_t)max_steps * 4, tail, (size_t)(max_steps - n) * 4,
                               (size_t)(max_steps - n) * 4, (size_t)B * kMel, cudaMemcpyDeviceToHost, s));
   }
-  T2_CUDA(cudaMemcpyAsync(mel_lengths_host, w.lens, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+  T2_CUDA(cudaMemcpyAsync(a->mel_lengths_host, w.lens, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
   T2_CUDA(cudaStreamSynchronize(s));
   return T2_OK;
-}
-
-int t2_infer_host(T2Model* m, const int64_t* text_host, int32_t B, int32_t T_text, int32_t max_steps,
-                  float gate_threshold, uint64_t seed, int32_t impl, float* mel_post_host,
-                  int32_t* mel_lengths_host, int32_t* n_steps_host, void* ws, size_t ws_bytes, void* stream) {
-  return infer_host(m, text_host, nullptr, B, T_text, max_steps, gate_threshold, seed, impl, mel_post_host, mel_lengths_host,
-                    n_steps_host, ws, ws_bytes, (cudaStream_t)stream);
-}
-
-int t2_infer_host_lengths(T2Model* m, const T2InferArgs* a, void* stream) {
-  if (!a) return fail(T2_ERR_INVALID, "infer_host_lengths: null args");
-  if (!a->input_lengths_host) return fail(T2_ERR_INVALID, "infer_host_lengths: null input_lengths_host (use t2_infer_host)");
-  return infer_host(m, a->text_host, a->input_lengths_host, a->B, a->T_text, a->max_steps, a->gate_threshold, a->seed, a->impl,
-                    a->mel_post_host, a->mel_lengths_host, a->n_steps_host, a->ws, a->ws_bytes, (cudaStream_t)stream,
-                    a->row_seeds_host);
 }
 
 int t2_decoder_profile(const T2DecoderArgs* a, int64_t* out_host) {

@@ -41,12 +41,15 @@ inline void decoder_stash_layout(Carve& c, int B, int T, DecoderStash* s) {
 }
 inline size_t decoder_stash_bytes(int B, int T) { Carve c(nullptr); DecoderStash s; decoder_stash_layout(c, B, T, &s); return c.bytes(); }
 
+// an attention window or per-row step limits are set (t2b200.h): the persistent kernel's limited instantiation runs
+inline bool decoder_has_limits(const T2DecoderArgs* a) { return a->window_front != 0 || a->window_back != 0 || a->max_steps; }
+
 // t2_decoder_workspace_bytes is the larger of the two implementations' layouts
 size_t stepwise_ws_bytes(int B, int T);
 size_t persistent_ws_bytes(int B, int T, int cap);
 DecoderCtrl* persistent_ws_ctrl(const T2DecoderArgs* a);   // the control block (and phase profile) of a persistent run
 int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
-int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, cudaStream_t s);   // lim: or null
+int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
 int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s);
 size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel);
 size_t prenet_backward_ws_bytes(int M);
@@ -55,8 +58,8 @@ bool persistent_supported(const T2Model* m, const T2DecoderArgs* a);
 // resumable persistent decoder (t2_decoder_stream_*): state = per 64-row slice, status = [steps run, stopped] per slice
 size_t persistent_stream_state_bytes(int B, int T_enc);
 int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, cudaStream_t s);
-int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, void* state, int32_t* status,
-                          int n, const int32_t* status_host, const int32_t* row_step0, cudaStream_t s);
+int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n, const int32_t* status_host,
+                          const int32_t* row_step0, cudaStream_t s);
 // continuous batching: rows (ascending) back to the state begin gives them + their processed memory; a chunk's frames of
 // the listed rows to the requests' own buffers
 int persistent_stream_admit(T2Model* m, const T2DecoderArgs* a, void* state, const int32_t* rows, int n_rows, cudaStream_t s);

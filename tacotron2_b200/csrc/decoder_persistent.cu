@@ -1321,9 +1321,9 @@ static int processed_memory(T2Model* m, const T2DecoderArgs* a, int b0, int nb, 
 }
 
 // the parameters of the launch over batch rows [b0, b0 + 64) (or to B) whose state is block `blk` of `buf`: the whole loop
-// [0, cap), no resume state; lim: the caller's limits or null
-static void slice_params(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, const SliceBuffer& buf,
-                         const SliceState& blk, int b0, KParams* pp) {
+// [0, cap), no resume state
+static void slice_params(T2Model* m, const T2DecoderArgs* a, const SliceBuffer& buf, const SliceState& blk, int b0,
+                         KParams* pp) {
   PersistentPack* pk = (PersistentPack*)m->pk;
   KParams& p = *pp;
   const int T = a->T_enc, cap = a->n_steps_cap;
@@ -1350,12 +1350,12 @@ static void slice_params(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimi
     p.forced_align = a->forced_align + (size_t)b0 * cap * T; p.forced_lengths = a->forced_lengths + b0;
     p.pa = nullptr;
   }
-  if (lim) {
+  if (decoder_has_limits(a)) {
     // a window wider than T_enc on either side masks nothing, so no window (window_front == 0) and overly wide ones run
     // as (T_enc, T_enc); this also keeps p + win_front inside int
-    p.win_back = lim->window_front == 0 || lim->window_back > T ? T : lim->window_back;
-    p.win_front = lim->window_front == 0 || lim->window_front > T ? T : lim->window_front;
-    p.max_steps = lim->max_steps ? lim->max_steps + b0 : nullptr;
+    p.win_back = a->window_front == 0 || a->window_back > T ? T : a->window_back;
+    p.win_front = a->window_front == 0 || a->window_front > T ? T : a->window_front;
+    p.max_steps = a->max_steps ? a->max_steps + b0 : nullptr;
   }
 }
 
@@ -1392,7 +1392,7 @@ static int launch_persistent(KParams& p, cudaStream_t s) {
   return T2_OK;
 }
 
-int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, cudaStream_t s) {
+int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
   const int cap = a->n_steps_cap;
   const bool infer = a->mode == T2_MODE_INFER;
   DecoderStash st;
@@ -1414,7 +1414,7 @@ int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, const T2DecoderLi
   // batch rows are independent: more than 64 rows run as consecutive launches of <= 64 rows on the one block
   for (int b0 = 0; b0 < a->B; b0 += kRows) {
     KParams p;
-    slice_params(m, a, lim, buf, blk, b0, &p);
+    slice_params(m, a, buf, blk, b0, &p);
     // counters, zero images and q (model.py:258-284): the block's regions before pa
     T2_CUDA(cudaMemsetAsync(blk.ctrl, 0, (uint8_t*)blk.pa - (uint8_t*)blk.ctrl, s));
     if (p.pa) T2_CUDA(cudaMemsetAsync(p.pa, 0, pa_buffer_floats(a->T_enc) * 4, s));   // zero attention weights -> pa = +0.0
@@ -1451,8 +1451,8 @@ int persistent_stream_begin(T2Model* m, const T2DecoderArgs* a, void* state, int
   return processed_memory(m, a, 0, a->B, stream_state(state, a->B, a->T_enc).pm, s);
 }
 
-int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, const T2DecoderLimits* lim, void* state, int32_t* status,
-                          int n, const int32_t* status_host, const int32_t* row_step0, cudaStream_t s) {
+int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, void* state, int32_t* status, int n, const int32_t* status_host,
+                          const int32_t* row_step0, cudaStream_t s) {
   const SliceBuffer buf = stream_state(state, a->B, a->T_enc);
   for (int b0 = 0, si = 0; b0 < a->B; b0 += kRows, ++si) {
     const int t0 = status_host ? status_host[2 * si] : 0;
@@ -1460,7 +1460,7 @@ int persistent_stream_run(T2Model* m, const T2DecoderArgs* a, const T2DecoderLim
     const SliceState blk = buf.block(si);
     T2_CUDA(cudaMemsetAsync(blk.ctrl, 0, sizeof(DecoderCtrl), s));   // everything else is zeroed by begin / admit
     KParams p;
-    slice_params(m, a, lim, buf, blk, b0, &p);                       // pa: left by the previous chunk
+    slice_params(m, a, buf, blk, b0, &p);                            // pa: left by the previous chunk
     p.t_begin = t0;
     p.t_end = n < a->n_steps_cap - t0 ? t0 + n : a->n_steps_cap;
     p.rs_acc = blk.acc; p.rs_cell = blk.cell; p.rs_att = blk.att; p.rs_done = blk.done; p.rs_status = status + 2 * si;

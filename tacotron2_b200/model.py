@@ -117,6 +117,12 @@ class _EngineOwner(object):
         eng.ensure(named, force=force)
         return eng
 
+    def _t2_device(self):
+        """The device of the module's parameters, the one its engine runs on (known without building the engine)."""
+        for p_ in self._t2_root().parameters():
+            return p_.device
+        return torch.device("cpu")
+
     def _t2_out_dtype(self):
         for p_ in self.parameters():
             return p_.dtype
@@ -138,31 +144,6 @@ def _require_no_grad(module, what):
 def _wants_grad(module, *tensors):
     return torch.is_grad_enabled() and (any(t is not None and t.requires_grad for t in tensors) or
                                         any(p_.requires_grad for p_ in module.parameters()))
-
-
-def _check_lengths(lengths, B, T, name):
-    """Per-row lengths of a ragged inference batch: (B,) integers, each in 1..T, on the host or the device.  Raises before
-    anything is launched; returns them as a tensor (None stays None)."""
-    if lengths is None:
-        return None
-    if not torch.is_tensor(lengths):
-        lengths = torch.as_tensor(lengths)
-    if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
-        raise TypeError("tacotron2_b200: %s must hold integers (got %s)" % (name, lengths.dtype))
-    if tuple(lengths.shape) != (B,):
-        raise ValueError("tacotron2_b200: %s must have shape (%d,) (got %s)" % (name, B, tuple(lengths.shape)))
-    host = lengths.cpu()
-    lo, hi = int(host.min()), int(host.max())
-    if lo < 1 or hi > T:
-        raise ValueError("tacotron2_b200: %s must lie in 1..%d (got %d..%d)" % (name, T, lo, hi))
-    return lengths
-
-
-def _ragged(lengths, T):
-    """Whether some text of the batch is shorter than T_text.  Then each row's postnet is its own B=1 postnet: every layer
-    is zero past the row's frame count.  An equal-length batch (no lengths, or all of them T_text) keeps the batched
-    postnet, whose hidden layers run over the zero frames past an early-stopping row's end (README "batched inference")."""
-    return lengths is not None and int(lengths.min()) < T
 
 
 def _require_no_grad_with_lengths(module, what):
@@ -346,7 +327,7 @@ class Encoder(_EngineOwner, nn.Module):
         input_lengths[b] is zero, as pad_packed_sequence leaves it."""
         if input_lengths is None:
             return self._run(x, None)
-        lengths = _check_lengths(input_lengths, x.size(0), x.size(2), "input_lengths")
+        lengths, _ = _engine_mod.row_lengths(input_lengths, x.size(0), x.size(2), "input_lengths", self._t2_device())
         _require_no_grad_with_lengths(self, "Encoder.inference")
         eng = self._t2_engine()
         out = eng.encoder(embedded=x.transpose(1, 2).detach(), lengths=lengths, training=False, per_row=True)
@@ -438,27 +419,6 @@ class Decoder(_EngineOwner, nn.Module):
             mel, gate, align, _ = self._teacher_forward(memory, decoder_inputs, memory_lengths, False)
         return mel.transpose(1, 2).to(dt), gate.to(dt), align.to(dt)
 
-    def _row_seeds(self, seeds, B, device, what):
-        """seeds (see inference) as the engine's per-row keys, or None; refused with masks and in training mode."""
-        if seeds is None:
-            return None
-        if self.training:
-            raise ValueError("tacotron2_b200: %s: seeds need eval mode (training-mode BatchNorm mixes the rows and the "
-                             "hidden-state dropout is not keyed per row)" % what)
-        if current_masks()["prenet"] is not None:
-            raise ValueError("tacotron2_b200: %s: seeds and injected prenet masks exclude each other" % what)
-        return _engine_mod.row_seeds(seeds, B, device, "tacotron2_b200: " + what)
-
-    def _forced(self, alignments, alignment_lengths, memory, device, what):
-        """alignments / alignment_lengths (see inference) as the engine's (map, lengths), or (None, None)."""
-        return _engine_mod.forced_alignment(alignments, alignment_lengths, memory.size(0), memory.size(1), device,
-                                            self.training, "tacotron2_b200: " + what)
-
-    def _limits(self, attention_window, max_decoder_steps, memory, device, forced, what):
-        """attention_window / max_decoder_steps (see inference) as the engine's (window, caps, longest)."""
-        return _engine_mod.decoder_limits(attention_window, max_decoder_steps, memory.size(0), device, forced,
-                                          "tacotron2_b200: " + what)
-
     def _warn_max_steps(self, lengths, gate, n, caps):
         """model.py:445-447 after a free run of n steps: the warning, once, if a row stopped at its step limit without its
         gate firing at that step.  Without caps the limit is max_decoder_steps (the reference's B = 1 rule over the whole
@@ -502,51 +462,54 @@ class Decoder(_EngineOwner, nn.Module):
         max_decoder_steps[b] steps, whichever comes first, and the run ends when every row has stopped (injected masks are
         (max of them, 2, B, 256)); None: self.max_decoder_steps for every row.  Row b equals bit for bit its own B = 1
         call with self.max_decoder_steps = max_decoder_steps[b] and the same window.  Neither goes with alignments."""
-        memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
+        opts = self._options("Decoder.inference", memory, "memory_lengths", memory_lengths, seeds, alignments,
+                             alignment_lengths, attention_window, max_decoder_steps)
+        return self._inference(memory, opts)
+
+    def _options(self, what, x, lengths_name, lengths, seeds, alignments, alignment_lengths, attention_window,
+                 max_decoder_steps):
+        """The options of an inference call over x (B, T_enc, ...) checked once, in the engine's form."""
+        return _engine_mod.inference_options(
+            what, x.size(0), x.size(1), self._t2_device(), training=self.training,
+            prenet_masks=current_masks()["prenet"] is not None, lengths=lengths, lengths_name=lengths_name, seeds=seeds,
+            alignments=alignments, alignment_lengths=alignment_lengths, attention_window=attention_window,
+            max_decoder_steps=max_decoder_steps)
+
+    def _inference(self, memory, opts):
+        """inference() with its options already in the engine's form (an _engine.InferenceOptions)."""
         eng = self._t2_engine()
-        row_seeds = self._row_seeds(seeds, memory.size(0), eng.device, "Decoder.inference")
-        fa, fl = self._forced(alignments, alignment_lengths, memory, eng.device, "Decoder.inference")
-        window, caps, longest = self._limits(attention_window, max_decoder_steps, memory, eng.device, fa is not None,
-                                             "Decoder.inference")
         masks = current_masks()
         mel, gate, align, lengths, n_steps = eng.decoder(
-            memory, _capi.MODE_INFER, fa.size(1) if fa is not None else (longest or self.max_decoder_steps),
-            memory_lengths=memory_lengths, training=self.training, prenet_keep=masks["prenet"],
-            att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold, row_seeds=row_seeds,
-            forced_align=fa, forced_lengths=fl, window=window, max_steps=caps)
+            memory, _capi.MODE_INFER, opts.cap or self.max_decoder_steps, training=self.training,
+            prenet_keep=masks["prenet"], att_keep=masks["att"], dec_keep=masks["dec"], gate_threshold=self.gate_threshold,
+            **opts.decoder_kwargs())
         n = int(n_steps.item())                      # the one host sync of the whole loop (model.py:443 syncs every step)
         self.mel_lengths = lengths
-        if fa is None:
-            self._warn_max_steps(lengths, gate, n, caps)
+        if opts.forced_align is None:
+            self._warn_max_steps(lengths, gate, n, opts.max_steps)
         dt = memory.dtype
         return (mel[:, :n].transpose(1, 2).to(dt), gate[:, :n].unsqueeze(-1).to(dt), align[:, :n].to(dt))
 
-    def _stream_chunks(self, memory, chunk_steps, halo, memory_lengths=None, row_seeds=None, forced=(None, None),
-                       limits=(None, None, None)):
+    def _stream_chunks(self, memory, chunk_steps, halo, opts):
         """The persistent decoder in chunks of chunk_steps steps.  Yields (t0, t1, finished, stream): frames [t0, t1) are
         the new ones that every row has produced and that no frame within `halo` steps of them can still change, i.e. all
         frames up to the steps run less `halo` while any row is live, and all of them once every 64-row slice has
-        stopped.  Before the last tuple, self.mel_lengths and the max-steps warning are set as by inference().  forced:
-        the engine's (map, lengths) of a forced run, whose map decides the steps; limits: the engine's (window, caps,
-        longest) of a limited one."""
+        stopped.  Before the last tuple, self.mel_lengths and the max-steps warning are set as by inference().  opts: the
+        run's options in the engine's form (an _engine.InferenceOptions)."""
         chunk_steps = int(chunk_steps)
         if chunk_steps < 1:
             raise ValueError("tacotron2_b200: chunk_steps must be >= 1 (got %d)" % chunk_steps)
         eng = self._t2_engine()
-        fa, fl = forced
-        window, caps, longest = limits
-        st = eng.decoder_stream(memory, fa.size(1) if fa is not None else (longest or self.max_decoder_steps),
-                                prenet_keep=current_masks()["prenet"], gate_threshold=self.gate_threshold,
-                                memory_lengths=memory_lengths, row_seeds=row_seeds, forced_align=fa, forced_lengths=fl,
-                                window=window, max_steps=caps)
+        st = eng.decoder_stream(memory, opts.cap or self.max_decoder_steps, prenet_keep=current_masks()["prenet"],
+                                gate_threshold=self.gate_threshold, **opts.decoder_kwargs())
         t0 = 0
         while True:
             live_steps, n, finished = st.run(chunk_steps)
             t1 = n if finished else max(t0, live_steps - halo)
             if finished:
                 self.mel_lengths = st.mel_lengths
-                if fa is None:                                                                  # as inference()
-                    self._warn_max_steps(st.mel_lengths, st.gate, n, caps)
+                if opts.forced_align is None:                                                   # as inference()
+                    self._warn_max_steps(st.mel_lengths, st.gate, n, opts.max_steps)
             if t1 > t0 or finished:
                 yield t0, t1, finished, st
             if finished:
@@ -565,14 +528,10 @@ class Decoder(_EngineOwner, nn.Module):
         if self.training:
             raise RuntimeError("tacotron2_b200: Decoder.inference_stream needs eval mode (in training mode inference() "
                                "applies the attention / decoder dropout, which the resumable decoder does not)")
-        memory_lengths = _check_lengths(memory_lengths, memory.size(0), memory.size(1), "memory_lengths")
-        row_seeds = self._row_seeds(seeds, memory.size(0), self._t2_engine().device, "Decoder.inference_stream")
-        forced = self._forced(alignments, alignment_lengths, memory, self._t2_engine().device, "Decoder.inference_stream")
-        limits = self._limits(attention_window, max_decoder_steps, memory, self._t2_engine().device, forced[0] is not None,
-                              "Decoder.inference_stream")
+        opts = self._options("Decoder.inference_stream", memory, "memory_lengths", memory_lengths, seeds, alignments,
+                             alignment_lengths, attention_window, max_decoder_steps)
         dt = memory.dtype
-        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, memory_lengths, row_seeds, forced,
-                                                        limits):
+        for t0, t1, finished, st in self._stream_chunks(memory, chunk_steps, 0, opts):
             yield dict(frames=(t0, t1), mel_outputs=st.mel[:, t0:t1].transpose(1, 2).to(dt),
                        gate_outputs=st.gate[:, t0:t1].unsqueeze(-1).to(dt), alignments=st.align[:, t0:t1].to(dt),
                        mel_lengths=st.mel_lengths.clone(), finished=finished)
@@ -736,19 +695,13 @@ class Tacotron2(_EngineOwner, nn.Module):
         out-of-domain text (README "robust synthesis"; Decoder.inference has the contract).  Row b then equals
         ``inference(inputs[b:b+1, :L_b], attention_window=w)`` with ``decoder.max_decoder_steps = max_decoder_steps[b]``
         bit for bit.  Neither goes with alignments."""
-        lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
+        opts = self.decoder._options("Tacotron2.inference", inputs, "input_lengths", input_lengths, seeds, alignments,
+                                     alignment_lengths, attention_window, max_decoder_steps)
         eng = self._t2_engine()
-        row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference")
-        fa, fl = _engine_mod.forced_alignment(alignments, alignment_lengths, inputs.size(0), inputs.size(1), eng.device,
-                                              self.training, "tacotron2_b200: Tacotron2.inference")
-        window, caps, _ = _engine_mod.decoder_limits(attention_window, max_decoder_steps, inputs.size(0), eng.device,
-                                                     fa is not None, "tacotron2_b200: Tacotron2.inference")
-        memory = eng.encoder(text=inputs, lengths=lengths_in, training=self.training, keep=current_masks()["enc"],
-                             per_row=lengths_in is not None)
+        memory = eng.encoder(text=inputs, lengths=opts.lengths, training=self.training, keep=current_masks()["enc"],
+                             per_row=opts.lengths is not None)
         memory = memory.to(self._t2_out_dtype())     # a .half() model hands half tensors between its modules (ipynb:89-90)
-        mel_outputs, gate_outputs, alignments = self.decoder.inference(memory, memory_lengths=lengths_in, seeds=row_seeds,
-                                                                       alignments=fa, alignment_lengths=fl,
-                                                                       attention_window=window, max_decoder_steps=caps)
+        mel_outputs, gate_outputs, alignments = self.decoder._inference(memory, opts)
         lengths = self.decoder.mel_lengths
         self.mel_lengths = lengths
         mel_btc = mel_outputs.transpose(1, 2)
@@ -758,7 +711,7 @@ class Tacotron2(_EngineOwner, nn.Module):
         # a forced run knows its lengths before it runs: every row's postnet is its own, as for a ragged batch
         mel_outputs_postnet = eng.postnet(mel_btc, lengths if multi else None, True, self.training,
                                           current_masks()["post"],
-                                          per_row=_ragged(lengths_in, inputs.size(1)) or (fa is not None and multi)
+                                          per_row=opts.ragged or (opts.forced_align is not None and multi)
                                           ).to(mel_outputs.dtype)
         if multi:
             pad = ~get_mask_from_lengths(lengths.long(), mel_outputs.size(2))
@@ -782,22 +735,17 @@ class Tacotron2(_EngineOwner, nn.Module):
         if self.training:
             raise RuntimeError("tacotron2_b200: inference_stream needs eval mode (training-mode BatchNorm uses the statistics "
                                "of the whole sequence, so no postnet frame is final before the decoder ends)")
-        lengths_in = _check_lengths(input_lengths, inputs.size(0), inputs.size(1), "input_lengths")
+        opts = self.decoder._options("Tacotron2.inference_stream", inputs, "input_lengths", input_lengths, seeds,
+                                     alignments, alignment_lengths, attention_window, max_decoder_steps)
         eng = self._t2_engine()
-        row_seeds = self.decoder._row_seeds(seeds, inputs.size(0), eng.device, "Tacotron2.inference_stream")
-        forced = _engine_mod.forced_alignment(alignments, alignment_lengths, inputs.size(0), inputs.size(1), eng.device,
-                                              False, "tacotron2_b200: Tacotron2.inference_stream")
-        limits = _engine_mod.decoder_limits(attention_window, max_decoder_steps, inputs.size(0), eng.device,
-                                            forced[0] is not None, "tacotron2_b200: Tacotron2.inference_stream")
-        memory = eng.encoder(text=inputs, lengths=lengths_in, training=False, keep=current_masks()["enc"],
-                             per_row=lengths_in is not None)
+        memory = eng.encoder(text=inputs, lengths=opts.lengths, training=False, keep=current_masks()["enc"],
+                             per_row=opts.lengths is not None)
         dt = self._t2_out_dtype()
         memory = memory.to(dt)
         multi = inputs.size(0) > 1
-        ragged = _ragged(lengths_in, inputs.size(1)) or (forced[0] is not None and multi)     # as inference()
+        ragged = opts.ragged or (opts.forced_align is not None and multi)     # as inference()
         halo = POSTNET_HALO
-        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, lengths_in, row_seeds, forced,
-                                                                limits):
+        for t0, t1, finished, st in self.decoder._stream_chunks(memory, chunk_steps, halo, opts):
             if finished:
                 self.mel_lengths = st.mel_lengths
             lengths = st.mel_lengths
@@ -840,8 +788,8 @@ class Tacotron2(_EngineOwner, nn.Module):
         if self.training:
             raise RuntimeError("tacotron2_b200: inference_server needs eval mode (training-mode BatchNorm uses the statistics "
                                "of the whole sequence, so no postnet frame is final before the decoder ends)")
-        window = _engine_mod.decoder_limits(attention_window, None, 1, torch.device("cpu"), False,
-                                            "tacotron2_b200: inference_server")[0]
+        window = _engine_mod.inference_options("inference_server", 1, 1, torch.device("cpu"),
+                                               attention_window=attention_window).window
         server = InferenceServer(None, slots, max_text_len, chunk_steps, self.decoder.max_decoder_steps)
         server.backend = EngineBackend(self, server.slots, server.max_text_len, server.chunk_steps, seed, window)
         return server
@@ -852,20 +800,19 @@ class Tacotron2(_EngineOwner, nn.Module):
         max_text_len: default the longest text; max_decoder_steps: one limit for all, or one per text.  seeds: one per text
         (as for inference()); result i then equals ``inference(texts[i][None], seeds=[seeds[i]])`` bit for bit.
         attention_window: one window for every text (see inference_server)."""
-        window = _engine_mod.decoder_limits(attention_window, None, 1, torch.device("cpu"), False,
-                                            "tacotron2_b200: inference_many")[0]
         texts = list(texts)
+        opts = _engine_mod.inference_options("inference_many", len(texts), 1, torch.device("cpu"), seeds=seeds,
+                                             attention_window=attention_window)
         if not texts:
             return []
         if max_text_len is None:
             max_text_len = max(int(torch.as_tensor(t).numel()) for t in texts)
         limits = max_decoder_steps if isinstance(max_decoder_steps, (list, tuple)) else [max_decoder_steps] * len(texts)
         per_text = [None] * len(texts)
-        if seeds is not None:       # checked before anything runs; the server takes each as a Python int
-            bits = _engine_mod.row_seeds(seeds, len(texts), torch.device("cpu"), "tacotron2_b200: inference_many")
-            per_text = [int(v) & 0xFFFFFFFFFFFFFFFF for v in bits.tolist()]
+        if opts.row_seeds is not None:      # the server takes each as a Python int
+            per_text = [int(v) & 0xFFFFFFFFFFFFFFFF for v in opts.row_seeds.tolist()]
         server = self.inference_server(min(int(slots), len(texts)), max(1, max_text_len), chunk_steps,
-                                       attention_window=window)
+                                       attention_window=opts.window)
         ids = [server.submit(t, limit, seed=sd) for t, limit, sd in zip(texts, limits, per_text)]
         results = {r["id"]: r for r in server.run()}
         return [results[i] for i in ids]

@@ -17,6 +17,8 @@ import numbers
 
 import torch
 
+from ._engine import seed_pattern
+
 WARNING = "Warning! Reached max decoder steps"      # the line Decoder.inference prints (model.py:446)
 
 
@@ -104,8 +106,7 @@ class InferenceServer:
             if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
                 raise TypeError("tacotron2_b200: seed must be an integer (got %r)" % (seed,))
             seed = int(seed)
-            if not 0 <= seed < 1 << 64:
-                raise ValueError("tacotron2_b200: seed %d is outside [0, 2**64)" % seed)
+            seed_pattern(seed, "tacotron2_b200")
             if prenet_keep is not None:
                 raise ValueError("tacotron2_b200: seed and prenet_keep exclude each other")
         if self.seeded is None:
@@ -248,7 +249,7 @@ class EngineBackend:
         step0 = None
         if row_seeds is not None:
             seeds, steps = row_seeds
-            self.row_seeds.copy_(torch.tensor([v - (1 << 64) if v >= 1 << 63 else v for v in seeds], dtype=torch.int64))
+            self.row_seeds.copy_(torch.tensor([seed_pattern(v, "tacotron2_b200") for v in seeds], dtype=torch.int64))
             self.row_step0.copy_(torch.tensor(steps, dtype=torch.int32))
             step0 = self.row_step0
         st.args.dec.row_seeds = self.row_seeds.data_ptr() if row_seeds is not None else None

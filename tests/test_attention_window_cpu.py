@@ -1,20 +1,11 @@
-"""Constrained synthesis without a GPU: the C layout of ``T2DecoderLimits`` and of the grown ``T2DecoderStreamArgs``,
-the host-side checks of ``attention_window`` / ``max_decoder_steps``, and ``window_ranges``, the reference of the window
-that the GPU tests (tests/test_gpu_attention_window.py) check the engine's alignments against."""
-import ctypes
-import os
-import subprocess
-
+"""Constrained synthesis without a GPU: the host-side checks of ``attention_window`` / ``max_decoder_steps``, how they
+reach the decoder's arguments, and ``window_ranges``, the reference of the window that the GPU tests
+(tests/test_gpu_attention_window.py) check the engine's alignments against."""
 import pytest
 import torch
 
-from tacotron2_b200 import _capi, _engine
-from tests.common import ROOT
+from tacotron2_b200 import _engine
 
-FIELDS = {
-    "T2DecoderLimits": ["window_back", "window_front", "max_steps"],
-    "T2DecoderStreamArgs": ["dec", "state", "state_bytes", "status", "row_step0", "limits"],
-}
 CPU = torch.device("cpu")
 
 
@@ -32,36 +23,13 @@ def window_ranges(align, lengths, window):
     return (p - back).clamp(min=0), torch.minimum(p + front, lengths[:, None])
 
 
-def test_limit_fields_match_c_layout(tmp_path):
-    """sizeof / offsetof as gcc sees the header == the ctypes mirror; T2DecoderStreamArgs grows by the limits pointer at
-    its end, so none of its earlier fields move."""
-    src = tmp_path / "layout.c"
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "t2b200.h"', 'int main(void){']
-    for s, fs in FIELDS.items():
-        lines.append('printf("%s %%zu\\n", sizeof(%s));' % (s, s))
-        for f in fs:
-            lines.append('printf("%s.%s %%zu\\n", offsetof(%s, %s));' % (s, f, s, f))
-    lines.append('return 0;}')
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    out = dict(line.split() for line in subprocess.check_output([str(exe)]).decode().splitlines())
-    for s, fs in FIELDS.items():
-        cls = getattr(_capi, s)
-        assert int(out[s]) == ctypes.sizeof(cls), s
-        for f in fs:
-            assert int(out["%s.%s" % (s, f)]) == getattr(cls, f).offset, (s, f)
-    S = _capi.T2DecoderStreamArgs
-    assert S.limits.offset == S.row_step0.offset + 8 and ctypes.sizeof(S) == S.limits.offset + 8
-    assert ctypes.sizeof(_capi.T2DecoderLimits) == 16
-    assert "t2_decoder_run_limited" in _capi.EXPORTS
-
-
 def check(window=None, caps=None, B=3, forced=False):
-    return _engine.decoder_limits(window, caps, B, CPU, forced, "t")
+    amap = torch.zeros(B, 2, 4) if forced else None
+    opts = _engine.inference_options("t", B, 4, CPU, alignments=amap, attention_window=window, max_decoder_steps=caps)
+    return opts.window, opts.max_steps, None if opts.max_steps is None else opts.cap
 
 
-def test_valid_limits_are_taken_as_the_engine_wants_them():
+def test_builder_takes_valid_limits_as_the_decoder_wants_them():
     assert check() == (None, None, None)
     assert check((1, 3)) == ((1, 3), None, None)
     assert check([0, 1])[0] == (0, 1)
@@ -71,11 +39,13 @@ def test_valid_limits_are_taken_as_the_engine_wants_them():
         window, got, longest = check(None, caps)
         assert window is None and got.dtype == torch.int32 and got.is_contiguous() and got.tolist() == want
         assert longest == max(want)
-    lim = _engine.limits_struct((2, 5), torch.tensor([3, 4], dtype=torch.int32))
-    assert (lim.window_back, lim.window_front) == (2, 5) and lim.max_steps
-    lim = _engine.limits_struct(None, torch.tensor([3], dtype=torch.int32))
-    assert (lim.window_back, lim.window_front) == (0, 0)
-    assert _engine.limits_struct(None, None) is None
+    caps = torch.tensor([3, 4], dtype=torch.int32)
+    a = _engine.decoder_args(window=(2, 5), max_steps=caps)
+    assert (a.window_back, a.window_front, a.max_steps) == (2, 5, caps.data_ptr())
+    a = _engine.decoder_args(window=None, max_steps=caps[:1])
+    assert (a.window_back, a.window_front) == (0, 0) and a.max_steps
+    a = _engine.decoder_args(window=None, max_steps=None)
+    assert (a.window_back, a.window_front, a.max_steps) == (0, 0, None)      # zeroed: no limits
 
 
 @pytest.mark.parametrize("window,caps,forced,err,match", [
@@ -97,7 +67,7 @@ def test_valid_limits_are_taken_as_the_engine_wants_them():
     (None, 4.0, False, TypeError, "max_decoder_steps must hold integers"),
     (None, torch.ones(3, dtype=torch.bool), False, TypeError, "max_decoder_steps must hold integers"),
 ])
-def test_bad_limits_are_refused(window, caps, forced, err, match):
+def test_builder_refuses_bad_limits(window, caps, forced, err, match):
     with pytest.raises(err, match=match):
         check(window, caps, forced=forced)
 

@@ -79,7 +79,7 @@ def test_product_path_needs_cuda():
         model.inference(torch.zeros(1, 5, dtype=torch.long))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_at_abi_version_2():
     _ensure_built()
     header = open(os.path.join(ROOT, "include", "t2b200.h")).read()
     declared = set(re.findall(r"\b(t2_[a-z0-9_]+)\s*\(", header))
@@ -94,57 +94,49 @@ def test_library_exports_every_declared_symbol():
     S = _capi.selftest_lib()               # ... the self-test build of the same sources does
     for name in declared:
         assert hasattr(S, name), name
-    assert L.t2_abi_version() == 1
+    assert L.t2_abi_version() == 2
+
+
+def _mirror_fields(cls, prefix=""):
+    """(member designator, byte offset, ctypes type) of every field of a ctypes struct, nested structs' fields included."""
+    out = []
+    for name, ctype in cls._fields_:
+        off = getattr(cls, name).offset
+        out.append((prefix + name, off, ctype))
+        if isinstance(ctype, type) and issubclass(ctype, ctypes.Structure):
+            out += [(d, off + o, t) for d, o, t in _mirror_fields(ctype, prefix + name + ".")]
+    return out
 
 
 def test_ctypes_structs_match_c_layout(tmp_path):
-    """sizeof/offsetof of every args struct as gcc sees the header == the ctypes mirror."""
-    src = tmp_path / "layout.c"
-    fields = {
-        "T2Config": ["n_mel_channels", "postnet_n_convolutions", "p_attention_dropout", "bn_eps"],
-        "T2EncoderArgs": ["text", "embedded", "lengths", "B", "T", "training", "keep", "seed", "memory", "ws", "ws_bytes",
-                          "stash", "stash_bytes"],
-        "T2EncoderBwdArgs": ["text", "embedded", "lengths", "B", "T", "training", "keep", "seed", "stash", "stash_bytes",
-                             "d_memory", "d_embedded", "grads", "n_grads", "ws", "ws_bytes"],
-        "T2PostnetBwdArgs": ["B", "T", "training", "add_residual", "keep", "seed", "wgrad_lengths", "stash", "stash_bytes",
-                             "d_mel_post", "d_mel", "grads", "n_grads", "ws", "ws_bytes"],
-        "T2DecoderArgs": ["mode", "impl", "training", "memory", "memory_lengths", "B", "T_enc", "n_steps_cap",
-                          "teacher_prenet", "prenet_keep", "att_keep", "dec_keep", "seed", "gate_threshold",
-                          "score_mask_value", "mel", "gate", "align", "mel_lengths", "n_steps", "ws", "ws_bytes",
-                          "stash", "stash_bytes"],
-        "T2DecoderBwdArgs": ["memory", "memory_lengths", "B", "T_enc", "T_mel", "training", "teacher_prenet", "att_keep",
-                             "dec_keep", "seed", "score_mask_value", "align", "stash", "stash_bytes", "d_mel", "d_gate",
-                             "d_align", "d_memory", "d_prenet", "grads", "n_grads", "ws", "ws_bytes"],
-        "T2PrenetBwdArgs": ["frames", "M", "keep", "seed", "d_out", "grads", "n_grads", "ws", "ws_bytes"],
-        "T2AdamArgs": ["n", "params", "grads", "exp_avg", "exp_avg_sq", "numel", "lr", "beta1", "beta2", "eps", "weight_decay",
-                       "max_norm", "step", "grad_norm", "ws", "ws_bytes"],
-        "T2PostnetArgs": ["mel", "mel_batch_stride", "lengths", "B", "T", "training", "keep", "seed",
-                          "add_residual", "mel_post", "ws", "ws_bytes", "stash", "stash_bytes"],
-        "T2AmpAdamArgs": ["n", "model_params", "param_is_half", "grads", "grad_is_half", "master", "exp_avg", "exp_avg_sq", "numel",
-                          "lr", "beta1", "beta2", "eps", "weight_decay", "max_norm", "growth_interval", "growth_factor",
-                          "backoff_factor", "state", "grad_norm", "skipped", "ws", "ws_bytes"],
-        "T2LossArgs": ["mel", "mel_post", "gate", "mel_target", "gate_target", "output_lengths", "B", "C", "T", "loss", "d_mel",
-                       "d_mel_post", "d_gate", "ws", "ws_bytes"],
-        "T2MelSpecArgs": ["y", "B", "n_samples", "filter_length", "hop_length", "n_mel", "forward_basis", "mel_basis", "clip_val",
-                          "mel", "ws", "ws_bytes"],
-        "T2CollateArgs": ["text_flat", "text_offsets", "mel_flat", "mel_offsets", "B", "n_mel", "T_max", "L_pad", "order",
-                          "text_padded", "input_lengths", "mel_padded", "gate_padded", "output_lengths"],
-    }
+    """Every ctypes struct of _capi and every field of it, nested structs included, has the sizeof / offsetof gcc gives
+    include/t2b200.h; every EXPORTS name is declared there, and every t2_* function declared outside T2_SELFTEST is in
+    EXPORTS."""
+    structs = [c for c in vars(_capi).values()
+               if isinstance(c, type) and issubclass(c, ctypes.Structure) and c.__module__ == _capi.__name__]
+    assert len(structs) >= 20
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "t2b200.h"', 'int main(void){']
-    for s, fs in fields.items():
+    for cls in structs:
+        s = cls.__name__
         lines.append('printf("%s %%zu\\n", sizeof(%s));' % (s, s))
-        for f in fs:
-            lines.append('printf("%s.%s %%zu\\n", offsetof(%s, %s));' % (s, f, s, f))
+        for d, _, t in _mirror_fields(cls):
+            lines.append('printf("%s.%s %%zu %%zu\\n", offsetof(%s, %s), sizeof(((%s*)0)->%s));' % (s, d, s, d, s, d))
     lines.append('return 0;}')
+    src = tmp_path / "layout.c"
     src.write_text("\n".join(lines))
     exe = tmp_path / "layout"
     subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    out = dict(l.split() for l in subprocess.check_output([str(exe)]).decode().splitlines())
-    for s, fs in fields.items():
-        cls = getattr(_capi, s)
+    out = dict(l.split(" ", 1) for l in subprocess.check_output([str(exe)]).decode().splitlines())
+    for cls in structs:
+        s = cls.__name__
         assert int(out[s]) == ctypes.sizeof(cls), s
-        for f in fs:
-            assert int(out["%s.%s" % (s, f)]) == getattr(cls, f).offset, (s, f)
+        for d, off, t in _mirror_fields(cls):
+            assert out["%s.%s" % (s, d)].split() == [str(off), str(ctypes.sizeof(t))], (s, d)
+    header = open(os.path.join(ROOT, "include", "t2b200.h")).read()
+    product = re.sub(r"#ifdef T2_SELFTEST.*?#endif", "", header, flags=re.S)
+    declared = set(re.findall(r"\b(t2_[a-z0-9_]+)\s*\(", product))
+    assert set(_capi.EXPORTS) <= declared, set(_capi.EXPORTS) - declared
+    assert declared <= set(_capi.EXPORTS), declared - set(_capi.EXPORTS)
 
 
 def test_text_mel_collate_matches_reference_semantics():

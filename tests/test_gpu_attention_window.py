@@ -303,7 +303,7 @@ def test_bad_arguments_are_refused_before_any_launch():
 
 
 def test_library_refuses_invalid_limited_calls():
-    """t2_decoder_run_limited: limits with forced_align, TEACHER, a negative window side or a back without a window ->
+    """t2_decoder_run with limits: limits with forced_align, TEACHER, a negative window side or a back without a window ->
     T2_ERR_INVALID; the stepwise implementation, requested or chosen by AUTO -> T2_ERR_UNSUPPORTED.  The stream refuses
     the same, and admit refuses step limits."""
     model = _model()

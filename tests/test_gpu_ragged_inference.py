@@ -232,8 +232,8 @@ def test_stream_to_audio_equals_each_rows_own_text_to_audio():
 # 5. the host entry point and the refusals
 # ---------------------------------------------------------------------------------------------------------------------
 def test_infer_host_lengths_equals_inference():
-    """t2_infer_host_lengths takes a Philox seed rather than masks: inference() draws one seed per call it makes (encoder,
-    decoder, postnet), so with the counter reset the decoder's is the second."""
+    """t2_infer_host with input_lengths_host takes a Philox seed rather than masks: inference() draws one seed per call it
+    makes (encoder, decoder, postnet), so with the counter reset the decoder's is the second."""
     from tacotron2_b200 import _engine
     lengths, S = [30, 3, 17], 24
     text = ragged_text(lengths, 91)
@@ -270,4 +270,46 @@ def test_bad_lengths_are_refused_before_any_launch():
     out = (mel, torch.empty(3, dtype=torch.int32).pin_memory(), torch.empty(1, dtype=torch.int32).pin_memory())
     with pytest.raises(_capi.T2Error, match="outside"):
         eng.infer_host(text.cpu().pin_memory(), 4, out_host=out, input_lengths_host=torch.tensor([3, 0, 5]).pin_memory())
+    with pytest.raises(_capi.T2Error, match="error -1: .*row_seeds_host needs input_lengths_host"):
+        eng.infer_host(text.cpu().pin_memory(), 4, out_host=out, row_seeds_host=torch.tensor([1, 2, 3]))
     assert _capi.lib().t2_kernel_launch_count() == before
+
+
+def _count_syncs(fn):
+    """fn() under torch's sync debug mode: (its result, the synchronising calls, those made from tacotron2_b200/_engine.py
+    -- where the inference options are checked)."""
+    import warnings
+    with warnings.catch_warnings(record=True) as caught:
+        warnings.simplefilter("always")
+        torch.cuda.set_sync_debug_mode("warn")
+        try:
+            out = fn()
+        finally:
+            torch.cuda.set_sync_debug_mode(0)
+    syncs = [w for w in caught if "synchroniz" in str(w.message)]
+    return out, len(syncs), sum(os.path.basename(w.filename) == "_engine.py" for w in syncs)
+
+
+def test_options_are_checked_once_and_read_back_once(monkeypatch):
+    """Tacotron2.inference with device-side input_lengths, seeds and max_decoder_steps (or alignments with
+    alignment_lengths) checks its options in one builder call and reads each device-side option back to the host once."""
+    from tacotron2_b200 import _engine
+    B, T, S = 3, 20, 12
+    model = make_model(synth_state_dict(7, gate_bias=-10.0), S)
+    text = rand_text(B, T, 5).cuda()
+    lengths = torch.tensor([20, 7, 13], device="cuda")
+    seeds = torch.tensor([5, 6, 7], device="cuda")
+    caps = torch.tensor([4, 9, 12], device="cuda", dtype=torch.int32)
+    amap = torch.rand(B, 6, T, device="cuda")
+    alens = torch.tensor([6, 2, 5], device="cuda")
+    calls = []
+    build = _engine.inference_options
+    monkeypatch.setattr(_engine, "inference_options", lambda *a, **k: calls.append(a[0]) or build(*a, **k))
+    with torch.no_grad():
+        model.inference(text, input_lengths=lengths, seeds=seeds, max_decoder_steps=caps)      # warm-up: packs weights
+        for kw in (dict(max_decoder_steps=caps), dict(alignments=amap, alignment_lengths=alens)):
+            del calls[:]
+            _, total, in_builder = _count_syncs(lambda: model.inference(text, input_lengths=lengths, seeds=seeds, **kw))
+            print("%s: %d synchronising calls, %d of them reading options back" % (sorted(kw), total, in_builder))
+            assert calls == ["Tacotron2.inference"]
+            assert in_builder == 2                       # input_lengths and the step limits / alignment_lengths, once each

@@ -1,16 +1,11 @@
 """The continuous-batching scheduler (tacotron2_b200/serving.py) without a GPU, over a fake of the engine side that
-records every call and plays back a script of firing steps; and the C layout of the new argument struct."""
-import ctypes
-import os
-import subprocess
-
+records every call and plays back a script of firing steps."""
 import pytest
 import torch
 
 import tacotron2_b200 as t2
-from tacotron2_b200 import _capi
 from tacotron2_b200.serving import InferenceServer, chunk_seed
-from tests.common import ROOT, keep_mask
+from tests.common import keep_mask
 
 
 class FakeStream:
@@ -202,24 +197,3 @@ def test_servers_need_cuda_and_eval_mode():
         m.train().inference_server()
     with pytest.raises(RuntimeError, match="CUDA"):
         m.eval().inference_server(slots=2, max_text_len=4, chunk_steps=2)
-
-
-def test_collect_row_ctypes_struct_matches_c_layout(tmp_path):
-    src = tmp_path / "layout.c"
-    fields = {"T2CollectRow": ["row", "n_frames", "T_text", "reserved", "mel", "gate", "align"],
-              "T2DecoderStreamArgs": ["dec", "state", "state_bytes", "status"]}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "t2b200.h"', 'int main(void){']
-    for s, fs in fields.items():
-        lines.append('printf("%s %%zu\\n", sizeof(%s));' % (s, s))
-        for f in fs:
-            lines.append('printf("%s.%s %%zu\\n", offsetof(%s, %s));' % (s, f, s, f))
-    lines.append('return 0;}')
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    out = dict(l.split() for l in subprocess.check_output([str(exe)]).decode().splitlines())
-    for s, fs in fields.items():
-        cls = getattr(_capi, s)
-        assert int(out[s]) == ctypes.sizeof(cls), s
-        for f in fs:
-            assert int(out["%s.%s" % (s, f)]) == getattr(cls, f).offset, (s, f)
