@@ -489,6 +489,39 @@ typedef struct T2InferArgs {
 size_t t2_infer_workspace_bytes(const T2Model* m, int32_t B, int32_t T_text, int32_t max_steps);
 int    t2_infer_host(T2Model* m, const T2InferArgs* a, void* stream);
 
+/* ---- Durations from attention maps (tacotron2_b200.durations_from_alignments; DESIGN section 6.10) ----------------
+ * alignments (B, T_mel, T_text) fp32 row-major -> durations (B, T_text) int64, frames per symbol.  Row b reads only
+ * alignments[b, :L_mel, :L_text] (L_mel = mel_lengths[b], L_text = input_lengths[b]; a NULL array means T_mel / T_text
+ * for every row) and writes zeros from L_text on, so it equals its own B = 1 call on that slice.  The lengths live on the
+ * device: the call cannot refuse them without waiting for the GPU, so the device clamps them into [1, T_mel] /
+ * [1, T_text] (the Python mirror refuses them).  Weights must be finite and >= 0 (not checked here; the Python mirror
+ * does).
+ *   T2_DURATIONS_MAS: the monotonic path from (0, 0) to (L_mel - 1, L_text - 1) -- per frame it stays on its symbol or
+ *     advances by one -- that maximises the sum of log(max(a, 2^-126)), computed in fp64.  S[0][0] = c[0][0],
+ *     S[0][j > 0] = -inf, S[t][j] = c[t][j] + max(S[t-1][j], S[t-1][j-1]); the backtrack from j = L_text - 1 at
+ *     t = L_mel - 1 gives frame t to j and steps to j - 1 when j > 0 and (j == t or S[t-1][j-1] > S[t-1][j]), so ties
+ *     stay on the current symbol.  Every symbol gets at least one frame; a row with L_mel < L_text has no such path and
+ *     gets zeros.
+ *   T2_DURATIONS_ARGMAX: frame t < L_mel goes to the smallest j < L_text holding the frame's maximum over j < L_text;
+ *     a symbol may get 0 frames.
+ * T_text <= T2_DURATIONS_MAX_TEXT (one CTA of at most 256 threads holds a row's scores, 16 symbols per thread).
+ * Bad sizes, a bad method or a NULL alignments / durations / ws are T2_ERR_INVALID, too small a workspace
+ * T2_ERR_WORKSPACE, before anything is launched.  No handle, no allocation, no host synchronisation.
+ * Workspace: t2_durations_workspace_bytes(B, T_mel, T_text, method) (0 for arguments the call refuses). */
+#define T2_DURATIONS_MAS       0
+#define T2_DURATIONS_ARGMAX    1
+#define T2_DURATIONS_MAX_TEXT  4096
+typedef struct T2DurationsArgs {
+  const float* alignments;             /* (B, T_mel, T_text) */
+  const int32_t* input_lengths;        /* (B) device or NULL */
+  const int32_t* mel_lengths;          /* (B) device or NULL */
+  int32_t B, T_mel, T_text, method;
+  int64_t* durations;                  /* out (B, T_text) */
+  void* ws; size_t ws_bytes;
+} T2DurationsArgs;
+size_t t2_durations_workspace_bytes(int32_t B, int32_t T_mel, int32_t T_text, int32_t method);
+int    t2_durations(const T2DurationsArgs* a, void* stream);
+
 /* ---- WaveGlow vocoder inference (waveglow/glow.py: WaveGlow.infer, glow.py:251-293) ---------------
  * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  Supported configurations (the published
  * one, waveglow/config.json, is the comment beside each field): n_mel_channels 80, n_group 8, wn_kernel_size 3,

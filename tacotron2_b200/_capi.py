@@ -13,6 +13,8 @@ LIB_PATH = os.environ.get("T2B200_LIB") or os.path.join(_HERE, "libt2b200.so")  
 T2_NUM_WEIGHTS = 84
 IMPL_AUTO, IMPL_STEPWISE, IMPL_PERSISTENT = 0, 1, 2
 MODE_INFER, MODE_TEACHER = 0, 1
+DURATIONS_MAS, DURATIONS_ARGMAX = 0, 1
+DURATIONS_MAX_TEXT = 4096           # T2_DURATIONS_MAX_TEXT
 
 EXPORTS = [
     "t2_abi_version", "t2_last_error", "t2_device_info", "t2_model_create", "t2_model_refresh",
@@ -38,6 +40,7 @@ EXPORTS = [
     "t2_denoiser_workspace_bytes", "t2_denoiser_run", "t2_denoiser_run_window", "t2_denoiser_window_halo",
     "t2_stft_transform_workspace_bytes", "t2_stft_transform", "t2_stft_inverse_workspace_bytes", "t2_stft_inverse",
     "t2_griffin_lim_workspace_bytes", "t2_griffin_lim",
+    "t2_durations_workspace_bytes", "t2_durations",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686       # the published configuration's; t2_waveglow_num_weights gives any other's
 
@@ -155,6 +158,12 @@ class T2CollateArgs(C.Structure):
                 ("B", C.c_int32), ("n_mel", C.c_int32), ("T_max", C.c_int32), ("L_pad", C.c_int32), ("order", C.c_void_p),
                 ("text_padded", C.c_void_p), ("input_lengths", C.c_void_p), ("mel_padded", C.c_void_p),
                 ("gate_padded", C.c_void_p), ("output_lengths", C.c_void_p)]
+
+
+class T2DurationsArgs(C.Structure):
+    _fields_ = [("alignments", C.c_void_p), ("input_lengths", C.c_void_p), ("mel_lengths", C.c_void_p),
+                ("B", C.c_int32), ("T_mel", C.c_int32), ("T_text", C.c_int32), ("method", C.c_int32),
+                ("durations", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
 
 
 class T2PostnetArgs(C.Structure):
@@ -317,6 +326,9 @@ def lib():
         getattr(L, n + "_workspace_bytes").restype = C.c_size_t
         getattr(L, n + "_workspace_bytes").argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         getattr(L, n).argtypes = [C.c_void_p, C.POINTER(args), C.c_void_p]
+    L.t2_durations_workspace_bytes.restype = C.c_size_t
+    L.t2_durations_workspace_bytes.argtypes = [C.c_int32] * 4
+    L.t2_durations.argtypes = [C.POINTER(T2DurationsArgs), C.c_void_p]
     if L.t2_abi_version() != 2:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L

@@ -2,6 +2,7 @@
 workspaces, dropout-mask injection.  All arithmetic happens in the shared library."""
 import contextlib
 import ctypes as C
+import math
 import numbers
 import threading
 
@@ -299,6 +300,78 @@ def alignments_from_durations(durations):
     out = torch.zeros(B, int(lengths.max()), T, dtype=torch.float32, device=dev)
     out[row, step, sym] = 1.0
     return out, lengths
+
+
+_DURATION_METHODS = {"mas": _capi.DURATIONS_MAS, "argmax": _capi.DURATIONS_ARGMAX}
+
+
+def duration_inputs(alignments, input_lengths, mel_lengths, method, device_type="cuda"):
+    """The arguments of durations_from_alignments checked and put in the library's form: (alignments fp32 contiguous,
+    input_lengths and mel_lengths as (B,) int32 on its device or None, the method's code).  The map must live on a
+    device of type `device_type`.  Reads the device back once for the weights' range (and, for MAS, the rows without a
+    path) and once per device-side lengths tensor.  Raises TypeError / ValueError before anything is launched."""
+    what = "tacotron2_b200.durations_from_alignments"
+    if method not in _DURATION_METHODS:
+        raise ValueError("%s: method must be one of %s (got %r)" % (what, sorted(_DURATION_METHODS), method))
+    if not torch.is_tensor(alignments):
+        raise TypeError("%s: alignments must be a tensor (got %s)" % (what, type(alignments).__name__))
+    if not alignments.dtype.is_floating_point:
+        raise TypeError("%s: alignments must be a float tensor (got %s)" % (what, alignments.dtype))
+    if alignments.dim() != 3 or min(alignments.shape) < 1:
+        raise ValueError("%s: alignments must have shape (B, T_mel, T_text), none of them 0 (got %s)"
+                         % (what, tuple(alignments.shape)))
+    B, T_mel, T_text = (int(s) for s in alignments.shape)
+    if T_text > _capi.DURATIONS_MAX_TEXT:
+        raise ValueError("%s: T_text must be at most %d (got %d)" % (what, _capi.DURATIONS_MAX_TEXT, T_text))
+    if alignments.device.type != device_type:
+        raise ValueError("%s: alignments must be on a %s device (got %s); there is no CPU path"
+                         % (what, device_type.upper(), alignments.device))
+    dev = alignments.device
+    il, _ = row_lengths(input_lengths, B, T_text, "input_lengths", dev)
+    ml, _ = row_lengths(mel_lengths, B, T_mel, "mel_lengths", dev)
+    a = alignments.detach().to(torch.float32).contiguous()
+    probe = torch.stack(torch.aminmax(a)).double()
+    if method == "mas":
+        n_text = il if il is not None else torch.full((B,), T_text, dtype=torch.int32, device=dev)
+        n_mel = ml if ml is not None else torch.full((B,), T_mel, dtype=torch.int32, device=dev)
+        probe = torch.cat((probe, (n_mel < n_text).double()))
+    host = probe.tolist()                                       # the one host read of the weights
+    if not (math.isfinite(host[0]) and math.isfinite(host[1]) and host[0] >= 0):
+        raise ValueError("%s: alignments must be finite and >= 0 (got values in [%r, %r])" % (what, host[0], host[1]))
+    short = [b for b, v in enumerate(host[2:]) if v]
+    if short:
+        raise ValueError("%s: rows %s have fewer frames than symbols, so no monotonic path gives every symbol a frame "
+                         "(method='mas')" % (what, short))
+    return a, il, ml, _DURATION_METHODS[method]
+
+
+def durations_from_alignments(alignments, input_lengths=None, mel_lengths=None, method="mas"):
+    """Attention maps -> per-symbol frame counts: the inverse of alignments_from_durations.
+
+    alignments: (B, T_mel, T_text) float tensor of any float dtype on a CUDA device, finite and >= 0 (what
+    Tacotron2.inference, Decoder.inference and Tacotron2.forward return), read as fp32; T_text <= 4096.
+    input_lengths / mel_lengths: None (T_text / T_mel for every row) or B integers in 1..T_text / 1..T_mel, as a list, a
+    host or a device tensor (``model.mel_lengths`` after inference; ``input_lengths`` / ``output_lengths`` from
+    ``parse_batch`` for a teacher-forced batch).
+
+    Returns (B, T_text) int64 on the alignments' device.  Row b sums to mel_lengths[b], is zero from input_lengths[b]
+    on, and depends only on alignments[b, :mel_lengths[b], :input_lengths[b]], so it equals its own B = 1 call on that
+    slice.
+
+    method "mas" (monotonic alignment search): the path from (0, 0) to (L_mel - 1, L_text - 1) that stays on its symbol
+    or advances by one per frame and maximises the sum of log(max(a, 2**-126)), in fp64; every symbol gets at least one
+    frame, and where paths tie the later advance wins (a uniform map gives [1, ..., 1, L_mel - L_text + 1]).  Rows with
+    mel_lengths[b] < input_lengths[b] have no such path and are refused.  method "argmax": each frame goes to the first
+    symbol holding its maximum; a symbol may get 0 frames.  See DESIGN section 6.10."""
+    a, il, ml, code = duration_inputs(alignments, input_lengths, mel_lengths, method)
+    B, T_mel, T_text = (int(s) for s in a.shape)
+    L = _capi.lib()
+    out = torch.empty(B, T_text, dtype=torch.int64, device=a.device)
+    ws = _capi.byte_buffer(L.t2_durations_workspace_bytes(B, T_mel, T_text, code), a.device)
+    args = _capi.T2DurationsArgs(a.data_ptr(), _ptr(il), _ptr(ml), B, T_mel, T_text, code, out.data_ptr(),
+                                 ws.data_ptr(), ws.numel())
+    _capi.call(L.t2_durations, a.device, C.byref(args))
+    return out
 
 
 def _i32(x, device):
