@@ -13,6 +13,9 @@
  *       Decoder.decode                        model.py:340-379        (inside, the persistent loop)
  *       Attention.forward / LocationLayer     model.py:22-26, 43-86   (inside)
  *       initialize_decoder_states             model.py:258-289        (inside: processed_memory GEMM)
+ *     Decoder.decode, one step on caller state  model.py:340-379     -> t2_decoder_step
+ *     Attention.forward / LocationLayer alone   model.py:22-26, 43-86 -> t2_attention_forward
+ *     memory_layer(memory)                      model.py:288         -> t2_processed_memory
  *     Postnet.forward (+ residual add)        model.py:141-146, 511, 524  -> t2_postnet_forward
  *     Tacotron2.inference, host buffers       model.py:517-529     -> t2_infer_host
  *
@@ -220,6 +223,57 @@ int    t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream);
  * T2_ERR_INVALID: limits with forced_align, mode TEACHER, a negative window side, or window_back != 0 without a window;
  * T2_ERR_UNSUPPORTED: the stepwise implementation (requested, or chosen by AUTO for a T_enc the persistent kernel does
  * not take).  t2_infer_host takes no limits. */
+
+/* ---- One decoder step on the caller's state (Decoder.decode, model.py:340-379) ---------------------------------
+ * For hand-written decoder loops (tacotron2_b200: Decoder.initialize_decoder_states / decode).  One call runs the step
+ * after the prenet -- attention LSTM, attention, decoder LSTM, projection and gate -- on state arrays the caller holds,
+ * with the stepwise implementation's kernels and arithmetic: the step of decoder_run_stepwise's loop, bit for bit.
+ *   memory (B, T_enc, 512), processed_memory (B, T_enc, 128) (t2_processed_memory), mask (B, T_enc) uint8 or NULL:
+ *   1 = padded position, whose energy gets score_mask_value before the softmax (model.py:79-80), any pattern.
+ *   attention_hidden / attention_cell / decoder_hidden / decoder_cell (B, 1024), attention_weights /
+ *   attention_weights_cum (B, T_enc), attention_context (B, 512): read and updated in place.
+ *   decoder_input (B, 256): the prenet output.  mel (B, 80) and gate (B) out.
+ *   training != 0: dropout(p_attention_dropout / p_decoder_dropout) on the two hidden states (model.py:355-356,
+ *   370-371) with att_keep / dec_keep (B, 1024) uint8 keep masks, or NULL => Philox(seed) at the sites of step 0 of a
+ *   t2_decoder_run, so one call equals that run's first step.
+ * Every array starts on a 16-byte boundary (the GEMMs read rows as float4).
+ * 7 kernel launches, no host synchronisation, no allocation.  T2_ERR_INVALID for null or misaligned pointers, B outside [1, 1024],
+ * T_enc < 1 or too small a workspace (t2_decoder_step_workspace_bytes(m, B)); T2_ERR_UNSUPPORTED for T_enc > 1282 (the
+ * stepwise attention's shared memory); both before any launch. */
+typedef struct T2DecoderStepArgs {
+  int32_t B, T_enc;
+  const float* memory; const float* processed_memory; const uint8_t* mask;
+  float* attention_hidden; float* attention_cell; float* decoder_hidden; float* decoder_cell;
+  float* attention_weights; float* attention_weights_cum; float* attention_context;
+  const float* decoder_input;
+  float* mel; float* gate;
+  int32_t training; const uint8_t* att_keep; const uint8_t* dec_keep; uint64_t seed;
+  float score_mask_value;
+  void* ws; size_t ws_bytes;
+} T2DecoderStepArgs;
+size_t t2_decoder_step_workspace_bytes(const T2Model* m, int32_t B);
+int    t2_decoder_step(T2Model* m, const T2DecoderStepArgs* a, void* stream);
+
+/* Attention.forward, Attention.get_alignment_energies and LocationLayer.forward (model.py:22-26, 43-86) in one launch
+ * of the step's attention kernel.  attention_weights_cat (B, 2, T_enc): previous and cumulative weights, as given.
+ * query (B, 1024) and processed_memory (B, T_enc, 128) may be NULL (zero) when only `location` is wanted; memory
+ * (B, T_enc, 512) is read only for `context`; mask as for t2_decoder_step.  Outputs, each optional: energies (B, T_enc)
+ * before masking, location (B, T_enc, 128) the location term, weights (B, T_enc) the masked softmax, context (B, 512).
+ * No cumulative array is touched.  With the inputs of a t2_decoder_step, weights and context are that step's bit for
+ * bit.  Refusals as t2_decoder_step (at least one output, context needs memory, weights or context need query and
+ * processed_memory). */
+typedef struct T2AttentionArgs {
+  int32_t B, T_enc;
+  const float* query; const float* memory; const float* processed_memory; const float* attention_weights_cat;
+  const uint8_t* mask;
+  float score_mask_value;
+  float* energies; float* location; float* weights; float* context;
+} T2AttentionArgs;
+int    t2_attention_forward(T2Model* m, const T2AttentionArgs* a, void* stream);
+
+/* memory_layer(memory) (model.py:288): memory (B, T_enc, 512), 16-byte aligned -> out (B, T_enc, 128), the GEMM the stepwise decoder
+ * uses, so t2_decoder_step on it computes what t2_decoder_run (STEPWISE) computes. */
+int    t2_processed_memory(T2Model* m, const float* memory, int32_t B, int32_t T_enc, float* out, void* stream);
 
 /* ---- Resumable decoder stream: the INFER loop of t2_decoder_run in chunks of steps -------------
  * The same persistent kernel stops after a number of steps and resumes exactly where it stopped, so

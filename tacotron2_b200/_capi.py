@@ -41,6 +41,7 @@ EXPORTS = [
     "t2_stft_transform_workspace_bytes", "t2_stft_transform", "t2_stft_inverse_workspace_bytes", "t2_stft_inverse",
     "t2_griffin_lim_workspace_bytes", "t2_griffin_lim",
     "t2_durations_workspace_bytes", "t2_durations",
+    "t2_decoder_step_workspace_bytes", "t2_decoder_step", "t2_attention_forward", "t2_processed_memory",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686       # the published configuration's; t2_waveglow_num_weights gives any other's
 
@@ -89,6 +90,23 @@ class T2DecoderArgs(C.Structure):
                 ("stash", C.c_void_p), ("stash_bytes", C.c_size_t), ("row_seeds", C.c_void_p),
                 ("forced_align", C.c_void_p), ("forced_lengths", C.c_void_p),
                 ("window_back", C.c_int32), ("window_front", C.c_int32), ("max_steps", C.c_void_p)]
+
+
+class T2DecoderStepArgs(C.Structure):
+    _fields_ = [("B", C.c_int32), ("T_enc", C.c_int32),
+                ("memory", C.c_void_p), ("processed_memory", C.c_void_p), ("mask", C.c_void_p),
+                ("attention_hidden", C.c_void_p), ("attention_cell", C.c_void_p), ("decoder_hidden", C.c_void_p),
+                ("decoder_cell", C.c_void_p), ("attention_weights", C.c_void_p), ("attention_weights_cum", C.c_void_p),
+                ("attention_context", C.c_void_p), ("decoder_input", C.c_void_p), ("mel", C.c_void_p), ("gate", C.c_void_p),
+                ("training", C.c_int32), ("att_keep", C.c_void_p), ("dec_keep", C.c_void_p), ("seed", C.c_uint64),
+                ("score_mask_value", C.c_float), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
+class T2AttentionArgs(C.Structure):
+    _fields_ = [("B", C.c_int32), ("T_enc", C.c_int32), ("query", C.c_void_p), ("memory", C.c_void_p),
+                ("processed_memory", C.c_void_p), ("attention_weights_cat", C.c_void_p), ("mask", C.c_void_p),
+                ("score_mask_value", C.c_float), ("energies", C.c_void_p), ("location", C.c_void_p),
+                ("weights", C.c_void_p), ("context", C.c_void_p)]
 
 
 class T2DecoderStreamArgs(C.Structure):
@@ -260,6 +278,11 @@ def lib():
     L.t2_encoder_forward.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_encoder_infer.argtypes = [C.c_void_p, C.POINTER(T2EncoderArgs), C.c_void_p]
     L.t2_decoder_run.argtypes = [C.c_void_p, C.POINTER(T2DecoderArgs), C.c_void_p]
+    L.t2_decoder_step_workspace_bytes.restype = C.c_size_t
+    L.t2_decoder_step_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
+    L.t2_decoder_step.argtypes = [C.c_void_p, C.POINTER(T2DecoderStepArgs), C.c_void_p]
+    L.t2_attention_forward.argtypes = [C.c_void_p, C.POINTER(T2AttentionArgs), C.c_void_p]
+    L.t2_processed_memory.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     L.t2_decoder_stream_state_bytes.restype = C.c_size_t
     L.t2_decoder_stream_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.t2_decoder_stream_begin.argtypes = [C.c_void_p, C.POINTER(T2DecoderStreamArgs), C.c_void_p]

@@ -593,6 +593,46 @@ class Engine(_Handle):
                                    row_seeds, forced_align, forced_lengths, max_steps)
         return mel, gate, align, mel_lengths, n_steps
 
+    # -- the step API (Decoder.initialize_decoder_states / decode, Attention / LocationLayer forwards) ----------------
+    def processed_memory(self, memory):
+        """memory (B, T_enc, 512) fp32 contiguous on the device -> memory_layer(memory) (B, T_enc, 128) fp32."""
+        B, T = int(memory.shape[0]), int(memory.shape[1])
+        out = torch.empty(B, T, self.hp.attention_dim, device=self.device, dtype=torch.float32)
+        self._call(_capi.lib().t2_processed_memory, memory.data_ptr(), B, T, out.data_ptr())
+        return out
+
+    def decoder_step(self, memory, pm, mask, state, x, training, att_keep, dec_keep, seed, score_mask_value):
+        """One t2_decoder_step.  memory / pm fp32 contiguous, mask None or (B, T_enc) uint8, state: the seven fp32
+        contiguous arrays (ah, ac, dh, dc, aw, awc, ctx), updated in place; x (B, 256) fp32.  Returns mel (B, 80) and
+        gate (B, 1), fp32."""
+        L = _capi.lib()
+        B, T = int(memory.shape[0]), int(memory.shape[1])
+        mel = torch.empty(B, self.hp.n_mel_channels, device=self.device, dtype=torch.float32)
+        gate = torch.empty(B, 1, device=self.device, dtype=torch.float32)
+        ws = self._workspace("step", L.t2_decoder_step_workspace_bytes(self.handle, B))
+        ah, ac, dh, dc, aw, awc, ctx = state
+        a = _capi.T2DecoderStepArgs(B, T, memory.data_ptr(), pm.data_ptr(), _ptr(mask), ah.data_ptr(), ac.data_ptr(),
+                                    dh.data_ptr(), dc.data_ptr(), aw.data_ptr(), awc.data_ptr(), ctx.data_ptr(),
+                                    x.data_ptr(), mel.data_ptr(), gate.data_ptr(), int(bool(training)), _ptr(att_keep),
+                                    _ptr(dec_keep), seed, float(score_mask_value), ws.data_ptr(), ws.numel())
+        self._call(L.t2_decoder_step, C.byref(a))
+        return mel, gate
+
+    def attention(self, B, T, weights_cat, query=None, memory=None, pm=None, mask=None, score_mask_value=-float("inf"),
+                  energies=False, location=False, weights=False, context=False):
+        """One t2_attention_forward over fp32 contiguous inputs; returns the requested outputs (fp32) in the order
+        energies, location, weights, context."""
+        f32 = dict(device=self.device, dtype=torch.float32)
+        outs = dict(energies=torch.empty(B, T, **f32) if energies else None,
+                    location=torch.empty(B, T, self.hp.attention_dim, **f32) if location else None,
+                    weights=torch.empty(B, T, **f32) if weights else None,
+                    context=torch.empty(B, self.hp.encoder_embedding_dim, **f32) if context else None)
+        a = _capi.T2AttentionArgs(B, T, _ptr(query), _ptr(memory), _ptr(pm), weights_cat.data_ptr(), _ptr(mask),
+                                  float(score_mask_value), *[_ptr(outs[k]) for k in ("energies", "location", "weights",
+                                                                                     "context")])
+        self._call(_capi.lib().t2_attention_forward, C.byref(a))
+        return [v for v in outs.values() if v is not None]
+
     def decoder_stream(self, memory, n_steps_cap, prenet_keep=None, gate_threshold=0.5, score_mask_value=-float("inf"),
                        impl=None, seed=None, memory_lengths=None, row_seeds=None, forced_align=None, forced_lengths=None,
                        window=None, max_steps=None):

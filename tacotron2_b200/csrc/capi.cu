@@ -288,6 +288,51 @@ int t2_decoder_run(T2Model* m, const T2DecoderArgs* a, void* stream) {
   return decoder_run_stepwise(m, a, (cudaStream_t)stream);
 }
 
+// the step API's shape checks: T_enc past the stepwise attention's shared memory is T2_ERR_UNSUPPORTED
+static int check_step_shape(int B, int T, const char* what) {
+  if (B <= 0 || B > kMaxBatch) return fail(T2_ERR_INVALID, "%s: B=%d outside [1, %d]", what, B, kMaxBatch);
+  if (T <= 0) return fail(T2_ERR_INVALID, "%s: empty encoder memory (T_enc=%d)", what, T);
+  if (stepwise_attention_smem(T) > 200 * 1024)
+    return fail(T2_ERR_UNSUPPORTED, "%s: T_enc=%d too long for the stepwise attention kernel (at most 1282)", what, T);
+  return T2_OK;
+}
+
+size_t t2_decoder_step_workspace_bytes(const T2Model*, int32_t B) { return B > 0 ? decoder_step_ws_bytes(B) : 0; }
+int t2_decoder_step(T2Model* m, const T2DecoderStepArgs* a, void* stream) {
+  if (!m || !a) return fail(T2_ERR_INVALID, "decoder step: null model / args");
+  T2_TRY(check_step_shape(a->B, a->T_enc, "decoder step"));
+  if (!a->memory || !a->processed_memory || !a->attention_hidden || !a->attention_cell || !a->decoder_hidden ||
+      !a->decoder_cell || !a->attention_weights || !a->attention_weights_cum || !a->attention_context ||
+      !a->decoder_input || !a->mel || !a->gate || !a->ws)
+    return fail(T2_ERR_INVALID, "decoder step: null tensor pointer");
+  // the GEMMs read their A operands (decoder_input, both hidden states, the context) as float4
+  const void* arrays[] = {a->memory, a->processed_memory, a->attention_hidden, a->attention_cell, a->decoder_hidden,
+                          a->decoder_cell, a->attention_weights, a->attention_weights_cum, a->attention_context,
+                          a->decoder_input, a->mel, a->gate};
+  for (const void* p : arrays)
+    if ((uintptr_t)p & 15) return fail(T2_ERR_INVALID, "decoder step: array %p is not 16-byte aligned", p);
+  if (a->ws_bytes < decoder_step_ws_bytes(a->B)) return fail(T2_ERR_WORKSPACE, "decoder step workspace too small");
+  return decoder_step_run(m, a, (cudaStream_t)stream);
+}
+
+int t2_attention_forward(T2Model* m, const T2AttentionArgs* a, void* stream) {
+  if (!m || !a) return fail(T2_ERR_INVALID, "attention: null model / args");
+  T2_TRY(check_step_shape(a->B, a->T_enc, "attention"));
+  if (!a->attention_weights_cat) return fail(T2_ERR_INVALID, "attention: null attention_weights_cat");
+  if (!a->energies && !a->location && !a->weights && !a->context) return fail(T2_ERR_INVALID, "attention: no output");
+  if (a->context && !a->memory) return fail(T2_ERR_INVALID, "attention: context needs memory");
+  if ((a->weights || a->context) && (!a->query || !a->processed_memory))
+    return fail(T2_ERR_INVALID, "attention: weights and context need query and processed_memory");
+  return attention_forward(m, a, (cudaStream_t)stream);
+}
+
+int t2_processed_memory(T2Model* m, const float* memory, int32_t B, int32_t T_enc, float* out, void* stream) {
+  if (!m || !memory || !out) return fail(T2_ERR_INVALID, "processed memory: null argument");
+  if (B <= 0 || T_enc <= 0) return fail(T2_ERR_INVALID, "processed memory: B=%d, T_enc=%d", B, T_enc);
+  if ((uintptr_t)memory & 15) return fail(T2_ERR_INVALID, "processed memory: memory is not 16-byte aligned");
+  return processed_memory(m, memory, B, T_enc, out, (cudaStream_t)stream);
+}
+
 size_t t2_decoder_stream_state_bytes(const T2Model*, int32_t B, int32_t T_enc) {
   return B > 0 && T_enc > 0 ? persistent_stream_state_bytes(B, T_enc) : 0;
 }

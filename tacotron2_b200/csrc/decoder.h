@@ -46,9 +46,31 @@ inline bool decoder_has_limits(const T2DecoderArgs* a) { return a->window_front 
 
 // t2_decoder_workspace_bytes is the larger of the two implementations' layouts
 size_t stepwise_ws_bytes(int B, int T);
+size_t stepwise_attention_smem(int T);   // the stepwise attention kernel's shared memory (at most 200 KiB: T_enc <= 1282)
 size_t persistent_ws_bytes(int B, int T, int cap);
 DecoderCtrl* persistent_ws_ctrl(const T2DecoderArgs* a);   // the control block (and phase profile) of a persistent run
 int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
+// one step of the stepwise decoder (decoder_stepwise.cu), shared by decoder_run_stepwise and t2_decoder_step: the state
+// arrays are read and updated in place
+struct StepState { float *ah, *ac, *dh, *dc, *aw, *awc, *ctx; };
+struct StepIo {
+  const float* x2 = nullptr;                   // (B, 256) prenet output
+  const float* memory = nullptr; const float* pm = nullptr;
+  const int32_t* mem_len = nullptr; const uint8_t* mask = nullptr;
+  float score_mask_value = 0.f;
+  int B = 0, T = 0;
+  int training = 0; const uint8_t* att_keep = nullptr; const uint8_t* dec_keep = nullptr;   // (B, 1024) or Philox
+  uint64_t seed = 0; uint32_t site = 0;        // Philox sites site + 2 (attention) and site + 3 (decoder)
+  float* gates = nullptr;                      // (B, 4096) scratch
+  float* proj = nullptr;                       // (B, 81) out: mel | gate
+  float* align_out = nullptr; long align_stride_b = 0;
+  const int* skip = nullptr;
+};
+int decoder_step(T2Model* m, const StepState& st, const StepIo& io, cudaStream_t s);
+size_t decoder_step_ws_bytes(int B);
+int decoder_step_run(T2Model* m, const T2DecoderStepArgs* a, cudaStream_t s);
+int attention_forward(T2Model* m, const T2AttentionArgs* a, cudaStream_t s);
+int processed_memory(T2Model* m, const float* memory, int B, int T, float* out, cudaStream_t s);
 int decoder_run_persistent(T2Model* m, const T2DecoderArgs* a, cudaStream_t s);
 int decoder_backward(T2Model* m, const T2DecoderBwdArgs* a, cudaStream_t s);
 size_t decoder_backward_ws_bytes(int B, int T_enc, int T_mel);

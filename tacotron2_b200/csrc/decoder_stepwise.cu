@@ -46,16 +46,31 @@ __device__ inline float warp_max(float v) {
   return v;
 }
 
-__global__ void __launch_bounds__(256)
-attention_row_kernel(const float* __restrict__ ah, const float* __restrict__ Wq,
-                     const float* __restrict__ Wloc, const float* __restrict__ Wld,
-                     const float* __restrict__ v, const float* __restrict__ pm,
-                     const float* __restrict__ memory, const int32_t* __restrict__ mem_len,
-                     float score_mask_value, float* __restrict__ aw, float* __restrict__ awc,
-                     float* __restrict__ ctx, float* __restrict__ align_out, long align_stride_b,
-                     int T, const int* skip_flag) {
-  if (skip_flag && *skip_flag) return;
+// Row b reads its previous / cumulative weights at aw_in + b * in_stride and awc_in + b * in_stride: the decoder's
+// state arrays (in_stride = T) or the two channels of attention_weights_cat (B, 2, T) (in_stride = 2 T).  Every output
+// may be null; aw_out / awc_out may be aw_in / awc_in.
+struct AttnRowArgs {
+  const float *Wq, *Wloc, *Wld, *v;
+  const float* ah;                  // (B, 1024) query, or null (zero query)
+  const float* pm;                  // (B, T, 128) processed memory, or null (zero)
+  const float* memory;              // (B, T, 512); read only for ctx
+  const int32_t* mem_len;           // (B) or null: positions j >= mem_len[b] are masked
+  const uint8_t* mask;              // (B, T) or null: 1 = masked, as the reference's mask; replaces mem_len
+  float score_mask_value;
+  const float* aw_in; const float* awc_in; long in_stride;
+  float* aw_out; float* awc_out;    // new weights; awc_in + new weights
+  float* ctx;                       // (B, 512)
+  float* align_out; long align_stride_b;
+  float* energies_out;              // (B, T) energies before the mask
+  float* loc_out;                   // (B, T, 128) location term
+  int T;
+  const int* skip_flag;
+};
+
+__global__ void __launch_bounds__(256) attention_row_kernel(AttnRowArgs a) {
+  if (a.skip_flag && *a.skip_flag) return;
   extern __shared__ float sm[];
+  const int T = a.T;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int TP = T + kLocK - 1;                       // padded length
   float* q = sm;                                       // 128
@@ -67,26 +82,27 @@ attention_row_kernel(const float* __restrict__ ah, const float* __restrict__ Wq,
   float* e = loc + kLocF * T;                          // [T]
   float* red = e + T;                                  // [32]
 
-  // 1. processed query  q = W_q . ah[b]            (model.py:57)
-  const float* ahb = ah + (long)b * kARnn;
+  // 1. processed query  q = W_q . ah[b]            (model.py:57); no query: the location term alone
+  const float* ahb = a.ah + (long)b * kARnn;
   for (int d = warp; d < kAtt; d += 8) {
-    const float* wr = Wq + (long)d * kARnn;
+    const float* wr = a.Wq + (long)d * kARnn;
     float s = 0.f;
-    for (int k = lane; k < kARnn; k += 32) s = fmaf(wr[k], ahb[k], s);
+    if (a.ah)
+      for (int k = lane; k < kARnn; k += 32) s = fmaf(wr[k], ahb[k], s);
     s = warp_sum(s);
     if (lane == 0) q[d] = s;
   }
   for (int i = tid; i < kLocF * kAtt; i += 256) {      // transpose (128,32) -> [c][d]
     const int d = i / kLocF, c = i - d * kLocF;
-    wld_t[c * kAtt + d] = Wld[i];
+    wld_t[c * kAtt + d] = a.Wld[i];
   }
-  for (int i = tid; i < kLocF * 2 * kLocK; i += 256) wloc[i] = Wloc[i];
+  for (int i = tid; i < kLocF * 2 * kLocK; i += 256) wloc[i] = a.Wloc[i];
   const int half = (kLocK - 1) / 2;
   for (int i = tid; i < TP; i += 256) {
     const int j = i - half;
     const bool in = (j >= 0 && j < T);
-    pad0[i] = in ? aw[(long)b * T + j] : 0.f;
-    pad1[i] = in ? awc[(long)b * T + j] : 0.f;
+    pad0[i] = in ? a.aw_in[(long)b * a.in_stride + j] : 0.f;
+    pad1[i] = in ? a.awc_in[(long)b * a.in_stride + j] : 0.f;
   }
   __syncthreads();
   // 2. location conv (2 -> 32 channels, k = 31, zero padding 15)     (model.py:23)
@@ -102,7 +118,7 @@ attention_row_kernel(const float* __restrict__ ah, const float* __restrict__ Wq,
   }
   __syncthreads();
   // 3. energies  e_j = v . tanh(q + W_ld loc_j + pm_j)               (model.py:24-25, 58-60)
-  const int len = mem_len ? mem_len[b] : T;
+  const int len = a.mem_len ? a.mem_len[b] : T;
   for (int j = warp; j < T; j += 8) {
     float part = 0.f;
 #pragma unroll
@@ -111,11 +127,16 @@ attention_row_kernel(const float* __restrict__ ah, const float* __restrict__ Wq,
       float pa = 0.f;
 #pragma unroll
       for (int c = 0; c < kLocF; ++c) pa = fmaf(wld_t[c * kAtt + d], loc[c * T + j], pa);
-      const float x = q[d] + pa + pm[((long)b * T + j) * kAtt + d];
-      part = fmaf(v[d], tanhf(x), part);
+      if (a.loc_out) a.loc_out[((long)b * T + j) * kAtt + d] = pa;              // LocationLayer.forward
+      const float x = q[d] + pa + (a.pm ? a.pm[((long)b * T + j) * kAtt + d] : 0.f);
+      part = fmaf(a.v[d], tanhf(x), part);
     }
     part = warp_sum(part);
-    if (lane == 0) e[j] = (j < len) ? part : score_mask_value;     // model.py:79-80
+    if (lane == 0) {
+      if (a.energies_out) a.energies_out[(long)b * T + j] = part;               // get_alignment_energies
+      const bool masked = a.mask ? a.mask[(long)b * T + j] != 0 : j >= len;
+      e[j] = masked ? a.score_mask_value : part;                                 // model.py:79-80
+    }
   }
   __syncthreads();
   // 4. softmax over T                                                 (model.py:82)
@@ -144,17 +165,18 @@ attention_row_kernel(const float* __restrict__ ah, const float* __restrict__ Wq,
   for (int j = tid; j < T; j += 256) {
     const float p = e[j] * inv;
     e[j] = p;
-    aw[(long)b * T + j] = p;
-    awc[(long)b * T + j] += p;                                     // model.py:365
-    align_out[(long)b * align_stride_b + j] = p;
+    if (a.aw_out) a.aw_out[(long)b * T + j] = p;
+    if (a.awc_out) a.awc_out[(long)b * T + j] = a.awc_in[(long)b * a.in_stride + j] + p;   // model.py:365
+    if (a.align_out) a.align_out[(long)b * a.align_stride_b + j] = p;
   }
   __syncthreads();
   // 5. context = aw . memory                                          (model.py:83-84)
+  if (!a.ctx) return;
   for (int col = tid; col < kEnc; col += 256) {
-    const float* mp = memory + (long)b * T * kEnc + col;
+    const float* mp = a.memory + (long)b * T * kEnc + col;
     float s = 0.f;
     for (int j = 0; j < T; ++j) s = fmaf(e[j], mp[(long)j * kEnc], s);
-    ctx[(long)b * kEnc + col] = s;
+    a.ctx[(long)b * kEnc + col] = s;
   }
 }
 
@@ -204,6 +226,11 @@ size_t stepwise_attention_smem(int T) {
                           kLocF * T + T + 32);
 }
 
+static int attention_smem_opt_in(size_t att_smem) {
+  T2_CUDA(cudaFuncSetAttribute(attention_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
+  return T2_OK;
+}
+
 // workspace of the stepwise decoder
 struct StepwiseWs {
   float* pm;               // processed_memory (B, T, 128)          model.py:288
@@ -239,6 +266,68 @@ size_t stepwise_ws_bytes(int B, int T) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// one decoder step (Decoder.decode, model.py:340-379) after the prenet, on the state arrays `st`, in place
+// ---------------------------------------------------------------------------------------------
+int decoder_step(T2Model* m, const StepState& st, const StepIo& io, cudaStream_t s) {
+  const int B = io.B, T = io.T;
+  const int pw_blocks = (B * kARnn + 255) / 256;
+  const float p_att = m->cfg.p_attention_dropout, p_dec = m->cfg.p_decoder_dropout;
+  {  // attention LSTMCell on [prenet ; context]              (model.py:352-354)
+    GemmArgs g;
+    g.nseg = 3;
+    g.seg[0] = {io.x2, kPre, m->w[W_ARNN_WIH], kPre + kEnc, kPre};
+    g.seg[1] = {st.ctx, kEnc, m->w[W_ARNN_WIH] + kPre, kPre + kEnc, kEnc};
+    g.seg[2] = {st.ah, kARnn, m->w[W_ARNN_WHH], kARnn, kARnn};
+    g.M = B; g.N = 4 * kARnn; g.C = io.gates; g.ldc = 4 * kARnn; g.bias = m->arnn_b;
+    g.skip_flag = io.skip;
+    T2_TRY(gemm_f32(g, s));
+    const uint8_t* keep = io.training ? io.att_keep : nullptr;
+    const int ph = (io.training && !io.att_keep) ? 1 : 0;
+    lstm_pointwise_kernel<<<pw_blocks, 256, 0, s>>>(io.gates, st.ah, st.ac, B, kARnn, keep, ph,
+                                                    io.seed, io.site + 2, p_att, io.skip);
+    T2_LAUNCH_CHECK();
+  }
+  {  // attention (model.py:358-365): new weights, cumulative update, context
+    AttnRowArgs a;
+    a.Wq = m->w[W_ATT_QUERY]; a.Wloc = m->w[W_ATT_LOC_CONV]; a.Wld = m->w[W_ATT_LOC_DENSE]; a.v = m->w[W_ATT_V];
+    a.ah = st.ah; a.pm = io.pm; a.memory = io.memory; a.mem_len = io.mem_len; a.mask = io.mask;
+    a.score_mask_value = io.score_mask_value;
+    a.aw_in = st.aw; a.awc_in = st.awc; a.in_stride = T;
+    a.aw_out = st.aw; a.awc_out = st.awc; a.ctx = st.ctx;
+    a.align_out = io.align_out; a.align_stride_b = io.align_stride_b;
+    a.energies_out = nullptr; a.loc_out = nullptr;
+    a.T = T; a.skip_flag = io.skip;
+    attention_row_kernel<<<B, 256, stepwise_attention_smem(T), s>>>(a);
+    T2_LAUNCH_CHECK();
+  }
+  {  // decoder LSTMCell on [attention_hidden ; context]        (model.py:366-369)
+    GemmArgs g;
+    g.nseg = 3;
+    g.seg[0] = {st.ah, kARnn, m->w[W_DRNN_WIH], kARnn + kEnc, kARnn};
+    g.seg[1] = {st.ctx, kEnc, m->w[W_DRNN_WIH] + kARnn, kARnn + kEnc, kEnc};
+    g.seg[2] = {st.dh, kDRnn, m->w[W_DRNN_WHH], kDRnn, kDRnn};
+    g.M = B; g.N = 4 * kDRnn; g.C = io.gates; g.ldc = 4 * kDRnn; g.bias = m->drnn_b;
+    g.skip_flag = io.skip;
+    T2_TRY(gemm_f32(g, s));
+    const uint8_t* keep = io.training ? io.dec_keep : nullptr;
+    const int ph = (io.training && !io.dec_keep) ? 1 : 0;
+    lstm_pointwise_kernel<<<pw_blocks, 256, 0, s>>>(io.gates, st.dh, st.dc, B, kDRnn, keep, ph,
+                                                    io.seed, io.site + 3, p_dec, io.skip);
+    T2_LAUNCH_CHECK();
+  }
+  {  // linear_projection + gate_layer on [decoder_hidden ; context]   (model.py:373-378)
+    GemmArgs g;
+    g.nseg = 2;
+    g.seg[0] = {st.dh, kDRnn, m->projgate_w, kDRnn + kEnc, kDRnn};
+    g.seg[1] = {st.ctx, kEnc, m->projgate_w + kDRnn, kDRnn + kEnc, kEnc};
+    g.M = B; g.N = kMel + 1; g.C = io.proj; g.ldc = kMel + 1; g.bias = m->projgate_b;
+    g.skip_flag = io.skip;
+    T2_TRY(gemm_f32(g, s));
+  }
+  return T2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // host orchestration
 // ---------------------------------------------------------------------------------------------
 int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
@@ -252,18 +341,10 @@ int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
   T2_CUDA(cudaMemsetAsync(w.state_begin, 0, w.state_bytes, s));   // model.py:258-284 (zeros)
   T2_CUDA(cudaMemsetAsync(w.ctrl, 0, sizeof(DecoderCtrl), s));
 
-  // processed_memory = memory_layer(memory)                      (model.py:288)
-  {
-    GemmArgs g;
-    g.seg[0] = {a->memory, kEnc, m->w[W_ATT_MEMORY], kEnc, kEnc};
-    g.M = B * T; g.N = kAtt; g.C = w.pm; g.ldc = kAtt;
-    T2_TRY(gemm_f32(g, s));
-  }
-  T2_CUDA(cudaFuncSetAttribute(attention_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)att_smem));
+  T2_TRY(processed_memory(m, a->memory, B, T, w.pm, s));
+  T2_TRY(attention_smem_opt_in(att_smem));
   const int* skip = &w.ctrl->all_done;
-  const int pw_blocks = (B * kARnn + 255) / 256;
-  const float p_att = m->cfg.p_attention_dropout, p_dec = m->cfg.p_decoder_dropout;
+  const StepState st{w.ah, w.ac, w.dh, w.dc, w.aw, w.awc, w.ctx};
 
   for (int t = 0; t < cap; ++t) {
     const float* x2;
@@ -288,55 +369,89 @@ int decoder_run_stepwise(T2Model* m, const T2DecoderArgs* a, cudaStream_t s) {
     } else {
       x2 = a->teacher_prenet + (long)t * B * kPre;
     }
-    {  // attention LSTMCell on [prenet ; context]              (model.py:352-354)
-      GemmArgs g;
-      g.nseg = 3;
-      g.seg[0] = {x2, kPre, m->w[W_ARNN_WIH], kPre + kEnc, kPre};
-      g.seg[1] = {w.ctx, kEnc, m->w[W_ARNN_WIH] + kPre, kPre + kEnc, kEnc};
-      g.seg[2] = {w.ah, kARnn, m->w[W_ARNN_WHH], kARnn, kARnn};
-      g.M = B; g.N = 4 * kARnn; g.C = w.gates; g.ldc = 4 * kARnn; g.bias = m->arnn_b;
-      g.skip_flag = skip;
-      T2_TRY(gemm_f32(g, s));
-      const uint8_t* keep = (a->training && a->att_keep) ? a->att_keep + (long)t * B * kARnn : nullptr;
-      const int ph = (a->training && !a->att_keep) ? 1 : 0;
-      lstm_pointwise_kernel<<<pw_blocks, 256, 0, s>>>(w.gates, w.ah, w.ac, B, kARnn, keep, ph,
-                                                      a->seed, t * 4 + 2, p_att, skip);
-      T2_LAUNCH_CHECK();
-    }
-    attention_row_kernel<<<B, 256, att_smem, s>>>(
-        w.ah, m->w[W_ATT_QUERY], m->w[W_ATT_LOC_CONV], m->w[W_ATT_LOC_DENSE], m->w[W_ATT_V], w.pm,
-        a->memory, a->memory_lengths, a->score_mask_value, w.aw, w.awc, w.ctx,
-        a->align + (long)t * T, (long)cap * T, T, skip);
-    T2_LAUNCH_CHECK();
-    {  // decoder LSTMCell on [attention_hidden ; context]        (model.py:366-369)
-      GemmArgs g;
-      g.nseg = 3;
-      g.seg[0] = {w.ah, kARnn, m->w[W_DRNN_WIH], kARnn + kEnc, kARnn};
-      g.seg[1] = {w.ctx, kEnc, m->w[W_DRNN_WIH] + kARnn, kARnn + kEnc, kEnc};
-      g.seg[2] = {w.dh, kDRnn, m->w[W_DRNN_WHH], kDRnn, kDRnn};
-      g.M = B; g.N = 4 * kDRnn; g.C = w.gates; g.ldc = 4 * kDRnn; g.bias = m->drnn_b;
-      g.skip_flag = skip;
-      T2_TRY(gemm_f32(g, s));
-      const uint8_t* keep = (a->training && a->dec_keep) ? a->dec_keep + (long)t * B * kDRnn : nullptr;
-      const int ph = (a->training && !a->dec_keep) ? 1 : 0;
-      lstm_pointwise_kernel<<<pw_blocks, 256, 0, s>>>(w.gates, w.dh, w.dc, B, kDRnn, keep, ph,
-                                                      a->seed, t * 4 + 3, p_dec, skip);
-      T2_LAUNCH_CHECK();
-    }
-    {  // linear_projection + gate_layer on [decoder_hidden ; context]   (model.py:373-378)
-      GemmArgs g;
-      g.nseg = 2;
-      g.seg[0] = {w.dh, kDRnn, m->projgate_w, kDRnn + kEnc, kDRnn};
-      g.seg[1] = {w.ctx, kEnc, m->projgate_w + kDRnn, kDRnn + kEnc, kEnc};
-      g.M = B; g.N = kMel + 1; g.C = w.proj; g.ldc = kMel + 1; g.bias = m->projgate_b;
-      g.skip_flag = skip;
-      T2_TRY(gemm_f32(g, s));
-    }
+    StepIo io;
+    io.x2 = x2; io.memory = a->memory; io.pm = w.pm; io.mem_len = a->memory_lengths;
+    io.score_mask_value = a->score_mask_value; io.B = B; io.T = T;
+    io.training = a->training;
+    io.att_keep = a->att_keep ? a->att_keep + (long)t * B * kARnn : nullptr;
+    io.dec_keep = a->dec_keep ? a->dec_keep + (long)t * B * kDRnn : nullptr;
+    io.seed = a->seed; io.site = t * 4; io.gates = w.gates; io.proj = w.proj;
+    io.align_out = a->align + (long)t * T; io.align_stride_b = (long)cap * T; io.skip = skip;
+    T2_TRY(decoder_step(m, st, io, s));
     emit_kernel<<<1, 256, 0, s>>>(w.proj, a->mel, a->gate, B, t, cap, infer ? 1 : 0,
                                   a->gate_threshold, w.ctrl, a->mel_lengths, a->n_steps);
     T2_LAUNCH_CHECK();
   }
   finalize_lengths_kernel<<<1, 256, 0, s>>>(w.ctrl, a->mel_lengths, a->n_steps, B);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
+}
+
+// processed_memory = memory_layer(memory)                      (model.py:288)
+int processed_memory(T2Model* m, const float* memory, int B, int T, float* out, cudaStream_t s) {
+  GemmArgs g;
+  g.seg[0] = {memory, kEnc, m->w[W_ATT_MEMORY], kEnc, kEnc};
+  g.M = B * T; g.N = kAtt; g.C = out; g.ldc = kAtt;
+  return gemm_f32(g, s);
+}
+
+// ---------------------------------------------------------------------------------------------
+// t2_decoder_step: one decode() on the caller's state
+// ---------------------------------------------------------------------------------------------
+__global__ void split_proj_kernel(const float* __restrict__ proj, float* __restrict__ mel, float* __restrict__ gate, int B) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * (kMel + 1)) return;
+  const int b = i / (kMel + 1), c = i - b * (kMel + 1);
+  if (c < kMel) mel[b * kMel + c] = proj[i];
+  else gate[b] = proj[i];
+}
+
+static void step_ws_layout(Carve& c, int B, float** gates, float** proj) {
+  *gates = c.take<float>((size_t)B * 4 * kARnn);
+  *proj = c.take<float>((size_t)B * (kMel + 1));
+}
+size_t decoder_step_ws_bytes(int B) {
+  Carve c(nullptr);
+  float *g, *p;
+  step_ws_layout(c, B, &g, &p);
+  return c.bytes();
+}
+
+int decoder_step_run(T2Model* m, const T2DecoderStepArgs* a, cudaStream_t s) {
+  const int B = a->B, T = a->T_enc;
+  T2_TRY(attention_smem_opt_in(stepwise_attention_smem(T)));
+  float *gates, *proj;
+  Carve c(a->ws);
+  step_ws_layout(c, B, &gates, &proj);
+  const StepState st{a->attention_hidden, a->attention_cell, a->decoder_hidden, a->decoder_cell, a->attention_weights,
+                     a->attention_weights_cum, a->attention_context};
+  StepIo io;
+  io.x2 = a->decoder_input; io.memory = a->memory; io.pm = a->processed_memory; io.mask = a->mask;
+  io.score_mask_value = a->score_mask_value; io.B = B; io.T = T;
+  io.training = a->training; io.att_keep = a->att_keep; io.dec_keep = a->dec_keep;
+  io.seed = a->seed; io.site = 0;                  // the keys of step 0 of decoder_run_stepwise
+  io.gates = gates; io.proj = proj;
+  T2_TRY(decoder_step(m, st, io, s));
+  split_proj_kernel<<<(B * (kMel + 1) + 255) / 256, 256, 0, s>>>(proj, a->mel, a->gate, B);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// t2_attention_forward: Attention.forward / get_alignment_energies / LocationLayer.forward
+// ---------------------------------------------------------------------------------------------
+int attention_forward(T2Model* m, const T2AttentionArgs* a, cudaStream_t s) {
+  const int T = a->T_enc;
+  T2_TRY(attention_smem_opt_in(stepwise_attention_smem(T)));
+  AttnRowArgs r;
+  r.Wq = m->w[W_ATT_QUERY]; r.Wloc = m->w[W_ATT_LOC_CONV]; r.Wld = m->w[W_ATT_LOC_DENSE]; r.v = m->w[W_ATT_V];
+  r.ah = a->query; r.pm = a->processed_memory; r.memory = a->memory; r.mem_len = nullptr; r.mask = a->mask;
+  r.score_mask_value = a->score_mask_value;
+  r.aw_in = a->attention_weights_cat; r.awc_in = a->attention_weights_cat + T; r.in_stride = 2L * T;
+  r.aw_out = a->weights; r.awc_out = nullptr; r.ctx = a->context; r.align_out = nullptr; r.align_stride_b = 0;
+  r.energies_out = a->energies; r.loc_out = a->location;
+  r.T = T; r.skip_flag = nullptr;
+  attention_row_kernel<<<a->B, 256, stepwise_attention_smem(T), s>>>(r);
   T2_LAUNCH_CHECK();
   return T2_OK;
 }

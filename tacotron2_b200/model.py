@@ -26,31 +26,6 @@ from .layers import ConvNorm, LinearNorm
 from .utils import get_mask_from_lengths, to_gpu
 
 
-class LocationLayer(nn.Module):
-    """model.py:10-26 (parameters only; evaluated inside the decoder kernels)."""
-
-    def __init__(self, attention_n_filters, attention_kernel_size, attention_dim):
-        super(LocationLayer, self).__init__()
-        padding = int((attention_kernel_size - 1) / 2)
-        self.location_conv = ConvNorm(2, attention_n_filters, kernel_size=attention_kernel_size,
-                                      padding=padding, bias=False, stride=1, dilation=1)
-        self.location_dense = LinearNorm(attention_n_filters, attention_dim, bias=False, w_init_gain='tanh')
-
-
-class Attention(nn.Module):
-    """model.py:29-86 (parameters + score_mask_value, which train.py:76 overwrites from outside)."""
-
-    def __init__(self, attention_rnn_dim, embedding_dim, attention_dim, attention_location_n_filters,
-                 attention_location_kernel_size):
-        super(Attention, self).__init__()
-        self.query_layer = LinearNorm(attention_rnn_dim, attention_dim, bias=False, w_init_gain='tanh')
-        self.memory_layer = LinearNorm(embedding_dim, attention_dim, bias=False, w_init_gain='tanh')
-        self.v = LinearNorm(attention_dim, 1, bias=False)
-        self.location_layer = LocationLayer(attention_location_n_filters, attention_location_kernel_size,
-                                            attention_dim)
-        self.score_mask_value = -float("inf")
-
-
 class _EngineOwner(object):
     """Mixin: finds (or lazily creates) the Engine for this module.  Sub-modules of a Tacotron2 share
     the root's engine; a stand-alone Encoder / Decoder / Postnet builds its own (the weight-table
@@ -96,13 +71,13 @@ class _EngineOwner(object):
     def _t2_engine(self):
         root = self._t2_root()
         root._t2_link()
+        if "_t2_hparams" not in root.__dict__:
+            raise RuntimeError("tacotron2_b200: %s must be used as part of a Decoder / Tacotron2" % type(self).__name__)
         eng = root.__dict__.get("_t2_engine_obj")
         if eng is None:
             eng = Engine(root._t2_hparams)
             root.__dict__["_t2_engine_obj"] = eng
         prefix = root._t2_prefix
-        if "_t2_hparams" not in root.__dict__:
-            raise RuntimeError("tacotron2_b200: %s must be used as part of a Decoder / Tacotron2" % type(self).__name__)
         named = {}
         for k, v in root.named_parameters():
             named[prefix + k] = v
@@ -134,11 +109,54 @@ def _invalidate_after_load(module, incompatible_keys):
     module.invalidate_weights()
 
 
-def _require_no_grad(module, what):
+def _require_no_grad(module, what, why="the prenet's backward is part of Decoder.forward's, model.py:396-399"):
     if torch.is_grad_enabled() and any(p_.requires_grad for p_ in module.parameters()):
         raise NotImplementedError(
-            "tacotron2_b200: %s on its own has no autograd node (the prenet's backward is part of Decoder.forward's, "
-            "model.py:396-399); call it through Decoder.forward / Tacotron2.forward or under torch.no_grad()" % what)
+            "tacotron2_b200: %s on its own has no autograd node (%s); call it through Decoder.forward / "
+            "Tacotron2.forward or under torch.no_grad()" % (what, why))
+
+
+_STEP_NO_GRAD = "the step API has no per-step backward; training goes through Decoder.forward"
+STEP_MAX_T_ENC = 1282      # the stepwise attention kernel's shared memory (t2_decoder_step)
+
+
+def _f32(t):
+    """t as a contiguous fp32 tensor (itself when it already is one)."""
+    return t.detach().to(torch.float32).contiguous()
+
+
+def _step_tensor(t, name, shape, device, what):
+    """A float tensor of the given shape on `device`; TypeError / ValueError naming it otherwise."""
+    if not torch.is_tensor(t):
+        raise TypeError("tacotron2_b200: %s: %s must be a tensor (got %s)" % (what, name, type(t).__name__))
+    if not t.dtype.is_floating_point:
+        raise TypeError("tacotron2_b200: %s: %s must be a float tensor (got %s)" % (what, name, t.dtype))
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError("tacotron2_b200: %s: %s must have shape %s (got %s)" % (what, name, tuple(shape), tuple(t.shape)))
+    if t.device != device:
+        raise ValueError("tacotron2_b200: %s: %s must be on the model's device %s (got %s); there is no CPU path"
+                         % (what, name, device, t.device))
+    return t
+
+
+def _step_mask(mask, B, T, device, what):
+    """The reference's mask (None, or bool (B, T_enc), True = padding) as the library's uint8 (B, T_enc), or None."""
+    if mask is None:
+        return None
+    if not torch.is_tensor(mask) or mask.dtype != torch.bool:
+        raise TypeError("tacotron2_b200: %s: mask must be None or a bool tensor, True at padded positions (got %s)"
+                        % (what, mask.dtype if torch.is_tensor(mask) else type(mask).__name__))
+    if tuple(mask.shape) != (B, T):
+        raise ValueError("tacotron2_b200: %s: mask must have shape %s (got %s)" % (what, (B, T), tuple(mask.shape)))
+    if mask.device != device:
+        raise ValueError("tacotron2_b200: %s: mask must be on the model's device %s (got %s)" % (what, device, mask.device))
+    return mask.contiguous().view(torch.uint8)
+
+
+def _step_t_enc(T, what):
+    if T > STEP_MAX_T_ENC:
+        raise ValueError("tacotron2_b200: %s: T_enc=%d is longer than the step API takes (at most %d)"
+                         % (what, T, STEP_MAX_T_ENC))
 
 
 def _wants_grad(module, *tensors):
@@ -150,6 +168,83 @@ def _require_no_grad_with_lengths(module, what):
     if torch.is_grad_enabled() and any(p_.requires_grad for p_ in module.parameters()):
         raise NotImplementedError("tacotron2_b200: %s with per-row lengths has no autograd node; call it under "
                                   "torch.no_grad()" % what)
+
+
+class LocationLayer(_EngineOwner, nn.Module):
+    """model.py:10-26.  Evaluated inside the decoder kernels; forward() runs as part of a Decoder / Tacotron2."""
+    _t2_prefix = "decoder.attention_layer.location_layer."
+
+    def __init__(self, attention_n_filters, attention_kernel_size, attention_dim):
+        super(LocationLayer, self).__init__()
+        padding = int((attention_kernel_size - 1) / 2)
+        self.location_conv = ConvNorm(2, attention_n_filters, kernel_size=attention_kernel_size,
+                                      padding=padding, bias=False, stride=1, dilation=1)
+        self.location_dense = LinearNorm(attention_n_filters, attention_dim, bias=False, w_init_gain='tanh')
+
+    def forward(self, attention_weights_cat):
+        """model.py:22-26: attention_weights_cat (B, 2, T_enc) -> the location term (B, T_enc, attention_dim), on the
+        step API's attention kernel (T_enc <= 1282)."""
+        what = "LocationLayer.forward"
+        _require_no_grad(self, what, _STEP_NO_GRAD)
+        cat = _attention_cat(attention_weights_cat, self._t2_device(), what)
+        B, T = int(cat.shape[0]), int(cat.shape[2])
+        eng = self._t2_engine()
+        loc, = eng.attention(B, T, _f32(cat), location=True)
+        return loc.to(attention_weights_cat.dtype)
+
+
+def _attention_cat(cat, device, what):
+    if not torch.is_tensor(cat) or cat.dim() != 3 or cat.shape[1] != 2 or cat.shape[0] < 1 or cat.shape[2] < 1:
+        raise ValueError("tacotron2_b200: %s: attention_weights_cat must be a (B, 2, T_enc) tensor (got %s)"
+                         % (what, tuple(cat.shape) if torch.is_tensor(cat) else type(cat).__name__))
+    _step_tensor(cat, "attention_weights_cat", cat.shape, device, what)
+    _step_t_enc(int(cat.shape[2]), what)
+    return cat
+
+
+class Attention(_EngineOwner, nn.Module):
+    """model.py:29-86 (score_mask_value, which train.py:76 overwrites from outside, is read at every call).  Its
+    forwards run as part of a Decoder / Tacotron2."""
+    _t2_prefix = "decoder.attention_layer."
+
+    def __init__(self, attention_rnn_dim, embedding_dim, attention_dim, attention_location_n_filters,
+                 attention_location_kernel_size):
+        super(Attention, self).__init__()
+        self.query_layer = LinearNorm(attention_rnn_dim, attention_dim, bias=False, w_init_gain='tanh')
+        self.memory_layer = LinearNorm(embedding_dim, attention_dim, bias=False, w_init_gain='tanh')
+        self.v = LinearNorm(attention_dim, 1, bias=False)
+        self.location_layer = LocationLayer(attention_location_n_filters, attention_location_kernel_size,
+                                            attention_dim)
+        self.score_mask_value = -float("inf")
+
+    def _inputs(self, what, query, processed_memory, attention_weights_cat, memory=None, mask=None):
+        _require_no_grad(self, what, _STEP_NO_GRAD)
+        dev = self._t2_device()
+        cat = _attention_cat(attention_weights_cat, dev, what)
+        B, T = int(cat.shape[0]), int(cat.shape[2])
+        _step_tensor(query, "query", (B, self.query_layer.linear_layer.in_features), dev, what)
+        _step_tensor(processed_memory, "processed_memory", (B, T, self.query_layer.linear_layer.out_features), dev, what)
+        if memory is not None:
+            _step_tensor(memory, "memory", (B, T, self.memory_layer.linear_layer.in_features), dev, what)
+        return B, T, dict(weights_cat=_f32(cat), query=_f32(query), pm=_f32(processed_memory),
+                          memory=None if memory is None else _f32(memory), mask=_step_mask(mask, B, T, dev, what),
+                          score_mask_value=float(self.score_mask_value))
+
+    def get_alignment_energies(self, query, processed_memory, attention_weights_cat):
+        """model.py:43-63: query (B, attention_rnn_dim), processed_memory (B, T_enc, attention_dim),
+        attention_weights_cat (B, 2, T_enc) -> energies (B, T_enc), before any mask."""
+        B, T, kw = self._inputs("Attention.get_alignment_energies", query, processed_memory, attention_weights_cat)
+        energies, = self._t2_engine().attention(B, T, energies=True, **kw)
+        return energies.to(processed_memory.dtype)
+
+    def forward(self, attention_hidden_state, memory, processed_memory, attention_weights_cat, mask):
+        """model.py:65-86 -> (attention_context (B, 512), attention_weights (B, T_enc)) in memory's dtype.  mask: None or
+        bool (B, T_enc), True at padded positions, which get score_mask_value before the softmax.  Nothing cumulative is
+        updated.  On decode()'s inputs of a step it gives that step's weights and context bit for bit."""
+        B, T, kw = self._inputs("Attention.forward", attention_hidden_state, processed_memory, attention_weights_cat,
+                                memory, mask)
+        weights, context = self._t2_engine().attention(B, T, weights=True, context=True, **kw)
+        return context.to(memory.dtype), weights.to(memory.dtype)
 
 
 class _EncoderFn(torch.autograd.Function):
@@ -369,7 +464,7 @@ class Decoder(_EngineOwner, nn.Module):
         self._t2_link()
 
     def _t2_children(self):
-        return (self.prenet,)
+        return (self.prenet, self.attention_layer, self.attention_layer.location_layer)
 
     def get_go_frame(self, memory):
         """model.py:243-256."""
@@ -381,6 +476,110 @@ class Decoder(_EngineOwner, nn.Module):
         decoder_inputs = decoder_inputs.view(decoder_inputs.size(0),
                                              int(decoder_inputs.size(1) / self.n_frames_per_step), -1)
         return decoder_inputs.transpose(0, 1)
+
+    def parse_decoder_outputs(self, mel_outputs, gate_outputs, alignments):
+        """model.py:311-338: lists of per-step (B, n_mel), (B, 1) / (B,), (B, T_enc) -> mel (B, n_mel, T_out), gate
+        (B, T_out[, 1]), alignments (B, T_out, T_enc)."""
+        alignments = torch.stack(alignments).transpose(0, 1)
+        gate_outputs = torch.stack(gate_outputs).transpose(0, 1)
+        gate_outputs = gate_outputs.contiguous()
+        mel_outputs = torch.stack(mel_outputs).transpose(0, 1).contiguous()
+        mel_outputs = mel_outputs.view(mel_outputs.size(0), -1, self.n_mel_channels)
+        mel_outputs = mel_outputs.transpose(1, 2)
+        return mel_outputs, gate_outputs, alignments
+
+    # -- the step API: the reference's own decoder loop, one library call per step (README "custom decoder loops") ----
+    _STATE = ("attention_hidden", "attention_cell", "decoder_hidden", "decoder_cell", "attention_weights",
+              "attention_weights_cum", "attention_context")
+
+    def initialize_decoder_states(self, memory, mask):
+        """model.py:258-289: the seven recurrent states as zeros of the reference's shapes in memory's dtype, memory,
+        processed_memory = memory_layer(memory) (on the engine) and mask (None, or bool (B, T_enc), True at padded
+        positions).  T_enc is at most 1282 (the stepwise attention kernel's limit)."""
+        what = "Decoder.initialize_decoder_states"
+        _require_no_grad(self, what, _STEP_NO_GRAD)
+        dev = self._t2_device()
+        if not torch.is_tensor(memory) or memory.dim() != 3:
+            raise ValueError("tacotron2_b200: %s: memory must be a (B, T_enc, %d) tensor" % (what, self.encoder_embedding_dim))
+        B, T = int(memory.shape[0]), int(memory.shape[1])
+        if B < 1 or T < 1:
+            raise ValueError("tacotron2_b200: %s: memory must not be empty (got %s)" % (what, tuple(memory.shape)))
+        _step_tensor(memory, "memory", (B, T, self.encoder_embedding_dim), dev, what)
+        _step_t_enc(T, what)
+        _step_mask(mask, B, T, dev, what)
+        eng = self._t2_engine()
+        z = dict(device=memory.device, dtype=memory.dtype)
+        self.attention_hidden = torch.zeros(B, self.attention_rnn_dim, **z)
+        self.attention_cell = torch.zeros(B, self.attention_rnn_dim, **z)
+        self.decoder_hidden = torch.zeros(B, self.decoder_rnn_dim, **z)
+        self.decoder_cell = torch.zeros(B, self.decoder_rnn_dim, **z)
+        self.attention_weights = torch.zeros(B, T, **z)
+        self.attention_weights_cum = torch.zeros(B, T, **z)
+        self.attention_context = torch.zeros(B, self.encoder_embedding_dim, **z)
+        self.memory = memory
+        self.processed_memory = eng.processed_memory(_f32(memory)).to(memory.dtype)
+        self.mask = mask
+
+    def decode(self, decoder_input):
+        """model.py:340-379: one decoder step on the states the attributes hold at the call.  decoder_input (B, 256) is
+        the prenet output.  Returns (decoder_output (B, n_mel), gate_prediction (B, 1), attention_weights (B, T_enc)) in
+        memory's dtype.  As in the reference the six other states get new tensors, attention_weights_cum is updated in
+        place and the returned weights are the new attention_weights; nothing returned or stored by one call is changed
+        by the next.  Training mode applies the attention / decoder dropout with keys from a seed drawn per call
+        (injected att / dec masks of one step, (B, 1024), take precedence); score_mask_value is read at every call."""
+        what = "Decoder.decode"
+        _require_no_grad(self, what, _STEP_NO_GRAD)
+        memory = self.__dict__.get("memory")
+        if memory is None:
+            raise RuntimeError("tacotron2_b200: %s: call initialize_decoder_states(memory, mask) first" % what)
+        dev = self._t2_device()
+        B, T = int(memory.shape[0]), int(memory.shape[1])
+        _step_tensor(memory, "memory", (B, T, self.encoder_embedding_dim), dev, what)
+        _step_t_enc(T, what)
+        _step_tensor(decoder_input, "decoder_input", (B, self.prenet_dim), dev, what)
+        shapes = dict(attention_hidden=(B, self.attention_rnn_dim), attention_cell=(B, self.attention_rnn_dim),
+                      decoder_hidden=(B, self.decoder_rnn_dim), decoder_cell=(B, self.decoder_rnn_dim),
+                      attention_weights=(B, T), attention_weights_cum=(B, T),
+                      attention_context=(B, self.encoder_embedding_dim))
+        st = {k: _step_tensor(self.__dict__.get(k), k, shapes[k], dev, what) for k in self._STATE}
+        pm = _step_tensor(self.__dict__.get("processed_memory"), "processed_memory",
+                          (B, T, self.attention_layer.memory_layer.linear_layer.out_features), dev, what)
+        mask = _step_mask(self.__dict__.get("mask"), B, T, dev, what)
+        keys = dict(att=None, dec=None)
+        seed = 0
+        if self.training:
+            masks = current_masks()
+            for k, n in (("att", self.attention_rnn_dim), ("dec", self.decoder_rnn_dim)):
+                if masks[k] is not None:
+                    keys[k] = _engine_mod._u8(masks[k], dev).reshape(-1)
+                    if keys[k].numel() != B * n:
+                        raise ValueError("tacotron2_b200: %s: injected %s masks must hold one step, (B, %d) (got %s)"
+                                         % (what, k, n, tuple(masks[k].shape)))
+            seed = next_seed()
+        eng = self._t2_engine()
+        # the six states that get new tensors, copied into one fresh fp32 buffer the step updates in place
+        new = ("attention_hidden", "attention_cell", "decoder_hidden", "decoder_cell", "attention_context",
+               "attention_weights")
+        buf = torch.cat([st[k].detach().reshape(-1) for k in new]).to(torch.float32)
+        views, off = {}, 0
+        for k in new:
+            n = shapes[k][0] * shapes[k][1]
+            views[k] = buf[off:off + n].view(shapes[k])
+            off += n
+        cum = st["attention_weights_cum"]
+        cum32 = cum if (cum.dtype == torch.float32 and cum.is_contiguous()) else _f32(cum)
+        mel, gate = eng.decoder_step(
+            _f32(memory), _f32(pm), mask,
+            [views[k] for k in ("attention_hidden", "attention_cell", "decoder_hidden", "decoder_cell",
+                                "attention_weights")] + [cum32, views["attention_context"]],
+            _f32(decoder_input), self.training, keys["att"], keys["dec"], seed, float(self.attention_layer.score_mask_value))
+        if cum32 is not cum:
+            with torch.no_grad():
+                cum.copy_(cum32)
+        dt = memory.dtype
+        for k in new:
+            setattr(self, k, views[k] if dt == torch.float32 else views[k].to(dt))
+        return mel.to(dt), gate.to(dt), self.attention_weights
 
     def _teacher_forward(self, memory, decoder_inputs, memory_lengths, keep_stash):
         """Shared by the no-grad path and _DecoderFn.forward.  Returns (mel (B,T,80), gate, align, saved)."""
@@ -595,7 +794,8 @@ class Tacotron2(_EngineOwner, nn.Module):
         self._t2_link()
 
     def _t2_children(self):
-        return (self.encoder, self.decoder, self.postnet, self.decoder.prenet)
+        return (self.encoder, self.decoder, self.postnet, self.decoder.prenet, self.decoder.attention_layer,
+                self.decoder.attention_layer.location_layer)
 
     def parse_batch(self, batch):
         """model.py:473-485."""
