@@ -576,6 +576,59 @@ typedef struct T2DurationsArgs {
 size_t t2_durations_workspace_bytes(int32_t B, int32_t T_mel, int32_t T_text, int32_t method);
 int    t2_durations(const T2DurationsArgs* a, void* stream);
 
+/* ---- Pitch targets (tacotron2_b200.pyin / average_by_durations; DESIGN section 6.11) ------------------------------
+ * pYIN as librosa 0.10 computes it with center=True, pad_mode="constant", in fp64: y (B, n) fp32 row-major -> f0,
+ * voiced_flag and voiced_prob, each (B, F) with F = 1 + n / hop_length (the frame count of t2_mel_spectrogram at
+ * hop 256).  Row b reads only y[b, :L] (L = lengths[b]; a NULL array means n for every row), zero-pads it by
+ * frame_length / 2 on both sides and has 1 + L / hop_length frames, so it equals its own B = 1 call; its later frames
+ * get f0 0, voiced_flag 0 and voiced_prob 0.  Device lengths are clamped into [1, n] (the Python mirror refuses them).
+ * Samples must be finite (not checked here; the Python mirror does).
+ * The parameters arrive derived, as the host computes them from librosa's (tacotron2_b200.pitch.pyin_tables):
+ *   min_period = floor(sr / fmax), max_period = min(ceil(sr / fmin), frame_length - win_length - 1) > min_period;
+ *   n_bins = floor(12 bins_per_semitone log2(fmax / fmin)) + 1 <= T2_PYIN_MAX_BINS (the Viterbi CTA keeps 136 bytes
+ *   per bin in shared memory); width = the local-triangle transition width, h = width / 2;
+ *   thresholds[k] = linspace(0, 1, n_thresholds + 1)[k + 1], beta_probs = diff(beta.cdf(thresholds)),
+ *   beta_prefix[m] = numpy sum(beta_probs[:m]) (m = 0..n_thresholds);
+ *   boltzmann[N (N - 1) / 2 + p] = boltzmann.pmf(p, boltzmann_parameter, N) for N = 1..(max_period - min_period + 2) / 2,
+ *   p < N;
+ *   log_trans (2, 2h + 1, n_bins): [s][k][j] = log(T + tiny) of the transition from bin j - h + k to bin j within a
+ *   voicing half (s = 0) or across (s = 1), T = kron(transition_loop(2, 1 - switch_prob), transition_local(n_bins,
+ *   width, "triangle")); out of the band every entry is log(tiny) = log_tiny;
+ *   log_init_unvoiced = log(1 / n_bins + tiny); freqs[k] = fmin 2^(k / (12 bins_per_semitone)).
+ * f0 is freqs[state] on voiced frames and fill_na on unvoiced ones.  The decoded path equals the dense Viterbi's
+ * (numpy argmax ties: the smallest index).  Bad sizes or a NULL pointer are T2_ERR_INVALID, too small a workspace
+ * T2_ERR_WORKSPACE, before anything is launched.  2 launches, no handle, no allocation, no host synchronisation.
+ * Workspace: t2_pyin_workspace_bytes(a) (reads only the sizes; 0 for arguments the call refuses): per frame
+ * 4 n_bins + 10 ceil(lags / 2) + 12 bytes, lags = max_period - min_period + 1. */
+#define T2_PYIN_MAX_FRAME       2048
+#define T2_PYIN_MAX_BINS        1536
+#define T2_PYIN_MAX_THRESHOLDS  4096
+typedef struct T2PyinArgs {
+  const float* y;                      /* (B, n) */
+  const int32_t* lengths;              /* (B) device or NULL: samples per row */
+  int32_t B, n, sr, frame_length, win_length, hop_length;
+  int32_t min_period, max_period, n_thresholds, n_bins, bins_per_semitone, width;
+  double fmin, no_trough_prob, fill_na, log_tiny, log_init_unvoiced;
+  const double* thresholds;            /* (n_thresholds) */
+  const double* beta_probs;            /* (n_thresholds) */
+  const double* beta_prefix;           /* (n_thresholds + 1) */
+  const double* boltzmann;             /* (N_max (N_max + 1) / 2) */
+  const double* log_trans;             /* (2, 2 (width / 2) + 1, n_bins) */
+  const double* freqs;                 /* (n_bins) */
+  double* f0;                          /* out (B, F) */
+  uint8_t* voiced_flag;                /* out (B, F) */
+  double* voiced_prob;                 /* out (B, F) */
+  void* ws; size_t ws_bytes;
+} T2PyinArgs;
+size_t t2_pyin_workspace_bytes(const T2PyinArgs* a);
+int    t2_pyin(const T2PyinArgs* a, void* stream);
+/* values (B, F) fp64 and durations (B, T_text) int64, both on the device -> out (B, T_text) fp32: for symbol j the mean
+ * of the values[b, f] that are neither 0 nor NaN over f in [cum_j, cum_{j+1}) (cum = the row's running sum of
+ * durations), summed in fp64 in frame order; 0 for a span without any.  Negative durations count as 0 and spans are cut
+ * at F (the Python mirror refuses both).  One launch, no host synchronisation. */
+int    t2_average_by_durations(const double* values, const int64_t* durations, int32_t B, int32_t F, int32_t T_text,
+                               float* out, void* stream);
+
 /* ---- WaveGlow vocoder inference (waveglow/glow.py: WaveGlow.infer, glow.py:251-293) ---------------
  * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  Supported configurations (the published
  * one, waveglow/config.json, is the comment beside each field): n_mel_channels 80, n_group 8, wn_kernel_size 3,

@@ -3,6 +3,7 @@ and Griffin-Lim behind the NVIDIA/tacotron2 nn.Module API.  See DESIGN.md / INTE
 from ._engine import alignments_from_durations, dropout_masks, durations_from_alignments, invalidate_weights  # noqa: F401
 from .hparams import create_hparams  # noqa: F401
 from .layers import TacotronSTFT  # noqa: F401
+from .pitch import average_by_durations, pyin  # noqa: F401
 from .loss_function import Tacotron2Loss  # noqa: F401
 from .model import Decoder, Encoder, Postnet, Tacotron2  # noqa: F401
 from . import amp  # noqa: F401
@@ -16,4 +17,5 @@ from .serving import InferenceServer  # noqa: F401
 __all__ = ["Tacotron2", "Encoder", "Decoder", "Postnet", "Tacotron2Loss", "create_hparams", "dropout_masks",
            "FusedClipAdam", "AmpFusedClipAdam", "amp", "invalidate_weights", "TacotronSTFT",
            "WaveGlow", "waveglow_noise", "window_halo", "Denoiser", "denoiser_halo", "STFT", "griffin_lim",
-           "InferenceServer", "alignments_from_durations", "durations_from_alignments"]
+           "InferenceServer", "alignments_from_durations", "durations_from_alignments", "pyin",
+           "average_by_durations"]

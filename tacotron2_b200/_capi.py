@@ -15,6 +15,7 @@ IMPL_AUTO, IMPL_STEPWISE, IMPL_PERSISTENT = 0, 1, 2
 MODE_INFER, MODE_TEACHER = 0, 1
 DURATIONS_MAS, DURATIONS_ARGMAX = 0, 1
 DURATIONS_MAX_TEXT = 4096           # T2_DURATIONS_MAX_TEXT
+PYIN_MAX_FRAME, PYIN_MAX_BINS, PYIN_MAX_THRESHOLDS = 2048, 1536, 4096   # T2_PYIN_MAX_*
 
 EXPORTS = [
     "t2_abi_version", "t2_last_error", "t2_device_info", "t2_model_create", "t2_model_refresh",
@@ -41,6 +42,7 @@ EXPORTS = [
     "t2_stft_transform_workspace_bytes", "t2_stft_transform", "t2_stft_inverse_workspace_bytes", "t2_stft_inverse",
     "t2_griffin_lim_workspace_bytes", "t2_griffin_lim",
     "t2_durations_workspace_bytes", "t2_durations",
+    "t2_pyin_workspace_bytes", "t2_pyin", "t2_average_by_durations",
     "t2_decoder_step_workspace_bytes", "t2_decoder_step", "t2_attention_forward", "t2_processed_memory",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686       # the published configuration's; t2_waveglow_num_weights gives any other's
@@ -182,6 +184,15 @@ class T2DurationsArgs(C.Structure):
     _fields_ = [("alignments", C.c_void_p), ("input_lengths", C.c_void_p), ("mel_lengths", C.c_void_p),
                 ("B", C.c_int32), ("T_mel", C.c_int32), ("T_text", C.c_int32), ("method", C.c_int32),
                 ("durations", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
+class T2PyinArgs(C.Structure):
+    _fields_ = [("y", C.c_void_p), ("lengths", C.c_void_p)] + [
+        (n, C.c_int32) for n in ("B", "n", "sr", "frame_length", "win_length", "hop_length", "min_period",
+                                 "max_period", "n_thresholds", "n_bins", "bins_per_semitone", "width")] + [
+        (n, C.c_double) for n in ("fmin", "no_trough_prob", "fill_na", "log_tiny", "log_init_unvoiced")] + [
+        (n, C.c_void_p) for n in ("thresholds", "beta_probs", "beta_prefix", "boltzmann", "log_trans", "freqs",
+                                  "f0", "voiced_flag", "voiced_prob", "ws")] + [("ws_bytes", C.c_size_t)]
 
 
 class T2PostnetArgs(C.Structure):
@@ -352,6 +363,11 @@ def lib():
     L.t2_durations_workspace_bytes.restype = C.c_size_t
     L.t2_durations_workspace_bytes.argtypes = [C.c_int32] * 4
     L.t2_durations.argtypes = [C.POINTER(T2DurationsArgs), C.c_void_p]
+    L.t2_pyin_workspace_bytes.restype = C.c_size_t
+    L.t2_pyin_workspace_bytes.argtypes = [C.POINTER(T2PyinArgs)]
+    L.t2_pyin.argtypes = [C.POINTER(T2PyinArgs), C.c_void_p]
+    L.t2_average_by_durations.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                          C.c_void_p]
     if L.t2_abi_version() != 2:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L
