@@ -629,6 +629,42 @@ int    t2_pyin(const T2PyinArgs* a, void* stream);
 int    t2_average_by_durations(const double* values, const int64_t* durations, int32_t B, int32_t F, int32_t T_text,
                                float* out, void* stream);
 
+/* ---- Dynamic time warping (tacotron2_b200.dtw / mel_cepstral_distortion; DESIGN section 6.12) ---------------------
+ * x (B, D, T_x) and y (B, D, T_y), both fp32 (dtype T2_DTW_F32) or both fp64 (T2_DTW_F64), row-major -> per row b the
+ * cheapest monotonic path through C[i, j] = sqrt(sum_d (x[b, d, i] - y[b, d, j])^2) (fp64, summed in the order
+ * d = 0 .. D - 1 without contraction) from (0, 0) to (L_x - 1, L_y - 1) with steps (1, 1), (0, 1), (1, 0) and unit
+ * weights: D[0, 0] = C[0, 0], D[i, j] = C[i, j] + min(D[i-1, j-1], D[i, j-1], D[i-1, j]), ties to the diagonal, then
+ * (i, j - 1), then (i - 1, j).  Row b reads only x[b, :, :L_x] and y[b, :, :L_y] (L = the lengths; a NULL array means
+ * the full size; device lengths are clamped into [1, T], the Python mirror refuses them).
+ * Out: cost (B) fp64 = D[L_x - 1, L_y - 1]; path (B, T_x + T_y - 1, 2) int64, the (i, j) pairs from (0, 0) on, padded
+ * with -1; path_lengths (B) int64.  D > T2_DTW_MAX_DIM or T_x, T_y > T2_DTW_MAX_FRAMES are T2_ERR_UNSUPPORTED, other
+ * bad sizes or a NULL pointer T2_ERR_INVALID, too small a workspace T2_ERR_WORKSPACE, before anything is launched.
+ * 1 launch, no handle, no allocation, no host synchronisation.  Workspace: t2_dtw_workspace_bytes (0 for sizes the
+ * call refuses): the 2-bit predecessor map, (T_x + T_y - 1) W 8 bytes per row with W = min(ceil(T_x / 32),
+ * ceil(min(T_x, T_y) / 32) + 1), when it exceeds 96 KB (it stays in shared memory otherwise).
+ * t2_mel_cepstra: mel (B, n_mel, T) fp32 / fp64 -> cep (B, n_cep, T) fp64, cep[b, k, t] = sum_m table[k, m] mel[b, m, t]
+ * in the order m = 0 .. n_mel - 1 without contraction, for t < lengths[b] (NULL: T), 0 after; table (n_cep, n_mel) fp64
+ * on the device, 1 <= n_cep < n_mel <= T2_DTW_MAX_DIM, T <= T2_DTW_MAX_FRAMES, B <= 65535.  1 launch. */
+#define T2_DTW_MAX_FRAMES 8192
+#define T2_DTW_MAX_DIM    1024
+#define T2_DTW_F32        0
+#define T2_DTW_F64        1
+typedef struct T2DtwArgs {
+  const void* x;                       /* (B, D, T_x) */
+  const void* y;                       /* (B, D, T_y) */
+  const int32_t* x_lengths;            /* (B) device or NULL */
+  const int32_t* y_lengths;            /* (B) device or NULL */
+  int32_t B, D, T_x, T_y, dtype;
+  double* cost;                        /* out (B) */
+  int64_t* path;                       /* out (B, T_x + T_y - 1, 2) */
+  int64_t* path_lengths;               /* out (B) */
+  void* ws; size_t ws_bytes;
+} T2DtwArgs;
+size_t t2_dtw_workspace_bytes(int32_t B, int32_t D, int32_t T_x, int32_t T_y, int32_t dtype);
+int    t2_dtw(const T2DtwArgs* a, void* stream);
+int    t2_mel_cepstra(const void* mel, int32_t dtype, const int32_t* lengths, int32_t B, int32_t n_mel, int32_t T,
+                      const double* table, int32_t n_cep, double* cep, void* stream);
+
 /* ---- WaveGlow vocoder inference (waveglow/glow.py: WaveGlow.infer, glow.py:251-293) ---------------
  * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  Supported configurations (the published
  * one, waveglow/config.json, is the comment beside each field): n_mel_channels 80, n_group 8, wn_kernel_size 3,

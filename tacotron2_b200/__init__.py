@@ -4,6 +4,7 @@ from ._engine import alignments_from_durations, dropout_masks, durations_from_al
 from .hparams import create_hparams  # noqa: F401
 from .layers import TacotronSTFT  # noqa: F401
 from .pitch import average_by_durations, pyin  # noqa: F401
+from .evaluation import dtw, mel_cepstral_distortion, pitch_errors  # noqa: F401
 from .loss_function import Tacotron2Loss  # noqa: F401
 from .model import Decoder, Encoder, Postnet, Tacotron2  # noqa: F401
 from . import amp  # noqa: F401
@@ -18,4 +19,4 @@ __all__ = ["Tacotron2", "Encoder", "Decoder", "Postnet", "Tacotron2Loss", "creat
            "FusedClipAdam", "AmpFusedClipAdam", "amp", "invalidate_weights", "TacotronSTFT",
            "WaveGlow", "waveglow_noise", "window_halo", "Denoiser", "denoiser_halo", "STFT", "griffin_lim",
            "InferenceServer", "alignments_from_durations", "durations_from_alignments", "pyin",
-           "average_by_durations"]
+           "average_by_durations", "dtw", "mel_cepstral_distortion", "pitch_errors"]

@@ -16,6 +16,8 @@ MODE_INFER, MODE_TEACHER = 0, 1
 DURATIONS_MAS, DURATIONS_ARGMAX = 0, 1
 DURATIONS_MAX_TEXT = 4096           # T2_DURATIONS_MAX_TEXT
 PYIN_MAX_FRAME, PYIN_MAX_BINS, PYIN_MAX_THRESHOLDS = 2048, 1536, 4096   # T2_PYIN_MAX_*
+DTW_MAX_FRAMES, DTW_MAX_DIM = 8192, 1024                                # T2_DTW_MAX_FRAMES, T2_DTW_MAX_DIM
+DTW_F32, DTW_F64 = 0, 1
 
 EXPORTS = [
     "t2_abi_version", "t2_last_error", "t2_device_info", "t2_model_create", "t2_model_refresh",
@@ -43,6 +45,7 @@ EXPORTS = [
     "t2_griffin_lim_workspace_bytes", "t2_griffin_lim",
     "t2_durations_workspace_bytes", "t2_durations",
     "t2_pyin_workspace_bytes", "t2_pyin", "t2_average_by_durations",
+    "t2_dtw_workspace_bytes", "t2_dtw", "t2_mel_cepstra",
     "t2_decoder_step_workspace_bytes", "t2_decoder_step", "t2_attention_forward", "t2_processed_memory",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686       # the published configuration's; t2_waveglow_num_weights gives any other's
@@ -193,6 +196,12 @@ class T2PyinArgs(C.Structure):
         (n, C.c_double) for n in ("fmin", "no_trough_prob", "fill_na", "log_tiny", "log_init_unvoiced")] + [
         (n, C.c_void_p) for n in ("thresholds", "beta_probs", "beta_prefix", "boltzmann", "log_trans", "freqs",
                                   "f0", "voiced_flag", "voiced_prob", "ws")] + [("ws_bytes", C.c_size_t)]
+
+
+class T2DtwArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("x_lengths", C.c_void_p), ("y_lengths", C.c_void_p)] + [
+        (n, C.c_int32) for n in ("B", "D", "T_x", "T_y", "dtype")] + [
+        (n, C.c_void_p) for n in ("cost", "path", "path_lengths", "ws")] + [("ws_bytes", C.c_size_t)]
 
 
 class T2PostnetArgs(C.Structure):
@@ -368,6 +377,11 @@ def lib():
     L.t2_pyin.argtypes = [C.POINTER(T2PyinArgs), C.c_void_p]
     L.t2_average_by_durations.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                           C.c_void_p]
+    L.t2_dtw_workspace_bytes.restype = C.c_size_t
+    L.t2_dtw_workspace_bytes.argtypes = [C.c_int32] * 5
+    L.t2_dtw.argtypes = [C.POINTER(T2DtwArgs), C.c_void_p]
+    L.t2_mel_cepstra.argtypes = [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_int32,
+                                                                                         C.c_void_p, C.c_void_p]
     if L.t2_abi_version() != 2:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L
