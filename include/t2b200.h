@@ -740,6 +740,54 @@ void   t2_waveglow_window_halo(int32_t* left, int32_t* right);
 int    t2_waveglow_window_halo_config(const T2WaveGlowConfig* cfg, int32_t* left, int32_t* right);
 int    t2_waveglow_infer_window(T2WaveGlow* h, const T2WaveGlowWindowArgs* a, void* stream);
 
+/* ---- HiFi-GAN generator inference (the V1 / V2 / V3 generators of jik876/hifi-gan, models.py) ---------------------
+ * A separate handle: mel spectrogram (B, 80, T_mel) -> audio (B, 256 * T_mel).  Supported configurations (V1 is the
+ * comment beside each field): 80 mels; 1 ... 8 upsampling stages with even rates whose product is 256 and kernels
+ * k_i = 2 u_i; upsample_initial_channel and every stage's channel count (initial >> (i + 1)) multiples of 8 in
+ * 8 ... 512; 1 ... 8 resblock kernels, each odd and at most 15, with 3 dilations (resblock 1) or 2 (resblock 2) whose
+ * padding (k - 1) d / 2 is at most T2_HIFIGAN_MAX_PAD rows.  t2_hifigan_create returns T2_ERR_UNSUPPORTED for anything
+ * else, before any launch.  Precision tier as WaveGlow's: fp16 = 0 split-fp16 operands ("fp32 grade"), fp16 = 1 (a
+ * module converted with .half()) single fp16 operands; both accumulate in fp32. */
+#define T2_HIFIGAN_MAX_STAGES 8
+#define T2_HIFIGAN_MAX_KERNELS 8
+#define T2_HIFIGAN_MAX_PAD 64
+typedef struct T2HiFiGAN T2HiFiGAN;     /* opaque: configuration + packed device-side weights */
+typedef struct T2HiFiGANConfig {
+  int32_t n_mel_channels;                                       /* 80 */
+  int32_t resblock;                                             /* 1 (ResBlock1) or 2 (ResBlock2) */
+  int32_t n_upsamples;                                          /* 4 */
+  int32_t upsample_rates[T2_HIFIGAN_MAX_STAGES];                /* 8, 8, 2, 2 */
+  int32_t upsample_kernel_sizes[T2_HIFIGAN_MAX_STAGES];         /* 16, 16, 4, 4 */
+  int32_t upsample_initial_channel;                             /* 512 */
+  int32_t n_kernels;                                            /* 3 */
+  int32_t resblock_kernel_sizes[T2_HIFIGAN_MAX_KERNELS];        /* 3, 7, 11 */
+  int32_t resblock_dilation_sizes[T2_HIFIGAN_MAX_KERNELS][3];   /* (1, 3, 5) x 3; resblock 2 reads the first two */
+  int32_t fp16;                                                 /* 1: the weight table holds __half tensors */
+} T2HiFiGANConfig;
+
+/* Entries of the weight table: the generator's state_dict in its own order, (bias, weight_g, weight_v) for every
+ * convolution: conv_pre, ups.*, resblocks.* (ResBlock1: convs1.*, then convs2.*), conv_post.  A NULL weight_g entry
+ * means the weight norm was removed and the weight_v entry is the plain weight.  weight_g is folded along dim 0, the
+ * output channel of a Conv1d and the input channel of a ConvTranspose1d.  0 for a NULL or unsupported configuration. */
+int32_t t2_hifigan_num_weights(const T2HiFiGANConfig* cfg);
+int t2_hifigan_create(T2HiFiGAN** out, const T2HiFiGANConfig* cfg, const void* const* weights, int32_t n_weights,
+                      void* stream);
+int t2_hifigan_refresh(T2HiFiGAN* h, const void* const* weights, int32_t n_weights, void* stream);
+int t2_hifigan_destroy(T2HiFiGAN* h);
+
+/* mel (B, 80, T_mel), fp32 or (io_half) __half.  lengths (B) int32 in mel frames or NULL (values are clamped to
+ * [0, T_mel]): row b's samples [0, 256 lengths[b]) equal a call on that row's first lengths[b] frames alone, bit for
+ * bit; later samples are zero.  audio (B, 256 T_mel) out, in the mel's dtype.  B * (256 T_mel + the configuration's
+ * guard rows) must stay below 2^30, else T2_ERR_INVALID.  Workspace: t2_hifigan_workspace_bytes(h, B, T_mel); nothing
+ * is allocated and nothing waits for the device. */
+typedef struct T2HiFiGANArgs {
+  const void* mel; int32_t B, T_mel; const int32_t* lengths; int32_t io_half;
+  void* audio;
+  void* ws; size_t ws_bytes;
+} T2HiFiGANArgs;
+size_t t2_hifigan_workspace_bytes(const T2HiFiGAN* h, int32_t B, int32_t T_mel);
+int    t2_hifigan_infer(T2HiFiGAN* h, const T2HiFiGANArgs* a, void* stream);
+
 /* ---- WaveGlow denoiser (waveglow/denoiser.py: Denoiser, over stft.py:69-136 and audio_processing.py:7-56) -------
  * A separate handle holding the packed STFT bases.  The kernels are built for the reference default: filter_length
  * 1024, hop 256, win_length 1024, periodic Hann window; t2_denoiser_create returns T2_ERR_UNSUPPORTED for anything

@@ -10,6 +10,7 @@ from .model import Decoder, Encoder, Postnet, Tacotron2  # noqa: F401
 from . import amp  # noqa: F401
 from .glow import WaveGlow, waveglow_noise, window_halo  # noqa: F401
 from .denoiser import Denoiser, denoiser_halo  # noqa: F401
+from .hifigan import HiFiGAN  # noqa: F401
 from .stft import STFT  # noqa: F401
 from .audio_processing import griffin_lim  # noqa: F401
 from .optim import AmpFusedClipAdam, FusedClipAdam  # noqa: F401
@@ -17,6 +18,6 @@ from .serving import InferenceServer  # noqa: F401
 
 __all__ = ["Tacotron2", "Encoder", "Decoder", "Postnet", "Tacotron2Loss", "create_hparams", "dropout_masks",
            "FusedClipAdam", "AmpFusedClipAdam", "amp", "invalidate_weights", "TacotronSTFT",
-           "WaveGlow", "waveglow_noise", "window_halo", "Denoiser", "denoiser_halo", "STFT", "griffin_lim",
+           "WaveGlow", "waveglow_noise", "window_halo", "HiFiGAN", "Denoiser", "denoiser_halo", "STFT", "griffin_lim",
            "InferenceServer", "alignments_from_durations", "durations_from_alignments", "pyin",
            "average_by_durations", "dtw", "mel_cepstral_distortion", "pitch_errors"]

@@ -47,6 +47,8 @@ EXPORTS = [
     "t2_pyin_workspace_bytes", "t2_pyin", "t2_average_by_durations",
     "t2_dtw_workspace_bytes", "t2_dtw", "t2_mel_cepstra",
     "t2_decoder_step_workspace_bytes", "t2_decoder_step", "t2_attention_forward", "t2_processed_memory",
+    "t2_hifigan_num_weights", "t2_hifigan_create", "t2_hifigan_refresh", "t2_hifigan_destroy",
+    "t2_hifigan_workspace_bytes", "t2_hifigan_infer",
 ]
 T2_WAVEGLOW_NUM_WEIGHTS = 686       # the published configuration's; t2_waveglow_num_weights gives any other's
 
@@ -236,6 +238,19 @@ class T2WaveGlowWindowArgs(C.Structure):
                 ("z_frames", C.c_int32), ("at_end", C.c_int32)]
 
 
+class T2HiFiGANConfig(C.Structure):
+    _fields_ = [("n_mel_channels", C.c_int32), ("resblock", C.c_int32), ("n_upsamples", C.c_int32),
+                ("upsample_rates", C.c_int32 * 8), ("upsample_kernel_sizes", C.c_int32 * 8),
+                ("upsample_initial_channel", C.c_int32), ("n_kernels", C.c_int32),
+                ("resblock_kernel_sizes", C.c_int32 * 8), ("resblock_dilation_sizes", (C.c_int32 * 3) * 8),
+                ("fp16", C.c_int32)]
+
+
+class T2HiFiGANArgs(C.Structure):
+    _fields_ = [("mel", C.c_void_p), ("B", C.c_int32), ("T_mel", C.c_int32), ("lengths", C.c_void_p),
+                ("io_half", C.c_int32), ("audio", C.c_void_p), ("ws", C.c_void_p), ("ws_bytes", C.c_size_t)]
+
+
 class T2DenoiserConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("filter_length", "hop_length", "win_length", "window")]
 
@@ -382,6 +397,15 @@ def lib():
     L.t2_dtw.argtypes = [C.POINTER(T2DtwArgs), C.c_void_p]
     L.t2_mel_cepstra.argtypes = [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_int32,
                                                                                          C.c_void_p, C.c_void_p]
+    L.t2_hifigan_num_weights.restype = C.c_int32
+    L.t2_hifigan_num_weights.argtypes = [C.POINTER(T2HiFiGANConfig)]
+    L.t2_hifigan_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(T2HiFiGANConfig), C.POINTER(C.c_void_p),
+                                    C.c_int32, C.c_void_p]
+    L.t2_hifigan_refresh.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.c_void_p]
+    L.t2_hifigan_destroy.argtypes = [C.c_void_p]
+    L.t2_hifigan_workspace_bytes.restype = C.c_size_t
+    L.t2_hifigan_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    L.t2_hifigan_infer.argtypes = [C.c_void_p, C.POINTER(T2HiFiGANArgs), C.c_void_p]
     if L.t2_abi_version() != 2:
         raise RuntimeError("libt2b200.so ABI version mismatch")
     _lib = L

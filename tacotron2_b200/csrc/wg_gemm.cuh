@@ -10,6 +10,9 @@
 // The Tacotron2 convs (EPI_CONV) load one A tile of 132 rows per chunk instead: a k5 conv's 5 taps are that same tile
 // addressed with the descriptor start shifted by tap * 16 bytes, so the tile crosses shared memory once per chunk.
 //
+// The HiFi-GAN convolutions (EPI_HIFI, hifigan.cu) have up to 15 taps: their K is seg[0]'s chunks read at ntaps row
+// shifts seg[0].shift + tap * dil, tap-major.
+//
 // Tiers: fp32-grade = hi*hi + lo*hi + hi*lo (3 MMAs per K step); fp16 = hi*hi only, lo planes neither read nor written.
 #pragma once
 #include <float.h>
@@ -44,7 +47,7 @@ __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) {
 }
 
 enum { EPI_UPSAMPLE = 0, EPI_GATE = 1, EPI_RESSKIP = 2, EPI_SPECTRAL = 3, EPI_OVERLAP = 4, EPI_CONV = 5, EPI_PROJECT = 6,
-       EPI_MAGPHASE = 7 };
+       EPI_MAGPHASE = 7, EPI_HIFI = 8 };
 
 // A tile rows beyond the output tile: EPI_CONV's tile m0 reads padded rows [m0 - 2, m0 + 130), every other epilogue
 // 128 rows per segment.
@@ -79,6 +82,14 @@ struct GemmParams {
   float* out_f32; long ldo; int out_seq_rows;
   const float* residual; long res_batch_stride;
   int skip_cols;                                     // RESSKIP: skip columns (the WN width); later columns are padding
+  // HIFI: K = ntaps x seg[0]'s chunks, tap k at row shift seg[0].shift + k * dil.  Tile row q = b * span + t is input
+  // row t; column n = phase * cout + channel is output row t * phases + phase, plane row out_row0 + b * col_span + that
+  // (output rows >= col_span are not written).  Rows past len[b] * len_mul (or T * phases) are zeros.  x = acc + bias
+  // (+ res_in) goes to x_out (or null); act planes `out` get lrelu(x, slope).  mrf (fp32, rows (b * col_span + row) x
+  // cout): mrf = x (mrf_first) or mrf + x; with mrf_div > 0, `out` gets lrelu(mrf / mrf_div, slope) instead.
+  int ntaps, dil, phases;
+  const __half* res_in; __half* x_out;
+  float* mrf; int mrf_first; float mrf_div, slope;
 };
 
 template <int PASSES>
@@ -163,12 +174,17 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
         ptx::mbar_arrive_expect_tx(&a_full[sa], kABytes);
         const __half* base = nullptr; long rows = 0; int shift = 0, cc = 0, rem = c;
         bool found = false;
+        if (EPI == EPI_HIFI) {
+          const int tap = c / p.seg[0].nchunks;
+          base = p.seg[0].planes; rows = p.seg[0].rows; shift = p.seg[0].shift + tap * p.dil; cc = c - tap * p.seg[0].nchunks;
+        } else {
 #pragma unroll
         for (int s = 0; s < 4; ++s)
           if (!found && s < p.nseg) {
             if (rem < p.seg[s].nchunks) { base = p.seg[s].planes; rows = p.seg[s].rows; shift = p.seg[s].shift; cc = rem; found = true; }
             else rem -= p.seg[s].nchunks;
           }
+        }
         const long r0 = p.row0 + (long)mrow * kTile + shift;
         for (int g = 0; g < 8; ++g)
           for (int hl = 0; hl < (PASSES == 3 ? 2 : 1); ++hl) {
@@ -368,6 +384,54 @@ __global__ void __launch_bounds__(kThreads, 1) wg_gemm_kernel(const GemmParams p
               v[i] = in_row ? y * 4.f : 0.f;
             }
             *reinterpret_cast<float4*>(dst + c) = make_float4(v[0], v[1], v[2], v[3]);
+          }
+        }
+      } else if (EPI == EPI_HIFI) {
+        // thread = (tile row r, half of the columns)
+        constexpr int kHalf = NT * NH / 2;
+        if (b < p.B) {
+          const long lout = (long)p.T * p.phases;
+          const long lim = p.len ? min(lout, (long)max(p.len[b], 0) * p.len_mul) : lout;
+          for (int g = 0; g < kHalf / 8; ++g) {
+            const int cl = half * kHalf + g * 8, n = nt * NT * NH + cl;
+            if (n >= p.phases * p.cout) break;
+            const int ph = n / p.cout, ch = n - ph * p.cout;
+            const long to = (long)t * p.phases + ph;
+            if (to >= p.col_span) continue;
+            const bool live = to < lim;
+            const long orow = p.out_row0 + (long)b * p.col_span + to;
+            float v[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = row[cl + i] + p.bias[ch + i];
+            if (p.res_in) {
+              float rv[8];
+              load8<PASSES>(p.res_in, p.out_rows, ch >> 3, orow, rv);
+#pragma unroll
+              for (int i = 0; i < 8; ++i) v[i] += rv[i];
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = live ? v[i] : 0.f;
+            if (p.x_out) store8<PASSES>(p.x_out, p.out_rows, ch >> 3, orow, v);
+            if (p.mrf) {
+              float4* sm = reinterpret_cast<float4*>(p.mrf + ((long)b * p.col_span + to) * p.cout + ch);
+              float4 s0 = make_float4(v[0], v[1], v[2], v[3]), s1 = make_float4(v[4], v[5], v[6], v[7]);
+              if (!p.mrf_first) {
+                const float4 o0 = sm[0], o1 = sm[1];
+                s0 = make_float4(o0.x + v[0], o0.y + v[1], o0.z + v[2], o0.w + v[3]);
+                s1 = make_float4(o1.x + v[4], o1.y + v[5], o1.z + v[6], o1.w + v[7]);
+              }
+              if (p.mrf_div > 0.f) {
+                v[0] = s0.x / p.mrf_div; v[1] = s0.y / p.mrf_div; v[2] = s0.z / p.mrf_div; v[3] = s0.w / p.mrf_div;
+                v[4] = s1.x / p.mrf_div; v[5] = s1.y / p.mrf_div; v[6] = s1.z / p.mrf_div; v[7] = s1.w / p.mrf_div;
+              } else {
+                sm[0] = s0; sm[1] = s1;
+              }
+            }
+            if (p.out) {
+#pragma unroll
+              for (int i = 0; i < 8; ++i) v[i] = v[i] > 0.f ? v[i] : v[i] * p.slope;
+              store8<PASSES>(p.out, p.out_rows, ch >> 3, orow, v);
+            }
           }
         }
       } else if (EPI == EPI_CONV) {
