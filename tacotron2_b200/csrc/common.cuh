@@ -1,5 +1,6 @@
 // Shared host/device helpers for libt2b200 (sm_90a only).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -67,6 +68,11 @@ enum W : int {
   W_COUNT = 84
 };
 static_assert(W_POST_CONV0 + 5 * 7 == W_COUNT, "state_dict table");
+
+// element i of a weight tensor the caller passes in fp32 (half 0) or fp16 (half 1)
+__device__ __forceinline__ float ldw(const void* p, long i, int half) {
+  return half ? __half2float(reinterpret_cast<const __half*>(p)[i]) : reinterpret_cast<const float*>(p)[i];
+}
 
 // ---- buffer layouts ------------------------------------------------------------------------------
 // Bump allocator over one buffer.  Each buffer has one layout function that take()s its regions in order; the size

@@ -1,6 +1,6 @@
 // Tensor-core conv1d / GEMM for the Encoder (model.py:157-167, 174-175), the BiLSTM input projection
 // (model.py:169-171) and the Postnet (model.py:112-146): the split-fp16 implicit GEMM of wg_gemm.cuh with its conv
-// epilogue (EPI_CONV).  This file holds the operand formats and the host entry points.
+// epilogue (ConvEpi).  This file holds the operand formats, the epilogue and the host entry points.
 //
 //   out[(b,t), n] = epilogue( sum_{tap, ci} W[n][tap][ci] * x[(b, t + tap - pad), ci] )
 //
@@ -68,6 +68,30 @@ __global__ void embed_to_planes_kernel(const int64_t* __restrict__ text, const f
   store8<3>(planes, plane_rows, g, row, v);
 }
 
+__global__ void mel_to_planes_kernel(const void* __restrict__ mel, int io_half, int B, int T, const int32_t* __restrict__ len,
+                                     int guard, int span, __half* __restrict__ planes, long rows, int passes) {
+  const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int g = blockIdx.y;
+  if (row >= rows) return;
+  const long q = row - guard;
+  int b = -1, f = -1;
+  if (q >= 0) { b = (int)(q / span); f = (int)(q - (long)b * span); }
+  const bool valid = b >= 0 && b < B && f < (len == nullptr ? T : min(max(len[b], 0), T));
+  float v[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int c = g * 8 + i;
+    float x = 0.f;
+    if (valid && c < kMel) {
+      const long idx = ((long)b * kMel + c) * T + f;
+      x = io_half ? __half2float(reinterpret_cast<const __half*>(mel)[idx]) : reinterpret_cast<const float*>(mel)[idx];
+    }
+    v[i] = x;
+  }
+  if (passes == 3) store8<3>(planes, rows, g, row, v);
+  else store8<1>(planes, rows, g, row, v);
+}
+
 // W (cout, cin, taps) fp32 [or (cout, cin) when taps == 1] -> per (n-tile, chunk, tap) [hi | lo] SWIZZLE_128B
 // planes of NT rows x 64 channels; rows >= cout and channels >= cin are zero.
 __global__ void pack_conv_w_kernel(const float* __restrict__ w, int cout, int cin, int taps, int nt_rows,
@@ -96,6 +120,71 @@ __global__ void fold_bn_bias_kernel(const float* cbias, const float* g, const fl
   shift[c] = b[c] + ((cbias ? cbias[c] : 0.f) - mean[c]) * s;
 }
 
+
+// ---- the GEMM epilogue ----------------------------------------------------------------------------
+// Tile row q is padded row b * span + 2 + t (span = T + 4); y = act(acc * scale + bias), act 0 none, 1 relu, 2 tanh;
+// out_mode 0 writes the planes `out`, 1 fp32 rows (row of (b, t) = b * out_seq_rows + t, pitch ldo), 2 fp32
+// (B, cout, T) plus the residual (B, T, cout); len: frames t >= len[b] are zeros in modes 0 and 2.
+struct ConvEpi : EpiDefaults {
+  static constexpr KForm kK = KForm::kHaloTile;
+  // every tile is computed: the planes epilogue is what writes the zero padding rows the next layer reads
+  static constexpr bool kSkipTiles = false;
+  struct Params {
+    const float* bias; __half* out; long out_rows;
+    const float* scale; int act, out_mode, cout;
+    float* out_f32; long ldo; int out_seq_rows;
+    const float* residual; long res_batch_stride;
+  };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    // thread = (tile row r, every other group of 8 columns); frame pt of sequence b is tile row q
+    const int pt = t - 2;
+    const bool in_seq = b < m.B && pt >= 0 && pt < m.T;
+    // planes output: frames t >= len[b] are written as zeros, the padding a sequence of that length has alone
+    const bool in_len = in_seq && (p.out_mode != 0 || m.len == nullptr || pt < m.len[b]);
+    const int n0 = nt * NT * NH;
+    for (int c0 = half * 8; c0 < NT * NH; c0 += 16) {
+      float v[8];
+      const float4 v0 = *reinterpret_cast<const float4*>(row + c0);
+      const float4 v1 = *reinterpret_cast<const float4*>(row + c0 + 4);
+      v[0] = v0.x; v[1] = v0.y; v[2] = v0.z; v[3] = v0.w; v[4] = v1.x; v[5] = v1.y; v[6] = v1.z; v[7] = v1.w;
+      if (n0 + c0 >= p.cout) continue;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int n = n0 + c0 + i;
+        float x = v[i] * p.scale[n] + p.bias[n];
+        if (p.act == 1) x = fmaxf(x, 0.f);
+        else if (p.act == 2) x = tanhf(x);
+        v[i] = in_len ? x : 0.f;
+      }
+      if (p.out_mode == 0) {          // next layer's planes (zeros in the padding rows); plane row = q + 2
+        const int g = (n0 + c0) >> 3;
+        store8<3>(p.out, p.out_rows, g, q + 2, v);
+        // the 2 guard rows at both ends of the plane stay zero
+        if (q == 0 || q == (long)m.n_tiles_m * kTile - 1) {
+          const float z[8] = {};
+          const long gr = q == 0 ? 0 : q + 3;
+          for (int k = 0; k < 2; ++k) store8<3>(p.out, p.out_rows, g, gr + k, z);
+        }
+      } else if (in_seq && p.out_mode == 1) {   // fp32 rows (b * out_seq_rows + t, ldo)
+        float* o = p.out_f32 + ((long)b * p.out_seq_rows + pt) * p.ldo + n0 + c0;
+        *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
+        *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
+      } else if (in_seq && p.out_mode == 2) {   // (B, cout, T) + residual (B, T, cout), masked beyond len
+        const bool keep = m.len == nullptr || pt < m.len[b];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int n = n0 + c0 + i;
+          float x = v[i];
+          if (p.residual) x += p.residual[(long)b * p.res_batch_stride + (long)pt * p.cout + n];
+          p.out_f32[((long)b * p.cout + n) * m.T + pt] = keep ? x : 0.f;
+        }
+      }
+    }
+  }
+};
+
 }  // namespace
 
 // ---- host API -------------------------------------------------------------------------------------
@@ -103,7 +192,7 @@ long tc_plane_rows(int B, int T) {
   const long rpad = (long)B * (T + 4);
   return 4 + ((rpad + kTile - 1) / kTile) * kTile;
 }
-size_t tc_planes_bytes(int B, int T, int c_pad) { return (size_t)(c_pad / 8) * 2 * tc_plane_rows(B, T) * 16; }
+size_t tc_planes_bytes(int B, int T, int c_pad) { return planes_bytes(c_pad, tc_plane_rows(B, T)); }
 
 size_t tc_weights_bytes(int cout, int cin, int taps, int nt_rows) {
   return (size_t)((cout + nt_rows - 1) / nt_rows) * ((cin + 63) / 64) * taps * nt_rows * 256;
@@ -138,6 +227,14 @@ int tc_embed_to_planes(const int64_t* text, const float* emb, int n_symbols, con
   return T2_OK;
 }
 
+int tc_mel_to_planes(const void* mel, int io_half, int B, int T, const int32_t* len, int guard, int span, __half* planes,
+                     long rows, int passes, cudaStream_t s) {
+  mel_to_planes_kernel<<<dim3((unsigned)((rows + 127) / 128), 16), 128, 0, s>>>(mel, io_half, B, T, len, guard, span,
+                                                                               planes, rows, passes);
+  T2_LAUNCH_CHECK();
+  return T2_OK;
+}
+
 int tc_fold_bn(const float* cbias, const float* g, const float* b, const float* mean, const float* var, float eps,
                float* scale, float* shift, int C, cudaStream_t s) {
   fold_bn_bias_kernel<<<(C + 127) / 128, 128, 0, s>>>(cbias, g, b, mean, var, eps, scale, shift, C);
@@ -146,7 +243,7 @@ int tc_fold_bn(const float* cbias, const float* g, const float* b, const float* 
 }
 
 int tc_conv(const TcConvArgs& a, cudaStream_t s) {
-  GemmParams p;
+  Main p;
   memset(&p, 0, sizeof(p));
   const long rows = tc_plane_rows(a.B, a.T);
   // one segment from plane row 0: tile mt reads the padded rows [128 mt - 2, 128 mt + 130)
@@ -156,14 +253,12 @@ int tc_conv(const TcConvArgs& a, cudaStream_t s) {
   p.n_tiles_m = (int)((rows - 4) / kTile);
   // the grid covers every tile of the plane (rounded up to the cluster size)
   p.B = a.B; p.T = a.T; p.span = a.T + 4; p.lo = 0; p.hi = p.span; p.len = a.row_len;
-  p.scale = a.scale; p.bias = a.shift; p.act = a.act; p.out_mode = a.out_mode; p.cout = a.cout;
-  p.out = a.out_planes; p.out_rows = rows;
-  p.out_f32 = a.out_f32; p.ldo = a.ldo; p.out_seq_rows = a.out_seq_rows > 0 ? a.out_seq_rows : a.T;
-  p.residual = a.residual;
-  p.res_batch_stride = a.res_batch_stride ? a.res_batch_stride : (long)a.T * a.cout;
+  const ConvEpi::Params e{a.shift, a.out_planes, rows, a.scale, a.act, a.out_mode, a.cout,
+                          a.out_f32, a.ldo, a.out_seq_rows > 0 ? a.out_seq_rows : a.T,
+                          a.residual, a.res_batch_stride ? a.res_batch_stride : (long)a.T * a.cout};
   // weights are packed in stages of nt_rows rows; a CTA covers 2 stages' worth of columns when cout allows
-  if (a.nt_rows == 128) return launch_gemm<EPI_CONV, 3, 128, 2>(p, (a.cout + 255) / 256, s);
-  if (a.nt_rows == 80) return launch_gemm<EPI_CONV, 3, 80, 1>(p, (a.cout + 79) / 80, s);
+  if (a.nt_rows == 128) return launch_gemm<ConvEpi, 3, 128, 2>(p, e, (a.cout + 255) / 256, s);
+  if (a.nt_rows == 80) return launch_gemm<ConvEpi, 3, 80, 1>(p, e, (a.cout + 79) / 80, s);
   return fail(T2_ERR_INVALID, "tc_conv: unsupported n-tile %d", a.nt_rows);
 }
 

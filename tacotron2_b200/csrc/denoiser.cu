@@ -7,11 +7,11 @@
 //                       per 256-sample block (32 groups of 8 samples).
 //   forward             rows = frames; K = padded blocks f ... f + 3 (4 segments, row shifts -1 ... 2) x 256 samples;
 //                       N = the 1026 basis rows reordered so that each 256-column tile holds the real and imaginary rows
-//                       of the same 128 bins (5 tiles).  The epilogue (EPI_SPECTRAL) takes the magnitude, subtracts
+//                       of the same 128 bins (5 tiles).  The epilogue (SpectralEpi) takes the magnitude, subtracts
 //                       strength * bias, clamps at 0, rescales (re, im) and writes them as the next GEMM's planes.
 //   inverse             rows = output blocks; K = the 4 frames that overlap a block (segments at row shifts 0 ... 3,
 //                       each against its 256 columns of the inverse basis) x 1088 spectrum channels; N = 256.  The
-//                       overlap-add happens in the accumulator; the epilogue (EPI_OVERLAP) divides by window_sumsquare,
+//                       overlap-add happens in the accumulator; the epilogue (OverlapEpi) divides by window_sumsquare,
 //                       multiplies by 4, trims and writes fp32 audio.
 //
 // Rows of one sequence b: q = b * span + t, span = F + 4 for F = n / 256 + 1 frames.  The padded block i sits at plane
@@ -19,14 +19,15 @@
 // Only the fp32-grade tier (split fp16, 3 MMAs) exists: the reference denoises in fp32.
 //
 // The public STFT (stft.py:69-141) and Griffin-Lim (audio_processing.py:59-75) run on the same two GEMMs and planes:
-//   transform     row scale, pack, forward with EPI_MAGPHASE (fp32 magnitude and atan2 phase)
+//   transform     row scale, pack, forward with MagPhaseEpi (fp32 magnitude and atan2 phase)
 //   inverse       spec_pack_kernel ((magnitude, phase) -> spectrum planes), inverse
 //   Griffin-Lim   spec_pack_kernel, inverse, then per iteration: pack (of the previous signal), forward with
-//                 EPI_PROJECT (the target magnitude on the current phase), inverse: 3 n_iters + 2 launches.
+//                 ProjectEpi (the target magnitude on the current phase), inverse: 3 n_iters + 2 launches.
 // Their operands are scaled per row by a power of two taken on the device from the row's largest target magnitude (or
 // sample): the stored spectrum then peaks in [1, 2) and audio in [0.5, 1), the ranges in which the denoiser runs
 // unit-scale audio, whatever the caller's scale.  The fp32 outputs undo it exactly.
 #include <cooperative_groups.h>
+#include <float.h>
 #include <math.h>
 #include <string.h>
 #include <algorithm>
@@ -46,6 +47,15 @@ struct T2Denoiser {
 namespace t2 {
 namespace {
 
+// Spectrum planes (SpectrumEpi writes them, the inverse GEMM reads them): the real parts of the 513 bins in groups
+// 0 ... 64, the imaginary parts in groups 65 ... 129, zero up to 136 groups = 17 whole 64-channel chunks.
+constexpr int kBins = 513, kImGroup0 = 65, kSpecGroups = 136;
+// Operand ranges (a split fp16 value overflows at 65504).  The audio is packed as it is, so its samples must stay below
+// 65504 in magnitude.  The spectrum is stored as X / 512: |X| <= (sum of the window = 512) max |audio|, and the gate
+// never raises it for strength >= 0, so the stored value is bounded by max |audio| as well.  The inverse basis
+// (|w| <= 4.9e-4) is packed times 2^12 so that its lo halves stay out of fp16's subnormal range.  All three scales are
+// powers of two; OverlapEpi undoes them exactly.
+constexpr float kSpecScale = 1.f / 512.f, kInvBasisScale = 4096.f;
 constexpr int kFilter = 1024, kHop = 256, kBasisRows = 2 * kBins;
 constexpr int kFwdTiles = 5, kFwdN = kFwdTiles * 256;          // 5 x 128 bin slots >= 513 bins
 constexpr int kSpecCh = kSpecGroups * 8;                        // 1088 = 17 chunks
@@ -55,6 +65,109 @@ constexpr int kBlkGroups = kHop / 8;
 // the input blocks k - 3 ... k + 3.
 constexpr int kHalo = 3;
 constexpr int kPassesFp32 = 3;
+
+// ---- GEMM epilogues -------------------------------------------------------------------------------------------------
+// Denoiser forward transform (PROJECT false), and Griffin-Lim's projection (PROJECT true).  Columns [0, 128) of the
+// tile are the real parts of the bins nt * 128 + c, [128, 256) their imaginary parts.  Row t is frame t - 1 (t = 0:
+// the zero frame before the sequence).  Spectral: mag' = max(|X| - strength * bias, 0); project: mag' =
+// target[b, bin, t - 1] * row_scale[b].  X' = X mag' / |X|, and (mag', 0) where |X| = 0 (atan2(0, 0) = 0); written
+// to the spectrum planes `out`.
+template <bool PROJECT>
+struct SpectrumEpi : EpiDefaults {
+  struct Params {
+    __half* out; long out_rows;
+    const float* bias; float strength;                 // spectral
+    const float* target; const float* row_scale;       // project: magnitudes (B, 513, T - 1) fp32, powers of two
+  };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    const bool live = valid && t >= 1;
+    const float* tgt = PROJECT && live ? p.target + (long)b * kBins * (m.T - 1) + (t - 1) : nullptr;
+    const float rs = PROJECT && live ? p.row_scale[b] : 0.f;
+    for (int g = 0; g < 8; ++g) {
+      const int j = nt * 16 + half * 8 + g;        // bins 8 j ... 8 j + 7
+      float re[8], im[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float x = row[half * 64 + g * 8 + i], y = row[128 + half * 64 + g * 8 + i];
+        const int bin = 8 * j + i;
+        const float mag = sqrtf(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
+        float mg;
+        if (PROJECT) {
+          mg = live && bin < kBins ? tgt[(long)bin * (m.T - 1)] * rs : 0.f;
+        } else {
+          const float bias = bin < kBins ? p.bias[bin] : 0.f;
+          mg = fmaxf(__fsub_rn(mag, __fmul_rn(bias, p.strength)), 0.f);
+        }
+        const float s = mag > 0.f ? mg / mag : 0.f;
+        re[i] = live ? (mag > 0.f ? x * s : mg) * kSpecScale : 0.f;
+        im[i] = live ? y * s * kSpecScale : 0.f;
+      }
+      if (j < kImGroup0) store8<PASSES>(p.out, p.out_rows, j, q, re);
+      if (kImGroup0 + j < kSpecGroups) store8<PASSES>(p.out, p.out_rows, kImGroup0 + j, q, im);
+    }
+  }
+};
+using SpectralEpi = SpectrumEpi<false>;
+using ProjectEpi = SpectrumEpi<true>;
+
+// Public STFT transform: columns as above; row t in [1, T) is frame t - 1 of the (B, 513, T - 1) fp32 outputs.  The
+// magnitude leaves the packing scale (row_scale[b], a power of two, undoes it exactly); the phase does not depend on it.
+struct MagPhaseEpi : EpiDefaults {
+  struct Params { const float* row_scale; float* mag_out; float* phase_out; };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    if (data && t >= 1) {
+      const long F = m.T - 1;
+      const float us = valid ? p.row_scale[b] : 0.f;
+      float* mo = p.mag_out + (long)b * kBins * F + (t - 1);
+      float* po = p.phase_out + (long)b * kBins * F + (t - 1);
+      for (int c = 0; c < 64; ++c) {
+        const int bin = nt * 128 + half * 64 + c;
+        if (bin >= kBins) break;
+        const float x = row[half * 64 + c], y = row[128 + half * 64 + c];
+        mo[(long)bin * F] = valid ? sqrtf(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))) * us : 0.f;
+        po[(long)bin * F] = valid ? atan2f(y, x) : 0.f;
+      }
+    }
+  }
+};
+
+// Denoiser / STFT inverse transform.  Row t is block t of the trimmed output: the MMA has already added the four frames
+// t - 1 ... t + 2 that overlap it.  m.len[b] = 1 + the number of frames of row b (frame f exists when f >= 0 and
+// f + 1 < len); its output ends at block len - 2.  Row t writes fp32 audio block t - m.lo of row b (pitch
+// audio_pitch), divided by window_sumsquare, times 4 and times row_scale[b] when set (a power of two).
+struct OverlapEpi : EpiDefaults {
+  struct Params { float* audio; long audio_pitch; const double* wsq; const float* row_scale; };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    if (b < m.B && t >= m.lo && t < m.hi) {
+      const int fend = m.len[b];
+      const bool in_row = t + 2 < fend;
+      float* dst = p.audio + (long)b * p.audio_pitch + 256L * (t - m.lo) + half * 128;
+      for (int c = 0; c < 128; c += 4) {
+        float v[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int col = half * 128 + c + i;
+          // window_sumsquare: a float32 sum, one frame at a time in frame order, each add done in double
+          float env = 0.f;
+#pragma unroll
+          for (int f = t - 1; f <= t + 2; ++f)
+            if (f >= 0 && f + 1 < fend) env = (float)((double)env + p.wsq[256 * (t + 2 - f) + col]);
+          float y = row[col] * (1.f / (kSpecScale * kInvBasisScale));
+          if (p.row_scale) y *= p.row_scale[b];
+          if (env > FLT_MIN) y = y / env;
+          v[i] = in_row ? y * 4.f : 0.f;
+        }
+        *reinterpret_cast<float4*>(dst + c) = make_float4(v[0], v[1], v[2], v[3]);
+      }
+    }
+  }
+};
 
 // forward weights: packed row nn = tile * 256 + h * 128 + c is basis row bin (h = 0, real) or 513 + bin (h = 1,
 // imaginary) of bin = tile * 128 + c; rows of bins >= 513 are zero
@@ -67,7 +180,7 @@ __global__ void build_fwd_kernel(const float* __restrict__ fwd, float* __restric
 
 // inverse weights: row p (output sample of a block), k = sh * 1088 + ch.  Segment sh reads frame t - 1 + sh for output
 // block t, which lands 256 (3 - sh) samples into that frame.  Channel ch < 520 is the real part of bin ch, channel
-// 520 + bin the imaginary part (the spectrum plane layout of EPI_SPECTRAL); the padding channels are zero.  Packed
+// 520 + bin the imaginary part (the spectrum plane layout of SpectrumEpi); the padding channels are zero.  Packed
 // times kInvBasisScale.
 __global__ void build_inv_kernel(const float* __restrict__ inv, float* __restrict__ w) {
   const int p = blockIdx.x;
@@ -182,8 +295,8 @@ DnDims dn_dims(int B, int n) {
 void dn_layout(Carve& c, int B, int n, DnLayout* o) {
   const DnDims d = dn_dims(B, n);
   o->rows = (long)d.ntm * kTile + 4;
-  o->blk = c.take<__half>((size_t)kBlkGroups * 2 * o->rows * 8, 1024);
-  o->spec = c.take<__half>((size_t)kSpecGroups * 2 * o->rows * 8, 1024);
+  o->blk = c.take<__half>(planes_bytes(kHop, o->rows) / sizeof(__half), 1024);
+  o->spec = c.take<__half>(planes_bytes(kSpecCh, o->rows) / sizeof(__half), 1024);
   o->fend = c.take<int32_t>((size_t)B, 256);
 }
 
@@ -198,28 +311,30 @@ void st_layout(Carve& c, int B, int n, bool signal, StLayout* o) {
   o->sig = signal ? c.take<float>((size_t)B * n, 256) : nullptr;
 }
 
-// forward transform over the spectrum rows [lo, hi) of the layout (rows = frames; see the file comment)
-GemmParams forward_params(const T2Denoiser* m, const DnDims& d, const DnLayout& o, int B, int lo, int hi) {
-  GemmParams f;
+// forward transform over the spectrum rows [lo, hi) of the layout (rows = frames; see the file comment); the
+// epilogue writes the spectrum planes o.spec or the fp32 magnitude and phase
+Main forward_main(const T2Denoiser* m, const DnDims& d, const DnLayout& o, int B, int lo, int hi) {
+  Main f;
   memset(&f, 0, sizeof(f));
   for (int j = 0; j < 4; ++j) f.seg[j] = Seg{o.blk, o.rows, j - 1, kHop / 64};
   f.nseg = 4; f.nchunks = 4 * (kHop / 64); f.row0 = 1; f.wimg = m->fwd_img; f.n_tiles_m = d.ntm;
   f.B = B; f.span = d.span; f.T = d.F + 1; f.len = o.fend; f.len_mul = 1;
   f.lo = lo; f.hi = hi;
-  f.out = o.spec; f.out_rows = o.rows; f.out_row0 = 0;
   return f;
 }
 
 // inverse transform + overlap-add + envelope over the output blocks [lo, hi), written to audio (B, 256 (hi - lo))
-GemmParams inverse_params(const T2Denoiser* m, const DnDims& d, const DnLayout& o, int B, int lo, int hi, float* audio) {
-  GemmParams v;
+Main inverse_main(const T2Denoiser* m, const DnDims& d, const DnLayout& o, int B, int lo, int hi) {
+  Main v;
   memset(&v, 0, sizeof(v));
   for (int sh = 0; sh < 4; ++sh) v.seg[sh] = Seg{o.spec, o.rows, sh, kSpecCh / 64};
   v.nseg = 4; v.nchunks = 4 * (kSpecCh / 64); v.row0 = 0; v.wimg = m->inv_img; v.n_tiles_m = d.ntm;
   v.B = B; v.span = d.span; v.T = d.F - 1; v.len = o.fend; v.len_mul = 1;
   v.lo = lo; v.hi = hi;
-  v.audio = audio; v.audio_pitch = (long)kHop * (hi - lo); v.wsq = m->wsq;
   return v;
+}
+OverlapEpi::Params overlap_params(const T2Denoiser* m, int lo, int hi, float* audio, const float* row_scale) {
+  return OverlapEpi::Params{audio, (long)kHop * (hi - lo), m->wsq, row_scale};
 }
 
 // ---- per-row scales: the largest |value| of a row, over the CTAs of a cluster, to a power of two -----------------
@@ -434,11 +549,12 @@ int denoiser_run_window(T2Denoiser* m, const T2DenoiserWindowArgs* wa, cudaStrea
       a->audio, a->io_half, B, n, a->lengths, wa->at_end, s0, d.F, d.span, o.blk, o.rows, o.fend, nullptr);
   T2_LAUNCH_CHECK();
   // forward transform + spectral gate over the spectrum rows the output blocks read: [out0, out1 + 3)
-  GemmParams f = forward_params(m, d, o, B, out0, std::min(d.span, out1 + kHalo));
-  f.bias = a->bias; f.strength = a->strength;
-  T2_TRY((launch_gemm<EPI_SPECTRAL, kPassesFp32>(f, kFwdTiles, s)));
+  const SpectralEpi::Params fe{o.spec, o.rows, a->bias, a->strength, nullptr, nullptr};
+  T2_TRY((launch_gemm<SpectralEpi, kPassesFp32>(forward_main(m, d, o, B, out0, std::min(d.span, out1 + kHalo)), fe,
+                                                kFwdTiles, s)));
   // inverse transform + overlap-add + envelope over the output blocks [out0, out1)
-  T2_TRY((launch_gemm<EPI_OVERLAP, kPassesFp32>(inverse_params(m, d, o, B, out0, out1, a->out), 1, s)));
+  T2_TRY((launch_gemm<OverlapEpi, kPassesFp32>(inverse_main(m, d, o, B, out0, out1),
+                                               overlap_params(m, out0, out1, a->out, nullptr), 1, s)));
   return T2_OK;
 }
 
@@ -483,9 +599,8 @@ int stft_transform(T2Denoiser* m, const T2StftTransformArgs* a, cudaStream_t s) 
   pack_kernel<<<dim3((unsigned)((o.dn.rows + 127) / 128), kBlkGroups), 128, 0, s>>>(
       a->audio, 0, B, n, a->lengths, 1, 0, d.F, d.span, o.dn.blk, o.dn.rows, o.dn.fend, o.scale);
   T2_LAUNCH_CHECK();
-  GemmParams f = forward_params(m, d, o.dn, B, 0, d.F + 1);
-  f.row_scale = o.unscale; f.mag_out = a->magnitude; f.phase_out = a->phase;
-  T2_TRY((launch_gemm<EPI_MAGPHASE, kPassesFp32>(f, kFwdTiles, s)));
+  const MagPhaseEpi::Params e{o.unscale, a->magnitude, a->phase};
+  T2_TRY((launch_gemm<MagPhaseEpi, kPassesFp32>(forward_main(m, d, o.dn, B, 0, d.F + 1), e, kFwdTiles, s)));
   return T2_OK;
 }
 
@@ -500,9 +615,8 @@ static int spec_pack(const T2StftInverseArgs* a, const DnDims& d, const StLayout
 }
 static int inverse_to(T2Denoiser* m, int B, const DnDims& d, const StLayout& o, float* out, const float* unscale,
                       cudaStream_t s) {
-  GemmParams v = inverse_params(m, d, o.dn, B, 0, d.F - 1, out);
-  v.row_scale = unscale;
-  return launch_gemm<EPI_OVERLAP, kPassesFp32>(v, 1, s);
+  return launch_gemm<OverlapEpi, kPassesFp32>(inverse_main(m, d, o.dn, B, 0, d.F - 1),
+                                              overlap_params(m, 0, d.F - 1, out, unscale), 1, s);
 }
 
 int stft_inverse(T2Denoiser* m, const T2StftInverseArgs* a, cudaStream_t s) {
@@ -533,9 +647,9 @@ int griffin_lim(T2Denoiser* m, const T2GriffinLimArgs* g, cudaStream_t s) {
     pack_kernel<<<dim3((unsigned)((o.dn.rows + 127) / 128), kBlkGroups), 128, 0, s>>>(
         o.sig, 0, B, n, o.len, 1, 0, d.F, d.span, o.dn.blk, o.dn.rows, o.dn.fend, nullptr);
     T2_LAUNCH_CHECK();
-    GemmParams f = forward_params(m, d, o.dn, B, 0, std::min(d.span, d.F - 1 + kHalo));
-    f.target = a->magnitude; f.row_scale = o.scale;
-    T2_TRY((launch_gemm<EPI_PROJECT, kPassesFp32>(f, kFwdTiles, s)));
+    const ProjectEpi::Params pe{o.dn.spec, o.dn.rows, nullptr, 0.f, a->magnitude, o.scale};
+    T2_TRY((launch_gemm<ProjectEpi, kPassesFp32>(forward_main(m, d, o.dn, B, 0, std::min(d.span, d.F - 1 + kHalo)), pe,
+                                                 kFwdTiles, s)));
     const bool last = i == g->n_iters;
     T2_TRY(inverse_to(m, B, d, o, last ? a->out : o.sig, last ? o.unscale : nullptr, s));
   }

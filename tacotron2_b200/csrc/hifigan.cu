@@ -1,6 +1,6 @@
 // HiFi-GAN generator inference (jik876/hifi-gan, models.py: Generator, ResBlock1, ResBlock2) on sm_90a.
 //
-// Every convolution except conv_post is one implicit GEMM on wgmma (wg_gemm_kernel, EPI_HIFI) over k8 planes (see
+// Every convolution except conv_post is one implicit GEMM on wgmma (wg_gemm_kernel, HiFiEpi) over k8 planes (see
 // wg_gemm.cuh): for each group of 8 channels a hi and a lo plane of [rows][8] fp16, one row per sample at the stage's
 // rate.  A k-tap dilated Conv1d is K = k taps x ceil(C_in / 64) chunks of the same planes read at the row shifts
 // tap * d - pad.  A ConvTranspose1d of stride u, kernel 2u and padding u / 2 is polyphase: output sample q u + r reads
@@ -165,17 +165,16 @@ Stage stage(const Net& n, int s, int B, int T) {
   g.cpad = (g.C + 63) / 64 * 64;
   return g;
 }
-size_t plane_bytes(int cpad, long rows) { return (size_t)(cpad / 8) * 2 * rows * 16; }
 
 struct WsLayout { __half* mel; long mel_rows; int mel_span; __half* slot[kSlots]; float* mrf; };
 void ws_layout(Carve& c, const Net& n, int B, int T, WsLayout* o) {
   const Stage f = stage(n, -1, B, T);
   o->mel_rows = f.rows; o->mel_span = f.span;
-  o->mel = c.take<__half>((size_t)kMelGroups * 2 * f.rows * 8, 1024);
+  o->mel = c.take<__half>(planes_bytes(kMelGroups * 8, f.rows) / sizeof(__half), 1024);
   size_t slot = 0, mrf = 0;
   for (int s = -1; s < n.n_up; ++s) {
     const Stage g = stage(n, s, B, T);
-    slot = std::max(slot, plane_bytes(g.cpad, g.rows));
+    slot = std::max(slot, planes_bytes(g.cpad, g.rows));
     if (s >= 0) mrf = std::max(mrf, (size_t)g.ntm * kTile * g.C);
   }
   for (int i = 0; i < kSlots; ++i) o->slot[i] = c.take<__half>(slot / sizeof(__half), 1024);
@@ -183,10 +182,6 @@ void ws_layout(Carve& c, const Net& n, int B, int T, WsLayout* o) {
 }
 
 // ---- kernels ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float ldw(const void* p, long i, int half) {
-  return half ? __half2float(reinterpret_cast<const __half*>(p)[i]) : reinterpret_cast<const float*>(p)[i];
-}
-
 // the weight-norm scale g / ||v|| of dim-0 row blockIdx.x of v (1 when g is null: the weight is plain); 128 threads
 __global__ void wn_scale_kernel(const void* v, const void* g, int per_row, int half, float* scale) {
   __shared__ double red[4];
@@ -239,31 +234,72 @@ __device__ __forceinline__ long clamp_len(const int32_t* len, int b, int T) {
   return len == nullptr ? T : (long)min(max(len[b], 0), T);
 }
 
-// mel (B, 80, T) -> frame planes (16 groups, channels >= 80 zero); frames >= lengths[b] and guard rows zero; every
-// row written
-__global__ void mel_to_planes_kernel(const void* __restrict__ mel, int io_half, int B, int T, const int32_t* __restrict__ len,
-                                     int guard, int span, __half* __restrict__ planes, long rows, int passes) {
-  const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int g = blockIdx.y;
-  if (row >= rows) return;
-  const long q = row - guard;
-  int b = -1, f = -1;
-  if (q >= 0) { b = (int)(q / span); f = (int)(q - (long)b * span); }
-  const bool valid = b >= 0 && b < B && f < clamp_len(len, b, T);
-  float v[8];
+// ---- the GEMM epilogue ----------------------------------------------------------------------------------
+// Tile row q = b * span + t is input row t; column n = phase * cout + channel is output row t * phases + phase, plane
+// row out_row0 + b * col_span + that (output rows >= col_span are not written).  Rows past len[b] * len_mul (or
+// T * phases) are zeros.  x = acc + bias (+ res_in) goes to x_out (or null); act planes `out` get lrelu(x, slope).
+// mrf (fp32, rows (b * col_span + row) x cout): mrf = x (mrf_first) or mrf + x; with mrf_div > 0, `out` gets
+// lrelu(mrf / mrf_div, slope) instead.
+struct HiFiEpi : EpiDefaults {
+  static constexpr KForm kK = KForm::kTapShifts;
+  struct Params {
+    const float* bias; __half* out; long out_rows, out_row0; int col_span;
+    int phases, cout;
+    const __half* res_in; __half* x_out;
+    float* mrf; int mrf_first; float mrf_div, slope;
+  };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    // thread = (tile row r, half of the columns)
+    constexpr int kHalf = NT * NH / 2;
+    if (b < m.B) {
+      const long lout = (long)m.T * p.phases;
+      const long lim = m.len ? min(lout, (long)max(m.len[b], 0) * m.len_mul) : lout;
+      for (int g = 0; g < kHalf / 8; ++g) {
+        const int cl = half * kHalf + g * 8, n = nt * NT * NH + cl;
+        if (n >= p.phases * p.cout) break;
+        const int ph = n / p.cout, ch = n - ph * p.cout;
+        const long to = (long)t * p.phases + ph;
+        if (to >= p.col_span) continue;
+        const bool live = to < lim;
+        const long orow = p.out_row0 + (long)b * p.col_span + to;
+        float v[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int c = g * 8 + i;
-    float x = 0.f;
-    if (valid && c < kMel) {
-      const long idx = ((long)b * kMel + c) * T + f;
-      x = io_half ? __half2float(reinterpret_cast<const __half*>(mel)[idx]) : reinterpret_cast<const float*>(mel)[idx];
+        for (int i = 0; i < 8; ++i) v[i] = row[cl + i] + p.bias[ch + i];
+        if (p.res_in) {
+          float rv[8];
+          load8<PASSES>(p.res_in, p.out_rows, ch >> 3, orow, rv);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) v[i] += rv[i];
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = live ? v[i] : 0.f;
+        if (p.x_out) store8<PASSES>(p.x_out, p.out_rows, ch >> 3, orow, v);
+        if (p.mrf) {
+          float4* sm = reinterpret_cast<float4*>(p.mrf + ((long)b * p.col_span + to) * p.cout + ch);
+          float4 s0 = make_float4(v[0], v[1], v[2], v[3]), s1 = make_float4(v[4], v[5], v[6], v[7]);
+          if (!p.mrf_first) {
+            const float4 o0 = sm[0], o1 = sm[1];
+            s0 = make_float4(o0.x + v[0], o0.y + v[1], o0.z + v[2], o0.w + v[3]);
+            s1 = make_float4(o1.x + v[4], o1.y + v[5], o1.z + v[6], o1.w + v[7]);
+          }
+          if (p.mrf_div > 0.f) {
+            v[0] = s0.x / p.mrf_div; v[1] = s0.y / p.mrf_div; v[2] = s0.z / p.mrf_div; v[3] = s0.w / p.mrf_div;
+            v[4] = s1.x / p.mrf_div; v[5] = s1.y / p.mrf_div; v[6] = s1.z / p.mrf_div; v[7] = s1.w / p.mrf_div;
+          } else {
+            sm[0] = s0; sm[1] = s1;
+          }
+        }
+        if (p.out) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) v[i] = v[i] > 0.f ? v[i] : v[i] * p.slope;
+          store8<PASSES>(p.out, p.out_rows, ch >> 3, orow, v);
+        }
+      }
     }
-    v[i] = x;
   }
-  if (passes == 3) store8<3>(planes, rows, g, row, v);
-  else store8<1>(planes, rows, g, row, v);
-}
+};
 
 // conv_post + tanh (models.py Generator.forward's last lines) on CUDA cores: one thread per output sample, its
 // C x 7 products summed in channel-major, tap-minor order; samples >= 256 lengths[b] are zero
@@ -336,10 +372,10 @@ size_t ws_bytes(const T2HiFiGAN* m, int B, int T) {
 }
 
 template <int PASSES>
-int gemm_hifi(const GemmParams& g, const Conv& c, cudaStream_t s) {
-  if (c.nt_rows == 64) return launch_gemm<EPI_HIFI, PASSES, 64, 1>(g, c.n_pad / 64, s);
-  if (c.ncols <= 128) return launch_gemm<EPI_HIFI, PASSES, 128, 1>(g, c.n_pad / 128, s);
-  return launch_gemm<EPI_HIFI, PASSES, 128, 2>(g, c.n_pad / 256, s);
+int gemm_hifi(const Main& g, const HiFiEpi::Params& e, const Conv& c, cudaStream_t s) {
+  if (c.nt_rows == 64) return launch_gemm<HiFiEpi, PASSES, 64, 1>(g, e, c.n_pad / 64, s);
+  if (c.ncols <= 128) return launch_gemm<HiFiEpi, PASSES, 128, 1>(g, e, c.n_pad / 128, s);
+  return launch_gemm<HiFiEpi, PASSES, 128, 2>(g, e, c.n_pad / 256, s);
 }
 
 // the GEMM of convolution c from planes `in` (stage layout si) to stage layout so's outputs
@@ -349,21 +385,18 @@ struct Io {
 };
 int run_conv(const T2HiFiGAN* m, const Conv& c, const Stage& si, const Stage& so, int B, const int32_t* len, const Io& io,
              cudaStream_t s) {
-  GemmParams g;
+  Main g;
   memset(&g, 0, sizeof(g));
   const int G = m->net.guard;
   g.seg[0] = Seg{io.in, si.rows, c.up ? -1 : -c.pad, c.cin_pad / 64};
-  g.nseg = 1; g.ntaps = c.ntaps; g.dil = c.up ? 1 : c.dil; g.nchunks = c.ntaps * (c.cin_pad / 64);
+  g.nseg = 1; g.dil = c.up ? 1 : c.dil; g.nchunks = c.ntaps * (c.cin_pad / 64);
   g.row0 = G; g.wimg = c.img; g.n_tiles_m = si.ntm;
   // every row up to the last sequence's guard is written, so that the guard rows are zero in this layout too
   g.B = B; g.span = si.span; g.T = si.L; g.lo = 0; g.hi = si.span;
   g.len = len; g.len_mul = so.R;
-  g.bias = c.bias;
-  g.out = io.act; g.out_rows = so.rows; g.out_row0 = G; g.col_span = so.span;
-  g.phases = c.up ? c.up : 1; g.cout = c.cout;
-  g.res_in = io.res; g.x_out = io.x; g.mrf = io.mrf; g.mrf_first = io.mrf_first; g.mrf_div = io.mrf_div;
-  g.slope = io.slope;
-  return m->fp16 ? gemm_hifi<1>(g, c, s) : gemm_hifi<3>(g, c, s);
+  const HiFiEpi::Params e{c.bias, io.act, so.rows, G, so.span, c.up ? c.up : 1, c.cout, io.res, io.x,
+                          io.mrf, io.mrf_first, io.mrf_div, io.slope};
+  return m->fp16 ? gemm_hifi<1>(g, e, c, s) : gemm_hifi<3>(g, e, c, s);
 }
 
 // What a GEMM reads of a slot in stage layout st that no epilogue writes: rows [0, guard), before the first sequence,
@@ -390,9 +423,7 @@ int infer(T2HiFiGAN* m, const T2HiFiGANArgs* a, cudaStream_t s) {
   WsLayout o;
   ws_layout(c, n, B, T, &o);
   __half* const* sl = o.slot;
-  mel_to_planes_kernel<<<dim3((unsigned)((o.mel_rows + 127) / 128), kMelGroups), 128, 0, s>>>(
-      a->mel, a->io_half, B, T, a->lengths, G, o.mel_span, o.mel, o.mel_rows, passes);
-  T2_LAUNCH_CHECK();
+  T2_TRY(tc_mel_to_planes(a->mel, a->io_half, B, T, a->lengths, G, o.mel_span, o.mel, o.mel_rows, passes, s));
   const Stage f = stage(n, -1, B, T);
   Stage mel_st = f;
   mel_st.rows = o.mel_rows; mel_st.cpad = kMelGroups * 8;

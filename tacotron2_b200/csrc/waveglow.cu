@@ -95,6 +95,81 @@ constexpr int kUpK = 4 * 128;               // upsample K: 4 taps x 80 mels padd
 // the frames f-3 ... f.  So the audio of frames [t0, t1) is fixed by the frames [t0 - halo_right - 3, t1 + halo_right)
 // (Shape::halo_left / halo_right; 99 and 96 frames published).
 
+// ---- GEMM epilogues -------------------------------------------------------------------------------------
+// gate: columns [0, 128) of the tile are the tanh inputs of channels nt*128 + c, [128, 256) their sigmoid inputs
+// (the packed column order of build_gate_kernel); tanh * sigmoid goes to the acts planes
+struct GateEpi : EpiDefaults {
+  struct Params { const float* bias; __half* out; long out_rows, out_row0; };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    const float* bias = p.bias + nt * 256;
+    for (int g = 0; g < 8; ++g) {
+      const int c0 = half * 64 + g * 8;
+      float v[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float xt = row[c0 + i] + bias[c0 + i], xs = row[128 + c0 + i] + bias[128 + c0 + i];
+        v[i] = valid ? tanhf(xt) * (1.f / (1.f + expf(-xs))) : 0.f;
+      }
+      store8<PASSES>(p.out, p.out_rows, nt * 16 + (c0 >> 3), p.out_row0 + q, v);
+    }
+  }
+};
+
+// res/skip: output columns < res_cols are the residual half, added to the h planes `out`; the next skip_cols columns
+// are the skip half, stored (first) or added to the fp32 skip rows; later columns are padding
+struct ResSkipEpi : EpiDefaults {
+  struct Params { const float* bias; __half* out; long out_rows, out_row0; float* skip; int first, res_cols, skip_cols; };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    // each thread's 128 columns lie wholly in the residual half or the skip half (the WN width is a multiple of 128)
+    const int n0 = nt * 256 + half * 128;
+    if (n0 < p.res_cols) {             // audio = audio + res_skip_acts[:, :C]  (glow.py:170)
+      for (int g = 0; g < 16; ++g) {
+        const int c0 = n0 + g * 8;
+        float v[8];
+        load8<PASSES>(p.out, p.out_rows, c0 >> 3, p.out_row0 + q, v);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = valid ? v[i] + (row[c0 - nt * 256 + i] + p.bias[c0 + i]) : 0.f;
+        store8<PASSES>(p.out, p.out_rows, c0 >> 3, p.out_row0 + q, v);
+      }
+    } else if (n0 - p.res_cols < p.skip_cols) {   // output = output + res_skip_acts[:, C:]  (glow.py:171, 173)
+      float* sk = p.skip + q * p.skip_cols + (n0 - p.res_cols);
+      for (int c = 0; c < 128; c += 4) {
+        float4 x = make_float4(row[half * 128 + c] + p.bias[n0 + c], row[half * 128 + c + 1] + p.bias[n0 + c + 1],
+                               row[half * 128 + c + 2] + p.bias[n0 + c + 2], row[half * 128 + c + 3] + p.bias[n0 + c + 3]);
+        if (!p.first) {
+          const float4 o = *reinterpret_cast<const float4*>(sk + c);
+          x.x += o.x; x.y += o.y; x.z += o.z; x.w += o.w;
+        }
+        *reinterpret_cast<float4*>(sk + c) = x;
+      }
+    }
+  }
+};
+
+// upsample: column tile nt = mel channel, column = phase; frame row t writes the conditioning planes' group columns
+// 32 t ... 32 t + 31 of sequence b (plane row out_row0 + b * col_span + column)
+struct UpsampleEpi : EpiDefaults {
+  struct Params { const float* bias; __half* out; long out_rows, out_row0; int col_span; };
+  template <int PASSES, int NT, int NH>
+  static __device__ __forceinline__ void apply(const Main& m, const Params& p, const float* row, int r, int half, long q,
+                                               int b, int t, int nt, bool data, bool valid) {
+    if (data) {
+      const float bo = p.bias[nt];
+      const long crow = p.out_row0 + (long)b * p.col_span + 32L * t + half * 16;
+      for (int k = 0; k < 16; ++k) {
+        float v[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = row[half * 128 + k * 8 + i] + bo;
+        store8<PASSES>(p.out, p.out_rows, nt, crow + k, v);
+      }
+    }
+  }
+};
+
 // ---- Philox normal draws ----------------------------------------------------------------------------
 // z(b, c, t): Philox4x32-10 with counter (t, b, c, kNoiseTag) and key (seed lo, seed hi); Box-Muller on the first
 // two output words: u1 = ((o0 >> 8) + 1) 2^-24 in (0, 1], u2 = (o1 >> 8) 2^-24, z = sqrt(-2 ln u1) cos(2 pi u2).
@@ -240,36 +315,7 @@ __global__ void __launch_bounds__(128) flow_tail_kernel(const TailParams<C> p, c
   }
 }
 
-// mel (B, 80, T) -> frame-domain planes (16 groups, channels >= 80 zero); frames >= len zero; every row written
-__global__ void mel_to_planes_kernel(const void* __restrict__ mel, int io_half, int B, int T, const int32_t* __restrict__ len,
-                                     __half* __restrict__ planes, long rows, int passes) {
-  const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int g = blockIdx.y;
-  if (row >= rows) return;
-  const long q = row - kFGuard;
-  const int span = T + kFGuard;
-  int b = -1, f = -1;
-  if (q >= 0) { b = (int)(q / span); f = (int)(q - (long)b * span); }
-  const bool valid = b >= 0 && b < B && f < T && (len == nullptr || f < len[b]);
-  float v[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int c = g * 8 + i;
-    float x = 0.f;
-    if (valid && c < 80) {
-      const long idx = ((long)b * 80 + c) * T + f;
-      x = io_half ? __half2float(reinterpret_cast<const __half*>(mel)[idx]) : reinterpret_cast<const float*>(mel)[idx];
-    }
-    v[i] = x;
-  }
-  if (passes == 3) store8<3>(planes, rows, g, row, v);
-  else store8<1>(planes, rows, g, row, v);
-}
-
 // ---- weight packing ----------------------------------------------------------------------------------
-__device__ __forceinline__ float ldw(const void* p, long i, int half) {
-  return half ? __half2float(reinterpret_cast<const __half*>(p)[i]) : reinterpret_cast<const float*>(p)[i];
-}
 // g / ||v|| of row n of a weight-normed tensor (1 when g is null: the weight is plain); 256 threads
 __device__ float wn_scale(const void* v, const void* g, long n, int per_row, int half) {
   __shared__ float red[8];
@@ -427,10 +473,10 @@ void ws_layout(Carve& c, const Shape& sh, int B, int T, WsLayout* o) {
   const Dims d = dims_of(sh, B, T);
   o->x_rows = kFGuard + (long)d.ntf * kTile;
   o->rows = sh.guard() + (long)d.ntm * kTile + sh.guard();
-  o->x = c.take<__half>((size_t)16 * 2 * o->x_rows * 8, 1024);
-  o->spect = c.take<__half>((size_t)80 * 2 * o->rows * 8, 1024);
-  o->h = c.take<__half>((size_t)(sh.C / 8) * 2 * o->rows * 8, 1024);
-  o->acts = c.take<__half>((size_t)(sh.C / 8) * 2 * o->rows * 8, 1024);
+  o->x = c.take<__half>(planes_bytes(128, o->x_rows) / sizeof(__half), 1024);
+  o->spect = c.take<__half>(planes_bytes(kCond, o->rows) / sizeof(__half), 1024);
+  o->h = c.take<__half>(planes_bytes(sh.C, o->rows) / sizeof(__half), 1024);
+  o->acts = c.take<__half>(planes_bytes(sh.C, o->rows) / sizeof(__half), 1024);
   o->skip = c.take<float>((size_t)d.ntm * kTile * sh.C, 1024);
   o->aud = c.take<float>((size_t)d.ntm * kTile * 8, 1024);
 }
@@ -615,10 +661,9 @@ static int run_flows(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, const WsLayo
   };
   WG_STOP_POINT();
   T2_TRY(tail(flows, flows - 1));
-  GemmParams g;
+  Main g;
   memset(&g, 0, sizeof(g));
   g.row0 = guard; g.n_tiles_m = d.ntm; g.B = B; g.span = d.span; g.T = d.L; g.len = a->lengths; g.len_mul = 32;
-  g.out_rows = o.rows; g.out_row0 = guard; g.skip = o.skip; g.skip_cols = C;
   const int cc = C / 64;                     // 64-channel chunks of h and acts
   for (int k = flows - 1; k >= 0; --k) {
     widen(k + 1, &g.lo, &g.hi);
@@ -627,16 +672,17 @@ static int run_flows(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, const WsLayo
       // in_layer(audio) + cond_layer(spect)[slice] -> tanh * sigmoid  (glow.py:161-166)
       g.seg[0] = Seg{o.h, o.rows, -dil, cc}; g.seg[1] = Seg{o.h, o.rows, 0, cc}; g.seg[2] = Seg{o.h, o.rows, dil, cc};
       g.seg[3] = Seg{o.spect, o.rows, 0, 10};
-      g.nseg = 4; g.nchunks = 3 * cc + 10; g.wimg = m->gate_img[k][l]; g.bias = m->gate_bias + ((size_t)k * L + l) * 2 * C;
-      g.out = o.acts;
+      g.nseg = 4; g.nchunks = 3 * cc + 10; g.wimg = m->gate_img[k][l];
+      const GateEpi::Params ge{m->gate_bias + ((size_t)k * L + l) * 2 * C, o.acts, o.rows, guard};
       WG_STOP_POINT();
-      T2_TRY(gemm<EPI_GATE>(g, C / 128, fp16, s));
+      T2_TRY(gemm<GateEpi>(g, ge, C / 128, fp16, s));
       // res_skip_layers (glow.py:168-173)
       g.seg[0] = Seg{o.acts, o.rows, 0, cc};
-      g.nseg = 1; g.nchunks = cc; g.wimg = m->rs_img[k][l]; g.bias = m->rs_bias + ((size_t)k * L + l) * 2 * C;
-      g.out = o.h; g.first = l == 0; g.res_cols = l < L - 1 ? C : 0;
+      g.nseg = 1; g.nchunks = cc; g.wimg = m->rs_img[k][l];
+      const ResSkipEpi::Params re{m->rs_bias + ((size_t)k * L + l) * 2 * C, o.h, o.rows, guard, o.skip, l == 0,
+                                  l < L - 1 ? C : 0, C};
       WG_STOP_POINT();
-      T2_TRY(gemm<EPI_RESSKIP>(g, sh.rs_tiles(l), fp16, s));
+      T2_TRY(gemm<ResSkipEpi>(g, re, sh.rs_tiles(l), fp16, s));
     }
     WG_STOP_POINT();
     T2_TRY(tail(k, k > 0 ? k - 1 : -1));
@@ -675,22 +721,21 @@ int waveglow_infer_window(T2WaveGlow* m, const T2WaveGlowWindowArgs* wa, cudaStr
   // Guard rows must read as zero: they are cleared here and only ever rewritten with zeros.  With per-flow ranges
   // (below) the rows a flow does not need are not rewritten and may hold stale values from earlier flows or calls
   // (skip and aud are not cleared at all); that is safe because no needed row reads an unneeded one.
-  T2_CUDA(cudaMemsetAsync(o.spect, 0, (size_t)80 * 2 * o.rows * 16, s));
-  T2_CUDA(cudaMemsetAsync(o.h, 0, (size_t)(sh.C / 8) * 2 * o.rows * 16, s));
-  T2_CUDA(cudaMemsetAsync(o.acts, 0, (size_t)(sh.C / 8) * 2 * o.rows * 16, s));
+  T2_CUDA(cudaMemsetAsync(o.spect, 0, planes_bytes(kCond, o.rows), s));
+  T2_CUDA(cudaMemsetAsync(o.h, 0, planes_bytes(sh.C, o.rows), s));
+  T2_CUDA(cudaMemsetAsync(o.acts, 0, planes_bytes(sh.C, o.rows), s));
   WG_STOP_POINT();
-  mel_to_planes_kernel<<<dim3((unsigned)((o.x_rows + 127) / 128), 16), 128, 0, s>>>(a->mel, a->io_half, B, T, a->lengths,
-                                                                                  o.x, o.x_rows, passes);
-  T2_LAUNCH_CHECK();
+  // frame-domain planes: kFGuard zero rows before each sequence's frames and after them
+  T2_TRY(tc_mel_to_planes(a->mel, a->io_half, B, T, a->lengths, kFGuard, d.spanf, o.x, o.x_rows, passes, s));
   // upsample + trim + unfold (glow.py:252-258)
-  GemmParams u;
+  Main u;
   memset(&u, 0, sizeof(u));
   for (int j = 0; j < 4; ++j) u.seg[j] = Seg{o.x, o.x_rows, -j, 2};
   u.nseg = 4; u.nchunks = 8; u.row0 = kFGuard; u.wimg = m->up_img; u.n_tiles_m = d.ntf;
-  u.B = B; u.span = d.spanf; u.T = T; u.lo = 0; u.hi = T; u.bias = m->up_bias;
-  u.out = o.spect; u.out_rows = o.rows; u.out_row0 = guard; u.col_span = d.span;
+  u.B = B; u.span = d.spanf; u.T = T; u.lo = 0; u.hi = T;
+  const UpsampleEpi::Params ue{m->up_bias, o.spect, o.rows, guard, d.span};
   WG_STOP_POINT();
-  T2_TRY(gemm<EPI_UPSAMPLE>(u, 80, fp16, s));
+  T2_TRY(gemm<UpsampleEpi>(u, ue, 80, fp16, s));
 
   // Per-flow column ranges.  The audio columns [32 out0, 32 out1) need the output of the flow that runs with n flows
   // still to follow over those columns widened by n * reach; that flow's WN layers run over one reach more.
