@@ -142,6 +142,53 @@ def _integer_tensor(x, name, what):
     return t
 
 
+def _float_tensor(t, name, what, shape, dims, device_type, dtypes=None):
+    """Refuses t as argument `name` of `what` unless it is a tensor of a floating dtype (one of `dtypes` if given) with
+    a number of dims in `dims` (the allowed shapes written as `shape`), no extent 0, on a device of type `device_type`:
+    TypeError / ValueError."""
+    if not torch.is_tensor(t):
+        raise TypeError("%s: %s must be a tensor (got %s)" % (what, name, type(t).__name__))
+    if dtypes is None and not t.dtype.is_floating_point:
+        raise TypeError("%s: %s must be a float tensor (got %s)" % (what, name, t.dtype))
+    if dtypes is not None and t.dtype not in dtypes:
+        names = " or ".join(str(d).replace("torch.", "") for d in dtypes)
+        raise TypeError("%s: %s must be %s (got %s)" % (what, name, names, t.dtype))
+    if t.dim() not in dims or min(t.shape) < 1:
+        raise ValueError("%s: %s must have shape %s, none of them 0 (got %s)" % (what, name, shape, tuple(t.shape)))
+    if t.device.type != device_type:
+        raise ValueError("%s: %s must be on a %s device (got %s); there is no CPU path"
+                         % (what, name, device_type.upper(), t.device))
+
+
+def _number(x, name, what, lo=None, hi=None, lo_open=False, integer=False):
+    """x as argument `name` of `what`: a real number (an integer if `integer`), finite and in [lo, hi] ((lo, hi] if
+    lo_open), as a float (int); TypeError / ValueError otherwise."""
+    if isinstance(x, bool) or not isinstance(x, numbers.Real) or (integer and not isinstance(x, numbers.Integral)):
+        raise TypeError("%s: %s must be %s (got %r)" % (what, name, "an integer" if integer else "a real number", x))
+    x = int(x) if integer else float(x)
+    if (not integer and not math.isfinite(x)) or (lo is not None and (x <= lo if lo_open else x < lo)) or \
+            (hi is not None and x > hi):
+        rng = "%s%s, %s]" % ("(" if lo_open else "[", lo if lo is not None else "-inf", hi if hi is not None else "inf")
+        raise ValueError("%s: %s must lie in %s (got %r)" % (what, name, rng, x))
+    return x
+
+
+_TABLES = {}
+_TABLES_LOCK = threading.Lock()
+
+
+def _cached_table(key, build):
+    """build() -- host tables put on a device -- cached under `key`; a 17th key drops the 16 cached ones."""
+    with _TABLES_LOCK:
+        t = _TABLES.get(key)
+        if t is None:
+            t = build()
+            if len(_TABLES) >= 16:
+                _TABLES.clear()
+            _TABLES[key] = t
+        return t
+
+
 def row_lengths(lengths, B, T, name, device):
     """Per-row lengths of a ragged inference batch: (B,) integers, each in 1..T, as a list, a host or a device tensor.
     Returns (lengths as int32 on `device`, whether some row is shorter than T), reading a device tensor back once;
@@ -313,19 +360,10 @@ def duration_inputs(alignments, input_lengths, mel_lengths, method, device_type=
     what = "tacotron2_b200.durations_from_alignments"
     if method not in _DURATION_METHODS:
         raise ValueError("%s: method must be one of %s (got %r)" % (what, sorted(_DURATION_METHODS), method))
-    if not torch.is_tensor(alignments):
-        raise TypeError("%s: alignments must be a tensor (got %s)" % (what, type(alignments).__name__))
-    if not alignments.dtype.is_floating_point:
-        raise TypeError("%s: alignments must be a float tensor (got %s)" % (what, alignments.dtype))
-    if alignments.dim() != 3 or min(alignments.shape) < 1:
-        raise ValueError("%s: alignments must have shape (B, T_mel, T_text), none of them 0 (got %s)"
-                         % (what, tuple(alignments.shape)))
+    _float_tensor(alignments, "alignments", what, "(B, T_mel, T_text)", (3,), device_type)
     B, T_mel, T_text = (int(s) for s in alignments.shape)
     if T_text > _capi.DURATIONS_MAX_TEXT:
         raise ValueError("%s: T_text must be at most %d (got %d)" % (what, _capi.DURATIONS_MAX_TEXT, T_text))
-    if alignments.device.type != device_type:
-        raise ValueError("%s: alignments must be on a %s device (got %s); there is no CPU path"
-                         % (what, device_type.upper(), alignments.device))
     dev = alignments.device
     il, _ = row_lengths(input_lengths, B, T_text, "input_lengths", dev)
     ml, _ = row_lengths(mel_lengths, B, T_mel, "mel_lengths", dev)

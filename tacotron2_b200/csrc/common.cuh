@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+#include <type_traits>
 
 #include "../../include/t2b200.h"
 
@@ -72,6 +73,48 @@ static_assert(W_POST_CONV0 + 5 * 7 == W_COUNT, "state_dict table");
 // element i of a weight tensor the caller passes in fp32 (half 0) or fp16 (half 1)
 __device__ __forceinline__ float ldw(const void* p, long i, int half) {
   return half ? __half2float(reinterpret_cast<const __half*>(p)[i]) : reinterpret_cast<const float*>(p)[i];
+}
+
+// row b's length: lengths[b] clamped into 1..T (device lengths are never trusted), or T without lengths
+__device__ __forceinline__ int clamp_length(const int32_t* __restrict__ lengths, int b, int T) {
+  return lengths ? min(max(lengths[b], 1), T) : T;
+}
+
+// ---- kernel launches -----------------------------------------------------------------------------
+// A launch with more than the default 48 KiB of dynamic shared memory needs the kernel's opt-in first.
+template <typename Kernel>
+int allow_dynamic_smem(Kernel kernel, size_t bytes) {
+  if (bytes > 48 * 1024)
+    T2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  return T2_OK;
+}
+
+// Row sweeps (MAS in durations.cu, DTW in dtw.cu): one CTA per row, K cells per thread (the smallest power of two with
+// K max_threads >= cells) and n = 32 ceil(cells / (32 K)) threads.  Dynamic shared memory holds each warp's edge values
+// ([2][K][n / 32] fp64, double buffered), then the sweep's bit map of bit_bytes when that fits kSweepSmemBitBytes
+// (smem_bits; two CTAs then fit an SM); a larger map lives in the workspace.
+constexpr size_t kSweepSmemBitBytes = 96 * 1024;
+struct SweepPlan { int K, threads; bool smem_bits; size_t smem_bytes; };
+inline SweepPlan sweep_plan(int cells, int max_threads, size_t bit_bytes) {
+  SweepPlan p;
+  p.K = 1;
+  while (p.K * max_threads < cells) p.K *= 2;
+  p.threads = ((cells + p.K - 1) / p.K + 31) / 32 * 32;
+  p.smem_bits = bit_bytes <= kSweepSmemBitBytes;
+  p.smem_bytes = 2 * (size_t)p.K * (p.threads / 32) * sizeof(double) + (p.smem_bits ? bit_bytes : 0);
+  return p;
+}
+
+// f(std::integral_constant<int, K>()) for a sweep's K: the callers' sizes keep K in {1, 2, 4, 8, 16}
+template <typename F>
+int with_sweep_k(int K, F&& f) {
+  switch (K) {
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 4: return f(std::integral_constant<int, 4>());
+    case 8: return f(std::integral_constant<int, 8>());
+    default: return f(std::integral_constant<int, 16>());
+  }
 }
 
 // ---- buffer layouts ------------------------------------------------------------------------------

@@ -25,31 +25,19 @@ namespace t2 {
 namespace {
 
 constexpr int kDtwMaxThreads = 512;
-constexpr size_t kDtwSmemBitBytes = 96 * 1024;      // predecessor maps up to this size stay on chip (two CTAs fit an SM)
 constexpr int kCepThreads = 128;
 
-// launch shape for T_x frames of x: K cells per thread (a power of two, <= 16 at T_x = 8192), n threads; `words` 32-cell
-// blocks of i per diagonal (a diagonal holds at most min(T_x, T_y) consecutive cells)
-struct DtwPlan { int K, threads, words; bool smem_bits; size_t bit_bytes, smem_bytes; };
+// launch shape for T_x frames of x (K <= 16 at T_x = 8192): a sweep over the cells i whose predecessor map has `words`
+// 32-cell blocks of i per diagonal (a diagonal holds at most min(T_x, T_y) consecutive cells)
+struct DtwPlan : SweepPlan { int words; };
 DtwPlan dtw_plan(int T_x, int T_y) {
-  DtwPlan p;
-  p.K = 1;
-  while (p.K * kDtwMaxThreads < T_x) p.K *= 2;
-  p.threads = ((T_x + p.K - 1) / p.K + 31) / 32 * 32;
-  p.words = std::min((T_x + 31) / 32, (std::min(T_x, T_y) + 31) / 32 + 1);
-  p.bit_bytes = (size_t)(T_x + T_y - 1) * p.words * sizeof(uint2);
-  p.smem_bits = p.bit_bytes <= kDtwSmemBitBytes;
-  p.smem_bytes = 2 * (size_t)p.K * (p.threads / 32) * sizeof(double) + (p.smem_bits ? p.bit_bytes : 0);
-  return p;
+  const int words = std::min((T_x + 31) / 32, (std::min(T_x, T_y) + 31) / 32 + 1);
+  return {sweep_plan(T_x, kDtwMaxThreads, (size_t)(T_x + T_y - 1) * words * sizeof(uint2)), words};
 }
 
 void dtw_ws_layout(Carve& c, int B, int T_x, int T_y, uint2** bits) {
   const DtwPlan p = dtw_plan(T_x, T_y);
   *bits = p.smem_bits ? nullptr : c.take<uint2>((size_t)B * (T_x + T_y - 1) * p.words);
-}
-
-__device__ __forceinline__ int clamp_length(const int32_t* __restrict__ lengths, int b, int T) {
-  return lengths ? min(max(lengths[b], 1), T) : T;
 }
 
 template <typename T, int K, int G = (K < 8 ? K : 8)>
@@ -211,24 +199,12 @@ __global__ void __launch_bounds__(kCepThreads) cepstra_kernel(const T* __restric
 
 template <typename T, int K>
 int launch_dtw(const T2DtwArgs* a, const DtwPlan& p, uint2* gbits, cudaStream_t s) {
-  if (p.smem_bytes > 48 * 1024)
-    T2_CUDA(cudaFuncSetAttribute(dtw_kernel<T, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
+  T2_TRY(allow_dynamic_smem(dtw_kernel<T, K>, p.smem_bytes));
   dtw_kernel<T, K><<<a->B, p.threads, p.smem_bytes, s>>>(
       static_cast<const T*>(a->x), static_cast<const T*>(a->y), a->x_lengths, a->y_lengths, a->D, a->T_x, a->T_y,
       p.words, gbits, a->cost, a->path, a->path_lengths);
   T2_LAUNCH_CHECK();
   return T2_OK;
-}
-
-template <typename T>
-int launch_dtw(const T2DtwArgs* a, const DtwPlan& p, uint2* gbits, cudaStream_t s) {
-  switch (p.K) {
-    case 1: return launch_dtw<T, 1>(a, p, gbits, s);
-    case 2: return launch_dtw<T, 2>(a, p, gbits, s);
-    case 4: return launch_dtw<T, 4>(a, p, gbits, s);
-    case 8: return launch_dtw<T, 8>(a, p, gbits, s);
-    default: return launch_dtw<T, 16>(a, p, gbits, s);
-  }
 }
 
 int dtw_sizes_status(int B, int D, int T_x, int T_y, int dtype) {
@@ -266,7 +242,10 @@ int t2_dtw(const T2DtwArgs* a, void* stream) {
   dtw_ws_layout(c, a->B, a->T_x, a->T_y, &bits);
   const DtwPlan p = dtw_plan(a->T_x, a->T_y);
   cudaStream_t s = (cudaStream_t)stream;
-  return a->dtype == T2_DTW_F32 ? launch_dtw<float>(a, p, bits, s) : launch_dtw<double>(a, p, bits, s);
+  return with_sweep_k(p.K, [&](auto K) {
+    return a->dtype == T2_DTW_F32 ? launch_dtw<float, decltype(K)::value>(a, p, bits, s)
+                                  : launch_dtw<double, decltype(K)::value>(a, p, bits, s);
+  });
 }
 
 int t2_mel_cepstra(const void* mel, int32_t dtype, const int32_t* lengths, int32_t B, int32_t n_mel, int32_t T,

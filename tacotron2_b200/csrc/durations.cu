@@ -20,21 +20,14 @@ namespace t2 {
 namespace {
 
 constexpr int kMasMaxThreads = 256;
-constexpr size_t kMasSmemBitBytes = 96 * 1024;    // bit maps up to this size stay on chip (two CTAs fit an SM)
 constexpr int kArgmaxWarps = 8;                     // frames per CTA of the argmax kernel
 
-// MAS launch shape for T_text symbols: K symbols per thread (a power of two, <= 16 at T_text = 4096), n threads
-struct MasPlan { int K, threads, words; bool smem_bits; size_t smem_bytes; };
+// MAS launch shape for T_text symbols (K <= 16 at T_text = 4096): a sweep over the symbols whose bit map has `words`
+// words per frame
+struct MasPlan : SweepPlan { int words; };
 MasPlan mas_plan(int T_mel, int T_text) {
-  MasPlan p;
-  p.K = 1;
-  while (p.K * kMasMaxThreads < T_text) p.K *= 2;
-  p.threads = ((T_text + p.K - 1) / p.K + 31) / 32 * 32;
-  p.words = (T_text + 31) / 32;
-  const size_t bits = (size_t)T_mel * p.words * sizeof(uint32_t);
-  p.smem_bits = bits <= kMasSmemBitBytes;
-  p.smem_bytes = 2 * (size_t)p.K * (p.threads / 32) * sizeof(double) + (p.smem_bits ? bits : 0);
-  return p;
+  const int words = (T_text + 31) / 32;
+  return {sweep_plan(T_text, kMasMaxThreads, (size_t)T_mel * words * sizeof(uint32_t)), words};
 }
 
 struct DurationsWs { uint32_t* bits; int32_t* best; };
@@ -47,10 +40,6 @@ void durations_ws_layout(Carve& c, int B, int T_mel, int T_text, int method, Dur
   } else {
     w->best = c.take<int32_t>((size_t)B * T_mel);                                    // argmax symbol per frame
   }
-}
-
-__device__ __forceinline__ int clamp_length(const int32_t* __restrict__ lengths, int b, int T) {
-  return lengths ? min(max(lengths[b], 1), T) : T;
 }
 
 template <int K>
@@ -190,8 +179,7 @@ __global__ void count_kernel(const int32_t* __restrict__ best, const int32_t* __
 
 template <int K>
 int launch_mas(const T2DurationsArgs* a, const MasPlan& p, uint32_t* gbits, cudaStream_t s) {
-  if (p.smem_bytes > 48 * 1024)
-    T2_CUDA(cudaFuncSetAttribute(mas_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes));
+  T2_TRY(allow_dynamic_smem(mas_kernel<K>, p.smem_bytes));
   mas_kernel<K><<<a->B, p.threads, p.smem_bytes, s>>>(a->alignments, a->input_lengths, a->mel_lengths, a->T_mel,
                                                        a->T_text, p.words, gbits, a->durations);
   T2_LAUNCH_CHECK();
@@ -240,13 +228,7 @@ int t2_durations(const T2DurationsArgs* a, void* stream) {
     return T2_OK;
   }
   const MasPlan p = mas_plan(a->T_mel, a->T_text);
-  switch (p.K) {
-    case 1: return launch_mas<1>(a, p, w.bits, s);
-    case 2: return launch_mas<2>(a, p, w.bits, s);
-    case 4: return launch_mas<4>(a, p, w.bits, s);
-    case 8: return launch_mas<8>(a, p, w.bits, s);
-    default: return launch_mas<16>(a, p, w.bits, s);
-  }
+  return with_sweep_k(p.K, [&](auto K) { return launch_mas<decltype(K)::value>(a, p, w.bits, s); });
 }
 
 }  // extern "C"

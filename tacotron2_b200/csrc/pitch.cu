@@ -49,16 +49,12 @@ size_t viterbi_smem_bytes(const T2PyinArgs& a) {
   return sizeof(double) * (4 * n + n + 8 * n) + sizeof(int) * 8 * n + 64;
 }
 
-__device__ __forceinline__ int row_samples(const int32_t* __restrict__ lengths, int b, int n) {
-  return lengths ? min(max(lengths[b], 1), n) : n;
-}
-
 __global__ void __launch_bounds__(kFrameThreads) pyin_frame_kernel(T2PyinArgs a, PyinWs w) {
   extern __shared__ double sm[];
   const int f = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31;
   const int fl = a.frame_length, W = a.win_length, maxp = a.max_period, minp = a.min_period, lags = pyin_lags(a);
   const int nb = a.n_bins, nthr = a.n_thresholds, K = pyin_max_troughs(a);
-  const int F = pyin_frames(a.n, a.hop_length), L = row_samples(a.lengths, b, a.n);
+  const int F = pyin_frames(a.n, a.hop_length), L = clamp_length(a.lengths, b, a.n);
   const size_t bf = (size_t)b * F + f;
   if (f >= pyin_frames(L, a.hop_length)) {             // past the row's end: no observations, voiced_prob 0
     if (tid == 0) { w.count[bf] = 0; w.log_u[bf] = 0.0; a.voiced_prob[bf] = 0.0; }
@@ -245,7 +241,7 @@ __global__ void __launch_bounds__(kViterbiThreads) pyin_viterbi_kernel(T2PyinArg
   extern __shared__ double sm[];
   const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
   const int nb = a.n_bins, S = 2 * nb, h = a.width / 2, bw = 2 * h + 1, K = pyin_max_troughs(a);
-  const int F = pyin_frames(a.n, a.hop_length), Fb = pyin_frames(row_samples(a.lengths, b, a.n), a.hop_length);
+  const int F = pyin_frames(a.n, a.hop_length), Fb = pyin_frames(clamp_length(a.lengths, b, a.n), a.hop_length);
   double* v = sm;                                        // [2][S] scores of the previous / current frame
   double* lobs = v + 2 * S;                              // [nb] the frame's voiced log observations
   double* sv = lobs + nb;                                // [2][4 nb] scan values: prefix / suffix of each half
@@ -438,10 +434,8 @@ int t2_pyin(const T2PyinArgs* a, void* stream) {
   PyinWs w;
   pyin_ws_layout(c, *a, &w);
   const size_t fsm = frame_smem_bytes(*a), vsm = viterbi_smem_bytes(*a);
-  if (fsm > 48 * 1024)
-    T2_CUDA(cudaFuncSetAttribute(pyin_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsm));
-  if (vsm > 48 * 1024)
-    T2_CUDA(cudaFuncSetAttribute(pyin_viterbi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vsm));
+  T2_TRY(allow_dynamic_smem(pyin_frame_kernel, fsm));
+  T2_TRY(allow_dynamic_smem(pyin_viterbi_kernel, vsm));
   const int F = pyin_frames(a->n, a->hop_length);
   pyin_frame_kernel<<<dim3(F, a->B), kFrameThreads, fsm, s>>>(*a, w);
   T2_LAUNCH_CHECK();

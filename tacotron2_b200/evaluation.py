@@ -4,14 +4,12 @@ batches of frame sequences of different lengths --, ``mel_cepstral_distortion`` 
 section 6.12.  The contract is the numpy fp64 oracle ``tests/dtw_oracle.py``."""
 import ctypes as C
 import math
-import numbers
-import threading
 
 import numpy as np
 import torch
 
 from . import _capi
-from ._engine import _integer_tensor, row_lengths
+from ._engine import _cached_table, _float_tensor, _integer_tensor, _number, row_lengths
 
 _DTW = "tacotron2_b200.dtw"
 _MCD = "tacotron2_b200.mel_cepstral_distortion"
@@ -20,24 +18,12 @@ MCD_SCALE = 10.0 * math.sqrt(2.0) / math.log(10.0)     # dB per unit of Euclidea
 _DTYPES = {torch.float32: _capi.DTW_F32, torch.float64: _capi.DTW_F64}
 
 
-def _frames(t, name, what, device_type):
-    if not torch.is_tensor(t):
-        raise TypeError("%s: %s must be a tensor (got %s)" % (what, name, type(t).__name__))
-    if t.dtype not in _DTYPES:
-        raise TypeError("%s: %s must be float32 or float64 (got %s)" % (what, name, t.dtype))
-    if t.dim() != 3 or min(t.shape) < 1:
-        raise ValueError("%s: %s must have shape (B, D, T), none of them 0 (got %s)" % (what, name, tuple(t.shape)))
-    if t.device.type != device_type:
-        raise ValueError("%s: %s must be on a %s device (got %s); there is no CPU path"
-                         % (what, name, device_type.upper(), t.device))
-
-
 def dtw_inputs(x, y, x_lengths=None, y_lengths=None, what=_DTW, device_type="cuda"):
     """The arguments of dtw checked and put in the library's form: (x, y contiguous, x_lengths and y_lengths as (B,)
     int32 on their device or None, the dtype code).  Reads a device-side lengths tensor back once.  Raises TypeError /
     ValueError before anything is launched."""
-    _frames(x, "x", what, device_type)
-    _frames(y, "y", what, device_type)
+    _float_tensor(x, "x", what, "(B, D, T)", (3,), device_type, _DTYPES)
+    _float_tensor(y, "y", what, "(B, D, T)", (3,), device_type, _DTYPES)
     if x.dtype != y.dtype:
         raise TypeError("%s: x and y must have the same dtype (got %s and %s)" % (what, x.dtype, y.dtype))
     if x.device != y.device:
@@ -55,18 +41,6 @@ def dtw_inputs(x, y, x_lengths=None, y_lengths=None, what=_DTW, device_type="cud
     return x.detach().contiguous(), y.detach().contiguous(), xl, yl, _DTYPES[x.dtype]
 
 
-_WS = _capi.Workspace()
-_WS_LOCK = threading.Lock()
-
-
-def _workspace(tag, nbytes, device):
-    """A cached device buffer of at least nbytes, one per tag, device and current stream (so calls on two streams never
-    share one)."""
-    key = (tag, str(device), torch.cuda.current_stream(device).cuda_stream)
-    with _WS_LOCK:
-        return _WS.get(key, max(int(nbytes), 1), device)
-
-
 def _dtw_call(x, y, xl, yl, code):
     B, D, T_x = (int(s) for s in x.shape)
     T_y = int(y.shape[2])
@@ -75,8 +49,7 @@ def _dtw_call(x, y, xl, yl, code):
     path = torch.empty(B, T_x + T_y - 1, 2, dtype=torch.int64, device=dev)
     path_lengths = torch.empty(B, dtype=torch.int64, device=dev)
     L = _capi.lib()
-    nbytes = L.t2_dtw_workspace_bytes(B, D, T_x, T_y, code)
-    ws = _workspace("dtw", nbytes, dev)
+    ws = _capi.byte_buffer(L.t2_dtw_workspace_bytes(B, D, T_x, T_y, code), dev)
     args = _capi.T2DtwArgs(x.data_ptr(), y.data_ptr(), None if xl is None else xl.data_ptr(),
                            None if yl is None else yl.data_ptr(), B, D, T_x, T_y, code, cost.data_ptr(),
                            path.data_ptr(), path_lengths.data_ptr(), ws.data_ptr(), ws.numel())
@@ -109,32 +82,22 @@ def dct_table(n_mel, n_cep):
     return np.sqrt(2.0 / n_mel) * np.cos(np.pi * k * (2 * m + 1) / (2 * n_mel))
 
 
-_TABLES = {}
-
-
 def _device_table(n_mel, n_cep, device):
-    key = (n_mel, n_cep, str(device))
-    with _WS_LOCK:
-        t = _TABLES.get(key)
-        if t is None:
-            if len(_TABLES) >= 16:
-                _TABLES.clear()
-            t = _TABLES[key] = torch.from_numpy(dct_table(n_mel, n_cep)).to(device)
-        return t
+    key = ("dct", n_mel, n_cep, str(device))
+    return _cached_table(key, lambda: torch.from_numpy(dct_table(n_mel, n_cep)).to(device))
 
 
 def mcd_inputs(mel_x, mel_y, x_lengths=None, y_lengths=None, n_cep=24, device_type="cuda"):
     """The arguments of mel_cepstral_distortion checked: dtw_inputs' tuple and n_cep.  Raises TypeError / ValueError
     before anything is launched."""
-    if isinstance(n_cep, bool) or not isinstance(n_cep, numbers.Integral):
-        raise TypeError("%s: n_cep must be an integer (got %r)" % (_MCD, n_cep))
+    n_cep = _number(n_cep, "n_cep", _MCD, integer=True)
     args = dtw_inputs(mel_x, mel_y, x_lengths, y_lengths, _MCD, device_type)
     B, n_mel = (int(s) for s in args[0].shape[:2])
     if B > 65535:
         raise ValueError("%s: B must be at most 65535 (got %d)" % (_MCD, B))
     if not 1 <= n_cep <= n_mel - 1:
         raise ValueError("%s: n_cep must lie in 1..n_mel - 1 = %d (got %d)" % (_MCD, n_mel - 1, n_cep))
-    return args, int(n_cep)
+    return args, n_cep
 
 
 def mel_cepstral_distortion(mel_x, mel_y, x_lengths=None, y_lengths=None, n_cep=24):
@@ -155,9 +118,8 @@ def mel_cepstral_distortion(mel_x, mel_y, x_lengths=None, y_lengths=None, n_cep=
     table = _device_table(n_mel, n_cep, dev)
     L = _capi.lib()
     ceps = []
-    for tag, t, ln, T in (("cep_x", x, xl, T_x), ("cep_y", y, yl, T_y)):
-        buf = _workspace(tag, B * n_cep * T * 8, dev)
-        cep = buf[:B * n_cep * T * 8].view(torch.float64).view(B, n_cep, T)
+    for t, ln, T in ((x, xl, T_x), (y, yl, T_y)):
+        cep = torch.empty(B, n_cep, T, dtype=torch.float64, device=dev)
         _capi.call(L.t2_mel_cepstra, dev, t.data_ptr(), code, None if ln is None else ln.data_ptr(), B, n_mel, T,
                    table.data_ptr(), n_cep, cep.data_ptr())
         ceps.append(cep)
@@ -166,14 +128,9 @@ def mel_cepstral_distortion(mel_x, mel_y, x_lengths=None, y_lengths=None, n_cep=
 
 
 def _pitch_track(f0, voiced, name, device_type):
-    if not torch.is_tensor(f0) or not f0.dtype.is_floating_point:
-        raise TypeError("%s: f0_%s must be a float tensor (got %s)"
-                        % (_PITCH, name, f0.dtype if torch.is_tensor(f0) else type(f0).__name__))
-    if f0.dim() != 2 or min(f0.shape) < 1:
-        raise ValueError("%s: f0_%s must have shape (B, F), none of them 0 (got %s)" % (_PITCH, name, tuple(f0.shape)))
-    if f0.device.type != device_type:
-        raise ValueError("%s: f0_%s must be on a %s device (got %s); there is no CPU path"
-                         % (_PITCH, name, device_type.upper(), f0.device))
+    if not torch.is_tensor(f0):
+        raise TypeError("%s: f0_%s must be a float tensor (got %s)" % (_PITCH, name, type(f0).__name__))
+    _float_tensor(f0, "f0_" + name, _PITCH, "(B, F)", (2,), device_type)
     if not torch.is_tensor(voiced) or voiced.dtype != torch.bool:
         raise TypeError("%s: voiced_%s must be a bool tensor (got %s)"
                         % (_PITCH, name, voiced.dtype if torch.is_tensor(voiced) else type(voiced).__name__))

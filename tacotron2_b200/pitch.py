@@ -5,29 +5,17 @@ over each symbol's frames, with the durations of ``durations_from_alignments``. 
 The host turns librosa's parameters into small fp64 tables (beta probabilities, Boltzmann pmf, the transition band,
 the bin frequencies) exactly as ``tests/pyin_oracle.py`` computes them, and the kernels of ``pitch.cu`` only read them."""
 import ctypes as C
-import math
 import numbers
-import threading
 
 import numpy as np
 import torch
 
 from . import _capi
-from ._engine import _integer_tensor, row_lengths
+from ._engine import _cached_table, _float_tensor, _integer_tensor, _number, row_lengths
 
 TINY = np.finfo(np.float64).tiny
 _PYIN = "tacotron2_b200.pyin"
 _AVG = "tacotron2_b200.average_by_durations"
-
-
-def _number(x, name, lo=None, hi=None, lo_open=False, integer=False):
-    if isinstance(x, bool) or not isinstance(x, numbers.Real) or (integer and not isinstance(x, numbers.Integral)):
-        raise TypeError("%s: %s must be %s (got %r)" % (_PYIN, name, "an integer" if integer else "a real number", x))
-    x = int(x) if integer else float(x)
-    if not math.isfinite(x) or (lo is not None and (x <= lo if lo_open else x < lo)) or (hi is not None and x > hi):
-        rng = "%s%s, %s]" % ("(" if lo_open else "[", lo if lo is not None else "-inf", hi if hi is not None else "inf")
-        raise ValueError("%s: %s must lie in %s (got %r)" % (_PYIN, name, rng, x))
-    return x
 
 
 def _transition_local(n, width):
@@ -62,15 +50,16 @@ def pyin_params(sr, fmin, fmax, frame_length=1024, win_length=None, hop_length=N
                          % (_PYIN, center))
     if pad_mode != "constant":
         raise ValueError("%s: pad_mode must be 'constant' (zero padding; got %r)" % (_PYIN, pad_mode))
-    sr = _number(sr, "sr", 0, None, True, integer=True)
-    frame_length = _number(frame_length, "frame_length", 2, _capi.PYIN_MAX_FRAME, integer=True)
-    win_length = frame_length // 2 if win_length is None else _number(win_length, "win_length", 1, frame_length - 1,
+    sr = _number(sr, "sr", _PYIN, 0, None, True, integer=True)
+    frame_length = _number(frame_length, "frame_length", _PYIN, 2, _capi.PYIN_MAX_FRAME, integer=True)
+    win_length = frame_length // 2 if win_length is None else _number(win_length, "win_length", _PYIN, 1,
+                                                                       frame_length - 1, integer=True)
+    hop_length = frame_length // 4 if hop_length is None else _number(hop_length, "hop_length", _PYIN, 1, None,
                                                                        integer=True)
-    hop_length = frame_length // 4 if hop_length is None else _number(hop_length, "hop_length", 1, None, integer=True)
     if hop_length < 1:
         raise ValueError("%s: hop_length must be at least 1 (frame_length %d)" % (_PYIN, frame_length))
-    fmin = _number(fmin, "fmin", 0, None, True)
-    fmax = _number(fmax, "fmax", 0, None, True)
+    fmin = _number(fmin, "fmin", _PYIN, 0, None, True)
+    fmax = _number(fmax, "fmax", _PYIN, 0, None, True)
     if fmin >= fmax:
         raise ValueError("%s: fmin (%r) must be below fmax (%r)" % (_PYIN, fmin, fmax))
     if fmax > sr / 2:
@@ -81,15 +70,15 @@ def pyin_params(sr, fmin, fmax, frame_length=1024, win_length=None, hop_length=N
         raise ValueError("%s: max_period = min(ceil(sr / fmin), frame_length - win_length - 1) = %d must exceed "
                          "min_period = floor(sr / fmax) = %d: lower fmin or raise frame_length / fmax"
                          % (_PYIN, max_period, min_period))
-    n_thresholds = _number(n_thresholds, "n_thresholds", 1, _capi.PYIN_MAX_THRESHOLDS, integer=True)
+    n_thresholds = _number(n_thresholds, "n_thresholds", _PYIN, 1, _capi.PYIN_MAX_THRESHOLDS, integer=True)
     if not isinstance(beta_parameters, (tuple, list)) or len(beta_parameters) != 2:
         raise TypeError("%s: beta_parameters must be a pair (got %r)" % (_PYIN, beta_parameters))
-    beta = tuple(_number(p, "beta_parameters", 0, None, True) for p in beta_parameters)
-    boltzmann_parameter = _number(boltzmann_parameter, "boltzmann_parameter", 0, None, True)
-    resolution = _number(resolution, "resolution", 0, 1, True)
-    max_transition_rate = _number(max_transition_rate, "max_transition_rate", 0)
-    switch_prob = _number(switch_prob, "switch_prob", 0, 1)
-    no_trough_prob = _number(no_trough_prob, "no_trough_prob", 0, 1)
+    beta = tuple(_number(p, "beta_parameters", _PYIN, 0, None, True) for p in beta_parameters)
+    boltzmann_parameter = _number(boltzmann_parameter, "boltzmann_parameter", _PYIN, 0, None, True)
+    resolution = _number(resolution, "resolution", _PYIN, 0, 1, True)
+    max_transition_rate = _number(max_transition_rate, "max_transition_rate", _PYIN, 0)
+    switch_prob = _number(switch_prob, "switch_prob", _PYIN, 0, 1)
+    no_trough_prob = _number(no_trough_prob, "no_trough_prob", _PYIN, 0, 1)
     if isinstance(fill_na, bool) or not isinstance(fill_na, numbers.Real):
         raise TypeError("%s: fill_na must be a real number (got %r)" % (_PYIN, fill_na))
     bps = int(np.ceil(1.0 / resolution))
@@ -137,38 +126,20 @@ def pyin_tables(p):
                 log_trans=band, freqs=freqs, log_tiny=float(log_tiny), log_init_unvoiced=float(p_init))
 
 
-_TABLES = {}
-_TABLES_LOCK = threading.Lock()
-
-
 def _device_tables(p, device):
     """pyin_tables(p) on `device`, cached per parameter set and device (built outside any graph capture)."""
-    key = (tuple(sorted((k, v) for k, v in p.items() if k != "fill_na")), str(device))
-    with _TABLES_LOCK:
-        t = _TABLES.get(key)
-        if t is None:
-            host = pyin_tables(p)
-            t = {k: (torch.from_numpy(np.ascontiguousarray(v)).to(device) if isinstance(v, np.ndarray) else v)
-                 for k, v in host.items()}
-            if len(_TABLES) >= 16:
-                _TABLES.clear()
-            _TABLES[key] = t
-        return t
+    def build():
+        return {k: (torch.from_numpy(np.ascontiguousarray(v)).to(device) if isinstance(v, np.ndarray) else v)
+                for k, v in pyin_tables(p).items()}
+    key = ("pyin", tuple(sorted((k, v) for k, v in p.items() if k != "fill_na")), str(device))
+    return _cached_table(key, build)
 
 
 def pyin_inputs(y, lengths, device_type="cuda"):
     """y and lengths checked and put in the library's form: (y (B, n) fp32 contiguous, lengths (B,) int32 on y's device
     or None, whether y was 1-D).  Reads the device back once for the samples' finiteness (and once for device-side
     lengths).  Raises TypeError / ValueError before anything is launched."""
-    if not torch.is_tensor(y):
-        raise TypeError("%s: y must be a tensor (got %s)" % (_PYIN, type(y).__name__))
-    if not y.dtype.is_floating_point:
-        raise TypeError("%s: y must be a float tensor (got %s)" % (_PYIN, y.dtype))
-    if y.dim() not in (1, 2) or min(y.shape) < 1:
-        raise ValueError("%s: y must have shape (n,) or (B, n), none of them 0 (got %s)" % (_PYIN, tuple(y.shape)))
-    if y.device.type != device_type:
-        raise ValueError("%s: y must be on a %s device (got %s); there is no CPU path"
-                         % (_PYIN, device_type.upper(), y.device))
+    _float_tensor(y, "y", _PYIN, "(n,) or (B, n)", (1, 2), device_type)
     one = y.dim() == 1
     x = y.detach().reshape(1, -1) if one else y.detach()
     B, n = (int(s) for s in x.shape)
@@ -227,15 +198,7 @@ def pyin(y, fmin, fmax, sr=22050, frame_length=1024, win_length=None, hop_length
 def average_inputs(values, durations, device_type="cuda"):
     """values and durations checked and put in the library's form: (values (B, F) fp64 contiguous, durations (B, T)
     int64 contiguous).  Reads the device back once.  Raises TypeError / ValueError before anything is launched."""
-    if not torch.is_tensor(values):
-        raise TypeError("%s: values must be a tensor (got %s)" % (_AVG, type(values).__name__))
-    if not values.dtype.is_floating_point:
-        raise TypeError("%s: values must be a float tensor (got %s)" % (_AVG, values.dtype))
-    if values.dim() != 2 or min(values.shape) < 1:
-        raise ValueError("%s: values must have shape (B, F), none of them 0 (got %s)" % (_AVG, tuple(values.shape)))
-    if values.device.type != device_type:
-        raise ValueError("%s: values must be on a %s device (got %s); there is no CPU path"
-                         % (_AVG, device_type.upper(), values.device))
+    _float_tensor(values, "values", _AVG, "(B, F)", (2,), device_type)
     d = _integer_tensor(durations, "durations", _AVG)
     B, F = (int(s) for s in values.shape)
     if d.dim() != 2 or d.shape[0] != B or d.shape[1] < 1:
